@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the B200 hot path (BASELINE.json metric): utterances/sec through frontend+encoder
+"""Benchmark of the CUDA hot path (BASELINE.json metric): utterances/sec through frontend+encoder
 forward and batched beam-search decode, synthetic 80-dim fbank (1000 frames), random-init weights.
 
     python bench.py [--gpus N --steps K --warmup W]            # this repo's CUDA path
@@ -201,7 +201,8 @@ def measured_peaks():
             p = json.load(f)
         return p, 'measured'
     except Exception:
-        return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback'
+        # NVIDIA H100 SXM data sheet (dense bf16, HBM3); a power-limited card reaches less
+        return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0}, 'H100 SXM data sheet'
 
 
 # ------------------------------------------------------------------------------------------------
@@ -386,6 +387,16 @@ def dist_barrier(world):
     torch.cuda.synchronize()
 
 
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy (float64 for integer ids, which it holds exactly; float32 otherwise)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        a = t.double().numpy() if not t.is_floating_point() else t.float().numpy()
+        np.save(os.path.join(out_dir, f'{name}.npy'), a)
+
+
 def ids_digest(ids):
     import hashlib
     return hashlib.sha1(ids.detach().to('cpu', torch.int64).contiguous().numpy().tobytes()).hexdigest()
@@ -453,7 +464,14 @@ def run_b200(args):
     if use_persist and not persist_ok:
         raise SystemExit(f'bench.py: --decode persistent, but the probe failed: {probe_note}')
     probe = make_rec(True) if use_persist else None
-    L = args.lanes if args.lanes > 0 else (3 if use_persist else 16)
+    # persistent path: as many lanes as batches whose 16-CTA row groups (one CTA per SM: 227 KB of shared memory) fit on the
+    # SMs at once, plus one queued batch -- 3 on a 132-SM H100.  Every recognize_ids() waits on the host for the executed
+    # step count, so with only the resident batches the GPU idles whenever a lane is in that host phase, and the throughput
+    # depends on how the lanes' phases happen to align (measured: +-10 % run to run with 2 lanes, +-2 % with 3).  The queued
+    # batch needs the cluster barrier (clusters are gang-scheduled), selected below.
+    groups = -(-B_PER_GPU // max(1, 128 // BEAM))
+    sms = ops.num_sms()
+    L = args.lanes if args.lanes > 0 else (max(1, sms // (groups * 16)) + 1 if use_persist else 16)
     L = max(1, L)
     # lone-batch diagnostics: one recogniser per decode path (graph path captured under the latency tile policy)
     rec_graph, rec_pers = make_rec(False), probe
@@ -467,9 +485,13 @@ def run_b200(args):
     ops.set_tile_policy(policy)
     lanes = [(torch.cuda.Stream(device=dev), make_rec(use_persist)) for _ in range(L)]
 
+    last_out = {}
+
     def step_resident(rec, i):
         x, m = ring_dev[i % RING]
-        return rec.recognize_ids(x, m)
+        out = rec.recognize_ids(x, m)
+        last_out[i] = out      # what a caller of the timed path receives, by step index (--dump-outputs)
+        return out
 
     out_pin = {}
 
@@ -568,25 +590,34 @@ def run_b200(args):
     # with full rounds finish sooner (K = 20 -> 2 rounds of 10)
     rounds = -(-args.steps // L)
     L_eff = min(L, -(-args.steps // rounds))
-    # group barrier of the persistent kernel: a cluster of 16 CTAs fills a GPC, so clusters cap the GPU at 8 row groups in
-    # flight; 3 batches x 3 groups want 9 -> plain CTAs + the software barrier (all 148 SMs) for the multi-lane region, the
-    # hardware cluster barrier for the lone-batch latency above (ops.set_decode_barrier, include/otb200.h)
-    groups = -(-B_PER_GPU // max(1, 128 // BEAM))
-    grp_barrier = args.barrier if args.barrier != 'auto' else ('software' if (use_persist and L_eff * groups > 8) else 'default')
+    # group barrier of the persistent kernel: the hardware cluster barrier (clusters are gang-scheduled, so any number of
+    # groups in flight makes progress; a cluster of 16 CTAs fills a GPC) -- requested explicitly when not every CTA in flight
+    # can be resident, so that a device without clusters fails instead of spinning -- unless more groups are in flight than
+    # clusters fit at once (8) AND every CTA of them is resident at the same time, which the software barrier needs
+    # (ops.set_decode_barrier, include/otb200.h)
+    all_resident = L_eff * groups * 16 <= sms
+    grp_barrier = args.barrier if args.barrier != 'auto' else (
+        'software' if (use_persist and L_eff * groups > 8 and all_resident) else ('default' if all_resident else 'cluster'))
+    if use_persist and grp_barrier == 'software' and not all_resident:
+        raise SystemExit(f'bench.py: the software group barrier needs all {L_eff * groups * 16} CTAs of {L_eff} batches '
+                         f'resident at once, the GPU has {sms} SMs (use fewer --lanes or --barrier cluster)')
     if use_persist:
         ops.set_decode_barrier(grp_barrier)
     if L > 1:
         timed(step_resident, 2 * L, L)      # untimed multi-lane pass: thread start-up, allocator growth per stream
-    # The timed region is EXACTLY `steps` steps between barrier + synchronize; it is repeated until ~1 s of device time has
-    # been measured so that the per-step cost does not depend on the driver's step count (VERDICT r1 weak #14).
-    probe_ms = timed(step_resident, args.steps, L_eff)
-    repeats = int(min(64, max(1, -(-args.min_ms // max(probe_ms, 1e-3)))))
+    # The timed region is EXACTLY `steps` steps between barrier + synchronize.
+    repeats = 1
+    last_out.clear()
     sampler = ClockSampler(local) if rank == 0 else None
     if sampler:
         sampler.start()
     n0 = ops.COUNTERS['launches']
     res_ms = [timed(step_resident, args.steps, L_eff) for _ in range(repeats)]
     launches = (ops.COUNTERS['launches'] - n0) // repeats
+    if args.dump_outputs and rank == 0:
+        ids_l, scores_l, n_l = last_out[args.steps - 1]
+        dump_outputs(args.dump_outputs, {'nbest_ids': ids_l, 'nbest_scores': scores_l,
+                                         'decode_steps': torch.tensor([float(n_l)])})
     if L > 1:
         timed(step_e2e, 2 * L, L)           # untimed: per-stream allocator pools and pinned result buffers of the e2e path
     e2e_ms = [timed(step_e2e, args.steps, L_eff) for _ in range(repeats)]
@@ -601,7 +632,7 @@ def run_b200(args):
     line = None
     if rank == 0:
         peaks, src = measured_peaks()
-        peak_tf, peak_tf_burst, peak_bw = peaks.get('bf16_tflops_sustained', 1400.0), peaks.get('bf16_tflops', 1590.0), peaks.get('hbm_gbs', 6650.0)
+        peak_tf, peak_tf_burst, peak_bw = peaks.get('bf16_tflops_sustained', 989.0), peaks.get('bf16_tflops', 989.0), peaks.get('hbm_gbs', 3350.0)
         T2 = ops.conv_geometry(T_FRAMES, F_BINS)[2]
         w_bytes, kv_bytes = decode_step_bytes(model, B_PER_GPU, T2)
         ms_step = ms_total / args.steps
@@ -610,12 +641,7 @@ def run_b200(args):
         def fr(flop, nbytes, ms, tf_peak):
             return {'tflops': flop / (ms * 1e-3) / 1e12, 'frac_tensor': flop / (ms * 1e-3) / 1e12 / tf_peak,
                     'gbs': nbytes / (ms * 1e-3) / 1e9, 'frac_hbm': nbytes / (ms * 1e-3) / 1e9 / peak_bw}
-        traffic = None
-        try:    # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full capture
-            with open(os.path.join(ROOT, 'profiles', 'r2_traffic.json')) as f:
-                traffic = json.load(f).get('decode_group_kernel' if use_persist else 'gemm_tc_kernel')
-        except Exception:
-            pass
+        traffic = None          # DRAM traffic counters are not measured here
         if use_persist:
             # dominant kernel = the persistent decode kernel: one launch per batch, ~90 % of the device time of a pass
             ach = dec_bytes / (dec_kernel_ms * 1e-3) / 1e9
@@ -624,7 +650,7 @@ def run_b200(args):
                                   f'utterances on 3 row groups x 16 CTAs; {dec_kernel_ms:.2f} ms per launch (CUDA events on its stream, lone batch, '
                                   f'median of 6); algorithmic bytes per launch = {MAX_LEN} steps x ({w_bytes / 1e6:.1f} MB decoder weights + '
                                   f'{kv_bytes / 1e6:.1f} MB cross-attention K/V) = {dec_bytes / 1e9:.2f} GB (SURVEY.md 8d), {DEC_FLOP / 1e9:.0f} GFLOP; '
-                                  'latency-bound: 38 group barriers and ~60 dependent phases per step (profiles/r2_decode_phases_*.txt); the self-attention '
+                                  'latency-bound: 38 group barriers and ~60 dependent phases per step; the self-attention '
                                   'K/V prefix (<= 133 MB per batch, read through an ancestry table) is not counted in the algorithmic bytes',
                         'alt': fr(DEC_FLOP, dec_bytes, dec_kernel_ms, peak_tf_burst),
                         'peak_source': f'MEASURED_PEAKS.json ({src}); burst bf16 figure for the lone kernel, sustained for whole steps'}
@@ -678,7 +704,7 @@ def run_b200(args):
             'roofline': roofline,
             'validation': {'ids_sha1': digest, 'expected_sha1': expected, 'match': (digest == expected) if expected else None,
                            'steps_executed': int(steps0), 'one_best_equal_to_bf16_policy_oracle': oracle_agree,
-                           'note': 'expected_sha1 = digest of the same decode path recorded on a B200 by tools/gpu_r2_digest.sh '
+                           'note': 'expected_sha1 = digest of the same decode path recorded on an H100 (tests/golden/bench_digest.json) '
                                    '(regression check); the oracle count is informational: default-initialised weights give '
                                    'near-ties that bf16 rounding resolves differently'},
             'clocks': clocks,
@@ -819,7 +845,7 @@ def graph_path_roofline(model, lanes, ring_dev, dev, peaks, src, traffic):
     n_out = Nw_ // 2 if epi == 2 else Nw_
     nbytes = 2.0 * (M_ * K_ + Nw_ * K_ + M_ * n_out) + (2.0 * M_ * n_out if epi in (4, 5) else 0.0)
     tf, gbs = flops / (avg_ms * 1e-3) / 1e12, nbytes / (avg_ms * 1e-3) / 1e9
-    peak_tf, peak_bw = peaks.get('bf16_tflops', 1590.0), peaks.get('hbm_gbs', 6650.0)
+    peak_tf, peak_bw = peaks.get('bf16_tflops', 989.0), peaks.get('hbm_gbs', 3350.0)
     use_hbm = gbs / peak_bw > tf / peak_tf
     ach, peak = (gbs, peak_bw) if use_hbm else (tf, peak_tf)
     return {'bound': 'hbm' if use_hbm else 'tensor', 'achieved': ach, 'peak': peak, 'unit': 'GB/s' if use_hbm else 'TFLOP/s',
@@ -905,7 +931,7 @@ def measure_conformer(args, steps):
                                    f'{B} utt x {T_FRAMES} frames per GPU (BASELINE config 4)',
                        'parallelism': f'dp{world} (utterance sharding, no data-path collective)'},
             'roofline': {'bound': 'tensor', 'achieved': ach, 'peak': peaks.get('bf16_tflops_sustained'),
-                         'unit': 'TFLOP/s', 'frac': ach / peaks.get('bf16_tflops_sustained', 1400.0),
+                         'unit': 'TFLOP/s', 'frac': ach / peaks.get('bf16_tflops_sustained', 989.0),
                          'traffic': None, 'kernel': 'whole encoder pass (898 GFLOP algorithmic per batch)',
                          'peak_source': src}}
 
@@ -922,7 +948,7 @@ def run_conformer(args):
 
 def train_params():
     """BASELINE config 5: the config-2 model with every dropout rate 0 (the reference's residual_dropout 0.1 is stochastic;
-    the B200 training path implements the deterministic network, DESIGN.md 6)."""
+    the CUDA training path implements the deterministic network, DESIGN.md 6)."""
     p = model_params()
     for part in ('frontend', 'encoder', 'decoder'):
         for k in list(p[part]):
@@ -1037,7 +1063,7 @@ def measure_train(args, steps):
                     'h2d_bytes_per_step': item[0].numel() * 4 + item[1].numel() + item[2].numel() * 8, 'd2h_bytes_per_step': 4},
             'gpu_launches': launches, 'final_loss': final_loss,
             'roofline': {'bound': 'tensor', 'achieved': ach, 'peak': peaks.get('bf16_tflops_sustained'), 'unit': 'TFLOP/s',
-                         'frac': ach / peaks.get('bf16_tflops_sustained', 1400.0), 'traffic': None,
+                         'frac': ach / peaks.get('bf16_tflops_sustained', 989.0), 'traffic': None,
                          'kernel': 'whole training step (3 x 448.9 GFLOP algorithmic per 32-utterance batch)',
                          'peak_source': src},
             'clocks': clocks}
@@ -1067,14 +1093,16 @@ def main():
     ap.add_argument('--workload', default='transformer', choices=['transformer', 'conformer', 'train'],
                     help="'conformer' = BASELINE config 4 (encoder forward only), 'train' = config 5 (training step); "
                          "default is the headline workload")
-    ap.add_argument('--lanes', type=int, default=0, help='utterance batches kept in flight per GPU (streams); 0 = auto: 3 for the '
-                                                       'persistent decode kernel (48 SMs per batch), 16 for the per-step graph')
+    ap.add_argument('--lanes', type=int, default=0, help='utterance batches kept in flight per GPU (streams); 0 = auto: as many as '
+                                                       'fit the SMs plus one for the persistent decode kernel (48 CTAs per batch), 16 for the per-step graph')
     ap.add_argument('--barrier', default='auto', choices=['auto', 'cluster', 'software'],
                     help='group barrier of the persistent decode kernel in the timed multi-lane region (auto: software when more than 8 '
-                         'row groups are in flight, else thread-block clusters)')
+                         'row groups are in flight and all their CTAs fit the SMs at once, else thread-block clusters)')
     ap.add_argument('--decode', default='auto', choices=['auto', 'persistent', 'graph'],
                     help='decode path: one persistent launch per batch (csrc/decode_group.cu) or one CUDA-graph replay per step')
-    ap.add_argument('--min-ms', type=float, default=1000.0, help='repeat the timed K-step region until this much device time is measured')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='after the timed steps, write the n-best ids / scores of the last timed step as DIR/<name>.npy '
+                         '(transformer workload)')
     ap.add_argument('--no-extras', dest='extras', action='store_false',
                     help='skip the BASELINE config 4 / 5 measurements appended to the default run')
     ap.add_argument('--tile-policy', default='auto', choices=['auto', 'latency', 'throughput'],
@@ -1085,10 +1113,12 @@ def main():
     if args.probe_persistent:
         return run_probe_persistent()
     guard_stdout()
+    if args.dump_outputs and (args.impl != 'b200' or args.workload != 'transformer'):
+        raise SystemExit('bench.py: --dump-outputs is implemented for the transformer workload of the CUDA path')
     if args.impl == 'reference':
         return run_reference(args)
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py: no CUDA device -- the B200 path has no CPU fallback (use --impl reference)')
+        raise SystemExit('bench.py: no CUDA device -- the CUDA path has no CPU fallback (use --impl reference)')
     if args.workload == 'conformer':
         return run_conformer(args)
     if args.workload == 'train':

@@ -1,5 +1,5 @@
 /*
- * libotb200 -- B200 (sm_100a) hot path for the OpenTransformer speech transformer, C ABI.
+ * libotb200 -- H100 (sm_90a) hot path for the OpenTransformer speech transformer, C ABI.
  *
  * The reference has no FFI / operator API: its boundary is the Python nn.Module surface
  * (SURVEY.md 8b).  Every entry point below therefore names the reference *module method* whose
@@ -42,10 +42,9 @@ enum {
 const char* otb_last_error(void);
 int otb_version(void);
 int otb_num_sms(void);
-/* Tiling policy of small GEMMs (M <= 512 rows, the decode step): 0 (default) = shortest launch -- narrow tiles, the
- * residual+LayerNorm row split over a 4-CTA cluster; 1 = least SM-time -- the widest tile on the fewest CTAs, for
- * servers that keep several utterance batches in flight on separate streams (+10-15 % aggregate throughput, +30 %
- * latency of a lone batch on B200).  Process-wide; set it before CUDA graphs are captured. */
+/* Tiling policy of small GEMMs (M <= 512 rows, the decode step): 0 (default) = shortest launch -- the tiling with the
+ * fewest MMA waves; 1 = least SM-time -- the widest tile on the fewest CTAs, for servers that keep several utterance
+ * batches in flight on separate streams.  Process-wide; set it before CUDA graphs are captured. */
 int otb_set_tile_policy(int policy);
 /* Profiling aid: buf (device, u64 [grid*8]) receives per-CTA clock64 phase stamps of the next GEMMs; NULL disables. */
 int otb_debug_gemm_timing(unsigned long long* buf);
@@ -56,8 +55,9 @@ int otb_debug_gemm_mode(int mode);
 int otb_debug_decode_timing(unsigned long long* buf, int step);
 /* Serving knob of otb_decode_persistent (no counterpart in the reference): how the 16 CTAs of a row group synchronise.
  * 1 = thread-block cluster of 16 + barrier.cluster (lowest latency; one cluster per GPC, i.e. at most 8 groups in flight),
- * 0 = plain CTAs + a release/acquire counter in L2 (all 148 SMs usable: best throughput with 3 batches in flight),
- * -1 = default (clusters when the device grants them, unless OTB_DG_CLUSTER=0).  Process-wide. */
+ * 0 = plain CTAs + a release/acquire counter in L2 (every SM usable; every CTA of every batch in flight must be resident),
+ * -1 = default (clusters when the device grants them, unless OTB_DG_CLUSTER=0).  With 1, a launch on a device that refuses
+ * clusters of 16 fails instead of falling back to the software barrier.  Process-wide. */
 int otb_set_decode_barrier(int kind);
 
 /* Conv2dLayer output geometry, kernel 3, stride 2, padding (0,1)  (frontend/conv.py:10-11,27):
@@ -71,13 +71,13 @@ int otb_conv1_relu(const float* x, const float* w, const float* bias, void* out,
                    void* stream);
 
 /* Conv2dLayer.forward #2 + the transpose/reshape of ConvFrontEnd.forward (frontend/conv.py:63-64,145)
- * as a tcgen05 implicit GEMM.  in = conv1 buffer; w bf16 [C2, 9*C1] with k = (kh*3+kw)*C1 + c;
+ * as a wgmma implicit GEMM.  in = conv1 buffer; w bf16 [C2, 9*C1] with k = (kh*3+kw)*C1 + c;
  * out bf16 [B*T2, F2*C2] with feature index f*C2 + c (the caller permutes output_layer.weight columns
  * from the reference's c*F2 + f order once at load time). */
 int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2,
                    void* stream);
 
-/* nn.Linear with a fused epilogue on tcgen05 tensor cores: out[M,N] = epi(a[M,K] w[N(,2N),K]^T + bias).
+/* nn.Linear with a fused epilogue on wgmma tensor cores: out[M,N] = epi(a[M,K] w[N(,2N),K]^T + bias).
  * a, w bf16 (lda, ldw in elements, multiples of 8); out bf16 or f32 (out_f32); unused pointers NULL.
  * row_len/row_period: optional key-padding mask, rows with (m % row_period) >= row_len[m / row_period]
  * produce 0 before the residual is added (conformer.py:46,55 masked_fill).
@@ -186,8 +186,8 @@ int otb_beam_finalize(const otb_beam_state* st, float penalty, float lamda, int 
 /* ---- Persistent decode loop --------------------------------------------------------------------------------
  * The whole loop of SpeechToTextRecognizer.recognize (recognize/speech2text.py:60-68: decode_step :95-153 ->
  * TransformerDecoder.inference, decoder/transformer.py:185-208) for ALL steps in one launch (csrc/decode_group.cu):
- * the hypotheses of up to 128 / beam utterances form one 128-row tcgen05 tile owned by a group of 16 co-operating CTAs
- * (projections split by output column / contraction slice, weights streamed from L2 by TMA, accumulators in TMEM,
+ * the hypotheses of up to 128 / beam utterances form one 128-row wgmma tile owned by a group of 16 co-operating CTAs
+ * (projections split by output column / contraction slice, weights streamed from L2 by TMA, accumulators in registers,
  * activations exchanged through L2 behind a group-local barrier), search state on the device, no kernel launch or host
  * round trip inside the loop.  Post-norm GLU decoder, d_model 256, 4 heads, d_ff 2048, beam <= 16, T <= 256 memory
  * frames, max_steps <= st->Lmax <= 128, ceil(B / (128 / beam)) * 16 <= number of SMs (other configurations: per-step
@@ -232,12 +232,12 @@ int otb_attention_lse(const void* q, int ldq, int q_rows, const void* k, int ldk
                       int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse,
                       void* stream);
 /* Backward of otb_attention (no bd / resid): dq, dk, dv written at column offsets d*_col0 + 64*h of their matrices
- * (e.g. the three thirds of one [M,3d] dqkv buffer).  dsum f32 [B,H,Tq] is scratch.  tcgen05, scores recomputed. */
+ * (e.g. the three thirds of one [M,3d] dqkv buffer).  dsum f32 [B,H,Tq] is scratch.  wgmma, scores recomputed. */
 int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
                       const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
                       int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
                       int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, void* stream);
-/* nn.Linear weight gradient dW[N,K] (fp32) = dy[M,N]^T x[M,K] (bf16), tcgen05 with MN-major operands + split-K.
+/* nn.Linear weight gradient dW[N,K] (fp32) = dy[M,N]^T x[M,K] (bf16), wgmma with MN-major operands + split-K.
  * (The input gradient dx = dy W is otb_linear with the transposed weight.)  accumulate != 0: dW += ... (gradient
  * accumulation straight into the optimizer's flat gradient buffer, the way autograd accumulates into .grad). */
 int otb_linear_wgrad(const void* dy, int lddy, const void* x, int ldx, float* dw, int lddw, int M, int N, int K, int accumulate,

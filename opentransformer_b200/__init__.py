@@ -1,4 +1,4 @@
-"""opentransformer_b200 -- the OpenTransformer speech-transformer hot path as hand-written sm_100a
+"""opentransformer_b200 -- the OpenTransformer speech-transformer hot path as hand-written sm_90a
 CUDA kernels behind the reference's nn.Module / Recognizer interface (see DESIGN.md)."""
 from ._lib import LIB_PATH, exported_symbols  # noqa: F401
 

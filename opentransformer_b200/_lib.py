@@ -110,7 +110,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f'{LIB_PATH} is missing: build it with `python -m opentransformer_b200.build` '
-                '(there is no CPU fallback for the B200 hot path)')
+                '(there is no CPU fallback for the CUDA hot path)')
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGS.items():
             fn = getattr(l, name)

@@ -1,8 +1,8 @@
-"""Build libotb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libotb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m opentransformer_b200.build [--force]
 
-The .so lands next to this file (git-ignored, but shipped to the GPU box by gpurun).
+The .so lands next to this file (git-ignored; build() recreates it from a clean checkout).
 cudart is linked statically and libcuda is resolved at run time through
 cudaGetDriverEntryPoint, so the library also *loads* on a machine without a GPU driver.
 """
@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libotb200.so')
 SOURCES = ['gemm_tc.cu', 'attn_tc.cu', 'attn_bwd.cu', 'backward.cu', 'ops_simt.cu', 'beam.cu', 'decode_group.cu', 'loss.cu', 'ctc.cu', 'fbank.cu', 'capi.cu']
 HEADERS = ['otb_internal.h', 'ptx.cuh', 'beam_common.cuh', 'launch.cuh', os.path.join('..', '..', 'include', 'otb200.h')]
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-std=c++17', '-lineinfo',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-lineinfo',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v', '--expt-relaxed-constexpr']
 
 
@@ -51,7 +51,7 @@ def build(force=False, verbose=False):
         if p.returncode != 0:
             raise RuntimeError(f'nvcc failed on {s}:\n{out}')
         objs.append(o)
-    cmd = [_nvcc(), '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-cudart', 'static']
+    cmd = [_nvcc(), '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-cudart', 'static']
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

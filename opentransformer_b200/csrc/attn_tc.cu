@@ -1,5 +1,5 @@
-// Fused masked multi-head attention for sm_100a (d_k = 64):  softmax(Q K^T / sqrt(d_k) + mask) V
-// Both contractions run on tcgen05 tensor cores with the score tile and the output tile in TMEM;
+// Fused masked multi-head attention for sm_90a (d_k = 64):  softmax(Q K^T / sqrt(d_k) + mask) V
+// Both contractions run on wgmma tensor cores with the score tile and the output tile in registers;
 // the key-padding mask comes from lengths[b] (masks are always contiguous prefixes, SURVEY.md 8a),
 // the causal mask from row/column indices, so no [B,h,T,T] tensor is ever materialised.
 //
@@ -8,12 +8,12 @@
 //   :41 (merge heads).  The reference also returns the [B,h,T1,T2] weights; no caller reads them
 //   (model/speech2text.py:50,54), so they are not produced here.
 //
-// One CTA = 128 query rows of one (batch, head); 128 threads, thread i owns query row i (TMEM lane i).
-// Keys are consumed in blocks of 128 with an online softmax:
+// One CTA = 128 query rows of one (batch, head); 256 threads = two warpgroups, warpgroup w owns query rows
+// [64 w, 64 w + 64).  Keys are consumed in blocks of 128 with an online softmax:
 //   TMA: Q tile [128x64], K block [128x64] (K-major) and V block [128 keys x 64] (MN-major B operand)
-//   S  = Q K^T      : 4 x UMMA 128x128x16  -> TMEM columns [0,128)
+//   S  = Q K^T      : 4 x wgmma 64x128x16 per warpgroup (registers)
 //   P  = exp2(S*c - m) as bf16 written to smem in the canonical K-major SWIZZLE_128B layout
-//   O' = P V        : 8 x UMMA 128x64x16   -> TMEM columns [128,192), rescaled + accumulated in registers
+//   O  = O*alpha + P V : 8 x wgmma 64x64x16 per warpgroup, accumulated in registers
 #include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
@@ -29,7 +29,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 
 template <bool HAS_BD>
-__global__ void __launch_bounds__(128, 2)
+__global__ void __launch_bounds__(256, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
     PDL_TRIGGER();
@@ -40,215 +40,160 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     uint8_t* sK = smem + 16384;
     uint8_t* sV = smem + 32768;
     uint8_t* sP = smem + 49152;  // 2 k-blocks x [128 rows x 128 B]
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 49152 + 32768);  // q, k, v, s, o
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 5);
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 49152 + 32768);  // q, k, v
 
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int wg = warp >> 2;
     const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
     const int kv_len = p.kv_len ? min(p.kv_len[b], p.Tk) : p.Tk;
     int kv_end = kv_len;
     if (p.causal) kv_end = min(kv_end, q0 + 128);
     const int nblk = (kv_end + 127) / 128;
 
-    if (warp == 0) {
-        if (tid == 0) {
-            for (int i = 0; i < 5; ++i) mbar_init(&bar[i], 1);
-            fence_barrier_init();
-            tma_prefetch_desc(&tmQ);
-            tma_prefetch_desc(&tmK);
-            tma_prefetch_desc(&tmV);
-            // Q and the first K/V block are requested before the TMEM allocation / CTA sync
-            mbar_arrive_expect_tx(&bar[0], 16384);
-            tma_load_2d(sQ, &tmQ, &bar[0], p.q_col0 + h * 64, b * p.Tq + q0);
-            if (nblk > 0) {
-                mbar_arrive_expect_tx(&bar[1], 16384);
-                tma_load_2d(sK, &tmK, &bar[1], p.k_col0 + h * 64, b * p.Tk);
-                mbar_arrive_expect_tx(&bar[2], 16384);
-                tma_load_2d(sV, &tmV, &bar[2], p.v_col0 + h * 64, b * p.Tk);
-            }
+    if (tid == 0) {
+        for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
+        fence_barrier_init();
+        tma_prefetch_desc(&tmQ);
+        tma_prefetch_desc(&tmK);
+        tma_prefetch_desc(&tmV);
+        mbar_arrive_expect_tx(&bar[0], 16384);
+        tma_load_2d(sQ, &tmQ, &bar[0], p.q_col0 + h * 64, b * p.Tq + q0);
+        if (nblk > 0) {
+            mbar_arrive_expect_tx(&bar[1], 16384);
+            tma_load_2d(sK, &tmK, &bar[1], p.k_col0 + h * 64, b * p.Tk);
+            mbar_arrive_expect_tx(&bar[2], 16384);
+            tma_load_2d(sV, &tmV, &bar[2], p.v_col0 + h * 64, b * p.Tk);
         }
-        __syncwarp();
-        tmem_alloc(tmem_slot, 256);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t t_row = tmem_base + ((uint32_t)(warp * 32) << 16);
 
-    const int qi = q0 + tid;  // query index inside the utterance
-    float m_run = -INFINITY, l_run = 0.f;
-    float acc[64];
+    // this thread's two tile rows (accumulator fragment rows) and its column offset inside every 8-column group
+    const int rl0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    int lim[2];
+    const float* bd_row[2] = {nullptr, nullptr};
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, false);
-    constexpr uint32_t idesc_o = umma_idesc_bf16(64, true);
+    for (int hh = 0; hh < 2; ++hh) {
+        const int qi = q0 + rl0 + 8 * hh;
+        lim[hh] = p.causal ? min(kv_len, qi + 1) : kv_len;  // keys [0, lim) are visible to this row
+        if (HAS_BD) {
+            const int qc = min(qi, p.Tq - 1);
+            bd_row[hh] = p.bd + (((size_t)h * p.B + b) * p.Tq + qc) * p.ldbd + (p.Tq - 1 - qc);
+        }
+    }
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    const uint32_t qa = smem_u32(sQ) + wg * 8192, ka = smem_u32(sK), va = smem_u32(sV);
+    const uint32_t pa = smem_u32(sP) + wg * 8192;
 
     for (int blk = 0; blk < nblk; ++blk) {
         const uint32_t ph = blk & 1;
         const int key0 = blk * 128;
-        if (tid == 0) {
-            if (blk == 0) mbar_wait(&bar[0], 0);
-            mbar_wait(&bar[1], ph);
-            tc_fence_after();
-            const uint32_t qa = smem_u32(sQ), ka = smem_u32(sK);
+        if (blk == 0) mbar_wait(&bar[0], 0);
+        mbar_wait(&bar[1], ph);
+        float s[64];
+        wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-                umma_bf16(tmem_base, umma_desc_sw128(qa + k * 32), umma_desc_sw128(ka + k * 32), idesc_s, (uint32_t)(k != 0));
-            umma_commit(&bar[3]);
-        }
-        __syncwarp();
-        mbar_wait(&bar[3], ph);
-        tc_fence_after();
+        for (int k = 0; k < 4; ++k) wgmma_n128<0, 0>(s, gmma_desc_sw128(qa + k * 32), gmma_desc_sw128(ka + k * 32), (uint32_t)(k != 0));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+        __syncthreads();
         if (tid == 0 && blk + 1 < nblk) {   // S = QK^T has consumed the K block: prefetch the next one
             mbar_arrive_expect_tx(&bar[1], 16384);
             tma_load_2d(sK, &tmK, &bar[1], p.k_col0 + h * 64, b * p.Tk + key0 + 128);
         }
-        __syncwarp();
 
-        // ---- pass 1: row maximum of the visible raw scores (the positive scale is applied afterwards)
-        const int lim = p.causal ? min(kv_len, qi + 1) : kv_len;  // keys [0, lim) are visible to this row
-        const float* bd_row = nullptr;
-        if (HAS_BD) {
-            const int qc = min(qi, p.Tq - 1);
-            bd_row = p.bd + (((size_t)h * p.B + b) * p.Tq + qc) * p.ldbd + (p.Tq - 1 - qc);
-        }
-        float m_blk = -INFINITY;
-#pragma unroll 1
-        for (int c = 0; c < 128; c += 32) {
-            uint32_t r[32];
-            tmem_ld32(t_row + c, r);
-            tmem_ld_wait();
-            const int k0 = key0 + c;
-            if (k0 + 32 <= lim) {
+        // ---- row maximum of the visible raw scores (the positive scale is applied afterwards); a row is spread over 4 lanes
+        float m_blk[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float sv = __uint_as_float(r[i]);
-                    if (HAS_BD) sv += bd_row[k0 + i];
-                    m_blk = fmaxf(m_blk, sv);
-                }
-            } else if (k0 < lim) {
+        for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float sv = __uint_as_float(r[i]);
-                    if (HAS_BD && k0 + i < lim) sv += bd_row[k0 + i];
-                    m_blk = fmaxf(m_blk, (k0 + i < lim) ? sv : -INFINITY);
+            for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int key = key0 + jj * 8 + cq + e;
+                    float sv = s[4 * jj + 2 * hh + e];
+                    if (HAS_BD && key < lim[hh]) sv += bd_row[hh][key];
+                    sv = (key < lim[hh]) ? sv : -INFINITY;
+                    s[4 * jj + 2 * hh + e] = sv;
+                    m_blk[hh] = fmaxf(m_blk[hh], sv);
                 }
             }
         }
-        m_blk *= p.scale_log2;  // -inf stays -inf
-        const float m_new = fmaxf(m_run, m_blk);
-        const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-        const float alpha = (m_run == -INFINITY) ? 0.f : ex2_approx(m_run - m_use);
-        float l_blk = 0.f;
-        // ---- pass 2: probabilities -> bf16 -> smem (K-major, 128B swizzle)
-#pragma unroll 1
-        for (int c = 0; c < 128; c += 32) {
-            uint32_t r[32];
-            tmem_ld32(t_row + c, r);
-            tmem_ld_wait();
-            float pv[32];
-            const int k0 = key0 + c;
-            if (k0 + 32 <= lim) {
+        float alpha[2], m_use[2], l_blk[2] = {0.f, 0.f};
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float sv = __uint_as_float(r[i]);
-                    if (HAS_BD) sv += bd_row[k0 + i];
-                    pv[i] = ex2_approx(fmaf(sv, p.scale_log2, -m_use));
-                    l_blk += pv[i];
-                }
-            } else {
+        for (int hh = 0; hh < 2; ++hh) {
+            m_blk[hh] = fmaxf(m_blk[hh], __shfl_xor_sync(0xffffffffu, m_blk[hh], 1));
+            m_blk[hh] = fmaxf(m_blk[hh], __shfl_xor_sync(0xffffffffu, m_blk[hh], 2));
+            m_blk[hh] *= p.scale_log2;  // -inf stays -inf
+            const float m_new = fmaxf(m_run[hh], m_blk[hh]);
+            m_use[hh] = (m_new == -INFINITY) ? 0.f : m_new;
+            alpha[hh] = (m_run[hh] == -INFINITY) ? 0.f : ex2_approx(m_run[hh] - m_use[hh]);
+            m_run[hh] = m_new;
+        }
+        // ---- probabilities -> bf16 -> smem (K-major, 128B swizzle)
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float sv = __uint_as_float(r[i]);
-                    if (HAS_BD && k0 + i < lim) sv += bd_row[k0 + i];
-                    pv[i] = (k0 + i < lim) ? ex2_approx(fmaf(sv, p.scale_log2, -m_use)) : 0.f;
-                    l_blk += pv[i];
-                }
-            }
-            uint8_t* prow = sP + (c >> 6) * 16384 + tid * 128;
-            const int chunk0 = (c & 63) >> 3;  // 16-byte chunk index inside the 128-byte row
+        for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                uint4 u;
-                u.x = pack_bf16(pv[8 * j], pv[8 * j + 1]);
-                u.y = pack_bf16(pv[8 * j + 2], pv[8 * j + 3]);
-                u.z = pack_bf16(pv[8 * j + 4], pv[8 * j + 5]);
-                u.w = pack_bf16(pv[8 * j + 6], pv[8 * j + 7]);
-                *reinterpret_cast<uint4*>(prow + (((chunk0 + j) ^ (tid & 7)) << 4)) = u;
+            for (int hh = 0; hh < 2; ++hh) {
+                const float sv0 = s[4 * jj + 2 * hh], sv1 = s[4 * jj + 2 * hh + 1];
+                const float p0 = (sv0 == -INFINITY) ? 0.f : ex2_approx(fmaf(sv0, p.scale_log2, -m_use[hh]));
+                const float p1 = (sv1 == -INFINITY) ? 0.f : ex2_approx(fmaf(sv1, p.scale_log2, -m_use[hh]));
+                l_blk[hh] += p0 + p1;
+                const int row = rl0 + 8 * hh;
+                const int kc = jj * 8 + cq;
+                *reinterpret_cast<uint32_t*>(sP + (kc >> 6) * 16384 + row * 128 + (((((kc & 63) >> 3) ^ (row & 7))) << 4) + (kc & 7) * 2) =
+                    pack_bf16(p0, p1);
             }
         }
-        l_run = l_run * alpha + l_blk;
-        m_run = m_new;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            l_blk[hh] += __shfl_xor_sync(0xffffffffu, l_blk[hh], 1);
+            l_blk[hh] += __shfl_xor_sync(0xffffffffu, l_blk[hh], 2);
+            l_run[hh] = l_run[hh] * alpha[hh] + l_blk[hh];
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
         fence_proxy_async_smem();  // P (generic-proxy stores) -> visible to the tensor core's async proxy
-        tc_fence_before();
         __syncthreads();
 
-        if (tid == 0) {
-            mbar_wait(&bar[2], ph);
-            tc_fence_after();
-            const uint32_t pa = smem_u32(sP), va = smem_u32(sV);
+        mbar_wait(&bar[2], ph);
+        wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 8; ++kk)
-                umma_bf16(tmem_base + 128, umma_desc_sw128(pa + (kk >> 2) * 16384 + (kk & 3) * 32),
-                          umma_desc_sw128(va + kk * 2048), idesc_o, (uint32_t)(kk != 0));
-            umma_commit(&bar[4]);
-        }
-        __syncwarp();
-        mbar_wait(&bar[4], ph);
-        tc_fence_after();
+        for (int kk = 0; kk < 8; ++kk)
+            wgmma_n64<0, 1>(o, gmma_desc_sw128(pa + (kk >> 2) * 16384 + (kk & 3) * 32), gmma_desc_sw128(va + kk * 2048, 1024, 8192), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        __syncthreads();  // K/V/P smem may now be overwritten by the next block
         if (tid == 0 && blk + 1 < nblk) {   // PV has consumed the V block: prefetch the next one
             mbar_arrive_expect_tx(&bar[2], 16384);
             tma_load_2d(sV, &tmV, &bar[2], p.v_col0 + h * 64, b * p.Tk + key0 + 128);
         }
-        __syncwarp();
-#pragma unroll
-        for (int c = 0; c < 64; c += 32) {
-            uint32_t r[32];
-            tmem_ld32(t_row + 128 + c, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) acc[c + i] = acc[c + i] * alpha + __uint_as_float(r[i]);
-        }
-        tc_fence_before();
-        __syncthreads();  // S/O TMEM and K/V/P smem may now be overwritten by the next block
     }
 
-    if (qi < p.Tq) {
-        if (p.lse) p.lse[((size_t)b * p.H + h) * p.Tq + qi] = (l_run > 0.f) ? m_run + log2f(l_run) : INFINITY;
-        const float inv = (l_run > 0.f) ? 1.0f / l_run : 0.f;
-        bf16* o = p.out + (size_t)(b * p.Tq + qi) * p.ldo + h * 64;
-        if (p.resid) {
-            const bf16* rr = p.resid + (size_t)(b * p.Tq + qi) * p.ldr + h * 64;
 #pragma unroll
-            for (int i = 0; i < 64; i += 8) {
-                const uint4 u = *reinterpret_cast<const uint4*>(rr + i);
-                const float2 a = unpack_bf16(u.x), bb = unpack_bf16(u.y), c = unpack_bf16(u.z), e = unpack_bf16(u.w);
-                acc[i] = acc[i] * inv + a.x; acc[i + 1] = acc[i + 1] * inv + a.y;
-                acc[i + 2] = acc[i + 2] * inv + bb.x; acc[i + 3] = acc[i + 3] * inv + bb.y;
-                acc[i + 4] = acc[i + 4] * inv + c.x; acc[i + 5] = acc[i + 5] * inv + c.y;
-                acc[i + 6] = acc[i + 6] * inv + e.x; acc[i + 7] = acc[i + 7] * inv + e.y;
+    for (int hh = 0; hh < 2; ++hh) {
+        const int qi = q0 + rl0 + 8 * hh;
+        if (qi >= p.Tq) continue;
+        if (p.lse && (lane & 3) == 0) p.lse[((size_t)b * p.H + h) * p.Tq + qi] = (l_run[hh] > 0.f) ? m_run[hh] + log2f(l_run[hh]) : INFINITY;
+        const float inv = (l_run[hh] > 0.f) ? 1.0f / l_run[hh] : 0.f;
+        bf16* orow = p.out + (size_t)(b * p.Tq + qi) * p.ldo + h * 64;
+        const bf16* rrow = p.resid ? p.resid + (size_t)(b * p.Tq + qi) * p.ldr + h * 64 : nullptr;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            const int c = jj * 8 + cq;
+            float v0 = o[4 * jj + 2 * hh] * inv, v1 = o[4 * jj + 2 * hh + 1] * inv;
+            if (rrow) {
+                const float2 r = unpack_bf16(*reinterpret_cast<const uint32_t*>(rrow + c));
+                v0 += r.x;
+                v1 += r.y;
             }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 64; ++i) acc[i] *= inv;
+            *reinterpret_cast<uint32_t*>(orow + c) = pack_bf16(v0, v1);
         }
-#pragma unroll
-        for (int i = 0; i < 64; i += 8) {
-            uint4 u;
-            u.x = pack_bf16(acc[i], acc[i + 1]);
-            u.y = pack_bf16(acc[i + 2], acc[i + 3]);
-            u.z = pack_bf16(acc[i + 4], acc[i + 5]);
-            u.w = pack_bf16(acc[i + 6], acc[i + 7]);
-            *reinterpret_cast<uint4*>(o + i) = u;
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 256);
     }
 }
 
@@ -268,8 +213,8 @@ const char* attn_launch(cudaStream_t st, const void* q, int ldq, int q_rows, con
         attr_set = true;
     }
     dim3 grid((p.Tq + 127) / 128, p.H, p.B);
-    cudaError_t e = p.bd ? launch_pdl(attn_tc_kernel<true>, grid, dim3(128), ATT_SMEM, st, tq, tk, tv, p)
-                         : launch_pdl(attn_tc_kernel<false>, grid, dim3(128), ATT_SMEM, st, tq, tk, tv, p);
+    cudaError_t e = p.bd ? launch_pdl(attn_tc_kernel<true>, grid, dim3(256), ATT_SMEM, st, tq, tk, tv, p)
+                         : launch_pdl(attn_tc_kernel<false>, grid, dim3(256), ATT_SMEM, st, tq, tk, tv, p);
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 

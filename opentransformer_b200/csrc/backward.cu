@@ -372,7 +372,7 @@ namespace otb {
 // Layouts as in the forward: conv1 activation h1 = NHWC bf16 [B, T1p = 2*(T2+1), F1p = 2*F2, C]; conv2 output rows are
 // (b, t2, f2) with C2 channels.  conv2's weight / input gradients are GEMMs over the explicit im2col matrix
 //   col[(b,t2,f2), (kh*3+kw)*C + c] = h1[b, 2*t2+kh, 2*f2+kw-1, c]      (f = -1 is the left zero padding)
-// (wgrad: dW2 = dpre2^T col on the TN tcgen05 kernel; dgrad: dcol = dpre2 W2, then the gather below).
+// (wgrad: dW2 = dpre2^T col on the TN wgmma kernel; dgrad: dcol = dpre2 W2, then the gather below).
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) im2col_s2_kernel(const bf16* __restrict__ h1, bf16* __restrict__ col, int B, int T2,
                                                         int F2, int C, int T1p, int F1p) {

@@ -8,7 +8,7 @@
 //   ctc_grad_kernel        one CTA per (utterance, frame): d loss / d logit[k] = scale_b (softmax[k] - sum_{s: l_s = k}
 //                          exp(alpha_t(s) + beta_t(s) - logp[k] + nll_b)), scale_b = 1 / (B max(target_len_b, 1)) ('mean'
 //                          divides every utterance by its target length, then averages), zero for padded frames and for
-//                          infeasible utterances (zero_infinity).  bf16 output for the tcgen05 backward GEMMs.
+//                          infeasible utterances (zero_infinity).  bf16 output for the wgmma backward GEMMs.
 // HBM-bound integer/float work: the [B T', V] log-prob matrix is read once by each kernel.
 #include <math.h>
 

@@ -1,16 +1,16 @@
-// Persistent beam-search decode kernel for sm_100a, round 2: the WHOLE decode loop of SpeechToTextRecognizer.recognize
+// Persistent beam-search decode kernel for sm_90a: the WHOLE decode loop of SpeechToTextRecognizer.recognize
 // (otrans/recognize/speech2text.py:60-68 -> decode_step :95-153 -> TransformerDecoder.inference,
-// otrans/decoder/transformer.py:185-208) in ONE launch, GEMMs on tcgen05 tensor cores.
+// otrans/decoder/transformer.py:185-208) in ONE launch, GEMMs on wgmma tensor cores.
 //
 // Round 1 ran a decode step as 52 dependent kernels (7-13 us each for 2-4 us of work: 0.50 ms per beam step) or as one
 // cluster of 4 CTAs per utterance streaming ALL decoder weights through mma.sync for its 10 rows (830 MB of L2 traffic per
-// step).  This kernel keeps the rows of up to 12 utterances (beam 10 -> 120 hypotheses) together as ONE 128-row tcgen05
+// step).  This kernel keeps the rows of up to 12 utterances (beam 10 -> 120 hypotheses) together as ONE 128-row wgmma
 // tile and gives each such ROW GROUP to P = 16 co-operating CTAs:
 //
 //   * the wide projections are split over the group's CTAs by OUTPUT column (QKV: 48 columns per CTA; GLU: 128 hidden
 //     features per CTA) or, for w_2, by CONTRACTION slice (the CTA's own 128 hidden features; the 16 fp32 partial products are
-//     summed by a row-partitioned pass that also applies the residual and LayerNorm 3): tcgen05.mma 128 x N x 16, operands
-//     by TMA straight into the UMMA shared-memory layout, accumulators in TMEM, all 16 warps drain them;
+//     summed by a row-partitioned pass that also applies the residual and LayerNorm 3): the four warpgroups each form a 64-row x N/2
+//     quarter with wgmma, operands by TMA straight into the 128B-swizzled shared-memory layout, accumulators in registers;
 //   * the d x d projections between the attention cores (W_o, the cross-attention query projection, the second W_o) run on
 //     the OWNER of the rows: CTA j holds rows [8 j, 8 j + 8), streams the whole 128 KB weight matrix by TMA one phase ahead
 //     and forms the product transposed with mma.sync (weights = m16 operand, the 8 rows = n8 operand); bias + residual +
@@ -20,7 +20,7 @@
 //     into shared memory, online softmax per lane group; the context rows stay in shared memory for W_o;
 //   * cross-attention of the <= 16 hypotheses of an utterance against its <= 256 encoder frames is one m16 problem per
 //     (utterance, head), three per CTA, all three side by side on warp groups of 4: mma.sync on K / V tiles that TMA
-//     prefetches during the preceding barrier (tcgen05 has no M < 64 shape);
+//     prefetches during the preceding barrier (wgmma has no M < 64 shape);
 //   * activations cross CTAs through L2 at 6 group barriers per layer: QKV | self-attention + W_o + LN1 + W_q |
 //     cross-attention | W_o + LN2 | GLU + w_2 partial | reduction + LN3.  The group is launched as ONE thread-block cluster
 //     of 16 CTAs (barrier.cluster, release / acquire) or as plain CTAs with a release / acquire counter in L2
@@ -30,7 +30,7 @@
 //     log-softmax + per-row top-k (lane-maxima threshold), finished masking, beam^2 pruning, ancestry update -- follows
 //     beam.cu exactly (ties -> lower index), so ids / parents are bit-exact with the oracle's beam_step driven by this
 //     kernel's log-probs.
-// What each change bought, with the phase stamps behind it: profiles/r2_bench_history.md, DESIGN.md 4.4.
+// Design notes: DESIGN.md 4.4.
 //
 // Supported: post-norm decoder, GLU feed-forward with d_ff = 2048, d_model 256, 4 heads, beam <= 16, memory length <= 256
 // frames, max_len <= 128.  Anything else runs on the per-step graph path (recognize.BeamDecoder.step).
@@ -67,15 +67,11 @@ struct DgMisc {
     uint64_t a_full[4];       // A operand k-blocks landed (TMA from ctx / xbuf)
     uint64_t w1_full[4];      // W1 k-blocks landed
     uint64_t st_full[2];      // big stage landed
-    uint64_t st_empty[2];     // big stage consumed (tcgen05.commit)
-    uint64_t acc_full[2];     // accumulator complete (tcgen05.commit)
-    uint64_t acc_empty[2];    // (unused since v6: the CTA barrier behind a drained chunk frees the accumulator half)
     uint64_t pw_full[4];      // k-blocks of the out-projection weights (self-attention W_o, then cross-attention W_o) landed
     uint64_t pq_full[4];      // k-blocks of the cross-attention query projection landed
     uint64_t lg_full;         // logits rows of an utterance landed (TMA gather of the beam phase)
     uint64_t kx_full[3];      // encoder K/V tile of a cross-attention problem landed in stage 0 / stage 1 / the A tile
     uint64_t kv_full[32];     // self-attention: [row of the block][half-buffer] (16 used) -- 8 cached K rows + 8 V rows, all heads, landed (bulk copies)
-    uint32_t tmem_slot;
     int flag;                 // broadcast scratch
     alignas(16) uint32_t zero16[4];       // (unused since v22: the row-block projections have no padding rows any more)
     alignas(16) float bias[256];          // per-phase bias slice
@@ -158,10 +154,12 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     const CUtensorMap* map_x2 = maps + nl * 6 + 4;
     const CUtensorMap* map_lg = maps + nl * 6 + 5;
     int* bar = p.bar + g * 32;                        // 128-byte separated counters
-    const bool is_tma = (warp == 0 && lane == 0), is_mma = (warp == 1 && lane == 0);
-    const int equad = warp & 3;                       // TMEM lane quadrant this warp may read
-    const int ecg = warp >> 2;                        // column group of the warp in a 16-warp epilogue
-    const int erow = equad * 32 + lane;               // TMEM lane == tile row of an epilogue thread
+    const bool is_tma = (warp == 0 && lane == 0);
+    // wgmma tiles: the four warpgroups split a 128-row product into 64-row halves (mh) x column halves (nh); accumulator
+    // fragment of a thread: rows frow, frow + 8, columns 8 i + fcq + {0, 1} of its quarter
+    const int mh = (warp >> 2) & 1, nh = warp >> 3;
+    const int frow = mh * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int fcq = 2 * (lane & 3);
 
     if (tid == 0) {
         for (int i = 0; i < 4; ++i) {
@@ -174,9 +172,6 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         }
         for (int i = 0; i < 2; ++i) {
             mbar_init(&ms.st_full[i], 1);
-            mbar_init(&ms.st_empty[i], 1);
-            mbar_init(&ms.acc_full[i], 1);
-            mbar_init(&ms.acc_empty[i], 128);
         }
         mbar_init(&ms.lg_full, 1);
         for (int i = 0; i < 32; ++i) mbar_init(&ms.kv_full[i], 1);
@@ -184,15 +179,10 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         ms.flag = 0;
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&ms.tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = ms.tmem_slot;
-    const uint32_t t_row = tmem + ((uint32_t)(equad * 32) << 16);
 
     // parity of the NEXT completion of every mbarrier, tracked identically by all threads (every thread walks the same phases)
-    uint32_t par_kb = 0, par_a = 0, par_w1 = 0, par_stf = 0, par_ste = 0, par_accf = 0, par_pw = 0, par_pq = 0, par_lg = 0, par_kvw = 0, par_kx = 0;   // bit i = barrier i
+    uint32_t par_kb = 0, par_a = 0, par_w1 = 0, par_stf = 0, par_pw = 0, par_pq = 0, par_lg = 0, par_kvw = 0, par_kx = 0;   // bit i = barrier i
     int bar_target = 0;
 
     const bool dbg_cta = (p.dbg_clk != nullptr && blockIdx.x < DG_P && tid == 0);     // every CTA of group 0: [cta][256] stamps
@@ -207,8 +197,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     // thread between arrive and wait -- prefetches that do not depend on the other CTAs (weights, encoder K/V tiles); the
     // leading CTA barrier guarantees that every warp of THIS CTA is done with the shared memory those prefetches overwrite.
     // Launched as thread-block clusters of 16 (p.cluster) the group IS the cluster: hardware barrier.cluster with release /
-    // acquire semantics (~1-3 k cycles measured, profiles/r2_decode_phases_*.txt); otherwise one atomic + an acquire poll on a
-    // counter in L2 (~4 k cycles).
+    // acquire semantics; otherwise one atomic + an acquire poll on a counter in L2.
     int dbg_b = 0;      // group barriers since the start of the step; the six of layer 2 (12..17) get inner stamps (slots 212..229)
     auto gsync = [&](auto pre) {
         __syncthreads();
@@ -448,52 +437,44 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         v[3] = v[3] * rb * g1 + t1;
     };
 
-    // ---- small GEMM: acc[128 x nB] = A[128 x 256] * Bslice^T, B slice prefetched into sSB (kb_full).  a_map != null: A is fetched
-    // here by TMA (a_full), else it was built in shared memory by the CTA.  epi(c, r16) is called by the 128 epilogue threads for
-    // every 16-column chunk of their row.  Ends with a CTA barrier.
-    auto gemm_small = [&](int nB, const CUtensorMap* a_map, const float* bias, int b_row0, auto pre_epi, auto epi) {
+    // ---- small GEMM: acc[128 x 48] = A[128 x 256] * Bslice^T, B slice prefetched into sSB (kb_full).  a_map != null: A is fetched
+    // here by TMA (a_full), else it was built in shared memory by the CTA.  Each warpgroup forms a 64 x 24 quarter with wgmma;
+    // epi(row, col, v0, v1) is called for every pair of adjacent columns of the thread's accumulator fragment.  Ends with a
+    // CTA barrier.
+    auto gemm_small = [&](const CUtensorMap* a_map, const float* bias, int b_row0, auto epi) {
+        constexpr int nB = 48;
         if (tid < nB) ms.bias[tid] = bias[b_row0 + tid];
-        if (is_tma) {
-            if (a_map != nullptr) load_a(a_map);
-        } else if (is_mma) {
-            const uint32_t idesc = umma_idesc_bf16(nB);
-            for (int kb = 0; kb < 4; ++kb) {
-                mbar_wait(&ms.kb_full[kb], (par_kb >> kb) & 1);
-                if (a_map != nullptr) mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(sA + kb * 16384), b_addr = smem_u32(sSB + kb * nB * 128);
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_bf16(tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, (uint32_t)((kb | k) != 0));
-            }
-            umma_commit(&ms.acc_full[0]);
+        if (is_tma && a_map != nullptr) load_a(a_map);
+        // every operand wait precedes the wgmma chain: wgmma issued behind a divergent spin loop is serialised by ptxas
+        for (int kb = 0; kb < 4; ++kb) {
+            mbar_wait(&ms.kb_full[kb], (par_kb >> kb) & 1);
+            if (a_map != nullptr) mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
         }
-        __syncthreads();   // bias slice visible to the epilogue threads; the issuing lanes are back with their warps
-        // epilogue: warp w reads TMEM lanes [32 (w & 3), +32) (the hardware restriction) and the 16-column chunks w >> 2,
-        // (w >> 2) + 4, ...: the 48-column QKV slice is drained by 12 warps at once instead of 4 warps three times
-        if (ecg * 16 < nB) {
-            pre_epi();      // e.g. the residual slice: its L2 round trip overlaps the operand loads and the MMAs
-            mbar_wait(&ms.acc_full[0], par_accf & 1);
-            tc_fence_after();
-            for (int c = ecg * 16; c < nB; c += 64) {
-                uint32_t r[16];
-                tmem_ld16(t_row + c, r);
-                tmem_ld_wait();
-                epi(c, r);
-            }
-            tc_fence_before();
+        __syncwarp();
+        float acc[12];
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < 4; ++kb) {
+            const uint32_t a_addr = smem_u32(sA + kb * 16384) + mh * 8192, b_addr = smem_u32(sSB + kb * nB * 128) + nh * 24 * 128;
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                wgmma_n24<0, 0>(acc, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + k * 32), (uint32_t)((kb | k) != 0));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        __syncthreads();   // bias slice visible to every thread
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) epi(frow + 8 * hh, nh * 24 + i * 8 + fcq, acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
         }
         par_kb ^= 0xF;
         if (a_map != nullptr) par_a ^= 0xF;
-        par_accf ^= 1;
         __syncthreads();
     };
-    // Buffers that only this kernel reads back (w_2 partial products, logits) are stored in the order the TMEM epilogue produces
-    // them: [column group][row][16 bytes].  A thread owns a ROW of the accumulator, so its 16-byte pieces land next to the
-    // pieces of the neighbouring rows: every store instruction of a warp writes 512 contiguous bytes, with no shared-memory
-    // transpose (v4 staged 32 x 32 tiles through padded shared memory on 4 warps: 15 k cycles per layer for the partial
-    // products and 46 k per step for the logits before the barrier behind them opened).  The readers gather 16-byte pieces of
-    // consecutive rows, which are again contiguous.
+    // Buffers that only this kernel reads back (w_2 partial products, logits) are stored as [column group of 4][row][16 bytes]:
+    // the readers gather 16-byte pieces of consecutive rows, which are contiguous.
     const size_t part_slab = (size_t)64 * 128;          // uint4 per (contraction slice, group): 64 column groups x 128 rows
     const int ldv4 = p.ldv >> 2;
     uint4* lg4 = reinterpret_cast<uint4*>(p.logits) + (size_t)g * ldv4 * 128;     // this group's logits, [ldv / 4][128 rows] x 16 B
@@ -511,20 +492,15 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         for (int l = 0; l < nl; ++l) {
             const DgLayer& ly = p.layers[l];
             // ---------------- QKV projection of the newest token (attention.py:68-73): 48 of the 768 columns per CTA
-            gemm_small(48, l == 0 ? nullptr : map_x, ly.bqkv, j * 48, nop, [&](int c, const uint32_t (&r)[16]) {
-                if (erow >= nrows) return;
-                const int col = j * 48 + c;               // 16-column chunks never straddle the q | k | v boundaries
-                uint4 o[2];
-                uint32_t* ow = reinterpret_cast<uint32_t*>(o);
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    ow[i] = pack_bf16(__uint_as_float(r[2 * i]) + ms.bias[c + 2 * i], __uint_as_float(r[2 * i + 1]) + ms.bias[c + 2 * i + 1]);
+            gemm_small(l == 0 ? nullptr : map_x, ly.bqkv, j * 48, [&](int r, int c, float v0, float v1) {
+                if (r >= nrows) return;
+                const int col = j * 48 + c;               // column pairs never straddle the q | k | v boundaries
+                const uint32_t o = pack_bf16(v0 + ms.bias[c], v1 + ms.bias[c + 1]);
                 bf16* dst;
-                if (col < DG_D) dst = p.qbuf + (size_t)(row0 + erow) * DG_D + col;
-                else if (col < 2 * DG_D) dst = p.kc + kv_off(l, step, row0 + erow) + (col - DG_D);
-                else dst = p.vc + kv_off(l, step, row0 + erow) + (col - 2 * DG_D);
-                reinterpret_cast<uint4*>(dst)[0] = o[0];
-                reinterpret_cast<uint4*>(dst)[1] = o[1];
+                if (col < DG_D) dst = p.qbuf + (size_t)(row0 + r) * DG_D + col;
+                else if (col < 2 * DG_D) dst = p.kc + kv_off(l, step, row0 + r) + (col - DG_D);
+                else dst = p.vc + kv_off(l, step, row0 + r) + (col - 2 * DG_D);
+                *reinterpret_cast<uint32_t*>(dst) = o;
             });
             gsync([&] {      // first half of W_o streams in behind the self-attention (both stages are its K/V staging area)
                 for (int kb = 0; kb < 2; ++kb) load_proj_kb(maps + l * 6 + 1, ms.pw_full, kb, sA + kb * 32768);
@@ -923,93 +899,85 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
             if (is_tma) load_a(map_x2);
             {
                 if (tid < 256) ms.bias[tid] = ly.b1[(tid < 128 ? 0 : DG_DFF - 128) + j * 128 + tid];
-                if (is_mma) {
-                    const uint32_t idesc = umma_idesc_bf16(256);
-                    for (int kb = 0; kb < 4; ++kb) {
-                        mbar_wait(&ms.w1_full[kb], (par_w1 >> kb) & 1);
-                        mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
-                        tc_fence_after();
-                        const uint32_t a_addr = smem_u32(sA + kb * 16384);
-                        const uint32_t b_addr = smem_u32(sST + (kb >> 1) * DG_STAGE + (kb & 1) * 32768);
+                // W1: value and gate features [64 nh, 64 nh + 64) of this CTA's 128, rows [64 mh, +64), two wgmma 64 x 64 chains
+                float av[32], ag[32];
+                for (int kb = 0; kb < 4; ++kb) {
+                    mbar_wait(&ms.w1_full[kb], (par_w1 >> kb) & 1);
+                    mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
+                }
+                __syncwarp();
+                wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_bf16(tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, (uint32_t)((kb | k) != 0));
+                for (int kb = 0; kb < 4; ++kb) {
+                    const uint32_t a_addr = smem_u32(sA + kb * 16384) + mh * 8192;
+                    const uint32_t b_addr = smem_u32(sST + (kb >> 1) * DG_STAGE + (kb & 1) * 32768) + nh * 8192;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        wgmma_n64<0, 0>(av, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + k * 32), (uint32_t)((kb | k) != 0));
+                        wgmma_n64<0, 0>(ag, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + 16384 + k * 32), (uint32_t)((kb | k) != 0));
                     }
-                    umma_commit(&ms.acc_full[0]);
-                } else if (is_tma) {
-                    // W2[:, 128 j .. 128 j + 128) (this CTA's contraction slice) follows into stage 0 as soon as W1 has been consumed
-                    mbar_wait(&ms.acc_full[0], par_accf & 1);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs(av);
+                wgmma_fence_regs(ag);
+                __syncthreads();      // every warpgroup is done with x2 (A tile) and W1: both may be overwritten
+                if (is_tma) {
+                    // W2[:, 128 j .. 128 j + 128) (this CTA's contraction slice) follows into stage 0
                     mbar_arrive_expect_tx(&ms.st_full[0], 65536);
                     tma_load_2d_hint(sST, maps + l * 6 + 5, &ms.st_full[0], j * 128, 0, TMA_EVICT_LAST);
                     tma_load_2d_hint(sST + 32768, maps + l * 6 + 5, &ms.st_full[0], j * 128 + 64, 0, TMA_EVICT_LAST);
                 }
-                __syncthreads();
-                {
-                    mbar_wait(&ms.acc_full[0], par_accf & 1);
-                    tc_fence_after();
-                    // h = (a + b_a) * sigmoid(g + b_g) -> bf16, written over the (dead) A tile as a [128 x 128] K-major operand;
-                    // all 16 warps: warp w takes rows [32 (w & 3), +32) and hidden features [32 (w >> 2), +32)
-                    const bool glu4 = (p.flags & 1) != 0;      // A/B switch (OTB_DG_FLAGS=1): the v5 epilogue on warps 4-7 only
-                    const int gc0 = glu4 ? (ecg == 1 ? 0 : 128) : ecg * 32, gc1 = glu4 ? 128 : ecg * 32 + 32;
-#pragma unroll 1
-                    for (int c = gc0; c < gc1; c += 16) {
-                        uint32_t ra[16], rg[16];
-                        tmem_ld16(t_row + c, ra);
-                        tmem_ld16(t_row + 128 + c, rg);
-                        tmem_ld_wait();
-                        uint4 o[2];
-                        uint32_t* ow = reinterpret_cast<uint32_t*>(o);
+                // h = (a + b_a) * sigmoid(g + b_g) -> bf16, written over the (dead) A tile as a [128 x 128] K-major operand
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const float a0 = __uint_as_float(ra[2 * i]) + ms.bias[c + 2 * i], a1 = __uint_as_float(ra[2 * i + 1]) + ms.bias[c + 2 * i + 1];
-                            const float g0 = __uint_as_float(rg[2 * i]) + ms.bias[128 + c + 2 * i], g1 = __uint_as_float(rg[2 * i + 1]) + ms.bias[128 + c + 2 * i + 1];
-                            ow[i] = pack_bf16(a0 * dg_sigmoid(g0), a1 * dg_sigmoid(g1));
-                        }
-                        const int c8 = c >> 3;
-                        *reinterpret_cast<uint4*>(sA + (c8 >> 3) * 16384 + sw128(erow, c8 & 7)) = o[0];
-                        *reinterpret_cast<uint4*>(sA + ((c8 + 1) >> 3) * 16384 + sw128(erow, (c8 + 1) & 7)) = o[1];
+                for (int i = 0; i < 8; ++i) {
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const int f = nh * 64 + i * 8 + fcq, r = frow + 8 * hh;
+                        const float a0 = av[4 * i + 2 * hh] + ms.bias[f], a1 = av[4 * i + 2 * hh + 1] + ms.bias[f + 1];
+                        const float g0 = ag[4 * i + 2 * hh] + ms.bias[128 + f], g1 = ag[4 * i + 2 * hh + 1] + ms.bias[128 + f + 1];
+                        *reinterpret_cast<uint32_t*>(sA + (f >> 6) * 16384 + sw128(r, (f & 63) >> 3) + (f & 7) * 2) =
+                            pack_bf16(a0 * dg_sigmoid(g0), a1 * dg_sigmoid(g1));
                     }
-                    tc_fence_before();
-                    fence_proxy_async_smem();
                 }
+                fence_proxy_async_smem();
                 par_w1 ^= 0xF;
                 par_a ^= 0xF;
-                par_accf ^= 1;
                 __syncthreads();
                 DG_STAMP();   // W1 + GLU
-                // w_2 partial: acc2[128 x 256] = h[128 x 128] * W2[:, slice]^T   (TMEM columns 256..511)
-                if (is_mma) {
-                    const uint32_t idesc = umma_idesc_bf16(256);
-                    mbar_wait(&ms.st_full[0], par_stf & 1);
-                    tc_fence_after();
-                    for (int kb = 0; kb < 2; ++kb) {
-                        const uint32_t a_addr = smem_u32(sA + kb * 16384), b_addr = smem_u32(sST + kb * 32768);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_bf16(tmem + 256, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, (uint32_t)((kb | k) != 0));
-                    }
-                    umma_commit(&ms.acc_full[1]);
-                }
-                __syncwarp();
+                // w_2 partial: acc2[128 x 256] = h[128 x 128] * W2[:, slice]^T; warpgroup (mh, nh): rows [64 mh, +64) x columns [128 nh, +128)
                 {
-                    // fp32 partial products; warp w: rows [32 (w & 3), +32), columns [64 (w >> 2), +64) as 16 pieces of 4 columns
-                    mbar_wait(&ms.acc_full[1], (par_accf >> 1) & 1);
-                    tc_fence_after();
-                    uint4* dst = reinterpret_cast<uint4*>(p.part) + ((size_t)j * p.G + g) * part_slab + (size_t)(ecg * 16) * 128 + erow;
+                    mbar_wait(&ms.st_full[0], par_stf & 1);
+                    // fp32 partial products in the [column group of 4][row] order the reduction reads; two 64-column passes
+                    // keep the accumulator within the register budget of 512 threads
+                    float* dst = reinterpret_cast<float*>(p.part) + ((size_t)j * p.G + g) * part_slab * 4;
 #pragma unroll 1
-                    for (int hq = 0; hq < 2; ++hq) {
-                        uint32_t r[32];
-                        tmem_ld32(t_row + 256 + ecg * 64 + hq * 32, r);
-                        tmem_ld_wait();
-                        if (erow < nrows) {
+                    for (int hb = 0; hb < 2; ++hb) {
+                        float pc[32];
+                        __syncwarp();
+                        wgmma_fence();
 #pragma unroll
-                            for (int q = 0; q < 8; ++q) dst[(size_t)(hq * 8 + q) * 128] = make_uint4(r[4 * q], r[4 * q + 1], r[4 * q + 2], r[4 * q + 3]);
+                        for (int kb = 0; kb < 2; ++kb) {
+                            const uint32_t a_addr = smem_u32(sA + kb * 16384) + mh * 8192;
+                            const uint32_t b_addr = smem_u32(sST + kb * 32768) + nh * 16384 + hb * 8192;
+#pragma unroll
+                            for (int k = 0; k < 4; ++k)
+                                wgmma_n64<0, 0>(pc, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + k * 32), (uint32_t)((kb | k) != 0));
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        wgmma_fence_regs(pc);
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) {
+#pragma unroll
+                            for (int hh = 0; hh < 2; ++hh) {
+                                const int c = nh * 128 + hb * 64 + i * 8 + fcq, r = frow + 8 * hh;
+                                if (r < nrows) *reinterpret_cast<float2*>(dst + ((size_t)(c >> 2) * 128 + r) * 4 + (c & 3)) = make_float2(pc[4 * i + 2 * hh], pc[4 * i + 2 * hh + 1]);
+                            }
                         }
                     }
-                    tc_fence_before();
                 }
                 par_stf ^= 1;
-                par_accf ^= 2;
             }
             const bool last_layer = (l + 1 == nl);
             gsync([&] {
@@ -1085,70 +1053,49 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         {
             int my_chunks = 0;
             for (int c = j; c < n_vchunks; c += DG_P) ++my_chunks;
-            const uint32_t idesc = umma_idesc_bf16(128);
-            auto issue_chunk = [&](int i) {      // MMA thread: chunk i -> TMEM columns [128 (i & 1), +128)
-                const int s = i & 1;
-                mbar_wait(&ms.st_full[s], ((par_stf >> s) & 1) ^ (uint32_t)((i >> 1) & 1));
-                tc_fence_after();
-                for (int kb = 0; kb < 4; ++kb) {
-                    const uint32_t a_addr = smem_u32(sA + kb * 16384), b_addr = smem_u32(sST + s * DG_STAGE + kb * 16384);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        umma_bf16(tmem + s * 128, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, (uint32_t)((kb | k) != 0));
-                }
-                umma_commit(&ms.st_empty[s]);
-                umma_commit(&ms.acc_full[s]);
-            };
-            if (is_tma) {
-                load_a(map_x);
-            } else if (is_mma) {
-                for (int kb = 0; kb < 4; ++kb) mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
-                if (my_chunks > 0) issue_chunk(0);
-            }
-            // All 16 warps drain a chunk: warp w stores rows [32 (w & 3), +32) x columns [32 (w >> 2), +32) as eight 16-byte pieces
-            // per row in the [column group][row] order (512 contiguous bytes per warp instruction).  The MMAs of chunk i + 1 are
-            // issued before chunk i is drained (other TMEM half); the CTA barrier at the end of an iteration is what frees a half.
+            if (is_tma) load_a(map_x);
+            __syncwarp();
+            for (int kb = 0; kb < 4; ++kb) mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
+            // chunk i: wgmma 64 x 64 per warpgroup (rows [64 mh, +64), columns [64 nh, +64) of the chunk), logits + bias stored in the
+            // [column group][row] order (columns [V, ldv) as -inf: no bounds checks in the readers); the weights of chunk i + 2
+            // stream into the stage as soon as every warpgroup has multiplied chunk i
             for (int i = 0; i < my_chunks; ++i) {
                 const int s = i & 1;
                 const int col0 = (j + i * DG_P) * 128;
                 if (tid < 128) ms.bias[s * 128 + tid] = (p.bout != nullptr && col0 + tid < V) ? p.bout[col0 + tid] : 0.f;
-                if (is_mma && i + 1 < my_chunks) issue_chunk(i + 1);
-                if (is_tma && i + 2 < my_chunks) {        // chunks 0 and 1 were prefetched; stage s is free once chunk i has been multiplied
-                    mbar_wait(&ms.st_empty[s], ((par_ste >> s) & 1) ^ (uint32_t)((i >> 1) & 1));
-                    load_wout(j + (i + 2) * DG_P, s);
-                }
-                __syncthreads();
-                mbar_wait(&ms.acc_full[s], ((par_accf >> s) & 1) ^ (uint32_t)((i >> 1) & 1));
-                tc_fence_after();
-                const int cc0 = col0 + ecg * 32;
-                if (cc0 < p.ldv) {
-                    uint32_t r[32];
-                    tmem_ld32(t_row + s * 128 + ecg * 32, r);
-                    tmem_ld_wait();
-                    if (erow < nrows) {
-                        const float* bs = ms.bias + s * 128 + ecg * 32;
-                        uint4* dst = lg4 + (size_t)(cc0 >> 2) * 128 + erow;
-                        const bool full32 = cc0 + 32 <= V;     // warp-uniform; columns [V, ldv) are stored as -inf (no bounds checks in the readers)
+                mbar_wait(&ms.st_full[s], ((par_stf >> s) & 1) ^ (uint32_t)((i >> 1) & 1));
+                float lc[32];
+                __syncwarp();
+                wgmma_fence();
 #pragma unroll
-                        for (int q = 0; q < 8; ++q) {
-                            uint4 o;
-                            o.x = (full32 || cc0 + 4 * q < V) ? __float_as_uint(__uint_as_float(r[4 * q]) + bs[4 * q]) : 0xff800000u;
-                            o.y = (full32 || cc0 + 4 * q + 1 < V) ? __float_as_uint(__uint_as_float(r[4 * q + 1]) + bs[4 * q + 1]) : 0xff800000u;
-                            o.z = (full32 || cc0 + 4 * q + 2 < V) ? __float_as_uint(__uint_as_float(r[4 * q + 2]) + bs[4 * q + 2]) : 0xff800000u;
-                            o.w = (full32 || cc0 + 4 * q + 3 < V) ? __float_as_uint(__uint_as_float(r[4 * q + 3]) + bs[4 * q + 3]) : 0xff800000u;
-                            dst[(size_t)q * 128] = o;
-                        }
+                for (int kb = 0; kb < 4; ++kb) {
+                    const uint32_t a_addr = smem_u32(sA + kb * 16384) + mh * 8192, b_addr = smem_u32(sST + s * DG_STAGE + kb * 16384) + nh * 8192;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        wgmma_n64<0, 0>(lc, gmma_desc_sw128(a_addr + k * 32), gmma_desc_sw128(b_addr + k * 32), (uint32_t)((kb | k) != 0));
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs(lc);
+                __syncthreads();      // stage s consumed by every warpgroup; bias slice visible
+                if (is_tma && i + 2 < my_chunks) load_wout(j + (i + 2) * DG_P, s);
+                float* lgf = reinterpret_cast<float*>(lg4);
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const int cl = nh * 64 + q * 8 + fcq, c = col0 + cl, r = frow + 8 * hh;
+                        if (r >= nrows || c >= p.ldv) continue;
+                        const float o0 = (c < V) ? lc[4 * q + 2 * hh] + ms.bias[s * 128 + cl] : -INFINITY;
+                        const float o1 = (c + 1 < V) ? lc[4 * q + 2 * hh + 1] + ms.bias[s * 128 + cl + 1] : -INFINITY;
+                        *reinterpret_cast<float2*>(lgf + ((size_t)(c >> 2) * 128 + r) * 4 + (c & 3)) = make_float2(o0, o1);
                     }
                 }
-                tc_fence_before();
-                __syncthreads();
             }
             // parity bookkeeping: barrier pair s was used ceil((my_chunks - s) / 2) times
             const uint32_t u0n = (uint32_t)((my_chunks + 1) >> 1), u1n = (uint32_t)(my_chunks >> 1);
             par_a ^= 0xF;
             par_stf ^= (u0n & 1) | ((u1n & 1) << 1);
-            par_ste ^= (u0n & 1) | ((u1n & 1) << 1);
-            par_accf ^= (u0n & 1) | ((u1n & 1) << 1);
         }
         gsync(nop);
         DG_STAMP();
@@ -1406,7 +1353,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         if (group_done) break;      // every hypothesis of every utterance of this group ended (uniform across the group)
     }
     // drain the QKV-weight prefetch that was issued for a step that will not run
-    if (is_mma)
+    if (is_tma)
         for (int kb = 0; kb < 4; ++kb) mbar_wait(&ms.kb_full[kb], (par_kb >> kb) & 1);
 
     // A group that ended early keeps emitting EOS from its (sorted) hypotheses with identity parents while the reference loops
@@ -1423,12 +1370,6 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
             atomicMax(&p.st.ctrl[0], group_done ? steps_done : p.max_steps);
             if (!group_done) atomicAdd(&p.st.ctrl[2], 1);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 512);
     }
 #undef DG_STAMP
 #undef DG_STAMP2
@@ -1532,12 +1473,13 @@ const char* decode_group_launch(cudaStream_t st, const MegaParams& mp, void* wor
         }
         attr_set = true;
     }
-    // Preferred launch: one thread-block CLUSTER of 16 CTAs per row group (non-portable cluster size; a B200 GPC holds 16-20
-    // SMs, so up to 8 such clusters are co-resident): the group barrier becomes barrier.cluster (hardware, ~0.3 us, and the
+    // Preferred launch: one thread-block CLUSTER of 16 CTAs per row group (non-portable cluster size; a GPC holds about
+    // 16-18 SMs, so at most one such cluster per GPC is co-resident): the group barrier becomes barrier.cluster (hardware, ~0.3 us, and the
     // CTAs of a group are co-scheduled by construction).  OTB_DG_CLUSTER=0, or a device that refuses the cluster shape, falls
     // back to the software barrier on a counter in L2 (plain launch; needs G * 16 <= #SMs co-resident CTAs).  A GPC fits ONE
-    // such cluster, so at most 8 groups (2 batches of 32 utterances) run at a time under clusters; a server that keeps 3 batches
-    // in flight (144 CTAs) selects the software barrier with otb_set_decode_barrier(0): +15-20 % throughput, +10 % latency.
+    // such cluster, so at most 8 groups run at a time under clusters.  The software barrier spins: it is only safe when every
+    // CTA of every batch in flight (all streams together) is resident at once, e.g. 2 batches of 32 utterances (96 CTAs) on a
+    // 132-SM H100.
     if (cluster_ok < 0) {
         const char* e_ = getenv("OTB_DG_CLUSTER");
         cluster_ok = (e_ && e_[0] == '0') ? 0 : 1;
@@ -1562,8 +1504,11 @@ const char* decode_group_launch(cudaStream_t st, const MegaParams& mp, void* wor
             }
         }
     }
+    // an explicit request for clusters is never served by the spinning software barrier: the caller may keep more CTAs in
+    // flight than can be resident at once, which only gang-scheduled clusters tolerate
+    if (g_dg_barrier == 1 && !cluster_ok) return "decode_persistent: thread-block clusters of 16 are not available on this device";
     const int use_cluster = (cluster_ok && g_dg_barrier != 0) ? 1 : 0;
-    const int Gpad = (p.flags & 128) ? (G > 10 ? G : 10) : G;      // experiment: a grid of >= 148 CTAs (the padding CTAs return at once)
+    const int Gpad = (p.flags & 128) ? (G > 10 ? G : 10) : G;      // experiment: a grid of >= 160 CTAs (the padding CTAs return at once)
     p.cluster = use_cluster;
     if (use_cluster) {
         cudaLaunchConfig_t cfg;

@@ -1,4 +1,4 @@
-// tcgen05 GEMM for sm_100a:  C[M,N] = A[M,K] * W[N,K]^T  (bf16 operands, fp32 accumulate in TMEM)
+// wgmma GEMM for sm_90a:  C[M,N] = A[M,K] * W[N,K]^T  (bf16 operands, fp32 accumulate in registers)
 // with the fused epilogues the speech-transformer hot path needs (bias / ReLU / GLU / x*sqrt(d)+PE /
 // residual / residual+LayerNorm / swish / gelu / tanh) and an implicit-GEMM mode for the 3x3 stride-2
 // Conv2d subsampling layer (A gathered by a 5-D TMA tensor map, one 64-channel tap per k-block).
@@ -7,22 +7,19 @@
 //   otrans/module/attention.py:68,128-129,44   otrans/module/ffn.py:39-41
 //   otrans/frontend/conv.py:63-64,146          otrans/decoder/transformer.py:181
 //
-// Structure (persistent, one CTA per SM, 640 threads):
-//   warp 0 lane 0 : TMA producer   (A tile 128x64, B tile BNx64 per k-block, SWIZZLE_128B)
-//   warp 1 lane 0 : tcgen05.mma issuer (UMMA 128 x BN x 16, 4 per k-block), tcgen05.commit -> mbarriers
-//   warp 2        : TMEM allocator (2 accumulator stages x BN columns)
-//   warps 4..19   : epilogue, four warpgroups: warp w reads TMEM lanes 32*(w%4).., warpgroup (w-4)/4 takes
-//                   one quarter of the tile's columns.  tcgen05.ld -> registers -> fused math (bias / LN
-//                   parameters broadcast from smem) -> staged in smem -> coalesced 16-byte global stores
-//                   (one full output row segment per warp instruction; the residual tile is fetched the
-//                   same way).  Round-1 profile: per-thread row stores were 32 sectors/request and the
-//                   epilogue, not the MMA, bounded every GEMM (profiles/r1_*).
-// Residual + LayerNorm epilogue (N = d_model <= 256): the output row is split over a thread-block CLUSTER
-// of N/64 CTAs (64 columns each); per-row partial (sum, sum of squares) are exchanged through distributed
-// shared memory (st.shared::cluster + remote mbarrier arrive), so the LN-fused GEMMs run on 4x more SMs
-// than a one-CTA-per-row-block tiling would (63 -> 252 CTAs at cfg 2, 3 -> 12 in the decode loop).
-// Three pipelines: smem full/empty ring (TMA <-> MMA), TMEM full/empty (MMA <-> epilogue), static
-// round-robin tile scheduler, so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Structure (persistent, one CTA per SM, NWG consumer warpgroups + one producer warp):
+//   last warp, lane 0  : TMA producer (A tile BMx64, B tile BNx64 per k-block, SWIZZLE_128B) into a STAGES-deep
+//                        full/empty mbarrier ring
+//   warpgroups 0..NWG-1: consumers, warpgroup c owns tile rows [64 c, 64 c + 64): wgmma 64 x BN x 16 per k-block with
+//                                one k-block in flight, accumulator in registers; then the fused epilogue on the accumulator
+//                                fragment -> staged rows in smem -> coalesced 16-byte global stores (one full output row
+//                                segment per warp instruction; the residual tile is fetched the same way, before the main
+//                                loop, so its latency overlaps the MMAs).
+// Residual + LayerNorm epilogue (N = d_model <= 256): the tile spans the whole row, the row statistics are reduced over
+// the four lanes that share an accumulator row.  BN <= 128: two consumer warpgroups, 128-row tiles; BN = 256 (only the
+// d_model = 256 LayerNorm GEMM): one consumer warpgroup with 64-row tiles, so that its 128 accumulator registers per
+// thread fit (a CTA of 288 threads is allocated registers like one of 384: at most 168 per thread).  Static round-robin tile scheduler; the producer runs ahead into the next
+// tile while the consumers drain the current one.
 #include <stdlib.h>
 #include <string.h>
 
@@ -36,69 +33,66 @@ namespace otb {
 int g_tile_policy = 0;   // otb_set_tile_policy: 0 = lowest latency of a lone launch, 1 = least SM-time (concurrent batches)
 unsigned long long* g_gemm_dbg = nullptr;
 int g_gemm_dbg_mode = 0;
+// debug buffer layout (otb_debug_gemm_timing): [256 CTAs][8] phase stamps, then per-k-block traces of the first tile
+static constexpr int DBG_CTAS = 256;
 #define DBG_STAMP(i) do { if (p.dbg) p.dbg[blockIdx.x * 8 + (i)] = clock64(); } while (0)
-// per-k-block traces of the first tile: kind 0 = TMA issue, 1 = full barrier observed by the MMA thread
-#define DBG_KB(kind, kb) do { if (p.dbg && (kb) < 64) p.dbg[148 * 8 + (blockIdx.x * 2 + (kind)) * 64 + (kb)] = clock64(); } while (0)
-
-// epilogue sub-phase stamps of the SECOND tile of every CTA (steady state): [148*8 + 148*2*64 + cta*16 + i]
-#define DBG_EPI(i) do { if (p.dbg && it == 1 && et == 0) p.dbg[148 * 8 + 148 * 2 * 64 + blockIdx.x * 16 + (i)] = clock64(); } while (0)
+// per-k-block traces of the first tile: kind 0 = TMA issue, 1 = full barrier observed by the consumers
+#define DBG_KB(kind, kb) do { if (p.dbg && (kb) < 64) p.dbg[DBG_CTAS * 8 + (blockIdx.x * 2 + (kind)) * 64 + (kb)] = clock64(); } while (0)
 
 static constexpr int BM = 128;
 static constexpr int BK = 64;
-static constexpr int kThreads = 640;
-static constexpr int kEpiThreads = 512;
 static constexpr int STG_PITCH_MAX = 512 + 16;          // bytes per staged row (+16 B pad: conflict-free 16 B accesses)
 static constexpr int STG_BYTES = BM * STG_PITCH_MAX;    // 67,584
-static constexpr int AUX_BYTES = 6144 + 8192;           // barriers, TMEM slot, bias / gamma / beta, row map | LN stats (wide tiles)
+static constexpr int AUX_BYTES = 6144;                  // barriers, bias / gamma / beta, row map
 
 template <int BN>
 struct GemmCfg {
+    static constexpr int NWG = (BN == 256) ? 1 : 2;    // consumer warpgroups
+    static constexpr int BM = 64 * NWG;                // tile rows
+    static constexpr int THREADS = 128 * NWG + 32;
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int STAGES = (BN == 256) ? 3 : (BN == 128 ? 4 : 6);
-    static constexpr int TMEM_COLS = 2 * BN;  // power of two for BN in {64,128,256}
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + AUX_BYTES + 1024;
 };
+static_assert(GemmCfg<256>::SMEM_BYTES <= 227 * 1024, "gemm_tc_kernel: shared-memory budget (227 KB per CTA)");
 
 // sigmoid(x) = 0.5 * tanh(x / 2) + 0.5 with ONE MUFU op (tanh.approx, |rel err| ~ 2^-11, far below the bf16 output
-// rounding) instead of ex2 + rcp: the GLU epilogue of the K = 256 GEMMs is MUFU-bound (32 K sigmoids per 128x128 tile).
+// rounding) instead of ex2 + rcp: the GLU epilogue of the K = 256 GEMMs is MUFU-bound.
 __device__ __forceinline__ float fast_sigmoid(float x) {
     float t;
     asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
     return fmaf(0.5f, t, 0.5f);
 }
 
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 512;" ::: "memory"); }
+template <int NT>
+__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
 
-// 16 fp32 values -> staged row (bf16 or f32), 16-byte shared stores
-__device__ __forceinline__ void stage16(uint8_t* row_ptr, int col, int out_f32, const float (&v)[16]) {
-    if (out_f32) {
-        float4* d = reinterpret_cast<float4*>(row_ptr + col * 4);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) d[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-    } else {
-        uint4* d = reinterpret_cast<uint4*>(row_ptr + col * 2);
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            uint4 u;
-            u.x = pack_bf16(v[8 * i], v[8 * i + 1]);
-            u.y = pack_bf16(v[8 * i + 2], v[8 * i + 3]);
-            u.z = pack_bf16(v[8 * i + 4], v[8 * i + 5]);
-            u.w = pack_bf16(v[8 * i + 6], v[8 * i + 7]);
-            d[i] = u;
-        }
-    }
+// one k16 step of the warpgroup's 64 x BN accumulator
+template <int BN, int T>
+__device__ __forceinline__ void mma_bn(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t acc) {
+    if constexpr (BN == 64) wgmma_n64<T, T>(d, a, b, acc);
+    else if constexpr (BN == 128) wgmma_n128<T, T>(d, a, b, acc);
+    else wgmma_n256<T, T>(d, a, b, acc);
+}
+
+// two adjacent output values -> staged row (bf16 pair or two floats)
+__device__ __forceinline__ void stage2(uint8_t* row_ptr, int col, int out_f32, float a, float b) {
+    if (out_f32) *reinterpret_cast<float2*>(row_ptr + col * 4) = make_float2(a, b);
+    else *reinterpret_cast<uint32_t*>(row_ptr + col * 2) = pack_bf16(a, b);
 }
 
 // TN = true: weight-gradient mode, C[M,N] = A^T B with A = dY [K rows, M cols] and B = X [K rows, N cols], both row-major,
 // i.e. both operands are MN-major in shared memory (64x64 TMA boxes, LBO = 8 KB between 64-wide MN groups, SBO = 1 KB
 // between 8-row K groups).  p.splitk > 1 splits the contraction over `splitk` tiles that accumulate with fp32 atomics.
 template <int BN, int EPI, bool TN = false>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(GemmCfg<BN>::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
     using Cfg = GemmCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
+    constexpr int BM = Cfg::BM;
+    constexpr int kEpiThreads = 128 * Cfg::NWG;
     constexpr int BN_OUT = (EPI == EPI_GLU) ? BN / 2 : BN;  // output columns per tile
 
     extern __shared__ uint8_t smem_raw[];
@@ -107,21 +101,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint8_t* aux = stg + STG_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tfull_bar = empty_bar + STAGES;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint64_t* ln_bar = tempty_bar + 2;                     // [2] cluster LayerNorm statistics exchange (alternate per tile)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ln_bar + 2);
     float* s_bias = reinterpret_cast<float*>(aux + 256);   // [256]  (GLU: value half | gate half)
     float* s_gamma = s_bias + 256;                          // [256]
     float* s_beta = s_gamma + 256;                          // [256]
     int* s_rowmap = reinterpret_cast<int*>(s_beta + 256);   // [128] output row of each tile row, -1 = skip
-    // LN partial statistics [2 tile parities][cluster ranks * 4 quarters <= 16][128 rows]: in the upper part of the
-    // staging buffer when the LN tile is 64 wide (staging needs 128 x 144 B), else (one CTA per row block, at most
-    // 4 partials per parity) in the pipeline-stage area's tail
-    float2* s_stats = (BN == 64) ? reinterpret_cast<float2*>(stg + 32768)
-                                 : (BN == 128 ? reinterpret_cast<float2*>(stg + 36864) : reinterpret_cast<float2*>(aux + 6144));   // BN 128: 2 x 8 x 128 partials = 16 KB above the 34 KB of staged rows
-    const uint32_t cl_rank = (EPI == EPI_RESID_LN) ? cluster_ctarank() : 0;
-    const uint32_t cl_size = (EPI == EPI_RESID_LN) ? cluster_nctarank() : 1;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -175,428 +158,299 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
     };
 
-    // Producer state (meaningful in warp 0 lane 0 only): next load = (p_tile, p_kb) into p_stage.
-    int p_tile = blockIdx.x, p_kb = kb_begin(blockIdx.x), p_stage = 0;
-    uint32_t p_phase = 0;
-    if (warp == 0) {
-        if (lane == 0) {
-            tma_prefetch_desc(&tmA);
-            tma_prefetch_desc(&tmB);
-            for (int i = 0; i < STAGES; ++i) {
-                mbar_init(&full_bar[i], 1);
-                mbar_init(&empty_bar[i], 1);
-            }
-            for (int i = 0; i < 2; ++i) {
-                mbar_init(&tfull_bar[i], 1);
-                mbar_init(&tempty_bar[i], kEpiThreads);
-            }
-            mbar_init(&ln_bar[0], 1);
-            mbar_init(&ln_bar[1], 1);
-            fence_barrier_init();
-            PDL_WAIT();   // predecessor grid complete: its outputs (our A operand) may now be fetched
-            // the first STAGES slots are free by construction: start the loads before the CTA-wide sync so
-            // their latency overlaps the TMEM allocation
-            for (int i = 0; i < STAGES && p_tile < num_tiles; ++i) {
-                issue_load(p_tile, p_kb, p_stage);
-                if (i == 0) DBG_STAMP(2);
-                if (p_tile == (int)blockIdx.x) DBG_KB(0, p_kb);
-                if (++p_kb >= kb_end(p_tile)) { p_tile += gridDim.x; p_kb = kb_begin(p_tile); }
-                if (++p_stage == STAGES) { p_stage = 0; p_phase ^= 1; }
-            }
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmA);
+        tma_prefetch_desc(&tmB);
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], Cfg::NWG);   // one arrival per consumer warpgroup
         }
-        __syncwarp();
+        fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    PDL_WAIT();   // every thread, before its first global access (barrier init / TMEM allocation above overlap the predecessor)
-    if (EPI == EPI_RESID_LN && cl_size > 1) cluster_sync_all();  // peers' mbarriers exist before any remote arrive
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    PDL_WAIT();   // predecessor grid complete: its outputs (our A operand, residual) may now be read
     if (threadIdx.x == 0) DBG_STAMP(1);
 
-    if (warp == 0) {
+    if (warp == 4 * Cfg::NWG) {
         // ------------------------------------------------------------------ TMA producer (lane 0)
         if (lane == 0) {
-            while (p_tile < num_tiles) {
-                mbar_wait(&empty_bar[p_stage], p_phase ^ 1);
-                issue_load(p_tile, p_kb, p_stage);
-                if (p_tile == (int)blockIdx.x) DBG_KB(0, p_kb);
-                if (++p_kb >= kb_end(p_tile)) { p_tile += gridDim.x; p_kb = kb_begin(p_tile); }
-                if (++p_stage == STAGES) { p_stage = 0; p_phase ^= 1; }
+            int stage = 0;
+            uint32_t phase = 0;
+            bool first = true;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                for (int kb = kb_begin(tile), kb1 = kb_end(tile); kb < kb1; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    issue_load(tile, kb, stage);
+                    if (first) { DBG_STAMP(2); first = false; }
+                    if (tile == (int)blockIdx.x) DBG_KB(0, kb);
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (lane 0)
-        constexpr uint32_t idesc = umma_idesc_bf16(BN, TN, 128, TN);
-        if (lane == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-            const int as = it & 1;
-            const uint32_t aph = (it >> 1) & 1;
-            mbar_wait(&tempty_bar[as], aph ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(as * BN);
-            const int kb0 = kb_begin(tile), kb1 = kb_end(tile);
-            for (int kb = kb0; kb < kb1; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                if (it == 0 && kb == kb0) DBG_STAMP(3);
-                if (it == 0) DBG_KB(1, kb);
-                const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                const uint32_t b_addr = a_addr + Cfg::A_BYTES;
-                if (p.dbg_mode != 2) {
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        if (TN)   // MN-major operands: one k16 step = 16 rows of 128 B
-                            umma_bf16(d_tmem, umma_desc_sw128(a_addr + k * 2048, 1024, 8192),
-                                      umma_desc_sw128(b_addr + k * 2048, 1024, 8192), idesc, (uint32_t)(((kb - kb0) | k) != 0));
-                        else
-                            umma_bf16(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc,
-                                      (uint32_t)((kb | k) != 0));
-                    }
-                }
-                umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs have read it
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(&tfull_bar[as]);  // accumulator complete -> epilogue
-            if (it == 0) DBG_STAMP(4);
+        return;
+    }
+
+    // ------------------------------------------------------------------ consumers (256 threads, 2 warpgroups)
+    const int et = threadIdx.x;             // consumer thread
+    const int cw = et >> 7;                 // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
+    const int ewarp = et >> 5;              // 0..7
+    const int rl0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's accumulator rows: rl0, rl0 + 8
+    const int cq = 2 * (lane & 3);                              // its columns in every 8-column group: cq, cq + 1
+    const int esize = p.out_f32 ? 4 : 2;
+    const int pitch = BN_OUT * esize + 16;
+
+    if (EPI == EPI_RESID_LN) {  // LayerNorm affine parameters (the tile spans the whole row)
+        for (int i = et; i < BN; i += kEpiThreads) {
+            s_gamma[i] = p.gamma[i];
+            s_beta[i] = p.beta[i];
         }
+    }
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        const int mn_ = TN ? tile / splitk : tile;
+        const int m_blk = mn_ / n_tiles, n_blk = mn_ % n_tiles;
+        const int col_base = n_blk * BN_OUT;             // first output column of the tile
+        const int ncols = min(BN_OUT, p.N - col_base);   // valid output columns
+
+        // ---- (a) per-tile smem setup: bias slice, row map, residual tile (all coalesced, loads batched)
+        for (int i = et; i < BN; i += kEpiThreads) {
+            int c;
+            if (EPI == EPI_GLU) c = (i < BN_OUT) ? col_base + i : p.N + col_base + (i - BN_OUT);
+            else c = col_base + i;
+            const bool ok = (EPI == EPI_GLU) ? ((i % BN_OUT) < ncols) : (i < ncols);
+            s_bias[i] = (p.bias != nullptr && ok) ? p.bias[c] : 0.f;
         }
-        __syncwarp();
-    } else if (warp >= 4) {
-        // ------------------------------------------------------------------ epilogue (512 threads, 16 warps)
-        // warp w reads TMEM lanes 32*(w%4)..; the four warpgroups split the tile's columns into quarters and
-        // walk them in 16-column chunks (4 warps per SM sub-partition hide the TMEM / MUFU / LDS latencies
-        // that bounded the 8-warp version, profiles/r1_gemm_phases_v2.txt).
-        const int et = threadIdx.x - 128;       // 0..511
-        const int ewarp = warp - 4;             // 0..15
-        const int quad = ewarp & 3;             // TMEM lane quadrant == warp % 4
-        const int part = ewarp >> 2;            // column quarter handled by this warpgroup
-        const int row_in_tile = quad * 32 + lane;
-        const int esize = p.out_f32 ? 4 : 2;
-        const int pitch = BN_OUT * esize + 16;
-        uint8_t* my_row = stg + row_in_tile * pitch;
-        constexpr int PART = BN_OUT / 4;        // output columns per warpgroup (16, 32 or 64)
-
-        if (EPI == EPI_RESID_LN) {  // this CTA's 64-column slice of the LayerNorm affine parameters
-            for (int i = et; i < BN; i += kEpiThreads) {
-                s_gamma[i] = p.gamma[cl_rank * BN + i];
-                s_beta[i] = p.beta[cl_rank * BN + i];
+        if (et < BM) {
+            const int rr = et;
+            int out_row;
+            bool ok;
+            if (p.conv) {
+                const int r = rr / p.conv_F2, f = rr % p.conv_F2;
+                const int bt = m_blk * p.conv_R + r;
+                const int b = bt / p.conv_T1h, t = bt % p.conv_T1h;
+                ok = (r < p.conv_R) && (b < p.conv_B) && (t < p.conv_T2);
+                out_row = (b * p.conv_T2 + t) * p.conv_F2 + f;
+            } else {
+                out_row = m_blk * BM + rr;
+                ok = out_row < p.M;
             }
+            s_rowmap[rr] = ok ? out_row : -1;
         }
-        int it = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-            const int mn_ = TN ? tile / splitk : tile;
-            const int m_blk = mn_ / n_tiles, n_blk = mn_ % n_tiles;
-            const int as = it & 1;
-            const uint32_t aph = (it >> 1) & 1;
-            const int col_base = n_blk * BN_OUT;             // first output column of the tile
-            const int ncols = min(BN_OUT, p.N - col_base);   // valid output columns
-            DBG_EPI(0);
-
-            // ---- (a) per-tile smem setup: bias slice, row map, residual tile (all coalesced, loads batched)
-            if (et < BN) {
-                const int i = et;
-                int c;
-                if (EPI == EPI_GLU) c = (i < BN_OUT) ? col_base + i : p.N + col_base + (i - BN_OUT);
-                else c = col_base + i;
-                const bool ok = (EPI == EPI_GLU) ? ((i % BN_OUT) < ncols) : (i < ncols);
-                s_bias[i] = (p.bias != nullptr && ok) ? p.bias[c] : 0.f;
-            } else if (et >= 256 && et < 256 + BM) {
-                const int rr = et - 256;
-                int out_row;
-                bool ok;
-                if (p.conv) {
-                    const int r = rr / p.conv_F2, f = rr % p.conv_F2;
-                    const int bt = m_blk * p.conv_R + r;
-                    const int b = bt / p.conv_T1h, t = bt % p.conv_T1h;
-                    ok = (r < p.conv_R) && (b < p.conv_B) && (t < p.conv_T2);
-                    out_row = (b * p.conv_T2 + t) * p.conv_F2 + f;
-                } else {
-                    out_row = m_blk * BM + rr;
-                    ok = out_row < p.M;
-                }
-                s_rowmap[rr] = ok ? out_row : -1;
-            }
-            if (EPI == EPI_RESID || EPI == EPI_RESID_LN) {
-                // residual rows are contiguous (no conv mode); 16-byte chunks, up to 8 independent loads per thread
-                if ((ncols & 7) == 0) {
-                    const int cpr = ncols >> 3;                        // 16-byte chunks per row
-                    const int rows_here = min(BM, p.M - m_blk * BM);
-                    const int total = rows_here * cpr;
-                    const bf16* rbase = p.resid + (size_t)(m_blk * BM) * p.ldr + col_base;
-                    for (int q0 = et; q0 < total; q0 += kEpiThreads * 8) {
-                        uint4 tmp[8];
+        if (EPI == EPI_RESID || EPI == EPI_RESID_LN) {
+            // residual rows are contiguous (no conv mode); 16-byte chunks, up to 8 independent loads per thread
+            if ((ncols & 7) == 0) {
+                const int cpr = ncols >> 3;                        // 16-byte chunks per row
+                const int rows_here = min(BM, p.M - m_blk * BM);
+                const int total = rows_here * cpr;
+                const bf16* rbase = p.resid + (size_t)(m_blk * BM) * p.ldr + col_base;
+                for (int q0 = et; q0 < total; q0 += kEpiThreads * 8) {
+                    uint4 tmp[8];
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int q = q0 + j * kEpiThreads;
-                            if (q < total) tmp[j] = *reinterpret_cast<const uint4*>(rbase + (size_t)(q / cpr) * p.ldr + (q % cpr) * 8);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int q = q0 + j * kEpiThreads;
-                            if (q < total) *reinterpret_cast<uint4*>(stg + (q / cpr) * pitch + (q % cpr) * 16) = tmp[j];
-                        }
+                    for (int j = 0; j < 8; ++j) {
+                        const int q = q0 + j * kEpiThreads;
+                        if (q < total) tmp[j] = *reinterpret_cast<const uint4*>(rbase + (size_t)(q / cpr) * p.ldr + (q % cpr) * 8);
                     }
-                } else {
-                    for (int r = ewarp; r < BM; r += 16) {
-                        const int grow = m_blk * BM + r;
-                        if (grow >= p.M) continue;
-                        const bf16* src = p.resid + (size_t)grow * p.ldr + col_base;
-                        for (int c = lane; c < ncols; c += 32) reinterpret_cast<bf16*>(stg + r * pitch)[c] = src[c];
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const int q = q0 + j * kEpiThreads;
+                        if (q < total) *reinterpret_cast<uint4*>(stg + (q / cpr) * pitch + (q % cpr) * 16) = tmp[j];
                     }
-                }
-            }
-            epi_bar();
-            DBG_EPI(1);
-
-            // row validity / padding mask of this thread's row
-            const int out_row = s_rowmap[row_in_tile];
-            bool row_live = true;
-            if (p.row_len != nullptr && out_row >= 0) {
-                const int b = out_row / p.row_period, t = out_row % p.row_period;
-                row_live = t < p.row_len[b];
-            }
-
-            mbar_wait(&tfull_bar[as], aph);
-            tc_fence_after();
-            if (it == 0 && et == 0) DBG_STAMP(5);
-            DBG_EPI(2);
-            const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * BN);
-
-            if (EPI == EPI_RESID_LN) {
-                // Each thread owns PART = BN/4 columns of its row (16-column chunks).  Pass 1: v = resid + acc + bias,
-                // (sum, sum of squares); v is parked back in TMEM when it does not fit one chunk.  The partials of
-                // the 4 column quarters x cl_size CTAs meet through (distributed) shared memory.  Pass 2 normalises.
-                float v[16];
-                float s1 = 0.f, s2 = 0.f;
-#pragma unroll 1
-                for (int c = part * PART; c < (part + 1) * PART; c += 16) {
-                    uint32_t r[16];
-                    tmem_ld16(t_row + c, r);
-                    tmem_ld_wait();
-                    const uint4* rs = reinterpret_cast<const uint4*>(my_row + c * 2);
-                    const float4* bs = reinterpret_cast<const float4*>(s_bias + c);
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const uint4 u = rs[i];
-                        const float4 b0 = bs[2 * i], b1 = bs[2 * i + 1];
-                        const float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y), f2 = unpack_bf16(u.z), f3 = unpack_bf16(u.w);
-                        const float rr[8] = {f0.x, f0.y, f1.x, f1.y, f2.x, f2.y, f3.x, f3.y};
-                        const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            float x = __uint_as_float(r[8 * i + j]) + bb[j];
-                            x = (row_live ? x : 0.f) + rr[j];
-                            v[8 * i + j] = x;
-                            s1 += x;
-                            s2 += x * x;
-                            r[8 * i + j] = __float_as_uint(x);
-                        }
-                    }
-                    if (PART > 16) tmem_st16(t_row + c, r);
-                }
-                if (PART > 16) tmem_st_wait();
-                if (PART == 16) {
-                    tc_fence_before();
-                    mbar_arrive(&tempty_bar[as]);  // accumulator consumed: the next tile's MMAs may start
-                }
-                // Tiles alternate between two (stats buffer, mbarrier) pairs: a peer that runs ahead signals the
-                // OTHER barrier, so statistics of consecutive tiles can never be mixed.  Each remote store carries
-                // its own byte count (st.async ... complete_tx), the owner expects 8 B x 512 threads x cl_size.
-                const int par = it & 1;
-                const int nslot = 4 * (int)cl_size;
-                float2* my_slot = &s_stats[(par * nslot + (int)cl_rank * 4 + part) * BM + row_in_tile];
-                if (cl_size == 1) {
-                    *my_slot = make_float2(s1, s2);     // whole row in this CTA: plain shared memory + named barrier
-                    epi_bar();
-                } else {
-                    if (et == 0) mbar_arrive_expect_tx(&ln_bar[par], (uint32_t)(8 * kEpiThreads) * cl_size);
-                    const uint32_t slot = smem_u32(my_slot);
-                    const uint32_t bar_local = smem_u32(&ln_bar[par]);
-                    for (uint32_t dst = 0; dst < cl_size; ++dst)
-                        st_async_f32x2(mapa_shared(slot, dst), s1, s2, mapa_shared(bar_local, dst));
-                    mbar_wait_cluster(&ln_bar[par], (uint32_t)((it >> 1) & 1));
-                }
-                float t1 = 0.f, t2 = 0.f;
-                for (int j = 0; j < 4 * (int)cl_size; ++j) {
-                    const float2 o = s_stats[(par * nslot + j) * BM + row_in_tile];
-                    t1 += o.x;
-                    t2 += o.y;
-                }
-                const float inv_n = 1.0f / (float)(BN * cl_size);
-                const float mean = t1 * inv_n;
-                const float var = fmaxf(t2 * inv_n - mean * mean, 0.f);
-                const float rstd = rsqrtf(var + p.eps);
-#pragma unroll 1
-                for (int c = part * PART; c < (part + 1) * PART; c += 16) {
-                    if (PART > 16) {
-                        uint32_t r[16];
-                        tmem_ld16(t_row + c, r);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-                    }
-                    const float4* gs = reinterpret_cast<const float4*>(s_gamma + c);
-                    const float4* es = reinterpret_cast<const float4*>(s_beta + c);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float4 g = gs[i], e = es[i];
-                        v[4 * i] = (v[4 * i] - mean) * rstd * g.x + e.x;
-                        v[4 * i + 1] = (v[4 * i + 1] - mean) * rstd * g.y + e.y;
-                        v[4 * i + 2] = (v[4 * i + 2] - mean) * rstd * g.z + e.z;
-                        v[4 * i + 3] = (v[4 * i + 3] - mean) * rstd * g.w + e.w;
-                    }
-                    stage16(my_row, c, 0, v);
-                }
-                if (PART > 16) {
-                    tc_fence_before();
-                    mbar_arrive(&tempty_bar[as]);
-                }
-            } else if (EPI == EPI_GLU) {
-#pragma unroll 1
-                for (int c = part * PART; c < (part + 1) * PART; c += 16) {
-                    uint32_t ra[16], rg[16];
-                    tmem_ld16(t_row + c, ra);
-                    tmem_ld16(t_row + BN_OUT + c, rg);
-                    tmem_ld_wait();
-                    float v[16];
-                    const float4* ba = reinterpret_cast<const float4*>(s_bias + c);
-                    const float4* bg = reinterpret_cast<const float4*>(s_bias + BN_OUT + c);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float4 x = ba[i], y = bg[i];
-                        const float av[4] = {x.x, x.y, x.z, x.w}, gv[4] = {y.x, y.y, y.z, y.w};
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const float a = __uint_as_float(ra[4 * i + j]) + av[j];
-                            const float g = __uint_as_float(rg[4 * i + j]) + gv[j];
-                            v[4 * i + j] = row_live ? a * fast_sigmoid(g) : 0.f;
-                        }
-                    }
-                    stage16(my_row, c, p.out_f32, v);
                 }
             } else {
-#pragma unroll 1
-                for (int c = part * PART; c < (part + 1) * PART; c += 16) {
-                    uint32_t r[16];
-                    tmem_ld16(t_row + c, r);
-                    tmem_ld_wait();
-                    if (c >= ncols) continue;  // warp-uniform
-                    float v[16];
-                    float res[16];
-                    if (EPI == EPI_RESID) {
-                        const uint4* rs = reinterpret_cast<const uint4*>(my_row + c * 2);
+                for (int r = ewarp; r < BM; r += kEpiThreads / 32) {
+                    const int grow = m_blk * BM + r;
+                    if (grow >= p.M) continue;
+                    const bf16* src = p.resid + (size_t)grow * p.ldr + col_base;
+                    for (int c = lane; c < ncols; c += 32) reinterpret_cast<bf16*>(stg + r * pitch)[c] = src[c];
+                }
+            }
+        }
+
+        // ---- (b) main loop: one k-block of wgmmas in flight; the stage of the previous k-block is released behind it
+        float acc[BN / 2];
 #pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            const uint4 u = rs[i];
-                            const float2 f0 = unpack_bf16(u.x), f1 = unpack_bf16(u.y), f2 = unpack_bf16(u.z),
-                                         f3 = unpack_bf16(u.w);
-                            res[8 * i] = f0.x; res[8 * i + 1] = f0.y; res[8 * i + 2] = f1.x; res[8 * i + 3] = f1.y;
-                            res[8 * i + 4] = f2.x; res[8 * i + 5] = f2.y; res[8 * i + 6] = f3.x; res[8 * i + 7] = f3.y;
-                        }
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        const int kb0 = kb_begin(tile), kb1 = kb_end(tile);
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            if (it == 0 && et == 0) DBG_KB(1, kb);
+            if (it == 0 && kb == kb0 && et == 0) DBG_STAMP(3);
+            const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+            const uint32_t b_addr = a_addr + Cfg::A_BYTES;
+            if (p.dbg_mode != 2) {
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    if (TN)   // MN-major operands: one k16 step = 16 rows of 128 B; this warpgroup's 64 M columns = A block cw
+                        mma_bn<BN, 1>(acc, gmma_desc_sw128(a_addr + cw * 8192 + k * 2048, 1024, 8192),
+                                      gmma_desc_sw128(b_addr + k * 2048, 1024, 8192), (uint32_t)(((kb - kb0) | k) != 0));
+                    else
+                        mma_bn<BN, 0>(acc, gmma_desc_sw128(a_addr + cw * 8192 + k * 32), gmma_desc_sw128(b_addr + k * 32),
+                                      (uint32_t)(((kb - kb0) | k) != 0));
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+            }
+            if (prev >= 0 && (et & 127) == 0) mbar_arrive(&empty_bar[prev]);   // the k-block before this one has been read
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (prev >= 0 && (et & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        if (it == 0 && et == 0) DBG_STAMP(4);
+        epi_bar<kEpiThreads>();   // bias, row map and residual tile of this tile are in shared memory
+        if (it == 0 && et == 0) DBG_STAMP(5);
+
+        // ---- (c) fused epilogue on the accumulator fragment: rows rl0 + 8 hh, columns 8 jj + cq + {0, 1}
+        int out_row[2];
+        bool row_live[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            out_row[hh] = s_rowmap[rl0 + 8 * hh];
+            row_live[hh] = true;
+            if (p.row_len != nullptr && out_row[hh] >= 0) {
+                const int b = out_row[hh] / p.row_period, t = out_row[hh] % p.row_period;
+                row_live[hh] = t < p.row_len[b];
+            }
+        }
+        if (EPI == EPI_RESID_LN) {
+            float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jj = 0; jj < BN / 8; ++jj) {
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int c = jj * 8 + cq;
+                    const float2 r = unpack_bf16(*reinterpret_cast<const uint32_t*>(stg + (rl0 + 8 * hh) * pitch + c * 2));
+                    float x0 = acc[4 * jj + 2 * hh] + s_bias[c], x1 = acc[4 * jj + 2 * hh + 1] + s_bias[c + 1];
+                    x0 = (row_live[hh] ? x0 : 0.f) + r.x;
+                    x1 = (row_live[hh] ? x1 : 0.f) + r.y;
+                    acc[4 * jj + 2 * hh] = x0;
+                    acc[4 * jj + 2 * hh + 1] = x1;
+                    s1[hh] += x0 + x1;
+                    s2[hh] += x0 * x0 + x1 * x1;
+                }
+            }
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+                for (int o = 1; o < 4; o <<= 1) {
+                    s1[hh] += __shfl_xor_sync(0xffffffffu, s1[hh], o);
+                    s2[hh] += __shfl_xor_sync(0xffffffffu, s2[hh], o);
+                }
+                const float inv_n = 1.0f / (float)BN;
+                const float mean = s1[hh] * inv_n;
+                const float var = fmaxf(s2[hh] * inv_n - mean * mean, 0.f);
+                const float rstd = rsqrtf(var + p.eps);
+                uint8_t* row_ptr = stg + (rl0 + 8 * hh) * pitch;
+#pragma unroll
+                for (int jj = 0; jj < BN / 8; ++jj) {
+                    const int c = jj * 8 + cq;
+                    stage2(row_ptr, c, 0, (acc[4 * jj + 2 * hh] - mean) * rstd * s_gamma[c] + s_beta[c],
+                           (acc[4 * jj + 2 * hh + 1] - mean) * rstd * s_gamma[c + 1] + s_beta[c + 1]);
+                }
+            }
+        } else if (EPI == EPI_GLU) {
+#pragma unroll
+            for (int jj = 0; jj < BN_OUT / 8; ++jj) {
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int c = jj * 8 + cq;
+                    float v[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float a = acc[4 * jj + 2 * hh + e] + s_bias[c + e];
+                        const float g = acc[4 * (jj + BN_OUT / 8) + 2 * hh + e] + s_bias[BN_OUT + c + e];
+                        v[e] = row_live[hh] ? a * fast_sigmoid(g) : 0.f;
                     }
-                    const float* trow = nullptr;
-                    if (EPI == EPI_TABLE)
-                        trow = p.table + (size_t)((out_row >= 0 ? out_row : 0) % p.period) * p.N + col_base + c;
-                    const uint32_t dseed = (EPI == EPI_RESID && p.drop_seed != nullptr) ? *p.drop_seed : 0u;
-                    float bv[16];
-                    {
-                        const float4* bs = reinterpret_cast<const float4*>(s_bias + c);
+                    stage2(stg + (rl0 + 8 * hh) * pitch, c, p.out_f32, v[0], v[1]);
+                }
+            }
+        } else {
+            const uint32_t dseed = (EPI == EPI_RESID && p.drop_seed != nullptr) ? *p.drop_seed : 0u;
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float4 b4 = bs[i];
-                            bv[4 * i] = b4.x; bv[4 * i + 1] = b4.y; bv[4 * i + 2] = b4.z; bv[4 * i + 3] = b4.w;
-                        }
-                    }
+            for (int jj = 0; jj < BN / 8; ++jj) {
+                if (jj * 8 >= ncols) break;
 #pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        float x = __uint_as_float(r[i]) + bv[i];
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int c = jj * 8 + cq;
+                    uint8_t* row_ptr = stg + (rl0 + 8 * hh) * pitch;
+                    float2 res = make_float2(0.f, 0.f);
+                    if (EPI == EPI_RESID) res = unpack_bf16(*reinterpret_cast<const uint32_t*>(row_ptr + c * 2));
+                    float v[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        float x = acc[4 * jj + 2 * hh + e] + s_bias[c + e];
                         if (EPI == EPI_RELU) x = fmaxf(x, 0.f);
                         if (EPI == EPI_SWISH) x = x * fast_sigmoid(x);
                         if (EPI == EPI_GELU) x = 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
                         if (EPI == EPI_TANH) x = tanhf(x);
-                        if (EPI == EPI_TABLE) x = x * p.alpha + ((c + i < ncols) ? __ldg(trow + i) : 0.f);
-                        if (!row_live) x = 0.f;
+                        if (EPI == EPI_TABLE)
+                            x = x * p.alpha + ((c + e < ncols) ? __ldg(p.table + (size_t)((out_row[hh] >= 0 ? out_row[hh] : 0) % p.period) * p.N + col_base + c + e) : 0.f);
+                        if (!row_live[hh]) x = 0.f;
                         if (EPI == EPI_RESID && p.drop_seed != nullptr)   // nn.Dropout on the sub-layer output (transformer.py:54,61)
-                            x = drop_keep(dseed, p.drop_site, (uint32_t)out_row, (uint32_t)(col_base + c + i), p.drop_thresh) ? x * p.drop_scale : 0.f;
-                        if (EPI == EPI_RESID) x = res[i] + p.alpha * x;
-                        v[i] = x;
+                            x = drop_keep(dseed, p.drop_site, (uint32_t)out_row[hh], (uint32_t)(col_base + c + e), p.drop_thresh) ? x * p.drop_scale : 0.f;
+                        if (EPI == EPI_RESID) x = (e ? res.y : res.x) + p.alpha * x;
+                        v[e] = x;
                     }
-                    stage16(my_row, c, p.out_f32, v);
+                    stage2(row_ptr, c, p.out_f32, v[0], v[1]);
                 }
             }
-            DBG_EPI(3);
-            if (EPI != EPI_RESID_LN) {
-                tc_fence_before();
-                mbar_arrive(&tempty_bar[as]);  // TMEM stage is free for the next tile's MMAs
-            }
-            epi_bar();
-            DBG_EPI(4);
-
-            // ---- (e) coalesced copy-out: consecutive threads write consecutive 16-byte chunks of a row
-            const int row_bytes = ncols * esize;
-            if ((row_bytes & 15) == 0) {
-                const int cpr = row_bytes >> 4;
-                const int total = BM * cpr;
-                uint8_t* obase = reinterpret_cast<uint8_t*>(p.out) + (size_t)col_base * esize;
-                const size_t ld_bytes = (size_t)p.ldc * esize;
-                for (int q0 = et; q0 < total; q0 += kEpiThreads * 4) {
-                    uint4 tmp[4];
-                    int orow[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int q = q0 + j * kEpiThreads;
-                        orow[j] = -1;
-                        if (q < total) {
-                            const int r = q / cpr;
-                            orow[j] = s_rowmap[r];
-                            tmp[j] = *reinterpret_cast<const uint4*>(stg + r * pitch + (q % cpr) * 16);
-                        }
-                    }
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int q = q0 + j * kEpiThreads;
-                        if (orow[j] < 0) continue;
-                        if (TN && (splitk > 1 || p.accum)) {   // partial sums meet in the fp32 output (pre-zeroed, or a running gradient)
-                            float* dst = reinterpret_cast<float*>(obase + (size_t)orow[j] * ld_bytes + (q % cpr) * 16);
-                            atomicAdd(dst, __uint_as_float(tmp[j].x));
-                            atomicAdd(dst + 1, __uint_as_float(tmp[j].y));
-                            atomicAdd(dst + 2, __uint_as_float(tmp[j].z));
-                            atomicAdd(dst + 3, __uint_as_float(tmp[j].w));
-                        } else {
-                            *reinterpret_cast<uint4*>(obase + (size_t)orow[j] * ld_bytes + (q % cpr) * 16) = tmp[j];
-                        }
-                    }
-                }
-            } else {
-                for (int r = ewarp; r < BM; r += 16) {
-                    const int orow = s_rowmap[r];
-                    if (orow < 0) continue;
-                    const uint8_t* src = stg + r * pitch;
-                    uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)orow * p.ldc + col_base) * esize;
-                    for (int off = lane * 2; off < row_bytes; off += 64)
-                        *reinterpret_cast<uint16_t*>(dst + off) = *reinterpret_cast<const uint16_t*>(src + off);
-                }
-            }
-            DBG_EPI(5);
-            epi_bar();  // staging / bias smem may be rewritten for the next tile
-            DBG_EPI(6);
-            if (it == 0 && et == 0) DBG_STAMP(6);
         }
-    }
+        epi_bar<kEpiThreads>();
 
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x == 0) DBG_STAMP(7);
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+        // ---- (d) coalesced copy-out: consecutive threads write consecutive 16-byte chunks of a row
+        const int row_bytes = ncols * esize;
+        if ((row_bytes & 15) == 0) {
+            const int cpr = row_bytes >> 4;
+            const int total = BM * cpr;
+            uint8_t* obase = reinterpret_cast<uint8_t*>(p.out) + (size_t)col_base * esize;
+            const size_t ld_bytes = (size_t)p.ldc * esize;
+            for (int q0 = et; q0 < total; q0 += kEpiThreads * 4) {
+                uint4 tmp[4];
+                int orow[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int q = q0 + j * kEpiThreads;
+                    orow[j] = -1;
+                    if (q < total) {
+                        const int r = q / cpr;
+                        orow[j] = s_rowmap[r];
+                        tmp[j] = *reinterpret_cast<const uint4*>(stg + r * pitch + (q % cpr) * 16);
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int q = q0 + j * kEpiThreads;
+                    if (orow[j] < 0) continue;
+                    if (TN && (splitk > 1 || p.accum)) {   // partial sums meet in the fp32 output (pre-zeroed, or a running gradient)
+                        float* dst = reinterpret_cast<float*>(obase + (size_t)orow[j] * ld_bytes + (q % cpr) * 16);
+                        atomicAdd(dst, __uint_as_float(tmp[j].x));
+                        atomicAdd(dst + 1, __uint_as_float(tmp[j].y));
+                        atomicAdd(dst + 2, __uint_as_float(tmp[j].z));
+                        atomicAdd(dst + 3, __uint_as_float(tmp[j].w));
+                    } else {
+                        *reinterpret_cast<uint4*>(obase + (size_t)orow[j] * ld_bytes + (q % cpr) * 16) = tmp[j];
+                    }
+                }
+            }
+        } else {
+            for (int r = ewarp; r < BM; r += kEpiThreads / 32) {
+                const int orow = s_rowmap[r];
+                if (orow < 0) continue;
+                const uint8_t* src = stg + r * pitch;
+                uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)orow * p.ldc + col_base) * esize;
+                for (int off = lane * 2; off < row_bytes; off += 64)
+                    *reinterpret_cast<uint16_t*>(dst + off) = *reinterpret_cast<const uint16_t*>(src + off);
+            }
+        }
+        epi_bar<kEpiThreads>();  // staging / bias smem may be rewritten for the next tile
+        if (it == 0 && et == 0) DBG_STAMP(6);
     }
+    if (et == 0) DBG_STAMP(7);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -672,7 +526,7 @@ int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -688,43 +542,8 @@ static const char* launch_inst(cudaStream_t st, const CUtensorMap& ta, const CUt
             return "cudaFuncSetAttribute(max dynamic smem) failed";
         attr_set = true;
     }
-    int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-    if (EPI == EPI_RESID_LN && p.N / BN > 1) {
-        const int cl = p.N / BN;              // CTAs per cluster == n-tiles per row block
-        grid = (grid / cl) * cl;              // whole clusters only (num_tiles is a multiple of cl)
-        if (grid < cl) return "gemm: grid smaller than one cluster";
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(grid);
-        cfg.blockDim = dim3(kThreads);
-        cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = cl;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        // co-resident clusters (GPC boundaries strand a few SMs): never launch more than fit in one wave
-        static int max_clusters[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-        if (cl <= 8 && max_clusters[cl] == 0) {
-            int n = 0;
-            if (cudaOccupancyMaxActiveClusters(&n, gemm_tc_kernel<BN, EPI>, &cfg) != cudaSuccess || n < 1) n = num_sms() / cl / 2;
-            max_clusters[cl] = n;
-        }
-        if (cl <= 8 && grid > max_clusters[cl] * cl) {
-            grid = max_clusters[cl] * cl;
-            cfg.gridDim = dim3(grid);
-        }
-        prefer_max_smem_carveout(gemm_tc_kernel<BN, EPI>);
-        cfg.numAttrs = pdl_enabled() ? 2 : 1;     // (the occupancy query above ran with the cluster attribute only)
-        cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI>, ta, tb, p);
-        return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
-    }
-    cudaError_t e = launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(grid), dim3(kThreads), Cfg::SMEM_BYTES, st, ta, tb, p);
+    const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
+    cudaError_t e = launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, ta, tb, p);
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
@@ -747,39 +566,22 @@ static const char* launch_bn(cudaStream_t st, const CUtensorMap& ta, const CUten
 
 // Pick the N tile that wastes the fewest MMA cycles across the persistent grid.
 static int choose_bn(int m_tiles, int n_cols, int epi, int out_f32) {
-    // Decode regime (<= 4 row blocks, M = batch x beam rows): every launch lasts 8-20 us whatever its tiling
-    // (profiles/r1_ncu_decode_gemms_summary.txt) and utterance batches run concurrently on other streams, whose aggregate
-    // throughput is bound by the SM-time the launches occupy (sum of CTAs x duration = 137 us of the whole GPU per decode
-    // step, profiles/r1_bench_history.md).  So small problems take the WIDEST tile: 2-4x fewer CTAs for +1-2 us of latency.
-    // Measured (profiles/r1_bench_history.md): policy 1 raises 8-lane throughput by 10-15 % and lengthens a lone 60-step
-    // decode from 31.5 to 40.9 ms; the serving layer picks the policy (otb_set_tile_policy), latency is the default.
+    // Decode regime (<= 4 row blocks, M = batch x beam rows): a launch lasts about as long whatever its tiling, and
+    // utterance batches running concurrently on other streams are bound by the SM-time the launches occupy.  Under the
+    // throughput policy small problems therefore take the WIDEST tile (fewer CTAs for slightly more latency); the serving
+    // layer picks the policy (otb_set_tile_policy), latency is the default.
     const bool decode = (m_tiles <= 4) && g_tile_policy == 1;
-    if (epi == EPI_RESID_LN) {
-        // A tcgen05.mma from shared memory costs ~160 cycles for any N <= 256 (profiles/r1_bench_history.md), so a
-        // 256-wide tile does the same main loop as four 64-wide ones: with enough row blocks to occupy the SMs (or under
-        // the throughput policy) keep the whole row in one CTA; a lone small problem (decode, M = 320) is split over a
-        // cluster of N/64 CTAs with DSMEM statistics, which shortens its launch by 2-4 us.
-        // OTB_LN_BN = 64 | 128 | 256 overrides the column tile of the large-M case (tuning aid: the row is then split over
-        // a cluster of N / BN CTAs with DSMEM statistics; 63 -> 126 -> 252 CTAs at cfg 2)
-        static const int forced = [] { const char* e = getenv("OTB_LN_BN"); return e ? atoi(e) : 0; }();
-        if (forced == 64 || forced == 128 || forced == 256) {
-            if (m_tiles >= 32 && forced <= n_cols && n_cols % forced == 0) return forced;
-        }
-        // measured at cfg 2 (63 row blocks, N = 256; tools/encoder_time.py): one CTA per row block 1.509 ms per encoder pass,
-        // the row split over a cluster of two 128-wide CTAs (126 CTAs) 1.436 ms, over four 64-wide CTAs 1.592 ms.  The split
-        // is NOT the default: its statistics are combined from per-CTA (sum, sum of squares) partials, and on the benchmark
-        // batch the 1-best agreement with the bf16-policy oracle dropped from 31 to 29 of 32 utterances for 5 % of 1.4 ms.
-        return (m_tiles >= 32 || decode) ? n_cols : 64;
-    }
+    // residual + LayerNorm: the tile spans the whole row (N <= 256), so the row statistics never leave the CTA
+    if (epi == EPI_RESID_LN) return n_cols;
     const int sms = num_sms();
     int best = 0;
     double best_cost = 1e30;
-    const int cands[3] = {256, 128, 64};
-    for (int i = 0; i < 3; ++i) {
+    const int cands[2] = {128, 64};   // 256-wide tiles run on one warpgroup (64-row tiles): kept for the LayerNorm row only
+    for (int i = 0; i < 2; ++i) {
         const int bn = cands[i];
         const int bn_out = (epi == EPI_GLU) ? bn / 2 : bn;
         if (bn_out * (out_f32 ? 4 : 2) > 512) continue;  // staged row must fit the staging pitch
-        if (bn_out < 64) continue;                       // each epilogue warpgroup needs >= 16 columns
+        if (bn_out < 64) continue;                       // at least 128-byte staged row segments for the copy-out
         const int n_tiles = (n_cols + bn_out - 1) / bn_out;
         const long tiles = (long)m_tiles * n_tiles;
         const long waves = (tiles + sms - 1) / sms;
@@ -809,7 +611,9 @@ const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, 
     if (bn == 0) return "gemm: no tile configuration";
     const int bn_out = (epi == EPI_GLU) ? bn / 2 : bn;
     const int n_tiles = (p.N + bn_out - 1) / bn_out;
-    const int num_tiles = m_tiles * n_tiles;
+    const int bm = (bn == 256) ? GemmCfg<256>::BM : BM;   // rows per tile of the chosen configuration
+    if (p.conv && bm != BM) return "gemm: conv mode needs 128-row tiles";
+    const int num_tiles = (p.conv ? m_tiles : (p.M + bm - 1) / bm) * n_tiles;
 
     CUtensorMap ta, tb;
     const char* err;
@@ -817,7 +621,7 @@ const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, 
         if (!conv_map) return "gemm: conv mode needs a conv tensor map";
         ta = *conv_map;
     } else {
-        if ((err = encode_tmap_2d(&ta, A, (uint64_t)p.K, (uint64_t)p.M, (uint64_t)lda, BK, BM))) return err;
+        if ((err = encode_tmap_2d(&ta, A, (uint64_t)p.K, (uint64_t)p.M, (uint64_t)lda, BK, (uint32_t)bm))) return err;
     }
     const uint32_t box_rows = (epi == EPI_GLU) ? (uint32_t)(bn / 2) : (uint32_t)bn;
     if ((err = encode_tmap_2d(&tb, W, (uint64_t)p.K, (uint64_t)w_rows, (uint64_t)ldw, BK, box_rows))) return err;
@@ -869,7 +673,7 @@ const char* gemm_wgrad_launch(cudaStream_t st, const void* dY, int lddy, const v
                 return "cudaFuncSetAttribute(wgrad) failed";
             attr = true;
         }
-        e = launch_pdl(gemm_tc_kernel<128, EPI_BIAS, true>, dim3(grid), dim3(kThreads), Cfg::SMEM_BYTES, st, ta, tb, p);
+        e = launch_pdl(gemm_tc_kernel<128, EPI_BIAS, true>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, ta, tb, p);
     } else {
         using Cfg = GemmCfg<64>;
         static bool attr = false;
@@ -878,7 +682,7 @@ const char* gemm_wgrad_launch(cudaStream_t st, const void* dY, int lddy, const v
                 return "cudaFuncSetAttribute(wgrad) failed";
             attr = true;
         }
-        e = launch_pdl(gemm_tc_kernel<64, EPI_BIAS, true>, dim3(grid), dim3(kThreads), Cfg::SMEM_BYTES, st, ta, tb, p);
+        e = launch_pdl(gemm_tc_kernel<64, EPI_BIAS, true>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, ta, tb, p);
     }
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

@@ -1,17 +1,14 @@
 // Kernel launch with programmatic dependent launch (PDL).
 //
-// Measured on B200 (profiles/r1_gemm_phases_v5.txt vs the ncu launch lists): the decode-step kernels spend 2-4 us
-// inside their code but last 7-13 us from launch to completion -- launch latency, CTA scheduling, shared-memory
-// carve-out and the drain of the previous kernel are paid serially, 52 times per beam step.  With the
+// Small decode-step kernels spend a few microseconds inside their code but pay launch latency, CTA scheduling,
+// shared-memory carve-out and the drain of the previous kernel serially, 52 times per beam step.  With the
 // programmatic-stream-serialization attribute the next kernel of the stream is scheduled while its predecessor is still
 // running: every kernel launched through launch_pdl() starts with PDL_TRIGGER() (dependents may be scheduled) and executes
 // PDL_WAIT() (griddepcontrol.wait: the predecessor grid has completed and its memory is visible) before its first
 // global-memory access, so correctness is unchanged while launch + prologue overlap the predecessor's tail.  Works inside
 // CUDA-graph capture (programmatic dependency edges).
-// Round-1 measurement (profiles/r1_bench_history.md): all 110 GPU tests pass with the attribute on, but the captured
-// decode step did not get faster (33.4 vs 32.3 ms per 60-step decode, 8-lane throughput 3313 vs 3339 utt/s) -- the
-// graph's kernel-to-kernel edges already hide the launch latency, what remains is inside the kernels and their
-// completion.  The attribute is therefore OFF by default (OTB_PDL=1 enables it); the two instructions are no-ops for a
+// Inside a captured CUDA graph the kernel-to-kernel edges already hide most of the launch latency, so the attribute is
+// OFF by default (OTB_PDL=1 enables it); the two instructions are no-ops for a
 // kernel launched without it.
 #pragma once
 #include <cuda_runtime.h>

@@ -17,7 +17,7 @@ namespace otb {
 // utterance: the 49 input rows are staged in smem once, each thread keeps the 3x3 filters + bias of
 // its 8 channels in registers and walks over (row, f1) positions, one 16-byte store per position,
 // fully coalesced along (f1, c).  (With 8 rows per CTA the 80 weight loads per thread outnumbered the
-// stores 8:1 -- 65 us for 22 MB, profiles/r1_ncu_layer_v5_summary.txt.)
+// stores 8:1.)
 // ------------------------------------------------------------------------------------------------
 static constexpr int CONV1_ROWS = 24;
 
@@ -173,8 +173,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const bf16* __restrict__
 }
 
 // N <= 256 fast path: one warp normalises 4 rows at a time so that 4 independent 16-byte loads (and 4
-// independent reduction chains) are in flight per lane -- the one-row-per-warp version was latency-bound
-// (14.8 us for 16 MB at Conformer cfg 4, profiles/r1_launches_conformer_v0.csv).
+// independent reduction chains) are in flight per lane -- the one-row-per-warp version was latency-bound.
 __global__ void __launch_bounds__(256) layernorm256_kernel(const bf16* __restrict__ x, int ldx, void* __restrict__ out,
                                                            int ldo, int out_f32, const float* __restrict__ g1,
                                                            const float* __restrict__ b1, const float* __restrict__ g2,

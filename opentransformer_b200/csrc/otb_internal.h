@@ -10,7 +10,7 @@ namespace otb {
 
 typedef __nv_bfloat16 bf16;
 
-// ---- epilogues of the tcgen05 GEMM (C = A[M,K] * W[N,K]^T, fp32 accumulate in TMEM) ----
+// ---- epilogues of the wgmma GEMM (C = A[M,K] * W[N,K]^T, fp32 accumulate in registers) ----
 enum Epilogue : int {
     EPI_BIAS = 0,      // out = acc + bias
     EPI_RELU = 1,      // out = relu(acc + bias)
@@ -160,7 +160,7 @@ struct MegaParams {
     float* dbg_logp;      // optional [max_steps, N, V]
     float* dbg_scores;    // optional [max_steps, N]
 };
-// ---- persistent decode kernel, round 2 (decode_group.cu): row groups of <= 128 hypotheses x 16 CTAs, tcgen05 GEMMs
+// ---- persistent decode kernel, round 2 (decode_group.cu): row groups of <= 128 hypotheses x 16 CTAs, wgmma GEMMs
 struct DgLayer {
     const float *bqkv, *bo, *bq, *bo2, *b1, *b2;
     const float *g1, *be1, *g2, *be2, *g3, *be3;

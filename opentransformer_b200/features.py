@@ -1,4 +1,4 @@
-"""Log-mel filterbank features + CMVN on the B200 (SURVEY.md 8f row 3): the step immediately before the hot path.
+"""Log-mel filterbank features + CMVN on the GPU (SURVEY.md 8f row 3): the step immediately before the hot path.
 
 Mirror of what otrans/data/audio.py:117-133 does on DataLoader worker CPUs per utterance,
 

@@ -1,9 +1,9 @@
-"""Transformer language model for shallow fusion on the B200 path.
+"""Transformer language model for shallow fusion on the CUDA path.
 
 Mirror of otrans/model/lm.py:93-171 (TransformerLanguageModel): embedding + sinusoidal positions +
 ``num_blocks`` post-norm TransformerEncoderLayers (GLU FFN) under a causal mask + tied output projection.
 Same constructor (``params`` dict of the YAML ``model:`` section), ``state_dict`` keys and ``predict``
-signature; the layers are the same sm_100a kernels as the acoustic encoder (causal flag on the attention
+signature; the layers are the same sm_90a kernels as the acoustic encoder (causal flag on the attention
 kernel).  The recogniser adds ``lm_weight * log_probs`` inside the fused log-softmax/top-k kernel
 (recognize/speech2text.py:102-105 -> otb_logsoftmax_topk).  Inference only.
 """

@@ -2,7 +2,7 @@
 
 Mirror of otrans/model/speech2text.py:14-87, otrans/model/__init__.py:6-9 and the three
 string-keyed registries (frontend/__init__.py:8-12, encoder/__init__.py:10-13,
-decoder/__init__.py:8-10).  A YAML `model:` section of the reference builds the B200 model
+decoder/__init__.py:8-10).  A YAML `model:` section of the reference builds the CUDA model
 unchanged; checkpoints written by the reference load through load_model() key for key.
 """
 import torch
@@ -18,7 +18,7 @@ BuildDecoder = {'transformer': TransformerDecoder}
 
 class CTCAssistor(nn.Module):
     """model/ctc.py:12-66: the joint-CTC head, Linear(hidden, vocab) + nn.CTCLoss(blank = 0, zero_infinity).  Parameter
-    holder (key `output_layer.*`, checkpoint section 'ctc'); compute is the tcgen05 GEMM + otb_ctc_loss."""
+    holder (key `output_layer.*`, checkpoint section 'ctc'); compute is the wgmma GEMM + otb_ctc_loss."""
 
     def __init__(self, hidden_size, vocab_size, blank=0, lookahead_steps=-1):
         super().__init__()

@@ -9,7 +9,7 @@ shapes as the reference so existing checkpoints load unchanged (SURVEY.md 8b):
 
 The nn.Linear / nn.LayerNorm / nn.Conv2d / nn.Embedding objects below are *parameter holders*
 only (they give identical key names and default init); their ``forward`` is never called.  All
-compute goes through ``ops`` -> libotb200.so (hand-written sm_100a kernels).  There is no CPU path:
+compute goes through ``ops`` -> libotb200.so (hand-written sm_90a kernels).  There is no CPU path:
 calling a module with CPU tensors raises.
 
 Numerics: GEMM operands / activations are bf16, accumulation fp32, LayerNorm / softmax statistics
@@ -84,7 +84,7 @@ class Conv2dLayer(nn.Module):
         super().__init__()
         ks = kernel_size if isinstance(kernel_size, (list, tuple)) else [kernel_size, kernel_size]
         if list(ks) != [3, 3] or stride != 2 or batch_norm or residual or act_func_type != 'relu':
-            raise NotImplementedError('B200 ConvFrontEnd supports the shipped configuration only: '
+            raise NotImplementedError('ConvFrontEnd supports the shipped configuration only: '
                                       '3x3 kernels, stride 2, relu, no batch_norm / residual')
         self.conv_layer = nn.Conv2d(in_channel, out_channel, (3, 3), stride=2, padding=(0, 1))
         self.output_size = (input_size + 2 - 3) // 2 + 1
@@ -184,7 +184,7 @@ class MultiHeadedSelfAttention(nn.Module):
         if share_qvk_proj:
             raise NotImplementedError('share_qvk_proj')
         if d_model != n_heads * 64:
-            raise NotImplementedError('the sm_100a attention kernel is specialised for d_k = 64')
+            raise NotImplementedError('the sm_90a attention kernel is specialised for d_k = 64')
         self.qvk_proj = nn.Linear(d_model, d_model * 3)
         self.output_proj = nn.Linear(d_model, d_model)
 
@@ -197,7 +197,7 @@ class MultiHeadedCrossAttention(nn.Module):
         if share_vk_proj:
             raise NotImplementedError('share_vk_proj')
         if d_model != n_heads * 64:
-            raise NotImplementedError('the sm_100a attention kernel is specialised for d_k = 64')
+            raise NotImplementedError('the sm_90a attention kernel is specialised for d_k = 64')
         self.q_proj = nn.Linear(d_model, d_model)
         self.vk_proj = nn.Linear(memory_dim, d_model * 2)
         self.output_proj = nn.Linear(d_model, d_model)
@@ -386,7 +386,7 @@ class MultiHeadedSelfAttentionWithRelPos(nn.Module):
         if dropout_rate or skip_term_b or share_qvk_proj:
             raise NotImplementedError('rel-pos attention: dropout / skip_term_b / share_qvk_proj')
         if d_model != n_heads * 64:
-            raise NotImplementedError('the sm_100a attention kernel is specialised for d_k = 64')
+            raise NotImplementedError('the sm_90a attention kernel is specialised for d_k = 64')
         self.nheads, self.d_model = n_heads, d_model
         self.qvk_proj = nn.Linear(d_model, d_model * 3)
         self.pos_proj = nn.Linear(d_model, d_model, bias=False)

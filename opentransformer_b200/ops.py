@@ -56,7 +56,7 @@ def _p(t):
 
 def _need(t, dtype, name):
     if not t.is_cuda:
-        raise RuntimeError(f'{name} must be a CUDA tensor: the B200 hot path has no CPU fallback')
+        raise RuntimeError(f'{name} must be a CUDA tensor: the CUDA hot path has no CPU fallback')
     if t.dtype != dtype:
         raise TypeError(f'{name} must be {dtype}, got {t.dtype}')
     if not t.is_contiguous():
@@ -119,7 +119,7 @@ def linear(a, w, bias=None, epilogue=EPI_BIAS, out=None, out_f32=False, resid=No
     such as one head's 64 columns of a wider matrix are fine: the TMA map takes the row pitch)."""
     for t, n in ((a, 'a'), (w, 'w')):
         if not t.is_cuda:
-            raise RuntimeError(f'{n} must be a CUDA tensor: the B200 hot path has no CPU fallback')
+            raise RuntimeError(f'{n} must be a CUDA tensor: the CUDA hot path has no CPU fallback')
         if t.dtype != BF16 or t.dim() != 2 or t.stride(1) != 1:
             raise TypeError(f'{n} must be a 2-D bf16 tensor with unit column stride')
     M, K = a.shape

@@ -1,10 +1,10 @@
-"""Batched beam-search recogniser on the B200 hot path.
+"""Batched beam-search recogniser on the CUDA hot path.
 
 Mirror of otrans/recognize/speech2text.py (SpeechToTextRecognizer) and the bits of
 otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``encode`` / ``decode`` /
 ``decode_step`` seams and return types.  What changes underneath:
 
-  * encode: conv front end + encoder run as hand-written sm_100a kernels (bf16 tensor cores);
+  * encode: conv front end + encoder run as hand-written sm_90a kernels (bf16 tensor cores);
   * decode: the reference re-runs the whole decoder over the whole prefix -- and the cross-attention
     K/V projection of the beam-tiled memory -- at every step (decoder/transformer.py:204,
     attention.py:129).  Here cross K/V are projected ONCE per utterance (shared by the beams), self-attention
@@ -107,7 +107,7 @@ class BeamDecoder:
         if decoder.pos_emb.scale_learnable:
             raise NotImplementedError('decoder with learnable positional scale')
         # persistent path: the whole loop in ONE launch (csrc/decode_group.cu: row groups of <= 128 hypotheses x 16 CTAs,
-        # tcgen05 GEMMs, group-local barriers) when the configuration is the shipped one (post-norm GLU decoder, d_model 256,
+        # wgmma GEMMs, group-local barriers) when the configuration is the shipped one (post-norm GLU decoder, d_model 256,
         # 4 heads, d_ff 2048, <= 256 memory frames); anything else takes the per-step graph.
         self.persistent = bool(persistent) and self.mega_supported()
         self._mega_model = None
@@ -182,8 +182,7 @@ class BeamDecoder:
                 x = ops.layernorm(x, *p['ln2'])
             q = ops.linear(x, p['wq'], p['bq'])
             # the `beam` hypotheses of utterance b are the query rows [b*beam, (b+1)*beam) of one attention problem
-            # (a SIMT kernel specialised for <= 16 query rows was measured at 14.9 us against 10.0 us for this tcgen05 kernel
-            # padded to 128 rows and was dropped: profiles/r1_bench_history.md)
+            # (the attention kernel pads the problem to 128 query rows)
             ctx = ops.attention(q, self.kvx[l], self.kvx[l], self.B, H, self.beam, self.T, kv_len=self.mem_len,
                                 k_col0=0, v_col0=d)
             x = _proj_resid_ln(ctx, p['wo2'], p['bo2'], x, None if nb else p['ln2'])
@@ -260,9 +259,8 @@ class BeamDecoder:
     def run(self, max_steps, poll_every=8):
         """Run up to max_steps decode steps; stops early once the device reports every hypothesis ended
         (speech2text.py:66-67).  Steps launched after the end are no-ops on the search state.
-        (A sync-free variant -- the flag copied asynchronously to pinned memory and inspected one poll later -- shortened a
-        lone decode by 0.5 ms but cost 8 concurrent lanes 18 % of their throughput: free-running lanes fall into lockstep
-        and queue for the same SMs, whereas this 4-byte poll staggers them.  profiles/r1_bench_history.md)"""
+        (A sync-free variant -- the flag copied asynchronously to pinned memory and inspected one poll later -- lets
+        free-running lanes fall into lockstep and queue for the same SMs, whereas this 4-byte poll staggers them.)"""
         if self.persistent and self.lm_logp is None:
             self.run_persistent(max_steps)
             return int(self._read_ctrl()[0])
@@ -275,7 +273,7 @@ class BeamDecoder:
 
 
 class SpeechToTextRecognizer(Recognizer):
-    """otrans/recognize/speech2text.py:6-93 on the B200 path."""
+    """otrans/recognize/speech2text.py:6-93 on the CUDA path."""
 
     def __init__(self, model, lm=None, lm_weight=0.1, ctc_weight=0.0, beam_width=5, nbest=1, max_len=50,
                  idx2unit=None, penalty=0, lamda=5, ngpu=1, apply_cache=False, use_graph=True, persistent=None):

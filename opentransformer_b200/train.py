@@ -1,11 +1,11 @@
-"""Training step of the speech transformer on the B200 path (SURVEY.md 8a rows 16-17, 8e).
+"""Training step of the speech transformer on the CUDA path (SURVEY.md 8a rows 16-17, 8e).
 
 Mirror of the inner step of otrans/train/trainer.py:206-234 for `SpeechToText` (model/speech2text.py:39-64):
 
     loss, _ = model(inputs, targets); loss.backward(); clip_grad_norm_(params, 5); scheduler.step(); optimizer.step()
 
 The reference differentiates its forward through torch autograd.  Here the backward is written by hand as a reverse
-walk over a tape of saved bf16 activations, so that every contraction runs on the tcgen05 kernels (dgrad = otb_linear
+walk over a tape of saved bf16 activations, so that every contraction runs on the wgmma kernels (dgrad = otb_linear
 with the transposed weight, residual gradients fused into its epilogue; wgrad = otb_linear_wgrad; attention backward =
 otb_attention_bwd) and everything else on the HBM-bound backward kernels (csrc/backward.cu).  The only torch autograd
 node is `_SpeechToTextLoss`, which makes `model(inputs, targets)[0].backward()` populate `.grad` of the fp32 master
@@ -549,7 +549,7 @@ class FusedTrainer:
 
     def _graph_for(self, inputs, mask, truth, tlen=None):
         """The ~870 launches of one micro-batch captured once per input geometry and replayed: launched one by one from
-        Python the step is host-bound (14.6 ms against 10.2 ms of kernel time, profiles/r1_launches_train_v0.csv).
+        Python the step is host-bound.
         Real ASR batches have a new (T, L) almost every step, so a geometry runs EAGERLY until it has recurred
         `graph_after` times, and at most `max_graphs` graphs are kept (least recently used first out): use_graph pays off
         with bucketed / padded batches (otrans/data/bucket.py), it must not grow memory without bound otherwise.

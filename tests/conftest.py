@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a real B200 (run with -m gpu under gpurun)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA GPU with sm_90a (H100)')
 
 
 @pytest.fixture(scope='session')

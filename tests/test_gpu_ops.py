@@ -1,6 +1,6 @@
 """GPU parity of every C-ABI op against a plain fp32 torch restatement of the same op (the checker),
 on bf16-rounded operands so that only accumulation order / output rounding differ.  Integer results
-(beam search) are compared bit-exactly against oracle/.  Run with -m gpu on a B200."""
+(beam search) are compared bit-exactly against oracle/.  Run with -m gpu on an H100."""
 import math
 import os
 

@@ -1,6 +1,7 @@
-"""The oracle port against the REFERENCE ITSELF, where oracle/_ref exists (the reference's own Python modules, byte-compiled
-by oracle/build_ref.py in the build container; git-ignored, travels with gpurun).  Complements tests/test_oracle_golden.py
-(committed fixtures): here the reference code runs live on fresh random models.  Nothing reads /root/reference."""
+"""The oracle port against the REFERENCE ITSELF: tests/golden/live_ref_<case>.pt hold small random models (state dicts),
+their inputs and what the reference's own modules computed from them -- encoder states, recognize() hypotheses and scores,
+training loss and every parameter gradient (written by tests/golden/make_live_ref.py from the reference's byte-compiled
+modules).  Complements tests/test_oracle_golden.py, which pins the shipped configurations."""
 import os
 import sys
 
@@ -12,10 +13,10 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 from oracle import beam_search as obs      # noqa: E402
-from oracle import build_ref               # noqa: E402
 from oracle import speech_model as om      # noqa: E402
 
-pytestmark = pytest.mark.skipif(build_ref.load() is None, reason='oracle/_ref not built (no reference tree in this environment)')
+def _case(name):
+    return torch.load(os.path.join(ROOT, 'tests', 'golden', f'live_ref_{name}.pt'), weights_only=False)
 
 
 def _params(normalize_before, activation):
@@ -35,39 +36,24 @@ def _params(normalize_before, activation):
 
 @pytest.mark.parametrize('normalize_before,activation', [(False, 'glu'), (True, 'relu')])
 def test_port_equals_live_reference(normalize_before, activation):
-    from otrans.model import End2EndModel
-    from otrans.recognize.speech2text import SpeechToTextRecognizer
-    params = _params(normalize_before, activation)
-    torch.manual_seed(4321)
-    ref = End2EndModel['speech2text'](params).eval()
-    with torch.no_grad():
-        ref.decoder.embedding.weight.mul_(0.15)
-        ref.decoder.output_layer.bias[1] = 1.5          # hypotheses end at different steps
-    sd = {k: v.detach().clone().float() for k, v in ref.state_dict().items() if k.split('.')[0] in ('frontend', 'encoder', 'decoder')}
-    g = torch.Generator().manual_seed(5)
-    B, T, beam, max_len = 3, 64, 3, 9
-    lens = torch.tensor([64, 50, 37])
-    mask = torch.arange(T)[None] < lens[:, None]
-    x = torch.randn(B, T, 20, generator=g) * mask.unsqueeze(2)
+    c = _case(f'recognize-{normalize_before}-{activation}')
+    params, sd, x, mask, beam, max_len = c['params'], c['sd'], c['x'], c['mask'], c['beam'], c['max_len']
+    B = x.shape[0]
     with torch.no_grad():
         # encoder states: reference modules vs the port
-        fx, fm = ref.frontend(x, mask)
-        mem_ref, mm_ref, _ = ref.encoder(fx, fm)
         mem, mm = om.encode(x, mask, sd, params)
-        assert torch.equal(mm, mm_ref)
-        torch.testing.assert_close(mem[mm], mem_ref[mm_ref], rtol=1e-4, atol=2e-5)
+        assert torch.equal(mm, c['mm_ref'])
+        torch.testing.assert_close(mem[mm], c['mem_ref'][c['mm_ref']], rtol=1e-4, atol=2e-5)
         # the whole recognize(): ids bit-exact, scores to fp32 tolerance
-        rec = SpeechToTextRecognizer(ref, beam_width=beam, nbest=beam, max_len=max_len, idx2unit={i: str(i) for i in range(40)},
-                                     penalty=0.6, lamda=5, ngpu=0)
-        hyps, scores_ref = rec.recognize(x, mask)
         nb, ns, _, _ = obs.recognize(x, mask, sd, params, beam=beam, nbest=beam, max_len=max_len, penalty=0.6, lamda=5)
+    hyps = c['hyps']
     for b in range(B):
         for r in range(beam):
             port = [int(t) for t in nb[b, r].tolist()]
             port = port[:port.index(1)] if 1 in port else port
             want = [int(t) for t in hyps[b][r].split()] if hyps[b][r] else []
             assert port == want, (b, r, port, want)
-    torch.testing.assert_close(ns, scores_ref.float(), rtol=1e-4, atol=1e-4)
+    torch.testing.assert_close(ns, c['scores_ref'], rtol=1e-4, atol=1e-4)
 
 
 @pytest.mark.parametrize('normalize_before,activation', [(False, 'glu'), (True, 'glu'), (False, 'relu'), (True, 'relu')])
@@ -75,35 +61,11 @@ def test_port_gradients_equal_live_reference_autograd(normalize_before, activati
     """model.train(); loss, _ = model(inputs, targets); loss.backward() through the REFERENCE's own modules (trainer.py:206-217)
     vs oracle/train_step.loss_and_grads: the loss and every parameter gradient -- in particular for the pre-norm and ReLU
     stacks whose hand-written CUDA backward is tested against this port (tests/test_gpu_train.py)."""
-    from otrans.model import End2EndModel
     from oracle import train_step as ot
-    params = _params(normalize_before, activation)
-    torch.manual_seed(99)
-    ref = End2EndModel['speech2text'](params)
-    ref.train()
-    g = torch.Generator().manual_seed(7)
-    with torch.no_grad():
-        for n, p in ref.named_parameters():
-            if 'norm' in n:
-                p.add_(0.2 * torch.randn(p.shape, generator=g))
-            elif n.endswith('.bias'):
-                p.add_(0.05 * torch.randn(p.shape, generator=g))
-        ref.decoder.embedding.weight.mul_(0.12)
-    sd = {k: v.detach().clone().float() for k, v in ref.state_dict().items() if k.split('.')[0] in ('frontend', 'encoder', 'decoder')}
-    B, T, L = 3, 70, 8
-    lens = torch.tensor([70, 55, 41])
-    mask = torch.arange(T)[None] < lens[:, None]
-    x = torch.randn(B, T, 20, generator=g) * mask.unsqueeze(2)
-    tgt = torch.randint(3, 40, (B, L), generator=g)
-    tgt[:, 0] = 1
-    tgt[0, L - 2:] = torch.tensor([1, 0])
-    tgt[1, L - 1] = 1
-    tgt[2, 4:] = torch.tensor([1, 0, 0, 0])
-    loss_ref, _ = ref({'inputs': x, 'mask': mask}, {'targets': tgt, 'targets_length': None})
-    loss_ref.backward()
-    g_ref = {n: p.grad.clone() for n, p in ref.named_parameters() if p.grad is not None}
-    loss, grads = ot.loss_and_grads(x, mask, tgt, sd, params)
-    torch.testing.assert_close(loss, loss_ref.detach(), rtol=1e-5, atol=1e-5)
+    c = _case(f'gradients-{normalize_before}-{activation}')
+    loss, grads = ot.loss_and_grads(c['x'], c['mask'], c['tgt'], c['sd'], c['params'])
+    torch.testing.assert_close(loss, c['loss_ref'], rtol=1e-5, atol=1e-5)
+    g_ref = c['g_ref']
     assert set(grads) == set(g_ref), set(grads) ^ set(g_ref)
     for n in grads:
         torch.testing.assert_close(grads[n], g_ref[n], rtol=2e-4, atol=2e-6, msg=lambda m, n=n: f'{n}: {m}')
@@ -113,44 +75,16 @@ def test_port_gradients_equal_live_reference_autograd(normalize_before, activati
 def test_port_encoder_states_equal_live_reference_for_relpos_encoders(kind):
     """Conformer (macaron FFN, rel-pos attention without output projection, conv module with BatchNorm running statistics,
     only post_ffn_norm applied: SURVEY.md 8a quirks) and the rel-pos Transformer encoder: valid-frame states of the port vs
-    the live reference modules, recognize() ids bit-exact."""
-    from otrans.model import End2EndModel
-    from otrans.recognize.speech2text import SpeechToTextRecognizer
-    params = _params(False, 'glu')
-    if kind == 'conformer':
-        params['encoder_type'] = 'conformer'
-        params['encoder'] = dict(d_model=32, d_ff=24, cov_kernel_size=5, n_heads=4, nblocks=2, pos_dropout=0.0, slf_attn_dropout=0.0,
-                                 ffn_dropout=0.0, residual_dropout=0.0, conv_dropout=0.0, macaron_style=True, ffn_scale=0.5,
-                                 conv_bias=True, activation='glu', positional_encoding=True, relative_positional=True)
-    else:
-        params['encoder']['relative_positional'] = True
-    torch.manual_seed(77)
-    ref = End2EndModel['speech2text'](params).eval()
-    g = torch.Generator().manual_seed(11)
+    the reference modules, recognize() ids bit-exact."""
+    c = _case(f'relpos-{kind}')
+    params, sd, x, mask, beam, max_len = c['params'], c['sd'], c['x'], c['mask'], c['beam'], c['max_len']
     with torch.no_grad():
-        for n, buf in ref.named_buffers():
-            if n.endswith('running_mean'):
-                buf.add_(0.3 * torch.randn(buf.shape, generator=g))
-            if n.endswith('running_var'):
-                buf.mul_(1.0 + 0.5 * torch.rand(buf.shape, generator=g))
-        ref.decoder.embedding.weight.mul_(0.15)
-        ref.decoder.output_layer.bias[1] = 1.5
-    sd = {k: v.detach().clone().float() for k, v in ref.state_dict().items() if k.split('.')[0] in ('frontend', 'encoder', 'decoder')}
-    B, T, beam, max_len = 3, 72, 3, 7
-    lens = torch.tensor([72, 60, 33])
-    mask = torch.arange(T)[None] < lens[:, None]
-    x = torch.randn(B, T, 20, generator=g) * mask.unsqueeze(2)
-    with torch.no_grad():
-        fx, fm = ref.frontend(x, mask)
-        mem_ref, mm_ref, _ = ref.encoder(fx, fm)
         mem, mm = om.encode(x, mask, sd, params)
-        assert torch.equal(mm, mm_ref)
-        torch.testing.assert_close(mem[mm], mem_ref[mm_ref], rtol=1e-4, atol=2e-5)
-        rec = SpeechToTextRecognizer(ref, beam_width=beam, nbest=1, max_len=max_len, idx2unit={i: str(i) for i in range(40)},
-                                     penalty=0.6, lamda=5, ngpu=0)
-        hyps, _ = rec.recognize(x, mask)
+        assert torch.equal(mm, c['mm_ref'])
+        torch.testing.assert_close(mem[mm], c['mem_ref'][c['mm_ref']], rtol=1e-4, atol=2e-5)
         nb, _, _, _ = obs.recognize(x, mask, sd, params, beam=beam, nbest=1, max_len=max_len, penalty=0.6, lamda=5)
-    for b in range(B):
+    hyps = c['hyps']
+    for b in range(x.shape[0]):
         port = [int(t) for t in nb[b, 0].tolist()]
         port = port[:port.index(1)] if 1 in port else port
         want = [int(t) for t in hyps[b][0].split()] if hyps[b][0] else []

@@ -1,5 +1,5 @@
 """Encoder-forward time of the benchmark configuration (32 utterances x 1000 frames, cfg 2/3): median of 20 passes, CUDA events.
-Used for A/B runs of tiling switches (OTB_LN_BN=64|128|256)."""
+Used for A/B runs of two builds (OTB_LIB_PATH)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -24,5 +24,5 @@ with torch.no_grad():
         ts.append(e0.elapsed_time(e1))
 ts.sort()
 flop = 410e9
-print(f'OTB_LN_BN={os.environ.get("OTB_LN_BN", "default")}: encoder forward median {ts[10]:.3f} ms, min {ts[0]:.3f} ms = '
+print(f'encoder forward median {ts[10]:.3f} ms, min {ts[0]:.3f} ms = '
       f'{flop / ts[10] / 1e9:.0f} TFLOP/s (410 GFLOP per 32 utterances)')

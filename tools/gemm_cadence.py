@@ -5,7 +5,7 @@ import torch
 from opentransformer_b200 import ops, _lib
 dev = torch.device('cuda:0')
 L = _lib.lib()
-buf = torch.zeros(148 * 8 + 148 * 2 * 64, dtype=torch.int64, device=dev)
+buf = torch.zeros(256 * 8 + 256 * 2 * 64, dtype=torch.int64, device=dev)
 for (M, N, K) in [(7968, 2048, 2048), (7968, 1024, 2048), (7968, 64, 2048)]:
     a = torch.randn(M, K, device=dev).to(torch.bfloat16)
     w = torch.randn(N, K, device=dev).to(torch.bfloat16)
@@ -20,7 +20,7 @@ for (M, N, K) in [(7968, 2048, 2048), (7968, 1024, 2048), (7968, 64, 2048)]:
         ops.linear(a, w, None, ops.EPI_BIAS, out=out)
         torch.cuda.synchronize()
         L.otb_debug_gemm_timing(None)
-        kbt = buf[148 * 8:].view(148, 2, 64).cpu()
+        kbt = buf[256 * 8:].view(256, 2, 64).cpu()
         ful = [int(v) for v in kbt[3, 1] if int(v) > 0]
         iss = [int(v) for v in kbt[3, 0] if int(v) > 0]
         d = [ful[i + 1] - ful[i] for i in range(8, min(len(ful) - 1, 30))]

@@ -1,4 +1,4 @@
-"""How many small dependent kernels per second can L concurrent CUDA-graph lanes push through one B200?
+"""How many small dependent kernels per second can L concurrent CUDA-graph lanes push through one GPU?
 Each lane = one stream replaying a graph of 52 tiny dependent kernels (the shape of one decode step)."""
 import sys, os, threading, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

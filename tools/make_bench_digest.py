@@ -37,7 +37,7 @@ try:
 except Exception:
     out = {}
 out.update({'oracle_sha1': hashlib.sha1(ids.numpy().tobytes()).hexdigest(), 'shape': list(ids.shape),
-            'generator': 'tools/make_bench_digest.py (oracle, policy bf16); gpu_* keys: tools/gpu_r2_digest.sh on a B200',
+            'generator': 'tools/make_bench_digest.py (oracle, policy bf16); gpu_* keys: validation.ids_sha1 of bench.py on an H100',
             'oracle_ids': ids[:, 0].tolist()})
 with open(path, 'w') as f:
     json.dump(out, f)
