@@ -100,7 +100,7 @@ int otb_linear_dropout_resid(const void* a, int lda, const void* w, int ldw, con
 int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask, int M, int N, float p, const uint32_t* seed,
                     uint32_t site, void* stream);
 
-/* Fused masked multi-head attention, d_k = 64 (attention.py:80,34-41): for batch b, head h
+/* Fused masked multi-head attention, d_k = 64 (attention.py:80,34-41; otb_attention_dk below also takes 96): for batch b, head h
  *   out[b*Tq+i, h*64:(h+1)*64] = softmax_j((q_i . k_j + bd) / 8, j < kv_len[b], causal: j <= i) V
  * q/k/v are row-major bf16 matrices; batch b owns rows [b*Tq, (b+1)*Tq) of q and [b*Tk, (b+1)*Tk) of k,v;
  * head h starts at column q_col0/k_col0/v_col0 + 64*h.  bd (optional, f32 [H,B,Tq,ldbd]) holds
@@ -110,6 +110,14 @@ int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask,
 int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
                   void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
                   int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, void* stream);
+
+/* otb_attention with an explicit head width d_k, 64 or 96 (any other value returns non-zero with otb_last_error()):
+ * head h occupies columns col0 + d_k*h .. col0 + d_k*(h+1) of q/k/v and out, the scores are scaled by 1/sqrt(d_k).
+ * d_k = 96 is the width of the shipped Conformer configuration (d_model 384, 4 heads).  Inference only: the
+ * backward (otb_attention_lse / otb_attention_bwd) is 64-wide. */
+int otb_attention_dk(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
+                     void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
+                     int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, int d_k, void* stream);
 
 /* ConformerConvolutionModule middle (module/conformer.py:48-52): depthwise Conv1d(k, pad (k-1)/2) over time +
  * eval-mode BatchNorm1d + swish.  x, out bf16 [B*T, d]; w f32 [k, d] and b f32 [d] carry the BatchNorm affine
@@ -143,6 +151,9 @@ int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int 
  * [Lmax,N,d]; anc i32 [2,N,Lmax]; *step_ptr = 0-based position; out bf16 [N,d]. */
 int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
                          int H, int Lmax, void* stream);
+/* otb_decode_self_attn with an explicit head width d_k, 64 or 96 (d = H*d_k); otb_decode_self_attn is d_k = 64. */
+int otb_decode_self_attn_dk(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
+                            int H, int Lmax, int d_k, void* stream);
 
 /* LabelSmoothingLoss.forward (module/loss.py:21-48) fused: per-token KL(smoothed one-hot || softmax), PAD rows 0,
  * mean over non-PAD tokens.  logits f32 [rows, ldl]; targets i64 [rows]; tok_loss f32 [rows]; loss f32 [1];

@@ -55,6 +55,8 @@ _SIGS = {
     'otb_dropout_bwd': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_float, _P, ctypes.c_uint32, _P]),
     'otb_attention': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int,
                               _P, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P]),
+    'otb_attention_dk': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int,
+                                 _P, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, c_int, _P]),
     'otb_dwconv_swish': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_layernorm': (c_int, [_P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_float, c_int, c_int, _P]),
     'otb_scale_add_table': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, c_int, c_int, c_int, _P]),
@@ -62,6 +64,7 @@ _SIGS = {
     'otb_embed_posenc': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, _P, c_int, _P]),
     'otb_log_softmax': (c_int, [_P, c_int, _P, c_int, c_int, c_int, _P]),
     'otb_decode_self_attn': (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
+    'otb_decode_self_attn_dk': (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_ls_ce': (c_int, [_P, c_int, _P, c_int, c_int, c_float, c_int, _P, _P, _P, _P, c_int, _P]),
     'otb_beam_init': (c_int, [POINTER(BeamStateC), _P]),
     'otb_beam_step': (c_int, [_P, c_int, c_int, _P, c_int, c_float, POINTER(BeamStateC), _P, _P, _P]),

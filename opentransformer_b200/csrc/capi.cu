@@ -174,30 +174,53 @@ int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask,
                                               p, seed, site));
 }
 
+}  // extern "C"
+
+namespace otb {
+// otb_attention, otb_attention_lse and otb_attention_dk
+static int attention_impl(const char* where, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v,
+                          int ldv, void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
+                          int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse, int d_k,
+                          void* stream) {
+    if (!q || !k || !v || !out) return fail(where, "null operand");
+    if (d_k != 64 && d_k != 96) return fail(where, "head width d_k must be 64 or 96");
+    if (q_col0 % 8 || k_col0 % 8 || v_col0 % 8 || ldo % 8) return fail(where, "column offsets / ldo must be multiples of 8");
+    AttnParams p;
+    p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk;
+    p.kv_len = kv_len; p.causal = causal;
+    p.scale_log2 = 1.4426950408889634f / sqrtf((float)d_k);   // log2(e) / sqrt(d_k); exactly 0.125 log2(e) at d_k 64
+    p.out = reinterpret_cast<bf16*>(out); p.ldo = ldo;
+    p.q_col0 = q_col0; p.k_col0 = k_col0; p.v_col0 = v_col0;
+    p.bd = bd; p.ldbd = ldbd;
+    p.resid = reinterpret_cast<const bf16*>(resid); p.ldr = ldr;
+    p.lse = lse;
+    if (resid && (ldr % 8)) return fail(where, "ldr must be a multiple of 8");
+    RET(where, attn_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p, d_k));
+}
+}  // namespace otb
+
+extern "C" {
+
 int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
                   void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
                   int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, void* stream) {
-    return otb_attention_lse(q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0,
-                             v_col0, bd, ldbd, resid, ldr, nullptr, stream);
+    return attention_impl("otb_attention", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, B, H, Tq, Tk, kv_len, causal, q_col0,
+                          k_col0, v_col0, bd, ldbd, resid, ldr, nullptr, 64, stream);
+}
+
+int otb_attention_dk(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
+                     void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
+                     int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, int d_k, void* stream) {
+    return attention_impl("otb_attention_dk", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, B, H, Tq, Tk, kv_len, causal, q_col0,
+                          k_col0, v_col0, bd, ldbd, resid, ldr, nullptr, d_k, stream);
 }
 
 int otb_attention_lse(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
                       void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
                       int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse,
                       void* stream) {
-    if (!q || !k || !v || !out) return fail("otb_attention", "null operand");
-    if (q_col0 % 8 || k_col0 % 8 || v_col0 % 8 || ldo % 8) return fail("otb_attention", "column offsets / ldo must be multiples of 8");
-    AttnParams p;
-    p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk;
-    p.kv_len = kv_len; p.causal = causal;
-    p.scale_log2 = 0.125f * 1.4426950408889634f;
-    p.out = reinterpret_cast<bf16*>(out); p.ldo = ldo;
-    p.q_col0 = q_col0; p.k_col0 = k_col0; p.v_col0 = v_col0;
-    p.bd = bd; p.ldbd = ldbd;
-    p.resid = reinterpret_cast<const bf16*>(resid); p.ldr = ldr;
-    p.lse = lse;
-    if (resid && (ldr % 8)) return fail("otb_attention", "ldr must be a multiple of 8");
-    RET("otb_attention", attn_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p));
+    return attention_impl("otb_attention", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, B, H, Tq, Tk, kv_len, causal, q_col0,
+                          k_col0, v_col0, bd, ldbd, resid, ldr, lse, 64, stream);
 }
 
 int otb_layernorm(const void* x, int ldx, void* out, int ldo, int out_f32, const float* g1, const float* b1,
@@ -245,10 +268,16 @@ int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int 
 
 int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
                          int H, int Lmax, void* stream) {
+    return otb_decode_self_attn_dk(qkv, kc, vc, anc, step_ptr, out, N, H, Lmax, 64, stream);
+}
+
+int otb_decode_self_attn_dk(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
+                            int H, int Lmax, int d_k, void* stream) {
     if (!qkv || !kc || !vc || !anc || !step_ptr || !out) return fail("otb_decode_self_attn", "null operand");
+    if (d_k != 64 && d_k != 96) return fail("otb_decode_self_attn", "head width d_k must be 64 or 96");
     RET("otb_decode_self_attn",
         decode_self_attn_launch(ST(stream), reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(kc),
-                                reinterpret_cast<bf16*>(vc), anc, step_ptr, reinterpret_cast<bf16*>(out), N, H, Lmax));
+                                reinterpret_cast<bf16*>(vc), anc, step_ptr, reinterpret_cast<bf16*>(out), N, H, Lmax, d_k));
 }
 
 int otb_ls_ce(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,

@@ -380,52 +380,71 @@ const char* log_softmax_launch(cudaStream_t st, const float* x, int ldx, float* 
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
+// Chunk c of a staged K/V row goes to position rot_chunk(c + s) in row s (bank-conflict-free rows); i >= 0.
+template <int CH>
+__device__ __forceinline__ int rot_chunk(int i) {
+    if constexpr (CH == 8) return i & 7;
+    else return (int)((unsigned)i % CH);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Decode-time self-attention with a per-hypothesis KV cache (the `cache` the reference stubbed out,
 // decoder/transformer.py:92-126,188-203).  One query (the newest token) per hypothesis; the prefix
 // K/V of hypothesis n at position s' < step live in slot anc[n][s'] of step s' (beam reordering
-// moves 4-byte ancestry entries, never K/V rows).  Warp = (hypothesis, head), d_k = 64, lane owns
-// two dims.  Also appends the current K/V to the cache.
+// moves 4-byte ancestry entries, never K/V rows).  Warp = (hypothesis, head), d_k = DK (64 or 96).
+// Also appends the current K/V to the cache.
 //   qkv   bf16 [N, 3d] (Q | K | V of the current token, attention.py:73 split order)
 //   kc,vc bf16 [Lmax, N, d]
 //   anc   int32 [2, N, Lmax]  (ping-pong, buffer (step & 1) is current)
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 6) decode_self_attn_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc,
+template <int DK>
+__global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc,
                                                                bf16* __restrict__ vc, const int* __restrict__ anc,
                                                                const int* __restrict__ step_ptr, bf16* __restrict__ out,
                                                                int N, int H, int Lmax, float scale, int keys_pad) {
     PDL_TRIGGER();
     PDL_WAIT();
     // Lanes run over KEYS: each lane owns up to KPL cached positions, resolves their slots through the
-    // ancestry table and pulls the whole 128-byte K and V rows with 16-byte loads -- all loads of a lane are
+    // ancestry table and pulls the whole K and V rows (DK * 2 bytes) with 16-byte loads -- all loads of a lane are
     // independent, so the kernel costs ~3 dependent memory round trips (anc -> K/V -> out) instead of a
     // serial walk over the prefix.  V rows go through smem so that the P.V reduction is a column sum.
     constexpr int KPL = 4;               // keys per lane -> up to 128 cached positions
-    extern __shared__ uint4 sv_raw[];    // [warps][128 keys][8 x 16 B]  V rows (bf16)
+    constexpr int CH = DK / 8;           // 16-byte chunks per K / V row
+    extern __shared__ uint4 sv_raw[];    // [warps][keys_pad][CH x 16 B]  V rows (bf16)
     const int n = blockIdx.x;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nw = blockDim.x >> 5;
-    const int d = H * 64;
+    const int d = H * DK;
     const int step = *step_ptr;
     const int nkeys = step + 1;
     const int* an = anc + ((size_t)(step & 1) * N + n) * Lmax;
-    uint4* sv = sv_raw + (size_t)wib * keys_pad * 8;    // [keys_pad][8 x 16 B] per warp
-    // q lives in shared memory (every lane needs all 64 dims: 64 registers per thread otherwise, which capped the kernel
+    uint4* sv = sv_raw + (size_t)wib * keys_pad * CH;    // [keys_pad][CH x 16 B] per warp
+    // q lives in shared memory (every lane needs all DK dims: 64 registers per thread otherwise, which capped the kernel
     // at 3 resident CTAs per SM -- the SM-time of this latency-bound kernel is what concurrent batches compete for)
-    float* sq = reinterpret_cast<float*>(sv_raw + (size_t)(blockDim.x >> 5) * keys_pad * 8) + wib * 64;
+    float* sq = reinterpret_cast<float*>(sv_raw + (size_t)(blockDim.x >> 5) * keys_pad * CH) + wib * DK;
     for (int h = wib; h < H; h += nw) {
-        const bf16* base = qkv + (size_t)n * 3 * d + h * 64;
-        // append the newest K/V to the cache (lane owns dims 2*lane, 2*lane+1)
+        const bf16* base = qkv + (size_t)n * 3 * d + h * DK;
+        // append the newest K/V to the cache (lane owns dims 2*lane, 2*lane+1; at DK 96 lanes 0..15 also own 64+2*lane, +1)
         const uint32_t kcur = *reinterpret_cast<const uint32_t*>(base + d + 2 * lane);
         const uint32_t vcur = *reinterpret_cast<const uint32_t*>(base + 2 * d + 2 * lane);
-        const size_t cur_off = ((size_t)step * N + n) * d + h * 64 + 2 * lane;
+        const size_t cur_off = ((size_t)step * N + n) * d + h * DK + 2 * lane;
         *reinterpret_cast<uint32_t*>(kc + cur_off) = kcur;
         *reinterpret_cast<uint32_t*>(vc + cur_off) = vcur;
+        if (DK == 96 && lane < 16) {
+            *reinterpret_cast<uint32_t*>(kc + cur_off + 64) = *reinterpret_cast<const uint32_t*>(base + d + 64 + 2 * lane);
+            *reinterpret_cast<uint32_t*>(vc + cur_off + 64) = *reinterpret_cast<const uint32_t*>(base + 2 * d + 64 + 2 * lane);
+        }
         {
             const float2 qq = unpack_bf16(*reinterpret_cast<const uint32_t*>(base + 2 * lane));
+            float2 qh = make_float2(0.f, 0.f);
+            if (DK == 96 && lane < 16) qh = unpack_bf16(*reinterpret_cast<const uint32_t*>(base + 64 + 2 * lane));
             __syncwarp();
             sq[2 * lane] = qq.x;
             sq[2 * lane + 1] = qq.y;
+            if (DK == 96 && lane < 16) {
+                sq[64 + 2 * lane] = qh.x;
+                sq[64 + 2 * lane + 1] = qh.y;
+            }
             __syncwarp();
         }
         int slot[KPL];
@@ -441,16 +460,16 @@ __global__ void __launch_bounds__(128, 6) decode_self_attn_kernel(const bf16* __
             const int s = lane + 32 * j;
             sc[j] = -INFINITY;
             if (s < nkeys) {   // warp-divergent only in the last group
-                const bf16* krow = (s == step) ? base + d : kc + ((size_t)s * N + slot[j]) * d + h * 64;
-                const bf16* vrow = (s == step) ? base + 2 * d : vc + ((size_t)s * N + slot[j]) * d + h * 64;
-                uint4 ku[8], vu[8];
+                const bf16* krow = (s == step) ? base + d : kc + ((size_t)s * N + slot[j]) * d + h * DK;
+                const bf16* vrow = (s == step) ? base + 2 * d : vc + ((size_t)s * N + slot[j]) * d + h * DK;
+                uint4 ku[CH], vu[CH];
 #pragma unroll
-                for (int i = 0; i < 8; ++i) ku[i] = *reinterpret_cast<const uint4*>(krow + 8 * i);
+                for (int i = 0; i < CH; ++i) ku[i] = *reinterpret_cast<const uint4*>(krow + 8 * i);
 #pragma unroll
-                for (int i = 0; i < 8; ++i) vu[i] = *reinterpret_cast<const uint4*>(vrow + 8 * i);
+                for (int i = 0; i < CH; ++i) vu[i] = *reinterpret_cast<const uint4*>(vrow + 8 * i);
                 float dot = 0.f;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
+                for (int i = 0; i < CH; ++i) {
                     const float2 a = unpack_bf16(ku[i].x), b = unpack_bf16(ku[i].y), c = unpack_bf16(ku[i].z),
                                  e = unpack_bf16(ku[i].w);
                     const float4 q0 = *reinterpret_cast<const float4*>(sq + 8 * i);      // broadcast reads
@@ -460,7 +479,7 @@ __global__ void __launch_bounds__(128, 6) decode_self_attn_kernel(const bf16* __
                 sc[j] = dot * scale;
                 mx = fmaxf(mx, sc[j]);
 #pragma unroll
-                for (int i = 0; i < 8; ++i) sv[s * 8 + ((i + s) & 7)] = vu[i];   // rotate chunks: conflict-free rows
+                for (int i = 0; i < CH; ++i) sv[s * CH + rot_chunk<CH>(i + s)] = vu[i];   // rotate chunks: conflict-free rows
             }
         }
         mx = warp_max(mx);
@@ -472,47 +491,84 @@ __global__ void __launch_bounds__(128, 6) decode_self_attn_kernel(const bf16* __
         }
         l = warp_sum(l);
         __syncwarp();
-        // P.V as a column sum over the staged V rows: lane owns output dims 2*lane, 2*lane+1
-        const uint32_t* svw = reinterpret_cast<const uint32_t*>(sv);
-        float ax = 0.f, ay = 0.f;
+        if constexpr (DK == 64) {
+            // P.V as a column sum over the staged V rows: lane owns output dims 2*lane, 2*lane+1
+            const uint32_t* svw = reinterpret_cast<const uint32_t*>(sv);
+            float ax = 0.f, ay = 0.f;
 #pragma unroll
-        for (int j = 0; j < KPL; ++j) {
-            const int cnt = min(32, nkeys - 32 * j);
-            if (cnt <= 0) break;   // warp-uniform
+            for (int j = 0; j < KPL; ++j) {
+                const int cnt = min(32, nkeys - 32 * j);
+                if (cnt <= 0) break;   // warp-uniform
 #pragma unroll 4
-            for (int t = 0; t < cnt; ++t) {
-                const int s = t + 32 * j;
-                const float pw = __shfl_sync(0xffffffffu, sc[j], t);
-                // dims 2*lane.. live in 16-byte chunk (lane >> 2), word (lane & 3); chunks were rotated by s
-                const uint32_t vv = svw[(s * 8 + (((lane >> 2) + s) & 7)) * 4 + (lane & 3)];
-                const float2 vf = unpack_bf16(vv);
-                ax = fmaf(pw, vf.x, ax);
-                ay = fmaf(pw, vf.y, ay);
+                for (int t = 0; t < cnt; ++t) {
+                    const int s = t + 32 * j;
+                    const float pw = __shfl_sync(0xffffffffu, sc[j], t);
+                    // dims 2*lane.. live in 16-byte chunk (lane >> 2), word (lane & 3); chunks were rotated by s
+                    const uint32_t vv = svw[(s * 8 + (((lane >> 2) + s) & 7)) * 4 + (lane & 3)];
+                    const float2 vf = unpack_bf16(vv);
+                    ax = fmaf(pw, vf.x, ax);
+                    ay = fmaf(pw, vf.y, ay);
+                }
             }
+            const float inv = 1.0f / l;
+            *reinterpret_cast<uint32_t*>(out + (size_t)n * d + h * 64 + 2 * lane) = pack_bf16(ax * inv, ay * inv);
+        } else {
+            // P.V as a column sum: lanes 0..23 own 4 output dims each, 4*lane .. 4*lane+3 = 8-byte half (lane & 1) of
+            // 16-byte chunk (lane >> 1); lanes 24..31 repeat lane 23's reads and store nothing
+            const uint2* svh = reinterpret_cast<const uint2*>(sv);
+            const int ln = min(lane, 23);
+            float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+#pragma unroll
+            for (int j = 0; j < KPL; ++j) {
+                const int cnt = min(32, nkeys - 32 * j);
+                if (cnt <= 0) break;   // warp-uniform
+#pragma unroll 4
+                for (int t = 0; t < cnt; ++t) {
+                    const int s = t + 32 * j;
+                    const float pw = __shfl_sync(0xffffffffu, sc[j], t);
+                    const uint2 vv = svh[(s * CH + rot_chunk<CH>((ln >> 1) + s)) * 2 + (ln & 1)];
+                    const float2 v01 = unpack_bf16(vv.x), v23 = unpack_bf16(vv.y);
+                    a0 = fmaf(pw, v01.x, a0);
+                    a1 = fmaf(pw, v01.y, a1);
+                    a2 = fmaf(pw, v23.x, a2);
+                    a3 = fmaf(pw, v23.y, a3);
+                }
+            }
+            const float inv = 1.0f / l;
+            if (lane < 24)
+                *reinterpret_cast<uint2*>(out + (size_t)n * d + h * DK + 4 * lane) =
+                    make_uint2(pack_bf16(a0 * inv, a1 * inv), pack_bf16(a2 * inv, a3 * inv));
         }
-        const float inv = 1.0f / l;
-        *reinterpret_cast<uint32_t*>(out + (size_t)n * d + h * 64 + 2 * lane) = pack_bf16(ax * inv, ay * inv);
         __syncwarp();
     }
 }
 
-const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
-                                    const int* step_ptr, bf16* out, int N, int H, int Lmax) {
-    if (Lmax > 128) return "decode_self_attn: at most 128 cached positions (max_len <= 128)";
+template <int DK>
+static const char* decode_self_attn_launch_dk(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
+                                              const int* step_ptr, bf16* out, int N, int H, int Lmax) {
     const int warps = H < 4 ? H : 4;
     // V staging sized by the longest prefix this search can reach (not the 128-key maximum): at max_len 60 this halves the
     // shared memory per CTA and doubles the resident CTAs of this latency-bound kernel (less SM-time per decode step)
     const int keys_pad = (Lmax + 31) / 32 * 32;
-    const size_t smem = (size_t)warps * keys_pad * 128 + (size_t)warps * 64 * sizeof(float);   // V rows | q per warp
+    const size_t smem = (size_t)warps * keys_pad * DK * 2 + (size_t)warps * DK * sizeof(float);   // V rows | q per warp
     static bool attr_set = false;
     if (!attr_set) {
-        if (cudaFuncSetAttribute(decode_self_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024) != cudaSuccess)
+        if (cudaFuncSetAttribute(decode_self_attn_kernel<DK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (DK == 64 ? 80 : 100) * 1024) !=
+            cudaSuccess)
             return "cudaFuncSetAttribute(decode_self_attn) failed";
         attr_set = true;
     }
-    cudaError_t e = launch_pdl(decode_self_attn_kernel, dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax,
-                               0.125f, keys_pad);
+    cudaError_t e = launch_pdl(decode_self_attn_kernel<DK>, dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H,
+                               Lmax, DK == 64 ? 0.125f : 1.0f / sqrtf((float)DK), keys_pad);
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+}
+
+const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
+                                    const int* step_ptr, bf16* out, int N, int H, int Lmax, int d_k) {
+    if (Lmax > 128) return "decode_self_attn: at most 128 cached positions (max_len <= 128)";
+    if (d_k == 64) return decode_self_attn_launch_dk<64>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax);
+    if (d_k == 96) return decode_self_attn_launch_dk<96>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax);
+    return "decode_self_attn: head width d_k must be 64 or 96";
 }
 
 // ------------------------------------------------------------------------------------------------

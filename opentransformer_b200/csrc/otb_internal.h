@@ -202,8 +202,9 @@ extern int g_dg_barrier;
 size_t decode_group_workspace_bytes(int N, int n_layers, int Lmax, int B, int beam, int V);
 const char* decode_group_launch(cudaStream_t st, const MegaParams& p, void* workspace, size_t workspace_bytes);
 
+// d_k: head width, 64 or 96 (head h starts at column col0 + d_k * h)
 const char* attn_launch(cudaStream_t st, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows,
-                        const void* v, int ldv, const AttnParams& p);
+                        const void* v, int ldv, const AttnParams& p, int d_k);
 const char* conv1_launch(cudaStream_t st, const float* x, const float* w, const float* bias, bf16* out, int B, int T,
                          int F, int T1, int F1, int T1pad, int F1pad, int C1);
 const char* layernorm_launch(cudaStream_t st, const bf16* x, int ldx, void* out, int ldo, int out_f32, const float* g1,
@@ -218,7 +219,7 @@ const char* embed_posenc_launch(cudaStream_t st, const long long* tok, int tok_s
                                 int vocab);
 const char* log_softmax_launch(cudaStream_t st, const float* x, int ldx, float* out, int ldo, int rows, int V);
 const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
-                                    const int* step_ptr, bf16* out, int N, int H, int Lmax);
+                                    const int* step_ptr, bf16* out, int N, int H, int Lmax, int d_k);
 const char* beam_init_launch(cudaStream_t stream, BeamState st);
 const char* beam_step_launch(cudaStream_t stream, const float* logp, int ldl, int V, const float* lm_logp, int ld_lm,
                              float lm_weight, BeamState st, long long* dbg_ktok, int* dbg_offs, const float* pre_val,

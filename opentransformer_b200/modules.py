@@ -176,6 +176,13 @@ class ConvFrontEnd(nn.Module):
 # ------------------------------------------------------------------------------------------------
 # parameter holders shared by encoder / decoder layers
 # ------------------------------------------------------------------------------------------------
+def _check_heads(d_model, n_heads):
+    """The attention kernels are built for 64- and 96-wide heads (the Transformer and Conformer configs)."""
+    if d_model % n_heads or d_model // n_heads not in ops.HEAD_DIMS:
+        raise NotImplementedError(f'the sm_90a attention kernels support head widths d_k in {ops.HEAD_DIMS}; '
+                                  f'd_model {d_model} / {n_heads} heads is not one of them')
+
+
 class MultiHeadedSelfAttention(nn.Module):
     """Keys: qvk_proj.{weight,bias} [3d,d] (split order Q,K,V -- attention.py:73), output_proj.*"""
 
@@ -183,8 +190,7 @@ class MultiHeadedSelfAttention(nn.Module):
         super().__init__()
         if share_qvk_proj:
             raise NotImplementedError('share_qvk_proj')
-        if d_model != n_heads * 64:
-            raise NotImplementedError('the sm_90a attention kernel is specialised for d_k = 64')
+        _check_heads(d_model, n_heads)
         self.qvk_proj = nn.Linear(d_model, d_model * 3)
         self.output_proj = nn.Linear(d_model, d_model)
 
@@ -196,8 +202,7 @@ class MultiHeadedCrossAttention(nn.Module):
         super().__init__()
         if share_vk_proj:
             raise NotImplementedError('share_vk_proj')
-        if d_model != n_heads * 64:
-            raise NotImplementedError('the sm_90a attention kernel is specialised for d_k = 64')
+        _check_heads(d_model, n_heads)
         self.q_proj = nn.Linear(d_model, d_model)
         self.vk_proj = nn.Linear(memory_dim, d_model * 2)
         self.output_proj = nn.Linear(d_model, d_model)
@@ -304,7 +309,7 @@ class TransformerEncoderLayer(nn.Module):
             return _ffn(x, pk['ffn'], x, None if self.normalize_before else pk['ln2'])
         qkv = ops.linear(x, pk['wqkv'], pk['bqkv'])
         ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d,
-                            v_col0=2 * d)
+                            v_col0=2 * d, d_k=d // H)
         x = _proj_resid_ln(ctx, pk['wo'], pk['bo'], x, None if self.normalize_before else pk['ln1'])
         if self.normalize_before:
             x = ops.layernorm(x, *pk['ln2'])
@@ -385,8 +390,7 @@ class MultiHeadedSelfAttentionWithRelPos(nn.Module):
         super().__init__()
         if dropout_rate or skip_term_b or share_qvk_proj:
             raise NotImplementedError('rel-pos attention: dropout / skip_term_b / share_qvk_proj')
-        if d_model != n_heads * 64:
-            raise NotImplementedError('the sm_90a attention kernel is specialised for d_k = 64')
+        _check_heads(d_model, n_heads)
         self.nheads, self.d_model = n_heads, d_model
         self.qvk_proj = nn.Linear(d_model, d_model * 3)
         self.pos_proj = nn.Linear(d_model, d_model, bias=False)
@@ -407,14 +411,15 @@ class MultiHeadedSelfAttentionWithRelPos(nn.Module):
     def run(self, y, x_resid, pk, B, T, lengths, pos_bf16):
         """y = LN(x) bf16 [B*T,d]; returns x_resid + attention (no output projection)."""
         d, H = self.d_model, self.nheads
+        dk = d // H
         ext = ops.linear(y, pk['wext'], pk['bext'])                       # [M, 4d]
         pproj = ops.linear(pos_bf16, pk['wpos'])                          # [2T-1, d]  pos_proj(PE[-(T-1)..T-1])
         ld = (2 * T - 1 + 3) // 4 * 4
         bd = torch.empty(H, B * T, ld, dtype=torch.float32, device=y.device)
         for h in range(H):  # BD_full[h] = (q+v)_h P_h^T ; the attention kernel reads the j-i+T-1 diagonal band
-            ops.linear(ext[:, d + 64 * h: d + 64 * (h + 1)], pproj[:, 64 * h: 64 * (h + 1)], out=bd[h])
+            ops.linear(ext[:, d + dk * h: d + dk * (h + 1)], pproj[:, dk * h: dk * (h + 1)], out=bd[h])
         return ops.attention(ext, ext, ext, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=2 * d, v_col0=3 * d,
-                             bd=bd, resid=x_resid)
+                             bd=bd, resid=x_resid, d_k=dk)
 
 
 class ConformerConvolutionModule(nn.Module):
@@ -488,7 +493,7 @@ class ConformerEncoderBlock(nn.Module):
             return self.mha.run(y, x, pk['mha'], B, T, lengths, pos_bf16)
         d, H, m = x.shape[1], self.n_heads, pk['mha']
         qkv = ops.linear(y, m['wqkv'], m['bqkv'])
-        ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=d, v_col0=2 * d)
+        ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
         return ops.linear(ctx, m['wo'], m['bo'], EPI_RESID, resid=x)
 
     def _conv(self, x, pk, B, T, lengths):
@@ -701,13 +706,13 @@ class TransformerDecoder(nn.Module):
             if nb:
                 x = ops.layernorm(x, *p['ln1'])
             qkv = ops.linear(x, p['wqkv'], p['bqkv'])
-            ctx = ops.attention(qkv, qkv, qkv, B, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d)
+            ctx = ops.attention(qkv, qkv, qkv, B, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
             x = _proj_resid_ln(ctx, p['wo'], p['bo'], x, None if nb else p['ln1'])
             if nb:
                 x = ops.layernorm(x, *p['ln2'])
             q = ops.linear(x, p['wq'], p['bq'])
             kv = ops.linear(memory_bf16, p['wkv'], p['bkv'])
-            ctx = ops.attention(q, kv, kv, B, H, L, T, kv_len=mem_len, k_col0=0, v_col0=d)
+            ctx = ops.attention(q, kv, kv, B, H, L, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H)
             x = _proj_resid_ln(ctx, p['wo2'], p['bo2'], x, None if nb else p['ln2'])
             if nb:
                 x = ops.layernorm(x, *p['ln3'])
@@ -767,7 +772,8 @@ class TransformerDecoder(nn.Module):
             if nb:
                 x = ops.layernorm(x, *p['ln2'])
             q = ops.linear(x, p['wq'], p['bq'])
-            ctx = ops.attention(q, c.kvx[l], c.kvx[l], c.batch, H, c.beam, c.T, kv_len=c.mem_len, k_col0=0, v_col0=d)
+            ctx = ops.attention(q, c.kvx[l], c.kvx[l], c.batch, H, c.beam, c.T, kv_len=c.mem_len, k_col0=0, v_col0=d,
+                                d_k=d // H)
             x = _proj_resid_ln(ctx, p['wo2'], p['bo2'], x, None if nb else p['ln2'])
             if nb:
                 x = ops.layernorm(x, *p['ln3'])

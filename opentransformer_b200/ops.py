@@ -176,21 +176,33 @@ def dropout_mask(M, N, p, seed, site):
     return mask
 
 
+HEAD_DIMS = (64, 96)   # head widths the attention kernels are built for
+
+
+def check_head_dim(d_k):
+    if d_k not in HEAD_DIMS:
+        raise NotImplementedError(f'the sm_90a attention kernels support head widths d_k in {HEAD_DIMS}, got {d_k}')
+
+
 def attention(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, v_col0=0, out=None, bd=None,
-              resid=None):
-    """q/k/v: bf16 2-D matrices (may be the same [M,3d] buffer with different column offsets)."""
+              resid=None, d_k=64):
+    """q/k/v: bf16 2-D matrices (may be the same [M,3d] buffer with different column offsets); head h of each starts
+    at column col0 + d_k*h.  Returns bf16 [B*Tq, H*d_k]."""
     for t, n in ((q, 'q'), (k, 'k'), (v, 'v')):
         _need(t, BF16, n)
-    d = H * 64
+    check_head_dim(d_k)
+    d = H * d_k
     if out is None:
         out = torch.empty(B * Tq, d, dtype=BF16, device=q.device)
     if kv_len is not None:
         _need(kv_len, torch.int32, 'kv_len')
-    check(_lib.lib().otb_attention(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0),
-                                   _p(out), out.stride(0), B, H, Tq, Tk, _p(kv_len), 1 if causal else 0, q_col0,
-                                   k_col0, v_col0, _p(bd), bd.shape[-1] if bd is not None else 0, _p(resid),
-                                   resid.stride(0) if resid is not None else 0, _stream()),
-          'otb_attention')
+    args = (_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out), out.stride(0), B, H, Tq,
+            Tk, _p(kv_len), 1 if causal else 0, q_col0, k_col0, v_col0, _p(bd), bd.shape[-1] if bd is not None else 0, _p(resid),
+            resid.stride(0) if resid is not None else 0)
+    if d_k == 64:
+        check(_lib.lib().otb_attention(*args, _stream()), 'otb_attention')
+    else:
+        check(_lib.lib().otb_attention_dk(*args, d_k, _stream()), 'otb_attention_dk')
     _count()
     return out
 
@@ -302,10 +314,20 @@ def ls_cross_entropy(logits, targets, V, smoothing=0.1, pad_id=0, want_grad=Fals
 
 
 def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None):
+    """kc/vc bf16 [Lmax, N, d]: the head width d_k = d // H is taken from the cache."""
+    d = kc.shape[-1]
+    if d % H:
+        raise ValueError(f'decode_self_attn: cache width {d} is not a multiple of H = {H}')
+    d_k = d // H
+    check_head_dim(d_k)
     if out is None:
-        out = torch.empty(N, H * 64, dtype=BF16, device=qkv.device)
-    check(_lib.lib().otb_decode_self_attn(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax,
-                                          _stream()), 'otb_decode_self_attn')
+        out = torch.empty(N, d, dtype=BF16, device=qkv.device)
+    if d_k == 64:
+        check(_lib.lib().otb_decode_self_attn(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax,
+                                              _stream()), 'otb_decode_self_attn')
+    else:
+        check(_lib.lib().otb_decode_self_attn_dk(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax, d_k,
+                                                 _stream()), 'otb_decode_self_attn_dk')
     _count()
     return out
 

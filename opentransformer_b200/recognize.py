@@ -184,7 +184,7 @@ class BeamDecoder:
             # the `beam` hypotheses of utterance b are the query rows [b*beam, (b+1)*beam) of one attention problem
             # (the attention kernel pads the problem to 128 query rows)
             ctx = ops.attention(q, self.kvx[l], self.kvx[l], self.B, H, self.beam, self.T, kv_len=self.mem_len,
-                                k_col0=0, v_col0=d)
+                                k_col0=0, v_col0=d, d_k=d // H)
             x = _proj_resid_ln(ctx, p['wo2'], p['bo2'], x, None if nb else p['ln2'])
             if nb:
                 x = ops.layernorm(x, *p['ln3'])

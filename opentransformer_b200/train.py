@@ -47,6 +47,11 @@ class TrainPack:
             raise NotImplementedError('training path: conv front end + Transformer encoder / decoder only (round 1)')
         if enc.relative_positional:
             raise NotImplementedError('training path: absolute positions only')
+        for name, d_model, blocks in (('encoder', enc.d_model, enc.blocks), ('decoder', dec.d_model, dec.blocks)):
+            for blk in blocks:
+                if d_model != 64 * blk.n_heads:   # the attention backward (otb_attention_bwd) is written for 64-wide heads
+                    raise NotImplementedError(f'training path: 64-wide attention heads only; the {name} has d_model {d_model} '
+                                              f'with {blk.n_heads} heads')
         if fe.front_end_layer_norm or enc.pos_emb.scale_learnable or dec.pos_emb.scale_learnable:
             raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale')
         for blk in list(enc.blocks) + list(dec.blocks):
