@@ -73,10 +73,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         for (int i = 0; i < 2; ++i) mbar_init(&bar[i], 1);
         fence_barrier_init();
         tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmdO);
-        mbar_arrive_expect_tx(&bar[0], 32768);
-        tma_load_2d(sQ, &tmQ, &bar[0], p.q_col0 + h * 64, b * p.Tq + q0);
-        tma_load_2d(sdO, &tmdO, &bar[0], h * 64, b * p.Tq + q0);
-        if (nblk > 0) {
+        if (nblk > 0) {   // no visible key (kv_len 0): dQ is zero and no load may be left in flight when the CTA exits
+            mbar_arrive_expect_tx(&bar[0], 32768);
+            tma_load_2d(sQ, &tmQ, &bar[0], p.q_col0 + h * 64, b * p.Tq + q0);
+            tma_load_2d(sdO, &tmdO, &bar[0], h * 64, b * p.Tq + q0);
             mbar_arrive_expect_tx(&bar[1], 32768);
             tma_load_2d(sK, &tmK, &bar[1], p.k_col0 + h * 64, b * p.Tk);
             tma_load_2d(sV, &tmV, &bar[1], p.v_col0 + h * 64, b * p.Tk);

@@ -71,10 +71,12 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
         tma_prefetch_desc(&tmQ);
         tma_prefetch_desc(&tmK);
         tma_prefetch_desc(&tmV);
-        mbar_arrive_expect_tx(&bar[0], TILE);
-#pragma unroll
-        for (int x = 0; x < NB; ++x) tma_load_2d(sQ + x * 16384, &tmQ, &bar[0], p.q_col0 + h * DK + x * 64, b * p.Tq + q0);
+        // a row block with no visible key (kv_len 0) reads nothing: a Q load nobody waits for would still be landing in
+        // shared memory after the CTA has exited
         if (nblk > 0) {
+            mbar_arrive_expect_tx(&bar[0], TILE);
+#pragma unroll
+            for (int x = 0; x < NB; ++x) tma_load_2d(sQ + x * 16384, &tmQ, &bar[0], p.q_col0 + h * DK + x * 64, b * p.Tq + q0);
             mbar_arrive_expect_tx(&bar[1], TILE);
 #pragma unroll
             for (int x = 0; x < NB; ++x) tma_load_2d(sK + x * 16384, &tmK, &bar[1], p.k_col0 + h * DK + x * 64, b * p.Tk);

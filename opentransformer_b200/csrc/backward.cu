@@ -496,7 +496,9 @@ const char* col2im_s2_relu_launch(cudaStream_t st, const bf16* dcol, const bf16*
 }
 const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* x, float* out, int B, int T, int F, int T1,
                                int F1, int T2, int F2, int C) {
-    if (C < 1 || C > 256 || 256 % C) return "conv1_wgrad: C must divide 256";
+    // one thread per (channel, position lane): C <= 256 leaves at least one lane per channel (threads past the last full
+    // lane idle, e.g. C = 192); C > 256 would leave none and silently return zeros
+    if (C < 8 || C > 256 || C % 8) return "conv1_wgrad: C must be a multiple of 8, at most 256";
     const size_t smem = (size_t)17 * (F + 2) * sizeof(float);
     if (smem > 40 * 1024) return "conv1_wgrad: F too large";
     cudaError_t e = cudaMemsetAsync(out, 0, (size_t)C * 10 * 4, st);

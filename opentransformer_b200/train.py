@@ -52,6 +52,10 @@ class TrainPack:
                 if d_model != 64 * blk.n_heads:   # the attention backward (otb_attention_bwd) is written for 64-wide heads
                     raise NotImplementedError(f'training path: 64-wide attention heads only; the {name} has d_model {d_model} '
                                               f'with {blk.n_heads} heads')
+        C1 = fe.conv1.conv_layer.out_channels
+        if (C1 + 63) // 64 * 64 > 256:       # the conv1 weight gradient (otb_conv1_wgrad) runs one channel per thread
+            raise NotImplementedError(f'training path: mid_channel {C1} pads to {(C1 + 63) // 64 * 64} channels; the conv1 weight '
+                                      'gradient takes at most 256')
         if fe.front_end_layer_norm or enc.pos_emb.scale_learnable or dec.pos_emb.scale_learnable:
             raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale')
         for blk in list(enc.blocks) + list(dec.blocks):
@@ -483,8 +487,13 @@ class FusedTrainer:
         self.model = model
         self.params = [(n, p) for n, p in model.named_parameters() if p.requires_grad]
         dev = self.params[0][1].device
-        total = sum(p.numel() for _, p in self.params)
-        self.flat_p = torch.empty(total, dtype=torch.float32, device=dev)
+        # every parameter starts on a multiple of 8 elements: the kernels that write the fp32 gradient views (wgrad, colsum)
+        # and read the bf16 weight views through TMA need 16-byte aligned rows, whatever the sizes before them (an odd-sized
+        # bias such as the 4234-wide output bias would otherwise misalign the CTC head's weight that follows it).
+        # The gaps hold zeros, which the norm and the Adam step leave at zero.
+        span = {n: (p.numel() + 7) // 8 * 8 for n, p in self.params}
+        total = sum(span.values())
+        self.flat_p = torch.zeros(total, dtype=torch.float32, device=dev)
         self.flat_g = torch.zeros(total, dtype=torch.float32, device=dev)
         self.m = torch.zeros(total, dtype=torch.float32, device=dev)
         self.v = torch.zeros(total, dtype=torch.float32, device=dev)
@@ -498,7 +507,7 @@ class FusedTrainer:
                 self.flat_p[o:o + k].copy_(p.detach().reshape(-1))
                 p.data = self.flat_p[o:o + k].view_as(p)            # parameters now alias the flat buffer
                 self.offsets[n] = (o, k)
-                o += k
+                o += span[n]
         self.sink = {n: self.flat_g[o:o + k].view_as(p) for (n, p), (o, k) in zip(self.params, [self.offsets[n] for n, _ in self.params])}
         self._by_ptr = {p.data_ptr(): (self.offsets[n], p.shape) for n, p in self.params}
         self.betas, self.eps, self.wd, self.clip = betas, eps, weight_decay, clip_grad
