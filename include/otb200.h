@@ -78,14 +78,21 @@ int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, 
                    void* stream);
 
 /* nn.Linear with a fused epilogue on wgmma tensor cores: out[M,N] = epi(a[M,K] w[N(,2N),K]^T + bias).
- * a, w bf16 (lda, ldw in elements, multiples of 8); out bf16 or f32 (out_f32); unused pointers NULL.
- * row_len/row_period: optional key-padding mask, rows with (m % row_period) >= row_len[m / row_period]
- * produce 0 before the residual is added (conformer.py:46,55 masked_fill).
+ * a, w bf16 (lda, ldw in elements, multiples of 8); out bf16 or f32 (out_f32; RESID and RESID_LN write bf16 only and
+ * refuse out_f32); unused pointers NULL.  Only the [M, N] window of out (row pitch ldc) is written.
+ * row_len/row_period: optional key-padding mask (conformer.py:46,55 masked_fill).  A masked row, one with
+ * (m % row_period) >= row_len[m / row_period], has its GEMM result and bias replaced by 0 before the epilogue's
+ * residual is added: it yields resid for RESID, LayerNorm(resid) * gamma + beta for RESID_LN, and 0 for every other
+ * epilogue (TABLE included: a masked row gets 0, not its table row).
  * Replaces attention.py:68,128-129,44; ffn.py:39-41; frontend/conv.py:146; decoder/transformer.py:181. */
 int otb_linear(const void* a, int lda, const void* w, int ldw, const float* bias, void* out, int ldc, int M, int N,
                int K, int epilogue, int out_f32, const void* resid, int ldr, const float* gamma, const float* beta,
                float eps, float alpha, const float* table, int period, const int* row_len, int row_period,
                void* stream);
+/* Host only, launches nothing: the N tile width (64, 128 or 256) otb_linear would launch for an M x N output with this
+ * epilogue and output type under the current tile policy (otb_set_tile_policy), in *bn.  Returns non-zero, with the
+ * message otb_linear would give, for the combinations otb_linear refuses whatever its operands. */
+int otb_gemm_config(int M, int N, int epilogue, int out_f32, int* bn);
 
 /* Training-mode residual connection with nn.Dropout on the sub-layer output (encoder/transformer.py:32-33,54,61;
  * decoder/transformer.py:36-38 `residual_dropout`): out bf16 = resid + alpha * keep * (a w^T + bias) / (1 - p), where

@@ -50,6 +50,7 @@ _SIGS = {
     'otb_conv2_relu': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_linear': (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, _P,
                            c_float, c_float, _P, c_int, _P, c_int, _P]),
+    'otb_gemm_config': (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int)]),
     'otb_linear_dropout_resid': (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, c_float, c_float, _P,
                                          ctypes.c_uint32, _P]),
     'otb_dropout_bwd': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_float, _P, ctypes.c_uint32, _P]),

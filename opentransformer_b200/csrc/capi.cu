@@ -151,6 +151,16 @@ int otb_linear(const void* a, int lda, const void* w, int ldw, const float* bias
     RET("otb_linear", gemm_launch(ST(stream), a, lda, w, ldw, w_rows, epilogue, p, nullptr));
 }
 
+int otb_gemm_config(int M, int N, int epilogue, int out_f32, int* bn) {
+    if (epilogue < 0 || epilogue > EPI_TANH) return fail("otb_gemm_config", "unknown epilogue");
+    if (M <= 0 || N <= 0) return fail("otb_gemm_config", "gemm: empty problem");
+    int b = 0;
+    const char* e = gemm_tile((M + 127) / 128, N, epilogue, out_f32 ? 1 : 0, &b);
+    if (e) return fail("otb_gemm_config", e);
+    if (bn) *bn = b;
+    return 0;
+}
+
 int otb_linear_dropout_resid(const void* a, int lda, const void* w, int ldw, const float* bias, void* out, int ldc, int M, int N, int K,
                              const void* resid, int ldr, float alpha, float p_drop, const uint32_t* seed, uint32_t site, void* stream) {
     if (!a || !w || !out || !resid || !seed) return fail("otb_linear_dropout_resid", "null operand");

@@ -334,6 +334,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     s2[hh] += x0 * x0 + x1 * x1;
                 }
             }
+            const float inv_n = 1.0f / (float)BN;
+            float mean[2], var[2];
+            bool recentre[2];
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
 #pragma unroll
@@ -341,16 +344,38 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     s1[hh] += __shfl_xor_sync(0xffffffffu, s1[hh], o);
                     s2[hh] += __shfl_xor_sync(0xffffffffu, s2[hh], o);
                 }
-                const float inv_n = 1.0f / (float)BN;
-                const float mean = s1[hh] * inv_n;
-                const float var = fmaxf(s2[hh] * inv_n - mean * mean, 0.f);
-                const float rstd = rsqrtf(var + p.eps);
+                mean[hh] = s1[hh] * inv_n;
+                var[hh] = fmaxf(s2[hh] * inv_n - mean[hh] * mean[hh], 0.f);
+                // E[x^2] - mean^2 loses about log2(mean^2 / var) bits to cancellation: beyond 6 of them, recompute the
+                // variance of the centred values (a second pass over the registers, as layernorm_kernel does)
+                recentre[hh] = mean[hh] * mean[hh] > 64.f * var[hh];
+            }
+            if (__any_sync(0xffffffffu, recentre[0] || recentre[1])) {   // warp-uniform: the whole warp shuffles
+                float q[2] = {0.f, 0.f};
+#pragma unroll
+                for (int jj = 0; jj < BN / 8; ++jj) {
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const float d0 = acc[4 * jj + 2 * hh] - mean[hh], d1 = acc[4 * jj + 2 * hh + 1] - mean[hh];
+                        q[hh] = fmaf(d0, d0, fmaf(d1, d1, q[hh]));
+                    }
+                }
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+                    for (int o = 1; o < 4; o <<= 1) q[hh] += __shfl_xor_sync(0xffffffffu, q[hh], o);
+                    if (recentre[hh]) var[hh] = q[hh] * inv_n;
+                }
+            }
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                const float rstd = rsqrtf(var[hh] + p.eps);
                 uint8_t* row_ptr = stg + (rl0 + 8 * hh) * pitch;
 #pragma unroll
                 for (int jj = 0; jj < BN / 8; ++jj) {
                     const int c = jj * 8 + cq;
-                    stage2(row_ptr, c, 0, (acc[4 * jj + 2 * hh] - mean) * rstd * s_gamma[c] + s_beta[c],
-                           (acc[4 * jj + 2 * hh + 1] - mean) * rstd * s_gamma[c + 1] + s_beta[c + 1]);
+                    stage2(row_ptr, c, 0, (acc[4 * jj + 2 * hh] - mean[hh]) * rstd * s_gamma[c] + s_beta[c],
+                           (acc[4 * jj + 2 * hh + 1] - mean[hh]) * rstd * s_gamma[c + 1] + s_beta[c + 1]);
                 }
             }
         } else if (EPI == EPI_GLU) {
@@ -443,8 +468,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 if (orow < 0) continue;
                 const uint8_t* src = stg + r * pitch;
                 uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)orow * p.ldc + col_base) * esize;
-                for (int off = lane * 2; off < row_bytes; off += 64)
-                    *reinterpret_cast<uint16_t*>(dst + off) = *reinterpret_cast<const uint16_t*>(src + off);
+                if (TN && (splitk > 1 || p.accum)) {   // as above, one fp32 element at a time (ncols % 4 != 0)
+                    for (int c = lane; c < ncols; c += 32)
+                        atomicAdd(reinterpret_cast<float*>(dst) + c, reinterpret_cast<const float*>(src)[c]);
+                } else {
+                    for (int off = lane * 2; off < row_bytes; off += 64)
+                        *reinterpret_cast<uint16_t*>(dst + off) = *reinterpret_cast<const uint16_t*>(src + off);
+                }
             }
         }
         epi_bar<kEpiThreads>();  // staging / bias smem may be rewritten for the next tile
@@ -593,6 +623,18 @@ static int choose_bn(int m_tiles, int n_cols, int epi, int out_f32) {
     return best;
 }
 
+// The checks of gemm_launch that depend only on the output shape, the epilogue and the output type, and the tile width
+// it launches (m_tiles 128-row blocks, current tile policy).  Host only: otb_gemm_config answers with it.
+const char* gemm_tile(int m_tiles, int N, int epi, int out_f32, int* bn) {
+    if (epi == EPI_RESID_LN && !(N == 64 || N == 128 || N == 256))
+        return "gemm: fused residual+LayerNorm epilogue needs N in {64,128,256}";
+    if (epi == EPI_RESID_LN && out_f32) return "gemm: fused residual+LayerNorm epilogue writes bf16";
+    // the residual tile is staged as bf16 in the rows the fp32 results would overwrite
+    if (epi == EPI_RESID && out_f32) return "gemm: residual epilogue writes bf16";
+    *bn = choose_bn(m_tiles, N, epi, out_f32);
+    return *bn == 0 ? "gemm: no tile configuration" : nullptr;
+}
+
 const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, int ldw, int w_rows, int epi,
                         GemmParams p, const CUtensorMap* conv_map) {
     if (p.M <= 0 || p.N <= 0 || p.K <= 0) return "gemm: empty problem";
@@ -604,11 +646,9 @@ const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, 
     if ((epi == EPI_RESID || epi == EPI_RESID_LN) && ((p.ldr % 8) || (reinterpret_cast<uintptr_t>(p.resid) & 15)))
         return "gemm: residual must be 16-byte aligned with ldr % 8 == 0";
     const int m_tiles = p.conv ? (p.conv_B * p.conv_T1h + p.conv_R - 1) / p.conv_R : (p.M + BM - 1) / BM;
-    if (epi == EPI_RESID_LN && !(p.N == 64 || p.N == 128 || p.N == 256))
-        return "gemm: fused residual+LayerNorm epilogue needs N in {64,128,256}";
-    if (epi == EPI_RESID_LN && p.out_f32) return "gemm: fused residual+LayerNorm epilogue writes bf16";
-    const int bn = choose_bn(m_tiles, p.N, epi, p.out_f32);
-    if (bn == 0) return "gemm: no tile configuration";
+    int bn = 0;
+    const char* err;
+    if ((err = gemm_tile(m_tiles, p.N, epi, p.out_f32, &bn))) return err;
     const int bn_out = (epi == EPI_GLU) ? bn / 2 : bn;
     const int n_tiles = (p.N + bn_out - 1) / bn_out;
     const int bm = (bn == 256) ? GemmCfg<256>::BM : BM;   // rows per tile of the chosen configuration
@@ -616,7 +656,6 @@ const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, 
     const int num_tiles = (p.conv ? m_tiles : (p.M + bm - 1) / bm) * n_tiles;
 
     CUtensorMap ta, tb;
-    const char* err;
     if (p.conv) {
         if (!conv_map) return "gemm: conv mode needs a conv tensor map";
         ta = *conv_map;

@@ -59,6 +59,8 @@ struct GemmParams {
 
 const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, int ldw, int w_rows, int epi,
                         GemmParams p, const CUtensorMap* conv_map);
+// shape / epilogue checks of gemm_launch and the tile width it picks for m_tiles 128-row blocks (host only)
+const char* gemm_tile(int m_tiles, int N, int epi, int out_f32, int* bn);
 
 const char* gemm_wgrad_launch(cudaStream_t st, const void* dY, int lddy, const void* X, int ldx, float* out, int ldc,
                               int Mact, int Nw, int Kw, int accumulate);

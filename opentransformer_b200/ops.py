@@ -139,6 +139,14 @@ def linear(a, w, bias=None, epilogue=EPI_BIAS, out=None, out_f32=False, resid=No
     return out
 
 
+def gemm_config(M, N, epilogue=EPI_BIAS, out_f32=False):
+    """N tile width (64, 128 or 256) linear() launches for an M x N output under the current tile policy
+    (otb_gemm_config: host only, no GPU needed); raises RuntimeError where linear() would refuse the combination."""
+    bn = ctypes.c_int()
+    check(_lib.lib().otb_gemm_config(M, N, epilogue, 1 if out_f32 else 0, bn), 'otb_gemm_config')
+    return bn.value
+
+
 def linear_dropout_resid(a, w, bias, resid, p, seed, site, alpha=1.0, out=None):
     """out = resid + alpha * dropout_p(a @ w^T + bias): training-mode residual connection (otb_linear_dropout_resid).
     seed: int32/uint32 device tensor [1] (read at run time), site: dropout site id."""

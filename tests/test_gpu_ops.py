@@ -128,7 +128,18 @@ def test_sinusoid_table_matches_torch_cpu_formula():
 # ------------------------------------------------------------------------------------------------ conv front end
 @pytest.mark.parametrize('B,T,Fdim,C1,C2', [(2, 200, 80, 64, 128), (3, 1000, 80, 64, 128), (2, 91, 40, 64, 128),
                                             (1, 77, 83, 64, 64), (2, 64, 20, 128, 256)])
-def test_conv_subsampling(B, T, Fdim, C1, C2):
+@pytest.mark.parametrize('policy', ['latency', 'throughput'])
+def test_conv_subsampling(B, T, Fdim, C1, C2, policy):
+    """conv1 + conv2's implicit GEMM.  Under the throughput policy the two shapes with at most 4 row blocks (T 91 and 64)
+    take 128-wide tiles where the latency policy takes 64-wide ones."""
+    ops.set_tile_policy(policy)
+    try:
+        _conv_subsampling(B, T, Fdim, C1, C2)
+    finally:
+        ops.set_tile_policy('latency')
+
+
+def _conv_subsampling(B, T, Fdim, C1, C2):
     x = _rnd(B, T, Fdim, seed=1)
     w1 = _rnd(C1, 1, 3, 3, scale=0.3, seed=2)
     b1 = _rnd(C1, scale=0.1, seed=3)
