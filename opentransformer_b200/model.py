@@ -101,10 +101,6 @@ class SpeechToText(nn.Module):
             return (1 - self.ctc_weight) * loss + self.ctc_weight * lc, {'CTCLoss': float(lc)}
         return loss, None
 
-    def _logits_padded(self, inputs, mask, targets_in):
-        mem, lengths, B, T2 = self.encode_bf16(inputs, mask)
-        return self.decoder.forward_bf16(targets_in, mem, lengths, B, targets_in.shape[1], T2)
-
     def save_checkpoint(self, params, name):
         chk = {'params': params, 'frontend': self.frontend.state_dict(),
                'encoder': self.encoder.state_dict(), 'decoder': self.decoder.state_dict()}

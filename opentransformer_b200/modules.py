@@ -255,6 +255,15 @@ def _proj_resid_ln(ctx, w, b, resid, ln):
     return ops.layernorm(y, *ln) if ln is not None else y
 
 
+def _self_attn(y, resid, p, H, B, T, lengths, causal=False, ln=None):
+    """resid + output_proj(MHA(y)) (+ LayerNorm): QKV GEMM -> fused attention -> output projection with the residual."""
+    d = y.shape[1]
+    qkv = ops.linear(y, p['wqkv'], p['bqkv'])
+    ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d, v_col0=2 * d,
+                        d_k=d // H)
+    return _proj_resid_ln(ctx, p['wo'], p['bo'], resid, ln)
+
+
 def _ffn_pack(ff):
     return {'w1': _w(ff.w_1), 'b1': _b(ff.w_1), 'w2': _w(ff.w_2), 'b2': _b(ff.w_2),
             'act': ACT_EPILOGUE[ff.activation]}
@@ -295,25 +304,21 @@ class TransformerEncoderLayer(nn.Module):
     def run(self, x, pk, B, T, lengths, causal=False, pos_bf16=None):
         """x bf16 [B*T, d] -> bf16 [B*T, d]   (encoder/transformer.py:41-65); causal=True is the tril mask the
         Transformer LM feeds to the same layer (model/lm.py:14-18,148-151)."""
-        d, H = x.shape[1], self.n_heads
-        if self.normalize_before:
+        nb = self.normalize_before
+        if nb:
             x = ops.layernorm(x, *pk['ln1'])          # residual is taken AFTER the norm (transformer.py:42-44)
+        ln = None if nb else pk['ln1']
         if self.relative_positional:
             if causal:
                 raise NotImplementedError('causal rel-pos attention')
             x = self.slf_attn.run(x, x, pk['rel'], B, T, lengths, pos_bf16)       # x + attention (no output projection)
-            if not self.normalize_before:
-                x = ops.layernorm(x, *pk['ln1'])
-            if self.normalize_before:
-                x = ops.layernorm(x, *pk['ln2'])
-            return _ffn(x, pk['ffn'], x, None if self.normalize_before else pk['ln2'])
-        qkv = ops.linear(x, pk['wqkv'], pk['bqkv'])
-        ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d,
-                            v_col0=2 * d, d_k=d // H)
-        x = _proj_resid_ln(ctx, pk['wo'], pk['bo'], x, None if self.normalize_before else pk['ln1'])
-        if self.normalize_before:
+            if ln is not None:
+                x = ops.layernorm(x, *ln)
+        else:
+            x = _self_attn(x, x, pk, self.n_heads, B, T, lengths, causal, ln)
+        if nb:
             x = ops.layernorm(x, *pk['ln2'])
-        return _ffn(x, pk['ffn'], x, None if self.normalize_before else pk['ln2'])
+        return _ffn(x, pk['ffn'], x, None if nb else pk['ln2'])
 
 
 class TransformerEncoder(nn.Module):
@@ -491,10 +496,7 @@ class ConformerEncoderBlock(nn.Module):
         y = ops.layernorm(x, *pk['mha_ln'])
         if self.relative_positional:
             return self.mha.run(y, x, pk['mha'], B, T, lengths, pos_bf16)
-        d, H, m = x.shape[1], self.n_heads, pk['mha']
-        qkv = ops.linear(y, m['wqkv'], m['bqkv'])
-        ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
-        return ops.linear(ctx, m['wo'], m['bo'], EPI_RESID, resid=x)
+        return _self_attn(y, x, pk['mha'], self.n_heads, B, T, lengths)
 
     def _conv(self, x, pk, B, T, lengths):
         return self.conv.run(ops.layernorm(x, *pk['conv_ln']), x, pk['conv'], B, T, lengths)
@@ -692,6 +694,37 @@ class TransformerDecoder(nn.Module):
     def ld_logits(self):
         return (self.vocab_size + 7) // 8 * 8
 
+    def _layers(self, pk, x, self_attn, cross_attn):
+        """The decoder layers (decoder/transformer.py:54-90) and the final after_norm over x bf16 [rows, d].  Only the
+        attention contexts depend on the caller: self_attn(l, qkv) and cross_attn(l, q) return those of layer l."""
+        nb = self.normalize_before
+        for l, p in enumerate(pk['blocks']):
+            if nb:
+                x = ops.layernorm(x, *p['ln1'])
+            qkv = ops.linear(x, p['wqkv'], p['bqkv'])
+            x = _proj_resid_ln(self_attn(l, qkv), p['wo'], p['bo'], x, None if nb else p['ln1'])
+            if nb:
+                x = ops.layernorm(x, *p['ln2'])
+            q = ops.linear(x, p['wq'], p['bq'])
+            x = _proj_resid_ln(cross_attn(l, q), p['wo2'], p['bo2'], x, None if nb else p['ln2'])
+            if nb:
+                x = ops.layernorm(x, *p['ln3'])
+            x = _ffn(x, p['ffn'], x, None if nb else p['ln3'])
+        if nb:
+            x = ops.layernorm(x, *pk['after'])
+        return x
+
+    def decode_cached_bf16(self, pk, x, kc, vc, anc, step_ptr, kvx, mem_len, beam, T):
+        """The layers on the newest token of N = batch * beam hypotheses, x bf16 [N, d].  Self-attention reads the cached
+        keys / values kc, vc [layer, position, row, d] through the ancestry table `anc`; cross-attention reads the memory's
+        K|V kvx [layer, batch * T, 2d], projected once per utterance."""
+        d, H, N, Lmax, batch = self.d_model, self.n_heads, x.shape[0], kc.shape[1], mem_len.shape[0]
+        return self._layers(
+            pk, x, lambda l, qkv: ops.decode_self_attn(qkv, kc[l], vc[l], anc, step_ptr, N, H, Lmax),
+            # the `beam` hypotheses of utterance b are the query rows [b*beam, (b+1)*beam) of one attention problem
+            # (the attention kernel pads the problem to 128 query rows)
+            lambda l, q: ops.attention(q, kvx[l], kvx[l], batch, H, beam, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H))
+
     def forward_bf16(self, targets, memory_bf16, mem_len, B, L, T):
         """targets i64 [B,L]; memory bf16 [B*T, D] -> logits f32 [B*L, ld_logits] (first V columns valid)."""
         _no_train(self)
@@ -701,24 +734,16 @@ class TransformerDecoder(nn.Module):
         if self.pos_emb.scale_learnable:
             raise NotImplementedError('decoder with learnable positional scale')
         x = ops.embed_posenc(targets.contiguous(), pk['emb'], table, B * L, d, period=L)
-        for blk, p in zip(self.blocks, pk['blocks']):
-            nb = blk.normalize_before
-            if nb:
-                x = ops.layernorm(x, *p['ln1'])
-            qkv = ops.linear(x, p['wqkv'], p['bqkv'])
-            ctx = ops.attention(qkv, qkv, qkv, B, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
-            x = _proj_resid_ln(ctx, p['wo'], p['bo'], x, None if nb else p['ln1'])
-            if nb:
-                x = ops.layernorm(x, *p['ln2'])
-            q = ops.linear(x, p['wq'], p['bq'])
+
+        def self_attn(l, qkv):
+            return ops.attention(qkv, qkv, qkv, B, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
+
+        def cross_attn(l, q):       # the memory's K|V, projected per layer after the query GEMM
+            p = pk['blocks'][l]
             kv = ops.linear(memory_bf16, p['wkv'], p['bkv'])
-            ctx = ops.attention(q, kv, kv, B, H, L, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H)
-            x = _proj_resid_ln(ctx, p['wo2'], p['bo2'], x, None if nb else p['ln2'])
-            if nb:
-                x = ops.layernorm(x, *p['ln3'])
-            x = _ffn(x, p['ffn'], x, None if nb else p['ln3'])
-        if self.normalize_before:
-            x = ops.layernorm(x, *pk['after'])
+            return ops.attention(q, kv, kv, B, H, L, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H)
+
+        x = self._layers(pk, x, self_attn, cross_attn)
         return ops.linear(x, pk['wout'], pk['bout'], EPI_BIAS, out_f32=True, n_out=self.ld_logits)
 
     def forward(self, targets, memory, memory_mask):
@@ -758,28 +783,10 @@ class TransformerDecoder(nn.Module):
             raise ValueError('DecoderCache is full (max_len reached)')
         if self.pos_emb.scale_learnable:
             raise NotImplementedError('decoder with learnable positional scale')
-        d, H, N = self.d_model, self.n_heads, c.N
         c.step_dev.fill_(c.step)
         tok = preds[:, -1].contiguous()
-        x = ops.embed_posenc(tok, pk['emb'], c.table, N, d, step_ptr=c.step_dev)
-        for l, (blk, p) in enumerate(zip(self.blocks, pk['blocks'])):
-            nb = blk.normalize_before
-            if nb:
-                x = ops.layernorm(x, *p['ln1'])
-            qkv = ops.linear(x, p['wqkv'], p['bqkv'])
-            ctx = ops.decode_self_attn(qkv, c.kc[l], c.vc[l], c.anc, c.step_dev, N, H, c.Lmax)
-            x = _proj_resid_ln(ctx, p['wo'], p['bo'], x, None if nb else p['ln1'])
-            if nb:
-                x = ops.layernorm(x, *p['ln2'])
-            q = ops.linear(x, p['wq'], p['bq'])
-            ctx = ops.attention(q, c.kvx[l], c.kvx[l], c.batch, H, c.beam, c.T, kv_len=c.mem_len, k_col0=0, v_col0=d,
-                                d_k=d // H)
-            x = _proj_resid_ln(ctx, p['wo2'], p['bo2'], x, None if nb else p['ln2'])
-            if nb:
-                x = ops.layernorm(x, *p['ln3'])
-            x = _ffn(x, p['ffn'], x, None if nb else p['ln3'])
-        if self.normalize_before:
-            x = ops.layernorm(x, *pk['after'])
+        x = ops.embed_posenc(tok, pk['emb'], c.table, c.N, self.d_model, step_ptr=c.step_dev)
+        x = self.decode_cached_bf16(pk, x, c.kc, c.vc, c.anc, c.step_dev, c.kvx, c.mem_len, c.beam, c.T)
         logits = ops.linear(x, pk['wout'], pk['bout'], EPI_BIAS, out_f32=True, n_out=self.ld_logits)
         c.step += 1
         attn = {'dec_block_%d' % i: {'slf_attn_weights': None, 'src_attn_weights': None} for i in range(len(self.blocks))}

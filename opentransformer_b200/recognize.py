@@ -16,7 +16,6 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
 import torch
 
 from . import ops
-from .modules import _lengths, _ffn, _proj_resid_ln
 
 PAD, BOS, EOS = 0, 1, 1   # otrans/data/__init__.py:7-10
 
@@ -169,28 +168,8 @@ class BeamDecoder:
     def _step_kernels(self):
         dec, st = self.dec, self.state
         pk = dec.packed()
-        d, H, N = dec.d_model, dec.n_heads, self.N
-        x = ops.embed_posenc(st.last_tok, pk['emb'], self.table, N, d, step_ptr=st.step_ptr)
-        for l, (blk, p) in enumerate(zip(dec.blocks, pk['blocks'])):
-            nb = blk.normalize_before
-            if nb:
-                x = ops.layernorm(x, *p['ln1'])
-            qkv = ops.linear(x, p['wqkv'], p['bqkv'])
-            ctx = ops.decode_self_attn(qkv, self.kc[l], self.vc[l], st.anc, st.step_ptr, N, H, self.Lmax)
-            x = _proj_resid_ln(ctx, p['wo'], p['bo'], x, None if nb else p['ln1'])
-            if nb:
-                x = ops.layernorm(x, *p['ln2'])
-            q = ops.linear(x, p['wq'], p['bq'])
-            # the `beam` hypotheses of utterance b are the query rows [b*beam, (b+1)*beam) of one attention problem
-            # (the attention kernel pads the problem to 128 query rows)
-            ctx = ops.attention(q, self.kvx[l], self.kvx[l], self.B, H, self.beam, self.T, kv_len=self.mem_len,
-                                k_col0=0, v_col0=d, d_k=d // H)
-            x = _proj_resid_ln(ctx, p['wo2'], p['bo2'], x, None if nb else p['ln2'])
-            if nb:
-                x = ops.layernorm(x, *p['ln3'])
-            x = _ffn(x, p['ffn'], x, None if nb else p['ln3'])
-        if dec.normalize_before:
-            x = ops.layernorm(x, *pk['after'])
+        x = ops.embed_posenc(st.last_tok, pk['emb'], self.table, self.N, dec.d_model, step_ptr=st.step_ptr)
+        x = dec.decode_cached_bf16(pk, x, self.kc, self.vc, st.anc, st.step_ptr, self.kvx, self.mem_len, self.beam, self.T)
         ops.linear(x, pk['wout'], pk['bout'], out=self.logits)
         ops.logsoftmax_topk(self.logits, dec.vocab_size, self.beam, self.lm_logp, self.lm_weight,
                             out_val=self.topk_val, out_idx=self.topk_idx,
@@ -330,19 +309,7 @@ class SpeechToTextRecognizer(Recognizer):
 
     # ---- fast path ------------------------------------------------------------------------------
     def _encode_bf16(self, inputs, inputs_mask):
-        fe, enc = self.model.frontend, self.model.encoder
-        B, T, _ = inputs.shape
-        _, _, T2, _ = ops.conv_geometry(T, fe.input_size)
-        lengths = _lengths(fe.output_mask(inputs_mask))
-        fused = getattr(enc, 'fuse_abs_posenc', None)
-        if fused is not None and fused():
-            scale, table = enc.pos_emb.scale_and_table(T2, inputs.device)
-            x, _ = fe.forward_bf16(inputs, scale, table)
-        else:
-            x, _ = fe.forward_bf16(inputs)
-            x = enc.apply_posenc_bf16(x, B, T2)
-        mem = enc.forward_bf16(x, B, T2, lengths)
-        return mem, lengths, B, T2
+        return self.model.encode_bf16(inputs, inputs_mask)
 
     def _decoder_for(self, B, T2, device):
         key = (B, self.beam_width, T2, self.max_len, device.index)

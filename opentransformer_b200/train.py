@@ -17,6 +17,7 @@ epilogue, replayed in the backward; csrc/dropout.cuh); the other dropout rates m
 otherwise.  Conformer / pre-norm training is not built yet and raises.
 """
 import math
+from collections import namedtuple
 
 import torch
 
@@ -33,6 +34,10 @@ def _bf(t):
 
 def _f(t):
     return t.detach().float().contiguous()
+
+
+_Lin = namedtuple('_Lin', 'w wt b name')      # W [N,K], W^T [K,N], fp32 bias, qualified module name
+_Norm = namedtuple('_Norm', 'g b name')
 
 
 class TrainPack:
@@ -70,6 +75,7 @@ class TrainPack:
                 raise NotImplementedError(f'training path: only residual_dropout is implemented, got {other}; set them to 0.0')
             if not (0.0 <= float(rates.get('residual_dropout', 0.0)) < 1.0):
                 raise ValueError('residual_dropout must be in [0, 1)')
+        self._names = {m: n for n, m in model.named_modules()}
         self.fe = self._frontend(fe)
         self.enc = [self._enc_layer(b) for b in enc.blocks]
         self.dec = [self._dec_layer(b) for b in dec.blocks]
@@ -91,11 +97,10 @@ class TrainPack:
 
     def _lin(self, lin):
         w = self._w(lin.weight)
-        return w, w.t().contiguous(), _f(lin.bias)
+        return _Lin(w, w.t().contiguous(), _f(lin.bias), self._names[lin])
 
-    @staticmethod
-    def _ln(norm):
-        return _f(norm.weight), _f(norm.bias)
+    def _ln(self, norm):
+        return _Norm(_f(norm.weight), _f(norm.bias), self._names[norm])
 
     def _frontend(self, fe):
         pk = dict(fe._build_pack())
@@ -136,23 +141,27 @@ class _Grads(dict):
             self[name] = value.contiguous()
 
 
-def _ln_bwd(dy, z, gamma, grads, wname, bname):
+def _norm(x, ln):
+    return ops.layernorm(x, ln.g, ln.b)
+
+
+def _ln_bwd(dy, z, ln, grads):
     acc = grads.sink is not None
-    dz, dg, db = ops.layernorm_bwd(dy, z, gamma, dgamma=grads.out(wname), dbeta=grads.out(bname), accumulate=acc)
+    wname, bname = ln.name + '.weight', ln.name + '.bias'
+    dz, dg, db = ops.layernorm_bwd(dy, z, ln.g, dgamma=grads.out(wname), dbeta=grads.out(bname), accumulate=acc)
     grads[wname], grads[bname] = dg, db
     return dz
 
 
-def _linear_bwd(dy, x, wt, grads, wname, bname, resid=None):
+def _linear_bwd(dy, x, lin, grads, resid=None):
     """Gradients of y = x W^T + b: parameter grads into `grads`, returns dx (+ resid) as bf16."""
     acc = grads.sink is not None
+    wname, bname = lin.name + '.weight', lin.name + '.bias'
     grads[wname] = ops.linear_wgrad(dy, x, out=grads.out(wname), accumulate=acc)
     grads[bname] = ops.colsum(dy, out=grads.out(bname), accumulate=acc)
-    if wt is None:
-        return None
     if resid is not None:
-        return ops.linear(dy, wt, None, EPI_RESID, resid=resid)
-    return ops.linear(dy, wt)
+        return ops.linear(dy, lin.wt, None, EPI_RESID, resid=resid)
+    return ops.linear(dy, lin.wt)
 
 
 ENC_SITE, DEC_SITE = 0, 1000      # dropout site ids: encoder layer i -> 2 i + {0, 1}; decoder layer i -> 1000 + 3 i + {0, 1, 2}
@@ -161,9 +170,9 @@ ENC_SITE, DEC_SITE = 0, 1000      # dropout site ids: encoder layer i -> 2 i + {
 def _ffn_fwd(p, x):
     """First half of the position-wise feed-forward (ffn.py:38-41): returns (pre-activation u or None, hidden h)."""
     if p['act'] == 'glu':
-        u = ops.linear(x, p['w1'][0], p['w1'][2])
+        u = ops.linear(x, p['w1'].w, p['w1'].b)
         return u, ops.glu_fwd(u)
-    return None, ops.linear(x, p['w1'][0], p['w1'][2], EPI_RELU)      # ReLU fused into the GEMM; its backward needs only h
+    return None, ops.linear(x, p['w1'].w, p['w1'].b, EPI_RELU)      # ReLU fused into the GEMM; its backward needs only h
 
 
 def _ffn_act_bwd(p, dh, u, h):
@@ -180,15 +189,100 @@ def dropout_sites(model):
     return out
 
 
-def _resid(ctx, w, b, x, rate, seed, site):
-    """x + dropout(ctx W^T + b): the residual connection of a sub-layer in training mode (transformer.py:54,61)."""
+def _resid(ctx, lin, x, drop, k):
+    """x + dropout(ctx W^T + b): the residual connection of sub-layer k in training mode (transformer.py:54,61).
+    drop = (rate, seed tensor, site id of the layer's sub-layer 0)."""
+    rate, seed, site = drop
     if rate > 0.0:
-        return ops.linear_dropout_resid(ctx, w, b, x, rate, seed, site)
-    return ops.linear(ctx, w, b, EPI_RESID, resid=x)
+        return ops.linear_dropout_resid(ctx, lin.w, lin.b, x, rate, seed, site + k)
+    return ops.linear(ctx, lin.w, lin.b, EPI_RESID, resid=x)
 
 
-def _drop_bwd(dz, rate, seed, site):
-    return ops.dropout_bwd(dz, rate, seed, site) if rate > 0.0 else dz
+def _drop_bwd(dz, drop, k):
+    rate, seed, site = drop
+    return ops.dropout_bwd(dz, rate, seed, site + k) if rate > 0.0 else dz
+
+
+# What a layer saves for its backward.  Sub-layer k has input u_k and residual sum z_k = u_k + drop(f_k(u_k)).  Pre-norm
+# (the reference takes the residual AFTER the norm): u_1 = norm1(a), u_k+1 = norm_k+1(z_k), the output is z_last.
+# Post-norm: u_1 = a, u_k+1 = norm_k(z_k), the output is norm_last(z_last).  a is the layer input; ffn_u is the GLU's
+# pre-activation (None with ReLU) and h the feed-forward's hidden activation.
+_EncTape = namedtuple('_EncTape', 'a u1 qkv ctx lse z1 u2 ffn_u h z2')
+_DecTape = namedtuple('_DecTape', 'a u1 qkv ctx lse z1 u2 q kv ctx2 lse2 z2 u3 ffn_u h z3')
+
+
+def _enc_layer_fwd(p, a, pre, B, H, T, lengths, drop):
+    """One encoder layer in training mode (encoder/transformer.py:41-65) -> (output, _EncTape)."""
+    d = a.shape[1]
+    u1 = _norm(a, p['ln1']) if pre else a
+    qkv = ops.linear(u1, p['qkv'].w, p['qkv'].b)
+    ctx, lse = ops.attention_train(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=d, v_col0=2 * d)
+    z1 = _resid(ctx, p['o'], u1, drop, 0)
+    u2 = _norm(z1, p['ln2'] if pre else p['ln1'])
+    ffn_u, h = _ffn_fwd(p, u2)
+    z2 = _resid(h, p['w2'], u2, drop, 1)
+    out = z2 if pre else _norm(z2, p['ln2'])
+    return out, _EncTape(a=a, u1=u1, qkv=qkv, ctx=ctx, lse=lse, z1=z1, u2=u2, ffn_u=ffn_u, h=h, z2=z2)
+
+
+def _enc_layer_bwd(p, t, dout, pre, g, B, H, T, lengths, drop):
+    """Backward of _enc_layer_fwd: parameter gradients into g; returns the gradient of the layer input."""
+    d = t.a.shape[1]
+    dz2 = dout if pre else _ln_bwd(dout, t.z2, p['ln2'], g)
+    # the sub-layer branch sees the replayed dropout mask, the residual branch (resid=) the plain gradient
+    dh = _linear_bwd(_drop_bwd(dz2, drop, 1), t.h, p['w2'], g)
+    du2 = _linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.u2, p['w1'], g, resid=dz2)
+    dz1 = _ln_bwd(du2, t.z1, p['ln2'] if pre else p['ln1'], g)
+    dctx = _linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
+    dqkv = torch.empty_like(t.qkv)
+    ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B, H, T, T, dqkv, dqkv, dqkv, kv_len=lengths, q_col0=0,
+                      k_col0=d, v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
+    du1 = _linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
+    return _ln_bwd(du1, t.a, p['ln1'], g) if pre else du1
+
+
+def _dec_layer_fwd(p, a, mem, pre, B, H, L, T, lengths, drop):
+    """One decoder layer in training mode (decoder/transformer.py:54-90) over the memory mem -> (output, _DecTape)."""
+    d = a.shape[1]
+    u1 = _norm(a, p['ln1']) if pre else a
+    qkv = ops.linear(u1, p['qkv'].w, p['qkv'].b)
+    ctx, lse = ops.attention_train(qkv, qkv, qkv, B, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d)
+    z1 = _resid(ctx, p['o'], u1, drop, 0)
+    u2 = _norm(z1, p['ln2'] if pre else p['ln1'])
+    q = ops.linear(u2, p['q'].w, p['q'].b)
+    kv = ops.linear(mem, p['kv'].w, p['kv'].b)
+    ctx2, lse2 = ops.attention_train(q, kv, kv, B, H, L, T, kv_len=lengths, k_col0=0, v_col0=d)
+    z2 = _resid(ctx2, p['o2'], u2, drop, 1)
+    u3 = _norm(z2, p['ln3'] if pre else p['ln2'])
+    ffn_u, h = _ffn_fwd(p, u3)
+    z3 = _resid(h, p['w2'], u3, drop, 2)
+    out = z3 if pre else _norm(z3, p['ln3'])
+    return out, _DecTape(a=a, u1=u1, qkv=qkv, ctx=ctx, lse=lse, z1=z1, u2=u2, q=q, kv=kv, ctx2=ctx2, lse2=lse2, z2=z2,
+                         u3=u3, ffn_u=ffn_u, h=h, z3=z3)
+
+
+def _dec_layer_bwd(p, t, dout, dmem, mem, pre, g, B, H, L, T, lengths, drop):
+    """Backward of _dec_layer_fwd: parameter gradients into g; returns the gradient of the layer input and dmem plus
+    this layer's gradient of the memory (added by the K|V dgrad GEMM's residual epilogue)."""
+    d = t.a.shape[1]
+    dz3 = dout if pre else _ln_bwd(dout, t.z3, p['ln3'], g)
+    dh = _linear_bwd(_drop_bwd(dz3, drop, 2), t.h, p['w2'], g)
+    du3 = _linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.u3, p['w1'], g, resid=dz3)
+    dz2 = _ln_bwd(du3, t.z2, p['ln3'] if pre else p['ln2'], g)
+    dctx2 = _linear_bwd(_drop_bwd(dz2, drop, 1), t.ctx2, p['o2'], g)
+    dq = torch.empty_like(t.q)
+    dkv = torch.empty_like(t.kv)
+    ops.attention_bwd(t.q, t.kv, t.kv, t.ctx2, dctx2, t.lse2, B, H, L, T, dq, dkv, dkv, kv_len=lengths, k_col0=0, v_col0=d,
+                      dq_col0=0, dk_col0=0, dv_col0=d)
+    dmem = _linear_bwd(dkv, mem, p['kv'], g, resid=dmem)
+    du2 = _linear_bwd(dq, t.u2, p['q'], g, resid=dz2)
+    dz1 = _ln_bwd(du2, t.z1, p['ln2'] if pre else p['ln1'], g)
+    dctx = _linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
+    dqkv = torch.empty_like(t.qkv)
+    ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B, H, L, L, dqkv, dqkv, dqkv, causal=True, q_col0=0, k_col0=d,
+                      v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
+    du1 = _linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
+    return (_ln_bwd(du1, t.a, p['ln1'], g) if pre else du1), dmem
 
 
 def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True, grad_sink=None, grad_scale=1.0,
@@ -224,31 +318,13 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F)                       # [B*T2, F2*C2]
     scale, table = enc.pos_emb.scale_and_table(T2, dev)
     x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_TABLE, alpha=scale, table=table, period=T2)
+    e_drop = [(r, drop_seed, ENC_SITE + 2 * i) for i, r in enumerate(e_rates)]
     enc_tape = []
-    for i, p in enumerate(pk.enc):
-        if pk.enc_pre:
-            # pre-norm as the reference writes it (encoder/transformer.py:41-63): the residual is taken AFTER the norm,
-            # x = n + sublayer(n) with n = norm(x); the stack ends with one more LayerNorm
-            xn = ops.layernorm(x, *p['ln1'])
-            qkv = ops.linear(xn, p['qkv'][0], p['qkv'][2])
-            ctx, lse = ops.attention_train(qkv, qkv, qkv, B, H, T2, T2, kv_len=lengths, q_col0=0, k_col0=d, v_col0=2 * d)
-            z1 = _resid(ctx, p['o'][0], p['o'][2], xn, e_rates[i], drop_seed, ENC_SITE + 2 * i)
-            x1 = ops.layernorm(z1, *p['ln2'])
-            u, h = _ffn_fwd(p, x1)
-            z2 = _resid(h, p['w2'][0], p['w2'][2], x1, e_rates[i], drop_seed, ENC_SITE + 2 * i + 1)
-            enc_tape.append((x, qkv, ctx, lse, z1, x1, u, h, xn))
-            x = z2
-            continue
-        qkv = ops.linear(x, p['qkv'][0], p['qkv'][2])
-        ctx, lse = ops.attention_train(qkv, qkv, qkv, B, H, T2, T2, kv_len=lengths, q_col0=0, k_col0=d, v_col0=2 * d)
-        z1 = _resid(ctx, p['o'][0], p['o'][2], x, e_rates[i], drop_seed, ENC_SITE + 2 * i)
-        x1 = ops.layernorm(z1, *p['ln1'])
-        u, h = _ffn_fwd(p, x1)
-        z2 = _resid(h, p['w2'][0], p['w2'][2], x1, e_rates[i], drop_seed, ENC_SITE + 2 * i + 1)
-        enc_tape.append((x, qkv, ctx, lse, z1, x1, u, h, z2))
-        x = ops.layernorm(z2, *p['ln2'])
+    for p, drop in zip(pk.enc, e_drop):
+        x, t = _enc_layer_fwd(p, x, pk.enc_pre, B, H, T2, lengths, drop)
+        enc_tape.append(t)
     enc_last = x
-    mem = ops.layernorm(x, *pk.enc_norm) if pk.enc_pre else x
+    mem = _norm(x, pk.enc_norm) if pk.enc_pre else x
 
     tgt_in = truth[:, :-1].contiguous()
     tgt_out = truth[:, 1:].contiguous()
@@ -256,41 +332,15 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     Hd = dec.n_heads
     _, dtable = dec.pos_emb.scale_and_table(L, dev)
     y = ops.embed_posenc(tgt_in, pk.out['emb'], dtable, B * L, d, period=L)
+    d_drop = [(r, drop_seed, DEC_SITE + 3 * i) for i, r in enumerate(d_rates)]
     dec_tape = []
-    for i, p in enumerate(pk.dec):
-        if pk.dec_pre:      # decoder/transformer.py:54-90 with normalize_before: y = n + sublayer(n), n = norm(y), three times
-            yn = ops.layernorm(y, *p['ln1'])
-            qkv = ops.linear(yn, p['qkv'][0], p['qkv'][2])
-            ctx, lse = ops.attention_train(qkv, qkv, qkv, B, Hd, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d)
-            z1 = _resid(ctx, p['o'][0], p['o'][2], yn, d_rates[i], drop_seed, DEC_SITE + 3 * i)
-            y1 = ops.layernorm(z1, *p['ln2'])
-            q = ops.linear(y1, p['q'][0], p['q'][2])
-            kv = ops.linear(mem, p['kv'][0], p['kv'][2])
-            ctx2, lse2 = ops.attention_train(q, kv, kv, B, Hd, L, T2, kv_len=lengths, k_col0=0, v_col0=d)
-            z2 = _resid(ctx2, p['o2'][0], p['o2'][2], y1, d_rates[i], drop_seed, DEC_SITE + 3 * i + 1)
-            y2 = ops.layernorm(z2, *p['ln3'])
-            u, h = _ffn_fwd(p, y2)
-            z3 = _resid(h, p['w2'][0], p['w2'][2], y2, d_rates[i], drop_seed, DEC_SITE + 3 * i + 2)
-            dec_tape.append((y, qkv, ctx, lse, z1, y1, q, kv, ctx2, lse2, z2, y2, u, h, yn))
-            y = z3
-            continue
-        qkv = ops.linear(y, p['qkv'][0], p['qkv'][2])
-        ctx, lse = ops.attention_train(qkv, qkv, qkv, B, Hd, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d)
-        z1 = _resid(ctx, p['o'][0], p['o'][2], y, d_rates[i], drop_seed, DEC_SITE + 3 * i)
-        y1 = ops.layernorm(z1, *p['ln1'])
-        q = ops.linear(y1, p['q'][0], p['q'][2])
-        kv = ops.linear(mem, p['kv'][0], p['kv'][2])
-        ctx2, lse2 = ops.attention_train(q, kv, kv, B, Hd, L, T2, kv_len=lengths, k_col0=0, v_col0=d)
-        z2 = _resid(ctx2, p['o2'][0], p['o2'][2], y1, d_rates[i], drop_seed, DEC_SITE + 3 * i + 1)
-        y2 = ops.layernorm(z2, *p['ln2'])
-        u, h = _ffn_fwd(p, y2)
-        z3 = _resid(h, p['w2'][0], p['w2'][2], y2, d_rates[i], drop_seed, DEC_SITE + 3 * i + 2)
-        dec_tape.append((y, qkv, ctx, lse, z1, y1, q, kv, ctx2, lse2, z2, y2, u, h, z3))
-        y = ops.layernorm(z3, *p['ln3'])
+    for p, drop in zip(pk.dec, d_drop):
+        y, t = _dec_layer_fwd(p, y, mem, pk.dec_pre, B, Hd, L, T2, lengths, drop)
+        dec_tape.append(t)
     V = dec.vocab_size
     dec_last = y
     if pk.dec_pre:
-        y = ops.layernorm(y, *pk.dec_norm)
+        y = _norm(y, pk.dec_norm)
     logits = ops.linear(y, pk.out['wout'], pk.out['bout'], EPI_BIAS, out_f32=True, n_out=pk.ld_logits)
     sm = model.smoothing if smoothing is None else smoothing
     loss_ctc, dctc = None, None
@@ -321,52 +371,9 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     dy = ops.linear(dlogits, pk.out['wout_t'])                                   # [B*L, d]
     dmem = None
     if pk.dec_pre:
-        dy = _ln_bwd(dy, dec_last, pk.dec_norm[0], g, 'decoder.after_norm.weight', 'decoder.after_norm.bias')
+        dy = _ln_bwd(dy, dec_last, pk.dec_norm, g)
     for i in reversed(range(len(pk.dec))):
-        p, pre = pk.dec[i], f'decoder.blocks.{i}.'
-        rt, st0 = d_rates[i], DEC_SITE + 3 * i
-        if pk.dec_pre:
-            (y0, qkv, ctx, lse, z1, y1, q, kv, ctx2, lse2, z2, y2, u, h, yn) = dec_tape[i]
-            # z3 = y2 + drop(ffn(y2)), y2 = norm3(z2): dy is the gradient of z3
-            dh = _linear_bwd(_drop_bwd(dy, rt, drop_seed, st0 + 2), h, p['w2'][1], g, pre + 'feed_forward.w_2.weight', pre + 'feed_forward.w_2.bias')
-            du = _ffn_act_bwd(p, dh, u, h)
-            dy2 = _linear_bwd(du, y2, p['w1'][1], g, pre + 'feed_forward.w_1.weight', pre + 'feed_forward.w_1.bias', resid=dy)
-            dz2 = _ln_bwd(dy2, z2, p['ln3'][0], g, pre + 'norm3.weight', pre + 'norm3.bias')
-            dctx2 = _linear_bwd(_drop_bwd(dz2, rt, drop_seed, st0 + 1), ctx2, p['o2'][1], g, pre + 'src_attn.output_proj.weight', pre + 'src_attn.output_proj.bias')
-            dq = torch.empty_like(q)
-            dkv = torch.empty_like(kv)
-            ops.attention_bwd(q, kv, kv, ctx2, dctx2, lse2, B, Hd, L, T2, dq, dkv, dkv, kv_len=lengths, k_col0=0, v_col0=d,
-                              dq_col0=0, dk_col0=0, dv_col0=d)
-            dmem = _linear_bwd(dkv, mem, p['kv'][1], g, pre + 'src_attn.vk_proj.weight', pre + 'src_attn.vk_proj.bias', resid=dmem)
-            dy1 = _linear_bwd(dq, y1, p['q'][1], g, pre + 'src_attn.q_proj.weight', pre + 'src_attn.q_proj.bias', resid=dz2)
-            dz1 = _ln_bwd(dy1, z1, p['ln2'][0], g, pre + 'norm2.weight', pre + 'norm2.bias')
-            dctx = _linear_bwd(_drop_bwd(dz1, rt, drop_seed, st0), ctx, p['o'][1], g, pre + 'slf_attn.output_proj.weight', pre + 'slf_attn.output_proj.bias')
-            dqkv = torch.empty_like(qkv)
-            ops.attention_bwd(qkv, qkv, qkv, ctx, dctx, lse, B, Hd, L, L, dqkv, dqkv, dqkv, causal=True, q_col0=0, k_col0=d,
-                              v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
-            dyn = _linear_bwd(dqkv, yn, p['qkv'][1], g, pre + 'slf_attn.qvk_proj.weight', pre + 'slf_attn.qvk_proj.bias', resid=dz1)
-            dy = _ln_bwd(dyn, y0, p['ln1'][0], g, pre + 'norm1.weight', pre + 'norm1.bias')
-            continue
-        (y0, qkv, ctx, lse, z1, y1, q, kv, ctx2, lse2, z2, y2, u, h, z3) = dec_tape[i]
-        dz3 = _ln_bwd(dy, z3, p['ln3'][0], g, pre + 'norm3.weight', pre + 'norm3.bias')
-        # the sub-layer branch sees the replayed dropout mask, the residual branch (resid= below) the plain gradient
-        dh = _linear_bwd(_drop_bwd(dz3, rt, drop_seed, st0 + 2), h, p['w2'][1], g, pre + 'feed_forward.w_2.weight', pre + 'feed_forward.w_2.bias')
-        du = _ffn_act_bwd(p, dh, u, h)
-        dy2 = _linear_bwd(du, y2, p['w1'][1], g, pre + 'feed_forward.w_1.weight', pre + 'feed_forward.w_1.bias', resid=dz3)
-        dz2 = _ln_bwd(dy2, z2, p['ln2'][0], g, pre + 'norm2.weight', pre + 'norm2.bias')
-        dctx2 = _linear_bwd(_drop_bwd(dz2, rt, drop_seed, st0 + 1), ctx2, p['o2'][1], g, pre + 'src_attn.output_proj.weight', pre + 'src_attn.output_proj.bias')
-        dq = torch.empty_like(q)
-        dkv = torch.empty_like(kv)
-        ops.attention_bwd(q, kv, kv, ctx2, dctx2, lse2, B, Hd, L, T2, dq, dkv, dkv, kv_len=lengths, k_col0=0, v_col0=d,
-                          dq_col0=0, dk_col0=0, dv_col0=d)
-        dmem = _linear_bwd(dkv, mem, p['kv'][1], g, pre + 'src_attn.vk_proj.weight', pre + 'src_attn.vk_proj.bias', resid=dmem)
-        dy1 = _linear_bwd(dq, y1, p['q'][1], g, pre + 'src_attn.q_proj.weight', pre + 'src_attn.q_proj.bias', resid=dz2)
-        dz1 = _ln_bwd(dy1, z1, p['ln1'][0], g, pre + 'norm1.weight', pre + 'norm1.bias')
-        dctx = _linear_bwd(_drop_bwd(dz1, rt, drop_seed, st0), ctx, p['o'][1], g, pre + 'slf_attn.output_proj.weight', pre + 'slf_attn.output_proj.bias')
-        dqkv = torch.empty_like(qkv)
-        ops.attention_bwd(qkv, qkv, qkv, ctx, dctx, lse, B, Hd, L, L, dqkv, dqkv, dqkv, causal=True, q_col0=0, k_col0=d,
-                          v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
-        dy = _linear_bwd(dqkv, y0, p['qkv'][1], g, pre + 'slf_attn.qvk_proj.weight', pre + 'slf_attn.qvk_proj.bias', resid=dz1)
+        dy, dmem = _dec_layer_bwd(pk.dec[i], dec_tape[i], dy, dmem, mem, pk.dec_pre, g, B, Hd, L, T2, lengths, d_drop[i])
     # embedding (decoder/transformer.py:163,169); with tied weights the output-layer gradient lands in the same tensor
     if pk.tied:
         ops.embed_bwd(tgt_in, dy, dwout, math.sqrt(d))          # atomics on top of the output-layer gradient
@@ -388,34 +395,9 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
         wc_t[:, :V] = wc.t()
         dx = ops.linear(dctc, wc_t, None, EPI_RESID, resid=dmem)
     if pk.enc_pre:
-        dx = _ln_bwd(dx, enc_last, pk.enc_norm[0], g, 'encoder.norm.weight', 'encoder.norm.bias')
+        dx = _ln_bwd(dx, enc_last, pk.enc_norm, g)
     for i in reversed(range(len(pk.enc))):
-        p, pre = pk.enc[i], f'encoder.blocks.{i}.'
-        rt, st0 = e_rates[i], ENC_SITE + 2 * i
-        if pk.enc_pre:
-            (x0, qkv, ctx, lse, z1, x1, u, h, xn) = enc_tape[i]
-            dh = _linear_bwd(_drop_bwd(dx, rt, drop_seed, st0 + 1), h, p['w2'][1], g, pre + 'feed_forward.w_2.weight', pre + 'feed_forward.w_2.bias')
-            du = _ffn_act_bwd(p, dh, u, h)
-            dx1 = _linear_bwd(du, x1, p['w1'][1], g, pre + 'feed_forward.w_1.weight', pre + 'feed_forward.w_1.bias', resid=dx)
-            dz1 = _ln_bwd(dx1, z1, p['ln2'][0], g, pre + 'norm2.weight', pre + 'norm2.bias')
-            dctx = _linear_bwd(_drop_bwd(dz1, rt, drop_seed, st0), ctx, p['o'][1], g, pre + 'slf_attn.output_proj.weight', pre + 'slf_attn.output_proj.bias')
-            dqkv = torch.empty_like(qkv)
-            ops.attention_bwd(qkv, qkv, qkv, ctx, dctx, lse, B, H, T2, T2, dqkv, dqkv, dqkv, kv_len=lengths, q_col0=0, k_col0=d,
-                              v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
-            dxn = _linear_bwd(dqkv, xn, p['qkv'][1], g, pre + 'slf_attn.qvk_proj.weight', pre + 'slf_attn.qvk_proj.bias', resid=dz1)
-            dx = _ln_bwd(dxn, x0, p['ln1'][0], g, pre + 'norm1.weight', pre + 'norm1.bias')
-            continue
-        (x0, qkv, ctx, lse, z1, x1, u, h, z2) = enc_tape[i]
-        dz2 = _ln_bwd(dx, z2, p['ln2'][0], g, pre + 'norm2.weight', pre + 'norm2.bias')
-        dh = _linear_bwd(_drop_bwd(dz2, rt, drop_seed, st0 + 1), h, p['w2'][1], g, pre + 'feed_forward.w_2.weight', pre + 'feed_forward.w_2.bias')
-        du = _ffn_act_bwd(p, dh, u, h)
-        dx1 = _linear_bwd(du, x1, p['w1'][1], g, pre + 'feed_forward.w_1.weight', pre + 'feed_forward.w_1.bias', resid=dz2)
-        dz1 = _ln_bwd(dx1, z1, p['ln1'][0], g, pre + 'norm1.weight', pre + 'norm1.bias')
-        dctx = _linear_bwd(_drop_bwd(dz1, rt, drop_seed, st0), ctx, p['o'][1], g, pre + 'slf_attn.output_proj.weight', pre + 'slf_attn.output_proj.bias')
-        dqkv = torch.empty_like(qkv)
-        ops.attention_bwd(qkv, qkv, qkv, ctx, dctx, lse, B, H, T2, T2, dqkv, dqkv, dqkv, kv_len=lengths, q_col0=0, k_col0=d,
-                          v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
-        dx = _linear_bwd(dqkv, x0, p['qkv'][1], g, pre + 'slf_attn.qvk_proj.weight', pre + 'slf_attn.qvk_proj.bias', resid=dz1)
+        dx = _enc_layer_bwd(pk.enc[i], enc_tape[i], dx, pk.enc_pre, g, B, H, T2, lengths, e_drop[i])
 
     # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE  ->  conv2 (implicit-GEMM forward, im2col GEMMs backward) -> conv1
     dyl = ops.scale_add_table(dx, scale)                                          # d(h2 Wo^T + bo) = sqrt(d) * dx

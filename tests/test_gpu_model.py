@@ -162,7 +162,16 @@ def test_conformer_encoder_states_match_oracle(relpos):
 
 
 def test_decoder_logits_match_oracle_teacher_forced():
+    _decoder_logits_vs_oracle(False, 'glu')
+
+
+def test_decoder_logits_match_oracle_teacher_forced_prenorm_relu():
+    _decoder_logits_vs_oracle(True, 'relu')
+
+
+def _decoder_logits_vs_oracle(normalize_before, activation):
     params = _params(n_enc=1, n_dec=3)
+    params['decoder'].update(normalize_before=normalize_before, activation=activation)
     model, sd = _build(params)
     x, mask = _batch(3, 300, 80, [300, 211, 250])
     mem_ref, mmask = om.encode(x, mask, sd, params)
@@ -205,9 +214,18 @@ def test_model_forward_loss_matches_oracle():
 
 
 def test_beam_search_lockstep_with_oracle():
+    _beam_search_lockstep(False, 'glu')
+
+
+def test_beam_search_lockstep_with_oracle_prenorm_relu():
+    _beam_search_lockstep(True, 'relu')
+
+
+def _beam_search_lockstep(normalize_before, activation):
     """Drive the oracle's beam_step with the CUDA decoder's log-probs: every integer decision of every
     step must be bit-exact, and the KV-cached log-probs must equal the oracle's full-prefix recompute."""
     params = _params(n_enc=1, n_dec=2)
+    params['decoder'].update(normalize_before=normalize_before, activation=activation)
     model, sd = _build(params)
     B, beam, max_len = 3, 4, 9
     x, mask = _batch(B, 200, 80, [200, 150, 173])
@@ -483,11 +501,20 @@ def test_end_to_end_best_hypothesis_vs_fp32_oracle():
 
 
 def test_decoder_kv_cache_through_the_reference_seam():
+    _kv_cache_through_the_seam(False, 'glu')
+
+
+def test_decoder_kv_cache_through_the_reference_seam_prenorm_relu():
+    _kv_cache_through_the_seam(True, 'relu')
+
+
+def _kv_cache_through_the_seam(normalize_before, activation):
     """The cache the reference stubbed out (decoder/transformer.py:92-126,188-203), through its own seam:
     decoder.inference(preds, memory, mask, cache) with cache = decoder.init_cache(...) runs one token per call, and
     SpeechToTextRecognizer.decode_step reorders it by the surviving parents.  Must agree with the full-prefix recompute
     (cache None, the reference's behaviour) and with the oracle in lock-step."""
     params = _params(n_enc=1, n_dec=3)
+    params['decoder'].update(normalize_before=normalize_before, activation=activation)
     model, sd = _build(params)
     B, beam, max_len = 3, 4, 8
     x, mask = _batch(B, 200, 80, [200, 150, 173])
