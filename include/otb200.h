@@ -56,8 +56,8 @@ int otb_debug_decode_timing(unsigned long long* buf, int step);
 /* Serving knob of otb_decode_persistent (no counterpart in the reference): how the 16 CTAs of a row group synchronise.
  * 1 = thread-block cluster of 16 + barrier.cluster (lowest latency; one cluster per GPC, i.e. at most 8 groups in flight),
  * 0 = plain CTAs + a release/acquire counter in L2 (every SM usable; every CTA of every batch in flight must be resident),
- * -1 = default (clusters when the device grants them, unless OTB_DG_CLUSTER=0).  With 1, a launch on a device that refuses
- * clusters of 16 fails instead of falling back to the software barrier.  Process-wide. */
+ * -1 = default: clusters when the device grants clusters of 16 (probed once), else the software barrier.  With 1, a launch
+ * on a device that refuses clusters of 16 fails instead of falling back to the software barrier.  Process-wide. */
 int otb_set_decode_barrier(int kind);
 
 /* Conv2dLayer output geometry, kernel 3, stride 2, padding (0,1)  (frontend/conv.py:10-11,27):

@@ -22,12 +22,6 @@ namespace otb {
 static constexpr int ABW_SMEM_DQ = 16384 * 4 + 32768 + 256 + 1024 + 1024;           // Q, dO, K, V, dS, barriers, L/D
 static constexpr int ABW_SMEM_DKV = 16384 * 4 + 32768 * 2 + 1024 + 256 + 1024;      // K, V, Q, dO, P^T, dS^T, L/D
 
-__device__ __forceinline__ float ex2a(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
 // bf16 pair (row, col), (row, col + 1) of a [128 rows x 128] tile in the K-major SW128 layout (two 64-column k-blocks)
 __device__ __forceinline__ void put_pair(uint8_t* tile, int row, int col, float a, float b) {
     *reinterpret_cast<uint32_t*>(tile + (col >> 6) * 16384 + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) =
@@ -150,7 +144,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                     for (int e = 0; e < 2; ++e) {
                         const int i = 4 * jj + 2 * hh + e;
                         const int key = key0 + kh * 64 + jj * 8 + cq + e;
-                        const float pv = ex2a(fmaf(sc[i], p.scale_log2, -Lr[hh]));
+                        const float pv = ex2_approx(fmaf(sc[i], p.scale_log2, -Lr[hh]));
                         const float v = pv * (dp[i] - Dr[hh]) * scale;
                         ds[e] = (q_ok[hh] && key < lim[hh]) ? v : 0.f;
                     }
@@ -271,7 +265,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
                             const int c = qh * 64 + jj * 8 + cq + e;
                             const int qi = i0 + c;
                             const bool vis = k_ok[hh] && qi < p.Tq && (!p.causal || kj[hh] <= qi);
-                            const float pv = ex2a(fmaf(st[i], p.scale_log2, -sL[c]));
+                            const float pv = ex2_approx(fmaf(st[i], p.scale_log2, -sL[c]));
                             const float dvv = pv * (dpt[i] - sD[c]) * scale;
                             pt[e] = vis ? pv : 0.f;
                             ds[e] = vis ? dvv : 0.f;

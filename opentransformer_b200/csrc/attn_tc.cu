@@ -36,12 +36,6 @@ struct AttnCfg {
     static constexpr int SMEM = TILE * 3 + 32768 + 128 + 1024;
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
 template <int DK, bool HAS_BD>
 __global__ void __launch_bounds__(256, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,

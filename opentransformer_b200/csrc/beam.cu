@@ -124,15 +124,6 @@ __global__ void __launch_bounds__(KMAX * 32) beam_step_kernel(const float* __res
     }
 }
 
-// single thread: step += 1; done when every hypothesis ended at this step (speech2text.py:66-67)
-__global__ void beam_advance_kernel(int* ctrl, int N, int Lmax) {
-    if (ctrl[1] || ctrl[0] >= Lmax) return;
-    const int ended = ctrl[2];
-    ctrl[2] = 0;
-    ctrl[0] += 1;
-    if (ended == N) ctrl[1] = 1;
-}
-
 const char* beam_step_launch(cudaStream_t stream, const float* logp, int ldl, int V, const float* lm_logp, int ld_lm,
                              float lm_weight, BeamState st, long long* dbg_ktok, int* dbg_offs, const float* pre_val,
                              const int* pre_idx) {
@@ -308,12 +299,7 @@ __global__ void __launch_bounds__(TOPK_THREADS) logsoftmax_topk_kernel(const flo
             const float v = srow[idx];
             if (v > bv) { bv = v; bi = idx; }      // ascending scan + strict '>' keeps the lower index on ties
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
-        }
+        warp_best(bv, bi);
         if (bi != 0x7fffffff && ((bi - lo) & 31) == lane) srow[bi] = -INFINITY;
         if (lane == 0) { cand_v[warp * KMAX + r] = bv; cand_i[warp * KMAX + r] = bi; }
         __syncwarp();
@@ -327,12 +313,7 @@ __global__ void __launch_bounds__(TOPK_THREADS) logsoftmax_topk_kernel(const flo
             int bi = (lane < 8 && pos < k) ? cand_i[lane * KMAX + pos] : 0x7fffffff;
             const float mv = bv;
             const int mi = bi;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                if (better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
-            }
+            warp_best(bv, bi);
             if (mi == bi && mv == bv && lane < 8) ++pos;
             if (lane == 0) { out_val[(size_t)row * k + r] = bv; out_idx[(size_t)row * k + r] = bi; }
         }

@@ -1,6 +1,7 @@
 // Device helpers shared by the beam-search kernels (beam.cu) and the persistent decode kernel
-// (decode_mega.cu): comparison rule (ties -> LOWER index, torch.topk's tie order is implementation-defined),
-// per-lane sorted candidate lists and a warp-wide top-k.
+// (decode_group.cu): comparison rule (ties -> LOWER index, torch.topk's tie order is implementation-defined),
+// the warp arg-max step built on it, per-lane sorted candidate lists and a warp-wide top-k.  Both decode paths
+// select through `better` / `warp_best`, which is what keeps their ids bit-exact with each other.
 #pragma once
 #include <math.h>
 
@@ -13,6 +14,16 @@ static constexpr long long EOS_ID = 1;  // otrans/data/__init__.py:9-10 (BOS == 
 
 __device__ __forceinline__ bool better(float va, int ia, float vb, int ib) {
     return (va > vb) || (va == vb && ia < ib);
+}
+
+// Warp-wide arg-max of (bv, bi) under `better`: every lane ends with the winner.
+__device__ __forceinline__ void warp_best(float& bv, int& bi) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
 }
 
 // Per-lane sorted (descending) list of the K best (value, index) pairs, statically indexed.
@@ -61,12 +72,7 @@ __device__ __forceinline__ void warp_topk(F get, int n, int k, float* out_v, int
     for (int r = 0; r < k; ++r) {
         float bv = tl.v[0];
         int bi = tl.i[0];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
-        }
+        warp_best(bv, bi);
         if (tl.i[0] == bi && tl.v[0] == bv) tl.pop();  // indices are unique -> exactly one lane pops
         if (lane == 0) { out_v[r] = bv; out_i[r] = bi; }
     }

@@ -345,35 +345,17 @@ int otb_decode_persistent(const otb_mega_model* model, const void* kvx, const in
                           float* dbg_logp, float* dbg_scores, void* stream) {
     if (!model || !kvx || !mem_len || !kc || !vc || !st || !workspace) return fail("otb_decode_persistent", "null operand");
     if (model->n_layers < 1 || model->n_layers > OTB_MEGA_MAX_LAYERS) return fail("otb_decode_persistent", "1..8 decoder layers");
-    MegaParams p;
-    memset(&p, 0, sizeof(p));
-    p.n_layers = model->n_layers; p.d = model->d_model; p.H = model->n_heads; p.dff = model->d_ff; p.V = model->vocab;
-    p.emb = reinterpret_cast<const bf16*>(model->emb);
-    p.wout = reinterpret_cast<const bf16*>(model->wout);
-    p.bout = model->bout;
-    p.pe = model->pe;
-    if (!p.emb || !p.wout || !p.pe) return fail("otb_decode_persistent", "null model tensor");
+    if (!model->emb || !model->wout || !model->pe) return fail("otb_decode_persistent", "null model tensor");
     for (int l = 0; l < model->n_layers; ++l) {
         const otb_mega_layer& s = model->layers[l];
-        MegaLayer& d = p.layers[l];
-        d.wqkv = (const bf16*)s.wqkv; d.wo = (const bf16*)s.wo; d.wq = (const bf16*)s.wq; d.wo2 = (const bf16*)s.wo2;
-        d.w1 = (const bf16*)s.w1; d.w2 = (const bf16*)s.w2;
-        d.bqkv = s.bqkv; d.bo = s.bo; d.bq = s.bq; d.bo2 = s.bo2; d.b1 = s.b1; d.b2 = s.b2;
-        d.g1 = s.g1; d.be1 = s.be1; d.g2 = s.g2; d.be2 = s.be2; d.g3 = s.g3; d.be3 = s.be3;
         const void* need[18] = {s.wqkv, s.wo, s.wq, s.wo2, s.w1, s.w2, s.bqkv, s.bo, s.bq, s.bo2, s.b1, s.b2,
                                 s.g1, s.be1, s.g2, s.be2, s.g3, s.be3};
         for (int i = 0; i < 18; ++i)
             if (!need[i]) return fail("otb_decode_persistent", "null layer tensor (biases are required)");
     }
-    p.kvx = reinterpret_cast<const bf16*>(kvx);
-    p.mem_len = mem_len;
-    p.kc = reinterpret_cast<bf16*>(kc);
-    p.vc = reinterpret_cast<bf16*>(vc);
-    p.st = to_state(st);
-    p.B = B; p.T = T; p.max_steps = max_steps;
-    p.eps = model->ln_eps;
-    p.dbg_logp = dbg_logp; p.dbg_scores = dbg_scores;
-    RET("otb_decode_persistent", decode_group_launch(ST(stream), p, workspace, (size_t)workspace_bytes));
+    RET("otb_decode_persistent", decode_group_launch(ST(stream), *model, reinterpret_cast<const bf16*>(kvx), mem_len,
+                                                     reinterpret_cast<bf16*>(kc), reinterpret_cast<bf16*>(vc), to_state(st), B, T,
+                                                     max_steps, dbg_logp, dbg_scores, workspace, (size_t)workspace_bytes));
 }
 
 int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,

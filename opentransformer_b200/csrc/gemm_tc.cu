@@ -58,14 +58,6 @@ struct GemmCfg {
 };
 static_assert(GemmCfg<256>::SMEM_BYTES <= 227 * 1024, "gemm_tc_kernel: shared-memory budget (227 KB per CTA)");
 
-// sigmoid(x) = 0.5 * tanh(x / 2) + 0.5 with ONE MUFU op (tanh.approx, |rel err| ~ 2^-11, far below the bf16 output
-// rounding) instead of ex2 + rcp: the GLU epilogue of the K = 256 GEMMs is MUFU-bound.
-__device__ __forceinline__ float fast_sigmoid(float x) {
-    float t;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
-    return fmaf(0.5f, t, 0.5f);
-}
-
 template <int NT>
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
 

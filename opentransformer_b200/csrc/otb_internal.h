@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/otb200.h"
+
 namespace otb {
 
 typedef __nv_bfloat16 bf16;
@@ -138,71 +140,15 @@ struct BeamState {
     int N, beam, Lmax;
 };
 
-// ---- persistent decode kernel (decode_mega.cu)
-static constexpr int OTB_MEGA_MAX_LAYERS_INT = 8;
-struct MegaLayer {   // one TransformerDecoderLayer: bf16 weights [N,K] row-major, fp32 biases / LayerNorm affine
-    const bf16 *wqkv, *wo, *wq, *wo2, *w1, *w2;
-    const float *bqkv, *bo, *bq, *bo2, *b1, *b2;
-    const float *g1, *be1, *g2, *be2, *g3, *be3;
-};
-struct MegaParams {
-    int n_layers, d, H, dff, V;
-    const bf16* emb;      // [V, d] embedding
-    const bf16* wout;     // [V, d] output layer (== emb when tied)
-    const float* bout;    // [V] or null
-    const float* pe;      // [>= max_steps, d] sinusoid table
-    MegaLayer layers[OTB_MEGA_MAX_LAYERS_INT];
-    const bf16* kvx;      // [n_layers, B*T, 2d] cross-attention K | V
-    const int* mem_len;   // [B]
-    bf16* kc;             // [n_layers, Lmax, N, d]
-    bf16* vc;
-    BeamState st;
-    int B, T, max_steps;
-    float eps;
-    float* dbg_logp;      // optional [max_steps, N, V]
-    float* dbg_scores;    // optional [max_steps, N]
-};
-// ---- persistent decode kernel, round 2 (decode_group.cu): row groups of <= 128 hypotheses x 16 CTAs, wgmma GEMMs
-struct DgLayer {
-    const float *bqkv, *bo, *bq, *bo2, *b1, *b2;
-    const float *g1, *be1, *g2, *be2, *g3, *be3;
-};
-struct DgParams {
-    int n_layers, V, G, utts_per_group;
-    int cluster;               // 1: launched as thread-block clusters of 16 (group == cluster, hardware barrier)
-    const bf16* emb;
-    const float* bout;
-    const float* pe;
-    DgLayer layers[OTB_MEGA_MAX_LAYERS_INT];
-    const CUtensorMap* maps;   // device array: per layer {wqkv, wo, wq, wo2, w1, w2}, then wout, ctx, kvx
-    const int* mem_len;
-    bf16* kc;
-    bf16* vc;
-    BeamState st;
-    int B, T, max_steps;
-    float eps;
-    bf16* qbuf;                // [N, d]   self-attention queries of the newest token
-    bf16* ctx;                 // [N + 128, d] attention context (self, then cross)
-    bf16* xbuf;                // [N + 128, d] layer input x (embedding / LayerNorm 3 of the previous layer)
-    bf16* x2buf;               // [N, d]   LayerNorm 2 output (residual of the feed-forward)
-    float* pre;                // [N, d]   pre-LayerNorm rows (residual + projection + bias), fp32
-    bf16* q2;                  // [N, d]   cross-attention queries
-    int flags;                 // experiment switches (OTB_DG_FLAGS)
-    float* part;               // [16 slices][groups][64 column groups][128 rows][4] w_2 partial products (fp32)
-    float* logits;             // [N, ldv] output-layer logits of the step
-    int ldv;
-    int* bar;                  // [G, 32]  group barrier counters
-    int* gstate;               // [G, Lmax] ended-hypothesis count per step
-    float* dbg_logp;
-    float* dbg_scores;
-    unsigned long long* dbg_clk;
-    int dbg_step;
-};
+// ---- persistent decode kernel (decode_group.cu): row groups of <= 128 hypotheses x 16 CTAs, wgmma GEMMs.  The model is
+// the public otb_mega_model; the launch checks that the kernel supports it.
 extern unsigned long long* g_dg_dbg;
 extern int g_dg_dbg_step;
 extern int g_dg_barrier;
 size_t decode_group_workspace_bytes(int N, int n_layers, int Lmax, int B, int beam, int V);
-const char* decode_group_launch(cudaStream_t st, const MegaParams& p, void* workspace, size_t workspace_bytes);
+const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const bf16* kvx, const int* mem_len, bf16* kc,
+                                bf16* vc, const BeamState& bs, int B, int T, int max_steps, float* dbg_logp,
+                                float* dbg_scores, void* workspace, size_t workspace_bytes);
 
 // d_k: head width, 64 or 96 (head h starts at column col0 + d_k * h)
 const char* attn_launch(cudaStream_t st, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows,

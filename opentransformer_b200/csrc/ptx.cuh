@@ -1,6 +1,6 @@
 // Thin inline-PTX wrappers for the sm_90a features the hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), thread-block clusters, wgmma and its shared-memory
-// descriptors.  No CUTLASS/CuTe dependency.
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma and its shared-memory descriptors, and the MUFU
+// approximations the softmax and gate epilogues share.  No CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -50,59 +50,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {
         if (((++spins) & 0xFFF) == 0 && (clock64() - t0) > 4000000000LL) __trap();
     }
-}
-
-// ---------------------------------------------------------------- thread-block clusters / DSMEM
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-    return r;
-}
-// shared::cta address in THIS CTA -> shared::cluster address of the same variable in CTA `rank`
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void st_cluster_f32x2(uint32_t cluster_addr, float a, float b) {
-    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");
-}
-// remote 8-byte store that also signals `bytes` on an mbarrier living in the SAME (remote) CTA as the data
-__device__ __forceinline__ void st_async_f32x2(uint32_t cluster_addr, float a, float b, uint32_t cluster_mbar) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(cluster_addr),
-                 "f"(a), "f"(b), "r"(cluster_mbar)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-    if (mbar_try_wait_cluster(bar, parity)) return;
-    long long t0 = clock64();
-    uint32_t spins = 0;
-    while (!mbar_try_wait_cluster(bar, parity)) {
-        if (((++spins) & 0xFFF) == 0 && (clock64() - t0) > 4000000000LL) __trap();
-    }
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -223,6 +170,19 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
+}
+// 2^x with one MUFU op (flushes denormals; ex2(-inf) = 0)
+__device__ __forceinline__ float ex2_approx(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+// sigmoid(x) = 0.5 * tanh(x / 2) + 0.5 with ONE MUFU op (tanh.approx, |rel err| ~ 2^-11, far below the bf16 output
+// rounding) instead of ex2 + rcp: the GLU epilogues are MUFU-bound.
+__device__ __forceinline__ float fast_sigmoid(float x) {
+    float t;
+    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
+    return fmaf(0.5f, t, 0.5f);
 }
 
 }  // namespace otb

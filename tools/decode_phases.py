@@ -17,7 +17,7 @@ with torch.no_grad():
 x, mask = bench.synthetic_batch(32, 0)
 x, mask = x.to(dev), mask.to(dev)
 L = _lib.lib()
-PH = ('qkv gemm', 'barrier', 'self-attn', 'barrier', 'W_o+LN1', 'q-proj', 'barrier', 'cross-attn', 'barrier', 'W_o2+LN2', 'barrier',
+PH = ('qkv gemm', 'barrier', 'self-attn', 'W_o+LN1', 'q-proj', 'barrier', 'cross-attn', 'barrier', 'W_o2+LN2', 'barrier',
       'w1+glu', 'w2 partial', 'barrier', 'reduce+LN3', 'barrier')
 NP = len(PH)
 names = ['start', 'embed']
@@ -62,7 +62,6 @@ with torch.no_grad():
               'wait half 3', dd(47, 48)[:6], 'compute', dd(48, 49)[:6], 'merge+store', dd(50, 51)[:6])
         # inner stamps of the six group barriers of layer 2: stamp index of the barrier's entry = 2 + 2*NP + position of 'barrier' - 1
         bpos = [i for i, nme in enumerate(PH) if nme == 'barrier']
-        del bpos[1]      # the entry behind the self-attention is a plain CTA barrier since v9, not a group barrier
         rows = []
         for k, bp in enumerate(bpos):
             entry = allt[:, 2 + 2 * NP + bp - 1]      # stamp taken after the leading __syncthreads of gsync
