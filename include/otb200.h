@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define OTB_VERSION 1
+#define OTB_VERSION 2
 
 /* GEMM epilogues (otb_linear) */
 enum {
@@ -107,24 +107,20 @@ int otb_linear_dropout_resid(const void* a, int lda, const void* w, int ldw, con
 int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask, int M, int N, float p, const uint32_t* seed,
                     uint32_t site, void* stream);
 
-/* Fused masked multi-head attention, d_k = 64 (attention.py:80,34-41; otb_attention_dk below also takes 96): for batch b, head h
- *   out[b*Tq+i, h*64:(h+1)*64] = softmax_j((q_i . k_j + bd) / 8, j < kv_len[b], causal: j <= i) V
+/* Fused masked multi-head attention (attention.py:80,34-41): for batch b, head h
+ *   out[b*Tq+i, h*d_k:(h+1)*d_k] = softmax_j((q_i . k_j + bd) / sqrt(d_k), j < kv_len[b], causal: j <= i) V
  * q/k/v are row-major bf16 matrices; batch b owns rows [b*Tq, (b+1)*Tq) of q and [b*Tk, (b+1)*Tk) of k,v;
- * head h starts at column q_col0/k_col0/v_col0 + 64*h.  bd (optional, f32 [H,B,Tq,ldbd]) holds
- * relative-position scores, bias(i,j) = bd[h,b,i, j-i+Tq-1] (the gather of attention.py:196-215 done by
- * indexing).  resid (optional, bf16 [B*Tq, ldr]) is added to the output (the rel-pos attention of the
- * shipped Conformer has no output projection, SURVEY.md 8a quirks). */
+ * head h starts at column q_col0/k_col0/v_col0 + d_k*h.  d_k is 64 or 96 (96 is the width of the shipped Conformer
+ * configuration, d_model 384 / 4 heads); any other value returns non-zero with otb_last_error().
+ * bd (optional, f32 [H,B,Tq,ldbd]) holds relative-position scores, bias(i,j) = bd[h,b,i, j-i+Tq-1] (the gather of
+ * attention.py:196-215 done by indexing).  resid (optional, bf16 [B*Tq, ldr]) is added to the output (the rel-pos
+ * attention of the shipped Conformer has no output projection, SURVEY.md 8a quirks).  lse (optional, f32 [B,H,Tq])
+ * receives the per-row log-sum-exp (log2 units) otb_attention_bwd needs; the backward is 64-wide, so lse requires
+ * d_k = 64. */
 int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
                   void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
-                  int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, void* stream);
-
-/* otb_attention with an explicit head width d_k, 64 or 96 (any other value returns non-zero with otb_last_error()):
- * head h occupies columns col0 + d_k*h .. col0 + d_k*(h+1) of q/k/v and out, the scores are scaled by 1/sqrt(d_k).
- * d_k = 96 is the width of the shipped Conformer configuration (d_model 384, 4 heads).  Inference only: the
- * backward (otb_attention_lse / otb_attention_bwd) is 64-wide. */
-int otb_attention_dk(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                     void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
-                     int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, int d_k, void* stream);
+                  int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse, int d_k,
+                  void* stream);
 
 /* ConformerConvolutionModule middle (module/conformer.py:48-52): depthwise Conv1d(k, pad (k-1)/2) over time +
  * eval-mode BatchNorm1d + swish.  x, out bf16 [B*T, d]; w f32 [k, d] and b f32 [d] carry the BatchNorm affine
@@ -155,18 +151,16 @@ int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int 
 
 /* Decode-step self-attention over a per-hypothesis KV cache (the cache API the reference left as a
  * stub, decoder/transformer.py:92-126,188-203): qkv bf16 [N,3d] of the newest token; kc/vc bf16
- * [Lmax,N,d]; anc i32 [2,N,Lmax]; *step_ptr = 0-based position; out bf16 [N,d]. */
+ * [Lmax,N,d]; anc i32 [2,N,Lmax]; *step_ptr = 0-based position; out bf16 [N,d]; head width d_k 64 or 96 (d = H*d_k). */
 int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
-                         int H, int Lmax, void* stream);
-/* otb_decode_self_attn with an explicit head width d_k, 64 or 96 (d = H*d_k); otb_decode_self_attn is d_k = 64. */
-int otb_decode_self_attn_dk(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
-                            int H, int Lmax, int d_k, void* stream);
+                         int H, int Lmax, int d_k, void* stream);
 
 /* LabelSmoothingLoss.forward (module/loss.py:21-48) fused: per-token KL(smoothed one-hot || softmax), PAD rows 0,
  * mean over non-PAD tokens.  logits f32 [rows, ldl]; targets i64 [rows]; tok_loss f32 [rows]; loss f32 [1];
- * n_valid i32 [1]; dlogits (optional, f32 [rows, ldd]) receives d loss / d logits. */
+ * n_valid i32 [1]; dlogits (optional) receives d(mean loss)/dlogits: f32 [rows, ldd] with dlogits_bf16 = 0, or bf16
+ * [rows, ldd] with dlogits_bf16 != 0 for the backward GEMMs (ldd >= V and a multiple of 8, columns [V, ldd) zeroed). */
 int otb_ls_ce(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,
-              float* tok_loss, float* loss, int32_t* n_valid, float* dlogits, int ldd, void* stream);
+              float* tok_loss, float* loss, int32_t* n_valid, void* dlogits, int ldd, int dlogits_bf16, void* stream);
 
 /* Device-resident beam-search state, N = B*beam hypotheses (all device pointers). */
 typedef struct {
@@ -244,13 +238,9 @@ int otb_decode_persistent(const otb_mega_model* model, const void* kvx, const in
  * train/trainer.py:206-234).  The reference differentiates through torch autograd; the entry points below are the
  * hand-written backward of each forward op above.  bf16 activations / gradients, fp32 parameter gradients. */
 
-/* otb_attention that also stores the per-row log-sum-exp (log2 units) [B,H,Tq] the backward needs. */
-int otb_attention_lse(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                      void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
-                      int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse,
-                      void* stream);
-/* Backward of otb_attention (no bd / resid): dq, dk, dv written at column offsets d*_col0 + 64*h of their matrices
- * (e.g. the three thirds of one [M,3d] dqkv buffer).  dsum f32 [B,H,Tq] is scratch.  wgmma, scores recomputed. */
+/* Backward of otb_attention (d_k = 64, no bd / resid; lse as that forward stored it): dq, dk, dv written at column offsets
+ * d*_col0 + 64*h of their matrices (e.g. the three thirds of one [M,3d] dqkv buffer).  dsum f32 [B,H,Tq] is scratch.
+ * wgmma, scores recomputed. */
 int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
                       const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
                       int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
@@ -272,17 +262,11 @@ int otb_glu_bwd(const void* dh, const void* u, void* du, int M, int F, void* str
 int otb_relu_bwd(const void* dy, const void* y, void* dx, long long n, void* stream);
 /* nn.Embedding backward: dE[tok[n]] += scale * dx[n]  (fp32 atomics). */
 int otb_embed_bwd(const int64_t* tok, const void* dx, float* dE, int N, int d, int vocab, float scale, void* stream);
-/* otb_ls_ce that also writes d(mean loss)/dlogits as bf16 [rows, ldd] (zero-padded columns) for the backward GEMMs. */
-int otb_ls_ce_train(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,
-                    float* tok_loss, float* loss, int32_t* n_valid, void* dlogits_bf16, int ldd, void* stream);
 /* out (+)= sum g^2 over a flat fp32 buffer (global gradient norm, trainer.py:221). */
 int otb_sumsq(const float* g, long long n, float* out, int zero_first, void* stream);
-/* clip_grad_norm_(max_norm) + torch.optim.Adam step on flat fp32 buffers; a non-finite norm skips the update
- * (trainer.py:229-230).  `sumsq` is the device scalar written by otb_sumsq; `step` is the 1-based update count. */
-int otb_adam_step(float* p, const float* g, float* m, float* v, long long n, const float* sumsq, float max_norm, float lr,
-                  float beta1, float beta2, float eps, float weight_decay, int step, void* stream);
 
-/* otb_adam_step with the step counters and the LR schedule on the DEVICE (no host sync, CUDA-graph friendly):
+/* clip_grad_norm_(max_norm) + torch.optim.Adam step on flat fp32 buffers (trainer.py:221-234); `sumsq` is the device scalar
+ * written by otb_sumsq.  The step counters and the LR schedule live on the DEVICE (no host sync, CUDA-graph friendly):
  * counters i32 [3] = {optimizer steps, scheduler global_step, skipped steps}; when sqrt(*sumsq) is finite both counts
  * advance and lr = factor * model_size^-0.5 * min(s^-0.5, s * warmup^-1.5) (TransformerScheduler, train/scheduler.py:137-138;
  * warmup_steps <= 0: lr = base_lr), else only `skipped` advances and nothing is updated -- the reference skips

@@ -284,16 +284,16 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g,
         atomicAdd(out, t);
     }
 }
-// hyper (optional, device f32 [4] = {lr, 1 - b1^t, 1 - b2^t, apply}) overrides lr / bc1 / bc2: written by adam_prepare_kernel,
-// which owns the step counters on the device so that a skipped (non-finite) step advances neither the LR schedule nor
-// Adam's bias-correction count -- exactly what trainer.py:229-233 does on the host.
+// hyper (device f32 [4] = {lr, 1 - b1^t, 1 - b2^t, apply}) is written by adam_prepare_kernel, which owns the step counters
+// on the device so that a skipped (non-finite) step advances neither the LR schedule nor Adam's bias-correction count --
+// exactly what trainer.py:229-233 does on the host.
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, size_t n, const float* __restrict__ sumsq,
-                                                   float max_norm, float lr, float b1, float b2, float eps, float wd,
-                                                   float bc1, float bc2, const float* __restrict__ hyper) {
+                                                   float max_norm, float b1, float b2, float eps, float wd,
+                                                   const float* __restrict__ hyper) {
     const float total = sqrtf(*sumsq);
     if (!isfinite(total)) return;                      // NaN / Inf gradients: skip the step (trainer.py:229-230)
-    if (hyper != nullptr) { lr = hyper[0]; bc1 = hyper[1]; bc2 = hyper[2]; }
+    const float lr = hyper[0], bc1 = hyper[1], bc2 = hyper[2];
     float coef = 1.0f;
     if (max_norm > 0.f) coef = fminf(1.0f, max_norm / (total + 1e-6f));
     const float step = lr / bc1, rs2 = rsqrtf(bc2);
@@ -340,17 +340,6 @@ const char* sumsq_launch(cudaStream_t st, const float* g, size_t n, float* out, 
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
-const char* adam_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
-                        float max_norm, float lr, float b1, float b2, float eps, float wd, int step) {
-    if (step < 1) return "adam: step must be >= 1";
-    const float bc1 = 1.0f - powf(b1, (float)step), bc2 = 1.0f - powf(b2, (float)step);
-    size_t blocks = (n + 1023) / 1024;
-    if (blocks > (size_t)(8 * num_sms())) blocks = 8 * num_sms();
-    if (blocks < 1) blocks = 1;
-    adam_kernel<<<(unsigned)blocks, 256, 0, st>>>(p, g, m, v, n, sumsq, max_norm, lr, b1, b2, eps, wd, bc1, bc2, nullptr);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
-}
 const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
                               float max_norm, float base_lr, float model_size, float warmup, float factor, float b1, float b2,
                               float eps, float wd, int* counters, float* hyper) {
@@ -358,7 +347,7 @@ const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* 
     size_t blocks = (n + 1023) / 1024;
     if (blocks > (size_t)(8 * num_sms())) blocks = 8 * num_sms();
     if (blocks < 1) blocks = 1;
-    adam_kernel<<<(unsigned)blocks, 256, 0, st>>>(p, g, m, v, n, sumsq, max_norm, 0.f, b1, b2, eps, wd, 1.f, 1.f, hyper);
+    adam_kernel<<<(unsigned)blocks, 256, 0, st>>>(p, g, m, v, n, sumsq, max_norm, b1, b2, eps, wd, hyper);
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }

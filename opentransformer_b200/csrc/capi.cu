@@ -137,7 +137,7 @@ int otb_linear(const void* a, int lda, const void* w, int ldw, const float* bias
     if (epilogue == EPI_RESID_LN && (!gamma || !beta)) return fail("otb_linear", "LayerNorm epilogue without gamma/beta");
     if (epilogue == EPI_TABLE && (!table || period < 1)) return fail("otb_linear", "table epilogue without table/period");
     if (row_len && row_period < 1) return fail("otb_linear", "row_len without row_period");
-    if (out_f32 ? (ldc < N) : (ldc < N)) return fail("otb_linear", "ldc < N");
+    if (ldc < N) return fail("otb_linear", "ldc < N");
     GemmParams p;
     memset(&p, 0, sizeof(p));
     p.M = M; p.N = N; p.K = K;
@@ -184,17 +184,14 @@ int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask,
                                               p, seed, site));
 }
 
-}  // extern "C"
-
-namespace otb {
-// otb_attention, otb_attention_lse and otb_attention_dk
-static int attention_impl(const char* where, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v,
-                          int ldv, void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
-                          int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse, int d_k,
-                          void* stream) {
-    if (!q || !k || !v || !out) return fail(where, "null operand");
-    if (d_k != 64 && d_k != 96) return fail(where, "head width d_k must be 64 or 96");
-    if (q_col0 % 8 || k_col0 % 8 || v_col0 % 8 || ldo % 8) return fail(where, "column offsets / ldo must be multiples of 8");
+int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
+                  void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
+                  int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse, int d_k,
+                  void* stream) {
+    if (!q || !k || !v || !out) return fail("otb_attention", "null operand");
+    if (d_k != 64 && d_k != 96) return fail("otb_attention", "head width d_k must be 64 or 96");
+    if (lse && d_k != 64) return fail("otb_attention", "lse is for the 64-wide backward: it needs d_k = 64");
+    if (q_col0 % 8 || k_col0 % 8 || v_col0 % 8 || ldo % 8) return fail("otb_attention", "column offsets / ldo must be multiples of 8");
     AttnParams p;
     p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk;
     p.kv_len = kv_len; p.causal = causal;
@@ -204,33 +201,8 @@ static int attention_impl(const char* where, const void* q, int ldq, int q_rows,
     p.bd = bd; p.ldbd = ldbd;
     p.resid = reinterpret_cast<const bf16*>(resid); p.ldr = ldr;
     p.lse = lse;
-    if (resid && (ldr % 8)) return fail(where, "ldr must be a multiple of 8");
-    RET(where, attn_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p, d_k));
-}
-}  // namespace otb
-
-extern "C" {
-
-int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                  void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
-                  int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, void* stream) {
-    return attention_impl("otb_attention", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, B, H, Tq, Tk, kv_len, causal, q_col0,
-                          k_col0, v_col0, bd, ldbd, resid, ldr, nullptr, 64, stream);
-}
-
-int otb_attention_dk(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                     void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
-                     int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, int d_k, void* stream) {
-    return attention_impl("otb_attention_dk", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, B, H, Tq, Tk, kv_len, causal, q_col0,
-                          k_col0, v_col0, bd, ldbd, resid, ldr, nullptr, d_k, stream);
-}
-
-int otb_attention_lse(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                      void* out, int ldo, int B, int H, int Tq, int Tk, const int* kv_len, int causal, int q_col0,
-                      int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse,
-                      void* stream) {
-    return attention_impl("otb_attention", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, B, H, Tq, Tk, kv_len, causal, q_col0,
-                          k_col0, v_col0, bd, ldbd, resid, ldr, lse, 64, stream);
+    if (resid && (ldr % 8)) return fail("otb_attention", "ldr must be a multiple of 8");
+    RET("otb_attention", attn_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p, d_k));
 }
 
 int otb_layernorm(const void* x, int ldx, void* out, int ldo, int out_f32, const float* g1, const float* b1,
@@ -277,12 +249,7 @@ int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int 
 }
 
 int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
-                         int H, int Lmax, void* stream) {
-    return otb_decode_self_attn_dk(qkv, kc, vc, anc, step_ptr, out, N, H, Lmax, 64, stream);
-}
-
-int otb_decode_self_attn_dk(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
-                            int H, int Lmax, int d_k, void* stream) {
+                         int H, int Lmax, int d_k, void* stream) {
     if (!qkv || !kc || !vc || !anc || !step_ptr || !out) return fail("otb_decode_self_attn", "null operand");
     if (d_k != 64 && d_k != 96) return fail("otb_decode_self_attn", "head width d_k must be 64 or 96");
     RET("otb_decode_self_attn",
@@ -291,10 +258,13 @@ int otb_decode_self_attn_dk(const void* qkv, void* kc, void* vc, const int* anc,
 }
 
 int otb_ls_ce(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,
-              float* tok_loss, float* loss, int32_t* n_valid, float* dlogits, int ldd, void* stream) {
+              float* tok_loss, float* loss, int32_t* n_valid, void* dlogits, int ldd, int dlogits_bf16, void* stream) {
     if (!logits || !targets || !tok_loss || !loss || !n_valid) return fail("otb_ls_ce", "null operand");
+    if (dlogits_bf16 && !dlogits) return fail("otb_ls_ce", "dlogits_bf16 without dlogits");
+    if (dlogits_bf16 && (ldd < V || ldd % 8)) return fail("otb_ls_ce", "a bf16 dlogits needs ldd >= V and a multiple of 8");
     RET("otb_ls_ce", ls_ce_launch(ST(stream), logits, ldl, reinterpret_cast<const long long*>(targets), rows, V, smoothing,
-                                  pad_id, tok_loss, loss, n_valid, dlogits, ldd));
+                                  pad_id, tok_loss, loss, n_valid, dlogits_bf16 ? nullptr : static_cast<float*>(dlogits), ldd,
+                                  dlogits_bf16 ? static_cast<bf16*>(dlogits) : nullptr));
 }
 
 int otb_beam_init(const otb_beam_state* st, void* stream) {
@@ -421,23 +391,9 @@ int otb_embed_bwd(const int64_t* tok, const void* dx, float* dE, int N, int d, i
                                           dE, N, d, vocab, scale));
 }
 
-int otb_ls_ce_train(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,
-                    float* tok_loss, float* loss, int32_t* n_valid, void* dlogits_bf16, int ldd, void* stream) {
-    if (!logits || !targets || !tok_loss || !loss || !n_valid || !dlogits_bf16) return fail("otb_ls_ce_train", "null operand");
-    if (ldd < V || ldd % 8) return fail("otb_ls_ce_train", "ldd must be >= V and a multiple of 8");
-    RET("otb_ls_ce_train", ls_ce_launch(ST(stream), logits, ldl, reinterpret_cast<const long long*>(targets), rows, V, smoothing,
-                                        pad_id, tok_loss, loss, n_valid, nullptr, ldd, reinterpret_cast<bf16*>(dlogits_bf16)));
-}
-
 int otb_sumsq(const float* g, long long n, float* out, int zero_first, void* stream) {
     if (!g || !out || n < 1) return fail("otb_sumsq", "bad arguments");
     RET("otb_sumsq", sumsq_launch(ST(stream), g, (size_t)n, out, zero_first));
-}
-
-int otb_adam_step(float* p, const float* g, float* m, float* v, long long n, const float* sumsq, float max_norm, float lr,
-                  float beta1, float beta2, float eps, float weight_decay, int step, void* stream) {
-    if (!p || !g || !m || !v || !sumsq || n < 1) return fail("otb_adam_step", "bad arguments");
-    RET("otb_adam_step", adam_launch(ST(stream), p, g, m, v, (size_t)n, sumsq, max_norm, lr, beta1, beta2, eps, weight_decay, step));
 }
 
 int otb_adam_step_sched(float* p, const float* g, float* m, float* v, long long n, const float* sumsq, float max_norm,

@@ -123,8 +123,6 @@ const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* 
                                int F1, int T2, int F2, int C);
 const char* spec_augment_launch(cudaStream_t st, float* x, const int* bands, int B, int T, int F, int nf, int nt);
 const char* sumsq_launch(cudaStream_t st, const float* g, size_t n, float* out, int zero_first);
-const char* adam_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
-                        float max_norm, float lr, float b1, float b2, float eps, float wd, int step);
 const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
                               float max_norm, float base_lr, float model_size, float warmup, float factor, float b1, float b2,
                               float eps, float wd, int* counters, float* hyper);

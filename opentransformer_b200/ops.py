@@ -64,6 +64,16 @@ def _need(t, dtype, name):
     return t
 
 
+def _mat(t, name):
+    """A GEMM operand: 2-D bf16 CUDA tensor with unit column stride (row-strided views such as one head's columns of a
+    wider matrix are fine: the TMA map takes the row pitch)."""
+    if not t.is_cuda:
+        raise RuntimeError(f'{name} must be a CUDA tensor: the CUDA hot path has no CPU fallback')
+    if t.dtype != BF16 or t.dim() != 2 or t.stride(1) != 1:
+        raise TypeError(f'{name} must be a 2-D bf16 tensor with unit column stride')
+    return t
+
+
 def set_decode_barrier(kind):
     """'cluster', 'software' or 'default': group barrier of the persistent decode kernel (otb_set_decode_barrier)."""
     check(_lib.lib().otb_set_decode_barrier({'default': -1, 'software': 0, 'cluster': 1}[kind]), 'otb_set_decode_barrier')
@@ -115,13 +125,8 @@ def conv2_relu(h1, w, bias, B, T, F, out=None):
 
 def linear(a, w, bias=None, epilogue=EPI_BIAS, out=None, out_f32=False, resid=None, gamma=None, beta=None,
            eps=1e-5, alpha=1.0, table=None, period=0, row_len=None, row_period=0, n_out=None):
-    """out[M,N] = epi(a[M,K] @ w[N(,2N),K]^T + bias).  a, w bf16 2-D, unit column stride (row-strided views
-    such as one head's 64 columns of a wider matrix are fine: the TMA map takes the row pitch)."""
-    for t, n in ((a, 'a'), (w, 'w')):
-        if not t.is_cuda:
-            raise RuntimeError(f'{n} must be a CUDA tensor: the CUDA hot path has no CPU fallback')
-        if t.dtype != BF16 or t.dim() != 2 or t.stride(1) != 1:
-            raise TypeError(f'{n} must be a 2-D bf16 tensor with unit column stride')
+    """out[M,N] = epi(a[M,K] @ w[N(,2N),K]^T + bias).  a, w: see _mat."""
+    _mat(a, 'a'); _mat(w, 'w')
     M, K = a.shape
     N = w.shape[0] // 2 if epilogue == EPI_GLU else w.shape[0]
     if w.shape[1] != K:
@@ -150,9 +155,7 @@ def gemm_config(M, N, epilogue=EPI_BIAS, out_f32=False):
 def linear_dropout_resid(a, w, bias, resid, p, seed, site, alpha=1.0, out=None):
     """out = resid + alpha * dropout_p(a @ w^T + bias): training-mode residual connection (otb_linear_dropout_resid).
     seed: int32/uint32 device tensor [1] (read at run time), site: dropout site id."""
-    for t, n in ((a, 'a'), (w, 'w'), (resid, 'resid')):
-        if not t.is_cuda or t.dtype != BF16 or t.dim() != 2 or t.stride(1) != 1:
-            raise TypeError(f'{n} must be a 2-D bf16 CUDA tensor with unit column stride')
+    _mat(a, 'a'); _mat(w, 'w'); _mat(resid, 'resid')
     M, K = a.shape
     N = w.shape[0]
     if out is None:
@@ -192,27 +195,30 @@ def check_head_dim(d_k):
         raise NotImplementedError(f'the sm_90a attention kernels support head widths d_k in {HEAD_DIMS}, got {d_k}')
 
 
+def _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, out=None, bd=None, resid=None, d_k=64,
+               with_lse=False):
+    """otb_attention -> (out bf16 [B*Tq, H*d_k], lse f32 [B,H,Tq] if with_lse else None)."""
+    for t, n in ((q, 'q'), (k, 'k'), (v, 'v')):
+        _need(t, BF16, n)
+    check_head_dim(d_k)
+    if out is None:
+        out = torch.empty(B * Tq, H * d_k, dtype=BF16, device=q.device)
+    lse = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device) if with_lse else None
+    if kv_len is not None:
+        _need(kv_len, torch.int32, 'kv_len')
+    check(_lib.lib().otb_attention(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out),
+                                   out.stride(0), B, H, Tq, Tk, _p(kv_len), 1 if causal else 0, q_col0, k_col0, v_col0, _p(bd),
+                                   bd.shape[-1] if bd is not None else 0, _p(resid), resid.stride(0) if resid is not None else 0,
+                                   _p(lse), d_k, _stream()), 'otb_attention')
+    _count()
+    return out, lse
+
+
 def attention(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, v_col0=0, out=None, bd=None,
               resid=None, d_k=64):
     """q/k/v: bf16 2-D matrices (may be the same [M,3d] buffer with different column offsets); head h of each starts
     at column col0 + d_k*h.  Returns bf16 [B*Tq, H*d_k]."""
-    for t, n in ((q, 'q'), (k, 'k'), (v, 'v')):
-        _need(t, BF16, n)
-    check_head_dim(d_k)
-    d = H * d_k
-    if out is None:
-        out = torch.empty(B * Tq, d, dtype=BF16, device=q.device)
-    if kv_len is not None:
-        _need(kv_len, torch.int32, 'kv_len')
-    args = (_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out), out.stride(0), B, H, Tq,
-            Tk, _p(kv_len), 1 if causal else 0, q_col0, k_col0, v_col0, _p(bd), bd.shape[-1] if bd is not None else 0, _p(resid),
-            resid.stride(0) if resid is not None else 0)
-    if d_k == 64:
-        check(_lib.lib().otb_attention(*args, _stream()), 'otb_attention')
-    else:
-        check(_lib.lib().otb_attention_dk(*args, d_k, _stream()), 'otb_attention_dk')
-    _count()
-    return out
+    return _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, out, bd, resid, d_k)[0]
 
 
 def dwconv_swish(x, w, b, B, T, out=None):
@@ -304,9 +310,9 @@ def logsoftmax_topk(logits, V, k, lm_logp=None, lm_weight=0.0, out_val=None, out
     return out_val, out_idx
 
 
-def ls_cross_entropy(logits, targets, V, smoothing=0.1, pad_id=0, want_grad=False):
-    """Label-smoothed CE (module/loss.py:21-48).  logits f32 [rows, ld]; targets i64 [rows].
-    Returns (loss f32 scalar tensor, dlogits f32 [rows, V] or None)."""
+def _ls_ce(logits, targets, V, smoothing, pad_id, grad_dtype):
+    """otb_ls_ce -> (loss f32 scalar tensor, dlogits or None): no gradient for grad_dtype None, f32 [rows, V] for float32,
+    bf16 [rows, ld] with ld = logits.stride(0) and zero pad columns for bfloat16."""
     _need(logits, torch.float32, 'logits')
     rows = logits.shape[0]
     targets = targets.contiguous().view(-1)
@@ -314,11 +320,18 @@ def ls_cross_entropy(logits, targets, V, smoothing=0.1, pad_id=0, want_grad=Fals
     tok = torch.empty(rows, dtype=torch.float32, device=dev)
     loss = torch.empty(1, dtype=torch.float32, device=dev)
     nv = torch.empty(1, dtype=torch.int32, device=dev)
-    dl = torch.empty(rows, V, dtype=torch.float32, device=dev) if want_grad else None
+    ldd = {None: 0, torch.float32: V, BF16: logits.stride(0)}[grad_dtype]
+    dl = torch.empty(rows, ldd, dtype=grad_dtype, device=dev) if grad_dtype is not None else None
     check(_lib.lib().otb_ls_ce(_p(logits), logits.stride(0), _p(targets), rows, V, smoothing, pad_id, _p(tok), _p(loss),
-                               _p(nv), _p(dl), V if want_grad else 0, _stream()), 'otb_ls_ce')
+                               _p(nv), _p(dl), ldd, 1 if grad_dtype == BF16 else 0, _stream()), 'otb_ls_ce')
     _count(3)
     return loss[0], dl
+
+
+def ls_cross_entropy(logits, targets, V, smoothing=0.1, pad_id=0, want_grad=False):
+    """Label-smoothed CE (module/loss.py:21-48).  logits f32 [rows, ld]; targets i64 [rows].
+    Returns (loss f32 scalar tensor, dlogits f32 [rows, V] or None)."""
+    return _ls_ce(logits, targets, V, smoothing, pad_id, torch.float32 if want_grad else None)
 
 
 def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None):
@@ -330,12 +343,8 @@ def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None):
     check_head_dim(d_k)
     if out is None:
         out = torch.empty(N, d, dtype=BF16, device=qkv.device)
-    if d_k == 64:
-        check(_lib.lib().otb_decode_self_attn(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax,
-                                              _stream()), 'otb_decode_self_attn')
-    else:
-        check(_lib.lib().otb_decode_self_attn_dk(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax, d_k,
-                                                 _stream()), 'otb_decode_self_attn_dk')
+    check(_lib.lib().otb_decode_self_attn(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax, d_k, _stream()),
+          'otb_decode_self_attn')
     _count()
     return out
 
@@ -415,24 +424,16 @@ def decode_persistent(model_c, kvx, mem_len, kc, vc, state, B, T, max_steps, wor
 # training step: backward kernels (include/otb200.h "Training step")
 # ------------------------------------------------------------------------------------------------
 def attention_train(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, v_col0=0):
-    """otb_attention + the per-row log-sum-exp the backward needs -> (out bf16 [B*Tq, H*64], lse f32 [B,H,Tq])."""
-    for t, n in ((q, 'q'), (k, 'k'), (v, 'v')):
-        _need(t, BF16, n)
-    out = torch.empty(B * Tq, H * 64, dtype=BF16, device=q.device)
-    lse = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device)
-    check(_lib.lib().otb_attention_lse(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0),
-                                       _p(out), out.stride(0), B, H, Tq, Tk, _p(kv_len), 1 if causal else 0, q_col0, k_col0,
-                                       v_col0, None, 0, None, 0, _p(lse), _stream()), 'otb_attention_lse')
-    _count()
-    return out, lse
+    """attention (d_k 64, the width of the backward) + the per-row log-sum-exp the backward needs
+    -> (out bf16 [B*Tq, H*64], lse f32 [B,H,Tq])."""
+    return _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, with_lse=True)
 
 
 def attention_bwd(q, k, v, out, dout, lse, B, H, Tq, Tk, dq, dk, dv, kv_len=None, causal=False, q_col0=0, k_col0=0,
                   v_col0=0, dq_col0=0, dk_col0=0, dv_col0=0):
     """Gradients of otb_attention written into dq/dk/dv (bf16 matrices, column offsets d*_col0)."""
     for t, n in ((q, 'q'), (k, 'k'), (v, 'v'), (out, 'out'), (dout, 'dout'), (dq, 'dq'), (dk, 'dk'), (dv, 'dv')):
-        if not t.is_cuda or t.dtype != BF16 or t.dim() != 2 or t.stride(1) != 1:
-            raise TypeError(f'{n} must be a 2-D bf16 CUDA tensor with unit column stride (no CPU fallback)')
+        _mat(t, n)
     dsum = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device)
     check(_lib.lib().otb_attention_bwd(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0),
                                        _p(out), out.stride(0), _p(dout), dout.stride(0), _p(lse), _p(dsum),
@@ -444,9 +445,7 @@ def attention_bwd(q, k, v, out, dout, lse, B, H, Tq, Tk, dq, dk, dv, kv_len=None
 
 def linear_wgrad(dy, x, out=None, accumulate=False):
     """dW f32 [N,K] (+)= dy[M,N]^T x[M,K]  (bf16 2-D, unit column stride)."""
-    for t, n in ((dy, 'dy'), (x, 'x')):
-        if not t.is_cuda or t.dtype != BF16 or t.dim() != 2 or t.stride(1) != 1:
-            raise TypeError(f'{n} must be a 2-D bf16 CUDA tensor with unit column stride')
+    _mat(dy, 'dy'); _mat(x, 'x')
     M, N = dy.shape
     K = x.shape[1]
     if x.shape[0] != M:
@@ -520,30 +519,11 @@ def embed_bwd(tok, dx, dE, scale):
 
 def ls_cross_entropy_train(logits, targets, V, smoothing=0.1, pad_id=0):
     """-> (loss f32 scalar tensor, dlogits bf16 [rows, ld] with ld = logits.stride(0); pad columns zero)."""
-    _need(logits, torch.float32, 'logits')
-    rows, ld = logits.shape[0], logits.stride(0)
-    targets = targets.contiguous().view(-1)
-    dev = logits.device
-    tok = torch.empty(rows, dtype=torch.float32, device=dev)
-    loss = torch.empty(1, dtype=torch.float32, device=dev)
-    nv = torch.empty(1, dtype=torch.int32, device=dev)
-    dl = torch.empty(rows, ld, dtype=BF16, device=dev)
-    check(_lib.lib().otb_ls_ce_train(_p(logits), ld, _p(targets), rows, V, smoothing, pad_id, _p(tok), _p(loss), _p(nv),
-                                     _p(dl), ld, _stream()), 'otb_ls_ce_train')
-    _count(3)
-    return loss[0], dl
+    return _ls_ce(logits, targets, V, smoothing, pad_id, BF16)
 
 
 def sumsq(g, out, zero_first=True):
     check(_lib.lib().otb_sumsq(_p(g), g.numel(), _p(out), 1 if zero_first else 0, _stream()), 'otb_sumsq')
-    _count()
-
-
-def adam_step(p, g, m, v, sumsq_buf, max_norm, lr, betas, eps, weight_decay, step):
-    for t, n in ((p, 'p'), (g, 'g'), (m, 'm'), (v, 'v')):
-        _need(t, torch.float32, n)
-    check(_lib.lib().otb_adam_step(_p(p), _p(g), _p(m), _p(v), p.numel(), _p(sumsq_buf), max_norm, lr, betas[0], betas[1],
-                                   eps, weight_decay, step, _stream()), 'otb_adam_step')
     _count()
 
 

@@ -1,5 +1,6 @@
 """CPU-side checks of the C-ABI boundary: the library builds/loads without a GPU driver and exports
-every symbol include/otb200.h declares.  No compute calls."""
+every symbol include/otb200.h declares, and the ctypes binding has the header's signatures and struct layouts.
+No compute calls."""
 import ctypes
 import os
 import re
@@ -15,10 +16,73 @@ def libpath():
     return build.build()
 
 
-def _header_symbols():
+def _header_text():
     text = open(os.path.join(ROOT, 'include', 'otb200.h')).read()
-    text = re.sub(r'/\*.*?\*/', '', text, flags=re.S)
-    return sorted(set(re.findall(r'\b(otb_[a-z0-9_]+)\s*\(', text)))
+    return re.sub(r'/\*.*?\*/|//[^\n]*', '', text, flags=re.S)
+
+
+def _header_symbols():
+    return sorted(set(re.findall(r'\b(otb_[a-z0-9_]+)\s*\(', _header_text())))
+
+
+# What a C type is at the ABI, the granularity at which ctypes can get it wrong.
+_C_KINDS = {'int': 'i32', 'int32_t': 'i32', 'uint32_t': 'u32', 'long long': 'i64', 'int64_t': 'i64', 'float': 'f32',
+            'void': 'void'}
+_C_STRUCTS = ('otb_beam_state', 'otb_mega_model')
+_DECLARATOR = re.compile(r'(.*?)(\**)\s*(\w+)\s*(?:\[(\w+)\])?$', re.S)   # type, stars, name, array length
+
+
+def _c_kind(type_text, stars, length=None, defines=None):
+    base = ' '.join(w for w in re.findall(r'\w+', type_text) if w != 'const')
+    if stars:
+        return f'ptr:{base}' if base in _C_STRUCTS else 'pointer'
+    if length is not None:
+        return f'{base}[{defines.get(length, length)}]'
+    return _C_KINDS[base]
+
+
+def _parse_header():
+    """-> ({function: (return kind, [argument kinds])}, {struct: [(field, kind)]}, {macro: value})."""
+    text = _header_text()
+    defines = dict(re.findall(r'^\s*#define\s+(\w+)\s+(\S+)', text, flags=re.M))
+    text = re.sub(r'^\s*#.*$', '', text, flags=re.M)
+    protos = {}
+    for ret, name, params in re.findall(r'([\w\s*]+?)\b(otb_\w+)\s*\(([^()]*)\)\s*;', text):
+        args = [] if params.strip() in ('', 'void') else [_DECLARATOR.match(p.strip()).groups() for p in params.split(',')]
+        protos[name] = (_c_kind(ret, '*' in ret), [_c_kind(t, s) for t, s, _, _ in args])
+    structs = {}
+    for body, name in re.findall(r'typedef\s+struct\s*\{(.*?)\}\s*(\w+)\s*;', text, flags=re.S):
+        fields = []
+        for decl in filter(None, (d.strip() for d in body.split(';'))):
+            first, *rest = decl.split(',')
+            base, stars, field, length = _DECLARATOR.match(first.strip()).groups()
+            fields.append((field, _c_kind(base, stars, length, defines)))
+            for more in rest:                       # `const void *wqkv, *wo, ...`: the base type carries over
+                _, stars, field, length = _DECLARATOR.match(more.strip()).groups()
+                fields.append((field, _c_kind(base, stars, length, defines)))
+        structs[name] = fields
+    return protos, structs, defines
+
+
+def _py_kind(t):
+    from opentransformer_b200 import _lib
+    if t is None:
+        return 'void'
+    if issubclass(t, ctypes._Pointer):
+        return {_lib.BeamStateC: 'ptr:otb_beam_state', _lib.MegaModelC: 'ptr:otb_mega_model'}.get(t._type_, 'pointer')
+    if issubclass(t, ctypes.Array):
+        element = {_lib.MegaLayerC: 'otb_mega_layer'}[t._type_]
+        return f'{element}[{t._length_}]'
+    code = t._type_
+    if code in ('P', 'z'):                          # c_void_p, c_char_p
+        return 'pointer'
+    if code == 'f':
+        return 'f32'
+    if code in 'bhilq':
+        return f'i{8 * ctypes.sizeof(t)}'
+    if code in 'BHILQ':
+        return f'u{8 * ctypes.sizeof(t)}'
+    raise AssertionError(f'no ABI kind for ctypes type {t}')
 
 
 def test_library_loads_and_exports_every_declared_symbol(libpath):
@@ -30,14 +94,35 @@ def test_library_loads_and_exports_every_declared_symbol(libpath):
 
 
 def test_python_binding_covers_the_header():
-    from opentransformer_b200 import exported_symbols
+    """Every prototype in the header has a ctypes binding with the same return and argument kinds, in order.  A binding
+    that drops an argument or passes c_int where the C function takes float still loads; it only goes wrong on the GPU."""
+    from opentransformer_b200 import _lib, exported_symbols
+    protos, _, _ = _parse_header()
+    assert sorted(protos) == _header_symbols()
     assert exported_symbols() == _header_symbols()
+    bad = []
+    for name, want in sorted(protos.items()):
+        res, args = _lib._SIGS[name]
+        got = (_py_kind(res), [_py_kind(a) for a in args])
+        if got != want:
+            bad.append(f'{name}: header {want}, _SIGS {got}')
+    assert not bad, 'ctypes signatures differ from include/otb200.h:\n' + '\n'.join(bad)
 
 
-def test_version_and_error_reporting(libpath):
+def test_ctypes_structs_match_the_header():
+    """Field names, order and kinds of the ctypes mirrors of the header's structs, and the layer capacity."""
+    from opentransformer_b200 import _lib
+    _, structs, defines = _parse_header()
+    for cname, mirror in (('otb_beam_state', _lib.BeamStateC), ('otb_mega_layer', _lib.MegaLayerC),
+                          ('otb_mega_model', _lib.MegaModelC)):
+        assert [(f, _py_kind(t)) for f, t in mirror._fields_] == structs[cname], f'{mirror.__name__} differs from {cname}'
+    assert _lib.MEGA_MAX_LAYERS == int(defines['OTB_MEGA_MAX_LAYERS'])
+
+
+def test_version_2_and_error_reporting(libpath):
     from opentransformer_b200 import _lib
     lib = _lib.lib()
-    assert lib.otb_version() == 1
+    assert lib.otb_version() == 2
     t1 = ctypes.c_int()
     assert lib.otb_conv_geometry(1000, 80, t1, None, None, None) == 0 and t1.value == 499
     assert lib.otb_conv_geometry(3, 80, None, None, None, None) != 0       # too short -> status, not abort

@@ -150,7 +150,7 @@ def test_attention_backward(B, H, Tq, Tk, causal, ragged, cross):
     assert _rel(out, ref) < 1e-2 and rq < 2e-2 and rk < 2e-2 and rv < 2e-2
 
 
-def test_ls_ce_train_grad_and_adam():
+def test_ls_ce_train_grad_and_fixed_lr_scheduled_adam():
     rows, V, ld = 90, 4234, 4240
     g = torch.Generator().manual_seed(5)
     logits = torch.zeros(rows, ld, device=DEV)
@@ -174,18 +174,24 @@ def test_ls_ce_train_grad_and_adam():
     opt = torch.optim.Adam([pr], lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6)
     p, m, v = p0.clone(), torch.zeros(n, device=DEV), torch.zeros(n, device=DEV)
     ss = torch.zeros(1, device=DEV)
+    counters = torch.zeros(3, dtype=torch.int32, device=DEV)
+    hyper = torch.zeros(4, device=DEV)
+
+    def adam(grad):   # warmup_steps 0: the fixed lr 1e-3, step count kept on the device
+        ops.adam_step_sched(p, grad, m, v, ss, 5.0, 1e-3, 256, 0, 1.0, (0.9, 0.98), 1e-9, 1e-6, counters, hyper)
+
     for step in range(1, 4):
         gr = (torch.randn(n, generator=g) * (10.0 if step == 2 else 0.01)).to(DEV)
         pr.grad = gr.clone()
         torch.nn.utils.clip_grad_norm_([pr], 5.0)
         opt.step()
         ops.sumsq(gr, ss)
-        ops.adam_step(p, gr, m, v, ss, 5.0, 1e-3, (0.9, 0.98), 1e-9, 1e-6, step)
+        adam(gr)
         torch.testing.assert_close(p, pr.detach(), rtol=1e-5, atol=1e-6)
     bad = torch.full((n,), float('nan'), device=DEV)
     before = p.clone()
     ops.sumsq(bad, ss)
-    ops.adam_step(p, bad, m, v, ss, 5.0, 1e-3, (0.9, 0.98), 1e-9, 1e-6, 4)
+    adam(bad)
     assert torch.equal(p, before), 'non-finite gradient norm must skip the update (trainer.py:229-230)'
 
 
