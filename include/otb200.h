@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define OTB_VERSION 2
+#define OTB_VERSION 3
 
 /* GEMM epilogues (otb_linear) */
 enum {
@@ -46,10 +46,6 @@ int otb_num_sms(void);
  * fewest MMA waves; 1 = least SM-time -- the widest tile on the fewest CTAs, for servers that keep several utterance
  * batches in flight on separate streams.  Process-wide; set it before CUDA graphs are captured. */
 int otb_set_tile_policy(int policy);
-/* Profiling aid: buf (device, u64 [grid*8]) receives per-CTA clock64 phase stamps of the next GEMMs; NULL disables. */
-int otb_debug_gemm_timing(unsigned long long* buf);
-/* Profiling aid: 0 = normal, 1 = GEMM mainloop without TMA traffic, 2 = without MMAs (results are garbage). */
-int otb_debug_gemm_mode(int mode);
 /* Profiling aid: buf (device, u64 [>= 256]) receives clock64 stamps at every phase boundary of decode step `step`
  * of the next otb_decode_persistent launches (group 0, CTA 0); NULL disables. */
 int otb_debug_decode_timing(unsigned long long* buf, int step);

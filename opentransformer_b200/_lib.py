@@ -40,8 +40,6 @@ _SIGS = {
     'otb_last_error': (c_char_p, []),
     'otb_version': (c_int, []),
     'otb_num_sms': (c_int, []),
-    'otb_debug_gemm_timing': (c_int, [_P]),
-    'otb_debug_gemm_mode': (c_int, [c_int]),
     'otb_set_tile_policy': (c_int, [c_int]),
     'otb_debug_decode_timing': (c_int, [_P, c_int]),
     'otb_set_decode_barrier': (c_int, [c_int]),

@@ -14,6 +14,7 @@
 // warpgroup with operands staged by TMA (K-major tiles; the [rows x 64] tile that is contracted over its rows is read as
 // an MN-major B operand, exactly like V in the forward); dS / P^T tiles are written by the threads as bf16 in the
 // canonical 128B-swizzled layout.  Score tiles are formed in two 64-column halves to bound the register footprint.
+#include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
 
@@ -322,17 +323,9 @@ const char* attn_bwd_launch(cudaStream_t st, const void* q, int ldq, int q_rows,
     if ((err = encode_tmap_2d(&tk, k, (uint64_t)ldk, (uint64_t)k_rows, (uint64_t)ldk, 64, 128))) return err;
     if ((err = encode_tmap_2d(&tv, v, (uint64_t)ldv, (uint64_t)k_rows, (uint64_t)ldv, 64, 128))) return err;
     if ((err = encode_tmap_2d(&tdo, p.dout, (uint64_t)p.lddo, (uint64_t)q_rows, (uint64_t)p.lddo, 64, 128))) return err;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ABW_SMEM_DQ) != cudaSuccess ||
-            cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ABW_SMEM_DKV) != cudaSuccess)
-            return "cudaFuncSetAttribute(attn_bwd smem) failed";
-        attr_set = true;
-    }
-    attn_bwd_dq_kernel<<<dim3((p.Tq + 127) / 128, p.H, p.B), 256, ABW_SMEM_DQ, st>>>(tq, tk, tv, tdo, p);
-    attn_bwd_dkv_kernel<<<dim3((p.Tk + 127) / 128, p.H, p.B), 256, ABW_SMEM_DKV, st>>>(tq, tk, tv, tdo, p);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    if ((err = launch<attn_bwd_dq_kernel>(dim3((p.Tq + 127) / 128, p.H, p.B), 256, ABW_SMEM_DQ, st, tq, tk, tv, tdo, p)))
+        return err;
+    return launch<attn_bwd_dkv_kernel>(dim3((p.Tk + 127) / 128, p.H, p.B), 256, ABW_SMEM_DKV, st, tq, tk, tv, tdo, p);
 }
 
 }  // namespace otb

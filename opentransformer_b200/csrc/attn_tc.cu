@@ -40,8 +40,6 @@ template <int DK, bool HAS_BD>
 __global__ void __launch_bounds__(256, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-    PDL_TRIGGER();
-    PDL_WAIT();   // before the first global read (kv_len) -- launch latency and CTA scheduling still overlap the predecessor
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr int NB = AttnCfg<DK>::BOXES, TILE = AttnCfg<DK>::TILE;
@@ -223,17 +221,9 @@ template <int DK>
 static const char* attn_launch_dk(cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                                   const AttnParams& p) {
     constexpr int SMEM = AttnCfg<DK>::SMEM;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(attn_tc_kernel<DK, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess ||
-            cudaFuncSetAttribute(attn_tc_kernel<DK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM) != cudaSuccess)
-            return "cudaFuncSetAttribute(attn smem) failed";
-        attr_set = true;
-    }
     dim3 grid((p.Tq + 127) / 128, p.H, p.B);
-    cudaError_t e = p.bd ? launch_pdl(attn_tc_kernel<DK, true>, grid, dim3(256), SMEM, st, tq, tk, tv, p)
-                         : launch_pdl(attn_tc_kernel<DK, false>, grid, dim3(256), SMEM, st, tq, tk, tv, p);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return p.bd ? launch<attn_tc_kernel<DK, true>>(grid, dim3(256), SMEM, st, tq, tk, tv, p)
+                : launch<attn_tc_kernel<DK, false>>(grid, dim3(256), SMEM, st, tq, tk, tv, p);
 }
 
 const char* attn_launch(cudaStream_t st, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows,

@@ -4,6 +4,7 @@
 #include <math.h>
 
 #include "dropout.cuh"
+#include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
 
@@ -56,9 +57,7 @@ const char* colsum_launch(cudaStream_t st, const bf16* x, int ldx, float* out, i
     int gy = (M + 255) / 256;
     if (gy > 64) gy = 64;
     if (gy < 1) gy = 1;
-    colsum_kernel<<<dim3((N + 63) / 64, gy), 256, 0, st>>>(x, ldx, out, M, N);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<colsum_kernel>(dim3((N + 63) / 64, gy), 256, 0, st, x, ldx, out, M, N);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -137,9 +136,7 @@ const char* layernorm_bwd_launch(cudaStream_t st, const bf16* dy, int lddy, cons
     if (e != cudaSuccess) return cudaGetErrorString(e);
     int grid = (M + 7) / 8;
     if (grid > 4 * num_sms()) grid = 4 * num_sms();
-    layernorm_bwd_kernel<<<grid, 256, 0, st>>>(dy, lddy, z, ldz, gamma, dz, lddz, dgamma, dbeta, eps, M, N);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<layernorm_bwd_kernel>(grid, 256, 0, st, dy, lddy, z, ldz, gamma, dz, lddz, dgamma, dbeta, eps, M, N);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -180,10 +177,8 @@ __global__ void __launch_bounds__(256) glu_bwd_kernel(const bf16* __restrict__ d
 const char* glu_launch(cudaStream_t st, const bf16* u, const bf16* dh, bf16* out, int M, int F) {
     if (F % 8) return "glu: F must be a multiple of 8";
     const size_t n = (size_t)M * (F / 8);
-    if (dh) glu_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dh, u, out, M, F);
-    else glu_fwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(u, out, M, F);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    return dh ? launch<glu_bwd_kernel>(grid, 256, 0, st, dh, u, out, M, F) : launch<glu_fwd_kernel>(grid, 256, 0, st, u, out, M, F);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -225,16 +220,13 @@ const char* dropout_bwd_launch(cudaStream_t st, const bf16* dy, int lddy, bf16* 
     if (!(p >= 0.f && p < 1.f)) return "dropout: p must be in [0, 1)";
     if (!seed) return "dropout: null seed";
     const size_t n = (size_t)M * (N / 2);
-    dropout_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dy, lddy, out, ldo, mask, M, N, drop_threshold(p), 1.0f / (1.0f - p), seed, site);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<dropout_bwd_kernel>((unsigned)((n + 255) / 256), 256, 0, st, dy, lddy, out, ldo, mask, M, N,
+                                      drop_threshold(p), 1.0f / (1.0f - p), seed, site);
 }
 
 const char* relu_bwd_launch(cudaStream_t st, const bf16* dy, const bf16* y, bf16* dx, size_t n) {
     if (n % 8) return "relu_bwd: n must be a multiple of 8";
-    relu_bwd_kernel<<<(unsigned)((n / 8 + 255) / 256), 256, 0, st>>>(dy, y, dx, n / 8);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<relu_bwd_kernel>((unsigned)((n / 8 + 255) / 256), 256, 0, st, dy, y, dx, n / 8);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -256,9 +248,7 @@ __global__ void __launch_bounds__(256) embed_bwd_kernel(const long long* __restr
 }
 const char* embed_bwd_launch(cudaStream_t st, const long long* tok, const bf16* dx, float* dE, int N, int d, int vocab, float scale) {
     if (d % 8) return "embed_bwd: d must be a multiple of 8";
-    embed_bwd_kernel<<<(N + 7) / 8, 256, 0, st>>>(tok, dx, dE, N, d, vocab, scale);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<embed_bwd_kernel>((N + 7) / 8, 256, 0, st, tok, dx, dE, N, d, vocab, scale);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -336,20 +326,17 @@ const char* sumsq_launch(cudaStream_t st, const float* g, size_t n, float* out, 
     size_t blocks = (n + 2047) / 2048;
     if (blocks > (size_t)(8 * num_sms())) blocks = 8 * num_sms();
     if (blocks < 1) blocks = 1;
-    sumsq_kernel<<<(unsigned)blocks, 256, 0, st>>>(g, n, out);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<sumsq_kernel>((unsigned)blocks, 256, 0, st, g, n, out);
 }
 const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
                               float max_norm, float base_lr, float model_size, float warmup, float factor, float b1, float b2,
                               float eps, float wd, int* counters, float* hyper) {
-    adam_prepare_kernel<<<1, 1, 0, st>>>(sumsq, counters, hyper, base_lr, model_size, warmup, factor, b1, b2);
+    const char* err = launch<adam_prepare_kernel>(1, 1, 0, st, sumsq, counters, hyper, base_lr, model_size, warmup, factor, b1, b2);
+    if (err) return err;
     size_t blocks = (n + 1023) / 1024;
     if (blocks > (size_t)(8 * num_sms())) blocks = 8 * num_sms();
     if (blocks < 1) blocks = 1;
-    adam_kernel<<<(unsigned)blocks, 256, 0, st>>>(p, g, m, v, n, sumsq, max_norm, b1, b2, eps, wd, hyper);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<adam_kernel>((unsigned)blocks, 256, 0, st, p, g, m, v, n, sumsq, max_norm, b1, b2, eps, wd, hyper);
 }
 
 }  // namespace otb
@@ -471,17 +458,14 @@ __global__ void __launch_bounds__(256) conv1_wgrad_kernel(const bf16* __restrict
 const char* im2col_s2_launch(cudaStream_t st, const bf16* h1, bf16* col, int B, int T2, int F2, int C) {
     if (C % 8) return "im2col: C must be a multiple of 8";
     const size_t total = (size_t)B * T2 * F2 * 9 * (C / 8);
-    im2col_s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(h1, col, B, T2, F2, C, 2 * (T2 + 1), 2 * F2);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<im2col_s2_kernel>((unsigned)((total + 255) / 256), 256, 0, st, h1, col, B, T2, F2, C, 2 * (T2 + 1), 2 * F2);
 }
 const char* col2im_s2_relu_launch(cudaStream_t st, const bf16* dcol, const bf16* h1, bf16* dpre1, int B, int T1, int F1, int T2,
                                   int F2, int C) {
     if (C % 8) return "col2im: C must be a multiple of 8";
     const size_t total = (size_t)B * 2 * (T2 + 1) * 2 * F2 * (C / 8);
-    col2im_s2_relu_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(dcol, h1, dpre1, B, T1, F1, T2, F2, C, 2 * (T2 + 1), 2 * F2);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<col2im_s2_relu_kernel>((unsigned)((total + 255) / 256), 256, 0, st, dcol, h1, dpre1, B, T1, F1, T2, F2, C,
+                                         2 * (T2 + 1), 2 * F2);
 }
 const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* x, float* out, int B, int T, int F, int T1,
                                int F1, int T2, int F2, int C) {
@@ -493,9 +477,7 @@ const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* 
     cudaError_t e = cudaMemsetAsync(out, 0, (size_t)C * 10 * 4, st);
     if (e != cudaSuccess) return cudaGetErrorString(e);
     const int chunks = (T1 + 7) / 8;
-    conv1_wgrad_kernel<<<B * chunks, 256, smem, st>>>(dpre1, x, out, B, T, F, T1, F1, 2 * (T2 + 1), 2 * F2, C);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<conv1_wgrad_kernel>(B * chunks, 256, smem, st, dpre1, x, out, B, T, F, T1, F1, 2 * (T2 + 1), 2 * F2, C);
 }
 
 }  // namespace otb
@@ -522,9 +504,7 @@ __global__ void __launch_bounds__(256) spec_augment_kernel(float* __restrict__ x
 }
 const char* spec_augment_launch(cudaStream_t st, float* x, const int* bands, int B, int T, int F, int nf, int nt) {
     const size_t n = (size_t)B * T * F;
-    spec_augment_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, bands, B, T, F, nf, nt);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<spec_augment_kernel>((unsigned)((n + 255) / 256), 256, 0, st, x, bands, B, T, F, nf, nt);
 }
 
 }  // namespace otb

@@ -30,8 +30,6 @@ __global__ void __launch_bounds__(KMAX * 32) beam_step_kernel(const float* __res
                                                               float lm_weight, BeamState st, long long* dbg_ktok,
                                                               int* dbg_offs, const float* __restrict__ pre_val,
                                                               const int* __restrict__ pre_idx) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     __shared__ float c_val[KMAX * KMAX];
     __shared__ int c_tok[KMAX * KMAX];
     __shared__ float sel_v[KMAX];
@@ -131,9 +129,8 @@ const char* beam_step_launch(cudaStream_t stream, const float* logp, int ldl, in
     if (st.N % st.beam) return "beam_step: N must be a multiple of beam";
     if (!logp && !pre_val) return "beam_step: need log-probs or a precomputed top-k";
     if ((pre_val == nullptr) != (pre_idx == nullptr)) return "beam_step: pre_val / pre_idx must both be given";
-    cudaError_t e = launch_pdl(beam_step_kernel, dim3(st.N / st.beam), dim3(st.beam * 32), 0, stream, logp, ldl, V, lm_logp, ld_lm,
-                               lm_weight, st, dbg_ktok, dbg_offs, pre_val, pre_idx);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<beam_step_kernel>(dim3(st.N / st.beam), dim3(st.beam * 32), 0, stream, logp, ldl, V, lm_logp, ld_lm,
+                                    lm_weight, st, dbg_ktok, dbg_offs, pre_val, pre_idx);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -153,9 +150,7 @@ __global__ void beam_reconstruct_kernel(BeamState st, long long* preds, int ld, 
 
 const char* beam_reconstruct_launch(cudaStream_t stream, BeamState st, long long* preds, int ld, int steps) {
     if (steps < 0 || steps > st.Lmax || ld < steps + 1) return "beam_reconstruct: bad steps / ld";
-    beam_reconstruct_kernel<<<(st.N + 127) / 128, 128, 0, stream>>>(st, preds, ld, steps);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<beam_reconstruct_kernel>((st.N + 127) / 128, 128, 0, stream, st, preds, ld, steps);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -206,9 +201,7 @@ __global__ void beam_finalize_kernel(BeamState st, float penalty, float lamda, i
 const char* beam_finalize_launch(cudaStream_t stream, BeamState st, float penalty, float lamda, int nbest,
                                  long long* out_preds, float* out_scores) {
     if (nbest < 1) return "beam_finalize: nbest < 1";
-    beam_finalize_kernel<<<st.N / st.beam, 32, 0, stream>>>(st, penalty, lamda, nbest, out_preds, out_scores);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<beam_finalize_kernel>(st.N / st.beam, 32, 0, stream, st, penalty, lamda, nbest, out_preds, out_scores);
 }
 
 // initial state (speech2text.py:54-58): preds = BOS, scores = [0, -inf, ...] per utterance, flags = 0
@@ -223,9 +216,7 @@ __global__ void beam_init_kernel(BeamState st) {
 
 const char* beam_init_launch(cudaStream_t stream, BeamState st) {
     int n = st.N < 4 ? 4 : st.N;
-    beam_init_kernel<<<(n + 127) / 128, 128, 0, stream>>>(st);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<beam_init_kernel>((n + 127) / 128, 128, 0, stream, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -243,8 +234,6 @@ __global__ void __launch_bounds__(TOPK_THREADS) logsoftmax_topk_kernel(const flo
                                                                        float lm_weight, int k, float* __restrict__ out_val,
                                                                        int* __restrict__ out_idx,
                                                                        float* __restrict__ out_logp, int ld_logp) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     extern __shared__ float srow[];   // [V]
     __shared__ float red[8];
     __shared__ float bc;
@@ -326,15 +315,8 @@ const char* logsoftmax_topk_launch(cudaStream_t stream, const float* logits, int
     if (k < 1 || k > KMAX) return "logsoftmax_topk: k must be in [1,16]";
     if (V < 1 || V > 48 * 1024) return "logsoftmax_topk: vocabulary too large for one CTA's shared memory";
     const size_t smem = (size_t)V * sizeof(float);
-    static bool attr_set = false;
-    if (!attr_set && smem > 40 * 1024) {
-        if (cudaFuncSetAttribute(logsoftmax_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
-            return "cudaFuncSetAttribute(logsoftmax_topk) failed";
-        attr_set = true;
-    }
-    cudaError_t e = launch_pdl(logsoftmax_topk_kernel, dim3(rows), dim3(TOPK_THREADS), smem, stream, logits, ldl, V, lm_logp, ld_lm,
-                               lm_weight, k, out_val, out_idx, out_logp, ld_logp);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<logsoftmax_topk_kernel>(dim3(rows), dim3(TOPK_THREADS), smem, stream, logits, ldl, V, lm_logp, ld_lm,
+                                          lm_weight, k, out_val, out_idx, out_logp, ld_logp);
 }
 
 }  // namespace otb

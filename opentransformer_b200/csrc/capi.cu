@@ -46,18 +46,9 @@ const char* otb_last_error(void) { return g_err; }
 int otb_version(void) { return OTB_VERSION; }
 int otb_num_sms(void) { return num_sms(); }
 
-/* debug / profiling aid: when buf != NULL every GEMM CTA writes 8 clock64 phase stamps to buf[cta*8 ..] */
-int otb_debug_gemm_timing(unsigned long long* buf) {
-    g_gemm_dbg = buf;
-    return 0;
-}
 int otb_set_tile_policy(int policy) {
     if (policy != 0 && policy != 1) return fail("otb_set_tile_policy", "policy must be 0 (latency) or 1 (throughput)");
     g_tile_policy = policy;
-    return 0;
-}
-int otb_debug_gemm_mode(int mode) {
-    g_gemm_dbg_mode = mode;
     return 0;
 }
 

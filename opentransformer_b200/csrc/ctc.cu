@@ -12,6 +12,7 @@
 // HBM-bound integer/float work: the [B T', V] log-prob matrix is read once by each kernel.
 #include <math.h>
 
+#include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
 
@@ -172,11 +173,13 @@ const char* ctc_launch(cudaStream_t st, const float* logp, int ldl, int B, int T
     if (max_tgt < 0 || 2 * max_tgt + 1 > CTC_SMAX) return "ctc: targets longer than 64 labels are not supported";
     if (blank < 0 || blank >= V) return "ctc: bad blank id";
     const int S_ws = 2 * max_tgt + 1;
-    ctc_alpha_beta_kernel<<<B, 160, 0, st>>>(logp, ldl, T, in_len, targets, ldt, tgt_len, blank, V, nll, ws, S_ws);
-    ctc_mean_kernel<<<1, 256, 0, st>>>(nll, tgt_len, B, loss);
-    if (dlogits) ctc_grad_kernel<<<B * T, 256, 0, st>>>(logp, ldl, T, V, in_len, targets, ldt, tgt_len, blank, nll, ws, S_ws, B, grad_scale, dlogits, ldd);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    const char* err;
+    if ((err = launch<ctc_alpha_beta_kernel>(B, 160, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len, blank, V, nll, ws, S_ws)))
+        return err;
+    if ((err = launch<ctc_mean_kernel>(1, 256, 0, st, nll, tgt_len, B, loss))) return err;
+    if (!dlogits) return nullptr;
+    return launch<ctc_grad_kernel>(B * T, 256, 0, st, logp, ldl, T, V, in_len, targets, ldt, tgt_len, blank, nll, ws, S_ws, B,
+                                   grad_scale, dlogits, ldd);
 }
 
 }  // namespace otb

@@ -39,6 +39,7 @@
 #include <cuda_fp16.h>
 
 #include "beam_common.cuh"
+#include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
 
@@ -1441,17 +1442,6 @@ size_t decode_group_workspace_bytes(int N, int n_layers, int Lmax, int B, int be
     return dg_workspace(nullptr, p, N, n_layers, Lmax, dg_groups(B, beam), V);
 }
 
-// launch configuration of one thread-block cluster of 16 CTAs per row group (non-portable cluster size)
-static cudaLaunchConfig_t dg_cluster_config(int G, cudaStream_t st, cudaLaunchAttribute* at) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(G * DG_P); cfg.blockDim = dim3(DG_THREADS); cfg.dynamicSmemBytes = DG_SMEM; cfg.stream = st;
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = DG_P; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cfg;
-}
-
 const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const bf16* kvx, const int* mem_len, bf16* kc,
                                 bf16* vc, const BeamState& bs, int B, int T, int max_steps, float* dbg_logp,
                                 float* dbg_scores, void* workspace, size_t workspace_bytes) {
@@ -1506,14 +1496,6 @@ const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const 
     p.dbg_logp = dbg_logp; p.dbg_scores = dbg_scores;
     p.dbg_clk = g_dg_dbg; p.dbg_step = g_dg_dbg_step;
 
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(decode_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM) != cudaSuccess) {
-            (void)cudaGetLastError();
-            return "cudaFuncSetAttribute(decode_persistent) failed";
-        }
-        attr_set = true;
-    }
     // Preferred launch: one thread-block CLUSTER of 16 CTAs per row group (a GPC holds about 16-18 SMs, so at most one such
     // cluster per GPC is co-resident): the group barrier becomes barrier.cluster (hardware, ~0.3 us, and the CTAs of a group
     // are co-scheduled by construction).  Whether the device grants that shape is probed once.  Without it, or with
@@ -1521,12 +1503,20 @@ const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const 
     // #SMs co-resident CTAs).  The software barrier spins: it is only safe when every CTA of every batch in flight (all
     // streams together) is resident at once, e.g. 2 batches of 32 utterances (96 CTAs) on a 132-SM H100.
     static const bool cluster_ok = [] {
-        if (cudaFuncSetAttribute(decode_group_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
+        // the question is about a DG_SMEM launch, so the kernel's shared-memory cap has to be raised before it is asked
+        if (prepare<decode_group_kernel>() ||
+            cudaFuncSetAttribute(decode_group_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
             (void)cudaGetLastError();
             return false;
         }
+        // one row group: a cluster of 16 CTAs (non-portable cluster size)
         cudaLaunchAttribute at[1];
-        const cudaLaunchConfig_t q = dg_cluster_config(1, nullptr, at);
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = DG_P; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        cudaLaunchConfig_t q;
+        memset(&q, 0, sizeof(q));
+        q.gridDim = dim3(DG_P); q.blockDim = dim3(DG_THREADS); q.dynamicSmemBytes = DG_SMEM;
+        q.attrs = at; q.numAttrs = 1;
         int nclus = 0;
         if (cudaOccupancyMaxActiveClusters(&nclus, decode_group_kernel, &q) != cudaSuccess || nclus < 1) {
             (void)cudaGetLastError();
@@ -1538,16 +1528,8 @@ const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const 
     // flight than can be resident at once, which only gang-scheduled clusters tolerate
     if (g_dg_barrier == 1 && !cluster_ok) return "decode_persistent: thread-block clusters of 16 are not available on this device";
     p.cluster = (cluster_ok && g_dg_barrier != 0) ? 1 : 0;
-    if (p.cluster) {
-        cudaLaunchAttribute at[1];
-        const cudaLaunchConfig_t cfg = dg_cluster_config(G, st, at);
-        e = cudaLaunchKernelEx(&cfg, decode_group_kernel, p);
-        if (e != cudaSuccess) (void)cudaGetLastError();
-        return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
-    }
-    decode_group_kernel<<<G * DG_P, DG_THREADS, DG_SMEM, st>>>(p);
-    e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return p.cluster ? launch<decode_group_kernel, DG_P>(G * DG_P, DG_THREADS, DG_SMEM, st, p)
+                     : launch<decode_group_kernel>(G * DG_P, DG_THREADS, DG_SMEM, st, p);
 }
 
 }  // namespace otb

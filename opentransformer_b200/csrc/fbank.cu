@@ -10,6 +10,7 @@
 // pre-emphasis, windowing and an in-place radix-2 FFT; the filterbank row of mel bin f covers fft bins [lo_f, hi_f) only.
 #include <math.h>
 
+#include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
 
@@ -130,17 +131,13 @@ const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const 
                          float preemph) {
     if (B < 1 || Tmax < 1 || F < 1) return "fbank: empty problem";
     if (frame_len < 2 || frame_len > FB_NFFT || frame_shift < 1) return "fbank: frame length must be <= 512 samples (25 ms at <= 20 kHz)";
-    fbank_kernel<<<dim3(Tmax, B), 256, 0, st>>>(wave, ld_wave, n_samples, window, bank, bank_range, out, Tmax, F, frame_len, frame_shift,
-                                                preemph, 1.1920928955078125e-07f);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<fbank_kernel>(dim3(Tmax, B), 256, 0, st, wave, ld_wave, n_samples, window, bank, bank_range, out, Tmax, F,
+                                frame_len, frame_shift, preemph, 1.1920928955078125e-07f);
 }
 const char* utt_cmvn_launch(cudaStream_t st, float* x, int B, int Tmax, int F, const int* n_frames, const float* gmean, const float* gstd) {
     if (B < 1 || Tmax < 1 || F < 1) return "cmvn: empty problem";
     if ((gmean == nullptr) != (gstd == nullptr)) return "cmvn: global mean / std must both be given";
-    utt_cmvn_kernel<<<B, 512, 0, st>>>(x, Tmax, F, n_frames, gmean, gstd);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<utt_cmvn_kernel>(B, 512, 0, st, x, Tmax, F, n_frames, gmean, gstd);
 }
 
 }  // namespace otb

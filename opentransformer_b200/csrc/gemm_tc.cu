@@ -31,13 +31,6 @@
 namespace otb {
 
 int g_tile_policy = 0;   // otb_set_tile_policy: 0 = lowest latency of a lone launch, 1 = least SM-time (concurrent batches)
-unsigned long long* g_gemm_dbg = nullptr;
-int g_gemm_dbg_mode = 0;
-// debug buffer layout (otb_debug_gemm_timing): [256 CTAs][8] phase stamps, then per-k-block traces of the first tile
-static constexpr int DBG_CTAS = 256;
-#define DBG_STAMP(i) do { if (p.dbg) p.dbg[blockIdx.x * 8 + (i)] = clock64(); } while (0)
-// per-k-block traces of the first tile: kind 0 = TMA issue, 1 = full barrier observed by the consumers
-#define DBG_KB(kind, kb) do { if (p.dbg && (kb) < 64) p.dbg[DBG_CTAS * 8 + (blockIdx.x * 2 + (kind)) * 64 + (kb)] = clock64(); } while (0)
 
 static constexpr int BM = 128;
 static constexpr int BK = 64;
@@ -100,8 +93,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    PDL_TRIGGER();   // the next kernel of the stream may be scheduled; it waits (griddepcontrol.wait) for this grid to finish
-    if (threadIdx.x == 0) DBG_STAMP(0);
 
     const int m_tiles = p.conv ? (p.conv_B * p.conv_T1h + p.conv_R - 1) / p.conv_R : (p.M + BM - 1) / BM;
     const int n_tiles = (p.N + BN_OUT - 1) / BN_OUT;
@@ -125,10 +116,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * 8192, &tmA, &full_bar[stage], m_blk * BM + j * 64, kb * BK);
 #pragma unroll
             for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &tmB, &full_bar[stage], n_blk * BN + j * 64, kb * BK);
-            return;
-        }
-        if (p.dbg_mode == 1) {  // profiling aid: signal "full" without moving any data
-            mbar_arrive(&full_bar[stage]);
             return;
         }
         mbar_arrive_expect_tx(&full_bar[stage], a_tx + (uint32_t)Cfg::B_BYTES);
@@ -160,21 +147,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         fence_barrier_init();
     }
     __syncthreads();
-    PDL_WAIT();   // predecessor grid complete: its outputs (our A operand, residual) may now be read
-    if (threadIdx.x == 0) DBG_STAMP(1);
 
     if (warp == 4 * Cfg::NWG) {
         // ------------------------------------------------------------------ TMA producer (lane 0)
         if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            bool first = true;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 for (int kb = kb_begin(tile), kb1 = kb_end(tile); kb < kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     issue_load(tile, kb, stage);
-                    if (first) { DBG_STAMP(2); first = false; }
-                    if (tile == (int)blockIdx.x) DBG_KB(0, kb);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -268,24 +250,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         int prev = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase);
-            if (it == 0 && et == 0) DBG_KB(1, kb);
-            if (it == 0 && kb == kb0 && et == 0) DBG_STAMP(3);
             const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
             const uint32_t b_addr = a_addr + Cfg::A_BYTES;
-            if (p.dbg_mode != 2) {
-                wgmma_fence();
+            wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    if (TN)   // MN-major operands: one k16 step = 16 rows of 128 B; this warpgroup's 64 M columns = A block cw
-                        mma_bn<BN, 1>(acc, gmma_desc_sw128(a_addr + cw * 8192 + k * 2048, 1024, 8192),
-                                      gmma_desc_sw128(b_addr + k * 2048, 1024, 8192), (uint32_t)(((kb - kb0) | k) != 0));
-                    else
-                        mma_bn<BN, 0>(acc, gmma_desc_sw128(a_addr + cw * 8192 + k * 32), gmma_desc_sw128(b_addr + k * 32),
-                                      (uint32_t)(((kb - kb0) | k) != 0));
-                }
-                wgmma_commit();
-                wgmma_wait<1>();
+            for (int k = 0; k < BK / 16; ++k) {
+                if (TN)   // MN-major operands: one k16 step = 16 rows of 128 B; this warpgroup's 64 M columns = A block cw
+                    mma_bn<BN, 1>(acc, gmma_desc_sw128(a_addr + cw * 8192 + k * 2048, 1024, 8192),
+                                  gmma_desc_sw128(b_addr + k * 2048, 1024, 8192), (uint32_t)(((kb - kb0) | k) != 0));
+                else
+                    mma_bn<BN, 0>(acc, gmma_desc_sw128(a_addr + cw * 8192 + k * 32), gmma_desc_sw128(b_addr + k * 32),
+                                  (uint32_t)(((kb - kb0) | k) != 0));
             }
+            wgmma_commit();
+            wgmma_wait<1>();
             if (prev >= 0 && (et & 127) == 0) mbar_arrive(&empty_bar[prev]);   // the k-block before this one has been read
             prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -293,9 +271,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
         if (prev >= 0 && (et & 127) == 0) mbar_arrive(&empty_bar[prev]);
-        if (it == 0 && et == 0) DBG_STAMP(4);
         epi_bar<kEpiThreads>();   // bias, row map and residual tile of this tile are in shared memory
-        if (it == 0 && et == 0) DBG_STAMP(5);
 
         // ---- (c) fused epilogue on the accumulator fragment: rows rl0 + 8 hh, columns 8 jj + cq + {0, 1}
         int out_row[2];
@@ -470,9 +446,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
         }
         epi_bar<kEpiThreads>();  // staging / bias smem may be rewritten for the next tile
-        if (it == 0 && et == 0) DBG_STAMP(6);
     }
-    if (et == 0) DBG_STAMP(7);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -553,20 +527,12 @@ int num_sms() {
     return n;
 }
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool TN = false>
 static const char* launch_inst(cudaStream_t st, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
                                int num_tiles) {
     using Cfg = GemmCfg<BN>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 Cfg::SMEM_BYTES) != cudaSuccess)
-            return "cudaFuncSetAttribute(max dynamic smem) failed";
-        attr_set = true;
-    }
     const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-    cudaError_t e = launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, ta, tb, p);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<gemm_tc_kernel<BN, EPI, TN>>(dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, ta, tb, p);
 }
 
 template <int BN>
@@ -630,8 +596,6 @@ const char* gemm_tile(int m_tiles, int N, int epi, int out_f32, int* bn) {
 const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, int ldw, int w_rows, int epi,
                         GemmParams p, const CUtensorMap* conv_map) {
     if (p.M <= 0 || p.N <= 0 || p.K <= 0) return "gemm: empty problem";
-    p.dbg = g_gemm_dbg;
-    p.dbg_mode = g_gemm_dbg_mode;
     if (p.K % 8) return "gemm: K must be a multiple of 8";
     if (p.ldc % (p.out_f32 ? 4 : 8)) return "gemm: ldc must keep rows 16-byte aligned (ldc % 8 == 0 for bf16, % 4 for f32)";
     if (reinterpret_cast<uintptr_t>(p.out) & 15) return "gemm: out must be 16-byte aligned";
@@ -676,7 +640,6 @@ const char* gemm_wgrad_launch(cudaStream_t st, const void* dY, int lddy, const v
     memset(&p, 0, sizeof(p));
     p.M = Nw; p.N = Kw; p.K = Mact;
     p.out = out; p.ldc = ldc; p.out_f32 = 1; p.alpha = 1.f;
-    p.dbg = nullptr; p.dbg_mode = 0;
     const int bn = (Kw > 64) ? 128 : 64;
     const int m_tiles = (Nw + BM - 1) / BM, n_tiles = (Kw + bn - 1) / bn;
     const int num_kb = (Mact + BK - 1) / BK;
@@ -694,28 +657,8 @@ const char* gemm_wgrad_launch(cudaStream_t st, const void* dY, int lddy, const v
     if ((err = encode_tmap_2d(&ta, dY, (uint64_t)Nw, (uint64_t)Mact, (uint64_t)lddy, 64, 64))) return err;
     if ((err = encode_tmap_2d(&tb, X, (uint64_t)Kw, (uint64_t)Mact, (uint64_t)ldx, 64, 64))) return err;
     const int num_tiles = m_tiles * n_tiles * splitk;
-    const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-    cudaError_t e;
-    if (bn == 128) {
-        using Cfg = GemmCfg<128>;
-        static bool attr = false;
-        if (!attr) {
-            if (cudaFuncSetAttribute(gemm_tc_kernel<128, EPI_BIAS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess)
-                return "cudaFuncSetAttribute(wgrad) failed";
-            attr = true;
-        }
-        e = launch_pdl(gemm_tc_kernel<128, EPI_BIAS, true>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, ta, tb, p);
-    } else {
-        using Cfg = GemmCfg<64>;
-        static bool attr = false;
-        if (!attr) {
-            if (cudaFuncSetAttribute(gemm_tc_kernel<64, EPI_BIAS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess)
-                return "cudaFuncSetAttribute(wgrad) failed";
-            attr = true;
-        }
-        e = launch_pdl(gemm_tc_kernel<64, EPI_BIAS, true>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, ta, tb, p);
-    }
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return bn == 128 ? launch_inst<128, EPI_BIAS, true>(st, ta, tb, p, num_tiles)
+                     : launch_inst<64, EPI_BIAS, true>(st, ta, tb, p, num_tiles);
 }
 
 }  // namespace otb

@@ -7,6 +7,7 @@
 // (loss.py:31,46) and the mean is taken over the non-PAD tokens (:44-46).
 #include <math.h>
 
+#include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
 
@@ -95,11 +96,12 @@ __global__ void __launch_bounds__(256) ls_mean_kernel(const float* __restrict__ 
 const char* ls_ce_launch(cudaStream_t st, const float* logits, int ldl, const long long* tgt, int rows, int V, float eps,
                          int pad_id, float* tok_loss, float* loss, int* n_valid, float* dlogits, int ldd, bf16* dlogits_bf16) {
     if (rows < 1 || V < 2) return "ls_ce: empty problem";
-    ls_count_kernel<<<1, 256, 0, st>>>(tgt, rows, pad_id, n_valid);
-    ls_ce_kernel<<<rows, 256, 0, st>>>(logits, ldl, tgt, V, eps, pad_id, tok_loss, dlogits_bf16 ? nullptr : dlogits, ldd, n_valid, dlogits_bf16);
-    ls_mean_kernel<<<1, 256, 0, st>>>(tok_loss, rows, n_valid, loss);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    const char* err;
+    if ((err = launch<ls_count_kernel>(1, 256, 0, st, tgt, rows, pad_id, n_valid))) return err;
+    if ((err = launch<ls_ce_kernel>(rows, 256, 0, st, logits, ldl, tgt, V, eps, pad_id, tok_loss, dlogits_bf16 ? nullptr : dlogits,
+                                    ldd, n_valid, dlogits_bf16)))
+        return err;
+    return launch<ls_mean_kernel>(1, 256, 0, st, tok_loss, rows, n_valid, loss);
 }
 
 }  // namespace otb

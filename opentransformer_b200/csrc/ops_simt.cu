@@ -25,8 +25,6 @@ __global__ void __launch_bounds__(256) conv1_relu_nhwc_kernel(const float* __res
                                                               const float* __restrict__ bias, bf16* __restrict__ out,
                                                               int B, int T, int F, int T1, int F1, int T1pad,
                                                               int F1pad, int C1) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     extern __shared__ float sx[];  // [2*CONV1_ROWS + 1][F + 2]  (one zero column each side)
     const int chunks = (T1 + CONV1_ROWS - 1) / CONV1_ROWS;
     const int b = blockIdx.x / chunks, t1_0 = (blockIdx.x % chunks) * CONV1_ROWS;
@@ -85,9 +83,8 @@ const char* conv1_launch(cudaStream_t st, const float* x, const float* w, const 
     size_t smem = (size_t)(2 * CONV1_ROWS + 1) * (F + 2) * sizeof(float);
     if (smem > 48 * 1024) return "conv1: F too large";
     const int chunks = (T1 + CONV1_ROWS - 1) / CONV1_ROWS;
-    cudaError_t e = launch_pdl(conv1_relu_nhwc_kernel, dim3(B * chunks), dim3(256), smem, st, x, w, bias, out, B, T, F, T1, F1, T1pad,
-                               F1pad, C1);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<conv1_relu_nhwc_kernel>(dim3(B * chunks), dim3(256), smem, st, x, w, bias, out, B, T, F, T1, F1, T1pad,
+                                          F1pad, C1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -100,8 +97,6 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const bf16* __restrict__
                                                         int ldo, int out_f32, const float* __restrict__ g1,
                                                         const float* __restrict__ b1, const float* __restrict__ g2,
                                                         const float* __restrict__ b2, float eps, int M, int N) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= M) return;
@@ -178,8 +173,6 @@ __global__ void __launch_bounds__(256) layernorm256_kernel(const bf16* __restric
                                                            int ldo, int out_f32, const float* __restrict__ g1,
                                                            const float* __restrict__ b1, const float* __restrict__ g2,
                                                            const float* __restrict__ b2, float eps, int M, int N) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     constexpr int R = 4;
     const int lane = threadIdx.x & 31;
     const int row0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * R;
@@ -257,21 +250,18 @@ const char* layernorm_launch(cudaStream_t st, const bf16* x, int ldx, void* out,
     if ((out_f32 && ldo % 4) || (!out_f32 && ldo % 8)) return "layernorm: bad output stride";
     if (N <= 256) {
         const int rows_per_block = 8 * 4;
-        cudaError_t e = launch_pdl(layernorm256_kernel, dim3((M + rows_per_block - 1) / rows_per_block), dim3(256), 0, st, x, ldx, out,
-                                   ldo, out_f32, g1, b1, g2, b2, eps, M, N);
-        return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+        return launch<layernorm256_kernel>(dim3((M + rows_per_block - 1) / rows_per_block), dim3(256), 0, st, x, ldx, out, ldo,
+                                           out_f32, g1, b1, g2, b2, eps, M, N);
     }
     const int rows_per_block = 8;
     dim3 grid((M + rows_per_block - 1) / rows_per_block);
     const int ch = (N + 255) / 256;
-    cudaError_t e;
     switch (ch) {
-        case 1: e = launch_pdl(layernorm_kernel<1>, grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N); break;
-        case 2: e = launch_pdl(layernorm_kernel<2>, grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N); break;
-        case 3: e = launch_pdl(layernorm_kernel<3>, grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N); break;
-        default: e = launch_pdl(layernorm_kernel<4>, grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N); break;
+        case 1: return launch<layernorm_kernel<1>>(grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N);
+        case 2: return launch<layernorm_kernel<2>>(grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N);
+        case 3: return launch<layernorm_kernel<3>>(grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N);
+        default: return launch<layernorm_kernel<4>>(grid, dim3(256), 0, st, x, ldx, out, ldo, out_f32, g1, b1, g2, b2, eps, M, N);
     }
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -289,9 +279,7 @@ __global__ void sinusoid_table_kernel(float* __restrict__ out, int n_pos, int d,
 
 const char* sinusoid_table_launch(cudaStream_t st, float* out, int n_pos, int d, int first_pos) {
     const int n = n_pos * d;
-    sinusoid_table_kernel<<<(n + 255) / 256, 256, 0, st>>>(out, n_pos, d, first_pos);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<sinusoid_table_kernel>((n + 255) / 256, 256, 0, st, out, n_pos, d, first_pos);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -302,8 +290,6 @@ const char* sinusoid_table_launch(cudaStream_t st, float* out, int n_pos, int d,
 __global__ void embed_posenc_kernel(const long long* __restrict__ tok, int tok_stride, const bf16* __restrict__ emb,
                                     const float* __restrict__ table, bf16* __restrict__ out, int N, int d, int period,
                                     const int* __restrict__ step_ptr, float xscale, int vocab) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (n >= N) return;
@@ -330,9 +316,8 @@ const char* embed_posenc_launch(cudaStream_t st, const long long* tok, int tok_s
                                 const float* table, bf16* out, int N, int d, int period, const int* step_ptr,
                                 int vocab) {
     if (d % 8) return "embed: d must be a multiple of 8";
-    cudaError_t e = launch_pdl(embed_posenc_kernel, dim3((N + 7) / 8), dim3(256), 0, st, tok, tok_stride, emb, table, out, N, d, period,
-                               step_ptr, sqrtf((float)d), vocab);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<embed_posenc_kernel>(dim3((N + 7) / 8), dim3(256), 0, st, tok, tok_stride, emb, table, out, N, d, period,
+                                       step_ptr, sqrtf((float)d), vocab);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -340,8 +325,6 @@ const char* embed_posenc_launch(cudaStream_t st, const long long* tok, int tok_s
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) log_softmax_kernel(const float* __restrict__ x, int ldx, float* __restrict__ out,
                                                           int ldo, int V) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     __shared__ float red[8];
     __shared__ float bc;
     const float* xr = x + (size_t)blockIdx.x * ldx;
@@ -376,8 +359,7 @@ __global__ void __launch_bounds__(256) log_softmax_kernel(const float* __restric
 }
 
 const char* log_softmax_launch(cudaStream_t st, const float* x, int ldx, float* out, int ldo, int rows, int V) {
-    cudaError_t e = launch_pdl(log_softmax_kernel, dim3(rows), dim3(256), 0, st, x, ldx, out, ldo, V);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<log_softmax_kernel>(dim3(rows), dim3(256), 0, st, x, ldx, out, ldo, V);
 }
 
 // Chunk c of a staged K/V row goes to position rot_chunk(c + s) in row s (bank-conflict-free rows); i >= 0.
@@ -402,8 +384,6 @@ __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel
                                                                bf16* __restrict__ vc, const int* __restrict__ anc,
                                                                const int* __restrict__ step_ptr, bf16* __restrict__ out,
                                                                int N, int H, int Lmax, float scale, int keys_pad) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     // Lanes run over KEYS: each lane owns up to KPL cached positions, resolves their slots through the
     // ancestry table and pulls the whole K and V rows (DK * 2 bytes) with 16-byte loads -- all loads of a lane are
     // independent, so the kernel costs ~3 dependent memory round trips (anc -> K/V -> out) instead of a
@@ -551,16 +531,8 @@ static const char* decode_self_attn_launch_dk(cudaStream_t st, const bf16* qkv, 
     // shared memory per CTA and doubles the resident CTAs of this latency-bound kernel (less SM-time per decode step)
     const int keys_pad = (Lmax + 31) / 32 * 32;
     const size_t smem = (size_t)warps * keys_pad * DK * 2 + (size_t)warps * DK * sizeof(float);   // V rows | q per warp
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(decode_self_attn_kernel<DK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (DK == 64 ? 80 : 100) * 1024) !=
-            cudaSuccess)
-            return "cudaFuncSetAttribute(decode_self_attn) failed";
-        attr_set = true;
-    }
-    cudaError_t e = launch_pdl(decode_self_attn_kernel<DK>, dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H,
-                               Lmax, DK == 64 ? 0.125f : 1.0f / sqrtf((float)DK), keys_pad);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<decode_self_attn_kernel<DK>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax,
+                                               DK == 64 ? 0.125f : 1.0f / sqrtf((float)DK), keys_pad);
 }
 
 const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
@@ -578,8 +550,6 @@ const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, 
 // ------------------------------------------------------------------------------------------------
 __global__ void scale_add_table_kernel(const void* __restrict__ x, int ldx, int x_f32, bf16* __restrict__ out, int ldo,
                                        float alpha, const float* __restrict__ table, int period, int M, int N) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int row = (int)(i / N), col = (int)(i % N);
     if (row >= M) return;
@@ -592,9 +562,8 @@ __global__ void scale_add_table_kernel(const void* __restrict__ x, int ldx, int 
 const char* scale_add_table_launch(cudaStream_t st, const void* x, int ldx, int x_f32, bf16* out, int ldo, float alpha,
                                    const float* table, int period, int M, int N) {
     const size_t n = (size_t)M * N;
-    cudaError_t e = launch_pdl(scale_add_table_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, x, ldx, x_f32, out, ldo, alpha,
-                               table, period, M, N);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<scale_add_table_kernel>(dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, x, ldx, x_f32, out, ldo, alpha,
+                                          table, period, M, N);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -606,8 +575,6 @@ const char* scale_add_table_launch(cudaStream_t st, const void* x, int ldx, int 
 __global__ void __launch_bounds__(256) dwconv_swish_kernel(const bf16* __restrict__ x, const float* __restrict__ w,
                                                            const float* __restrict__ b, bf16* __restrict__ out, int B,
                                                            int T, int d, int k) {
-    PDL_TRIGGER();
-    PDL_WAIT();
     const int cg = d / 8;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)B * T * cg) return;
@@ -644,8 +611,7 @@ const char* dwconv_swish_launch(cudaStream_t st, const bf16* x, const float* w, 
                                 int d, int k) {
     if (d % 8 || !(k & 1)) return "dwconv: d must be a multiple of 8 and k odd";
     const size_t n = (size_t)B * T * (d / 8);
-    cudaError_t e = launch_pdl(dwconv_swish_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, x, w, b, out, B, T, d, k);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return launch<dwconv_swish_kernel>(dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, x, w, b, out, B, T, d, k);
 }
 
 }  // namespace otb

@@ -55,8 +55,6 @@ struct GemmParams {
     const unsigned* drop_seed;    // device scalar, null = no dropout
     unsigned drop_site, drop_thresh;
     float drop_scale;
-    unsigned long long* dbg;  // optional [grid][8] clock64 phase stamps (otb_debug_gemm_timing)
-    int dbg_mode;             // 0 normal; 1 = no TMA traffic (MMA-only cadence); 2 = no MMA (TMA-only cadence)
 };
 
 const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, int ldw, int w_rows, int epi,
@@ -191,8 +189,6 @@ const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const 
 const char* utt_cmvn_launch(cudaStream_t st, float* x, int B, int Tmax, int F, const int* n_frames, const float* gmean, const float* gstd);
 
 int num_sms();
-extern unsigned long long* g_gemm_dbg;
-extern int g_gemm_dbg_mode;
 extern int g_tile_policy;
 void set_error(const char* msg);
 

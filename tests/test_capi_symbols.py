@@ -119,14 +119,28 @@ def test_ctypes_structs_match_the_header():
     assert _lib.MEGA_MAX_LAYERS == int(defines['OTB_MEGA_MAX_LAYERS'])
 
 
-def test_version_2_and_error_reporting(libpath):
+def test_version_3_and_error_reporting(libpath):
     from opentransformer_b200 import _lib
     lib = _lib.lib()
-    assert lib.otb_version() == 2
+    assert lib.otb_version() == 3
     t1 = ctypes.c_int()
     assert lib.otb_conv_geometry(1000, 80, t1, None, None, None) == 0 and t1.value == 499
     assert lib.otb_conv_geometry(3, 80, None, None, None, None) != 0       # too short -> status, not abort
     assert b'otb_conv_geometry' in lib.otb_last_error()
+
+
+def test_every_kernel_launches_through_one_helper():
+    """Kernels are launched, and their shared-memory cap raised, only inside csrc/launch.cuh, so every kernel gets the same
+    carve-out, cap and error handling.  No environment switch and no programmatic dependent launch anywhere."""
+    csrc = os.path.join(ROOT, 'opentransformer_b200', 'csrc')
+    bad = []
+    for name in sorted(os.listdir(csrc)):
+        text = open(os.path.join(csrc, name)).read()
+        words = ['getenv', 'griddepcontrol', 'PDL_']
+        if name != 'launch.cuh':
+            words += ['<<<', 'cudaLaunchKernelEx', 'cudaFuncAttributeMaxDynamicSharedMemorySize']
+        bad += [f'{name}: {w}' for w in words if w in text]
+    assert not bad, 'outside the single launch path:\n' + '\n'.join(bad)
 
 
 def test_conv_geometry_matches_reference_formula(libpath):
