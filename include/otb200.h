@@ -241,6 +241,35 @@ int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk
                       const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
                       int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
                       int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, void* stream);
+/* otb_attention_bwd for rel-pos attention: the forward was otb_attention with the band bd f32 [H, B*Tq, ldbd] (Tq == Tk, not
+ * causal, d_k = 64).  The band is added to the recomputed scores, and its gradient dS (the gradient of the raw score sum, which
+ * includes 1/sqrt(d_k)) is written to dbd bf16 [H, B*Tq, lddbd] at column j - i + Tq - 1 (lddbd: 2 Tq - 1 rounded up to 8).
+ * The caller zeroes dbd: entries without a visible key are not written. */
+int otb_attention_bwd_bd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
+                         const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
+                         int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
+                         int Tq, int Tk, const int* kv_len, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd,
+                         void* dbd, int lddbd, void* stream);
+/* Residual dropout without a GEMM in front: out = resid + alpha * keep(seed, site, row, col) / (1 - p) * x, with the mask of
+ * otb_linear_dropout_resid / otb_dropout_bwd.  resid may be NULL (out = alpha * dropout_p(x): also the backward of such a
+ * site).  row_len (optional, i32 [M / row_period]): rows with row % row_period >= row_len[row / row_period] read x as zero.
+ * seed may be NULL when p = 0.  bf16 [M, N], N and the row pitches multiples of 8. */
+int otb_dropout_add(const void* x, int ldx, const void* resid, int ldr, void* out, int ldo, int M, int N, float alpha, float p,
+                    const uint32_t* seed, uint32_t site, const int32_t* row_len, int row_period, void* stream);
+/* Conformer convolution module, middle part, in training mode (module/conformer.py:46-52): x bf16 [B*T, d] = GLU output, read as
+ * zero on padded frames (t >= len[b]); c f32 [B*T, d] = depthwise_conv(x) + wb (w f32 [d, k] as nn.Conv1d stores it, k odd,
+ * wb may be NULL); BatchNorm with batch statistics over all B*T rows -> stats f32 [2, d] = (mean, 1/sqrt(biased var + eps));
+ * running_mean / running_var (optional) updated with `momentum` and the unbiased variance, *num_batches (optional) += 1;
+ * out bf16 [B*T, d] = swish(BN(c)), zero on padded frames. */
+int otb_conformer_conv_train(const void* x, const int32_t* len, const float* w, const float* wb, const float* gamma, const float* beta,
+                             float* running_mean, float* running_var, int64_t* num_batches, float momentum, float eps, float* c,
+                             float* stats, void* out, int B, int T, int d, int k, void* stream);
+/* Its backward: dy bf16 [B*T, d] (gradient of out), x / c / stats as the forward left them; red f32 [2, d] and dc f32 [B*T, d]
+ * are scratch.  dx bf16 [B*T, d] (zero on padded frames); dw f32 [d, k], dwb f32 [d] (NULL without conv bias), dgamma, dbeta
+ * f32 [d]: overwritten, or added to with accumulate != 0. */
+int otb_conformer_conv_bwd(const void* dy, const void* x, const int32_t* len, const float* w, const float* gamma, const float* beta,
+                           const float* c, const float* stats, float* red, float* dc, void* dx, float* dw, float* dwb, float* dgamma,
+                           float* dbeta, int accumulate, int B, int T, int d, int k, void* stream);
 /* nn.Linear weight gradient dW[N,K] (fp32) = dy[M,N]^T x[M,K] (bf16), wgmma with MN-major operands + split-K.
  * (The input gradient dx = dy W is otb_linear with the transposed weight.)  accumulate != 0: dW += ... (gradient
  * accumulation straight into the optimizer's flat gradient buffer, the way autograd accumulates into .grad). */

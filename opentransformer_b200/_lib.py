@@ -70,6 +70,14 @@ _SIGS = {
     'otb_beam_finalize': (c_int, [POINTER(BeamStateC), c_float, c_float, c_int, _P, _P, _P]),
     'otb_attention_bwd': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_int, c_int,
                                   _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P]),
+    'otb_attention_bwd_bd': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_int, c_int,
+                                     _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P, c_int,
+                                     _P, c_int, _P]),
+    'otb_dropout_add': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_float, c_float, _P, ctypes.c_uint32, _P, c_int, _P]),
+    'otb_conformer_conv_train': (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_float, c_float, _P, _P, _P, c_int, c_int, c_int, c_int,
+                                         _P]),
+    'otb_conformer_conv_bwd': (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int,
+                                       _P]),
     'otb_linear_wgrad': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_colsum': (c_int, [_P, c_int, _P, c_int, c_int, c_int, _P]),
     'otb_layernorm_bwd': (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, _P, _P, c_float, c_int, c_int, c_int, _P]),

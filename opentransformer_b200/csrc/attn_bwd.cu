@@ -14,6 +14,11 @@
 // warpgroup with operands staged by TMA (K-major tiles; the [rows x 64] tile that is contracted over its rows is read as
 // an MN-major B operand, exactly like V in the forward); dS / P^T tiles are written by the threads as bf16 in the
 // canonical 128B-swizzled layout.  Score tiles are formed in two 64-column halves to bound the register footprint.
+//
+// HAS_BD (rel-pos attention, attention.py:196-253): the forward added the band BD[h, b, i, j - i + Tq - 1] (fp32, Tq == Tk) to
+// the raw scores; both kernels add it to the recomputed scores the same way.  The dQ kernel also writes dS, the gradient of
+// the raw score sum (it includes 1/sqrt(d_k)), into the bf16 band gradient dBD at the same place.  Each (i, j) belongs to one
+// CTA, so no atomics: entries without a visible key are left as the caller zeroed them.
 #include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
@@ -43,6 +48,7 @@ __device__ __forceinline__ void store_rows64(const float (&acc)[32], bf16* base,
 }
 
 // ------------------------------------------------------------------------------------------------ dQ
+template <bool HAS_BD>
 __global__ void __launch_bounds__(256, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const AttnBwdParams p) {
@@ -110,6 +116,17 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         Lr[hh] = sL[rl0 + 8 * hh];
         Dr[hh] = sD[rl0 + 8 * hh];
     }
+    const float* bd_row[2] = {nullptr, nullptr};   // row i of the band, shifted so that key j is element j
+    bf16* dbd_row[2] = {nullptr, nullptr};
+    if constexpr (HAS_BD) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            const int qc = min(q0 + rl0 + 8 * hh, p.Tq - 1);
+            const size_t row = ((size_t)h * p.B + b) * p.Tq + qc;
+            bd_row[hh] = p.bd + row * p.ldbd + (p.Tq - 1 - qc);
+            dbd_row[hh] = p.dbd + row * p.lddbd + (p.Tq - 1 - qc);
+        }
+    }
     const uint32_t qa = smem_u32(sQ) + wg * 8192, da = smem_u32(sdO) + wg * 8192, ka = smem_u32(sK), va = smem_u32(sV);
     const uint32_t sa = smem_u32(sdS) + wg * 8192;
     const float scale = 0.125f;
@@ -145,9 +162,16 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                     for (int e = 0; e < 2; ++e) {
                         const int i = 4 * jj + 2 * hh + e;
                         const int key = key0 + kh * 64 + jj * 8 + cq + e;
-                        const float pv = ex2_approx(fmaf(sc[i], p.scale_log2, -Lr[hh]));
+                        float s = sc[i];
+                        if constexpr (HAS_BD) {
+                            if (q_ok[hh] && key < lim[hh]) s += bd_row[hh][key];
+                        }
+                        const float pv = ex2_approx(fmaf(s, p.scale_log2, -Lr[hh]));
                         const float v = pv * (dp[i] - Dr[hh]) * scale;
                         ds[e] = (q_ok[hh] && key < lim[hh]) ? v : 0.f;
+                        if constexpr (HAS_BD) {
+                            if (q_ok[hh] && key < lim[hh]) dbd_row[hh][key] = __float2bfloat16_rn(v);
+                        }
                     }
                     put_pair(sdS, rl0 + 8 * hh, kh * 64 + jj * 8 + cq, ds[0], ds[1]);
                 }
@@ -173,6 +197,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 }
 
 // ------------------------------------------------------------------------------------------------ dK, dV
+template <bool HAS_BD>
 __global__ void __launch_bounds__(256, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const AttnBwdParams p) {
@@ -266,7 +291,11 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
                             const int c = qh * 64 + jj * 8 + cq + e;
                             const int qi = i0 + c;
                             const bool vis = k_ok[hh] && qi < p.Tq && (!p.causal || kj[hh] <= qi);
-                            const float pv = ex2_approx(fmaf(st[i], p.scale_log2, -sL[c]));
+                            float s = st[i];
+                            if constexpr (HAS_BD) {
+                                if (vis) s += p.bd[(((size_t)h * p.B + b) * p.Tq + qi) * p.ldbd + (kj[hh] - qi + p.Tq - 1)];
+                            }
+                            const float pv = ex2_approx(fmaf(s, p.scale_log2, -sL[c]));
                             const float dvv = pv * (dpt[i] - sD[c]) * scale;
                             pt[e] = vis ? pv : 0.f;
                             ds[e] = vis ? dvv : 0.f;
@@ -323,9 +352,13 @@ const char* attn_bwd_launch(cudaStream_t st, const void* q, int ldq, int q_rows,
     if ((err = encode_tmap_2d(&tk, k, (uint64_t)ldk, (uint64_t)k_rows, (uint64_t)ldk, 64, 128))) return err;
     if ((err = encode_tmap_2d(&tv, v, (uint64_t)ldv, (uint64_t)k_rows, (uint64_t)ldv, 64, 128))) return err;
     if ((err = encode_tmap_2d(&tdo, p.dout, (uint64_t)p.lddo, (uint64_t)q_rows, (uint64_t)p.lddo, 64, 128))) return err;
-    if ((err = launch<attn_bwd_dq_kernel>(dim3((p.Tq + 127) / 128, p.H, p.B), 256, ABW_SMEM_DQ, st, tq, tk, tv, tdo, p)))
-        return err;
-    return launch<attn_bwd_dkv_kernel>(dim3((p.Tk + 127) / 128, p.H, p.B), 256, ABW_SMEM_DKV, st, tq, tk, tv, tdo, p);
+    const dim3 gq((p.Tq + 127) / 128, p.H, p.B), gk((p.Tk + 127) / 128, p.H, p.B);
+    if (p.bd) {
+        if ((err = launch<attn_bwd_dq_kernel<true>>(gq, 256, ABW_SMEM_DQ, st, tq, tk, tv, tdo, p))) return err;
+        return launch<attn_bwd_dkv_kernel<true>>(gk, 256, ABW_SMEM_DKV, st, tq, tk, tv, tdo, p);
+    }
+    if ((err = launch<attn_bwd_dq_kernel<false>>(gq, 256, ABW_SMEM_DQ, st, tq, tk, tv, tdo, p))) return err;
+    return launch<attn_bwd_dkv_kernel<false>>(gk, 256, ABW_SMEM_DKV, st, tq, tk, tv, tdo, p);
 }
 
 }  // namespace otb

@@ -224,6 +224,42 @@ const char* dropout_bwd_launch(cudaStream_t st, const bf16* dy, int lddy, bf16* 
                                       drop_threshold(p), 1.0f / (1.0f - p), seed, site);
 }
 
+// out = resid + alpha * dropout_p(rowmask(x)) without a GEMM in front (rel-pos attention has no output projection; the
+// Conformer's conv module masks its output before the dropout, module/conformer.py:55).  Same keep(seed, site, row, col) as
+// the GEMM epilogue and dropout_bwd_kernel.  resid null: out = alpha * dropout_p(rowmask(x)), which is also the backward of
+// such a site (the mask and scale are the forward's); p = 0 without row_len: a plain sum.  Rows with
+// row % row_period >= row_len[row / row_period] read x as zero.  Thread = 8 columns of one row.
+__global__ void __launch_bounds__(256) dropout_add_kernel(const bf16* __restrict__ x, int ldx, const bf16* __restrict__ resid, int ldr,
+                                                          bf16* __restrict__ out, int ldo, int M, int N, float alpha, unsigned thresh,
+                                                          float scale, const unsigned* __restrict__ seed_ptr, unsigned site,
+                                                          const int* __restrict__ row_len, int row_period) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int cg = N / 8;
+    const int row = (int)(i / cg), c0 = (int)(i % cg) * 8;
+    if (row >= M) return;
+    float v[8], r[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    unpack8(*reinterpret_cast<const uint4*>(x + (size_t)row * ldx + c0), v);
+    if (resid) unpack8(*reinterpret_cast<const uint4*>(resid + (size_t)row * ldr + c0), r);
+    const bool live = !row_len || row % row_period < row_len[row / row_period];
+    const unsigned seed = seed_ptr ? *seed_ptr : 0u;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const bool keep = live && (thresh == 0u || drop_keep(seed, site, (uint32_t)row, (uint32_t)(c0 + j), thresh));
+        r[j] += keep ? alpha * (v[j] * scale) : 0.f;
+    }
+    *reinterpret_cast<uint4*>(out + (size_t)row * ldo + c0) = pack8(r);
+}
+const char* dropout_add_launch(cudaStream_t st, const bf16* x, int ldx, const bf16* resid, int ldr, bf16* out, int ldo, int M, int N,
+                               float alpha, float p, const unsigned* seed, unsigned site, const int* row_len, int row_period) {
+    if (M < 1 || N < 8 || N % 8 || ldx % 8 || ldo % 8 || (resid && ldr % 8)) return "dropout_add: N and the row pitches must be multiples of 8";
+    if (!(p >= 0.f && p < 1.f)) return "dropout: p must be in [0, 1)";
+    if (p > 0.f && !seed) return "dropout: null seed";
+    if (row_len && row_period < 1) return "dropout_add: row_len without row_period";
+    const size_t n = (size_t)M * (N / 8);
+    return launch<dropout_add_kernel>((unsigned)((n + 255) / 256), 256, 0, st, x, ldx, resid, ldr, out, ldo, M, N, alpha,
+                                      drop_threshold(p), 1.0f / (1.0f - p), seed, site, row_len, row_period);
+}
+
 const char* relu_bwd_launch(cudaStream_t st, const bf16* dy, const bf16* y, bf16* dx, size_t n) {
     if (n % 8) return "relu_bwd: n must be a multiple of 8";
     return launch<relu_bwd_kernel>((unsigned)((n / 8 + 255) / 256), 256, 0, st, dy, y, dx, n / 8);

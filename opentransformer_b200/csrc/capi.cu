@@ -319,13 +319,14 @@ int otb_decode_persistent(const otb_mega_model* model, const void* kvx, const in
                                                      max_steps, dbg_logp, dbg_scores, workspace, (size_t)workspace_bytes));
 }
 
-int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                      const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
-                      int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
-                      int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, void* stream) {
-    if (!q || !k || !v || !out || !dout || !lse || !dsum || !dq || !dk || !dv) return fail("otb_attention_bwd", "null operand");
+static int attention_bwd(const char* where, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v,
+                         int ldv, const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq, int lddq,
+                         int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H, int Tq, int Tk,
+                         const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd, void* dbd,
+                         int lddbd, void* stream) {
+    if (!q || !k || !v || !out || !dout || !lse || !dsum || !dq || !dk || !dv) return fail(where, "null operand");
     if ((q_col0 | k_col0 | v_col0 | dq_col0 | dk_col0 | dv_col0 | ldo | lddo | lddq | lddk | lddv) % 8)
-        return fail("otb_attention_bwd", "column offsets / leading dimensions must be multiples of 8");
+        return fail(where, "column offsets / leading dimensions must be multiples of 8");
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
     p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk; p.kv_len = kv_len; p.causal = causal;
@@ -337,7 +338,58 @@ int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk
     p.dq = reinterpret_cast<bf16*>(dq); p.lddq = lddq; p.dq_col0 = dq_col0;
     p.dk = reinterpret_cast<bf16*>(dk); p.lddk = lddk; p.dk_col0 = dk_col0;
     p.dv = reinterpret_cast<bf16*>(dv); p.lddv = lddv; p.dv_col0 = dv_col0;
-    RET("otb_attention_bwd", attn_bwd_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p));
+    p.bd = bd; p.ldbd = ldbd;
+    p.dbd = reinterpret_cast<bf16*>(dbd); p.lddbd = lddbd;
+    RET(where, attn_bwd_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p));
+}
+
+int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
+                      const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
+                      int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
+                      int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, void* stream) {
+    return attention_bwd("otb_attention_bwd", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, dout, lddo, lse, dsum, dq, lddq,
+                         dq_col0, dk, lddk, dk_col0, dv, lddv, dv_col0, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0,
+                         nullptr, 0, nullptr, 0, stream);
+}
+
+int otb_attention_bwd_bd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
+                         const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
+                         int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
+                         int Tq, int Tk, const int* kv_len, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd,
+                         void* dbd, int lddbd, void* stream) {
+    if (!bd || !dbd) return fail("otb_attention_bwd_bd", "null band or band gradient");
+    if (Tq != Tk) return fail("otb_attention_bwd_bd", "the rel-pos band needs Tq == Tk");
+    if (ldbd < 2 * Tq - 1 || lddbd < 2 * Tq - 1 || lddbd % 8)
+        return fail("otb_attention_bwd_bd", "band pitches must hold 2 Tq - 1 columns; the gradient's must be a multiple of 8");
+    return attention_bwd("otb_attention_bwd_bd", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, dout, lddo, lse, dsum, dq, lddq,
+                         dq_col0, dk, lddk, dk_col0, dv, lddv, dv_col0, B, H, Tq, Tk, kv_len, 0, q_col0, k_col0, v_col0, bd, ldbd,
+                         dbd, lddbd, stream);
+}
+
+int otb_dropout_add(const void* x, int ldx, const void* resid, int ldr, void* out, int ldo, int M, int N, float alpha, float p,
+                    const uint32_t* seed, uint32_t site, const int32_t* row_len, int row_period, void* stream) {
+    if (!x || !out) return fail("otb_dropout_add", "null operand");
+    RET("otb_dropout_add", dropout_add_launch(ST(stream), reinterpret_cast<const bf16*>(x), ldx, reinterpret_cast<const bf16*>(resid), ldr,
+                                              reinterpret_cast<bf16*>(out), ldo, M, N, alpha, p, seed, site, row_len, row_period));
+}
+
+int otb_conformer_conv_train(const void* x, const int32_t* len, const float* w, const float* wb, const float* gamma, const float* beta,
+                             float* running_mean, float* running_var, int64_t* num_batches, float momentum, float eps, float* c,
+                             float* stats, void* out, int B, int T, int d, int k, void* stream) {
+    if (!x || !len || !w || !gamma || !beta || !c || !stats || !out) return fail("otb_conformer_conv_train", "null operand");
+    RET("otb_conformer_conv_train", conv_bn_train_launch(ST(stream), reinterpret_cast<const bf16*>(x), len, w, wb, gamma, beta,
+                                                         running_mean, running_var, reinterpret_cast<long long*>(num_batches),
+                                                         momentum, eps, c, stats, reinterpret_cast<bf16*>(out), B, T, d, k));
+}
+
+int otb_conformer_conv_bwd(const void* dy, const void* x, const int32_t* len, const float* w, const float* gamma, const float* beta,
+                           const float* c, const float* stats, float* red, float* dc, void* dx, float* dw, float* dwb, float* dgamma,
+                           float* dbeta, int accumulate, int B, int T, int d, int k, void* stream) {
+    if (!dy || !x || !len || !w || !gamma || !beta || !c || !stats || !red || !dc || !dx || !dw || !dgamma || !dbeta)
+        return fail("otb_conformer_conv_bwd", "null operand");
+    RET("otb_conformer_conv_bwd", conv_bn_bwd_launch(ST(stream), reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), len,
+                                                     w, gamma, beta, c, stats, red, dc, reinterpret_cast<bf16*>(dx), dw, dwb, dgamma,
+                                                     dbeta, accumulate, B, T, d, k));
 }
 
 int otb_linear_wgrad(const void* dy, int lddy, const void* x, int ldx, float* dw, int lddw, int M, int N, int K, int accumulate,

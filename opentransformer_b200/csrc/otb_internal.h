@@ -103,6 +103,10 @@ struct AttnBwdParams {
     bf16* dq; int lddq, dq_col0;
     bf16* dk; int lddk, dk_col0;
     bf16* dv; int lddv, dv_col0;
+    const float* bd;    // optional rel-pos band of the forward (AttnParams::bd, Tq == Tk), null for plain attention
+    int ldbd;
+    bf16* dbd;          // with bd: its gradient [H,B,Tq,lddbd], zeroed by the caller; dS(i,j) lands at column j - i + Tq - 1
+    int lddbd;
 };
 const char* attn_bwd_launch(cudaStream_t st, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows,
                             const void* v, int ldv, const AttnBwdParams& p);
@@ -155,6 +159,15 @@ const char* layernorm_launch(cudaStream_t st, const bf16* x, int ldx, void* out,
                              const float* b1, const float* g2, const float* b2, float eps, int M, int N);
 const char* scale_add_table_launch(cudaStream_t st, const void* x, int ldx, int x_f32, bf16* out, int ldo, float alpha,
                                    const float* table, int period, int M, int N);
+// Conformer convolution module in training mode (conformer_train.cu)
+const char* conv_bn_train_launch(cudaStream_t st, const bf16* x, const int* len, const float* w, const float* wb, const float* gamma,
+                                 const float* beta, float* run_mean, float* run_var, long long* n_batches, float momentum, float eps,
+                                 float* c, float* stats, bf16* out, int B, int T, int d, int k);
+const char* conv_bn_bwd_launch(cudaStream_t st, const bf16* dy, const bf16* x, const int* len, const float* w, const float* gamma,
+                               const float* beta, const float* c, const float* stats, float* red, float* dc, bf16* dx, float* dw,
+                               float* dwb, float* dgamma, float* dbeta, int accumulate, int B, int T, int d, int k);
+const char* dropout_add_launch(cudaStream_t st, const bf16* x, int ldx, const bf16* resid, int ldr, bf16* out, int ldo, int M, int N,
+                               float alpha, float p, const unsigned* seed, unsigned site, const int* row_len, int row_period);
 const char* dwconv_swish_launch(cudaStream_t st, const bf16* x, const float* w, const float* b, bf16* out, int B, int T,
                                 int d, int k);
 const char* sinusoid_table_launch(cudaStream_t st, float* out, int n_pos, int d, int first_pos);

@@ -46,3 +46,13 @@ def allreduce_mean_(flat, group=None):
         dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
         flat.mul_(1.0 / world)
     return flat
+
+
+def broadcast_from_first_(tensors, group=None):
+    """In place: every rank takes the first rank's values of `tensors` (the model's buffers, as the reference's
+    DistributedDataParallel broadcasts them from rank 0 before each forward).  No-op without a process group."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) < 2:
+        return
+    src = dist.get_global_rank(group, 0) if group is not None else 0
+    for t in tensors:
+        dist.broadcast(t, src=src, group=group)

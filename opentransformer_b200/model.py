@@ -91,6 +91,12 @@ class SpeechToText(nn.Module):
             from . import train
             loss, ctc = train.loss_with_grad(self, inputs['inputs'], inputs['mask'], truth, tlen)
             return loss, ({'CTCLoss': float(ctc)} if ctc is not None else None)
+        if self.training and isinstance(self.encoder, ConformerEncoder):
+            # train() without gradients: BatchNorm must use the batch statistics and update its running buffers, as the
+            # reference does; the inference path below would fold the running statistics instead
+            from . import train
+            loss, ctc = train.loss_train_mode(self, inputs['inputs'], inputs['mask'], truth, tlen)
+            return loss, ({'CTCLoss': float(ctc)} if ctc is not None else None)
         mem, lengths, B, T2 = self.encode_bf16(inputs['inputs'], inputs['mask'])
         tin = truth[:, :-1].contiguous()
         logits_pad = self.decoder.forward_bf16(tin, mem, lengths, B, tin.shape[1], T2)

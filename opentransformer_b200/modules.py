@@ -416,15 +416,23 @@ class MultiHeadedSelfAttentionWithRelPos(nn.Module):
     def run(self, y, x_resid, pk, B, T, lengths, pos_bf16):
         """y = LN(x) bf16 [B*T,d]; returns x_resid + attention (no output projection)."""
         d, H = self.d_model, self.nheads
-        dk = d // H
         ext = ops.linear(y, pk['wext'], pk['bext'])                       # [M, 4d]
         pproj = ops.linear(pos_bf16, pk['wpos'])                          # [2T-1, d]  pos_proj(PE[-(T-1)..T-1])
-        ld = (2 * T - 1 + 3) // 4 * 4
-        bd = torch.empty(H, B * T, ld, dtype=torch.float32, device=y.device)
-        for h in range(H):  # BD_full[h] = (q+v)_h P_h^T ; the attention kernel reads the j-i+T-1 diagonal band
-            ops.linear(ext[:, d + dk * h: d + dk * (h + 1)], pproj[:, dk * h: dk * (h + 1)], out=bd[h])
+        bd = rel_pos_band(ext, pproj, H, B, T)
         return ops.attention(ext, ext, ext, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=2 * d, v_col0=3 * d,
-                             bd=bd, resid=x_resid, d_k=dk)
+                             bd=bd, resid=x_resid, d_k=d // H)
+
+
+def rel_pos_band(ext, pproj, H, B, T):
+    """BD f32 [H, B*T, ld]: row i of head h holds (q_i+v)_h . P_h[m] for m = 0 .. 2T-2 (the attention kernels read the
+    j-i+T-1 diagonal band).  ext = [q+u | q+v | k | v] bf16 [B*T, 4d]; pproj = pos_proj(PE[-(T-1)..T-1]) bf16 [2T-1, d]."""
+    d = ext.shape[1] // 4
+    dk = d // H
+    ld = (2 * T - 1 + 3) // 4 * 4
+    bd = torch.empty(H, B * T, ld, dtype=torch.float32, device=ext.device)
+    for h in range(H):  # BD_full[h] = (q+v)_h P_h^T
+        ops.linear(ext[:, d + dk * h: d + dk * (h + 1)], pproj[:, dk * h: dk * (h + 1)], out=bd[h])
+    return bd
 
 
 class ConformerConvolutionModule(nn.Module):
@@ -464,6 +472,11 @@ class ConformerEncoderBlock(nn.Module):
         super().__init__()
         self.conv_first, self.macaron_style, self.ffn_scale = conv_first, macaron_style, ffn_scale
         self.relative_positional, self.n_heads = relative_positional, n_heads
+        # training-time rates (encoder/conformer.py:53-72); inference ignores them, train.py checks them.  conv_dropout builds
+        # a Dropout the reference never applies (module/conformer.py:34,36-57).
+        self.dropout_rates = {'slf_attn_dropout': slf_attn_dropout, 'ffn_dropout': ffn_dropout,
+                              'residual_dropout': residual_dropout, 'conv_dropout': conv_dropout}
+        self.conv_bias = conv_bias
         if macaron_style:
             self.pre_ffn = PositionwiseFeedForward(d_model, d_ff, ffn_dropout, activation=activation)
             self.macaron_ffn_norm = nn.LayerNorm(d_model)

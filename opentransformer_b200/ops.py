@@ -178,6 +178,24 @@ def dropout_bwd(dy, p, seed, site):
     return out
 
 
+def dropout_add(x, resid, p=0.0, seed=None, site=0, alpha=1.0, row_len=None, row_period=0, out=None):
+    """out = resid + alpha * dropout_p(x) with the mask of (seed, site) (otb_dropout_add); resid None: alpha * dropout_p(x),
+    also the backward of such a site.  row_len / row_period: rows past their utterance's length read x as zero."""
+    _mat(x, 'x')
+    if resid is not None:
+        _mat(resid, 'resid')
+    if row_len is not None:
+        _need(row_len, torch.int32, 'row_len')
+    M, N = x.shape
+    if out is None:
+        out = torch.empty(M, N, dtype=BF16, device=x.device)
+    check(_lib.lib().otb_dropout_add(_p(x), x.stride(0), _p(resid), resid.stride(0) if resid is not None else 0, _p(out), out.stride(0),
+                                     M, N, float(alpha), float(p), _p(seed), int(site), _p(row_len), int(row_period), _stream()),
+          'otb_dropout_add')
+    _count()
+    return out
+
+
 def dropout_mask(M, N, p, seed, site):
     """u8 [M,N] keep mask of a dropout site (parity tests replay it in the oracle)."""
     mask = torch.empty(M, N, dtype=torch.uint8, device=seed.device)
@@ -423,24 +441,76 @@ def decode_persistent(model_c, kvx, mem_len, kc, vc, state, B, T, max_steps, wor
 # ------------------------------------------------------------------------------------------------
 # training step: backward kernels (include/otb200.h "Training step")
 # ------------------------------------------------------------------------------------------------
-def attention_train(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, v_col0=0):
+def attention_train(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, v_col0=0, bd=None):
     """attention (d_k 64, the width of the backward) + the per-row log-sum-exp the backward needs
-    -> (out bf16 [B*Tq, H*64], lse f32 [B,H,Tq])."""
-    return _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, with_lse=True)
+    -> (out bf16 [B*Tq, H*64], lse f32 [B,H,Tq]).  bd: the rel-pos band, as for attention()."""
+    return _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, bd=bd, with_lse=True)
+
+
+def rel_band_ld(T):
+    """Row pitch of the bf16 band gradient dBD: 2T - 1 columns rounded up to 8 (a TMA operand of the band GEMMs)."""
+    return (2 * T - 1 + 7) // 8 * 8
 
 
 def attention_bwd(q, k, v, out, dout, lse, B, H, Tq, Tk, dq, dk, dv, kv_len=None, causal=False, q_col0=0, k_col0=0,
-                  v_col0=0, dq_col0=0, dk_col0=0, dv_col0=0):
-    """Gradients of otb_attention written into dq/dk/dv (bf16 matrices, column offsets d*_col0)."""
+                  v_col0=0, dq_col0=0, dk_col0=0, dv_col0=0, bd=None, dbd=None):
+    """Gradients of otb_attention written into dq/dk/dv (bf16 matrices, column offsets d*_col0).  With the rel-pos band bd
+    f32 [H, B*Tq, ld] of the forward, its gradient is written into dbd bf16 [H, B*Tq, rel_band_ld(Tq)], which the caller
+    zeroes (otb_attention_bwd_bd)."""
     for t, n in ((q, 'q'), (k, 'k'), (v, 'v'), (out, 'out'), (dout, 'dout'), (dq, 'dq'), (dk, 'dk'), (dv, 'dv')):
         _mat(t, n)
     dsum = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device)
-    check(_lib.lib().otb_attention_bwd(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0),
-                                       _p(out), out.stride(0), _p(dout), dout.stride(0), _p(lse), _p(dsum),
-                                       _p(dq), dq.stride(0), dq_col0, _p(dk), dk.stride(0), dk_col0, _p(dv), dv.stride(0),
-                                       dv_col0, B, H, Tq, Tk, _p(kv_len), 1 if causal else 0, q_col0, k_col0, v_col0,
-                                       _stream()), 'otb_attention_bwd')
+    args = (_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out), out.stride(0), _p(dout),
+            dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), dq_col0, _p(dk), dk.stride(0), dk_col0, _p(dv), dv.stride(0),
+            dv_col0, B, H, Tq, Tk, _p(kv_len))
+    if bd is None:
+        check(_lib.lib().otb_attention_bwd(*args, 1 if causal else 0, q_col0, k_col0, v_col0, _stream()), 'otb_attention_bwd')
+    else:
+        if causal:
+            raise ValueError('attention_bwd: the rel-pos band is for non-causal self-attention')
+        _need(bd, torch.float32, 'bd'); _need(dbd, BF16, 'dbd')
+        check(_lib.lib().otb_attention_bwd_bd(*args, q_col0, k_col0, v_col0, _p(bd), bd.shape[-1], _p(dbd), dbd.shape[-1],
+                                              _stream()), 'otb_attention_bwd_bd')
     _count(2)
+
+
+def conformer_conv_train(x, lengths, w, wb, gamma, beta, running_mean, running_var, num_batches, B, T, momentum=0.1, eps=1e-5):
+    """Training-mode middle of the Conformer convolution module (otb_conformer_conv_train): x bf16 [B*T, d] GLU output,
+    w f32 [d, k] depthwise weight, wb f32 [d] or None; BatchNorm over batch statistics, running buffers updated in place.
+    -> (out bf16 [B*T, d] = swish(BN(conv(x))) zero on padded frames, c f32 [B*T, d] conv output, stats f32 [2, d])."""
+    _need(x, BF16, 'x'); _need(lengths, torch.int32, 'lengths'); _need(w, torch.float32, 'w')
+    _need(gamma, torch.float32, 'gamma'); _need(beta, torch.float32, 'beta')
+    M, d = x.shape
+    c = torch.empty(M, d, dtype=torch.float32, device=x.device)
+    stats = torch.empty(2, d, dtype=torch.float32, device=x.device)
+    out = torch.empty_like(x)
+    check(_lib.lib().otb_conformer_conv_train(_p(x), _p(lengths), _p(w), _p(wb), _p(gamma), _p(beta), _p(running_mean), _p(running_var),
+                                              _p(num_batches), float(momentum), float(eps), _p(c), _p(stats), _p(out), B, T, d,
+                                              w.shape[-1], _stream()), 'otb_conformer_conv_train')
+    _count(4)
+    return out, c, stats
+
+
+def conformer_conv_bwd(dy, x, lengths, w, gamma, beta, c, stats, B, T, dw=None, dwb=None, dgamma=None, dbeta=None, accumulate=False,
+                       has_bias=True):
+    """Backward of conformer_conv_train -> (dx bf16 [B*T, d], dw f32 [d, k], dwb f32 [d] or None, dgamma, dbeta); with accumulate
+    the given gradient tensors are added to."""
+    _need(dy, BF16, 'dy'); _need(x, BF16, 'x')
+    M, d = x.shape
+    dev = x.device
+    f32 = dict(dtype=torch.float32, device=dev)
+    dw = dw if dw is not None else torch.empty(d, w.shape[-1], **f32)
+    dwb = (dwb if dwb is not None else torch.empty(d, **f32)) if has_bias else None
+    dgamma = dgamma if dgamma is not None else torch.empty(d, **f32)
+    dbeta = dbeta if dbeta is not None else torch.empty(d, **f32)
+    red = torch.empty(2, d, **f32)
+    dc = torch.empty(M, d, **f32)
+    dx = torch.empty_like(x)
+    check(_lib.lib().otb_conformer_conv_bwd(_p(dy), _p(x), _p(lengths), _p(w), _p(gamma), _p(beta), _p(c), _p(stats), _p(red), _p(dc),
+                                            _p(dx), _p(dw), _p(dwb), _p(dgamma), _p(dbeta), 1 if accumulate else 0, B, T, d, w.shape[-1],
+                                            _stream()), 'otb_conformer_conv_bwd')
+    _count(4)
+    return dx, dw, dwb, dgamma, dbeta
 
 
 def linear_wgrad(dy, x, out=None, accumulate=False):

@@ -14,7 +14,8 @@ parameters exactly like the reference module.
 Scope: the shipped Speech-Transformer configuration -- conv front end, post-norm Transformer encoder / decoder with GLU
 feed-forward, tied or untied output layer, `residual_dropout` as shipped (0.1: counter-based masks in the residual GEMM's
 epilogue, replayed in the backward; csrc/dropout.cuh); the other dropout rates must be 0 (as shipped) and raise
-otherwise.  Conformer / pre-norm training is not built yet and raises.
+otherwise.  The encoder may also be the shipped Conformer layout with 64-wide heads (macaron feed-forward, rel-pos
+attention, then the convolution module with training-mode BatchNorm; encoder/conformer.py:75-89).
 """
 import math
 from collections import namedtuple
@@ -23,8 +24,8 @@ import torch
 
 from . import ops
 from . import modules
-from .dp import allreduce_mean_
-from .modules import TransformerDecoder, TransformerEncoder, ConvFrontEnd, _lengths
+from .dp import allreduce_mean_, broadcast_from_first_
+from .modules import ConformerEncoder, TransformerDecoder, TransformerEncoder, ConvFrontEnd, _lengths
 from .ops import BF16, EPI_BIAS, EPI_RESID, EPI_TABLE, EPI_RELU
 
 
@@ -48,10 +49,12 @@ class TrainPack:
     def __init__(self, model, bf16_of=None):
         self._bf16_of = bf16_of
         fe, enc, dec = model.frontend, model.encoder, model.decoder
-        if not isinstance(fe, ConvFrontEnd) or not isinstance(enc, TransformerEncoder) or not isinstance(dec, TransformerDecoder):
-            raise NotImplementedError('training path: conv front end + Transformer encoder / decoder only (round 1)')
-        if enc.relative_positional:
-            raise NotImplementedError('training path: absolute positions only')
+        self.conformer = isinstance(enc, ConformerEncoder)
+        if not isinstance(fe, ConvFrontEnd) or not isinstance(enc, (TransformerEncoder, ConformerEncoder)) \
+                or not isinstance(dec, TransformerDecoder):
+            raise NotImplementedError('training path: conv front end + Transformer or Conformer encoder + Transformer decoder only')
+        if not self.conformer and enc.relative_positional:
+            raise NotImplementedError('training path: the Transformer encoder with absolute positions only')
         for name, d_model, blocks in (('encoder', enc.d_model, enc.blocks), ('decoder', dec.d_model, dec.blocks)):
             for blk in blocks:
                 if d_model != 64 * blk.n_heads:   # the attention backward (otb_attention_bwd) is written for 64-wide heads
@@ -61,13 +64,16 @@ class TrainPack:
         if (C1 + 63) // 64 * 64 > 256:       # the conv1 weight gradient (otb_conv1_wgrad) runs one channel per thread
             raise NotImplementedError(f'training path: mid_channel {C1} pads to {(C1 + 63) // 64 * 64} channels; the conv1 weight '
                                       'gradient takes at most 256')
+        if self.conformer:
+            _check_conformer(enc)
         if fe.front_end_layer_norm or enc.pos_emb.scale_learnable or dec.pos_emb.scale_learnable:
-            raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale')
+            raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale (pos_dropout > 0)')
         for blk in list(enc.blocks) + list(dec.blocks):
-            if blk.feed_forward.activation not in ('glu', 'relu'):
+            if _ffn_of(blk).activation not in ('glu', 'relu'):
                 raise NotImplementedError('training path: GLU or ReLU feed-forward only')
             rates = getattr(blk, 'dropout_rates', {})
-            other = {k: v for k, v in rates.items() if k != 'residual_dropout' and float(v) > 0.0}
+            # conv_dropout: the reference builds the Dropout and never applies it (module/conformer.py:34,36-57)
+            other = {k: v for k, v in rates.items() if k not in ('residual_dropout', 'conv_dropout') and float(v) > 0.0}
             if other:
                 # the reference applies these in train mode (attention.py:45, ffn.py:40); training WITHOUT them would be a
                 # different network, so refuse instead of silently dropping the regulariser.  residual_dropout -- the only
@@ -77,10 +83,10 @@ class TrainPack:
                 raise ValueError('residual_dropout must be in [0, 1)')
         self._names = {m: n for n, m in model.named_modules()}
         self.fe = self._frontend(fe)
-        self.enc = [self._enc_layer(b) for b in enc.blocks]
+        self.enc = [self._conf_layer(b) if self.conformer else self._enc_layer(b) for b in enc.blocks]
         self.dec = [self._dec_layer(b) for b in dec.blocks]
         # pre-norm stacks end with one more LayerNorm (encoder/transformer.py:96-97,131-132; decoder/transformer.py:151-152,178-179)
-        self.enc_pre, self.dec_pre = bool(enc.normalize_before), bool(dec.normalize_before)
+        self.enc_pre, self.dec_pre = bool(getattr(enc, 'normalize_before', False)), bool(dec.normalize_before)
         self.enc_norm = self._ln(enc.norm) if self.enc_pre else None
         self.dec_norm = self._ln(dec.after_norm) if self.dec_pre else None
         V, d = dec.vocab_size, dec.d_model
@@ -113,11 +119,57 @@ class TrainPack:
         return {'qkv': self._lin(a.qvk_proj), 'o': self._lin(a.output_proj), 'w1': self._lin(f.w_1), 'w2': self._lin(f.w_2),
                 'ln1': self._ln(b.norm1), 'ln2': self._ln(b.norm2), 'act': f.activation}
 
+    def _conf_layer(self, b):
+        """A Conformer block: the rel-pos projection as ONE GEMM producing [q+u | q+v | k | v] (W_ext = [Wq; Wq; Wk; Wv],
+        b_ext = [bq + u; bq + v; bk; bv], as the inference pack), and the convolution module with BatchNorm unfolded."""
+        a, cv = b.mha, b.conv
+        w = self._w(a.qvk_proj.weight)
+        d = w.shape[1]
+        wext = torch.cat([w[:d], w], 0)
+        bq = _f(a.qvk_proj.bias)
+        bext = torch.cat([bq[:d] + _f(a.posu).reshape(d), bq[:d] + _f(a.posv).reshape(d), bq[d:]])
+        dw, bn = cv.depthwise_conv, cv.batch_norm
+        return {'mac_ln': self._ln(b.macaron_ffn_norm), 'w1': self._lin(b.pre_ffn.w_1), 'w2': self._lin(b.pre_ffn.w_2),
+                'act': b.pre_ffn.activation, 'scale': float(b.ffn_scale),
+                'mha_ln': self._ln(b.mha_norm), 'wext': wext, 'wext_t': wext.t().contiguous(), 'bext': bext,
+                'wpos': self._w(a.pos_proj.weight), 'attn': self._names[a],
+                'conv_ln': self._ln(b.conv_norm), 'pw1': self._lin(cv.pointwise_conv1), 'pw2': self._lin(cv.pointwise_conv2),
+                'dw': _f(dw.weight).view(d, -1), 'dwb': _f(dw.bias), 'dw_name': self._names[dw],
+                'bn': bn, 'bn_g': _f(bn.weight), 'bn_b': _f(bn.bias), 'bn_name': self._names[bn],
+                'post_ln': self._ln(b.post_ffn_norm), 'final_ln': self._ln(b.final_norm)}
+
     def _dec_layer(self, b):
         a, c, f = b.slf_attn, b.src_attn, b.feed_forward
         return {'qkv': self._lin(a.qvk_proj), 'o': self._lin(a.output_proj), 'q': self._lin(c.q_proj),
                 'kv': self._lin(c.vk_proj), 'o2': self._lin(c.output_proj), 'w1': self._lin(f.w_1), 'w2': self._lin(f.w_2),
                 'ln1': self._ln(b.norm1), 'ln2': self._ln(b.norm2), 'ln3': self._ln(b.norm3), 'act': f.activation}
+
+
+def _ffn_of(blk):
+    return blk.pre_ffn if hasattr(blk, 'pre_ffn') else blk.feed_forward
+
+
+def _check_conformer(enc):
+    """The Conformer layout the training path builds: the reference's shipped block (conformer_baseline.yaml)."""
+    if not (enc.positional_encoding and enc.relative_positional):
+        raise NotImplementedError('training path: the Conformer with relative positional encoding only '
+                                  '(positional_encoding and relative_positional True)')
+    for blk in enc.blocks:
+        if not blk.macaron_style or blk.conv_first:
+            raise NotImplementedError('training path: the Conformer block with macaron_style True and conv_first False only')
+        if not blk.conv_bias:
+            raise NotImplementedError('training path: the Conformer convolution module with conv_bias True only')
+        bn = blk.conv.batch_norm
+        if bn.momentum is None or not bn.track_running_stats or not bn.affine:
+            raise NotImplementedError('training path: BatchNorm1d with momentum, running statistics and affine parameters')
+
+
+def unused_parameters(model):
+    """Names of the parameters the forward never reads: a Conformer block's post_ffn (the reference applies only
+    post_ffn_norm, encoder/conformer.py:87-89), so their .grad stays None and the optimizer never moves them."""
+    if not isinstance(model.encoder, ConformerEncoder):
+        return set()
+    return {n for n, _ in model.named_parameters() if '.post_ffn.' in n and n.startswith('encoder.blocks.')}
 
 
 class _Grads(dict):
@@ -164,7 +216,13 @@ def _linear_bwd(dy, x, lin, grads, resid=None):
     return ops.linear(dy, lin.wt)
 
 
-ENC_SITE, DEC_SITE = 0, 1000      # dropout site ids: encoder layer i -> 2 i + {0, 1}; decoder layer i -> 1000 + 3 i + {0, 1, 2}
+# dropout site ids: Transformer encoder layer i -> 2 i + {0, 1}; Conformer block i -> 3 i + {0, 1, 2} (macaron feed-forward,
+# attention, convolution module); decoder layer i -> 1000 + 3 i + {0, 1, 2}
+ENC_SITE, DEC_SITE = 0, 1000
+
+
+def _enc_sites(enc):
+    return 3 if isinstance(enc, ConformerEncoder) else 2
 
 
 def _ffn_fwd(p, x):
@@ -182,20 +240,21 @@ def _ffn_act_bwd(p, dh, u, h):
 def dropout_sites(model):
     """[(site id, 'encoder' | 'decoder', rate)] of every residual-dropout site (what a parity test must replay)."""
     out = []
+    n = _enc_sites(model.encoder)
     for i, b in enumerate(model.encoder.blocks):
-        out += [(ENC_SITE + 2 * i + k, 'encoder', float(b.dropout_rates['residual_dropout'])) for k in range(2)]
+        out += [(ENC_SITE + n * i + k, 'encoder', float(b.dropout_rates['residual_dropout'])) for k in range(n)]
     for i, b in enumerate(model.decoder.blocks):
         out += [(DEC_SITE + 3 * i + k, 'decoder', float(b.dropout_rates['residual_dropout'])) for k in range(3)]
     return out
 
 
-def _resid(ctx, lin, x, drop, k):
-    """x + dropout(ctx W^T + b): the residual connection of sub-layer k in training mode (transformer.py:54,61).
+def _resid(ctx, lin, x, drop, k, alpha=1.0):
+    """x + alpha * dropout(ctx W^T + b): the residual connection of sub-layer k in training mode (transformer.py:54,61).
     drop = (rate, seed tensor, site id of the layer's sub-layer 0)."""
     rate, seed, site = drop
     if rate > 0.0:
-        return ops.linear_dropout_resid(ctx, lin.w, lin.b, x, rate, seed, site + k)
-    return ops.linear(ctx, lin.w, lin.b, EPI_RESID, resid=x)
+        return ops.linear_dropout_resid(ctx, lin.w, lin.b, x, rate, seed, site + k, alpha=alpha)
+    return ops.linear(ctx, lin.w, lin.b, EPI_RESID, resid=x, alpha=alpha)
 
 
 def _drop_bwd(dz, drop, k):
@@ -285,6 +344,113 @@ def _dec_layer_bwd(p, t, dout, dmem, mem, pre, g, B, H, L, T, lengths, drop):
     return (_ln_bwd(du1, t.a, p['ln1'], g) if pre else du1), dmem
 
 
+# A Conformer block (encoder/conformer.py:75-89, macaron, rel-pos attention, then the convolution module):
+#   x1 = x0 + ffn_scale * drop(pre_ffn(y0)),  y0 = macaron_ffn_norm(x0)          (h: GLU / ReLU output, ffn_u: GLU input)
+#   x2 = x1 + drop(relmha(y1)),               y1 = mha_norm(x1)                  (ext = [q+u | q+v | k | v], pproj = pos_proj(PE))
+#   x3 = x2 + drop(mask(conv(y2))),           y2 = conv_norm(x2)                 (cu: pointwise_conv1 output, g = GLU(cu),
+#                                                                                 c / stats: depthwise conv and BatchNorm statistics,
+#                                                                                 s = swish(BN(c)) zero on padded frames)
+#   out = final_norm(z),                      z = post_ffn_norm(x3)
+_ConfTape = namedtuple('_ConfTape', 'x0 y0 ffn_u h x1 y1 ext pproj ctx lse x2 y2 cu g c stats s x3 z')
+
+
+def _conformer_block_fwd(p, x0, B, H, T, lengths, pe, drop):
+    """One Conformer block in training mode -> (output, _ConfTape).  pe: bf16 PE[-(T-1) .. T-1]; the BatchNorm running
+    statistics are updated on the device."""
+    rate, seed, site = drop
+    d = x0.shape[1]
+    y0 = _norm(x0, p['mac_ln'])
+    ffn_u, h = _ffn_fwd(p, y0)
+    x1 = _resid(h, p['w2'], x0, drop, 0, alpha=p['scale'])
+    y1 = _norm(x1, p['mha_ln'])
+    ext = ops.linear(y1, p['wext'], p['bext'])
+    pproj = ops.linear(pe, p['wpos'])
+    bd = modules.rel_pos_band(ext, pproj, H, B, T)
+    ctx, lse = ops.attention_train(ext, ext, ext, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=2 * d, v_col0=3 * d, bd=bd)
+    del bd                   # recomputed by the backward: [H, B*T, 2T] fp32 is the largest tensor of the block
+    x2 = ops.dropout_add(ctx, x1, rate, seed, site + 1)
+    y2 = _norm(x2, p['conv_ln'])
+    cu = ops.linear(y2, p['pw1'].w, p['pw1'].b)
+    g = ops.glu_fwd(cu)
+    bn = p['bn']
+    s, c, stats = ops.conformer_conv_train(g, lengths, p['dw'], p['dwb'], p['bn_g'], p['bn_b'], bn.running_mean, bn.running_var,
+                                           bn.num_batches_tracked, B, T, momentum=bn.momentum, eps=bn.eps)
+    co = ops.linear(s, p['pw2'].w, p['pw2'].b)
+    x3 = ops.dropout_add(co, x2, rate, seed, site + 2, row_len=lengths, row_period=T)
+    z = _norm(x3, p['post_ln'])
+    return _norm(z, p['final_ln']), _ConfTape(x0=x0, y0=y0, ffn_u=ffn_u, h=h, x1=x1, y1=y1, ext=ext, pproj=pproj, ctx=ctx, lse=lse,
+                                              x2=x2, y2=y2, cu=cu, g=g, c=c, stats=stats, s=s, x3=x3, z=z)
+
+
+def _acc_out(g, name, shape, dev):
+    """The gradient tensor of `name` that kernels ADD into: the optimizer's sink, else a fresh zero tensor."""
+    out = g.out(name)
+    if out is None:
+        out = torch.zeros(shape, dtype=torch.float32, device=dev)
+    g[name] = out
+    return out
+
+
+def _relpos_attn_bwd(p, t, dctx, g, B, H, T, lengths, pe):
+    """Backward of the rel-pos attention (attention.py:196-253): attention with the band, the band's GEMMs, pos_proj,
+    posu / posv and qvk_proj (whose q rows feed both q+u and q+v).  Returns the gradient of y1 (bf16)."""
+    d = dctx.shape[1]
+    dk, M, n, dev = d // H, B * T, 2 * T - 1, dctx.device
+    bd = modules.rel_pos_band(t.ext, t.pproj, H, B, T)
+    ldb = ops.rel_band_ld(T)
+    dbd = torch.zeros(H, M, ldb, dtype=BF16, device=dev)
+    de = torch.empty_like(t.ext)                                                 # d[q+u | q+v | k | v]
+    ops.attention_bwd(t.ext, t.ext, t.ext, t.ctx, dctx, t.lse, B, H, T, T, de, de, de, kv_len=lengths, q_col0=0, k_col0=2 * d,
+                      v_col0=3 * d, dq_col0=0, dk_col0=2 * d, dv_col0=3 * d, bd=bd, dbd=dbd)
+    del bd
+    pt = torch.zeros(d, ldb, dtype=BF16, device=dev)                            # P^T, zero columns up to the band pitch
+    pt[:, :n] = t.pproj.t()
+    dp = torch.empty(ldb, d, dtype=torch.float32, device=dev)
+    for h in range(H):
+        ops.linear(dbd[h], pt[dk * h: dk * (h + 1)], out=de[:, d + dk * h: d + dk * (h + 1)])       # d(q+v)_h = dBD_h P_h
+        ops.linear_wgrad(dbd[h], t.ext[:, d + dk * h: d + dk * (h + 1)], out=dp[:, dk * h: dk * (h + 1)])   # dP_h = dBD_h^T (q+v)_h
+    acc = g.sink is not None
+    pname = p['attn'] + '.pos_proj.weight'
+    g[pname] = ops.linear_wgrad(ops.scale_add_table(dp[:n]), pe, out=g.out(pname), accumulate=acc)     # dW_pos = dP^T PE
+    qn = p['attn'] + '.qvk_proj'
+    dw = _acc_out(g, qn + '.weight', (3 * d, d), dev)
+    db = _acc_out(g, qn + '.bias', (3 * d,), dev)
+    for part in (de[:, :d], de[:, d:2 * d]):        # q+u and q+v both come from the q rows
+        ops.linear_wgrad(part, t.y1, out=dw[:d], accumulate=True)
+        ops.colsum(part, out=db[:d], accumulate=True)
+    ops.linear_wgrad(de[:, 2 * d:], t.y1, out=dw[d:], accumulate=True)
+    ops.colsum(de[:, 2 * d:], out=db[d:], accumulate=True)
+    for k, name in enumerate(('posu', 'posv')):
+        ops.colsum(de[:, k * d:(k + 1) * d], out=_acc_out(g, p['attn'] + '.' + name, (1, 1, H, dk), dev).view(d), accumulate=True)
+    return ops.linear(de, p['wext_t'])
+
+
+def _conformer_block_bwd(p, t, dout, g, B, H, T, lengths, pe, drop):
+    """Backward of _conformer_block_fwd: parameter gradients into g; returns the gradient of the block input."""
+    rate, seed, site = drop
+    acc = g.sink is not None
+    dz = _ln_bwd(dout, t.z, p['final_ln'], g)
+    dx3 = _ln_bwd(dz, t.x3, p['post_ln'], g)
+    # convolution module: its output was masked, then dropped
+    dco = ops.dropout_add(dx3, None, rate, seed, site + 2, row_len=lengths, row_period=T)
+    ds = _linear_bwd(dco, t.s, p['pw2'], g)
+    dwn, bwn, bn = p['dw_name'] + '.weight', p['dw_name'] + '.bias', p['bn_name']
+    dg, dwv, g[bwn], g[bn + '.weight'], g[bn + '.bias'] = ops.conformer_conv_bwd(
+        ds, t.g, lengths, p['dw'], p['bn_g'], p['bn_b'], t.c, t.stats, B, T, dw=g.out(dwn).view(p['dw'].shape) if acc else None,
+        dwb=g.out(bwn), dgamma=g.out(bn + '.weight'), dbeta=g.out(bn + '.bias'), accumulate=acc)
+    g[dwn] = g.out(dwn) if acc else dwv.view(dwv.shape[0], 1, -1)             # nn.Conv1d's [d, 1, k]
+    dy2 = _linear_bwd(ops.glu_bwd(dg, t.cu), t.y2, p['pw1'], g)
+    dx2 = ops.dropout_add(_ln_bwd(dy2, t.x2, p['conv_ln'], g), dx3)
+    # rel-pos attention (no output projection)
+    dy1 = _relpos_attn_bwd(p, t, _drop_bwd(dx2, drop, 1), g, B, H, T, lengths, pe)
+    dx1 = ops.dropout_add(_ln_bwd(dy1, t.x1, p['mha_ln'], g), dx2)
+    # macaron feed-forward, scaled by ffn_scale
+    df = ops.dropout_add(dx1, None, rate, seed, site, alpha=p['scale'])
+    dh = _linear_bwd(df, t.h, p['w2'], g)
+    dy0 = _linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.y0, p['w1'], g)
+    return ops.dropout_add(_ln_bwd(dy0, t.x0, p['mac_ln'], g), dx1)
+
+
 def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True, grad_sink=None, grad_scale=1.0,
                      bf16_of=None, drop_seed=None, truth_length=None, return_ctc=False):
     """One forward (+ backward) pass.  inputs f32 [B,T,F], mask bool [B,T], truth i64 [B,L+1] (BOS ... EOS PAD*).
@@ -300,6 +466,7 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
         raise ValueError('forward_backward: ctc_weight > 0 needs truth_length')
     pk = TrainPack(model, bf16_of)
     dev = inputs.device
+    conformer = pk.conformer
     e_rates = [float(b.dropout_rates['residual_dropout']) for b in enc.blocks]
     d_rates = [float(b.dropout_rates['residual_dropout']) for b in dec.blocks]
     if drop_seed is None and any(r > 0.0 for r in e_rates + d_rates):
@@ -316,13 +483,24 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     # ------------------------------------------------------------------ forward
     h1 = ops.conv1_relu(x_in, fpk['w1'], fpk['b1'])
     h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F)                       # [B*T2, F2*C2]
-    scale, table = enc.pos_emb.scale_and_table(T2, dev)
-    x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_TABLE, alpha=scale, table=table, period=T2)
-    e_drop = [(r, drop_seed, ENC_SITE + 2 * i) for i, r in enumerate(e_rates)]
+    fused_pe = enc.fuse_abs_posenc()
+    if fused_pe:
+        scale, table = enc.pos_emb.scale_and_table(T2, dev)
+        x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_TABLE, alpha=scale, table=table, period=T2)
+    else:               # rel-pos encoders take the front end's output as is (encoder/conformer.py:141-149)
+        x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_BIAS)
+    ns = _enc_sites(enc)
+    e_drop = [(r, drop_seed, ENC_SITE + ns * i) for i, r in enumerate(e_rates)]
     enc_tape = []
+    pe = enc._rel_pos(T2, dev) if conformer else None
     for p, drop in zip(pk.enc, e_drop):
-        x, t = _enc_layer_fwd(p, x, pk.enc_pre, B, H, T2, lengths, drop)
+        if conformer:
+            x, t = _conformer_block_fwd(p, x, B, H, T2, lengths, pe, drop)
+        else:
+            x, t = _enc_layer_fwd(p, x, pk.enc_pre, B, H, T2, lengths, drop)
         enc_tape.append(t)
+    if conformer:       # the running statistics moved: the inference pack, which folds BatchNorm, must be rebuilt
+        modules.bump_param_generation()
     enc_last = x
     mem = _norm(x, pk.enc_norm) if pk.enc_pre else x
 
@@ -397,10 +575,14 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     if pk.enc_pre:
         dx = _ln_bwd(dx, enc_last, pk.enc_norm, g)
     for i in reversed(range(len(pk.enc))):
-        dx = _enc_layer_bwd(pk.enc[i], enc_tape[i], dx, pk.enc_pre, g, B, H, T2, lengths, e_drop[i])
+        if conformer:
+            dx = _conformer_block_bwd(pk.enc[i], enc_tape[i], dx, g, B, H, T2, lengths, pe, e_drop[i])
+        else:
+            dx = _enc_layer_bwd(pk.enc[i], enc_tape[i], dx, pk.enc_pre, g, B, H, T2, lengths, e_drop[i])
 
-    # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE  ->  conv2 (implicit-GEMM forward, im2col GEMMs backward) -> conv1
-    dyl = ops.scale_add_table(dx, scale)                                          # d(h2 Wo^T + bo) = sqrt(d) * dx
+    # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE (abs-pos; rel-pos: x = h2 Wo^T + bo) -> conv2 (implicit-GEMM forward,
+    # im2col GEMMs backward) -> conv1
+    dyl = ops.scale_add_table(dx, scale) if fused_pe else dx                      # d(h2 Wo^T + bo) = sqrt(d) * dx
     D_out = fe.output_size
     dwo = ops.linear_wgrad(dyl, h2)                                               # [D, F2*C2], feature index f*C2 + c
     g.put('frontend.output_layer.weight', dwo.view(D_out, F2, C2).permute(0, 2, 1).reshape(D_out, C2 * F2))
@@ -421,17 +603,23 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     return (loss, g, loss_ctc) if return_ctc else (loss, g)
 
 
+def _next_drop_seed(model, device):
+    """The dropout seed of the next training forward (a fresh mask per forward), on the device."""
+    seed = getattr(model, '_drop_seed', None)
+    if seed is None or seed.device != device:
+        seed = torch.randint(0, 2 ** 31 - 1, (1,), dtype=torch.int32).to(device)
+        model._drop_seed = seed
+    seed.add_(1)
+    return seed
+
+
 class _SpeechToTextLoss(torch.autograd.Function):
     """loss = SpeechToText.forward(...) as ONE autograd node over the fp32 master parameters."""
 
     @staticmethod
     def forward(ctx, model, inputs, mask, truth, tlen, names, *params):
         with torch.no_grad():
-            seed = getattr(model, '_drop_seed', None)
-            if seed is None or seed.device != inputs.device:      # a fresh dropout mask per training forward
-                seed = torch.randint(0, 2 ** 31 - 1, (1,), dtype=torch.int32).to(inputs.device)
-                model._drop_seed = seed
-            seed.add_(1)
+            seed = _next_drop_seed(model, inputs.device)
             loss, grads, ctc = forward_backward(model, inputs, mask, truth, drop_seed=seed, truth_length=tlen, return_ctc=True)
         ctx.grads = [grads.get(n) for n in names]
         ctx.shapes = [p.shape for p in params]
@@ -454,6 +642,16 @@ def loss_with_grad(model, inputs, mask, truth, truth_length=None):
     return loss, getattr(model, '_last_ctc_loss', None)
 
 
+def loss_train_mode(model, inputs, mask, truth, truth_length=None):
+    """Training-mode SpeechToText.forward without gradients (model.train() under torch.no_grad(), e.g. a validation loop
+    that does not call eval()): the forward the reference runs in train() -- for a Conformer, BatchNorm with the batch
+    statistics, and the running statistics updated -- with no backward.  -> (loss, CTC loss or None)."""
+    with torch.no_grad():
+        loss, _, ctc = forward_backward(model, inputs, mask, truth, want_grads=False, drop_seed=_next_drop_seed(model, inputs.device),
+                                        truth_length=truth_length, return_ctc=True)
+    return loss, ctc
+
+
 def transformer_lr(step, model_size, warmup_steps, factor=1.0):
     """TransformerScheduler.get_step_lr (otrans/train/scheduler.py:137-138)."""
     return factor * model_size ** (-0.5) * min(step ** (-0.5), step * warmup_steps ** (-1.5))
@@ -467,7 +665,9 @@ class FusedTrainer:
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6, clip_grad=5.0, model_size=256,
                  warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True):
         self.model = model
-        self.params = [(n, p) for n, p in model.named_parameters() if p.requires_grad]
+        # parameters the forward never reads (a Conformer's post_ffn) stay out of the flat buffers: no gradient, no weight decay
+        unused = unused_parameters(model)
+        self.params = [(n, p) for n, p in model.named_parameters() if p.requires_grad and n not in unused]
         dev = self.params[0][1].device
         # every parameter starts on a multiple of 8 elements: the kernels that write the fp32 gradient views (wgrad, colsum)
         # and read the bf16 weight views through TMA need 16-byte aligned rows, whatever the sizes before them (an odd-sized
@@ -512,6 +712,9 @@ class FusedTrainer:
         self.max_graphs = 8           # LRU bound: every graph owns a private pool with the whole activation tape
         self._graphs = {}             # key -> (graph, inputs, mask, truth, loss, launches), most recently used last
         self._seen = {}
+        # training-mode BatchNorm buffers (Conformer): updated by every micro-step, inside the graph when one is replayed
+        self.bn_buffers = [t for n, t in model.named_buffers() if n.startswith('encoder.') and
+                           n.rsplit('.', 1)[-1] in ('running_mean', 'running_var', 'num_batches_tracked')]
 
     @property
     def opt_steps(self):
@@ -564,6 +767,7 @@ class FusedTrainer:
             sx, sm, st = inputs.clone(), mask.clone(), truth.clone()
             stl = tlen.to(torch.int32).to(inputs.device).clone() if tlen is not None else None
             snap = self.flat_g.clone()
+            bn_snap = [t.clone() for t in self.bn_buffers]          # the warm-up must not count as a step
             cur = torch.cuda.current_stream()
             side = torch.cuda.Stream()
             side.wait_stream(cur)
@@ -571,6 +775,8 @@ class FusedTrainer:
                 self._micro(sx, sm, st, stl)
             cur.wait_stream(side)
             self.flat_g.copy_(snap)
+            for t, v in zip(self.bn_buffers, bn_snap):
+                t.copy_(v)
             graph = torch.cuda.CUDAGraph()
             n0 = ops.COUNTERS['launches']
             with torch.cuda.graph(graph):
@@ -585,6 +791,9 @@ class FusedTrainer:
         """One micro-batch; every `accum_steps` calls an optimizer step.  Returns the (un-scaled) loss tensor.
         truth_length (targets['targets_length']) is needed by joint-CTC models only."""
         with torch.no_grad():
+            # data parallel: BatchNorm running statistics follow the first rank's (DistributedDataParallel's
+            # broadcast_buffers): each rank's forward updates them from its own shard, so they would drift apart
+            broadcast_from_first_(self.bn_buffers, self.group)
             ent = self._graph_for(inputs, mask, truth, truth_length) if self.use_graph else None
             if ent is not None:
                 graph, sx, sm, st, loss, launches, stl = ent
@@ -595,6 +804,8 @@ class FusedTrainer:
                     stl.copy_(truth_length)
                 graph.replay()
                 ops.COUNTERS['launches'] += launches
+                if self.bn_buffers:
+                    modules.bump_param_generation()     # the replay moved the running statistics
             else:
                 loss = self._micro(inputs, mask, truth, truth_length)
             self.micro += 1
