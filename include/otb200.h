@@ -300,6 +300,30 @@ int otb_adam_step_sched(float* p, const float* g, float* m, float* v, long long 
                         float base_lr, float model_size, float warmup_steps, float factor, float beta1, float beta2, float eps,
                         float weight_decay, int32_t* counters, float* hyper, void* stream);
 
+/* ---- Recurrent language model (model/lm.py:31-90, rnnlm.yaml): nn.LSTM layers, gates ordered i, f, g, o.  Sequences are
+ * time-major (row t*B + b, as nn.LSTM without batch_first).  The input projection gx f32 [L*B, 4H] = x W_ih^T + b_ih + b_hh
+ * is otb_linear in front; these run the recurrence as persistent cooperative kernels (CTA j keeps the W_hh slice of its
+ * hidden units in shared memory; one grid barrier per step).  H must be a multiple of 8 and the slice must fit shared
+ * memory (otb_lstm_config); otherwise they return an error and launch nothing.  barrier u32 [2]: zeroed once, then reused
+ * by launches that run one after another (one per stream).
+ *
+ * Host-only plan for hidden size H on a device with `sms` SMs and `smem_optin` bytes of opt-in shared memory per block:
+ * hidden units per CTA, and the dynamic shared memory of the forward and backward kernels; an error where they refuse H. */
+int otb_lstm_config(int H, int sms, int smem_optin, int* units, int* smem_fwd, int* smem_bwd);
+/* Forward of one layer: w_hh bf16 [4H, H]; h0 / c0 f32 [B, H] or NULL (zero state); y bf16 [L*B, H] = h_t; h_n / c_n f32
+ * [B, H] = the last step's h and c (fp32; outputs must not alias the inputs).  For training, gates (f32 [L*B, 4H],
+ * post-activation, may alias gx) and c_all (f32 [L*B, H], c_t) record what otb_lstm_bwd reads; both NULL or both set. */
+int otb_lstm_fwd(const float* gx, const void* w_hh, const float* h0, const float* c0, void* y, float* h_n, float* c_n, float* gates,
+                 float* c_all, uint32_t* barrier, int L, int B, int H, void* stream);
+/* Backward through time of one layer run with zero or given c0: dy bf16 [L*B, H] = gradient of y (h_n and c_n get none);
+ * gates / c_all as otb_lstm_fwd recorded them -> dg bf16 [L*B, 4H] = gradient of the pre-activation gates, from which
+ * dW_hh = dg[B:]^T y[:-B] and dW_ih = dg^T x (otb_linear_wgrad), db = colsum(dg) and dx = dg W_ih (otb_linear).
+ * dc f32 [B, H] is scratch. */
+int otb_lstm_bwd(const void* dy, const void* w_hh, const float* gates, const float* c_all, const float* c0, void* dg, float* dc,
+                 uint32_t* barrier, int L, int B, int H, void* stream);
+/* nn.Embedding lookup without scale: out bf16 [N, d] = emb[tok[n]] (d a multiple of 8; out-of-range ids read row 0). */
+int otb_embedding(const int64_t* tok, const void* emb, void* out, int N, int d, int vocab, void* stream);
+
 /* Log-mel filterbank features on the device (data/audio.py:117-120: ta.compliance.kaldi.fbank with Kaldi defaults, dither 0):
  * wave f32 [B, ld_wave] (zero padded), n_samples i32 [B]; window f32 [frame_len] (povey); bank f32 [F, 256] triangular mel
  * weights over the first 256 bins of the 512-point spectrum and bank_range i32 [F, 2] their non-zero [lo, hi) ranges (built

@@ -95,6 +95,10 @@ _SIGS = {
     'otb_conv_col2im_relu': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv1_wgrad': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_spec_augment': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_lstm_config': (c_int, [c_int, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
+    'otb_lstm_fwd': (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
+    'otb_lstm_bwd': (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),
+    'otb_embedding': (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
     'otb_decode_persistent_workspace': (c_int64, [c_int, c_int, c_int, c_int, c_int, c_int]),
     'otb_decode_persistent': (c_int, [POINTER(MegaModelC), _P, _P, _P, _P, POINTER(BeamStateC), c_int, c_int, c_int, _P, c_int64,
                                       _P, _P, _P]),

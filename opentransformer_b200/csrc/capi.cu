@@ -494,4 +494,34 @@ int otb_spec_augment(float* x, const int32_t* bands, int B, int T, int F, int n_
     RET("otb_spec_augment", spec_augment_launch(ST(stream), x, bands, B, T, F, n_freq, n_time));
 }
 
+int otb_lstm_config(int H, int sms, int smem_optin, int* units, int* smem_fwd, int* smem_bwd) {
+    LstmPlan pl;
+    if (const char* e = lstm_plan(H, sms, smem_optin, &pl)) return fail("otb_lstm_config", e);
+    if (units) *units = pl.units;
+    if (smem_fwd) *smem_fwd = (int)pl.smem_fwd;
+    if (smem_bwd) *smem_bwd = (int)pl.smem_bwd;
+    return 0;
+}
+
+int otb_lstm_fwd(const float* gx, const void* w_hh, const float* h0, const float* c0, void* y, float* h_n, float* c_n, float* gates,
+                 float* c_all, uint32_t* barrier, int L, int B, int H, void* stream) {
+    if (!gx || !w_hh || !y || !h_n || !c_n || !barrier) return fail("otb_lstm_fwd", "null operand");
+    if ((gates == nullptr) != (c_all == nullptr)) return fail("otb_lstm_fwd", "gates and c_all are recorded together");
+    RET("otb_lstm_fwd", lstm_fwd_launch(ST(stream), gx, reinterpret_cast<const bf16*>(w_hh), h0, c0, reinterpret_cast<bf16*>(y), h_n,
+                                        c_n, gates, c_all, barrier, L, B, H));
+}
+
+int otb_lstm_bwd(const void* dy, const void* w_hh, const float* gates, const float* c_all, const float* c0, void* dg, float* dc,
+                 uint32_t* barrier, int L, int B, int H, void* stream) {
+    if (!dy || !w_hh || !gates || !c_all || !dg || !dc || !barrier) return fail("otb_lstm_bwd", "null operand");
+    RET("otb_lstm_bwd", lstm_bwd_launch(ST(stream), reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(w_hh), gates, c_all,
+                                        c0, reinterpret_cast<bf16*>(dg), dc, barrier, L, B, H));
+}
+
+int otb_embedding(const int64_t* tok, const void* emb, void* out, int N, int d, int vocab, void* stream) {
+    if (!tok || !emb || !out || N < 1 || vocab < 1) return fail("otb_embedding", "bad arguments");
+    RET("otb_embedding", embedding_launch(ST(stream), reinterpret_cast<const long long*>(tok), reinterpret_cast<const bf16*>(emb),
+                                          reinterpret_cast<bf16*>(out), N, d, vocab));
+}
+
 }  // extern "C"

@@ -139,19 +139,6 @@ __device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
     asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void dg_mma16816(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                            uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldmatrix_x2(uint32_t addr, uint32_t& r0, uint32_t& r1) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr));
-}
 __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
@@ -425,8 +412,8 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                 ldmatrix_x4(wb + sw128(warp * 16 + (m & 1) * 8 + rr, 2 * ks + (m >> 1)), a0, a1, a2, a3);
                 // activation fragment (k16 x n8): (rows 0-7, k lo) (rows 0-7, k hi); lanes 16-31 pass valid but unused addresses
                 ldmatrix_x2(abase + a_off(rr, kb * 8 + ks * 2 + (m & 1)), b0, b1);
-                if (ks & 1) dg_mma16816(acc2, a0, a1, a2, a3, b0, b1);      // two independent accumulation chains
-                else dg_mma16816(acc, a0, a1, a2, a3, b0, b1);
+                if (ks & 1) mma_m16n8k16_bf16(acc2, a0, a1, a2, a3, b0, b1);      // two independent accumulation chains
+                else mma_m16n8k16_bf16(acc, a0, a1, a2, a3, b0, b1);
             }
         }
 #pragma unroll
@@ -762,8 +749,8 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                         const int key = w4 * 64 + kq * 16 + (m >> 1) * 8 + rr;
                         uint32_t b0, b1, b2, b3;
                         ldmatrix_x4(smem_u32(sK) + sw128(key, 2 * ks + (m & 1)), b0, b1, b2, b3);
-                        dg_mma16816(sc[2 * kq], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b0, b1);
-                        dg_mma16816(sc[2 * kq + 1], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b2, b3);
+                        mma_m16n8k16_bf16(sc[2 * kq], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b0, b1);
+                        mma_m16n8k16_bf16(sc[2 * kq + 1], qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], b2, b3);
                     }
                 }
             }
@@ -832,8 +819,8 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                     for (int dn = 0; dn < 2; ++dn) {
                         uint32_t v0, v1, v2, v3;
                         ldmatrix_x4_trans(smem_u32(sV) + sw128(key0 + m * 8 + rr, w4 * 2 + dn), v0, v1, v2, v3);   // keys key0 .. key0+31
-                        dg_mma16816(oc[dn], a0, a1, a2, a3, v0, v1);
-                        dg_mma16816(oc2[dn], c0, c1, c2, c3, v2, v3);
+                        mma_m16n8k16_bf16(oc[dn], a0, a1, a2, a3, v0, v1);
+                        mma_m16n8k16_bf16(oc2[dn], c0, c1, c2, c3, v2, v3);
                     }
                 }
             }

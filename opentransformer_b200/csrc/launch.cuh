@@ -1,7 +1,8 @@
 // The one way the library launches a kernel:  launch<kernel>(grid, block, dynamic smem, stream, args...)
 //
 // It returns nullptr or the CUDA error string, and clears the error it caused, so that a refused launch cannot be
-// blamed on a later call.  Cluster > 1 launches thread-block clusters of that many CTAs along x.
+// blamed on a later call.  Cluster > 1 launches thread-block clusters of that many CTAs along x; Cooperative launches a
+// grid whose CTAs are all resident at once (the launch fails instead of queueing CTAs), for kernels with a grid barrier.
 //
 // Before the first launch of each kernel, prepare<kernel>() sets two of its function attributes, once per process (a
 // function-local static of a template instantiated per kernel: C++ initialises it exactly once, even when several
@@ -39,8 +40,9 @@ const char* prepare() {
     return err == cudaSuccess ? nullptr : cudaGetErrorString(err);
 }
 
-template <auto Kern, unsigned Cluster = 1, typename... Args>
+template <auto Kern, unsigned Cluster = 1, bool Cooperative = false, typename... Args>
 const char* launch(dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+    static_assert(Cluster == 1 || !Cooperative, "a launch is either clustered or cooperative");
     if (const char* err = prepare<Kern>()) return err;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
@@ -54,6 +56,13 @@ const char* launch(dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&..
         cluster.val.clusterDim.y = 1;
         cluster.val.clusterDim.z = 1;
         cfg.attrs = &cluster;
+        cfg.numAttrs = 1;
+    }
+    cudaLaunchAttribute coop;
+    if (Cooperative) {
+        coop.id = cudaLaunchAttributeCooperative;
+        coop.val.cooperative = 1;
+        cfg.attrs = &coop;
         cfg.numAttrs = 1;
     }
     const cudaError_t e = cudaLaunchKernelEx(&cfg, Kern, std::forward<Args>(args)...);

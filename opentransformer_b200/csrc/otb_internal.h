@@ -201,6 +201,18 @@ const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const 
                          float preemph);
 const char* utt_cmvn_launch(cudaStream_t st, float* x, int B, int Tmax, int F, const int* n_frames, const float* gmean, const float* gstd);
 
+// LSTM recurrence (lstm.cu): units per CTA, grid and dynamic shared memory of the two persistent kernels for hidden size H
+struct LstmPlan {
+    int units, grid;
+    size_t smem_fwd, smem_bwd;
+};
+const char* lstm_plan(int H, int sms, int smem_optin, LstmPlan* plan);
+const char* lstm_fwd_launch(cudaStream_t st, const float* gx, const bf16* w, const float* h0, const float* c0, bf16* y, float* hn,
+                            float* cn, float* gates, float* call, unsigned* bar, int L, int B, int H);
+const char* lstm_bwd_launch(cudaStream_t st, const bf16* dy, const bf16* w, const float* gates, const float* call, const float* c0,
+                            bf16* dg, float* dc, unsigned* bar, int L, int B, int H);
+const char* embedding_launch(cudaStream_t st, const long long* tok, const bf16* emb, bf16* out, int N, int d, int vocab);
+
 int num_sms();
 extern int g_tile_policy;
 void set_error(const char* msg);

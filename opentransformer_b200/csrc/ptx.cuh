@@ -1,5 +1,5 @@
 // Thin inline-PTX wrappers for the sm_90a features the hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma and its shared-memory descriptors, and the MUFU
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma and its shared-memory descriptors, mma.sync / ldmatrix, and the MUFU
 // approximations the softmax and gate epilogues share.  No CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
@@ -151,6 +151,21 @@ __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t a_desc, uin
         : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
+
+// ---------------------------------------------------------------- mma.sync m16n8k16 (bf16 in, fp32 accumulate) and ldmatrix
+__device__ __forceinline__ void mma_m16n8k16_bf16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
+                                                  uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+__device__ __forceinline__ void ldmatrix_x2(uint32_t addr, uint32_t& r0, uint32_t& r1) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr));
+}
 
 // ---------------------------------------------------------------- small numeric helpers
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {

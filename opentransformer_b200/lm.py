@@ -1,16 +1,25 @@
-"""Transformer language model for shallow fusion on the CUDA path.
+"""Language models for shallow fusion and training on the CUDA path: the two model types of otrans/model/lm.py.
 
-Mirror of otrans/model/lm.py:93-171 (TransformerLanguageModel): embedding + sinusoidal positions +
-``num_blocks`` post-norm TransformerEncoderLayers (GLU FFN) under a causal mask + tied output projection.
-Same constructor (``params`` dict of the YAML ``model:`` section), ``state_dict`` keys and ``predict``
-signature; the layers are the same sm_90a kernels as the acoustic encoder (causal flag on the attention
-kernel).  The recogniser adds ``lm_weight * log_probs`` inside the fused log-softmax/top-k kernel
-(recognize/speech2text.py:102-105 -> otb_logsoftmax_topk).  Inference only.
+TransformerLanguageModel mirrors lm.py:93-171: embedding + sinusoidal positions + ``num_blocks`` post-norm
+TransformerEncoderLayers (GLU FFN) under a causal mask + tied output projection, on the same sm_90a kernels as the acoustic
+encoder (causal flag on the attention kernel).  Inference only.
+
+RecurrentLanguageModel mirrors lm.py:31-90 (rnnlm.yaml): embedding -> ``num_layers`` nn.LSTM layers (dropout between them
+in training) -> output projection, optionally tied to the embedding.  Each layer is one GEMM for the input projection of all
+positions and the persistent recurrence kernels of csrc/lstm.cu; ``lm.train(); loss, _ = lm(inputs, targets);
+loss.backward()`` fills ``.grad`` of every parameter through a hand-written backward through time.
+
+Both keep the reference's constructor (``params`` dict of the YAML ``model:`` section), ``state_dict`` keys and ``predict``
+signature.  The recogniser adds ``lm_weight * log_probs`` inside the fused log-softmax/top-k kernel
+(recognize/speech2text.py:102-105 -> otb_logsoftmax_topk).
 """
+import math
+
 import torch
 import torch.nn as nn
 
 from . import ops
+from . import train
 from .modules import BF16, PositionalEncoding, TransformerEncoderLayer, _Packed, _b, _no_train, _w
 
 
@@ -79,4 +88,177 @@ class TransformerLanguageModel(nn.Module):
         torch.save({'params': params, 'model': self.state_dict()}, name)
 
 
-LanguageModel = {'transformer_lm': TransformerLanguageModel}
+RNNLM_SITE = 2000      # dropout site of the output of LSTM layer k: RNNLM_SITE + k (train.ENC_SITE / DEC_SITE for the speech model)
+
+
+class _LSTMParams(nn.Module):
+    """Parameter holder with nn.LSTM's names, shapes and initialisation (weight_ih_l{k} [4H, I], weight_hh_l{k} [4H, H],
+    bias_ih_l{k}, bias_hh_l{k} [4H]; gates ordered i, f, g, o).  Its forward is never run: the layers run on csrc/lstm.cu."""
+
+    def __init__(self, input_size, hidden_size, num_layers):
+        super().__init__()
+        self.num_layers, self.hidden_size = num_layers, hidden_size
+        for k in range(num_layers):
+            i = input_size if k == 0 else hidden_size
+            for name, shape in (('weight_ih', (4 * hidden_size, i)), ('weight_hh', (4 * hidden_size, hidden_size)),
+                                ('bias_ih', (4 * hidden_size,)), ('bias_hh', (4 * hidden_size,))):
+                self.register_parameter(f'{name}_l{k}', nn.Parameter(torch.empty(shape)))
+        bound = 1.0 / math.sqrt(hidden_size)
+        for p in self.parameters():
+            nn.init.uniform_(p, -bound, bound)
+
+
+class RecurrentLanguageModel(nn.Module):
+    def __init__(self, params):
+        super().__init__()
+        self.params = params
+        self.model_type = 'recurrent_lm'
+        self.vocab_size = params['vocab_size']
+        self.share_embedding = params['share_embedding']
+        self.smoothing = params['smoothing']
+        self.num_layers = params['num_layers']
+        self.hidden_size = params['hidden_size']
+        self.dropout = float(params['dropout'])          # residual_dropout is accepted and unused, as in the reference
+        if self.hidden_size % 8:
+            raise NotImplementedError(f'RecurrentLanguageModel: the LSTM kernels need hidden_size a multiple of 8, got {self.hidden_size}')
+        self.embedding = nn.Embedding(self.vocab_size, self.hidden_size)
+        self.rnn = _LSTMParams(self.hidden_size, self.hidden_size, self.num_layers)
+        self.output_project = nn.Linear(self.hidden_size, self.vocab_size)
+        if self.share_embedding:
+            self.output_project.weight = self.embedding.weight
+        self._pack = _Packed(self, self._build_pack)
+        self._checked = None
+
+    @property
+    def ld_logits(self):
+        return (self.vocab_size + 7) // 8 * 8
+
+    def _build_pack(self):
+        emb = self.embedding.weight.detach().to(BF16).contiguous()
+        tied = self.output_project.weight is self.embedding.weight
+        wout = emb if tied else _w(self.output_project)
+        wout_t = torch.zeros(self.hidden_size, self.ld_logits, dtype=BF16, device=emb.device)    # dgrad of the logits GEMM
+        wout_t[:, :self.vocab_size] = wout.t()
+        layers = []
+        for k in range(self.num_layers):
+            w_ih = getattr(self.rnn, f'weight_ih_l{k}').detach().to(BF16).contiguous()
+            bias = (getattr(self.rnn, f'bias_ih_l{k}') + getattr(self.rnn, f'bias_hh_l{k}')).detach().float().contiguous()
+            layers.append({'ih': train._Lin(w_ih, w_ih.t().contiguous(), bias, f'rnn.ih_l{k}'),
+                           'w_hh': getattr(self.rnn, f'weight_hh_l{k}').detach().to(BF16).contiguous()})
+        return {'emb': emb, 'wout': wout, 'wout_t': wout_t, 'bout': _b(self.output_project), 'tied': tied, 'layers': layers}
+
+    def _check_device(self, device):
+        """The recurrence kernels keep a slice of W_hh per CTA in shared memory: refuse a hidden size whose slice does not
+        fit this device."""
+        if self._checked != device:
+            prop = torch.cuda.get_device_properties(device)
+            ops.lstm_config(self.hidden_size, prop.multi_processor_count, prop.shared_memory_per_block_optin)
+            self._checked = device
+
+    def _run(self, tok, pk, hidden=None, drop_seed=None, record=False):
+        """tok i64 [L, N] (time-major) -> (output of the top layer bf16 [L*N, H], h_n, c_n f32 [layers, N, H], tape).
+        hidden: (h0, c0) f32 [layers, N, H] or None; drop_seed: the dropout seed (training), else no dropout; record: keep
+        what the backward reads (per layer: input, gates, c_t, output)."""
+        self._check_device(tok.device)
+        L, N = tok.shape
+        x = ops.embedding(tok.reshape(-1), pk['emb'])
+        hs, cs, tape = [], [], []
+        for k, p in enumerate(pk['layers']):
+            gx = ops.linear(x, p['ih'].w, p['ih'].b, out_f32=True)
+            h0 = hidden[0][k].float().contiguous() if hidden is not None else None
+            c0 = hidden[1][k].float().contiguous() if hidden is not None else None
+            y, h_n, c_n, gates, c_all = ops.lstm_fwd(gx, p['w_hh'], L, N, h0, c0, train=record)
+            hs.append(h_n)
+            cs.append(c_n)
+            if record:
+                tape.append((x, gates, c_all, y))
+            x = y
+            if drop_seed is not None and self.dropout > 0.0 and k + 1 < self.num_layers:
+                x = ops.dropout_add(y, None, self.dropout, drop_seed, RNNLM_SITE + k)
+        return x, torch.stack(hs), torch.stack(cs), tape
+
+    def _logits(self, x, pk):
+        return ops.linear(x, pk['wout'], pk['bout'], ops.EPI_BIAS, out_f32=True, n_out=self.ld_logits)
+
+    def init_hidden_states(self, batch_size, device):
+        return torch.zeros([self.num_layers, batch_size, self.hidden_size]).to(device)
+
+    def predict(self, pred, hidden=None):
+        """model/lm.py:80-86: pred i64 [N, L], hidden (h, c) f32 [layers, N, H] or None (zero state)
+        -> (log-probs f32 [N, L, V], (h_n, c_n) f32 [layers, N, H])."""
+        N, L = pred.shape
+        with torch.no_grad():
+            pk = self._pack.get()
+            x, h_n, c_n, _ = self._run(pred.t().contiguous(), pk, hidden)
+            logp = ops.log_softmax(self._logits(x, pk), self.vocab_size)
+            return logp.view(L, N, self.vocab_size).transpose(0, 1).contiguous(), (h_n, c_n)
+
+    def forward(self, inputs, targets):
+        """model/lm.py:62-73: label-smoothed CE of the next-token logits, PAD ignored -> (loss, None).  In training mode with
+        gradients enabled, loss.backward() fills .grad of every parameter."""
+        if self.training and torch.is_grad_enabled():
+            named = [(n, p) for n, p in self.named_parameters() if p.requires_grad]
+            loss = _RecurrentLMLoss.apply(self, inputs['inputs'], targets['targets'], [n for n, _ in named], *[p for _, p in named])
+            return loss, None
+        with torch.no_grad():
+            seed = train._next_drop_seed(self, inputs['inputs'].device) if self.training else None
+            pk = self._pack.get()
+            x, _, _, _ = self._run(inputs['inputs'].t().contiguous(), pk, drop_seed=seed)
+            loss, _ = ops.ls_cross_entropy(self._logits(x, pk), targets['targets'].t().contiguous(), self.vocab_size, self.smoothing)
+        return loss, None
+
+    def save_checkpoint(self, params, name):
+        torch.save({'params': params, 'model': self.state_dict()}, name)
+
+
+def forward_backward(lm, inputs, targets, drop_seed=None):
+    """Training-mode forward and hand-written backward of RecurrentLanguageModel: inputs / targets i64 [N, L] (targets
+    PAD-padded) -> (loss 0-d f32, {parameter name -> fp32 gradient}).  drop_seed: int32 device tensor [1], needed when
+    dropout > 0 (applied to the output of every layer but the last)."""
+    if drop_seed is None and lm.dropout > 0.0 and lm.num_layers > 1:
+        raise ValueError('forward_backward: dropout > 0 needs a drop_seed tensor')
+    pk = lm._pack.get()
+    tok = inputs.t().contiguous()
+    L, N = tok.shape
+    V = lm.vocab_size
+    x, _, _, tape = lm._run(tok, pk, drop_seed=drop_seed, record=True)
+    loss, dlogits = ops.ls_cross_entropy_train(lm._logits(x, pk), targets.t().contiguous(), V, lm.smoothing)
+    g = train._Grads()
+    dwout, dy = train._output_layer_bwd(dlogits, x, pk['wout_t'], V, pk['tied'], g, 'embedding.weight', 'output_project')
+    for k in reversed(range(lm.num_layers)):
+        p = pk['layers'][k]
+        xk, gates, c_all, y = tape[k]
+        dg = ops.lstm_bwd(dy, p['w_hh'], gates, c_all, L, N)
+        # W_hh sees h_{t-1}: the rows of step t >= 1 against the output of step t - 1 (zero initial state)
+        whh = f'rnn.weight_hh_l{k}'
+        g[whh] = ops.linear_wgrad(dg[N:], y[:-N]) if L > 1 else torch.zeros(p['w_hh'].shape, dtype=torch.float32, device=dg.device)
+        dx = train._linear_bwd(dg, xk, p['ih'], g)
+        g[f'rnn.weight_ih_l{k}'] = g.pop(f'rnn.ih_l{k}.weight')
+        g[f'rnn.bias_ih_l{k}'] = g.pop(f'rnn.ih_l{k}.bias')
+        g[f'rnn.bias_hh_l{k}'] = g[f'rnn.bias_ih_l{k}'].clone()       # both biases enter the gates alike
+        if k > 0 and drop_seed is not None and lm.dropout > 0.0:
+            dx = ops.dropout_add(dx, None, lm.dropout, drop_seed, RNNLM_SITE + k - 1)
+        dy = dx
+    train._embedding_bwd(tok, dy, dwout, 1.0, pk['tied'], g, 'embedding.weight', 'output_project')
+    return loss, g
+
+
+class _RecurrentLMLoss(torch.autograd.Function):
+    """loss = RecurrentLanguageModel.forward(...) in training mode as ONE autograd node over the fp32 parameters."""
+
+    @staticmethod
+    def forward(ctx, lm, inputs, targets, names, *params):
+        with torch.no_grad():
+            seed = train._next_drop_seed(lm, inputs.device)
+            loss, grads = forward_backward(lm, inputs, targets, drop_seed=seed)
+        ctx.grads = [grads.get(n) for n in names]
+        ctx.shapes = [p.shape for p in params]
+        return loss.clone()
+
+    @staticmethod
+    def backward(ctx, gloss):
+        return (None, None, None, None) + tuple(None if gr is None else gr.view(shp) * gloss
+                                                for gr, shp in zip(ctx.grads, ctx.shapes))
+
+
+LanguageModel = {'transformer_lm': TransformerLanguageModel, 'rnn_lm': RecurrentLanguageModel}

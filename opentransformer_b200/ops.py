@@ -651,3 +651,76 @@ def conv1_wgrad(dpre1, x, B, T, F, C1):
     _count()
     return out
 
+
+
+# ------------------------------------------------------------------------------------------------
+# recurrent language model: LSTM recurrence (include/otb200.h "Recurrent language model")
+# ------------------------------------------------------------------------------------------------
+def lstm_config(H, sms, smem_optin):
+    """-> (hidden units per CTA, forward / backward dynamic shared memory) of the LSTM recurrence kernels for hidden size H on
+    a device with `sms` SMs and `smem_optin` bytes of opt-in shared memory per block (otb_lstm_config: host only).  Raises
+    NotImplementedError where otb_lstm_fwd / otb_lstm_bwd refuse H."""
+    u, f, b = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    if _lib.lib().otb_lstm_config(int(H), int(sms), int(smem_optin), u, f, b) != 0:
+        raise NotImplementedError(_lib.lib().otb_last_error().decode('utf-8', 'replace'))
+    return u.value, f.value, b.value
+
+
+_LSTM_BARRIERS = {}
+
+
+def _lstm_barrier(device):
+    """The grid-barrier counter of the LSTM kernels, one per stream: launches on one stream run one after another, and the
+    counter's generation scheme needs no reset between them."""
+    stream = torch.cuda.current_stream(device)
+    key = (stream.device.index, stream.cuda_stream)
+    bar = _LSTM_BARRIERS.get(key)
+    if bar is None:
+        bar = _LSTM_BARRIERS[key] = torch.zeros(2, dtype=torch.int32, device=device)
+    return bar
+
+
+def lstm_fwd(gx, w_hh, L, B, h0=None, c0=None, train=False):
+    """One LSTM layer over gx f32 [L*B, 4H] (time-major input projection incl. both biases), w_hh bf16 [4H, H], h0 / c0 f32
+    [B, H] or None -> (y bf16 [L*B, H], h_n f32 [B, H], c_n f32 [B, H], gates, c_all); with train the post-activation gates
+    (written over gx) and c_t f32 [L*B, H] for lstm_bwd, else None."""
+    _need(gx, torch.float32, 'gx'); _need(w_hh, BF16, 'w_hh')
+    H = w_hh.shape[1]
+    for t, n in ((h0, 'h0'), (c0, 'c0')):
+        if t is not None:
+            _need(t, torch.float32, n)
+    dev = gx.device
+    y = torch.empty(L * B, H, dtype=BF16, device=dev)
+    h_n = torch.empty(B, H, dtype=torch.float32, device=dev)
+    c_n = torch.empty(B, H, dtype=torch.float32, device=dev)
+    gates = gx if train else None
+    c_all = torch.empty(L * B, H, dtype=torch.float32, device=dev) if train else None
+    check(_lib.lib().otb_lstm_fwd(_p(gx), _p(w_hh), _p(h0), _p(c0), _p(y), _p(h_n), _p(c_n), _p(gates), _p(c_all),
+                                  _p(_lstm_barrier(dev)), L, B, H, _stream()), 'otb_lstm_fwd')
+    _count()
+    return y, h_n, c_n, gates, c_all
+
+
+def lstm_bwd(dy, w_hh, gates, c_all, L, B, c0=None):
+    """Backward through time of lstm_fwd(train=True): dy bf16 [L*B, H] -> dG bf16 [L*B, 4H] (pre-activation gates)."""
+    _need(dy, BF16, 'dy'); _need(w_hh, BF16, 'w_hh'); _need(gates, torch.float32, 'gates'); _need(c_all, torch.float32, 'c_all')
+    H = w_hh.shape[1]
+    dev = dy.device
+    dg = torch.empty(L * B, 4 * H, dtype=BF16, device=dev)
+    dc = torch.empty(B, H, dtype=torch.float32, device=dev)
+    check(_lib.lib().otb_lstm_bwd(_p(dy), _p(w_hh), _p(gates), _p(c_all), _p(c0), _p(dg), _p(dc), _p(_lstm_barrier(dev)), L, B, H,
+                                  _stream()), 'otb_lstm_bwd')
+    _count()
+    return dg
+
+
+def embedding(tok, emb, out=None):
+    """nn.Embedding lookup: tok i64 [N] -> bf16 [N, d] = emb[tok] (no scale)."""
+    _need(emb, BF16, 'emb')
+    tok = tok.contiguous().view(-1)
+    N, d = tok.numel(), emb.shape[1]
+    if out is None:
+        out = torch.empty(N, d, dtype=BF16, device=emb.device)
+    check(_lib.lib().otb_embedding(_p(tok), _p(emb), _p(out), N, d, emb.shape[0], _stream()), 'otb_embedding')
+    _count()
+    return out

@@ -38,8 +38,11 @@ class Recognizer:
         self.lm_weight = lm_weight
 
     def lm_decode(self, preds, hidden=None):
-        """recognize/base.py:26-37 (Transformer LM branch)."""
-        return self.lm.predict(preds, last_frame=True), hidden
+        """recognize/base.py:26-37: the Transformer LM re-reads the whole prefix, the RNN LM reads the newest token from
+        `hidden`."""
+        if self.lm.model_type == 'transformer_lm':
+            return self.lm.predict(preds, last_frame=True), hidden
+        return self.lm.predict(preds[:, -1:], hidden)
 
     def translate(self, seqs):
         results = []
@@ -71,6 +74,15 @@ class Recognizer:
                 nbest_list.append(' '.join(pred))
             results.append(nbest_list)
         return results
+
+
+def lm_log_probs(lm, preds):
+    """The LM term of one shallow-fusion step (speech2text.py:102-105 through base.py:26-37): log-probs f32 [N, V] of the
+    token after each prefix preds i64 [N, l].  The RNN LM gets the newest token and NO carried state: the reference hands
+    lm_decode cache['lm'] = None at every step (speech2text.py:41,103) and never stores the hidden state it returns."""
+    if lm.model_type == 'transformer_lm':
+        return lm.predict(preds, last_frame=True).squeeze(1).contiguous()
+    return lm.predict(preds[:, -1:], None)[0].squeeze(1).contiguous()
 
 
 class BeamDecoder:
@@ -209,14 +221,14 @@ class BeamDecoder:
         ops.COUNTERS['launches'] += self.launches_per_step
 
     def run_with_lm(self, max_steps, lm, lm_weight):
-        """Shallow fusion (speech2text.py:102-105, base.py:26-37): every step the LM re-scores the full prefixes
-        (as the reference's TransformerLanguageModel.predict does) and lm_weight * log-probs are added inside the
+        """Shallow fusion (speech2text.py:102-105, base.py:26-37): every step the LM scores the prefixes (lm_log_probs: the
+        Transformer LM re-reads them in full, the RNN LM reads the newest token) and lm_weight * log-probs are added inside the
         fused log-softmax/top-k kernel.  Eager mode: the prefix length is host-side state."""
         assert not self.use_graph, 'LM fusion runs the decode loop eagerly'
         self.lm_weight = float(lm_weight)
         for i in range(max_steps):
             preds = self.state.reconstruct(i)                       # [N, i+1], column 0 = BOS
-            self.lm_logp = lm.predict(preds, last_frame=True).squeeze(1).contiguous()
+            self.lm_logp = lm_log_probs(lm, preds)
             self._step_kernels()
             if int(self._read_ctrl()[1]):
                 break
@@ -257,9 +269,9 @@ class SpeechToTextRecognizer(Recognizer):
     def __init__(self, model, lm=None, lm_weight=0.1, ctc_weight=0.0, beam_width=5, nbest=1, max_len=50,
                  idx2unit=None, penalty=0, lamda=5, ngpu=1, apply_cache=False, use_graph=True, persistent=None):
         super().__init__(model, idx2unit, lm, lm_weight, ngpu)
-        if lm is not None and getattr(lm, 'model_type', None) != 'transformer_lm':
-            raise NotImplementedError('shallow fusion is implemented for the Transformer LM (opentransformer_b200.lm); '
-                                      'the RNN LM is out of scope')
+        if lm is not None and getattr(lm, 'model_type', None) not in ('transformer_lm', 'recurrent_lm'):
+            raise NotImplementedError('shallow fusion is implemented for the Transformer and the recurrent LM '
+                                      '(opentransformer_b200.lm)')
         self.beam_width, self.max_len, self.nbest = beam_width, max_len, nbest
         self.penalty, self.lamda = penalty, lamda
         self.ctc_weight, self.lm_weight = ctc_weight, lm_weight
@@ -297,7 +309,7 @@ class SpeechToTextRecognizer(Recognizer):
         st.flag.copy_(flag.view(-1).to(torch.uint8))
         lm_logp, lm_w = None, 0.0
         if self.lm is not None and self.lm_weight:
-            lm_logp = self.lm.predict(preds, last_frame=True).squeeze(1).contiguous()
+            lm_logp = lm_log_probs(self.lm, preds)
             lm_w = float(self.lm_weight)
         st.step(log_probs.contiguous(), log_probs.shape[-1], lm_logp, lm_w)
         parent = st.par_hist[0].long()

@@ -451,6 +451,32 @@ def _conformer_block_bwd(p, t, dout, g, B, H, T, lengths, pe, drop):
     return ops.dropout_add(_ln_bwd(dy0, t.x0, p['mac_ln'], g), dx1)
 
 
+def _output_layer_bwd(dlogits, y, wout_t, V, tied, g, emb_name, out_name):
+    """Backward of the output layer logits = y W^T + b (f32 [rows, ld], ld = V padded): the weight gradient goes into
+    emb_name's tensor when the weight is tied to the embedding, the bias gradient into g.  -> (dW f32 [V, d], dy bf16)."""
+    acc = g.sink is not None
+    wname = emb_name if tied else out_name + '.weight'
+    # dlogits[:, :V] as a strided view: the TMA map stops at column V, so the result has exactly V rows
+    dwout = ops.linear_wgrad(dlogits[:, :V], y, out=g.out(wname), accumulate=acc)          # [V, d]
+    g.put(out_name + '.bias', ops.colsum(dlogits)[:V])
+    return dwout, ops.linear(dlogits, wout_t)                                     # [rows, d]
+
+
+def _embedding_bwd(tok, dx, dwout, scale, tied, g, emb_name, out_name):
+    """Backward of x = scale * E[tok]: with tied weights the output layer's gradient dwout is the same tensor, and the
+    embedding's lands on top of it."""
+    if tied:
+        ops.embed_bwd(tok, dx, dwout, scale)          # atomics on top of the output-layer gradient
+        g[emb_name] = dwout
+    else:
+        g[out_name + '.weight'] = dwout
+        demb = g.out(emb_name)
+        if demb is None:
+            demb = torch.zeros_like(dwout)
+        ops.embed_bwd(tok, dx, demb, scale)
+        g[emb_name] = demb
+
+
 def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True, grad_sink=None, grad_scale=1.0,
                      bf16_of=None, drop_seed=None, truth_length=None, return_ctc=False):
     """One forward (+ backward) pass.  inputs f32 [B,T,F], mask bool [B,T], truth i64 [B,L+1] (BOS ... EOS PAD*).
@@ -542,27 +568,14 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     # ------------------------------------------------------------------ backward
     g = _Grads(grad_sink)
     acc = grad_sink is not None
-    wname = 'decoder.embedding.weight' if pk.tied else 'decoder.output_layer.weight'
-    # dlogits[:, :V] as a strided view: the TMA map stops at column V, so the result has exactly V rows
-    dwout = ops.linear_wgrad(dlogits[:, :V], y, out=g.out(wname), accumulate=acc)          # [V, d]
-    g.put('decoder.output_layer.bias', ops.colsum(dlogits)[:V])
-    dy = ops.linear(dlogits, pk.out['wout_t'])                                   # [B*L, d]
+    dwout, dy = _output_layer_bwd(dlogits, y, pk.out['wout_t'], V, pk.tied, g, 'decoder.embedding.weight', 'decoder.output_layer')
     dmem = None
     if pk.dec_pre:
         dy = _ln_bwd(dy, dec_last, pk.dec_norm, g)
     for i in reversed(range(len(pk.dec))):
         dy, dmem = _dec_layer_bwd(pk.dec[i], dec_tape[i], dy, dmem, mem, pk.dec_pre, g, B, Hd, L, T2, lengths, d_drop[i])
-    # embedding (decoder/transformer.py:163,169); with tied weights the output-layer gradient lands in the same tensor
-    if pk.tied:
-        ops.embed_bwd(tgt_in, dy, dwout, math.sqrt(d))          # atomics on top of the output-layer gradient
-        g['decoder.embedding.weight'] = dwout
-    else:
-        g['decoder.output_layer.weight'] = dwout
-        demb = g.out('decoder.embedding.weight')
-        if demb is None:
-            demb = torch.zeros(V, d, dtype=torch.float32, device=dev)
-        ops.embed_bwd(tgt_in, dy, demb, math.sqrt(d))
-        g['decoder.embedding.weight'] = demb
+    # embedding (decoder/transformer.py:163,169)
+    _embedding_bwd(tgt_in, dy, dwout, math.sqrt(d), pk.tied, g, 'decoder.embedding.weight', 'decoder.output_layer')
 
     dx = dmem
     if ctc_w > 0.0:     # CTC head: parameter gradients, and its gradient with respect to the memory joins the decoder's
