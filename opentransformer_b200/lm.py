@@ -2,7 +2,10 @@
 
 TransformerLanguageModel mirrors lm.py:93-171: embedding + sinusoidal positions + ``num_blocks`` post-norm
 TransformerEncoderLayers (GLU FFN) under a causal mask + tied output projection, on the same sm_90a kernels as the acoustic
-encoder (causal flag on the attention kernel).  Inference only.
+encoder (causal flag on the attention kernel).  ``lm.train(); loss, _ = lm(inputs, targets); loss.backward()`` fills
+``.grad`` of every parameter through the speech encoder layer's hand-written training forward and backward (train.py) with
+the causal mask, and ``train.FusedTrainer`` takes the model for the whole optimizer step (transformer_lm.yaml's
+TransformerScheduler is the one it keeps on the device).  Training needs 64-wide heads, the width of the attention backward.
 
 RecurrentLanguageModel mirrors lm.py:31-90 (rnnlm.yaml): embedding -> ``num_layers`` nn.LSTM layers (dropout between them
 in training) -> output projection, optionally tied to the embedding.  Each layer is one GEMM for the input projection of all
@@ -78,7 +81,19 @@ class TransformerLanguageModel(nn.Module):
             return ops.log_softmax(flat, self.vocab_size).view(N, L, self.vocab_size)
 
     def forward(self, inputs, targets):
-        """model/lm.py:126-141, forward only: label-smoothed CE of the next-token prediction."""
+        """model/lm.py:126-141: label-smoothed CE of the next-token prediction, PAD ignored -> (loss, None).  In training
+        mode with gradients enabled, loss.backward() fills .grad of every parameter; in training mode without gradients
+        the training forward (residual dropout on) runs alone."""
+        if self.training:
+            check_trainable(self)
+            if torch.is_grad_enabled():
+                named = [(n, p) for n, p in self.named_parameters() if p.requires_grad]
+                loss = _LMLoss.apply(transformer_forward_backward, self, inputs['inputs'], targets['targets'],
+                                     [n for n, _ in named], *[p for _, p in named])
+                return loss, None
+            seed = train._next_drop_seed(self, inputs['inputs'].device)
+            loss, _ = transformer_forward_backward(self, inputs['inputs'], targets['targets'], want_grads=False, drop_seed=seed)
+            return loss, None
         with torch.no_grad():
             logits = self.logits_bf16(inputs['inputs'])
             loss, _ = ops.ls_cross_entropy(logits, targets['targets'].contiguous(), self.vocab_size, self.smoothing)
@@ -86,6 +101,71 @@ class TransformerLanguageModel(nn.Module):
 
     def save_checkpoint(self, params, name):
         torch.save({'params': params, 'model': self.state_dict()}, name)
+
+
+# dropout sites of the Transformer LM's block i: TLM_SITE + 2 i + {0: after self-attention, 1: after the feed-forward}
+# (train.ENC_SITE / DEC_SITE for the speech model, RNNLM_SITE for the recurrent LM)
+TLM_SITE = 3000
+
+
+def check_trainable(lm):
+    """Refuse, before any device work, what the training path of TransformerLanguageModel does not cover.
+    -> the residual_dropout rate of every block."""
+    rates = []
+    for blk in lm.blocks:
+        if lm.d_model != 64 * blk.n_heads:      # the attention backward (otb_attention_bwd) is written for 64-wide heads
+            raise NotImplementedError(f'training path: 64-wide attention heads only; the language model has d_model '
+                                      f'{lm.d_model} with {blk.n_heads} heads')
+        rate = float(blk.dropout_rates['residual_dropout'])
+        if not 0.0 <= rate < 1.0:
+            raise ValueError('residual_dropout must be in [0, 1)')
+        rates.append(rate)
+    return rates
+
+
+def transformer_forward_backward(lm, inputs, targets, want_grads=True, grad_sink=None, grad_scale=1.0, bf16_of=None,
+                                 drop_seed=None):
+    """Training-mode forward (and hand-written backward) of TransformerLanguageModel (model/lm.py:126-141): inputs / targets
+    i64 [N, L] (targets PAD-padded) -> (loss 0-d f32, {parameter name -> fp32 gradient} or None without want_grads).
+    grad_sink / grad_scale / bf16_of / drop_seed as in train.forward_backward (drop_seed is needed when residual_dropout > 0).
+
+    The mask is get_seq_mask (lm.py:14-18): the causal tril only, no key-padding mask.  Padding sits at the end of a row,
+    so a padded position sees earlier padded positions but no scored position ever reads one, and PAD targets are left out
+    of the loss: causal attention without kv_len gives the reference's loss and gradients exactly."""
+    rates = check_trainable(lm)
+    if drop_seed is None and any(r > 0.0 for r in rates):
+        raise ValueError('transformer_forward_backward: residual_dropout > 0 needs a drop_seed tensor')
+    pk = train.LayerPack(lm, bf16_of)
+    blocks = [pk._enc_layer(b) for b in lm.blocks]
+    emb = pk._w(lm.embedding.weight)
+    tied = lm.output_project.weight is lm.embedding.weight
+    wout = emb if tied else pk._w(lm.output_project.weight)
+    bout = lm.output_project.bias.detach().float().contiguous()
+    tok = inputs.contiguous()
+    N, L = tok.shape
+    d, H, V = lm.d_model, lm.blocks[0].n_heads, lm.vocab_size
+    _, table = lm.pos_embedding.scale_and_table(L, tok.device)
+    x = ops.embed_posenc(tok, emb, table, N * L, d, period=L)                       # x * sqrt(d) + PE, dropout 0
+    drops = [(r, drop_seed, TLM_SITE + 2 * i) for i, r in enumerate(rates)]
+    tape = []
+    for p, drop in zip(blocks, drops):
+        x, t = train._enc_layer_fwd(p, x, False, N, H, L, None, drop, causal=True)
+        tape.append(t)
+    logits = ops.linear(x, wout, bout, ops.EPI_BIAS, out_f32=True, n_out=lm.ld_logits)
+    if not want_grads:
+        loss, _ = ops.ls_cross_entropy(logits, targets.contiguous(), V, lm.smoothing)
+        return loss, None
+    loss, dlogits = ops.ls_cross_entropy_train(logits, targets.contiguous(), V, lm.smoothing)
+    if grad_scale != 1.0:
+        dlogits = ops.scale_add_table(dlogits, grad_scale)                           # loss / accum_steps (trainer.py:216)
+    wout_t = torch.zeros(d, lm.ld_logits, dtype=BF16, device=emb.device)            # [d, V padded]: dgrad of the logits GEMM
+    wout_t[:, :V] = wout.t()
+    g = train._Grads(grad_sink)
+    dwout, dx = train._output_layer_bwd(dlogits, x, wout_t, V, tied, g, 'embedding.weight', 'output_project')
+    for i in reversed(range(len(blocks))):
+        dx = train._enc_layer_bwd(blocks[i], tape[i], dx, False, g, N, H, L, None, drops[i], causal=True)
+    train._embedding_bwd(tok, dx, dwout, math.sqrt(d), tied, g, 'embedding.weight', 'output_project')
+    return loss, g
 
 
 RNNLM_SITE = 2000      # dropout site of the output of LSTM layer k: RNNLM_SITE + k (train.ENC_SITE / DEC_SITE for the speech model)
@@ -198,7 +278,8 @@ class RecurrentLanguageModel(nn.Module):
         gradients enabled, loss.backward() fills .grad of every parameter."""
         if self.training and torch.is_grad_enabled():
             named = [(n, p) for n, p in self.named_parameters() if p.requires_grad]
-            loss = _RecurrentLMLoss.apply(self, inputs['inputs'], targets['targets'], [n for n, _ in named], *[p for _, p in named])
+            loss = _LMLoss.apply(forward_backward, self, inputs['inputs'], targets['targets'], [n for n, _ in named],
+                                 *[p for _, p in named])
             return loss, None
         with torch.no_grad():
             seed = train._next_drop_seed(self, inputs['inputs'].device) if self.training else None
@@ -243,22 +324,23 @@ def forward_backward(lm, inputs, targets, drop_seed=None):
     return loss, g
 
 
-class _RecurrentLMLoss(torch.autograd.Function):
-    """loss = RecurrentLanguageModel.forward(...) in training mode as ONE autograd node over the fp32 parameters."""
+class _LMLoss(torch.autograd.Function):
+    """loss = LM.forward(...) in training mode as ONE autograd node over the fp32 parameters; fb is the model's
+    forward_backward (transformer_forward_backward or forward_backward)."""
 
     @staticmethod
-    def forward(ctx, lm, inputs, targets, names, *params):
+    def forward(ctx, fb, lm, inputs, targets, names, *params):
         with torch.no_grad():
             seed = train._next_drop_seed(lm, inputs.device)
-            loss, grads = forward_backward(lm, inputs, targets, drop_seed=seed)
+            loss, grads = fb(lm, inputs, targets, drop_seed=seed)
         ctx.grads = [grads.get(n) for n in names]
         ctx.shapes = [p.shape for p in params]
         return loss.clone()
 
     @staticmethod
     def backward(ctx, gloss):
-        return (None, None, None, None) + tuple(None if gr is None else gr.view(shp) * gloss
-                                                for gr, shp in zip(ctx.grads, ctx.shapes))
+        return (None, None, None, None, None) + tuple(None if gr is None else gr.view(shp) * gloss
+                                                      for gr, shp in zip(ctx.grads, ctx.shapes))
 
 
 LanguageModel = {'transformer_lm': TransformerLanguageModel, 'rnn_lm': RecurrentLanguageModel}

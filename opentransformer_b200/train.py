@@ -16,6 +16,8 @@ feed-forward, tied or untied output layer, `residual_dropout` as shipped (0.1: c
 epilogue, replayed in the backward; csrc/dropout.cuh); the other dropout rates must be 0 (as shipped) and raise
 otherwise.  The encoder may also be the shipped Conformer layout with 64-wide heads (macaron feed-forward, rel-pos
 attention, then the convolution module with training-mode BatchNorm; encoder/conformer.py:75-89).
+The Transformer language model (lm.transformer_forward_backward) trains through the encoder layer's forward and backward
+below with the causal mask, and FusedTrainer takes it as well.
 """
 import math
 from collections import namedtuple
@@ -41,13 +43,36 @@ _Lin = namedtuple('_Lin', 'w wt b name')      # W [N,K], W^T [K,N], fp32 bias, q
 _Norm = namedtuple('_Norm', 'g b name')
 
 
-class TrainPack:
-    """bf16 operands of one training step: W [N,K] for the forward / wgrad, W^T [K,N] for the dgrad GEMMs.
-    `bf16_of(param)` (optional) returns a bf16 copy of a parameter without a per-tensor cast kernel (FusedTrainer casts
-    its flat fp32 master buffer once per step and hands out views)."""
+class LayerPack:
+    """bf16 operands of the layers of one training step: W [N,K] for the forward / wgrad, W^T [K,N] for the dgrad GEMMs,
+    named by their module's qualified name in `model`.  `bf16_of(param)` (optional) returns a bf16 copy of a parameter
+    without a per-tensor cast kernel (FusedTrainer casts its flat fp32 master buffer once per step and hands out views)."""
 
     def __init__(self, model, bf16_of=None):
         self._bf16_of = bf16_of
+        self._names = {m: n for n, m in model.named_modules()}
+
+    def _w(self, param):
+        return self._bf16_of(param) if self._bf16_of is not None else _bf(param)
+
+    def _lin(self, lin):
+        w = self._w(lin.weight)
+        return _Lin(w, w.t().contiguous(), _f(lin.bias), self._names[lin])
+
+    def _ln(self, norm):
+        return _Norm(_f(norm.weight), _f(norm.bias), self._names[norm])
+
+    def _enc_layer(self, b):
+        a, f = b.slf_attn, b.feed_forward
+        return {'qkv': self._lin(a.qvk_proj), 'o': self._lin(a.output_proj), 'w1': self._lin(f.w_1), 'w2': self._lin(f.w_2),
+                'ln1': self._ln(b.norm1), 'ln2': self._ln(b.norm2), 'act': f.activation}
+
+
+class TrainPack(LayerPack):
+    """The LayerPack of a SpeechToText model: front end, encoder and decoder layers and the output layer."""
+
+    def __init__(self, model, bf16_of=None):
+        super().__init__(model, bf16_of)
         fe, enc, dec = model.frontend, model.encoder, model.decoder
         self.conformer = isinstance(enc, ConformerEncoder)
         if not isinstance(fe, ConvFrontEnd) or not isinstance(enc, (TransformerEncoder, ConformerEncoder)) \
@@ -81,7 +106,6 @@ class TrainPack:
                 raise NotImplementedError(f'training path: only residual_dropout is implemented, got {other}; set them to 0.0')
             if not (0.0 <= float(rates.get('residual_dropout', 0.0)) < 1.0):
                 raise ValueError('residual_dropout must be in [0, 1)')
-        self._names = {m: n for n, m in model.named_modules()}
         self.fe = self._frontend(fe)
         self.enc = [self._conf_layer(b) if self.conformer else self._enc_layer(b) for b in enc.blocks]
         self.dec = [self._dec_layer(b) for b in dec.blocks]
@@ -98,26 +122,11 @@ class TrainPack:
         wout_t[:, :V] = wout.t()
         self.out = {'emb': emb, 'wout': wout, 'wout_t': wout_t, 'bout': _f(dec.output_layer.bias)}
 
-    def _w(self, param):
-        return self._bf16_of(param) if self._bf16_of is not None else _bf(param)
-
-    def _lin(self, lin):
-        w = self._w(lin.weight)
-        return _Lin(w, w.t().contiguous(), _f(lin.bias), self._names[lin])
-
-    def _ln(self, norm):
-        return _Norm(_f(norm.weight), _f(norm.bias), self._names[norm])
-
     def _frontend(self, fe):
         pk = dict(fe._build_pack())
         pk['w2_t'] = pk['w2'].t().contiguous()           # [9*C1p, C2]
         pk['wo_t'] = pk['wo'].t().contiguous()           # [F2*C2, D]
         return pk
-
-    def _enc_layer(self, b):
-        a, f = b.slf_attn, b.feed_forward
-        return {'qkv': self._lin(a.qvk_proj), 'o': self._lin(a.output_proj), 'w1': self._lin(f.w_1), 'w2': self._lin(f.w_2),
-                'ln1': self._ln(b.norm1), 'ln2': self._ln(b.norm2), 'act': f.activation}
 
     def _conf_layer(self, b):
         """A Conformer block: the rel-pos projection as ONE GEMM producing [q+u | q+v | k | v] (W_ext = [Wq; Wq; Wk; Wv],
@@ -166,8 +175,9 @@ def _check_conformer(enc):
 
 def unused_parameters(model):
     """Names of the parameters the forward never reads: a Conformer block's post_ffn (the reference applies only
-    post_ffn_norm, encoder/conformer.py:87-89), so their .grad stays None and the optimizer never moves them."""
-    if not isinstance(model.encoder, ConformerEncoder):
+    post_ffn_norm, encoder/conformer.py:87-89), so their .grad stays None and the optimizer never moves them.  A model
+    without an encoder (a language model) reads all of its parameters."""
+    if not isinstance(getattr(model, 'encoder', None), ConformerEncoder):
         return set()
     return {n for n, _ in model.named_parameters() if '.post_ffn.' in n and n.startswith('encoder.blocks.')}
 
@@ -270,12 +280,13 @@ _EncTape = namedtuple('_EncTape', 'a u1 qkv ctx lse z1 u2 ffn_u h z2')
 _DecTape = namedtuple('_DecTape', 'a u1 qkv ctx lse z1 u2 q kv ctx2 lse2 z2 u3 ffn_u h z3')
 
 
-def _enc_layer_fwd(p, a, pre, B, H, T, lengths, drop):
-    """One encoder layer in training mode (encoder/transformer.py:41-65) -> (output, _EncTape)."""
+def _enc_layer_fwd(p, a, pre, B, H, T, lengths, drop, causal=False):
+    """One encoder layer in training mode (encoder/transformer.py:41-65) -> (output, _EncTape).  causal=True: the tril
+    mask the Transformer LM feeds to the same layer (model/lm.py:14-18)."""
     d = a.shape[1]
     u1 = _norm(a, p['ln1']) if pre else a
     qkv = ops.linear(u1, p['qkv'].w, p['qkv'].b)
-    ctx, lse = ops.attention_train(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=d, v_col0=2 * d)
+    ctx, lse = ops.attention_train(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d, v_col0=2 * d)
     z1 = _resid(ctx, p['o'], u1, drop, 0)
     u2 = _norm(z1, p['ln2'] if pre else p['ln1'])
     ffn_u, h = _ffn_fwd(p, u2)
@@ -284,7 +295,7 @@ def _enc_layer_fwd(p, a, pre, B, H, T, lengths, drop):
     return out, _EncTape(a=a, u1=u1, qkv=qkv, ctx=ctx, lse=lse, z1=z1, u2=u2, ffn_u=ffn_u, h=h, z2=z2)
 
 
-def _enc_layer_bwd(p, t, dout, pre, g, B, H, T, lengths, drop):
+def _enc_layer_bwd(p, t, dout, pre, g, B, H, T, lengths, drop, causal=False):
     """Backward of _enc_layer_fwd: parameter gradients into g; returns the gradient of the layer input."""
     d = t.a.shape[1]
     dz2 = dout if pre else _ln_bwd(dout, t.z2, p['ln2'], g)
@@ -294,8 +305,8 @@ def _enc_layer_bwd(p, t, dout, pre, g, B, H, T, lengths, drop):
     dz1 = _ln_bwd(du2, t.z1, p['ln2'] if pre else p['ln1'], g)
     dctx = _linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
     dqkv = torch.empty_like(t.qkv)
-    ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B, H, T, T, dqkv, dqkv, dqkv, kv_len=lengths, q_col0=0,
-                      k_col0=d, v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
+    ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B, H, T, T, dqkv, dqkv, dqkv, kv_len=lengths, causal=causal,
+                      q_col0=0, k_col0=d, v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
     du1 = _linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
     return _ln_bwd(du1, t.a, p['ln1'], g) if pre else du1
 
@@ -673,10 +684,19 @@ def transformer_lr(step, model_size, warmup_steps, factor=1.0):
 class FusedTrainer:
     """The inner step of Trainer.train_one_epoch (trainer.py:206-234) on flat fp32 buffers:
     forward + hand-written backward -> (data-parallel) gradient all-reduce over NCCL -> global-norm clip + Adam in two
-    kernels, no host synchronisation.  Parameters become views into one flat buffer (state_dict keys / shapes unchanged)."""
+    kernels, no host synchronisation.  Parameters become views into one flat buffer (state_dict keys / shapes unchanged).
+    `model` is a SpeechToText or a TransformerLanguageModel (transformer_lm.yaml trains with the same scheduler)."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6, clip_grad=5.0, model_size=256,
                  warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True):
+        from . import lm          # lm imports this module
+        if isinstance(model, lm.RecurrentLanguageModel):
+            raise NotImplementedError('FusedTrainer: the recurrent LM trains with a step-linear scheduler that is not on the '
+                                      'device; train it through loss.backward() and a torch optimizer')
+        self._lm_forward_backward = None
+        if isinstance(model, lm.TransformerLanguageModel):
+            lm.check_trainable(model)
+            self._lm_forward_backward = lm.transformer_forward_backward
         self.model = model
         # parameters the forward never reads (a Conformer's post_ffn) stay out of the flat buffers: no gradient, no weight decay
         unused = unused_parameters(model)
@@ -750,23 +770,29 @@ class FusedTrainer:
         (o, k), shape = self._by_ptr[param.data_ptr()]
         return self.flat_bf16[o:o + k].view(shape)
 
-    def _micro(self, inputs, mask, truth, tlen=None):
+    def _micro(self, batch):
         """forward + backward of one micro-batch; gradients / accum_steps are ADDED into the flat buffer by the backward
-        kernels themselves (no per-parameter add)."""
+        kernels themselves (no per-parameter add).  batch: (inputs, mask, truth, truth_length or None) of a SpeechToText,
+        (inputs, targets) of a language model."""
         self.flat_bf16.copy_(self.flat_p)
         self.drop_seed.add_(1)
-        loss, _ = forward_backward(self.model, inputs, mask, truth, grad_sink=self.sink, grad_scale=1.0 / self.accum_steps,
-                                   bf16_of=self._bf16_of, drop_seed=self.drop_seed, truth_length=tlen)
+        kw = dict(grad_sink=self.sink, grad_scale=1.0 / self.accum_steps, bf16_of=self._bf16_of, drop_seed=self.drop_seed)
+        if self._lm_forward_backward is not None:
+            loss, _ = self._lm_forward_backward(self.model, *batch, **kw)
+        else:
+            inputs, mask, truth, tlen = batch
+            loss, _ = forward_backward(self.model, inputs, mask, truth, truth_length=tlen, **kw)
         return loss
 
-    def _graph_for(self, inputs, mask, truth, tlen=None):
+    def _graph_for(self, batch):
         """The ~870 launches of one micro-batch captured once per input geometry and replayed: launched one by one from
         Python the step is host-bound.
         Real ASR batches have a new (T, L) almost every step, so a geometry runs EAGERLY until it has recurred
         `graph_after` times, and at most `max_graphs` graphs are kept (least recently used first out): use_graph pays off
         with bucketed / padded batches (otrans/data/bucket.py), it must not grow memory without bound otherwise.
         Returns None when this call should run eagerly."""
-        key = (tuple(inputs.shape), tuple(truth.shape), inputs.device.index)
+        dev = batch[0].device
+        key = tuple(None if t is None else tuple(t.shape) for t in batch) + (dev.index,)
         ent = self._graphs.pop(key, None)
         if ent is None:
             n = self._seen.get(key, 0) + 1
@@ -777,15 +803,14 @@ class FusedTrainer:
                 return None
             while len(self._graphs) >= self.max_graphs:
                 self._graphs.pop(next(iter(self._graphs)))        # drops the graph and its memory pool
-            sx, sm, st = inputs.clone(), mask.clone(), truth.clone()
-            stl = tlen.to(torch.int32).to(inputs.device).clone() if tlen is not None else None
+            static = tuple(None if t is None else t.to(dev).clone() for t in batch)
             snap = self.flat_g.clone()
             bn_snap = [t.clone() for t in self.bn_buffers]          # the warm-up must not count as a step
             cur = torch.cuda.current_stream()
             side = torch.cuda.Stream()
             side.wait_stream(cur)
             with torch.cuda.stream(side):          # warm-up outside capture: lazy kernel attributes, cached tables
-                self._micro(sx, sm, st, stl)
+                self._micro(static)
             cur.wait_stream(side)
             self.flat_g.copy_(snap)
             for t, v in zip(self.bn_buffers, bn_snap):
@@ -793,34 +818,45 @@ class FusedTrainer:
             graph = torch.cuda.CUDAGraph()
             n0 = ops.COUNTERS['launches']
             with torch.cuda.graph(graph):
-                loss = self._micro(sx, sm, st, stl)
+                loss = self._micro(static)
             launches = ops.COUNTERS['launches'] - n0
             ops.COUNTERS['launches'] = n0           # capture records, it does not launch
-            ent = (graph, sx, sm, st, loss, launches, stl)
+            ent = (graph, static, loss, launches)
         self._graphs[key] = ent       # (re-)insert as most recently used
         return ent
 
-    def step(self, inputs, mask, truth, truth_length=None):
+    def step(self, inputs, *batch, truth_length=None):
         """One micro-batch; every `accum_steps` calls an optimizer step.  Returns the (un-scaled) loss tensor.
-        truth_length (targets['targets_length']) is needed by joint-CTC models only."""
+        SpeechToText: step(inputs, mask, truth, truth_length=None); truth_length (targets['targets_length']) is needed by
+        joint-CTC models only.  TransformerLanguageModel: step(inputs, targets), i64 [N, L] each (the reference's
+        inputs['inputs'] and targets['targets'])."""
+        if self._lm_forward_backward is not None:
+            if len(batch) != 1 or truth_length is not None:
+                raise TypeError('FusedTrainer.step(inputs, targets) for a language model')
+            batch = (inputs, batch[0])
+        else:
+            if len(batch) == 3:
+                batch, truth_length = batch[:2], batch[2]
+            if len(batch) != 2:
+                raise TypeError('FusedTrainer.step(inputs, mask, truth, truth_length=None) for a SpeechToText model')
+            # forward_backward reads the label counts as int32
+            batch = (inputs,) + batch + (None if truth_length is None else truth_length.to(torch.int32),)
         with torch.no_grad():
             # data parallel: BatchNorm running statistics follow the first rank's (DistributedDataParallel's
             # broadcast_buffers): each rank's forward updates them from its own shard, so they would drift apart
             broadcast_from_first_(self.bn_buffers, self.group)
-            ent = self._graph_for(inputs, mask, truth, truth_length) if self.use_graph else None
+            ent = self._graph_for(batch) if self.use_graph else None
             if ent is not None:
-                graph, sx, sm, st, loss, launches, stl = ent
-                sx.copy_(inputs)
-                sm.copy_(mask)
-                st.copy_(truth)
-                if stl is not None:
-                    stl.copy_(truth_length)
+                graph, static, loss, launches = ent
+                for s, t in zip(static, batch):
+                    if s is not None:
+                        s.copy_(t)
                 graph.replay()
                 ops.COUNTERS['launches'] += launches
                 if self.bn_buffers:
                     modules.bump_param_generation()     # the replay moved the running statistics
             else:
-                loss = self._micro(inputs, mask, truth, truth_length)
+                loss = self._micro(batch)
             self.micro += 1
             if self.micro % self.accum_steps == 0:
                 # the one exchange step of data-parallel training (SURVEY.md 8e): mean of the flat gradient over ranks,
