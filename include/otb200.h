@@ -344,6 +344,23 @@ int otb_ctc_loss(const float* logp, int ldl, int B, int T, int V, const int32_t*
                  const int32_t* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, void* dlogits_bf16, int ldd,
                  float grad_scale, void* stream);
 
+/* CTC decoding (CTCRecognizer, recognize/ctc.py) on the CTC head's logits f32 [B*T, ld]; in_len i32 [B] valid frames.
+ * otb_ctc_frame_topk: per frame, the K (1..min(64, V)) best tokens as log-probs (log-softmax over the first V columns), best
+ *   first, ties to the lower index: top_lp f32 [B*T, K], top_id i32 [B*T, K]; frames at or past in_len, and ranks beyond
+ *   the number of non-NaN logits of a row, get -inf / -1 (the greedy and beam kernels skip id -1).
+ * otb_ctc_greedy: the greedy collapse on top_id[:, 0] (row pitch ldk): a frame's token is kept unless it is 0 (PAD), blank,
+ *   or the previous frame's token.  ids i32 [B, T] (compacted, 0 after the end), lengths i32 [B], scores f32 [B] = sum of
+ *   the best log-probs over the valid frames.
+ * otb_ctc_prefix_beam: CTC prefix beam search (no LM) over each frame's top-K tokens, beam 1..16, one CTA per utterance.
+ *   nodes i32 [B, 1 + T*beam, 2] workspace (back-pointer table); ids i32 [B, beam, T] best first (0 after the end),
+ *   lengths i32 [B, beam], scores f32 [B, beam] = log(p_blank + p_nonblank) (-inf for unused slots). */
+int otb_ctc_frame_topk(const float* logits, int ld, int B, int T, int V, const int32_t* in_len, int K, float* top_lp,
+                       int32_t* top_id, void* stream);
+int otb_ctc_greedy(const float* top_lp, const int32_t* top_id, int ldk, int B, int T, const int32_t* in_len, int blank,
+                   int32_t* ids, int32_t* lengths, float* scores, void* stream);
+int otb_ctc_prefix_beam(const float* top_lp, const int32_t* top_id, int K, int B, int T, const int32_t* in_len, int blank, int beam,
+                        int32_t* nodes, int32_t* ids, int32_t* lengths, float* scores, void* stream);
+
 /* Conv2d front end backward (frontend/conv.py:50-76 under autograd).  h1 = conv1 activation buffer (layout of
  * otb_conv1_relu).  col bf16 [B*T2*F2, 9*C1] = im2col of h1 for conv2 (k = (kh*3+kw)*C1 + c): conv2's weight gradient is
  * otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu folds dcol

@@ -467,6 +467,26 @@ int otb_ctc_loss(const float* logp, int ldl, int B, int T, int V, const int32_t*
                                    blank, nll, loss, ws, reinterpret_cast<bf16*>(dlogits_bf16), ldd, grad_scale));
 }
 
+int otb_ctc_frame_topk(const float* logits, int ld, int B, int T, int V, const int32_t* in_len, int K, float* top_lp,
+                       int32_t* top_id, void* stream) {
+    if (!logits || !in_len || !top_lp || !top_id) return fail("otb_ctc_frame_topk", "null operand");
+    if (ld < V) return fail("otb_ctc_frame_topk", "row pitch < V");
+    RET("otb_ctc_frame_topk", ctc_frame_topk_launch(ST(stream), logits, ld, B, T, V, in_len, K, top_lp, top_id));
+}
+
+int otb_ctc_greedy(const float* top_lp, const int32_t* top_id, int ldk, int B, int T, const int32_t* in_len, int blank,
+                   int32_t* ids, int32_t* lengths, float* scores, void* stream) {
+    if (!top_lp || !top_id || !in_len || !ids || !lengths || !scores) return fail("otb_ctc_greedy", "null operand");
+    RET("otb_ctc_greedy", ctc_greedy_launch(ST(stream), top_lp, top_id, ldk, B, T, in_len, blank, ids, lengths, scores));
+}
+
+int otb_ctc_prefix_beam(const float* top_lp, const int32_t* top_id, int K, int B, int T, const int32_t* in_len, int blank, int beam,
+                        int32_t* nodes, int32_t* ids, int32_t* lengths, float* scores, void* stream) {
+    if (!top_lp || !top_id || !in_len || !nodes || !ids || !lengths || !scores) return fail("otb_ctc_prefix_beam", "null operand");
+    RET("otb_ctc_prefix_beam", ctc_prefix_beam_launch(ST(stream), top_lp, top_id, K, B, T, in_len, blank, beam, nodes, ids,
+                                                      lengths, scores));
+}
+
 int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
     int T1, F1, T2, F2;
     if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;

@@ -20,13 +20,6 @@ namespace otb {
 
 static constexpr int CTC_SMAX = 129;   // 2 * 64 + 1 states
 
-__device__ __forceinline__ float log_add(float a, float b) {
-    if (a == -INFINITY) return b;
-    if (b == -INFINITY) return a;
-    const float m = fmaxf(a, b);
-    return m + log1pf(expf(fminf(a, b) - m));
-}
-
 __global__ void __launch_bounds__(160) ctc_alpha_beta_kernel(const float* __restrict__ logp, int ldl, int T, const int* __restrict__ in_len,
                                                              const long long* __restrict__ targets, int ldt,
                                                              const int* __restrict__ tgt_len, int blank, int V, float* __restrict__ nll,

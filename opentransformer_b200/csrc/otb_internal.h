@@ -195,6 +195,12 @@ const char* ls_ce_launch(cudaStream_t st, const float* logits, int ldl, const lo
 const char* ctc_launch(cudaStream_t st, const float* logp, int ldl, int B, int T, int V, const int* in_len, const long long* targets,
                        int ldt, const int* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, bf16* dlogits, int ldd,
                        float grad_scale);
+const char* ctc_frame_topk_launch(cudaStream_t st, const float* logits, int ld, int B, int T, int V, const int* in_len, int K,
+                                  float* top_lp, int* top_id);
+const char* ctc_greedy_launch(cudaStream_t st, const float* top_lp, const int* top_id, int ldk, int B, int T, const int* in_len,
+                              int blank, int* ids, int* lengths, float* scores);
+const char* ctc_prefix_beam_launch(cudaStream_t st, const float* top_lp, const int* top_id, int K, int B, int T, const int* in_len,
+                                   int blank, int beam, int* nodes, int* ids, int* lengths, float* scores);
 
 const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const int* n_samples, int B, const float* window,
                          const float* bank, const int* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift,

@@ -186,6 +186,13 @@ __device__ __forceinline__ float warp_max(float v) {
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
+// log(e^a + e^b) in fp32, exact at -inf: the CTC log-add (csrc/ctc.cu's loss, csrc/ctc_decode.cu's prefix beam search)
+__device__ __forceinline__ float log_add(float a, float b) {
+    if (a == -INFINITY) return b;
+    if (b == -INFINITY) return a;
+    const float m = fmaxf(a, b);
+    return m + log1pf(expf(fminf(a, b) - m));
+}
 // 2^x with one MUFU op (flushes denormals; ex2(-inf) = 0)
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;

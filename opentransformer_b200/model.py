@@ -131,4 +131,72 @@ class SpeechToText(nn.Module):
         pass
 
 
-End2EndModel = {'speech2text': SpeechToText}
+class CTCModel(nn.Module):
+    """model/ctc.py:69-131: conv front end + encoder + CTCAssistor, trained with nn.CTCLoss(blank 0, 'mean', zero_infinity)
+    on truth[:, 1:-1] (no <S/E>) with targets_length - 1 labels.  Submodules `frontend`, `encoder`, `assistor`: the
+    reference's state_dict keys and checkpoint sections.
+
+    forward: train() with gradients -> one autograd node over the hand-written backward (train.ctc_forward_backward);
+    train() without gradients -> the training-mode forward (a Conformer's BatchNorm uses the batch statistics); eval() ->
+    the fused inference path (encode_bf16, head GEMM, otb_ctc_loss)."""
+
+    def __init__(self, params):
+        super().__init__()
+        self.params = params
+        self.frontend = BuildFrontEnd[params['frontend_type']](**params['frontend'])
+        self.encoder = BuildEncoder[params['encoder_type']](**params['encoder'])
+        self.vocab_size = params['vocab_size']
+        self.assistor = CTCAssistor(hidden_size=params['encoder_output_size'], vocab_size=self.vocab_size,
+                                    lookahead_steps=params['lookahead_steps'] if 'lookahead_steps' in params else -1)
+
+    encode_bf16 = SpeechToText.encode_bf16
+
+    def logits_bf16(self, inputs, mask):
+        """front end + encoder + CTC head -> (logits f32 [B*T', ld] (first V columns valid), lengths i32 [B], B, T')."""
+        mem, lengths, B, T2 = self.encode_bf16(inputs, mask)
+        return self.assistor.logits_bf16(mem), lengths, B, T2
+
+    def forward(self, inputs, targets):
+        """CTCModel.forward (model/ctc.py:83-96) -> (loss, None).  targets['targets_length'] (label count including <S/E>,
+        data/loader.py:94) is required."""
+        truth, tlen = targets['targets'], targets.get('targets_length')
+        if tlen is None:
+            raise ValueError("CTCModel needs targets['targets_length'] (label count including <S/E>, data/loader.py:94)")
+        from . import train
+        if self.training and torch.is_grad_enabled():
+            loss, _ = train.loss_with_grad(self, inputs['inputs'], inputs['mask'], truth, tlen)
+            return loss, None
+        if self.training:
+            loss, _ = train.loss_train_mode(self, inputs['inputs'], inputs['mask'], truth, tlen)
+            return loss, None
+        logits, lengths, B, T2 = self.logits_bf16(inputs['inputs'], inputs['mask'])
+        tl = (tlen.to(logits.device).to(torch.int32) - 1).contiguous()
+        loss, _, _ = ops.ctc_loss(logits, B, T2, self.vocab_size, lengths, truth[:, 1:-1].contiguous(), tl, self.assistor.blank)
+        return loss, None
+
+    def inference(self, inputs, inputs_mask):
+        """-> (log_probs f32 [B, T', V], lengths i32 [B]) of front end + encoder + head.  The reference's CTCModel.inference
+        (model/ctc.py:98-103) skips the front end and unpacks the encoder's three return values into two, so it cannot run;
+        this is what it evidently intends (DESIGN.md 6)."""
+        logits, lengths, B, T2 = self.logits_bf16(inputs, inputs_mask)
+        return ops.log_softmax(logits, self.vocab_size).view(B, T2, -1), lengths
+
+    recognize = inference
+
+    def save_checkpoint(self, params, name):
+        torch.save({'params': params, 'frontend': self.frontend.state_dict(), 'encoder': self.encoder.state_dict(),
+                    'ctc': self.assistor.state_dict()}, name)
+
+    def load_model(self, chkpt):
+        """eval.py:36-57 for a CTC checkpoint: sections 'frontend' (when present), 'encoder' and 'ctc'."""
+        if 'frontend' in chkpt:
+            self.frontend.load_state_dict(chkpt['frontend'])
+        self.encoder.load_state_dict(chkpt['encoder'])
+        if 'ctc' in chkpt:
+            self.assistor.load_state_dict(chkpt['ctc'])
+
+    def set_epoch(self, epoch):
+        pass
+
+
+End2EndModel = {'ctc': CTCModel, 'speech2text': SpeechToText}

@@ -630,6 +630,63 @@ def ctc_loss(logits, B, T, V, in_len, targets, tgt_len, blank=0, want_grad=False
     return loss[0], nll, dl
 
 
+def ctc_frame_topk(logits, B, T, V, in_len, K):
+    """Per frame of logits f32 [B*T, ld]: the K best tokens' log-probs (log-softmax over V) and ids, best first, ties to the
+    lower id (otb_ctc_frame_topk).  -> (top_lp f32 [B*T, K], top_id i32 [B*T, K]); frames at or past in_len: -inf / -1."""
+    if logits.dim() != 2 or logits.shape[0] != B * T or logits.shape[1] < V:
+        raise ValueError(f'ctc_frame_topk: logits must be [B*T = {B * T}, >= V = {V}], got {tuple(logits.shape)}')
+    _ctc_lengths(in_len, B)
+    _need(logits, torch.float32, 'logits'); _need(in_len, torch.int32, 'in_len')
+    dev = logits.device
+    lp = torch.empty(B * T, K, dtype=torch.float32, device=dev)
+    ids = torch.empty(B * T, K, dtype=torch.int32, device=dev)
+    check(_lib.lib().otb_ctc_frame_topk(_p(logits), logits.stride(0), B, T, V, _p(in_len), K, _p(lp), _p(ids), _stream()),
+          'otb_ctc_frame_topk')
+    _count()
+    return lp, ids
+
+
+def _ctc_lengths(in_len, B):
+    if in_len.dim() != 1 or in_len.shape[0] != B:
+        raise ValueError(f'in_len must be [B = {B}], got {tuple(in_len.shape)}')
+
+
+def _ctc_topk_pair(top_lp, top_id, B, T, in_len):
+    """top_lp / top_id: the [B*T, K] pair of ctc_frame_topk."""
+    if top_id.dim() != 2 or top_id.shape[0] != B * T or top_lp.shape != top_id.shape:
+        raise ValueError(f'top_lp and top_id must both be [B*T = {B * T}, K], got {tuple(top_lp.shape)} and {tuple(top_id.shape)}')
+    _ctc_lengths(in_len, B)
+    _need(top_lp, torch.float32, 'top_lp'); _need(top_id, torch.int32, 'top_id'); _need(in_len, torch.int32, 'in_len')
+
+
+def ctc_greedy(top_lp, top_id, B, T, in_len, blank=0):
+    """Greedy CTC collapse of the best token per frame (otb_ctc_greedy).  -> (ids i32 [B, T], lengths i32 [B], scores f32 [B])."""
+    _ctc_topk_pair(top_lp, top_id, B, T, in_len)
+    dev = top_lp.device
+    ids = torch.empty(B, T, dtype=torch.int32, device=dev)
+    lengths = torch.empty(B, dtype=torch.int32, device=dev)
+    scores = torch.empty(B, dtype=torch.float32, device=dev)
+    check(_lib.lib().otb_ctc_greedy(_p(top_lp), _p(top_id), top_id.shape[1], B, T, _p(in_len), blank, _p(ids), _p(lengths),
+                                    _p(scores), _stream()), 'otb_ctc_greedy')
+    _count()
+    return ids, lengths, scores
+
+
+def ctc_prefix_beam(top_lp, top_id, B, T, in_len, beam, blank=0):
+    """CTC prefix beam search over each frame's top-K tokens (otb_ctc_prefix_beam), one launch for the batch.
+    -> (ids i32 [B, beam, T] best first, lengths i32 [B, beam], scores f32 [B, beam])."""
+    _ctc_topk_pair(top_lp, top_id, B, T, in_len)
+    dev = top_lp.device
+    nodes = torch.empty(B, 1 + T * beam, 2, dtype=torch.int32, device=dev)
+    ids = torch.empty(B, beam, T, dtype=torch.int32, device=dev)
+    lengths = torch.empty(B, beam, dtype=torch.int32, device=dev)
+    scores = torch.empty(B, beam, dtype=torch.float32, device=dev)
+    check(_lib.lib().otb_ctc_prefix_beam(_p(top_lp), _p(top_id), top_id.shape[1], B, T, _p(in_len), blank, beam, _p(nodes), _p(ids),
+                                         _p(lengths), _p(scores), _stream()), 'otb_ctc_prefix_beam')
+    _count()
+    return ids, lengths, scores
+
+
 def conv_im2col(h1, B, T, F, C1):
     _, _, T2, F2 = conv_geometry(T, F)
     col = torch.empty(B * T2 * F2, 9 * C1, dtype=BF16, device=h1.device)

@@ -350,11 +350,59 @@ class SpeechToTextRecognizer(Recognizer):
         return self.nbest_translate(preds), scores
 
 
+CTC_CUTOFF_TOP_N = 40      # ctcdecode's cutoff_top_n default (cutoff_prob 1.0), which recognize/ctc.py:20-24 leaves in place
+
+
+class CTCRecognizer(Recognizer):
+    """otrans/recognize/ctc.py:7-76 on the CUDA path: CTCModel.inference's head logits -> otb_ctc_frame_topk -> the greedy
+    collapse (otb_ctc_greedy, mode 'greedy') or the CTC prefix beam search (otb_ctc_prefix_beam, mode 'beam': ctcdecode's
+    search without a scorer, over each frame's 40 best tokens).  `lm` is stored and never used, as in the reference;
+    `alpha` / `beta` are ignored, as ctcdecode ignores them without an n-gram scorer, and an n-gram LM (`ngram_lm`,
+    KenLM) is refused."""
+
+    def __init__(self, model, lm=None, lm_weight=0.1, ngram_lm=None, beam_width=5, idx2unit=None, ngpu=1, mode='greedy',
+                 alpha=0.1, beta=0.0):
+        if ngram_lm is not None:
+            raise NotImplementedError('CTCRecognizer: n-gram LM scoring (KenLM) is not implemented; use ngram_lm=None')
+        if mode not in ('greedy', 'beam'):
+            raise ValueError(f"CTCRecognizer: mode must be 'greedy' or 'beam', got {mode!r}")
+        if mode == 'beam' and not 1 <= beam_width <= 16:
+            raise NotImplementedError(f'CTCRecognizer: the prefix beam search takes beam_width 1..16, got {beam_width}')
+        super().__init__(model, idx2unit, lm, lm_weight, ngpu)
+        self.beam_width, self.mode = beam_width, mode
+        self.alpha, self.beta = alpha, beta
+
+    def recognize_ids(self, inputs, inputs_mask):
+        """-> (ids i64 [B, nbest, T'] best first, 0 after each hypothesis' end; lengths i32 [B, nbest]; scores f32 [B, nbest]),
+        on the device.  nbest is 1 in greedy mode (score: the best path's log-prob) and beam_width in beam mode (score:
+        the prefix's log-probability over all its alignments)."""
+        with torch.no_grad():
+            logits, lengths, B, T2 = self.model.logits_bf16(inputs, inputs_mask)
+            V = self.model.vocab_size
+            if self.mode == 'greedy':
+                lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, 1)
+                ids, n, sc = ops.ctc_greedy(lp, tok, B, T2, lengths, self.model.assistor.blank)
+                return ids.long().view(B, 1, T2), n.view(B, 1), sc.view(B, 1)
+            lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, min(CTC_CUTOFF_TOP_N, V))
+            ids, n, sc = ops.ctc_prefix_beam(lp, tok, B, T2, lengths, self.beam_width, self.model.assistor.blank)
+            return ids.long(), n, sc
+
+    def recognize(self, inputs, inputs_mask):
+        """recognize/ctc.py:27-36: translate() of the 1-best token lists (the id lists when idx2unit is None)."""
+        ids, n, _ = self.recognize_ids(inputs, inputs_mask)
+        best = [row[:k] for row, k in zip(ids[:, 0].cpu().tolist(), n[:, 0].cpu().tolist())]
+        return best if self.idx2unit is None else self.translate(best)
+
+
 def build_recognizer(model_type, model, lm, args, idx2unit):
-    """otrans/recognize/__init__.py:5-16 (speech2text only; CTC is out of scope, SURVEY.md 2)."""
+    """otrans/recognize/__init__.py:5-21."""
     if model_type == 'speech2text':
         return SpeechToTextRecognizer(
             model=model, lm=lm, lm_weight=args.lm_weight, ctc_weight=args.ctc_weight, beam_width=args.beam_width,
             nbest=args.nbest, max_len=args.max_len, idx2unit=idx2unit, penalty=args.penalty, lamda=args.lamda,
             ngpu=args.ngpu)
+    if model_type == 'ctc':
+        return CTCRecognizer(
+            model=model, lm=lm, lm_weight=args.lm_weight, ngram_lm=args.ngram_lm, beam_width=args.beam_width,
+            idx2unit=idx2unit, ngpu=args.ngpu, mode=args.mode, alpha=args.alpha, beta=args.beta)
     raise NotImplementedError(model_type)

@@ -18,6 +18,8 @@ otherwise.  The encoder may also be the shipped Conformer layout with 64-wide he
 attention, then the convolution module with training-mode BatchNorm; encoder/conformer.py:75-89).
 The Transformer language model (lm.transformer_forward_backward) trains through the encoder layer's forward and backward
 below with the causal mask, and FusedTrainer takes it as well.
+The CTC-only model (model.CTCModel, model/ctc.py) trains through the same front-end + encoder halves (_encoder_fwd /
+_encoder_bwd) with the CTC head and otb_ctc_loss in place of the decoder (ctc_forward_backward).
 """
 import math
 from collections import namedtuple
@@ -68,19 +70,24 @@ class LayerPack:
                 'ln1': self._ln(b.norm1), 'ln2': self._ln(b.norm2), 'act': f.activation}
 
 
-class TrainPack(LayerPack):
-    """The LayerPack of a SpeechToText model: front end, encoder and decoder layers and the output layer."""
+class EncoderPack(LayerPack):
+    """The LayerPack of the front end and the encoder: all a CTCModel trains, and the first half of a SpeechToText's
+    TrainPack.  `dec` (the SpeechToText's decoder) joins the checks, which run in one order for both models."""
 
-    def __init__(self, model, bf16_of=None):
+    def __init__(self, model, bf16_of=None, dec=None):
         super().__init__(model, bf16_of)
-        fe, enc, dec = model.frontend, model.encoder, model.decoder
+        fe, enc = model.frontend, model.encoder
         self.conformer = isinstance(enc, ConformerEncoder)
-        if not isinstance(fe, ConvFrontEnd) or not isinstance(enc, (TransformerEncoder, ConformerEncoder)) \
+        if dec is None:
+            if not isinstance(fe, ConvFrontEnd) or not isinstance(enc, (TransformerEncoder, ConformerEncoder)):
+                raise NotImplementedError('training path: conv front end + Transformer or Conformer encoder only')
+        elif not isinstance(fe, ConvFrontEnd) or not isinstance(enc, (TransformerEncoder, ConformerEncoder)) \
                 or not isinstance(dec, TransformerDecoder):
             raise NotImplementedError('training path: conv front end + Transformer or Conformer encoder + Transformer decoder only')
         if not self.conformer and enc.relative_positional:
             raise NotImplementedError('training path: the Transformer encoder with absolute positions only')
-        for name, d_model, blocks in (('encoder', enc.d_model, enc.blocks), ('decoder', dec.d_model, dec.blocks)):
+        stacks = [('encoder', enc.d_model, enc.blocks)] + ([('decoder', dec.d_model, dec.blocks)] if dec is not None else [])
+        for name, d_model, blocks in stacks:
             for blk in blocks:
                 if d_model != 64 * blk.n_heads:   # the attention backward (otb_attention_bwd) is written for 64-wide heads
                     raise NotImplementedError(f'training path: 64-wide attention heads only; the {name} has d_model {d_model} '
@@ -91,9 +98,9 @@ class TrainPack(LayerPack):
                                       'gradient takes at most 256')
         if self.conformer:
             _check_conformer(enc)
-        if fe.front_end_layer_norm or enc.pos_emb.scale_learnable or dec.pos_emb.scale_learnable:
+        if fe.front_end_layer_norm or enc.pos_emb.scale_learnable or (dec is not None and dec.pos_emb.scale_learnable):
             raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale (pos_dropout > 0)')
-        for blk in list(enc.blocks) + list(dec.blocks):
+        for blk in list(enc.blocks) + (list(dec.blocks) if dec is not None else []):
             if _ffn_of(blk).activation not in ('glu', 'relu'):
                 raise NotImplementedError('training path: GLU or ReLU feed-forward only')
             rates = getattr(blk, 'dropout_rates', {})
@@ -108,19 +115,9 @@ class TrainPack(LayerPack):
                 raise ValueError('residual_dropout must be in [0, 1)')
         self.fe = self._frontend(fe)
         self.enc = [self._conf_layer(b) if self.conformer else self._enc_layer(b) for b in enc.blocks]
-        self.dec = [self._dec_layer(b) for b in dec.blocks]
         # pre-norm stacks end with one more LayerNorm (encoder/transformer.py:96-97,131-132; decoder/transformer.py:151-152,178-179)
-        self.enc_pre, self.dec_pre = bool(getattr(enc, 'normalize_before', False)), bool(dec.normalize_before)
+        self.enc_pre = bool(getattr(enc, 'normalize_before', False))
         self.enc_norm = self._ln(enc.norm) if self.enc_pre else None
-        self.dec_norm = self._ln(dec.after_norm) if self.dec_pre else None
-        V, d = dec.vocab_size, dec.d_model
-        self.ld_logits = dec.ld_logits
-        emb = self._w(dec.embedding.weight)
-        self.tied = dec.output_layer.weight is dec.embedding.weight
-        wout = emb if self.tied else self._w(dec.output_layer.weight)
-        wout_t = torch.zeros(d, self.ld_logits, dtype=BF16, device=emb.device)      # [d, V padded]: dgrad of the logits GEMM
-        wout_t[:, :V] = wout.t()
-        self.out = {'emb': emb, 'wout': wout, 'wout_t': wout_t, 'bout': _f(dec.output_layer.bias)}
 
     def _frontend(self, fe):
         pk = dict(fe._build_pack())
@@ -146,6 +143,25 @@ class TrainPack(LayerPack):
                 'dw': _f(dw.weight).view(d, -1), 'dwb': _f(dw.bias), 'dw_name': self._names[dw],
                 'bn': bn, 'bn_g': _f(bn.weight), 'bn_b': _f(bn.bias), 'bn_name': self._names[bn],
                 'post_ln': self._ln(b.post_ffn_norm), 'final_ln': self._ln(b.final_norm)}
+
+
+class TrainPack(EncoderPack):
+    """The LayerPack of a SpeechToText model: front end, encoder and decoder layers and the output layer."""
+
+    def __init__(self, model, bf16_of=None):
+        super().__init__(model, bf16_of, dec=model.decoder)
+        dec = model.decoder
+        self.dec = [self._dec_layer(b) for b in dec.blocks]
+        self.dec_pre = bool(dec.normalize_before)
+        self.dec_norm = self._ln(dec.after_norm) if self.dec_pre else None
+        V, d = dec.vocab_size, dec.d_model
+        self.ld_logits = dec.ld_logits
+        emb = self._w(dec.embedding.weight)
+        self.tied = dec.output_layer.weight is dec.embedding.weight
+        wout = emb if self.tied else self._w(dec.output_layer.weight)
+        wout_t = torch.zeros(d, self.ld_logits, dtype=BF16, device=emb.device)      # [d, V padded]: dgrad of the logits GEMM
+        wout_t[:, :V] = wout.t()
+        self.out = {'emb': emb, 'wout': wout, 'wout_t': wout_t, 'bout': _f(dec.output_layer.bias)}
 
     def _dec_layer(self, b):
         a, c, f = b.slf_attn, b.src_attn, b.feed_forward
@@ -253,7 +269,7 @@ def dropout_sites(model):
     n = _enc_sites(model.encoder)
     for i, b in enumerate(model.encoder.blocks):
         out += [(ENC_SITE + n * i + k, 'encoder', float(b.dropout_rates['residual_dropout'])) for k in range(n)]
-    for i, b in enumerate(model.decoder.blocks):
+    for i, b in enumerate(model.decoder.blocks if getattr(model, 'decoder', None) is not None else []):
         out += [(DEC_SITE + 3 * i + k, 'decoder', float(b.dropout_rates['residual_dropout'])) for k in range(3)]
     return out
 
@@ -488,40 +504,25 @@ def _embedding_bwd(tok, dx, dwout, scale, tied, g, emb_name, out_name):
         g[emb_name] = demb
 
 
-def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True, grad_sink=None, grad_scale=1.0,
-                     bf16_of=None, drop_seed=None, truth_length=None, return_ctc=False):
-    """One forward (+ backward) pass.  inputs f32 [B,T,F], mask bool [B,T], truth i64 [B,L+1] (BOS ... EOS PAD*).
-    Returns (loss 0-d f32 tensor, {parameter name -> fp32 gradient}) with names as in model.named_parameters().
-    grad_sink: name -> fp32 tensor the gradients (x grad_scale) are ADDED into (gradient accumulation buffer).
-    drop_seed: int32 device tensor [1], the dropout seed of THIS pass (read on the device); required when any
-    residual_dropout rate is non-zero.  truth_length: i32/i64 [B] label counts incl. <S/E> (targets['targets_length'],
-    data/loader.py:94) -- required when model.ctc_weight > 0: the loss is then (1 - w) * attention + w * CTC
-    (model/speech2text.py:60-62) and the CTC head's gradients flow into the encoder through the memory."""
-    fe, enc, dec = model.frontend, model.encoder, model.decoder
-    ctc_w = float(getattr(model, 'ctc_weight', 0.0) or 0.0)
-    if ctc_w > 0.0 and truth_length is None:
-        raise ValueError('forward_backward: ctc_weight > 0 needs truth_length')
-    pk = TrainPack(model, bf16_of)
+_EncTrace = namedtuple('_EncTrace', 'x_in h1 h2 tape pe scale lengths enc_last drops B T F T2 F2')
+
+
+def _encoder_fwd(model, pk, inputs, mask, e_rates, drop_seed):
+    """Front end + encoder in training mode, the half shared by SpeechToText and CTCModel -> (memory bf16 [B*T', d],
+    _EncTrace: what _encoder_bwd reads)."""
+    fe, enc = model.frontend, model.encoder
     dev = inputs.device
     conformer = pk.conformer
-    e_rates = [float(b.dropout_rates['residual_dropout']) for b in enc.blocks]
-    d_rates = [float(b.dropout_rates['residual_dropout']) for b in dec.blocks]
-    if drop_seed is None and any(r > 0.0 for r in e_rates + d_rates):
-        raise ValueError('forward_backward: residual_dropout > 0 needs a drop_seed tensor')
     B, T, F = inputs.shape
-    H, d = enc.blocks[0].n_heads, enc.d_model
+    H = enc.blocks[0].n_heads
     x_in = inputs.contiguous().float()
     _, _, T2, F2 = ops.conv_geometry(T, F)
-    T1, F1 = (T - 3) // 2 + 1, (F - 1) // 2 + 1
     lengths = _lengths(fe.output_mask(mask))
     fpk = pk.fe
-    C1p, C2 = fpk['C1p'], fpk['w2'].shape[0]
-
-    # ------------------------------------------------------------------ forward
     h1 = ops.conv1_relu(x_in, fpk['w1'], fpk['b1'])
     h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F)                       # [B*T2, F2*C2]
-    fused_pe = enc.fuse_abs_posenc()
-    if fused_pe:
+    scale = None
+    if enc.fuse_abs_posenc():
         scale, table = enc.pos_emb.scale_and_table(T2, dev)
         x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_TABLE, alpha=scale, table=table, period=T2)
     else:               # rel-pos encoders take the front end's output as is (encoder/conformer.py:141-149)
@@ -538,8 +539,94 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
         enc_tape.append(t)
     if conformer:       # the running statistics moved: the inference pack, which folds BatchNorm, must be rebuilt
         modules.bump_param_generation()
-    enc_last = x
     mem = _norm(x, pk.enc_norm) if pk.enc_pre else x
+    return mem, _EncTrace(x_in=x_in, h1=h1, h2=h2, tape=enc_tape, pe=pe, scale=scale, lengths=lengths, enc_last=x, drops=e_drop,
+                          B=B, T=T, F=F, T2=T2, F2=F2)
+
+
+def _encoder_bwd(model, pk, tr, dx, g):
+    """Backward of _encoder_fwd from dx = the gradient of the memory (bf16 [B*T', d]): encoder layers in reverse, then the
+    front end.  Parameter gradients go into g."""
+    fe, enc = model.frontend, model.encoder
+    acc = g.sink is not None
+    B, T, F, T2, F2 = tr.B, tr.T, tr.F, tr.T2, tr.F2
+    H = enc.blocks[0].n_heads
+    fpk = pk.fe
+    C1p, C2 = fpk['C1p'], fpk['w2'].shape[0]
+    if pk.enc_pre:
+        dx = _ln_bwd(dx, tr.enc_last, pk.enc_norm, g)
+    for i in reversed(range(len(pk.enc))):
+        if pk.conformer:
+            dx = _conformer_block_bwd(pk.enc[i], tr.tape[i], dx, g, B, H, T2, tr.lengths, tr.pe, tr.drops[i])
+        else:
+            dx = _enc_layer_bwd(pk.enc[i], tr.tape[i], dx, pk.enc_pre, g, B, H, T2, tr.lengths, tr.drops[i])
+
+    # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE (abs-pos; rel-pos: x = h2 Wo^T + bo) -> conv2 (implicit-GEMM forward,
+    # im2col GEMMs backward) -> conv1
+    h1, h2 = tr.h1, tr.h2
+    dyl = ops.scale_add_table(dx, tr.scale) if tr.scale is not None else dx      # d(h2 Wo^T + bo) = sqrt(d) * dx
+    D_out = fe.output_size
+    dwo = ops.linear_wgrad(dyl, h2)                                               # [D, F2*C2], feature index f*C2 + c
+    g.put('frontend.output_layer.weight', dwo.view(D_out, F2, C2).permute(0, 2, 1).reshape(D_out, C2 * F2))
+    g['frontend.output_layer.bias'] = ops.colsum(dyl, out=g.out('frontend.output_layer.bias'), accumulate=acc)
+    dh2 = ops.linear(dyl, fpk['wo_t'])                                            # [B*T2, F2*C2]
+    dpre2 = ops.relu_bwd(dh2, h2).view(B * T2 * F2, C2)
+    col = ops.conv_im2col(h1, B, T, F, C1p)
+    C1 = fe.conv1.conv_layer.out_channels
+    dw2 = ops.linear_wgrad(dpre2, col)                                            # [C2, 9*C1p], k = (kh*3+kw)*C1p + c
+    g.put('frontend.conv2.conv_layer.weight', dw2.view(C2, 3, 3, C1p)[..., :C1].permute(0, 3, 1, 2))
+    g['frontend.conv2.conv_layer.bias'] = ops.colsum(dpre2, out=g.out('frontend.conv2.conv_layer.bias'), accumulate=acc)
+    dcol = ops.linear(dpre2, fpk['w2_t'])                                         # [B*T2*F2, 9*C1p]
+    del col
+    dpre1 = ops.conv_col2im_relu(dcol, h1, B, T, F, C1p)
+    g1 = ops.conv1_wgrad(dpre1, tr.x_in, B, T, F, C1p)                            # [C1p, 9 taps + bias]
+    g.put('frontend.conv1.conv_layer.weight', g1[:C1, :9].reshape(C1, 1, 3, 3))
+    g.put('frontend.conv1.conv_layer.bias', g1[:C1, 9])
+
+
+def _ctc_head_fwd(model, pk, mem):
+    """CTCAssistor's output layer on the memory (model/ctc.py:33-46) -> (logits f32 [B*T', ld], its bf16 weight)."""
+    wc = pk._w(model.assistor.output_layer.weight)
+    return ops.linear(mem, wc, _f(model.assistor.output_layer.bias), EPI_BIAS, out_f32=True, n_out=model.assistor.ld_logits), wc
+
+
+def _ctc_head_bwd(dctc, mem, wc, V, g, resid=None):
+    """Backward of _ctc_head_fwd from dctc (bf16 [B*T', ld]): the head's gradients into g; returns the gradient of the
+    memory (+ resid)."""
+    acc = g.sink is not None
+    wname_c = 'assistor.output_layer.weight'
+    g[wname_c] = ops.linear_wgrad(dctc[:, :V], mem, out=g.out(wname_c), accumulate=acc)
+    g.put('assistor.output_layer.bias', ops.colsum(dctc)[:V])
+    wc_t = torch.zeros(mem.shape[1], dctc.shape[1], dtype=BF16, device=mem.device)
+    wc_t[:, :V] = wc.t()
+    if resid is not None:
+        return ops.linear(dctc, wc_t, None, EPI_RESID, resid=resid)
+    return ops.linear(dctc, wc_t)
+
+
+def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True, grad_sink=None, grad_scale=1.0,
+                     bf16_of=None, drop_seed=None, truth_length=None, return_ctc=False):
+    """One forward (+ backward) pass.  inputs f32 [B,T,F], mask bool [B,T], truth i64 [B,L+1] (BOS ... EOS PAD*).
+    Returns (loss 0-d f32 tensor, {parameter name -> fp32 gradient}) with names as in model.named_parameters().
+    grad_sink: name -> fp32 tensor the gradients (x grad_scale) are ADDED into (gradient accumulation buffer).
+    drop_seed: int32 device tensor [1], the dropout seed of THIS pass (read on the device); required when any
+    residual_dropout rate is non-zero.  truth_length: i32/i64 [B] label counts incl. <S/E> (targets['targets_length'],
+    data/loader.py:94) -- required when model.ctc_weight > 0: the loss is then (1 - w) * attention + w * CTC
+    (model/speech2text.py:60-62) and the CTC head's gradients flow into the encoder through the memory."""
+    enc, dec = model.encoder, model.decoder
+    ctc_w = float(getattr(model, 'ctc_weight', 0.0) or 0.0)
+    if ctc_w > 0.0 and truth_length is None:
+        raise ValueError('forward_backward: ctc_weight > 0 needs truth_length')
+    pk = TrainPack(model, bf16_of)
+    dev = inputs.device
+    e_rates = [float(b.dropout_rates['residual_dropout']) for b in enc.blocks]
+    d_rates = [float(b.dropout_rates['residual_dropout']) for b in dec.blocks]
+    if drop_seed is None and any(r > 0.0 for r in e_rates + d_rates):
+        raise ValueError('forward_backward: residual_dropout > 0 needs a drop_seed tensor')
+
+    # ------------------------------------------------------------------ forward
+    mem, tr = _encoder_fwd(model, pk, inputs, mask, e_rates, drop_seed)
+    B, T2, lengths, d = tr.B, tr.T2, tr.lengths, enc.d_model
 
     tgt_in = truth[:, :-1].contiguous()
     tgt_out = truth[:, 1:].contiguous()
@@ -560,8 +647,7 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     sm = model.smoothing if smoothing is None else smoothing
     loss_ctc, dctc = None, None
     if ctc_w > 0.0:     # CTCAssistor on the encoder states (model/ctc.py:33-52)
-        wc = pk._w(model.assistor.output_layer.weight)
-        ctc_logits = ops.linear(mem, wc, _f(model.assistor.output_layer.bias), EPI_BIAS, out_f32=True, n_out=model.assistor.ld_logits)
+        ctc_logits, wc = _ctc_head_fwd(model, pk, mem)
         loss_ctc, _, dctc = ops.ctc_loss(ctc_logits, B, T2, V, lengths, tgt_out, truth_length.to(torch.int32).to(dev).contiguous(),
                                          model.assistor.blank, want_grad=want_grads, grad_scale=ctc_w * grad_scale)
     if not want_grads:
@@ -578,7 +664,6 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
 
     # ------------------------------------------------------------------ backward
     g = _Grads(grad_sink)
-    acc = grad_sink is not None
     dwout, dy = _output_layer_bwd(dlogits, y, pk.out['wout_t'], V, pk.tied, g, 'decoder.embedding.weight', 'decoder.output_layer')
     dmem = None
     if pk.dec_pre:
@@ -590,41 +675,36 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
 
     dx = dmem
     if ctc_w > 0.0:     # CTC head: parameter gradients, and its gradient with respect to the memory joins the decoder's
-        wname_c = 'assistor.output_layer.weight'
-        g[wname_c] = ops.linear_wgrad(dctc[:, :V], mem, out=g.out(wname_c), accumulate=acc)
-        g.put('assistor.output_layer.bias', ops.colsum(dctc)[:V])
-        wc_t = torch.zeros(d, dctc.shape[1], dtype=BF16, device=dev)
-        wc_t[:, :V] = wc.t()
-        dx = ops.linear(dctc, wc_t, None, EPI_RESID, resid=dmem)
-    if pk.enc_pre:
-        dx = _ln_bwd(dx, enc_last, pk.enc_norm, g)
-    for i in reversed(range(len(pk.enc))):
-        if conformer:
-            dx = _conformer_block_bwd(pk.enc[i], enc_tape[i], dx, g, B, H, T2, lengths, pe, e_drop[i])
-        else:
-            dx = _enc_layer_bwd(pk.enc[i], enc_tape[i], dx, pk.enc_pre, g, B, H, T2, lengths, e_drop[i])
-
-    # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE (abs-pos; rel-pos: x = h2 Wo^T + bo) -> conv2 (implicit-GEMM forward,
-    # im2col GEMMs backward) -> conv1
-    dyl = ops.scale_add_table(dx, scale) if fused_pe else dx                      # d(h2 Wo^T + bo) = sqrt(d) * dx
-    D_out = fe.output_size
-    dwo = ops.linear_wgrad(dyl, h2)                                               # [D, F2*C2], feature index f*C2 + c
-    g.put('frontend.output_layer.weight', dwo.view(D_out, F2, C2).permute(0, 2, 1).reshape(D_out, C2 * F2))
-    g['frontend.output_layer.bias'] = ops.colsum(dyl, out=g.out('frontend.output_layer.bias'), accumulate=acc)
-    dh2 = ops.linear(dyl, fpk['wo_t'])                                            # [B*T2, F2*C2]
-    dpre2 = ops.relu_bwd(dh2, h2).view(B * T2 * F2, C2)
-    col = ops.conv_im2col(h1, B, T, F, C1p)
-    C1 = fe.conv1.conv_layer.out_channels
-    dw2 = ops.linear_wgrad(dpre2, col)                                            # [C2, 9*C1p], k = (kh*3+kw)*C1p + c
-    g.put('frontend.conv2.conv_layer.weight', dw2.view(C2, 3, 3, C1p)[..., :C1].permute(0, 3, 1, 2))
-    g['frontend.conv2.conv_layer.bias'] = ops.colsum(dpre2, out=g.out('frontend.conv2.conv_layer.bias'), accumulate=acc)
-    dcol = ops.linear(dpre2, fpk['w2_t'])                                         # [B*T2*F2, 9*C1p]
-    del col
-    dpre1 = ops.conv_col2im_relu(dcol, h1, B, T, F, C1p)
-    g1 = ops.conv1_wgrad(dpre1, x_in, B, T, F, C1p)                               # [C1p, 9 taps + bias]
-    g.put('frontend.conv1.conv_layer.weight', g1[:C1, :9].reshape(C1, 1, 3, 3))
-    g.put('frontend.conv1.conv_layer.bias', g1[:C1, 9])
+        dx = _ctc_head_bwd(dctc, mem, wc, V, g, resid=dmem)
+    _encoder_bwd(model, pk, tr, dx, g)
     return (loss, g, loss_ctc) if return_ctc else (loss, g)
+
+
+def ctc_forward_backward(model, inputs, mask, truth, truth_length, want_grads=True, grad_sink=None, grad_scale=1.0,
+                         bf16_of=None, drop_seed=None):
+    """CTCModel.forward (model/ctc.py:83-96) in training mode, and its backward: front end + encoder, the CTC head, and
+    nn.CTCLoss(blank 0, 'mean', zero_infinity) against truth[:, 1:-1] with truth_length - 1 labels -- the CTC-only model
+    drops <S/E>, joint CTC keeps it.  The loss gradient (x grad_scale) runs back through the head into the shared encoder
+    backward.  Arguments and return value as forward_backward's; truth_length is required."""
+    enc = model.encoder
+    if truth_length is None:
+        raise ValueError('ctc_forward_backward: a CTCModel needs truth_length')
+    pk = EncoderPack(model, bf16_of)
+    dev = inputs.device
+    e_rates = [float(b.dropout_rates['residual_dropout']) for b in enc.blocks]
+    if drop_seed is None and any(r > 0.0 for r in e_rates):
+        raise ValueError('ctc_forward_backward: residual_dropout > 0 needs a drop_seed tensor')
+    mem, tr = _encoder_fwd(model, pk, inputs, mask, e_rates, drop_seed)
+    V = model.vocab_size
+    logits, wc = _ctc_head_fwd(model, pk, mem)
+    tlen = (truth_length.to(dev).to(torch.int32) - 1).contiguous()
+    loss, _, dctc = ops.ctc_loss(logits, tr.B, tr.T2, V, tr.lengths, truth[:, 1:-1].contiguous(), tlen, model.assistor.blank,
+                                 want_grad=want_grads, grad_scale=grad_scale)
+    if not want_grads:
+        return loss, None
+    g = _Grads(grad_sink)
+    _encoder_bwd(model, pk, tr, _ctc_head_bwd(dctc, mem, wc, V, g), g)
+    return loss, g
 
 
 def _next_drop_seed(model, device):
@@ -637,14 +717,23 @@ def _next_drop_seed(model, device):
     return seed
 
 
+def _model_forward_backward(model, inputs, mask, truth, truth_length, **kw):
+    """forward_backward of a SpeechToText, ctc_forward_backward of a CTCModel -> (loss, grads, joint-CTC loss or None)."""
+    from .model import CTCModel
+    if isinstance(model, CTCModel):
+        loss, grads = ctc_forward_backward(model, inputs, mask, truth, truth_length, **kw)
+        return loss, grads, None
+    return forward_backward(model, inputs, mask, truth, truth_length=truth_length, return_ctc=True, **kw)
+
+
 class _SpeechToTextLoss(torch.autograd.Function):
-    """loss = SpeechToText.forward(...) as ONE autograd node over the fp32 master parameters."""
+    """loss = SpeechToText.forward(...) or CTCModel.forward(...) as ONE autograd node over the fp32 master parameters."""
 
     @staticmethod
     def forward(ctx, model, inputs, mask, truth, tlen, names, *params):
         with torch.no_grad():
             seed = _next_drop_seed(model, inputs.device)
-            loss, grads, ctc = forward_backward(model, inputs, mask, truth, drop_seed=seed, truth_length=tlen, return_ctc=True)
+            loss, grads, ctc = _model_forward_backward(model, inputs, mask, truth, tlen, drop_seed=seed)
         ctx.grads = [grads.get(n) for n in names]
         ctx.shapes = [p.shape for p in params]
         model._last_ctc_loss = ctc
@@ -659,7 +748,8 @@ class _SpeechToTextLoss(torch.autograd.Function):
 
 
 def loss_with_grad(model, inputs, mask, truth, truth_length=None):
-    """Training-mode SpeechToText.forward: (loss tensor whose .backward() fills `.grad` of every parameter, CTC loss or None)."""
+    """Training-mode SpeechToText.forward or CTCModel.forward: (loss tensor whose .backward() fills `.grad` of every parameter,
+    joint-CTC loss or None)."""
     named = [(n, p) for n, p in model.named_parameters() if p.requires_grad]
     names = [n for n, _ in named]
     loss = _SpeechToTextLoss.apply(model, inputs, mask, truth, truth_length, names, *[p for _, p in named])
@@ -667,12 +757,12 @@ def loss_with_grad(model, inputs, mask, truth, truth_length=None):
 
 
 def loss_train_mode(model, inputs, mask, truth, truth_length=None):
-    """Training-mode SpeechToText.forward without gradients (model.train() under torch.no_grad(), e.g. a validation loop
-    that does not call eval()): the forward the reference runs in train() -- for a Conformer, BatchNorm with the batch
-    statistics, and the running statistics updated -- with no backward.  -> (loss, CTC loss or None)."""
+    """Training-mode SpeechToText.forward or CTCModel.forward without gradients (model.train() under torch.no_grad(), e.g. a
+    validation loop that does not call eval()): the forward the reference runs in train() -- for a Conformer, BatchNorm with
+    the batch statistics, and the running statistics updated -- with no backward.  -> (loss, joint-CTC loss or None)."""
     with torch.no_grad():
-        loss, _, ctc = forward_backward(model, inputs, mask, truth, want_grads=False, drop_seed=_next_drop_seed(model, inputs.device),
-                                        truth_length=truth_length, return_ctc=True)
+        loss, _, ctc = _model_forward_backward(model, inputs, mask, truth, truth_length, want_grads=False,
+                                               drop_seed=_next_drop_seed(model, inputs.device))
     return loss, ctc
 
 
@@ -685,11 +775,12 @@ class FusedTrainer:
     """The inner step of Trainer.train_one_epoch (trainer.py:206-234) on flat fp32 buffers:
     forward + hand-written backward -> (data-parallel) gradient all-reduce over NCCL -> global-norm clip + Adam in two
     kernels, no host synchronisation.  Parameters become views into one flat buffer (state_dict keys / shapes unchanged).
-    `model` is a SpeechToText or a TransformerLanguageModel (transformer_lm.yaml trains with the same scheduler)."""
+    `model` is a SpeechToText, a CTCModel or a TransformerLanguageModel (transformer_lm.yaml trains with the same scheduler)."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6, clip_grad=5.0, model_size=256,
                  warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True):
         from . import lm          # lm imports this module
+        from .model import CTCModel
         if isinstance(model, lm.RecurrentLanguageModel):
             raise NotImplementedError('FusedTrainer: the recurrent LM trains with a step-linear scheduler that is not on the '
                                       'device; train it through loss.backward() and a torch optimizer')
@@ -697,6 +788,7 @@ class FusedTrainer:
         if isinstance(model, lm.TransformerLanguageModel):
             lm.check_trainable(model)
             self._lm_forward_backward = lm.transformer_forward_backward
+        self._ctc = isinstance(model, CTCModel)
         self.model = model
         # parameters the forward never reads (a Conformer's post_ffn) stay out of the flat buffers: no gradient, no weight decay
         unused = unused_parameters(model)
@@ -773,7 +865,7 @@ class FusedTrainer:
     def _micro(self, batch):
         """forward + backward of one micro-batch; gradients / accum_steps are ADDED into the flat buffer by the backward
         kernels themselves (no per-parameter add).  batch: (inputs, mask, truth, truth_length or None) of a SpeechToText,
-        (inputs, targets) of a language model."""
+        (inputs, targets) of a language model; a CTCModel's as a SpeechToText's."""
         self.flat_bf16.copy_(self.flat_p)
         self.drop_seed.add_(1)
         kw = dict(grad_sink=self.sink, grad_scale=1.0 / self.accum_steps, bf16_of=self._bf16_of, drop_seed=self.drop_seed)
@@ -781,7 +873,10 @@ class FusedTrainer:
             loss, _ = self._lm_forward_backward(self.model, *batch, **kw)
         else:
             inputs, mask, truth, tlen = batch
-            loss, _ = forward_backward(self.model, inputs, mask, truth, truth_length=tlen, **kw)
+            if self._ctc:
+                loss, _ = ctc_forward_backward(self.model, inputs, mask, truth, tlen, **kw)
+            else:
+                loss, _ = forward_backward(self.model, inputs, mask, truth, truth_length=tlen, **kw)
         return loss
 
     def _graph_for(self, batch):
@@ -828,8 +923,9 @@ class FusedTrainer:
     def step(self, inputs, *batch, truth_length=None):
         """One micro-batch; every `accum_steps` calls an optimizer step.  Returns the (un-scaled) loss tensor.
         SpeechToText: step(inputs, mask, truth, truth_length=None); truth_length (targets['targets_length']) is needed by
-        joint-CTC models only.  TransformerLanguageModel: step(inputs, targets), i64 [N, L] each (the reference's
-        inputs['inputs'] and targets['targets'])."""
+        joint-CTC models only.  CTCModel: step(inputs, mask, truth, truth_length), truth_length required.
+        TransformerLanguageModel: step(inputs, targets), i64 [N, L] each (the reference's inputs['inputs'] and
+        targets['targets'])."""
         if self._lm_forward_backward is not None:
             if len(batch) != 1 or truth_length is not None:
                 raise TypeError('FusedTrainer.step(inputs, targets) for a language model')
@@ -839,6 +935,8 @@ class FusedTrainer:
                 batch, truth_length = batch[:2], batch[2]
             if len(batch) != 2:
                 raise TypeError('FusedTrainer.step(inputs, mask, truth, truth_length=None) for a SpeechToText model')
+            if self._ctc and truth_length is None:
+                raise TypeError('FusedTrainer.step(inputs, mask, truth, truth_length) for a CTCModel: truth_length is required')
             # forward_backward reads the label counts as int32
             batch = (inputs,) + batch + (None if truth_length is None else truth_length.to(torch.int32),)
         with torch.no_grad():
