@@ -4,13 +4,16 @@ TransformerLanguageModel mirrors lm.py:93-171: embedding + sinusoidal positions 
 TransformerEncoderLayers (GLU FFN) under a causal mask + tied output projection, on the same sm_90a kernels as the acoustic
 encoder (causal flag on the attention kernel).  ``lm.train(); loss, _ = lm(inputs, targets); loss.backward()`` fills
 ``.grad`` of every parameter through the speech encoder layer's hand-written training forward and backward (train.py) with
-the causal mask, and ``train.FusedTrainer`` takes the model for the whole optimizer step (transformer_lm.yaml's
-TransformerScheduler is the one it keeps on the device).  Training needs 64-wide heads, the width of the attention backward.
+the causal mask.  Training needs 64-wide heads, the width of the attention backward.
 
 RecurrentLanguageModel mirrors lm.py:31-90 (rnnlm.yaml): embedding -> ``num_layers`` nn.LSTM layers (dropout between them
 in training) -> output projection, optionally tied to the embedding.  Each layer is one GEMM for the input projection of all
 positions and the persistent recurrence kernels of csrc/lstm.cu; ``lm.train(); loss, _ = lm(inputs, targets);
 loss.backward()`` fills ``.grad`` of every parameter through a hand-written backward through time.
+
+Both plug into training by train.py's contract (``train_pass`` / ``check_fused_trainer``, and ``train_batch`` where
+``train.FusedTrainer`` takes the model: the Transformer LM, whose TransformerScheduler is the one it keeps on the device; the
+recurrent LM's step-linear scheduler is not, so it is refused).
 
 Both keep the reference's constructor (``params`` dict of the YAML ``model:`` section), ``state_dict`` keys and ``predict``
 signature.  The recogniser adds ``lm_weight * log_probs`` inside the fused log-softmax/top-k kernel
@@ -85,19 +88,62 @@ class TransformerLanguageModel(nn.Module):
         mode with gradients enabled, loss.backward() fills .grad of every parameter; in training mode without gradients
         the training forward (residual dropout on) runs alone."""
         if self.training:
-            check_trainable(self)
-            if torch.is_grad_enabled():
-                named = [(n, p) for n, p in self.named_parameters() if p.requires_grad]
-                loss = _LMLoss.apply(transformer_forward_backward, self, inputs['inputs'], targets['targets'],
-                                     [n for n, _ in named], *[p for _, p in named])
-                return loss, None
-            seed = train._next_drop_seed(self, inputs['inputs'].device)
-            loss, _ = transformer_forward_backward(self, inputs['inputs'], targets['targets'], want_grads=False, drop_seed=seed)
-            return loss, None
+            self.check_trainable()          # before the dropout seed is drawn: no device work ahead of a refusal
+            run = train.loss_with_grad if torch.is_grad_enabled() else train.loss_train_mode
+            return run(self, inputs['inputs'], targets['targets']), None
         with torch.no_grad():
             logits = self.logits_bf16(inputs['inputs'])
             loss, _ = ops.ls_cross_entropy(logits, targets['targets'].contiguous(), self.vocab_size, self.smoothing)
         return loss, None
+
+    def check_trainable(self):
+        """Refuse, before any device work, what the training path does not cover -> the residual_dropout rate of every block."""
+        train.check_heads('language model', self.d_model, self.blocks)
+        return train.check_blocks(self.blocks)
+
+    check_fused_trainer = check_trainable
+
+    def train_batch(self, inputs, targets):
+        return inputs, targets
+
+    def train_pass(self, inputs, targets, want_grads=True, grad_sink=None, grad_scale=1.0, bf16_of=None, drop_seed=None):
+        """Training-mode forward (and hand-written backward) of model/lm.py:126-141, by train.py's contract: inputs / targets
+        i64 [N, L] (targets PAD-padded) -> (loss 0-d f32, {parameter name -> fp32 gradient} or None).
+
+        The mask is get_seq_mask (lm.py:14-18): the causal tril only, no key-padding mask.  Padding sits at the end of a row,
+        so a padded position sees earlier padded positions but no scored position ever reads one, and PAD targets are left out
+        of the loss: causal attention without kv_len gives the reference's loss and gradients exactly."""
+        rates = self.check_trainable()
+        train.need_drop_seed(drop_seed, rates)
+        pk = train.LayerPack(self, bf16_of)
+        blocks = [pk.enc_layer(b) for b in self.blocks]
+        emb = pk.w(self.embedding.weight)
+        tied = self.output_project.weight is self.embedding.weight
+        wout = emb if tied else pk.w(self.output_project.weight)
+        bout = self.output_project.bias.detach().float().contiguous()
+        tok = inputs.contiguous()
+        N, L = tok.shape
+        d, H, V = self.d_model, self.blocks[0].n_heads, self.vocab_size
+        _, table = self.pos_embedding.scale_and_table(L, tok.device)
+        x = ops.embed_posenc(tok, emb, table, N * L, d, period=L)                       # x * sqrt(d) + PE, dropout 0
+        drops = [(r, drop_seed, TLM_SITE + 2 * i) for i, r in enumerate(rates)]
+        tape = []
+        for p, drop in zip(blocks, drops):
+            x, t = train.enc_layer_fwd(p, x, False, N, H, L, None, drop, causal=True)
+            tape.append(t)
+        logits = train.head_fwd(x, wout, bout, self.ld_logits)
+        if not want_grads:
+            loss, _ = ops.ls_cross_entropy(logits, targets.contiguous(), V, self.smoothing)
+            return loss, None
+        loss, dlogits = ops.ls_cross_entropy_train(logits, targets.contiguous(), V, self.smoothing)
+        if grad_scale != 1.0:
+            dlogits = ops.scale_add_table(dlogits, grad_scale)                           # loss / accum_steps (trainer.py:216)
+        g = train.Grads(grad_sink)
+        dx = train.head_bwd(dlogits, x, wout, g, 'embedding.weight' if tied else 'output_project.weight', 'output_project.bias')
+        for i in reversed(range(len(blocks))):
+            dx = train.enc_layer_bwd(blocks[i], tape[i], dx, False, g, N, H, L, None, drops[i], causal=True)
+        train.embedding_bwd(tok, dx, emb, math.sqrt(d), g, 'embedding.weight')
+        return loss, g
 
     def save_checkpoint(self, params, name):
         torch.save({'params': params, 'model': self.state_dict()}, name)
@@ -107,66 +153,7 @@ class TransformerLanguageModel(nn.Module):
 # (train.ENC_SITE / DEC_SITE for the speech model, RNNLM_SITE for the recurrent LM)
 TLM_SITE = 3000
 
-
-def check_trainable(lm):
-    """Refuse, before any device work, what the training path of TransformerLanguageModel does not cover.
-    -> the residual_dropout rate of every block."""
-    rates = []
-    for blk in lm.blocks:
-        if lm.d_model != 64 * blk.n_heads:      # the attention backward (otb_attention_bwd) is written for 64-wide heads
-            raise NotImplementedError(f'training path: 64-wide attention heads only; the language model has d_model '
-                                      f'{lm.d_model} with {blk.n_heads} heads')
-        rate = float(blk.dropout_rates['residual_dropout'])
-        if not 0.0 <= rate < 1.0:
-            raise ValueError('residual_dropout must be in [0, 1)')
-        rates.append(rate)
-    return rates
-
-
-def transformer_forward_backward(lm, inputs, targets, want_grads=True, grad_sink=None, grad_scale=1.0, bf16_of=None,
-                                 drop_seed=None):
-    """Training-mode forward (and hand-written backward) of TransformerLanguageModel (model/lm.py:126-141): inputs / targets
-    i64 [N, L] (targets PAD-padded) -> (loss 0-d f32, {parameter name -> fp32 gradient} or None without want_grads).
-    grad_sink / grad_scale / bf16_of / drop_seed as in train.forward_backward (drop_seed is needed when residual_dropout > 0).
-
-    The mask is get_seq_mask (lm.py:14-18): the causal tril only, no key-padding mask.  Padding sits at the end of a row,
-    so a padded position sees earlier padded positions but no scored position ever reads one, and PAD targets are left out
-    of the loss: causal attention without kv_len gives the reference's loss and gradients exactly."""
-    rates = check_trainable(lm)
-    if drop_seed is None and any(r > 0.0 for r in rates):
-        raise ValueError('transformer_forward_backward: residual_dropout > 0 needs a drop_seed tensor')
-    pk = train.LayerPack(lm, bf16_of)
-    blocks = [pk._enc_layer(b) for b in lm.blocks]
-    emb = pk._w(lm.embedding.weight)
-    tied = lm.output_project.weight is lm.embedding.weight
-    wout = emb if tied else pk._w(lm.output_project.weight)
-    bout = lm.output_project.bias.detach().float().contiguous()
-    tok = inputs.contiguous()
-    N, L = tok.shape
-    d, H, V = lm.d_model, lm.blocks[0].n_heads, lm.vocab_size
-    _, table = lm.pos_embedding.scale_and_table(L, tok.device)
-    x = ops.embed_posenc(tok, emb, table, N * L, d, period=L)                       # x * sqrt(d) + PE, dropout 0
-    drops = [(r, drop_seed, TLM_SITE + 2 * i) for i, r in enumerate(rates)]
-    tape = []
-    for p, drop in zip(blocks, drops):
-        x, t = train._enc_layer_fwd(p, x, False, N, H, L, None, drop, causal=True)
-        tape.append(t)
-    logits = ops.linear(x, wout, bout, ops.EPI_BIAS, out_f32=True, n_out=lm.ld_logits)
-    if not want_grads:
-        loss, _ = ops.ls_cross_entropy(logits, targets.contiguous(), V, lm.smoothing)
-        return loss, None
-    loss, dlogits = ops.ls_cross_entropy_train(logits, targets.contiguous(), V, lm.smoothing)
-    if grad_scale != 1.0:
-        dlogits = ops.scale_add_table(dlogits, grad_scale)                           # loss / accum_steps (trainer.py:216)
-    wout_t = torch.zeros(d, lm.ld_logits, dtype=BF16, device=emb.device)            # [d, V padded]: dgrad of the logits GEMM
-    wout_t[:, :V] = wout.t()
-    g = train._Grads(grad_sink)
-    dwout, dx = train._output_layer_bwd(dlogits, x, wout_t, V, tied, g, 'embedding.weight', 'output_project')
-    for i in reversed(range(len(blocks))):
-        dx = train._enc_layer_bwd(blocks[i], tape[i], dx, False, g, N, H, L, None, drops[i], causal=True)
-    train._embedding_bwd(tok, dx, dwout, math.sqrt(d), tied, g, 'embedding.weight', 'output_project')
-    return loss, g
-
+transformer_forward_backward = TransformerLanguageModel.train_pass      # the pass as a function of the model
 
 RNNLM_SITE = 2000      # dropout site of the output of LSTM layer k: RNNLM_SITE + k (train.ENC_SITE / DEC_SITE for the speech model)
 
@@ -216,16 +203,13 @@ class RecurrentLanguageModel(nn.Module):
     def _build_pack(self):
         emb = self.embedding.weight.detach().to(BF16).contiguous()
         tied = self.output_project.weight is self.embedding.weight
-        wout = emb if tied else _w(self.output_project)
-        wout_t = torch.zeros(self.hidden_size, self.ld_logits, dtype=BF16, device=emb.device)    # dgrad of the logits GEMM
-        wout_t[:, :self.vocab_size] = wout.t()
         layers = []
         for k in range(self.num_layers):
             w_ih = getattr(self.rnn, f'weight_ih_l{k}').detach().to(BF16).contiguous()
             bias = (getattr(self.rnn, f'bias_ih_l{k}') + getattr(self.rnn, f'bias_hh_l{k}')).detach().float().contiguous()
-            layers.append({'ih': train._Lin(w_ih, w_ih.t().contiguous(), bias, f'rnn.ih_l{k}'),
+            layers.append({'ih': train.Lin(w_ih, w_ih.t().contiguous(), bias, f'rnn.weight_ih_l{k}', f'rnn.bias_ih_l{k}'),
                            'w_hh': getattr(self.rnn, f'weight_hh_l{k}').detach().to(BF16).contiguous()})
-        return {'emb': emb, 'wout': wout, 'wout_t': wout_t, 'bout': _b(self.output_project), 'tied': tied, 'layers': layers}
+        return {'emb': emb, 'wout': emb if tied else _w(self.output_project), 'bout': _b(self.output_project), 'layers': layers}
 
     def _check_device(self, device):
         """The recurrence kernels keep a slice of W_hh per CTA in shared memory: refuse a hidden size whose slice does not
@@ -258,7 +242,7 @@ class RecurrentLanguageModel(nn.Module):
         return x, torch.stack(hs), torch.stack(cs), tape
 
     def _logits(self, x, pk):
-        return ops.linear(x, pk['wout'], pk['bout'], ops.EPI_BIAS, out_f32=True, n_out=self.ld_logits)
+        return train.head_fwd(x, pk['wout'], pk['bout'], self.ld_logits)
 
     def init_hidden_states(self, batch_size, device):
         return torch.zeros([self.num_layers, batch_size, self.hidden_size]).to(device)
@@ -276,71 +260,53 @@ class RecurrentLanguageModel(nn.Module):
     def forward(self, inputs, targets):
         """model/lm.py:62-73: label-smoothed CE of the next-token logits, PAD ignored -> (loss, None).  In training mode with
         gradients enabled, loss.backward() fills .grad of every parameter."""
-        if self.training and torch.is_grad_enabled():
-            named = [(n, p) for n, p in self.named_parameters() if p.requires_grad]
-            loss = _LMLoss.apply(forward_backward, self, inputs['inputs'], targets['targets'], [n for n, _ in named],
-                                 *[p for _, p in named])
-            return loss, None
+        if self.training:
+            run = train.loss_with_grad if torch.is_grad_enabled() else train.loss_train_mode
+            return run(self, inputs['inputs'], targets['targets']), None
         with torch.no_grad():
-            seed = train._next_drop_seed(self, inputs['inputs'].device) if self.training else None
             pk = self._pack.get()
-            x, _, _, _ = self._run(inputs['inputs'].t().contiguous(), pk, drop_seed=seed)
+            x, _, _, _ = self._run(inputs['inputs'].t().contiguous(), pk)
             loss, _ = ops.ls_cross_entropy(self._logits(x, pk), targets['targets'].t().contiguous(), self.vocab_size, self.smoothing)
         return loss, None
 
+    def check_fused_trainer(self):
+        raise NotImplementedError('FusedTrainer: the recurrent LM trains with a step-linear scheduler that is not on the '
+                                  'device; train it through loss.backward() and a torch optimizer')
+
+    def train_pass(self, inputs, targets, want_grads=True, drop_seed=None):
+        """Training-mode forward and hand-written backward, by train.py's contract (FusedTrainer does not take this model, so
+        without its grad_sink / grad_scale / bf16_of): inputs / targets i64 [N, L] (targets PAD-padded) -> (loss 0-d f32,
+        {parameter name -> fp32 gradient} or None).  drop_seed: int32 device tensor [1], needed when dropout > 0
+        (applied to the output of every layer but the last)."""
+        train.need_drop_seed(drop_seed, [self.dropout] * (self.num_layers - 1))
+        pk = self._pack.get()
+        tok = inputs.t().contiguous()
+        L, N = tok.shape
+        V = self.vocab_size
+        x, _, _, tape = self._run(tok, pk, drop_seed=drop_seed, record=want_grads)
+        if not want_grads:
+            loss, _ = ops.ls_cross_entropy(self._logits(x, pk), targets.t().contiguous(), V, self.smoothing)
+            return loss, None
+        loss, dlogits = ops.ls_cross_entropy_train(self._logits(x, pk), targets.t().contiguous(), V, self.smoothing)
+        g = train.Grads()
+        tied = self.output_project.weight is self.embedding.weight
+        dy = train.head_bwd(dlogits, x, pk['wout'], g, 'embedding.weight' if tied else 'output_project.weight', 'output_project.bias')
+        for k in reversed(range(self.num_layers)):
+            p = pk['layers'][k]
+            xk, gates, c_all, y = tape[k]
+            dg = ops.lstm_bwd(dy, p['w_hh'], gates, c_all, L, N)
+            # W_hh sees h_{t-1}: the rows of step t >= 1 against the output of step t - 1 (zero initial state)
+            whh = f'rnn.weight_hh_l{k}'
+            g[whh] = ops.linear_wgrad(dg[N:], y[:-N]) if L > 1 else torch.zeros(p['w_hh'].shape, dtype=torch.float32, device=dg.device)
+            dy = train.linear_bwd(dg, xk, p['ih'], g)
+            g[f'rnn.bias_hh_l{k}'] = g[p['ih'].bname].clone()       # both biases enter the gates alike
+            if k > 0 and drop_seed is not None and self.dropout > 0.0:
+                dy = ops.dropout_add(dy, None, self.dropout, drop_seed, RNNLM_SITE + k - 1)
+        train.embedding_bwd(tok, dy, pk['emb'], 1.0, g, 'embedding.weight')
+        return loss, g
+
     def save_checkpoint(self, params, name):
         torch.save({'params': params, 'model': self.state_dict()}, name)
-
-
-def forward_backward(lm, inputs, targets, drop_seed=None):
-    """Training-mode forward and hand-written backward of RecurrentLanguageModel: inputs / targets i64 [N, L] (targets
-    PAD-padded) -> (loss 0-d f32, {parameter name -> fp32 gradient}).  drop_seed: int32 device tensor [1], needed when
-    dropout > 0 (applied to the output of every layer but the last)."""
-    if drop_seed is None and lm.dropout > 0.0 and lm.num_layers > 1:
-        raise ValueError('forward_backward: dropout > 0 needs a drop_seed tensor')
-    pk = lm._pack.get()
-    tok = inputs.t().contiguous()
-    L, N = tok.shape
-    V = lm.vocab_size
-    x, _, _, tape = lm._run(tok, pk, drop_seed=drop_seed, record=True)
-    loss, dlogits = ops.ls_cross_entropy_train(lm._logits(x, pk), targets.t().contiguous(), V, lm.smoothing)
-    g = train._Grads()
-    dwout, dy = train._output_layer_bwd(dlogits, x, pk['wout_t'], V, pk['tied'], g, 'embedding.weight', 'output_project')
-    for k in reversed(range(lm.num_layers)):
-        p = pk['layers'][k]
-        xk, gates, c_all, y = tape[k]
-        dg = ops.lstm_bwd(dy, p['w_hh'], gates, c_all, L, N)
-        # W_hh sees h_{t-1}: the rows of step t >= 1 against the output of step t - 1 (zero initial state)
-        whh = f'rnn.weight_hh_l{k}'
-        g[whh] = ops.linear_wgrad(dg[N:], y[:-N]) if L > 1 else torch.zeros(p['w_hh'].shape, dtype=torch.float32, device=dg.device)
-        dx = train._linear_bwd(dg, xk, p['ih'], g)
-        g[f'rnn.weight_ih_l{k}'] = g.pop(f'rnn.ih_l{k}.weight')
-        g[f'rnn.bias_ih_l{k}'] = g.pop(f'rnn.ih_l{k}.bias')
-        g[f'rnn.bias_hh_l{k}'] = g[f'rnn.bias_ih_l{k}'].clone()       # both biases enter the gates alike
-        if k > 0 and drop_seed is not None and lm.dropout > 0.0:
-            dx = ops.dropout_add(dx, None, lm.dropout, drop_seed, RNNLM_SITE + k - 1)
-        dy = dx
-    train._embedding_bwd(tok, dy, dwout, 1.0, pk['tied'], g, 'embedding.weight', 'output_project')
-    return loss, g
-
-
-class _LMLoss(torch.autograd.Function):
-    """loss = LM.forward(...) in training mode as ONE autograd node over the fp32 parameters; fb is the model's
-    forward_backward (transformer_forward_backward or forward_backward)."""
-
-    @staticmethod
-    def forward(ctx, fb, lm, inputs, targets, names, *params):
-        with torch.no_grad():
-            seed = train._next_drop_seed(lm, inputs.device)
-            loss, grads = fb(lm, inputs, targets, drop_seed=seed)
-        ctx.grads = [grads.get(n) for n in names]
-        ctx.shapes = [p.shape for p in params]
-        return loss.clone()
-
-    @staticmethod
-    def backward(ctx, gloss):
-        return (None, None, None, None, None) + tuple(None if gr is None else gr.view(shp) * gloss
-                                                      for gr, shp in zip(ctx.grads, ctx.shapes))
 
 
 LanguageModel = {'transformer_lm': TransformerLanguageModel, 'rnn_lm': RecurrentLanguageModel}

@@ -9,6 +9,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from . import train
 from .modules import ConformerEncoder, ConvFrontEnd, TransformerDecoder, TransformerEncoder, _lengths
 
 BuildFrontEnd = {'conv': ConvFrontEnd}
@@ -87,15 +88,11 @@ class SpeechToText(nn.Module):
         tlen = targets.get('targets_length') if self.ctc_weight > 0.0 else None
         if self.ctc_weight > 0.0 and tlen is None:
             raise ValueError("joint CTC needs targets['targets_length'] (label count including <S/E>, data/loader.py:94)")
-        if self.training and torch.is_grad_enabled():
-            from . import train
-            loss, ctc = train.loss_with_grad(self, inputs['inputs'], inputs['mask'], truth, tlen)
-            return loss, ({'CTCLoss': float(ctc)} if ctc is not None else None)
-        if self.training and isinstance(self.encoder, ConformerEncoder):
-            # train() without gradients: BatchNorm must use the batch statistics and update its running buffers, as the
-            # reference does; the inference path below would fold the running statistics instead
-            from . import train
-            loss, ctc = train.loss_train_mode(self, inputs['inputs'], inputs['mask'], truth, tlen)
+        # train() without gradients: a Conformer's BatchNorm must use the batch statistics and update its running buffers, as
+        # the reference does; the inference path below would fold the running statistics instead
+        if self.training and (torch.is_grad_enabled() or isinstance(self.encoder, ConformerEncoder)):
+            run = train.loss_with_grad if torch.is_grad_enabled() else train.loss_train_mode
+            loss, ctc = run(self, inputs['inputs'], inputs['mask'], truth, tlen), self._last_ctc_loss
             return loss, ({'CTCLoss': float(ctc)} if ctc is not None else None)
         mem, lengths, B, T2 = self.encode_bf16(inputs['inputs'], inputs['mask'])
         tin = truth[:, :-1].contiguous()
@@ -106,6 +103,15 @@ class SpeechToText(nn.Module):
                                     truth[:, 1:].contiguous(), tlen.to(torch.int32).to(mem.device).contiguous(), self.assistor.blank)
             return (1 - self.ctc_weight) * loss + self.ctc_weight * lc, {'CTCLoss': float(lc)}
         return loss, None
+
+    train_pass = train.forward_backward
+
+    def train_batch(self, inputs, mask, truth, truth_length=None):
+        """FusedTrainer.step's arguments as train_pass takes them; it reads the label counts as int32."""
+        return inputs, mask, truth, None if truth_length is None else truth_length.to(torch.int32)
+
+    def check_fused_trainer(self):
+        """Nothing is refused up front: the first pass builds the TrainPack, whose constructor checks the model."""
 
     def save_checkpoint(self, params, name):
         chk = {'params': params, 'frontend': self.frontend.state_dict(),
@@ -136,7 +142,7 @@ class CTCModel(nn.Module):
     on truth[:, 1:-1] (no <S/E>) with targets_length - 1 labels.  Submodules `frontend`, `encoder`, `assistor`: the
     reference's state_dict keys and checkpoint sections.
 
-    forward: train() with gradients -> one autograd node over the hand-written backward (train.ctc_forward_backward);
+    forward: train() with gradients -> one autograd node over the hand-written backward (train_pass);
     train() without gradients -> the training-mode forward (a Conformer's BatchNorm uses the batch statistics); eval() ->
     the fused inference path (encode_bf16, head GEMM, otb_ctc_loss)."""
 
@@ -162,13 +168,9 @@ class CTCModel(nn.Module):
         truth, tlen = targets['targets'], targets.get('targets_length')
         if tlen is None:
             raise ValueError("CTCModel needs targets['targets_length'] (label count including <S/E>, data/loader.py:94)")
-        from . import train
-        if self.training and torch.is_grad_enabled():
-            loss, _ = train.loss_with_grad(self, inputs['inputs'], inputs['mask'], truth, tlen)
-            return loss, None
         if self.training:
-            loss, _ = train.loss_train_mode(self, inputs['inputs'], inputs['mask'], truth, tlen)
-            return loss, None
+            run = train.loss_with_grad if torch.is_grad_enabled() else train.loss_train_mode
+            return run(self, inputs['inputs'], inputs['mask'], truth, tlen), None
         logits, lengths, B, T2 = self.logits_bf16(inputs['inputs'], inputs['mask'])
         tl = (tlen.to(logits.device).to(torch.int32) - 1).contiguous()
         loss, _, _ = ops.ctc_loss(logits, B, T2, self.vocab_size, lengths, truth[:, 1:-1].contiguous(), tl, self.assistor.blank)
@@ -182,6 +184,14 @@ class CTCModel(nn.Module):
         return ops.log_softmax(logits, self.vocab_size).view(B, T2, -1), lengths
 
     recognize = inference
+
+    train_pass = train.ctc_forward_backward
+    check_fused_trainer = SpeechToText.check_fused_trainer
+
+    def train_batch(self, inputs, mask, truth, truth_length=None):
+        if truth_length is None:
+            raise TypeError('FusedTrainer.step(inputs, mask, truth, truth_length) for a CTCModel: truth_length is required')
+        return SpeechToText.train_batch(self, inputs, mask, truth, truth_length)
 
     def save_checkpoint(self, params, name):
         torch.save({'params': params, 'frontend': self.frontend.state_dict(), 'encoder': self.encoder.state_dict(),

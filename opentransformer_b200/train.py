@@ -7,19 +7,31 @@ Mirror of the inner step of otrans/train/trainer.py:206-234 for `SpeechToText` (
 The reference differentiates its forward through torch autograd.  Here the backward is written by hand as a reverse
 walk over a tape of saved bf16 activations, so that every contraction runs on the wgmma kernels (dgrad = otb_linear
 with the transposed weight, residual gradients fused into its epilogue; wgrad = otb_linear_wgrad; attention backward =
-otb_attention_bwd) and everything else on the HBM-bound backward kernels (csrc/backward.cu).  The only torch autograd
-node is `_SpeechToTextLoss`, which makes `model(inputs, targets)[0].backward()` populate `.grad` of the fp32 master
-parameters exactly like the reference module.
+otb_attention_bwd) and everything else on the HBM-bound backward kernels (csrc/backward.cu).
+
+How a model plugs into training -- three methods on its class, and nothing here asks which class it is:
+
+    model.train_pass(*batch, want_grads=True, grad_sink=None, grad_scale=1.0, bf16_of=None, drop_seed=None)
+        -> (loss 0-d f32, {parameter name -> fp32 gradient} or None without want_grads)
+    model.train_batch(*step arguments) -> batch       FusedTrainer.step's arguments, validated, as train_pass takes them
+                                                      (not on a model check_fused_trainer always refuses)
+    model.check_fused_trainer()                       what FusedTrainer refuses at construction, before any device work
+
+batch is (inputs, mask, truth, truth_length or None) for a SpeechToText (forward_backward) and a CTCModel
+(ctc_forward_backward), (inputs, targets) for the language models (lm.py).  grad_sink: name -> fp32 tensor the gradients
+(x grad_scale) are ADDED into (a gradient accumulation buffer); bf16_of: see LayerPack; drop_seed: int32 device tensor [1],
+the dropout seed of THIS pass (read on the device), required when a dropout rate is non-zero.  The only torch autograd node is `_TrainingLoss` (loss_with_grad), which
+makes `model(inputs, targets)[0].backward()` populate `.grad` of the fp32 master parameters exactly like the reference
+module; loss_train_mode is the same pass without gradients, and FusedTrainer's micro-step is train_pass into its grad_sink.
 
 Scope: the shipped Speech-Transformer configuration -- conv front end, post-norm Transformer encoder / decoder with GLU
 feed-forward, tied or untied output layer, `residual_dropout` as shipped (0.1: counter-based masks in the residual GEMM's
 epilogue, replayed in the backward; csrc/dropout.cuh); the other dropout rates must be 0 (as shipped) and raise
 otherwise.  The encoder may also be the shipped Conformer layout with 64-wide heads (macaron feed-forward, rel-pos
 attention, then the convolution module with training-mode BatchNorm; encoder/conformer.py:75-89).
-The Transformer language model (lm.transformer_forward_backward) trains through the encoder layer's forward and backward
-below with the causal mask, and FusedTrainer takes it as well.
-The CTC-only model (model.CTCModel, model/ctc.py) trains through the same front-end + encoder halves (_encoder_fwd /
-_encoder_bwd) with the CTC head and otb_ctc_loss in place of the decoder (ctc_forward_backward).
+The CTC-only model (model/ctc.py) is the front-end + encoder half (_encoder_fwd / _encoder_bwd) with the CTC head and
+otb_ctc_loss in place of the decoder; the Transformer language model is the encoder layer (enc_layer_fwd / enc_layer_bwd)
+under the causal mask.  All four models share the vocabulary head (head_fwd / head_bwd) and embedding_bwd.
 """
 import math
 from collections import namedtuple
@@ -41,7 +53,7 @@ def _f(t):
     return t.detach().float().contiguous()
 
 
-_Lin = namedtuple('_Lin', 'w wt b name')      # W [N,K], W^T [K,N], fp32 bias, qualified module name
+Lin = namedtuple('Lin', 'w wt b wname bname')      # W [N,K], W^T [K,N], fp32 bias, the names of the two parameters
 _Norm = namedtuple('_Norm', 'g b name')
 
 
@@ -54,67 +66,86 @@ class LayerPack:
         self._bf16_of = bf16_of
         self._names = {m: n for n, m in model.named_modules()}
 
-    def _w(self, param):
+    def w(self, param):
         return self._bf16_of(param) if self._bf16_of is not None else _bf(param)
 
     def _lin(self, lin):
-        w = self._w(lin.weight)
-        return _Lin(w, w.t().contiguous(), _f(lin.bias), self._names[lin])
+        w, name = self.w(lin.weight), self._names[lin]
+        return Lin(w, w.t().contiguous(), _f(lin.bias), name + '.weight', name + '.bias')
 
     def _ln(self, norm):
         return _Norm(_f(norm.weight), _f(norm.bias), self._names[norm])
 
-    def _enc_layer(self, b):
+    def enc_layer(self, b):
         a, f = b.slf_attn, b.feed_forward
         return {'qkv': self._lin(a.qvk_proj), 'o': self._lin(a.output_proj), 'w1': self._lin(f.w_1), 'w2': self._lin(f.w_2),
                 'ln1': self._ln(b.norm1), 'ln2': self._ln(b.norm2), 'act': f.activation}
 
 
+def check_heads(name, d_model, blocks):
+    """The attention backward (otb_attention_bwd) is written for 64-wide heads: refuse any other width in the stack `name`."""
+    for blk in blocks:
+        if d_model != 64 * blk.n_heads:
+            raise NotImplementedError(f'training path: 64-wide attention heads only; the {name} has d_model {d_model} '
+                                      f'with {blk.n_heads} heads')
+
+
+def check_blocks(blocks):
+    """The feed-forward and dropout rules of a stack of blocks -> the residual_dropout rate of every block."""
+    out = []
+    for blk in blocks:
+        if _ffn_of(blk).activation not in ('glu', 'relu'):
+            raise NotImplementedError('training path: GLU or ReLU feed-forward only')
+        rates = getattr(blk, 'dropout_rates', {})
+        # conv_dropout: the reference builds the Dropout and never applies it (module/conformer.py:34,36-57)
+        other = {k: v for k, v in rates.items() if k not in ('residual_dropout', 'conv_dropout') and float(v) > 0.0}
+        if other:
+            # the reference applies these in train mode (attention.py:45, ffn.py:40); training WITHOUT them would be a
+            # different network, so refuse instead of silently dropping the regulariser.  residual_dropout -- the only
+            # non-zero rate of the shipped configs -- IS implemented (otb_linear_dropout_resid / otb_dropout_bwd).
+            raise NotImplementedError(f'training path: only residual_dropout is implemented, got {other}; set them to 0.0')
+        out.append(float(rates.get('residual_dropout', 0.0)))
+        if not (0.0 <= out[-1] < 1.0):
+            raise ValueError('residual_dropout must be in [0, 1)')
+    return out
+
+
+def need_drop_seed(drop_seed, rates):
+    if drop_seed is None and any(r > 0.0 for r in rates):
+        raise ValueError('training pass: a dropout rate > 0 needs a drop_seed tensor')
+
+
 class EncoderPack(LayerPack):
     """The LayerPack of the front end and the encoder: all a CTCModel trains, and the first half of a SpeechToText's
-    TrainPack.  `dec` (the SpeechToText's decoder) joins the checks, which run in one order for both models."""
+    TrainPack.  Its constructor refuses what the training path does not cover, before any device work.  Where the model
+    has a decoder the checks take it in beside the encoder, each rule over both stacks before the next rule, so that the
+    refusal a configuration with two faults gets does not depend on the stack a fault sits in (96-wide decoder heads and a
+    320-channel front end: the heads).  `rates`: stack name -> the residual_dropout rate of every block."""
 
-    def __init__(self, model, bf16_of=None, dec=None):
+    def __init__(self, model, bf16_of=None):
         super().__init__(model, bf16_of)
-        fe, enc = model.frontend, model.encoder
+        fe, enc, dec = model.frontend, model.encoder, getattr(model, 'decoder', None)
         self.conformer = isinstance(enc, ConformerEncoder)
-        if dec is None:
-            if not isinstance(fe, ConvFrontEnd) or not isinstance(enc, (TransformerEncoder, ConformerEncoder)):
-                raise NotImplementedError('training path: conv front end + Transformer or Conformer encoder only')
-        elif not isinstance(fe, ConvFrontEnd) or not isinstance(enc, (TransformerEncoder, ConformerEncoder)) \
-                or not isinstance(dec, TransformerDecoder):
-            raise NotImplementedError('training path: conv front end + Transformer or Conformer encoder + Transformer decoder only')
+        if not (isinstance(fe, ConvFrontEnd) and isinstance(enc, (TransformerEncoder, ConformerEncoder))
+                and (dec is None or isinstance(dec, TransformerDecoder))):
+            raise NotImplementedError('training path: conv front end + Transformer or Conformer encoder'
+                                      + (' + Transformer decoder' if dec is not None else '') + ' only')
         if not self.conformer and enc.relative_positional:
             raise NotImplementedError('training path: the Transformer encoder with absolute positions only')
-        stacks = [('encoder', enc.d_model, enc.blocks)] + ([('decoder', dec.d_model, dec.blocks)] if dec is not None else [])
-        for name, d_model, blocks in stacks:
-            for blk in blocks:
-                if d_model != 64 * blk.n_heads:   # the attention backward (otb_attention_bwd) is written for 64-wide heads
-                    raise NotImplementedError(f'training path: 64-wide attention heads only; the {name} has d_model {d_model} '
-                                              f'with {blk.n_heads} heads')
+        stacks = [('encoder', enc)] + ([('decoder', dec)] if dec is not None else [])
+        for name, stack in stacks:
+            check_heads(name, stack.d_model, stack.blocks)
         C1 = fe.conv1.conv_layer.out_channels
         if (C1 + 63) // 64 * 64 > 256:       # the conv1 weight gradient (otb_conv1_wgrad) runs one channel per thread
             raise NotImplementedError(f'training path: mid_channel {C1} pads to {(C1 + 63) // 64 * 64} channels; the conv1 weight '
                                       'gradient takes at most 256')
         if self.conformer:
             _check_conformer(enc)
-        if fe.front_end_layer_norm or enc.pos_emb.scale_learnable or (dec is not None and dec.pos_emb.scale_learnable):
+        if fe.front_end_layer_norm or any(stack.pos_emb.scale_learnable for _, stack in stacks):
             raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale (pos_dropout > 0)')
-        for blk in list(enc.blocks) + (list(dec.blocks) if dec is not None else []):
-            if _ffn_of(blk).activation not in ('glu', 'relu'):
-                raise NotImplementedError('training path: GLU or ReLU feed-forward only')
-            rates = getattr(blk, 'dropout_rates', {})
-            # conv_dropout: the reference builds the Dropout and never applies it (module/conformer.py:34,36-57)
-            other = {k: v for k, v in rates.items() if k not in ('residual_dropout', 'conv_dropout') and float(v) > 0.0}
-            if other:
-                # the reference applies these in train mode (attention.py:45, ffn.py:40); training WITHOUT them would be a
-                # different network, so refuse instead of silently dropping the regulariser.  residual_dropout -- the only
-                # non-zero rate of the shipped configs -- IS implemented (otb_linear_dropout_resid / otb_dropout_bwd).
-                raise NotImplementedError(f'training path: only residual_dropout is implemented, got {other}; set them to 0.0')
-            if not (0.0 <= float(rates.get('residual_dropout', 0.0)) < 1.0):
-                raise ValueError('residual_dropout must be in [0, 1)')
+        self.rates = {name: check_blocks(stack.blocks) for name, stack in stacks}
         self.fe = self._frontend(fe)
-        self.enc = [self._conf_layer(b) if self.conformer else self._enc_layer(b) for b in enc.blocks]
+        self.enc = [self._conf_layer(b) if self.conformer else self.enc_layer(b) for b in enc.blocks]
         # pre-norm stacks end with one more LayerNorm (encoder/transformer.py:96-97,131-132; decoder/transformer.py:151-152,178-179)
         self.enc_pre = bool(getattr(enc, 'normalize_before', False))
         self.enc_norm = self._ln(enc.norm) if self.enc_pre else None
@@ -129,7 +160,7 @@ class EncoderPack(LayerPack):
         """A Conformer block: the rel-pos projection as ONE GEMM producing [q+u | q+v | k | v] (W_ext = [Wq; Wq; Wk; Wv],
         b_ext = [bq + u; bq + v; bk; bv], as the inference pack), and the convolution module with BatchNorm unfolded."""
         a, cv = b.mha, b.conv
-        w = self._w(a.qvk_proj.weight)
+        w = self.w(a.qvk_proj.weight)
         d = w.shape[1]
         wext = torch.cat([w[:d], w], 0)
         bq = _f(a.qvk_proj.bias)
@@ -138,7 +169,7 @@ class EncoderPack(LayerPack):
         return {'mac_ln': self._ln(b.macaron_ffn_norm), 'w1': self._lin(b.pre_ffn.w_1), 'w2': self._lin(b.pre_ffn.w_2),
                 'act': b.pre_ffn.activation, 'scale': float(b.ffn_scale),
                 'mha_ln': self._ln(b.mha_norm), 'wext': wext, 'wext_t': wext.t().contiguous(), 'bext': bext,
-                'wpos': self._w(a.pos_proj.weight), 'attn': self._names[a],
+                'wpos': self.w(a.pos_proj.weight), 'attn': self._names[a],
                 'conv_ln': self._ln(b.conv_norm), 'pw1': self._lin(cv.pointwise_conv1), 'pw2': self._lin(cv.pointwise_conv2),
                 'dw': _f(dw.weight).view(d, -1), 'dwb': _f(dw.bias), 'dw_name': self._names[dw],
                 'bn': bn, 'bn_g': _f(bn.weight), 'bn_b': _f(bn.bias), 'bn_name': self._names[bn],
@@ -149,19 +180,17 @@ class TrainPack(EncoderPack):
     """The LayerPack of a SpeechToText model: front end, encoder and decoder layers and the output layer."""
 
     def __init__(self, model, bf16_of=None):
-        super().__init__(model, bf16_of, dec=model.decoder)
+        super().__init__(model, bf16_of)
         dec = model.decoder
         self.dec = [self._dec_layer(b) for b in dec.blocks]
         self.dec_pre = bool(dec.normalize_before)
         self.dec_norm = self._ln(dec.after_norm) if self.dec_pre else None
-        V, d = dec.vocab_size, dec.d_model
-        self.ld_logits = dec.ld_logits
-        emb = self._w(dec.embedding.weight)
-        self.tied = dec.output_layer.weight is dec.embedding.weight
-        wout = emb if self.tied else self._w(dec.output_layer.weight)
-        wout_t = torch.zeros(d, self.ld_logits, dtype=BF16, device=emb.device)      # [d, V padded]: dgrad of the logits GEMM
-        wout_t[:, :V] = wout.t()
-        self.out = {'emb': emb, 'wout': wout, 'wout_t': wout_t, 'bout': _f(dec.output_layer.bias)}
+        self.emb = self.w(dec.embedding.weight)
+        # the output layer's weight gradient goes by the embedding's name when the two are one tensor
+        tied = dec.output_layer.weight is dec.embedding.weight
+        self.wout = self.emb if tied else self.w(dec.output_layer.weight)
+        self.wout_name = 'decoder.embedding.weight' if tied else 'decoder.output_layer.weight'
+        self.bout = _f(dec.output_layer.bias)
 
     def _dec_layer(self, b):
         a, c, f = b.slf_attn, b.src_attn, b.feed_forward
@@ -198,7 +227,7 @@ def unused_parameters(model):
     return {n for n, _ in model.named_parameters() if '.post_ffn.' in n and n.startswith('encoder.blocks.')}
 
 
-class _Grads(dict):
+class Grads(dict):
     """name -> fp32 gradient.  With `sink` (name -> fp32 view of the optimizer's flat gradient buffer) the kernels ADD
     their result straight into the sink (otb_linear_wgrad / otb_colsum / otb_layernorm_bwd accumulate flags) -- what
     autograd's AccumulateGrad does, without one torch add per parameter."""
@@ -231,12 +260,11 @@ def _ln_bwd(dy, z, ln, grads):
     return dz
 
 
-def _linear_bwd(dy, x, lin, grads, resid=None):
+def linear_bwd(dy, x, lin, grads, resid=None):
     """Gradients of y = x W^T + b: parameter grads into `grads`, returns dx (+ resid) as bf16."""
     acc = grads.sink is not None
-    wname, bname = lin.name + '.weight', lin.name + '.bias'
-    grads[wname] = ops.linear_wgrad(dy, x, out=grads.out(wname), accumulate=acc)
-    grads[bname] = ops.colsum(dy, out=grads.out(bname), accumulate=acc)
+    grads[lin.wname] = ops.linear_wgrad(dy, x, out=grads.out(lin.wname), accumulate=acc)
+    grads[lin.bname] = ops.colsum(dy, out=grads.out(lin.bname), accumulate=acc)
     if resid is not None:
         return ops.linear(dy, lin.wt, None, EPI_RESID, resid=resid)
     return ops.linear(dy, lin.wt)
@@ -296,7 +324,7 @@ _EncTape = namedtuple('_EncTape', 'a u1 qkv ctx lse z1 u2 ffn_u h z2')
 _DecTape = namedtuple('_DecTape', 'a u1 qkv ctx lse z1 u2 q kv ctx2 lse2 z2 u3 ffn_u h z3')
 
 
-def _enc_layer_fwd(p, a, pre, B, H, T, lengths, drop, causal=False):
+def enc_layer_fwd(p, a, pre, B, H, T, lengths, drop, causal=False):
     """One encoder layer in training mode (encoder/transformer.py:41-65) -> (output, _EncTape).  causal=True: the tril
     mask the Transformer LM feeds to the same layer (model/lm.py:14-18)."""
     d = a.shape[1]
@@ -311,19 +339,19 @@ def _enc_layer_fwd(p, a, pre, B, H, T, lengths, drop, causal=False):
     return out, _EncTape(a=a, u1=u1, qkv=qkv, ctx=ctx, lse=lse, z1=z1, u2=u2, ffn_u=ffn_u, h=h, z2=z2)
 
 
-def _enc_layer_bwd(p, t, dout, pre, g, B, H, T, lengths, drop, causal=False):
-    """Backward of _enc_layer_fwd: parameter gradients into g; returns the gradient of the layer input."""
+def enc_layer_bwd(p, t, dout, pre, g, B, H, T, lengths, drop, causal=False):
+    """Backward of enc_layer_fwd: parameter gradients into g; returns the gradient of the layer input."""
     d = t.a.shape[1]
     dz2 = dout if pre else _ln_bwd(dout, t.z2, p['ln2'], g)
     # the sub-layer branch sees the replayed dropout mask, the residual branch (resid=) the plain gradient
-    dh = _linear_bwd(_drop_bwd(dz2, drop, 1), t.h, p['w2'], g)
-    du2 = _linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.u2, p['w1'], g, resid=dz2)
+    dh = linear_bwd(_drop_bwd(dz2, drop, 1), t.h, p['w2'], g)
+    du2 = linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.u2, p['w1'], g, resid=dz2)
     dz1 = _ln_bwd(du2, t.z1, p['ln2'] if pre else p['ln1'], g)
-    dctx = _linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
+    dctx = linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
     dqkv = torch.empty_like(t.qkv)
     ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B, H, T, T, dqkv, dqkv, dqkv, kv_len=lengths, causal=causal,
                       q_col0=0, k_col0=d, v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
-    du1 = _linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
+    du1 = linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
     return _ln_bwd(du1, t.a, p['ln1'], g) if pre else du1
 
 
@@ -352,22 +380,22 @@ def _dec_layer_bwd(p, t, dout, dmem, mem, pre, g, B, H, L, T, lengths, drop):
     this layer's gradient of the memory (added by the K|V dgrad GEMM's residual epilogue)."""
     d = t.a.shape[1]
     dz3 = dout if pre else _ln_bwd(dout, t.z3, p['ln3'], g)
-    dh = _linear_bwd(_drop_bwd(dz3, drop, 2), t.h, p['w2'], g)
-    du3 = _linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.u3, p['w1'], g, resid=dz3)
+    dh = linear_bwd(_drop_bwd(dz3, drop, 2), t.h, p['w2'], g)
+    du3 = linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.u3, p['w1'], g, resid=dz3)
     dz2 = _ln_bwd(du3, t.z2, p['ln3'] if pre else p['ln2'], g)
-    dctx2 = _linear_bwd(_drop_bwd(dz2, drop, 1), t.ctx2, p['o2'], g)
+    dctx2 = linear_bwd(_drop_bwd(dz2, drop, 1), t.ctx2, p['o2'], g)
     dq = torch.empty_like(t.q)
     dkv = torch.empty_like(t.kv)
     ops.attention_bwd(t.q, t.kv, t.kv, t.ctx2, dctx2, t.lse2, B, H, L, T, dq, dkv, dkv, kv_len=lengths, k_col0=0, v_col0=d,
                       dq_col0=0, dk_col0=0, dv_col0=d)
-    dmem = _linear_bwd(dkv, mem, p['kv'], g, resid=dmem)
-    du2 = _linear_bwd(dq, t.u2, p['q'], g, resid=dz2)
+    dmem = linear_bwd(dkv, mem, p['kv'], g, resid=dmem)
+    du2 = linear_bwd(dq, t.u2, p['q'], g, resid=dz2)
     dz1 = _ln_bwd(du2, t.z1, p['ln2'] if pre else p['ln1'], g)
-    dctx = _linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
+    dctx = linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
     dqkv = torch.empty_like(t.qkv)
     ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B, H, L, L, dqkv, dqkv, dqkv, causal=True, q_col0=0, k_col0=d,
                       v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
-    du1 = _linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
+    du1 = linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
     return (_ln_bwd(du1, t.a, p['ln1'], g) if pre else du1), dmem
 
 
@@ -460,54 +488,57 @@ def _conformer_block_bwd(p, t, dout, g, B, H, T, lengths, pe, drop):
     dx3 = _ln_bwd(dz, t.x3, p['post_ln'], g)
     # convolution module: its output was masked, then dropped
     dco = ops.dropout_add(dx3, None, rate, seed, site + 2, row_len=lengths, row_period=T)
-    ds = _linear_bwd(dco, t.s, p['pw2'], g)
+    ds = linear_bwd(dco, t.s, p['pw2'], g)
     dwn, bwn, bn = p['dw_name'] + '.weight', p['dw_name'] + '.bias', p['bn_name']
     dg, dwv, g[bwn], g[bn + '.weight'], g[bn + '.bias'] = ops.conformer_conv_bwd(
         ds, t.g, lengths, p['dw'], p['bn_g'], p['bn_b'], t.c, t.stats, B, T, dw=g.out(dwn).view(p['dw'].shape) if acc else None,
         dwb=g.out(bwn), dgamma=g.out(bn + '.weight'), dbeta=g.out(bn + '.bias'), accumulate=acc)
     g[dwn] = g.out(dwn) if acc else dwv.view(dwv.shape[0], 1, -1)             # nn.Conv1d's [d, 1, k]
-    dy2 = _linear_bwd(ops.glu_bwd(dg, t.cu), t.y2, p['pw1'], g)
+    dy2 = linear_bwd(ops.glu_bwd(dg, t.cu), t.y2, p['pw1'], g)
     dx2 = ops.dropout_add(_ln_bwd(dy2, t.x2, p['conv_ln'], g), dx3)
     # rel-pos attention (no output projection)
     dy1 = _relpos_attn_bwd(p, t, _drop_bwd(dx2, drop, 1), g, B, H, T, lengths, pe)
     dx1 = ops.dropout_add(_ln_bwd(dy1, t.x1, p['mha_ln'], g), dx2)
     # macaron feed-forward, scaled by ffn_scale
     df = ops.dropout_add(dx1, None, rate, seed, site, alpha=p['scale'])
-    dh = _linear_bwd(df, t.h, p['w2'], g)
-    dy0 = _linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.y0, p['w1'], g)
+    dh = linear_bwd(df, t.h, p['w2'], g)
+    dy0 = linear_bwd(_ffn_act_bwd(p, dh, t.ffn_u, t.h), t.y0, p['w1'], g)
     return ops.dropout_add(_ln_bwd(dy0, t.x0, p['mac_ln'], g), dx1)
 
 
-def _output_layer_bwd(dlogits, y, wout_t, V, tied, g, emb_name, out_name):
-    """Backward of the output layer logits = y W^T + b (f32 [rows, ld], ld = V padded): the weight gradient goes into
-    emb_name's tensor when the weight is tied to the embedding, the bias gradient into g.  -> (dW f32 [V, d], dy bf16)."""
-    acc = g.sink is not None
-    wname = emb_name if tied else out_name + '.weight'
+def head_fwd(y, w, b, ld):
+    """A vocabulary head, logits = y W^T + b -> f32 [rows, ld] (ld = V padded, the first V columns valid): the attention
+    decoder's output layer, the CTC head and the language models' output projection."""
+    return ops.linear(y, w, b, EPI_BIAS, out_f32=True, n_out=ld)
+
+
+def head_bwd(dlogits, y, w, g, wname, bname, resid=None):
+    """Backward of head_fwd from dlogits [rows, ld]: the gradient of W (bf16 [V, d]) into g[wname] -- the embedding's name
+    when the head is tied to it, and embedding_bwd then lands on top -- and of b into g[bname].  Returns dy (+ resid) as
+    bf16 [rows, d].  The zero-padded W^T of the dgrad GEMM is built here, every pass: the weights move every step."""
+    V, d = w.shape
     # dlogits[:, :V] as a strided view: the TMA map stops at column V, so the result has exactly V rows
-    dwout = ops.linear_wgrad(dlogits[:, :V], y, out=g.out(wname), accumulate=acc)          # [V, d]
-    g.put(out_name + '.bias', ops.colsum(dlogits)[:V])
-    return dwout, ops.linear(dlogits, wout_t)                                     # [rows, d]
+    g[wname] = ops.linear_wgrad(dlogits[:, :V], y, out=g.out(wname), accumulate=g.sink is not None)
+    g.put(bname, ops.colsum(dlogits)[:V])
+    wt = torch.zeros(d, dlogits.shape[1], dtype=BF16, device=w.device)
+    wt[:, :V] = w.t()
+    if resid is not None:
+        return ops.linear(dlogits, wt, None, EPI_RESID, resid=resid)
+    return ops.linear(dlogits, wt)
 
 
-def _embedding_bwd(tok, dx, dwout, scale, tied, g, emb_name, out_name):
-    """Backward of x = scale * E[tok]: with tied weights the output layer's gradient dwout is the same tensor, and the
-    embedding's lands on top of it."""
-    if tied:
-        ops.embed_bwd(tok, dx, dwout, scale)          # atomics on top of the output-layer gradient
-        g[emb_name] = dwout
-    else:
-        g[out_name + '.weight'] = dwout
-        demb = g.out(emb_name)
-        if demb is None:
-            demb = torch.zeros_like(dwout)
-        ops.embed_bwd(tok, dx, demb, scale)
-        g[emb_name] = demb
+def embedding_bwd(tok, dx, emb, scale, g, name):
+    """Backward of x = scale * E[tok] (E: emb) into g[name].  With a tied head g[name] already holds the head's gradient,
+    and the embedding's lands on top of it (fp32 atomics)."""
+    if name not in g:
+        _acc_out(g, name, emb.shape, dx.device)
+    ops.embed_bwd(tok, dx, g[name], scale)
 
 
 _EncTrace = namedtuple('_EncTrace', 'x_in h1 h2 tape pe scale lengths enc_last drops B T F T2 F2')
 
 
-def _encoder_fwd(model, pk, inputs, mask, e_rates, drop_seed):
+def _encoder_fwd(model, pk, inputs, mask, drop_seed):
     """Front end + encoder in training mode, the half shared by SpeechToText and CTCModel -> (memory bf16 [B*T', d],
     _EncTrace: what _encoder_bwd reads)."""
     fe, enc = model.frontend, model.encoder
@@ -528,14 +559,14 @@ def _encoder_fwd(model, pk, inputs, mask, e_rates, drop_seed):
     else:               # rel-pos encoders take the front end's output as is (encoder/conformer.py:141-149)
         x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_BIAS)
     ns = _enc_sites(enc)
-    e_drop = [(r, drop_seed, ENC_SITE + ns * i) for i, r in enumerate(e_rates)]
+    e_drop = [(r, drop_seed, ENC_SITE + ns * i) for i, r in enumerate(pk.rates['encoder'])]
     enc_tape = []
     pe = enc._rel_pos(T2, dev) if conformer else None
     for p, drop in zip(pk.enc, e_drop):
         if conformer:
             x, t = _conformer_block_fwd(p, x, B, H, T2, lengths, pe, drop)
         else:
-            x, t = _enc_layer_fwd(p, x, pk.enc_pre, B, H, T2, lengths, drop)
+            x, t = enc_layer_fwd(p, x, pk.enc_pre, B, H, T2, lengths, drop)
         enc_tape.append(t)
     if conformer:       # the running statistics moved: the inference pack, which folds BatchNorm, must be rebuilt
         modules.bump_param_generation()
@@ -559,7 +590,7 @@ def _encoder_bwd(model, pk, tr, dx, g):
         if pk.conformer:
             dx = _conformer_block_bwd(pk.enc[i], tr.tape[i], dx, g, B, H, T2, tr.lengths, tr.pe, tr.drops[i])
         else:
-            dx = _enc_layer_bwd(pk.enc[i], tr.tape[i], dx, pk.enc_pre, g, B, H, T2, tr.lengths, tr.drops[i])
+            dx = enc_layer_bwd(pk.enc[i], tr.tape[i], dx, pk.enc_pre, g, B, H, T2, tr.lengths, tr.drops[i])
 
     # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE (abs-pos; rel-pos: x = h2 Wo^T + bo) -> conv2 (implicit-GEMM forward,
     # im2col GEMMs backward) -> conv1
@@ -584,48 +615,33 @@ def _encoder_bwd(model, pk, tr, dx, g):
     g.put('frontend.conv1.conv_layer.bias', g1[:C1, 9])
 
 
-def _ctc_head_fwd(model, pk, mem):
-    """CTCAssistor's output layer on the memory (model/ctc.py:33-46) -> (logits f32 [B*T', ld], its bf16 weight)."""
-    wc = pk._w(model.assistor.output_layer.weight)
-    return ops.linear(mem, wc, _f(model.assistor.output_layer.bias), EPI_BIAS, out_f32=True, n_out=model.assistor.ld_logits), wc
+def _ctc_head(model, pk):
+    """CTCAssistor's output layer (model/ctc.py:33-46) as head_fwd / head_bwd take it: (bf16 weight, fp32 bias, ld)."""
+    lin = model.assistor.output_layer
+    return pk.w(lin.weight), _f(lin.bias), model.assistor.ld_logits
 
 
-def _ctc_head_bwd(dctc, mem, wc, V, g, resid=None):
-    """Backward of _ctc_head_fwd from dctc (bf16 [B*T', ld]): the head's gradients into g; returns the gradient of the
-    memory (+ resid)."""
-    acc = g.sink is not None
-    wname_c = 'assistor.output_layer.weight'
-    g[wname_c] = ops.linear_wgrad(dctc[:, :V], mem, out=g.out(wname_c), accumulate=acc)
-    g.put('assistor.output_layer.bias', ops.colsum(dctc)[:V])
-    wc_t = torch.zeros(mem.shape[1], dctc.shape[1], dtype=BF16, device=mem.device)
-    wc_t[:, :V] = wc.t()
-    if resid is not None:
-        return ops.linear(dctc, wc_t, None, EPI_RESID, resid=resid)
-    return ops.linear(dctc, wc_t)
+_CTC_HEAD = ('assistor.output_layer.weight', 'assistor.output_layer.bias')      # its gradients' names
 
 
-def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True, grad_sink=None, grad_scale=1.0,
-                     bf16_of=None, drop_seed=None, truth_length=None, return_ctc=False):
-    """One forward (+ backward) pass.  inputs f32 [B,T,F], mask bool [B,T], truth i64 [B,L+1] (BOS ... EOS PAD*).
-    Returns (loss 0-d f32 tensor, {parameter name -> fp32 gradient}) with names as in model.named_parameters().
-    grad_sink: name -> fp32 tensor the gradients (x grad_scale) are ADDED into (gradient accumulation buffer).
-    drop_seed: int32 device tensor [1], the dropout seed of THIS pass (read on the device); required when any
-    residual_dropout rate is non-zero.  truth_length: i32/i64 [B] label counts incl. <S/E> (targets['targets_length'],
-    data/loader.py:94) -- required when model.ctc_weight > 0: the loss is then (1 - w) * attention + w * CTC
-    (model/speech2text.py:60-62) and the CTC head's gradients flow into the encoder through the memory."""
+def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=True, grad_sink=None, grad_scale=1.0,
+                     bf16_of=None, drop_seed=None):
+    """SpeechToText.train_pass (the contract is at the top of this file).  inputs f32 [B,T,F], mask bool [B,T], truth i64
+    [B,L+1] (BOS ... EOS PAD*); the gradients are named as in model.named_parameters().  truth_length: i32/i64 [B] label
+    counts incl. <S/E> (targets['targets_length'], data/loader.py:94) -- required when model.ctc_weight > 0: the loss is
+    then (1 - w) * attention + w * CTC (model/speech2text.py:60-62), the CTC head's gradients flow into the encoder through
+    the memory, and the CTC term alone is left on model._last_ctc_loss (None without joint CTC) for SpeechToText.forward
+    to report, as the reference does."""
     enc, dec = model.encoder, model.decoder
     ctc_w = float(getattr(model, 'ctc_weight', 0.0) or 0.0)
     if ctc_w > 0.0 and truth_length is None:
         raise ValueError('forward_backward: ctc_weight > 0 needs truth_length')
     pk = TrainPack(model, bf16_of)
     dev = inputs.device
-    e_rates = [float(b.dropout_rates['residual_dropout']) for b in enc.blocks]
-    d_rates = [float(b.dropout_rates['residual_dropout']) for b in dec.blocks]
-    if drop_seed is None and any(r > 0.0 for r in e_rates + d_rates):
-        raise ValueError('forward_backward: residual_dropout > 0 needs a drop_seed tensor')
+    need_drop_seed(drop_seed, pk.rates['encoder'] + pk.rates['decoder'])
 
     # ------------------------------------------------------------------ forward
-    mem, tr = _encoder_fwd(model, pk, inputs, mask, e_rates, drop_seed)
+    mem, tr = _encoder_fwd(model, pk, inputs, mask, drop_seed)
     B, T2, lengths, d = tr.B, tr.T2, tr.lengths, enc.d_model
 
     tgt_in = truth[:, :-1].contiguous()
@@ -633,8 +649,8 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     L = tgt_in.shape[1]
     Hd = dec.n_heads
     _, dtable = dec.pos_emb.scale_and_table(L, dev)
-    y = ops.embed_posenc(tgt_in, pk.out['emb'], dtable, B * L, d, period=L)
-    d_drop = [(r, drop_seed, DEC_SITE + 3 * i) for i, r in enumerate(d_rates)]
+    y = ops.embed_posenc(tgt_in, pk.emb, dtable, B * L, d, period=L)
+    d_drop = [(r, drop_seed, DEC_SITE + 3 * i) for i, r in enumerate(pk.rates['decoder'])]
     dec_tape = []
     for p, drop in zip(pk.dec, d_drop):
         y, t = _dec_layer_fwd(p, y, mem, pk.dec_pre, B, Hd, L, T2, lengths, drop)
@@ -643,19 +659,20 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
     dec_last = y
     if pk.dec_pre:
         y = _norm(y, pk.dec_norm)
-    logits = ops.linear(y, pk.out['wout'], pk.out['bout'], EPI_BIAS, out_f32=True, n_out=pk.ld_logits)
-    sm = model.smoothing if smoothing is None else smoothing
+    logits = head_fwd(y, pk.wout, pk.bout, dec.ld_logits)
     loss_ctc, dctc = None, None
     if ctc_w > 0.0:     # CTCAssistor on the encoder states (model/ctc.py:33-52)
-        ctc_logits, wc = _ctc_head_fwd(model, pk, mem)
-        loss_ctc, _, dctc = ops.ctc_loss(ctc_logits, B, T2, V, lengths, tgt_out, truth_length.to(torch.int32).to(dev).contiguous(),
+        wc, bc, ldc = _ctc_head(model, pk)
+        loss_ctc, _, dctc = ops.ctc_loss(head_fwd(mem, wc, bc, ldc), B, T2, V, lengths, tgt_out,
+                                         truth_length.to(torch.int32).to(dev).contiguous(),
                                          model.assistor.blank, want_grad=want_grads, grad_scale=ctc_w * grad_scale)
+    model._last_ctc_loss = loss_ctc
     if not want_grads:
-        loss, _ = ops.ls_cross_entropy(logits, tgt_out, V, sm)
+        loss, _ = ops.ls_cross_entropy(logits, tgt_out, V, model.smoothing)
         if ctc_w > 0.0:
             loss = (1.0 - ctc_w) * loss + ctc_w * loss_ctc
-        return (loss, None, loss_ctc) if return_ctc else (loss, None)
-    loss, dlogits = ops.ls_cross_entropy_train(logits, tgt_out, V, sm)
+        return loss, None
+    loss, dlogits = ops.ls_cross_entropy_train(logits, tgt_out, V, model.smoothing)
     att_scale = grad_scale * (1.0 - ctc_w)
     if att_scale != 1.0:
         dlogits = ops.scale_add_table(dlogits, att_scale)                        # loss / accum_steps (trainer.py:216), x (1 - w)
@@ -663,51 +680,46 @@ def forward_backward(model, inputs, mask, truth, smoothing=None, want_grads=True
         loss = (1.0 - ctc_w) * loss + ctc_w * loss_ctc
 
     # ------------------------------------------------------------------ backward
-    g = _Grads(grad_sink)
-    dwout, dy = _output_layer_bwd(dlogits, y, pk.out['wout_t'], V, pk.tied, g, 'decoder.embedding.weight', 'decoder.output_layer')
+    g = Grads(grad_sink)
+    dy = head_bwd(dlogits, y, pk.wout, g, pk.wout_name, 'decoder.output_layer.bias')
     dmem = None
     if pk.dec_pre:
         dy = _ln_bwd(dy, dec_last, pk.dec_norm, g)
     for i in reversed(range(len(pk.dec))):
         dy, dmem = _dec_layer_bwd(pk.dec[i], dec_tape[i], dy, dmem, mem, pk.dec_pre, g, B, Hd, L, T2, lengths, d_drop[i])
-    # embedding (decoder/transformer.py:163,169)
-    _embedding_bwd(tgt_in, dy, dwout, math.sqrt(d), pk.tied, g, 'decoder.embedding.weight', 'decoder.output_layer')
+    embedding_bwd(tgt_in, dy, pk.emb, math.sqrt(d), g, 'decoder.embedding.weight')       # decoder/transformer.py:163,169
 
     dx = dmem
     if ctc_w > 0.0:     # CTC head: parameter gradients, and its gradient with respect to the memory joins the decoder's
-        dx = _ctc_head_bwd(dctc, mem, wc, V, g, resid=dmem)
+        dx = head_bwd(dctc, mem, wc, g, *_CTC_HEAD, resid=dmem)
     _encoder_bwd(model, pk, tr, dx, g)
-    return (loss, g, loss_ctc) if return_ctc else (loss, g)
+    return loss, g
 
 
 def ctc_forward_backward(model, inputs, mask, truth, truth_length, want_grads=True, grad_sink=None, grad_scale=1.0,
                          bf16_of=None, drop_seed=None):
-    """CTCModel.forward (model/ctc.py:83-96) in training mode, and its backward: front end + encoder, the CTC head, and
-    nn.CTCLoss(blank 0, 'mean', zero_infinity) against truth[:, 1:-1] with truth_length - 1 labels -- the CTC-only model
-    drops <S/E>, joint CTC keeps it.  The loss gradient (x grad_scale) runs back through the head into the shared encoder
-    backward.  Arguments and return value as forward_backward's; truth_length is required."""
-    enc = model.encoder
+    """CTCModel.train_pass: CTCModel.forward (model/ctc.py:83-96) in training mode, and its backward: front end + encoder,
+    the CTC head, and nn.CTCLoss(blank 0, 'mean', zero_infinity) against truth[:, 1:-1] with truth_length - 1 labels -- the
+    CTC-only model drops <S/E>, joint CTC keeps it.  The loss gradient (x grad_scale) runs back through the head into the
+    shared encoder backward.  Arguments as forward_backward's; truth_length is required."""
     if truth_length is None:
         raise ValueError('ctc_forward_backward: a CTCModel needs truth_length')
     pk = EncoderPack(model, bf16_of)
-    dev = inputs.device
-    e_rates = [float(b.dropout_rates['residual_dropout']) for b in enc.blocks]
-    if drop_seed is None and any(r > 0.0 for r in e_rates):
-        raise ValueError('ctc_forward_backward: residual_dropout > 0 needs a drop_seed tensor')
-    mem, tr = _encoder_fwd(model, pk, inputs, mask, e_rates, drop_seed)
+    need_drop_seed(drop_seed, pk.rates['encoder'])
+    mem, tr = _encoder_fwd(model, pk, inputs, mask, drop_seed)
     V = model.vocab_size
-    logits, wc = _ctc_head_fwd(model, pk, mem)
-    tlen = (truth_length.to(dev).to(torch.int32) - 1).contiguous()
-    loss, _, dctc = ops.ctc_loss(logits, tr.B, tr.T2, V, tr.lengths, truth[:, 1:-1].contiguous(), tlen, model.assistor.blank,
-                                 want_grad=want_grads, grad_scale=grad_scale)
+    wc, bc, ld = _ctc_head(model, pk)
+    tlen = (truth_length.to(inputs.device).to(torch.int32) - 1).contiguous()
+    loss, _, dctc = ops.ctc_loss(head_fwd(mem, wc, bc, ld), tr.B, tr.T2, V, tr.lengths, truth[:, 1:-1].contiguous(), tlen,
+                                 model.assistor.blank, want_grad=want_grads, grad_scale=grad_scale)
     if not want_grads:
         return loss, None
-    g = _Grads(grad_sink)
-    _encoder_bwd(model, pk, tr, _ctc_head_bwd(dctc, mem, wc, V, g), g)
+    g = Grads(grad_sink)
+    _encoder_bwd(model, pk, tr, head_bwd(dctc, mem, wc, g, *_CTC_HEAD), g)
     return loss, g
 
 
-def _next_drop_seed(model, device):
+def next_drop_seed(model, device):
     """The dropout seed of the next training forward (a fresh mask per forward), on the device."""
     seed = getattr(model, '_drop_seed', None)
     if seed is None or seed.device != device:
@@ -717,53 +729,36 @@ def _next_drop_seed(model, device):
     return seed
 
 
-def _model_forward_backward(model, inputs, mask, truth, truth_length, **kw):
-    """forward_backward of a SpeechToText, ctc_forward_backward of a CTCModel -> (loss, grads, joint-CTC loss or None)."""
-    from .model import CTCModel
-    if isinstance(model, CTCModel):
-        loss, grads = ctc_forward_backward(model, inputs, mask, truth, truth_length, **kw)
-        return loss, grads, None
-    return forward_backward(model, inputs, mask, truth, truth_length=truth_length, return_ctc=True, **kw)
-
-
-class _SpeechToTextLoss(torch.autograd.Function):
-    """loss = SpeechToText.forward(...) or CTCModel.forward(...) as ONE autograd node over the fp32 master parameters."""
+class _TrainingLoss(torch.autograd.Function):
+    """loss = model.train_pass(*batch) as ONE autograd node over the fp32 master parameters."""
 
     @staticmethod
-    def forward(ctx, model, inputs, mask, truth, tlen, names, *params):
+    def forward(ctx, model, batch, names, *params):
         with torch.no_grad():
-            seed = _next_drop_seed(model, inputs.device)
-            loss, grads, ctc = _model_forward_backward(model, inputs, mask, truth, tlen, drop_seed=seed)
+            loss, grads = model.train_pass(*batch, drop_seed=next_drop_seed(model, batch[0].device))
         ctx.grads = [grads.get(n) for n in names]
         ctx.shapes = [p.shape for p in params]
-        model._last_ctc_loss = ctc
         return loss.clone()
 
     @staticmethod
     def backward(ctx, gloss):
-        out = []
-        for gr, shp in zip(ctx.grads, ctx.shapes):
-            out.append(None if gr is None else (gr.view(shp) * gloss))
-        return (None, None, None, None, None, None) + tuple(out)
+        return (None, None, None) + tuple(None if gr is None else gr.view(shp) * gloss
+                                          for gr, shp in zip(ctx.grads, ctx.shapes))
 
 
-def loss_with_grad(model, inputs, mask, truth, truth_length=None):
-    """Training-mode SpeechToText.forward or CTCModel.forward: (loss tensor whose .backward() fills `.grad` of every parameter,
-    joint-CTC loss or None)."""
+def loss_with_grad(model, *batch):
+    """A model's forward in training mode with gradients enabled: the loss tensor whose .backward() fills `.grad` of every
+    parameter."""
     named = [(n, p) for n, p in model.named_parameters() if p.requires_grad]
-    names = [n for n, _ in named]
-    loss = _SpeechToTextLoss.apply(model, inputs, mask, truth, truth_length, names, *[p for _, p in named])
-    return loss, getattr(model, '_last_ctc_loss', None)
+    return _TrainingLoss.apply(model, batch, [n for n, _ in named], *[p for _, p in named])
 
 
-def loss_train_mode(model, inputs, mask, truth, truth_length=None):
-    """Training-mode SpeechToText.forward or CTCModel.forward without gradients (model.train() under torch.no_grad(), e.g. a
-    validation loop that does not call eval()): the forward the reference runs in train() -- for a Conformer, BatchNorm with
-    the batch statistics, and the running statistics updated -- with no backward.  -> (loss, joint-CTC loss or None)."""
+def loss_train_mode(model, *batch):
+    """A model's forward in training mode without gradients (model.train() under torch.no_grad(), e.g. a validation loop
+    that does not call eval()): the forward the reference runs in train() -- dropout on, a Conformer's BatchNorm with the
+    batch statistics and its running statistics updated -- with no backward.  -> loss."""
     with torch.no_grad():
-        loss, _, ctc = _model_forward_backward(model, inputs, mask, truth, truth_length, want_grads=False,
-                                               drop_seed=_next_drop_seed(model, inputs.device))
-    return loss, ctc
+        return model.train_pass(*batch, want_grads=False, drop_seed=next_drop_seed(model, batch[0].device))[0]
 
 
 def transformer_lr(step, model_size, warmup_steps, factor=1.0):
@@ -775,20 +770,11 @@ class FusedTrainer:
     """The inner step of Trainer.train_one_epoch (trainer.py:206-234) on flat fp32 buffers:
     forward + hand-written backward -> (data-parallel) gradient all-reduce over NCCL -> global-norm clip + Adam in two
     kernels, no host synchronisation.  Parameters become views into one flat buffer (state_dict keys / shapes unchanged).
-    `model` is a SpeechToText, a CTCModel or a TransformerLanguageModel (transformer_lm.yaml trains with the same scheduler)."""
+    `model` is any model with the training contract at the top of this file."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6, clip_grad=5.0, model_size=256,
                  warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True):
-        from . import lm          # lm imports this module
-        from .model import CTCModel
-        if isinstance(model, lm.RecurrentLanguageModel):
-            raise NotImplementedError('FusedTrainer: the recurrent LM trains with a step-linear scheduler that is not on the '
-                                      'device; train it through loss.backward() and a torch optimizer')
-        self._lm_forward_backward = None
-        if isinstance(model, lm.TransformerLanguageModel):
-            lm.check_trainable(model)
-            self._lm_forward_backward = lm.transformer_forward_backward
-        self._ctc = isinstance(model, CTCModel)
+        model.check_fused_trainer()
         self.model = model
         # parameters the forward never reads (a Conformer's post_ffn) stay out of the flat buffers: no gradient, no weight decay
         unused = unused_parameters(model)
@@ -863,20 +849,12 @@ class FusedTrainer:
         return self.flat_bf16[o:o + k].view(shape)
 
     def _micro(self, batch):
-        """forward + backward of one micro-batch; gradients / accum_steps are ADDED into the flat buffer by the backward
-        kernels themselves (no per-parameter add).  batch: (inputs, mask, truth, truth_length or None) of a SpeechToText,
-        (inputs, targets) of a language model; a CTCModel's as a SpeechToText's."""
+        """forward + backward of one micro-batch (what model.train_batch returned); gradients / accum_steps are ADDED into
+        the flat buffer by the backward kernels themselves (no per-parameter add)."""
         self.flat_bf16.copy_(self.flat_p)
         self.drop_seed.add_(1)
-        kw = dict(grad_sink=self.sink, grad_scale=1.0 / self.accum_steps, bf16_of=self._bf16_of, drop_seed=self.drop_seed)
-        if self._lm_forward_backward is not None:
-            loss, _ = self._lm_forward_backward(self.model, *batch, **kw)
-        else:
-            inputs, mask, truth, tlen = batch
-            if self._ctc:
-                loss, _ = ctc_forward_backward(self.model, inputs, mask, truth, tlen, **kw)
-            else:
-                loss, _ = forward_backward(self.model, inputs, mask, truth, truth_length=tlen, **kw)
+        loss, _ = self.model.train_pass(*batch, grad_sink=self.sink, grad_scale=1.0 / self.accum_steps, bf16_of=self._bf16_of,
+                                        drop_seed=self.drop_seed)
         return loss
 
     def _graph_for(self, batch):
@@ -920,25 +898,15 @@ class FusedTrainer:
         self._graphs[key] = ent       # (re-)insert as most recently used
         return ent
 
-    def step(self, inputs, *batch, truth_length=None):
+    def step(self, *batch, truth_length=None):
         """One micro-batch; every `accum_steps` calls an optimizer step.  Returns the (un-scaled) loss tensor.
-        SpeechToText: step(inputs, mask, truth, truth_length=None); truth_length (targets['targets_length']) is needed by
-        joint-CTC models only.  CTCModel: step(inputs, mask, truth, truth_length), truth_length required.
-        TransformerLanguageModel: step(inputs, targets), i64 [N, L] each (the reference's inputs['inputs'] and
-        targets['targets'])."""
-        if self._lm_forward_backward is not None:
-            if len(batch) != 1 or truth_length is not None:
-                raise TypeError('FusedTrainer.step(inputs, targets) for a language model')
-            batch = (inputs, batch[0])
-        else:
-            if len(batch) == 3:
-                batch, truth_length = batch[:2], batch[2]
-            if len(batch) != 2:
-                raise TypeError('FusedTrainer.step(inputs, mask, truth, truth_length=None) for a SpeechToText model')
-            if self._ctc and truth_length is None:
-                raise TypeError('FusedTrainer.step(inputs, mask, truth, truth_length) for a CTCModel: truth_length is required')
-            # forward_backward reads the label counts as int32
-            batch = (inputs,) + batch + (None if truth_length is None else truth_length.to(torch.int32),)
+        The arguments are the model's batch, which its train_batch validates (TypeError): step(inputs, mask, truth,
+        truth_length=None) for a SpeechToText, truth_length (targets['targets_length']) needed by joint-CTC models only;
+        the same with truth_length required for a CTCModel; step(inputs, targets), i64 [N, L] each (the reference's
+        inputs['inputs'] and targets['targets']), for a TransformerLanguageModel."""
+        if truth_length is not None:
+            batch += (truth_length,)
+        batch = self.model.train_batch(*batch)
         with torch.no_grad():
             # data parallel: BatchNorm running statistics follow the first rank's (DistributedDataParallel's
             # broadcast_buffers): each rank's forward updates them from its own shard, so they would drift apart
