@@ -361,6 +361,19 @@ int otb_ctc_greedy(const float* top_lp, const int32_t* top_id, int ldk, int B, i
 int otb_ctc_prefix_beam(const float* top_lp, const int32_t* top_id, int K, int B, int T, const int32_t* in_len, int blank, int beam,
                         int32_t* nodes, int32_t* ids, int32_t* lengths, float* scores, void* stream);
 
+/* CTC forced alignment: the best path (Viterbi) through the CTC trellis of each utterance's target, one CTA per utterance.
+ * rows f32 [B*T, ld]: log-probs when lse is NULL, else logits with lse f32 [B*T] each frame's log-sum-exp (lp = row - lse);
+ * only the columns the targets name and the blank are read.  in_len i32 [B] valid frames; targets i64 [B, ldt], the first
+ * tgt_len[b] entries count (0 <= tgt_len <= max_tgt <= 1023); bp u8 [B, T, 2 max_tgt + 1] workspace (back-pointers).
+ * labels i32 [B, T] = the token aligned to each frame (blank included), -1 at or past in_len; frame_scores f32 [B, T] = its
+ * log-prob (-inf where the label is -1); spans i32 [B, max_tgt, 2] = [start, end) of each target token in frames, -1 past
+ * tgt_len; path_score f32 [B] = the path's log-prob.  Ties prefer the state itself, then one back, then two back; the end
+ * state prefers the last token's blank.  An utterance without an alignment of finite log-prob (too few frames, a blank or
+ * out-of-range token, tgt_len outside 0..max_tgt) gets path_score -inf and labels / spans -1. */
+int otb_ctc_align(const float* rows, int ld, int B, int T, int V, const float* lse, const int32_t* in_len, const int64_t* targets,
+                  int ldt, const int32_t* tgt_len, int max_tgt, int blank, uint8_t* bp, int32_t* labels, float* frame_scores,
+                  int32_t* spans, float* path_score, void* stream);
+
 /* Conv2d front end backward (frontend/conv.py:50-76 under autograd).  h1 = conv1 activation buffer (layout of
  * otb_conv1_relu).  col bf16 [B*T2*F2, 9*C1] = im2col of h1 for conv2 (k = (kh*3+kw)*C1 + c): conv2's weight gradient is
  * otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu folds dcol

@@ -487,6 +487,17 @@ int otb_ctc_prefix_beam(const float* top_lp, const int32_t* top_id, int K, int B
                                                       lengths, scores));
 }
 
+int otb_ctc_align(const float* rows, int ld, int B, int T, int V, const float* lse, const int32_t* in_len, const int64_t* targets,
+                  int ldt, const int32_t* tgt_len, int max_tgt, int blank, uint8_t* bp, int32_t* labels, float* frame_scores,
+                  int32_t* spans, float* path_score, void* stream) {
+    if (!rows || !in_len || !tgt_len || !bp || !labels || !frame_scores || !path_score || (max_tgt > 0 && (!targets || !spans)))
+        return fail("otb_ctc_align", "null operand");
+    if (ld < V) return fail("otb_ctc_align", "row pitch < V");
+    if (max_tgt > 0 && ldt < max_tgt) return fail("otb_ctc_align", "target row pitch < max_tgt");
+    RET("otb_ctc_align", ctc_align_launch(ST(stream), rows, ld, B, T, V, lse, in_len, reinterpret_cast<const long long*>(targets), ldt,
+                                          tgt_len, max_tgt, blank, bp, labels, frame_scores, spans, path_score));
+}
+
 int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
     int T1, F1, T2, F2;
     if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;

@@ -201,6 +201,9 @@ const char* ctc_greedy_launch(cudaStream_t st, const float* top_lp, const int* t
                               int blank, int* ids, int* lengths, float* scores);
 const char* ctc_prefix_beam_launch(cudaStream_t st, const float* top_lp, const int* top_id, int K, int B, int T, const int* in_len,
                                    int blank, int beam, int* nodes, int* ids, int* lengths, float* scores);
+const char* ctc_align_launch(cudaStream_t st, const float* rows, int ld, int B, int T, int V, const float* lse, const int* in_len,
+                             const long long* targets, int ldt, const int* tgt_len, int max_tgt, int blank, uint8_t* bp, int* labels,
+                             float* frame_scores, int* spans, float* path_score);
 
 const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const int* n_samples, int B, const float* window,
                          const float* bank, const int* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift,

@@ -17,6 +17,25 @@ BuildEncoder = {'transformer': TransformerEncoder, 'conformer': ConformerEncoder
 BuildDecoder = {'transformer': TransformerDecoder}
 
 
+def ctc_align_logits(logits, lengths, B, T2, V, tokens, n_tokens, blank):
+    """ops.ctc_align of a CTC head's logits f32 [B*T', ld] (first V columns valid) against tokens [B, Lmax] (n_tokens [B]
+    of each row count), after the head's log-softmax."""
+    lp = ops.log_softmax(logits, V).view(B, T2, V)
+    n_tokens = n_tokens.to(device=logits.device, dtype=torch.int32).contiguous()
+    return ops.ctc_align(lp, lengths, tokens, n_tokens, blank=blank)
+
+
+def encoder_frames_to_input(spans, frame_shift=None):
+    """Spans [start, end) in encoder frames (CTCModel.align, SpeechToText.align, CTCRecognizer.recognize_spans) -> spans in
+    input (fbank) frames, [4 start, 4 (end - 1) + 7): the front end's two 3x3 stride-2 convolutions, which do not pad in
+    time, make encoder frame t see input frames [4t, 4t + 7).  With frame_shift (seconds between input frames, e.g. 0.01)
+    the result is in seconds, float64.  Entries of -1 (no span) stay -1."""
+    out = torch.stack((4 * spans[..., 0], 4 * spans[..., 1] + 3), dim=-1)
+    if frame_shift is not None:
+        out = out.double() * frame_shift
+    return torch.where(spans < 0, -1, out)
+
+
 class CTCAssistor(nn.Module):
     """model/ctc.py:12-66: the joint-CTC head, Linear(hidden, vocab) + nn.CTCLoss(blank = 0, zero_infinity).  Parameter
     holder (key `output_layer.*`, checkpoint section 'ctc'); compute is the wgmma GEMM + otb_ctc_loss."""
@@ -104,6 +123,19 @@ class SpeechToText(nn.Module):
             return (1 - self.ctc_weight) * loss + self.ctc_weight * lc, {'CTCLoss': float(lc)}
         return loss, None
 
+    def align(self, inputs, inputs_mask, targets, targets_length):
+        """CTC forced alignment through the joint-CTC head, of the targets its loss scores: targets[:, 1:] with
+        targets_length tokens (the reference's collate: <S/E> first, targets_length counts the labels after it, the closing
+        <S/E> included).  -> ops.ctc_align's (labels i32 [B, T'], frame_scores f32 [B, T'], spans i32 [B, L, 2],
+        path_score f32 [B]) on the device; spans are in encoder frames (encoder_frames_to_input converts them).  Runs the
+        inference path, also in train().  A model without a CTC head (ctc_weight 0) raises ValueError."""
+        if self.ctc_weight <= 0.0:
+            raise ValueError('SpeechToText.align needs the joint-CTC head: this model has ctc_weight 0')
+        with torch.no_grad():
+            mem, lengths, B, T2 = self.encode_bf16(inputs, inputs_mask)
+            return ctc_align_logits(self.assistor.logits_bf16(mem), lengths, B, T2, self.decoder.vocab_size, targets[:, 1:],
+                                    targets_length, self.assistor.blank)
+
     train_pass = train.forward_backward
 
     def train_batch(self, inputs, mask, truth, truth_length=None):
@@ -184,6 +216,19 @@ class CTCModel(nn.Module):
         return ops.log_softmax(logits, self.vocab_size).view(B, T2, -1), lengths
 
     recognize = inference
+
+    def align(self, inputs, inputs_mask, targets, targets_length):
+        """CTC forced alignment of the transcripts, in forward's convention: targets[:, 1:-1] with targets_length - 1 tokens
+        (the reference's collate, <S/E> at both ends and counted in targets_length).  One pass of the front end, encoder and
+        head, then otb_ctc_align.  -> (labels i32 [B, T'] the token of each encoder frame, blank included, -1 past the
+        utterance; frame_scores f32 [B, T'] its log-prob; spans i32 [B, L, 2] [start, end) of each token in encoder frames
+        (encoder_frames_to_input converts them); path_score f32 [B] the best alignment's log-prob), on the device.  An
+        utterance too short for its transcript gets -inf and -1.  Runs the inference path, also in train(): a Conformer's
+        BatchNorm uses its running statistics and no dropout is applied."""
+        with torch.no_grad():
+            logits, lengths, B, T2 = self.logits_bf16(inputs, inputs_mask)
+            return ctc_align_logits(logits, lengths, B, T2, self.vocab_size, targets[:, 1:-1], targets_length - 1,
+                                    self.assistor.blank)
 
     train_pass = train.ctc_forward_backward
     check_fused_trainer = SpeechToText.check_fused_trainer

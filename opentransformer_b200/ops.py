@@ -687,6 +687,52 @@ def ctc_prefix_beam(top_lp, top_id, B, T, in_len, beam, blank=0):
     return ids, lengths, scores
 
 
+CTC_ALIGN_MAX_TOKENS = 1023
+
+
+def ctc_align(rows, in_len, targets, tgt_len, lse=None, blank=0):
+    """CTC forced alignment (otb_ctc_align): the best path of each utterance through the CTC trellis of its target, blank =
+    `blank`.  rows f32 [B, T', V] with unit column stride (any row pitch, e.g. rows[:, :, :V] of a padded head output):
+    log-probs, or logits when lse f32 [B, T'] gives each frame's log-sum-exp.  in_len i32 [B] valid frames; targets int
+    [B, Lmax] (Lmax <= 1023), of which the first tgt_len[b] (i32 [B]) count.
+    -> (labels i32 [B, T'] the token of each frame, blank included, -1 at or past in_len; frame_scores f32 [B, T'] its
+    log-prob (-inf where the label is -1); spans i32 [B, Lmax, 2] [start, end) of each target token in frames of `rows`,
+    -1 past tgt_len; path_score f32 [B]).  An utterance without an alignment (fewer frames than tokens plus adjacent
+    repeats, a blank or out-of-range token, no frames for a non-empty target) gets path_score -inf and labels / spans -1.
+    Ties prefer staying in a state, then one state back, then two; the end prefers the last token's blank."""
+    if rows.dim() != 3 or rows.stride(2) != 1 or rows.stride(0) != rows.shape[1] * rows.stride(1):
+        raise ValueError(f'ctc_align: rows must be [B, T, V] with unit column stride and evenly pitched rows, got '
+                         f'{tuple(rows.shape)} strides {rows.stride()}')
+    B, T, V = rows.shape
+    if targets.dim() != 2 or targets.shape[0] != B:
+        raise ValueError(f'ctc_align: targets must be [B = {B}, Lmax], got {tuple(targets.shape)}')
+    if targets.shape[1] > CTC_ALIGN_MAX_TOKENS:
+        raise ValueError(f'ctc_align: targets of up to {CTC_ALIGN_MAX_TOKENS} tokens are supported, got {targets.shape[1]}')
+    _ctc_lengths(in_len, B)
+    _ctc_lengths(tgt_len, B)
+    if lse is not None and tuple(lse.shape) != (B, T):
+        raise ValueError(f'ctc_align: lse must be [B = {B}, T = {T}], got {tuple(lse.shape)}')
+    if not rows.is_cuda:
+        raise RuntimeError('rows must be a CUDA tensor: the CUDA hot path has no CPU fallback')
+    if rows.dtype != torch.float32:
+        raise TypeError(f'rows must be torch.float32, got {rows.dtype}')
+    _need(in_len, torch.int32, 'in_len'); _need(tgt_len, torch.int32, 'tgt_len')
+    if lse is not None:
+        _need(lse, torch.float32, 'lse')
+    targets = targets.to(device=rows.device, dtype=torch.int64).contiguous()
+    Lmax, dev = targets.shape[1], rows.device
+    bp = torch.empty(B, T, 2 * Lmax + 1, dtype=torch.uint8, device=dev)
+    labels = torch.empty(B, T, dtype=torch.int32, device=dev)
+    scores = torch.empty(B, T, dtype=torch.float32, device=dev)
+    spans = torch.empty(B, Lmax, 2, dtype=torch.int32, device=dev)
+    path = torch.empty(B, dtype=torch.float32, device=dev)
+    check(_lib.lib().otb_ctc_align(_p(rows), rows.stride(1), B, T, V, _p(lse), _p(in_len), _p(targets) if Lmax else None,
+                                   max(Lmax, 1), _p(tgt_len), Lmax, blank, _p(bp), _p(labels), _p(scores),
+                                   _p(spans) if Lmax else None, _p(path), _stream()), 'otb_ctc_align')
+    _count()
+    return labels, scores, spans, path
+
+
 def conv_im2col(h1, B, T, F, C1):
     _, _, T2, F2 = conv_geometry(T, F)
     col = torch.empty(B * T2 * F2, 9 * C1, dtype=BF16, device=h1.device)

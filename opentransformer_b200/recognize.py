@@ -16,6 +16,7 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
 import torch
 
 from . import ops
+from .model import ctc_align_logits
 
 PAD, BOS, EOS = 0, 1, 1   # otrans/data/__init__.py:7-10
 
@@ -377,15 +378,30 @@ class CTCRecognizer(Recognizer):
         on the device.  nbest is 1 in greedy mode (score: the best path's log-prob) and beam_width in beam mode (score:
         the prefix's log-probability over all its alignments)."""
         with torch.no_grad():
+            return self._decode(*self.model.logits_bf16(inputs, inputs_mask))
+
+    def _decode(self, logits, lengths, B, T2):
+        V = self.model.vocab_size
+        if self.mode == 'greedy':
+            lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, 1)
+            ids, n, sc = ops.ctc_greedy(lp, tok, B, T2, lengths, self.model.assistor.blank)
+            return ids.long().view(B, 1, T2), n.view(B, 1), sc.view(B, 1)
+        lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, min(CTC_CUTOFF_TOP_N, V))
+        ids, n, sc = ops.ctc_prefix_beam(lp, tok, B, T2, lengths, self.beam_width, self.model.assistor.blank)
+        return ids.long(), n, sc
+
+    def recognize_spans(self, inputs, inputs_mask):
+        """recognize_ids, plus where each token of the 1-best lies: the 1-best is force-aligned (otb_ctc_align) against the
+        same logits, so the front end and encoder run once.  -> (ids, lengths, scores as recognize_ids; spans i32
+        [B, min(T', 1023), 2] [start, end) in encoder frames of the 1-best's tokens, -1 past its length, and -1 throughout
+        for a 1-best longer than the aligner's 1023 tokens), on the device.
+        model.encoder_frames_to_input converts the spans to input frames or seconds."""
+        with torch.no_grad():
             logits, lengths, B, T2 = self.model.logits_bf16(inputs, inputs_mask)
-            V = self.model.vocab_size
-            if self.mode == 'greedy':
-                lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, 1)
-                ids, n, sc = ops.ctc_greedy(lp, tok, B, T2, lengths, self.model.assistor.blank)
-                return ids.long().view(B, 1, T2), n.view(B, 1), sc.view(B, 1)
-            lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, min(CTC_CUTOFF_TOP_N, V))
-            ids, n, sc = ops.ctc_prefix_beam(lp, tok, B, T2, lengths, self.beam_width, self.model.assistor.blank)
-            return ids.long(), n, sc
+            ids, n, sc = self._decode(logits, lengths, B, T2)
+            best = ids[:, 0, :min(T2, ops.CTC_ALIGN_MAX_TOKENS)]
+            _, _, spans, _ = ctc_align_logits(logits, lengths, B, T2, self.model.vocab_size, best, n[:, 0], self.model.assistor.blank)
+            return ids, n, sc, spans
 
     def recognize(self, inputs, inputs_mask):
         """recognize/ctc.py:27-36: translate() of the 1-best token lists (the id lists when idx2unit is None)."""
