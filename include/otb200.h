@@ -374,6 +374,31 @@ int otb_ctc_align(const float* rows, int ld, int B, int T, int V, const float* l
                   int ldt, const int32_t* tgt_len, int max_tgt, int blank, uint8_t* bp, int32_t* labels, float* frame_scores,
                   int32_t* spans, float* path_score, void* stream);
 
+/* CTC prefix scoring for joint CTC/attention decoding (Watanabe et al. 2017): the CTC term of the beam search's step score.
+ * lp f32 [B*T, ld] log-probs of the joint-CTC head, in_len i32 [B] valid frames.  For a hypothesis g (its tokens after
+ * <S/E>), gamma(g)[t] = {log-prob that frames 0..t emit exactly g ending in a non-blank, ... ending in a blank} and psi(g) =
+ * the log-probability that the labels start with g; the closing <S/E> is a label like any other, so psi(g <S/E>) is the
+ * log-probability of the whole label sequence g <S/E>.  gamma f32 [2, N, T, 2] and psi f32 [2, N] hold the state of the N
+ * hypotheses of a search; the half in use is the parity of its step counter (st->ctrl[0]).
+ * otb_ctc_prefix_init: gamma and psi of the empty prefix for every row, in half 0. */
+int otb_ctc_prefix_init(const float* lp, int ld, int B, int T, const int32_t* in_len, int blank, int beam, float* gamma,
+                        float* psi, void* stream);
+/* One step's scores: for every unfinished hypothesis n and each of its P candidates (cand_val f32 / cand_id i32 [N, P] of
+ * otb_logsoftmax_topk with k = P, beam <= P <= 16; cand_val = logp_att + lm_weight * lm_logp[cand_id] when lm_logp is given)
+ * gamma_cand f32 [N, P, T, 2] and psi_cand f32 [N, P] of the hypothesis extended by the candidate, the joint score
+ * (1 - ctc_weight) logp_att + ctc_weight (psi_cand - psi) + lm_weight lm_logp (-inf where psi_cand is -inf, never NaN), and
+ * the `beam` best candidates by it into out_val f32 / out_idx i32 [N, beam] (descending, ties to the lower id), the layout
+ * otb_beam_step_topk takes.  Does nothing once the search has ended. */
+int otb_ctc_prefix_score(const float* lp, int ld, int T, int V, const int32_t* in_len, int blank, const float* gamma,
+                         const float* psi, const float* cand_val, const int32_t* cand_id, int P, const float* lm_logp, int ld_lm,
+                         float lm_weight, float ctc_weight, const otb_beam_state* st, float* gamma_cand, float* psi_cand,
+                         float* out_val, int32_t* out_idx, void* stream);
+/* After otb_beam_step_topk: every new row takes gamma_cand / psi_cand of its parent's candidate that names its token into
+ * the other half of gamma / psi; a row whose token is <S/E> keeps its parent's state.  Does nothing once the search has
+ * ended. */
+int otb_ctc_prefix_advance(const otb_beam_state* st, const int32_t* cand_id, int P, int T, const int32_t* in_len,
+                           const float* gamma_cand, const float* psi_cand, float* gamma, float* psi, void* stream);
+
 /* Conv2d front end backward (frontend/conv.py:50-76 under autograd).  h1 = conv1 activation buffer (layout of
  * otb_conv1_relu).  col bf16 [B*T2*F2, 9*C1] = im2col of h1 for conv2 (k = (kh*3+kw)*C1 + c): conv2's weight gradient is
  * otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu folds dcol

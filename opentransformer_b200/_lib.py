@@ -95,6 +95,10 @@ _SIGS = {
     'otb_ctc_greedy': (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P]),
     'otb_ctc_prefix_beam': (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P]),
     'otb_ctc_align': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
+    'otb_ctc_prefix_init': (c_int, [_P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P]),
+    'otb_ctc_prefix_score': (c_int, [_P, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P, c_int, _P, c_int, c_float, c_float,
+                                     POINTER(BeamStateC), _P, _P, _P, _P, _P]),
+    'otb_ctc_prefix_advance': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     'otb_conv_im2col': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv_col2im_relu': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv1_wgrad': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),

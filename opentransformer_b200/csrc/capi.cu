@@ -498,6 +498,31 @@ int otb_ctc_align(const float* rows, int ld, int B, int T, int V, const float* l
                                           tgt_len, max_tgt, blank, bp, labels, frame_scores, spans, path_score));
 }
 
+int otb_ctc_prefix_init(const float* lp, int ld, int B, int T, const int32_t* in_len, int blank, int beam, float* gamma,
+                        float* psi, void* stream) {
+    if (!lp || !in_len || !gamma || !psi) return fail("otb_ctc_prefix_init", "null operand");
+    if (blank < 0 || blank >= ld) return fail("otb_ctc_prefix_init", "bad blank id");
+    RET("otb_ctc_prefix_init", ctc_prefix_init_launch(ST(stream), lp, ld, B, T, in_len, blank, beam, gamma, psi));
+}
+
+int otb_ctc_prefix_score(const float* lp, int ld, int T, int V, const int32_t* in_len, int blank, const float* gamma,
+                         const float* psi, const float* cand_val, const int32_t* cand_id, int P, const float* lm_logp, int ld_lm,
+                         float lm_weight, float ctc_weight, const otb_beam_state* st, float* gamma_cand, float* psi_cand,
+                         float* out_val, int32_t* out_idx, void* stream) {
+    if (!lp || !in_len || !gamma || !psi || !cand_val || !cand_id || !st || !gamma_cand || !psi_cand || !out_val || !out_idx)
+        return fail("otb_ctc_prefix_score", "null operand");
+    RET("otb_ctc_prefix_score", ctc_prefix_score_launch(ST(stream), lp, ld, T, V, in_len, blank, gamma, psi, cand_val, cand_id, P,
+                                                        lm_logp, ld_lm, lm_weight, ctc_weight, to_state(st), gamma_cand, psi_cand,
+                                                        out_val, out_idx));
+}
+
+int otb_ctc_prefix_advance(const otb_beam_state* st, const int32_t* cand_id, int P, int T, const int32_t* in_len,
+                           const float* gamma_cand, const float* psi_cand, float* gamma, float* psi, void* stream) {
+    if (!st || !cand_id || !in_len || !gamma_cand || !psi_cand || !gamma || !psi) return fail("otb_ctc_prefix_advance", "null operand");
+    RET("otb_ctc_prefix_advance", ctc_prefix_advance_launch(ST(stream), to_state(st), cand_id, P, T, in_len, gamma_cand, psi_cand,
+                                                            gamma, psi));
+}
+
 int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
     int T1, F1, T2, F2;
     if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;

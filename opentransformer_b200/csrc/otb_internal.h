@@ -205,6 +205,15 @@ const char* ctc_align_launch(cudaStream_t st, const float* rows, int ld, int B, 
                              const long long* targets, int ldt, const int* tgt_len, int max_tgt, int blank, uint8_t* bp, int* labels,
                              float* frame_scores, int* spans, float* path_score);
 
+const char* ctc_prefix_init_launch(cudaStream_t stream, const float* lp, int ld, int B, int T, const int* in_len, int blank,
+                                   int beam, float* gamma, float* psi);
+const char* ctc_prefix_score_launch(cudaStream_t stream, const float* lp, int ld, int T, int V, const int* in_len, int blank,
+                                    const float* gamma, const float* psi, const float* cand_val, const int* cand_id, int P,
+                                    const float* lm_logp, int ld_lm, float lm_weight, float ctc_weight, BeamState st,
+                                    float* gamma_cand, float* psi_cand, float* out_val, int* out_idx);
+const char* ctc_prefix_advance_launch(cudaStream_t stream, BeamState st, const int* cand_id, int P, int T, const int* in_len,
+                                      const float* gamma_cand, const float* psi_cand, float* gamma, float* psi);
+
 const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const int* n_samples, int B, const float* window,
                          const float* bank, const int* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift,
                          float preemph);

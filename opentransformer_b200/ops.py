@@ -733,6 +733,56 @@ def ctc_align(rows, in_len, targets, tgt_len, lse=None, blank=0):
     return labels, scores, spans, path
 
 
+CTC_PREFIX_MAX_CANDIDATES = 16      # KMAX of csrc/beam_common.cuh
+
+
+class CTCPrefixState:
+    """Device buffers of CTC prefix scoring (csrc/ctc_prefix.cu) for one search of N = batch * beam hypotheses over
+    log-probs lp f32 [batch * T, V] with P candidates per hypothesis: gamma f32 [2, N, T, 2] and psi f32 [2, N] of the
+    hypotheses (ping-pong on the step counter's parity), gamma_cand f32 [N, P, T, 2], psi_cand f32 [N, P] and the
+    candidates cand_val f32 / cand_id i32 [N, P] of one step."""
+
+    def __init__(self, batch, beam, T, V, P, device, blank=0):
+        if not beam <= P <= CTC_PREFIX_MAX_CANDIDATES:
+            raise ValueError(f'CTC prefix scoring takes beam <= P <= {CTC_PREFIX_MAX_CANDIDATES} candidates, got beam {beam}, P {P}')
+        self.B, self.beam, self.T, self.V, self.P, self.blank = batch, beam, T, V, P, blank
+        N = batch * beam
+        f32 = dict(dtype=torch.float32, device=device)
+        self.lp = torch.zeros(batch * T, V, **f32)
+        self.gamma = torch.zeros(2, N, T, 2, **f32)
+        self.psi = torch.zeros(2, N, **f32)
+        self.gamma_cand = torch.zeros(N, P, T, 2, **f32)
+        self.psi_cand = torch.zeros(N, P, **f32)
+        self.cand_val = torch.zeros(N, P, **f32)
+        self.cand_id = torch.zeros(N, P, dtype=torch.int32, device=device)
+
+    def init(self, in_len):
+        """gamma / psi of the empty prefix from self.lp (otb_ctc_prefix_init); in_len i32 [batch] valid frames."""
+        _ctc_lengths(in_len, self.B)
+        _need(in_len, torch.int32, 'in_len')
+        check(_lib.lib().otb_ctc_prefix_init(_p(self.lp), self.lp.stride(0), self.B, self.T, _p(in_len), self.blank, self.beam,
+                                             _p(self.gamma), _p(self.psi), _stream()), 'otb_ctc_prefix_init')
+        _count()
+
+    def score(self, state, in_len, ctc_weight, out_val, out_idx, lm_logp=None, lm_weight=0.0):
+        """otb_ctc_prefix_score on self.cand_val / self.cand_id (logsoftmax_topk with k = P of this step): fills gamma_cand /
+        psi_cand and writes each hypothesis' `beam` best candidates by the joint score to out_val f32 / out_idx i32
+        [N, beam], what BeamState.step_topk takes."""
+        check(_lib.lib().otb_ctc_prefix_score(_p(self.lp), self.lp.stride(0), self.T, self.V, _p(in_len), self.blank,
+                                              _p(self.gamma), _p(self.psi), _p(self.cand_val), _p(self.cand_id), self.P,
+                                              _p(lm_logp), lm_logp.stride(0) if lm_logp is not None else 0, lm_weight,
+                                              ctc_weight, ctypes.byref(state.c), _p(self.gamma_cand), _p(self.psi_cand),
+                                              _p(out_val), _p(out_idx), _stream()), 'otb_ctc_prefix_score')
+        _count()
+
+    def advance(self, state, in_len):
+        """otb_ctc_prefix_advance, after state.step_topk: the surviving hypotheses take their candidates' gamma / psi."""
+        check(_lib.lib().otb_ctc_prefix_advance(ctypes.byref(state.c), _p(self.cand_id), self.P, self.T, _p(in_len),
+                                                _p(self.gamma_cand), _p(self.psi_cand), _p(self.gamma), _p(self.psi), _stream()),
+              'otb_ctc_prefix_advance')
+        _count()
+
+
 def conv_im2col(h1, B, T, F, C1):
     _, _, T2, F2 = conv_geometry(T, F)
     col = torch.empty(B * T2 * F2, 9 * C1, dtype=BF16, device=h1.device)

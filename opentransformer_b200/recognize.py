@@ -11,7 +11,9 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
     K/V live in a per-hypothesis cache addressed through a 4-byte ancestry table, and one step is
     a fixed sequence of kernels captured in a CUDA graph and replayed;
   * beam step: one kernel per step (top-k, finished masking, pruning, back-pointers), no host sync
-    inside the loop except a 4-byte "all ended" poll every few steps.
+    inside the loop except a 4-byte "all ended" poll every few steps;
+  * joint CTC/attention decoding (ctc_weight > 0, which the reference stores and never reads): the CTC prefix score of the
+    joint-CTC head re-ranks each hypothesis' best candidates inside the step (csrc/ctc_prefix.cu, DESIGN.md 4.9).
 """
 import torch
 
@@ -91,9 +93,14 @@ class BeamDecoder:
 
     Buffers are allocated once; one decode step (decoder on the newest token -> log-softmax -> beam
     kernel) is captured into a CUDA graph on first use and replayed for every step.
+
+    ctc = (assistor, weight, P) adds the CTC prefix term of joint CTC/attention decoding (DESIGN.md 4.9): setup() takes
+    the head's log-probs, and a step scores each hypothesis' P best tokens with
+    (1 - weight) logp_att + weight (psi(g c) - psi(g)) + lm_weight lm before the beam kernel selects among the `beam`
+    best of them.  The persistent kernel does not take the term, so it is off then.
     """
 
-    def __init__(self, decoder, batch, beam, T, max_len, device, use_graph=True, persistent=False, keep_logp=None):
+    def __init__(self, decoder, batch, beam, T, max_len, device, use_graph=True, persistent=False, keep_logp=None, ctc=None):
         self.dec = decoder
         self.B, self.beam, self.T, self.Lmax = batch, beam, T, max_len
         self.N = batch * beam
@@ -118,10 +125,16 @@ class BeamDecoder:
         self.lm_weight = 0.0
         if decoder.pos_emb.scale_learnable:
             raise NotImplementedError('decoder with learnable positional scale')
+        self.ctc = self.ctc_head = None
+        self.ctc_weight = 0.0
+        if ctc is not None:
+            self.ctc_head, weight, P = ctc
+            self.ctc_weight = float(weight)
+            self.ctc = ops.CTCPrefixState(batch, beam, T, decoder.vocab_size, P, device, blank=self.ctc_head.blank)
         # persistent path: the whole loop in ONE launch (csrc/decode_group.cu: row groups of <= 128 hypotheses x 16 CTAs,
         # wgmma GEMMs, group-local barriers) when the configuration is the shipped one (post-norm GLU decoder, d_model 256,
         # 4 heads, d_ff 2048, <= 256 memory frames); anything else takes the per-step graph.
-        self.persistent = bool(persistent) and self.mega_supported()
+        self.persistent = bool(persistent) and self.ctc is None and self.mega_supported()
         self._mega_model = None
         self._mega_sig = None
         self._ws = None
@@ -171,12 +184,16 @@ class BeamDecoder:
                               self._ws, dbg_logp, dbg_scores)
 
     def setup(self, memory_bf16, mem_len):
-        """Project cross-attention K/V once per utterance and reset the search state."""
+        """Project cross-attention K/V once per utterance and reset the search state (with a CTC term: the head's
+        log-probs of every frame and the prefix state of the empty hypothesis)."""
         pk = self.dec.packed()
         self.mem_len.copy_(mem_len)
         for l, p in enumerate(pk['blocks']):
             ops.linear(memory_bf16, p['wkv'], p['bkv'], out=self.kvx[l])
         self.state.init()
+        if self.ctc is not None:
+            ops.log_softmax(self.ctc_head.logits_bf16(memory_bf16), self.dec.vocab_size, out=self.ctc.lp)
+            self.ctc.init(self.mem_len)
 
     def _step_kernels(self):
         dec, st = self.dec, self.state
@@ -184,10 +201,18 @@ class BeamDecoder:
         x = ops.embed_posenc(st.last_tok, pk['emb'], self.table, self.N, dec.d_model, step_ptr=st.step_ptr)
         x = dec.decode_cached_bf16(pk, x, self.kc, self.vc, st.anc, st.step_ptr, self.kvx, self.mem_len, self.beam, self.T)
         ops.linear(x, pk['wout'], pk['bout'], out=self.logits)
-        ops.logsoftmax_topk(self.logits, dec.vocab_size, self.beam, self.lm_logp, self.lm_weight,
-                            out_val=self.topk_val, out_idx=self.topk_idx,
-                            out_logp=self.logp if self.keep_logp else None)
+        out_logp = self.logp if self.keep_logp else None
+        if self.ctc is None:
+            ops.logsoftmax_topk(self.logits, dec.vocab_size, self.beam, self.lm_logp, self.lm_weight,
+                                out_val=self.topk_val, out_idx=self.topk_idx, out_logp=out_logp)
+            st.step_topk(self.topk_val, self.topk_idx)
+            return
+        ctc = self.ctc
+        ops.logsoftmax_topk(self.logits, dec.vocab_size, ctc.P, self.lm_logp, self.lm_weight,
+                            out_val=ctc.cand_val, out_idx=ctc.cand_id, out_logp=out_logp)
+        ctc.score(st, self.mem_len, self.ctc_weight, self.topk_val, self.topk_idx, self.lm_logp, self.lm_weight)
         st.step_topk(self.topk_val, self.topk_idx)
+        ctc.advance(st, self.mem_len)
 
     def step(self):
         if not self.use_graph:
@@ -198,7 +223,8 @@ class BeamDecoder:
             self.graph = None
         if self.graph is None:
             self._graph_pk = self.dec.packed()
-            # warm-up outside capture (lazy func attributes, caches), then restore the state it advanced
+            # warm-up outside capture (lazy func attributes, caches), then restore the state it advanced (the CTC prefix
+            # state needs no copy: a step reads the half of its ping-pong that the step counter names and writes the other)
             snap = [t.clone() for t in (self.state.tok_hist, self.state.par_hist, self.state.last_tok,
                                         self.state.scores, self.state.flag, self.state.anc, self.state.ctrl)]
             s = torch.cuda.Stream()
@@ -268,14 +294,28 @@ class SpeechToTextRecognizer(Recognizer):
     """otrans/recognize/speech2text.py:6-93 on the CUDA path."""
 
     def __init__(self, model, lm=None, lm_weight=0.1, ctc_weight=0.0, beam_width=5, nbest=1, max_len=50,
-                 idx2unit=None, penalty=0, lamda=5, ngpu=1, apply_cache=False, use_graph=True, persistent=None):
+                 idx2unit=None, penalty=0, lamda=5, ngpu=1, apply_cache=False, use_graph=True, persistent=None,
+                 ctc_candidates=None):
+        """ctc_weight w > 0: joint CTC/attention decoding (DESIGN.md 4.9).  Each hypothesis' ctc_candidates best tokens by
+        the attention (+ LM) score (default min(16, 2 beam_width), between beam_width and 16) are scored
+        (1 - w) logp_att + w (psi(g c) - psi(g)) + lm_weight lm with the CTC prefix score psi of the model's joint-CTC head,
+        and the search goes on with the beam_width best of them.  The model must have the head (params['ctc_weight'] > 0)."""
+        if not 0.0 <= ctc_weight <= 1.0:
+            raise ValueError(f'SpeechToTextRecognizer: ctc_weight must be in [0, 1], got {ctc_weight}')
+        if ctc_weight > 0.0 and getattr(model, 'ctc_weight', 0.0) <= 0.0:
+            raise ValueError('SpeechToTextRecognizer: ctc_weight > 0 needs the joint-CTC head: this model has ctc_weight 0')
+        if ctc_candidates is None:
+            ctc_candidates = max(beam_width, min(ops.CTC_PREFIX_MAX_CANDIDATES, 2 * beam_width))
+        if ctc_weight > 0.0 and not beam_width <= ctc_candidates <= ops.CTC_PREFIX_MAX_CANDIDATES:
+            raise ValueError(f'SpeechToTextRecognizer: ctc_candidates must be in [beam_width = {beam_width}, '
+                             f'{ops.CTC_PREFIX_MAX_CANDIDATES}], got {ctc_candidates}')
         super().__init__(model, idx2unit, lm, lm_weight, ngpu)
         if lm is not None and getattr(lm, 'model_type', None) not in ('transformer_lm', 'recurrent_lm'):
             raise NotImplementedError('shallow fusion is implemented for the Transformer and the recurrent LM '
                                       '(opentransformer_b200.lm)')
         self.beam_width, self.max_len, self.nbest = beam_width, max_len, nbest
         self.penalty, self.lamda = penalty, lamda
-        self.ctc_weight, self.lm_weight = ctc_weight, lm_weight
+        self.ctc_weight, self.lm_weight, self.ctc_candidates = ctc_weight, lm_weight, ctc_candidates
         self.attn_weights = {}
         self.apply_cache = False
         self.use_graph = use_graph
@@ -298,8 +338,12 @@ class SpeechToTextRecognizer(Recognizer):
         kernel.  With cache['decoder'] = model.decoder.init_cache(memory, mask, max_len, beam) the decoder runs KV-cached
         (one token per call) and the cache is reordered by the surviving hypotheses' parents -- the feature the reference
         left as a stub (decoder/transformer.py:188-203, reselect_hidden* :195-218); with None it recomputes the full prefix
-        like the reference.  The fast path used by recognize() is BeamDecoder."""
+        like the reference.  The fast path used by recognize() is BeamDecoder; the CTC term of joint decoding exists there
+        only, so a recognizer with ctc_weight > 0 refuses this seam."""
         from .modules import DecoderCache
+        if self.ctc_weight > 0.0:
+            raise NotImplementedError('decode_step is attention-only: joint CTC/attention decoding (ctc_weight > 0) runs in '
+                                      'recognize() / recognize_ids()')
         n = scores.size(0)
         batch = n // self.beam_width
         dcache = cache.get('decoder') if isinstance(cache, dict) else None
@@ -325,26 +369,50 @@ class SpeechToTextRecognizer(Recognizer):
         return self.model.encode_bf16(inputs, inputs_mask)
 
     def _decoder_for(self, B, T2, device):
-        key = (B, self.beam_width, T2, self.max_len, device.index)
+        # the CTC weight and candidate count are launch arguments that a captured step bakes in
+        ctc = (self.model.assistor, self.ctc_weight, self.ctc_candidates) if self.ctc_weight > 0.0 else None
+        key = (B, self.beam_width, T2, self.max_len, device.index, ctc[1:] if ctc else None)
         bd = self._decoders.get(key)
         if bd is None:
             bd = BeamDecoder(self.model.decoder, B, self.beam_width, T2, self.max_len, device,
-                             self.use_graph and self.lm is None, persistent=self.persistent and self.lm is None)
+                             self.use_graph and self.lm is None, persistent=self.persistent and self.lm is None, ctc=ctc)
             self._decoders[key] = bd
         return bd
+
+    def _search(self, inputs, inputs_mask):
+        """Encoder pass and beam search -> (recognize_ids' return, memory bf16 [B*T', D], lengths i32 [B], the BeamDecoder)."""
+        mem, mem_len, B, T2 = self._encode_bf16(inputs, inputs_mask)
+        bd = self._decoder_for(B, T2, inputs.device)
+        bd.setup(mem, mem_len)
+        if self.lm is not None:
+            steps = bd.run_with_lm(self.max_len, self.lm, self.lm_weight)
+        else:
+            steps = bd.run(self.max_len)
+        preds, scores = bd.state.finalize(self.penalty, self.lamda, self.nbest)
+        return (preds[:, :, :steps], scores, steps), mem, mem_len, bd
 
     def recognize_ids(self, inputs, inputs_mask):
         """-> (nbest ids i64 [B,nbest,steps], scores f32 [B,nbest], steps)"""
         with torch.no_grad():
-            mem, mem_len, B, T2 = self._encode_bf16(inputs, inputs_mask)
-            bd = self._decoder_for(B, T2, inputs.device)
-            bd.setup(mem, mem_len)
-            if self.lm is not None:
-                steps = bd.run_with_lm(self.max_len, self.lm, self.lm_weight)
-            else:
-                steps = bd.run(self.max_len)
-            preds, scores = bd.state.finalize(self.penalty, self.lamda, self.nbest)
-        return preds[:, :, :steps], scores, steps
+            return self._search(inputs, inputs_mask)[0]
+
+    def recognize_spans(self, inputs, inputs_mask):
+        """recognize_ids, plus where each token of the 1-best lies: the 1-best up to and including its closing <S/E> (one is
+        appended to a hypothesis that reached max_len without it; the head is trained on the closing <S/E> as a label) is
+        force-aligned (otb_ctc_align) against the joint-CTC head's log-probs of the same encoder pass.  Any ctc_weight, 0
+        included, but the model must have the head.  -> (ids, scores, steps as recognize_ids; spans i32 [B, steps + 1, 2]
+        [start, end) in encoder frames of the 1-best's tokens, -1 past its closing <S/E> and throughout where the
+        utterance has too few frames for it), on the device.  model.encoder_frames_to_input converts the spans."""
+        if getattr(self.model, 'ctc_weight', 0.0) <= 0.0:
+            raise ValueError('SpeechToTextRecognizer.recognize_spans needs the joint-CTC head: this model has ctc_weight 0')
+        with torch.no_grad():
+            (ids, scores, steps), mem, mem_len, bd = self._search(inputs, inputs_mask)
+            B, V = ids.shape[0], self.model.decoder.vocab_size
+            lp = bd.ctc.lp if bd.ctc is not None else ops.log_softmax(self.model.assistor.logits_bf16(mem), V)
+            best = torch.cat((ids[:, 0], torch.full((B, 1), EOS, dtype=ids.dtype, device=ids.device)), dim=1)
+            n_tok = ((best == EOS).int().argmax(dim=1) + 1).to(torch.int32)
+            _, _, spans, _ = ops.ctc_align(lp.view(B, -1, V), mem_len, best, n_tok, blank=self.model.assistor.blank)
+        return ids, scores, steps, spans
 
     def recognize(self, inputs, inputs_mask):
         preds, scores, _ = self.recognize_ids(inputs, inputs_mask)
@@ -416,7 +484,7 @@ def build_recognizer(model_type, model, lm, args, idx2unit):
         return SpeechToTextRecognizer(
             model=model, lm=lm, lm_weight=args.lm_weight, ctc_weight=args.ctc_weight, beam_width=args.beam_width,
             nbest=args.nbest, max_len=args.max_len, idx2unit=idx2unit, penalty=args.penalty, lamda=args.lamda,
-            ngpu=args.ngpu)
+            ngpu=args.ngpu, ctc_candidates=getattr(args, 'ctc_candidates', None))
     if model_type == 'ctc':
         return CTCRecognizer(
             model=model, lm=lm, lm_weight=args.lm_weight, ngram_lm=args.ngram_lm, beam_width=args.beam_width,
