@@ -399,6 +399,23 @@ int otb_ctc_prefix_score(const float* lp, int ld, int T, int V, const int32_t* i
 int otb_ctc_prefix_advance(const otb_beam_state* st, const int32_t* cand_id, int P, int T, const int32_t* in_len,
                            const float* gamma_cand, const float* psi_cand, float* gamma, float* psi, void* stream);
 
+/* N-best rescoring (the recognizers' apply_rescoring / apply_lm_rescoring; no reference entry point computes it:
+ * eval.py's -resc / -lm_resc / -rw are parsed and never used).
+ * otb_token_logprob: out f32 [rows] = logits[r, target[r]] - logsumexp(logits[r, :V]) of logits f32 [rows, ld], 0 where
+ * target[r] < 0 (the row is not read) and NaN where target[r] >= V.  ld % 4 == 0 and a 16-byte aligned base.  Each row is
+ * read once; the reduction order is fixed, so repeated calls are bit-identical. */
+int otb_token_logprob(const float* logits, int ld, int rows, int V, const int32_t* target, float* out, void* stream);
+/* One warp per utterance over its K <= 32 first-pass hypotheses, hypothesis h = b * K + k: tgt i32 [B*K, Lp] its scored
+ * tokens y <S/E> (-1 after), len i32 [B*K] the length n of y, s1 f32 [B*K] its first-pass score, tok_lp f32 [M, B*K, Lp]
+ * the token log-probs of M second-pass models.  A hypothesis equal to one of a lower k of its utterance is dropped; the
+ * others score s = s1 + weight * sum_m sum_{t <= n} tok_lp[m, h, t] (position order, then model order, fp32 without
+ * contraction).  Ranked: kept before dropped, then descending s, then k.  The first nbest (<= K) go to ids i64
+ * [B, nbest, Lout] (y, then pad_id), out_len i32 [B, nbest] (n; 0 when dropped) and out_score f32 [B, nbest] (-inf when
+ * dropped). */
+int otb_nbest_rescore(const int32_t* tgt, int Lp, const int32_t* len, const float* s1, const float* tok_lp, int M, int B, int K,
+                      float weight, int nbest, int Lout, int64_t pad_id, int64_t* ids, int32_t* out_len, float* out_score,
+                      void* stream);
+
 /* Conv2d front end backward (frontend/conv.py:50-76 under autograd).  h1 = conv1 activation buffer (layout of
  * otb_conv1_relu).  col bf16 [B*T2*F2, 9*C1] = im2col of h1 for conv2 (k = (kh*3+kw)*C1 + c): conv2's weight gradient is
  * otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu folds dcol

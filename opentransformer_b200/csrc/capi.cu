@@ -523,6 +523,19 @@ int otb_ctc_prefix_advance(const otb_beam_state* st, const int32_t* cand_id, int
                                                             gamma, psi));
 }
 
+int otb_token_logprob(const float* logits, int ld, int rows, int V, const int32_t* target, float* out, void* stream) {
+    if (rows > 0 && (!logits || !target || !out)) return fail("otb_token_logprob", "null operand");
+    RET("otb_token_logprob", token_logprob_launch(ST(stream), logits, ld, rows, V, target, out));
+}
+
+int otb_nbest_rescore(const int32_t* tgt, int Lp, const int32_t* len, const float* s1, const float* tok_lp, int M, int B, int K,
+                      float weight, int nbest, int Lout, int64_t pad_id, int64_t* ids, int32_t* out_len, float* out_score,
+                      void* stream) {
+    if (!tgt || !len || !s1 || (M > 0 && !tok_lp) || !ids || !out_len || !out_score) return fail("otb_nbest_rescore", "null operand");
+    RET("otb_nbest_rescore", nbest_rescore_launch(ST(stream), tgt, Lp, len, s1, tok_lp, M, B, K, weight, nbest, Lout, (long long)pad_id,
+                                                  reinterpret_cast<long long*>(ids), out_len, out_score));
+}
+
 int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
     int T1, F1, T2, F2;
     if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;

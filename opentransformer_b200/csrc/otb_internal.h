@@ -214,6 +214,11 @@ const char* ctc_prefix_score_launch(cudaStream_t stream, const float* lp, int ld
 const char* ctc_prefix_advance_launch(cudaStream_t stream, BeamState st, const int* cand_id, int P, int T, const int* in_len,
                                       const float* gamma_cand, const float* psi_cand, float* gamma, float* psi);
 
+const char* token_logprob_launch(cudaStream_t stream, const float* logits, int ld, int rows, int V, const int* target, float* out);
+const char* nbest_rescore_launch(cudaStream_t stream, const int* tgt, int Lp, const int* len, const float* s1, const float* tok_lp,
+                                 int M, int B, int K, float weight, int nbest, int Lout, long long pad_id, long long* ids,
+                                 int* out_len, float* out_score);
+
 const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const int* n_samples, int B, const float* window,
                          const float* bank, const int* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift,
                          float preemph);

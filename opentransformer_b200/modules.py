@@ -740,21 +740,28 @@ class TransformerDecoder(nn.Module):
 
     def forward_bf16(self, targets, memory_bf16, mem_len, B, L, T):
         """targets i64 [B,L]; memory bf16 [B*T, D] -> logits f32 [B*L, ld_logits] (first V columns valid)."""
+        return self.score_bf16(targets, memory_bf16, mem_len, B, 1, L, T)
+
+    def score_bf16(self, inputs, memory_bf16, mem_len, B, K, Lp, T):
+        """Teacher-forced logits of K sequences per utterance (the second pass of n-best rescoring): inputs i64 [B*K, Lp],
+        memory bf16 [B*T, D] -> logits f32 [B*K*Lp, ld_logits] (first V columns valid).  Self-attention is causal within
+        each of the B*K sequences; cross-attention treats the K*Lp query rows of utterance b as one problem against its
+        memory, so the memory's K|V is projected once per utterance, not once per sequence."""
         _no_train(self)
         pk = self._pack.get()
         d, H = self.d_model, self.n_heads
-        scale, table = self.pos_emb.scale_and_table(L, memory_bf16.device)
+        scale, table = self.pos_emb.scale_and_table(Lp, memory_bf16.device)
         if self.pos_emb.scale_learnable:
             raise NotImplementedError('decoder with learnable positional scale')
-        x = ops.embed_posenc(targets.contiguous(), pk['emb'], table, B * L, d, period=L)
+        x = ops.embed_posenc(inputs.contiguous(), pk['emb'], table, B * K * Lp, d, period=Lp)
 
         def self_attn(l, qkv):
-            return ops.attention(qkv, qkv, qkv, B, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
+            return ops.attention(qkv, qkv, qkv, B * K, H, Lp, Lp, causal=True, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
 
         def cross_attn(l, q):       # the memory's K|V, projected per layer after the query GEMM
             p = pk['blocks'][l]
             kv = ops.linear(memory_bf16, p['wkv'], p['bkv'])
-            return ops.attention(q, kv, kv, B, H, L, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H)
+            return ops.attention(q, kv, kv, B, H, K * Lp, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H)
 
         x = self._layers(pk, x, self_attn, cross_attn)
         return ops.linear(x, pk['wout'], pk['bout'], EPI_BIAS, out_f32=True, n_out=self.ld_logits)

@@ -783,6 +783,45 @@ class CTCPrefixState:
         _count()
 
 
+def token_logprob(logits, V, target):
+    """out f32 [rows] = log_softmax(logits[r, :V])[target[r]], 0 where target[r] < 0 (otb_token_logprob): each row is read
+    once and no [rows, V] log-softmax is written.  logits f32 [rows, ld] with ld % 4 == 0; target i32 [rows]."""
+    if not logits.is_cuda:
+        raise RuntimeError('logits must be a CUDA tensor: the CUDA hot path has no CPU fallback')
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
+        raise TypeError('token_logprob: logits must be a 2-D f32 tensor with unit column stride')
+    rows = logits.shape[0]
+    if target.shape != (rows,):
+        raise ValueError(f'token_logprob: target must be [rows = {rows}], got {tuple(target.shape)}')
+    _need(target, torch.int32, 'target')
+    out = torch.empty(rows, dtype=torch.float32, device=logits.device)
+    check(_lib.lib().otb_token_logprob(_p(logits), logits.stride(0), rows, V, _p(target), _p(out), _stream()), 'otb_token_logprob')
+    _count()
+    return out
+
+
+def nbest_rescore(tgt, lengths, s1, tok_lp, weight, nbest, width, pad_id):
+    """Re-rank each utterance's K first-pass hypotheses by s = s1 + weight * (sum of their second-pass token log-probs)
+    (otb_nbest_rescore, DESIGN.md 4.10).  tgt i32 [B, K, Lp] the scored tokens y <S/E> (-1 after), lengths i32 [B, K] the
+    length of y, s1 f32 [B, K], tok_lp f32 [M, B, K, Lp] the token log-probs of M models.  -> (ids i64 [B, nbest, width]
+    y then pad_id, lengths i32 [B, nbest], scores f32 [B, nbest]); duplicates of a better first-pass hypothesis rank last
+    with score -inf, length 0 and pad_id throughout."""
+    B, K, Lp = tgt.shape
+    if lengths.shape != (B, K) or s1.shape != (B, K) or tok_lp.dim() != 4 or tuple(tok_lp.shape[1:]) != (B, K, Lp):
+        raise ValueError(f'nbest_rescore: need lengths / s1 [B, K] = [{B}, {K}] and tok_lp [M, {B}, {K}, {Lp}], got '
+                         f'{tuple(lengths.shape)}, {tuple(s1.shape)}, {tuple(tok_lp.shape)}')
+    _need(tgt, torch.int32, 'tgt'); _need(lengths, torch.int32, 'lengths'); _need(s1, torch.float32, 's1')
+    _need(tok_lp, torch.float32, 'tok_lp')
+    dev = tgt.device
+    ids = torch.empty(B, nbest, width, dtype=torch.int64, device=dev)
+    out_len = torch.empty(B, nbest, dtype=torch.int32, device=dev)
+    scores = torch.empty(B, nbest, dtype=torch.float32, device=dev)
+    check(_lib.lib().otb_nbest_rescore(_p(tgt), Lp, _p(lengths), _p(s1), _p(tok_lp), tok_lp.shape[0], B, K, float(weight), nbest,
+                                       width, int(pad_id), _p(ids), _p(out_len), _p(scores), _stream()), 'otb_nbest_rescore')
+    _count()
+    return ids, out_len, scores
+
+
 def conv_im2col(h1, B, T, F, C1):
     _, _, T2, F2 = conv_geometry(T, F)
     col = torch.empty(B * T2 * F2, 9 * C1, dtype=BF16, device=h1.device)

@@ -13,7 +13,10 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
   * beam step: one kernel per step (top-k, finished masking, pruning, back-pointers), no host sync
     inside the loop except a 4-byte "all ended" poll every few steps;
   * joint CTC/attention decoding (ctc_weight > 0, which the reference stores and never reads): the CTC prefix score of the
-    joint-CTC head re-ranks each hypothesis' best candidates inside the step (csrc/ctc_prefix.cu, DESIGN.md 4.9).
+    joint-CTC head re-ranks each hypothesis' best candidates inside the step (csrc/ctc_prefix.cu, DESIGN.md 4.9);
+  * n-best rescoring (apply_rescoring / apply_lm_rescoring / rescore_weight, which the reference parses and never passes
+    on): a teacher-forced second pass of the attention decoder or an LM re-ranks the first pass's n-best
+    (csrc/rescore.cu, DESIGN.md 4.10).
 """
 import torch
 
@@ -86,6 +89,74 @@ def lm_log_probs(lm, preds):
     if lm.model_type == 'transformer_lm':
         return lm.predict(preds, last_frame=True).squeeze(1).contiguous()
     return lm.predict(preds[:, -1:], None)[0].squeeze(1).contiguous()
+
+
+def lm_token_logprob(lm, inputs, targets):
+    """Token log-probs f32 [N, Lp] of targets i32 [N, Lp] (-1 after a sequence's end: 0 there) under the LM teacher-forced
+    on inputs i64 [N, Lp]: the Transformer LM's full-sequence logits, the recurrent LM's from a zero state.  Neither lets a
+    position see later ones, so the padding after a sequence's end needs no mask."""
+    N, Lp = targets.shape
+    if lm.model_type == 'transformer_lm':
+        return ops.token_logprob(lm.logits_bf16(inputs), lm.vocab_size, targets.reshape(-1)).view(N, Lp)
+    pk = lm._pack.get()
+    x, _, _, _ = lm._run(inputs.t().contiguous(), pk)                      # time-major rows
+    return ops.token_logprob(lm._logits(x, pk), lm.vocab_size, targets.t().reshape(-1)).view(Lp, N).t()
+
+
+def second_pass_rows(ids, lengths=None):
+    """The sequences a second pass scores, from first-pass ids [B, K, W] (DESIGN.md 4.10): hypothesis y is its row cut at
+    the first <S/E> (and at `lengths` [B, K] when given: the CTC n-best's rows end in 0s), and the scored sequence is
+    y <S/E>.  -> (inputs i64 [B*K, Lp] = BOS y PAD..., targets i32 [B, K, Lp] = y <S/E> -1..., n i32 [B, K] the length
+    of y, Lp = max n + 1).  Reading Lp is the one host synchronisation."""
+    B, K, W = ids.shape
+    dev = ids.device
+    ext = torch.cat((ids.long(), torch.full((B, K, 1), EOS, dtype=torch.int64, device=dev)), dim=2)
+    if lengths is not None:
+        ext = torch.where(torch.arange(W + 1, device=dev) >= lengths[..., None], EOS, ext)
+    n = (ext == EOS).int().argmax(dim=2)                                      # the first <S/E>
+    Lp = int(n.max()) + 1
+    pos = torch.arange(Lp, device=dev)
+    targets = torch.where(pos < n[..., None], ext[:, :, :Lp], torch.where(pos == n[..., None], EOS, -1)).int()
+    inputs = torch.cat((torch.full((B, K, 1), BOS, dtype=torch.int64, device=dev), targets[:, :, :-1].clamp_min(PAD).long()), 2)
+    return inputs.view(B * K, Lp), targets, n.int(), Lp
+
+
+def rescore_nbest(ids, scores, scorers, weight, nbest, width=None, pad=EOS, lengths=None):
+    """N-best rescoring (DESIGN.md 4.10): first-pass ids [B, K, W] (cut as second_pass_rows does) with scores f32 [B, K];
+    scorers: functions (inputs i64 [B*K, Lp], targets i32 [B*K, Lp], K, Lp) -> token log-probs f32 [B*K, Lp] of one
+    second-pass model each.  s = first-pass score + weight * sum of the models' sums; ranked per utterance by descending s,
+    ties in first-pass order, duplicates last with -inf.  -> ops.nbest_rescore's (ids i64 [B, nbest, width or Lp] padded
+    with `pad`, lengths i32 [B, nbest], scores f32 [B, nbest])."""
+    B, K, _ = ids.shape
+    inputs, targets, n, Lp = second_pass_rows(ids, lengths)
+    flat = targets.view(B * K, Lp)
+    tok_lp = torch.stack([f(inputs, flat, K, Lp).reshape(B, K, Lp) for f in scorers])
+    return ops.nbest_rescore(targets, n, scores.float().contiguous(), tok_lp.contiguous(), weight, nbest, width or Lp, pad)
+
+
+def check_lm_rescoring(who, lm, vocab_size):
+    if lm is None:
+        raise ValueError(f'{who}: apply_lm_rescoring needs an lm')
+    if getattr(lm, 'model_type', None) not in ('transformer_lm', 'recurrent_lm'):
+        raise NotImplementedError(f'{who}: LM rescoring is implemented for the Transformer and the recurrent LM '
+                                  '(opentransformer_b200.lm)')
+    if lm.vocab_size != vocab_size:
+        raise ValueError(f'{who}: the LM has {lm.vocab_size} tokens and the model {vocab_size}: rescoring needs one vocabulary')
+
+
+def ctc_decode(logits, lengths, B, T2, V, blank, mode, beam_width):
+    """CTC decoding of a CTC head's logits f32 [B*T', ld] (CTCRecognizer; SpeechToTextRecognizer's first pass under
+    apply_rescoring): otb_ctc_frame_topk, then the greedy collapse (otb_ctc_greedy, mode 'greedy') or the prefix beam search
+    over each frame's 40 best tokens (otb_ctc_prefix_beam, mode 'beam').  -> (ids i64 [B, nbest, T'] best first, 0 after
+    each hypothesis' end; lengths i32 [B, nbest]; scores f32 [B, nbest]); nbest is 1 in greedy mode and beam_width in beam
+    mode."""
+    if mode == 'greedy':
+        lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, 1)
+        ids, n, sc = ops.ctc_greedy(lp, tok, B, T2, lengths, blank)
+        return ids.long().view(B, 1, T2), n.view(B, 1), sc.view(B, 1)
+    lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, min(CTC_CUTOFF_TOP_N, V))
+    ids, n, sc = ops.ctc_prefix_beam(lp, tok, B, T2, lengths, beam_width, blank)
+    return ids.long(), n, sc
 
 
 class BeamDecoder:
@@ -295,11 +366,28 @@ class SpeechToTextRecognizer(Recognizer):
 
     def __init__(self, model, lm=None, lm_weight=0.1, ctc_weight=0.0, beam_width=5, nbest=1, max_len=50,
                  idx2unit=None, penalty=0, lamda=5, ngpu=1, apply_cache=False, use_graph=True, persistent=None,
-                 ctc_candidates=None):
+                 ctc_candidates=None, apply_rescoring=False, apply_lm_rescoring=False, rescore_weight=1.0):
         """ctc_weight w > 0: joint CTC/attention decoding (DESIGN.md 4.9).  Each hypothesis' ctc_candidates best tokens by
         the attention (+ LM) score (default min(16, 2 beam_width), between beam_width and 16) are scored
         (1 - w) logp_att + w (psi(g c) - psi(g)) + lm_weight lm with the CTC prefix score psi of the model's joint-CTC head,
-        and the search goes on with the beam_width best of them.  The model must have the head (params['ctc_weight'] > 0)."""
+        and the search goes on with the beam_width best of them.  The model must have the head (params['ctc_weight'] > 0).
+
+        N-best rescoring (DESIGN.md 4.10; eval.py's -resc / -lm_resc / -rw): each hypothesis' score becomes
+        s = first-pass score + rescore_weight * (sum of its second-pass log-probs), and the nbest best by s are returned.
+        apply_rescoring: the first pass is the CTC prefix beam search (beam_width hypotheses) over the joint-CTC head, the
+        second pass the attention decoder; no attention beam search runs.  apply_lm_rescoring: the LM is not fused into the
+        search (the persistent decode kernel stays eligible) but scores all beam_width hypotheses of the first pass."""
+        has_head = getattr(model, 'ctc_weight', 0.0) > 0.0
+        if apply_rescoring and not has_head:
+            raise ValueError('SpeechToTextRecognizer: apply_rescoring needs the joint-CTC head: this model has ctc_weight 0')
+        if apply_rescoring and ctc_weight > 0.0:
+            raise ValueError('SpeechToTextRecognizer: apply_rescoring (CTC first pass, attention second) and ctc_weight > 0 '
+                             '(the CTC term inside the attention search) are two uses of the joint-CTC head; choose one')
+        if apply_rescoring and not 1 <= beam_width <= 16:
+            raise NotImplementedError(f'SpeechToTextRecognizer: the CTC prefix beam search of apply_rescoring takes beam_width '
+                                      f'1..16, got {beam_width}')
+        if apply_lm_rescoring:
+            check_lm_rescoring('SpeechToTextRecognizer', lm, model.decoder.vocab_size)
         if not 0.0 <= ctc_weight <= 1.0:
             raise ValueError(f'SpeechToTextRecognizer: ctc_weight must be in [0, 1], got {ctc_weight}')
         if ctc_weight > 0.0 and getattr(model, 'ctc_weight', 0.0) <= 0.0:
@@ -322,6 +410,8 @@ class SpeechToTextRecognizer(Recognizer):
         # None = automatic: the persistent decode kernel (one launch per batch, csrc/decode_group.cu) whenever the decoder,
         # the batch geometry and the options (no LM fusion) fit it; False forces the per-step CUDA-graph path
         self.persistent = True if persistent is None else bool(persistent)
+        self.apply_rescoring, self.apply_lm_rescoring = bool(apply_rescoring), bool(apply_lm_rescoring)
+        self.rescore_weight = float(rescore_weight)
         self._decoders = {}
 
     # ---- reference-facing seams -------------------------------------------------------------
@@ -374,22 +464,45 @@ class SpeechToTextRecognizer(Recognizer):
         key = (B, self.beam_width, T2, self.max_len, device.index, ctc[1:] if ctc else None)
         bd = self._decoders.get(key)
         if bd is None:
+            fused = self._lm_fused()
             bd = BeamDecoder(self.model.decoder, B, self.beam_width, T2, self.max_len, device,
-                             self.use_graph and self.lm is None, persistent=self.persistent and self.lm is None, ctc=ctc)
+                             self.use_graph and not fused, persistent=self.persistent and not fused, ctc=ctc)
             self._decoders[key] = bd
         return bd
 
+    def _lm_fused(self):
+        """The LM enters the search by shallow fusion (it rescores the n-best instead under apply_lm_rescoring)."""
+        return self.lm is not None and not self.apply_lm_rescoring
+
     def _search(self, inputs, inputs_mask):
-        """Encoder pass and beam search -> (recognize_ids' return, memory bf16 [B*T', D], lengths i32 [B], the BeamDecoder)."""
+        """Encoder pass, search and (when asked) rescoring -> (recognize_ids' return, memory bf16 [B*T', D], lengths i32 [B],
+        the BeamDecoder or None when the first pass is the CTC prefix beam search)."""
         mem, mem_len, B, T2 = self._encode_bf16(inputs, inputs_mask)
+        scorers = []
+        if self.apply_rescoring:
+            dec = self.model.decoder
+            scorers.append(lambda x, y, K, Lp: ops.token_logprob(dec.score_bf16(x, mem, mem_len, B, K, Lp, T2), dec.vocab_size,
+                                                                 y.reshape(-1)))
+        if self.apply_lm_rescoring:
+            scorers.append(lambda x, y, K, Lp: lm_token_logprob(self.lm, x, y))
+        nbest = min(self.nbest, self.beam_width)
+        if self.apply_rescoring:
+            ids, n, sc = ctc_decode(self.model.assistor.logits_bf16(mem), mem_len, B, T2, self.model.decoder.vocab_size,
+                                    self.model.assistor.blank, 'beam', self.beam_width)
+            preds, _, scores = rescore_nbest(ids, sc, scorers, self.rescore_weight, nbest, lengths=n)
+            return (preds, scores, preds.shape[2]), mem, mem_len, None
         bd = self._decoder_for(B, T2, inputs.device)
         bd.setup(mem, mem_len)
-        if self.lm is not None:
+        if self._lm_fused():
             steps = bd.run_with_lm(self.max_len, self.lm, self.lm_weight)
         else:
             steps = bd.run(self.max_len)
-        preds, scores = bd.state.finalize(self.penalty, self.lamda, self.nbest)
-        return (preds[:, :, :steps], scores, steps), mem, mem_len, bd
+        if not scorers:
+            preds, scores = bd.state.finalize(self.penalty, self.lamda, self.nbest)
+            return (preds[:, :, :steps], scores, steps), mem, mem_len, bd
+        preds, scores = bd.state.finalize(self.penalty, self.lamda, self.beam_width)
+        preds, _, scores = rescore_nbest(preds[:, :, :steps], scores, scorers, self.rescore_weight, nbest, width=steps)
+        return (preds, scores, steps), mem, mem_len, bd
 
     def recognize_ids(self, inputs, inputs_mask):
         """-> (nbest ids i64 [B,nbest,steps], scores f32 [B,nbest], steps)"""
@@ -408,7 +521,7 @@ class SpeechToTextRecognizer(Recognizer):
         with torch.no_grad():
             (ids, scores, steps), mem, mem_len, bd = self._search(inputs, inputs_mask)
             B, V = ids.shape[0], self.model.decoder.vocab_size
-            lp = bd.ctc.lp if bd.ctc is not None else ops.log_softmax(self.model.assistor.logits_bf16(mem), V)
+            lp = bd.ctc.lp if bd is not None and bd.ctc is not None else ops.log_softmax(self.model.assistor.logits_bf16(mem), V)
             best = torch.cat((ids[:, 0], torch.full((B, 1), EOS, dtype=ids.dtype, device=ids.device)), dim=1)
             n_tok = ((best == EOS).int().argmax(dim=1) + 1).to(torch.int32)
             _, _, spans, _ = ops.ctc_align(lp.view(B, -1, V), mem_len, best, n_tok, blank=self.model.assistor.blank)
@@ -425,21 +538,30 @@ CTC_CUTOFF_TOP_N = 40      # ctcdecode's cutoff_top_n default (cutoff_prob 1.0),
 class CTCRecognizer(Recognizer):
     """otrans/recognize/ctc.py:7-76 on the CUDA path: CTCModel.inference's head logits -> otb_ctc_frame_topk -> the greedy
     collapse (otb_ctc_greedy, mode 'greedy') or the CTC prefix beam search (otb_ctc_prefix_beam, mode 'beam': ctcdecode's
-    search without a scorer, over each frame's 40 best tokens).  `lm` is stored and never used, as in the reference;
-    `alpha` / `beta` are ignored, as ctcdecode ignores them without an n-gram scorer, and an n-gram LM (`ngram_lm`,
-    KenLM) is refused."""
+    search without a scorer, over each frame's 40 best tokens).  `lm` is stored and used only by apply_lm_rescoring, as the
+    reference never uses it; `alpha` / `beta` are ignored, as ctcdecode ignores them without an n-gram scorer, and an
+    n-gram LM (`ngram_lm`, KenLM) is refused.
+
+    apply_lm_rescoring (beam mode): the prefix beam search's n-best is re-ranked by
+    s = prefix log-probability + rescore_weight * log P_lm(y <S/E>) (DESIGN.md 4.10)."""
 
     def __init__(self, model, lm=None, lm_weight=0.1, ngram_lm=None, beam_width=5, idx2unit=None, ngpu=1, mode='greedy',
-                 alpha=0.1, beta=0.0):
+                 alpha=0.1, beta=0.0, apply_lm_rescoring=False, rescore_weight=1.0):
         if ngram_lm is not None:
             raise NotImplementedError('CTCRecognizer: n-gram LM scoring (KenLM) is not implemented; use ngram_lm=None')
         if mode not in ('greedy', 'beam'):
             raise ValueError(f"CTCRecognizer: mode must be 'greedy' or 'beam', got {mode!r}")
         if mode == 'beam' and not 1 <= beam_width <= 16:
             raise NotImplementedError(f'CTCRecognizer: the prefix beam search takes beam_width 1..16, got {beam_width}')
+        if apply_lm_rescoring:
+            if mode == 'greedy':
+                raise ValueError("CTCRecognizer: apply_lm_rescoring re-ranks an n-best; the greedy mode has one hypothesis, "
+                                 "use mode='beam'")
+            check_lm_rescoring('CTCRecognizer', lm, model.vocab_size)
         super().__init__(model, idx2unit, lm, lm_weight, ngpu)
         self.beam_width, self.mode = beam_width, mode
         self.alpha, self.beta = alpha, beta
+        self.apply_lm_rescoring, self.rescore_weight = bool(apply_lm_rescoring), float(rescore_weight)
 
     def recognize_ids(self, inputs, inputs_mask):
         """-> (ids i64 [B, nbest, T'] best first, 0 after each hypothesis' end; lengths i32 [B, nbest]; scores f32 [B, nbest]),
@@ -449,14 +571,12 @@ class CTCRecognizer(Recognizer):
             return self._decode(*self.model.logits_bf16(inputs, inputs_mask))
 
     def _decode(self, logits, lengths, B, T2):
-        V = self.model.vocab_size
-        if self.mode == 'greedy':
-            lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, 1)
-            ids, n, sc = ops.ctc_greedy(lp, tok, B, T2, lengths, self.model.assistor.blank)
-            return ids.long().view(B, 1, T2), n.view(B, 1), sc.view(B, 1)
-        lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, min(CTC_CUTOFF_TOP_N, V))
-        ids, n, sc = ops.ctc_prefix_beam(lp, tok, B, T2, lengths, self.beam_width, self.model.assistor.blank)
-        return ids.long(), n, sc
+        ids, n, sc = ctc_decode(logits, lengths, B, T2, self.model.vocab_size, self.model.assistor.blank, self.mode,
+                                self.beam_width)
+        if not self.apply_lm_rescoring:
+            return ids, n, sc
+        return rescore_nbest(ids, sc, [lambda x, y, K, Lp: lm_token_logprob(self.lm, x, y)], self.rescore_weight,
+                             self.beam_width, width=T2, pad=PAD, lengths=n)
 
     def recognize_spans(self, inputs, inputs_mask):
         """recognize_ids, plus where each token of the 1-best lies: the 1-best is force-aligned (otb_ctc_align) against the
@@ -484,9 +604,14 @@ def build_recognizer(model_type, model, lm, args, idx2unit):
         return SpeechToTextRecognizer(
             model=model, lm=lm, lm_weight=args.lm_weight, ctc_weight=args.ctc_weight, beam_width=args.beam_width,
             nbest=args.nbest, max_len=args.max_len, idx2unit=idx2unit, penalty=args.penalty, lamda=args.lamda,
-            ngpu=args.ngpu, ctc_candidates=getattr(args, 'ctc_candidates', None))
+            ngpu=args.ngpu, ctc_candidates=getattr(args, 'ctc_candidates', None),
+            apply_rescoring=getattr(args, 'apply_rescoring', False),
+            apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False), rescore_weight=getattr(args, 'rescore_weight', 1.0))
     if model_type == 'ctc':
+        if getattr(args, 'apply_rescoring', False):
+            raise ValueError('build_recognizer: apply_rescoring re-scores with the attention decoder, and a CTC model has none')
         return CTCRecognizer(
             model=model, lm=lm, lm_weight=args.lm_weight, ngram_lm=args.ngram_lm, beam_width=args.beam_width,
-            idx2unit=idx2unit, ngpu=args.ngpu, mode=args.mode, alpha=args.alpha, beta=args.beta)
+            idx2unit=idx2unit, ngpu=args.ngpu, mode=args.mode, alpha=args.alpha, beta=args.beta,
+            apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False), rescore_weight=getattr(args, 'rescore_weight', 1.0))
     raise NotImplementedError(model_type)
