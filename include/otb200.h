@@ -129,9 +129,10 @@ int otb_layernorm(const void* x, int ldx, void* out, int ldo, int out_f32, const
                   const float* g2, const float* b2, float eps, int M, int N, void* stream);
 
 /* PositionalEncoding.forward stand-alone (module/pos.py:56): out bf16 = x * alpha + table[row % period];
- * x is f32 (x_f32 != 0) or bf16; table may be NULL (pure scale / dtype conversion). */
+ * x is f32 (x_f32 != 0) or bf16; table may be NULL (pure scale / dtype conversion).  alpha_dev (may be NULL): a device f32
+ * scalar alpha is multiplied by, read on the device (a loss-gradient scale that exists only on the device). */
 int otb_scale_add_table(const void* x, int ldx, int x_f32, void* out, int ldo, float alpha, const float* table,
-                        int period, int M, int N, void* stream);
+                        int period, int M, int N, const float* alpha_dev, void* stream);
 
 /* PositionalEncoding._embedding_from_positions (module/pos.py:30-42): out f32 [n_pos, d] for positions
  * first_pos .. first_pos + n_pos - 1 (negative allowed). */
@@ -295,10 +296,21 @@ int otb_sumsq(const float* g, long long n, float* out, int zero_first, void* str
  * counters i32 [3] = {optimizer steps, scheduler global_step, skipped steps}; when sqrt(*sumsq) is finite both counts
  * advance and lr = factor * model_size^-0.5 * min(s^-0.5, s * warmup^-1.5) (TransformerScheduler, train/scheduler.py:137-138;
  * warmup_steps <= 0: lr = base_lr), else only `skipped` advances and nothing is updated -- the reference skips
- * scheduler.step() and optimizer.step() together (trainer.py:229-233).  hyper f32 [4] receives {lr, 1-b1^t, 1-b2^t, applied}. */
+ * scheduler.step() and optimizer.step() together (trainer.py:229-233).  hyper f32 [4] receives {lr, 1-b1^t, 1-b2^t, applied}.
+ * Gradient noise (trainer.py:223-227) when noise_std > 0: the clipped gradient of every element whose bit is set in
+ * noise_mask (u8 [(n + 7) / 8], bit i & 7 of byte i >> 3) gets noise_std * z before the weight decay, z ~ N(0, 1) a
+ * counter hash of (*noise_seed, the step t, i) through Box-Muller (DESIGN.md 4.5).  noise_std = 0: seed and mask unused. */
 int otb_adam_step_sched(float* p, const float* g, float* m, float* v, long long n, const float* sumsq, float max_norm,
                         float base_lr, float model_size, float warmup_steps, float factor, float beta1, float beta2, float eps,
-                        float weight_decay, int32_t* counters, float* hyper, void* stream);
+                        float weight_decay, int32_t* counters, float* hyper, float noise_std, const int32_t* noise_seed,
+                        const uint8_t* noise_mask, void* stream);
+
+/* MixSpeech input (trainer.py:155-201): x f32 [B, T, F] and mask u8 [B, T] (0 / 1) of B >= 2 utterances -> P = B / 2 pairs,
+ * x_out f32 [P, T, F] = lambda * x[2p] + (1 - lambda) * x[2p + 1] (two separately rounded fp32 products, then their sum),
+ * mask_out u8 [P, T] = mask[2p] | mask[2p + 1].  lambda ~ Beta(1/2, 1/2) = sin^2(pi u / 2), u a counter hash of (*seed,
+ * *step) (both i32 device scalars); lam_out f32 [3] = {lambda, lambda * scale, (1 - lambda) * scale}. */
+int otb_mixspeech(const float* x, const uint8_t* mask, int B, int T, int F, const int32_t* seed, const int32_t* step, float scale,
+                  float* lam_out, float* x_out, uint8_t* mask_out, void* stream);
 
 /* ---- Recurrent language model (model/lm.py:31-90, rnnlm.yaml): nn.LSTM layers, gates ordered i, f, g, o.  Sequences are
  * time-major (row t*B + b, as nn.LSTM without batch_first).  The input projection gx f32 [L*B, 4H] = x W_ih^T + b_ih + b_hh
@@ -339,10 +351,11 @@ int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, cons
  * logp f32 [B*T, ldl] = log_softmax of the assistor's logits (otb_log_softmax); in_len i32 [B] valid frames; targets i64
  * [B, ldt] label rows (the first tgt_len[b] entries count); max_tgt >= every tgt_len (<= 64); nll f32 [B] per-utterance
  * negative log-likelihood (+inf if infeasible); loss f32 [1]; ws f32 [B, T, 2 max_tgt + 1] scratch (alpha + beta);
- * dlogits_bf16 (optional, bf16 [B*T, ldd]) = grad_scale * d loss / d logits (padded frames / infeasible utterances: 0). */
+ * dlogits_bf16 (optional, bf16 [B*T, ldd]) = grad_scale * d loss / d logits (padded frames / infeasible utterances: 0).
+ * grad_scale_dev (may be NULL): a device f32 scalar grad_scale is multiplied by, read on the device. */
 int otb_ctc_loss(const float* logp, int ldl, int B, int T, int V, const int32_t* in_len, const int64_t* targets, int ldt,
                  const int32_t* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, void* dlogits_bf16, int ldd,
-                 float grad_scale, void* stream);
+                 float grad_scale, const float* grad_scale_dev, void* stream);
 
 /* CTC decoding (CTCRecognizer, recognize/ctc.py) on the CTC head's logits f32 [B*T, ld]; in_len i32 [B] valid frames.
  * otb_ctc_frame_topk: per frame, the K (1..min(64, V)) best tokens as log-probs (log-softmax over the first V columns), best

@@ -56,7 +56,7 @@ _SIGS = {
                               _P, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P]),
     'otb_dwconv_swish': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_layernorm': (c_int, [_P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_float, c_int, c_int, _P]),
-    'otb_scale_add_table': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, c_int, c_int, c_int, _P]),
+    'otb_scale_add_table': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, c_int, c_int, c_int, _P, _P]),
     'otb_sinusoid_table': (c_int, [_P, c_int, c_int, c_int, _P]),
     'otb_embed_posenc': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, _P, c_int, _P]),
     'otb_log_softmax': (c_int, [_P, c_int, _P, c_int, c_int, c_int, _P]),
@@ -87,10 +87,12 @@ _SIGS = {
     'otb_embed_bwd': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_float, _P]),
     'otb_sumsq': (c_int, [_P, c_int64, _P, c_int, _P]),
     'otb_adam_step_sched': (c_int, [_P, _P, _P, _P, c_int64, _P, c_float, c_float, c_float, c_float, c_float, c_float, c_float,
-                                    c_float, c_float, _P, _P, _P]),
+                                    c_float, c_float, _P, _P, c_float, _P, _P, _P]),
+    'otb_mixspeech': (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_float, _P, _P, _P, _P]),
     'otb_fbank': (c_int, [_P, c_int, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
     'otb_utt_cmvn': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P]),
-    'otb_ctc_loss': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_int, c_float, _P]),
+    'otb_ctc_loss': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_int, c_float, _P,
+                             _P]),
     'otb_ctc_frame_topk': (c_int, [_P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P]),
     'otb_ctc_greedy': (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P]),
     'otb_ctc_prefix_beam': (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P]),

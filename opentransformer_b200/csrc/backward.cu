@@ -3,6 +3,7 @@
 // (otrans/train/trainer.py:206-234: loss.backward(), clip_grad_norm_, optimizer.step()).
 #include <math.h>
 
+#include "counter_rng.cuh"
 #include "dropout.cuh"
 #include "launch.cuh"
 #include "otb_internal.h"
@@ -313,19 +314,33 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g,
 // hyper (device f32 [4] = {lr, 1 - b1^t, 1 - b2^t, apply}) is written by adam_prepare_kernel, which owns the step counters
 // on the device so that a skipped (non-finite) step advances neither the LR schedule nor Adam's bias-correction count --
 // exactly what trainer.py:229-233 does on the host.
+// NOISE (trainer.py:223-227, gradient noise): the clipped gradient gets noise * z before the weight decay, z a standard
+// normal drawn from (*noise_seed, Adam step t = counters[0], element index) (counter_rng.cuh) on the elements whose bit is
+// set in noise_mask (the parameters: the alignment gaps of the flat buffer stay zero).  noise = sigma / accum_steps.
+template <bool NOISE>
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, size_t n, const float* __restrict__ sumsq,
                                                    float max_norm, float b1, float b2, float eps, float wd,
-                                                   const float* __restrict__ hyper) {
+                                                   const float* __restrict__ hyper, float noise, const int* __restrict__ noise_seed,
+                                                   const int* __restrict__ counters, const uint8_t* __restrict__ noise_mask) {
     const float total = sqrtf(*sumsq);
     if (!isfinite(total)) return;                      // NaN / Inf gradients: skip the step (trainer.py:229-230)
     const float lr = hyper[0], bc1 = hyper[1], bc2 = hyper[2];
     float coef = 1.0f;
     if (max_norm > 0.f) coef = fminf(1.0f, max_norm / (total + 1e-6f));
     const float step = lr / bc1, rs2 = rsqrtf(bc2);
+    uint32_t key = 0;
+    if constexpr (NOISE) key = rng_key((uint32_t)*noise_seed, (uint32_t)counters[0]);
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const float pi = p[i];
-        const float gi = g[i] * coef + wd * pi;
+        float gi;
+        if constexpr (NOISE) {
+            float gc = g[i] * coef;
+            if ((noise_mask[i >> 3] >> (i & 7)) & 1) gc = __fadd_rn(gc, __fmul_rn(noise, normal_at(key, i)));
+            gi = gc + wd * pi;
+        } else {
+            gi = g[i] * coef + wd * pi;
+        }
         const float mi = b1 * m[i] + (1.0f - b1) * gi;
         const float vi = b2 * v[i] + (1.0f - b2) * gi * gi;
         m[i] = mi;
@@ -366,13 +381,18 @@ const char* sumsq_launch(cudaStream_t st, const float* g, size_t n, float* out, 
 }
 const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
                               float max_norm, float base_lr, float model_size, float warmup, float factor, float b1, float b2,
-                              float eps, float wd, int* counters, float* hyper) {
+                              float eps, float wd, int* counters, float* hyper, float noise, const int* noise_seed,
+                              const uint8_t* noise_mask) {
     const char* err = launch<adam_prepare_kernel>(1, 1, 0, st, sumsq, counters, hyper, base_lr, model_size, warmup, factor, b1, b2);
     if (err) return err;
     size_t blocks = (n + 1023) / 1024;
     if (blocks > (size_t)(8 * num_sms())) blocks = 8 * num_sms();
     if (blocks < 1) blocks = 1;
-    return launch<adam_kernel>((unsigned)blocks, 256, 0, st, p, g, m, v, n, sumsq, max_norm, b1, b2, eps, wd, hyper);
+    if (noise > 0.f)
+        return launch<adam_kernel<true>>((unsigned)blocks, 256, 0, st, p, g, m, v, n, sumsq, max_norm, b1, b2, eps, wd, hyper, noise,
+                                         noise_seed, counters, noise_mask);
+    return launch<adam_kernel<false>>((unsigned)blocks, 256, 0, st, p, g, m, v, n, sumsq, max_norm, b1, b2, eps, wd, hyper, 0.f,
+                                      nullptr, nullptr, nullptr);
 }
 
 }  // namespace otb

@@ -205,11 +205,11 @@ int otb_layernorm(const void* x, int ldx, void* out, int ldo, int out_f32, const
 }
 
 int otb_scale_add_table(const void* x, int ldx, int x_f32, void* out, int ldo, float alpha, const float* table,
-                        int period, int M, int N, void* stream) {
+                        int period, int M, int N, const float* alpha_dev, void* stream) {
     if (!x || !out || M < 1 || N < 1) return fail("otb_scale_add_table", "bad arguments");
     if (table && period < 1) return fail("otb_scale_add_table", "table without period");
     RET("otb_scale_add_table", scale_add_table_launch(ST(stream), x, ldx, x_f32, reinterpret_cast<bf16*>(out), ldo, alpha,
-                                                      table, period, M, N));
+                                                      table, period, M, N, alpha_dev));
 }
 
 int otb_dwconv_swish(const void* x, const float* w, const float* b, void* out, int B, int T, int d, int k,
@@ -441,10 +441,20 @@ int otb_sumsq(const float* g, long long n, float* out, int zero_first, void* str
 
 int otb_adam_step_sched(float* p, const float* g, float* m, float* v, long long n, const float* sumsq, float max_norm,
                         float base_lr, float model_size, float warmup_steps, float factor, float beta1, float beta2, float eps,
-                        float weight_decay, int32_t* counters, float* hyper, void* stream) {
+                        float weight_decay, int32_t* counters, float* hyper, float noise_std, const int32_t* noise_seed,
+                        const uint8_t* noise_mask, void* stream) {
     if (!p || !g || !m || !v || !sumsq || !counters || !hyper || n < 1) return fail("otb_adam_step_sched", "bad arguments");
+    if (!(noise_std >= 0.f)) return fail("otb_adam_step_sched", "noise_std must be >= 0");
+    if (noise_std > 0.f && (!noise_seed || !noise_mask)) return fail("otb_adam_step_sched", "noise without seed or mask");
     RET("otb_adam_step_sched", adam_sched_launch(ST(stream), p, g, m, v, (size_t)n, sumsq, max_norm, base_lr, model_size, warmup_steps,
-                                                 factor, beta1, beta2, eps, weight_decay, counters, hyper));
+                                                 factor, beta1, beta2, eps, weight_decay, counters, hyper, noise_std, noise_seed,
+                                                 noise_mask));
+}
+
+int otb_mixspeech(const float* x, const uint8_t* mask, int B, int T, int F, const int32_t* seed, const int32_t* step, float scale,
+                  float* lam_out, float* x_out, uint8_t* mask_out, void* stream) {
+    if (!x || !mask || !seed || !step || !lam_out || !x_out || !mask_out) return fail("otb_mixspeech", "null operand");
+    RET("otb_mixspeech", mixspeech_launch(ST(stream), x, mask, B, T, F, seed, step, scale, lam_out, x_out, mask_out));
 }
 
 int otb_fbank(const float* wave, int ld_wave, const int32_t* n_samples, int B, const float* window, const float* bank,
@@ -460,11 +470,12 @@ int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, cons
 
 int otb_ctc_loss(const float* logp, int ldl, int B, int T, int V, const int32_t* in_len, const int64_t* targets, int ldt,
                  const int32_t* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, void* dlogits_bf16, int ldd,
-                 float grad_scale, void* stream) {
+                 float grad_scale, const float* grad_scale_dev, void* stream) {
     if (!logp || !in_len || !targets || !tgt_len || !nll || !loss || !ws) return fail("otb_ctc_loss", "null operand");
     if (ldl < V || (dlogits_bf16 && ldd < V)) return fail("otb_ctc_loss", "row pitch < V");
     RET("otb_ctc_loss", ctc_launch(ST(stream), logp, ldl, B, T, V, in_len, reinterpret_cast<const long long*>(targets), ldt, tgt_len, max_tgt,
-                                   blank, nll, loss, ws, reinterpret_cast<bf16*>(dlogits_bf16), ldd, grad_scale));
+                                   blank, nll, loss, ws, reinterpret_cast<bf16*>(dlogits_bf16), ldd, grad_scale,
+                                   grad_scale_dev));
 }
 
 int otb_ctc_frame_topk(const float* logits, int ld, int B, int T, int V, const int32_t* in_len, int K, float* top_lp,

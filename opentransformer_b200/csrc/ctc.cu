@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(256) ctc_grad_kernel(const float* __restrict__
                                                        const long long* __restrict__ targets, int ldt,
                                                        const int* __restrict__ tgt_len, int blank, const float* __restrict__ nll,
                                                        const float* __restrict__ ws, int S_ws, int B, float grad_scale,
-                                                       bf16* __restrict__ dlogits, int ldd) {
+                                                       bf16* __restrict__ dlogits, int ldd, const float* __restrict__ scale_dev) {
     __shared__ int lab[CTC_SMAX];
     __shared__ float occ[CTC_SMAX];
     const int row = blockIdx.x, b = row / T, t = row % T;
@@ -131,7 +131,9 @@ __global__ void __launch_bounds__(256) ctc_grad_kernel(const float* __restrict__
         return;
     }
     const float* lp = logp + (size_t)row * ldl;
-    const float scale = grad_scale / ((float)B * (float)max(tgt_len[b], 1));
+    // scale_dev (optional, read on the device): a loss weight known only on the device (MixSpeech's lambda / accum_steps)
+    const float gs = scale_dev ? grad_scale * *scale_dev : grad_scale;
+    const float scale = gs / ((float)B * (float)max(tgt_len[b], 1));
     for (int s = threadIdx.x; s < S; s += blockDim.x) {
         int l = blank;
         if (s & 1) {
@@ -161,7 +163,7 @@ __global__ void __launch_bounds__(256) ctc_grad_kernel(const float* __restrict__
 
 const char* ctc_launch(cudaStream_t st, const float* logp, int ldl, int B, int T, int V, const int* in_len, const long long* targets,
                        int ldt, const int* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, bf16* dlogits, int ldd,
-                       float grad_scale) {
+                       float grad_scale, const float* scale_dev) {
     if (B < 1 || T < 1 || V < 2) return "ctc: empty problem";
     if (max_tgt < 0 || 2 * max_tgt + 1 > CTC_SMAX) return "ctc: targets longer than 64 labels are not supported";
     if (blank < 0 || blank >= V) return "ctc: bad blank id";
@@ -172,7 +174,7 @@ const char* ctc_launch(cudaStream_t st, const float* logp, int ldl, int B, int T
     if ((err = launch<ctc_mean_kernel>(1, 256, 0, st, nll, tgt_len, B, loss))) return err;
     if (!dlogits) return nullptr;
     return launch<ctc_grad_kernel>(B * T, 256, 0, st, logp, ldl, T, V, in_len, targets, ldt, tgt_len, blank, nll, ws, S_ws, B,
-                                   grad_scale, dlogits, ldd);
+                                   grad_scale, dlogits, ldd, scale_dev);
 }
 
 }  // namespace otb

@@ -546,24 +546,27 @@ const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, 
 // ------------------------------------------------------------------------------------------------
 // Stand-alone PositionalEncoding.forward: out = x * alpha + table[row % period]   (module/pos.py:56)
 // (the fused path does this in the front-end Linear's epilogue; this kernel serves the module-level
-// drop-in API where frontend and encoder are called separately).  x f32 or bf16 -> bf16.
+// drop-in API where frontend and encoder are called separately).  x f32 or bf16 -> bf16.  alpha_dev (optional): alpha is
+// multiplied by this device scalar (a loss-gradient scale known only on the device, e.g. MixSpeech's lambda / accum_steps).
 // ------------------------------------------------------------------------------------------------
 __global__ void scale_add_table_kernel(const void* __restrict__ x, int ldx, int x_f32, bf16* __restrict__ out, int ldo,
-                                       float alpha, const float* __restrict__ table, int period, int M, int N) {
+                                       float alpha, const float* __restrict__ table, int period, int M, int N,
+                                       const float* __restrict__ alpha_dev) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int row = (int)(i / N), col = (int)(i % N);
     if (row >= M) return;
     const float v = x_f32 ? reinterpret_cast<const float*>(x)[(size_t)row * ldx + col]
                           : __bfloat162float(reinterpret_cast<const bf16*>(x)[(size_t)row * ldx + col]);
     const float t = table ? table[(size_t)(row % period) * N + col] : 0.f;
-    out[(size_t)row * ldo + col] = __float2bfloat16(v * alpha + t);
+    const float a = alpha_dev ? alpha * *alpha_dev : alpha;
+    out[(size_t)row * ldo + col] = __float2bfloat16(v * a + t);
 }
 
 const char* scale_add_table_launch(cudaStream_t st, const void* x, int ldx, int x_f32, bf16* out, int ldo, float alpha,
-                                   const float* table, int period, int M, int N) {
+                                   const float* table, int period, int M, int N, const float* alpha_dev) {
     const size_t n = (size_t)M * N;
     return launch<scale_add_table_kernel>(dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, x, ldx, x_f32, out, ldo, alpha,
-                                          table, period, M, N);
+                                          table, period, M, N, alpha_dev);
 }
 
 // ------------------------------------------------------------------------------------------------

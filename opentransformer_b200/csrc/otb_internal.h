@@ -127,7 +127,10 @@ const char* spec_augment_launch(cudaStream_t st, float* x, const int* bands, int
 const char* sumsq_launch(cudaStream_t st, const float* g, size_t n, float* out, int zero_first);
 const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
                               float max_norm, float base_lr, float model_size, float warmup, float factor, float b1, float b2,
-                              float eps, float wd, int* counters, float* hyper);
+                              float eps, float wd, int* counters, float* hyper, float noise, const int* noise_seed,
+                              const uint8_t* noise_mask);
+const char* mixspeech_launch(cudaStream_t st, const float* x, const uint8_t* mask, int B, int T, int F, const int* seed, const int* step,
+                             float scale, float* lam_out, float* x_out, uint8_t* mask_out);
 
 struct BeamState {
     int* tok_hist;
@@ -158,7 +161,7 @@ const char* conv1_launch(cudaStream_t st, const float* x, const float* w, const 
 const char* layernorm_launch(cudaStream_t st, const bf16* x, int ldx, void* out, int ldo, int out_f32, const float* g1,
                              const float* b1, const float* g2, const float* b2, float eps, int M, int N);
 const char* scale_add_table_launch(cudaStream_t st, const void* x, int ldx, int x_f32, bf16* out, int ldo, float alpha,
-                                   const float* table, int period, int M, int N);
+                                   const float* table, int period, int M, int N, const float* alpha_dev);
 // Conformer convolution module in training mode (conformer_train.cu)
 const char* conv_bn_train_launch(cudaStream_t st, const bf16* x, const int* len, const float* w, const float* wb, const float* gamma,
                                  const float* beta, float* run_mean, float* run_var, long long* n_batches, float momentum, float eps,
@@ -194,7 +197,7 @@ const char* ls_ce_launch(cudaStream_t st, const float* logits, int ldl, const lo
 
 const char* ctc_launch(cudaStream_t st, const float* logp, int ldl, int B, int T, int V, const int* in_len, const long long* targets,
                        int ldt, const int* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, bf16* dlogits, int ldd,
-                       float grad_scale);
+                       float grad_scale, const float* scale_dev);
 const char* ctc_frame_topk_launch(cudaStream_t st, const float* logits, int ld, int B, int T, int V, const int* in_len, int K,
                                   float* top_lp, int* top_id);
 const char* ctc_greedy_launch(cudaStream_t st, const float* top_lp, const int* top_id, int ldk, int B, int T, const int* in_len,

@@ -137,6 +137,7 @@ class SpeechToText(nn.Module):
                                     targets_length, self.assistor.blank)
 
     train_pass = train.forward_backward
+    mix_batch = train.mixspeech_halves
 
     def train_batch(self, inputs, mask, truth, truth_length=None):
         """FusedTrainer.step's arguments as train_pass takes them; it reads the label counts as int32."""
@@ -231,6 +232,7 @@ class CTCModel(nn.Module):
                                     self.assistor.blank)
 
     train_pass = train.ctc_forward_backward
+    mix_batch = train.mixspeech_halves
     check_fused_trainer = SpeechToText.check_fused_trainer
 
     def train_batch(self, inputs, mask, truth, truth_length=None):

@@ -262,13 +262,16 @@ def layernorm(x, g1, b1, g2=None, b2=None, eps=1e-5, out=None, out_f32=False):
     return out
 
 
-def scale_add_table(x, alpha=1.0, table=None, period=1, out=None):
-    """bf16 out = x * alpha + table[row % period]; x f32 or bf16 2-D."""
+def scale_add_table(x, alpha=1.0, table=None, period=1, out=None, scale_dev=None):
+    """bf16 out = x * alpha + table[row % period]; x f32 or bf16 2-D.  scale_dev: an f32 device scalar alpha is multiplied
+    by on the device (a loss-gradient scale that never goes to the host)."""
     M, N = x.shape
     if out is None:
         out = torch.empty(M, N, dtype=BF16, device=x.device)
+    if scale_dev is not None:
+        _need(scale_dev, torch.float32, 'scale_dev')
     check(_lib.lib().otb_scale_add_table(_p(x), x.stride(0), 1 if x.dtype == torch.float32 else 0, _p(out),
-                                         out.stride(0), alpha, _p(table), period, M, N, _stream()),
+                                         out.stride(0), alpha, _p(table), period, M, N, _p(scale_dev), _stream()),
           'otb_scale_add_table')
     _count()
     return out
@@ -598,21 +601,63 @@ def sumsq(g, out, zero_first=True):
 
 
 def adam_step_sched(p, g, m, v, sumsq_buf, max_norm, base_lr, model_size, warmup_steps, factor, betas, eps, weight_decay,
-                    counters, hyper):
-    """clip + Adam with the step counters / Noam schedule evaluated on the device (otb_adam_step_sched)."""
+                    counters, hyper, noise_std=0.0, noise_seed=None, noise_mask=None):
+    """clip + Adam with the step counters / Noam schedule evaluated on the device (otb_adam_step_sched).  noise_std > 0:
+    gradient noise noise_std * N(0, 1) after the clip on the elements whose bit is set in noise_mask (u8 [(n + 7) // 8],
+    noise_bitmask), drawn from the i32 device scalar noise_seed and the step count."""
     for t, n in ((p, 'p'), (g, 'g'), (m, 'm'), (v, 'v'), (hyper, 'hyper')):
         _need(t, torch.float32, n)
     _need(counters, torch.int32, 'counters')
+    if noise_std < 0:
+        raise ValueError('adam_step_sched: noise_std must be >= 0')
+    if noise_std > 0:
+        _need(noise_seed, torch.int32, 'noise_seed'); _need(noise_mask, torch.uint8, 'noise_mask')
+        if noise_mask.numel() < (p.numel() + 7) // 8:
+            raise ValueError('adam_step_sched: noise_mask needs (n + 7) // 8 bytes')
     check(_lib.lib().otb_adam_step_sched(_p(p), _p(g), _p(m), _p(v), p.numel(), _p(sumsq_buf), max_norm, base_lr,
                                          float(model_size), float(warmup_steps or 0), factor, betas[0], betas[1], eps,
-                                         weight_decay, _p(counters), _p(hyper), _stream()), 'otb_adam_step_sched')
+                                         weight_decay, _p(counters), _p(hyper), float(noise_std),
+                                         _p(noise_seed) if noise_std > 0 else None, _p(noise_mask) if noise_std > 0 else None,
+                                         _stream()), 'otb_adam_step_sched')
     _count(2)
 
 
-def ctc_loss(logits, B, T, V, in_len, targets, tgt_len, blank=0, want_grad=False, grad_scale=1.0):
+def noise_bitmask(n, spans):
+    """The noise_mask of adam_step_sched: u8 [(n + 7) // 8] with bit i & 7 of byte i >> 3 set for every i in one of the
+    [offset, offset + count) spans (the parameters of a flat buffer), little bit order.  Built on the host."""
+    bits = torch.zeros((n + 7) // 8 * 8, dtype=torch.bool)
+    for o, k in spans:
+        bits[o:o + k] = True
+    weights = torch.tensor([1 << j for j in range(8)], dtype=torch.int32)
+    return (bits.view(-1, 8).to(torch.int32) * weights).sum(1).to(torch.uint8)
+
+
+def mixspeech(x, mask, seed, step, scale, lam_out):
+    """MixSpeech's input (otb_mixspeech): x f32 [B, T, F], mask bool [B, T], B >= 2 -> (x_mix f32 [B // 2, T, F], mask_mix
+    bool [B // 2, T]); lambda is drawn on the device from the i32 device scalars seed / step, and lam_out f32 [3] receives
+    {lambda, lambda * scale, (1 - lambda) * scale}."""
+    _need(x, torch.float32, 'x'); _need(mask, torch.bool, 'mask'); _need(lam_out, torch.float32, 'lam_out')
+    _need(seed, torch.int32, 'seed'); _need(step, torch.int32, 'step')
+    if x.dim() != 3 or mask.shape != x.shape[:2]:
+        raise ValueError(f'mixspeech: x [B, T, F] and mask [B, T], got {tuple(x.shape)} and {tuple(mask.shape)}')
+    B, T, F = x.shape
+    if B < 2:
+        raise ValueError('MixSpeech mixes pairs of utterances: it needs a batch of at least 2')
+    x_out = torch.empty(B // 2, T, F, dtype=torch.float32, device=x.device)
+    m_out = torch.empty(B // 2, T, dtype=torch.bool, device=x.device)
+    check(_lib.lib().otb_mixspeech(_p(x), _p(mask), B, T, F, _p(seed), _p(step), float(scale), _p(lam_out), _p(x_out), _p(m_out),
+                                   _stream()), 'otb_mixspeech')
+    _count()
+    return x_out, m_out
+
+
+def ctc_loss(logits, B, T, V, in_len, targets, tgt_len, blank=0, want_grad=False, grad_scale=1.0, scale_dev=None):
     """nn.CTCLoss(blank, 'mean', zero_infinity=True) on logits f32 [B*T, ld] (model/ctc.py:48-52).
-    -> (loss 0-d, nll f32 [B], dlogits bf16 [B*T, ld] or None)."""
+    -> (loss 0-d, nll f32 [B], dlogits bf16 [B*T, ld] or None).  The gradient is scaled by grad_scale, times the f32 device
+    scalar scale_dev when one is given (read on the device)."""
     _need(logits, torch.float32, 'logits'); _need(in_len, torch.int32, 'in_len'); _need(tgt_len, torch.int32, 'tgt_len')
+    if scale_dev is not None:
+        _need(scale_dev, torch.float32, 'scale_dev')
     targets = targets.contiguous()
     dev = logits.device
     ld = logits.stride(0)
@@ -624,7 +669,8 @@ def ctc_loss(logits, B, T, V, in_len, targets, tgt_len, blank=0, want_grad=False
     ws = torch.empty(B, T, 2 * max_tgt + 1, dtype=torch.float32, device=dev)
     dl = torch.empty(B * T, ld, dtype=BF16, device=dev) if want_grad else None
     check(_lib.lib().otb_ctc_loss(_p(logp), ld, B, T, V, _p(in_len), _p(targets), targets.stride(0), _p(tgt_len), max_tgt, blank,
-                                  _p(nll), _p(loss), _p(ws), _p(dl), ld if want_grad else 0, float(grad_scale), _stream()),
+                                  _p(nll), _p(loss), _p(ws), _p(dl), ld if want_grad else 0, float(grad_scale),
+                                  _p(scale_dev), _stream()),
           'otb_ctc_loss')
     _count(4 if want_grad else 3)
     return loss[0], nll, dl

@@ -16,10 +16,13 @@ How a model plugs into training -- three methods on its class, and nothing here 
     model.train_batch(*step arguments) -> batch       FusedTrainer.step's arguments, validated, as train_pass takes them
                                                       (not on a model check_fused_trainer always refuses)
     model.check_fused_trainer()                       what FusedTrainer refuses at construction, before any device work
+    model.mix_batch(*batch, seed=, step=, scale=, lam=) -> (batch of pass 1, batch of pass 2)
+                                                      MixSpeech's two half-batches (mixspeech_halves; speech models only)
 
 batch is (inputs, mask, truth, truth_length or None) for a SpeechToText (forward_backward) and a CTCModel
 (ctc_forward_backward), (inputs, targets) for the language models (lm.py).  grad_sink: name -> fp32 tensor the gradients
-(x grad_scale) are ADDED into (a gradient accumulation buffer); bf16_of: see LayerPack; drop_seed: int32 device tensor [1],
+(x grad_scale) are ADDED into (a gradient accumulation buffer); grad_scale: a float, or an f32 0-d device tensor that the
+kernels making the loss gradient read on the device (MixSpeech's lambda / accum_steps); bf16_of: see LayerPack; drop_seed: int32 device tensor [1],
 the dropout seed of THIS pass (read on the device), required when a dropout rate is non-zero.  The only torch autograd node is `_TrainingLoss` (loss_with_grad), which
 makes `model(inputs, targets)[0].backward()` populate `.grad` of the fp32 master parameters exactly like the reference
 module; loss_train_mode is the same pass without gradients, and FusedTrainer's micro-step is train_pass into its grad_sink.
@@ -624,6 +627,14 @@ def _ctc_head(model, pk):
 _CTC_HEAD = ('assistor.output_layer.weight', 'assistor.output_layer.bias')      # its gradients' names
 
 
+def _loss_scale(grad_scale, w):
+    """The loss-gradient scale w * grad_scale as the kernels take it: (host factor, f32 device scalar or None).  A float
+    grad_scale is folded on the host, exactly as before; a device tensor is multiplied in by the kernel."""
+    if torch.is_tensor(grad_scale):
+        return w, grad_scale
+    return w * grad_scale, None
+
+
 def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=True, grad_sink=None, grad_scale=1.0,
                      bf16_of=None, drop_seed=None):
     """SpeechToText.train_pass (the contract is at the top of this file).  inputs f32 [B,T,F], mask bool [B,T], truth i64
@@ -663,9 +674,10 @@ def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=T
     loss_ctc, dctc = None, None
     if ctc_w > 0.0:     # CTCAssistor on the encoder states (model/ctc.py:33-52)
         wc, bc, ldc = _ctc_head(model, pk)
+        cs, cdev = _loss_scale(grad_scale, ctc_w)
         loss_ctc, _, dctc = ops.ctc_loss(head_fwd(mem, wc, bc, ldc), B, T2, V, lengths, tgt_out,
                                          truth_length.to(torch.int32).to(dev).contiguous(),
-                                         model.assistor.blank, want_grad=want_grads, grad_scale=ctc_w * grad_scale)
+                                         model.assistor.blank, want_grad=want_grads, grad_scale=cs, scale_dev=cdev)
     model._last_ctc_loss = loss_ctc
     if not want_grads:
         loss, _ = ops.ls_cross_entropy(logits, tgt_out, V, model.smoothing)
@@ -673,9 +685,10 @@ def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=T
             loss = (1.0 - ctc_w) * loss + ctc_w * loss_ctc
         return loss, None
     loss, dlogits = ops.ls_cross_entropy_train(logits, tgt_out, V, model.smoothing)
-    att_scale = grad_scale * (1.0 - ctc_w)
-    if att_scale != 1.0:
-        dlogits = ops.scale_add_table(dlogits, att_scale)                        # loss / accum_steps (trainer.py:216), x (1 - w)
+    att_scale, att_dev = _loss_scale(grad_scale, 1.0 - ctc_w)
+    if att_dev is not None or att_scale != 1.0:
+        # loss / accum_steps (trainer.py:216), x (1 - w)
+        dlogits = ops.scale_add_table(dlogits, att_scale, scale_dev=att_dev)
     if ctc_w > 0.0:
         loss = (1.0 - ctc_w) * loss + ctc_w * loss_ctc
 
@@ -710,13 +723,36 @@ def ctc_forward_backward(model, inputs, mask, truth, truth_length, want_grads=Tr
     V = model.vocab_size
     wc, bc, ld = _ctc_head(model, pk)
     tlen = (truth_length.to(inputs.device).to(torch.int32) - 1).contiguous()
+    cs, cdev = _loss_scale(grad_scale, 1.0)
     loss, _, dctc = ops.ctc_loss(head_fwd(mem, wc, bc, ld), tr.B, tr.T2, V, tr.lengths, truth[:, 1:-1].contiguous(), tlen,
-                                 model.assistor.blank, want_grad=want_grads, grad_scale=grad_scale)
+                                 model.assistor.blank, want_grad=want_grads, grad_scale=cs, scale_dev=cdev)
     if not want_grads:
         return loss, None
     g = Grads(grad_sink)
     _encoder_bwd(model, pk, tr, head_bwd(dctc, mem, wc, g, *_CTC_HEAD), g)
     return loss, g
+
+
+def mixspeech_halves(model, inputs, mask, truth, truth_length=None, *, seed, step, scale, lam):
+    """mix_batch of the speech models (SpeechToText, CTCModel): MixSpeech (trainer.py:155-201) on a batch as train_batch
+    returns it.  With P = B // 2 pairs (an odd last utterance is dropped) and lambda ~ Beta(1/2, 1/2) drawn on the device
+    from the i32 device scalars seed / step, otb_mixspeech makes x_mix = lambda x[0::2] + (1 - lambda) x[1::2] and mask_mix
+    = mask[0::2] | mask[1::2]; lam (f32 [3]) receives {lambda, lambda * scale, (1 - lambda) * scale}.  -> the batches of
+    the two passes, (x_mix, mask_mix, truth[0::2], truth_length[0::2]) and the same with [1::2]: pass 1 is weighted by
+    lambda and pass 2 by 1 - lambda (their loss-gradient scales are lam[1] and lam[2]).  B < 2 raises ValueError."""
+    if inputs.dim() != 3:
+        raise ValueError(f'MixSpeech mixes [B, T, F] features, got inputs of shape {tuple(inputs.shape)}')
+    B = inputs.shape[0]
+    if B < 2:
+        raise ValueError('MixSpeech mixes pairs of utterances: it needs a batch of at least 2')
+    n = B // 2 * 2
+    x_mix, m_mix = ops.mixspeech(inputs.contiguous().float(), mask.contiguous(), seed, step, scale, lam)
+
+    def half(k):
+        tl = None if truth_length is None else truth_length[k:n:2].contiguous()
+        return x_mix, m_mix, truth[k:n:2].contiguous(), tl
+
+    return half(0), half(1)
 
 
 def next_drop_seed(model, device):
@@ -770,10 +806,24 @@ class FusedTrainer:
     """The inner step of Trainer.train_one_epoch (trainer.py:206-234) on flat fp32 buffers:
     forward + hand-written backward -> (data-parallel) gradient all-reduce over NCCL -> global-norm clip + Adam in two
     kernels, no host synchronisation.  Parameters become views into one flat buffer (state_dict keys / shapes unchanged).
-    `model` is any model with the training contract at the top of this file."""
+    `model` is any model with the training contract at the top of this file.
+
+    mixspeech=True (run.py -ms, trainer.py:155-201): every micro-step mixes pairs of utterances with lambda ~ Beta(1/2,
+    1/2) drawn on the device (model.mix_batch) and runs the model twice on the mix, once per target half, each pass with
+    its own dropout seed; the loss is lambda L1 + (1 - lambda) L2.  Speech models only (NotImplementedError otherwise).
+    `last_lambda` is the device scalar of the last micro-step's lambda.
+    grad_noise = sigma > 0 (train: grad_noise, trainer.py:223-227): sigma / accum_steps * N(0, 1) is added to every trained
+    gradient element after the clip and before Adam, inside the fused Adam launch.  The reference's loop adds it to every
+    parameter with requires_grad and raises TypeError on a Conformer, whose post_ffn parameters have no gradient; this
+    trainer leaves them out (unused_parameters) and adds noise to what it trains."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6, clip_grad=5.0, model_size=256,
-                 warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True):
+                 warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True, mixspeech=False,
+                 grad_noise=0.0):
+        if mixspeech and not hasattr(model, 'mix_batch'):
+            raise NotImplementedError(f'MixSpeech mixes [B, T, F] speech features; {type(model).__name__} takes token inputs')
+        if not grad_noise >= 0.0:
+            raise ValueError(f'grad_noise must be >= 0, got {grad_noise}')
         model.check_fused_trainer()
         self.model = model
         # parameters the forward never reads (a Conformer's post_ffn) stay out of the flat buffers: no gradient, no weight decay
@@ -826,6 +876,20 @@ class FusedTrainer:
         # training-mode BatchNorm buffers (Conformer): updated by every micro-step, inside the graph when one is replayed
         self.bn_buffers = [t for n, t in model.named_buffers() if n.startswith('encoder.') and
                            n.rsplit('.', 1)[-1] in ('running_mean', 'running_var', 'num_batches_tracked')]
+        # MixSpeech: lambda is a counter hash of (mix seed, micro-step), both on the device; last_lambda holds {lambda,
+        # lambda / accum_steps, (1 - lambda) / accum_steps}, the last two the loss-gradient scales of the two passes
+        self.mixspeech = bool(mixspeech)
+        self.grad_noise = float(grad_noise)
+        self.mix_seed = self.mix_step = self._lam = self.noise_seed = self.noise_mask = None
+        if self.mixspeech:
+            self.mix_seed = torch.randint(0, 2 ** 31 - 1, (1,), dtype=torch.int32).to(dev)
+            self.mix_step = torch.zeros(1, dtype=torch.int32, device=dev)
+            self._lam = torch.zeros(3, dtype=torch.float32, device=dev)
+        if self.grad_noise > 0.0:
+            # every rank must add the same noise (the reference seeds all ranks alike, run.py:23-26)
+            self.noise_seed = torch.randint(0, 2 ** 31 - 1, (1,), dtype=torch.int32).to(dev)
+            self.noise_mask = ops.noise_bitmask(total, [self.offsets[n] for n, _ in self.params]).to(dev)
+        broadcast_from_first_([t for t in (self.mix_seed, self.noise_seed) if t is not None], process_group)
 
     @property
     def opt_steps(self):
@@ -844,6 +908,11 @@ class FusedTrainer:
             return transformer_lr(self.global_step, self.model_size, self.warmup, self.factor)
         return self.base_lr
 
+    @property
+    def last_lambda(self):
+        """MixSpeech's lambda of the last micro-step: f32 0-d device tensor (None without mixspeech)."""
+        return None if self._lam is None else self._lam[0]
+
     def _bf16_of(self, param):
         (o, k), shape = self._by_ptr[param.data_ptr()]
         return self.flat_bf16[o:o + k].view(shape)
@@ -852,10 +921,27 @@ class FusedTrainer:
         """forward + backward of one micro-batch (what model.train_batch returned); gradients / accum_steps are ADDED into
         the flat buffer by the backward kernels themselves (no per-parameter add)."""
         self.flat_bf16.copy_(self.flat_p)
+        if self.mixspeech:
+            return self._micro_mix(batch)
         self.drop_seed.add_(1)
         loss, _ = self.model.train_pass(*batch, grad_sink=self.sink, grad_scale=1.0 / self.accum_steps, bf16_of=self._bf16_of,
                                         drop_seed=self.drop_seed)
         return loss
+
+    def _micro_mix(self, batch):
+        """MixSpeech micro-step: the mix, then two passes over it (not one merged 2P-row pass: the reference's two forwards
+        draw independent dropout masks and update a Conformer's BatchNorm statistics twice), their gradients scaled by
+        lambda / accum_steps and (1 - lambda) / accum_steps on the device.  lambda never goes to the host."""
+        self.mix_step.add_(1)
+        halves = self.model.mix_batch(*batch, seed=self.mix_seed, step=self.mix_step, scale=1.0 / self.accum_steps, lam=self._lam)
+        losses = []
+        for k, half in enumerate(halves):
+            self.drop_seed.add_(1)
+            loss, _ = self.model.train_pass(*half, grad_sink=self.sink, grad_scale=self._lam[1 + k], bf16_of=self._bf16_of,
+                                            drop_seed=self.drop_seed)
+            losses.append(loss)
+        lam = self._lam[0]
+        return lam * losses[0] + (1 - lam) * losses[1]         # trainer.py:197
 
     def _graph_for(self, batch):
         """The ~870 launches of one micro-batch captured once per input geometry and replayed: launched one by one from
@@ -879,6 +965,8 @@ class FusedTrainer:
             static = tuple(None if t is None else t.to(dev).clone() for t in batch)
             snap = self.flat_g.clone()
             bn_snap = [t.clone() for t in self.bn_buffers]          # the warm-up must not count as a step
+            if self.mixspeech:      # nor draw lambda or masks: a resumed run continues the same sequence
+                bn_snap += [self.drop_seed.clone(), self.mix_step.clone()]
             cur = torch.cuda.current_stream()
             side = torch.cuda.Stream()
             side.wait_stream(cur)
@@ -886,7 +974,7 @@ class FusedTrainer:
                 self._micro(static)
             cur.wait_stream(side)
             self.flat_g.copy_(snap)
-            for t, v in zip(self.bn_buffers, bn_snap):
+            for t, v in zip(self.bn_buffers + ([self.drop_seed, self.mix_step] if self.mixspeech else []), bn_snap):
                 t.copy_(v)
             graph = torch.cuda.CUDAGraph()
             n0 = ops.COUNTERS['launches']
@@ -898,6 +986,98 @@ class FusedTrainer:
         self._graphs[key] = ent       # (re-)insert as most recently used
         return ent
 
+    # ---- optimizer state: the reference's checkpoint (trainer.py:280-290, loaded by run.py:54-61 with -ct -ios) ----
+
+    def _torch_adam(self):
+        """A torch.optim.Adam over the reference's parameter list (run.py:42-44: every parameter with requires_grad, a
+        Conformer's post_ffn included) with this trainer's hyper-parameters and no state."""
+        params = [p for p in self.model.parameters() if p.requires_grad]
+        return torch.optim.Adam(params, lr=self.lr(), betas=self.betas, eps=self.eps, weight_decay=self.wd)
+
+    def state_dict(self):
+        """{'global_step', 'optim', 'fused_trainer'} -- what the reference's save_optimizer_state_dict writes, plus this
+        trainer's own counters.  'optim' is torch.optim.Adam.state_dict() of the reference's parameter list, built by torch
+        itself from the flat buffers (exp_avg, exp_avg_sq and step of every trained parameter; a parameter the trainer
+        leaves out, such as a Conformer's post_ffn, keeps its index and has no state, as torch's Adam leaves a parameter
+        whose gradient stays None), so run.py -ct -ios loads the file unchanged.  'fused_trainer' holds the skipped steps
+        and the random state (dropout seed, MixSpeech seed and micro-step, noise seed), so that a resumed run continues the
+        same sequence.  Save at the end of an accumulation window: a gradient still accumulating is not saved (the
+        reference does not save it either)."""
+        t, global_step, skipped = self.counters.tolist()
+        opt = self._torch_adam()
+        by_id = {id(p): n for n, p in self.model.named_parameters()}
+        if t > 0:
+            for p in opt.param_groups[0]['params']:
+                n = by_id[id(p)]
+                if n not in self.offsets:
+                    continue
+                o, k = self.offsets[n]
+                opt.state[p] = {'step': torch.tensor(float(t)), 'exp_avg': self.m[o:o + k].view(p.shape).clone(),
+                                'exp_avg_sq': self.v[o:o + k].view(p.shape).clone()}
+
+        def host(x):
+            return None if x is None else int(x.reshape(-1)[0])
+
+        own = {'skipped_steps': skipped, 'drop_seed': host(self.drop_seed), 'mix_seed': host(self.mix_seed),
+               'mix_step': host(self.mix_step), 'noise_seed': host(self.noise_seed)}
+        return {'global_step': global_step, 'optim': opt.state_dict(), 'fused_trainer': own}
+
+    def load_state_dict(self, ckpt):
+        """Resume from state_dict()'s format, or a file the reference's Trainer wrote ({'global_step', 'optim'}): Adam's
+        moments go into the flat buffers and counters = [Adam step, global_step, skipped or 0], so the next update uses
+        lr(global_step + 1) and Adam step + 1, as the reference's does after run.py -ct -ios.  The file's betas, eps and
+        weight_decay replace the constructor's, as torch's loader does; the learning rate stays this trainer's schedule.
+        The file is validated by torch.optim.Adam.load_state_dict after these refusals (ValueError, before any device work):
+        no 'global_step', a different parameter count or shape, amsgrad, unequal step counts over the trained parameters."""
+        if 'global_step' not in ckpt:
+            raise ValueError("optimizer checkpoint without 'global_step' (trainer.py:280-288 writes it)")
+        sd = ckpt['optim']
+        groups = sd['param_groups']
+        named = [(n, p) for n, p in self.model.named_parameters() if p.requires_grad]
+        ids = [i for g in groups for i in g['params']]
+        if len(ids) != len(named):
+            raise ValueError(f'optimizer checkpoint for {len(ids)} parameters, this model trains {len(named)}')
+        if any(g.get('amsgrad', False) for g in groups):
+            raise ValueError('optimizer checkpoint with amsgrad=True: FusedTrainer runs plain Adam')
+        steps = set()
+        for pid, (n, p) in zip(ids, named):
+            st = sd['state'].get(pid)
+            if st is None:
+                if n in self.offsets:
+                    steps.add(0)
+                continue
+            for key in ('exp_avg', 'exp_avg_sq'):
+                if tuple(st[key].shape) != tuple(p.shape):
+                    raise ValueError(f'optimizer checkpoint: {key} of {n} has shape {tuple(st[key].shape)}, the parameter '
+                                     f'{tuple(p.shape)}')
+            if n in self.offsets:
+                steps.add(int(float(st['step'])))
+        if len(steps) > 1:
+            raise ValueError(f'optimizer checkpoint with unequal Adam step counts over the trained parameters: {sorted(steps)}')
+        opt = self._torch_adam()
+        opt.load_state_dict(sd)
+        g = opt.param_groups[0]
+        self.betas, self.eps, self.wd = tuple(g['betas']), g['eps'], g['weight_decay']
+        t = steps.pop() if steps else 0
+        with torch.no_grad():
+            self.m.zero_()
+            self.v.zero_()
+            for n, p in named:
+                st = opt.state.get(p)
+                if n not in self.offsets or not st:
+                    continue
+                o, k = self.offsets[n]
+                self.m[o:o + k].copy_(st['exp_avg'].reshape(-1))
+                self.v[o:o + k].copy_(st['exp_avg_sq'].reshape(-1))
+            own = ckpt.get('fused_trainer') or {}
+            self.counters.copy_(torch.tensor([t, int(ckpt['global_step']), int(own.get('skipped_steps', 0))], dtype=torch.int32))
+            for name in ('drop_seed', 'mix_seed', 'mix_step', 'noise_seed'):
+                dst = getattr(self, name)
+                if dst is not None and own.get(name) is not None:
+                    dst.fill_(int(own[name]))
+            self.flat_g.zero_()
+        self.micro = 0
+
     def step(self, *batch, truth_length=None):
         """One micro-batch; every `accum_steps` calls an optimizer step.  Returns the (un-scaled) loss tensor.
         The arguments are the model's batch, which its train_batch validates (TypeError): step(inputs, mask, truth,
@@ -907,6 +1087,8 @@ class FusedTrainer:
         if truth_length is not None:
             batch += (truth_length,)
         batch = self.model.train_batch(*batch)
+        if self.mixspeech and batch[0].shape[0] < 2:
+            raise ValueError('MixSpeech mixes pairs of utterances: it needs a batch of at least 2')
         with torch.no_grad():
             # data parallel: BatchNorm running statistics follow the first rank's (DistributedDataParallel's
             # broadcast_buffers): each rank's forward updates them from its own shard, so they would drift apart
@@ -930,7 +1112,9 @@ class FusedTrainer:
                 allreduce_mean_(self.flat_g, self.group)
                 ops.sumsq(self.flat_g, self.sumsq)
                 ops.adam_step_sched(self.flat_p, self.flat_g, self.m, self.v, self.sumsq, self.clip, self.base_lr, self.model_size,
-                                    self.warmup, self.factor, self.betas, self.eps, self.wd, self.counters, self.hyper)
+                                    self.warmup, self.factor, self.betas, self.eps, self.wd, self.counters, self.hyper,
+                                    noise_std=self.grad_noise / self.accum_steps, noise_seed=self.noise_seed,
+                                    noise_mask=self.noise_mask)
                 self.flat_g.zero_()
                 modules.bump_param_generation()     # bf16 shadow copies (modules._Packed) must be rebuilt
         return loss
