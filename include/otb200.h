@@ -429,6 +429,25 @@ int otb_nbest_rescore(const int32_t* tgt, int Lp, const int32_t* len, const floa
                       float weight, int nbest, int Lout, int64_t pad_id, int64_t* ids, int32_t* out_len, float* out_score,
                       void* stream);
 
+/* Minimum word error rate training (Prabhavalkar et al. 2018; the reference has no counterpart).
+ * otb_edit_distance: out i32 [N] = the Levenshtein distance (unit costs) between hypothesis i, the first hyp_len[i] tokens of
+ * hyp i32 [N, ldh], and reference i / K, the first ref_len[i / K] tokens of ref i32 [ceil(N / K), ldr].  Lengths are clamped
+ * to [0, max_hyp] and [0, max_ref]; max_hyp, max_ref <= 1023 (refused otherwise, before any launch).  Exact. */
+int otb_edit_distance(const int32_t* hyp, int ldh, const int32_t* hyp_len, const int32_t* ref, int ldr, const int32_t* ref_len, int N,
+                      int K, int max_hyp, int max_ref, int32_t* out, void* stream);
+/* One warp per utterance over its K <= 32 hypotheses, h = b * K + k, laid out as otb_nbest_rescore's: tgt i32 [B*K, Lp] the
+ * scored tokens y <S/E> (-1 after), len i32 [B*K] the length n of y (clamped to [0, Lp - 1]), err i32 [B*K] its edit distance W,
+ * tok_lp f32 [B*K, Lp] its token log-probs.  A hypothesis equal to one of a lower k is dropped.  Over the kept ones: l = sum_{t <= n} tok_lp[h, t]
+ * (position order, fp32 without contraction), P = softmax(l), loss f32 [B] = sum_k P_k (W_k - mean W) and coeff f32 [B*K] =
+ * P_k (W_k - sum_j P_j W_j) * scale (* *scale_dev when scale_dev is not NULL); coeff is 0 for a dropped hypothesis. */
+int otb_mwer_coeff(const int32_t* len, const int32_t* err, const float* tok_lp, int Lp, const int32_t* tgt, int B, int K, float scale,
+                   const float* scale_dev, float* coeff, float* loss, void* stream);
+/* dlogits bf16 [rows, ld] = coeff[r / Lp] * (onehot(target[r]) - softmax(logits[r, :V])) of logits f32 [rows, ld], with
+ * tok_lp f32 [rows] = otb_token_logprob of the same logits and targets (its log-sum-exp is reused); columns >= V, rows with
+ * target < 0 or >= V and rows with coeff 0 are zero.  ld % 4 == 0 and 16-byte aligned logits. */
+int otb_mwer_grad(const float* logits, int ld, int rows, int V, const int32_t* target, const float* tok_lp, const float* coeff, int Lp,
+                  void* dlogits, void* stream);
+
 /* Conv2d front end backward (frontend/conv.py:50-76 under autograd).  h1 = conv1 activation buffer (layout of
  * otb_conv1_relu).  col bf16 [B*T2*F2, 9*C1] = im2col of h1 for conv2 (k = (kh*3+kw)*C1 + c): conv2's weight gradient is
  * otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu folds dcol

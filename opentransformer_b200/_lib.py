@@ -103,6 +103,9 @@ _SIGS = {
     'otb_ctc_prefix_advance': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     'otb_token_logprob': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P]),
     'otb_nbest_rescore': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_float, c_int, c_int, c_int64, _P, _P, _P, _P]),
+    'otb_edit_distance': (c_int, [_P, c_int, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P, _P]),
+    'otb_mwer_coeff': (c_int, [_P, _P, _P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P]),
+    'otb_mwer_grad': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
     'otb_conv_im2col': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv_col2im_relu': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv1_wgrad': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),

@@ -547,6 +547,24 @@ int otb_nbest_rescore(const int32_t* tgt, int Lp, const int32_t* len, const floa
                                                   reinterpret_cast<long long*>(ids), out_len, out_score));
 }
 
+int otb_edit_distance(const int32_t* hyp, int ldh, const int32_t* hyp_len, const int32_t* ref, int ldr, const int32_t* ref_len, int N,
+                      int K, int max_hyp, int max_ref, int32_t* out, void* stream) {
+    if (N > 0 && (!hyp || !hyp_len || !ref || !ref_len || !out)) return fail("otb_edit_distance", "null operand");
+    RET("otb_edit_distance", edit_distance_launch(ST(stream), hyp, ldh, hyp_len, ref, ldr, ref_len, N, K, max_hyp, max_ref, out));
+}
+
+int otb_mwer_coeff(const int32_t* len, const int32_t* err, const float* tok_lp, int Lp, const int32_t* tgt, int B, int K, float scale,
+                   const float* scale_dev, float* coeff, float* loss, void* stream) {
+    if (!len || !err || !tok_lp || !tgt || !coeff || !loss) return fail("otb_mwer_coeff", "null operand");
+    RET("otb_mwer_coeff", mwer_coeff_launch(ST(stream), len, err, tok_lp, Lp, tgt, B, K, scale, scale_dev, coeff, loss));
+}
+
+int otb_mwer_grad(const float* logits, int ld, int rows, int V, const int32_t* target, const float* tok_lp, const float* coeff, int Lp,
+                  void* dlogits, void* stream) {
+    if (rows > 0 && (!logits || !target || !tok_lp || !coeff || !dlogits)) return fail("otb_mwer_grad", "null operand");
+    RET("otb_mwer_grad", mwer_grad_launch(ST(stream), logits, ld, rows, V, target, tok_lp, coeff, Lp, reinterpret_cast<bf16*>(dlogits)));
+}
+
 int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
     int T1, F1, T2, F2;
     if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;

@@ -222,6 +222,13 @@ const char* nbest_rescore_launch(cudaStream_t stream, const int* tgt, int Lp, co
                                  int M, int B, int K, float weight, int nbest, int Lout, long long pad_id, long long* ids,
                                  int* out_len, float* out_score);
 
+const char* edit_distance_launch(cudaStream_t stream, const int* hyp, int ldh, const int* hyp_len, const int* ref, int ldr,
+                                 const int* ref_len, int N, int K, int max_h, int max_r, int* out);
+const char* mwer_coeff_launch(cudaStream_t stream, const int* len, const int* err, const float* tok_lp, int Lp, const int* tgt, int B,
+                              int K, float scale, const float* scale_dev, float* coeff, float* loss);
+const char* mwer_grad_launch(cudaStream_t stream, const float* logits, int ld, int rows, int V, const int* target, const float* tok_lp,
+                             const float* coeff, int Lp, bf16* dlogits);
+
 const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const int* n_samples, int B, const float* window,
                          const float* bank, const int* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift,
                          float preemph);

@@ -868,6 +868,76 @@ def nbest_rescore(tgt, lengths, s1, tok_lp, weight, nbest, width, pad_id):
     return ids, out_len, scores
 
 
+EDIT_DISTANCE_MAX_TOKENS = 1023
+
+
+def edit_distance(hyp, hyp_len, ref, ref_len, K=1):
+    """Levenshtein distances (unit costs) of hypothesis rows against reference rows (otb_edit_distance): hyp int [N, Lh] of
+    which the first hyp_len[i] (i32 [N]) count, ref int [ceil(N / K), Lr] with ref_len i32 [ceil(N / K)]; hypothesis i is
+    compared with reference i // K.  Lh, Lr <= 1023.  -> i32 [N], exact."""
+    if hyp.dim() != 2 or ref.dim() != 2:
+        raise ValueError(f'edit_distance: hyp and ref must be 2-D, got {tuple(hyp.shape)} and {tuple(ref.shape)}')
+    N, Lh = hyp.shape
+    Lr = ref.shape[1]
+    if max(Lh, Lr) > EDIT_DISTANCE_MAX_TOKENS:
+        raise ValueError(f'edit_distance: sequences of up to {EDIT_DISTANCE_MAX_TOKENS} tokens are supported, got rows of {Lh} '
+                         f'and {Lr}')
+    if K < 1 or ref.shape[0] != -(-N // K) or hyp_len.shape != (N,) or ref_len.shape != (ref.shape[0],):
+        raise ValueError(f'edit_distance: need K >= 1, ref [ceil(N / K)] rows and lengths [N] / [ceil(N / K)], got K {K}, hyp '
+                         f'{tuple(hyp.shape)}, ref {tuple(ref.shape)}, lengths {tuple(hyp_len.shape)}, {tuple(ref_len.shape)}')
+    hyp = hyp.to(torch.int32).contiguous()
+    ref = ref.to(torch.int32).contiguous()
+    for t, n in ((hyp, 'hyp'), (ref, 'ref'), (hyp_len, 'hyp_len'), (ref_len, 'ref_len')):
+        _need(t, torch.int32, n)
+    out = torch.empty(N, dtype=torch.int32, device=hyp.device)
+    check(_lib.lib().otb_edit_distance(_p(hyp), max(Lh, 1), _p(hyp_len), _p(ref), max(Lr, 1), _p(ref_len), N, K, Lh, Lr, _p(out),
+                                       _stream()), 'otb_edit_distance')
+    _count()
+    return out
+
+
+def mwer_coeff(tgt, lengths, err, tok_lp, grad_scale=1.0, scale_dev=None):
+    """The expected-risk term of each utterance's K hypotheses (otb_mwer_coeff, DESIGN.md 4.11).  tgt i32 [B, K, Lp] the scored
+    tokens y <S/E> (-1 after), lengths i32 [B, K] the length of y, err i32 [B, K] the edit distances, tok_lp f32 [B, K, Lp].
+    -> (loss f32 [B] = sum_k P_k (W_k - mean W) over the kept hypotheses, coeff f32 [B, K] = dloss/dl_k * grad_scale (times
+    the f32 device scalar scale_dev when given); 0 for a duplicate of a better-ranked hypothesis)."""
+    B, K, Lp = tgt.shape
+    if lengths.shape != (B, K) or err.shape != (B, K) or tok_lp.shape != (B, K, Lp):
+        raise ValueError(f'mwer_coeff: need lengths / err [B, K] = [{B}, {K}] and tok_lp [{B}, {K}, {Lp}], got '
+                         f'{tuple(lengths.shape)}, {tuple(err.shape)}, {tuple(tok_lp.shape)}')
+    _need(tgt, torch.int32, 'tgt'); _need(lengths, torch.int32, 'lengths'); _need(err, torch.int32, 'err')
+    _need(tok_lp, torch.float32, 'tok_lp')
+    if scale_dev is not None:
+        _need(scale_dev, torch.float32, 'scale_dev')
+    coeff = torch.empty(B, K, dtype=torch.float32, device=tgt.device)
+    loss = torch.empty(B, dtype=torch.float32, device=tgt.device)
+    check(_lib.lib().otb_mwer_coeff(_p(lengths), _p(err), _p(tok_lp), Lp, _p(tgt), B, K, float(grad_scale), _p(scale_dev), _p(coeff),
+                                    _p(loss), _stream()), 'otb_mwer_coeff')
+    _count()
+    return loss, coeff
+
+
+def mwer_grad(logits, V, target, tok_lp, coeff):
+    """bf16 dlogits [rows, ld] = coeff[r // Lp] * (onehot(target[r]) - softmax(logits[r, :V])) (otb_mwer_grad): logits f32
+    [rows, ld] (ld % 4 == 0), target i32 [rows] (-1: a zero row), tok_lp f32 [rows] = token_logprob(logits, V, target),
+    coeff f32 [rows // Lp] (the hypotheses of Lp rows each); padding columns are zero."""
+    if not logits.is_cuda:
+        raise RuntimeError('logits must be a CUDA tensor: the CUDA hot path has no CPU fallback')
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
+        raise TypeError('mwer_grad: logits must be a 2-D f32 tensor with unit column stride')
+    rows, ld = logits.shape[0], logits.stride(0)
+    coeff = coeff.reshape(-1)
+    if target.shape != (rows,) or tok_lp.shape != (rows,) or coeff.numel() < 1 or rows % coeff.numel():
+        raise ValueError(f'mwer_grad: need target / tok_lp [rows = {rows}] and coeff dividing the rows, got {tuple(target.shape)}, '
+                         f'{tuple(tok_lp.shape)}, {tuple(coeff.shape)}')
+    _need(target, torch.int32, 'target'); _need(tok_lp, torch.float32, 'tok_lp'); _need(coeff, torch.float32, 'coeff')
+    out = torch.empty(rows, ld, dtype=BF16, device=logits.device)
+    check(_lib.lib().otb_mwer_grad(_p(logits), ld, rows, V, _p(target), _p(tok_lp), _p(coeff), rows // coeff.numel(), _p(out),
+                                   _stream()), 'otb_mwer_grad')
+    _count()
+    return out
+
+
 def conv_im2col(h1, B, T, F, C1):
     _, _, T2, F2 = conv_geometry(T, F)
     col = torch.empty(B * T2 * F2, 9 * C1, dtype=BF16, device=h1.device)

@@ -121,6 +121,24 @@ def second_pass_rows(ids, lengths=None):
     return inputs.view(B * K, Lp), targets, n.int(), Lp
 
 
+def error_counts(ids, lengths, truth, truth_length):
+    """eval.py's token error counts of one batch, on the device and without a host synchronisation: ids [B, K, W] a
+    recognizer's n-best as recognize_ids returns it, each row cut at its first <S/E> (and at lengths i32 [B, K] when given:
+    the CTC recognizers' rows), scored by otb_edit_distance against truth[b, 1 : truth_length[b]] (truth i64 [B, L + 1],
+    truth_length [B] label counts incl. <S/E>).  -> i64 0-d tensors (errors of the 1-best, sum over utterances of the
+    fewest errors in the n-best, reference tokens): eval.py's false_tokens, top_n_false_tokens and total_tokens.  Both
+    sides of the comparison are at most 1023 tokens long.  Word merging (-p2w) is not applied."""
+    B, K, W = ids.shape
+    dev = ids.device
+    ext = torch.cat((ids.long(), torch.full((B, K, 1), EOS, dtype=torch.int64, device=dev)), dim=2)
+    if lengths is not None:
+        ext = torch.where(torch.arange(W + 1, device=dev) >= lengths[..., None], EOS, ext)
+    n = (ext == EOS).int().argmax(dim=2).to(torch.int32)                         # the first <S/E>, as second_pass_rows cuts
+    ref_len = (truth_length.to(dev).to(torch.int32) - 1).contiguous()
+    err = ops.edit_distance(ids.reshape(B * K, W), n.view(-1), truth[:, 1:].to(dev), ref_len, K).view(B, K).long()
+    return err[:, 0].sum(), err.min(dim=1).values.sum(), ref_len.long().sum()
+
+
 def rescore_nbest(ids, scores, scorers, weight, nbest, width=None, pad=EOS, lengths=None):
     """N-best rescoring (DESIGN.md 4.10): first-pass ids [B, K, W] (cut as second_pass_rows does) with scores f32 [B, K];
     scorers: functions (inputs i64 [B*K, Lp], targets i32 [B*K, Lp], K, Lp) -> token log-probs f32 [B*K, Lp] of one
@@ -366,7 +384,7 @@ class SpeechToTextRecognizer(Recognizer):
 
     def __init__(self, model, lm=None, lm_weight=0.1, ctc_weight=0.0, beam_width=5, nbest=1, max_len=50,
                  idx2unit=None, penalty=0, lamda=5, ngpu=1, apply_cache=False, use_graph=True, persistent=None,
-                 ctc_candidates=None, apply_rescoring=False, apply_lm_rescoring=False, rescore_weight=1.0):
+                 ctc_candidates=None, apply_rescoring=False, apply_lm_rescoring=False, rescore_weight=1.0, max_decoders=None):
         """ctc_weight w > 0: joint CTC/attention decoding (DESIGN.md 4.9).  Each hypothesis' ctc_candidates best tokens by
         the attention (+ LM) score (default min(16, 2 beam_width), between beam_width and 16) are scored
         (1 - w) logp_att + w (psi(g c) - psi(g)) + lm_weight lm with the CTC prefix score psi of the model's joint-CTC head,
@@ -376,7 +394,10 @@ class SpeechToTextRecognizer(Recognizer):
         s = first-pass score + rescore_weight * (sum of its second-pass log-probs), and the nbest best by s are returned.
         apply_rescoring: the first pass is the CTC prefix beam search (beam_width hypotheses) over the joint-CTC head, the
         second pass the attention decoder; no attention beam search runs.  apply_lm_rescoring: the LM is not fused into the
-        search (the persistent decode kernel stays eligible) but scores all beam_width hypotheses of the first pass."""
+        search (the persistent decode kernel stays eligible) but scores all beam_width hypotheses of the first pass.
+
+        max_decoders: at most this many BeamDecoders (one per batch geometry: batch, encoder frames; each owns its KV caches
+        and search buffers) are kept, least recently used first out; None keeps one per geometry seen."""
         has_head = getattr(model, 'ctc_weight', 0.0) > 0.0
         if apply_rescoring and not has_head:
             raise ValueError('SpeechToTextRecognizer: apply_rescoring needs the joint-CTC head: this model has ctc_weight 0')
@@ -413,6 +434,9 @@ class SpeechToTextRecognizer(Recognizer):
         self.apply_rescoring, self.apply_lm_rescoring = bool(apply_rescoring), bool(apply_lm_rescoring)
         self.rescore_weight = float(rescore_weight)
         self._decoders = {}
+        if max_decoders is not None and max_decoders < 1:
+            raise ValueError(f'SpeechToTextRecognizer: max_decoders must be >= 1 or None, got {max_decoders}')
+        self.max_decoders = max_decoders
 
     # ---- reference-facing seams -------------------------------------------------------------
     def encode(self, inputs, inputs_mask, cache=None):
@@ -462,12 +486,14 @@ class SpeechToTextRecognizer(Recognizer):
         # the CTC weight and candidate count are launch arguments that a captured step bakes in
         ctc = (self.model.assistor, self.ctc_weight, self.ctc_candidates) if self.ctc_weight > 0.0 else None
         key = (B, self.beam_width, T2, self.max_len, device.index, ctc[1:] if ctc else None)
-        bd = self._decoders.get(key)
+        bd = self._decoders.pop(key, None)
         if bd is None:
+            while self.max_decoders is not None and len(self._decoders) >= self.max_decoders:
+                self._decoders.pop(next(iter(self._decoders)))          # the least recently used goes, with its buffers
             fused = self._lm_fused()
             bd = BeamDecoder(self.model.decoder, B, self.beam_width, T2, self.max_len, device,
                              self.use_graph and not fused, persistent=self.persistent and not fused, ctc=ctc)
-            self._decoders[key] = bd
+        self._decoders[key] = bd          # (re-)inserted as the most recently used
         return bd
 
     def _lm_fused(self):

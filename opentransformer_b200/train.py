@@ -274,8 +274,9 @@ def linear_bwd(dy, x, lin, grads, resid=None):
 
 
 # dropout site ids: Transformer encoder layer i -> 2 i + {0, 1}; Conformer block i -> 3 i + {0, 1, 2} (macaron feed-forward,
-# attention, convolution module); decoder layer i -> 1000 + 3 i + {0, 1, 2}
-ENC_SITE, DEC_SITE = 0, 1000
+# attention, convolution module); decoder layer i -> 1000 + 3 i + {0, 1, 2}; the same decoder layer in the MWER branch,
+# over the n-best (forward_backward's nbest) -> 4000 + 3 i + {0, 1, 2}, clear of the language models' 2000 + / 3000 + (lm.py)
+ENC_SITE, DEC_SITE, MWER_SITE = 0, 1000, 4000
 
 
 def _enc_sites(enc):
@@ -358,17 +359,20 @@ def enc_layer_bwd(p, t, dout, pre, g, B, H, T, lengths, drop, causal=False):
     return _ln_bwd(du1, t.a, p['ln1'], g) if pre else du1
 
 
-def _dec_layer_fwd(p, a, mem, pre, B, H, L, T, lengths, drop):
-    """One decoder layer in training mode (decoder/transformer.py:54-90) over the memory mem -> (output, _DecTape)."""
+def _dec_layer_fwd(p, a, mem, pre, B, H, L, T, lengths, drop, K=1):
+    """One decoder layer in training mode (decoder/transformer.py:54-90) over the memory mem -> (output, _DecTape).
+    a holds K sequences of L rows per utterance: self-attention is causal within each of the B*K sequences, and
+    cross-attention treats the K*L query rows of utterance b as one problem against its memory (score_bf16's layout), so
+    the memory's K|V is projected once per utterance."""
     d = a.shape[1]
     u1 = _norm(a, p['ln1']) if pre else a
     qkv = ops.linear(u1, p['qkv'].w, p['qkv'].b)
-    ctx, lse = ops.attention_train(qkv, qkv, qkv, B, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d)
+    ctx, lse = ops.attention_train(qkv, qkv, qkv, B * K, H, L, L, causal=True, q_col0=0, k_col0=d, v_col0=2 * d)
     z1 = _resid(ctx, p['o'], u1, drop, 0)
     u2 = _norm(z1, p['ln2'] if pre else p['ln1'])
     q = ops.linear(u2, p['q'].w, p['q'].b)
     kv = ops.linear(mem, p['kv'].w, p['kv'].b)
-    ctx2, lse2 = ops.attention_train(q, kv, kv, B, H, L, T, kv_len=lengths, k_col0=0, v_col0=d)
+    ctx2, lse2 = ops.attention_train(q, kv, kv, B, H, K * L, T, kv_len=lengths, k_col0=0, v_col0=d)
     z2 = _resid(ctx2, p['o2'], u2, drop, 1)
     u3 = _norm(z2, p['ln3'] if pre else p['ln2'])
     ffn_u, h = _ffn_fwd(p, u3)
@@ -378,9 +382,9 @@ def _dec_layer_fwd(p, a, mem, pre, B, H, L, T, lengths, drop):
                          u3=u3, ffn_u=ffn_u, h=h, z3=z3)
 
 
-def _dec_layer_bwd(p, t, dout, dmem, mem, pre, g, B, H, L, T, lengths, drop):
+def _dec_layer_bwd(p, t, dout, dmem, mem, pre, g, B, H, L, T, lengths, drop, K=1):
     """Backward of _dec_layer_fwd: parameter gradients into g; returns the gradient of the layer input and dmem plus
-    this layer's gradient of the memory (added by the K|V dgrad GEMM's residual epilogue)."""
+    this layer's gradient of the memory (added by the K|V dgrad GEMM's residual epilogue), summed over the K sequences."""
     d = t.a.shape[1]
     dz3 = dout if pre else _ln_bwd(dout, t.z3, p['ln3'], g)
     dh = linear_bwd(_drop_bwd(dz3, drop, 2), t.h, p['w2'], g)
@@ -389,14 +393,14 @@ def _dec_layer_bwd(p, t, dout, dmem, mem, pre, g, B, H, L, T, lengths, drop):
     dctx2 = linear_bwd(_drop_bwd(dz2, drop, 1), t.ctx2, p['o2'], g)
     dq = torch.empty_like(t.q)
     dkv = torch.empty_like(t.kv)
-    ops.attention_bwd(t.q, t.kv, t.kv, t.ctx2, dctx2, t.lse2, B, H, L, T, dq, dkv, dkv, kv_len=lengths, k_col0=0, v_col0=d,
+    ops.attention_bwd(t.q, t.kv, t.kv, t.ctx2, dctx2, t.lse2, B, H, K * L, T, dq, dkv, dkv, kv_len=lengths, k_col0=0, v_col0=d,
                       dq_col0=0, dk_col0=0, dv_col0=d)
     dmem = linear_bwd(dkv, mem, p['kv'], g, resid=dmem)
     du2 = linear_bwd(dq, t.u2, p['q'], g, resid=dz2)
     dz1 = _ln_bwd(du2, t.z1, p['ln2'] if pre else p['ln1'], g)
     dctx = linear_bwd(_drop_bwd(dz1, drop, 0), t.ctx, p['o'], g)
     dqkv = torch.empty_like(t.qkv)
-    ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B, H, L, L, dqkv, dqkv, dqkv, causal=True, q_col0=0, k_col0=d,
+    ops.attention_bwd(t.qkv, t.qkv, t.qkv, t.ctx, dctx, t.lse, B * K, H, L, L, dqkv, dqkv, dqkv, causal=True, q_col0=0, k_col0=d,
                       v_col0=2 * d, dq_col0=0, dk_col0=d, dv_col0=2 * d)
     du1 = linear_bwd(dqkv, t.u1, p['qkv'], g, resid=dz1)
     return (_ln_bwd(du1, t.a, p['ln1'], g) if pre else du1), dmem
@@ -635,72 +639,142 @@ def _loss_scale(grad_scale, w):
     return w * grad_scale, None
 
 
+def _dec_fwd(dec, pk, tgt_in, mem, B, K, L, T2, lengths, drops):
+    """The decoder in training mode, teacher-forced on tgt_in i64 [B*K, L] (K sequences per utterance) over the memory ->
+    (the output layer's input bf16 [B*K*L, d], the last layer's output, the layers' tapes)."""
+    _, dtable = dec.pos_emb.scale_and_table(L, mem.device)
+    y = ops.embed_posenc(tgt_in, pk.emb, dtable, B * K * L, dec.d_model, period=L)
+    tape = []
+    for p, drop in zip(pk.dec, drops):
+        y, t = _dec_layer_fwd(p, y, mem, pk.dec_pre, B, dec.n_heads, L, T2, lengths, drop, K)
+        tape.append(t)
+    last = y
+    if pk.dec_pre:
+        y = _norm(y, pk.dec_norm)
+    return y, last, tape
+
+
+def _dec_bwd(dec, pk, tgt_in, dlogits, y, last, tape, mem, dmem, g, B, K, L, T2, lengths, drops):
+    """Backward of _dec_fwd and the output layer from dlogits: parameter gradients into g; returns dmem plus the decoder's
+    gradient of the memory."""
+    dy = head_bwd(dlogits, y, pk.wout, g, pk.wout_name, 'decoder.output_layer.bias')
+    if pk.dec_pre:
+        dy = _ln_bwd(dy, last, pk.dec_norm, g)
+    for i in reversed(range(len(pk.dec))):
+        dy, dmem = _dec_layer_bwd(pk.dec[i], tape[i], dy, dmem, mem, pk.dec_pre, g, B, dec.n_heads, L, T2, lengths, drops[i], K)
+    embedding_bwd(tgt_in, dy, pk.emb, math.sqrt(dec.d_model), g, 'decoder.embedding.weight')       # decoder/transformer.py:163,169
+    return dmem
+
+
+def _mwer_references(truth, truth_length):
+    """The sequences the n-best is scored against, as eval.py compares them: truth[b, 1 : truth_length[b]] (the transcript
+    between BOS and its closing <S/E>; without truth_length, up to the first <S/E>) -> (i32 [B, L], lengths i32 [B])."""
+    ref = truth[:, 1:].to(torch.int32).contiguous()
+    if truth_length is not None:
+        return ref, (truth_length.to(ref.device).to(torch.int32) - 1).contiguous()
+    return ref, (ref == 1).int().argmax(dim=1).to(torch.int32)
+
+
+def _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad_scale, g, dmem):
+    """The MWER term (DESIGN.md 4.11) on the n-best (hypothesis inputs i64 [B*K, Lp] = BOS y PAD..., targets [B*K, Lp] =
+    y <S/E> -1..., K), over the memory of the cross-entropy branch: the decoder teacher-forced on the K hypotheses of each
+    utterance, their token log-probs, the edit distances to the references, and with g the backward of
+    sum_b L_MWER,b / B (x grad_scale) on top of dmem.  -> (mean_b L_MWER,b, dmem)."""
+    hyp_in, hyp_tgt, K = nbest
+    dec, B, T2, lengths = model.decoder, tr.B, tr.T2, tr.lengths
+    Lp = hyp_in.shape[1]
+    if tuple(hyp_in.shape) != (B * K, Lp) or tuple(hyp_tgt.shape) != (B * K, Lp):
+        raise ValueError(f'forward_backward: the n-best rows must be [B*K, Lp] = [{B * K}, Lp], got {tuple(hyp_in.shape)} and '
+                         f'{tuple(hyp_tgt.shape)}')
+    tgt = hyp_tgt.to(torch.int32).contiguous()
+    n = ((tgt >= 0).sum(dim=1) - 1).to(torch.int32)                              # the length of y
+    ref, ref_len = _mwer_references(truth, truth_length)
+    err = ops.edit_distance(tgt, n, ref, ref_len, K)
+    drops = [(r, drop_seed, MWER_SITE + 3 * i) for i, r in enumerate(pk.rates['decoder'])]
+    hyp_in = hyp_in.contiguous()
+    y, last, tape = _dec_fwd(dec, pk, hyp_in, mem, B, K, Lp, T2, lengths, drops)
+    logits = head_fwd(y, pk.wout, pk.bout, dec.ld_logits)
+    flat = tgt.view(-1)
+    tok = ops.token_logprob(logits, dec.vocab_size, flat)
+    ms, mdev = _loss_scale(grad_scale, 1.0 / B)
+    loss_b, coeff = ops.mwer_coeff(tgt.view(B, K, Lp), n.view(B, K), err.view(B, K), tok.view(B, K, Lp), ms, mdev)
+    if g is not None:
+        dlogits = ops.mwer_grad(logits, dec.vocab_size, flat, tok, coeff)
+        del logits
+        dmem = _dec_bwd(dec, pk, hyp_in, dlogits, y, last, tape, mem, dmem, g, B, K, Lp, T2, lengths, drops)
+    return loss_b.mean(), dmem
+
+
 def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=True, grad_sink=None, grad_scale=1.0,
-                     bf16_of=None, drop_seed=None):
+                     bf16_of=None, drop_seed=None, nbest=None, mwer_ce_weight=0.01):
     """SpeechToText.train_pass (the contract is at the top of this file).  inputs f32 [B,T,F], mask bool [B,T], truth i64
     [B,L+1] (BOS ... EOS PAD*); the gradients are named as in model.named_parameters().  truth_length: i32/i64 [B] label
     counts incl. <S/E> (targets['targets_length'], data/loader.py:94) -- required when model.ctc_weight > 0: the loss is
     then (1 - w) * attention + w * CTC (model/speech2text.py:60-62), the CTC head's gradients flow into the encoder through
     the memory, and the CTC term alone is left on model._last_ctc_loss (None without joint CTC) for SpeechToText.forward
-    to report, as the reference does."""
-    enc, dec = model.encoder, model.decoder
+    to report, as the reference does.
+
+    nbest = (hypothesis inputs i64 [B*K, Lp], their targets [B*K, Lp], K), second_pass_rows' layout: minimum word error
+    rate training (DESIGN.md 4.11).  The loss becomes mean_b L_MWER,b + mwer_ce_weight * (the loss above); the decoder
+    also runs on the K hypotheses of each utterance over the same memory, with its own dropout sites (MWER_SITE), and both
+    branches' memory gradients go into the one encoder backward."""
+    dec = model.decoder
     ctc_w = float(getattr(model, 'ctc_weight', 0.0) or 0.0)
     if ctc_w > 0.0 and truth_length is None:
         raise ValueError('forward_backward: ctc_weight > 0 needs truth_length')
     pk = TrainPack(model, bf16_of)
     dev = inputs.device
     need_drop_seed(drop_seed, pk.rates['encoder'] + pk.rates['decoder'])
+    ce_w = 1.0
+    if nbest is not None:
+        ce_w = float(mwer_ce_weight)
+        if want_grads and grad_sink is None:        # two decoder passes add their gradients into the same tensors
+            unused = unused_parameters(model)
+            grad_sink = {n: torch.zeros(p.shape, dtype=torch.float32, device=dev) for n, p in model.named_parameters()
+                         if n not in unused}
 
     # ------------------------------------------------------------------ forward
     mem, tr = _encoder_fwd(model, pk, inputs, mask, drop_seed)
-    B, T2, lengths, d = tr.B, tr.T2, tr.lengths, enc.d_model
+    B, T2, lengths = tr.B, tr.T2, tr.lengths
 
     tgt_in = truth[:, :-1].contiguous()
     tgt_out = truth[:, 1:].contiguous()
     L = tgt_in.shape[1]
-    Hd = dec.n_heads
-    _, dtable = dec.pos_emb.scale_and_table(L, dev)
-    y = ops.embed_posenc(tgt_in, pk.emb, dtable, B * L, d, period=L)
     d_drop = [(r, drop_seed, DEC_SITE + 3 * i) for i, r in enumerate(pk.rates['decoder'])]
-    dec_tape = []
-    for p, drop in zip(pk.dec, d_drop):
-        y, t = _dec_layer_fwd(p, y, mem, pk.dec_pre, B, Hd, L, T2, lengths, drop)
-        dec_tape.append(t)
+    y, dec_last, dec_tape = _dec_fwd(dec, pk, tgt_in, mem, B, 1, L, T2, lengths, d_drop)
     V = dec.vocab_size
-    dec_last = y
-    if pk.dec_pre:
-        y = _norm(y, pk.dec_norm)
     logits = head_fwd(y, pk.wout, pk.bout, dec.ld_logits)
     loss_ctc, dctc = None, None
     if ctc_w > 0.0:     # CTCAssistor on the encoder states (model/ctc.py:33-52)
         wc, bc, ldc = _ctc_head(model, pk)
-        cs, cdev = _loss_scale(grad_scale, ctc_w)
+        cs, cdev = _loss_scale(grad_scale, ctc_w * ce_w)
         loss_ctc, _, dctc = ops.ctc_loss(head_fwd(mem, wc, bc, ldc), B, T2, V, lengths, tgt_out,
                                          truth_length.to(torch.int32).to(dev).contiguous(),
                                          model.assistor.blank, want_grad=want_grads, grad_scale=cs, scale_dev=cdev)
     model._last_ctc_loss = loss_ctc
+    g, dmem = None, None
     if not want_grads:
         loss, _ = ops.ls_cross_entropy(logits, tgt_out, V, model.smoothing)
         if ctc_w > 0.0:
             loss = (1.0 - ctc_w) * loss + ctc_w * loss_ctc
-        return loss, None
-    loss, dlogits = ops.ls_cross_entropy_train(logits, tgt_out, V, model.smoothing)
-    att_scale, att_dev = _loss_scale(grad_scale, 1.0 - ctc_w)
-    if att_dev is not None or att_scale != 1.0:
-        # loss / accum_steps (trainer.py:216), x (1 - w)
-        dlogits = ops.scale_add_table(dlogits, att_scale, scale_dev=att_dev)
-    if ctc_w > 0.0:
-        loss = (1.0 - ctc_w) * loss + ctc_w * loss_ctc
+    else:
+        loss, dlogits = ops.ls_cross_entropy_train(logits, tgt_out, V, model.smoothing)
+        att_scale, att_dev = _loss_scale(grad_scale, (1.0 - ctc_w) * ce_w)
+        if att_dev is not None or att_scale != 1.0:
+            # loss / accum_steps (trainer.py:216), x (1 - w)
+            dlogits = ops.scale_add_table(dlogits, att_scale, scale_dev=att_dev)
+        if ctc_w > 0.0:
+            loss = (1.0 - ctc_w) * loss + ctc_w * loss_ctc
 
-    # ------------------------------------------------------------------ backward
-    g = Grads(grad_sink)
-    dy = head_bwd(dlogits, y, pk.wout, g, pk.wout_name, 'decoder.output_layer.bias')
-    dmem = None
-    if pk.dec_pre:
-        dy = _ln_bwd(dy, dec_last, pk.dec_norm, g)
-    for i in reversed(range(len(pk.dec))):
-        dy, dmem = _dec_layer_bwd(pk.dec[i], dec_tape[i], dy, dmem, mem, pk.dec_pre, g, B, Hd, L, T2, lengths, d_drop[i])
-    embedding_bwd(tgt_in, dy, pk.emb, math.sqrt(d), g, 'decoder.embedding.weight')       # decoder/transformer.py:163,169
+        # -------------------------------------------------------------- backward
+        g = Grads(grad_sink)
+        dmem = _dec_bwd(dec, pk, tgt_in, dlogits, y, dec_last, dec_tape, mem, dmem, g, B, 1, L, T2, lengths, d_drop)
+    if nbest is not None:
+        del logits, dec_tape
+        loss_mwer, dmem = _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad_scale, g, dmem)
+        loss = loss_mwer + ce_w * loss
+    if not want_grads:
+        return loss, None
 
     dx = dmem
     if ctc_w > 0.0:     # CTC head: parameter gradients, and its gradient with respect to the memory joins the decoder's
@@ -797,6 +871,20 @@ def loss_train_mode(model, *batch):
         return model.train_pass(*batch, want_grads=False, drop_seed=next_drop_seed(model, batch[0].device))[0]
 
 
+def _check_mwer(model, nbest, ce_weight, max_len, mixspeech):
+    """What FusedTrainer refuses for minimum word error rate training, before any device work."""
+    if not isinstance(getattr(model, 'decoder', None), TransformerDecoder):
+        raise NotImplementedError(f'MWER training scores an attention decoder\'s n-best; {type(model).__name__} has none')
+    if not 2 <= nbest <= 16:
+        raise ValueError(f'mwer_nbest must be 0 (off) or in 2..16, got {nbest}')
+    if not ce_weight >= 0.0:
+        raise ValueError(f'mwer_ce_weight must be >= 0, got {ce_weight}')
+    if not 1 <= max_len <= 1022:
+        raise ValueError(f'mwer_max_len must be in 1..1022, got {max_len}')
+    if mixspeech:
+        raise NotImplementedError('MWER training and MixSpeech are two different pairs of passes; choose one')
+
+
 def transformer_lr(step, model_size, warmup_steps, factor=1.0):
     """TransformerScheduler.get_step_lr (otrans/train/scheduler.py:137-138)."""
     return factor * model_size ** (-0.5) * min(step ** (-0.5), step * warmup_steps ** (-1.5))
@@ -815,15 +903,21 @@ class FusedTrainer:
     grad_noise = sigma > 0 (train: grad_noise, trainer.py:223-227): sigma / accum_steps * N(0, 1) is added to every trained
     gradient element after the clip and before Adam, inside the fused Adam launch.  The reference's loop adds it to every
     parameter with requires_grad and raises TypeError on a Conformer, whose post_ffn parameters have no gradient; this
-    trainer leaves them out (unused_parameters) and adds noise to what it trains."""
+    trainer leaves them out (unused_parameters) and adds noise to what it trains.
+    mwer_nbest = K in 2..16: minimum word error rate training (DESIGN.md 4.11).  Every micro-step first decodes the
+    micro-batch's K-best with the current weights (beam_width = nbest = K, penalty 0, max_len = mwer_max_len) on the
+    inference path, in eval mode and outside any CUDA graph, then trains on mean_b L_MWER,b + mwer_ce_weight * (the
+    model's loss).  Attention-decoder models only (NotImplementedError otherwise); not with mixspeech."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6, clip_grad=5.0, model_size=256,
                  warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True, mixspeech=False,
-                 grad_noise=0.0):
+                 grad_noise=0.0, mwer_nbest=0, mwer_ce_weight=0.01, mwer_max_len=60):
         if mixspeech and not hasattr(model, 'mix_batch'):
             raise NotImplementedError(f'MixSpeech mixes [B, T, F] speech features; {type(model).__name__} takes token inputs')
         if not grad_noise >= 0.0:
             raise ValueError(f'grad_noise must be >= 0, got {grad_noise}')
+        if mwer_nbest:
+            _check_mwer(model, mwer_nbest, mwer_ce_weight, mwer_max_len, mixspeech)
         model.check_fused_trainer()
         self.model = model
         # parameters the forward never reads (a Conformer's post_ffn) stay out of the flat buffers: no gradient, no weight decay
@@ -890,6 +984,17 @@ class FusedTrainer:
             self.noise_seed = torch.randint(0, 2 ** 31 - 1, (1,), dtype=torch.int32).to(dev)
             self.noise_mask = ops.noise_bitmask(total, [self.offsets[n] for n, _ in self.params]).to(dev)
         broadcast_from_first_([t for t in (self.mix_seed, self.noise_seed) if t is not None], process_group)
+        self.mwer_nbest, self.mwer_ce_weight = int(mwer_nbest), float(mwer_ce_weight)
+        self._recognizer = None
+        if self.mwer_nbest:
+            from .recognize import SpeechToTextRecognizer
+            training = model.training
+            # one cached BeamDecoder: ragged batches bring a new frame count almost every step, and a decoder kept for an
+            # older one would hold its KV caches and the bf16 weights of the step it last decoded; the weights move every
+            # optimizer step, so a kept decoder would only save its buffer allocation
+            self._recognizer = SpeechToTextRecognizer(model, beam_width=self.mwer_nbest, nbest=self.mwer_nbest,
+                                                      max_len=mwer_max_len, penalty=0, ngpu=0, max_decoders=1)
+            model.train(training)
 
     @property
     def opt_steps(self):
@@ -924,9 +1029,26 @@ class FusedTrainer:
         if self.mixspeech:
             return self._micro_mix(batch)
         self.drop_seed.add_(1)
+        kw = {}
+        if self.mwer_nbest:         # the n-best rows ride at the end of the batch (_with_nbest)
+            batch, kw = batch[:-2], {'nbest': batch[-2:] + (self.mwer_nbest,), 'mwer_ce_weight': self.mwer_ce_weight}
         loss, _ = self.model.train_pass(*batch, grad_sink=self.sink, grad_scale=1.0 / self.accum_steps, bf16_of=self._bf16_of,
-                                        drop_seed=self.drop_seed)
+                                        drop_seed=self.drop_seed, **kw)
         return loss
+
+    def _with_nbest(self, batch):
+        """MWER: the micro-batch's K-best decoded with the current weights on the inference path (eval mode, so no
+        dropout and a Conformer's BatchNorm on its running statistics), appended to the batch as second_pass_rows' rows
+        (hypothesis inputs i64 [B*K, Lp], targets i32 [B*K, Lp]).  Reading Lp is a host synchronisation; as part of the
+        batch the rows make Lp and K part of the CUDA-graph key."""
+        from .recognize import second_pass_rows
+        self.model.eval()
+        try:
+            ids, _, _ = self._recognizer.recognize_ids(batch[0], batch[1])
+        finally:
+            self.model.train()
+        hyp_in, tgt, _, Lp = second_pass_rows(ids)
+        return batch + (hyp_in, tgt.view(-1, Lp))
 
     def _micro_mix(self, batch):
         """MixSpeech micro-step: the mix, then two passes over it (not one merged 2P-row pass: the reference's two forwards
@@ -1093,6 +1215,8 @@ class FusedTrainer:
             # data parallel: BatchNorm running statistics follow the first rank's (DistributedDataParallel's
             # broadcast_buffers): each rank's forward updates them from its own shard, so they would drift apart
             broadcast_from_first_(self.bn_buffers, self.group)
+            if self.mwer_nbest:
+                batch = self._with_nbest(batch)
             ent = self._graph_for(batch) if self.use_graph else None
             if ent is not None:
                 graph, static, loss, launches = ent
