@@ -118,6 +118,14 @@ int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, in
                   int k_col0, int v_col0, const float* bd, int ldbd, const void* resid, int ldr, float* lse, int d_k,
                   void* stream);
 
+/* Attention weights of otb_attention (module/attention.py:34-36): out f32 [B, H, Tq, Tk], contiguous and caller-allocated,
+ * = softmax(Q K^T / sqrt(d_k) (+ bd) + mask) over the same q / k operands, column offsets, kv_len, causal flag and band
+ * (Tq == Tk, not causal).  Masked entries are exactly 0; every entry of a batch entry with kv_len 0 is NaN.  q_col0,
+ * k_col0, ldq and ldk must be multiples of 8; d_k 64 or 96.  No allocation and no host synchronisation. */
+int otb_attention_probs(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, float* out, int B, int H,
+                        int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, const float* bd, int ldbd,
+                        int d_k, void* stream);
+
 /* ConformerConvolutionModule middle (module/conformer.py:48-52): depthwise Conv1d(k, pad (k-1)/2) over time +
  * eval-mode BatchNorm1d + swish.  x, out bf16 [B*T, d]; w f32 [k, d] and b f32 [d] carry the BatchNorm affine
  * folded in by the caller (w' = w * gamma/sqrt(var+eps), b' = (b - mean) * gamma/sqrt(var+eps) + beta). */

@@ -54,6 +54,8 @@ _SIGS = {
     'otb_dropout_bwd': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_float, _P, ctypes.c_uint32, _P]),
     'otb_attention': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int,
                               _P, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P]),
+    'otb_attention_probs': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int,
+                                    _P, c_int, c_int, _P]),
     'otb_dwconv_swish': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_layernorm': (c_int, [_P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_float, c_int, c_int, _P]),
     'otb_scale_add_table': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, c_int, c_int, c_int, _P, _P]),

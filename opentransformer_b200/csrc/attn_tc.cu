@@ -5,8 +5,8 @@
 //
 // Replaces BasedAttention.compute_context + the QK^T matmul:
 //   otrans/module/attention.py:80 (scores), :34 (masked_fill -inf), :36 (softmax), :37 (weights @ V),
-//   :41 (merge heads).  The reference also returns the [B,h,T1,T2] weights; no caller reads them
-//   (model/speech2text.py:50,54), so they are not produced here.
+//   :41 (merge heads).  The reference also returns the [B,h,T1,T2] weights.  This kernel never forms them; the modules'
+//   return_attn_weights switch has them written by a separate kernel over the same operands (attn_probs.cu).
 //
 // One CTA = 128 query rows of one (batch, head); 256 threads = two warpgroups, warpgroup w owns query rows
 // [64 w, 64 w + 64).  Keys are consumed in blocks of 128 with an online softmax:

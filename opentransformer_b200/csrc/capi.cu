@@ -196,6 +196,24 @@ int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, in
     RET("otb_attention", attn_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p, d_k));
 }
 
+int otb_attention_probs(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, float* out, int B, int H,
+                        int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, const float* bd, int ldbd,
+                        int d_k, void* stream) {
+    if (!q || !k || !out) return fail("otb_attention_probs", "null operand");
+    if (d_k != 64 && d_k != 96) return fail("otb_attention_probs", "head width d_k must be 64 or 96");
+    if (bd && (Tq != Tk || causal)) return fail("otb_attention_probs", "the rel-pos band needs Tq == Tk and no causal mask");
+    if (q_col0 % 8 || k_col0 % 8 || ldq % 8 || ldk % 8)
+        return fail("otb_attention_probs", "column offsets / leading dimensions must be multiples of 8");
+    AttnProbsParams p;
+    p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk;
+    p.kv_len = kv_len; p.causal = causal;
+    p.scale_log2 = 1.4426950408889634f / sqrtf((float)d_k);   // as otb_attention
+    p.q_col0 = q_col0; p.k_col0 = k_col0;
+    p.bd = bd; p.ldbd = ldbd;
+    p.out = out;
+    RET("otb_attention_probs", attn_probs_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, p, d_k));
+}
+
 int otb_layernorm(const void* x, int ldx, void* out, int ldo, int out_f32, const float* g1, const float* b1,
                   const float* g2, const float* b2, float eps, int M, int N, void* stream) {
     if (!x || !out || !g1 || !b1) return fail("otb_layernorm", "null operand");

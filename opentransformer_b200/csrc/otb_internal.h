@@ -156,6 +156,19 @@ const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const 
 // d_k: head width, 64 or 96 (head h starts at column col0 + d_k * h)
 const char* attn_launch(cudaStream_t st, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows,
                         const void* v, int ldv, const AttnParams& p, int d_k);
+// attention weights (attn_probs.cu): the score operands of attn_launch, P written as f32 [B, H, Tq, Tk]
+struct AttnProbsParams {
+    int B, H, Tq, Tk;
+    const int* kv_len;  // [B] or null
+    int causal;
+    float scale_log2;   // (1/sqrt(dk)) * log2(e)
+    int q_col0, k_col0;
+    const float* bd;    // optional rel-pos band as AttnParams::bd (Tq == Tk, not causal)
+    int ldbd;
+    float* out;         // [B, H, Tq, Tk], row pitch Tk
+};
+const char* attn_probs_launch(cudaStream_t st, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows,
+                              const AttnProbsParams& p, int d_k);
 const char* conv1_launch(cudaStream_t st, const float* x, const float* w, const float* bias, bf16* out, int B, int T,
                          int F, int T1, int F1, int T1pad, int F1pad, int C1);
 const char* layernorm_launch(cudaStream_t st, const bf16* x, int ldx, void* out, int ldo, int out_f32, const float* g1,

@@ -79,8 +79,9 @@ class SpeechToText(nn.Module):
                                         lookahead_steps=params['lookahead_steps'] if 'lookahead_steps' in params else 0)
         self.smoothing = params.get('smoothing', 0.0)
 
-    def encode_bf16(self, inputs, mask):
-        """frontend + encoder on the fused path -> (memory bf16 [B*T',D], lengths i32 [B], B, T')."""
+    def encode_bf16(self, inputs, mask, attn_sink=None):
+        """frontend + encoder on the fused path -> (memory bf16 [B*T',D], lengths i32 [B], B, T').  attn_sink (a list):
+        each encoder block's attention weights f32 [B, H, T', T'] are appended to it."""
         fe, enc = self.frontend, self.encoder
         B, T, _ = inputs.shape
         _, _, T2, _ = ops.conv_geometry(T, fe.input_size)
@@ -91,7 +92,7 @@ class SpeechToText(nn.Module):
         else:
             x, _ = fe.forward_bf16(inputs)
             x = enc.apply_posenc_bf16(x, B, T2)
-        return enc.forward_bf16(x, B, T2, lengths), lengths, B, T2
+        return enc.forward_bf16(x, B, T2, lengths, attn_sink), lengths, B, T2
 
     def forward_logits(self, inputs, mask, targets_in):
         """encoder + teacher-forced decoder (the forward half of speech2text.py:39-56) -> logits f32 [B,L,V]."""

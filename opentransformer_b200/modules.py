@@ -255,10 +255,13 @@ def _proj_resid_ln(ctx, w, b, resid, ln):
     return ops.layernorm(y, *ln) if ln is not None else y
 
 
-def _self_attn(y, resid, p, H, B, T, lengths, causal=False, ln=None):
-    """resid + output_proj(MHA(y)) (+ LayerNorm): QKV GEMM -> fused attention -> output projection with the residual."""
+def _self_attn(y, resid, p, H, B, T, lengths, causal=False, ln=None, attn_sink=None):
+    """resid + output_proj(MHA(y)) (+ LayerNorm): QKV GEMM -> fused attention -> output projection with the residual.
+    attn_sink (a list): the attention weights f32 [B, H, T, T] are appended to it."""
     d = y.shape[1]
     qkv = ops.linear(y, p['wqkv'], p['bqkv'])
+    if attn_sink is not None:
+        attn_sink.append(ops.attention_probs(qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d, d_k=d // H))
     ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d, v_col0=2 * d,
                         d_k=d // H)
     return _proj_resid_ln(ctx, p['wo'], p['bo'], resid, ln)
@@ -267,6 +270,11 @@ def _self_attn(y, resid, p, H, B, T, lengths, causal=False, ln=None):
 def _ffn_pack(ff):
     return {'w1': _w(ff.w_1), 'b1': _b(ff.w_1), 'w2': _w(ff.w_2), 'b2': _b(ff.w_2),
             'act': ACT_EPILOGUE[ff.activation]}
+
+
+def encoder_attn_weights(n_blocks, sink):
+    """The encoders' attn_weights dict (encoder/transformer.py:126-129): the maps collected in sink, or None maps."""
+    return {'enc_block_%d' % i: {'slf_attn_weights': sink[i] if sink is not None else None} for i in range(n_blocks)}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -301,9 +309,9 @@ class TransformerEncoderLayer(nn.Module):
             pk.update({'wqkv': _w(a.qvk_proj), 'bqkv': _b(a.qvk_proj), 'wo': _w(a.output_proj), 'bo': _b(a.output_proj)})
         return pk
 
-    def run(self, x, pk, B, T, lengths, causal=False, pos_bf16=None):
+    def run(self, x, pk, B, T, lengths, causal=False, pos_bf16=None, attn_sink=None):
         """x bf16 [B*T, d] -> bf16 [B*T, d]   (encoder/transformer.py:41-65); causal=True is the tril mask the
-        Transformer LM feeds to the same layer (model/lm.py:14-18,148-151)."""
+        Transformer LM feeds to the same layer (model/lm.py:14-18,148-151).  attn_sink: see _self_attn."""
         nb = self.normalize_before
         if nb:
             x = ops.layernorm(x, *pk['ln1'])          # residual is taken AFTER the norm (transformer.py:42-44)
@@ -311,11 +319,11 @@ class TransformerEncoderLayer(nn.Module):
         if self.relative_positional:
             if causal:
                 raise NotImplementedError('causal rel-pos attention')
-            x = self.slf_attn.run(x, x, pk['rel'], B, T, lengths, pos_bf16)       # x + attention (no output projection)
+            x = self.slf_attn.run(x, x, pk['rel'], B, T, lengths, pos_bf16, attn_sink)   # x + attention (no output projection)
             if ln is not None:
                 x = ops.layernorm(x, *ln)
         else:
-            x = _self_attn(x, x, pk, self.n_heads, B, T, lengths, causal, ln)
+            x = _self_attn(x, x, pk, self.n_heads, B, T, lengths, causal, ln, attn_sink)
         if nb:
             x = ops.layernorm(x, *pk['ln2'])
         return _ffn(x, pk['ffn'], x, None if nb else pk['ln2'])
@@ -324,8 +332,10 @@ class TransformerEncoderLayer(nn.Module):
 class TransformerEncoder(nn.Module):
     """forward(inputs f32 [B,T,D], mask bool [B,T]) -> (f32 [B,T,D], mask, attn_weights)
 
-    ``attn_weights`` maps 'enc_block_i' -> {'slf_attn_weights': None}: the reference materialises and
-    returns [B,h,T,T] weights that no caller reads (SURVEY.md 8a row 5); the fused kernel never forms them.
+    ``attn_weights`` maps 'enc_block_i' -> {'slf_attn_weights': P}.  The fused attention kernel never forms P, so by
+    default P is None; with ``return_attn_weights = True`` it is the reference's f32 [B, h, T, T] softmax
+    (encoder/transformer.py:126-129), written by one extra kernel per block (otb_attention_probs).  The encoder output
+    is the same either way.
     """
 
     def __init__(self, d_model=256, n_heads=4, d_ff=2048, n_blocks=6, pos_dropout=0.0, slf_attn_dropout=0.0,
@@ -345,6 +355,7 @@ class TransformerEncoder(nn.Module):
         self._pack = _Packed(self, lambda: {'blocks': [b.pack() for b in self.blocks],
                                             'norm': _ln(self.norm) if normalize_before else None})
         self._pos_cache = {}
+        self.return_attn_weights = False
 
     def _rel_pos(self, T, device):
         key = (T, device.index)
@@ -354,13 +365,14 @@ class TransformerEncoder(nn.Module):
             self._pos_cache[key] = p
         return p
 
-    def forward_bf16(self, x, B, T, lengths):
-        """x bf16 [B*T, d] with the positional encoding already applied (abs-pos) / the raw front-end output (rel-pos)."""
+    def forward_bf16(self, x, B, T, lengths, attn_sink=None):
+        """x bf16 [B*T, d] with the positional encoding already applied (abs-pos) / the raw front-end output (rel-pos).
+        attn_sink (a list): each block's attention weights f32 [B, H, T, T] are appended to it."""
         _no_train(self)
         pk = self._pack.get()
         pos = self._rel_pos(T, x.device) if self.relative_positional else None
         for blk, bpk in zip(self.blocks, pk['blocks']):
-            x = blk.run(x, bpk, B, T, lengths, pos_bf16=pos)
+            x = blk.run(x, bpk, B, T, lengths, pos_bf16=pos, attn_sink=attn_sink)
         if self.normalize_before:
             x = ops.layernorm(x, *pk['norm'])
         return x
@@ -378,9 +390,9 @@ class TransformerEncoder(nn.Module):
     def forward(self, inputs, mask):
         B, T, D = inputs.shape
         x = self.apply_posenc_bf16(inputs.contiguous().view(B * T, D), B, T)
-        y = self.forward_bf16(x, B, T, _lengths(mask))
-        attn = {'enc_block_%d' % i: {'slf_attn_weights': None} for i in range(len(self.blocks))}
-        return y.float().view(B, T, D), mask, attn
+        sink = [] if self.return_attn_weights else None
+        y = self.forward_bf16(x, B, T, _lengths(mask), sink)
+        return y.float().view(B, T, D), mask, encoder_attn_weights(len(self.blocks), sink)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -413,12 +425,15 @@ class MultiHeadedSelfAttentionWithRelPos(nn.Module):
         b_ext = torch.cat([b[:d] + u, b[:d] + v, b[d:2 * d], b[2 * d:]], 0)
         return {'wext': w_ext.to(BF16).contiguous(), 'bext': b_ext.contiguous(), 'wpos': _w(self.pos_proj)}
 
-    def run(self, y, x_resid, pk, B, T, lengths, pos_bf16):
-        """y = LN(x) bf16 [B*T,d]; returns x_resid + attention (no output projection)."""
+    def run(self, y, x_resid, pk, B, T, lengths, pos_bf16, attn_sink=None):
+        """y = LN(x) bf16 [B*T,d]; returns x_resid + attention (no output projection).  attn_sink (a list): the attention
+        weights f32 [B, H, T, T] are appended to it."""
         d, H = self.d_model, self.nheads
         ext = ops.linear(y, pk['wext'], pk['bext'])                       # [M, 4d]
         pproj = ops.linear(pos_bf16, pk['wpos'])                          # [2T-1, d]  pos_proj(PE[-(T-1)..T-1])
         bd = rel_pos_band(ext, pproj, H, B, T)
+        if attn_sink is not None:   # scores (q+u) k^T + BD, as the fused kernel below forms them
+            attn_sink.append(ops.attention_probs(ext, ext, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=2 * d, bd=bd, d_k=d // H))
         return ops.attention(ext, ext, ext, B, H, T, T, kv_len=lengths, q_col0=0, k_col0=2 * d, v_col0=3 * d,
                              bd=bd, resid=x_resid, d_k=d // H)
 
@@ -505,26 +520,27 @@ class ConformerEncoderBlock(nn.Module):
             pk['mha'] = {'wqkv': _w(a.qvk_proj), 'bqkv': _b(a.qvk_proj), 'wo': _w(a.output_proj), 'bo': _b(a.output_proj)}
         return pk
 
-    def _attn(self, x, pk, B, T, lengths, pos_bf16):
+    def _attn(self, x, pk, B, T, lengths, pos_bf16, attn_sink):
         y = ops.layernorm(x, *pk['mha_ln'])
         if self.relative_positional:
-            return self.mha.run(y, x, pk['mha'], B, T, lengths, pos_bf16)
-        return _self_attn(y, x, pk['mha'], self.n_heads, B, T, lengths)
+            return self.mha.run(y, x, pk['mha'], B, T, lengths, pos_bf16, attn_sink)
+        return _self_attn(y, x, pk['mha'], self.n_heads, B, T, lengths, attn_sink=attn_sink)
 
     def _conv(self, x, pk, B, T, lengths):
         return self.conv.run(ops.layernorm(x, *pk['conv_ln']), x, pk['conv'], B, T, lengths)
 
-    def run(self, x, pk, B, T, lengths, pos_bf16):
-        """ConformerEncoderBlock.forward (encoder/conformer.py:75-89) with the residual dropout disabled."""
+    def run(self, x, pk, B, T, lengths, pos_bf16, attn_sink=None):
+        """ConformerEncoderBlock.forward (encoder/conformer.py:75-89) with the residual dropout disabled.  attn_sink: see
+        MultiHeadedSelfAttentionWithRelPos.run."""
         if self.macaron_style:
             y = ops.layernorm(x, *pk['mac_ln'])
             f = pk['pre_ffn']
             h = ops.linear(y, f['w1'], f['b1'], f['act'])
             x = ops.linear(h, f['w2'], f['b2'], EPI_RESID, resid=x, alpha=self.ffn_scale)
         if self.conv_first:
-            x = self._attn(self._conv(x, pk, B, T, lengths), pk, B, T, lengths, pos_bf16)
+            x = self._attn(self._conv(x, pk, B, T, lengths), pk, B, T, lengths, pos_bf16, attn_sink)
         else:
-            x = self._conv(self._attn(x, pk, B, T, lengths, pos_bf16), pk, B, T, lengths)
+            x = self._conv(self._attn(x, pk, B, T, lengths, pos_bf16, attn_sink), pk, B, T, lengths)
         return ops.layernorm(x, *pk['post_ln'], *pk['final_ln'])   # post_ffn_norm then final_norm, one kernel
 
 
@@ -533,7 +549,9 @@ class ConformerEncoder(nn.Module):
 
     The reference applies F.dropout(p=residual_dropout) with training=True even in eval() (conformer.py:53,58,63,72),
     i.e. its inference is stochastic for residual_dropout > 0 (SURVEY.md 8a).  This implementation is the
-    deterministic network (no dropout at inference); parity is defined against residual_dropout = 0.0."""
+    deterministic network (no dropout at inference); parity is defined against residual_dropout = 0.0.
+
+    ``attn_weights`` as TransformerEncoder's: None maps unless ``return_attn_weights`` is set."""
 
     def __init__(self, d_model, d_ff, cov_kernel_size, n_heads, nblocks=12, pos_dropout=0.0, slf_attn_dropout=0.0,
                  ffn_dropout=0.0, residual_dropout=0.1, conv_dropout=0.0, macaron_style=True, ffn_scale=0.5,
@@ -551,6 +569,7 @@ class ConformerEncoder(nn.Module):
                                   relative_positional, activation) for _ in range(nblocks)])
         self._pack = _Packed(self, lambda: [b.pack() for b in self.blocks])
         self._pos_cache = {}
+        self.return_attn_weights = False
 
     def fuse_abs_posenc(self):
         return self.positional_encoding and not self.relative_positional
@@ -569,20 +588,21 @@ class ConformerEncoder(nn.Module):
             self._pos_cache[key] = p
         return p
 
-    def forward_bf16(self, x, B, T, lengths):
+    def forward_bf16(self, x, B, T, lengths, attn_sink=None):
+        """attn_sink (a list): each block's attention weights f32 [B, H, T, T] are appended to it."""
         _no_train(self)
         pks = self._pack.get()
         pos = self._rel_pos(T, x.device) if (self.positional_encoding and self.relative_positional) else None
         for blk, pk in zip(self.blocks, pks):
-            x = blk.run(x, pk, B, T, lengths, pos)
+            x = blk.run(x, pk, B, T, lengths, pos, attn_sink)
         return x
 
     def forward(self, inputs, mask):
         B, T, D = inputs.shape
         x = self.apply_posenc_bf16(inputs.contiguous().view(B * T, D), B, T)
-        y = self.forward_bf16(x, B, T, _lengths(mask))
-        attn = {'enc_block_%d' % i: {'slf_attn_weights': None} for i in range(len(self.blocks))}
-        return y.float().view(B, T, D), mask, attn
+        sink = [] if self.return_attn_weights else None
+        y = self.forward_bf16(x, B, T, _lengths(mask), sink)
+        return y.float().view(B, T, D), mask, encoder_attn_weights(len(self.blocks), sink)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -669,7 +689,11 @@ class TransformerDecoder(nn.Module):
     """forward(targets i64 [B,L], memory f32 [B,T,D], memory_mask bool [B,T]) -> (logits f32 [B,L,V], attn)
     inference(preds i64 [N,l], memory, memory_mask, cache) -> (log_probs f32 [N,V], cache, attn)
     (decoder/transformer.py:161-208).  `cache` is passed through untouched exactly like the reference;
-    the KV-cached incremental path lives in recognize.BeamDecoder."""
+    the KV-cached incremental path lives in recognize.BeamDecoder.
+
+    ``attn`` maps 'dec_block_i' -> {'slf_attn_weights', 'src_attn_weights'}: None by default; with
+    ``return_attn_weights = True``, forward (and inference without a DecoderCache) returns the reference's f32 maps,
+    [B, h, L, L] under the causal mask and [B, h, L, T] under the memory lengths."""
 
     def __init__(self, vocab_size, d_model=256, n_heads=4, d_ff=2048, memory_dim=256, n_blocks=6, pos_dropout=0.0,
                  slf_attn_dropout=0.0, src_attn_dropout=0.0, ffn_dropout=0.0, residual_dropout=0.1,
@@ -692,6 +716,7 @@ class TransformerDecoder(nn.Module):
             assert self.embedding.weight.size() == self.output_layer.weight.size()
             self.output_layer.weight = self.embedding.weight   # tied (decoder/transformer.py:156-158)
         self._pack = _Packed(self, self._build_pack)
+        self.return_attn_weights = False
 
     def _build_pack(self):
         emb = self.embedding.weight.detach().to(BF16).contiguous()
@@ -738,11 +763,13 @@ class TransformerDecoder(nn.Module):
             # (the attention kernel pads the problem to 128 query rows)
             lambda l, q: ops.attention(q, kvx[l], kvx[l], batch, H, beam, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H))
 
-    def forward_bf16(self, targets, memory_bf16, mem_len, B, L, T):
-        """targets i64 [B,L]; memory bf16 [B*T, D] -> logits f32 [B*L, ld_logits] (first V columns valid)."""
-        return self.score_bf16(targets, memory_bf16, mem_len, B, 1, L, T)
+    def forward_bf16(self, targets, memory_bf16, mem_len, B, L, T, attn_sink=None):
+        """targets i64 [B,L]; memory bf16 [B*T, D] -> logits f32 [B*L, ld_logits] (first V columns valid).
+        attn_sink (a list): each layer's self- and cross-attention weights, f32 [B, H, L, L] and [B, H, L, T], are
+        appended to it in that order."""
+        return self.score_bf16(targets, memory_bf16, mem_len, B, 1, L, T, attn_sink)
 
-    def score_bf16(self, inputs, memory_bf16, mem_len, B, K, Lp, T):
+    def score_bf16(self, inputs, memory_bf16, mem_len, B, K, Lp, T, attn_sink=None):
         """Teacher-forced logits of K sequences per utterance (the second pass of n-best rescoring): inputs i64 [B*K, Lp],
         memory bf16 [B*T, D] -> logits f32 [B*K*Lp, ld_logits] (first V columns valid).  Self-attention is causal within
         each of the B*K sequences; cross-attention treats the K*Lp query rows of utterance b as one problem against its
@@ -756,11 +783,15 @@ class TransformerDecoder(nn.Module):
         x = ops.embed_posenc(inputs.contiguous(), pk['emb'], table, B * K * Lp, d, period=Lp)
 
         def self_attn(l, qkv):
+            if attn_sink is not None:
+                attn_sink.append(ops.attention_probs(qkv, qkv, B * K, H, Lp, Lp, causal=True, q_col0=0, k_col0=d, d_k=d // H))
             return ops.attention(qkv, qkv, qkv, B * K, H, Lp, Lp, causal=True, q_col0=0, k_col0=d, v_col0=2 * d, d_k=d // H)
 
         def cross_attn(l, q):       # the memory's K|V, projected per layer after the query GEMM
             p = pk['blocks'][l]
             kv = ops.linear(memory_bf16, p['wkv'], p['bkv'])
+            if attn_sink is not None:
+                attn_sink.append(ops.attention_probs(q, kv, B, H, K * Lp, T, kv_len=mem_len, k_col0=0, d_k=d // H))
             return ops.attention(q, kv, kv, B, H, K * Lp, T, kv_len=mem_len, k_col0=0, v_col0=d, d_k=d // H)
 
         x = self._layers(pk, x, self_attn, cross_attn)
@@ -770,8 +801,10 @@ class TransformerDecoder(nn.Module):
         B, L = targets.shape
         T, D = memory.shape[1], memory.shape[2]
         mem = ops.scale_add_table(memory.contiguous().view(B * T, D))   # f32 -> bf16
-        logits = self.forward_bf16(targets, mem, _lengths(memory_mask), B, L, T)
-        attn = {'dec_block_%d' % i: {'slf_attn_weights': None, 'src_attn_weights': None}
+        sink = [] if self.return_attn_weights else None
+        logits = self.forward_bf16(targets, mem, _lengths(memory_mask), B, L, T, sink)
+        attn = {'dec_block_%d' % i: {'slf_attn_weights': sink[2 * i] if sink is not None else None,
+                                     'src_attn_weights': sink[2 * i + 1] if sink is not None else None}
                 for i in range(len(self.blocks))}
         return logits.view(B, L, -1)[:, :, :self.vocab_size], attn
 
@@ -784,7 +817,8 @@ class TransformerDecoder(nn.Module):
         """decoder/transformer.py:185-208.  cache None (the reference's only working mode): the whole prefix is recomputed.
         cache = DecoderCache (``init_cache``): only the newest token preds[:, -1] is run through the layers against the cached
         keys / values -- O(l) instead of O(l^2) per step -- and the same object is returned; the caller reorders it after
-        pruning (SpeechToTextRecognizer.decode_step does)."""
+        pruning (SpeechToTextRecognizer.decode_step does).  The cached path returns None maps even with
+        return_attn_weights set: it never forms the attention weights of the earlier positions."""
         assert preds.dim() == 2
         if isinstance(cache, DecoderCache):
             return self._inference_cached(preds, cache)

@@ -239,6 +239,31 @@ def attention(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0
     return _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, out, bd, resid, d_k)[0]
 
 
+def attention_probs(q, k, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, bd=None, d_k=64, out=None):
+    """The attention weights of attention() over the same q / k operands, column offsets, mask and band
+    (otb_attention_probs) -> f32 [B, H, Tq, Tk]: masked entries 0, batch entries with kv_len 0 all NaN."""
+    for t, n in ((q, 'q'), (k, 'k')):
+        _need(t, BF16, n)
+    check_head_dim(d_k)
+    if kv_len is not None:
+        _need(kv_len, torch.int32, 'kv_len')
+    if bd is not None:
+        _need(bd, torch.float32, 'bd')
+        if Tq != Tk or causal:
+            raise ValueError('attention_probs: the rel-pos band is for non-causal self-attention (Tq == Tk)')
+    if out is None:
+        out = torch.empty(B, H, Tq, Tk, dtype=torch.float32, device=q.device)
+    else:
+        _need(out, torch.float32, 'out')
+        if tuple(out.shape) != (B, H, Tq, Tk):
+            raise ValueError(f'attention_probs: out must be [{B}, {H}, {Tq}, {Tk}], got {tuple(out.shape)}')
+    check(_lib.lib().otb_attention_probs(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(out), B, H, Tq, Tk,
+                                         _p(kv_len), 1 if causal else 0, q_col0, k_col0, _p(bd),
+                                         bd.shape[-1] if bd is not None else 0, d_k, _stream()), 'otb_attention_probs')
+    _count()
+    return out
+
+
 def dwconv_swish(x, w, b, B, T, out=None):
     """depthwise conv over time + folded BatchNorm + swish; x bf16 [B*T, d], w f32 [k, d], b f32 [d]."""
     _need(x, BF16, 'x'); _need(w, torch.float32, 'w'); _need(b, torch.float32, 'b')

@@ -22,6 +22,7 @@ import torch
 
 from . import ops
 from .model import ctc_align_logits
+from .modules import encoder_attn_weights
 
 PAD, BOS, EOS = 0, 1, 1   # otrans/data/__init__.py:7-10
 
@@ -440,9 +441,12 @@ class SpeechToTextRecognizer(Recognizer):
 
     # ---- reference-facing seams -------------------------------------------------------------
     def encode(self, inputs, inputs_mask, cache=None):
+        """-> (memory, memory_mask, cache, attention weights): the encoder's attn_weights dict when
+        model.encoder.return_attn_weights is set, else {}."""
         mem, mem_len, B, T2 = self._encode_bf16(inputs, inputs_mask)
         memory = mem.float().view(B, T2, -1)
-        return memory, self.model.frontend.output_mask(inputs_mask), {'frontend': None}, {}
+        maps = self.attn_weights['encoder'] if self.model.encoder.return_attn_weights else {}
+        return memory, self.model.frontend.output_mask(inputs_mask), {'frontend': None}, maps
 
     def decode(self, preds, memory, memory_mask, cache=None):
         return self.model.decoder.inference(preds, memory, memory_mask, cache)
@@ -480,7 +484,16 @@ class SpeechToTextRecognizer(Recognizer):
 
     # ---- fast path ------------------------------------------------------------------------------
     def _encode_bf16(self, inputs, inputs_mask):
-        return self.model.encode_bf16(inputs, inputs_mask)
+        """The encoder pass of every path.  With model.encoder.return_attn_weights set it also fills self.attn_weights
+        as the reference's recognize does (recognize/speech2text.py:43-47): {'encoder': the encoder's attn_weights dict,
+        'decoder': []}; otherwise attn_weights stays {}."""
+        enc = self.model.encoder
+        if not enc.return_attn_weights:
+            return self.model.encode_bf16(inputs, inputs_mask)
+        sink = []
+        out = self.model.encode_bf16(inputs, inputs_mask, attn_sink=sink)
+        self.attn_weights = {'encoder': encoder_attn_weights(len(enc.blocks), sink), 'decoder': []}
+        return out
 
     def _decoder_for(self, B, T2, device):
         # the CTC weight and candidate count are launch arguments that a captured step bakes in

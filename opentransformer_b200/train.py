@@ -1042,11 +1042,14 @@ class FusedTrainer:
         (hypothesis inputs i64 [B*K, Lp], targets i32 [B*K, Lp]).  Reading Lp is a host synchronisation; as part of the
         batch the rows make Lp and K part of the CUDA-graph key."""
         from .recognize import second_pass_rows
+        enc = self.model.encoder
+        maps, enc.return_attn_weights = enc.return_attn_weights, False    # training produces no attention maps
         self.model.eval()
         try:
             ids, _, _ = self._recognizer.recognize_ids(batch[0], batch[1])
         finally:
             self.model.train()
+            enc.return_attn_weights = maps
         hyp_in, tgt, _, Lp = second_pass_rows(ids)
         return batch + (hyp_in, tgt.view(-1, Lp))
 
