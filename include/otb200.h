@@ -156,7 +156,9 @@ int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int 
 
 /* Decode-step self-attention over a per-hypothesis KV cache (the cache API the reference left as a
  * stub, decoder/transformer.py:92-126,188-203): qkv bf16 [N,3d] of the newest token; kc/vc bf16
- * [Lmax,N,d]; anc i32 [2,N,Lmax]; *step_ptr = 0-based position; out bf16 [N,d]; head width d_k 64 or 96 (d = H*d_k). */
+ * [Lmax,N,d]; anc i32 [2,N,Lmax]; *step_ptr = 0-based position; out bf16 [N,d]; head width d_k 64 or 96 (d = H*d_k).
+ * Lmax <= 1023; above 128 the prefix is read in chunks of 128 keys with an online softmax.  Shared memory per CTA:
+ * min(H, 4) * (min(Lmax rounded up to 32, 128) * d_k * 2 + d_k * 4) bytes. */
 int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
                          int H, int Lmax, int d_k, void* stream);
 
@@ -357,8 +359,10 @@ int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, cons
 /* Joint-CTC loss of SpeechToText.forward (model/speech2text.py:60-72 -> CTCAssistor.compute_loss, model/ctc.py:48-52):
  * nn.CTCLoss(blank, reduction 'mean', zero_infinity = True) and its gradient with respect to the LOGITS.
  * logp f32 [B*T, ldl] = log_softmax of the assistor's logits (otb_log_softmax); in_len i32 [B] valid frames; targets i64
- * [B, ldt] label rows (the first tgt_len[b] entries count); max_tgt >= every tgt_len (<= 64); nll f32 [B] per-utterance
- * negative log-likelihood (+inf if infeasible); loss f32 [1]; ws f32 [B, T, 2 max_tgt + 1] scratch (alpha + beta);
+ * [B, ldt] label rows (the first tgt_len[b] entries count); max_tgt >= every tgt_len, at most 1023 (one state per thread up
+ * to 64, two per thread above); nll f32 [B] per-utterance
+ * negative log-likelihood (+inf if infeasible); loss f32 [1]; ws f32 [B, T, 2 max_tgt + 1] scratch (alpha + beta; 262 MB
+ * at B 32, T 1000, max_tgt 1023);
  * dlogits_bf16 (optional, bf16 [B*T, ldd]) = grad_scale * d loss / d logits (padded frames / infeasible utterances: 0).
  * grad_scale_dev (may be NULL): a device f32 scalar grad_scale is multiplied by, read on the device. */
 int otb_ctc_loss(const float* logp, int ldl, int B, int T, int V, const int32_t* in_len, const int64_t* targets, int ldt,

@@ -2,7 +2,9 @@
 //   loss_ctc = nn.CTCLoss(blank = 0, reduction 'mean', zero_infinity = True)(log_softmax(output_layer(memory)).transpose(0,1),
 //                                                                              targets_out, memory_length, targets_length)
 // Forward AND gradient with respect to the logits in two kernels (the reference differentiates F.ctc_loss by autograd):
-//   ctc_alpha_beta_kernel  one CTA per utterance, thread = state of the blank-extended label sequence (S = 2 L + 1 <= 129):
+//   ctc_alpha_beta_kernel  one CTA per utterance over the S = 2 L + 1 states of the blank-extended label sequence: one
+//                          state per thread up to 64 labels (S <= 129, 160 threads), two per thread up to 1023 (S <= 2047,
+//                          1024 threads):
 //                          forward variables alpha_t(s) over the valid frames (log domain, fp32), the utterance's negative
 //                          log-likelihood, then the backward variables; ws[b,t,s] <- alpha_t(s) + beta_t(s)
 //   ctc_grad_kernel        one CTA per (utterance, frame): d loss / d logit[k] = scale_b (softmax[k] - sum_{s: l_s = k}
@@ -18,7 +20,8 @@
 
 namespace otb {
 
-static constexpr int CTC_SMAX = 129;   // 2 * 64 + 1 states
+static constexpr int CTC_SMAX = 129;        // 2 * 64 + 1 states: targets of up to 64 labels
+static constexpr int CTC_SMAX_LONG = 2047;  // 2 * 1023 + 1 states: targets of up to 1023 labels
 
 __global__ void __launch_bounds__(160) ctc_alpha_beta_kernel(const float* __restrict__ logp, int ldl, int T, const int* __restrict__ in_len,
                                                              const long long* __restrict__ targets, int ldt,
@@ -95,6 +98,111 @@ __global__ void __launch_bounds__(160) ctc_alpha_beta_kernel(const float* __rest
     }
 }
 
+// Targets of 65..1023 labels: the kernel above with SPT states per thread, state s = threadIdx.x + j NT (j < SPT), so
+// that S <= 2047 fits 1024 threads.  Every state of a frame reads the previous frame's row in buf: one barrier per frame.
+// (A loop over one state per thread schedules differently from the kernel above, which keeps its code for <= 64 labels.)
+template <int SMAX, int NT>
+__global__ void __launch_bounds__(NT) ctc_alpha_beta_multi_kernel(const float* __restrict__ logp, int ldl, int T, const int* __restrict__ in_len,
+                                                            const long long* __restrict__ targets, int ldt,
+                                                            const int* __restrict__ tgt_len, int blank, int V, float* __restrict__ nll,
+                                                            float* __restrict__ ws, int S_ws) {
+    constexpr int SPT = (SMAX + NT - 1) / NT;
+    __shared__ int lab[SMAX + 2];
+    __shared__ float buf[2][SMAX + 2];
+    const int b = blockIdx.x;
+    const int L = min(tgt_len[b], (SMAX - 1) / 2);
+    const int S = 2 * L + 1;
+    const int Tb = min(in_len[b], T);
+#pragma unroll
+    for (int j = 0; j < SPT; ++j) {
+        const int s = threadIdx.x + j * NT;
+        if (s < S + 2) {
+            int l = blank;
+            if (s < S && (s & 1)) {
+                long long v = targets[(size_t)b * ldt + (s >> 1)];
+                l = (v < 0 || v >= V) ? blank : (int)v;
+            }
+            lab[s] = l;
+        }
+    }
+    __syncthreads();
+    const float* lp = logp + (size_t)b * T * ldl;
+    float* w = ws + (size_t)b * T * S_ws;
+    if (Tb < 1) {   // no frames: infeasible unless the target is empty too (PyTorch: inf -> 0 with zero_infinity)
+        if (threadIdx.x == 0) nll[b] = INFINITY;
+        return;
+    }
+    int my[SPT];
+    bool skip_ok[SPT];
+    float a[SPT];
+    // ---- forward variables
+#pragma unroll
+    for (int j = 0; j < SPT; ++j) {
+        const int s = threadIdx.x + j * NT;
+        my[j] = (s < S) ? lab[s] : blank;
+        skip_ok[j] = (s >= 2 && s < S && my[j] != blank && my[j] != lab[s - 2]);
+        a[j] = -INFINITY;
+        if (s == 0) a[j] = lp[blank];
+        if (s == 1 && S > 1) a[j] = lp[my[j]];
+        if (s < S) { buf[0][s] = a[j]; w[s] = a[j]; }
+    }
+    __syncthreads();
+    int cur = 0;
+    for (int t = 1; t < Tb; ++t) {
+#pragma unroll
+        for (int j = 0; j < SPT; ++j) {
+            const int s = threadIdx.x + j * NT;
+            if (s < S) {
+                float v = buf[cur][s];
+                if (s >= 1) v = log_add(v, buf[cur][s - 1]);
+                if (skip_ok[j]) v = log_add(v, buf[cur][s - 2]);
+                a[j] = (v == -INFINITY) ? -INFINITY : v + lp[(size_t)t * ldl + my[j]];
+                buf[cur ^ 1][s] = a[j];
+                w[(size_t)t * S_ws + s] = a[j];
+            }
+        }
+        cur ^= 1;
+        __syncthreads();
+    }
+    float total = buf[cur][S - 1];
+    if (S > 1) total = log_add(total, buf[cur][S - 2]);
+    __syncthreads();
+    if (threadIdx.x == 0) nll[b] = -total;          // +inf when no alignment exists
+    // ---- backward variables; ws <- alpha + beta
+    bool skip_fw[SPT];
+    float be[SPT];
+#pragma unroll
+    for (int j = 0; j < SPT; ++j) {
+        const int s = threadIdx.x + j * NT;
+        skip_fw[j] = (s + 2 < S && lab[s + 2] != blank && lab[s + 2] != my[j]);
+        be[j] = -INFINITY;
+        if (s == S - 1) be[j] = lp[(size_t)(Tb - 1) * ldl + blank];
+        if (s == S - 2 && S > 1) be[j] = lp[(size_t)(Tb - 1) * ldl + my[j]];
+        if (s < S) {
+            buf[0][s] = be[j];
+            w[(size_t)(Tb - 1) * S_ws + s] += be[j];
+        }
+    }
+    __syncthreads();
+    cur = 0;
+    for (int t = Tb - 2; t >= 0; --t) {
+#pragma unroll
+        for (int j = 0; j < SPT; ++j) {
+            const int s = threadIdx.x + j * NT;
+            if (s < S) {
+                float v = buf[cur][s];
+                if (s + 1 < S) v = log_add(v, buf[cur][s + 1]);
+                if (skip_fw[j]) v = log_add(v, buf[cur][s + 2]);
+                be[j] = (v == -INFINITY) ? -INFINITY : v + lp[(size_t)t * ldl + my[j]];
+                buf[cur ^ 1][s] = be[j];
+                w[(size_t)t * S_ws + s] += be[j];
+            }
+        }
+        cur ^= 1;
+        __syncthreads();
+    }
+}
+
 // loss = mean_b (finite nll_b ? nll_b / max(tgt_len_b, 1) : 0)   (single CTA)
 __global__ void ctc_mean_kernel(const float* __restrict__ nll, const int* __restrict__ tgt_len, int B, float* loss) {
     __shared__ float red[32];
@@ -113,15 +221,20 @@ __global__ void ctc_mean_kernel(const float* __restrict__ nll, const int* __rest
     }
 }
 
+// Each label's occupancies are summed in ascending state order by the label's first state, which writes d[label].
+// SORT false (targets <= 64 labels): every state scans the states before it for its label, O(S^2) per frame.
+// SORT true (up to 1023 labels): the (label, state) pairs are sorted in shared memory (bitonic, O(S log^2 S) work in
+// O(log^2 S) barriers), so each label's states form one ascending run that its first state walks.
+template <int SMAX, bool SORT>
 __global__ void __launch_bounds__(256) ctc_grad_kernel(const float* __restrict__ logp, int ldl, int T, int V, const int* __restrict__ in_len,
                                                        const long long* __restrict__ targets, int ldt,
                                                        const int* __restrict__ tgt_len, int blank, const float* __restrict__ nll,
                                                        const float* __restrict__ ws, int S_ws, int B, float grad_scale,
                                                        bf16* __restrict__ dlogits, int ldd, const float* __restrict__ scale_dev) {
-    __shared__ int lab[CTC_SMAX];
-    __shared__ float occ[CTC_SMAX];
+    __shared__ int lab[SMAX];
+    __shared__ float occ[SMAX];
     const int row = blockIdx.x, b = row / T, t = row % T;
-    const int L = min(tgt_len[b], (CTC_SMAX - 1) / 2);
+    const int L = min(tgt_len[b], (SMAX - 1) / 2);
     const int S = 2 * L + 1;
     const float nl = nll[b];
     bf16* d = dlogits + (size_t)row * ldd;
@@ -146,18 +259,50 @@ __global__ void __launch_bounds__(256) ctc_grad_kernel(const float* __restrict__
     }
     for (int k = threadIdx.x; k < ldd; k += blockDim.x) d[k] = __float2bfloat16(k < V ? scale * expf(lp[k]) : 0.f);
     __syncthreads();
-    // first occurrence of every label owns the combined entry (same-CTA global writes after the barrier: the later write wins)
-    for (int s = threadIdx.x; s < S; s += blockDim.x) {
-        const int l = lab[s];
-        bool first = true;
-        float tot = 0.f;
-        for (int s2 = 0; s2 < S; ++s2) {
-            if (lab[s2] == l) {
-                if (s2 < s) { first = false; break; }
-                tot += occ[s2];
+    if constexpr (!SORT) {
+        // first occurrence of every label owns the combined entry (same-CTA global writes after the barrier: the later write wins)
+        for (int s = threadIdx.x; s < S; s += blockDim.x) {
+            const int l = lab[s];
+            bool first = true;
+            float tot = 0.f;
+            for (int s2 = 0; s2 < S; ++s2) {
+                if (lab[s2] == l) {
+                    if (s2 < s) { first = false; break; }
+                    tot += occ[s2];
+                }
+            }
+            if (first) d[l] = __float2bfloat16(scale * (expf(lp[l]) - tot));
+        }
+    } else {
+        constexpr int NK = 2048;                      // power of two >= SMAX
+        static_assert(SMAX <= NK, "sort width");
+        __shared__ unsigned long long key[NK];        // label << 32 | state; padding sorts last
+        const int n = S <= 1 ? 1 : 1 << (32 - __clz(S - 1));
+        for (int i = threadIdx.x; i < n; i += blockDim.x)
+            key[i] = i < S ? ((unsigned long long)(unsigned)lab[i] << 32 | (unsigned)i) : ~0ull;
+        __syncthreads();
+        for (int k = 2; k <= n; k <<= 1) {
+            for (int j = k >> 1; j > 0; j >>= 1) {
+                for (int i = threadIdx.x; i < n; i += blockDim.x) {
+                    const int p = i ^ j;
+                    if (p > i) {
+                        const unsigned long long x = key[i], y = key[p];
+                        if (((i & k) == 0) == (x > y)) {
+                            key[i] = y;
+                            key[p] = x;
+                        }
+                    }
+                }
+                __syncthreads();
             }
         }
-        if (first) d[l] = __float2bfloat16(scale * (expf(lp[l]) - tot));
+        for (int i = threadIdx.x; i < S; i += blockDim.x) {
+            const unsigned l = (unsigned)(key[i] >> 32);
+            if (i > 0 && (unsigned)(key[i - 1] >> 32) == l) continue;
+            float tot = 0.f;
+            for (int r = i; r < S && (unsigned)(key[r] >> 32) == l; ++r) tot += occ[(unsigned)key[r]];
+            d[l] = __float2bfloat16(scale * (expf(lp[l]) - tot));
+        }
     }
 }
 
@@ -165,16 +310,22 @@ const char* ctc_launch(cudaStream_t st, const float* logp, int ldl, int B, int T
                        int ldt, const int* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, bf16* dlogits, int ldd,
                        float grad_scale, const float* scale_dev) {
     if (B < 1 || T < 1 || V < 2) return "ctc: empty problem";
-    if (max_tgt < 0 || 2 * max_tgt + 1 > CTC_SMAX) return "ctc: targets longer than 64 labels are not supported";
+    if (max_tgt < 0 || 2 * max_tgt + 1 > CTC_SMAX_LONG) return "ctc: targets longer than 1023 labels are not supported";
     if (blank < 0 || blank >= V) return "ctc: bad blank id";
     const int S_ws = 2 * max_tgt + 1;
+    const bool lng = S_ws > CTC_SMAX;
     const char* err;
-    if ((err = launch<ctc_alpha_beta_kernel>(B, 160, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len, blank, V, nll, ws, S_ws)))
+    if ((err = lng ? launch<ctc_alpha_beta_multi_kernel<CTC_SMAX_LONG, 1024>>(B, 1024, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len,
+                                                                        blank, V, nll, ws, S_ws)
+                   : launch<ctc_alpha_beta_kernel>(B, 160, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len, blank,
+                                                                  V, nll, ws, S_ws)))
         return err;
     if ((err = launch<ctc_mean_kernel>(1, 256, 0, st, nll, tgt_len, B, loss))) return err;
     if (!dlogits) return nullptr;
-    return launch<ctc_grad_kernel>(B * T, 256, 0, st, logp, ldl, T, V, in_len, targets, ldt, tgt_len, blank, nll, ws, S_ws, B,
-                                   grad_scale, dlogits, ldd, scale_dev);
+    return lng ? launch<ctc_grad_kernel<CTC_SMAX_LONG, true>>(B * T, 256, 0, st, logp, ldl, T, V, in_len, targets, ldt, tgt_len, blank,
+                                                              nll, ws, S_ws, B, grad_scale, dlogits, ldd, scale_dev)
+               : launch<ctc_grad_kernel<CTC_SMAX, false>>(B * T, 256, 0, st, logp, ldl, T, V, in_len, targets, ldt, tgt_len, blank,
+                                                          nll, ws, S_ws, B, grad_scale, dlogits, ldd, scale_dev);
 }
 
 }  // namespace otb

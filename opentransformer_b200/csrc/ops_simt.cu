@@ -379,7 +379,7 @@ __device__ __forceinline__ int rot_chunk(int i) {
 //   kc,vc bf16 [Lmax, N, d]
 //   anc   int32 [2, N, Lmax]  (ping-pong, buffer (step & 1) is current)
 // ------------------------------------------------------------------------------------------------
-template <int DK>
+template <int DK, bool CHUNKED>
 __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc,
                                                                bf16* __restrict__ vc, const int* __restrict__ anc,
                                                                const int* __restrict__ step_ptr, bf16* __restrict__ out,
@@ -388,7 +388,10 @@ __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel
     // ancestry table and pulls the whole K and V rows (DK * 2 bytes) with 16-byte loads -- all loads of a lane are
     // independent, so the kernel costs ~3 dependent memory round trips (anc -> K/V -> out) instead of a
     // serial walk over the prefix.  V rows go through smem so that the P.V reduction is a column sum.
-    constexpr int KPL = 4;               // keys per lane -> up to 128 cached positions
+    // CHUNKED (prefixes of 129..1023 positions): the prefix is walked in chunks of 32 KPL keys with an online softmax (running
+    // max and sum, P.V accumulators rescaled between chunks), and the V staging holds one chunk.  Without it the one
+    // chunk is the whole prefix (at most 128 positions).
+    constexpr int KPL = 4;               // keys per lane -> 128 cached positions per chunk
     constexpr int CH = DK / 8;           // 16-byte chunks per K / V row
     extern __shared__ uint4 sv_raw[];    // [warps][keys_pad][CH x 16 B]  V rows (bf16)
     const int n = blockIdx.x;
@@ -427,97 +430,120 @@ __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel
             }
             __syncwarp();
         }
-        int slot[KPL];
+        float mx = -INFINITY, l = 0.f;
+        // P.V accumulators: at DK 64 lane owns output dims 2*lane, 2*lane+1 (acc[0..1]); at DK 96 lanes 0..23 own
+        // 4*lane .. 4*lane+3 (acc[0..3])
+        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+        const int c_end = CHUNKED ? nkeys : 1;
+        for (int c0 = 0; c0 < c_end; c0 += 32 * KPL) {
+            int slot[KPL];
 #pragma unroll
-        for (int j = 0; j < KPL; ++j) {
-            const int s = lane + 32 * j;
-            slot[j] = (s < step) ? an[s] : n;
-        }
-        float sc[KPL];
-        float mx = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < KPL; ++j) {
-            const int s = lane + 32 * j;
-            sc[j] = -INFINITY;
-            if (s < nkeys) {   // warp-divergent only in the last group
-                const bf16* krow = (s == step) ? base + d : kc + ((size_t)s * N + slot[j]) * d + h * DK;
-                const bf16* vrow = (s == step) ? base + 2 * d : vc + ((size_t)s * N + slot[j]) * d + h * DK;
-                uint4 ku[CH], vu[CH];
-#pragma unroll
-                for (int i = 0; i < CH; ++i) ku[i] = *reinterpret_cast<const uint4*>(krow + 8 * i);
-#pragma unroll
-                for (int i = 0; i < CH; ++i) vu[i] = *reinterpret_cast<const uint4*>(vrow + 8 * i);
-                float dot = 0.f;
-#pragma unroll
-                for (int i = 0; i < CH; ++i) {
-                    const float2 a = unpack_bf16(ku[i].x), b = unpack_bf16(ku[i].y), c = unpack_bf16(ku[i].z),
-                                 e = unpack_bf16(ku[i].w);
-                    const float4 q0 = *reinterpret_cast<const float4*>(sq + 8 * i);      // broadcast reads
-                    const float4 q1 = *reinterpret_cast<const float4*>(sq + 8 * i + 4);
-                    dot += q0.x * a.x + q0.y * a.y + q0.z * b.x + q0.w * b.y + q1.x * c.x + q1.y * c.y + q1.z * e.x + q1.w * e.y;
-                }
-                sc[j] = dot * scale;
-                mx = fmaxf(mx, sc[j]);
-#pragma unroll
-                for (int i = 0; i < CH; ++i) sv[s * CH + rot_chunk<CH>(i + s)] = vu[i];   // rotate chunks: conflict-free rows
+            for (int j = 0; j < KPL; ++j) {
+                const int s = c0 + lane + 32 * j;
+                slot[j] = (s < step) ? an[s] : n;
             }
-        }
-        mx = warp_max(mx);
-        float l = 0.f;
+            float sc[KPL];
+            float cmx = -INFINITY;
 #pragma unroll
-        for (int j = 0; j < KPL; ++j) {
-            sc[j] = (lane + 32 * j < nkeys) ? __expf(sc[j] - mx) : 0.f;
-            l += sc[j];
+            for (int j = 0; j < KPL; ++j) {
+                const int s = c0 + lane + 32 * j, sl = lane + 32 * j;   // position in the prefix / in the chunk
+                sc[j] = -INFINITY;
+                if (s < nkeys) {   // warp-divergent only in the last group
+                    const bf16* krow = (s == step) ? base + d : kc + ((size_t)s * N + slot[j]) * d + h * DK;
+                    const bf16* vrow = (s == step) ? base + 2 * d : vc + ((size_t)s * N + slot[j]) * d + h * DK;
+                    uint4 ku[CH], vu[CH];
+#pragma unroll
+                    for (int i = 0; i < CH; ++i) ku[i] = *reinterpret_cast<const uint4*>(krow + 8 * i);
+#pragma unroll
+                    for (int i = 0; i < CH; ++i) vu[i] = *reinterpret_cast<const uint4*>(vrow + 8 * i);
+                    float dot = 0.f;
+#pragma unroll
+                    for (int i = 0; i < CH; ++i) {
+                        const float2 a = unpack_bf16(ku[i].x), b = unpack_bf16(ku[i].y), c = unpack_bf16(ku[i].z),
+                                     e = unpack_bf16(ku[i].w);
+                        const float4 q0 = *reinterpret_cast<const float4*>(sq + 8 * i);      // broadcast reads
+                        const float4 q1 = *reinterpret_cast<const float4*>(sq + 8 * i + 4);
+                        dot += q0.x * a.x + q0.y * a.y + q0.z * b.x + q0.w * b.y + q1.x * c.x + q1.y * c.y + q1.z * e.x + q1.w * e.y;
+                    }
+                    sc[j] = dot * scale;
+                    cmx = fmaxf(cmx, sc[j]);
+#pragma unroll
+                    for (int i = 0; i < CH; ++i) sv[sl * CH + rot_chunk<CH>(i + sl)] = vu[i];   // rotate chunks: conflict-free rows
+                }
+            }
+            cmx = warp_max(cmx);
+            float corr = 0.f;   // rescales the previous chunks' sum and accumulators to the new running max
+            if constexpr (CHUNKED) {
+                const float m = fmaxf(mx, cmx);
+                corr = __expf(mx - m);
+                mx = m;
+            } else {
+                mx = cmx;
+            }
+            float cl = 0.f;
+#pragma unroll
+            for (int j = 0; j < KPL; ++j) {
+                sc[j] = (c0 + lane + 32 * j < nkeys) ? __expf(sc[j] - mx) : 0.f;
+                cl += sc[j];
+            }
+            cl = warp_sum(cl);
+            if constexpr (CHUNKED) {
+                l = l * corr + cl;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) acc[i] *= corr;
+            } else {
+                l = cl;
+            }
+            __syncwarp();
+            if constexpr (DK == 64) {
+                // P.V as a column sum over the staged V rows
+                const uint32_t* svw = reinterpret_cast<const uint32_t*>(sv);
+#pragma unroll
+                for (int j = 0; j < KPL; ++j) {
+                    const int cnt = min(32, nkeys - c0 - 32 * j);
+                    if (cnt <= 0) break;   // warp-uniform
+#pragma unroll 4
+                    for (int t = 0; t < cnt; ++t) {
+                        const int s = t + 32 * j;
+                        const float pw = __shfl_sync(0xffffffffu, sc[j], t);
+                        // dims 2*lane.. live in 16-byte chunk (lane >> 2), word (lane & 3); chunks were rotated by s
+                        const uint32_t vv = svw[(s * 8 + (((lane >> 2) + s) & 7)) * 4 + (lane & 3)];
+                        const float2 vf = unpack_bf16(vv);
+                        acc[0] = fmaf(pw, vf.x, acc[0]);
+                        acc[1] = fmaf(pw, vf.y, acc[1]);
+                    }
+                }
+            } else {
+                // P.V as a column sum: 8-byte half (lane & 1) of 16-byte chunk (lane >> 1); lanes 24..31 repeat lane 23's
+                // reads and store nothing
+                const uint2* svh = reinterpret_cast<const uint2*>(sv);
+                const int ln = min(lane, 23);
+#pragma unroll
+                for (int j = 0; j < KPL; ++j) {
+                    const int cnt = min(32, nkeys - c0 - 32 * j);
+                    if (cnt <= 0) break;   // warp-uniform
+#pragma unroll 4
+                    for (int t = 0; t < cnt; ++t) {
+                        const int s = t + 32 * j;
+                        const float pw = __shfl_sync(0xffffffffu, sc[j], t);
+                        const uint2 vv = svh[(s * CH + rot_chunk<CH>((ln >> 1) + s)) * 2 + (ln & 1)];
+                        const float2 v01 = unpack_bf16(vv.x), v23 = unpack_bf16(vv.y);
+                        acc[0] = fmaf(pw, v01.x, acc[0]);
+                        acc[1] = fmaf(pw, v01.y, acc[1]);
+                        acc[2] = fmaf(pw, v23.x, acc[2]);
+                        acc[3] = fmaf(pw, v23.y, acc[3]);
+                    }
+                }
+            }
+            if constexpr (CHUNKED) __syncwarp();   // the next chunk overwrites the staged V rows
         }
-        l = warp_sum(l);
-        __syncwarp();
+        const float inv = 1.0f / l;
         if constexpr (DK == 64) {
-            // P.V as a column sum over the staged V rows: lane owns output dims 2*lane, 2*lane+1
-            const uint32_t* svw = reinterpret_cast<const uint32_t*>(sv);
-            float ax = 0.f, ay = 0.f;
-#pragma unroll
-            for (int j = 0; j < KPL; ++j) {
-                const int cnt = min(32, nkeys - 32 * j);
-                if (cnt <= 0) break;   // warp-uniform
-#pragma unroll 4
-                for (int t = 0; t < cnt; ++t) {
-                    const int s = t + 32 * j;
-                    const float pw = __shfl_sync(0xffffffffu, sc[j], t);
-                    // dims 2*lane.. live in 16-byte chunk (lane >> 2), word (lane & 3); chunks were rotated by s
-                    const uint32_t vv = svw[(s * 8 + (((lane >> 2) + s) & 7)) * 4 + (lane & 3)];
-                    const float2 vf = unpack_bf16(vv);
-                    ax = fmaf(pw, vf.x, ax);
-                    ay = fmaf(pw, vf.y, ay);
-                }
-            }
-            const float inv = 1.0f / l;
-            *reinterpret_cast<uint32_t*>(out + (size_t)n * d + h * 64 + 2 * lane) = pack_bf16(ax * inv, ay * inv);
+            *reinterpret_cast<uint32_t*>(out + (size_t)n * d + h * 64 + 2 * lane) = pack_bf16(acc[0] * inv, acc[1] * inv);
         } else {
-            // P.V as a column sum: lanes 0..23 own 4 output dims each, 4*lane .. 4*lane+3 = 8-byte half (lane & 1) of
-            // 16-byte chunk (lane >> 1); lanes 24..31 repeat lane 23's reads and store nothing
-            const uint2* svh = reinterpret_cast<const uint2*>(sv);
-            const int ln = min(lane, 23);
-            float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-            for (int j = 0; j < KPL; ++j) {
-                const int cnt = min(32, nkeys - 32 * j);
-                if (cnt <= 0) break;   // warp-uniform
-#pragma unroll 4
-                for (int t = 0; t < cnt; ++t) {
-                    const int s = t + 32 * j;
-                    const float pw = __shfl_sync(0xffffffffu, sc[j], t);
-                    const uint2 vv = svh[(s * CH + rot_chunk<CH>((ln >> 1) + s)) * 2 + (ln & 1)];
-                    const float2 v01 = unpack_bf16(vv.x), v23 = unpack_bf16(vv.y);
-                    a0 = fmaf(pw, v01.x, a0);
-                    a1 = fmaf(pw, v01.y, a1);
-                    a2 = fmaf(pw, v23.x, a2);
-                    a3 = fmaf(pw, v23.y, a3);
-                }
-            }
-            const float inv = 1.0f / l;
             if (lane < 24)
                 *reinterpret_cast<uint2*>(out + (size_t)n * d + h * DK + 4 * lane) =
-                    make_uint2(pack_bf16(a0 * inv, a1 * inv), pack_bf16(a2 * inv, a3 * inv));
+                    make_uint2(pack_bf16(acc[0] * inv, acc[1] * inv), pack_bf16(acc[2] * inv, acc[3] * inv));
         }
         __syncwarp();
     }
@@ -527,17 +553,22 @@ template <int DK>
 static const char* decode_self_attn_launch_dk(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
                                               const int* step_ptr, bf16* out, int N, int H, int Lmax) {
     const int warps = H < 4 ? H : 4;
-    // V staging sized by the longest prefix this search can reach (not the 128-key maximum): at max_len 60 this halves the
+    // V staging sized by the longest prefix this search can reach, up to one 128-key chunk: at max_len 60 this halves the
     // shared memory per CTA and doubles the resident CTAs of this latency-bound kernel (less SM-time per decode step)
-    const int keys_pad = (Lmax + 31) / 32 * 32;
+    const bool chunked = Lmax > 128;
+    const int keys_pad = chunked ? 128 : (Lmax + 31) / 32 * 32;
     const size_t smem = (size_t)warps * keys_pad * DK * 2 + (size_t)warps * DK * sizeof(float);   // V rows | q per warp
-    return launch<decode_self_attn_kernel<DK>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax,
-                                               DK == 64 ? 0.125f : 1.0f / sqrtf((float)DK), keys_pad);
+    const float scale = DK == 64 ? 0.125f : 1.0f / sqrtf((float)DK);
+    if (chunked)
+        return launch<decode_self_attn_kernel<DK, true>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H,
+                                                         Lmax, scale, keys_pad);
+    return launch<decode_self_attn_kernel<DK, false>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H,
+                                                      Lmax, scale, keys_pad);
 }
 
 const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
                                     const int* step_ptr, bf16* out, int N, int H, int Lmax, int d_k) {
-    if (Lmax > 128) return "decode_self_attn: at most 128 cached positions (max_len <= 128)";
+    if (Lmax > 1023) return "decode_self_attn: at most 1023 cached positions (max_len <= 1023)";
     if (d_k == 64) return decode_self_attn_launch_dk<64>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax);
     if (d_k == 96) return decode_self_attn_launch_dk<96>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax);
     return "decode_self_attn: head width d_k must be 64 or 96";

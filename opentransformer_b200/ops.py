@@ -380,6 +380,9 @@ def ls_cross_entropy(logits, targets, V, smoothing=0.1, pad_id=0, want_grad=Fals
     return _ls_ce(logits, targets, V, smoothing, pad_id, torch.float32 if want_grad else None)
 
 
+DECODE_MAX_LEN = 1023   # cached positions of otb_decode_self_attn: the longest KV-cached beam search (max_len)
+
+
 def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None):
     """kc/vc bf16 [Lmax, N, d]: the head width d_k = d // H is taken from the cache."""
     d = kc.shape[-1]
@@ -676,10 +679,16 @@ def mixspeech(x, mask, seed, step, scale, lam_out):
     return x_out, m_out
 
 
+CTC_LOSS_MAX_LABELS = 1023   # padded target width of otb_ctc_loss
+
+
 def ctc_loss(logits, B, T, V, in_len, targets, tgt_len, blank=0, want_grad=False, grad_scale=1.0, scale_dev=None):
     """nn.CTCLoss(blank, 'mean', zero_infinity=True) on logits f32 [B*T, ld] (model/ctc.py:48-52).
     -> (loss 0-d, nll f32 [B], dlogits bf16 [B*T, ld] or None).  The gradient is scaled by grad_scale, times the f32 device
-    scalar scale_dev when one is given (read on the device)."""
+    scalar scale_dev when one is given (read on the device).  targets [B, L] takes L <= 1023 (padded width); the scratch
+    is f32 [B, T, 2 L + 1] (262 MB at B 32, T 1000, L 1023)."""
+    if targets.shape[1] > CTC_LOSS_MAX_LABELS:
+        raise ValueError(f'ctc_loss: targets are {targets.shape[1]} labels wide; at most {CTC_LOSS_MAX_LABELS} are supported')
     _need(logits, torch.float32, 'logits'); _need(in_len, torch.int32, 'in_len'); _need(tgt_len, torch.int32, 'tgt_len')
     if scale_dev is not None:
         _need(scale_dev, torch.float32, 'scale_dev')

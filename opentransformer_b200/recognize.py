@@ -163,6 +163,12 @@ def check_lm_rescoring(who, lm, vocab_size):
         raise ValueError(f'{who}: the LM has {lm.vocab_size} tokens and the model {vocab_size}: rescoring needs one vocabulary')
 
 
+def check_max_len(who, max_len):
+    """The KV-cached search takes max_len <= 1023 (otb_decode_self_attn); past 128 it runs on the per-step graph path."""
+    if max_len > ops.DECODE_MAX_LEN:
+        raise ValueError(f'{who}: max_len must be at most {ops.DECODE_MAX_LEN}, got {max_len}')
+
+
 def ctc_decode(logits, lengths, B, T2, V, blank, mode, beam_width):
     """CTC decoding of a CTC head's logits f32 [B*T', ld] (CTCRecognizer; SpeechToTextRecognizer's first pass under
     apply_rescoring): otb_ctc_frame_topk, then the greedy collapse (otb_ctc_greedy, mode 'greedy') or the prefix beam search
@@ -191,6 +197,7 @@ class BeamDecoder:
     """
 
     def __init__(self, decoder, batch, beam, T, max_len, device, use_graph=True, persistent=False, keep_logp=None, ctc=None):
+        check_max_len('BeamDecoder', max_len)
         self.dec = decoder
         self.B, self.beam, self.T, self.Lmax = batch, beam, T, max_len
         self.N = batch * beam
@@ -399,6 +406,7 @@ class SpeechToTextRecognizer(Recognizer):
 
         max_decoders: at most this many BeamDecoders (one per batch geometry: batch, encoder frames; each owns its KV caches
         and search buffers) are kept, least recently used first out; None keeps one per geometry seen."""
+        check_max_len('SpeechToTextRecognizer', max_len)
         has_head = getattr(model, 'ctc_weight', 0.0) > 0.0
         if apply_rescoring and not has_head:
             raise ValueError('SpeechToTextRecognizer: apply_rescoring needs the joint-CTC head: this model has ctc_weight 0')
