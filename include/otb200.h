@@ -322,6 +322,14 @@ int otb_adam_step_sched(float* p, const float* g, float* m, float* v, long long 
 int otb_mixspeech(const float* x, const uint8_t* mask, int B, int T, int F, const int32_t* seed, const int32_t* step, float scale,
                   float* lam_out, float* x_out, uint8_t* mask_out, void* stream);
 
+/* Low-frame-rate frame stacking (frontend/concat.py:11-56, the concat front ends): x f32 [B, T, F] -> out bf16 [B*T2, ldo],
+ * row b*T2 + i = the n frames x[b, i*s .. i*s + n - 1] flattened frame-major (column j*F + f, nn.Unfold's order), frames at
+ * or past T read as zero.  Columns [0, W) are written, W = n*F rounded up to 8; columns n*F .. W - 1 are zero and columns
+ * from W to ldo are not touched (ldo >= W, a multiple of 8; out 16-byte aligned).  With table f32 [T2, n*F] each of the
+ * n*F columns of row i becomes y * alpha + table[i] (two separately rounded fp32 operations), else y * alpha. */
+int otb_frame_stack(const float* x, int B, int T, int F, int n, int s, int T2, void* out, int ldo, float alpha, const float* table,
+                    void* stream);
+
 /* ---- Recurrent language model (model/lm.py:31-90, rnnlm.yaml): nn.LSTM layers, gates ordered i, f, g, o.  Sequences are
  * time-major (row t*B + b, as nn.LSTM without batch_first).  The input projection gx f32 [L*B, 4H] = x W_ih^T + b_ih + b_hh
  * is otb_linear in front; these run the recurrence as persistent cooperative kernels (CTA j keeps the W_hh slice of its

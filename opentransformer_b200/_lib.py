@@ -91,6 +91,7 @@ _SIGS = {
     'otb_adam_step_sched': (c_int, [_P, _P, _P, _P, c_int64, _P, c_float, c_float, c_float, c_float, c_float, c_float, c_float,
                                     c_float, c_float, _P, _P, c_float, _P, _P, _P]),
     'otb_mixspeech': (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_float, _P, _P, _P, _P]),
+    'otb_frame_stack': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_float, _P, _P]),
     'otb_fbank': (c_int, [_P, c_int, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
     'otb_utt_cmvn': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P]),
     'otb_ctc_loss': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_int, c_float, _P,

@@ -475,6 +475,12 @@ int otb_mixspeech(const float* x, const uint8_t* mask, int B, int T, int F, cons
     RET("otb_mixspeech", mixspeech_launch(ST(stream), x, mask, B, T, F, seed, step, scale, lam_out, x_out, mask_out));
 }
 
+int otb_frame_stack(const float* x, int B, int T, int F, int n, int s, int T2, void* out, int ldo, float alpha, const float* table,
+                    void* stream) {
+    if (!x || !out) return fail("otb_frame_stack", "null operand");
+    RET("otb_frame_stack", frame_stack_launch(ST(stream), x, B, T, F, n, s, T2, reinterpret_cast<bf16*>(out), ldo, alpha, table));
+}
+
 int otb_fbank(const float* wave, int ld_wave, const int32_t* n_samples, int B, const float* window, const float* bank,
               const int32_t* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift, float preemph, void* stream) {
     if (!wave || !n_samples || !window || !bank || !bank_range || !out) return fail("otb_fbank", "null operand");

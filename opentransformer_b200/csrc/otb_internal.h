@@ -131,6 +131,8 @@ const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* 
                               const uint8_t* noise_mask);
 const char* mixspeech_launch(cudaStream_t st, const float* x, const uint8_t* mask, int B, int T, int F, const int* seed, const int* step,
                              float scale, float* lam_out, float* x_out, uint8_t* mask_out);
+const char* frame_stack_launch(cudaStream_t st, const float* x, int B, int T, int F, int n, int s, int T2, bf16* out, int ldo,
+                               float alpha, const float* table);
 
 struct BeamState {
     int* tok_hist;

@@ -10,9 +10,10 @@ import torch.nn as nn
 
 from . import ops
 from . import train
-from .modules import ConformerEncoder, ConvFrontEnd, TransformerDecoder, TransformerEncoder, _lengths
+from .modules import (ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder,
+                      TransformerEncoder, _lengths)
 
-BuildFrontEnd = {'conv': ConvFrontEnd}
+BuildFrontEnd = {'concat': ConcatFeatureFrontEnd, 'concat-with-linear': ConcatWithLinearFrontEnd, 'conv': ConvFrontEnd}
 BuildEncoder = {'transformer': TransformerEncoder, 'conformer': ConformerEncoder}
 BuildDecoder = {'transformer': TransformerDecoder}
 
@@ -25,12 +26,14 @@ def ctc_align_logits(logits, lengths, B, T2, V, tokens, n_tokens, blank):
     return ops.ctc_align(lp, lengths, tokens, n_tokens, blank=blank)
 
 
-def encoder_frames_to_input(spans, frame_shift=None):
+def encoder_frames_to_input(spans, frame_shift=None, frontend=None):
     """Spans [start, end) in encoder frames (CTCModel.align, SpeechToText.align, CTCRecognizer.recognize_spans) -> spans in
-    input (fbank) frames, [4 start, 4 (end - 1) + 7): the front end's two 3x3 stride-2 convolutions, which do not pad in
-    time, make encoder frame t see input frames [4t, 4t + 7).  With frame_shift (seconds between input frames, e.g. 0.01)
-    the result is in seconds, float64.  Entries of -1 (no span) stay -1."""
-    out = torch.stack((4 * spans[..., 0], 4 * spans[..., 1] + 3), dim=-1)
+    input (fbank) frames, [s start, s (end - 1) + w), where encoder frame t sees input frames [s t, s t + w): the front
+    end's input_window() (s, w) -- (4, 7) for the conv front end, whose two 3x3 stride-2 convolutions do not pad in time,
+    and (stride, n) for the concat front ends.  Without a front end the conv front end's window is used.  With frame_shift
+    (seconds between input frames, e.g. 0.01) the result is in seconds, float64.  Entries of -1 (no span) stay -1."""
+    s, w = frontend.input_window() if frontend is not None else (4, 7)
+    out = torch.stack((s * spans[..., 0], s * (spans[..., 1] - 1) + w), dim=-1)
     if frame_shift is not None:
         out = out.double() * frame_shift
     return torch.where(spans < 0, -1, out)
@@ -84,7 +87,7 @@ class SpeechToText(nn.Module):
         each encoder block's attention weights f32 [B, H, T', T'] are appended to it."""
         fe, enc = self.frontend, self.encoder
         B, T, _ = inputs.shape
-        _, _, T2, _ = ops.conv_geometry(T, fe.input_size)
+        T2 = fe.output_length(T)
         lengths = _lengths(fe.output_mask(mask))
         if enc.fuse_abs_posenc():
             scale, table = enc.pos_emb.scale_and_table(T2, inputs.device)
@@ -172,7 +175,7 @@ class SpeechToText(nn.Module):
 
 
 class CTCModel(nn.Module):
-    """model/ctc.py:69-131: conv front end + encoder + CTCAssistor, trained with nn.CTCLoss(blank 0, 'mean', zero_infinity)
+    """model/ctc.py:69-131: front end + encoder + CTCAssistor, trained with nn.CTCLoss(blank 0, 'mean', zero_infinity)
     on truth[:, 1:-1] (no <S/E>) with targets_length - 1 labels.  Submodules `frontend`, `encoder`, `assistor`: the
     reference's state_dict keys and checkpoint sections.
 

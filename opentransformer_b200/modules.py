@@ -4,6 +4,7 @@ Same class names, constructor kwargs (the YAML sub-dicts verbatim) and ``state_d
 shapes as the reference so existing checkpoints load unchanged (SURVEY.md 8b):
 
     ConvFrontEnd        <- otrans/frontend/conv.py:86-159
+    ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd <- otrans/frontend/concat.py:11-56
     TransformerEncoder  <- otrans/encoder/transformer.py:93-134
     TransformerDecoder  <- otrans/decoder/transformer.py:129-208
 
@@ -135,9 +136,18 @@ class ConvFrontEnd(nn.Module):
             pk['ln'] = _ln(self.layer_norm)
         return pk
 
+    def output_length(self, T):
+        """T input frames -> T' output frames."""
+        return ops.conv_geometry(T, self.input_size)[2]
+
+    def input_window(self):
+        """(stride, width): output frame t sees input frames [stride t, stride t + width) (two 3x3 stride-2 convolutions
+        that do not pad in time)."""
+        return 4, 7
+
     def output_mask(self, mask):
         # Conv2dLayer.return_output_mask twice (frontend/conv.py:78-83): mask[:, 1::2][:, :t]
-        _, _, t2, _ = ops.conv_geometry(mask.shape[1], self.input_size)
+        t2 = self.output_length(mask.shape[1])
         t1 = (mask.shape[1] - 3) // 2 + 1
         m = mask[:, 1::2][:, :t1]
         return m[:, 1::2][:, :t2]
@@ -171,6 +181,116 @@ class ConvFrontEnd(nn.Module):
     def inference(self, x, mask, cache):
         y, m = self.forward(x, mask)
         return y, m, cache
+
+
+class ConcatFeatureFrontEnd(nn.Module):
+    """Low-frame-rate input (frontend/concat.py:11-43): output frame i stacks the n = left_frames + 1 + right_frames input
+    frames from i * stride, stride = int(frame_rate / 10), frame-major (feature j * F + f, nn.Unfold's order); the input is
+    zero-padded at the end so that (T_p - n) is a multiple of the stride.  No parameters.
+    forward(x f32 [B,T,F], mask bool [B,T]) -> (f32 [B,T',n F], bool [B,T']).
+
+    What the reference cannot run is refused with ValueError before any device work: right_frames >= stride (its mask
+    and output lengths then differ for every T), frame_rate < 10 (stride 0) and, per call, T_p < n (nn.Unfold fails)."""
+
+    def __init__(self, input_size, left_frames, right_frames, frame_rate=30):
+        super().__init__()
+        self.left_frames, self.right_frames, self.frame_rate = left_frames, right_frames, frame_rate
+        self.stride = int(frame_rate / 10)
+        self.input_size = input_size
+        self.nframes = left_frames + right_frames + 1
+        self.output_size = self.nframes * input_size
+        if frame_rate < 10:
+            raise ValueError(f'concat front end: frame_rate {frame_rate} gives stride int(frame_rate / 10) = 0; it must be >= 10')
+        if left_frames < 0 or right_frames < 0:
+            raise ValueError('concat front end: left_frames and right_frames must be >= 0')
+        if right_frames >= self.stride:
+            raise ValueError(f'concat front end: right_frames {right_frames} must be less than the stride {self.stride}: the '
+                             'reference\'s output mask (mask[:, left_frames::stride]) is longer than its output otherwise')
+
+    def _padded(self, T):
+        """T -> T_p, the length after the reference's zero padding (concat.py:27-30), refused where nn.Unfold fails."""
+        n, s = self.nframes, self.stride
+        Tp = T + (s - (T - n) % s) % s
+        if Tp < n:
+            raise ValueError(f'concat front end: {T} input frames pad to {Tp}, fewer than the {n} frames one output stacks')
+        return Tp
+
+    def output_length(self, T):
+        """T input frames -> T' = (T_p - n) // stride + 1 output frames."""
+        return (self._padded(T) - self.nframes) // self.stride + 1
+
+    def input_window(self):
+        """(stride, width): output frame t stacks input frames [stride t, stride t + n)."""
+        return self.stride, self.nframes
+
+    def output_mask(self, mask):
+        """The input mask padded with False to T_p, then [:, left_frames::stride] (concat.py:29,38)."""
+        B, T = mask.shape
+        pad = self._padded(T) - T
+        if pad:
+            mask = torch.cat([mask, torch.zeros(B, pad, dtype=mask.dtype, device=mask.device)], dim=1)
+        return mask[:, self.left_frames::self.stride]
+
+    def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
+        """x f32 [B,T,F] -> (bf16 [B*T', W], T'), W = n F rounded up to 8 (zero columns past n F).  When posenc_* are
+        given, x*scale+PE is applied in the same pass (otb_frame_stack's epilogue)."""
+        B, T, F = x.shape
+        if F != self.input_size:
+            raise ValueError(f'expected {self.input_size} features, got {F}')
+        T2 = self.output_length(T)
+        alpha = 1.0 if posenc_table is None else posenc_scale
+        return ops.frame_stack(x.contiguous().float(), self.nframes, self.stride, T2, alpha, posenc_table), T2
+
+    def forward(self, x, mask):
+        m = self.output_mask(mask)
+        y, T2 = self.forward_bf16(x)
+        return y[:, :self.output_size].float().view(x.shape[0], T2, self.output_size), m
+
+    def inference(self, x, mask, cache):
+        """(x, mask, cache) -> (y, mask', cache), as ConvFrontEnd.inference; the reference's BaseFrontEnd.inference takes
+        no cache, so its recognizer cannot run these front ends (DESIGN.md 6)."""
+        y, m = self.forward(x, mask)
+        return y, m, cache
+
+
+class ConcatWithLinearFrontEnd(ConcatFeatureFrontEnd):
+    """ConcatFeatureFrontEnd + Linear(n F, output_size) (frontend/concat.py:46-56).  Keys: linear.weight / linear.bias.
+    As in the reference, the attribute output_size stays n F (the stacked width); the Linear's own width is
+    linear.out_features.  The stacked rows (bf16, K padded to a multiple of 8) feed the wgmma GEMM, whose epilogue also
+    applies x*sqrt(d)+PE when the encoder lets it.  dropout > 0 is refused: the reference applies it in eval mode too
+    (F.dropout with training left True, concat.py:55)."""
+
+    def __init__(self, input_size, output_size, left_frames, right_frames, frame_rate=30, dropout=0.0):
+        super().__init__(input_size, left_frames, right_frames, frame_rate)
+        if dropout:
+            raise NotImplementedError('concat-with-linear front end: dropout > 0 (the reference applies it in eval mode too, '
+                                      'concat.py:55); use dropout 0.0')
+        self.linear = nn.Linear(self.output_size, output_size)
+        self.dropout = dropout
+        self._pack = _Packed(self, lambda: (self.pack_linear(_w(self.linear)), _b(self.linear)))
+
+    def pack_linear(self, w):
+        """The Linear weight bf16 [D, n F] as the GEMM takes it: K zero-padded to the stacked rows' width."""
+        K = (self.output_size + 7) // 8 * 8
+        if K == w.shape[1]:
+            return w.contiguous()
+        wp = torch.zeros(w.shape[0], K, dtype=BF16, device=w.device)
+        wp[:, :w.shape[1]] = w
+        return wp
+
+    def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
+        """x f32 [B,T,F] -> (bf16 [B*T', D], T').  When posenc_* are given, x*scale+PE is fused into the Linear epilogue."""
+        _no_train(self)
+        stack, T2 = super().forward_bf16(x)
+        w, b = self._pack.get()
+        if posenc_table is not None:
+            return ops.linear(stack, w, b, EPI_TABLE, alpha=posenc_scale, table=posenc_table, period=T2), T2
+        return ops.linear(stack, w, b, EPI_BIAS), T2
+
+    def forward(self, x, mask):
+        m = self.output_mask(mask)
+        y, T2 = self.forward_bf16(x)
+        return y.float().view(x.shape[0], T2, -1), m
 
 
 # ------------------------------------------------------------------------------------------------

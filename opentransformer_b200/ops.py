@@ -679,6 +679,32 @@ def mixspeech(x, mask, seed, step, scale, lam_out):
     return x_out, m_out
 
 
+def frame_stack(x, n, s, T2, alpha=1.0, table=None, out=None):
+    """Low-frame-rate stacking of the concat front ends (otb_frame_stack): x f32 [B, T, F] -> bf16 [B*T2, W], W = n*F
+    rounded up to 8; row b*T2 + i = x[b, i*s : i*s + n] flattened frame-major, frames at or past T zero, columns n*F .. W - 1
+    zero.  table f32 [T2, n*F] (optional): y * alpha + table[i] on the n*F columns.  out: a bf16 [B*T2, >= W] matrix with
+    unit column stride; its columns past W are left as they are."""
+    _need(x, torch.float32, 'x')
+    if x.dim() != 3:
+        raise ValueError(f'frame_stack: x must be [B, T, F], got {tuple(x.shape)}')
+    B, T, F = x.shape
+    W = (n * F + 7) // 8 * 8
+    if table is not None:
+        _need(table, torch.float32, 'table')
+        if tuple(table.shape) != (T2, n * F):
+            raise ValueError(f'frame_stack: table must be [{T2}, {n * F}], got {tuple(table.shape)}')
+    if out is None:
+        out = torch.empty(B * T2, W, dtype=BF16, device=x.device)
+    else:
+        _mat(out, 'out')
+        if out.shape[0] != B * T2 or out.shape[1] < W:
+            raise ValueError(f'frame_stack: out must be [{B * T2}, >= {W}], got {tuple(out.shape)}')
+    check(_lib.lib().otb_frame_stack(_p(x), B, T, F, n, s, T2, _p(out), out.stride(0), float(alpha), _p(table), _stream()),
+          'otb_frame_stack')
+    _count()
+    return out
+
+
 CTC_LOSS_MAX_LABELS = 1023   # padded target width of otb_ctc_loss
 
 

@@ -44,7 +44,8 @@ import torch
 from . import ops
 from . import modules
 from .dp import allreduce_mean_, broadcast_from_first_
-from .modules import ConformerEncoder, TransformerDecoder, TransformerEncoder, ConvFrontEnd, _lengths
+from .modules import (ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder,
+                      TransformerEncoder, _lengths)
 from .ops import BF16, EPI_BIAS, EPI_RESID, EPI_TABLE, EPI_RELU
 
 
@@ -129,22 +130,23 @@ class EncoderPack(LayerPack):
         super().__init__(model, bf16_of)
         fe, enc, dec = model.frontend, model.encoder, getattr(model, 'decoder', None)
         self.conformer = isinstance(enc, ConformerEncoder)
-        if not (isinstance(fe, ConvFrontEnd) and isinstance(enc, (TransformerEncoder, ConformerEncoder))
+        if not (isinstance(fe, (ConvFrontEnd, ConcatFeatureFrontEnd)) and isinstance(enc, (TransformerEncoder, ConformerEncoder))
                 and (dec is None or isinstance(dec, TransformerDecoder))):
-            raise NotImplementedError('training path: conv front end + Transformer or Conformer encoder'
+            raise NotImplementedError('training path: conv or concat front end + Transformer or Conformer encoder'
                                       + (' + Transformer decoder' if dec is not None else '') + ' only')
         if not self.conformer and enc.relative_positional:
             raise NotImplementedError('training path: the Transformer encoder with absolute positions only')
         stacks = [('encoder', enc)] + ([('decoder', dec)] if dec is not None else [])
         for name, stack in stacks:
             check_heads(name, stack.d_model, stack.blocks)
-        C1 = fe.conv1.conv_layer.out_channels
-        if (C1 + 63) // 64 * 64 > 256:       # the conv1 weight gradient (otb_conv1_wgrad) runs one channel per thread
-            raise NotImplementedError(f'training path: mid_channel {C1} pads to {(C1 + 63) // 64 * 64} channels; the conv1 weight '
-                                      'gradient takes at most 256')
+        if isinstance(fe, ConvFrontEnd):
+            C1 = fe.conv1.conv_layer.out_channels
+            if (C1 + 63) // 64 * 64 > 256:       # the conv1 weight gradient (otb_conv1_wgrad) runs one channel per thread
+                raise NotImplementedError(f'training path: mid_channel {C1} pads to {(C1 + 63) // 64 * 64} channels; the conv1 '
+                                          'weight gradient takes at most 256')
         if self.conformer:
             _check_conformer(enc)
-        if fe.front_end_layer_norm or any(stack.pos_emb.scale_learnable for _, stack in stacks):
+        if getattr(fe, 'front_end_layer_norm', False) or any(stack.pos_emb.scale_learnable for _, stack in stacks):
             raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale (pos_dropout > 0)')
         self.rates = {name: check_blocks(stack.blocks) for name, stack in stacks}
         self.fe = self._frontend(fe)
@@ -154,6 +156,12 @@ class EncoderPack(LayerPack):
         self.enc_norm = self._ln(enc.norm) if self.enc_pre else None
 
     def _frontend(self, fe):
+        """The front end's operands: the conv front end's packed weights and their transposes; concat-with-linear's
+        Linear (K padded as the stacked rows); nothing for concat."""
+        if isinstance(fe, ConcatWithLinearFrontEnd):
+            return {'w': fe.pack_linear(self.w(fe.linear.weight)), 'b': _f(fe.linear.bias)}
+        if isinstance(fe, ConcatFeatureFrontEnd):
+            return {}
         pk = dict(fe._build_pack())
         pk['w2_t'] = pk['w2'].t().contiguous()           # [9*C1p, C2]
         pk['wo_t'] = pk['wo'].t().contiguous()           # [F2*C2, D]
@@ -542,6 +550,8 @@ def embedding_bwd(tok, dx, emb, scale, g, name):
     ops.embed_bwd(tok, dx, g[name], scale)
 
 
+# h1, h2: the conv front end's activations (h2 the input of its Linear); for concat-with-linear h2 holds the stacked rows,
+# the input of its Linear, and h1 is None; for concat both are None
 _EncTrace = namedtuple('_EncTrace', 'x_in h1 h2 tape pe scale lengths enc_last drops B T F T2 F2')
 
 
@@ -554,17 +564,28 @@ def _encoder_fwd(model, pk, inputs, mask, drop_seed):
     B, T, F = inputs.shape
     H = enc.blocks[0].n_heads
     x_in = inputs.contiguous().float()
-    _, _, T2, F2 = ops.conv_geometry(T, F)
+    T2 = fe.output_length(T)
     lengths = _lengths(fe.output_mask(mask))
     fpk = pk.fe
-    h1 = ops.conv1_relu(x_in, fpk['w1'], fpk['b1'])
-    h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F)                       # [B*T2, F2*C2]
-    scale = None
+    scale, table = None, None
     if enc.fuse_abs_posenc():
         scale, table = enc.pos_emb.scale_and_table(T2, dev)
-        x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_TABLE, alpha=scale, table=table, period=T2)
-    else:               # rel-pos encoders take the front end's output as is (encoder/conformer.py:141-149)
-        x = ops.linear(h2, fpk['wo'], fpk['bo'], EPI_BIAS)
+    # rel-pos encoders take the front end's output as is (encoder/conformer.py:141-149)
+    h1, h2, F2 = None, None, None
+    if isinstance(fe, ConvFrontEnd):
+        F2 = ops.conv_geometry(T, F)[3]
+        h1 = ops.conv1_relu(x_in, fpk['w1'], fpk['b1'])
+        h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F)                   # [B*T2, F2*C2]
+        lin = (fpk['wo'], fpk['bo'])
+    elif isinstance(fe, ConcatWithLinearFrontEnd):
+        h2 = ops.frame_stack(x_in, fe.nframes, fe.stride, T2)                     # [B*T2, n F rounded up to 8]
+        lin = (fpk['w'], fpk['b'])
+    if h2 is None:      # concat: the stacked frames are the encoder's input
+        x = ops.frame_stack(x_in, fe.nframes, fe.stride, T2, 1.0 if scale is None else scale, table)
+    elif scale is not None:
+        x = ops.linear(h2, *lin, EPI_TABLE, alpha=scale, table=table, period=T2)
+    else:
+        x = ops.linear(h2, *lin, EPI_BIAS)
     ns = _enc_sites(enc)
     e_drop = [(r, drop_seed, ENC_SITE + ns * i) for i, r in enumerate(pk.rates['encoder'])]
     enc_tape = []
@@ -590,7 +611,6 @@ def _encoder_bwd(model, pk, tr, dx, g):
     B, T, F, T2, F2 = tr.B, tr.T, tr.F, tr.T2, tr.F2
     H = enc.blocks[0].n_heads
     fpk = pk.fe
-    C1p, C2 = fpk['C1p'], fpk['w2'].shape[0]
     if pk.enc_pre:
         dx = _ln_bwd(dx, tr.enc_last, pk.enc_norm, g)
     for i in reversed(range(len(pk.enc))):
@@ -600,8 +620,16 @@ def _encoder_bwd(model, pk, tr, dx, g):
             dx = enc_layer_bwd(pk.enc[i], tr.tape[i], dx, pk.enc_pre, g, B, H, T2, tr.lengths, tr.drops[i])
 
     # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE (abs-pos; rel-pos: x = h2 Wo^T + bo) -> conv2 (implicit-GEMM forward,
-    # im2col GEMMs backward) -> conv1
+    # im2col GEMMs backward) -> conv1.  The concat front ends stack without gradient (concat.py:35-37): concat-with-linear
+    # stops at its Linear's parameters, concat at the encoder's input.
     h1, h2 = tr.h1, tr.h2
+    if isinstance(fe, ConcatFeatureFrontEnd):
+        if isinstance(fe, ConcatWithLinearFrontEnd):
+            dyl = ops.scale_add_table(dx, tr.scale) if tr.scale is not None else dx
+            g.put('frontend.linear.weight', ops.linear_wgrad(dyl, h2)[:, :fe.output_size])   # the padding columns cut off
+            g['frontend.linear.bias'] = ops.colsum(dyl, out=g.out('frontend.linear.bias'), accumulate=acc)
+        return
+    C1p, C2 = fpk['C1p'], fpk['w2'].shape[0]
     dyl = ops.scale_add_table(dx, tr.scale) if tr.scale is not None else dx      # d(h2 Wo^T + bo) = sqrt(d) * dx
     D_out = fe.output_size
     dwo = ops.linear_wgrad(dyl, h2)                                               # [D, F2*C2], feature index f*C2 + c
