@@ -26,7 +26,24 @@ import torch.nn as nn
 
 from . import ops
 from . import train
-from .modules import BF16, PositionalEncoding, TransformerEncoderLayer, _Packed, _b, _no_train, _w
+from .modules import BF16, PositionalEncoding, SelfAttnCache, TransformerEncoderLayer, _Packed, _b, _no_train, _w
+
+
+class LMCache(SelfAttnCache):
+    """The incremental state of the Transformer LM that the reference stubbed out (recognize/speech2text.py:142-143 leaves
+    the reorder of cache['lm'] commented out), as the `cache` of ``TransformerLanguageModel.predict(targets, True, cache)``:
+    the self-attention K/V of every position each block has seen [block, position, row, d_model] (SelfAttnCache).  One
+    call consumes one new token per row; ``reorder(parent_rows)`` follows beam pruning without moving K/V rows.
+
+    Build it with ``TransformerLanguageModel.init_cache``."""
+
+    def __init__(self, lm, n_rows, max_len, anc=None, step_ptr=None):
+        if n_rows < 1:
+            raise ValueError(f'LMCache: n_rows must be >= 1, got {n_rows}')
+        if not 1 <= max_len <= ops.DECODE_MAX_LEN:
+            raise ValueError(f'LMCache: max_len must be in [1, {ops.DECODE_MAX_LEN}], got {max_len}')
+        super().__init__('LM', lm._pack.get(), lm.num_blocks, n_rows, lm.d_model, max_len, lm.embedding.weight.device, anc,
+                         step_ptr)
 
 
 class TransformerLanguageModel(nn.Module):
@@ -39,6 +56,7 @@ class TransformerLanguageModel(nn.Module):
         self.vocab_size = params['vocab_size']
         self.num_blocks = params['num_blocks']
         self.d_model = params['d_model']
+        self.n_heads = params['n_heads']
         self.embedding = nn.Embedding(self.vocab_size, self.d_model)
         self.pos_embedding = PositionalEncoding(self.d_model, 0.0)
         self.blocks = nn.ModuleList([
@@ -72,8 +90,42 @@ class TransformerLanguageModel(nn.Module):
             x = blk.run(x, p, N, L, None, causal=True)
         return ops.linear(x, pk['wout'], pk['bout'], ops.EPI_BIAS, out_f32=True, n_out=self.ld_logits)
 
-    def predict(self, targets, last_frame=True):
-        """model/lm.py:143-163: log-probs [N,1,V] of the last position, or [N,L,V] of all positions."""
+    def init_cache(self, n_rows, max_len):
+        """KV cache for ``predict(targets, True, cache)`` over n_rows sequences of at most max_len positions (LMCache)."""
+        _no_train(self)
+        return LMCache(self, n_rows, max_len)
+
+    def cached_log_probs(self, pk, tok, c, out=None):
+        """The newest position of every row through the blocks against the KV cache c (LMCache): tok i64 [N] at the position
+        c.step_dev names -> log-probs f32 [N, V].  Each block's K/V of that position are written into the cache; earlier
+        positions are read through c.anc."""
+        N, H = c.N, self.n_heads
+        x = ops.embed_posenc(tok, pk['emb'], c.table, N, self.d_model, step_ptr=c.step_dev)
+        for l, (blk, p) in enumerate(zip(self.blocks, pk['blocks'])):
+            x = blk.run(x, p, N, 1, None, context=lambda qkv, l=l: ops.decode_self_attn(qkv, c.kc[l], c.vc[l], c.anc,
+                                                                                        c.step_dev, N, H, c.Lmax))
+        logits = ops.linear(x, pk['wout'], pk['bout'], ops.EPI_BIAS, out_f32=True, n_out=self.ld_logits)
+        return ops.log_softmax(logits, self.vocab_size, out=out)
+
+    def predict(self, targets, last_frame=True, cache=None):
+        """model/lm.py:143-163: log-probs [N,1,V] of the last position, or [N,L,V] of all positions.
+
+        cache None (the reference's only mode): the whole prefix is recomputed.  cache = LMCache (``init_cache``): targets
+        is [N, cache.step + 1] and only targets[:, -1] runs through the blocks, at position cache.step, against the cached
+        K/V of the earlier positions; the caller reorders the cache after beam pruning
+        (SpeechToTextRecognizer.decode_step does)."""
+        if cache is not None:
+            if not isinstance(cache, LMCache):
+                raise TypeError(f'predict: cache must be an LMCache (init_cache) or None, got {type(cache).__name__}')
+            if not last_frame:
+                raise ValueError('predict with an LMCache returns the newest position only: last_frame must be True')
+            _no_train(self)
+            pk = self._pack.get()
+            cache.begin_step(pk, targets)
+            with torch.no_grad():
+                lp = self.cached_log_probs(pk, targets[:, -1].contiguous(), cache)
+            cache.step += 1
+            return lp.unsqueeze(1)
         N, L = targets.shape
         with torch.no_grad():
             logits = self.logits_bf16(targets).view(N, L, -1)
@@ -219,10 +271,10 @@ class RecurrentLanguageModel(nn.Module):
             ops.lstm_config(self.hidden_size, prop.multi_processor_count, prop.shared_memory_per_block_optin)
             self._checked = device
 
-    def _run(self, tok, pk, hidden=None, drop_seed=None, record=False):
+    def _run(self, tok, pk, hidden=None, drop_seed=None, record=False, barrier=None):
         """tok i64 [L, N] (time-major) -> (output of the top layer bf16 [L*N, H], h_n, c_n f32 [layers, N, H], tape).
         hidden: (h0, c0) f32 [layers, N, H] or None; drop_seed: the dropout seed (training), else no dropout; record: keep
-        what the backward reads (per layer: input, gates, c_t, output)."""
+        what the backward reads (per layer: input, gates, c_t, output); barrier: see ops.lstm_fwd."""
         self._check_device(tok.device)
         L, N = tok.shape
         x = ops.embedding(tok.reshape(-1), pk['emb'])
@@ -231,7 +283,7 @@ class RecurrentLanguageModel(nn.Module):
             gx = ops.linear(x, p['ih'].w, p['ih'].b, out_f32=True)
             h0 = hidden[0][k].float().contiguous() if hidden is not None else None
             c0 = hidden[1][k].float().contiguous() if hidden is not None else None
-            y, h_n, c_n, gates, c_all = ops.lstm_fwd(gx, p['w_hh'], L, N, h0, c0, train=record)
+            y, h_n, c_n, gates, c_all = ops.lstm_fwd(gx, p['w_hh'], L, N, h0, c0, train=record, barrier=barrier)
             hs.append(h_n)
             cs.append(c_n)
             if record:

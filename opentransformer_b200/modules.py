@@ -375,11 +375,15 @@ def _proj_resid_ln(ctx, w, b, resid, ln):
     return ops.layernorm(y, *ln) if ln is not None else y
 
 
-def _self_attn(y, resid, p, H, B, T, lengths, causal=False, ln=None, attn_sink=None):
+def _self_attn(y, resid, p, H, B, T, lengths, causal=False, ln=None, attn_sink=None, context=None):
     """resid + output_proj(MHA(y)) (+ LayerNorm): QKV GEMM -> fused attention -> output projection with the residual.
-    attn_sink (a list): the attention weights f32 [B, H, T, T] are appended to it."""
+    attn_sink (a list): the attention weights f32 [B, H, T, T] are appended to it.  context(qkv) -> bf16 [rows, d]: the
+    attention context of a KV-cached step (the newest position of each row against its cached prefix) instead of the
+    attention over the rows of this call."""
     d = y.shape[1]
     qkv = ops.linear(y, p['wqkv'], p['bqkv'])
+    if context is not None:
+        return _proj_resid_ln(context(qkv), p['wo'], p['bo'], resid, ln)
     if attn_sink is not None:
         attn_sink.append(ops.attention_probs(qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d, d_k=d // H))
     ctx = ops.attention(qkv, qkv, qkv, B, H, T, T, kv_len=lengths, causal=causal, q_col0=0, k_col0=d, v_col0=2 * d,
@@ -429,21 +433,22 @@ class TransformerEncoderLayer(nn.Module):
             pk.update({'wqkv': _w(a.qvk_proj), 'bqkv': _b(a.qvk_proj), 'wo': _w(a.output_proj), 'bo': _b(a.output_proj)})
         return pk
 
-    def run(self, x, pk, B, T, lengths, causal=False, pos_bf16=None, attn_sink=None):
+    def run(self, x, pk, B, T, lengths, causal=False, pos_bf16=None, attn_sink=None, context=None):
         """x bf16 [B*T, d] -> bf16 [B*T, d]   (encoder/transformer.py:41-65); causal=True is the tril mask the
-        Transformer LM feeds to the same layer (model/lm.py:14-18,148-151).  attn_sink: see _self_attn."""
+        Transformer LM feeds to the same layer (model/lm.py:14-18,148-151).  attn_sink, context: see _self_attn (the
+        Transformer LM's KV-cached step passes context)."""
         nb = self.normalize_before
         if nb:
             x = ops.layernorm(x, *pk['ln1'])          # residual is taken AFTER the norm (transformer.py:42-44)
         ln = None if nb else pk['ln1']
         if self.relative_positional:
-            if causal:
+            if causal or context is not None:
                 raise NotImplementedError('causal rel-pos attention')
             x = self.slf_attn.run(x, x, pk['rel'], B, T, lengths, pos_bf16, attn_sink)   # x + attention (no output projection)
             if ln is not None:
                 x = ops.layernorm(x, *ln)
         else:
-            x = _self_attn(x, x, pk, self.n_heads, B, T, lengths, causal, ln, attn_sink)
+            x = _self_attn(x, x, pk, self.n_heads, B, T, lengths, causal, ln, attn_sink, context)
         if nb:
             x = ops.layernorm(x, *pk['ln2'])
         return _ffn(x, pk['ffn'], x, None if nb else pk['ln2'])
@@ -728,46 +733,40 @@ class ConformerEncoder(nn.Module):
 # ------------------------------------------------------------------------------------------------
 # decoder
 # ------------------------------------------------------------------------------------------------
-class DecoderCache:
-    """The decoder cache the reference stubbed out (decoder/transformer.py:92-126,188-203; README TODO), as the opaque
-    `cache` object of ``TransformerDecoder.inference(preds, memory, memory_mask, cache)``:
+class SelfAttnCache:
+    """The self-attention half of the KV caches of the incremental decoder (DecoderCache) and the Transformer LM (LMCache):
+    K/V of every decoded position [layer, position, row, d], the ping-pong ancestry table anc [2, N, max_len], the device
+    step counter and the positional table.  Beam pruning never moves K/V rows, it rewrites a 4-byte ancestry entry per
+    (row, position): ``reorder(parent_rows)``.  The cache is tied to the weight pack its K/V were computed with.
 
-      * cross-attention K/V of the memory, projected ONCE (the reference re-runs vk_proj on the beam-tiled memory at every
-        step, attention.py:129).  When the memory rows are the beam-tiled copies of `batch` utterances
-        (recognize/speech2text.py:51-52) pass ``beam`` so that each utterance is projected once and shared by its beams;
-      * self-attention K/V of every decoded position [layer, position, row, d]; beam pruning never moves K/V rows, it
-        rewrites a 4-byte ancestry entry per (row, position) -- ``reorder(parent_rows)`` is what `decode_step` calls where
-        the reference intended reselect_hidden* (recognize/speech2text.py:195-218).
+    anc / step_ptr: a search that keeps its own ancestry and step counter (recognize.BeamDecoder's BeamState) passes them
+    in, and its beam kernel reorders the cache; such a cache is never reordered from the host."""
 
-    Build it with ``TransformerDecoder.init_cache``.  One `inference` call consumes exactly one new token per row."""
+    def __init__(self, what, pk, n_layers, n_rows, d, max_len, device, anc=None, step_ptr=None):
+        self._what, self._pk = what, pk
+        self.N, self.Lmax, self.step = n_rows, max_len, 0
+        self.kc = torch.zeros(n_layers, max_len, n_rows, d, dtype=BF16, device=device)
+        self.vc = torch.zeros(n_layers, max_len, n_rows, d, dtype=BF16, device=device)
+        self.anc = torch.zeros(2, n_rows, max_len, dtype=torch.int32, device=device) if anc is None else anc
+        self.step_dev = torch.zeros(1, dtype=torch.int32, device=device) if step_ptr is None else step_ptr
+        self.table = ops.sinusoid_table(max_len + 1, d, 0, device)
 
-    def __init__(self, decoder, memory, memory_mask, max_len, beam=1):
-        n, T, D = memory.shape
-        if n % beam:
-            raise ValueError('DecoderCache: memory rows must be a multiple of beam')
-        dev = memory.device
-        self.N, self.T, self.beam, self.Lmax, self.step = n, T, beam, max_len, 0
-        self.batch = n // beam
-        nl, d = len(decoder.blocks), decoder.d_model
-        pk = decoder.packed()
-        self._pk = pk            # the cache is tied to this weight pack (K/V were projected with it)
-        mem = memory.contiguous().view(self.batch, beam, T, D)[:, 0]                 # one copy per utterance
-        msk = memory_mask.contiguous().view(self.batch, beam, T)[:, 0]
-        mem_bf16 = ops.scale_add_table(mem.contiguous().view(self.batch * T, D).float())
-        self.mem_len = _lengths(msk)
-        self.kvx = torch.empty(nl, self.batch * T, 2 * d, dtype=BF16, device=dev)
-        for l, p in enumerate(pk['blocks']):
-            ops.linear(mem_bf16, p['wkv'], p['bkv'], out=self.kvx[l])
-        self.kc = torch.zeros(nl, max_len, n, d, dtype=BF16, device=dev)
-        self.vc = torch.zeros(nl, max_len, n, d, dtype=BF16, device=dev)
-        self.anc = torch.zeros(2, n, max_len, dtype=torch.int32, device=dev)
-        self.step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.table = ops.sinusoid_table(max_len + 1, d, 0, dev)
+    def begin_step(self, pk, preds):
+        """Refuse, before any device work, an incremental call that does not fit the cache (preds i64 [N, step + 1]: one
+        new token per row and call), then point the device step counter at the new position."""
+        name = type(self).__name__
+        if pk is not self._pk:
+            raise RuntimeError(f'{name} was built with different {self._what} weights (parameters changed since init_cache)')
+        if preds.dim() != 2 or preds.shape[0] != self.N or preds.shape[1] != self.step + 1:
+            raise ValueError(f'cached inference expects preds [N={self.N}, {self.step + 1}] (one new token per call), got {tuple(preds.shape)}')
+        if self.step >= self.Lmax:
+            raise ValueError(f'{name} is full (max_len reached)')
+        self.step_dev.fill_(self.step)
 
     def reorder(self, parent_rows):
         """Row n of the next step continues row parent_rows[n] (i64/i32 [N], global row indices)."""
         if self.step == 0:
-            raise RuntimeError('DecoderCache.reorder before the first inference step')
+            raise RuntimeError(f'{type(self).__name__}.reorder before the first inference step')
         s = self.step - 1                     # the position that was just decoded
         cur, nxt = s & 1, (s & 1) ^ 1
         par = parent_rows.view(-1).long()
@@ -777,6 +776,37 @@ class DecoderCache:
     def advance_without_reorder(self):
         """Greedy / teacher-forced use (no pruning): every row continues itself."""
         self.reorder(torch.arange(self.N, device=self.anc.device))
+
+
+class DecoderCache(SelfAttnCache):
+    """The decoder cache the reference stubbed out (decoder/transformer.py:92-126,188-203; README TODO), as the opaque
+    `cache` object of ``TransformerDecoder.inference(preds, memory, memory_mask, cache)``:
+
+      * cross-attention K/V of the memory, projected ONCE (the reference re-runs vk_proj on the beam-tiled memory at every
+        step, attention.py:129).  When the memory rows are the beam-tiled copies of `batch` utterances
+        (recognize/speech2text.py:51-52) pass ``beam`` so that each utterance is projected once and shared by its beams;
+      * self-attention K/V of every decoded position (SelfAttnCache); ``reorder(parent_rows)`` is what `decode_step` calls
+        where the reference intended reselect_hidden* (recognize/speech2text.py:195-218).
+
+    Build it with ``TransformerDecoder.init_cache``.  One `inference` call consumes exactly one new token per row."""
+
+    def __init__(self, decoder, memory, memory_mask, max_len, beam=1):
+        n, T, D = memory.shape
+        if n % beam:
+            raise ValueError('DecoderCache: memory rows must be a multiple of beam')
+        dev = memory.device
+        nl, d = len(decoder.blocks), decoder.d_model
+        pk = decoder.packed()
+        super().__init__('decoder', pk, nl, n, d, max_len, dev)
+        self.T, self.beam = T, beam
+        self.batch = n // beam
+        mem = memory.contiguous().view(self.batch, beam, T, D)[:, 0]                 # one copy per utterance
+        msk = memory_mask.contiguous().view(self.batch, beam, T)[:, 0]
+        mem_bf16 = ops.scale_add_table(mem.contiguous().view(self.batch * T, D).float())
+        self.mem_len = _lengths(msk)
+        self.kvx = torch.empty(nl, self.batch * T, 2 * d, dtype=BF16, device=dev)
+        for l, p in enumerate(pk['blocks']):
+            ops.linear(mem_bf16, p['wkv'], p['bkv'], out=self.kvx[l])
 
 
 class TransformerDecoderLayer(nn.Module):
@@ -949,15 +979,9 @@ class TransformerDecoder(nn.Module):
     def _inference_cached(self, preds, c):
         _no_train(self)
         pk = self._pack.get()
-        if pk is not c._pk:
-            raise RuntimeError('DecoderCache was built with different decoder weights (parameters changed since init_cache)')
-        if preds.shape[0] != c.N or preds.shape[1] != c.step + 1:
-            raise ValueError(f'cached inference expects preds [N={c.N}, {c.step + 1}] (one new token per call), got {tuple(preds.shape)}')
-        if c.step >= c.Lmax:
-            raise ValueError('DecoderCache is full (max_len reached)')
         if self.pos_emb.scale_learnable:
             raise NotImplementedError('decoder with learnable positional scale')
-        c.step_dev.fill_(c.step)
+        c.begin_step(pk, preds)
         tok = preds[:, -1].contiguous()
         x = ops.embed_posenc(tok, pk['emb'], c.table, c.N, self.d_model, step_ptr=c.step_dev)
         x = self.decode_cached_bf16(pk, x, c.kc, c.vc, c.anc, c.step_dev, c.kvx, c.mem_len, c.beam, c.T)

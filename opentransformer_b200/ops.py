@@ -1048,10 +1048,11 @@ def _lstm_barrier(device):
     return bar
 
 
-def lstm_fwd(gx, w_hh, L, B, h0=None, c0=None, train=False):
+def lstm_fwd(gx, w_hh, L, B, h0=None, c0=None, train=False, barrier=None):
     """One LSTM layer over gx f32 [L*B, 4H] (time-major input projection incl. both biases), w_hh bf16 [4H, H], h0 / c0 f32
     [B, H] or None -> (y bf16 [L*B, H], h_n f32 [B, H], c_n f32 [B, H], gates, c_all); with train the post-activation gates
-    (written over gx) and c_t f32 [L*B, H] for lstm_bwd, else None."""
+    (written over gx) and c_t f32 [L*B, H] for lstm_bwd, else None.  barrier: an i32 [2] zero-initialised grid-barrier
+    counter owned by the caller (a captured CUDA graph must not allocate one), else the current stream's."""
     _need(gx, torch.float32, 'gx'); _need(w_hh, BF16, 'w_hh')
     H = w_hh.shape[1]
     for t, n in ((h0, 'h0'), (c0, 'c0')):
@@ -1064,7 +1065,7 @@ def lstm_fwd(gx, w_hh, L, B, h0=None, c0=None, train=False):
     gates = gx if train else None
     c_all = torch.empty(L * B, H, dtype=torch.float32, device=dev) if train else None
     check(_lib.lib().otb_lstm_fwd(_p(gx), _p(w_hh), _p(h0), _p(c0), _p(y), _p(h_n), _p(c_n), _p(gates), _p(c_all),
-                                  _p(_lstm_barrier(dev)), L, B, H, _stream()), 'otb_lstm_fwd')
+                                  _p(barrier if barrier is not None else _lstm_barrier(dev)), L, B, H, _stream()), 'otb_lstm_fwd')
     _count()
     return y, h_n, c_n, gates, c_all
 

@@ -21,6 +21,7 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
 import torch
 
 from . import ops
+from .lm import LMCache
 from .model import ctc_align_logits
 from .modules import encoder_attn_weights
 
@@ -163,6 +164,15 @@ def check_lm_rescoring(who, lm, vocab_size):
         raise ValueError(f'{who}: the LM has {lm.vocab_size} tokens and the model {vocab_size}: rescoring needs one vocabulary')
 
 
+def check_lm_fusion(who, lm, vocab_size):
+    if getattr(lm, 'model_type', None) not in ('transformer_lm', 'recurrent_lm'):
+        raise NotImplementedError('shallow fusion is implemented for the Transformer and the recurrent LM '
+                                  '(opentransformer_b200.lm)')
+    if lm.vocab_size != vocab_size:
+        raise ValueError(f'{who}: the LM has {lm.vocab_size} tokens and the model {vocab_size}: shallow fusion needs one '
+                         'vocabulary')
+
+
 def check_max_len(who, max_len):
     """The KV-cached search takes max_len <= 1023 (otb_decode_self_attn); past 128 it runs on the per-step graph path."""
     if max_len > ops.DECODE_MAX_LEN:
@@ -194,10 +204,20 @@ class BeamDecoder:
     the head's log-probs, and a step scores each hypothesis' P best tokens with
     (1 - weight) logp_att + weight (psi(g c) - psi(g)) + lm_weight lm before the beam kernel selects among the `beam`
     best of them.  The persistent kernel does not take the term, so it is off then.
+
+    lm = (lm, weight) fuses a language model (speech2text.py:101-105): every step computes its log-probs into lm_logp
+    [N, V] inside the same step (and the same captured graph) before the fused log-softmax/top-k adds weight * lm_logp.
+    The Transformer LM runs its newest position against a KV cache [blocks, max_len, N, d_lm] addressed by the search's own
+    ancestry and step counter, so beam pruning reorders it for free; the recurrent LM reads the newest token from a zero
+    state, as the reference does (cache['lm'] = None at every step).  The persistent kernel does not take an LM, so it is
+    off then.
     """
 
-    def __init__(self, decoder, batch, beam, T, max_len, device, use_graph=True, persistent=False, keep_logp=None, ctc=None):
+    def __init__(self, decoder, batch, beam, T, max_len, device, use_graph=True, persistent=False, keep_logp=None, ctc=None,
+                 lm=None):
         check_max_len('BeamDecoder', max_len)
+        if lm is not None:
+            check_lm_fusion('BeamDecoder', lm[0], decoder.vocab_size)
         self.dec = decoder
         self.B, self.beam, self.T, self.Lmax = batch, beam, T, max_len
         self.N = batch * beam
@@ -217,9 +237,20 @@ class BeamDecoder:
         self.keep_logp = (not use_graph) if keep_logp is None else bool(keep_logp)
         self.use_graph = use_graph
         self.graph = None
-        self._graph_pk = None      # the bf16 weight pack whose device pointers the captured graph bakes in (kept alive with it)
+        self._graph_pk = None      # the bf16 weight packs whose device pointers the captured graph bakes in (kept alive with it)
         self.lm_logp = None
         self.lm_weight = 0.0
+        self.lm = self.lm_cache = self._lstm_bar = None
+        if lm is not None:
+            self.lm, weight = lm
+            self.lm_weight = float(weight)
+            self.lm_logp = torch.zeros(self.N, decoder.vocab_size, dtype=torch.float32, device=device)
+            if self.lm.model_type == 'transformer_lm':
+                self.lm_cache = LMCache(self.lm, self.N, max_len, anc=self.state.anc, step_ptr=self.state.step_ptr)
+            else:
+                self.lm._check_device(device)
+                # the recurrence kernel's grid barrier, allocated here and not inside the capture (one step never syncs on it)
+                self._lstm_bar = torch.zeros(2, dtype=torch.int32, device=device)
         if decoder.pos_emb.scale_learnable:
             raise NotImplementedError('decoder with learnable positional scale')
         self.ctc = self.ctc_head = None
@@ -231,7 +262,7 @@ class BeamDecoder:
         # persistent path: the whole loop in ONE launch (csrc/decode_group.cu: row groups of <= 128 hypotheses x 16 CTAs,
         # wgmma GEMMs, group-local barriers) when the configuration is the shipped one (post-norm GLU decoder, d_model 256,
         # 4 heads, d_ff 2048, <= 256 memory frames); anything else takes the per-step graph.
-        self.persistent = bool(persistent) and self.ctc is None and self.mega_supported()
+        self.persistent = bool(persistent) and self.ctc is None and self.lm is None and self.mega_supported()
         self._mega_model = None
         self._mega_sig = None
         self._ws = None
@@ -292,9 +323,25 @@ class BeamDecoder:
             ops.log_softmax(self.ctc_head.logits_bf16(memory_bf16), self.dec.vocab_size, out=self.ctc.lp)
             self.ctc.init(self.mem_len)
 
+    def _packs(self):
+        return (self.dec.packed(),) if self.lm is None else (self.dec.packed(), self.lm._pack.get())
+
+    def _lm_step(self):
+        """The fused LM's log-probs of every hypothesis' next token -> lm_logp."""
+        lm, st = self.lm, self.state
+        pk = lm._pack.get()
+        if self.lm_cache is not None:
+            lm.cached_log_probs(pk, st.last_tok, self.lm_cache, out=self.lm_logp)
+            return
+        # lm_log_probs' kernels for the RNN LM (predict of the newest token, zero state)
+        x, _, _, _ = lm._run(st.last_tok.view(1, self.N), pk, barrier=self._lstm_bar)
+        ops.log_softmax(lm._logits(x, pk), lm.vocab_size, out=self.lm_logp)
+
     def _step_kernels(self):
         dec, st = self.dec, self.state
         pk = dec.packed()
+        if self.lm is not None:
+            self._lm_step()
         x = ops.embed_posenc(st.last_tok, pk['emb'], self.table, self.N, dec.d_model, step_ptr=st.step_ptr)
         x = dec.decode_cached_bf16(pk, x, self.kc, self.vc, st.anc, st.step_ptr, self.kvx, self.mem_len, self.beam, self.T)
         ops.linear(x, pk['wout'], pk['bout'], out=self.logits)
@@ -314,12 +361,13 @@ class BeamDecoder:
     def step(self):
         if not self.use_graph:
             return self._step_kernels()
-        if self.graph is not None and self._graph_pk is not self.dec.packed():
-            # parameters changed (load_state_dict / optimizer step): the pack was rebuilt at new addresses, the captured
+        packs = self._packs()
+        if self.graph is not None and any(a is not b for a, b in zip(self._graph_pk, packs)):
+            # parameters changed (load_state_dict / optimizer step): a pack was rebuilt at new addresses, the captured
             # kernels would read the old (stale or recycled) weights -- drop the graph and capture again
             self.graph = None
         if self.graph is None:
-            self._graph_pk = self.dec.packed()
+            self._graph_pk = packs
             # warm-up outside capture (lazy func attributes, caches), then restore the state it advanced (the CTC prefix
             # state needs no copy: a step reads the half of its ping-pong that the step counter names and writes the other)
             snap = [t.clone() for t in (self.state.tok_hist, self.state.par_hist, self.state.last_tok,
@@ -343,21 +391,6 @@ class BeamDecoder:
                 t.copy_(c)
         self.graph.replay()
         ops.COUNTERS['launches'] += self.launches_per_step
-
-    def run_with_lm(self, max_steps, lm, lm_weight):
-        """Shallow fusion (speech2text.py:102-105, base.py:26-37): every step the LM scores the prefixes (lm_log_probs: the
-        Transformer LM re-reads them in full, the RNN LM reads the newest token) and lm_weight * log-probs are added inside the
-        fused log-softmax/top-k kernel.  Eager mode: the prefix length is host-side state."""
-        assert not self.use_graph, 'LM fusion runs the decode loop eagerly'
-        self.lm_weight = float(lm_weight)
-        for i in range(max_steps):
-            preds = self.state.reconstruct(i)                       # [N, i+1], column 0 = BOS
-            self.lm_logp = lm_log_probs(lm, preds)
-            self._step_kernels()
-            if int(self._read_ctrl()[1]):
-                break
-        self.lm_logp = None
-        return int(self._read_ctrl()[0])
 
     def _read_ctrl(self):
         """{step, done, ...} of the search state on the host.  The copy lands in pinned memory and the thread SLEEPS on a
@@ -418,6 +451,8 @@ class SpeechToTextRecognizer(Recognizer):
                                       f'1..16, got {beam_width}')
         if apply_lm_rescoring:
             check_lm_rescoring('SpeechToTextRecognizer', lm, model.decoder.vocab_size)
+        elif lm is not None:
+            check_lm_fusion('SpeechToTextRecognizer', lm, model.decoder.vocab_size)
         if not 0.0 <= ctc_weight <= 1.0:
             raise ValueError(f'SpeechToTextRecognizer: ctc_weight must be in [0, 1], got {ctc_weight}')
         if ctc_weight > 0.0 and getattr(model, 'ctc_weight', 0.0) <= 0.0:
@@ -428,9 +463,6 @@ class SpeechToTextRecognizer(Recognizer):
             raise ValueError(f'SpeechToTextRecognizer: ctc_candidates must be in [beam_width = {beam_width}, '
                              f'{ops.CTC_PREFIX_MAX_CANDIDATES}], got {ctc_candidates}')
         super().__init__(model, idx2unit, lm, lm_weight, ngpu)
-        if lm is not None and getattr(lm, 'model_type', None) not in ('transformer_lm', 'recurrent_lm'):
-            raise NotImplementedError('shallow fusion is implemented for the Transformer and the recurrent LM '
-                                      '(opentransformer_b200.lm)')
         self.beam_width, self.max_len, self.nbest = beam_width, max_len, nbest
         self.penalty, self.lamda = penalty, lamda
         self.ctc_weight, self.lm_weight, self.ctc_candidates = ctc_weight, lm_weight, ctc_candidates
@@ -438,7 +470,7 @@ class SpeechToTextRecognizer(Recognizer):
         self.apply_cache = False
         self.use_graph = use_graph
         # None = automatic: the persistent decode kernel (one launch per batch, csrc/decode_group.cu) whenever the decoder,
-        # the batch geometry and the options (no LM fusion) fit it; False forces the per-step CUDA-graph path
+        # the batch geometry and the options (no CTC term, no LM fusion) fit it; False forces the per-step CUDA-graph path
         self.persistent = True if persistent is None else bool(persistent)
         self.apply_rescoring, self.apply_lm_rescoring = bool(apply_rescoring), bool(apply_lm_rescoring)
         self.rescore_weight = float(rescore_weight)
@@ -473,6 +505,7 @@ class SpeechToTextRecognizer(Recognizer):
         n = scores.size(0)
         batch = n // self.beam_width
         dcache = cache.get('decoder') if isinstance(cache, dict) else None
+        lcache = cache.get('lm') if isinstance(cache, dict) else None
         log_probs, dcache, _ = self.decode(preds, memory, memory_mask, dcache)
         st = ops.BeamState(batch, self.beam_width, 1, scores.device)
         st.init()
@@ -480,13 +513,18 @@ class SpeechToTextRecognizer(Recognizer):
         st.flag.copy_(flag.view(-1).to(torch.uint8))
         lm_logp, lm_w = None, 0.0
         if self.lm is not None and self.lm_weight:
-            lm_logp = lm_log_probs(self.lm, preds)
+            if isinstance(lcache, LMCache):
+                lm_logp = self.lm.predict(preds, True, lcache).squeeze(1)
+            else:
+                lm_logp = lm_log_probs(self.lm, preds)
             lm_w = float(self.lm_weight)
         st.step(log_probs.contiguous(), log_probs.shape[-1], lm_logp, lm_w)
         parent = st.par_hist[0].long()
         tok = st.tok_hist[0].long()
         if isinstance(dcache, DecoderCache):
             dcache.reorder(parent)
+        if lm_logp is not None and isinstance(lcache, LMCache):
+            lcache.reorder(parent)
         preds_symbol = torch.cat((preds.index_select(0, parent), tok.view(-1, 1)), dim=1)
         return preds_symbol, cache, st.scores.view(-1, 1).clone(), (tok == EOS).view(-1, 1)
 
@@ -504,16 +542,17 @@ class SpeechToTextRecognizer(Recognizer):
         return out
 
     def _decoder_for(self, B, T2, device):
-        # the CTC weight and candidate count are launch arguments that a captured step bakes in
+        # the CTC weight and candidate count, the fused LM's weights and lm_weight are launch arguments that a captured step
+        # bakes in
         ctc = (self.model.assistor, self.ctc_weight, self.ctc_candidates) if self.ctc_weight > 0.0 else None
-        key = (B, self.beam_width, T2, self.max_len, device.index, ctc[1:] if ctc else None)
+        lm = (self.lm, float(self.lm_weight)) if self._lm_fused() else None
+        key = (B, self.beam_width, T2, self.max_len, device.index, ctc[1:] if ctc else None, lm)
         bd = self._decoders.pop(key, None)
         if bd is None:
             while self.max_decoders is not None and len(self._decoders) >= self.max_decoders:
                 self._decoders.pop(next(iter(self._decoders)))          # the least recently used goes, with its buffers
-            fused = self._lm_fused()
-            bd = BeamDecoder(self.model.decoder, B, self.beam_width, T2, self.max_len, device,
-                             self.use_graph and not fused, persistent=self.persistent and not fused, ctc=ctc)
+            bd = BeamDecoder(self.model.decoder, B, self.beam_width, T2, self.max_len, device, self.use_graph,
+                             persistent=self.persistent, ctc=ctc, lm=lm)
         self._decoders[key] = bd          # (re-)inserted as the most recently used
         return bd
 
@@ -540,10 +579,7 @@ class SpeechToTextRecognizer(Recognizer):
             return (preds, scores, preds.shape[2]), mem, mem_len, None
         bd = self._decoder_for(B, T2, inputs.device)
         bd.setup(mem, mem_len)
-        if self._lm_fused():
-            steps = bd.run_with_lm(self.max_len, self.lm, self.lm_weight)
-        else:
-            steps = bd.run(self.max_len)
+        steps = bd.run(self.max_len)
         if not scorers:
             preds, scores = bd.state.finalize(self.penalty, self.lamda, self.nbest)
             return (preds[:, :, :steps], scores, steps), mem, mem_len, bd

@@ -7,7 +7,7 @@ decoder's <S/E> bias at -1e4 so that the attention search runs all 60 steps, 32 
     otb_ctc_prefix_beam), the decoder scoring (score_bf16), otb_token_logprob, and the rerank (second_pass_rows +
     otb_nbest_rescore);
   - the second pass on fixed synthetic n-bests of 32 and 64 tokens (random weights give the CTC pass arbitrary lengths);
-  - an LM: shallow fusion (the per-step path, which an LM makes eager) against apply_lm_rescoring (persistent first pass,
+  - an LM: shallow fusion (the per-step graph path) against apply_lm_rescoring (persistent first pass,
     the LM over the 10 hypotheses), with the transformer_lm.yaml LM (6 blocks, d_model 256, GLU d_ff 1024) at the model's
     4234-token vocabulary;
   - otb_token_logprob's achieved bandwidth: the bytes of the logits rows it reads (rows with a target) over its time.
@@ -113,7 +113,7 @@ def main():
                 add(f'second_pass_synthetic_{L}_tokens', timed(lambda: second_pass(*rows[:3], rows[3]), a.iters))
                 lg = model.decoder.score_bf16(rows[0], mem, mem_len, B, K, rows[3], T2)
                 add(f'token_logprob_synthetic_{L}_tokens', timed(lambda: ops.token_logprob(lg, V, rows[1].view(-1)), 10 * a.iters))
-            add('lm_shallow_fusion_eager', timed(lambda: rec_fused.recognize_ids(x, mask), max(1, a.iters // 5), warmup=1))
+            add('lm_shallow_fusion', timed(lambda: rec_fused.recognize_ids(x, mask), max(1, a.iters // 5), warmup=1))
             add('apply_lm_rescoring', timed(lambda: rec_lm_resc.recognize_ids(x, mask), a.iters))
         res['token_logprob_bandwidth'] = {}
         for name, rows, rows_live in (('ctc_nbest', B * K * Lp, live_rows),
