@@ -56,22 +56,32 @@ int otb_debug_decode_timing(unsigned long long* buf, int step);
  * on a device that refuses clusters of 16 fails instead of falling back to the software barrier.  Process-wide. */
 int otb_set_decode_barrier(int kind);
 
-/* Conv2dLayer output geometry, kernel 3, stride 2, padding (0,1)  (frontend/conv.py:10-11,27):
- * T1 = (T-3)/2+1, F1 = (F-1)/2+1, T2 = (T1-3)/2+1, F2 = (F1-1)/2+1.  The conv1 activation buffer is
- * NHWC bf16 [B, 2*(T2+1), 2*F2, C1]. */
+/* Conv2dLayer output geometry of the two-layer conv front end (frontend/conv.py:10-11,15-48): layer i has kernel
+ * (kt_i, kf_i), stride (st_i, sf_i) and padding (0, kf_i / 2), so per axis n' = (n + 2 p - k) / s + 1.  Kernel sizes
+ * 1..7 and strides 1..4; an input with fewer than one output frame is refused.  out (may be NULL) receives
+ * {T1, F1, T2, F2, T1p, F1p}: the conv1 activation buffer is NHWC bf16 [B, T1p, F1p, C1] (T1p a multiple of st2, F1p of
+ * sf2; conv2 reads it per stride phase). */
+int otb_conv_geometry2(int T, int F, int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, int* out);
+/* otb_conv_geometry2 at the shipped geometry (3x3, stride 2, both layers), T >= 7: T1 = (T-3)/2+1, F1 = (F-1)/2+1,
+ * T2 = (T1-3)/2+1, F2 = (F1-1)/2+1; conv1 buffer [B, 2*(T2+1), 2*F2, C1]. */
 int otb_conv_geometry(int T, int F, int* T1, int* F1, int* T2, int* F2);
 
 /* Conv2dLayer.forward #1 (frontend/conv.py:50-76; C_in = 1): relu(conv2d(x, w) + b).
- * x f32 [B,T,F]; w f32 [C1,1,3,3]; bias f32 [C1]; out bf16 NHWC [B, 2*(T2+1), 2*F2, C1]. */
+ * x f32 [B,T,F]; w f32 [C1,1,kt1,kf1]; bias f32 [C1]; out bf16 NHWC conv1 buffer (otb_conv_geometry2), columns F1 ..
+ * F1p-1 written as zero.  C1 % 8 == 0, at most 2048 (1024 for kernels wider than 3, 512 wider than 5). */
+int otb_conv1_relu2(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1, int kt1, int kf1,
+                    int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
 int otb_conv1_relu(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1,
-                   void* stream);
+                   void* stream);   /* the shipped geometry */
 
 /* Conv2dLayer.forward #2 + the transpose/reshape of ConvFrontEnd.forward (frontend/conv.py:63-64,145)
- * as a wgmma implicit GEMM.  in = conv1 buffer; w bf16 [C2, 9*C1] with k = (kh*3+kw)*C1 + c;
+ * as a wgmma implicit GEMM.  in = conv1 buffer; w bf16 [C2, kt2*kf2*C1] with k = (kh*kf2+kw)*C1 + c;
  * out bf16 [B*T2, F2*C2] with feature index f*C2 + c (the caller permutes output_layer.weight columns
- * from the reference's c*F2 + f order once at load time). */
+ * from the reference's c*F2 + f order once at load time).  C1 % 64 == 0, C2 % 8 == 0, F2 <= 128. */
+int otb_conv2_relu2(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2, int kt1,
+                    int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
 int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2,
-                   void* stream);
+                   void* stream);   /* the shipped geometry */
 
 /* nn.Linear with a fused epilogue on wgmma tensor cores: out[M,N] = epi(a[M,K] w[N(,2N),K]^T + bias).
  * a, w bf16 (lda, ldw in elements, multiples of 8); out bf16 or f32 (out_f32; RESID and RESID_LN write bf16 only and
@@ -469,10 +479,17 @@ int otb_mwer_grad(const float* logits, int ld, int rows, int V, const int32_t* t
                   void* dlogits, void* stream);
 
 /* Conv2d front end backward (frontend/conv.py:50-76 under autograd).  h1 = conv1 activation buffer (layout of
- * otb_conv1_relu).  col bf16 [B*T2*F2, 9*C1] = im2col of h1 for conv2 (k = (kh*3+kw)*C1 + c): conv2's weight gradient is
- * otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu folds dcol
- * back onto the conv1 grid and applies ReLU' -> dpre1 (h1 layout).  otb_conv1_wgrad: out f32 [C1, 10] = 9 tap
- * gradients + the bias gradient of conv1 (C_in = 1). */
+ * otb_conv1_relu2).  col bf16 [B*T2*F2, kt2*kf2*C1] = im2col of h1 for conv2 (k = (kh*kf2+kw)*C1 + c): conv2's weight
+ * gradient is otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu2
+ * folds dcol back onto the conv1 grid and applies ReLU' -> dpre1 (h1 layout).  otb_conv1_wgrad2: out f32
+ * [C1, kt1*kf1 + 1] = tap gradients + the bias gradient of conv1 (C_in = 1; C1 <= 256).  The entry points without the
+ * 2 take the shipped geometry. */
+int otb_conv_im2col2(const void* h1, void* col, int B, int T, int F, int C1, int kt1, int kf1, int st1, int sf1, int kt2,
+                     int kf2, int st2, int sf2, void* stream);
+int otb_conv_col2im_relu2(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, int kt1, int kf1,
+                          int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
+int otb_conv1_wgrad2(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, int kt1, int kf1, int st1,
+                     int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
 int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream);
 int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, void* stream);
 int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, void* stream);

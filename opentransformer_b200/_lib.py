@@ -44,6 +44,9 @@ _SIGS = {
     'otb_debug_decode_timing': (c_int, [_P, c_int]),
     'otb_set_decode_barrier': (c_int, [c_int]),
     'otb_conv_geometry': (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
+    'otb_conv_geometry2': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int)]),
+    'otb_conv1_relu2': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv2_relu2': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_conv1_relu': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv2_relu': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_linear': (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, _P,
@@ -112,6 +115,9 @@ _SIGS = {
     'otb_conv_im2col': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv_col2im_relu': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_conv1_wgrad': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv_im2col2': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv_col2im_relu2': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv1_wgrad2': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_spec_augment': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_lstm_config': (c_int, [c_int, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     'otb_lstm_fwd': (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),

@@ -401,38 +401,38 @@ namespace otb {
 
 // ------------------------------------------------------------------------------------------------
 // Conv2d subsampling front end, backward (frontend/conv.py:50-76 under autograd).
-// Layouts as in the forward: conv1 activation h1 = NHWC bf16 [B, T1p = 2*(T2+1), F1p = 2*F2, C]; conv2 output rows are
-// (b, t2, f2) with C2 channels.  conv2's weight / input gradients are GEMMs over the explicit im2col matrix
-//   col[(b,t2,f2), (kh*3+kw)*C + c] = h1[b, 2*t2+kh, 2*f2+kw-1, c]      (f = -1 is the left zero padding)
+// Layouts as in the forward (ConvGeom): conv1 activation h1 = NHWC bf16 [B, T1p = st2*T1s, F1p = sf2*F1s, C]; conv2 output
+// rows are (b, t2, f2) with C2 channels.  conv2's weight / input gradients are GEMMs over the explicit im2col matrix
+//   col[(b,t2,f2), (kh*kf2+kw)*C + c] = h1[b, st2*t2+kh, sf2*f2+kw-pf2, c]      (f outside [0, F1) is the zero padding)
 // (wgrad: dW2 = dpre2^T col on the TN wgmma kernel; dgrad: dcol = dpre2 W2, then the gather below).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) im2col_s2_kernel(const bf16* __restrict__ h1, bf16* __restrict__ col, int B, int T2,
-                                                        int F2, int C, int T1p, int F1p) {
-    const int cg = C / 8;
-    const size_t total = (size_t)B * T2 * F2 * 9 * cg;
+__global__ void __launch_bounds__(256) im2col_kernel(const bf16* __restrict__ h1, bf16* __restrict__ col, int B, int T2,
+                                                     int F2, int C, int T1p, int F1p, int F1, int kt, int kf, int st, int sf) {
+    const int cg = C / 8, ntap = kt * kf;
+    const size_t total = (size_t)B * T2 * F2 * ntap * cg;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const int c8 = (int)(i % cg);
     size_t r = i / cg;
-    const int tap = (int)(r % 9);
-    r /= 9;
+    const int tap = (int)(r % ntap);
+    r /= ntap;
     const int f2 = (int)(r % F2);
     r /= F2;
     const int t2 = (int)(r % T2), b = (int)(r / T2);
-    const int kh = tap / 3, kw = tap % 3;
-    const int t = 2 * t2 + kh, f = 2 * f2 + kw - 1;
+    const int kh = tap / kf, kw = tap % kf;
+    const int t = st * t2 + kh, f = sf * f2 + kw - kf / 2;
     uint4 v = make_uint4(0, 0, 0, 0);
-    if (f >= 0) v = *reinterpret_cast<const uint4*>(h1 + (((size_t)b * T1p + t) * F1p + f) * C + c8 * 8);
-    *reinterpret_cast<uint4*>(col + (((size_t)(b * T2 + t2) * F2 + f2) * 9 + tap) * C + c8 * 8) = v;
+    if (f >= 0 && f < F1) v = *reinterpret_cast<const uint4*>(h1 + (((size_t)b * T1p + t) * F1p + f) * C + c8 * 8);
+    *reinterpret_cast<uint4*>(col + (((size_t)(b * T2 + t2) * F2 + f2) * ntap + tap) * C + c8 * 8) = v;
 }
 
 // dpre1[b,t1,f1,c] = relu'(h1) * sum over the (kh,kw) taps that read this input position of dcol[(b,t2,f2),(kh,kw,c)],
-// t2 = (t1-kh)/2, f2 = (f1+1-kw)/2 (both must be integral and in range).  Output in the h1 layout (positions outside
+// t2 = (t1-kh)/st2, f2 = (f1+pf2-kw)/sf2 (both must be integral and in range).  Output in the h1 layout (positions outside
 // [0,T1) x [0,F1) are written as zero so that the buffer is fully defined).
-__global__ void __launch_bounds__(256) col2im_s2_relu_kernel(const bf16* __restrict__ dcol, const bf16* __restrict__ h1,
-                                                             bf16* __restrict__ dpre1, int B, int T1, int F1, int T2, int F2,
-                                                             int C, int T1p, int F1p) {
-    const int cg = C / 8;
+__global__ void __launch_bounds__(256) col2im_relu_kernel(const bf16* __restrict__ dcol, const bf16* __restrict__ h1,
+                                                          bf16* __restrict__ dpre1, int B, int T1, int F1, int T2, int F2,
+                                                          int C, int T1p, int F1p, int kt, int kf, int st, int sf) {
+    const int cg = C / 8, ntap = kt * kf;
     const size_t total = (size_t)B * T1p * F1p * cg;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
@@ -443,18 +443,18 @@ __global__ void __launch_bounds__(256) col2im_s2_relu_kernel(const bf16* __restr
     const int t1 = (int)(r % T1p), b = (int)(r / T1p);
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (t1 < T1 && f1 < F1) {
-        for (int kh = 0; kh < 3; ++kh) {
+        for (int kh = 0; kh < kt; ++kh) {
             const int tt = t1 - kh;
-            if (tt < 0 || (tt & 1)) continue;
-            const int t2 = tt >> 1;
+            if (tt < 0 || tt % st) continue;
+            const int t2 = tt / st;
             if (t2 >= T2) continue;
-            for (int kw = 0; kw < 3; ++kw) {
-                const int ff = f1 + 1 - kw;
-                if (ff < 0 || (ff & 1)) continue;
-                const int f2 = ff >> 1;
+            for (int kw = 0; kw < kf; ++kw) {
+                const int ff = f1 + kf / 2 - kw;
+                if (ff < 0 || ff % sf) continue;
+                const int f2 = ff / sf;
                 if (f2 >= F2) continue;
                 float v[8];
-                unpack8(*reinterpret_cast<const uint4*>(dcol + (((size_t)(b * T2 + t2) * F2 + f2) * 9 + kh * 3 + kw) * C + c8 * 8), v);
+                unpack8(*reinterpret_cast<const uint4*>(dcol + (((size_t)(b * T2 + t2) * F2 + f2) * ntap + kh * kf + kw) * C + c8 * 8), v);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) acc[j] += v[j];
             }
@@ -467,73 +467,92 @@ __global__ void __launch_bounds__(256) col2im_s2_relu_kernel(const bf16* __restr
     *reinterpret_cast<uint4*>(dpre1 + i * 8) = pack8(acc);
 }
 
-// conv1 (C_in = 1) weight / bias gradient: dW1[c, kh*3+kw] = sum dpre1[b,t1,f1,c] * x[b, 2*t1+kh, 2*f1+kw-1], db1[c] = sum dpre1
-// out f32 [C, 10] (9 taps + bias), zeroed by the launcher.  CTA = (b, 8 rows of t1); thread = (channel, position lane).
+// conv1 (C_in = 1) weight / bias gradient: dW1[c, kh*kf+kw] = sum dpre1[b,t1,f1,c] * x[b, st*t1+kh, sf*f1+kw-pf], db1[c] =
+// sum dpre1.  out f32 [C, kt*kf + 1] (taps + bias), zeroed by the launcher.  CTA = (b, 8 rows of t1); thread = (channel,
+// position lane).  KMAX bounds kt and kf: the per-thread sums are registers indexed at compile time.
+template <int KMAX>
 __global__ void __launch_bounds__(256) conv1_wgrad_kernel(const bf16* __restrict__ dpre1, const float* __restrict__ x,
                                                           float* __restrict__ out, int B, int T, int F, int T1, int F1,
-                                                          int T1p, int F1p, int C) {
-    extern __shared__ float sx[];   // [17][F + 2]
-    __shared__ float red[256 * 10];
+                                                          int T1p, int F1p, int C, int kt, int kf, int st, int sf) {
+    extern __shared__ float sx[];   // [st*7 + kt][F + 2*pf], then red [256][kt*kf + 1]
     constexpr int ROWS = 8;
+    const int pf = kf / 2, ntap = kt * kf, nout = ntap + 1;
     const int chunks = (T1 + ROWS - 1) / ROWS;
     const int b = blockIdx.x / chunks, t1_0 = (blockIdx.x % chunks) * ROWS;
     const int nrows = min(ROWS, T1 - t1_0);
-    const int W2 = F + 2;
-    for (int i = threadIdx.x; i < (2 * nrows + 1) * W2; i += blockDim.x) {
-        const int r = i / W2, f = i % W2 - 1;
-        sx[i] = (f >= 0 && f < F) ? x[((size_t)b * T + 2 * t1_0 + r) * F + f] : 0.f;
+    const int W2 = F + 2 * pf;
+    float* red = sx + (st * (ROWS - 1) + kt) * W2;
+    for (int i = threadIdx.x; i < (st * (nrows - 1) + kt) * W2; i += blockDim.x) {
+        const int r = i / W2, f = i % W2 - pf;
+        sx[i] = (f >= 0 && f < F) ? x[((size_t)b * T + st * t1_0 + r) * F + f] : 0.f;
     }
     __syncthreads();
     const int lanes = blockDim.x / C;
     const int c = threadIdx.x % C, pl = threadIdx.x / C;
-    float acc[10];
+    float acc[KMAX * KMAX + 1];
 #pragma unroll
-    for (int j = 0; j < 10; ++j) acc[j] = 0.f;
+    for (int j = 0; j < KMAX * KMAX + 1; ++j) acc[j] = 0.f;
     if (pl < lanes) {
         for (int pos = pl; pos < nrows * F1; pos += lanes) {
             const int r = pos / F1, f1 = pos % F1;
             const float g = __bfloat162float(dpre1[(((size_t)b * T1p + t1_0 + r) * F1p + f1) * C + c]);
 #pragma unroll
-            for (int kh = 0; kh < 3; ++kh)
+            for (int kh = 0; kh < KMAX; ++kh) {
+                if (kh >= kt) break;
 #pragma unroll
-                for (int kw = 0; kw < 3; ++kw) acc[kh * 3 + kw] = fmaf(g, sx[(2 * r + kh) * W2 + 2 * f1 + kw], acc[kh * 3 + kw]);
-            acc[9] += g;
+                for (int kw = 0; kw < KMAX; ++kw) {
+                    if (kw >= kf) break;
+                    acc[kh * KMAX + kw] = fmaf(g, sx[(st * r + kh) * W2 + sf * f1 + kw], acc[kh * KMAX + kw]);
+                }
+            }
+            acc[KMAX * KMAX] += g;
         }
     }
 #pragma unroll
-    for (int j = 0; j < 10; ++j) red[threadIdx.x * 10 + j] = acc[j];
+    for (int kh = 0; kh < KMAX; ++kh)
+#pragma unroll
+        for (int kw = 0; kw < KMAX; ++kw)
+            if (kh < kt && kw < kf) red[threadIdx.x * nout + kh * kf + kw] = acc[kh * KMAX + kw];
+    red[threadIdx.x * nout + ntap] = acc[KMAX * KMAX];
     __syncthreads();
-    for (int i = threadIdx.x; i < C * 10; i += blockDim.x) {
-        const int cc = i / 10, j = i % 10;
+    for (int i = threadIdx.x; i < C * nout; i += blockDim.x) {
+        const int cc = i / nout, j = i % nout;
         float s = 0.f;
-        for (int l = 0; l < lanes; ++l) s += red[(l * C + cc) * 10 + j];
-        atomicAdd(out + cc * 10 + j, s);
+        for (int l = 0; l < lanes; ++l) s += red[(l * C + cc) * nout + j];
+        atomicAdd(out + cc * nout + j, s);
     }
 }
 
-const char* im2col_s2_launch(cudaStream_t st, const bf16* h1, bf16* col, int B, int T2, int F2, int C) {
+const char* im2col_launch(cudaStream_t st, const bf16* h1, bf16* col, int B, const ConvGeom& g, int C) {
     if (C % 8) return "im2col: C must be a multiple of 8";
-    const size_t total = (size_t)B * T2 * F2 * 9 * (C / 8);
-    return launch<im2col_s2_kernel>((unsigned)((total + 255) / 256), 256, 0, st, h1, col, B, T2, F2, C, 2 * (T2 + 1), 2 * F2);
+    const size_t total = (size_t)B * g.T2 * g.F2 * g.kt2 * g.kf2 * (C / 8);
+    return launch<im2col_kernel>((unsigned)((total + 255) / 256), 256, 0, st, h1, col, B, g.T2, g.F2, C, g.st2 * g.T1s,
+                                 g.sf2 * g.F1s, g.F1, g.kt2, g.kf2, g.st2, g.sf2);
 }
-const char* col2im_s2_relu_launch(cudaStream_t st, const bf16* dcol, const bf16* h1, bf16* dpre1, int B, int T1, int F1, int T2,
-                                  int F2, int C) {
+const char* col2im_relu_launch(cudaStream_t st, const bf16* dcol, const bf16* h1, bf16* dpre1, int B, const ConvGeom& g, int C) {
     if (C % 8) return "col2im: C must be a multiple of 8";
-    const size_t total = (size_t)B * 2 * (T2 + 1) * 2 * F2 * (C / 8);
-    return launch<col2im_s2_relu_kernel>((unsigned)((total + 255) / 256), 256, 0, st, dcol, h1, dpre1, B, T1, F1, T2, F2, C,
-                                         2 * (T2 + 1), 2 * F2);
+    const size_t total = (size_t)B * g.st2 * g.T1s * g.sf2 * g.F1s * (C / 8);
+    return launch<col2im_relu_kernel>((unsigned)((total + 255) / 256), 256, 0, st, dcol, h1, dpre1, B, g.T1, g.F1, g.T2, g.F2, C,
+                                      g.st2 * g.T1s, g.sf2 * g.F1s, g.kt2, g.kf2, g.st2, g.sf2);
 }
-const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* x, float* out, int B, int T, int F, int T1,
-                               int F1, int T2, int F2, int C) {
+const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* x, float* out, int B, int T, int F,
+                               const ConvGeom& g, int C) {
     // one thread per (channel, position lane): C <= 256 leaves at least one lane per channel (threads past the last full
     // lane idle, e.g. C = 192); C > 256 would leave none and silently return zeros
     if (C < 8 || C > 256 || C % 8) return "conv1_wgrad: C must be a multiple of 8, at most 256";
-    const size_t smem = (size_t)17 * (F + 2) * sizeof(float);
-    if (smem > 40 * 1024) return "conv1_wgrad: F too large";
-    cudaError_t e = cudaMemsetAsync(out, 0, (size_t)C * 10 * 4, st);
+    const int nout = g.kt1 * g.kf1 + 1;
+    const size_t sx = (size_t)(g.st1 * 7 + g.kt1) * (F + 2 * (g.kf1 / 2)) * sizeof(float);
+    if (sx > 40 * 1024) return "conv1_wgrad: F too large";
+    const size_t smem = sx + (size_t)256 * nout * sizeof(float);
+    cudaError_t e = cudaMemsetAsync(out, 0, (size_t)C * nout * 4, st);
     if (e != cudaSuccess) return cudaGetErrorString(e);
-    const int chunks = (T1 + 7) / 8;
-    return launch<conv1_wgrad_kernel>(B * chunks, 256, smem, st, dpre1, x, out, B, T, F, T1, F1, 2 * (T2 + 1), 2 * F2, C);
+    const int chunks = (g.T1 + 7) / 8;
+    const int kmax = max(g.kt1, g.kf1);
+#define WGRAD_ARGS B * chunks, 256, smem, st, dpre1, x, out, B, T, F, g.T1, g.F1, g.st2 * g.T1s, g.sf2 * g.F1s, C, g.kt1, g.kf1, g.st1, g.sf1
+    if (kmax <= 3) return launch<conv1_wgrad_kernel<3>>(WGRAD_ARGS);
+    if (kmax <= 5) return launch<conv1_wgrad_kernel<5>>(WGRAD_ARGS);
+    return launch<conv1_wgrad_kernel<7>>(WGRAD_ARGS);
+#undef WGRAD_ARGS
 }
 
 }  // namespace otb

@@ -29,6 +29,26 @@ static BeamState to_state(const otb_beam_state* s) {
     return b;
 }
 
+// The front end's geometry (frontend/conv.py:10-11,27,78-83): per axis floor((n + 2 p - k) / s) + 1 with time unpadded
+// and p = kf / 2 in frequency.  T1s / F1s: conv1 buffer rows / columns per conv2 stride phase, enough for every row conv1
+// writes and every column conv2 reads (F1s >= F2 so the TMA box fits the view).
+static const char* conv_geometry(int T, int F, int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, ConvGeom* g) {
+    const int k[4] = {kt1, kf1, kt2, kf2}, s[4] = {st1, sf1, st2, sf2};
+    for (int i = 0; i < 4; ++i)
+        if (k[i] < 1 || k[i] > 7 || s[i] < 1 || s[i] > 4) return "kernel sizes 1..7 and strides 1..4 only";
+    if (F < 1) return "need F >= 1";
+    if (T < kt1) return "input too short for one conv1 frame";
+    g->kt1 = kt1; g->kf1 = kf1; g->st1 = st1; g->sf1 = sf1; g->kt2 = kt2; g->kf2 = kf2; g->st2 = st2; g->sf2 = sf2;
+    g->T1 = (T - kt1) / st1 + 1;
+    g->F1 = (F + 2 * (kf1 / 2) - kf1) / sf1 + 1;
+    if (g->T1 < kt2) return "input too short for one conv2 frame";
+    g->T2 = (g->T1 - kt2) / st2 + 1;
+    g->F2 = (g->F1 + 2 * (kf2 / 2) - kf2) / sf2 + 1;
+    g->T1s = (g->T1 + st2 - 1) / st2;
+    g->F1s = max((g->F1 + sf2 - 1) / sf2, g->F2);
+    return nullptr;
+}
+
 }  // namespace otb
 
 using namespace otb;
@@ -64,58 +84,84 @@ int otb_set_decode_barrier(int kind) {
     return 0;
 }
 
-int otb_conv_geometry(int T, int F, int* T1, int* F1, int* T2, int* F2) {
-    if (T < 7 || F < 1) return fail("otb_conv_geometry", "need T >= 7 and F >= 1");
-    const int t1 = (T - 3) / 2 + 1, f1 = (F - 1) / 2 + 1;
-    const int t2 = (t1 - 3) / 2 + 1, f2 = (f1 - 1) / 2 + 1;
-    if (T1) *T1 = t1;
-    if (F1) *F1 = f1;
-    if (T2) *T2 = t2;
-    if (F2) *F2 = f2;
+int otb_conv_geometry2(int T, int F, int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, int* out) {
+    ConvGeom g;
+    if (const char* e = conv_geometry(T, F, kt1, kf1, st1, sf1, kt2, kf2, st2, sf2, &g)) return fail("otb_conv_geometry2", e);
+    if (out) {
+        out[0] = g.T1; out[1] = g.F1; out[2] = g.T2; out[3] = g.F2;
+        out[4] = g.st2 * g.T1s; out[5] = g.sf2 * g.F1s;
+    }
     return 0;
+}
+
+int otb_conv_geometry(int T, int F, int* T1, int* F1, int* T2, int* F2) {
+    int g[6];
+    if (T < 7 || F < 1) return fail("otb_conv_geometry", "need T >= 7 and F >= 1");
+    if (otb_conv_geometry2(T, F, 3, 3, 2, 2, 3, 3, 2, 2, g)) return 1;
+    if (T1) *T1 = g[0];
+    if (F1) *F1 = g[1];
+    if (T2) *T2 = g[2];
+    if (F2) *F2 = g[3];
+    return 0;
+}
+
+int otb_conv1_relu2(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1, int kt1, int kf1,
+                    int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream) {
+    ConvGeom g;
+    if (const char* e = conv_geometry(T, F, kt1, kf1, st1, sf1, kt2, kf2, st2, sf2, &g)) return fail("otb_conv1_relu", e);
+    if (!x || !w || !bias || !out || B < 1) return fail("otb_conv1_relu", "null pointer or empty batch");
+    RET("otb_conv1_relu", conv1_launch(ST(stream), x, w, bias, reinterpret_cast<bf16*>(out), B, T, F, g, C1));
 }
 
 int otb_conv1_relu(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1,
                    void* stream) {
-    int T1, F1, T2, F2;
-    if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;
-    if (!x || !w || !bias || !out || B < 1) return fail("otb_conv1_relu", "null pointer or empty batch");
-    RET("otb_conv1_relu",
-        conv1_launch(ST(stream), x, w, bias, reinterpret_cast<bf16*>(out), B, T, F, T1, F1, 2 * (T2 + 1), 2 * F2, C1));
+    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
+    return otb_conv1_relu2(x, w, bias, out, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
 }
 
-int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2,
-                   void* stream) {
-    int T1, F1, T2, F2;
-    if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;
+int otb_conv2_relu2(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2, int kt1,
+                    int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream) {
+    ConvGeom g;
+    if (const char* e = conv_geometry(T, F, kt1, kf1, st1, sf1, kt2, kf2, st2, sf2, &g)) return fail("otb_conv2_relu", e);
     if (!in || !w || !bias || !out || B < 1) return fail("otb_conv2_relu", "null pointer or empty batch");
     if (C1 % 64) return fail("otb_conv2_relu", "C1 must be a multiple of 64 (one 128-byte tap per k-block)");
     if (C2 % 8) return fail("otb_conv2_relu", "C2 must be a multiple of 8");
-    if (F2 > 128) return fail("otb_conv2_relu", "F2 > 128 not supported");
-    const int T1h = T2 + 1;
-    int R = 128 / F2;
-    if (R > T1h) R = T1h;
+    if (g.F2 > 128) return fail("otb_conv2_relu", "F2 > 128 not supported");
+    int R = 128 / g.F2;
+    if (R > g.T1s) R = g.T1s;
     if (R > 256) R = 256;
     CUtensorMap cmap;
-    const char* e = encode_tmap_conv5d(&cmap, in, C1, F2, B * T1h, (uint32_t)F2, (uint32_t)R);
+    const char* e = encode_tmap_conv5d(&cmap, in, C1, g.sf2, g.F1s, g.st2, B * g.T1s, (uint32_t)g.F2, (uint32_t)R);
     if (e) return fail("otb_conv2_relu", e);
+    const int K = kt2 * kf2 * C1;
     GemmParams p;
     memset(&p, 0, sizeof(p));
-    p.M = B * T2 * F2;
+    p.M = B * g.T2 * g.F2;
     p.N = C2;
-    p.K = 9 * C1;
+    p.K = K;
     p.bias = bias;
     p.out = out;
     p.ldc = C2;
     p.alpha = 1.f;
     p.conv = 1;
-    p.conv_F2 = F2;
+    p.conv_F2 = g.F2;
     p.conv_R = R;
-    p.conv_T1h = T1h;
-    p.conv_T2 = T2;
+    p.conv_T1h = g.T1s;
+    p.conv_T2 = g.T2;
     p.conv_B = B;
     p.conv_cchunks = C1 / 64;
-    RET("otb_conv2_relu", gemm_launch(ST(stream), nullptr, 0, w, 9 * C1, C2, EPI_RELU, p, &cmap));
+    for (int kh = 0; kh < kt2; ++kh)
+        for (int kw = 0; kw < kf2; ++kw) {
+            const int d = kw - kf2 / 2, par_f = ((d % sf2) + sf2) % sf2, f0 = (d - par_f) / sf2;
+            p.conv_tap[kh * kf2 + kw] = (unsigned)par_f | (unsigned)(f0 + 8) << 8 | (unsigned)(kh % st2) << 16 | (unsigned)(kh / st2) << 24;
+        }
+    RET("otb_conv2_relu", gemm_launch(ST(stream), nullptr, 0, w, K, C2, EPI_RELU, p, &cmap));
+}
+
+int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2,
+                   void* stream) {
+    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
+    return otb_conv2_relu2(in, w, bias, out, B, T, F, C1, C2, 3, 3, 2, 2, 3, 3, 2, 2, stream);
 }
 
 int otb_linear(const void* a, int lda, const void* w, int ldw, const float* bias, void* out, int ldc, int M, int N,
@@ -589,27 +635,43 @@ int otb_mwer_grad(const float* logits, int ld, int rows, int V, const int32_t* t
     RET("otb_mwer_grad", mwer_grad_launch(ST(stream), logits, ld, rows, V, target, tok_lp, coeff, Lp, reinterpret_cast<bf16*>(dlogits)));
 }
 
-int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
-    int T1, F1, T2, F2;
-    if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;
+#define CONV_GEOM2 int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2
+#define CONV_ARGS2 kt1, kf1, st1, sf1, kt2, kf2, st2, sf2
+int otb_conv_im2col2(const void* h1, void* col, int B, int T, int F, int C1, CONV_GEOM2, void* stream) {
+    ConvGeom g;
+    if (const char* e = conv_geometry(T, F, CONV_ARGS2, &g)) return fail("otb_conv_im2col", e);
     if (!h1 || !col) return fail("otb_conv_im2col", "null operand");
-    RET("otb_conv_im2col", im2col_s2_launch(ST(stream), reinterpret_cast<const bf16*>(h1), reinterpret_cast<bf16*>(col), B, T2, F2, C1));
+    RET("otb_conv_im2col", im2col_launch(ST(stream), reinterpret_cast<const bf16*>(h1), reinterpret_cast<bf16*>(col), B, g, C1));
+}
+int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
+    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
+    return otb_conv_im2col2(h1, col, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
 }
 
-int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, void* stream) {
-    int T1, F1, T2, F2;
-    if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;
+int otb_conv_col2im_relu2(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, CONV_GEOM2, void* stream) {
+    ConvGeom g;
+    if (const char* e = conv_geometry(T, F, CONV_ARGS2, &g)) return fail("otb_conv_col2im_relu", e);
     if (!dcol || !h1 || !dpre1) return fail("otb_conv_col2im_relu", "null operand");
-    RET("otb_conv_col2im_relu", col2im_s2_relu_launch(ST(stream), reinterpret_cast<const bf16*>(dcol), reinterpret_cast<const bf16*>(h1),
-                                                      reinterpret_cast<bf16*>(dpre1), B, T1, F1, T2, F2, C1));
+    RET("otb_conv_col2im_relu", col2im_relu_launch(ST(stream), reinterpret_cast<const bf16*>(dcol), reinterpret_cast<const bf16*>(h1),
+                                                   reinterpret_cast<bf16*>(dpre1), B, g, C1));
+}
+int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, void* stream) {
+    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
+    return otb_conv_col2im_relu2(dcol, h1, dpre1, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
 }
 
-int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, void* stream) {
-    int T1, F1, T2, F2;
-    if (otb_conv_geometry(T, F, &T1, &F1, &T2, &F2)) return 1;
+int otb_conv1_wgrad2(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, CONV_GEOM2, void* stream) {
+    ConvGeom g;
+    if (const char* e = conv_geometry(T, F, CONV_ARGS2, &g)) return fail("otb_conv1_wgrad", e);
     if (!dpre1 || !x || !out) return fail("otb_conv1_wgrad", "null operand");
-    RET("otb_conv1_wgrad", conv1_wgrad_launch(ST(stream), reinterpret_cast<const bf16*>(dpre1), x, out, B, T, F, T1, F1, T2, F2, C1));
+    RET("otb_conv1_wgrad", conv1_wgrad_launch(ST(stream), reinterpret_cast<const bf16*>(dpre1), x, out, B, T, F, g, C1));
 }
+int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, void* stream) {
+    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
+    return otb_conv1_wgrad2(dpre1, x, out, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
+}
+#undef CONV_GEOM2
+#undef CONV_ARGS2
 
 int otb_spec_augment(float* x, const int32_t* bands, int B, int T, int F, int n_freq, int n_time, void* stream) {
     if (!x || !bands || B < 1 || T < 1 || F < 1 || n_freq < 0 || n_time < 0) return fail("otb_spec_augment", "bad arguments");

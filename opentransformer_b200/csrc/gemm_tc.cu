@@ -120,11 +120,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         mbar_arrive_expect_tx(&full_bar[stage], a_tx + (uint32_t)Cfg::B_BYTES);
         if (p.conv) {
-            // k-block -> (tap, channel chunk); tap (kh,kw): input row 2t'+kh, col 2f'+kw-1
+            // k-block -> (tap, channel chunk); tap (kh,kw): input row st t'+kh, col sf f'+kw-pf, i.e. stride phase
+            // (kh mod st, (kw-pf) mod sf) at offset (kh / st, floor((kw-pf) / sf)); negative columns are TMA zero fill
             const int tap = kb / p.conv_cchunks, cc = kb % p.conv_cchunks;
-            const int kh = tap / 3, kw = tap % 3;
-            const int par_f = (kw == 1) ? 0 : 1, f0 = (kw == 0) ? -1 : 0;
-            const int par_t = (kh == 1) ? 1 : 0, dt = (kh == 2) ? 1 : 0;
+            const unsigned c = p.conv_tap[tap];
+            const int par_f = c & 255, f0 = (int)((c >> 8) & 255) - 8, par_t = (c >> 16) & 255, dt = c >> 24;
             tma_load_5d(sa, &tmA, &full_bar[stage], cc * BK, par_f, f0, par_t, m_blk * p.conv_R + dt);
         } else {
             tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
@@ -500,14 +500,14 @@ const char* encode_tmap_2d_f32(CUtensorMap* m, const void* base, uint64_t cols, 
     return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled(2d, fp32) failed";
 }
 
-// conv1 output buffer [B, 2*T1h, 2*F1h, C] bf16 viewed as (c, f-parity, f/2, t-parity, b*T1h + t/2)
-const char* encode_tmap_conv5d(CUtensorMap* m, const void* base, int C, int F1h, int T1h_total, uint32_t boxF,
+// conv1 output buffer [B, st*T1s, sf*F1s, C] bf16 viewed as (c, f mod sf, f / sf, t mod st, b*T1s + t / st)
+const char* encode_tmap_conv5d(CUtensorMap* m, const void* base, int C, int sf, int F1s, int st, int T1s_total, uint32_t boxF,
                                uint32_t boxR) {
     PFN_encodeTiled enc = get_encode();
     if (!enc) return "cuTensorMapEncodeTiled unavailable (no CUDA driver?)";
-    cuuint64_t dims[5] = {(cuuint64_t)C, 2, (cuuint64_t)F1h, 2, (cuuint64_t)T1h_total};
-    cuuint64_t strides[4] = {(cuuint64_t)C * 2, (cuuint64_t)C * 4, (cuuint64_t)F1h * 2 * C * 2,
-                             (cuuint64_t)F1h * 2 * C * 4};
+    cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)sf, (cuuint64_t)F1s, (cuuint64_t)st, (cuuint64_t)T1s_total};
+    cuuint64_t strides[4] = {(cuuint64_t)C * 2, (cuuint64_t)C * sf * 2, (cuuint64_t)F1s * sf * C * 2,
+                             (cuuint64_t)F1s * sf * C * st * 2};
     cuuint32_t box[5] = {64, 1, boxF, 1, boxR};
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(base), dims, strides, box, estr,

@@ -9,82 +9,102 @@
 namespace otb {
 
 // ------------------------------------------------------------------------------------------------
-// conv1: Conv2d(1 -> C1, 3x3, stride 2, padding (0,1)) + ReLU      otrans/frontend/conv.py:63-64
+// conv1: Conv2d(1 -> C1, (kt, kf), stride (st, sf), padding (0, kf/2)) + ReLU      otrans/frontend/conv.py:27-37,63-64
 // in : x f32 [B, T, F]
-// out: bf16 NHWC [B, 2*T1h, 2*F1h, C1]; columns f >= F1 are written as zero (they are the right
+// out: bf16 NHWC [B, st2*T1s, sf2*F1s, C1] (ConvGeom); columns f >= F1 are written as zero (they are the right
 //      frequency padding of conv2); rows t >= T1 are never read for valid outputs and left untouched.
-// HBM-bound on the output write (82 MB at cfg 2).  One CTA = 24 consecutive output rows of one
-// utterance: the 49 input rows are staged in smem once, each thread keeps the 3x3 filters + bias of
-// its 8 channels in registers and walks over (row, f1) positions, one 16-byte store per position,
-// fully coalesced along (f1, c).  (With 8 rows per CTA the 80 weight loads per thread outnumbered the
-// stores 8:1.)
+// HBM-bound on the output write (82 MB at cfg 2).  One CTA = 24 consecutive output rows of one utterance: their
+// st*23 + kt input rows are staged in smem once, each thread keeps the filters + bias of its CPT channels in registers
+// and walks over (row, f1) positions, one store per position, fully coalesced along (f1, c).  (With 8 rows per CTA the
+// 80 weight loads per thread outnumbered the stores 8:1.)  KMAX bounds kt and kf: the filters of a thread take
+// KMAX^2 * CPT registers (72, 100, 98), indexed at compile time by unrolled loops that skip the taps past (kt, kf).
+// SHIPPED fixes the shipped geometry (3x3, stride 2) at compile time: the run-time strides and tap bounds cost the
+// shipped front end 17 % of conv1's time on H100.
 // ------------------------------------------------------------------------------------------------
 static constexpr int CONV1_ROWS = 24;
 
+template <int KMAX, int CPT, bool SHIPPED>
 __global__ void __launch_bounds__(256) conv1_relu_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                               const float* __restrict__ bias, bf16* __restrict__ out,
                                                               int B, int T, int F, int T1, int F1, int T1pad,
-                                                              int F1pad, int C1) {
-    extern __shared__ float sx[];  // [2*CONV1_ROWS + 1][F + 2]  (one zero column each side)
+                                                              int F1pad, int C1, int kt_, int kf_, int st_, int sf_) {
+    const int kt = SHIPPED ? 3 : kt_, kf = SHIPPED ? 3 : kf_, st = SHIPPED ? 2 : st_, sf = SHIPPED ? 2 : sf_;
+    extern __shared__ float sx[];  // [st*(CONV1_ROWS-1) + kt][F + 2*pf]  (pf = kf/2 zero columns each side)
+    const int pf = kf / 2;
     const int chunks = (T1 + CONV1_ROWS - 1) / CONV1_ROWS;
     const int b = blockIdx.x / chunks, t1_0 = (blockIdx.x % chunks) * CONV1_ROWS;
     const int nrows = min(CONV1_ROWS, T1 - t1_0);
-    const int W2 = F + 2;
-    const int in_rows = 2 * nrows + 1;
+    const int W2 = F + 2 * pf;
+    const int in_rows = st * (nrows - 1) + kt;
     for (int i = threadIdx.x; i < in_rows * W2; i += blockDim.x) {
-        const int r = i / W2, f = i % W2 - 1;
-        sx[i] = (f >= 0 && f < F) ? x[((size_t)b * T + 2 * t1_0 + r) * F + f] : 0.f;
+        const int r = i / W2, f = i % W2 - pf;
+        sx[i] = (f >= 0 && f < F) ? x[((size_t)b * T + st * t1_0 + r) * F + f] : 0.f;
     }
-    const int cgs = C1 / 8;             // channel groups of 8
+    const int cgs = C1 / CPT;           // channel groups of CPT
     const int ppp = blockDim.x / cgs;   // positions per pass
     const int cg = threadIdx.x % cgs, pos0 = threadIdx.x / cgs;
-    float wr[9][8], br[8];
+    const int ntap = kt * kf;
+    float wr[KMAX * KMAX][CPT], br[CPT];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        br[j] = bias[cg * 8 + j];
+    for (int j = 0; j < CPT; ++j) {
+        br[j] = bias[cg * CPT + j];
 #pragma unroll
-        for (int tap = 0; tap < 9; ++tap) wr[tap][j] = w[(cg * 8 + j) * 9 + tap];
+        for (int kh = 0; kh < KMAX; ++kh)
+#pragma unroll
+            for (int kw = 0; kw < KMAX; ++kw)
+                if (kh < kt && kw < kf) wr[kh * KMAX + kw][j] = w[(cg * CPT + j) * ntap + kh * kf + kw];
     }
     __syncthreads();
     if (pos0 >= ppp) return;
     const int npos = nrows * F1pad;
     for (int pos = pos0; pos < npos; pos += ppp) {
         const int r = pos / F1pad, f1 = pos % F1pad;
-        float v[8];
+        float v[CPT];
         if (f1 < F1) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = br[j];
+            for (int j = 0; j < CPT; ++j) v[j] = br[j];
 #pragma unroll
-            for (int kh = 0; kh < 3; ++kh)
+            for (int kh = 0; kh < KMAX; ++kh) {
+                if (kh >= kt) break;
 #pragma unroll
-                for (int kw = 0; kw < 3; ++kw) {
-                    const float xv = sx[(2 * r + kh) * W2 + 2 * f1 + kw];  // input col 2*f1 + kw - 1, +1 for the halo
+                for (int kw = 0; kw < KMAX; ++kw) {
+                    if (kw >= kf) break;
+                    const float xv = sx[(st * r + kh) * W2 + sf * f1 + kw];  // input col sf*f1 + kw - pf, +pf for the halo
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) v[j] = fmaf(xv, wr[kh * 3 + kw][j], v[j]);
+                    for (int j = 0; j < CPT; ++j) v[j] = fmaf(xv, wr[kh * KMAX + kw][j], v[j]);
                 }
+            }
 #pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
+            for (int j = 0; j < CPT; ++j) v[j] = fmaxf(v[j], 0.f);
         } else {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = 0.f;
+            for (int j = 0; j < CPT; ++j) v[j] = 0.f;
         }
-        uint4 u;
-        u.x = pack_bf16(v[0], v[1]);
-        u.y = pack_bf16(v[2], v[3]);
-        u.z = pack_bf16(v[4], v[5]);
-        u.w = pack_bf16(v[6], v[7]);
-        *reinterpret_cast<uint4*>(out + (((size_t)b * T1pad + t1_0 + r) * F1pad + f1) * C1 + cg * 8) = u;
+        uint32_t u[CPT / 2];
+#pragma unroll
+        for (int j = 0; j < CPT / 2; ++j) u[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
+        bf16* dst = out + (((size_t)b * T1pad + t1_0 + r) * F1pad + f1) * C1 + cg * CPT;
+        if constexpr (CPT == 8) *reinterpret_cast<uint4*>(dst) = make_uint4(u[0], u[1], u[2], u[3]);
+        else if constexpr (CPT == 4) *reinterpret_cast<uint2*>(dst) = make_uint2(u[0], u[1]);
+        else *reinterpret_cast<uint32_t*>(dst) = u[0];
     }
 }
 
 const char* conv1_launch(cudaStream_t st, const float* x, const float* w, const float* bias, bf16* out, int B, int T,
-                         int F, int T1, int F1, int T1pad, int F1pad, int C1) {
-    if (C1 % 8 || C1 > 2048) return "conv1: C1 must be a multiple of 8 (<= 2048)";
-    size_t smem = (size_t)(2 * CONV1_ROWS + 1) * (F + 2) * sizeof(float);
+                         int F, const ConvGeom& g, int C1) {
+    const int kmax = max(g.kt1, g.kf1);
+    const int cpt = kmax <= 3 ? 8 : kmax <= 5 ? 4 : 2;   // channels per thread: the filters fit the registers
+    if (C1 % 8 || C1 > 256 * cpt) return "conv1: C1 must be a multiple of 8, at most 2048 (1024 for kernels wider than 3, 512 wider than 5)";
+    size_t smem = (size_t)(g.st1 * (CONV1_ROWS - 1) + g.kt1) * (F + 2 * (g.kf1 / 2)) * sizeof(float);
     if (smem > 48 * 1024) return "conv1: F too large";
-    const int chunks = (T1 + CONV1_ROWS - 1) / CONV1_ROWS;
-    return launch<conv1_relu_nhwc_kernel>(dim3(B * chunks), dim3(256), smem, st, x, w, bias, out, B, T, F, T1, F1, T1pad,
-                                          F1pad, C1);
+    const int chunks = (g.T1 + CONV1_ROWS - 1) / CONV1_ROWS;
+    const int T1pad = g.st2 * g.T1s, F1pad = g.sf2 * g.F1s;
+#define CONV1_ARGS dim3(B * chunks), dim3(256), smem, st, x, w, bias, out, B, T, F, g.T1, g.F1, T1pad, F1pad, C1, g.kt1, g.kf1, g.st1, g.sf1
+    if (g.kt1 == 3 && g.kf1 == 3 && g.st1 == 2 && g.sf1 == 2) return launch<conv1_relu_nhwc_kernel<3, 8, true>>(CONV1_ARGS);
+    if (cpt == 8) return launch<conv1_relu_nhwc_kernel<3, 8, false>>(CONV1_ARGS);
+    if (cpt == 4) return launch<conv1_relu_nhwc_kernel<5, 4, false>>(CONV1_ARGS);
+    return launch<conv1_relu_nhwc_kernel<7, 2, false>>(CONV1_ARGS);
+#undef CONV1_ARGS
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -41,14 +41,17 @@ struct GemmParams {
     int period;
     const int* row_len;  // optional: rows with (m % row_period) >= row_len[m / row_period] produce 0 (before resid)
     int row_period;
-    // implicit-GEMM 3x3/stride-2 convolution mode (A operand gathered by a 5-D TMA map)
+    // implicit-GEMM convolution mode (A operand gathered by a 5-D TMA map, one k-block = one tap of 64 channels)
     int conv;
     int conv_F2;       // output frequency bins
     int conv_R;        // output time rows per M tile (R * F2 <= 128)
-    int conv_T1h;      // (padded input time rows) / 2
+    int conv_T1h;      // input time rows per utterance / time stride (ConvGeom::T1s)
     int conv_T2;       // valid output time rows per utterance
     int conv_B;        // batch
     int conv_cchunks;  // C_in / 64
+    // per tap (kh, kw) of conv2: bytes {f stride phase, f offset + 8, t stride phase, t offset}, computed on the host
+    // (integer division by run-time strides in the TMA producer cost the shipped conv2 a third of its time on H100)
+    unsigned conv_tap[49];
     int splitk;        // TN (weight-gradient) mode: number of contraction splits (fp32 atomics when > 1)
     int accum;         // TN mode: add into `out` instead of overwriting it
     // training-mode dropout of the projection BEFORE the residual add (EPI_RESID only): out = resid + alpha * keep * (.) / (1-p)
@@ -70,8 +73,18 @@ const char* encode_tmap_2d(CUtensorMap* m, const void* base, uint64_t cols, uint
                            uint32_t box_cols, uint32_t box_rows);
 const char* encode_tmap_2d_f32(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t ld_elems,
                                uint32_t box_cols, uint32_t box_rows);
-const char* encode_tmap_conv5d(CUtensorMap* m, const void* base, int C, int F1h, int T1h_total, uint32_t boxF,
+const char* encode_tmap_conv5d(CUtensorMap* m, const void* base, int C, int sf, int F1s, int st, int T1s_total, uint32_t boxF,
                                uint32_t boxR);
+
+// Two-layer Conv2d front end (frontend/conv.py:15-48,86-129): layer i has kernel (kt, kf), stride (st, sf) and padding
+// (0, kf / 2).  conv1's output buffer is NHWC bf16 [B, st2 * T1s, sf2 * F1s, C1]: conv2 reads it through the 5-D view
+// (c, f mod sf2, f / sf2, t mod st2, b * T1s + t / st2), and columns F1 .. sf2 * F1s - 1 are written as zero (the right
+// frequency padding of conv2).
+struct ConvGeom {
+    int kt1, kf1, st1, sf1, kt2, kf2, st2, sf2;
+    int T1, F1, T2, F2;
+    int T1s, F1s;
+};
 
 struct AttnParams {
     int B, H, Tq, Tk;
@@ -118,11 +131,10 @@ const char* relu_bwd_launch(cudaStream_t st, const bf16* dy, const bf16* y, bf16
 const char* dropout_bwd_launch(cudaStream_t st, const bf16* dy, int lddy, bf16* out, int ldo, unsigned char* mask, int M, int N, float p,
                                const unsigned* seed, unsigned site);
 const char* embed_bwd_launch(cudaStream_t st, const long long* tok, const bf16* dx, float* dE, int N, int d, int vocab, float scale);
-const char* im2col_s2_launch(cudaStream_t st, const bf16* h1, bf16* col, int B, int T2, int F2, int C);
-const char* col2im_s2_relu_launch(cudaStream_t st, const bf16* dcol, const bf16* h1, bf16* dpre1, int B, int T1, int F1, int T2,
-                                  int F2, int C);
-const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* x, float* out, int B, int T, int F, int T1,
-                               int F1, int T2, int F2, int C);
+const char* im2col_launch(cudaStream_t st, const bf16* h1, bf16* col, int B, const ConvGeom& g, int C);
+const char* col2im_relu_launch(cudaStream_t st, const bf16* dcol, const bf16* h1, bf16* dpre1, int B, const ConvGeom& g, int C);
+const char* conv1_wgrad_launch(cudaStream_t st, const bf16* dpre1, const float* x, float* out, int B, int T, int F,
+                               const ConvGeom& g, int C);
 const char* spec_augment_launch(cudaStream_t st, float* x, const int* bands, int B, int T, int F, int nf, int nt);
 const char* sumsq_launch(cudaStream_t st, const float* g, size_t n, float* out, int zero_first);
 const char* adam_sched_launch(cudaStream_t st, float* p, const float* g, float* m, float* v, size_t n, const float* sumsq,
@@ -172,7 +184,7 @@ struct AttnProbsParams {
 const char* attn_probs_launch(cudaStream_t st, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows,
                               const AttnProbsParams& p, int d_k);
 const char* conv1_launch(cudaStream_t st, const float* x, const float* w, const float* bias, bf16* out, int B, int T,
-                         int F, int T1, int F1, int T1pad, int F1pad, int C1);
+                         int F, const ConvGeom& g, int C1);
 const char* layernorm_launch(cudaStream_t st, const bf16* x, int ldx, void* out, int ldo, int out_f32, const float* g1,
                              const float* b1, const float* g2, const float* b2, float eps, int M, int N);
 const char* scale_add_table_launch(cudaStream_t st, const void* x, int ldx, int x_f32, bf16* out, int ldo, float alpha,

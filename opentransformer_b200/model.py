@@ -29,8 +29,9 @@ def ctc_align_logits(logits, lengths, B, T2, V, tokens, n_tokens, blank):
 def encoder_frames_to_input(spans, frame_shift=None, frontend=None):
     """Spans [start, end) in encoder frames (CTCModel.align, SpeechToText.align, CTCRecognizer.recognize_spans) -> spans in
     input (fbank) frames, [s start, s (end - 1) + w), where encoder frame t sees input frames [s t, s t + w): the front
-    end's input_window() (s, w) -- (4, 7) for the conv front end, whose two 3x3 stride-2 convolutions do not pad in time,
-    and (stride, n) for the concat front ends.  Without a front end the conv front end's window is used.  With frame_shift
+    end's input_window() (s, w) -- (st1 st2, kt1 + (kt2 - 1) st1) for the conv front end, whose convolutions do not pad in
+    time, and (stride, n) for the concat front ends.  Without a front end the shipped conv front end's window (4, 7) is
+    used.  With frame_shift
     (seconds between input frames, e.g. 0.01) the result is in seconds, float64.  Entries of -1 (no span) stay -1."""
     s, w = frontend.input_window() if frontend is not None else (4, 7)
     out = torch.stack((s * spans[..., 0], s * (spans[..., 1] - 1) + w), dim=-1)

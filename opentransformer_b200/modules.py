@@ -77,23 +77,60 @@ def _no_train(module):
 # ------------------------------------------------------------------------------------------------
 # front end
 # ------------------------------------------------------------------------------------------------
+CONV_KERNELS, CONV_STRIDES = range(1, 8), range(1, 5)
+
+
+def _conv_pair(v):
+    """An int or a [time, freq] pair, as nn.Conv2d reads kernel_size and stride."""
+    return (int(v), int(v)) if isinstance(v, int) else (int(v[0]), int(v[1]))
+
+
+def conv_frontend_geometry(layers, T=None, F=None):
+    """The conv front end's geometry (frontend/conv.py:10-11,27,78-83), for layers = ((kt1, kf1, st1, sf1), (kt2, kf2, st2,
+    sf2)).  Padding is (0, kf // 2): time is never padded.  Returns a dict:
+      'geom'   the 8 ints the CUDA entry points take;
+      'window' (stride, width): output frame t sees input frames [stride t, stride t + width);
+      'mask'   per layer (start, step): the reference's mask[:, kt // 2 :: st][:, :t];
+    and, given T and F, 'sizes' [(T1, F1), (T2, F2)] with n' = (n + 2 p - k) // s + 1 per axis.  A kernel or stride
+    outside 1..7 / 1..4 raises NotImplementedError; a T too short for one output frame raises ValueError (the reference's
+    conv2d raises there too)."""
+    (kt1, kf1, st1, sf1), (kt2, kf2, st2, sf2) = layers
+    if not all(k in CONV_KERNELS for k in (kt1, kf1, kt2, kf2)) or not all(s in CONV_STRIDES for s in (st1, sf1, st2, sf2)):
+        raise NotImplementedError(f'conv front end: kernel sizes 1..7 and strides 1..4 per axis are supported, got kernels '
+                                  f'({kt1}, {kf1}), ({kt2}, {kf2}) and strides ({st1}, {sf1}), ({st2}, {sf2})')
+    g = {'geom': (kt1, kf1, st1, sf1, kt2, kf2, st2, sf2), 'window': (st1 * st2, kt1 + (kt2 - 1) * st1),
+         'mask': ((kt1 // 2, st1), (kt2 // 2, st2))}
+    if T is not None:
+        sizes = []
+        for kt, kf, st, sf in layers:
+            if T < kt:
+                raise ValueError(f'conv front end: {T} frames are too short for a {kt}-frame kernel')
+            T, F = (T - kt) // st + 1, (F + 2 * (kf // 2) - kf) // sf + 1
+            sizes.append((T, F))
+        g['sizes'] = sizes
+    return g
+
+
 class Conv2dLayer(nn.Module):
-    """Parameter holder with the reference's key names (frontend/conv.py:15-48)."""
+    """Parameter holder with the reference's key names (frontend/conv.py:15-48).  act_func_type is accepted and ignored:
+    the reference applies F.relu whatever it says (conv.py:64).  dropout is the identity at inference."""
 
     def __init__(self, input_size, in_channel, out_channel, kernel_size, stride, dropout=0.1, batch_norm=False,
                  residual=False, act_func_type='relu'):
         super().__init__()
-        ks = kernel_size if isinstance(kernel_size, (list, tuple)) else [kernel_size, kernel_size]
-        if list(ks) != [3, 3] or stride != 2 or batch_norm or residual or act_func_type != 'relu':
-            raise NotImplementedError('ConvFrontEnd supports the shipped configuration only: '
-                                      '3x3 kernels, stride 2, relu, no batch_norm / residual')
-        self.conv_layer = nn.Conv2d(in_channel, out_channel, (3, 3), stride=2, padding=(0, 1))
-        self.output_size = (input_size + 2 - 3) // 2 + 1
+        if batch_norm or residual:
+            raise NotImplementedError('ConvFrontEnd never sets batch_norm / residual')
+        (kt, kf), (st, sf) = _conv_pair(kernel_size), _conv_pair(stride)
+        self.kernel_size, self.stride, self.dropout_p = kernel_size, stride, dropout
+        self.conv_layer = nn.Conv2d(in_channel, out_channel, (kt, kf), stride=(st, sf), padding=(0, kf // 2))
+        self.output_size = (input_size + 2 * (kf // 2) - kf) // sf + 1
         self.out_channel = out_channel
 
 
 class ConvFrontEnd(nn.Module):
-    """forward(x f32 [B,T,F], mask bool [B,T]) -> (f32 [B,T',D], bool [B,T'])   (frontend/conv.py:131-153)."""
+    """forward(x f32 [B,T,F], mask bool [B,T]) -> (f32 [B,T',D], bool [B,T'])   (frontend/conv.py:86-153).
+    Each layer's kernel_size and stride is an int or a [time, freq] pair, kernels 1..7 and strides 1..4
+    (conv_frontend_geometry)."""
 
     def __init__(self, input_size, output_size, in_channel=1, mid_channel=32, out_channel=128,
                  kernel_size=[[3, 3], [3, 3]], stride=[2, 2], dropout=0.0, act_func_type='relu',
@@ -103,10 +140,11 @@ class ConvFrontEnd(nn.Module):
         assert isinstance(stride, list) and len(stride) == 2
         if in_channel != 1:
             raise NotImplementedError('in_channel must be 1 (log-fbank input)')
-        if dropout:
-            raise NotImplementedError('frontend dropout > 0 is a training feature (round 2)')
         self.input_size, self.output_size = input_size, output_size
         self.front_end_layer_norm = front_end_layer_norm
+        self.dropout = dropout
+        self.layers = tuple(_conv_pair(k) + _conv_pair(s) for k, s in zip(kernel_size, stride))
+        self.geom = conv_frontend_geometry(self.layers)['geom']
         self.conv1 = Conv2dLayer(input_size, in_channel, mid_channel, kernel_size[0], stride[0], dropout)
         self.conv2 = Conv2dLayer(self.conv1.output_size, mid_channel, out_channel, kernel_size[1], stride[1], dropout)
         self.conv_output_size = self.conv2.output_size * out_channel
@@ -120,37 +158,42 @@ class ConvFrontEnd(nn.Module):
         c2 = self.conv2.conv_layer
         C1, C2 = c1.out_channels, c2.out_channels
         F2 = self.conv2.output_size
+        kt1, kf1, _, _, kt2, kf2, _, _ = self.geom
         C1p = (C1 + 63) // 64 * 64          # one 128-byte tap per k-block needs 64-channel multiples
-        w1 = torch.zeros(C1p, 1, 3, 3, device=c1.weight.device)
+        w1 = torch.zeros(C1p, 1, kt1, kf1, device=c1.weight.device)
         w1[:C1] = c1.weight.detach().float()
         b1 = torch.zeros(C1p, device=c1.weight.device)
         b1[:C1] = c1.bias.detach().float()
-        w2 = torch.zeros(C2, 3, 3, C1p, device=c1.weight.device)
-        w2[..., :C1] = c2.weight.detach().float().permute(0, 2, 3, 1)   # [C2,kh,kw,C1]: k = (kh*3+kw)*C1 + c
+        w2 = torch.zeros(C2, kt2, kf2, C1p, device=c1.weight.device)
+        w2[..., :C1] = c2.weight.detach().float().permute(0, 2, 3, 1)   # [C2,kh,kw,C1]: k = (kh*kf2+kw)*C1 + c
         # reference feature index is c*F2 + f (conv.py:145); conv2 kernel emits f*C2 + c -> permute columns once
         wo = self.output_layer.weight.detach().float().view(self.output_size, C2, F2).permute(0, 2, 1)
         pk = {'w1': w1.contiguous(), 'b1': b1.contiguous(), 'C1p': C1p,
-              'w2': w2.reshape(C2, 9 * C1p).to(BF16).contiguous(), 'b2': c2.bias.detach().float().contiguous(),
+              'w2': w2.reshape(C2, kt2 * kf2 * C1p).to(BF16).contiguous(), 'b2': c2.bias.detach().float().contiguous(),
               'wo': wo.reshape(self.output_size, F2 * C2).to(BF16).contiguous(), 'bo': _b(self.output_layer)}
         if self.front_end_layer_norm:
             pk['ln'] = _ln(self.layer_norm)
         return pk
 
+    def sizes(self, T):
+        """[(T1, F1), (T2, F2)] for T input frames (ValueError when too short)."""
+        return conv_frontend_geometry(self.layers, T, self.input_size)['sizes']
+
     def output_length(self, T):
         """T input frames -> T' output frames."""
-        return ops.conv_geometry(T, self.input_size)[2]
+        return self.sizes(T)[1][0]
 
     def input_window(self):
-        """(stride, width): output frame t sees input frames [stride t, stride t + width) (two 3x3 stride-2 convolutions
-        that do not pad in time)."""
-        return 4, 7
+        """(stride, width): output frame t sees input frames [stride t, stride t + width) (the convolutions do not pad in
+        time): (4, 7) for two 3x3 stride-2 layers."""
+        return conv_frontend_geometry(self.layers)['window']
 
     def output_mask(self, mask):
-        # Conv2dLayer.return_output_mask twice (frontend/conv.py:78-83): mask[:, 1::2][:, :t]
-        t2 = self.output_length(mask.shape[1])
-        t1 = (mask.shape[1] - 3) // 2 + 1
-        m = mask[:, 1::2][:, :t1]
-        return m[:, 1::2][:, :t2]
+        # Conv2dLayer.return_output_mask per layer (frontend/conv.py:78-83): mask[:, kt//2::st][:, :t]
+        g = conv_frontend_geometry(self.layers, mask.shape[1], self.input_size)
+        for (start, step), (t, _) in zip(g['mask'], g['sizes']):
+            mask = mask[:, start::step][:, :t]
+        return mask
 
     def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
         """x f32 [B,T,F] -> bf16 [B*T', D].  When posenc_* are given, x*scale+PE is fused into the Linear
@@ -161,9 +204,9 @@ class ConvFrontEnd(nn.Module):
         if F != self.input_size:
             raise ValueError(f'expected {self.input_size} features, got {F}')
         x = x.contiguous().float()
-        _, _, T2, F2 = ops.conv_geometry(T, F)
-        h1 = ops.conv1_relu(x, pk['w1'], pk['b1'])
-        h2 = ops.conv2_relu(h1, pk['w2'], pk['b2'], B, T, F)
+        T2 = self.output_length(T)
+        h1 = ops.conv1_relu(x, pk['w1'], pk['b1'], geom=self.geom)
+        h2 = ops.conv2_relu(h1, pk['w2'], pk['b2'], B, T, F, geom=self.geom)
         if posenc_table is not None and not self.front_end_layer_norm:
             y = ops.linear(h2, pk['wo'], pk['bo'], EPI_TABLE, alpha=posenc_scale, table=posenc_table, period=T2)
         else:

@@ -95,29 +95,41 @@ def conv_geometry(T, F):
     return t1.value, f1.value, t2.value, f2.value
 
 
-def conv1_relu(x, w, bias, out=None):
-    """x f32 [B,T,F]; w f32 [C1,1,3,3] -> bf16 NHWC [B, 2*(T2+1), 2*F2, C1]."""
+# (kt1, kf1, st1, sf1, kt2, kf2, st2, sf2) of the shipped conv front end: two 3x3 convolutions at stride 2
+CONV_SHIPPED = (3, 3, 2, 2, 3, 3, 2, 2)
+
+
+def conv_sizes(T, F, geom=CONV_SHIPPED):
+    """otb_conv_geometry2 -> (T1, F1, T2, F2, T1p, F1p): the two layers' output sizes and the conv1 activation buffer's rows
+    and columns.  The front end's own geometry (modules.conv_frontend_geometry) is what callers size their outputs by."""
+    out = (ctypes.c_int * 6)()
+    check(_lib.lib().otb_conv_geometry2(T, F, *geom, out), 'otb_conv_geometry2')
+    return tuple(out)
+
+
+def conv1_relu(x, w, bias, out=None, geom=CONV_SHIPPED):
+    """x f32 [B,T,F]; w f32 [C1,1,kt1,kf1] -> bf16 NHWC [B, T1p, F1p, C1] (conv_sizes; [B, 2*(T2+1), 2*F2, C1] shipped)."""
     _need(x, torch.float32, 'x'); _need(w, torch.float32, 'w'); _need(bias, torch.float32, 'bias')
     B, T, F = x.shape
     C1 = w.shape[0]
-    _, _, T2, F2 = conv_geometry(T, F)
+    T1p, F1p = conv_sizes(T, F, geom)[4:]
     if out is None:
-        out = torch.empty(B, 2 * (T2 + 1), 2 * F2, C1, dtype=BF16, device=x.device)
-    check(_lib.lib().otb_conv1_relu(_p(x), _p(w), _p(bias), _p(out), B, T, F, C1, _stream()), 'otb_conv1_relu')
+        out = torch.empty(B, T1p, F1p, C1, dtype=BF16, device=x.device)
+    check(_lib.lib().otb_conv1_relu2(_p(x), _p(w), _p(bias), _p(out), B, T, F, C1, *geom, _stream()), 'otb_conv1_relu')
     _count()
     return out
 
 
-def conv2_relu(h1, w, bias, B, T, F, out=None):
-    """h1 = conv1 buffer; w bf16 [C2, 9*C1] (kh,kw,c order) -> bf16 [B*T2, F2*C2] (feature = f*C2 + c)."""
+def conv2_relu(h1, w, bias, B, T, F, out=None, geom=CONV_SHIPPED):
+    """h1 = conv1 buffer; w bf16 [C2, kt2*kf2*C1] (kh,kw,c order) -> bf16 [B*T2, F2*C2] (feature = f*C2 + c)."""
     _need(h1, BF16, 'h1'); _need(w, BF16, 'w'); _need(bias, torch.float32, 'bias')
     C2, K = w.shape
-    C1 = K // 9
-    _, _, T2, F2 = conv_geometry(T, F)
+    C1 = K // (geom[4] * geom[5])
+    _, _, T2, F2, _, _ = conv_sizes(T, F, geom)
     if out is None:
         out = torch.empty(B * T2, F2 * C2, dtype=BF16, device=h1.device)
     with _Timed('conv2_gemm', 2.0 * B * T2 * F2 * C2 * K):
-        check(_lib.lib().otb_conv2_relu(_p(h1), _p(w), _p(bias), _p(out), B, T, F, C1, C2, _stream()),
+        check(_lib.lib().otb_conv2_relu2(_p(h1), _p(w), _p(bias), _p(out), B, T, F, C1, C2, *geom, _stream()),
               'otb_conv2_relu')
     _count()
     return out
@@ -998,24 +1010,25 @@ def mwer_grad(logits, V, target, tok_lp, coeff):
     return out
 
 
-def conv_im2col(h1, B, T, F, C1):
-    _, _, T2, F2 = conv_geometry(T, F)
-    col = torch.empty(B * T2 * F2, 9 * C1, dtype=BF16, device=h1.device)
-    check(_lib.lib().otb_conv_im2col(_p(h1), _p(col), B, T, F, C1, _stream()), 'otb_conv_im2col')
+def conv_im2col(h1, B, T, F, C1, geom=CONV_SHIPPED):
+    _, _, T2, F2, _, _ = conv_sizes(T, F, geom)
+    col = torch.empty(B * T2 * F2, geom[4] * geom[5] * C1, dtype=BF16, device=h1.device)
+    check(_lib.lib().otb_conv_im2col2(_p(h1), _p(col), B, T, F, C1, *geom, _stream()), 'otb_conv_im2col')
     _count()
     return col
 
 
-def conv_col2im_relu(dcol, h1, B, T, F, C1):
+def conv_col2im_relu(dcol, h1, B, T, F, C1, geom=CONV_SHIPPED):
     dpre1 = torch.empty_like(h1)
-    check(_lib.lib().otb_conv_col2im_relu(_p(dcol), _p(h1), _p(dpre1), B, T, F, C1, _stream()), 'otb_conv_col2im_relu')
+    check(_lib.lib().otb_conv_col2im_relu2(_p(dcol), _p(h1), _p(dpre1), B, T, F, C1, *geom, _stream()), 'otb_conv_col2im_relu')
     _count()
     return dpre1
 
 
-def conv1_wgrad(dpre1, x, B, T, F, C1):
-    out = torch.empty(C1, 10, dtype=torch.float32, device=x.device)
-    check(_lib.lib().otb_conv1_wgrad(_p(dpre1), _p(x), _p(out), B, T, F, C1, _stream()), 'otb_conv1_wgrad')
+def conv1_wgrad(dpre1, x, B, T, F, C1, geom=CONV_SHIPPED):
+    """-> f32 [C1, kt1*kf1 + 1]: conv1's tap gradients, then its bias gradient."""
+    out = torch.empty(C1, geom[0] * geom[1] + 1, dtype=torch.float32, device=x.device)
+    check(_lib.lib().otb_conv1_wgrad2(_p(dpre1), _p(x), _p(out), B, T, F, C1, *geom, _stream()), 'otb_conv1_wgrad')
     _count()
     return out
 

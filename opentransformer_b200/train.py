@@ -27,7 +27,8 @@ the dropout seed of THIS pass (read on the device), required when a dropout rate
 makes `model(inputs, targets)[0].backward()` populate `.grad` of the fp32 master parameters exactly like the reference
 module; loss_train_mode is the same pass without gradients, and FusedTrainer's micro-step is train_pass into its grad_sink.
 
-Scope: the shipped Speech-Transformer configuration -- conv front end, post-norm Transformer encoder / decoder with GLU
+Scope: the shipped Speech-Transformer configuration -- conv front end (any kernel and stride its kernels take, with or
+without front_end_layer_norm; its dropout must be 0), post-norm Transformer encoder / decoder with GLU
 feed-forward, tied or untied output layer, `residual_dropout` as shipped (0.1: counter-based masks in the residual GEMM's
 epilogue, replayed in the backward; csrc/dropout.cuh); the other dropout rates must be 0 (as shipped) and raise
 otherwise.  The encoder may also be the shipped Conformer layout with 64-wide heads (macaron feed-forward, rel-pos
@@ -144,10 +145,15 @@ class EncoderPack(LayerPack):
             if (C1 + 63) // 64 * 64 > 256:       # the conv1 weight gradient (otb_conv1_wgrad) runs one channel per thread
                 raise NotImplementedError(f'training path: mid_channel {C1} pads to {(C1 + 63) // 64 * 64} channels; the conv1 '
                                           'weight gradient takes at most 256')
+            if fe.dropout > 0.0:
+                raise NotImplementedError(f'training path: front-end dropout {fe.dropout} is not implemented; set it to 0.0')
+            if fe.front_end_layer_norm and (fe.output_size > 256 or fe.output_size % 8):
+                raise NotImplementedError(f'training path: front_end_layer_norm over output_size {fe.output_size}; its '
+                                          'backward (otb_layernorm_bwd) takes a multiple of 8, at most 256')
         if self.conformer:
             _check_conformer(enc)
-        if getattr(fe, 'front_end_layer_norm', False) or any(stack.pos_emb.scale_learnable for _, stack in stacks):
-            raise NotImplementedError('training path: front_end_layer_norm / learnable positional scale (pos_dropout > 0)')
+        if any(stack.pos_emb.scale_learnable for _, stack in stacks):
+            raise NotImplementedError('training path: learnable positional scale (pos_dropout > 0)')
         self.rates = {name: check_blocks(stack.blocks) for name, stack in stacks}
         self.fe = self._frontend(fe)
         self.enc = [self._conf_layer(b) if self.conformer else self.enc_layer(b) for b in enc.blocks]
@@ -163,8 +169,10 @@ class EncoderPack(LayerPack):
         if isinstance(fe, ConcatFeatureFrontEnd):
             return {}
         pk = dict(fe._build_pack())
-        pk['w2_t'] = pk['w2'].t().contiguous()           # [9*C1p, C2]
+        pk['w2_t'] = pk['w2'].t().contiguous()           # [kt2*kf2*C1p, C2]
         pk['wo_t'] = pk['wo'].t().contiguous()           # [F2*C2, D]
+        if fe.front_end_layer_norm:
+            pk['ln'] = self._ln(fe.layer_norm)
         return pk
 
     def _conf_layer(self, b):
@@ -550,9 +558,9 @@ def embedding_bwd(tok, dx, emb, scale, g, name):
     ops.embed_bwd(tok, dx, g[name], scale)
 
 
-# h1, h2: the conv front end's activations (h2 the input of its Linear); for concat-with-linear h2 holds the stacked rows,
-# the input of its Linear, and h1 is None; for concat both are None
-_EncTrace = namedtuple('_EncTrace', 'x_in h1 h2 tape pe scale lengths enc_last drops B T F T2 F2')
+# h1, h2: the conv front end's activations (h2 the input of its Linear, y its output when front_end_layer_norm follows);
+# for concat-with-linear h2 holds the stacked rows, the input of its Linear, and h1 is None; for concat all are None
+_EncTrace = namedtuple('_EncTrace', 'x_in h1 h2 y tape pe scale lengths enc_last drops B T F T2 F2')
 
 
 def _encoder_fwd(model, pk, inputs, mask, drop_seed):
@@ -571,17 +579,22 @@ def _encoder_fwd(model, pk, inputs, mask, drop_seed):
     if enc.fuse_abs_posenc():
         scale, table = enc.pos_emb.scale_and_table(T2, dev)
     # rel-pos encoders take the front end's output as is (encoder/conformer.py:141-149)
-    h1, h2, F2 = None, None, None
+    h1, h2, y, F2 = None, None, None, None
     if isinstance(fe, ConvFrontEnd):
-        F2 = ops.conv_geometry(T, F)[3]
-        h1 = ops.conv1_relu(x_in, fpk['w1'], fpk['b1'])
-        h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F)                   # [B*T2, F2*C2]
+        F2 = fe.sizes(T)[1][1]
+        h1 = ops.conv1_relu(x_in, fpk['w1'], fpk['b1'], geom=fe.geom)
+        h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F, geom=fe.geom)    # [B*T2, F2*C2]
         lin = (fpk['wo'], fpk['bo'])
     elif isinstance(fe, ConcatWithLinearFrontEnd):
         h2 = ops.frame_stack(x_in, fe.nframes, fe.stride, T2)                     # [B*T2, n F rounded up to 8]
         lin = (fpk['w'], fpk['b'])
     if h2 is None:      # concat: the stacked frames are the encoder's input
         x = ops.frame_stack(x_in, fe.nframes, fe.stride, T2, 1.0 if scale is None else scale, table)
+    elif 'ln' in fpk:   # front_end_layer_norm (conv.py:150-151), then the encoder's scale and positions
+        y = ops.linear(h2, *lin, EPI_BIAS)
+        x = _norm(y, fpk['ln'])
+        if scale is not None:
+            x = ops.scale_add_table(x, scale, table, T2)
     elif scale is not None:
         x = ops.linear(h2, *lin, EPI_TABLE, alpha=scale, table=table, period=T2)
     else:
@@ -599,7 +612,7 @@ def _encoder_fwd(model, pk, inputs, mask, drop_seed):
     if conformer:       # the running statistics moved: the inference pack, which folds BatchNorm, must be rebuilt
         modules.bump_param_generation()
     mem = _norm(x, pk.enc_norm) if pk.enc_pre else x
-    return mem, _EncTrace(x_in=x_in, h1=h1, h2=h2, tape=enc_tape, pe=pe, scale=scale, lengths=lengths, enc_last=x, drops=e_drop,
+    return mem, _EncTrace(x_in=x_in, h1=h1, h2=h2, y=y, tape=enc_tape, pe=pe, scale=scale, lengths=lengths, enc_last=x, drops=e_drop,
                           B=B, T=T, F=F, T2=T2, F2=F2)
 
 
@@ -630,24 +643,27 @@ def _encoder_bwd(model, pk, tr, dx, g):
             g['frontend.linear.bias'] = ops.colsum(dyl, out=g.out('frontend.linear.bias'), accumulate=acc)
         return
     C1p, C2 = fpk['C1p'], fpk['w2'].shape[0]
+    kt1, kf1, _, _, kt2, kf2, _, _ = fe.geom
     dyl = ops.scale_add_table(dx, tr.scale) if tr.scale is not None else dx      # d(h2 Wo^T + bo) = sqrt(d) * dx
+    if tr.y is not None:                                                          # through front_end_layer_norm
+        dyl = _ln_bwd(dyl, tr.y, fpk['ln'], g)
     D_out = fe.output_size
     dwo = ops.linear_wgrad(dyl, h2)                                               # [D, F2*C2], feature index f*C2 + c
     g.put('frontend.output_layer.weight', dwo.view(D_out, F2, C2).permute(0, 2, 1).reshape(D_out, C2 * F2))
     g['frontend.output_layer.bias'] = ops.colsum(dyl, out=g.out('frontend.output_layer.bias'), accumulate=acc)
     dh2 = ops.linear(dyl, fpk['wo_t'])                                            # [B*T2, F2*C2]
     dpre2 = ops.relu_bwd(dh2, h2).view(B * T2 * F2, C2)
-    col = ops.conv_im2col(h1, B, T, F, C1p)
+    col = ops.conv_im2col(h1, B, T, F, C1p, geom=fe.geom)
     C1 = fe.conv1.conv_layer.out_channels
-    dw2 = ops.linear_wgrad(dpre2, col)                                            # [C2, 9*C1p], k = (kh*3+kw)*C1p + c
-    g.put('frontend.conv2.conv_layer.weight', dw2.view(C2, 3, 3, C1p)[..., :C1].permute(0, 3, 1, 2))
+    dw2 = ops.linear_wgrad(dpre2, col)                                            # [C2, kt2*kf2*C1p], k = (kh*kf2+kw)*C1p + c
+    g.put('frontend.conv2.conv_layer.weight', dw2.view(C2, kt2, kf2, C1p)[..., :C1].permute(0, 3, 1, 2))
     g['frontend.conv2.conv_layer.bias'] = ops.colsum(dpre2, out=g.out('frontend.conv2.conv_layer.bias'), accumulate=acc)
-    dcol = ops.linear(dpre2, fpk['w2_t'])                                         # [B*T2*F2, 9*C1p]
+    dcol = ops.linear(dpre2, fpk['w2_t'])                                         # [B*T2*F2, kt2*kf2*C1p]
     del col
-    dpre1 = ops.conv_col2im_relu(dcol, h1, B, T, F, C1p)
-    g1 = ops.conv1_wgrad(dpre1, tr.x_in, B, T, F, C1p)                            # [C1p, 9 taps + bias]
-    g.put('frontend.conv1.conv_layer.weight', g1[:C1, :9].reshape(C1, 1, 3, 3))
-    g.put('frontend.conv1.conv_layer.bias', g1[:C1, 9])
+    dpre1 = ops.conv_col2im_relu(dcol, h1, B, T, F, C1p, geom=fe.geom)
+    g1 = ops.conv1_wgrad(dpre1, tr.x_in, B, T, F, C1p, geom=fe.geom)              # [C1p, kt1*kf1 taps + bias]
+    g.put('frontend.conv1.conv_layer.weight', g1[:C1, :kt1 * kf1].reshape(C1, 1, kt1, kf1))
+    g.put('frontend.conv1.conv_layer.bias', g1[:C1, kt1 * kf1])
 
 
 def _ctc_head(model, pk):
