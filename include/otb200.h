@@ -104,14 +104,18 @@ int otb_gemm_config(int M, int N, int epilogue, int out_f32, int* bn);
  * decoder/transformer.py:36-38 `residual_dropout`): out bf16 = resid + alpha * keep * (a w^T + bias) / (1 - p), where
  * keep(seed, site, row, col) is a counter-based Bernoulli(1-p) mask (csrc/dropout.cuh) -- a pure function of the per-step
  * seed (*seed is read on the DEVICE at run time, so a captured CUDA graph draws a fresh mask per replay), the dropout
- * site id and the element, so the backward replays it instead of storing it. */
+ * site id and the element, so the backward replays it instead of storing it.
+ * (p2, site2): a second, independent mask on the same tensor -- the attention's own dropout on its projected output
+ * (attention.py:46, `slf_attn_dropout` / `src_attn_dropout`) under the residual dropout:
+ *   out = resid + alpha * keep(site) * keep2(site2) * (a w^T + bias) / ((1 - p) (1 - p2)).
+ * p2 = 0 is exactly the one-mask call; p = 0 < p2 draws site2's mask alone. */
 int otb_linear_dropout_resid(const void* a, int lda, const void* w, int ldw, const float* bias, void* out, int ldc, int M, int N,
                              int K, const void* resid, int ldr, float alpha, float p, const uint32_t* seed, uint32_t site,
-                             void* stream);
-/* Backward of that dropout: out = dy * keep / (1 - p) (bf16 [M,N]); mask (optional, u8 [M,N]) receives keep -- with dy / out
- * NULL this only exports the mask (parity tests replay it in the oracle). */
+                             float p2, uint32_t site2, void* stream);
+/* Backward of that dropout: out = dy * keep * keep2 / ((1 - p) (1 - p2)) (bf16 [M,N]); mask (optional, u8 [M,N]) receives
+ * keep * keep2 -- with dy / out NULL this only exports the mask (parity tests replay it in the oracle). */
 int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask, int M, int N, float p, const uint32_t* seed,
-                    uint32_t site, void* stream);
+                    uint32_t site, float p2, uint32_t site2, void* stream);
 
 /* Fused masked multi-head attention (attention.py:80,34-41): for batch b, head h
  *   out[b*Tq+i, h*d_k:(h+1)*d_k] = softmax_j((q_i . k_j + bd) / sqrt(d_k), j < kv_len[b], causal: j <= i) V
@@ -304,6 +308,11 @@ int otb_layernorm_bwd(const void* dy, int lddy, const void* z, int ldz, const fl
 /* F.glu (ffn.py:18) un-fused for training: u = [a | g] bf16 [M,2F] -> h [M,F]; and its backward. */
 int otb_glu_fwd(const void* u, void* h, int M, int F, void* stream);
 int otb_glu_bwd(const void* dh, const void* u, void* du, int M, int F, void* stream);
+/* The other feed-forward activations (ffn.py:15-41) un-fused for training: h = act(u) and du = dh * act'(u), bf16 [M,N]
+ * contiguous and 16-byte aligned (any M, N >= 1), fp32 math.  act: OTB_EPI_GELU (F.gelu, erf form: act' = Phi(u) +
+ * u phi(u)), OTB_EPI_TANH or OTB_EPI_SWISH (u sigmoid(u)). */
+int otb_act_fwd(const void* u, void* h, int M, int N, int act, void* stream);
+int otb_act_bwd(const void* dh, const void* u, void* du, int M, int N, int act, void* stream);
 /* ReLU backward through the output (frontend/conv.py:64). */
 int otb_relu_bwd(const void* dy, const void* y, void* dx, long long n, void* stream);
 /* nn.Embedding backward: dE[tok[n]] += scale * dx[n]  (fp32 atomics). */

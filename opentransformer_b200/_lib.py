@@ -53,8 +53,8 @@ _SIGS = {
                            c_float, c_float, _P, c_int, _P, c_int, _P]),
     'otb_gemm_config': (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int)]),
     'otb_linear_dropout_resid': (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, c_float, c_float, _P,
-                                         ctypes.c_uint32, _P]),
-    'otb_dropout_bwd': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_float, _P, ctypes.c_uint32, _P]),
+                                         ctypes.c_uint32, c_float, ctypes.c_uint32, _P]),
+    'otb_dropout_bwd': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_float, _P, ctypes.c_uint32, c_float, ctypes.c_uint32, _P]),
     'otb_attention': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int,
                               _P, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P]),
     'otb_attention_probs': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int,
@@ -88,6 +88,8 @@ _SIGS = {
     'otb_layernorm_bwd': (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, _P, _P, c_float, c_int, c_int, c_int, _P]),
     'otb_glu_fwd': (c_int, [_P, _P, c_int, c_int, _P]),
     'otb_glu_bwd': (c_int, [_P, _P, _P, c_int, c_int, _P]),
+    'otb_act_fwd': (c_int, [_P, _P, c_int, c_int, c_int, _P]),
+    'otb_act_bwd': (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
     'otb_relu_bwd': (c_int, [_P, _P, _P, c_int64, _P]),
     'otb_embed_bwd': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_float, _P]),
     'otb_sumsq': (c_int, [_P, c_int64, _P, c_int, _P]),

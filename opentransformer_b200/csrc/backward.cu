@@ -183,6 +183,65 @@ const char* glu_launch(cudaStream_t st, const bf16* u, const bf16* dh, bf16* out
 }
 
 // ------------------------------------------------------------------------------------------------
+// The other feed-forward activations (ffn.py:15-41: w_2(dropout(act(w_1 x)))) for training, un-fused from the w_1 GEMM so
+// that the backward reads the bf16 pre-activation u:  h = act(u);  du = dh * act'(u).  ACT is the epilogue id of the same
+// activation (the recognition path fuses it into the GEMM epilogue):
+//   EPI_GELU   F.gelu, erf form          act'(u) = Phi(u) + u phi(u)
+//   EPI_TANH   torch.tanh                act'(u) = 1 - tanh(u)^2
+//   EPI_SWISH  u * sigmoid(u)            act'(u) = s (1 + u (1 - s)),  s = sigmoid(u)
+// bf16 [n] contiguous, fp32 math; thread = 8 elements (one 16-byte load per operand), the last thread takes n % 8 singly.
+// ------------------------------------------------------------------------------------------------
+template <int ACT>
+__device__ __forceinline__ float act_value(float x) {
+    if (ACT == EPI_GELU) return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
+    if (ACT == EPI_TANH) return tanhf(x);
+    return x / (1.0f + expf(-x));
+}
+template <int ACT>
+__device__ __forceinline__ float act_slope(float x) {
+    if (ACT == EPI_GELU) return 0.5f * (1.0f + erff(x * 0.70710678118654752f)) + x * 0.39894228040143268f * expf(-0.5f * x * x);
+    if (ACT == EPI_TANH) {
+        const float t = tanhf(x);
+        return 1.0f - t * t;
+    }
+    const float s = 1.0f / (1.0f + expf(-x));
+    return s * (1.0f + x * (1.0f - s));
+}
+template <int ACT, bool BWD>
+__global__ void __launch_bounds__(256) act_kernel(const bf16* __restrict__ u, const bf16* __restrict__ dh, bf16* __restrict__ out,
+                                                  size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i * 8 + 8 <= n) {
+        float v[8], d[8];
+        unpack8(reinterpret_cast<const uint4*>(u)[i], v);
+        if (BWD) unpack8(reinterpret_cast<const uint4*>(dh)[i], d);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = BWD ? d[j] * act_slope<ACT>(v[j]) : act_value<ACT>(v[j]);
+        reinterpret_cast<uint4*>(out)[i] = pack8(v);
+    } else {
+        for (size_t e = i * 8; e < n; ++e) {
+            const float x = __bfloat162float(u[e]);
+            out[e] = __float2bfloat16(BWD ? __bfloat162float(dh[e]) * act_slope<ACT>(x) : act_value<ACT>(x));
+        }
+    }
+}
+template <int ACT>
+static const char* act_launch_t(cudaStream_t st, const bf16* u, const bf16* dh, bf16* out, size_t n) {
+    const unsigned grid = (unsigned)((n + 8 * 256 - 1) / (8 * 256));
+    return dh ? launch<act_kernel<ACT, true>>(grid, 256, 0, st, u, dh, out, n) : launch<act_kernel<ACT, false>>(grid, 256, 0, st, u, dh, out, n);
+}
+const char* act_launch(cudaStream_t st, int act, const bf16* u, const bf16* dh, bf16* out, size_t n) {
+    if (((reinterpret_cast<uintptr_t>(u) | reinterpret_cast<uintptr_t>(dh) | reinterpret_cast<uintptr_t>(out)) & 15))
+        return "act: operands must be 16-byte aligned";
+    switch (act) {
+        case EPI_GELU: return act_launch_t<EPI_GELU>(st, u, dh, out, n);
+        case EPI_TANH: return act_launch_t<EPI_TANH>(st, u, dh, out, n);
+        case EPI_SWISH: return act_launch_t<EPI_SWISH>(st, u, dh, out, n);
+    }
+    return "act: the activation must be gelu, tanh or swish (OTB_EPI_GELU / TANH / SWISH)";
+}
+
+// ------------------------------------------------------------------------------------------------
 // ReLU backward through the OUTPUT (conv.py:64): dx = dy where y > 0 else 0; bf16, n multiple of 8; dx may alias dy.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) relu_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ y, bf16* __restrict__ dx, size_t n8) {
@@ -197,15 +256,23 @@ __global__ void __launch_bounds__(256) relu_bwd_kernel(const bf16* __restrict__ 
 }
 // Backward of the residual dropout (and the mask export for tests): out[m,n] = dy[m,n] * keep(seed, site, m, n) / (1-p);
 // mask (optional, u8 [M,N]) receives keep.  Same pure function as the forward GEMM epilogue (dropout.cuh): nothing was stored.
+// TWO: a second mask keep(seed, site2, m, n) on the same element (attention-output dropout under the residual dropout,
+// EPI_RESID_DROP2); scale is then 1 / ((1 - p) (1 - p2)).
+template <bool TWO>
 __global__ void __launch_bounds__(256) dropout_bwd_kernel(const bf16* __restrict__ dy, int lddy, bf16* __restrict__ out, int ldo,
                                                           unsigned char* __restrict__ mask, int M, int N, unsigned thresh, float scale,
-                                                          const unsigned* __restrict__ seed_ptr, unsigned site) {
+                                                          const unsigned* __restrict__ seed_ptr, unsigned site, unsigned thresh2,
+                                                          unsigned site2) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int row = (int)(i / (N / 2)), cp = (int)(i % (N / 2));
     if (row >= M) return;
     const unsigned seed = *seed_ptr;
-    const bool k0 = drop_keep(seed, site, (uint32_t)row, (uint32_t)(2 * cp), thresh);
-    const bool k1 = drop_keep(seed, site, (uint32_t)row, (uint32_t)(2 * cp + 1), thresh);
+    bool k0 = drop_keep(seed, site, (uint32_t)row, (uint32_t)(2 * cp), thresh);
+    bool k1 = drop_keep(seed, site, (uint32_t)row, (uint32_t)(2 * cp + 1), thresh);
+    if (TWO) {
+        k0 = k0 && drop_keep(seed, site2, (uint32_t)row, (uint32_t)(2 * cp), thresh2);
+        k1 = k1 && drop_keep(seed, site2, (uint32_t)row, (uint32_t)(2 * cp + 1), thresh2);
+    }
     if (mask) {
         mask[(size_t)row * N + 2 * cp] = k0 ? 1 : 0;
         mask[(size_t)row * N + 2 * cp + 1] = k1 ? 1 : 0;
@@ -216,13 +283,19 @@ __global__ void __launch_bounds__(256) dropout_bwd_kernel(const bf16* __restrict
     }
 }
 const char* dropout_bwd_launch(cudaStream_t st, const bf16* dy, int lddy, bf16* out, int ldo, unsigned char* mask, int M, int N, float p,
-                               const unsigned* seed, unsigned site) {
+                               const unsigned* seed, unsigned site, float p2, unsigned site2) {
     if (M < 1 || N < 2 || (N & 1) || (lddy & 1) || (ldo & 1)) return "dropout: N and the row pitches must be even";
-    if (!(p >= 0.f && p < 1.f)) return "dropout: p must be in [0, 1)";
+    if (!(p >= 0.f && p < 1.f) || !(p2 >= 0.f && p2 < 1.f)) return "dropout: p must be in [0, 1)";
     if (!seed) return "dropout: null seed";
     const size_t n = (size_t)M * (N / 2);
-    return launch<dropout_bwd_kernel>((unsigned)((n + 255) / 256), 256, 0, st, dy, lddy, out, ldo, mask, M, N,
-                                      drop_threshold(p), 1.0f / (1.0f - p), seed, site);
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    // as otb_linear_dropout_resid: two masks only when both rates are non-zero, else the one with a rate (or p's)
+    if (p > 0.f && p2 > 0.f)
+        return launch<dropout_bwd_kernel<true>>(grid, 256, 0, st, dy, lddy, out, ldo, mask, M, N, drop_threshold(p),
+                                                drop_scale2(p, p2), seed, site, drop_threshold(p2), site2);
+    if (p == 0.f && p2 > 0.f) { p = p2; site = site2; }
+    return launch<dropout_bwd_kernel<false>>(grid, 256, 0, st, dy, lddy, out, ldo, mask, M, N, drop_threshold(p), 1.0f / (1.0f - p),
+                                             seed, site, 0u, 0u);
 }
 
 // out = resid + alpha * dropout_p(rowmask(x)) without a GEMM in front (rel-pos attention has no output projection; the

@@ -199,10 +199,14 @@ int otb_gemm_config(int M, int N, int epilogue, int out_f32, int* bn) {
 }
 
 int otb_linear_dropout_resid(const void* a, int lda, const void* w, int ldw, const float* bias, void* out, int ldc, int M, int N, int K,
-                             const void* resid, int ldr, float alpha, float p_drop, const uint32_t* seed, uint32_t site, void* stream) {
+                             const void* resid, int ldr, float alpha, float p_drop, const uint32_t* seed, uint32_t site, float p2,
+                             uint32_t site2, void* stream) {
     if (!a || !w || !out || !resid || !seed) return fail("otb_linear_dropout_resid", "null operand");
-    if (!(p_drop >= 0.f && p_drop < 1.f)) return fail("otb_linear_dropout_resid", "p must be in [0, 1)");
+    if (!(p_drop >= 0.f && p_drop < 1.f) || !(p2 >= 0.f && p2 < 1.f)) return fail("otb_linear_dropout_resid", "p must be in [0, 1)");
     if (ldc < N) return fail("otb_linear_dropout_resid", "ldc < N");
+    // two masks only when both rates are non-zero; otherwise the one-mask instantiation with whichever rate is set
+    const bool two = p_drop > 0.f && p2 > 0.f;
+    if (p_drop == 0.f && p2 > 0.f) { p_drop = p2; site = site2; }
     GemmParams p;
     memset(&p, 0, sizeof(p));
     p.M = M; p.N = N; p.K = K;
@@ -211,14 +215,15 @@ int otb_linear_dropout_resid(const void* a, int lda, const void* w, int ldw, con
     p.resid = reinterpret_cast<const bf16*>(resid); p.ldr = ldr;
     p.alpha = alpha;
     p.drop_seed = seed; p.drop_site = site; p.drop_thresh = drop_threshold(p_drop); p.drop_scale = 1.0f / (1.0f - p_drop);
-    RET("otb_linear_dropout_resid", gemm_launch(ST(stream), a, lda, w, ldw, N, EPI_RESID, p, nullptr));
+    if (two) { p.drop_site2 = site2; p.drop_thresh2 = drop_threshold(p2); p.drop_scale = drop_scale2(p_drop, p2); }
+    RET("otb_linear_dropout_resid", gemm_launch(ST(stream), a, lda, w, ldw, N, two ? EPI_RESID_DROP2 : EPI_RESID, p, nullptr));
 }
 
 int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask, int M, int N, float p, const uint32_t* seed,
-                    uint32_t site, void* stream) {
+                    uint32_t site, float p2, uint32_t site2, void* stream) {
     if ((!dy || !out) && !mask) return fail("otb_dropout_bwd", "nothing to do");
     RET("otb_dropout_bwd", dropout_bwd_launch(ST(stream), reinterpret_cast<const bf16*>(dy), lddy, reinterpret_cast<bf16*>(out), ldo, mask, M, N,
-                                              p, seed, site));
+                                              p, seed, site, p2, site2));
 }
 
 int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
@@ -484,6 +489,18 @@ int otb_glu_bwd(const void* dh, const void* u, void* du, int M, int F, void* str
     if (!dh || !u || !du || M < 1 || F < 8) return fail("otb_glu_bwd", "bad arguments");
     RET("otb_glu_bwd", glu_launch(ST(stream), reinterpret_cast<const bf16*>(u), reinterpret_cast<const bf16*>(dh),
                                   reinterpret_cast<bf16*>(du), M, F));
+}
+
+int otb_act_fwd(const void* u, void* h, int M, int N, int act, void* stream) {
+    if (!u || !h || M < 1 || N < 1) return fail("otb_act_fwd", "bad arguments");
+    RET("otb_act_fwd", act_launch(ST(stream), act, reinterpret_cast<const bf16*>(u), nullptr, reinterpret_cast<bf16*>(h),
+                                  (size_t)M * (size_t)N));
+}
+
+int otb_act_bwd(const void* dh, const void* u, void* du, int M, int N, int act, void* stream) {
+    if (!dh || !u || !du || M < 1 || N < 1) return fail("otb_act_bwd", "bad arguments");
+    RET("otb_act_bwd", act_launch(ST(stream), act, reinterpret_cast<const bf16*>(u), reinterpret_cast<const bf16*>(dh),
+                                  reinterpret_cast<bf16*>(du), (size_t)M * (size_t)N));
 }
 
 int otb_relu_bwd(const void* dy, const void* y, void* dx, long long n, void* stream) {

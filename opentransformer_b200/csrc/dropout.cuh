@@ -25,5 +25,9 @@ inline uint32_t drop_threshold(float p) {
     const double t = (double)p * 4294967296.0;
     return t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
 }
+// the scale of two independent masks on one tensor (attention-output dropout under the residual dropout), rounded once
+inline float drop_scale2(float p, float p2) {
+    return (float)(1.0 / ((1.0 - (double)p) * (1.0 - (double)p2)));
+}
 
 }  // namespace otb

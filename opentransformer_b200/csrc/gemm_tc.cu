@@ -79,6 +79,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     constexpr int BM = Cfg::BM;
     constexpr int kEpiThreads = 128 * Cfg::NWG;
     constexpr int BN_OUT = (EPI == EPI_GLU) ? BN / 2 : BN;  // output columns per tile
+    constexpr bool kResid = EPI == EPI_RESID || EPI == EPI_RESID_DROP2;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -212,7 +213,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
             s_rowmap[rr] = ok ? out_row : -1;
         }
-        if (EPI == EPI_RESID || EPI == EPI_RESID_LN) {
+        if (kResid || EPI == EPI_RESID_LN) {
             // residual rows are contiguous (no conv mode); 16-byte chunks, up to 8 independent loads per thread
             if ((ncols & 7) == 0) {
                 const int cpr = ncols >> 3;                        // 16-byte chunks per row
@@ -363,7 +364,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         } else {
-            const uint32_t dseed = (EPI == EPI_RESID && p.drop_seed != nullptr) ? *p.drop_seed : 0u;
+            const uint32_t dseed = (kResid && p.drop_seed != nullptr) ? *p.drop_seed : 0u;
 #pragma unroll
             for (int jj = 0; jj < BN / 8; ++jj) {
                 if (jj * 8 >= ncols) break;
@@ -372,7 +373,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     const int c = jj * 8 + cq;
                     uint8_t* row_ptr = stg + (rl0 + 8 * hh) * pitch;
                     float2 res = make_float2(0.f, 0.f);
-                    if (EPI == EPI_RESID) res = unpack_bf16(*reinterpret_cast<const uint32_t*>(row_ptr + c * 2));
+                    if (kResid) res = unpack_bf16(*reinterpret_cast<const uint32_t*>(row_ptr + c * 2));
                     float v[2];
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -386,7 +387,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         if (!row_live[hh]) x = 0.f;
                         if (EPI == EPI_RESID && p.drop_seed != nullptr)   // nn.Dropout on the sub-layer output (transformer.py:54,61)
                             x = drop_keep(dseed, p.drop_site, (uint32_t)out_row[hh], (uint32_t)(col_base + c + e), p.drop_thresh) ? x * p.drop_scale : 0.f;
-                        if (EPI == EPI_RESID) x = (e ? res.y : res.x) + p.alpha * x;
+                        if (EPI == EPI_RESID_DROP2) {   // and, before it, the attention's own dropout on its output (attention.py:46)
+                            const uint32_t r = (uint32_t)out_row[hh], cc = (uint32_t)(col_base + c + e);
+                            x = (drop_keep(dseed, p.drop_site, r, cc, p.drop_thresh) && drop_keep(dseed, p.drop_site2, r, cc, p.drop_thresh2))
+                                    ? x * p.drop_scale : 0.f;
+                        }
+                        if (kResid) x = (e ? res.y : res.x) + p.alpha * x;
                         v[e] = x;
                     }
                     stage2(row_ptr, c, p.out_f32, v[0], v[1]);
@@ -544,6 +550,7 @@ static const char* launch_bn(cudaStream_t st, const CUtensorMap& ta, const CUten
         case EPI_GLU: return launch_inst<BN, EPI_GLU>(st, ta, tb, p, num_tiles);
         case EPI_TABLE: return launch_inst<BN, EPI_TABLE>(st, ta, tb, p, num_tiles);
         case EPI_RESID: return launch_inst<BN, EPI_RESID>(st, ta, tb, p, num_tiles);
+        case EPI_RESID_DROP2: return launch_inst<BN, EPI_RESID_DROP2>(st, ta, tb, p, num_tiles);
         case EPI_RESID_LN: return launch_inst<BN, EPI_RESID_LN>(st, ta, tb, p, num_tiles);
         case EPI_SWISH: return launch_inst<BN, EPI_SWISH>(st, ta, tb, p, num_tiles);
         case EPI_GELU: return launch_inst<BN, EPI_GELU>(st, ta, tb, p, num_tiles);
@@ -588,7 +595,7 @@ const char* gemm_tile(int m_tiles, int N, int epi, int out_f32, int* bn) {
         return "gemm: fused residual+LayerNorm epilogue needs N in {64,128,256}";
     if (epi == EPI_RESID_LN && out_f32) return "gemm: fused residual+LayerNorm epilogue writes bf16";
     // the residual tile is staged as bf16 in the rows the fp32 results would overwrite
-    if (epi == EPI_RESID && out_f32) return "gemm: residual epilogue writes bf16";
+    if ((epi == EPI_RESID || epi == EPI_RESID_DROP2) && out_f32) return "gemm: residual epilogue writes bf16";
     *bn = choose_bn(m_tiles, N, epi, out_f32);
     return *bn == 0 ? "gemm: no tile configuration" : nullptr;
 }
@@ -599,7 +606,7 @@ const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, 
     if (p.K % 8) return "gemm: K must be a multiple of 8";
     if (p.ldc % (p.out_f32 ? 4 : 8)) return "gemm: ldc must keep rows 16-byte aligned (ldc % 8 == 0 for bf16, % 4 for f32)";
     if (reinterpret_cast<uintptr_t>(p.out) & 15) return "gemm: out must be 16-byte aligned";
-    if ((epi == EPI_RESID || epi == EPI_RESID_LN) && ((p.ldr % 8) || (reinterpret_cast<uintptr_t>(p.resid) & 15)))
+    if ((epi == EPI_RESID || epi == EPI_RESID_DROP2 || epi == EPI_RESID_LN) && ((p.ldr % 8) || (reinterpret_cast<uintptr_t>(p.resid) & 15)))
         return "gemm: residual must be 16-byte aligned with ldr % 8 == 0";
     const int m_tiles = p.conv ? (p.conv_B * p.conv_T1h + p.conv_R - 1) / p.conv_R : (p.M + BM - 1) / BM;
     int bn = 0;

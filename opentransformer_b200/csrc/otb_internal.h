@@ -23,6 +23,9 @@ enum Epilogue : int {
     EPI_SWISH = 6,     // out = v * sigmoid(v), v = acc + bias
     EPI_GELU = 7,      // out = gelu(v) (erf form, as F.gelu)
     EPI_TANH = 8,      // out = tanh(v)
+    // internal (not an otb_linear epilogue): EPI_RESID with two independent dropout masks on (acc + bias), the
+    // attention's output dropout under the residual dropout (otb_linear_dropout_resid with both rates non-zero)
+    EPI_RESID_DROP2 = 9,
 };
 
 struct GemmParams {
@@ -57,7 +60,8 @@ struct GemmParams {
     // training-mode dropout of the projection BEFORE the residual add (EPI_RESID only): out = resid + alpha * keep * (.) / (1-p)
     const unsigned* drop_seed;    // device scalar, null = no dropout
     unsigned drop_site, drop_thresh;
-    float drop_scale;
+    float drop_scale;             // EPI_RESID_DROP2: 1 / ((1 - p) (1 - p2))
+    unsigned drop_site2, drop_thresh2;   // EPI_RESID_DROP2 only: the second mask
 };
 
 const char* gemm_launch(cudaStream_t st, const void* A, int lda, const void* W, int ldw, int w_rows, int epi,
@@ -129,7 +133,8 @@ const char* layernorm_bwd_launch(cudaStream_t st, const bf16* dy, int lddy, cons
 const char* glu_launch(cudaStream_t st, const bf16* u, const bf16* dh, bf16* out, int M, int F);
 const char* relu_bwd_launch(cudaStream_t st, const bf16* dy, const bf16* y, bf16* dx, size_t n);
 const char* dropout_bwd_launch(cudaStream_t st, const bf16* dy, int lddy, bf16* out, int ldo, unsigned char* mask, int M, int N, float p,
-                               const unsigned* seed, unsigned site);
+                               const unsigned* seed, unsigned site, float p2, unsigned site2);
+const char* act_launch(cudaStream_t st, int act, const bf16* u, const bf16* dh, bf16* out, size_t n);
 const char* embed_bwd_launch(cudaStream_t st, const long long* tok, const bf16* dx, float* dE, int N, int d, int vocab, float scale);
 const char* im2col_launch(cudaStream_t st, const bf16* h1, bf16* col, int B, const ConvGeom& g, int C);
 const char* col2im_relu_launch(cudaStream_t st, const bf16* dcol, const bf16* h1, bf16* dpre1, int B, const ConvGeom& g, int C);

@@ -14,6 +14,8 @@ from ._lib import check
 
 EPI_BIAS, EPI_RELU, EPI_GLU, EPI_TABLE, EPI_RESID, EPI_RESID_LN, EPI_SWISH, EPI_GELU, EPI_TANH = range(9)
 ACT_EPILOGUE = {'relu': EPI_RELU, 'glu': EPI_GLU, 'swish': EPI_SWISH, 'gelu': EPI_GELU, 'tanh': EPI_TANH}
+# the activations act_fwd / act_bwd take (training runs ReLU fused into the GEMM and GLU through glu_fwd / glu_bwd)
+TRAIN_ACT = {k: ACT_EPILOGUE[k] for k in ('gelu', 'tanh', 'swish')}
 BF16 = torch.bfloat16
 
 
@@ -164,28 +166,31 @@ def gemm_config(M, N, epilogue=EPI_BIAS, out_f32=False):
     return bn.value
 
 
-def linear_dropout_resid(a, w, bias, resid, p, seed, site, alpha=1.0, out=None):
+def linear_dropout_resid(a, w, bias, resid, p, seed, site, alpha=1.0, out=None, p2=0.0, site2=0):
     """out = resid + alpha * dropout_p(a @ w^T + bias): training-mode residual connection (otb_linear_dropout_resid).
-    seed: int32/uint32 device tensor [1] (read at run time), site: dropout site id."""
+    seed: int32/uint32 device tensor [1] (read at run time), site: dropout site id.  (p2, site2): a second independent
+    mask on the same tensor (the attention's output dropout): out = resid + alpha * dropout_p(dropout_p2(a @ w^T + bias))."""
     _mat(a, 'a'); _mat(w, 'w'); _mat(resid, 'resid')
     M, K = a.shape
     N = w.shape[0]
     if out is None:
         out = torch.empty(M, N, dtype=BF16, device=a.device)
     check(_lib.lib().otb_linear_dropout_resid(_p(a), a.stride(0), _p(w), w.stride(0), _p(bias), _p(out), out.stride(0), M, N, K,
-                                              _p(resid), resid.stride(0), alpha, float(p), _p(seed), int(site), _stream()),
+                                              _p(resid), resid.stride(0), alpha, float(p), _p(seed), int(site), float(p2), int(site2),
+                                              _stream()),
           'otb_linear_dropout_resid')
     _count()
     return out
 
 
-def dropout_bwd(dy, p, seed, site):
-    """dy * keep / (1 - p) with the mask of dropout site `site` replayed from (seed, site)."""
+def dropout_bwd(dy, p, seed, site, p2=0.0, site2=0):
+    """dy * keep / (1 - p) with the mask of dropout site `site` replayed from (seed, site); with p2 > 0 also the mask of
+    site2, as linear_dropout_resid drew them: dy * keep * keep2 / ((1 - p) (1 - p2))."""
     _need(dy, BF16, 'dy')
     M, N = dy.shape
     out = torch.empty_like(dy)
     check(_lib.lib().otb_dropout_bwd(_p(dy), dy.stride(0), _p(out), out.stride(0), None, M, N, float(p), _p(seed), int(site),
-                                     _stream()), 'otb_dropout_bwd')
+                                     float(p2), int(site2), _stream()), 'otb_dropout_bwd')
     _count()
     return out
 
@@ -208,11 +213,12 @@ def dropout_add(x, resid, p=0.0, seed=None, site=0, alpha=1.0, row_len=None, row
     return out
 
 
-def dropout_mask(M, N, p, seed, site):
-    """u8 [M,N] keep mask of a dropout site (parity tests replay it in the oracle)."""
+def dropout_mask(M, N, p, seed, site, p2=0.0, site2=0):
+    """u8 [M,N] keep mask of a dropout site (parity tests replay it in the oracle) -- any site, the attention-output sites
+    (train.ATTN_SITE + ...) included; with p2 > 0 the product of the masks of site and site2, as dropout_bwd applies it."""
     mask = torch.empty(M, N, dtype=torch.uint8, device=seed.device)
-    check(_lib.lib().otb_dropout_bwd(None, 0, None, 0, _p(mask), M, N, float(p), _p(seed), int(site), _stream()),
-          'otb_dropout_bwd')
+    check(_lib.lib().otb_dropout_bwd(None, 0, None, 0, _p(mask), M, N, float(p), _p(seed), int(site), float(p2), int(site2),
+                                     _stream()), 'otb_dropout_bwd')
     _count()
     return mask
 
@@ -608,6 +614,29 @@ def glu_bwd(dh, u):
     M, F2 = u.shape
     du = torch.empty(M, F2, dtype=BF16, device=u.device)
     check(_lib.lib().otb_glu_bwd(_p(dh), _p(u), _p(du), M, F2 // 2, _stream()), 'otb_glu_bwd')
+    _count()
+    return du
+
+
+def act_fwd(u, act):
+    """h = act(u) for act in 'gelu' (erf form), 'tanh', 'swish' (otb_act_fwd): the training feed-forward's activation,
+    un-fused from the w_1 GEMM so that u stays for the backward.  u bf16 [M, N] contiguous -> h bf16 [M, N]."""
+    _need(u, BF16, 'u')
+    M, N = u.shape
+    h = torch.empty_like(u)
+    check(_lib.lib().otb_act_fwd(_p(u), _p(h), M, N, TRAIN_ACT[act], _stream()), 'otb_act_fwd')
+    _count()
+    return h
+
+
+def act_bwd(dh, u, act):
+    """du = dh * act'(u) (otb_act_bwd), the backward of act_fwd."""
+    _need(u, BF16, 'u'); _need(dh, BF16, 'dh')
+    if dh.shape != u.shape:
+        raise ValueError(f'act_bwd: dh {tuple(dh.shape)} and u {tuple(u.shape)} differ')
+    M, N = u.shape
+    du = torch.empty_like(u)
+    check(_lib.lib().otb_act_bwd(_p(dh), _p(u), _p(du), M, N, TRAIN_ACT[act], _stream()), 'otb_act_bwd')
     _count()
     return du
 

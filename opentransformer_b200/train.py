@@ -28,11 +28,13 @@ makes `model(inputs, targets)[0].backward()` populate `.grad` of the fp32 master
 module; loss_train_mode is the same pass without gradients, and FusedTrainer's micro-step is train_pass into its grad_sink.
 
 Scope: the shipped Speech-Transformer configuration -- conv front end (any kernel and stride its kernels take, with or
-without front_end_layer_norm; its dropout must be 0), post-norm Transformer encoder / decoder with GLU
-feed-forward, tied or untied output layer, `residual_dropout` as shipped (0.1: counter-based masks in the residual GEMM's
-epilogue, replayed in the backward; csrc/dropout.cuh); the other dropout rates must be 0 (as shipped) and raise
-otherwise.  The encoder may also be the shipped Conformer layout with 64-wide heads (macaron feed-forward, rel-pos
-attention, then the convolution module with training-mode BatchNorm; encoder/conformer.py:75-89).
+without front_end_layer_norm; its dropout must be 0), post- or pre-norm Transformer encoder / decoder with any of the
+reference's feed-forward activations (glu, relu, gelu, tanh, swish), tied or untied output layer, `residual_dropout` as
+shipped (0.1: counter-based masks in the residual GEMM's epilogue, replayed in the backward; csrc/dropout.cuh) and the
+attention's output dropout (`slf_attn_dropout`, the decoder's `src_attn_dropout`: a second mask in the same epilogue);
+ffn_dropout and pos_dropout must be 0 (as shipped) and raise otherwise.  The encoder may also be the shipped Conformer
+layout with 64-wide heads (macaron feed-forward, rel-pos attention, then the convolution module with training-mode
+BatchNorm; encoder/conformer.py:75-89).
 The CTC-only model (model/ctc.py) is the front-end + encoder half (_encoder_fwd / _encoder_bwd) with the CTC head and
 otb_ctc_loss in place of the decoder; the Transformer language model is the encoder layer (enc_layer_fwd / enc_layer_bwd)
 under the causal mask.  All four models share the vocabulary head (head_fwd / head_bwd) and embedding_bwd.
@@ -95,24 +97,46 @@ def check_heads(name, d_model, blocks):
                                       f'with {blk.n_heads} heads')
 
 
+_ATTN_DROPOUT = ('slf_attn_dropout', 'src_attn_dropout')
+
+
 def check_blocks(blocks):
-    """The feed-forward and dropout rules of a stack of blocks -> the residual_dropout rate of every block."""
+    """The feed-forward and dropout rules of a stack of blocks -> the residual_dropout rate of every block (the attention
+    output's rates: attn_dropout_rates)."""
     out = []
     for blk in blocks:
-        if _ffn_of(blk).activation not in ('glu', 'relu'):
-            raise NotImplementedError('training path: GLU or ReLU feed-forward only')
+        if _ffn_of(blk).activation not in ('glu', 'relu') + tuple(ops.TRAIN_ACT):
+            raise NotImplementedError(f'training path: feed-forward activation {_ffn_of(blk).activation!r}')
         rates = getattr(blk, 'dropout_rates', {})
         # conv_dropout: the reference builds the Dropout and never applies it (module/conformer.py:34,36-57)
-        other = {k: v for k, v in rates.items() if k not in ('residual_dropout', 'conv_dropout') and float(v) > 0.0}
+        other = {k: v for k, v in rates.items() if k not in ('residual_dropout', 'conv_dropout') + _ATTN_DROPOUT and float(v) > 0.0}
         if other:
-            # the reference applies these in train mode (attention.py:45, ffn.py:40); training WITHOUT them would be a
-            # different network, so refuse instead of silently dropping the regulariser.  residual_dropout -- the only
-            # non-zero rate of the shipped configs -- IS implemented (otb_linear_dropout_resid / otb_dropout_bwd).
-            raise NotImplementedError(f'training path: only residual_dropout is implemented, got {other}; set them to 0.0')
+            # the reference applies these in train mode (ffn.py:40, pos.py); training WITHOUT them would be a different
+            # network, so refuse instead of silently dropping the regulariser.  residual_dropout and the attention output's
+            # dropout ARE implemented (otb_linear_dropout_resid / otb_dropout_bwd).
+            raise NotImplementedError(f'training path: only residual_dropout and the attention dropout are implemented, got '
+                                      f'{other}; set them to 0.0')
+        for k in ('residual_dropout',) + _ATTN_DROPOUT:
+            if not (0.0 <= float(rates.get(k, 0.0)) < 1.0):
+                raise ValueError(f'{k} must be in [0, 1)')
         out.append(float(rates.get('residual_dropout', 0.0)))
-        if not (0.0 <= out[-1] < 1.0):
-            raise ValueError('residual_dropout must be in [0, 1)')
     return out
+
+
+def attn_dropout_rates(blk):
+    """The attention-output dropout rate of each residual sub-layer of a block, in site order (attention.py:46: the
+    attention returns dropout(output_proj(context)), and the layer's residual dropout lands on top): a Transformer encoder
+    layer (slf_attn_dropout, 0 for the feed-forward), a decoder layer (slf_attn_dropout, src_attn_dropout, 0).  A
+    Conformer's rel-pos attention takes none (its constructor refuses a rate)."""
+    rates = getattr(blk, 'dropout_rates', {})
+    slf, src = float(rates.get('slf_attn_dropout', 0.0)), float(rates.get('src_attn_dropout', 0.0))
+    if hasattr(blk, 'src_attn'):
+        return (slf, src, 0.0)
+    return (0.0, 0.0, 0.0) if hasattr(blk, 'pre_ffn') else (slf, 0.0)
+
+
+def _flat(per_block):
+    return [r for rates in per_block for r in rates]
 
 
 def need_drop_seed(drop_seed, rates):
@@ -125,7 +149,8 @@ class EncoderPack(LayerPack):
     TrainPack.  Its constructor refuses what the training path does not cover, before any device work.  Where the model
     has a decoder the checks take it in beside the encoder, each rule over both stacks before the next rule, so that the
     refusal a configuration with two faults gets does not depend on the stack a fault sits in (96-wide decoder heads and a
-    320-channel front end: the heads).  `rates`: stack name -> the residual_dropout rate of every block."""
+    320-channel front end: the heads).  `rates`: stack name -> the residual_dropout rate of every block; `attn_rates`: stack
+    name -> attn_dropout_rates of every block."""
 
     def __init__(self, model, bf16_of=None):
         super().__init__(model, bf16_of)
@@ -155,6 +180,7 @@ class EncoderPack(LayerPack):
         if any(stack.pos_emb.scale_learnable for _, stack in stacks):
             raise NotImplementedError('training path: learnable positional scale (pos_dropout > 0)')
         self.rates = {name: check_blocks(stack.blocks) for name, stack in stacks}
+        self.attn_rates = {name: [attn_dropout_rates(b) for b in stack.blocks] for name, stack in stacks}
         self.fe = self._frontend(fe)
         self.enc = [self._conf_layer(b) if self.conformer else self.enc_layer(b) for b in enc.blocks]
         # pre-norm stacks end with one more LayerNorm (encoder/transformer.py:96-97,131-132; decoder/transformer.py:151-152,178-179)
@@ -291,8 +317,11 @@ def linear_bwd(dy, x, lin, grads, resid=None):
 
 # dropout site ids: Transformer encoder layer i -> 2 i + {0, 1}; Conformer block i -> 3 i + {0, 1, 2} (macaron feed-forward,
 # attention, convolution module); decoder layer i -> 1000 + 3 i + {0, 1, 2}; the same decoder layer in the MWER branch,
-# over the n-best (forward_backward's nbest) -> 4000 + 3 i + {0, 1, 2}, clear of the language models' 2000 + / 3000 + (lm.py)
+# over the n-best (forward_backward's nbest) -> 4000 + 3 i + {0, 1, 2}, clear of the language models' 2000 + / 3000 + (lm.py).
+# The attention-output mask of the sub-layer whose residual mask is site s is site ATTN_SITE + s: every residual range
+# above moved up by 5000, clear of all of them, so that turning the attention dropout on draws the same residual masks.
 ENC_SITE, DEC_SITE, MWER_SITE = 0, 1000, 4000
+ATTN_SITE = 5000
 
 
 def _enc_sites(enc):
@@ -301,18 +330,21 @@ def _enc_sites(enc):
 
 def _ffn_fwd(p, x):
     """First half of the position-wise feed-forward (ffn.py:38-41): returns (pre-activation u or None, hidden h)."""
-    if p['act'] == 'glu':
-        u = ops.linear(x, p['w1'].w, p['w1'].b)
-        return u, ops.glu_fwd(u)
-    return None, ops.linear(x, p['w1'].w, p['w1'].b, EPI_RELU)      # ReLU fused into the GEMM; its backward needs only h
+    if p['act'] == 'relu':
+        return None, ops.linear(x, p['w1'].w, p['w1'].b, EPI_RELU)  # ReLU fused into the GEMM; its backward needs only h
+    u = ops.linear(x, p['w1'].w, p['w1'].b)
+    return u, (ops.glu_fwd(u) if p['act'] == 'glu' else ops.act_fwd(u, p['act']))
 
 
 def _ffn_act_bwd(p, dh, u, h):
-    return ops.glu_bwd(dh, u) if p['act'] == 'glu' else ops.relu_bwd(dh, h)
+    if p['act'] == 'relu':
+        return ops.relu_bwd(dh, h)
+    return ops.glu_bwd(dh, u) if p['act'] == 'glu' else ops.act_bwd(dh, u, p['act'])
 
 
 def dropout_sites(model):
-    """[(site id, 'encoder' | 'decoder', rate)] of every residual-dropout site (what a parity test must replay)."""
+    """[(site id, 'encoder' | 'decoder', rate)] of every residual-dropout site (what a parity test must replay; the
+    attention-output sites: attn_dropout_sites)."""
     out = []
     n = _enc_sites(model.encoder)
     for i, b in enumerate(model.encoder.blocks):
@@ -322,24 +354,50 @@ def dropout_sites(model):
     return out
 
 
+def attn_dropout_sites(model):
+    """[(site id, 'encoder' | 'decoder', rate)] of every attention-output dropout site with a non-zero rate: the sub-layer
+    whose residual site is s draws its attention mask at ATTN_SITE + s (both masks on the same tensor)."""
+    out = []
+    n = _enc_sites(model.encoder)
+    for i, b in enumerate(model.encoder.blocks):
+        out += [(ATTN_SITE + ENC_SITE + n * i + k, 'encoder', r) for k, r in enumerate(attn_dropout_rates(b)) if r > 0.0]
+    for i, b in enumerate(model.decoder.blocks if getattr(model, 'decoder', None) is not None else []):
+        out += [(ATTN_SITE + DEC_SITE + 3 * i + k, 'decoder', r) for k, r in enumerate(attn_dropout_rates(b)) if r > 0.0]
+    return out
+
+
+def _drops(rates, attn_rates, seed, site0, per_layer):
+    """The `drop` of every layer of a stack: (residual rate, seed tensor, site id of the layer's sub-layer 0, attention-output
+    rate of each sub-layer)."""
+    return [(r, seed, site0 + per_layer * i, a) for i, (r, a) in enumerate(zip(rates, attn_rates))]
+
+
+def _attn_rate(drop, k):
+    """The attention-output dropout rate of sub-layer k; a drop of three (the language models') carries none."""
+    return drop[3][k] if len(drop) > 3 else 0.0
+
+
 def _resid(ctx, lin, x, drop, k, alpha=1.0):
-    """x + alpha * dropout(ctx W^T + b): the residual connection of sub-layer k in training mode (transformer.py:54,61).
-    drop = (rate, seed tensor, site id of the layer's sub-layer 0)."""
-    rate, seed, site = drop
-    if rate > 0.0:
-        return ops.linear_dropout_resid(ctx, lin.w, lin.b, x, rate, seed, site + k, alpha=alpha)
+    """x + alpha * dropout(ctx W^T + b): the residual connection of sub-layer k in training mode (transformer.py:54,61);
+    with an attention-output rate, the attention's own dropout first (attention.py:46).  drop = (rate, seed tensor, site id
+    of the layer's sub-layer 0[, attention-output rate of each sub-layer])."""
+    rate, seed, site = drop[:3]
+    pa = _attn_rate(drop, k)
+    if rate > 0.0 or pa > 0.0:
+        return ops.linear_dropout_resid(ctx, lin.w, lin.b, x, rate, seed, site + k, alpha=alpha, p2=pa, site2=ATTN_SITE + site + k)
     return ops.linear(ctx, lin.w, lin.b, EPI_RESID, resid=x, alpha=alpha)
 
 
 def _drop_bwd(dz, drop, k):
-    rate, seed, site = drop
-    return ops.dropout_bwd(dz, rate, seed, site + k) if rate > 0.0 else dz
+    rate, seed, site = drop[:3]
+    pa = _attn_rate(drop, k)
+    return ops.dropout_bwd(dz, rate, seed, site + k, p2=pa, site2=ATTN_SITE + site + k) if rate > 0.0 or pa > 0.0 else dz
 
 
 # What a layer saves for its backward.  Sub-layer k has input u_k and residual sum z_k = u_k + drop(f_k(u_k)).  Pre-norm
 # (the reference takes the residual AFTER the norm): u_1 = norm1(a), u_k+1 = norm_k+1(z_k), the output is z_last.
-# Post-norm: u_1 = a, u_k+1 = norm_k(z_k), the output is norm_last(z_last).  a is the layer input; ffn_u is the GLU's
-# pre-activation (None with ReLU) and h the feed-forward's hidden activation.
+# Post-norm: u_1 = a, u_k+1 = norm_k(z_k), the output is norm_last(z_last).  a is the layer input; ffn_u is the feed-forward's
+# pre-activation (None with ReLU, whose backward reads h) and h its hidden activation.
 _EncTape = namedtuple('_EncTape', 'a u1 qkv ctx lse z1 u2 ffn_u h z2')
 _DecTape = namedtuple('_DecTape', 'a u1 qkv ctx lse z1 u2 q kv ctx2 lse2 z2 u3 ffn_u h z3')
 
@@ -423,7 +481,7 @@ def _dec_layer_bwd(p, t, dout, dmem, mem, pre, g, B, H, L, T, lengths, drop, K=1
 
 
 # A Conformer block (encoder/conformer.py:75-89, macaron, rel-pos attention, then the convolution module):
-#   x1 = x0 + ffn_scale * drop(pre_ffn(y0)),  y0 = macaron_ffn_norm(x0)          (h: GLU / ReLU output, ffn_u: GLU input)
+#   x1 = x0 + ffn_scale * drop(pre_ffn(y0)),  y0 = macaron_ffn_norm(x0)          (h: activation output, ffn_u: its input)
 #   x2 = x1 + drop(relmha(y1)),               y1 = mha_norm(x1)                  (ext = [q+u | q+v | k | v], pproj = pos_proj(PE))
 #   x3 = x2 + drop(mask(conv(y2))),           y2 = conv_norm(x2)                 (cu: pointwise_conv1 output, g = GLU(cu),
 #                                                                                 c / stats: depthwise conv and BatchNorm statistics,
@@ -435,7 +493,7 @@ _ConfTape = namedtuple('_ConfTape', 'x0 y0 ffn_u h x1 y1 ext pproj ctx lse x2 y2
 def _conformer_block_fwd(p, x0, B, H, T, lengths, pe, drop):
     """One Conformer block in training mode -> (output, _ConfTape).  pe: bf16 PE[-(T-1) .. T-1]; the BatchNorm running
     statistics are updated on the device."""
-    rate, seed, site = drop
+    rate, seed, site = drop[:3]
     d = x0.shape[1]
     y0 = _norm(x0, p['mac_ln'])
     ffn_u, h = _ffn_fwd(p, y0)
@@ -505,7 +563,7 @@ def _relpos_attn_bwd(p, t, dctx, g, B, H, T, lengths, pe):
 
 def _conformer_block_bwd(p, t, dout, g, B, H, T, lengths, pe, drop):
     """Backward of _conformer_block_fwd: parameter gradients into g; returns the gradient of the block input."""
-    rate, seed, site = drop
+    rate, seed, site = drop[:3]
     acc = g.sink is not None
     dz = _ln_bwd(dout, t.z, p['final_ln'], g)
     dx3 = _ln_bwd(dz, t.x3, p['post_ln'], g)
@@ -599,8 +657,7 @@ def _encoder_fwd(model, pk, inputs, mask, drop_seed):
         x = ops.linear(h2, *lin, EPI_TABLE, alpha=scale, table=table, period=T2)
     else:
         x = ops.linear(h2, *lin, EPI_BIAS)
-    ns = _enc_sites(enc)
-    e_drop = [(r, drop_seed, ENC_SITE + ns * i) for i, r in enumerate(pk.rates['encoder'])]
+    e_drop = _drops(pk.rates['encoder'], pk.attn_rates['encoder'], drop_seed, ENC_SITE, _enc_sites(enc))
     enc_tape = []
     pe = enc._rel_pos(T2, dev) if conformer else None
     for p, drop in zip(pk.enc, e_drop):
@@ -734,7 +791,7 @@ def _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad
     n = ((tgt >= 0).sum(dim=1) - 1).to(torch.int32)                              # the length of y
     ref, ref_len = _mwer_references(truth, truth_length)
     err = ops.edit_distance(tgt, n, ref, ref_len, K)
-    drops = [(r, drop_seed, MWER_SITE + 3 * i) for i, r in enumerate(pk.rates['decoder'])]
+    drops = _drops(pk.rates['decoder'], pk.attn_rates['decoder'], drop_seed, MWER_SITE, 3)
     hyp_in = hyp_in.contiguous()
     y, last, tape = _dec_fwd(dec, pk, hyp_in, mem, B, K, Lp, T2, lengths, drops)
     logits = head_fwd(y, pk.wout, pk.bout, dec.ld_logits)
@@ -768,7 +825,7 @@ def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=T
         raise ValueError('forward_backward: ctc_weight > 0 needs truth_length')
     pk = TrainPack(model, bf16_of)
     dev = inputs.device
-    need_drop_seed(drop_seed, pk.rates['encoder'] + pk.rates['decoder'])
+    need_drop_seed(drop_seed, pk.rates['encoder'] + pk.rates['decoder'] + _flat(pk.attn_rates['encoder'] + pk.attn_rates['decoder']))
     ce_w = 1.0
     if nbest is not None:
         ce_w = float(mwer_ce_weight)
@@ -784,7 +841,7 @@ def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=T
     tgt_in = truth[:, :-1].contiguous()
     tgt_out = truth[:, 1:].contiguous()
     L = tgt_in.shape[1]
-    d_drop = [(r, drop_seed, DEC_SITE + 3 * i) for i, r in enumerate(pk.rates['decoder'])]
+    d_drop = _drops(pk.rates['decoder'], pk.attn_rates['decoder'], drop_seed, DEC_SITE, 3)
     y, dec_last, dec_tape = _dec_fwd(dec, pk, tgt_in, mem, B, 1, L, T2, lengths, d_drop)
     V = dec.vocab_size
     logits = head_fwd(y, pk.wout, pk.bout, dec.ld_logits)
@@ -836,7 +893,7 @@ def ctc_forward_backward(model, inputs, mask, truth, truth_length, want_grads=Tr
     if truth_length is None:
         raise ValueError('ctc_forward_backward: a CTCModel needs truth_length')
     pk = EncoderPack(model, bf16_of)
-    need_drop_seed(drop_seed, pk.rates['encoder'])
+    need_drop_seed(drop_seed, pk.rates['encoder'] + _flat(pk.attn_rates['encoder']))
     mem, tr = _encoder_fwd(model, pk, inputs, mask, drop_seed)
     V = model.vocab_size
     wc, bc, ld = _ctc_head(model, pk)
