@@ -451,6 +451,15 @@ int otb_ctc_prefix_score(const float* lp, int ld, int T, int V, const int32_t* i
 int otb_ctc_prefix_advance(const otb_beam_state* st, const int32_t* cand_id, int P, int T, const int32_t* in_len,
                            const float* gamma_cand, const float* psi_cand, float* gamma, float* psi, void* stream);
 
+/* CTC rescoring of an attention n-best (SpeechToTextRecognizer's apply_ctc_rescoring): out f32 [B*K] = log p_ctc(target_r |
+ * x_b) of target row r of utterance b = r / K, by the blank-extended forward recursion (log domain, fp32), one CTA per row.
+ * logp f32 [B*T, ld] the head's log-probs, of which the first in_len[b] (i32 [B], clamped to T) frames of utterance b count;
+ * targets i32 [B*K, Lp], 1 <= Lp <= 1024: a row's labels are its entries before the first negative one.  -inf where no
+ * alignment exists: a label equal to blank or outside [0, V), in_len <= 0, or too few frames for the labels and their
+ * repeats.  Forward only: no workspace. */
+int otb_ctc_nbest_score(const float* logp, int ld, int B, int T, int V, const int32_t* in_len, const int32_t* targets, int K,
+                        int Lp, int blank, float* out, void* stream);
+
 /* N-best rescoring (the recognizers' apply_rescoring / apply_lm_rescoring; no reference entry point computes it:
  * eval.py's -resc / -lm_resc / -rw are parsed and never used).
  * otb_token_logprob: out f32 [rows] = logits[r, target[r]] - logsumexp(logits[r, :V]) of logits f32 [rows, ld], 0 where

@@ -109,6 +109,7 @@ _SIGS = {
     'otb_ctc_prefix_score': (c_int, [_P, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P, c_int, _P, c_int, c_float, c_float,
                                      POINTER(BeamStateC), _P, _P, _P, _P, _P]),
     'otb_ctc_prefix_advance': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
+    'otb_ctc_nbest_score': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, _P]),
     'otb_token_logprob': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P]),
     'otb_nbest_rescore': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_float, c_int, c_int, c_int64, _P, _P, _P, _P]),
     'otb_edit_distance': (c_int, [_P, c_int, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P, _P]),

@@ -621,6 +621,12 @@ int otb_ctc_prefix_advance(const otb_beam_state* st, const int32_t* cand_id, int
                                                             gamma, psi));
 }
 
+int otb_ctc_nbest_score(const float* logp, int ld, int B, int T, int V, const int32_t* in_len, const int32_t* targets, int K,
+                        int Lp, int blank, float* out, void* stream) {
+    if (!logp || !in_len || !targets || !out) return fail("otb_ctc_nbest_score", "null operand");
+    RET("otb_ctc_nbest_score", ctc_nbest_score_launch(ST(stream), logp, ld, B, T, V, in_len, targets, K, Lp, blank, out));
+}
+
 int otb_token_logprob(const float* logits, int ld, int rows, int V, const int32_t* target, float* out, void* stream) {
     if (rows > 0 && (!logits || !target || !out)) return fail("otb_token_logprob", "null operand");
     RET("otb_token_logprob", token_logprob_launch(ST(stream), logits, ld, rows, V, target, out));

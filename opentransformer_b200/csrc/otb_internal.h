@@ -249,6 +249,9 @@ const char* ctc_prefix_score_launch(cudaStream_t stream, const float* lp, int ld
 const char* ctc_prefix_advance_launch(cudaStream_t stream, BeamState st, const int* cand_id, int P, int T, const int* in_len,
                                       const float* gamma_cand, const float* psi_cand, float* gamma, float* psi);
 
+const char* ctc_nbest_score_launch(cudaStream_t st, const float* logp, int ld, int B, int T, int V, const int* in_len,
+                                   const int* targets, int K, int Lp, int blank, float* out);
+
 const char* token_logprob_launch(cudaStream_t stream, const float* logits, int ld, int rows, int V, const int* target, float* out);
 const char* nbest_rescore_launch(cudaStream_t stream, const int* tgt, int Lp, const int* len, const float* s1, const float* tok_lp,
                                  int M, int B, int K, float weight, int nbest, int Lout, long long pad_id, long long* ids,

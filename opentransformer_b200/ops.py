@@ -930,6 +930,37 @@ class CTCPrefixState:
         _count()
 
 
+CTC_SCORE_MAX_LABELS = 1024      # max_len 1023 tokens and the closing <S/E>
+
+
+def ctc_nbest_score(logp, B, T, in_len, targets, blank=0):
+    """log p_ctc(targets[b, k] | utterance b) of K label rows per utterance (otb_ctc_nbest_score, DESIGN.md 4.18): the
+    blank-extended forward recursion in fp32 over the utterance's log-probs, no copy of them per row and no workspace.
+    logp f32 [B*T, V] (any row pitch, unit column stride) the head's log-softmax; in_len i32 [B] valid frames; targets i32
+    [B, K, Lp] (Lp <= 1024), a row's labels being its entries before the first negative one (second_pass_rows' y <S/E>
+    -1...).  -> f32 [B, K]; -inf where no alignment exists (a blank or out-of-range label, in_len 0, too few frames)."""
+    if logp.dim() != 2 or logp.shape[0] != B * T or logp.stride(1) != 1:
+        raise ValueError(f'ctc_nbest_score: logp must be [B*T = {B * T}, V] with unit column stride, got {tuple(logp.shape)}')
+    if targets.dim() != 3 or targets.shape[0] != B:
+        raise ValueError(f'ctc_nbest_score: targets must be [B = {B}, K, Lp], got {tuple(targets.shape)}')
+    _, K, Lp = targets.shape
+    if K < 1 or not 1 <= Lp <= CTC_SCORE_MAX_LABELS:
+        raise ValueError(f'ctc_nbest_score: targets must have K >= 1 rows of 1..{CTC_SCORE_MAX_LABELS} labels, got '
+                         f'{tuple(targets.shape)}')
+    _ctc_lengths(in_len, B)
+    for t, name, dtype in ((logp, 'logp', torch.float32), (targets, 'targets', torch.int32), (in_len, 'in_len', torch.int32)):
+        if t.dtype != dtype:
+            raise TypeError(f'ctc_nbest_score: {name} must be {dtype}, got {t.dtype}')
+    if not logp.is_cuda:
+        raise RuntimeError('logp must be a CUDA tensor: the CUDA hot path has no CPU fallback')
+    _need(targets, torch.int32, 'targets'); _need(in_len, torch.int32, 'in_len')
+    out = torch.empty(B, K, dtype=torch.float32, device=logp.device)
+    check(_lib.lib().otb_ctc_nbest_score(_p(logp), logp.stride(0), B, T, logp.shape[1], _p(in_len), _p(targets), K, Lp, blank,
+                                         _p(out), _stream()), 'otb_ctc_nbest_score')
+    _count()
+    return out
+
+
 def token_logprob(logits, V, target):
     """out f32 [rows] = log_softmax(logits[r, :V])[target[r]], 0 where target[r] < 0 (otb_token_logprob): each row is read
     once and no [rows, V] log-softmax is written.  logits f32 [rows, ld] with ld % 4 == 0; target i32 [rows]."""

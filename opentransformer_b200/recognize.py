@@ -16,7 +16,9 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
     joint-CTC head re-ranks each hypothesis' best candidates inside the step (csrc/ctc_prefix.cu, DESIGN.md 4.9);
   * n-best rescoring (apply_rescoring / apply_lm_rescoring / rescore_weight, which the reference parses and never passes
     on): a teacher-forced second pass of the attention decoder or an LM re-ranks the first pass's n-best
-    (csrc/rescore.cu, DESIGN.md 4.10).
+    (csrc/rescore.cu, DESIGN.md 4.10);
+  * CTC rescoring (apply_ctc_rescoring): the joint-CTC head's full-sequence log-likelihood re-ranks the attention search's
+    n-best (csrc/ctc_score.cu, DESIGN.md 4.18).
 """
 import torch
 
@@ -141,17 +143,33 @@ def error_counts(ids, lengths, truth, truth_length):
     return err[:, 0].sum(), err.min(dim=1).values.sum(), ref_len.long().sum()
 
 
-def rescore_nbest(ids, scores, scorers, weight, nbest, width=None, pad=EOS, lengths=None):
+def rescore_nbest(ids, scores, scorers, weight, nbest, width=None, pad=EOS, lengths=None, rows=None):
     """N-best rescoring (DESIGN.md 4.10): first-pass ids [B, K, W] (cut as second_pass_rows does) with scores f32 [B, K];
     scorers: functions (inputs i64 [B*K, Lp], targets i32 [B*K, Lp], K, Lp) -> token log-probs f32 [B*K, Lp] of one
     second-pass model each.  s = first-pass score + weight * sum of the models' sums; ranked per utterance by descending s,
     ties in first-pass order, duplicates last with -inf.  -> ops.nbest_rescore's (ids i64 [B, nbest, width or Lp] padded
-    with `pad`, lengths i32 [B, nbest], scores f32 [B, nbest])."""
+    with `pad`, lengths i32 [B, nbest], scores f32 [B, nbest]).  rows: second_pass_rows(ids, lengths) when the caller has
+    it already."""
     B, K, _ = ids.shape
-    inputs, targets, n, Lp = second_pass_rows(ids, lengths)
+    inputs, targets, n, Lp = rows if rows is not None else second_pass_rows(ids, lengths)
     flat = targets.view(B * K, Lp)
     tok_lp = torch.stack([f(inputs, flat, K, Lp).reshape(B, K, Lp) for f in scorers])
     return ops.nbest_rescore(targets, n, scores.float().contiguous(), tok_lp.contiguous(), weight, nbest, width or Lp, pad)
+
+
+def ctc_rescoring_terms(head, mem, mem_len, B, T2, V, targets, scores):
+    """The joint-CTC head's part of apply_ctc_rescoring (DESIGN.md 4.18): log p_ctc(y <S/E> | x) of each first-pass
+    hypothesis (targets i32 [B, K, Lp] as second_pass_rows builds them) over the head's log-probs of memory bf16 [B*T2, D].
+    -> (first-pass scores f32 [B, K] with -inf where the CTC score is -inf, the CTC term as rescore_nbest's token log-probs
+    f32 [B*K, Lp]: the sequence score at position 0, zeros elsewhere and for the -inf rows).  Moving the -inf of a
+    hypothesis without a CTC alignment into its first-pass score makes its rescored score -inf whatever the weight (w * -inf
+    would be NaN at w = 0 and +inf below), so it ranks after every hypothesis with one, in first-pass order."""
+    B, K, Lp = targets.shape
+    ctc = ops.ctc_nbest_score(ops.log_softmax(head.logits_bf16(mem), V), B, T2, mem_len, targets, head.blank)
+    feasible = ctc > float('-inf')
+    tok = torch.zeros(B * K, Lp, dtype=torch.float32, device=ctc.device)
+    tok[:, 0] = torch.where(feasible, ctc, 0.0).view(-1)
+    return torch.where(feasible, scores, float('-inf')), tok
 
 
 def check_lm_rescoring(who, lm, vocab_size):
@@ -425,7 +443,8 @@ class SpeechToTextRecognizer(Recognizer):
 
     def __init__(self, model, lm=None, lm_weight=0.1, ctc_weight=0.0, beam_width=5, nbest=1, max_len=50,
                  idx2unit=None, penalty=0, lamda=5, ngpu=1, apply_cache=False, use_graph=True, persistent=None,
-                 ctc_candidates=None, apply_rescoring=False, apply_lm_rescoring=False, rescore_weight=1.0, max_decoders=None):
+                 ctc_candidates=None, apply_rescoring=False, apply_lm_rescoring=False, rescore_weight=1.0, max_decoders=None,
+                 apply_ctc_rescoring=False):
         """ctc_weight w > 0: joint CTC/attention decoding (DESIGN.md 4.9).  Each hypothesis' ctc_candidates best tokens by
         the attention (+ LM) score (default min(16, 2 beam_width), between beam_width and 16) are scored
         (1 - w) logp_att + w (psi(g c) - psi(g)) + lm_weight lm with the CTC prefix score psi of the model's joint-CTC head,
@@ -436,6 +455,10 @@ class SpeechToTextRecognizer(Recognizer):
         apply_rescoring: the first pass is the CTC prefix beam search (beam_width hypotheses) over the joint-CTC head, the
         second pass the attention decoder; no attention beam search runs.  apply_lm_rescoring: the LM is not fused into the
         search (the persistent decode kernel stays eligible) but scores all beam_width hypotheses of the first pass.
+        apply_ctc_rescoring (DESIGN.md 4.18): the attention beam search runs as without it (on the persistent kernel when
+        eligible) and the joint-CTC head's log p_ctc(y <S/E> | x) of each of its beam_width hypotheses is a second-pass
+        score; with apply_lm_rescoring both scores add before rescore_weight.  A hypothesis the head cannot emit (no CTC
+        alignment) scores -inf and ranks after the others, in first-pass order.
 
         max_decoders: at most this many BeamDecoders (one per batch geometry: batch, encoder frames; each owns its KV caches
         and search buffers) are kept, least recently used first out; None keeps one per geometry seen."""
@@ -446,6 +469,15 @@ class SpeechToTextRecognizer(Recognizer):
         if apply_rescoring and ctc_weight > 0.0:
             raise ValueError('SpeechToTextRecognizer: apply_rescoring (CTC first pass, attention second) and ctc_weight > 0 '
                              '(the CTC term inside the attention search) are two uses of the joint-CTC head; choose one')
+        if apply_ctc_rescoring and not has_head:
+            raise ValueError('SpeechToTextRecognizer: apply_ctc_rescoring needs the joint-CTC head: this model has ctc_weight 0')
+        if apply_ctc_rescoring and ctc_weight > 0.0:
+            raise ValueError('SpeechToTextRecognizer: apply_ctc_rescoring (the CTC head re-ranking the attention n-best) and '
+                             'ctc_weight > 0 (the CTC term inside the attention search) are two uses of the joint-CTC head; '
+                             'choose one')
+        if apply_ctc_rescoring and apply_rescoring:
+            raise ValueError('SpeechToTextRecognizer: apply_ctc_rescoring re-ranks the attention search\'s n-best, and under '
+                             'apply_rescoring the first pass is the CTC head\'s own beam search; choose one')
         if apply_rescoring and not 1 <= beam_width <= 16:
             raise NotImplementedError(f'SpeechToTextRecognizer: the CTC prefix beam search of apply_rescoring takes beam_width '
                                       f'1..16, got {beam_width}')
@@ -473,6 +505,7 @@ class SpeechToTextRecognizer(Recognizer):
         # the batch geometry and the options (no CTC term, no LM fusion) fit it; False forces the per-step CUDA-graph path
         self.persistent = True if persistent is None else bool(persistent)
         self.apply_rescoring, self.apply_lm_rescoring = bool(apply_rescoring), bool(apply_lm_rescoring)
+        self.apply_ctc_rescoring = bool(apply_ctc_rescoring)
         self.rescore_weight = float(rescore_weight)
         self._decoders = {}
         if max_decoders is not None and max_decoders < 1:
@@ -580,11 +613,17 @@ class SpeechToTextRecognizer(Recognizer):
         bd = self._decoder_for(B, T2, inputs.device)
         bd.setup(mem, mem_len)
         steps = bd.run(self.max_len)
-        if not scorers:
+        if not scorers and not self.apply_ctc_rescoring:
             preds, scores = bd.state.finalize(self.penalty, self.lamda, self.nbest)
             return (preds[:, :, :steps], scores, steps), mem, mem_len, bd
         preds, scores = bd.state.finalize(self.penalty, self.lamda, self.beam_width)
-        preds, _, scores = rescore_nbest(preds[:, :, :steps], scores, scorers, self.rescore_weight, nbest, width=steps)
+        preds, rows = preds[:, :, :steps], None
+        if self.apply_ctc_rescoring:
+            rows = second_pass_rows(preds)
+            scores, ctc_tok = ctc_rescoring_terms(self.model.assistor, mem, mem_len, B, T2, self.model.decoder.vocab_size,
+                                                  rows[1], scores)
+            scorers.append(lambda x, y, K, Lp: ctc_tok)
+        preds, _, scores = rescore_nbest(preds, scores, scorers, self.rescore_weight, nbest, width=steps, rows=rows)
         return (preds, scores, steps), mem, mem_len, bd
 
     def recognize_ids(self, inputs, inputs_mask):
@@ -689,10 +728,14 @@ def build_recognizer(model_type, model, lm, args, idx2unit):
             nbest=args.nbest, max_len=args.max_len, idx2unit=idx2unit, penalty=args.penalty, lamda=args.lamda,
             ngpu=args.ngpu, ctc_candidates=getattr(args, 'ctc_candidates', None),
             apply_rescoring=getattr(args, 'apply_rescoring', False),
-            apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False), rescore_weight=getattr(args, 'rescore_weight', 1.0))
+            apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False), rescore_weight=getattr(args, 'rescore_weight', 1.0),
+            apply_ctc_rescoring=getattr(args, 'apply_ctc_rescoring', False))
     if model_type == 'ctc':
         if getattr(args, 'apply_rescoring', False):
             raise ValueError('build_recognizer: apply_rescoring re-scores with the attention decoder, and a CTC model has none')
+        if getattr(args, 'apply_ctc_rescoring', False):
+            raise ValueError('build_recognizer: apply_ctc_rescoring re-scores the n-best of the attention beam search, and a '
+                             'CTC model has none')
         return CTCRecognizer(
             model=model, lm=lm, lm_weight=args.lm_weight, ngram_lm=args.ngram_lm, beam_width=args.beam_width,
             idx2unit=idx2unit, ngpu=args.ngpu, mode=args.mode, alpha=args.alpha, beta=args.beta,
