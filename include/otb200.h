@@ -161,9 +161,10 @@ int otb_scale_add_table(const void* x, int ldx, int x_f32, void* out, int ldo, f
 int otb_sinusoid_table(float* out, int n_pos, int d, int first_pos, void* stream);
 
 /* embedding + PositionalEncoding.forward (decoder/transformer.py:163,169; pos.py:56):
- * out[n] = emb[tok[n*tok_stride]] * sqrt(d) + table[pos], pos = step_ptr ? *step_ptr : n % period. */
+ * out[n] = emb[tok[n*tok_stride]] * sqrt(d) + table[pos], pos = row_pos ? max(row_pos[n], 0) : step_ptr ? *step_ptr :
+ * n % period (row_pos: per-row positions, the LM-fused CTC search; NULL in every other caller). */
 int otb_embed_posenc(const int64_t* tok, int tok_stride, const void* emb, const float* table, void* out, int N,
-                     int d, int period, const int* step_ptr, int vocab, void* stream);
+                     int d, int period, const int* step_ptr, const int* row_pos, int vocab, void* stream);
 
 /* F.log_softmax over the last dim, fp32 (decoder/transformer.py:206). */
 int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int V, void* stream);
@@ -175,6 +176,13 @@ int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int 
  * min(H, 4) * (min(Lmax rounded up to 32, 128) * d_k * 2 + d_k * 4) bytes. */
 int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
                          int H, int Lmax, int d_k, void* stream);
+
+/* The same attention with a position per row (the LM-fused CTC prefix beam search, where slots hold prefixes of different
+ * lengths): row n's query is at position row_pos[n] (-1: the row computes nothing and gets zeros); kc/vc bf16
+ * [cache rows, d]; anc i32 [N, Lmax] lists the cache row of each position 0..row_pos[n] of row n, and the newest K/V are
+ * written to cache row anc[n][row_pos[n]]. */
+int otb_decode_self_attn_rows(const void* qkv, void* kc, void* vc, const int* anc, const int* row_pos, void* out, int N, int H,
+                              int Lmax, int d_k, void* stream);
 
 /* LabelSmoothingLoss.forward (module/loss.py:21-48) fused: per-token KL(smoothed one-hot || softmax), PAD rows 0,
  * mean over non-PAD tokens.  logits f32 [rows, ldl]; targets i64 [rows]; tok_loss f32 [rows]; loss f32 [1];
@@ -412,6 +420,24 @@ int otb_ctc_greedy(const float* top_lp, const int32_t* top_id, int ldk, int B, i
                    int32_t* ids, int32_t* lengths, float* scores, void* stream);
 int otb_ctc_prefix_beam(const float* top_lp, const int32_t* top_id, int K, int B, int T, const int32_t* in_len, int blank, int beam,
                         int32_t* nodes, int32_t* ids, int32_t* lengths, float* scores, void* stream);
+
+/* The prefix beam search with a neural LM as ctcdecode's scorer (DESIGN.md 4.19), ONE frame per call, one CTA per
+ * utterance; the frame index is ctl[0] (ctl i32 [2] zeroed before frame 0; the call moves ctl[0] on).  Extending slot i by
+ * token c adds lm_weight * lm[b*beam + i][c] + beta (lm f32 [B*beam, ld_lm], the LM's next-token log-probs of each slot's
+ * prefix after BOS).  slots: otb_ctc_prefix_beam_slots_bytes(B) bytes of slot state; nodes as otb_ctc_prefix_beam.  Per new
+ * slot (row b*beam + s): src i32 its source row, tok i64 its newest token (BOS = 1 for the empty prefix), ext i32 1 where it
+ * extended the source.  Transformer LM (anc non-null): anc i32 [B*beam, Lpos] cache rows (b*(1 + T*beam) + node) of each
+ * slot's prefix from position 0 (BOS), rewritten for the new slots, anc_tmp the same size of scratch, pos i32 [B*beam] each
+ * row's query position (-1: nothing to compute).  ids / lengths / scores as otb_ctc_prefix_beam, written at frame T - 1. */
+int otb_ctc_prefix_beam_slots_bytes(int B);
+int otb_ctc_prefix_beam_step(const float* top_lp, const int32_t* top_id, int K, int B, int T, const int32_t* in_len, int blank,
+                             int beam, const float* lm, int ld_lm, float lm_weight, float beta, void* slots, int32_t* ctl,
+                             int32_t* nodes, int32_t* src, int64_t* tok, int32_t* ext, int32_t* anc, int32_t* anc_tmp,
+                             int32_t* pos, int Lpos, int32_t* ids, int32_t* lengths, float* scores, void* stream);
+/* The fused search's LM rows and state follow its slots: row n of dst = row n of a where ext[n] != 0 (left as it is when a
+ * is NULL), else row idx[n] of b (row n without idx).  Rows of `width` 4-byte words, pitches in words. */
+int otb_ctc_lm_carry(void* dst, int ldd, const void* a, int lda, const void* b, int ldb, const int32_t* idx, const int32_t* ext,
+                     int rows, int width, void* stream);
 
 /* CTC forced alignment: the best path (Viterbi) through the CTC trellis of each utterance's target, one CTA per utterance.
  * rows f32 [B*T, ld]: log-probs when lse is NULL, else logits with lse f32 [B*T] each frame's log-sum-exp (lp = row - lse);

@@ -63,9 +63,10 @@ _SIGS = {
     'otb_layernorm': (c_int, [_P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_float, c_int, c_int, _P]),
     'otb_scale_add_table': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, c_int, c_int, c_int, _P, _P]),
     'otb_sinusoid_table': (c_int, [_P, c_int, c_int, c_int, _P]),
-    'otb_embed_posenc': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, _P, c_int, _P]),
+    'otb_embed_posenc': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, _P]),
     'otb_log_softmax': (c_int, [_P, c_int, _P, c_int, c_int, c_int, _P]),
     'otb_decode_self_attn': (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    'otb_decode_self_attn_rows': (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_ls_ce': (c_int, [_P, c_int, _P, c_int, c_int, c_float, c_int, _P, _P, _P, _P, c_int, c_int, _P]),
     'otb_beam_init': (c_int, [POINTER(BeamStateC), _P]),
     'otb_beam_step': (c_int, [_P, c_int, c_int, _P, c_int, c_float, POINTER(BeamStateC), _P, _P, _P]),
@@ -104,6 +105,10 @@ _SIGS = {
     'otb_ctc_frame_topk': (c_int, [_P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P]),
     'otb_ctc_greedy': (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P]),
     'otb_ctc_prefix_beam': (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P]),
+    'otb_ctc_prefix_beam_slots_bytes': (c_int, [c_int]),
+    'otb_ctc_prefix_beam_step': (c_int, [_P, _P, c_int, c_int, c_int, _P, c_int, c_int, _P, c_int, c_float, c_float, _P, _P,
+                                         _P, _P, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P]),
+    'otb_ctc_lm_carry': (c_int, [_P, c_int, _P, c_int, _P, c_int, _P, _P, c_int, c_int, _P]),
     'otb_ctc_align': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     'otb_ctc_prefix_init': (c_int, [_P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P]),
     'otb_ctc_prefix_score': (c_int, [_P, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P, c_int, _P, c_int, c_float, c_float,

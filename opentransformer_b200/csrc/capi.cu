@@ -294,13 +294,13 @@ int otb_sinusoid_table(float* out, int n_pos, int d, int first_pos, void* stream
 }
 
 int otb_embed_posenc(const int64_t* tok, int tok_stride, const void* emb, const float* table, void* out, int N,
-                     int d, int period, const int* step_ptr, int vocab, void* stream) {
+                     int d, int period, const int* step_ptr, const int* row_pos, int vocab, void* stream) {
     if (!tok || !emb || !table || !out) return fail("otb_embed_posenc", "null operand");
-    if (!step_ptr && period < 1) return fail("otb_embed_posenc", "need period or step_ptr");
+    if (!row_pos && !step_ptr && period < 1) return fail("otb_embed_posenc", "need period, step_ptr or row_pos");
     RET("otb_embed_posenc",
         embed_posenc_launch(ST(stream), reinterpret_cast<const long long*>(tok), tok_stride,
                             reinterpret_cast<const bf16*>(emb), table, reinterpret_cast<bf16*>(out), N, d, period,
-                            step_ptr, vocab));
+                            step_ptr, vocab, row_pos));
 }
 
 int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int V, void* stream) {
@@ -315,6 +315,15 @@ int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, co
     RET("otb_decode_self_attn",
         decode_self_attn_launch(ST(stream), reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(kc),
                                 reinterpret_cast<bf16*>(vc), anc, step_ptr, reinterpret_cast<bf16*>(out), N, H, Lmax, d_k));
+}
+
+int otb_decode_self_attn_rows(const void* qkv, void* kc, void* vc, const int* anc, const int* row_pos, void* out, int N, int H,
+                              int Lmax, int d_k, void* stream) {
+    if (!qkv || !kc || !vc || !anc || !row_pos || !out) return fail("otb_decode_self_attn_rows", "null operand");
+    if (d_k != 64 && d_k != 96) return fail("otb_decode_self_attn_rows", "head width d_k must be 64 or 96");
+    RET("otb_decode_self_attn_rows",
+        decode_self_attn_launch(ST(stream), reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(kc),
+                                reinterpret_cast<bf16*>(vc), anc, nullptr, reinterpret_cast<bf16*>(out), N, H, Lmax, d_k, row_pos));
 }
 
 int otb_ls_ce(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,
@@ -583,6 +592,28 @@ int otb_ctc_prefix_beam(const float* top_lp, const int32_t* top_id, int K, int B
     if (!top_lp || !top_id || !in_len || !nodes || !ids || !lengths || !scores) return fail("otb_ctc_prefix_beam", "null operand");
     RET("otb_ctc_prefix_beam", ctc_prefix_beam_launch(ST(stream), top_lp, top_id, K, B, T, in_len, blank, beam, nodes, ids,
                                                       lengths, scores));
+}
+
+int otb_ctc_prefix_beam_slots_bytes(int B) { return B < 1 ? -1 : ctc_prefix_beam_slots_bytes(B); }
+
+int otb_ctc_prefix_beam_step(const float* top_lp, const int32_t* top_id, int K, int B, int T, const int32_t* in_len, int blank,
+                             int beam, const float* lm, int ld_lm, float lm_weight, float beta, void* slots, int32_t* ctl,
+                             int32_t* nodes, int32_t* src, int64_t* tok, int32_t* ext, int32_t* anc, int32_t* anc_tmp,
+                             int32_t* pos, int Lpos, int32_t* ids, int32_t* lengths, float* scores, void* stream) {
+    if (!top_lp || !top_id || !in_len || !lm || !slots || !ctl || !nodes || !src || !tok || !ext || !ids || !lengths || !scores)
+        return fail("otb_ctc_prefix_beam_step", "null operand");
+    CtcStepArgs a;
+    a.top_lp = top_lp; a.top_id = top_id; a.K = K; a.T = T; a.in_len = in_len; a.blank = blank; a.beam = beam;
+    a.lm = lm; a.ld_lm = ld_lm; a.lm_w = lm_weight; a.beta = beta; a.slots = slots; a.ctl = ctl; a.nodes = nodes;
+    a.src = src; a.tok = reinterpret_cast<long long*>(tok); a.ext = ext; a.anc = anc; a.anc_tmp = anc_tmp; a.pos = pos;
+    a.Lpos = Lpos; a.ids = ids; a.lengths = lengths; a.scores = scores;
+    RET("otb_ctc_prefix_beam_step", ctc_prefix_beam_step_launch(ST(stream), a, B));
+}
+
+int otb_ctc_lm_carry(void* dst, int ldd, const void* a, int lda, const void* b, int ldb, const int32_t* idx, const int32_t* ext,
+                     int rows, int width, void* stream) {
+    if (!dst || !b) return fail("otb_ctc_lm_carry", "null operand");
+    RET("otb_ctc_lm_carry", ctc_lm_carry_launch(ST(stream), dst, ldd, a, lda, b, ldb, idx, ext, rows, width));
 }
 
 int otb_ctc_align(const float* rows, int ld, int B, int T, int V, const float* lse, const int32_t* in_len, const int64_t* targets,

@@ -305,15 +305,18 @@ const char* sinusoid_table_launch(cudaStream_t st, float* out, int n_pos, int d,
 // ------------------------------------------------------------------------------------------------
 // Embedding gather + positional encoding:  out[n] = emb[tok[n]] * sqrt(d) + PE[pos(n)]
 // otrans/decoder/transformer.py:163,169  (+ module/pos.py:56)
-// tok index:  tok[n * tok_stride + tok_off]; position: step_ptr ? *step_ptr : n % period
+// tok index:  tok[n * tok_stride + tok_off]; position: row_pos ? row_pos[n] : step_ptr ? *step_ptr : n % period
 // ------------------------------------------------------------------------------------------------
+template <bool ROW_POS>
 __global__ void embed_posenc_kernel(const long long* __restrict__ tok, int tok_stride, const bf16* __restrict__ emb,
                                     const float* __restrict__ table, bf16* __restrict__ out, int N, int d, int period,
-                                    const int* __restrict__ step_ptr, float xscale, int vocab) {
+                                    const int* __restrict__ step_ptr, float xscale, int vocab, const int* __restrict__ row_pos) {
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (n >= N) return;
-    const int pos = step_ptr ? *step_ptr : (n % period);
+    int pos;
+    if constexpr (ROW_POS) pos = max(row_pos[n], 0);      // a row without a position (-1) reads position 0
+    else pos = step_ptr ? *step_ptr : (n % period);
     long long t = tok[(size_t)n * tok_stride];
     if (t < 0 || t >= vocab) t = 0;
     const bf16* e = emb + (size_t)t * d;
@@ -334,10 +337,13 @@ __global__ void embed_posenc_kernel(const long long* __restrict__ tok, int tok_s
 
 const char* embed_posenc_launch(cudaStream_t st, const long long* tok, int tok_stride, const bf16* emb,
                                 const float* table, bf16* out, int N, int d, int period, const int* step_ptr,
-                                int vocab) {
+                                int vocab, const int* row_pos) {
     if (d % 8) return "embed: d must be a multiple of 8";
-    return launch<embed_posenc_kernel>(dim3((N + 7) / 8), dim3(256), 0, st, tok, tok_stride, emb, table, out, N, d, period,
-                                       step_ptr, sqrtf((float)d), vocab);
+    if (row_pos)
+        return launch<embed_posenc_kernel<true>>(dim3((N + 7) / 8), dim3(256), 0, st, tok, tok_stride, emb, table, out, N, d,
+                                                 period, step_ptr, sqrtf((float)d), vocab, row_pos);
+    return launch<embed_posenc_kernel<false>>(dim3((N + 7) / 8), dim3(256), 0, st, tok, tok_stride, emb, table, out, N, d, period,
+                                              step_ptr, sqrtf((float)d), vocab, row_pos);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -398,8 +404,11 @@ __device__ __forceinline__ int rot_chunk(int i) {
 //   qkv   bf16 [N, 3d] (Q | K | V of the current token, attention.py:73 split order)
 //   kc,vc bf16 [Lmax, N, d]
 //   anc   int32 [2, N, Lmax]  (ping-pong, buffer (step & 1) is current)
+// ROW_POS (the LM-fused CTC search, DESIGN.md 4.19): every row has its own position, step_ptr[n] (row_pos), and
+// kc / vc are [cache rows, d]: anc int32 [N, Lmax] lists the cache row of each position of row n, the newest included,
+// and the newest K/V go to that row.  A row with row_pos -1 computes nothing and gets zeros.
 // ------------------------------------------------------------------------------------------------
-template <int DK, bool CHUNKED>
+template <int DK, bool CHUNKED, bool ROW_POS = false>
 __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc,
                                                                bf16* __restrict__ vc, const int* __restrict__ anc,
                                                                const int* __restrict__ step_ptr, bf16* __restrict__ out,
@@ -418,9 +427,13 @@ __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nw = blockDim.x >> 5;
     const int d = H * DK;
-    const int step = *step_ptr;
+    const int step = ROW_POS ? step_ptr[n] : *step_ptr;            // ROW_POS: step_ptr holds the row positions
     const int nkeys = step + 1;
-    const int* an = anc + ((size_t)(step & 1) * N + n) * Lmax;
+    const int* an = ROW_POS ? anc + (size_t)n * Lmax : anc + ((size_t)(step & 1) * N + n) * Lmax;
+    if (ROW_POS && step < 0) {
+        for (int i = threadIdx.x; i < d / 2; i += blockDim.x) reinterpret_cast<uint32_t*>(out + (size_t)n * d)[i] = 0u;
+        return;
+    }
     uint4* sv = sv_raw + (size_t)wib * keys_pad * CH;    // [keys_pad][CH x 16 B] per warp
     // q lives in shared memory (every lane needs all DK dims: 64 registers per thread otherwise, which capped the kernel
     // at 3 resident CTAs per SM -- the SM-time of this latency-bound kernel is what concurrent batches compete for)
@@ -430,7 +443,7 @@ __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel
         // append the newest K/V to the cache (lane owns dims 2*lane, 2*lane+1; at DK 96 lanes 0..15 also own 64+2*lane, +1)
         const uint32_t kcur = *reinterpret_cast<const uint32_t*>(base + d + 2 * lane);
         const uint32_t vcur = *reinterpret_cast<const uint32_t*>(base + 2 * d + 2 * lane);
-        const size_t cur_off = ((size_t)step * N + n) * d + h * DK + 2 * lane;
+        const size_t cur_off = (ROW_POS ? (size_t)an[step] * d : ((size_t)step * N + n) * d) + h * DK + 2 * lane;
         *reinterpret_cast<uint32_t*>(kc + cur_off) = kcur;
         *reinterpret_cast<uint32_t*>(vc + cur_off) = vcur;
         if (DK == 96 && lane < 16) {
@@ -469,8 +482,9 @@ __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel
                 const int s = c0 + lane + 32 * j, sl = lane + 32 * j;   // position in the prefix / in the chunk
                 sc[j] = -INFINITY;
                 if (s < nkeys) {   // warp-divergent only in the last group
-                    const bf16* krow = (s == step) ? base + d : kc + ((size_t)s * N + slot[j]) * d + h * DK;
-                    const bf16* vrow = (s == step) ? base + 2 * d : vc + ((size_t)s * N + slot[j]) * d + h * DK;
+                    const size_t crow = ROW_POS ? (size_t)slot[j] : (size_t)s * N + slot[j];
+                    const bf16* krow = (s == step) ? base + d : kc + crow * d + h * DK;
+                    const bf16* vrow = (s == step) ? base + 2 * d : vc + crow * d + h * DK;
                     uint4 ku[CH], vu[CH];
 #pragma unroll
                     for (int i = 0; i < CH; ++i) ku[i] = *reinterpret_cast<const uint4*>(krow + 8 * i);
@@ -569,9 +583,9 @@ __global__ void __launch_bounds__(128, DK == 64 ? 6 : 4) decode_self_attn_kernel
     }
 }
 
-template <int DK>
+template <int DK, bool ROW_POS>
 static const char* decode_self_attn_launch_dk(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
-                                              const int* step_ptr, bf16* out, int N, int H, int Lmax) {
+                                              const int* step_ptr, bf16* out, int N, int H, int Lmax, const int* row_pos) {
     const int warps = H < 4 ? H : 4;
     // V staging sized by the longest prefix this search can reach, up to one 128-key chunk: at max_len 60 this halves the
     // shared memory per CTA and doubles the resident CTAs of this latency-bound kernel (less SM-time per decode step)
@@ -579,18 +593,24 @@ static const char* decode_self_attn_launch_dk(cudaStream_t st, const bf16* qkv, 
     const int keys_pad = chunked ? 128 : (Lmax + 31) / 32 * 32;
     const size_t smem = (size_t)warps * keys_pad * DK * 2 + (size_t)warps * DK * sizeof(float);   // V rows | q per warp
     const float scale = DK == 64 ? 0.125f : 1.0f / sqrtf((float)DK);
+    const int* pos = ROW_POS ? row_pos : step_ptr;         // the kernel reads the row positions through step_ptr
     if (chunked)
-        return launch<decode_self_attn_kernel<DK, true>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H,
-                                                         Lmax, scale, keys_pad);
-    return launch<decode_self_attn_kernel<DK, false>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, step_ptr, out, N, H,
-                                                      Lmax, scale, keys_pad);
+        return launch<decode_self_attn_kernel<DK, true, ROW_POS>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, pos, out,
+                                                                  N, H, Lmax, scale, keys_pad);
+    return launch<decode_self_attn_kernel<DK, false, ROW_POS>>(dim3(N), dim3(warps * 32), smem, st, qkv, kc, vc, anc, pos, out,
+                                                               N, H, Lmax, scale, keys_pad);
 }
 
 const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
-                                    const int* step_ptr, bf16* out, int N, int H, int Lmax, int d_k) {
+                                    const int* step_ptr, bf16* out, int N, int H, int Lmax, int d_k, const int* row_pos) {
     if (Lmax > 1023) return "decode_self_attn: at most 1023 cached positions (max_len <= 1023)";
-    if (d_k == 64) return decode_self_attn_launch_dk<64>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax);
-    if (d_k == 96) return decode_self_attn_launch_dk<96>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax);
+    if (row_pos) {
+        if (d_k == 64) return decode_self_attn_launch_dk<64, true>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax, row_pos);
+        if (d_k == 96) return decode_self_attn_launch_dk<96, true>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax, row_pos);
+    } else {
+        if (d_k == 64) return decode_self_attn_launch_dk<64, false>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax, row_pos);
+        if (d_k == 96) return decode_self_attn_launch_dk<96, false>(st, qkv, kc, vc, anc, step_ptr, out, N, H, Lmax, row_pos);
+    }
     return "decode_self_attn: head width d_k must be 64 or 96";
 }
 

@@ -208,10 +208,10 @@ const char* dwconv_swish_launch(cudaStream_t st, const bf16* x, const float* w, 
 const char* sinusoid_table_launch(cudaStream_t st, float* out, int n_pos, int d, int first_pos);
 const char* embed_posenc_launch(cudaStream_t st, const long long* tok, int tok_stride, const bf16* emb,
                                 const float* table, bf16* out, int N, int d, int period, const int* step_ptr,
-                                int vocab);
+                                int vocab, const int* row_pos = nullptr);
 const char* log_softmax_launch(cudaStream_t st, const float* x, int ldx, float* out, int ldo, int rows, int V);
 const char* decode_self_attn_launch(cudaStream_t st, const bf16* qkv, bf16* kc, bf16* vc, const int* anc,
-                                    const int* step_ptr, bf16* out, int N, int H, int Lmax, int d_k);
+                                    const int* step_ptr, bf16* out, int N, int H, int Lmax, int d_k, const int* row_pos = nullptr);
 const char* beam_init_launch(cudaStream_t stream, BeamState st);
 const char* beam_step_launch(cudaStream_t stream, const float* logp, int ldl, int V, const float* lm_logp, int ld_lm,
                              float lm_weight, BeamState st, long long* dbg_ktok, int* dbg_offs, const float* pre_val,
@@ -234,6 +234,35 @@ const char* ctc_frame_topk_launch(cudaStream_t st, const float* logits, int ld, 
                                   float* top_lp, int* top_id);
 const char* ctc_greedy_launch(cudaStream_t st, const float* top_lp, const int* top_id, int ldk, int B, int T, const int* in_len,
                               int blank, int* ids, int* lengths, float* scores);
+// One frame of the LM-fused CTC prefix beam search (ctc_prefix_beam_step_kernel, DESIGN.md 4.19).
+static constexpr int CTC_LM_BOS = 1;          // <S/E>: the LM's first input, and the token of a row with an empty prefix
+struct CtcStepArgs {
+    const float* top_lp;
+    const int* top_id;
+    int K, T;
+    const int* in_len;
+    int blank, beam;
+    const float* lm;          // f32 [B*beam, ld_lm]: row b*beam + i = log p_lm(. | BOS, prefix of slot i)
+    int ld_lm;
+    float lm_w, beta;
+    void* slots;              // [2, B] slot states (ctc_prefix_beam_slots_bytes)
+    int* ctl;                 // [2]: frame counter, arrival counter (both 0 before frame 0)
+    int* nodes;               // i32 [B, 1 + T*beam, 2]
+    int* src;                 // [B*beam] source row of each new slot
+    long long* tok;           // [B*beam] the LM input of each row: its newest token (BOS for the empty prefix)
+    int* ext;                 // [B*beam] 1 where the new slot extended its source
+    int* anc;                 // Transformer LM or null: i32 [B*beam, Lpos] cache rows of each slot's prefix
+    int* anc_tmp;             // i32 [B*beam, Lpos] scratch
+    int* pos;                 // [B*beam] query position of each row, -1: nothing to compute
+    int Lpos;
+    int* ids;                 // written at the last frame: i32 [B, beam, T], lengths i32 [B, beam], scores f32 [B, beam]
+    int* lengths;
+    float* scores;
+};
+const char* ctc_prefix_beam_step_launch(cudaStream_t st, const CtcStepArgs& a, int B);
+int ctc_prefix_beam_slots_bytes(int B);
+const char* ctc_lm_carry_launch(cudaStream_t st, void* dst, int ldd, const void* a, int lda, const void* b, int ldb, const int* idx,
+                                const int* ext, int rows, int width);
 const char* ctc_prefix_beam_launch(cudaStream_t st, const float* top_lp, const int* top_id, int K, int B, int T, const int* in_len,
                                    int blank, int beam, int* nodes, int* ids, int* lengths, float* scores);
 const char* ctc_align_launch(cudaStream_t st, const float* rows, int ld, int B, int T, int V, const float* lse, const int* in_len,

@@ -1,0 +1,161 @@
+"""LM shallow fusion in the CTC prefix beam search (DESIGN.md 4.19): ctcdecode's search with a neural LM as its scorer.
+
+One frame is the search step (otb_ctc_prefix_beam_step: one CTA per utterance, the frame index from a device counter, the
+slots in global memory) followed by one LM step over all B * beam rows; the frame is captured in a CUDA graph and replayed
+T' times from the host without a synchronisation.  The LM state follows the slots: a row that kept its prefix carries its
+source slot's LM row (and LSTM state), a row that extended runs the LM on its new token.
+
+  * Recurrent LM: (h, c) per slot, gathered by source slot, then the embedding, the input GEMM, one otb_lstm_fwd step per
+    layer, the head GEMM and otb_log_softmax.
+  * Transformer LM: the K/V of each prefix node (node ids 1 + t * beam + s of DESIGN.md 4.7, 0 the BOS) are stored once
+    per utterance, [blocks, B * (1 + T' * beam), d]; each row lists the cache rows of its prefix (anc, rewritten by the
+    search step) and queries at its own position (otb_embed_posenc / otb_decode_self_attn_rows with row_pos).
+"""
+import torch
+
+from . import ops
+
+BOS = 1
+
+
+class CTCFusedSearch:
+    """The fused search for one (batch, beam, frames, top-K) geometry; every buffer is allocated here, before capture."""
+
+    def __init__(self, lm, B, beam, T, K, device, lm_weight, beta, blank=0, use_graph=True):
+        if lm.model_type == 'transformer_lm' and T > ops.DECODE_MAX_LEN:
+            raise ValueError(f'CTC LM fusion: a prefix can be T\' = {T} tokens long and the Transformer LM\'s cached '
+                             f'attention takes at most {ops.DECODE_MAX_LEN} positions')
+        self.lm, self.B, self.W, self.T, self.K = lm, B, beam, T, K
+        self.lm_weight, self.beta, self.blank = float(lm_weight), float(beta), blank
+        self.use_graph = use_graph
+        self.N = N = B * beam
+        V = lm.vocab_size
+        i32 = dict(dtype=torch.int32, device=device)
+        self.top_lp = torch.zeros(B * T, K, dtype=torch.float32, device=device)
+        self.top_id = torch.zeros(B * T, K, **i32)
+        self.in_len = torch.zeros(B, **i32)
+        self.lm_rows = torch.zeros(N, V, dtype=torch.float32, device=device)
+        self.lm_old = torch.zeros(N, V, dtype=torch.float32, device=device)
+        self.slots = ops.ctc_prefix_beam_slots(B, device)
+        self.ctl = torch.zeros(2, **i32)
+        self.nodes = torch.zeros(B, 1 + T * beam, 2, **i32)
+        self.src = torch.zeros(N, **i32)
+        self.ext = torch.zeros(N, **i32)
+        self.tok = torch.full((N,), BOS, dtype=torch.int64, device=device)
+        self.ids = torch.zeros(B, beam, T, **i32)
+        self.lengths = torch.zeros(B, beam, **i32)
+        self.scores = torch.zeros(B, beam, dtype=torch.float32, device=device)
+        self.anc = self.anc_tmp = self.pos = None
+        if lm.model_type == 'transformer_lm':
+            # cache rows: per utterance the BOS node and one node per (frame, slot); positions 0 .. T' - 1
+            rows = B * (1 + T * beam)
+            self.kc = torch.zeros(lm.num_blocks, rows, lm.d_model, dtype=ops.BF16, device=device)
+            self.vc = torch.zeros(lm.num_blocks, rows, lm.d_model, dtype=ops.BF16, device=device)
+            self.anc = torch.zeros(N, T, **i32)
+            self.anc_tmp = torch.zeros(N, T, **i32)
+            self.pos = torch.zeros(N, **i32)
+            self.table = ops.sinusoid_table(T + 1, lm.d_model, 0, device)
+            slot = torch.arange(N, device=device) % beam
+            self._pos0 = torch.where(slot == 0, 0, -1).to(torch.int32)
+            self._bos_row = ((torch.arange(N, device=device) // beam) * (1 + T * beam)).to(torch.int32)
+        else:
+            lm._check_device(device)
+            shape = (lm.num_layers, N, lm.hidden_size)
+            self.h, self.c = torch.zeros(shape, device=device), torch.zeros(shape, device=device)
+            self.h_old, self.c_old = torch.zeros(shape, device=device), torch.zeros(shape, device=device)
+            self._lstm_bar = torch.zeros(2, **i32)
+        self.graph = None
+        self._graph_pk = None
+
+    # ---- the kernels of one LM step over all rows ------------------------------------------------------------------
+    def _lm_step(self):
+        """LM rows of every row's newest token -> lm_rows (and, for the recurrent LM, the new (h, c) per layer)."""
+        lm, N = self.lm, self.N
+        pk = lm._pack.get()
+        if self.anc is not None:
+            x = ops.embed_posenc(self.tok, pk['emb'], self.table, N, lm.d_model, row_pos=self.pos)
+            for l, (blk, p) in enumerate(zip(lm.blocks, pk['blocks'])):
+                x = blk.run(x, p, N, 1, None, context=lambda qkv, l=l: ops.decode_self_attn(
+                    qkv, self.kc[l], self.vc[l], self.anc, None, N, lm.n_heads, self.T, row_pos=self.pos))
+            logits = ops.linear(x, pk['wout'], pk['bout'], ops.EPI_BIAS, out_f32=True, n_out=lm.ld_logits)
+            ops.log_softmax(logits, lm.vocab_size, out=self.lm_rows)
+            return None
+        x = ops.embedding(self.tok, pk['emb'])
+        new = []
+        for k, p in enumerate(pk['layers']):
+            gx = ops.linear(x, p['ih'].w, p['ih'].b, out_f32=True)
+            x, h_n, c_n, _, _ = ops.lstm_fwd(gx, p['w_hh'], 1, N, self.h_old[k], self.c_old[k], barrier=self._lstm_bar)
+            new.append((h_n, c_n))
+        ops.log_softmax(lm._logits(x, pk), lm.vocab_size, out=self.lm_rows)
+        return new
+
+    def _take_state(self, new):
+        """Rows that extended take the LM step's (h, c), the others their source slot's (already gathered)."""
+        for k, (h_n, c_n) in enumerate(new):
+            ops.ctc_lm_carry(self.h[k], self.h_old[k], ext=self.ext, a=h_n)
+            ops.ctc_lm_carry(self.c[k], self.c_old[k], ext=self.ext, a=c_n)
+
+    def _frame(self):
+        ops.ctc_prefix_beam_step(self.top_lp, self.top_id, self.B, self.T, self.in_len, self.W, self.blank, self.lm_rows,
+                                 self.lm_weight, self.beta, self.slots, self.ctl, self.nodes, self.src, self.tok, self.ext,
+                                 self.ids, self.lengths, self.scores, self.anc, self.anc_tmp, self.pos)
+        ops.ctc_lm_carry(self.lm_old, self.lm_rows, idx=self.src, ext=self.ext)      # kept rows: the source's LM row
+        if self.anc is None:
+            for k in range(self.lm.num_layers):
+                ops.ctc_lm_carry(self.h_old[k], self.h[k], idx=self.src)
+                ops.ctc_lm_carry(self.c_old[k], self.c[k], idx=self.src)
+        new = self._lm_step()
+        ops.ctc_lm_carry(self.lm_rows, self.lm_old, ext=self.ext)                     # ... put back over the LM's output
+        if new is not None:
+            self._take_state(new)
+
+    def _start(self):
+        """Frame counter 0 and the LM on BOS for the empty prefix (slot 0 of every utterance)."""
+        self.ctl.zero_()
+        self.tok.fill_(BOS)
+        self.ext.fill_(1)
+        if self.anc is not None:
+            self.anc[:, 0] = self._bos_row
+            self.pos.copy_(self._pos0)
+        else:
+            self.h_old.zero_()
+            self.c_old.zero_()
+        new = self._lm_step()
+        if new is not None:
+            self._take_state(new)
+
+    def _capture(self):
+        # warm-up outside capture (the weight pack, kernel attributes), then capture one frame; _start() resets what the
+        # warm-up advanced
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            self._frame()
+        torch.cuda.current_stream().wait_stream(s)
+        self.graph = torch.cuda.CUDAGraph()
+        n0 = ops.COUNTERS['launches']
+        with torch.cuda.graph(self.graph):
+            self._frame()
+        self.launches_per_frame = ops.COUNTERS['launches'] - n0
+        ops.COUNTERS['launches'] = n0
+
+    def run(self, top_lp, top_id, in_len):
+        """top_lp / top_id [B*T', K] of ctc_frame_topk, in_len i32 [B] -> (ids i64 [B, beam, T'] best first, lengths i32
+        [B, beam], scores f32 [B, beam]: the fused totals log(p_b + p_nb))."""
+        self.top_lp.copy_(top_lp)
+        self.top_id.copy_(top_id)
+        self.in_len.copy_(in_len)
+        if self.use_graph:
+            pk = self.lm._pack.get()
+            if self.graph is None or self._graph_pk is not pk:
+                # the LM's pack was rebuilt (load_state_dict, an optimizer step): the graph bakes in its addresses
+                self._graph_pk = pk
+                self._capture()
+        self._start()
+        for _ in range(self.T):
+            if self.use_graph:
+                self.graph.replay()
+                ops.COUNTERS['launches'] += self.launches_per_frame
+            else:
+                self._frame()
+        return self.ids.long(), self.lengths.clone(), self.scores.clone()

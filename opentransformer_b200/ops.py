@@ -336,12 +336,15 @@ def sinusoid_table(n_pos, d, first_pos=0, device=None):
     return t
 
 
-def embed_posenc(tok, emb, table, N, d, period=1, tok_stride=1, step_ptr=None, out=None):
+def embed_posenc(tok, emb, table, N, d, period=1, tok_stride=1, step_ptr=None, out=None, row_pos=None):
+    """row_pos i32 [N]: a position per row (-1 reads position 0), instead of step_ptr's or period's."""
     _need(emb, BF16, 'emb')
+    if row_pos is not None:
+        _need(row_pos, torch.int32, 'row_pos')
     if out is None:
         out = torch.empty(N, d, dtype=BF16, device=emb.device)
     check(_lib.lib().otb_embed_posenc(_p(tok), tok_stride, _p(emb), _p(table), _p(out), N, d, period, _p(step_ptr),
-                                      emb.shape[0], _stream()), 'otb_embed_posenc')
+                                      _p(row_pos), emb.shape[0], _stream()), 'otb_embed_posenc')
     _count()
     return out
 
@@ -401,8 +404,10 @@ def ls_cross_entropy(logits, targets, V, smoothing=0.1, pad_id=0, want_grad=Fals
 DECODE_MAX_LEN = 1023   # cached positions of otb_decode_self_attn: the longest KV-cached beam search (max_len)
 
 
-def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None):
-    """kc/vc bf16 [Lmax, N, d]: the head width d_k = d // H is taken from the cache."""
+def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None, row_pos=None):
+    """kc/vc bf16 [Lmax, N, d]: the head width d_k = d // H is taken from the cache.
+    row_pos i32 [N] (otb_decode_self_attn_rows): a query position per row (-1: zeros), step_ptr unused, kc/vc bf16
+    [cache rows, d] and anc i32 [N, Lmax] the cache row of each position of each row, the newest included."""
     d = kc.shape[-1]
     if d % H:
         raise ValueError(f'decode_self_attn: cache width {d} is not a multiple of H = {H}')
@@ -410,6 +415,14 @@ def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None):
     check_head_dim(d_k)
     if out is None:
         out = torch.empty(N, d, dtype=BF16, device=qkv.device)
+    if row_pos is not None:
+        _need(row_pos, torch.int32, 'row_pos'); _need(anc, torch.int32, 'anc')
+        if anc.shape != (N, Lmax):
+            raise ValueError(f'decode_self_attn: with row_pos, anc must be [N = {N}, Lmax = {Lmax}], got {tuple(anc.shape)}')
+        check(_lib.lib().otb_decode_self_attn_rows(_p(qkv), _p(kc), _p(vc), _p(anc), _p(row_pos), _p(out), N, H, Lmax, d_k,
+                                                   _stream()), 'otb_decode_self_attn_rows')
+        _count()
+        return out
     check(_lib.lib().otb_decode_self_attn(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax, d_k, _stream()),
           'otb_decode_self_attn')
     _count()
@@ -832,6 +845,39 @@ def ctc_prefix_beam(top_lp, top_id, B, T, in_len, beam, blank=0):
                                          _p(lengths), _p(scores), _stream()), 'otb_ctc_prefix_beam')
     _count()
     return ids, lengths, scores
+
+
+def ctc_prefix_beam_slots(B, device):
+    """The slot state of otb_ctc_prefix_beam_step for B utterances (uint8 bytes)."""
+    return torch.zeros(int(_lib.lib().otb_ctc_prefix_beam_slots_bytes(B)), dtype=torch.uint8, device=device)
+
+
+def ctc_prefix_beam_step(top_lp, top_id, B, T, in_len, beam, blank, lm, lm_weight, beta, slots, ctl, nodes, src, tok, ext,
+                         ids, lengths, scores, anc=None, anc_tmp=None, pos=None):
+    """One frame of the LM-fused CTC prefix beam search (otb_ctc_prefix_beam_step, DESIGN.md 4.19) on preallocated
+    buffers: lm f32 [B*beam, V] the LM rows of the slots; ctl i32 [2] (frame, 0) before frame 0; nodes i32
+    [B, 1 + T*beam, 2]; src / ext i32 and tok i64 [B*beam] written; ids / lengths / scores as ctc_prefix_beam, written at
+    frame T - 1.  Transformer LM: anc / anc_tmp i32 [B*beam, Lpos], pos i32 [B*beam]."""
+    Lpos = anc.shape[1] if anc is not None else 0
+    check(_lib.lib().otb_ctc_prefix_beam_step(_p(top_lp), _p(top_id), top_id.shape[1], B, T, _p(in_len), blank, beam, _p(lm),
+                                              lm.stride(0), float(lm_weight), float(beta), _p(slots), _p(ctl), _p(nodes),
+                                              _p(src), _p(tok), _p(ext), _p(anc), _p(anc_tmp), _p(pos), Lpos, _p(ids),
+                                              _p(lengths), _p(scores), _stream()), 'otb_ctc_prefix_beam_step')
+    _count()
+
+
+def ctc_lm_carry(dst, b, idx=None, ext=None, a=None):
+    """Rows of 4-byte elements (otb_ctc_lm_carry): dst[n] = a[n] where ext[n] (dst[n] kept when a is None), else
+    b[idx[n]] (b[n] without idx)."""
+    rows, width = dst.shape[0], dst[0].numel()
+    for t in (dst, a, b):
+        if t is not None and (t.element_size() != 4 or t.stride(-1) != 1 or t[0].numel() != width):
+            raise ValueError('ctc_lm_carry: rows of equal width of 4-byte elements')
+    ld = lambda t: t.stride(0) if t is not None else 0
+    check(_lib.lib().otb_ctc_lm_carry(_p(dst), ld(dst), _p(a), ld(a), _p(b), ld(b), _p(idx), _p(ext), rows, width, _stream()),
+          'otb_ctc_lm_carry')
+    _count()
+    return dst
 
 
 CTC_ALIGN_MAX_TOKENS = 1023

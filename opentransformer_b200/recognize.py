@@ -18,11 +18,14 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
     on): a teacher-forced second pass of the attention decoder or an LM re-ranks the first pass's n-best
     (csrc/rescore.cu, DESIGN.md 4.10);
   * CTC rescoring (apply_ctc_rescoring): the joint-CTC head's full-sequence log-likelihood re-ranks the attention search's
-    n-best (csrc/ctc_score.cu, DESIGN.md 4.18).
+    n-best (csrc/ctc_score.cu, DESIGN.md 4.18);
+  * CTC LM fusion (CTCRecognizer(lm_fusion=True)): the neural LM is ctcdecode's scorer inside the CTC prefix beam search
+    (ctc_fusion.py, DESIGN.md 4.19).
 """
 import torch
 
 from . import ops
+from .ctc_fusion import CTCFusedSearch
 from .lm import LMCache
 from .model import ctc_align_logits
 from .modules import encoder_attn_weights
@@ -660,15 +663,27 @@ CTC_CUTOFF_TOP_N = 40      # ctcdecode's cutoff_top_n default (cutoff_prob 1.0),
 class CTCRecognizer(Recognizer):
     """otrans/recognize/ctc.py:7-76 on the CUDA path: CTCModel.inference's head logits -> otb_ctc_frame_topk -> the greedy
     collapse (otb_ctc_greedy, mode 'greedy') or the CTC prefix beam search (otb_ctc_prefix_beam, mode 'beam': ctcdecode's
-    search without a scorer, over each frame's 40 best tokens).  `lm` is stored and used only by apply_lm_rescoring, as the
-    reference never uses it; `alpha` / `beta` are ignored, as ctcdecode ignores them without an n-gram scorer, and an
-    n-gram LM (`ngram_lm`, KenLM) is refused.
+    search without a scorer, over each frame's 40 best tokens).  `lm` is used only by apply_lm_rescoring and lm_fusion, as
+    the reference never uses it; `alpha` is ignored, and `beta` too unless lm_fusion is on, as ctcdecode ignores them
+    without a scorer; an n-gram LM (`ngram_lm`, KenLM) is refused.
 
     apply_lm_rescoring (beam mode): the prefix beam search's n-best is re-ranked by
-    s = prefix log-probability + rescore_weight * log P_lm(y <S/E>) (DESIGN.md 4.10)."""
+    s = prefix log-probability + rescore_weight * log P_lm(y <S/E>) (DESIGN.md 4.10).
+
+    lm_fusion (beam mode, off by default): the LM is ctcdecode's scorer inside the search (DESIGN.md 4.19).  Extending a
+    prefix by token c adds lm_weight * log p_lm(c | <S/E>, prefix) + beta; the scores are those fused totals.  The search
+    runs one frame per replay of a captured CUDA graph (use_graph=False: the same kernels launched one by one)."""
 
     def __init__(self, model, lm=None, lm_weight=0.1, ngram_lm=None, beam_width=5, idx2unit=None, ngpu=1, mode='greedy',
-                 alpha=0.1, beta=0.0, apply_lm_rescoring=False, rescore_weight=1.0):
+                 alpha=0.1, beta=0.0, apply_lm_rescoring=False, rescore_weight=1.0, lm_fusion=False, use_graph=True):
+        if lm_fusion:
+            if lm is None:
+                raise ValueError('CTCRecognizer: lm_fusion needs an lm')
+            if mode != 'beam':
+                raise ValueError("CTCRecognizer: lm_fusion fuses the LM into the prefix beam search; use mode='beam'")
+            if apply_lm_rescoring:
+                raise ValueError('CTCRecognizer: lm_fusion and apply_lm_rescoring would count the same LM twice; choose one')
+            check_lm_fusion('CTCRecognizer', lm, model.vocab_size)
         if ngram_lm is not None:
             raise NotImplementedError('CTCRecognizer: n-gram LM scoring (KenLM) is not implemented; use ngram_lm=None')
         if mode not in ('greedy', 'beam'):
@@ -684,15 +699,43 @@ class CTCRecognizer(Recognizer):
         self.beam_width, self.mode = beam_width, mode
         self.alpha, self.beta = alpha, beta
         self.apply_lm_rescoring, self.rescore_weight = bool(apply_lm_rescoring), float(rescore_weight)
+        self.lm_fusion, self.use_graph = bool(lm_fusion), bool(use_graph)
+        self._searches = {}
+
+    def _check_frames(self, inputs):
+        """A Transformer LM's cached attention takes at most DECODE_MAX_LEN positions, and a prefix can be T' long."""
+        if self.lm_fusion and self.lm.model_type == 'transformer_lm':
+            T2 = self.model.frontend.output_length(inputs.shape[1])
+            if T2 > ops.DECODE_MAX_LEN:
+                raise ValueError(f"CTCRecognizer: lm_fusion with a Transformer LM takes at most {ops.DECODE_MAX_LEN} encoder "
+                                 f"frames (a prefix can be T' tokens long), got T' = {T2}")
+
+    def _fused_search(self, B, T2, K, device):
+        """The fused search of one geometry; the most recent few are kept (each owns its buffers and its graph)."""
+        key = (B, T2, K, device.index, self.lm, float(self.lm_weight), float(self.beta))   # launch arguments a graph bakes in
+        search = self._searches.pop(key, None)
+        if search is None:
+            while len(self._searches) >= 2:
+                self._searches.pop(next(iter(self._searches)))
+            search = CTCFusedSearch(self.lm, B, self.beam_width, T2, K, device, self.lm_weight, self.beta,
+                                    self.model.assistor.blank, self.use_graph)
+        self._searches[key] = search
+        return search
 
     def recognize_ids(self, inputs, inputs_mask):
         """-> (ids i64 [B, nbest, T'] best first, 0 after each hypothesis' end; lengths i32 [B, nbest]; scores f32 [B, nbest]),
         on the device.  nbest is 1 in greedy mode (score: the best path's log-prob) and beam_width in beam mode (score:
         the prefix's log-probability over all its alignments)."""
+        self._check_frames(inputs)
         with torch.no_grad():
             return self._decode(*self.model.logits_bf16(inputs, inputs_mask))
 
     def _decode(self, logits, lengths, B, T2):
+        if self.lm_fusion:
+            V = self.model.vocab_size
+            K = min(CTC_CUTOFF_TOP_N, V)
+            lp, tok = ops.ctc_frame_topk(logits, B, T2, V, lengths, K)
+            return self._fused_search(B, T2, K, logits.device).run(lp, tok, lengths)
         ids, n, sc = ctc_decode(logits, lengths, B, T2, self.model.vocab_size, self.model.assistor.blank, self.mode,
                                 self.beam_width)
         if not self.apply_lm_rescoring:
@@ -706,6 +749,7 @@ class CTCRecognizer(Recognizer):
         [B, min(T', 1023), 2] [start, end) in encoder frames of the 1-best's tokens, -1 past its length, and -1 throughout
         for a 1-best longer than the aligner's 1023 tokens), on the device.
         model.encoder_frames_to_input converts the spans to input frames or seconds."""
+        self._check_frames(inputs)
         with torch.no_grad():
             logits, lengths, B, T2 = self.model.logits_bf16(inputs, inputs_mask)
             ids, n, sc = self._decode(logits, lengths, B, T2)
@@ -739,5 +783,6 @@ def build_recognizer(model_type, model, lm, args, idx2unit):
         return CTCRecognizer(
             model=model, lm=lm, lm_weight=args.lm_weight, ngram_lm=args.ngram_lm, beam_width=args.beam_width,
             idx2unit=idx2unit, ngpu=args.ngpu, mode=args.mode, alpha=args.alpha, beta=args.beta,
-            apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False), rescore_weight=getattr(args, 'rescore_weight', 1.0))
+            apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False), rescore_weight=getattr(args, 'rescore_weight', 1.0),
+            lm_fusion=getattr(args, 'lm_fusion', False))
     raise NotImplementedError(model_type)
