@@ -278,20 +278,28 @@ __global__ void __launch_bounds__(TOPK_THREADS) logsoftmax_topk_kernel(const flo
         if (out_logp) out_logp[(size_t)row * ld_logp + i] = v;
     }
     __syncthreads();
-    // per-warp top-k over a contiguous slice: k rounds of (lane-local scan of smem, warp arg-max, knock out)
+    // per-warp top-k over a contiguous slice: k rounds of (lane-local scan of smem, warp arg-max), round r taking the best
+    // element ranked after round r-1's pick in the order (value descending, index ascending).  Elements equal to -inf are
+    // ranked like any other value, so a row with fewer than k finite values still yields real token ids, as torch.topk and
+    // warp_topk do.  (Knocking the pick out by overwriting it with -inf made picked elements and real -inf ones look alike,
+    // and a scan that skipped -inf returned index 0x7fffffff for them: found by tests/test_gpu_beam_ties.py, an LM that
+    // rules tokens out with lm_logp = -inf.)
     const int per = (V + 7) / 8;
     const int lo = warp * per, hi = min(V, lo + per);
+    float pv = INFINITY;
+    int pi = -1;
     for (int r = 0; r < k; ++r) {
         float bv = -INFINITY;
         int bi = 0x7fffffff;
         for (int idx = lo + lane; idx < hi; idx += 32) {
             const float v = srow[idx];
-            if (v > bv) { bv = v; bi = idx; }      // ascending scan + strict '>' keeps the lower index on ties
+            const bool after = (v < pv) || (v == pv && idx > pi);
+            if (after && better(v, idx, bv, bi)) { bv = v; bi = idx; }
         }
         warp_best(bv, bi);
-        if (bi != 0x7fffffff && ((bi - lo) & 31) == lane) srow[bi] = -INFINITY;
+        pv = bv;
+        pi = bi;
         if (lane == 0) { cand_v[warp * KMAX + r] = bv; cand_i[warp * KMAX + r] = bi; }
-        __syncwarp();
     }
     __syncthreads();
     if (warp == 0) {
