@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define OTB_VERSION 3
+#define OTB_VERSION 4
 
 /* GEMM epilogues (otb_linear) */
 enum {
@@ -56,32 +56,27 @@ int otb_debug_decode_timing(unsigned long long* buf, int step);
  * on a device that refuses clusters of 16 fails instead of falling back to the software barrier.  Process-wide. */
 int otb_set_decode_barrier(int kind);
 
-/* Conv2dLayer output geometry of the two-layer conv front end (frontend/conv.py:10-11,15-48): layer i has kernel
- * (kt_i, kf_i), stride (st_i, sf_i) and padding (0, kf_i / 2), so per axis n' = (n + 2 p - k) / s + 1.  Kernel sizes
- * 1..7 and strides 1..4; an input with fewer than one output frame is refused.  out (may be NULL) receives
- * {T1, F1, T2, F2, T1p, F1p}: the conv1 activation buffer is NHWC bf16 [B, T1p, F1p, C1] (T1p a multiple of st2, F1p of
- * sf2; conv2 reads it per stride phase). */
-int otb_conv_geometry2(int T, int F, int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, int* out);
-/* otb_conv_geometry2 at the shipped geometry (3x3, stride 2, both layers), T >= 7: T1 = (T-3)/2+1, F1 = (F-1)/2+1,
- * T2 = (T1-3)/2+1, F2 = (F1-1)/2+1; conv1 buffer [B, 2*(T2+1), 2*F2, C1]. */
-int otb_conv_geometry(int T, int F, int* T1, int* F1, int* T2, int* F2);
+/* The two-layer conv front end (frontend/conv.py:10-11,15-48,50-76,131-153).  Every conv entry point takes its geometry as
+ * eight ints kt1, kf1, st1, sf1, kt2, kf2, st2, sf2: layer i has kernel (kt_i, kf_i), stride (st_i, sf_i) and padding
+ * (0, kf_i / 2), so per axis n' = (n + 2 p - k) / s + 1.  Kernel sizes 1..7 and strides 1..4; an input with fewer than one
+ * output frame is refused.  The shipped front end is 3, 3, 2, 2, 3, 3, 2, 2 (two 3x3 convolutions at stride 2).
+ *
+ * Conv2dLayer output geometry, host only: out (may be NULL) receives {T1, F1, T2, F2, T1p, F1p}: the conv1 activation
+ * buffer is NHWC bf16 [B, T1p, F1p, C1] (T1p a multiple of st2, F1p of sf2; conv2 reads it per stride phase). */
+int otb_conv_geometry(int T, int F, int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, int* out);
 
-/* Conv2dLayer.forward #1 (frontend/conv.py:50-76; C_in = 1): relu(conv2d(x, w) + b).
- * x f32 [B,T,F]; w f32 [C1,1,kt1,kf1]; bias f32 [C1]; out bf16 NHWC conv1 buffer (otb_conv_geometry2), columns F1 ..
+/* Conv2dLayer.forward #1 (C_in = 1): relu(conv2d(x, w) + b).
+ * x f32 [B,T,F]; w f32 [C1,1,kt1,kf1]; bias f32 [C1]; out bf16 NHWC conv1 buffer (otb_conv_geometry), columns F1 ..
  * F1p-1 written as zero.  C1 % 8 == 0, at most 2048 (1024 for kernels wider than 3, 512 wider than 5). */
-int otb_conv1_relu2(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1, int kt1, int kf1,
-                    int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
-int otb_conv1_relu(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1,
-                   void* stream);   /* the shipped geometry */
+int otb_conv1_relu(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1, int kt1, int kf1,
+                   int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
 
 /* Conv2dLayer.forward #2 + the transpose/reshape of ConvFrontEnd.forward (frontend/conv.py:63-64,145)
  * as a wgmma implicit GEMM.  in = conv1 buffer; w bf16 [C2, kt2*kf2*C1] with k = (kh*kf2+kw)*C1 + c;
  * out bf16 [B*T2, F2*C2] with feature index f*C2 + c (the caller permutes output_layer.weight columns
  * from the reference's c*F2 + f order once at load time).  C1 % 64 == 0, C2 % 8 == 0, F2 <= 128. */
-int otb_conv2_relu2(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2, int kt1,
-                    int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
-int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2,
-                   void* stream);   /* the shipped geometry */
+int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2, int kt1,
+                   int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
 
 /* nn.Linear with a fused epilogue on wgmma tensor cores: out[M,N] = epi(a[M,K] w[N(,2N),K]^T + bias).
  * a, w bf16 (lda, ldw in elements, multiples of 8); out bf16 or f32 (out_f32; RESID and RESID_LN write bf16 only and
@@ -170,19 +165,17 @@ int otb_embed_posenc(const int64_t* tok, int tok_stride, const void* emb, const 
 int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int V, void* stream);
 
 /* Decode-step self-attention over a per-hypothesis KV cache (the cache API the reference left as a
- * stub, decoder/transformer.py:92-126,188-203): qkv bf16 [N,3d] of the newest token; kc/vc bf16
- * [Lmax,N,d]; anc i32 [2,N,Lmax]; *step_ptr = 0-based position; out bf16 [N,d]; head width d_k 64 or 96 (d = H*d_k).
+ * stub, decoder/transformer.py:92-126,188-203): qkv bf16 [N,3d] of the newest token; out bf16 [N,d]; head width d_k 64 or
+ * 96 (d = H*d_k).  Give exactly one of step_ptr and row_pos; the other is NULL.  Two cache layouts:
+ *   step_ptr (the beam search): *step_ptr = the 0-based position of every row; kc/vc bf16 [Lmax,N,d]; anc i32 [2,N,Lmax].
+ *   row_pos (the LM-fused CTC prefix beam search, where slots hold prefixes of different lengths): row n's query is at
+ *   position row_pos[n] (-1: the row computes nothing and gets zeros); kc/vc bf16 [cache rows, d]; anc i32 [N, Lmax]
+ *   lists the cache row of each position 0..row_pos[n] of row n, and the newest K/V are written to cache row
+ *   anc[n][row_pos[n]].
  * Lmax <= 1023; above 128 the prefix is read in chunks of 128 keys with an online softmax.  Shared memory per CTA:
  * min(H, 4) * (min(Lmax rounded up to 32, 128) * d_k * 2 + d_k * 4) bytes. */
-int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
-                         int H, int Lmax, int d_k, void* stream);
-
-/* The same attention with a position per row (the LM-fused CTC prefix beam search, where slots hold prefixes of different
- * lengths): row n's query is at position row_pos[n] (-1: the row computes nothing and gets zeros); kc/vc bf16
- * [cache rows, d]; anc i32 [N, Lmax] lists the cache row of each position 0..row_pos[n] of row n, and the newest K/V are
- * written to cache row anc[n][row_pos[n]]. */
-int otb_decode_self_attn_rows(const void* qkv, void* kc, void* vc, const int* anc, const int* row_pos, void* out, int N, int H,
-                              int Lmax, int d_k, void* stream);
+int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, const int* row_pos, void* out,
+                         int N, int H, int Lmax, int d_k, void* stream);
 
 /* LabelSmoothingLoss.forward (module/loss.py:21-48) fused: per-token KL(smoothed one-hot || softmax), PAD rows 0,
  * mean over non-PAD tokens.  logits f32 [rows, ldl]; targets i64 [rows]; tok_loss f32 [rows]; loss f32 [1];
@@ -205,19 +198,18 @@ typedef struct {
 
 /* recognize() initial state (recognize/speech2text.py:54-58). */
 int otb_beam_init(const otb_beam_state* st, void* stream);
-/* SpeechToTextRecognizer.decode_step after the decoder call (recognize/speech2text.py:102-153,156-192).
- * logp f32 [N, ldl] log-probs; lm_logp optional (shallow fusion, :102-105).  dbg_ktok i64 [N,beam] and
- * dbg_offs i32 [N] (optional) receive last_k_preds / offset_k_indices for parity traces. */
-int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight,
-                  const otb_beam_state* st, int64_t* dbg_ktok, int32_t* dbg_offs, void* stream);
+/* SpeechToTextRecognizer.decode_step after the decoder call (recognize/speech2text.py:102-153,156-192).  Give either
+ * logp f32 [N, ldl] log-probs, with lm_logp optional (shallow fusion, :102-105), or the per-hypothesis top-k already
+ * computed by otb_logsoftmax_topk (k == beam): topk_val f32 / topk_idx i32 [N, beam], with logp NULL and ldl, V, lm_logp,
+ * ld_lm, lm_weight unused.  dbg_ktok i64 [N,beam] and dbg_offs i32 [N] (optional) receive last_k_preds / offset_k_indices
+ * for parity traces. */
+int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, const float* topk_val,
+                  const int32_t* topk_idx, const otb_beam_state* st, int64_t* dbg_ktok, int32_t* dbg_offs, void* stream);
 /* Fused log_softmax (+ lm_weight * lm_logp) + per-row top-k (decoder/transformer.py:206 + speech2text.py:102-112):
  * logits f32 [rows, ldl] -> out_val f32 [rows,k] (log-prob values, descending), out_idx i32 [rows,k];
  * out_logp (optional, f32 [rows, ld_logp]) additionally receives the full log-prob rows. */
 int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, int k,
                         int rows, float* out_val, int32_t* out_idx, float* out_logp, int ld_logp, void* stream);
-/* otb_beam_step with the per-hypothesis top-k already computed by otb_logsoftmax_topk (k == beam). */
-int otb_beam_step_topk(const float* topk_val, const int32_t* topk_idx, const otb_beam_state* st, int64_t* dbg_ktok,
-                       int32_t* dbg_offs, void* stream);
 /* Materialise preds i64 [N, ld] (column 0 = BOS) after `steps` steps from the back-pointers. */
 int otb_beam_reconstruct(const otb_beam_state* st, int64_t* preds, int ld, int steps, void* stream);
 /* Tail of recognize() (recognize/speech2text.py:70-91). out_preds i64 [B,nbest,Lmax], out_scores f32 [B,nbest]. */
@@ -267,22 +259,17 @@ int otb_decode_persistent(const otb_mega_model* model, const void* kvx, const in
  * train/trainer.py:206-234).  The reference differentiates through torch autograd; the entry points below are the
  * hand-written backward of each forward op above.  bf16 activations / gradients, fp32 parameter gradients. */
 
-/* Backward of otb_attention (d_k = 64, no bd / resid; lse as that forward stored it): dq, dk, dv written at column offsets
+/* Backward of otb_attention (d_k = 64, no resid; lse as that forward stored it): dq, dk, dv written at column offsets
  * d*_col0 + 64*h of their matrices (e.g. the three thirds of one [M,3d] dqkv buffer).  dsum f32 [B,H,Tq] is scratch.
- * wgmma, scores recomputed. */
+ * wgmma, scores recomputed.  bd and dbd are both NULL, or both set for rel-pos attention: the forward was otb_attention with
+ * the band bd f32 [H, B*Tq, ldbd] (Tq == Tk, not causal).  The band is added to the recomputed scores, and its gradient dS
+ * (the gradient of the raw score sum, which includes 1/sqrt(d_k)) is written to dbd bf16 [H, B*Tq, lddbd] at column
+ * j - i + Tq - 1 (lddbd: 2 Tq - 1 rounded up to 8).  The caller zeroes dbd: entries without a visible key are not written. */
 int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
                       const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
                       int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
-                      int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, void* stream);
-/* otb_attention_bwd for rel-pos attention: the forward was otb_attention with the band bd f32 [H, B*Tq, ldbd] (Tq == Tk, not
- * causal, d_k = 64).  The band is added to the recomputed scores, and its gradient dS (the gradient of the raw score sum, which
- * includes 1/sqrt(d_k)) is written to dbd bf16 [H, B*Tq, lddbd] at column j - i + Tq - 1 (lddbd: 2 Tq - 1 rounded up to 8).
- * The caller zeroes dbd: entries without a visible key are not written. */
-int otb_attention_bwd_bd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                         const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
-                         int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
-                         int Tq, int Tk, const int* kv_len, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd,
-                         void* dbd, int lddbd, void* stream);
+                      int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd,
+                      void* dbd, int lddbd, void* stream);
 /* Residual dropout without a GEMM in front: out = resid + alpha * keep(seed, site, row, col) / (1 - p) * x, with the mask of
  * otb_linear_dropout_resid / otb_dropout_bwd.  resid may be NULL (out = alpha * dropout_p(x): also the backward of such a
  * site).  row_len (optional, i32 [M / row_period]): rows with row % row_period >= row_len[row / row_period] read x as zero.
@@ -465,15 +452,15 @@ int otb_ctc_prefix_init(const float* lp, int ld, int B, int T, const int32_t* in
  * otb_logsoftmax_topk with k = P, beam <= P <= 16; cand_val = logp_att + lm_weight * lm_logp[cand_id] when lm_logp is given)
  * gamma_cand f32 [N, P, T, 2] and psi_cand f32 [N, P] of the hypothesis extended by the candidate, the joint score
  * (1 - ctc_weight) logp_att + ctc_weight (psi_cand - psi) + lm_weight lm_logp (-inf where psi_cand is -inf, never NaN), and
- * the `beam` best candidates by it into out_val f32 / out_idx i32 [N, beam] (descending, ties to the lower id), the layout
- * otb_beam_step_topk takes.  Does nothing once the search has ended. */
+ * the `beam` best candidates by it into out_val f32 / out_idx i32 [N, beam] (descending, ties to the lower id), the top-k
+ * layout otb_beam_step takes.  Does nothing once the search has ended. */
 int otb_ctc_prefix_score(const float* lp, int ld, int T, int V, const int32_t* in_len, int blank, const float* gamma,
                          const float* psi, const float* cand_val, const int32_t* cand_id, int P, const float* lm_logp, int ld_lm,
                          float lm_weight, float ctc_weight, const otb_beam_state* st, float* gamma_cand, float* psi_cand,
                          float* out_val, int32_t* out_idx, void* stream);
-/* After otb_beam_step_topk: every new row takes gamma_cand / psi_cand of its parent's candidate that names its token into
- * the other half of gamma / psi; a row whose token is <S/E> keeps its parent's state.  Does nothing once the search has
- * ended. */
+/* After otb_beam_step on those top-k: every new row takes gamma_cand / psi_cand of its parent's candidate that names its
+ * token into the other half of gamma / psi; a row whose token is <S/E> keeps its parent's state.  Does nothing once the
+ * search has ended. */
 int otb_ctc_prefix_advance(const otb_beam_state* st, const int32_t* cand_id, int P, int T, const int32_t* in_len,
                            const float* gamma_cand, const float* psi_cand, float* gamma, float* psi, void* stream);
 
@@ -522,21 +509,18 @@ int otb_mwer_coeff(const int32_t* len, const int32_t* err, const float* tok_lp, 
 int otb_mwer_grad(const float* logits, int ld, int rows, int V, const int32_t* target, const float* tok_lp, const float* coeff, int Lp,
                   void* dlogits, void* stream);
 
-/* Conv2d front end backward (frontend/conv.py:50-76 under autograd).  h1 = conv1 activation buffer (layout of
- * otb_conv1_relu2).  col bf16 [B*T2*F2, kt2*kf2*C1] = im2col of h1 for conv2 (k = (kh*kf2+kw)*C1 + c): conv2's weight
- * gradient is otb_linear_wgrad(dpre2, col) and its input gradient dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu2
- * folds dcol back onto the conv1 grid and applies ReLU' -> dpre1 (h1 layout).  otb_conv1_wgrad2: out f32
- * [C1, kt1*kf1 + 1] = tap gradients + the bias gradient of conv1 (C_in = 1; C1 <= 256).  The entry points without the
- * 2 take the shipped geometry. */
-int otb_conv_im2col2(const void* h1, void* col, int B, int T, int F, int C1, int kt1, int kf1, int st1, int sf1, int kt2,
-                     int kf2, int st2, int sf2, void* stream);
-int otb_conv_col2im_relu2(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, int kt1, int kf1,
-                          int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
-int otb_conv1_wgrad2(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, int kt1, int kf1, int st1,
-                     int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
-int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream);
-int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, void* stream);
-int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, void* stream);
+/* Conv2d front end backward (frontend/conv.py:50-76 under autograd), at the geometry of the forward.  h1 = conv1
+ * activation buffer (layout of otb_conv1_relu).  col bf16 [B*T2*F2, kt2*kf2*C1] = im2col of h1 for conv2
+ * (k = (kh*kf2+kw)*C1 + c): conv2's weight gradient is otb_linear_wgrad(dpre2, col) and its input gradient
+ * dcol = otb_linear(dpre2, W2^T).  otb_conv_col2im_relu folds dcol back onto the conv1 grid and applies ReLU' -> dpre1
+ * (h1 layout).  otb_conv1_wgrad: out f32 [C1, kt1*kf1 + 1] = tap gradients + the bias gradient of conv1 (C_in = 1;
+ * C1 <= 256). */
+int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, int kt1, int kf1, int st1, int sf1, int kt2,
+                    int kf2, int st2, int sf2, void* stream);
+int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, int kt1, int kf1,
+                         int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
+int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, int kt1, int kf1, int st1,
+                    int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
 
 /* SpecAugment (data/augment.py:9-41) applied on the device: zero n_freq frequency bands and n_time time bands per
  * utterance.  x f32 [B,T,F] in place; bands i32 [B, 2*(n_freq+n_time)] = (f0, width)*n_freq, (t0, width)*n_time drawn

@@ -43,12 +43,9 @@ _SIGS = {
     'otb_set_tile_policy': (c_int, [c_int]),
     'otb_debug_decode_timing': (c_int, [_P, c_int]),
     'otb_set_decode_barrier': (c_int, [c_int]),
-    'otb_conv_geometry': (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
-    'otb_conv_geometry2': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int)]),
-    'otb_conv1_relu2': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv2_relu2': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv1_relu': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv2_relu': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv_geometry': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int)]),
+    'otb_conv1_relu': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv2_relu': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_linear': (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, _P,
                            c_float, c_float, _P, c_int, _P, c_int, _P]),
     'otb_gemm_config': (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int)]),
@@ -65,20 +62,16 @@ _SIGS = {
     'otb_sinusoid_table': (c_int, [_P, c_int, c_int, c_int, _P]),
     'otb_embed_posenc': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, _P, _P, c_int, _P]),
     'otb_log_softmax': (c_int, [_P, c_int, _P, c_int, c_int, c_int, _P]),
-    'otb_decode_self_attn': (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
-    'otb_decode_self_attn_rows': (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    'otb_decode_self_attn': (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'otb_ls_ce': (c_int, [_P, c_int, _P, c_int, c_int, c_float, c_int, _P, _P, _P, _P, c_int, c_int, _P]),
     'otb_beam_init': (c_int, [POINTER(BeamStateC), _P]),
-    'otb_beam_step': (c_int, [_P, c_int, c_int, _P, c_int, c_float, POINTER(BeamStateC), _P, _P, _P]),
-    'otb_beam_step_topk': (c_int, [_P, _P, POINTER(BeamStateC), _P, _P, _P]),
+    'otb_beam_step': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, _P, POINTER(BeamStateC), _P, _P, _P]),
     'otb_logsoftmax_topk': (c_int, [_P, c_int, c_int, _P, c_int, c_float, c_int, c_int, _P, _P, _P, c_int, _P]),
     'otb_beam_reconstruct': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P]),
     'otb_beam_finalize': (c_int, [POINTER(BeamStateC), c_float, c_float, c_int, _P, _P, _P]),
     'otb_attention_bwd': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_int, c_int,
-                                  _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P]),
-    'otb_attention_bwd_bd': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_int, c_int,
-                                     _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P, c_int,
-                                     _P, c_int, _P]),
+                                  _P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P,
+                                  c_int, _P, c_int, _P]),
     'otb_dropout_add': (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_float, c_float, _P, ctypes.c_uint32, _P, c_int, _P]),
     'otb_conformer_conv_train': (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_float, c_float, _P, _P, _P, c_int, c_int, c_int, c_int,
                                          _P]),
@@ -120,12 +113,9 @@ _SIGS = {
     'otb_edit_distance': (c_int, [_P, c_int, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P, _P]),
     'otb_mwer_coeff': (c_int, [_P, _P, _P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P]),
     'otb_mwer_grad': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
-    'otb_conv_im2col': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv_col2im_relu': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv1_wgrad': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv_im2col2': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv_col2im_relu2': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
-    'otb_conv1_wgrad2': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv_im2col': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv_col2im_relu': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'otb_conv1_wgrad': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_spec_augment': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_lstm_config': (c_int, [c_int, c_int, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     'otb_lstm_fwd': (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, _P]),

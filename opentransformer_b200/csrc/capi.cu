@@ -59,6 +59,9 @@ using namespace otb;
         if (_e) return fail(where, _e);       \
         return 0;                             \
     } while (0)
+// the eight ints of the conv front end's geometry: kernel (kt, kf) and stride (st, sf) of conv1, then of conv2
+#define CONV_GEOM int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2
+#define CONV_ARGS kt1, kf1, st1, sf1, kt2, kf2, st2, sf2
 
 extern "C" {
 
@@ -84,9 +87,9 @@ int otb_set_decode_barrier(int kind) {
     return 0;
 }
 
-int otb_conv_geometry2(int T, int F, int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, int* out) {
+int otb_conv_geometry(int T, int F, CONV_GEOM, int* out) {
     ConvGeom g;
-    if (const char* e = conv_geometry(T, F, kt1, kf1, st1, sf1, kt2, kf2, st2, sf2, &g)) return fail("otb_conv_geometry2", e);
+    if (const char* e = conv_geometry(T, F, CONV_ARGS, &g)) return fail("otb_conv_geometry", e);
     if (out) {
         out[0] = g.T1; out[1] = g.F1; out[2] = g.T2; out[3] = g.F2;
         out[4] = g.st2 * g.T1s; out[5] = g.sf2 * g.F1s;
@@ -94,35 +97,18 @@ int otb_conv_geometry2(int T, int F, int kt1, int kf1, int st1, int sf1, int kt2
     return 0;
 }
 
-int otb_conv_geometry(int T, int F, int* T1, int* F1, int* T2, int* F2) {
-    int g[6];
-    if (T < 7 || F < 1) return fail("otb_conv_geometry", "need T >= 7 and F >= 1");
-    if (otb_conv_geometry2(T, F, 3, 3, 2, 2, 3, 3, 2, 2, g)) return 1;
-    if (T1) *T1 = g[0];
-    if (F1) *F1 = g[1];
-    if (T2) *T2 = g[2];
-    if (F2) *F2 = g[3];
-    return 0;
-}
-
-int otb_conv1_relu2(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1, int kt1, int kf1,
-                    int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream) {
+int otb_conv1_relu(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1, CONV_GEOM,
+                   void* stream) {
     ConvGeom g;
-    if (const char* e = conv_geometry(T, F, kt1, kf1, st1, sf1, kt2, kf2, st2, sf2, &g)) return fail("otb_conv1_relu", e);
+    if (const char* e = conv_geometry(T, F, CONV_ARGS, &g)) return fail("otb_conv1_relu", e);
     if (!x || !w || !bias || !out || B < 1) return fail("otb_conv1_relu", "null pointer or empty batch");
     RET("otb_conv1_relu", conv1_launch(ST(stream), x, w, bias, reinterpret_cast<bf16*>(out), B, T, F, g, C1));
 }
 
-int otb_conv1_relu(const float* x, const float* w, const float* bias, void* out, int B, int T, int F, int C1,
+int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2, CONV_GEOM,
                    void* stream) {
-    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
-    return otb_conv1_relu2(x, w, bias, out, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
-}
-
-int otb_conv2_relu2(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2, int kt1,
-                    int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2, void* stream) {
     ConvGeom g;
-    if (const char* e = conv_geometry(T, F, kt1, kf1, st1, sf1, kt2, kf2, st2, sf2, &g)) return fail("otb_conv2_relu", e);
+    if (const char* e = conv_geometry(T, F, CONV_ARGS, &g)) return fail("otb_conv2_relu", e);
     if (!in || !w || !bias || !out || B < 1) return fail("otb_conv2_relu", "null pointer or empty batch");
     if (C1 % 64) return fail("otb_conv2_relu", "C1 must be a multiple of 64 (one 128-byte tap per k-block)");
     if (C2 % 8) return fail("otb_conv2_relu", "C2 must be a multiple of 8");
@@ -156,12 +142,6 @@ int otb_conv2_relu2(const void* in, const void* w, const float* bias, void* out,
             p.conv_tap[kh * kf2 + kw] = (unsigned)par_f | (unsigned)(f0 + 8) << 8 | (unsigned)(kh % st2) << 16 | (unsigned)(kh / st2) << 24;
         }
     RET("otb_conv2_relu", gemm_launch(ST(stream), nullptr, 0, w, K, C2, EPI_RELU, p, &cmap));
-}
-
-int otb_conv2_relu(const void* in, const void* w, const float* bias, void* out, int B, int T, int F, int C1, int C2,
-                   void* stream) {
-    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
-    return otb_conv2_relu2(in, w, bias, out, B, T, F, C1, C2, 3, 3, 2, 2, 3, 3, 2, 2, stream);
 }
 
 int otb_linear(const void* a, int lda, const void* w, int ldw, const float* bias, void* out, int ldc, int M, int N,
@@ -308,22 +288,14 @@ int otb_log_softmax(const float* x, int ldx, float* out, int ldo, int rows, int 
     RET("otb_log_softmax", log_softmax_launch(ST(stream), x, ldx, out, ldo, rows, V));
 }
 
-int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, void* out, int N,
-                         int H, int Lmax, int d_k, void* stream) {
-    if (!qkv || !kc || !vc || !anc || !step_ptr || !out) return fail("otb_decode_self_attn", "null operand");
+int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, const int* step_ptr, const int* row_pos, void* out,
+                         int N, int H, int Lmax, int d_k, void* stream) {
+    if (!qkv || !kc || !vc || !anc || !out) return fail("otb_decode_self_attn", "null operand");
+    if (!step_ptr == !row_pos) return fail("otb_decode_self_attn", "give exactly one of step_ptr and row_pos");
     if (d_k != 64 && d_k != 96) return fail("otb_decode_self_attn", "head width d_k must be 64 or 96");
     RET("otb_decode_self_attn",
         decode_self_attn_launch(ST(stream), reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(kc),
-                                reinterpret_cast<bf16*>(vc), anc, step_ptr, reinterpret_cast<bf16*>(out), N, H, Lmax, d_k));
-}
-
-int otb_decode_self_attn_rows(const void* qkv, void* kc, void* vc, const int* anc, const int* row_pos, void* out, int N, int H,
-                              int Lmax, int d_k, void* stream) {
-    if (!qkv || !kc || !vc || !anc || !row_pos || !out) return fail("otb_decode_self_attn_rows", "null operand");
-    if (d_k != 64 && d_k != 96) return fail("otb_decode_self_attn_rows", "head width d_k must be 64 or 96");
-    RET("otb_decode_self_attn_rows",
-        decode_self_attn_launch(ST(stream), reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(kc),
-                                reinterpret_cast<bf16*>(vc), anc, nullptr, reinterpret_cast<bf16*>(out), N, H, Lmax, d_k, row_pos));
+                                reinterpret_cast<bf16*>(vc), anc, step_ptr, reinterpret_cast<bf16*>(out), N, H, Lmax, d_k, row_pos));
 }
 
 int otb_ls_ce(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,
@@ -341,18 +313,13 @@ int otb_beam_init(const otb_beam_state* st, void* stream) {
     RET("otb_beam_init", beam_init_launch(ST(stream), to_state(st)));
 }
 
-int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight,
-                  const otb_beam_state* st, int64_t* dbg_ktok, int32_t* dbg_offs, void* stream) {
-    if (!st || !logp) return fail("otb_beam_step", "null operand");
+int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, const float* topk_val,
+                  const int32_t* topk_idx, const otb_beam_state* st, int64_t* dbg_ktok, int32_t* dbg_offs, void* stream) {
+    if (!st) return fail("otb_beam_step", "null state");
+    if (logp ? (topk_val || topk_idx) : (!topk_val || !topk_idx))
+        return fail("otb_beam_step", "give either logp or both topk_val and topk_idx");
     RET("otb_beam_step", beam_step_launch(ST(stream), logp, ldl, V, lm_logp, ld_lm, lm_weight, to_state(st),
-                                          reinterpret_cast<long long*>(dbg_ktok), dbg_offs, nullptr, nullptr));
-}
-
-int otb_beam_step_topk(const float* topk_val, const int32_t* topk_idx, const otb_beam_state* st, int64_t* dbg_ktok,
-                       int32_t* dbg_offs, void* stream) {
-    if (!st || !topk_val || !topk_idx) return fail("otb_beam_step_topk", "null operand");
-    RET("otb_beam_step_topk", beam_step_launch(ST(stream), nullptr, 0, 0, nullptr, 0, 0.f, to_state(st),
-                                               reinterpret_cast<long long*>(dbg_ktok), dbg_offs, topk_val, topk_idx));
+                                          reinterpret_cast<long long*>(dbg_ktok), dbg_offs, topk_val, topk_idx));
 }
 
 int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, int k,
@@ -397,14 +364,21 @@ int otb_decode_persistent(const otb_mega_model* model, const void* kvx, const in
                                                      max_steps, dbg_logp, dbg_scores, workspace, (size_t)workspace_bytes));
 }
 
-static int attention_bwd(const char* where, const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v,
-                         int ldv, const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq, int lddq,
-                         int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H, int Tq, int Tk,
-                         const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd, void* dbd,
-                         int lddbd, void* stream) {
-    if (!q || !k || !v || !out || !dout || !lse || !dsum || !dq || !dk || !dv) return fail(where, "null operand");
+int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
+                      const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
+                      int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
+                      int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd,
+                      void* dbd, int lddbd, void* stream) {
+    if (!q || !k || !v || !out || !dout || !lse || !dsum || !dq || !dk || !dv) return fail("otb_attention_bwd", "null operand");
     if ((q_col0 | k_col0 | v_col0 | dq_col0 | dk_col0 | dv_col0 | ldo | lddo | lddq | lddk | lddv) % 8)
-        return fail(where, "column offsets / leading dimensions must be multiples of 8");
+        return fail("otb_attention_bwd", "column offsets / leading dimensions must be multiples of 8");
+    if (!bd != !dbd) return fail("otb_attention_bwd", "bd and dbd must both be given or both be NULL");
+    if (bd) {
+        if (causal) return fail("otb_attention_bwd", "the rel-pos band is for non-causal attention");
+        if (Tq != Tk) return fail("otb_attention_bwd", "the rel-pos band needs Tq == Tk");
+        if (ldbd < 2 * Tq - 1 || lddbd < 2 * Tq - 1 || lddbd % 8)
+            return fail("otb_attention_bwd", "band pitches must hold 2 Tq - 1 columns; the gradient's must be a multiple of 8");
+    }
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
     p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk; p.kv_len = kv_len; p.causal = causal;
@@ -418,30 +392,7 @@ static int attention_bwd(const char* where, const void* q, int ldq, int q_rows, 
     p.dv = reinterpret_cast<bf16*>(dv); p.lddv = lddv; p.dv_col0 = dv_col0;
     p.bd = bd; p.ldbd = ldbd;
     p.dbd = reinterpret_cast<bf16*>(dbd); p.lddbd = lddbd;
-    RET(where, attn_bwd_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p));
-}
-
-int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                      const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
-                      int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
-                      int Tq, int Tk, const int* kv_len, int causal, int q_col0, int k_col0, int v_col0, void* stream) {
-    return attention_bwd("otb_attention_bwd", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, dout, lddo, lse, dsum, dq, lddq,
-                         dq_col0, dk, lddk, dk_col0, dv, lddv, dv_col0, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0,
-                         nullptr, 0, nullptr, 0, stream);
-}
-
-int otb_attention_bwd_bd(const void* q, int ldq, int q_rows, const void* k, int ldk, int k_rows, const void* v, int ldv,
-                         const void* out, int ldo, const void* dout, int lddo, const float* lse, float* dsum, void* dq,
-                         int lddq, int dq_col0, void* dk, int lddk, int dk_col0, void* dv, int lddv, int dv_col0, int B, int H,
-                         int Tq, int Tk, const int* kv_len, int q_col0, int k_col0, int v_col0, const float* bd, int ldbd,
-                         void* dbd, int lddbd, void* stream) {
-    if (!bd || !dbd) return fail("otb_attention_bwd_bd", "null band or band gradient");
-    if (Tq != Tk) return fail("otb_attention_bwd_bd", "the rel-pos band needs Tq == Tk");
-    if (ldbd < 2 * Tq - 1 || lddbd < 2 * Tq - 1 || lddbd % 8)
-        return fail("otb_attention_bwd_bd", "band pitches must hold 2 Tq - 1 columns; the gradient's must be a multiple of 8");
-    return attention_bwd("otb_attention_bwd_bd", q, ldq, q_rows, k, ldk, k_rows, v, ldv, out, ldo, dout, lddo, lse, dsum, dq, lddq,
-                         dq_col0, dk, lddk, dk_col0, dv, lddv, dv_col0, B, H, Tq, Tk, kv_len, 0, q_col0, k_col0, v_col0, bd, ldbd,
-                         dbd, lddbd, stream);
+    RET("otb_attention_bwd", attn_bwd_launch(ST(stream), q, ldq, q_rows, k, ldk, k_rows, v, ldv, p));
 }
 
 int otb_dropout_add(const void* x, int ldx, const void* resid, int ldr, void* out, int ldo, int M, int N, float alpha, float p,
@@ -689,43 +640,27 @@ int otb_mwer_grad(const float* logits, int ld, int rows, int V, const int32_t* t
     RET("otb_mwer_grad", mwer_grad_launch(ST(stream), logits, ld, rows, V, target, tok_lp, coeff, Lp, reinterpret_cast<bf16*>(dlogits)));
 }
 
-#define CONV_GEOM2 int kt1, int kf1, int st1, int sf1, int kt2, int kf2, int st2, int sf2
-#define CONV_ARGS2 kt1, kf1, st1, sf1, kt2, kf2, st2, sf2
-int otb_conv_im2col2(const void* h1, void* col, int B, int T, int F, int C1, CONV_GEOM2, void* stream) {
+int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, CONV_GEOM, void* stream) {
     ConvGeom g;
-    if (const char* e = conv_geometry(T, F, CONV_ARGS2, &g)) return fail("otb_conv_im2col", e);
+    if (const char* e = conv_geometry(T, F, CONV_ARGS, &g)) return fail("otb_conv_im2col", e);
     if (!h1 || !col) return fail("otb_conv_im2col", "null operand");
     RET("otb_conv_im2col", im2col_launch(ST(stream), reinterpret_cast<const bf16*>(h1), reinterpret_cast<bf16*>(col), B, g, C1));
 }
-int otb_conv_im2col(const void* h1, void* col, int B, int T, int F, int C1, void* stream) {
-    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
-    return otb_conv_im2col2(h1, col, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
-}
 
-int otb_conv_col2im_relu2(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, CONV_GEOM2, void* stream) {
+int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, CONV_GEOM, void* stream) {
     ConvGeom g;
-    if (const char* e = conv_geometry(T, F, CONV_ARGS2, &g)) return fail("otb_conv_col2im_relu", e);
+    if (const char* e = conv_geometry(T, F, CONV_ARGS, &g)) return fail("otb_conv_col2im_relu", e);
     if (!dcol || !h1 || !dpre1) return fail("otb_conv_col2im_relu", "null operand");
     RET("otb_conv_col2im_relu", col2im_relu_launch(ST(stream), reinterpret_cast<const bf16*>(dcol), reinterpret_cast<const bf16*>(h1),
                                                    reinterpret_cast<bf16*>(dpre1), B, g, C1));
 }
-int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, int T, int F, int C1, void* stream) {
-    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
-    return otb_conv_col2im_relu2(dcol, h1, dpre1, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
-}
 
-int otb_conv1_wgrad2(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, CONV_GEOM2, void* stream) {
+int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, CONV_GEOM, void* stream) {
     ConvGeom g;
-    if (const char* e = conv_geometry(T, F, CONV_ARGS2, &g)) return fail("otb_conv1_wgrad", e);
+    if (const char* e = conv_geometry(T, F, CONV_ARGS, &g)) return fail("otb_conv1_wgrad", e);
     if (!dpre1 || !x || !out) return fail("otb_conv1_wgrad", "null operand");
     RET("otb_conv1_wgrad", conv1_wgrad_launch(ST(stream), reinterpret_cast<const bf16*>(dpre1), x, out, B, T, F, g, C1));
 }
-int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, void* stream) {
-    if (otb_conv_geometry(T, F, nullptr, nullptr, nullptr, nullptr)) return 1;
-    return otb_conv1_wgrad2(dpre1, x, out, B, T, F, C1, 3, 3, 2, 2, 3, 3, 2, 2, stream);
-}
-#undef CONV_GEOM2
-#undef CONV_ARGS2
 
 int otb_spec_augment(float* x, const int32_t* bands, int B, int T, int F, int n_freq, int n_time, void* stream) {
     if (!x || !bands || B < 1 || T < 1 || F < 1 || n_freq < 0 || n_time < 0) return fail("otb_spec_augment", "bad arguments");

@@ -14,7 +14,7 @@
 // parity of the search's step counter, as for the ancestry table of the KV cache.  Three kernels:
 //   init     gamma(empty prefix) = running sum of the blank column, psi = 0, in half 0
 //   score    one warp per hypothesis, one lane per candidate: the recursion over T_b frames into the candidate scratch,
-//            then the joint step score of each candidate and the hypothesis' `beam` best, in otb_beam_step_topk's layout
+//            then the joint step score of each candidate and the hypothesis' `beam` best, in otb_beam_step's top-k layout
 //   advance  after the beam step: every new row takes its (parent, token)'s candidate state into the other half
 // score and advance read {step, done} of the search state on the device and do nothing once the search has ended.
 #include <math.h>

@@ -9,7 +9,7 @@ source slot's LM row (and LSTM state), a row that extended runs the LM on its ne
     layer, the head GEMM and otb_log_softmax.
   * Transformer LM: the K/V of each prefix node (node ids 1 + t * beam + s of DESIGN.md 4.7, 0 the BOS) are stored once
     per utterance, [blocks, B * (1 + T' * beam), d]; each row lists the cache rows of its prefix (anc, rewritten by the
-    search step) and queries at its own position (otb_embed_posenc / otb_decode_self_attn_rows with row_pos).
+    search step) and queries at its own position (otb_embed_posenc / otb_decode_self_attn with row_pos).
 """
 import torch
 

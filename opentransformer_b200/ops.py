@@ -66,13 +66,13 @@ def _need(t, dtype, name):
     return t
 
 
-def _mat(t, name):
-    """A GEMM operand: 2-D bf16 CUDA tensor with unit column stride (row-strided views such as one head's columns of a
-    wider matrix are fine: the TMA map takes the row pitch)."""
+def _mat(t, name, dtype=BF16):
+    """A matrix operand: 2-D CUDA tensor of `dtype` (a GEMM's bf16 by default) with unit column stride (row-strided views
+    such as one head's columns of a wider matrix are fine: the TMA map takes the row pitch)."""
     if not t.is_cuda:
         raise RuntimeError(f'{name} must be a CUDA tensor: the CUDA hot path has no CPU fallback')
-    if t.dtype != BF16 or t.dim() != 2 or t.stride(1) != 1:
-        raise TypeError(f'{name} must be a 2-D bf16 tensor with unit column stride')
+    if t.dtype != dtype or t.dim() != 2 or t.stride(1) != 1:
+        raise TypeError(f'{name} must be a 2-D {dtype} tensor with unit column stride')
     return t
 
 
@@ -91,22 +91,21 @@ def num_sms():
     return int(_lib.lib().otb_num_sms())
 
 
-def conv_geometry(T, F):
-    t1, f1, t2, f2 = (ctypes.c_int() for _ in range(4))
-    check(_lib.lib().otb_conv_geometry(T, F, t1, f1, t2, f2), 'otb_conv_geometry')
-    return t1.value, f1.value, t2.value, f2.value
-
-
 # (kt1, kf1, st1, sf1, kt2, kf2, st2, sf2) of the shipped conv front end: two 3x3 convolutions at stride 2
 CONV_SHIPPED = (3, 3, 2, 2, 3, 3, 2, 2)
 
 
 def conv_sizes(T, F, geom=CONV_SHIPPED):
-    """otb_conv_geometry2 -> (T1, F1, T2, F2, T1p, F1p): the two layers' output sizes and the conv1 activation buffer's rows
+    """otb_conv_geometry -> (T1, F1, T2, F2, T1p, F1p): the two layers' output sizes and the conv1 activation buffer's rows
     and columns.  The front end's own geometry (modules.conv_frontend_geometry) is what callers size their outputs by."""
     out = (ctypes.c_int * 6)()
-    check(_lib.lib().otb_conv_geometry2(T, F, *geom, out), 'otb_conv_geometry2')
+    check(_lib.lib().otb_conv_geometry(T, F, *geom, out), 'otb_conv_geometry')
     return tuple(out)
+
+
+def conv_geometry(T, F):
+    """(T1, F1, T2, F2) of the shipped conv front end."""
+    return conv_sizes(T, F)[:4]
 
 
 def conv1_relu(x, w, bias, out=None, geom=CONV_SHIPPED):
@@ -117,7 +116,7 @@ def conv1_relu(x, w, bias, out=None, geom=CONV_SHIPPED):
     T1p, F1p = conv_sizes(T, F, geom)[4:]
     if out is None:
         out = torch.empty(B, T1p, F1p, C1, dtype=BF16, device=x.device)
-    check(_lib.lib().otb_conv1_relu2(_p(x), _p(w), _p(bias), _p(out), B, T, F, C1, *geom, _stream()), 'otb_conv1_relu')
+    check(_lib.lib().otb_conv1_relu(_p(x), _p(w), _p(bias), _p(out), B, T, F, C1, *geom, _stream()), 'otb_conv1_relu')
     _count()
     return out
 
@@ -131,7 +130,7 @@ def conv2_relu(h1, w, bias, B, T, F, out=None, geom=CONV_SHIPPED):
     if out is None:
         out = torch.empty(B * T2, F2 * C2, dtype=BF16, device=h1.device)
     with _Timed('conv2_gemm', 2.0 * B * T2 * F2 * C2 * K):
-        check(_lib.lib().otb_conv2_relu2(_p(h1), _p(w), _p(bias), _p(out), B, T, F, C1, C2, *geom, _stream()),
+        check(_lib.lib().otb_conv2_relu(_p(h1), _p(w), _p(bias), _p(out), B, T, F, C1, C2, *geom, _stream()),
               'otb_conv2_relu')
     _count()
     return out
@@ -406,7 +405,7 @@ DECODE_MAX_LEN = 1023   # cached positions of otb_decode_self_attn: the longest 
 
 def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None, row_pos=None):
     """kc/vc bf16 [Lmax, N, d]: the head width d_k = d // H is taken from the cache.
-    row_pos i32 [N] (otb_decode_self_attn_rows): a query position per row (-1: zeros), step_ptr unused, kc/vc bf16
+    row_pos i32 [N]: a query position per row (-1: zeros) in place of step_ptr, which is then ignored; kc/vc bf16
     [cache rows, d] and anc i32 [N, Lmax] the cache row of each position of each row, the newest included."""
     d = kc.shape[-1]
     if d % H:
@@ -419,12 +418,9 @@ def decode_self_attn(qkv, kc, vc, anc, step_ptr, N, H, Lmax, out=None, row_pos=N
         _need(row_pos, torch.int32, 'row_pos'); _need(anc, torch.int32, 'anc')
         if anc.shape != (N, Lmax):
             raise ValueError(f'decode_self_attn: with row_pos, anc must be [N = {N}, Lmax = {Lmax}], got {tuple(anc.shape)}')
-        check(_lib.lib().otb_decode_self_attn_rows(_p(qkv), _p(kc), _p(vc), _p(anc), _p(row_pos), _p(out), N, H, Lmax, d_k,
-                                                   _stream()), 'otb_decode_self_attn_rows')
-        _count()
-        return out
-    check(_lib.lib().otb_decode_self_attn(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(out), N, H, Lmax, d_k, _stream()),
-          'otb_decode_self_attn')
+        step_ptr = None
+    check(_lib.lib().otb_decode_self_attn(_p(qkv), _p(kc), _p(vc), _p(anc), _p(step_ptr), _p(row_pos), _p(out), N, H, Lmax, d_k,
+                                          _stream()), 'otb_decode_self_attn')
     _count()
     return out
 
@@ -458,13 +454,14 @@ class BeamState:
     def step(self, logp, V, lm_logp=None, lm_weight=0.0, dbg_ktok=None, dbg_offs=None):
         _need(logp, torch.float32, 'logp')
         check(_lib.lib().otb_beam_step(_p(logp), logp.stride(0), V, _p(lm_logp),
-                                       lm_logp.stride(0) if lm_logp is not None else 0, lm_weight,
+                                       lm_logp.stride(0) if lm_logp is not None else 0, lm_weight, None, None,
                                        ctypes.byref(self.c), _p(dbg_ktok), _p(dbg_offs), _stream()), 'otb_beam_step')
         _count()
 
     def step_topk(self, topk_val, topk_idx, dbg_ktok=None, dbg_offs=None):
-        check(_lib.lib().otb_beam_step_topk(_p(topk_val), _p(topk_idx), ctypes.byref(self.c), _p(dbg_ktok),
-                                            _p(dbg_offs), _stream()), 'otb_beam_step_topk')
+        """The beam step on a per-hypothesis top-k (logsoftmax_topk with k = beam) instead of log-prob rows."""
+        check(_lib.lib().otb_beam_step(None, 0, 0, None, 0, 0.0, _p(topk_val), _p(topk_idx), ctypes.byref(self.c),
+                                       _p(dbg_ktok), _p(dbg_offs), _stream()), 'otb_beam_step')
         _count()
 
     def reconstruct(self, steps):
@@ -518,21 +515,21 @@ def attention_bwd(q, k, v, out, dout, lse, B, H, Tq, Tk, dq, dk, dv, kv_len=None
                   v_col0=0, dq_col0=0, dk_col0=0, dv_col0=0, bd=None, dbd=None):
     """Gradients of otb_attention written into dq/dk/dv (bf16 matrices, column offsets d*_col0).  With the rel-pos band bd
     f32 [H, B*Tq, ld] of the forward, its gradient is written into dbd bf16 [H, B*Tq, rel_band_ld(Tq)], which the caller
-    zeroes (otb_attention_bwd_bd)."""
+    zeroes."""
     for t, n in ((q, 'q'), (k, 'k'), (v, 'v'), (out, 'out'), (dout, 'dout'), (dq, 'dq'), (dk, 'dk'), (dv, 'dv')):
         _mat(t, n)
     dsum = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device)
-    args = (_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out), out.stride(0), _p(dout),
-            dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), dq_col0, _p(dk), dk.stride(0), dk_col0, _p(dv), dv.stride(0),
-            dv_col0, B, H, Tq, Tk, _p(kv_len))
-    if bd is None:
-        check(_lib.lib().otb_attention_bwd(*args, 1 if causal else 0, q_col0, k_col0, v_col0, _stream()), 'otb_attention_bwd')
-    else:
+    ldbd = lddbd = 0
+    if bd is not None:
         if causal:
             raise ValueError('attention_bwd: the rel-pos band is for non-causal self-attention')
         _need(bd, torch.float32, 'bd'); _need(dbd, BF16, 'dbd')
-        check(_lib.lib().otb_attention_bwd_bd(*args, q_col0, k_col0, v_col0, _p(bd), bd.shape[-1], _p(dbd), dbd.shape[-1],
-                                              _stream()), 'otb_attention_bwd_bd')
+        ldbd, lddbd = bd.shape[-1], dbd.shape[-1]
+    check(_lib.lib().otb_attention_bwd(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out),
+                                       out.stride(0), _p(dout), dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), dq_col0,
+                                       _p(dk), dk.stride(0), dk_col0, _p(dv), dv.stride(0), dv_col0, B, H, Tq, Tk, _p(kv_len),
+                                       1 if causal else 0, q_col0, k_col0, v_col0, _p(bd), ldbd, _p(dbd), lddbd, _stream()),
+          'otb_attention_bwd')
     _count(2)
 
 
@@ -1010,10 +1007,7 @@ def ctc_nbest_score(logp, B, T, in_len, targets, blank=0):
 def token_logprob(logits, V, target):
     """out f32 [rows] = log_softmax(logits[r, :V])[target[r]], 0 where target[r] < 0 (otb_token_logprob): each row is read
     once and no [rows, V] log-softmax is written.  logits f32 [rows, ld] with ld % 4 == 0; target i32 [rows]."""
-    if not logits.is_cuda:
-        raise RuntimeError('logits must be a CUDA tensor: the CUDA hot path has no CPU fallback')
-    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
-        raise TypeError('token_logprob: logits must be a 2-D f32 tensor with unit column stride')
+    _mat(logits, 'logits', torch.float32)
     rows = logits.shape[0]
     if target.shape != (rows,):
         raise ValueError(f'token_logprob: target must be [rows = {rows}], got {tuple(target.shape)}')
@@ -1099,10 +1093,7 @@ def mwer_grad(logits, V, target, tok_lp, coeff):
     """bf16 dlogits [rows, ld] = coeff[r // Lp] * (onehot(target[r]) - softmax(logits[r, :V])) (otb_mwer_grad): logits f32
     [rows, ld] (ld % 4 == 0), target i32 [rows] (-1: a zero row), tok_lp f32 [rows] = token_logprob(logits, V, target),
     coeff f32 [rows // Lp] (the hypotheses of Lp rows each); padding columns are zero."""
-    if not logits.is_cuda:
-        raise RuntimeError('logits must be a CUDA tensor: the CUDA hot path has no CPU fallback')
-    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
-        raise TypeError('mwer_grad: logits must be a 2-D f32 tensor with unit column stride')
+    _mat(logits, 'logits', torch.float32)
     rows, ld = logits.shape[0], logits.stride(0)
     coeff = coeff.reshape(-1)
     if target.shape != (rows,) or tok_lp.shape != (rows,) or coeff.numel() < 1 or rows % coeff.numel():
@@ -1119,14 +1110,14 @@ def mwer_grad(logits, V, target, tok_lp, coeff):
 def conv_im2col(h1, B, T, F, C1, geom=CONV_SHIPPED):
     _, _, T2, F2, _, _ = conv_sizes(T, F, geom)
     col = torch.empty(B * T2 * F2, geom[4] * geom[5] * C1, dtype=BF16, device=h1.device)
-    check(_lib.lib().otb_conv_im2col2(_p(h1), _p(col), B, T, F, C1, *geom, _stream()), 'otb_conv_im2col')
+    check(_lib.lib().otb_conv_im2col(_p(h1), _p(col), B, T, F, C1, *geom, _stream()), 'otb_conv_im2col')
     _count()
     return col
 
 
 def conv_col2im_relu(dcol, h1, B, T, F, C1, geom=CONV_SHIPPED):
     dpre1 = torch.empty_like(h1)
-    check(_lib.lib().otb_conv_col2im_relu2(_p(dcol), _p(h1), _p(dpre1), B, T, F, C1, *geom, _stream()), 'otb_conv_col2im_relu')
+    check(_lib.lib().otb_conv_col2im_relu(_p(dcol), _p(h1), _p(dpre1), B, T, F, C1, *geom, _stream()), 'otb_conv_col2im_relu')
     _count()
     return dpre1
 
@@ -1134,7 +1125,7 @@ def conv_col2im_relu(dcol, h1, B, T, F, C1, geom=CONV_SHIPPED):
 def conv1_wgrad(dpre1, x, B, T, F, C1, geom=CONV_SHIPPED):
     """-> f32 [C1, kt1*kf1 + 1]: conv1's tap gradients, then its bias gradient."""
     out = torch.empty(C1, geom[0] * geom[1] + 1, dtype=torch.float32, device=x.device)
-    check(_lib.lib().otb_conv1_wgrad2(_p(dpre1), _p(x), _p(out), B, T, F, C1, *geom, _stream()), 'otb_conv1_wgrad')
+    check(_lib.lib().otb_conv1_wgrad(_p(dpre1), _p(x), _p(out), B, T, F, C1, *geom, _stream()), 'otb_conv1_wgrad')
     _count()
     return out
 

@@ -119,14 +119,35 @@ def test_ctypes_structs_match_the_header():
     assert _lib.MEGA_MAX_LAYERS == int(defines['OTB_MEGA_MAX_LAYERS'])
 
 
-def test_version_3_and_error_reporting(libpath):
-    from opentransformer_b200 import _lib
+def test_version_4_and_error_reporting(libpath):
+    from opentransformer_b200 import _lib, ops
     lib = _lib.lib()
-    assert lib.otb_version() == 3
-    t1 = ctypes.c_int()
-    assert lib.otb_conv_geometry(1000, 80, t1, None, None, None) == 0 and t1.value == 499
-    assert lib.otb_conv_geometry(3, 80, None, None, None, None) != 0       # too short -> status, not abort
+    assert lib.otb_version() == 4
+    out = (ctypes.c_int * 6)()
+    assert lib.otb_conv_geometry(1000, 80, *ops.CONV_SHIPPED, out) == 0 and out[0] == 499
+    assert lib.otb_conv_geometry(3, 80, *ops.CONV_SHIPPED, out) != 0       # too short -> status, not abort
     assert b'otb_conv_geometry' in lib.otb_last_error()
+
+
+def _capi_definitions():
+    """-> [(name, body)] of every extern "C" otb_* function defined in csrc/capi.cu, comments stripped."""
+    text = open(os.path.join(ROOT, 'opentransformer_b200', 'csrc', 'capi.cu')).read()
+    text = re.sub(r'/\*.*?\*/|//[^\n]*', '', text, flags=re.S)
+    text = text[text.index('extern "C" {'):]
+    heads = list(re.finditer(r'^[A-Za-z][\w *]*?[ *](otb_\w+)\(', text, flags=re.M))
+    return [(h.group(1), text[h.end():heads[i + 1].start() if i + 1 < len(heads) else len(text)]) for i, h in enumerate(heads)]
+
+
+def test_every_entry_point_reports_under_its_own_name_and_calls_no_other():
+    """One C entry point per operation: each otb_* definition reports its errors (fail / RET) under its own name only, and
+    none forwards to another otb_* entry point, so the ABI does not grow wrappers that re-check and re-label errors."""
+    defs = _capi_definitions()
+    assert len(defs) == len(_header_symbols())
+    bad = []
+    for name, body in defs:
+        bad += [f'{name} reports as {w}' for w in re.findall(r'\b(?:fail|RET)\(\s*([^,]+?)\s*,', body) if w != f'"{name}"']
+        bad += [f'{name} calls {c}' for c in re.findall(r'\b(otb_\w+)\s*\(', body)]
+    assert not bad, '\n'.join(bad)
 
 
 def test_every_kernel_launches_through_one_helper():

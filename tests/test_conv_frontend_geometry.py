@@ -33,9 +33,9 @@ def test_restated_front_end_equals_the_reference(fixture):
         assert torch.equal(m, c['mask_out']), (kw['kernel_size'], kw['stride'])
 
 
-def test_port_geometry_equals_the_reference_module(fixture):
+def test_port_and_c_geometry_equal_the_reference_module(fixture):
     """T', the output mask and input_window of the port's module for T 1..64 and every (k, s) in 1..7 x 1..4; where the
-    reference's conv2d raises the port raises ValueError.  The C entry point (otb_conv_geometry2) agrees."""
+    reference's conv2d raises the port raises ValueError.  The C entry point (otb_conv_geometry) agrees."""
     from opentransformer_b200 import _lib
     from opentransformer_b200.modules import ConvFrontEnd
     fes = {}
@@ -49,11 +49,11 @@ def test_port_geometry_equals_the_reference_module(fixture):
                 fe.output_length(T)
             with pytest.raises(ValueError, match='too short'):
                 fe.output_mask(mask)
-            assert lib.otb_conv_geometry2(T, 9, k, k, s, s, k, k, s, s, out) != 0
+            assert lib.otb_conv_geometry(T, 9, k, k, s, s, k, k, s, s, out) != 0
             continue
         m = fe.output_mask(mask)
         assert (fe.output_length(T), m.shape[1]) == (T2, n_mask), (k, s, T)
-        assert lib.otb_conv_geometry2(T, 9, k, k, s, s, k, k, s, s, out) == 0
+        assert lib.otb_conv_geometry(T, 9, k, k, s, s, k, k, s, s, out) == 0
         assert list(out)[:4] == [v for hw in fe.sizes(T) for v in hw]
         assert fe.input_window() == (s * s, k + (k - 1) * s)
 

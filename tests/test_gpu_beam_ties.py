@@ -1,5 +1,5 @@
 """Ties and non-finite rows on the per-step graph path: the fused log-softmax + top-k (otb_logsoftmax_topk) and both beam
-steps (otb_beam_step, which ranks with warp_topk, and otb_beam_step_topk, which takes the fused top-k) against the tie-exact
+steps (otb_beam_step on log-probs, which ranks with warp_topk, and on the fused top-k) against the tie-exact
 restatement of tests/beam_ties_ref.py.  Rows with 127, 128, 129 and V equal maxima, a tie at the k-th place, V = 17 with
 k = 16 (every warp's slice of the fused kernel is shorter than k) and rows with fewer than k finite values (an LM that
 rules tokens out with lm_logp = -inf).  Both top-k kernels must return the same real token ids, lower index first,
@@ -90,8 +90,8 @@ def _state(B, beam, scores, flag):
 @pytest.mark.parametrize('kind,V,k', CASES)
 def test_graph_path_beam_steps_agree_on_ties(kind, V, k, start):
     """One beam step from the initial state (only hypothesis 0 alive) or from a state with equal scores across hypotheses
-    and finished hypotheses: otb_beam_step (log-probs + lm) and otb_beam_step_topk (the fused top-k) against the tie-exact
-    step on the same log-probs; tokens, parents, scores and flags bit-exact, and equal to each other."""
+    and finished hypotheses: otb_beam_step on log-probs + lm (BeamState.step) and on the fused top-k (BeamState.step_topk)
+    against the tie-exact step on the same log-probs; tokens, parents, scores and flags bit-exact, and equal to each other."""
     B, beam = 2, k
     n = B * beam
     x, lm = _rows(kind, n, V, k, seed=3 * V + k)
@@ -112,7 +112,7 @@ def test_graph_path_beam_steps_agree_on_ties(kind, V, k, start):
     st_b.step_topk(val.to(DEV).contiguous(), idx.int().to(DEV).contiguous())
     preds = torch.ones(n, 1, dtype=torch.long)
     lp_a = lp_plain.cpu() + (LM_W * lm if lm is not None else 0.0)
-    for name, st, lp in (('otb_beam_step', st_a, lp_a), ('otb_beam_step_topk', st_b, lp_fused)):
+    for name, st, lp in (('step', st_a, lp_a), ('step_topk', st_b, lp_fused)):
         tr = []
         _, r_scores, r_flag = btr.beam_step(lp, preds, scores, flag, beam, trace=tr)
         assert torch.equal(st.tok_hist[0].long().cpu(), tr[0]['tok']), f'{name}: tokens differ'

@@ -34,8 +34,8 @@ def _rel(a, b):
 # ------------------------------------------------------------------------------------------------ kernels
 @pytest.mark.parametrize('T', [7, 200, 249, 300])
 def test_relpos_attention_backward_matches_autograd(T):
-    """otb_attention_bwd_bd: dq, dk, dv and the band gradient dBD of softmax((QK^T + BD) / 8) V against fp64 autograd, with
-    ragged lengths and one utterance without any key."""
+    """otb_attention_bwd with the band: dq, dk, dv and the band gradient dBD of softmax((QK^T + BD) / 8) V against fp64
+    autograd, with ragged lengths and one utterance without any key."""
     g = torch.Generator().manual_seed(T)
     B, H, dk = 3, 4, 64
     d = H * dk

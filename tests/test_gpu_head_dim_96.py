@@ -113,7 +113,7 @@ def test_last_head_at_the_right_matrix_edge_96(width):
     assert bool((out[:, d:] == 7.0).all()), 'columns past H*96 were written'
 
 
-def test_merged_attention_entry_points_refuse_other_head_widths():
+def test_attention_and_decode_entry_points_refuse_other_head_widths():
     qkv = torch.zeros(8, 3 * 320, dtype=BF, device=DEV)
     with pytest.raises(NotImplementedError, match=r'\(64, 96\)'):
         ops.attention(qkv, qkv, qkv, 1, 4, 8, 8, k_col0=320, v_col0=640, d_k=80)
@@ -123,8 +123,8 @@ def test_merged_attention_entry_points_refuse_other_head_widths():
     assert lib.otb_attention(ops._p(qkv), qkv.stride(0), 8, ops._p(qkv), qkv.stride(0), 8, ops._p(qkv), qkv.stride(0),
                              ops._p(qkv), qkv.stride(0), 1, 4, 8, 8, None, 0, 0, 320, 640, None, 0, None, 0, None, 80, st) != 0
     assert b'64 or 96' in lib.otb_last_error()
-    assert lib.otb_decode_self_attn(ops._p(qkv), ops._p(qkv), ops._p(qkv), ops._p(qkv), ops._p(qkv), ops._p(qkv), 1, 4, 8, 80,
-                                    st) != 0
+    assert lib.otb_decode_self_attn(ops._p(qkv), ops._p(qkv), ops._p(qkv), ops._p(qkv), ops._p(qkv), None, ops._p(qkv), 1, 4, 8,
+                                    80, st) != 0
     assert b'64 or 96' in lib.otb_last_error()
     # the log-sum-exp feeds the 64-wide backward: a 96-wide forward that asks for it is refused (valid operands throughout)
     q96, out96 = torch.zeros(8, 3 * 384, dtype=BF, device=DEV), torch.empty(8, 384, dtype=BF, device=DEV)
