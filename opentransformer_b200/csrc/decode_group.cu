@@ -153,9 +153,15 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 __device__ __forceinline__ uint32_t sw128(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
 
 // ---------------------------------------------------------------------------------------------- the kernel
+// kStamps: the clock64 phase stamps of tools/decode_phases.py (otb_debug_decode_timing).  Only that instantiation carries
+// their state (stamp counters, the per-barrier slot pointer), which would otherwise be live across every phase and barrier;
+// the production instantiation (kStamps = false) has none of it.
+template <bool kStamps>
 __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __grid_constant__ DgParams p) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    // 1024-byte alignment by an offset from smem_raw, not by integer arithmetic on its address: the compiler then still knows
+    // every pointer below is a shared-memory address (32-bit registers, LDS / STS instead of generic loads and stores)
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     // Shared memory (227 KB per CTA): sA | stage 0 | stage 1 | sSB | DgMisc.  Which phase of a step uses which region (R reads,
     // W writes; "pf" = filled by a TMA prefetch issued at the group barrier IN FRONT of the phase, "tma" = filled by TMA
     // inside the phase once its previous user is done; sA0 = sSB [16 KB, 20 KB), sA1 = sSB [20 KB, 24 KB)):
@@ -188,13 +194,9 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     const int nutt = min(p.utts_per_group, p.B - u0);
     const int row0 = u0 * beam, nrows = nutt * beam;
     const int nl = p.n_layers;
-    const CUtensorMap* maps = p.maps;
-    auto layer_map = [&](int l, DgLayerMap m) { return maps + l * DG_LAYER_MAPS + m; };
-    const CUtensorMap* map_wout = maps + nl * DG_LAYER_MAPS + MAP_WOUT;
-    const CUtensorMap* map_kvx = maps + nl * DG_LAYER_MAPS + MAP_KVX;
-    const CUtensorMap* map_x = maps + nl * DG_LAYER_MAPS + MAP_X;
-    const CUtensorMap* map_x2 = maps + nl * DG_LAYER_MAPS + MAP_X2;
-    const CUtensorMap* map_lg = maps + nl * DG_LAYER_MAPS + MAP_LG;
+    // tensor-map addresses are formed from the parameters where they are used, not kept in registers across the step
+    auto layer_map = [&](int l, DgLayerMap m) { return p.maps + l * DG_LAYER_MAPS + m; };
+    auto shared_map = [&](DgSharedMap m) { return p.maps + p.n_layers * DG_LAYER_MAPS + m; };
     int* bar = p.bar + g * 32;                        // 128-byte separated counters
     const bool is_tma = (warp == 0 && lane == 0);
     // wgmma tiles: the four warpgroups split a 128-row product into 64-row halves (mh) x column halves (nh); accumulator
@@ -222,17 +224,20 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     }
     __syncthreads();
 
-    // parity of the NEXT completion of every mbarrier, tracked identically by all threads (every thread walks the same phases)
-    uint32_t par_kb = 0, par_a = 0, par_w1 = 0, par_stf = 0, par_pw = 0, par_pq = 0, par_lg = 0, par_kvw = 0, par_kx = 0;   // bit i = barrier i
+    // parity of the NEXT completion of every mbarrier, tracked identically by all threads (every thread walks the same phases):
+    // one register for all of them, bit PB_x + i = barrier i of the set x (nine words used to be live across every phase)
+    constexpr int PB_KB = 0, PB_A = 4, PB_W1 = 8, PB_PW = 12, PB_PQ = 16, PB_STF = 20, PB_KX = 22, PB_KVW = 25, PB_LG = 27;
+    uint32_t par = 0;
+    auto pbit = [&](int set, int i) { return (par >> (set + i)) & 1u; };
     int bar_target = 0;
 
-    const bool dbg_cta = (p.dbg_clk != nullptr && blockIdx.x < DG_P && tid == 0);     // every CTA of group 0: [cta][256] stamps
+    const bool dbg_cta = kStamps && (p.dbg_clk != nullptr && blockIdx.x < DG_P && tid == 0);     // every CTA of group 0: [cta][256] stamps
     int dbg_n = 0;
     bool dbg_on = false;
-#define DG_STAMP() do { if (dbg_on) p.dbg_clk[blockIdx.x * 256 + dbg_n++] = clock64(); } while (0)
+#define DG_STAMP() do { if (kStamps && dbg_on) p.dbg_clk[blockIdx.x * 256 + dbg_n++] = clock64(); } while (0)
     // sub-phase stamps of layer 2 in slots 200.. (tools/decode_phases.py prints them)
-#define DG_STAMP2(k) do { if (dbg_on && l == 2) p.dbg_clk[blockIdx.x * 256 + 200 + (k)] = clock64(); } while (0)
-#define DG_STAMP3(k) do { if (dbg_on) p.dbg_clk[blockIdx.x * 256 + 200 + (k)] = clock64(); } while (0)
+#define DG_STAMP2(k) do { if (kStamps && dbg_on && l == 2) p.dbg_clk[blockIdx.x * 256 + 200 + (k)] = clock64(); } while (0)
+#define DG_STAMP3(k) do { if (kStamps && dbg_on) p.dbg_clk[blockIdx.x * 256 + 200 + (k)] = clock64(); } while (0)
 
     // Group barrier: every CTA of the group has finished the phase (its global writes are visible).  `pre` runs on the TMA
     // thread between arrive and wait -- prefetches that do not depend on the other CTAs (weights, encoder K/V tiles); the
@@ -243,7 +248,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     auto gsync = [&](auto pre) {
         __syncthreads();
         DG_STAMP();
-        const bool rec = dbg_on && dbg_b >= 12 && dbg_b < 18;
+        const bool rec = kStamps && dbg_on && dbg_b >= 12 && dbg_b < 18;
         unsigned long long* slot = p.dbg_clk + blockIdx.x * 256 + 212 + (dbg_b - 12) * 3;
         ++dbg_b;
         if (p.cluster) {
@@ -329,13 +334,13 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         mbar_arrive_expect_tx(&ms.kx_full[s], 65536);
         // the encoder K / V tiles are streamed once per step (49 MB per batch): evict-first, so that they do not push the
         // decoder weights (re-read by every group, every step) out of L2
-        tma_load_2d_hint(dst, map_kvx, &ms.kx_full[s], h * 64, (l * p.B + u) * p.T, TMA_EVICT_FIRST);
-        tma_load_2d_hint(dst + 32768, map_kvx, &ms.kx_full[s], DG_D + h * 64, (l * p.B + u) * p.T, TMA_EVICT_FIRST);
+        tma_load_2d_hint(dst, shared_map(MAP_KVX), &ms.kx_full[s], h * 64, (l * p.B + u) * p.T, TMA_EVICT_FIRST);
+        tma_load_2d_hint(dst + 32768, shared_map(MAP_KVX), &ms.kx_full[s], DG_D + h * 64, (l * p.B + u) * p.T, TMA_EVICT_FIRST);
     };
     const int n_vchunks = (V + 127) / 128;
     auto load_wout = [&](int chunk, int s) {
         mbar_arrive_expect_tx(&ms.st_full[s], 65536);
-        for (int kb = 0; kb < 4; ++kb) tma_load_2d_hint(sST + s * DG_STAGE + kb * 16384, map_wout, &ms.st_full[s], kb * 64, chunk * 128, TMA_EVICT_LAST);
+        for (int kb = 0; kb < 4; ++kb) tma_load_2d_hint(sST + s * DG_STAGE + kb * 16384, shared_map(MAP_WOUT), &ms.st_full[s], kb * 64, chunk * 128, TMA_EVICT_LAST);
     };
     const int n_tasks = nutt * DG_H;   // cross-attention problems of this group; CTA j takes j, j + P, ...
 
@@ -395,7 +400,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         }
     };
     // acc[0..1] = out[era + {0,1}][ef0], acc[2..3] = out[era + {0,1}][ef0 + 8]; warp w owns output features [16 w, 16 w + 16)
-    auto rowgemm = [&](const uint8_t* A, uint64_t* full, uint32_t& par, auto kb_addr, float (&acc)[4]) {   // flips par
+    auto rowgemm = [&](const uint8_t* A, uint64_t* full, int pset, auto kb_addr, float (&acc)[4]) {   // flips the parities of pset
         float acc2[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int i = 0; i < 4; ++i) acc[i] = 0.f;
@@ -403,7 +408,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         const uint32_t abase = smem_u32(A);
 #pragma unroll 1
         for (int kb = 0; kb < 4; ++kb) {
-            mbar_wait(&full[kb], (par >> kb) & 1);
+            mbar_wait(&full[kb], pbit(pset, kb));
             const uint32_t wb = smem_u32(kb_addr(kb));
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks) {
@@ -418,7 +423,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         }
 #pragma unroll
         for (int i = 0; i < 4; ++i) acc[i] += acc2[i];
-        par ^= 0xF;
+        par ^= 0xFu << pset;
     };
     // LayerNorm of the 8 rows held as v[0..3] = (row a, f0) (row b, f0) (row a, f0 + 8) (row b, f0 + 8) (fp32: projection + bias
     // + residual): statistics over the 8 lane groups of a warp (shuffles) and the 16 warps (shared memory)
@@ -479,8 +484,8 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         if (is_tma && a_map != nullptr) load_a(a_map);
         // every operand wait precedes the wgmma chain: wgmma issued behind a divergent spin loop is serialised by ptxas
         for (int kb = 0; kb < 4; ++kb) {
-            mbar_wait(&ms.kb_full[kb], (par_kb >> kb) & 1);
-            if (a_map != nullptr) mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
+            mbar_wait(&ms.kb_full[kb], pbit(PB_KB, kb));
+            if (a_map != nullptr) mbar_wait(&ms.a_full[kb], pbit(PB_A, kb));
         }
         __syncwarp();
         float acc[12];
@@ -501,8 +506,8 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) epi(frow + 8 * hh, nh * 24 + i * 8 + fcq, acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
         }
-        par_kb ^= 0xF;
-        if (a_map != nullptr) par_a ^= 0xF;
+        par ^= 0xFu << PB_KB;
+        if (a_map != nullptr) par ^= 0xFu << PB_A;
         __syncthreads();
     };
     // Buffers that only this kernel reads back (w_2 partial products, logits) are stored as [column group of 4][row][16 bytes]:
@@ -578,8 +583,8 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
             DG_STAMP2(41);
             for (int hh = 0; hh < nh; ++hh) {
                 const int buf = hh & 1, k0 = hh * 8;
-                mbar_wait(&kvb[buf], (par_kvw >> buf) & 1);
-                par_kvw ^= (1u << buf);
+                mbar_wait(&kvb[buf], pbit(PB_KVW, buf));
+                par ^= 1u << (PB_KVW + buf);
                 if (hh < 4) DG_STAMP2(42 + 2 * hh);
                 const uint8_t* kb_ = kvst + buf * 8192 + h * 128 + c8 * 16;
                 uint4 ku[4], vu[4];
@@ -666,7 +671,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         __syncthreads();
         DG_STAMP2(10);
         float acc[4];
-        rowgemm(sA0, ms.pw_full, par_pw, [&](int kb) { return kb < 2 ? sA + kb * 32768 : sST + (kb - 2) * 32768; }, acc);
+        rowgemm(sA0, ms.pw_full, PB_PW, [&](int kb) { return kb < 2 ? sA + kb * 32768 : sST + (kb - 2) * 32768; }, acc);
         __syncthreads();      // every warp is done with W_o: its first half makes room for the second half of W_q
         DG_STAMP2(11);
         if (is_tma)
@@ -686,7 +691,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         *a_at(sA1, era + 1, ef0 + 8) = __float2bfloat16(v[3]);
         __syncthreads();
         DG_STAMP();   // W_o + LN1
-        rowgemm(sA1, ms.pq_full, par_pq, [&](int kb) { return kb < 2 ? sST + DG_STAGE + kb * 32768 : sA + (kb - 2) * 32768; }, acc);
+        rowgemm(sA1, ms.pq_full, PB_PQ, [&](int kb) { return kb < 2 ? sST + DG_STAGE + kb * 32768 : sA + (kb - 2) * 32768; }, acc);
         {
             const float b0 = qb0, b1 = qb1;
             if (live_a) {
@@ -733,7 +738,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                     qa[ks][3] = (gq + 8 < beam) ? *reinterpret_cast<const uint32_t*>(qb + (size_t)(gq + 8) * DG_D + d0 + 8) : 0u;
                 }
             }
-            mbar_wait(&ms.kx_full[st], ((par_kx >> st) & 1) ^ (uint32_t)((i / 3) & 1));
+            mbar_wait(&ms.kx_full[st], pbit(PB_KX, st) ^ (uint32_t)((i / 3) & 1));
             // S = Q K^T for this warp's 64 keys
             float sc[8][4];
 #pragma unroll
@@ -848,7 +853,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
 #pragma unroll
         for (int st = 0; st < 3; ++st) {
             const int uses = (n_mine > st) ? (n_mine - st + 2) / 3 : 0;
-            par_kx ^= (uint32_t)(uses & 1) << st;
+            par ^= (uint32_t)(uses & 1) << (PB_KX + st);
         }
     };
     // ---- rows [8 j, 8 j + 8): cross-attention W_o + bias + residual (x1, still in shared memory) -> LayerNorm 2
@@ -858,7 +863,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         const float pb0 = ly.bo2[ef0], pb1 = ly.bo2[ef0 + 8], pg0 = ly.g2[ef0], pg1 = ly.g2[ef0 + 8], pt0 = ly.be2[ef0], pt1 = ly.be2[ef0 + 8];
         __syncthreads();
         float acc[4];
-        rowgemm(sA0, ms.pw_full, par_pw, [&](int kb) { return kb < 2 ? sA + kb * 32768 : sST + (kb - 2) * 32768; }, acc);
+        rowgemm(sA0, ms.pw_full, PB_PW, [&](int kb) { return kb < 2 ? sA + kb * 32768 : sST + (kb - 2) * 32768; }, acc);
         __syncthreads();      // stage 0 (second half of W_o) is free: first half of W1
         if (is_tma) load_w1(l, 0);
         float v[4];
@@ -881,13 +886,13 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     };
     // ---- GLU feed-forward: hidden features [128 j, 128 j + 128) (ffn.py:18,39-41); A = x2 of all rows by TMA
     auto glu_w2 = [&](int l, const DgLayer& ly) {
-        if (is_tma) load_a(map_x2);
+        if (is_tma) load_a(shared_map(MAP_X2));
         if (tid < 256) ms.bias[tid] = ly.b1[(tid < 128 ? 0 : DG_DFF - 128) + j * 128 + tid];
         // W1: value and gate features [64 nh, 64 nh + 64) of this CTA's 128, rows [64 mh, +64), two wgmma 64 x 64 chains
         float av[32], ag[32];
         for (int kb = 0; kb < 4; ++kb) {
-            mbar_wait(&ms.w1_full[kb], (par_w1 >> kb) & 1);
-            mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
+            mbar_wait(&ms.w1_full[kb], pbit(PB_W1, kb));
+            mbar_wait(&ms.a_full[kb], pbit(PB_A, kb));
         }
         __syncwarp();
         wgmma_fence();
@@ -925,13 +930,12 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
             }
         }
         fence_proxy_async_smem();
-        par_w1 ^= 0xF;
-        par_a ^= 0xF;
+        par ^= (0xFu << PB_W1) | (0xFu << PB_A);
         __syncthreads();
         DG_STAMP();   // W1 + GLU
         // w_2 partial: acc2[128 x 256] = h[128 x 128] * W2[:, slice]^T; warpgroup (mh, nh): rows [64 mh, +64) x columns [128 nh, +128)
         {
-            mbar_wait(&ms.st_full[0], par_stf & 1);
+            mbar_wait(&ms.st_full[0], pbit(PB_STF, 0));
             // fp32 partial products in the [column group of 4][row] order the reduction reads; two 64-column passes
             // keep the accumulator within the register budget of 512 threads
             float* dst = reinterpret_cast<float*>(p.part) + ((size_t)j * p.G + g) * part_slab * 4;
@@ -961,7 +965,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                 }
             }
         }
-        par_stf ^= 1;
+        par ^= 1u << PB_STF;
     };
     // ---- sum of the 16 partial products + bias + residual (x2) + LayerNorm 3, rows [8 j, 8 j + 8) of the
     // tile: every load is a contiguous 512-byte half row, the row statistics stay inside the CTA, and the result is the
@@ -1023,9 +1027,9 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     auto logits = [&] {
         int my_chunks = 0;
         for (int c = j; c < n_vchunks; c += DG_P) ++my_chunks;
-        if (is_tma) load_a(map_x);
+        if (is_tma) load_a(shared_map(MAP_X));
         __syncwarp();
-        for (int kb = 0; kb < 4; ++kb) mbar_wait(&ms.a_full[kb], (par_a >> kb) & 1);
+        for (int kb = 0; kb < 4; ++kb) mbar_wait(&ms.a_full[kb], pbit(PB_A, kb));
         // chunk i: wgmma 64 x 64 per warpgroup (rows [64 mh, +64), columns [64 nh, +64) of the chunk), logits + bias stored in the
         // [column group][row] order (columns [V, ldv) as -inf: no bounds checks in the readers); the weights of chunk i + 2
         // stream into the stage as soon as every warpgroup has multiplied chunk i
@@ -1033,7 +1037,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
             const int s = i & 1;
             const int col0 = (j + i * DG_P) * 128;
             if (tid < 128) ms.bias[s * 128 + tid] = (p.bout != nullptr && col0 + tid < V) ? p.bout[col0 + tid] : 0.f;
-            mbar_wait(&ms.st_full[s], ((par_stf >> s) & 1) ^ (uint32_t)((i >> 1) & 1));
+            mbar_wait(&ms.st_full[s], pbit(PB_STF, s) ^ (uint32_t)((i >> 1) & 1));
             float lc[32];
             __syncwarp();
             wgmma_fence();
@@ -1064,8 +1068,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         }
         // parity bookkeeping: barrier pair s was used ceil((my_chunks - s) / 2) times
         const uint32_t u0n = (uint32_t)((my_chunks + 1) >> 1), u1n = (uint32_t)(my_chunks >> 1);
-        par_a ^= 0xF;
-        par_stf ^= (u0n & 1) | ((u1n & 1) << 1);
+        par ^= (0xFu << PB_A) | (((u0n & 1) | ((u1n & 1) << 1)) << PB_STF);
     };
     // ---- per utterance: log-softmax + top-`beam` of every hypothesis row (decoder/transformer.py:206,
     // speech2text.py:112), finished masking, beam^2 pruning, ancestry (speech2text.py:102-153); ties -> lower index
@@ -1094,10 +1097,10 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                 if (is_tma) {
                     mbar_arrive_expect_tx(&ms.lg_full, (uint32_t)(nbox * 64 * bpad * 16));
                     for (int bx = 0; bx < nbox; ++bx)
-                        tma_load_2d(smem + (size_t)bx * 64 * bpad * 16, map_lg, &ms.lg_full, lr0 * 4, g * ldv4 + bx * 64);
+                        tma_load_2d(smem + (size_t)bx * 64 * bpad * 16, shared_map(MAP_LG), &ms.lg_full, lr0 * 4, g * ldv4 + bx * 64);
                 }
-                mbar_wait(&ms.lg_full, par_lg);
-                par_lg ^= 1;
+                mbar_wait(&ms.lg_full, pbit(PB_LG, 0));
+                par ^= 1u << PB_LG;
             }
             if (ul == j) DG_STAMP();      // rows gathered
             if (warp < beam) {
@@ -1327,7 +1330,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
         for (int l = 0; l < nl; ++l) {
             const DgLayer& ly = p.layers[l];
             // QKV projection of the newest token (attention.py:68-73): 48 of the 768 columns per CTA; q -> qbuf, k / v -> cache
-            gemm_small(l == 0 ? nullptr : map_x, ly.bqkv, j * 48, [&](int r, int c, float v0, float v1) {
+            gemm_small(l == 0 ? nullptr : shared_map(MAP_X), ly.bqkv, j * 48, [&](int r, int c, float v0, float v1) {
                 if (r >= nrows) return;
                 const int col = j * 48 + c;               // column pairs never straddle the q | k | v boundaries
                 const uint32_t o = pack_bf16(v0 + ms.bias[c], v1 + ms.bias[c + 1]);
@@ -1394,7 +1397,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
     }
     // drain the QKV-weight prefetch that was issued for a step that will not run
     if (is_tma)
-        for (int kb = 0; kb < 4; ++kb) mbar_wait(&ms.kb_full[kb], (par_kb >> kb) & 1);
+        for (int kb = 0; kb < 4; ++kb) mbar_wait(&ms.kb_full[kb], pbit(PB_KB, kb));
     fill_history(steps_done, group_done);
 #undef DG_STAMP
 #undef DG_STAMP2
@@ -1491,8 +1494,9 @@ const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const 
     // streams together) is resident at once, e.g. 2 batches of 32 utterances (96 CTAs) on a 132-SM H100.
     static const bool cluster_ok = [] {
         // the question is about a DG_SMEM launch, so the kernel's shared-memory cap has to be raised before it is asked
-        if (prepare<decode_group_kernel>() ||
-            cudaFuncSetAttribute(decode_group_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
+        if (prepare<decode_group_kernel<false>>() || prepare<decode_group_kernel<true>>() ||
+            cudaFuncSetAttribute(decode_group_kernel<false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
+            cudaFuncSetAttribute(decode_group_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) {
             (void)cudaGetLastError();
             return false;
         }
@@ -1505,7 +1509,7 @@ const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const 
         q.gridDim = dim3(DG_P); q.blockDim = dim3(DG_THREADS); q.dynamicSmemBytes = DG_SMEM;
         q.attrs = at; q.numAttrs = 1;
         int nclus = 0;
-        if (cudaOccupancyMaxActiveClusters(&nclus, decode_group_kernel, &q) != cudaSuccess || nclus < 1) {
+        if (cudaOccupancyMaxActiveClusters(&nclus, decode_group_kernel<false>, &q) != cudaSuccess || nclus < 1) {
             (void)cudaGetLastError();
             return false;
         }
@@ -1515,8 +1519,11 @@ const char* decode_group_launch(cudaStream_t st, const otb_mega_model& m, const 
     // flight than can be resident at once, which only gang-scheduled clusters tolerate
     if (g_dg_barrier == 1 && !cluster_ok) return "decode_persistent: thread-block clusters of 16 are not available on this device";
     p.cluster = (cluster_ok && g_dg_barrier != 0) ? 1 : 0;
-    return p.cluster ? launch<decode_group_kernel, DG_P>(G * DG_P, DG_THREADS, DG_SMEM, st, p)
-                     : launch<decode_group_kernel>(G * DG_P, DG_THREADS, DG_SMEM, st, p);
+    if (p.dbg_clk != nullptr)      // otb_debug_decode_timing: the stamped instantiation
+        return p.cluster ? launch<decode_group_kernel<true>, DG_P>(G * DG_P, DG_THREADS, DG_SMEM, st, p)
+                         : launch<decode_group_kernel<true>>(G * DG_P, DG_THREADS, DG_SMEM, st, p);
+    return p.cluster ? launch<decode_group_kernel<false>, DG_P>(G * DG_P, DG_THREADS, DG_SMEM, st, p)
+                     : launch<decode_group_kernel<false>>(G * DG_P, DG_THREADS, DG_SMEM, st, p);
 }
 
 }  // namespace otb

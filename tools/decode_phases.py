@@ -1,4 +1,8 @@
-"""Per-stage clock64 breakdown of one decode step of the persistent kernel (debug aid, GPU only)."""
+"""Per-stage clock64 breakdown of one decode step of the persistent kernel (debug aid, GPU only).
+
+The stamps come from the stamped instantiation, decode_group_kernel<true>, which otb_debug_decode_timing selects; the
+production kernel (decode_group_kernel<false>) carries no stamp state.  Both run the same phases, but their registers are
+allocated separately, so a phase's cycles here can differ slightly from the production kernel's."""
 import sys, os, ctypes
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
