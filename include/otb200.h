@@ -369,14 +369,20 @@ int otb_lstm_bwd(const void* dy, const void* w_hh, const float* gates, const flo
 int otb_embedding(const int64_t* tok, const void* emb, void* out, int N, int d, int vocab, void* stream);
 
 /* Log-mel filterbank features on the device (data/audio.py:117-120: ta.compliance.kaldi.fbank with Kaldi defaults, dither 0):
- * wave f32 [B, ld_wave] (zero padded), n_samples i32 [B]; window f32 [frame_len] (povey); bank f32 [F, 256] triangular mel
- * weights over the first 256 bins of the 512-point spectrum and bank_range i32 [F, 2] their non-zero [lo, hi) ranges (built
- * by opentransformer_b200/features.py); out f32 [B, Tmax, F], frames >= 1 + (n - frame_len) / frame_shift are zero. */
-int otb_fbank(const float* wave, int ld_wave, const int32_t* n_samples, int B, const float* window, const float* bank,
-              const int32_t* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift, float preemph, void* stream);
+ * wave f32 [B, ld_wave] (zero padded), n_samples i32 [B]; gain f32 [B] or NULL scales each waveform where its samples are
+ * loaded, before DC removal (volume_perturb, audio.py:112-114); window f32 [frame_len] (povey), 2 <= frame_len <= 2048; the
+ * FFT has n_fft = round_to_power_of_two(frame_len) points; bank f32 [F, n_fft/2] triangular mel weights over the first
+ * n_fft/2 bins of the spectrum and bank_range i32 [F, 2] their non-zero [lo, hi) ranges (built by
+ * opentransformer_b200/features.py); out f32 [B, Tmax, F], frames >= 1 + (n - frame_len) / frame_shift are zero. */
+int otb_fbank(const float* wave, int ld_wave, const int32_t* n_samples, const float* gain, int B, const float* window,
+              const float* bank, const int32_t* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift, float preemph,
+              void* stream);
 /* `normalization` (data/audio.py:22-24): (x - mean) / std over all valid elements of each utterance (unbiased std), in place;
- * or, with gmean / gstd f32 [F], the global CMVN of audio.py:131-132.  x f32 [B, Tmax, F], n_frames i32 [B]. */
-int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, const float* gmean, const float* gstd, void* stream);
+ * or, with gmean / gstd f32 [F], the global CMVN of audio.py:131-132.  x f32 [B, Tmax, F], n_frames i32 [B].  noise f32
+ * [B, F] or NULL (gaussian_noise, audio.py:131-133) is added to every valid frame of utterance b in the same store; padded
+ * frames stay zero.  gmean 0 / gstd 1 leave x as it is and only add the noise. */
+int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, const float* gmean, const float* gstd, const float* noise,
+                 void* stream);
 
 /* Joint-CTC loss of SpeechToText.forward (model/speech2text.py:60-72 -> CTCAssistor.compute_loss, model/ctc.py:48-52):
  * nn.CTCLoss(blank, reduction 'mean', zero_infinity = True) and its gradient with respect to the LOGITS.

@@ -91,8 +91,8 @@ _SIGS = {
                                     c_float, c_float, _P, _P, c_float, _P, _P, _P]),
     'otb_mixspeech': (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_float, _P, _P, _P, _P]),
     'otb_frame_stack': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_float, _P, _P]),
-    'otb_fbank': (c_int, [_P, c_int, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
-    'otb_utt_cmvn': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P]),
+    'otb_fbank': (c_int, [_P, c_int, _P, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
+    'otb_utt_cmvn': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     'otb_ctc_loss': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_int, c_float, _P,
                              _P]),
     'otb_ctc_frame_topk': (c_int, [_P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P]),

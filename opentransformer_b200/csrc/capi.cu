@@ -504,15 +504,18 @@ int otb_frame_stack(const float* x, int B, int T, int F, int n, int s, int T2, v
     RET("otb_frame_stack", frame_stack_launch(ST(stream), x, B, T, F, n, s, T2, reinterpret_cast<bf16*>(out), ldo, alpha, table));
 }
 
-int otb_fbank(const float* wave, int ld_wave, const int32_t* n_samples, int B, const float* window, const float* bank,
-              const int32_t* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift, float preemph, void* stream) {
+int otb_fbank(const float* wave, int ld_wave, const int32_t* n_samples, const float* gain, int B, const float* window,
+              const float* bank, const int32_t* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift, float preemph,
+              void* stream) {
     if (!wave || !n_samples || !window || !bank || !bank_range || !out) return fail("otb_fbank", "null operand");
-    RET("otb_fbank", fbank_launch(ST(stream), wave, ld_wave, n_samples, B, window, bank, bank_range, out, Tmax, F, frame_len, frame_shift, preemph));
+    RET("otb_fbank", fbank_launch(ST(stream), wave, ld_wave, n_samples, gain, B, window, bank, bank_range, out, Tmax, F, frame_len,
+                                  frame_shift, preemph));
 }
 
-int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, const float* gmean, const float* gstd, void* stream) {
+int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, const float* gmean, const float* gstd, const float* noise,
+                 void* stream) {
     if (!x || !n_frames) return fail("otb_utt_cmvn", "null operand");
-    RET("otb_utt_cmvn", utt_cmvn_launch(ST(stream), x, B, Tmax, F, n_frames, gmean, gstd));
+    RET("otb_utt_cmvn", utt_cmvn_launch(ST(stream), x, B, Tmax, F, n_frames, gmean, gstd, noise));
 }
 
 int otb_ctc_loss(const float* logp, int ldl, int B, int T, int V, const int32_t* in_len, const int64_t* targets, int ldt,

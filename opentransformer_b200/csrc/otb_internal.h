@@ -293,10 +293,11 @@ const char* mwer_coeff_launch(cudaStream_t stream, const int* len, const int* er
 const char* mwer_grad_launch(cudaStream_t stream, const float* logits, int ld, int rows, int V, const int* target, const float* tok_lp,
                              const float* coeff, int Lp, bf16* dlogits);
 
-const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const int* n_samples, int B, const float* window,
-                         const float* bank, const int* bank_range, float* out, int Tmax, int F, int frame_len, int frame_shift,
-                         float preemph);
-const char* utt_cmvn_launch(cudaStream_t st, float* x, int B, int Tmax, int F, const int* n_frames, const float* gmean, const float* gstd);
+const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const int* n_samples, const float* gain, int B,
+                         const float* window, const float* bank, const int* bank_range, float* out, int Tmax, int F, int frame_len,
+                         int frame_shift, float preemph);
+const char* utt_cmvn_launch(cudaStream_t st, float* x, int B, int Tmax, int F, const int* n_frames, const float* gmean, const float* gstd,
+                            const float* noise);
 
 // LSTM recurrence (lstm.cu): units per CTA, grid and dynamic shared memory of the two persistent kernels for hidden size H
 struct LstmPlan {

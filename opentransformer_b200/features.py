@@ -1,21 +1,28 @@
 """Log-mel filterbank features + CMVN on the GPU (SURVEY.md 8f row 3): the step immediately before the hot path.
 
-Mirror of what otrans/data/audio.py:117-133 does on DataLoader worker CPUs per utterance,
+Mirror of what otrans/data/audio.py:112-136 does on DataLoader worker CPUs per utterance,
 
+    wavform *= 10 ** (random.uniform(-1.6, 1.6) / 20)                      # volume_perturb (training only)
     feature = ta.compliance.kaldi.fbank(wavform, num_mel_bins=..., sample_frequency=..., dither=0.0)
     feature = normalization(feature)            # (x - mean) / std over the whole utterance, or global CMVN
-    feature = spec_augment(feature)             # opentransformer_b200/augment.py
+    feature += torch.normal(torch.zeros(F), std=gaussian_noise)           # one vector per utterance (training only)
+    feature = spec_augment(feature)             # opentransformer_b200/augment.py (training only)
 
 batched on the device (csrc/fbank.cu): at thousands of utterances per second per GPU the CPU front end is the next wall.
 The mel filterbank follows Kaldi's definition as published by torchaudio.compliance.kaldi.get_mel_banks (mel(f) = 1127
 ln(1 + f / 700), num_bins + 2 equally spaced mel points between low_freq and Nyquist, triangles over the first N/2 FFT bins).
+The FFT has round_to_power_of_two(frame_len) points, at most 2048 (25 ms frames at sample rates up to 81.9 kHz).  One
+extractor serves one sample rate.
 """
 import math
 
+import numpy as np
 import torch
 
-from . import _lib, ops
+from . import _lib, augment, ops
 from ._lib import check
+
+MAX_FFT = 2048          # csrc/fbank.cu: shared-memory buffers of one frame
 
 
 def _mel(f):
@@ -48,18 +55,27 @@ def povey_window(n):
 
 
 class FbankExtractor:
-    """Batched fbank (+ CMVN) on the device.  ``__call__(waves)`` takes a list of 1-D float waveforms (as ta.load returns
-    them, any length) or a padded f32 [B, N] tensor with ``lengths`` and returns what collate_fn_with_eos_bos builds
-    (data/loader.py:66-108): features f32 [B, Tmax, F] zero padded, feature lengths, bool mask [B, Tmax]."""
+    """Batched fbank (+ CMVN, + the reference's training augmentations) on the device.  ``__call__(waves)`` takes a list of
+    1-D float waveforms (as ta.load returns them, any length) or a padded f32 [B, N] tensor with ``lengths`` and returns
+    what collate_fn_with_eos_bos builds (data/loader.py:66-108): features f32 [B, Tmax, F] zero padded, feature lengths,
+    bool mask [B, Tmax].
+
+    ``volume_perturb`` scales each waveform by 10 ** (U(-1.6, 1.6) / 20) before the fbank, ``gaussian_noise`` = sigma adds one
+    N(0, sigma) vector of F values per utterance to its valid frames after CMVN, and ``spec_augment`` masks bands last with
+    ``augment.spec_augment_`` (``spec_augment_config`` are its keyword arguments).  The gains and the noise are drawn on the
+    device from ``generator`` (a CUDA torch.Generator; torch's default one if None); SpecAugment draws its bands on the host
+    with the reference's RNG calls.  All three are off by default."""
 
     def __init__(self, num_mel_bins=80, sample_rate=16000, frame_length_ms=25.0, frame_shift_ms=10.0, preemphasis=0.97,
-                 normalization=True, global_mean=None, global_std=None, device=None):
+                 normalization=True, global_mean=None, global_std=None, device=None, volume_perturb=False, gaussian_noise=0.0,
+                 spec_augment=False, spec_augment_config=None, generator=None):
         self.F, self.sr = num_mel_bins, sample_rate
         self.frame_len = int(sample_rate * frame_length_ms * 0.001)
         self.frame_shift = int(sample_rate * frame_shift_ms * 0.001)
+        if not 2 <= self.frame_len <= MAX_FFT:
+            raise NotImplementedError(f'fbank kernel takes frames of 2 .. {MAX_FFT} samples (a FFT of at most {MAX_FFT} points); '
+                                      f'{frame_length_ms} ms at {sample_rate} Hz is {self.frame_len}')
         n_fft = 1 << (self.frame_len - 1).bit_length()               # round_to_power_of_two
-        if n_fft != 512:
-            raise NotImplementedError('fbank kernel is built for a 512-point FFT (25 ms frames at 16 kHz)')
         self.device = torch.device(device if device is not None else torch.cuda.current_device())
         bank, rng = mel_banks(num_mel_bins, n_fft, sample_rate)
         self.bank, self.range = bank.to(self.device), rng.to(self.device)
@@ -68,11 +84,45 @@ class FbankExtractor:
         self.normalization = normalization
         self.gmean = global_mean.float().to(self.device).contiguous() if global_mean is not None else None
         self.gstd = global_std.float().to(self.device).contiguous() if global_std is not None else None
+        # with normalization off the CMVN pass only adds the noise: global statistics 0 / 1 store x itself
+        self.unit_stats = None if normalization else (torch.zeros(num_mel_bins, device=self.device),
+                                                      torch.ones(num_mel_bins, device=self.device))
+        self.volume_perturb = bool(volume_perturb)
+        self.gaussian_noise = float(gaussian_noise)
+        self.spec_augment = bool(spec_augment)
+        self.spec_augment_config = dict(spec_augment_config or {})
+        self.generator = generator
+
+    @classmethod
+    def from_config(cls, data_params, sample_rate=16000, is_eval=False, device=None):
+        """The extractor AudioDataset(data_params, ..., is_eval) stands for (otrans/data/audio.py:31-73): num_mel_bins,
+        normalization with the optional global_cmvn prefix (<prefix>.mean.npy / .std.npy), and in training spec_augment
+        (+ spec_augment_config), volume_perturb and gaussian_noise.  speed_perturb is accepted and ignored, as the reference
+        has it commented out.  The reference calls spec_augment(feature) with its defaults; the shipped configs set the same
+        values, and here spec_augment_config is passed on."""
+        p = data_params
+        kind = p.get('feature_extractor', 'torchaudio')
+        if kind in ('psf', 'python_speech_feature'):
+            raise NotImplementedError('feature_extractor psf (python_speech_features.logfbank) is not built; use torchaudio')
+        if kind not in ('torchaudio', 'ta'):
+            raise ValueError(f'unknown feature_extractor {kind!r}')
+        gmean = gstd = None
+        if p['normalization'] and 'global_cmvn' in p:
+            gmean = torch.from_numpy(np.load(p['global_cmvn'] + '.mean.npy'))
+            gstd = torch.from_numpy(np.load(p['global_cmvn'] + '.std.npy'))
+        train = not is_eval
+        return cls(num_mel_bins=p['num_mel_bins'], sample_rate=sample_rate, normalization=p['normalization'], global_mean=gmean,
+                   global_std=gstd, device=device, volume_perturb=train and bool(p.get('volume_perturb', False)),
+                   gaussian_noise=float(p.get('gaussian_noise', 0.0)) if train else 0.0,
+                   spec_augment=train and bool(p.get('spec_augment', False)),
+                   spec_augment_config=p.get('spec_augment_config') if train else None)
 
     def n_frames(self, n_samples):
         return 0 if n_samples < self.frame_len else 1 + (n_samples - self.frame_len) // self.frame_shift
 
-    def __call__(self, waves, lengths=None):
+    def __call__(self, waves, lengths=None, gains=None, noise=None):
+        """``gains`` f32 [B] (linear factors) and ``noise`` f32 [B, F] replace what volume_perturb / gaussian_noise would
+        draw, for checking exact values; either applies whether or not its option is on."""
         if isinstance(waves, (list, tuple)):
             lens = [int(w.numel()) for w in waves]
             N = max(lens)
@@ -83,17 +133,35 @@ class FbankExtractor:
         waves = waves.to(self.device, torch.float32).contiguous()
         lengths = lengths.to(self.device, torch.int32).contiguous()
         B, N = waves.shape
+        if gains is None and self.volume_perturb:
+            db = torch.empty(B, dtype=torch.float32, device=self.device).uniform_(-1.6, 1.6, generator=self.generator)
+            gains = torch.pow(10.0, db / 20.0)
+        if noise is None and self.gaussian_noise > 0.0:
+            noise = torch.empty(B, self.F, dtype=torch.float32, device=self.device).normal_(0.0, self.gaussian_noise,
+                                                                                             generator=self.generator)
+        if gains is not None:
+            gains = torch.as_tensor(gains, dtype=torch.float32).to(self.device).contiguous()
+            if gains.shape != (B,):
+                raise ValueError(f'gains must be [B] = [{B}], got {tuple(gains.shape)}')
+        if noise is not None:
+            noise = torch.as_tensor(noise, dtype=torch.float32).to(self.device).contiguous()
+            if noise.shape != (B, self.F):
+                raise ValueError(f'noise must be [B, F] = [{B}, {self.F}], got {tuple(noise.shape)}')
         frames = torch.tensor([self.n_frames(int(n)) for n in lengths.cpu().tolist()], dtype=torch.int32)
         Tmax = max(1, int(frames.max()))
         out = torch.empty(B, Tmax, self.F, dtype=torch.float32, device=self.device)
         st = ops._stream()
-        check(_lib.lib().otb_fbank(ops._p(waves), N, ops._p(lengths), B, ops._p(self.window), ops._p(self.bank), ops._p(self.range),
-                                   ops._p(out), Tmax, self.F, self.frame_len, self.frame_shift, self.preemph, st), 'otb_fbank')
+        check(_lib.lib().otb_fbank(ops._p(waves), N, ops._p(lengths), ops._p(gains), B, ops._p(self.window), ops._p(self.bank),
+                                   ops._p(self.range), ops._p(out), Tmax, self.F, self.frame_len, self.frame_shift, self.preemph, st),
+              'otb_fbank')
         ops._count()
         frames_d = frames.to(self.device)
-        if self.normalization:
-            check(_lib.lib().otb_utt_cmvn(ops._p(out), B, Tmax, self.F, ops._p(frames_d), ops._p(self.gmean), ops._p(self.gstd), st),
-                  'otb_utt_cmvn')
+        if self.normalization or noise is not None:
+            gmean, gstd = (self.gmean, self.gstd) if self.normalization else self.unit_stats
+            check(_lib.lib().otb_utt_cmvn(ops._p(out), B, Tmax, self.F, ops._p(frames_d), ops._p(gmean), ops._p(gstd),
+                                          ops._p(noise), st), 'otb_utt_cmvn')
             ops._count()
+        if self.spec_augment:
+            augment.spec_augment_(out, frames.tolist(), **self.spec_augment_config)
         mask = torch.arange(Tmax, device=self.device)[None] < frames_d[:, None]
         return out, frames_d, mask
