@@ -178,9 +178,10 @@ int otb_decode_self_attn(const void* qkv, void* kc, void* vc, const int* anc, co
                          int N, int H, int Lmax, int d_k, void* stream);
 
 /* LabelSmoothingLoss.forward (module/loss.py:21-48) fused: per-token KL(smoothed one-hot || softmax), PAD rows 0,
- * mean over non-PAD tokens.  logits f32 [rows, ldl]; targets i64 [rows]; tok_loss f32 [rows]; loss f32 [1];
- * n_valid i32 [1]; dlogits (optional) receives d(mean loss)/dlogits: f32 [rows, ldd] with dlogits_bf16 = 0, or bf16
- * [rows, ldd] with dlogits_bf16 != 0 for the backward GEMMs (ldd >= V and a multiple of 8, columns [V, ldd) zeroed). */
+ * mean over in-range non-PAD tokens (a target outside [0, V) counts as PAD: loss 0, gradient 0, not in n_valid).
+ * logits f32 [rows, ldl]; targets i64 [rows]; tok_loss f32 [rows]; loss f32 [1]; n_valid i32 [1]; dlogits (optional)
+ * receives d(mean loss)/dlogits: f32 [rows, ldd] with dlogits_bf16 = 0, or bf16 [rows, ldd] with dlogits_bf16 != 0 for
+ * the backward GEMMs (ldd >= V and a multiple of 8, columns [V, ldd) zeroed). */
 int otb_ls_ce(const float* logits, int ldl, const int64_t* targets, int rows, int V, float smoothing, int pad_id,
               float* tok_loss, float* loss, int32_t* n_valid, void* dlogits, int ldd, int dlogits_bf16, void* stream);
 
@@ -207,7 +208,8 @@ int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int l
                   const int32_t* topk_idx, const otb_beam_state* st, int64_t* dbg_ktok, int32_t* dbg_offs, void* stream);
 /* Fused log_softmax (+ lm_weight * lm_logp) + per-row top-k (decoder/transformer.py:206 + speech2text.py:102-112):
  * logits f32 [rows, ldl] -> out_val f32 [rows,k] (log-prob values, descending), out_idx i32 [rows,k];
- * out_logp (optional, f32 [rows, ld_logp]) additionally receives the full log-prob rows. */
+ * out_logp (optional, f32 [rows, ld_logp]) additionally receives the full log-prob rows.  1 <= k <= min(16, V), V <= 49152;
+ * ties go to the lower vocabulary id. */
 int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, int k,
                         int rows, float* out_val, int32_t* out_idx, float* out_logp, int ld_logp, void* stream);
 /* Materialise preds i64 [N, ld] (column 0 = BOS) after `steps` steps from the back-pointers. */

@@ -322,6 +322,8 @@ const char* logsoftmax_topk_launch(cudaStream_t stream, const float* logits, int
                                    float* out_logp, int ld_logp) {
     if (k < 1 || k > KMAX) return "logsoftmax_topk: k must be in [1,16]";
     if (V < 1 || V > 48 * 1024) return "logsoftmax_topk: vocabulary too large for one CTA's shared memory";
+    // past V the scan has nothing left to pick and would return its sentinel (-inf, id 0x7fffffff) as a token
+    if (k > V) return "logsoftmax_topk: k must not exceed the vocabulary size V";
     const size_t smem = (size_t)V * sizeof(float);
     return launch<logsoftmax_topk_kernel>(dim3(rows), dim3(TOPK_THREADS), smem, stream, logits, ldl, V, lm_logp, ld_lm,
                                           lm_weight, k, out_val, out_idx, out_logp, ld_logp);

@@ -4,7 +4,8 @@
 //   loss_tok = sum_v conf_v (log conf_v - logp_v),  conf_v = eps/(V-1) (v != t), 1-eps (v == t)
 //            = C - eps/(V-1) * (sum_v x_v - V*lse) - (1 - eps - eps/(V-1)) * (x_t - lse)
 // from the row maximum, the log-sum-exp and the plain sum of the logits; PAD(0) targets give 0
-// (loss.py:31,46) and the mean is taken over the non-PAD tokens (:44-46).
+// (loss.py:31,46) and the mean is taken over the non-PAD tokens (:44-46).  A target outside [0, V) is scored like PAD
+// and not counted either.
 #include <math.h>
 
 #include "launch.cuh"
@@ -76,11 +77,16 @@ __global__ void __launch_bounds__(256) ls_ce_kernel(const float* __restrict__ lo
     }
 }
 
-// n_valid = #(target != PAD); loss = sum(tok_loss) / n_valid   (single CTA, deterministic order)
-__global__ void __launch_bounds__(256) ls_count_kernel(const long long* __restrict__ tgt, int rows, int pad_id, int* n_valid) {
+// n_valid = #(target != PAD and in [0, V)): exactly the rows ls_ce_kernel scores; loss = sum(tok_loss) / n_valid
+// (single CTA, deterministic order)
+__global__ void __launch_bounds__(256) ls_count_kernel(const long long* __restrict__ tgt, int rows, int V, int pad_id,
+                                                       int* n_valid) {
     __shared__ float red[8];
     float c = 0.f;
-    for (int i = threadIdx.x; i < rows; i += blockDim.x) c += (tgt[i] != pad_id) ? 1.f : 0.f;
+    for (int i = threadIdx.x; i < rows; i += blockDim.x) {
+        const long long t = tgt[i];
+        c += (t != pad_id && t >= 0 && t < V) ? 1.f : 0.f;
+    }
     c = block_reduce(c, red, false);
     if (threadIdx.x == 0) *n_valid = (int)(c + 0.5f);
 }
@@ -97,7 +103,7 @@ const char* ls_ce_launch(cudaStream_t st, const float* logits, int ldl, const lo
                          int pad_id, float* tok_loss, float* loss, int* n_valid, float* dlogits, int ldd, bf16* dlogits_bf16) {
     if (rows < 1 || V < 2) return "ls_ce: empty problem";
     const char* err;
-    if ((err = launch<ls_count_kernel>(1, 256, 0, st, tgt, rows, pad_id, n_valid))) return err;
+    if ((err = launch<ls_count_kernel>(1, 256, 0, st, tgt, rows, V, pad_id, n_valid))) return err;
     if ((err = launch<ls_ce_kernel>(rows, 256, 0, st, logits, ldl, tgt, V, eps, pad_id, tok_loss, dlogits_bf16 ? nullptr : dlogits,
                                     ldd, n_valid, dlogits_bf16)))
         return err;
