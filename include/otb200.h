@@ -212,6 +212,13 @@ int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int l
  * ties go to the lower vocabulary id. */
 int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, int k,
                         int rows, float* out_val, int32_t* out_idx, float* out_logp, int ld_logp, void* stream);
+/* One step of ancestral sampling from logits f32 [N, ldl] (DESIGN.md 4.11) on the beam state, rows never reordered: every
+ * live row n draws token = argmax_{v < V} (logits[n, v] - log(-log u)), ties to the lower id, with
+ * u = rng_u01(rng_key(rng_key(rng_key(seed, step), n), v)) (csrc/counter_rng.cuh), step = st->ctrl[0] and seed the int32
+ * device scalar *seed; the token is distributed as softmax(logits[n, :V]).  The row adds logits[n, token] -
+ * logsumexp(logits[n, :V]) to its score; <S/E> ends it, and an ended row emits <S/E> and keeps its score.  tok_hist,
+ * par_hist (= n), anc, last_tok, flag and ctrl move as otb_beam_step moves them.  1 <= V <= 49152, N >= 1. */
+int otb_sample_step(const float* logits, int ldl, int V, const otb_beam_state* st, const int32_t* seed, void* stream);
 /* Materialise preds i64 [N, ld] (column 0 = BOS) after `steps` steps from the back-pointers. */
 int otb_beam_reconstruct(const otb_beam_state* st, int64_t* preds, int ld, int steps, void* stream);
 /* Tail of recognize() (recognize/speech2text.py:70-91). out_preds i64 [B,nbest,Lmax], out_scores f32 [B,nbest]. */
@@ -511,6 +518,11 @@ int otb_edit_distance(const int32_t* hyp, int ldh, const int32_t* hyp_len, const
  * P_k (W_k - sum_j P_j W_j) * scale (* *scale_dev when scale_dev is not NULL); coeff is 0 for a dropped hypothesis. */
 int otb_mwer_coeff(const int32_t* len, const int32_t* err, const float* tok_lp, int Lp, const int32_t* tgt, int B, int K, float scale,
                    const float* scale_dev, float* coeff, float* loss, void* stream);
+/* The sampled estimator of the same gradient: one warp per utterance over its K <= 32 samples, drawn with replacement (no
+ * duplicate rule, no softmax).  err i32 [B*K] the edit distances W; loss f32 [B] = W^_b = mean_k W_k and coeff f32 [B*K] =
+ * (W_k - W^_b) / K * scale (* *scale_dev when scale_dev is not NULL), exactly 0 when all W of an utterance are equal. */
+int otb_mwer_sample_coeff(const int32_t* err, int B, int K, float scale, const float* scale_dev, float* coeff, float* loss,
+                          void* stream);
 /* dlogits bf16 [rows, ld] = coeff[r / Lp] * (onehot(target[r]) - softmax(logits[r, :V])) of logits f32 [rows, ld], with
  * tok_lp f32 [rows] = otb_token_logprob of the same logits and targets (its log-sum-exp is reused); columns >= V, rows with
  * target < 0 or >= V and rows with coeff 0 are zero.  ld % 4 == 0 and 16-byte aligned logits. */

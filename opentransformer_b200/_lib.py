@@ -67,6 +67,7 @@ _SIGS = {
     'otb_beam_init': (c_int, [POINTER(BeamStateC), _P]),
     'otb_beam_step': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, _P, POINTER(BeamStateC), _P, _P, _P]),
     'otb_logsoftmax_topk': (c_int, [_P, c_int, c_int, _P, c_int, c_float, c_int, c_int, _P, _P, _P, c_int, _P]),
+    'otb_sample_step': (c_int, [_P, c_int, c_int, POINTER(BeamStateC), _P, _P]),
     'otb_beam_reconstruct': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P]),
     'otb_beam_finalize': (c_int, [POINTER(BeamStateC), c_float, c_float, c_int, _P, _P, _P]),
     'otb_attention_bwd': (c_int, [_P, c_int, c_int, _P, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P, _P, _P, c_int, c_int,
@@ -112,6 +113,7 @@ _SIGS = {
     'otb_nbest_rescore': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_float, c_int, c_int, c_int64, _P, _P, _P, _P]),
     'otb_edit_distance': (c_int, [_P, c_int, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P, _P]),
     'otb_mwer_coeff': (c_int, [_P, _P, _P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P]),
+    'otb_mwer_sample_coeff': (c_int, [_P, c_int, c_int, c_float, _P, _P, _P, _P]),
     'otb_mwer_grad': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
     'otb_conv_im2col': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'otb_conv_col2im_relu': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),

@@ -18,6 +18,7 @@
 #include <math.h>
 
 #include "beam_common.cuh"
+#include "counter_rng.cuh"
 #include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
@@ -131,6 +132,131 @@ const char* beam_step_launch(cudaStream_t stream, const float* logp, int ldl, in
     if ((pre_val == nullptr) != (pre_idx == nullptr)) return "beam_step: pre_val / pre_idx must both be given";
     return launch<beam_step_kernel>(dim3(st.N / st.beam), dim3(st.beam * 32), 0, stream, logp, ldl, V, lm_logp, ld_lm,
                                     lm_weight, st, dbg_ktok, dbg_offs, pre_val, pre_idx);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Ancestral sampling step (DESIGN.md 4.11): every live row n draws token = argmax_v (x_v + g_v), v < V, ties to the lower
+// id, with g_v = -log(-log u) the Gumbel noise of the uniform
+//     u(seed, step, n, v) = rng_u01(rng_key(rng_key(rng_key(seed, step), n), v))          (counter_rng.cuh)
+// so the token is distributed as softmax(x).  The row adds x_token - logsumexp(x[:V]) to its score; drawing <S/E> ends it,
+// and an ended row emits <S/E> at no cost.  Rows are never reordered (each row's parent is itself), and the search state
+// moves under otb_beam_step's conventions (tok_hist, par_hist, anc ping-pong, last_tok, flag, ctrl), so reconstruction
+// and the KV-cached decoder's ancestry addressing work unchanged.  One CTA per row, one pass over its logits: an online
+// log-sum-exp (running max m and sum s of exp(x - m)) and the perturbed arg-max, both merged over warps and then the CTA.
+// ------------------------------------------------------------------------------------------------
+static constexpr int SAMPLE_MAX_V = 48 * 1024;
+
+// (m, s) <- the log-sum-exp state of both halves; -inf entries contribute nothing
+__device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os) {
+    const float M = fmaxf(m, om);
+    if (M == -INFINITY) return;                    // both empty
+    s = s * expf(m - M) + os * expf(om - M);
+    m = M;
+}
+
+// THREADS threads per row (a multiple of 32).  The launch takes 512 while the rows fit one CTA per SM and 256 past that,
+// as the sweep of 32 .. 512 (tools/sample_step_sweep.cu, DESIGN.md 4.11) favours
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS) sample_step_kernel(const float* __restrict__ logits, int ldl, int V, BeamState st,
+                                                              const int* __restrict__ seed) {
+    constexpr int WARPS = THREADS / 32;
+    __shared__ float r_m[WARPS], r_s[WARPS], r_z[WARPS];
+    __shared__ int r_i[WARPS];
+    __shared__ int s_tok, s_step, s_live, s_fin;
+    __shared__ float s_inc;
+    const int n = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // ctrl and the row's flag are read once, by thread 0, before any thread can reach the atomics below: the last CTA of
+    // the step rewrites ctrl[0] / ctrl[1] and this CTA's thread 0 rewrites flag[n], and a warp of this CTA that started
+    // late must not see either
+    if (tid == 0) {
+        s_step = st.ctrl[0];
+        s_live = !st.ctrl[1] && s_step < st.Lmax;
+        s_fin = st.flag[n] != 0;
+    }
+    __syncthreads();
+    if (!s_live) return;                            // the search has ended: the state stays frozen, as in beam_step
+    const int step = s_step;
+    const bool fin = s_fin;
+    if (!fin) {
+        const uint32_t hrow = mix32(rng_key(rng_key((uint32_t)*seed, (uint32_t)step), (uint32_t)n));
+        const float* x = logits + (size_t)n * ldl;
+        float m = -INFINITY, s = 0.f, bz = -INFINITY;
+        int bi = 0x7fffffff;
+        for (int v = tid; v < V; v += THREADS) {
+            const float xv = __ldg(x + v);
+            if (xv == -INFINITY) continue;          // probability 0: neither in the sum nor drawable
+            if (xv > m) {
+                s = s * expf(m - xv) + 1.f;
+                m = xv;
+            } else {
+                s += expf(xv - m);
+            }
+            const float u = rng_u01(mix32(hrow ^ (uint32_t)v));      // rng_key(row key, v)
+            const float z = xv - logf(-logf(u));
+            if (better(z, v, bz, bi)) { bz = z; bi = v; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float om = __shfl_xor_sync(0xffffffffu, m, o), os = __shfl_xor_sync(0xffffffffu, s, o);
+            lse_merge(m, s, om, os);
+        }
+        warp_best(bz, bi);
+        if (lane == 0) { r_m[warp] = m; r_s[warp] = s; r_z[warp] = bz; r_i[warp] = bi; }
+        __syncthreads();
+        if (tid == 0) {
+            for (int w = 1; w < WARPS; ++w) {       // fixed order: repeated calls are bit-identical
+                lse_merge(m, s, r_m[w], r_s[w]);
+                if (better(r_z[w], r_i[w], bz, bi)) { bz = r_z[w]; bi = r_i[w]; }
+            }
+            // a row without a finite logit has nothing to draw: token 0 (the lowest id) and score -inf
+            if (m == -INFINITY) {
+                s_tok = 0;
+                s_inc = -INFINITY;
+            } else {
+                s_tok = bi;
+                s_inc = x[bi] - (m + logf(s));
+            }
+        }
+        __syncthreads();
+    }
+    const int tok = fin ? (int)EOS_ID : s_tok;
+    const int cur = step & 1, nxt = cur ^ 1;
+    const int* a_old = st.anc + ((size_t)cur * st.N + n) * st.Lmax;
+    int* a_new = st.anc + ((size_t)nxt * st.N + n) * st.Lmax;
+    for (int t = tid; t < step; t += THREADS) a_new[t] = a_old[t];
+    if (tid == 0) {
+        a_new[step] = n;
+        st.tok_hist[(size_t)step * st.N + n] = tok;
+        st.par_hist[(size_t)step * st.N + n] = n;
+        if (!fin) st.scores[n] += s_inc;            // an ended row keeps its score
+        st.last_tok[n] = tok;
+        st.flag[n] = tok == (int)EOS_ID ? 1 : 0;
+        const int ended = tok == (int)EOS_ID ? 1 : 0;
+        if (ended) atomicAdd(&st.ctrl[2], 1);
+        __threadfence();
+        // the last CTA of this step advances {step, done}, as beam_step's does
+        if (atomicAdd(&st.ctrl[3], 1) == (int)gridDim.x - 1) {
+            const int total = atomicAdd(&st.ctrl[2], 0);
+            st.ctrl[2] = 0;
+            st.ctrl[3] = 0;
+            __threadfence();
+            if (total == st.N) st.ctrl[1] = 1;
+            st.ctrl[0] = step + 1;
+        }
+    }
+}
+
+static const char* sample_step_check(int ldl, int V, const BeamState& st) {
+    if (V < 1 || V > SAMPLE_MAX_V) return "sample_step: V must be in [1, 49152]";
+    if (ldl < V) return "sample_step: ldl < V";
+    if (st.N < 1 || st.Lmax < 1) return "sample_step: empty problem (need N >= 1 and Lmax >= 1)";
+    return nullptr;
+}
+
+const char* sample_step_launch(cudaStream_t stream, const float* logits, int ldl, int V, BeamState st, const int* seed) {
+    if (const char* e = sample_step_check(ldl, V, st)) return e;
+    if (st.N <= num_sms()) return launch<sample_step_kernel<512>>(dim3(st.N), dim3(512), 0, stream, logits, ldl, V, st, seed);
+    return launch<sample_step_kernel<256>>(dim3(st.N), dim3(256), 0, stream, logits, ldl, V, st, seed);
 }
 
 // ------------------------------------------------------------------------------------------------

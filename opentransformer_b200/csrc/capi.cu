@@ -329,6 +329,11 @@ int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_log
                                                       out_val, out_idx, out_logp, ld_logp));
 }
 
+int otb_sample_step(const float* logits, int ldl, int V, const otb_beam_state* st, const int32_t* seed, void* stream) {
+    if (!logits || !st || !seed) return fail("otb_sample_step", "null operand");
+    RET("otb_sample_step", sample_step_launch(ST(stream), logits, ldl, V, to_state(st), seed));
+}
+
 int otb_beam_reconstruct(const otb_beam_state* st, int64_t* preds, int ld, int steps, void* stream) {
     if (!st || !preds) return fail("otb_beam_reconstruct", "null operand");
     RET("otb_beam_reconstruct", beam_reconstruct_launch(ST(stream), to_state(st), reinterpret_cast<long long*>(preds), ld, steps));
@@ -635,6 +640,12 @@ int otb_mwer_coeff(const int32_t* len, const int32_t* err, const float* tok_lp, 
                    const float* scale_dev, float* coeff, float* loss, void* stream) {
     if (!len || !err || !tok_lp || !tgt || !coeff || !loss) return fail("otb_mwer_coeff", "null operand");
     RET("otb_mwer_coeff", mwer_coeff_launch(ST(stream), len, err, tok_lp, Lp, tgt, B, K, scale, scale_dev, coeff, loss));
+}
+
+int otb_mwer_sample_coeff(const int32_t* err, int B, int K, float scale, const float* scale_dev, float* coeff, float* loss,
+                          void* stream) {
+    if (!err || !coeff || !loss) return fail("otb_mwer_sample_coeff", "null operand");
+    RET("otb_mwer_sample_coeff", mwer_sample_coeff_launch(ST(stream), err, B, K, scale, scale_dev, coeff, loss));
 }
 
 int otb_mwer_grad(const float* logits, int ld, int rows, int V, const int32_t* target, const float* tok_lp, const float* coeff, int Lp,

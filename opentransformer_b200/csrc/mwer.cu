@@ -7,6 +7,9 @@
 //   mwer_coeff_kernel      one warp per utterance, lane k = hypothesis k (K <= 32): the duplicate test against lower lanes,
 //                          l_k = sum of its token log-probs in position order, P_k = softmax over the kept l, the loss
 //                          sum_k P_k (W_k - mean W) and the coefficient c_k = dL/dl_k * scale of the row gradient.
+//   mwer_sample_coeff_kernel  the sampled estimator: one warp per utterance, lane k = sample k (K <= 32).  Samples are
+//                          drawn with replacement, so every one counts (no duplicate rule) and there is no softmax: the
+//                          loss is W^_b = mean W and c_k = (W_k - W^_b) / K * scale, exactly 0 when all W are equal.
 //   mwer_grad_kernel       one warp per logits row: dlogits = c_k (onehot(target) - softmax(x)) as bf16, zero in padding
 //                          columns and in rows without a target or with c_k = 0 (those rows are not read).  The row's
 //                          log-sum-exp is the one otb_token_logprob formed: lse = x[target] - logprob, so the row is read
@@ -116,6 +119,22 @@ __global__ void __launch_bounds__(32) mwer_coeff_kernel(const int* __restrict__ 
     if (k == 0) loss[b] = risk;
 }
 
+__global__ void __launch_bounds__(32) mwer_sample_coeff_kernel(const int* __restrict__ err, int K, float scale,
+                                                               const float* __restrict__ scale_dev, float* __restrict__ coeff,
+                                                               float* __restrict__ loss) {
+    const int b = blockIdx.x, k = threadIdx.x;
+    const bool live = k < K;
+    const size_t h = (size_t)b * K + k;
+    const float W = live ? (float)err[h] : 0.f;
+    float sw = W;                       // integer-valued: the sum is exact below 2^24
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sw += __shfl_xor_sync(0xffffffffu, sw, o);
+    const float mean = sw / (float)K;
+    const float s = scale_dev != nullptr ? scale * *scale_dev : scale;
+    if (live) coeff[h] = (W - mean) / (float)K * s;
+    if (k == 0) loss[b] = mean;
+}
+
 __global__ void __launch_bounds__(MG_WARPS * 32) mwer_grad_kernel(const float* __restrict__ logits, int ld, int rows, int V,
                                                                   const int* __restrict__ target, const float* __restrict__ tok_lp,
                                                                   const float* __restrict__ coeff, int Lp, bf16* __restrict__ dlogits) {
@@ -166,6 +185,12 @@ const char* mwer_coeff_launch(cudaStream_t stream, const int* len, const int* er
     if (B < 1 || K < 1 || K > MWER_KMAX) return "mwer_coeff: need B >= 1 and 1 <= K <= 32";
     if (Lp < 1) return "mwer_coeff: need Lp >= 1";
     return launch<mwer_coeff_kernel>(B, 32, 0, stream, len, err, tok_lp, Lp, tgt, K, scale, scale_dev, coeff, loss);
+}
+
+const char* mwer_sample_coeff_launch(cudaStream_t stream, const int* err, int B, int K, float scale, const float* scale_dev,
+                                     float* coeff, float* loss) {
+    if (B < 1 || K < 1 || K > MWER_KMAX) return "mwer_sample_coeff: need B >= 1 and 1 <= K <= 32";
+    return launch<mwer_sample_coeff_kernel>(B, 32, 0, stream, err, K, scale, scale_dev, coeff, loss);
 }
 
 const char* mwer_grad_launch(cudaStream_t stream, const float* logits, int ld, int rows, int V, const int* target, const float* tok_lp,

@@ -219,6 +219,7 @@ const char* beam_step_launch(cudaStream_t stream, const float* logp, int ldl, in
 const char* logsoftmax_topk_launch(cudaStream_t stream, const float* logits, int ldl, int V, const float* lm_logp,
                                    int ld_lm, float lm_weight, int k, int rows, float* out_val, int* out_idx,
                                    float* out_logp, int ld_logp);
+const char* sample_step_launch(cudaStream_t stream, const float* logits, int ldl, int V, BeamState st, const int* seed);
 const char* beam_reconstruct_launch(cudaStream_t stream, BeamState st, long long* preds, int ld, int steps);
 const char* beam_finalize_launch(cudaStream_t stream, BeamState st, float penalty, float lamda, int nbest,
                                  long long* out_preds, float* out_scores);
@@ -290,6 +291,8 @@ const char* edit_distance_launch(cudaStream_t stream, const int* hyp, int ldh, c
                                  const int* ref_len, int N, int K, int max_h, int max_r, int* out);
 const char* mwer_coeff_launch(cudaStream_t stream, const int* len, const int* err, const float* tok_lp, int Lp, const int* tgt, int B,
                               int K, float scale, const float* scale_dev, float* coeff, float* loss);
+const char* mwer_sample_coeff_launch(cudaStream_t stream, const int* err, int B, int K, float scale, const float* scale_dev,
+                                     float* coeff, float* loss);
 const char* mwer_grad_launch(cudaStream_t stream, const float* logits, int ld, int rows, int V, const int* target, const float* tok_lp,
                              const float* coeff, int Lp, bf16* dlogits);
 

@@ -48,6 +48,13 @@ def allreduce_mean_(flat, group=None):
     return flat
 
 
+def rank_in(group=None):
+    """This process's rank in `group` (0 without a process group)."""
+    if not (dist.is_available() and dist.is_initialized()):
+        return 0
+    return dist.get_rank(group)
+
+
 def broadcast_from_first_(tensors, group=None):
     """In place: every rank takes the first rank's values of `tensors` (the model's buffers, as the reference's
     DistributedDataParallel broadcasts them from rank 0 before each forward).  No-op without a process group."""

@@ -481,6 +481,24 @@ class BeamState:
         return out_preds, out_scores
 
 
+SAMPLE_MAX_VOCAB = 48 * 1024
+
+
+def sample_step(logits, V, state, seed):
+    """One step of ancestral sampling on a BeamState (otb_sample_step, DESIGN.md 4.11): every live row draws its next token
+    from softmax(logits[n, :V]) by the Gumbel-max trick on the counter hash of (seed, step, row, token), adds the token's
+    log-prob to its score and ends on <S/E>; rows are never reordered.  logits f32 [N, ld]; seed i32 device tensor [1],
+    read at run time (a captured step draws fresh samples when the seed or the step counter changes)."""
+    _mat(logits, 'logits', torch.float32)
+    _need(seed, torch.int32, 'seed')
+    if logits.shape[0] != state.N or not 1 <= V <= min(SAMPLE_MAX_VOCAB, logits.shape[1]):
+        raise ValueError(f'sample_step: need logits [N = {state.N}, >= V] and 1 <= V <= {SAMPLE_MAX_VOCAB}, got '
+                         f'{tuple(logits.shape)} and V = {V}')
+    check(_lib.lib().otb_sample_step(_p(logits), logits.stride(0), V, ctypes.byref(state.c), _p(seed), _stream()),
+          'otb_sample_step')
+    _count()
+
+
 def decode_persistent_workspace(N, n_layers, Lmax, B, beam, vocab, device):
     n = int(_lib.lib().otb_decode_persistent_workspace(N, n_layers, Lmax, B, beam, vocab))
     if n < 0:
@@ -1085,6 +1103,24 @@ def mwer_coeff(tgt, lengths, err, tok_lp, grad_scale=1.0, scale_dev=None):
     loss = torch.empty(B, dtype=torch.float32, device=tgt.device)
     check(_lib.lib().otb_mwer_coeff(_p(lengths), _p(err), _p(tok_lp), Lp, _p(tgt), B, K, float(grad_scale), _p(scale_dev), _p(coeff),
                                     _p(loss), _stream()), 'otb_mwer_coeff')
+    _count()
+    return loss, coeff
+
+
+def mwer_sample_coeff(err, grad_scale=1.0, scale_dev=None):
+    """The sampled estimator's coefficients (otb_mwer_sample_coeff, DESIGN.md 4.11): err i32 [B, K] the edit distances of
+    K samples per utterance, drawn with replacement.  -> (loss f32 [B] = mean_k W_k, coeff f32 [B, K] = (W_k - mean W) / K *
+    grad_scale (times the f32 device scalar scale_dev when given)), exactly 0 when an utterance's W are all equal."""
+    if err.dim() != 2:
+        raise ValueError(f'mwer_sample_coeff: err must be [B, K], got {tuple(err.shape)}')
+    _need(err, torch.int32, 'err')
+    if scale_dev is not None:
+        _need(scale_dev, torch.float32, 'scale_dev')
+    B, K = err.shape
+    coeff = torch.empty(B, K, dtype=torch.float32, device=err.device)
+    loss = torch.empty(B, dtype=torch.float32, device=err.device)
+    check(_lib.lib().otb_mwer_sample_coeff(_p(err), B, K, float(grad_scale), _p(scale_dev), _p(coeff), _p(loss), _stream()),
+          'otb_mwer_sample_coeff')
     _count()
     return loss, coeff
 

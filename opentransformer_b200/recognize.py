@@ -232,11 +232,21 @@ class BeamDecoder:
     ancestry and step counter, so beam pruning reorders it for free; the recurrent LM reads the newest token from a zero
     state, as the reference does (cache['lm'] = None at every step).  The persistent kernel does not take an LM, so it is
     off then.
+
+    sample=True turns the search into ancestral sampling (DESIGN.md 4.11): the `beam` rows of an utterance all start live
+    at BOS with score 0, and each step draws every live row's next token from the decoder's softmax (ops.sample_step, the
+    Gumbel-max trick on a counter hash of (seed, step, row, token)) in place of the log-softmax / top-k / beam kernels.  Rows
+    are never reordered, and a row's score is the log-probability of its sample.  The seed is the i32 device scalar
+    `self.seed`, read by every replay of the captured step.  Not with an LM or a CTC term, and never on the persistent
+    kernel.
     """
 
     def __init__(self, decoder, batch, beam, T, max_len, device, use_graph=True, persistent=False, keep_logp=None, ctc=None,
-                 lm=None):
+                 lm=None, sample=False):
         check_max_len('BeamDecoder', max_len)
+        if sample and (lm is not None or ctc is not None):
+            raise NotImplementedError('BeamDecoder: sampling draws from the attention decoder alone; sampling with a fused LM '
+                                      'or a CTC term is not implemented')
         if lm is not None:
             check_lm_fusion('BeamDecoder', lm[0], decoder.vocab_size)
         self.dec = decoder
@@ -283,7 +293,10 @@ class BeamDecoder:
         # persistent path: the whole loop in ONE launch (csrc/decode_group.cu: row groups of <= 128 hypotheses x 16 CTAs,
         # wgmma GEMMs, group-local barriers) when the configuration is the shipped one (post-norm GLU decoder, d_model 256,
         # 4 heads, d_ff 2048, <= 256 memory frames); anything else takes the per-step graph.
-        self.persistent = bool(persistent) and self.ctc is None and self.lm is None and self.mega_supported()
+        self.sample = bool(sample)
+        self.seed = torch.zeros(1, dtype=torch.int32, device=device) if self.sample else None
+        self.persistent = (bool(persistent) and self.ctc is None and self.lm is None and not self.sample
+                           and self.mega_supported())
         self._mega_model = None
         self._mega_sig = None
         self._ws = None
@@ -340,6 +353,8 @@ class BeamDecoder:
         for l, p in enumerate(pk['blocks']):
             ops.linear(memory_bf16, p['wkv'], p['bkv'], out=self.kvx[l])
         self.state.init()
+        if self.sample:
+            self.state.scores.zero_()           # every row starts live (the beam's init leaves rows 1.. at -inf)
         if self.ctc is not None:
             ops.log_softmax(self.ctc_head.logits_bf16(memory_bf16), self.dec.vocab_size, out=self.ctc.lp)
             self.ctc.init(self.mem_len)
@@ -366,6 +381,9 @@ class BeamDecoder:
         x = ops.embed_posenc(st.last_tok, pk['emb'], self.table, self.N, dec.d_model, step_ptr=st.step_ptr)
         x = dec.decode_cached_bf16(pk, x, self.kc, self.vc, st.anc, st.step_ptr, self.kvx, self.mem_len, self.beam, self.T)
         ops.linear(x, pk['wout'], pk['bout'], out=self.logits)
+        if self.sample:
+            ops.sample_step(self.logits, dec.vocab_size, st, self.seed)
+            return
         out_logp = self.logp if self.keep_logp else None
         if self.ctc is None:
             ops.logsoftmax_topk(self.logits, dec.vocab_size, self.beam, self.lm_logp, self.lm_weight,
@@ -577,18 +595,19 @@ class SpeechToTextRecognizer(Recognizer):
         self.attn_weights = {'encoder': encoder_attn_weights(len(enc.blocks), sink), 'decoder': []}
         return out
 
-    def _decoder_for(self, B, T2, device):
+    def _decoder_for(self, B, T2, device, samples=0):
         # the CTC weight and candidate count, the fused LM's weights and lm_weight are launch arguments that a captured step
-        # bakes in
+        # bakes in; samples > 0: a sampling decoder of that many rows per utterance, kept apart from the beam decoders
         ctc = (self.model.assistor, self.ctc_weight, self.ctc_candidates) if self.ctc_weight > 0.0 else None
         lm = (self.lm, float(self.lm_weight)) if self._lm_fused() else None
-        key = (B, self.beam_width, T2, self.max_len, device.index, ctc[1:] if ctc else None, lm)
+        rows = samples or self.beam_width
+        key = (B, rows, T2, self.max_len, device.index, ctc[1:] if ctc else None, lm, 'sample' if samples else 'beam')
         bd = self._decoders.pop(key, None)
         if bd is None:
             while self.max_decoders is not None and len(self._decoders) >= self.max_decoders:
                 self._decoders.pop(next(iter(self._decoders)))          # the least recently used goes, with its buffers
-            bd = BeamDecoder(self.model.decoder, B, self.beam_width, T2, self.max_len, device, self.use_graph,
-                             persistent=self.persistent, ctc=ctc, lm=lm)
+            bd = BeamDecoder(self.model.decoder, B, rows, T2, self.max_len, device, self.use_graph,
+                             persistent=self.persistent, ctc=ctc, lm=lm, sample=bool(samples))
         self._decoders[key] = bd          # (re-)inserted as the most recently used
         return bd
 
@@ -655,6 +674,40 @@ class SpeechToTextRecognizer(Recognizer):
     def recognize(self, inputs, inputs_mask):
         preds, scores, _ = self.recognize_ids(inputs, inputs_mask)
         return self.nbest_translate(preds), scores
+
+    def sample_ids(self, inputs, inputs_mask, num_samples, seed=0):
+        """Draw num_samples (1..16) hypotheses per utterance from the attention decoder, y ~ P(y | x), by ancestral sampling
+        at temperature 1 (DESIGN.md 4.11): up to max_len tokens each, one captured step per token, the samples drawn
+        independently and with replacement.  seed: an int, or an i32 device tensor of one element (read on the device, so
+        a caller can advance it without a host synchronisation); the same seed and weights give the same samples.
+        -> (ids i64 [B, num_samples, steps] in sample order, <S/E> after each sample's end, as recognize_ids pads; lengths
+        i32 [B, num_samples], the tokens before <S/E>; log-probs f32 [B, num_samples], the sum of each sample's token
+        log-probs, its closing <S/E> included), on the device.  Not with LM fusion, a CTC term (ctc_weight > 0) or
+        apply_rescoring (NotImplementedError)."""
+        if self._lm_fused():
+            raise NotImplementedError('sample_ids: sampling from the LM-fused distribution is not implemented; build the '
+                                      'recognizer without lm (or with apply_lm_rescoring)')
+        if self.ctc_weight > 0.0:
+            raise NotImplementedError('sample_ids: sampling from the joint CTC/attention distribution (ctc_weight > 0) is not '
+                                      'implemented')
+        if self.apply_rescoring:
+            raise NotImplementedError('sample_ids: under apply_rescoring the first pass is the CTC prefix beam search; '
+                                      'sampling draws from the attention decoder alone')
+        if not isinstance(num_samples, int) or not 1 <= num_samples <= 16:
+            raise ValueError(f'sample_ids: num_samples must be in 1..16, got {num_samples}')
+        K = num_samples
+        with torch.no_grad():
+            mem, mem_len, B, T2 = self._encode_bf16(inputs, inputs_mask)
+            bd = self._decoder_for(B, T2, inputs.device, samples=K)
+            bd.setup(mem, mem_len)
+            if torch.is_tensor(seed):
+                bd.seed.copy_(seed.reshape(1))
+            else:
+                bd.seed.fill_((int(seed) + 2 ** 31) % 2 ** 32 - 2 ** 31)         # the seed's 32 bits as an i32
+            steps = bd.run(self.max_len)
+            ids = bd.state.reconstruct(steps)[:, 1:].reshape(B, K, steps)
+            lengths = (ids != EOS).sum(dim=2, dtype=torch.int32)      # an ended row emits only <S/E>
+            return ids, lengths, bd.state.scores.view(B, K).clone()
 
 
 CTC_CUTOFF_TOP_N = 40      # ctcdecode's cutoff_top_n default (cutoff_prob 1.0), which recognize/ctc.py:20-24 leaves in place

@@ -46,7 +46,7 @@ import torch
 
 from . import ops
 from . import modules
-from .dp import allreduce_mean_, broadcast_from_first_
+from .dp import allreduce_mean_, broadcast_from_first_, rank_in
 from .modules import (ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder,
                       TransformerEncoder, _lengths)
 from .ops import BF16, EPI_BIAS, EPI_RESID, EPI_TABLE, EPI_RELU
@@ -776,11 +776,13 @@ def _mwer_references(truth, truth_length):
     return ref, (ref == 1).int().argmax(dim=1).to(torch.int32)
 
 
-def _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad_scale, g, dmem):
+def _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad_scale, g, dmem, estimator='nbest'):
     """The MWER term (DESIGN.md 4.11) on the n-best (hypothesis inputs i64 [B*K, Lp] = BOS y PAD..., targets [B*K, Lp] =
     y <S/E> -1..., K), over the memory of the cross-entropy branch: the decoder teacher-forced on the K hypotheses of each
     utterance, their token log-probs, the edit distances to the references, and with g the backward of
-    sum_b L_MWER,b / B (x grad_scale) on top of dmem.  -> (mean_b L_MWER,b, dmem)."""
+    sum_b L_MWER,b / B (x grad_scale) on top of dmem.  -> (mean_b L_MWER,b, dmem).  estimator 'sample': the rows are K
+    samples drawn with replacement, and only the coefficients change (otb_mwer_sample_coeff: L_MWER,b = mean_k W_k and the
+    score-function coefficients (W_k - mean W) / K)."""
     hyp_in, hyp_tgt, K = nbest
     dec, B, T2, lengths = model.decoder, tr.B, tr.T2, tr.lengths
     Lp = hyp_in.shape[1]
@@ -798,7 +800,10 @@ def _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad
     flat = tgt.view(-1)
     tok = ops.token_logprob(logits, dec.vocab_size, flat)
     ms, mdev = _loss_scale(grad_scale, 1.0 / B)
-    loss_b, coeff = ops.mwer_coeff(tgt.view(B, K, Lp), n.view(B, K), err.view(B, K), tok.view(B, K, Lp), ms, mdev)
+    if estimator == 'sample':
+        loss_b, coeff = ops.mwer_sample_coeff(err.view(B, K), ms, mdev)
+    else:
+        loss_b, coeff = ops.mwer_coeff(tgt.view(B, K, Lp), n.view(B, K), err.view(B, K), tok.view(B, K, Lp), ms, mdev)
     if g is not None:
         dlogits = ops.mwer_grad(logits, dec.vocab_size, flat, tok, coeff)
         del logits
@@ -807,7 +812,7 @@ def _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad
 
 
 def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=True, grad_sink=None, grad_scale=1.0,
-                     bf16_of=None, drop_seed=None, nbest=None, mwer_ce_weight=0.01):
+                     bf16_of=None, drop_seed=None, nbest=None, mwer_ce_weight=0.01, mwer_estimator='nbest'):
     """SpeechToText.train_pass (the contract is at the top of this file).  inputs f32 [B,T,F], mask bool [B,T], truth i64
     [B,L+1] (BOS ... EOS PAD*); the gradients are named as in model.named_parameters().  truth_length: i32/i64 [B] label
     counts incl. <S/E> (targets['targets_length'], data/loader.py:94) -- required when model.ctc_weight > 0: the loss is
@@ -818,7 +823,11 @@ def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=T
     nbest = (hypothesis inputs i64 [B*K, Lp], their targets [B*K, Lp], K), second_pass_rows' layout: minimum word error
     rate training (DESIGN.md 4.11).  The loss becomes mean_b L_MWER,b + mwer_ce_weight * (the loss above); the decoder
     also runs on the K hypotheses of each utterance over the same memory, with its own dropout sites (MWER_SITE), and both
-    branches' memory gradients go into the one encoder backward."""
+    branches' memory gradients go into the one encoder backward.  mwer_estimator 'nbest' (the default) is the expected risk
+    over the n-best; 'sample' takes the rows as K samples from the model (SpeechToTextRecognizer.sample_ids) and trains on
+    the score-function estimate: L_MWER,b = mean_k W_k, whose gradient is estimated by sum_k (W_k - mean W) / K * dl_k."""
+    if mwer_estimator not in ('nbest', 'sample'):
+        raise ValueError(f"forward_backward: mwer_estimator must be 'nbest' or 'sample', got {mwer_estimator!r}")
     dec = model.decoder
     ctc_w = float(getattr(model, 'ctc_weight', 0.0) or 0.0)
     if ctc_w > 0.0 and truth_length is None:
@@ -872,7 +881,8 @@ def forward_backward(model, inputs, mask, truth, truth_length=None, want_grads=T
         dmem = _dec_bwd(dec, pk, tgt_in, dlogits, y, dec_last, dec_tape, mem, dmem, g, B, 1, L, T2, lengths, d_drop)
     if nbest is not None:
         del logits, dec_tape
-        loss_mwer, dmem = _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad_scale, g, dmem)
+        loss_mwer, dmem = _mwer_branch(model, pk, nbest, truth, truth_length, mem, tr, drop_seed, grad_scale, g, dmem,
+                                       mwer_estimator)
         loss = loss_mwer + ce_w * loss
     if not want_grads:
         return loss, None
@@ -972,12 +982,13 @@ def loss_train_mode(model, *batch):
         return model.train_pass(*batch, want_grads=False, drop_seed=next_drop_seed(model, batch[0].device))[0]
 
 
-def _check_mwer(model, nbest, ce_weight, max_len, mixspeech):
-    """What FusedTrainer refuses for minimum word error rate training, before any device work."""
+def _check_mwer(model, nbest, ce_weight, max_len, mixspeech, name='mwer_nbest'):
+    """What FusedTrainer refuses for minimum word error rate training, before any device work (name: the option that sets
+    K, mwer_nbest or mwer_samples)."""
     if not isinstance(getattr(model, 'decoder', None), TransformerDecoder):
         raise NotImplementedError(f'MWER training scores an attention decoder\'s n-best; {type(model).__name__} has none')
     if not 2 <= nbest <= 16:
-        raise ValueError(f'mwer_nbest must be 0 (off) or in 2..16, got {nbest}')
+        raise ValueError(f'{name} must be 0 (off) or in 2..16, got {nbest}')
     if not ce_weight >= 0.0:
         raise ValueError(f'mwer_ce_weight must be >= 0, got {ce_weight}')
     if not 1 <= max_len <= 1022:
@@ -1008,17 +1019,27 @@ class FusedTrainer:
     mwer_nbest = K in 2..16: minimum word error rate training (DESIGN.md 4.11).  Every micro-step first decodes the
     micro-batch's K-best with the current weights (beam_width = nbest = K, penalty 0, max_len = mwer_max_len) on the
     inference path, in eval mode and outside any CUDA graph, then trains on mean_b L_MWER,b + mwer_ce_weight * (the
-    model's loss).  Attention-decoder models only (NotImplementedError otherwise); not with mixspeech."""
+    model's loss).  Attention-decoder models only (NotImplementedError otherwise); not with mixspeech.
+    mwer_samples = K in 2..16: sampling-based MWER training (DESIGN.md 4.11), in place of mwer_nbest (not with it).  Every
+    micro-step draws K samples per utterance from the model (SpeechToTextRecognizer.sample_ids, eval mode, outside any
+    CUDA graph, max_len = mwer_max_len) and trains on mean_b mean_k W_k + mwer_ce_weight * (the model's loss) through the
+    score-function gradient.  The sampling seed is an i32 device scalar advanced every micro-step, the same on every rank;
+    each rank draws with it XOR a constant of its own, so the ranks' samples are independent.  state_dict saves it
+    ('sample_seed'), so a resumed run draws the same samples on every rank."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.98), eps=1e-9, weight_decay=1e-6, clip_grad=5.0, model_size=256,
                  warmup_steps=12000, factor=1.0, accum_steps=1, process_group=None, use_graph=True, mixspeech=False,
-                 grad_noise=0.0, mwer_nbest=0, mwer_ce_weight=0.01, mwer_max_len=60):
+                 grad_noise=0.0, mwer_nbest=0, mwer_ce_weight=0.01, mwer_max_len=60, mwer_samples=0):
         if mixspeech and not hasattr(model, 'mix_batch'):
             raise NotImplementedError(f'MixSpeech mixes [B, T, F] speech features; {type(model).__name__} takes token inputs')
         if not grad_noise >= 0.0:
             raise ValueError(f'grad_noise must be >= 0, got {grad_noise}')
+        if mwer_nbest and mwer_samples:
+            raise ValueError('mwer_nbest and mwer_samples are the two MWER estimators (n-best and sampled); choose one')
         if mwer_nbest:
             _check_mwer(model, mwer_nbest, mwer_ce_weight, mwer_max_len, mixspeech)
+        if mwer_samples:
+            _check_mwer(model, mwer_samples, mwer_ce_weight, mwer_max_len, mixspeech, name='mwer_samples')
         model.check_fused_trainer()
         self.model = model
         # parameters the forward never reads (a Conformer's post_ffn) stay out of the flat buffers: no gradient, no weight decay
@@ -1086,15 +1107,25 @@ class FusedTrainer:
             self.noise_mask = ops.noise_bitmask(total, [self.offsets[n] for n, _ in self.params]).to(dev)
         broadcast_from_first_([t for t in (self.mix_seed, self.noise_seed) if t is not None], process_group)
         self.mwer_nbest, self.mwer_ce_weight = int(mwer_nbest), float(mwer_ce_weight)
-        self._recognizer = None
-        if self.mwer_nbest:
+        self.mwer_samples = int(mwer_samples)
+        self._recognizer = self.sample_seed = None
+        if self.mwer_samples:
+            # one base seed on every rank, so that the one value state_dict saves resumes every rank; each rank draws with
+            # base ^ (rank * 0x9E3779B9), because the sampling hash keys on row ids that are local to a rank and the ranks'
+            # samples must be independent (rank 0 draws with the base itself)
+            self.sample_seed = torch.randint(0, 2 ** 31 - 1, (1,), dtype=torch.int32).to(dev)
+            broadcast_from_first_([self.sample_seed], process_group)
+            off = (rank_in(process_group) * 0x9E3779B9) & 0xFFFFFFFF
+            self._seed_xor = off - 2 ** 32 if off >= 2 ** 31 else off
+        if self.mwer_nbest or self.mwer_samples:
             from .recognize import SpeechToTextRecognizer
             training = model.training
             # one cached BeamDecoder: ragged batches bring a new frame count almost every step, and a decoder kept for an
             # older one would hold its KV caches and the bf16 weights of the step it last decoded; the weights move every
             # optimizer step, so a kept decoder would only save its buffer allocation
-            self._recognizer = SpeechToTextRecognizer(model, beam_width=self.mwer_nbest, nbest=self.mwer_nbest,
-                                                      max_len=mwer_max_len, penalty=0, ngpu=0, max_decoders=1)
+            K = self.mwer_nbest or self.mwer_samples
+            self._recognizer = SpeechToTextRecognizer(model, beam_width=K, nbest=K, max_len=mwer_max_len, penalty=0, ngpu=0,
+                                                      max_decoders=1)
             model.train(training)
 
     @property
@@ -1133,13 +1164,16 @@ class FusedTrainer:
         kw = {}
         if self.mwer_nbest:         # the n-best rows ride at the end of the batch (_with_nbest)
             batch, kw = batch[:-2], {'nbest': batch[-2:] + (self.mwer_nbest,), 'mwer_ce_weight': self.mwer_ce_weight}
+        elif self.mwer_samples:     # so do the sampled rows
+            batch, kw = batch[:-2], {'nbest': batch[-2:] + (self.mwer_samples,), 'mwer_ce_weight': self.mwer_ce_weight,
+                                     'mwer_estimator': 'sample'}
         loss, _ = self.model.train_pass(*batch, grad_sink=self.sink, grad_scale=1.0 / self.accum_steps, bf16_of=self._bf16_of,
                                         drop_seed=self.drop_seed, **kw)
         return loss
 
     def _with_nbest(self, batch):
-        """MWER: the micro-batch's K-best decoded with the current weights on the inference path (eval mode, so no
-        dropout and a Conformer's BatchNorm on its running statistics), appended to the batch as second_pass_rows' rows
+        """MWER: the micro-batch's K-best (mwer_samples: K samples) decoded with the current weights on the inference path
+        (eval mode, so no dropout and a Conformer's BatchNorm on its running statistics), appended to the batch as second_pass_rows' rows
         (hypothesis inputs i64 [B*K, Lp], targets i32 [B*K, Lp]).  Reading Lp is a host synchronisation; as part of the
         batch the rows make Lp and K part of the CUDA-graph key."""
         from .recognize import second_pass_rows
@@ -1147,7 +1181,12 @@ class FusedTrainer:
         maps, enc.return_attn_weights = enc.return_attn_weights, False    # training produces no attention maps
         self.model.eval()
         try:
-            ids, _, _ = self._recognizer.recognize_ids(batch[0], batch[1])
+            if self.mwer_samples:
+                self.sample_seed.add_(1)            # fresh samples every micro-step, without a host synchronisation
+                seed = self.sample_seed if not self._seed_xor else torch.bitwise_xor(self.sample_seed, self._seed_xor)
+                ids, _, _ = self._recognizer.sample_ids(batch[0], batch[1], self.mwer_samples, seed)
+            else:
+                ids, _, _ = self._recognizer.recognize_ids(batch[0], batch[1])
         finally:
             self.model.train()
             enc.return_attn_weights = maps
@@ -1246,6 +1285,8 @@ class FusedTrainer:
 
         own = {'skipped_steps': skipped, 'drop_seed': host(self.drop_seed), 'mix_seed': host(self.mix_seed),
                'mix_step': host(self.mix_step), 'noise_seed': host(self.noise_seed)}
+        if self.sample_seed is not None:
+            own['sample_seed'] = host(self.sample_seed)
         return {'global_step': global_step, 'optim': opt.state_dict(), 'fused_trainer': own}
 
     def load_state_dict(self, ckpt):
@@ -1297,7 +1338,7 @@ class FusedTrainer:
                 self.v[o:o + k].copy_(st['exp_avg_sq'].reshape(-1))
             own = ckpt.get('fused_trainer') or {}
             self.counters.copy_(torch.tensor([t, int(ckpt['global_step']), int(own.get('skipped_steps', 0))], dtype=torch.int32))
-            for name in ('drop_seed', 'mix_seed', 'mix_step', 'noise_seed'):
+            for name in ('drop_seed', 'mix_seed', 'mix_step', 'noise_seed', 'sample_seed'):
                 dst = getattr(self, name)
                 if dst is not None and own.get(name) is not None:
                     dst.fill_(int(own[name]))
@@ -1319,7 +1360,7 @@ class FusedTrainer:
             # data parallel: BatchNorm running statistics follow the first rank's (DistributedDataParallel's
             # broadcast_buffers): each rank's forward updates them from its own shard, so they would drift apart
             broadcast_from_first_(self.bn_buffers, self.group)
-            if self.mwer_nbest:
+            if self.mwer_nbest or self.mwer_samples:
                 batch = self._with_nbest(batch)
             ent = self._graph_for(batch) if self.use_graph else None
             if ent is not None:
