@@ -2,9 +2,8 @@
 //   loss_ctc = nn.CTCLoss(blank = 0, reduction 'mean', zero_infinity = True)(log_softmax(output_layer(memory)).transpose(0,1),
 //                                                                              targets_out, memory_length, targets_length)
 // Forward AND gradient with respect to the logits in two kernels (the reference differentiates F.ctc_loss by autograd):
-//   ctc_alpha_beta_kernel  one CTA per utterance over the S = 2 L + 1 states of the blank-extended label sequence: one
-//                          state per thread up to 64 labels (S <= 129, 160 threads), two per thread up to 1023 (S <= 2047,
-//                          1024 threads):
+//   ctc_alpha_beta_kernel  one CTA per utterance over the S = 2 L + 1 states of the trellis (ctc_trellis.cuh): one
+//                          state per thread up to 64 labels (<129, 160>), two per thread up to 1023 (<2047, 1024>):
 //                          forward variables alpha_t(s) over the valid frames (log domain, fp32), the utterance's negative
 //                          log-likelihood, then the backward variables; ws[b,t,s] <- alpha_t(s) + beta_t(s)
 //   ctc_grad_kernel        one CTA per (utterance, frame): d loss / d logit[k] = scale_b (softmax[k] - sum_{s: l_s = k}
@@ -14,6 +13,7 @@
 // HBM-bound integer/float work: the [B T', V] log-prob matrix is read once by each kernel.
 #include <math.h>
 
+#include "ctc_trellis.cuh"
 #include "launch.cuh"
 #include "otb_internal.h"
 #include "ptx.cuh"
@@ -23,184 +23,59 @@ namespace otb {
 static constexpr int CTC_SMAX = 129;        // 2 * 64 + 1 states: targets of up to 64 labels
 static constexpr int CTC_SMAX_LONG = 2047;  // 2 * 1023 + 1 states: targets of up to 1023 labels
 
-__global__ void __launch_bounds__(160) ctc_alpha_beta_kernel(const float* __restrict__ logp, int ldl, int T, const int* __restrict__ in_len,
-                                                             const long long* __restrict__ targets, int ldt,
-                                                             const int* __restrict__ tgt_len, int blank, int V, float* __restrict__ nll,
-                                                             float* __restrict__ ws, int S_ws) {
-    __shared__ int lab[CTC_SMAX + 2];
-    __shared__ float buf[2][CTC_SMAX + 2];
-    const int b = blockIdx.x, s = threadIdx.x;
-    const int L = min(tgt_len[b], (CTC_SMAX - 1) / 2);
-    const int S = 2 * L + 1;
-    const int Tb = min(in_len[b], T);
-    if (s < S + 2) {
-        int l = blank;
-        if (s < S && (s & 1)) {
-            long long v = targets[(size_t)b * ldt + (s >> 1)];
-            l = (v < 0 || v >= V) ? blank : (int)v;
-        }
-        lab[s] = l;
-    }
-    __syncthreads();
-    const float* lp = logp + (size_t)b * T * ldl;
-    float* w = ws + (size_t)b * T * S_ws;
-    if (Tb < 1) {   // no frames: infeasible unless the target is empty too (PyTorch: inf -> 0 with zero_infinity)
-        if (s == 0) nll[b] = INFINITY;
-        return;
-    }
-    const int my = (s < S) ? lab[s] : blank;
-    const bool skip_ok = (s >= 2 && s < S && my != blank && my != lab[s - 2]);
-    // ---- forward variables
-    float a = -INFINITY;
-    if (s == 0) a = lp[blank];
-    if (s == 1 && S > 1) a = lp[my];
-    if (s < S) { buf[0][s] = a; w[s] = a; }
-    __syncthreads();
-    int cur = 0;
-    for (int t = 1; t < Tb; ++t) {
-        if (s < S) {
-            float v = buf[cur][s];
-            if (s >= 1) v = log_add(v, buf[cur][s - 1]);
-            if (skip_ok) v = log_add(v, buf[cur][s - 2]);
-            a = (v == -INFINITY) ? -INFINITY : v + lp[(size_t)t * ldl + my];
-            buf[cur ^ 1][s] = a;
-            w[(size_t)t * S_ws + s] = a;
-        }
-        cur ^= 1;
-        __syncthreads();
-    }
-    float total = buf[cur][S - 1];
-    if (S > 1) total = log_add(total, buf[cur][S - 2]);
-    __syncthreads();
-    if (s == 0) nll[b] = -total;          // +inf when no alignment exists
-    // ---- backward variables; ws <- alpha + beta
-    const bool skip_fw = (s + 2 < S && lab[s + 2] != blank && lab[s + 2] != my);
-    float be = -INFINITY;
-    if (s == S - 1) be = lp[(size_t)(Tb - 1) * ldl + blank];
-    if (s == S - 2 && S > 1) be = lp[(size_t)(Tb - 1) * ldl + my];
-    if (s < S) {
-        buf[0][s] = be;
-        w[(size_t)(Tb - 1) * S_ws + s] += be;
-    }
-    __syncthreads();
-    cur = 0;
-    for (int t = Tb - 2; t >= 0; --t) {
-        if (s < S) {
-            float v = buf[cur][s];
-            if (s + 1 < S) v = log_add(v, buf[cur][s + 1]);
-            if (skip_fw) v = log_add(v, buf[cur][s + 2]);
-            be = (v == -INFINITY) ? -INFINITY : v + lp[(size_t)t * ldl + my];
-            buf[cur ^ 1][s] = be;
-            w[(size_t)t * S_ws + s] += be;
-        }
-        cur ^= 1;
-        __syncthreads();
-    }
-}
-
-// Targets of 65..1023 labels: the kernel above with SPT states per thread, state s = threadIdx.x + j NT (j < SPT), so
-// that S <= 2047 fits 1024 threads.  Every state of a frame reads the previous frame's row in buf: one barrier per frame.
-// (A loop over one state per thread schedules differently from the kernel above, which keeps its code for <= 64 labels.)
 template <int SMAX, int NT>
-__global__ void __launch_bounds__(NT) ctc_alpha_beta_multi_kernel(const float* __restrict__ logp, int ldl, int T, const int* __restrict__ in_len,
+__global__ void __launch_bounds__(NT) ctc_alpha_beta_kernel(const float* __restrict__ logp, int ldl, int T, const int* __restrict__ in_len,
                                                             const long long* __restrict__ targets, int ldt,
                                                             const int* __restrict__ tgt_len, int blank, int V, float* __restrict__ nll,
                                                             float* __restrict__ ws, int S_ws) {
     constexpr int SPT = (SMAX + NT - 1) / NT;
-    __shared__ int lab[SMAX + 2];
-    __shared__ float buf[2][SMAX + 2];
+    __shared__ float buf[2][SMAX];
     const int b = blockIdx.x;
     const int L = min(tgt_len[b], (SMAX - 1) / 2);
     const int S = 2 * L + 1;
     const int Tb = min(in_len[b], T);
-#pragma unroll
-    for (int j = 0; j < SPT; ++j) {
-        const int s = threadIdx.x + j * NT;
-        if (s < S + 2) {
-            int l = blank;
-            if (s < S && (s & 1)) {
-                long long v = targets[(size_t)b * ldt + (s >> 1)];
-                l = (v < 0 || v >= V) ? blank : (int)v;
-            }
-            lab[s] = l;
-        }
-    }
-    __syncthreads();
-    const float* lp = logp + (size_t)b * T * ldl;
-    float* w = ws + (size_t)b * T * S_ws;
     if (Tb < 1) {   // no frames: infeasible unless the target is empty too (PyTorch: inf -> 0 with zero_infinity)
         if (threadIdx.x == 0) nll[b] = INFINITY;
         return;
     }
-    int my[SPT];
-    bool skip_ok[SPT];
-    float a[SPT];
-    // ---- forward variables
+    const long long* tg = targets + (size_t)b * ldt;
+    const auto label = [&](int i) {     // an out-of-range label counts as the blank
+        const long long v = tg[i];
+        return (v < 0 || v >= V) ? blank : (int)v;
+    };
+    const float* lp = logp + (size_t)b * T * ldl;
+    float* w = ws + (size_t)b * T * S_ws;
+    unsigned col[SPT];
+    bool skip[SPT];
+    // ---- forward variables, from frame -1
 #pragma unroll
     for (int j = 0; j < SPT; ++j) {
-        const int s = threadIdx.x + j * NT;
-        my[j] = (s < S) ? lab[s] : blank;
-        skip_ok[j] = (s >= 2 && s < S && my[j] != blank && my[j] != lab[s - 2]);
-        a[j] = -INFINITY;
-        if (s == 0) a[j] = lp[blank];
-        if (s == 1 && S > 1) a[j] = lp[my[j]];
-        if (s < S) { buf[0][s] = a[j]; w[s] = a[j]; }
+        const int s = trellis_state(j, NT);
+        col[j] = trellis_col(s, S, blank, label);
+        skip[j] = trellis_skip(s, S, blank, label);
+        if (s < S) buf[0][s] = s == 0 ? 0.f : -INFINITY;
     }
     __syncthreads();
     int cur = 0;
-    for (int t = 1; t < Tb; ++t) {
-#pragma unroll
-        for (int j = 0; j < SPT; ++j) {
-            const int s = threadIdx.x + j * NT;
-            if (s < S) {
-                float v = buf[cur][s];
-                if (s >= 1) v = log_add(v, buf[cur][s - 1]);
-                if (skip_ok[j]) v = log_add(v, buf[cur][s - 2]);
-                a[j] = (v == -INFINITY) ? -INFINITY : v + lp[(size_t)t * ldl + my[j]];
-                buf[cur ^ 1][s] = a[j];
-                w[(size_t)t * S_ws + s] = a[j];
-            }
-        }
-        cur ^= 1;
-        __syncthreads();
-    }
-    float total = buf[cur][S - 1];
-    if (S > 1) total = log_add(total, buf[cur][S - 2]);
+    for (int t = 0; t < Tb; ++t)
+        trellis_step<TrellisLogAdd>(
+            buf, cur, NT, S, skip, [&](int j) { return lp[(size_t)t * ldl + col[j]]; },
+            [&](int, int s, TrellisLogAdd, float v) { w[(size_t)t * S_ws + s] = v; });
+    if (threadIdx.x == 0) nll[b] = -trellis_log_total(buf[cur], S);          // +inf when no alignment exists
     __syncthreads();
-    if (threadIdx.x == 0) nll[b] = -total;          // +inf when no alignment exists
-    // ---- backward variables; ws <- alpha + beta
-    bool skip_fw[SPT];
-    float be[SPT];
+    // ---- backward variables, from frame Tb; ws <- alpha + beta
 #pragma unroll
     for (int j = 0; j < SPT; ++j) {
-        const int s = threadIdx.x + j * NT;
-        skip_fw[j] = (s + 2 < S && lab[s + 2] != blank && lab[s + 2] != my[j]);
-        be[j] = -INFINITY;
-        if (s == S - 1) be[j] = lp[(size_t)(Tb - 1) * ldl + blank];
-        if (s == S - 2 && S > 1) be[j] = lp[(size_t)(Tb - 1) * ldl + my[j]];
-        if (s < S) {
-            buf[0][s] = be[j];
-            w[(size_t)(Tb - 1) * S_ws + s] += be[j];
-        }
+        const int s = trellis_state(j, NT);
+        skip[j] = trellis_skip(s + 2, S, blank, label);
+        if (s < S) buf[0][s] = s == S - 1 ? 0.f : -INFINITY;
     }
     __syncthreads();
     cur = 0;
-    for (int t = Tb - 2; t >= 0; --t) {
-#pragma unroll
-        for (int j = 0; j < SPT; ++j) {
-            const int s = threadIdx.x + j * NT;
-            if (s < S) {
-                float v = buf[cur][s];
-                if (s + 1 < S) v = log_add(v, buf[cur][s + 1]);
-                if (skip_fw[j]) v = log_add(v, buf[cur][s + 2]);
-                be[j] = (v == -INFINITY) ? -INFINITY : v + lp[(size_t)t * ldl + my[j]];
-                buf[cur ^ 1][s] = be[j];
-                w[(size_t)t * S_ws + s] += be[j];
-            }
-        }
-        cur ^= 1;
-        __syncthreads();
-    }
+    for (int t = Tb - 1; t >= 0; --t)
+        trellis_step<TrellisLogAdd, true>(
+            buf, cur, NT, S, skip, [&](int j) { return lp[(size_t)t * ldl + col[j]]; },
+            [&](int, int s, TrellisLogAdd, float v) { w[(size_t)t * S_ws + s] += v; });
 }
 
 // loss = mean_b (finite nll_b ? nll_b / max(tgt_len_b, 1) : 0)   (single CTA)
@@ -315,9 +190,9 @@ const char* ctc_launch(cudaStream_t st, const float* logp, int ldl, int B, int T
     const int S_ws = 2 * max_tgt + 1;
     const bool lng = S_ws > CTC_SMAX;
     const char* err;
-    if ((err = lng ? launch<ctc_alpha_beta_multi_kernel<CTC_SMAX_LONG, 1024>>(B, 1024, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len,
+    if ((err = lng ? launch<ctc_alpha_beta_kernel<CTC_SMAX_LONG, 1024>>(B, 1024, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len,
                                                                         blank, V, nll, ws, S_ws)
-                   : launch<ctc_alpha_beta_kernel>(B, 160, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len, blank,
+                   : launch<ctc_alpha_beta_kernel<CTC_SMAX, 160>>(B, 160, 0, st, logp, ldl, T, in_len, targets, ldt, tgt_len, blank,
                                                                   V, nll, ws, S_ws)))
         return err;
     if ((err = launch<ctc_mean_kernel>(1, 256, 0, st, nll, tgt_len, B, loss))) return err;

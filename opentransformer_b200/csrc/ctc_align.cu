@@ -1,13 +1,12 @@
 // CTC forced alignment: the best (Viterbi) path of each utterance through the CTC trellis of its target, on fp32 log-probs
 // (or logits with a per-frame log-sum-exp).  One CTA per utterance; DESIGN.md 4.8 states the layout, tie-break and limits.
 //
-//   l' = blank-extended target (state s: blank for even s, token s / 2 for odd s), S = 2 L + 1
-//   delta_t(s) = max(delta_{t-1}(s), delta_{t-1}(s-1), delta_{t-1}(s-2) if l'_s != blank and l'_s != l'_{s-2}) + lp_t(l'_s)
-//   with delta_{-1}(0) = 0 and every other delta_{-1} = -inf, so that frame 0 is the recursion's first step.
+//   delta_t(s) = the best of s's predecessors in the trellis (ctc_trellis.cuh) at frame t - 1, + lp_t(l'_s)
 //   end = S-1 unless delta(S-2) > delta(S-1); the path is walked back through the choices (0, 1 or 2 back) in bp.
 #include <math.h>
 #include <stdint.h>
 
+#include "ctc_trellis.cuh"
 #include "launch.cuh"
 #include "otb_internal.h"
 
@@ -23,12 +22,12 @@ __global__ void __launch_bounds__(ALIGN_THREADS_MAX, 1) ctc_align_kernel(
     const long long* __restrict__ targets, int ldt, const int* __restrict__ tgt_len, int max_tgt, int blank,
     uint8_t* bp_all, int* labels_all, float* __restrict__ frame_scores, int* __restrict__ spans, float* __restrict__ path_score) {
     __shared__ float delta[2][ALIGN_SMAX];
-    __shared__ int bad;
     __shared__ int end_state;
     const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
     const int L = tgt_len[b];
     const int Tb = max(0, min(in_len[b], T));
-    const int S = 2 * L + 1, S_ws = 2 * max_tgt + 1;
+    const bool Lok = L >= 0 && L <= max_tgt && (L == 0 || Tb > 0);
+    const int S = Lok ? 2 * L + 1 : 0, S_ws = 2 * max_tgt + 1;
     const long long* tg = targets + (size_t)b * ldt;
     const float* x = rows + (size_t)b * T * ld;
     const float* ls = lse ? lse + (size_t)b * T : nullptr;
@@ -37,68 +36,44 @@ __global__ void __launch_bounds__(ALIGN_THREADS_MAX, 1) ctc_align_kernel(
     float* fsc = frame_scores + (size_t)b * T;
     int* sp = spans + (size_t)b * max_tgt * 2;
 
-    const bool Lok = L >= 0 && L <= max_tgt && (L == 0 || Tb > 0);
-    if (tid == 0) bad = !Lok;
-    __syncthreads();
-    // ---- each thread's states s = tid + k nt: the column it reads and whether it may skip the blank before it
-    int col[ALIGN_PER_THREAD];
-    bool skip[ALIGN_PER_THREAD], live[ALIGN_PER_THREAD];
+    bool bad = !Lok;
+    for (int i = tid; i < (S >> 1); i += nt) {
+        const long long v = tg[i];
+        bad |= v < 0 || v >= V || v == blank;       // a blank or out-of-range token: no alignment exists
+    }
+    const auto label = [&](int i) { return (int)tg[i]; };
+    unsigned col[ALIGN_PER_THREAD];
+    bool skip[ALIGN_PER_THREAD];
 #pragma unroll
     for (int k = 0; k < ALIGN_PER_THREAD; ++k) {
-        const int s = tid + k * nt;
-        live[k] = Lok && s < S;
-        col[k] = blank;
-        skip[k] = false;
-        if (live[k] && (s & 1)) {
-            const long long v = tg[s >> 1];
-            if (v < 0 || v >= V || v == blank) bad = 1;      // a blank or out-of-range token: no alignment exists
-            else {
-                col[k] = (int)v;
-                skip[k] = s >= 3 && tg[(s >> 1) - 1] != v;
-            }
-        }
-        if (s < S_ws) delta[0][s] = s == 0 ? 0.f : -INFINITY;       // frame -1
+        const int s = trellis_state(k, nt);
+        col[k] = trellis_col(s, S, blank, label);
+        skip[k] = trellis_skip(s, S, blank, label);
+        if (s < S) delta[0][s] = s == 0 ? 0.f : -INFINITY;       // frame -1
     }
-    __syncthreads();
-    const bool ok = !bad;
+    const bool ok = !__syncthreads_or(bad);
     int cur = 0;
     if (ok && Tb > 0) {
         float v[ALIGN_PER_THREAD], nv[ALIGN_PER_THREAD];
         float m = ls ? ls[0] : 0.f, nm = 0.f;
 #pragma unroll
-        for (int k = 0; k < ALIGN_PER_THREAD; ++k) v[k] = live[k] ? x[col[k]] : 0.f;
+        for (int k = 0; k < ALIGN_PER_THREAD; ++k) v[k] = trellis_state(k, nt) < S ? x[col[k]] : 0.f;
         for (int t = 0; t < Tb; ++t) {
             // the gather of frame t + 1: only the columns of this thread's states, in flight across this frame's barrier
             if (t + 1 < Tb) {
                 const float* xn = x + (size_t)(t + 1) * ld;
 #pragma unroll
-                for (int k = 0; k < ALIGN_PER_THREAD; ++k) nv[k] = live[k] ? xn[col[k]] : 0.f;
+                for (int k = 0; k < ALIGN_PER_THREAD; ++k) nv[k] = trellis_state(k, nt) < S ? xn[col[k]] : 0.f;
                 if (ls) nm = ls[t + 1];
             }
-            const float* d = delta[cur];
-            float* dn = delta[cur ^ 1];
-            uint8_t* bpt = bp + (size_t)t * S_ws;
-#pragma unroll
-            for (int k = 0; k < ALIGN_PER_THREAD; ++k) {
-                if (!live[k]) continue;
-                const int s = tid + k * nt;
-                // prefer staying, then one back, then two back: a later choice must be strictly better
-                float best = d[s];
-                int c = 0;
-                if (s >= 1 && d[s - 1] > best) { best = d[s - 1]; c = 1; }
-                if (skip[k] && d[s - 2] > best) { best = d[s - 2]; c = 2; }
-                dn[s] = best + (v[k] - m);
-                bpt[s] = (uint8_t)c;
-            }
-            cur ^= 1;
-            __syncthreads();
+            trellis_step<TrellisMax>(delta, cur, nt, S, skip, [&](int k) { return v[k] - m; },
+                                     [&](int, int s, TrellisMax c, float) { bp[(size_t)t * S_ws + s] = (uint8_t)c.c; });
 #pragma unroll
             for (int k = 0; k < ALIGN_PER_THREAD; ++k) v[k] = nv[k];
             m = nm;
         }
     }
     // ---- the end state and the walk back (one thread: T_b dependent byte loads); spans of the odd states on the way
-    const int Lp = max(0, min(L, max_tgt));
     if (tid == 0) {
         float score = ok && Tb == 0 ? 0.f : -INFINITY;      // L == 0 and no frames: the empty path
         int e = -1;
@@ -136,7 +111,7 @@ __global__ void __launch_bounds__(ALIGN_THREADS_MAX, 1) ctc_align_kernel(
         fsc[t] = sc;
     }
     for (int i = tid; i < max_tgt; i += nt)
-        if (!found || i >= Lp) { sp[2 * i] = -1; sp[2 * i + 1] = -1; }
+        if (!found || i >= L) { sp[2 * i] = -1; sp[2 * i + 1] = -1; }
 }
 
 const char* ctc_align_launch(cudaStream_t st, const float* rows, int ld, int B, int T, int V, const float* lse, const int* in_len,

@@ -1,19 +1,17 @@
 // CTC rescoring of an attention n-best (DESIGN.md 4.18): out[r] = log p_ctc(target_r | x_b), b = r / K, of B*K target rows
 // over the utterance's shared log-prob matrix (no per-row copy of it).
 //   ctc_nbest_score_kernel  one CTA per target row, the K rows of an utterance in adjacent CTAs (they read the same frames,
-//                           so the per-frame label gather is served by L2).  The blank-extended forward recursion over the
-//                           S = 2 L + 1 states in the log domain and in fp32: alpha stays in registers (SPT states per
-//                           thread, s = threadIdx.x + j NT) and a two-row shared buffer hands each frame's values to the
-//                           states s + 1 and s + 2 -- one barrier per frame.  Each thread keeps the emission log-probs of
-//                           the next PF frames in flight, so the gather's L2 latency is not paid at every barrier.
-//                           Forward only: no beta, no [rows, T, S] scratch.
+//                           so the per-frame label gather is served by L2): the forward pass over the trellis
+//                           (ctc_trellis.cuh) in the log domain and in fp32.  Each thread keeps the emission log-probs of
+//                           its states for the next PF frames in flight, so the gather's L2 latency is not paid at every
+//                           barrier.  Forward only: no beta, no [rows, T, S] scratch.
 // L is the number of labels before the row's first negative entry.  A row gets -inf when no alignment exists: a label equal
 // to the blank or outside [0, V), an utterance with no frames, or too few frames for the labels and their repeats.
 #include <math.h>
 
+#include "ctc_trellis.cuh"
 #include "launch.cuh"
 #include "otb_internal.h"
-#include "ptx.cuh"
 
 namespace otb {
 
@@ -44,46 +42,34 @@ __global__ void __launch_bounds__(NT) ctc_nbest_score_kernel(const float* __rest
     }
     const int S = 2 * L + 1;
     const float* lp = logp + (size_t)b * T * ld;
-    int my[SPT];
-    bool skip_ok[SPT];
-    float a[SPT];
+    const auto label = [&](int i) { return y[i]; };
+    unsigned col[SPT];
+    bool skip[SPT];
     float e[CTC_SCORE_PF][SPT];     // e[d][j]: emission of state j at the frame the d-th step of an unrolled round reads
 #pragma unroll
     for (int j = 0; j < SPT; ++j) {
-        const int s = threadIdx.x + j * NT;
-        const bool lab = s < S && (s & 1);
-        my[j] = lab ? y[s >> 1] : blank;
-        skip_ok[j] = lab && s >= 3 && my[j] != y[(s >> 1) - 1];
-        a[j] = (s == 0) ? lp[blank] : (s == 1) ? lp[my[j]] : -INFINITY;
-        if (s < S) buf[0][s] = a[j];
+        const int s = trellis_state(j, NT);
+        col[j] = trellis_col(s, S, blank, label);
+        skip[j] = trellis_skip(s, S, blank, label);
+        if (s < S) buf[0][s] = s == 0 ? 0.f : -INFINITY;      // frame -1
 #pragma unroll
-        for (int d = 0; d < CTC_SCORE_PF; ++d) e[d][j] = (s < S && 1 + d < Tb) ? lp[(size_t)(1 + d) * ld + my[j]] : 0.f;
+        for (int d = 0; d < CTC_SCORE_PF; ++d) e[d][j] = (s < S && d < Tb) ? lp[(size_t)d * ld + col[j]] : 0.f;
     }
     __syncthreads();
     int cur = 0;
-    for (int t0 = 1; t0 < Tb; t0 += CTC_SCORE_PF) {
+    for (int t0 = 0; t0 < Tb; t0 += CTC_SCORE_PF) {
 #pragma unroll
         for (int d = 0; d < CTC_SCORE_PF; ++d) {
             const int t = t0 + d;
             if (t >= Tb) break;        // uniform over the CTA
-#pragma unroll
-            for (int j = 0; j < SPT; ++j) {
-                const int s = threadIdx.x + j * NT;
-                if (s < S) {
-                    const float em = e[d][j];
-                    if (t + CTC_SCORE_PF < Tb) e[d][j] = lp[(size_t)(t + CTC_SCORE_PF) * ld + my[j]];
-                    float v = a[j];
-                    if (s >= 1) v = log_add(v, buf[cur][s - 1]);
-                    if (skip_ok[j]) v = log_add(v, buf[cur][s - 2]);
-                    a[j] = (v == -INFINITY) ? -INFINITY : v + em;
-                    buf[cur ^ 1][s] = a[j];
-                }
-            }
-            cur ^= 1;
-            __syncthreads();
+            trellis_step<TrellisLogAdd>(buf, cur, NT, S, skip, [&](int j) {
+                const float em = e[d][j];
+                if (t + CTC_SCORE_PF < Tb) e[d][j] = lp[(size_t)(t + CTC_SCORE_PF) * ld + col[j]];
+                return em;
+            }, [](int, int, TrellisLogAdd, float) {});
         }
     }
-    if (threadIdx.x == 0) out[r] = S > 1 ? log_add(buf[cur][S - 1], buf[cur][S - 2]) : buf[cur][0];
+    if (threadIdx.x == 0) out[r] = trellis_log_total(buf[cur], S);
 }
 
 const char* ctc_nbest_score_launch(cudaStream_t st, const float* logp, int ld, int B, int T, int V, const int* in_len,

@@ -186,7 +186,8 @@ __device__ __forceinline__ float warp_max(float v) {
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
-// log(e^a + e^b) in fp32, exact at -inf: the CTC log-add (csrc/ctc.cu's loss, csrc/ctc_decode.cu's prefix beam search)
+// log(e^a + e^b) in fp32, exact at -inf: the CTC log-add (csrc/ctc_trellis.cuh's sum over paths for the loss and the n-best
+// score, csrc/ctc_decode.cu's prefix beam search)
 __device__ __forceinline__ float log_add(float a, float b) {
     if (a == -INFINITY) return b;
     if (b == -INFINITY) return a;
