@@ -1121,6 +1121,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
 #pragma unroll
                     for (int q = 0; q < 8; ++q) lmax = fmaxf(lmax, fmaxf(fmaxf(v[q].x, v[q].y), fmaxf(v[q].z, v[q].w)));
                 }
+                if (ul == j) DG_STAMP3(52);
                 const float rowmax = warp_max(lmax);
                 float T = -INFINITY;
                 {
@@ -1136,10 +1137,12 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                 // pass 2: sum of exp(x - max) (ex2.approx on a pre-scaled argument: 2 instructions per element, relative error
                 // 2^-22 -- the log-sum-exp moves by ~1e-7) and the candidates >= T; one ballot per 128 elements decides whether
                 // any lane has to look at its four values at all
+                if (ul == j) DG_STAMP3(53);
                 const float l2e = 1.4426950408889634f, nm = -rowmax * l2e;
                 float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
                 int ncand = 0;
-                // (a separate, unrolled sum pass in front of the candidate pass was tried: 22.7 k -> 25.5 k cycles)
+                // (a separate, unrolled sum pass in front of the candidate pass was tried: 22.7 k -> 25.5 k cycles; four 32-wide
+                // rounds per trip, their loads in flight together and one ballot skipping all four, left it at 9-10 k cycles per row)
                 for (int base = 0; base < ldv4; base += 32) {        // warp-uniform trip count: whole warps take part in the ballots
                     const int i0 = base + lane;
                     const float4 v = (i0 < ldv4) ? x4[(size_t)i0 * xs4] : ninf4;
@@ -1163,6 +1166,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                         }
                     }
                 }
+                if (ul == j) DG_STAMP3(54);
                 float sum = (s0 + s1) + (s2 + s3);
                 sum = warp_sum(sum);
                 const float lse = rowmax + logf(sum);
@@ -1215,6 +1219,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) decode_group_kernel(const __gri
                         if (lane == 0) { ms.row_v[r][k] = bv; ms.row_i[r][k] = bi; }
                     }
                 }
+                if (ul == j) DG_STAMP3(55);
                 // finished hypotheses keep emitting EOS at no cost (mask_finished_scores / mask_finished_preds, speech2text.py:156-192);
                 // candidate scores = scores + last_k_scores (:118)
                 __syncwarp();

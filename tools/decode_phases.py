@@ -61,6 +61,8 @@ with torch.no_grad():
             return [int(x) for x in (sub[:, b] - sub[:, a]).tolist()]
         print('    layer 2 W_o block, per CTA: rows in', dd(9, 10), 'GEMM', dd(10, 11))
         print('    beam step, per CTA: beam^2 top-k', dd(30, 31)[:12], 'ancestry', dd(31, 32)[:12], 'sync', dd(32, 33)[:12], 'state', dd(33, 35)[:12])
+        print('    row top-k of hypothesis 0, per CTA: lane maxima', [int(x) for x in (sub[:, 52] - allt[:, n - 4]).tolist()][:12],
+              'threshold', dd(52, 53)[:12], 'sum + candidates', dd(53, 54)[:12], 'ranking', dd(54, 55)[:12])
         print('    layer 2 self-attention, warp 0 task 1, per CTA: ancestry+q', dd(39, 40)[:6], 'issue 2 halves', dd(40, 41)[:6], 'wait half 0', dd(41, 42)[:6],
               'compute', dd(42, 43)[:6], 'wait half 1', dd(43, 44)[:6], 'compute', dd(44, 45)[:6], 'wait half 2', dd(45, 46)[:6], 'compute', dd(46, 47)[:6],
               'wait half 3', dd(47, 48)[:6], 'compute', dd(48, 49)[:6], 'merge+store', dd(50, 51)[:6])
