@@ -286,7 +286,8 @@ int otb_attention_bwd(const void* q, int ldq, int q_rows, const void* k, int ldk
 int otb_dropout_add(const void* x, int ldx, const void* resid, int ldr, void* out, int ldo, int M, int N, float alpha, float p,
                     const uint32_t* seed, uint32_t site, const int32_t* row_len, int row_period, void* stream);
 /* Conformer convolution module, middle part, in training mode (module/conformer.py:46-52): x bf16 [B*T, d] = GLU output, read as
- * zero on padded frames (t >= len[b]); c f32 [B*T, d] = depthwise_conv(x) + wb (w f32 [d, k] as nn.Conv1d stores it, k odd,
+ * zero on padded frames (t >= min(len[b], T): a length above T means every frame is valid, and no conv tap reads past the
+ * utterance's T rows); c f32 [B*T, d] = depthwise_conv(x) + wb (w f32 [d, k] as nn.Conv1d stores it, k odd,
  * wb may be NULL); BatchNorm with batch statistics over all B*T rows -> stats f32 [2, d] = (mean, 1/sqrt(biased var + eps));
  * running_mean / running_var (optional) updated with `momentum` and the unbiased variance, *num_batches (optional) += 1;
  * out bf16 [B*T, d] = swish(BN(c)), zero on padded frames. */
@@ -294,8 +295,8 @@ int otb_conformer_conv_train(const void* x, const int32_t* len, const float* w, 
                              float* running_mean, float* running_var, int64_t* num_batches, float momentum, float eps, float* c,
                              float* stats, void* out, int B, int T, int d, int k, void* stream);
 /* Its backward: dy bf16 [B*T, d] (gradient of out), x / c / stats as the forward left them; red f32 [2, d] and dc f32 [B*T, d]
- * are scratch.  dx bf16 [B*T, d] (zero on padded frames); dw f32 [d, k], dwb f32 [d] (NULL without conv bias), dgamma, dbeta
- * f32 [d]: overwritten, or added to with accumulate != 0. */
+ * are scratch; lengths are clamped to T as in the forward.  dx bf16 [B*T, d] (zero on padded frames); dw f32 [d, k], dwb
+ * f32 [d] (NULL without conv bias), dgamma, dbeta f32 [d]: overwritten, or added to with accumulate != 0. */
 int otb_conformer_conv_bwd(const void* dy, const void* x, const int32_t* len, const float* w, const float* gamma, const float* beta,
                            const float* c, const float* stats, float* red, float* dc, void* dx, float* dw, float* dwb, float* dgamma,
                            float* dbeta, int accumulate, int B, int T, int d, int k, void* stream);

@@ -43,7 +43,10 @@ __device__ __forceinline__ void store8(bf16* p, const float (&v)[8]) {
     u.x = pack_bf16(v[0], v[1]); u.y = pack_bf16(v[2], v[3]); u.z = pack_bf16(v[4], v[5]); u.w = pack_bf16(v[6], v[7]);
     *reinterpret_cast<uint4*>(p) = u;
 }
-__device__ __forceinline__ bool row_valid(const int* len, int row, int T) { return row % T < len[row / T]; }
+// Valid frames of an utterance: t < min(len, T).  A length above T means every frame is valid; the conv taps are bounded by
+// the clamped length too, so they never read the next utterance's rows (or past the buffer, for the last one).
+__device__ __forceinline__ int valid_len(const int* len, int row, int T) { return min(len[row / T], T); }
+__device__ __forceinline__ bool row_valid(const int* len, int row, int T) { return row % T < valid_len(len, row, T); }
 
 // Sum the 8 row lanes' partials of this CTA and add them to out[col .. col + 8) (one atomic per channel and CTA).
 __device__ __forceinline__ void reduce_add(float (&red)[RL][256], const float (&acc)[8], float* out, int d) {
@@ -71,7 +74,7 @@ __global__ void __launch_bounds__(256) dwconv_sum_kernel(const bf16* __restrict_
     float sum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (col < d) {
         for (int row = blockIdx.y * RL + rl; row < M; row += gridDim.y * RL) {
-            const int t = row % T, n = len[row / T];
+            const int t = row % T, n = valid_len(len, row, T);
             float acc[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) acc[j] = wb ? wb[col + j] : 0.f;
@@ -257,7 +260,7 @@ __global__ void __launch_bounds__(256) dwconv_wgrad_kernel(const float* __restri
                 continue;
             }
             const int tt = row % T + tap - pad;
-            if (tt < 0 || tt >= len[row / T]) continue;
+            if (tt < 0 || tt >= valid_len(len, row, T)) continue;
             float v[8];
             load8(x + (size_t)(row + tap - pad) * d + col, v);
 #pragma unroll
