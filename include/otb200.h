@@ -393,6 +393,14 @@ int otb_fbank(const float* wave, int ld_wave, const int32_t* n_samples, const fl
  * frames stay zero.  gmean 0 / gstd 1 leave x as it is and only add the noise. */
 int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, const float* gmean, const float* gstd, const float* noise,
                  void* stream);
+/* Band-limited resampling, one rate pair per row (speed perturbation, data/audio.py:63-67,106-110, and audio at another
+ * rate): row b of y equals torchaudio.functional.resample(x[b, :n_in[b]], orig[b], new_rate[b]) with its defaults
+ * (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99).  x f32 [B, ldx] (only the first n_in[b] <= ldx samples of a row
+ * are read), 1 <= B <= 65535; orig / new_rate i32 [B] on the device; y f32 [B, ldy], width <= ldy columns written; n_out i32 [B] = ceil(n *
+ * n_in / o) with o / n the rates divided by their gcd, at most width (a row longer than width is cut there); columns from
+ * n_out[b] to width are zero.  Rows with orig == new_rate are copied bit for bit; rows with a rate <= 0 are empty. */
+int otb_resample(const float* x, int ldx, const int32_t* n_in, const int32_t* orig, const int32_t* new_rate, float* y, int ldy,
+                 int32_t* n_out, int B, int width, void* stream);
 
 /* Joint-CTC loss of SpeechToText.forward (model/speech2text.py:60-72 -> CTCAssistor.compute_loss, model/ctc.py:48-52):
  * nn.CTCLoss(blank, reduction 'mean', zero_infinity = True) and its gradient with respect to the LOGITS.

@@ -94,6 +94,7 @@ _SIGS = {
     'otb_frame_stack': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, c_float, _P, _P]),
     'otb_fbank': (c_int, [_P, c_int, _P, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
     'otb_utt_cmvn': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
+    'otb_resample': (c_int, [_P, c_int, _P, _P, _P, _P, c_int, _P, c_int, c_int, _P]),
     'otb_ctc_loss': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, c_int, c_int, _P, _P, _P, _P, c_int, c_float, _P,
                              _P]),
     'otb_ctc_frame_topk': (c_int, [_P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P]),

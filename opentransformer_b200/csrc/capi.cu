@@ -523,6 +523,14 @@ int otb_utt_cmvn(float* x, int B, int Tmax, int F, const int32_t* n_frames, cons
     RET("otb_utt_cmvn", utt_cmvn_launch(ST(stream), x, B, Tmax, F, n_frames, gmean, gstd, noise));
 }
 
+int otb_resample(const float* x, int ldx, const int32_t* n_in, const int32_t* orig, const int32_t* new_rate, float* y, int ldy,
+                 int32_t* n_out, int B, int width, void* stream) {
+    if (!x || !n_in || !orig || !new_rate || !y || !n_out) return fail("otb_resample", "null operand");
+    if (B < 1 || width < 1) return fail("otb_resample", "need B >= 1 and width >= 1");
+    if (ldx < 1 || ldy < width) return fail("otb_resample", "row pitch smaller than the row");
+    RET("otb_resample", resample_launch(ST(stream), x, ldx, n_in, orig, new_rate, y, ldy, n_out, B, width));
+}
+
 int otb_ctc_loss(const float* logp, int ldl, int B, int T, int V, const int32_t* in_len, const int64_t* targets, int ldt,
                  const int32_t* tgt_len, int max_tgt, int blank, float* nll, float* loss, float* ws, void* dlogits_bf16, int ldd,
                  float grad_scale, const float* grad_scale_dev, void* stream) {

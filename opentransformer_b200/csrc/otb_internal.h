@@ -301,6 +301,8 @@ const char* fbank_launch(cudaStream_t st, const float* wave, int ld_wave, const 
                          int frame_shift, float preemph);
 const char* utt_cmvn_launch(cudaStream_t st, float* x, int B, int Tmax, int F, const int* n_frames, const float* gmean, const float* gstd,
                             const float* noise);
+const char* resample_launch(cudaStream_t st, const float* x, int ldx, const int* n_in, const int* orig, const int* new_rate, float* y,
+                            int ldy, int* n_out, int B, int width);
 
 // LSTM recurrence (lstm.cu): units per CTA, grid and dynamic shared memory of the two persistent kernels for hidden size H
 struct LstmPlan {

@@ -11,8 +11,9 @@ Mirror of what otrans/data/audio.py:112-136 does on DataLoader worker CPUs per u
 batched on the device (csrc/fbank.cu): at thousands of utterances per second per GPU the CPU front end is the next wall.
 The mel filterbank follows Kaldi's definition as published by torchaudio.compliance.kaldi.get_mel_banks (mel(f) = 1127
 ln(1 + f / 700), num_bins + 2 equally spaced mel points between low_freq and Nyquist, triangles over the first N/2 FFT bins).
-The FFT has round_to_power_of_two(frame_len) points, at most 2048 (25 ms frames at sample rates up to 81.9 kHz).  One
-extractor serves one sample rate.
+The FFT has round_to_power_of_two(frame_len) points, at most 2048 (25 ms frames at sample rates up to 81.9 kHz).  The
+features are at the extractor's sample rate; input at other rates, given per row, is resampled to it on the device
+(csrc/resample.cu) in the same pass as speed perturbation.
 """
 import math
 
@@ -23,6 +24,7 @@ from . import _lib, augment, ops
 from ._lib import check
 
 MAX_FFT = 2048          # csrc/fbank.cu: shared-memory buffers of one frame
+SPEEDS = (0.9, 1.0, 1.1)  # speed perturbation ratios, otrans/data/audio.py:106 random.choice([0.9, 1.0, 1.1])
 
 
 def _mel(f):
@@ -60,15 +62,18 @@ class FbankExtractor:
     what collate_fn_with_eos_bos builds (data/loader.py:66-108): features f32 [B, Tmax, F] zero padded, feature lengths,
     bool mask [B, Tmax].
 
-    ``volume_perturb`` scales each waveform by 10 ** (U(-1.6, 1.6) / 20) before the fbank, ``gaussian_noise`` = sigma adds one
-    N(0, sigma) vector of F values per utterance to its valid frames after CMVN, and ``spec_augment`` masks bands last with
-    ``augment.spec_augment_`` (``spec_augment_config`` are its keyword arguments).  The gains and the noise are drawn on the
-    device from ``generator`` (a CUDA torch.Generator; torch's default one if None); SpecAugment draws its bands on the host
-    with the reference's RNG calls.  All three are off by default."""
+    ``speed_perturb`` resamples each waveform from sample_rate to int(sample_rate * ratio), ratio drawn from SPEEDS
+    (0.9, 1.0, 1.1), and computes the fbank at sample_rate, as the reference's commented-out speed perturbation does
+    (otrans/data/audio.py:63-67,106-110); ``volume_perturb`` scales each waveform by 10 ** (U(-1.6, 1.6) / 20) before the
+    fbank, ``gaussian_noise`` = sigma adds one N(0, sigma) vector of F values per utterance to its valid frames after CMVN,
+    and ``spec_augment`` masks bands last with ``augment.spec_augment_`` (``spec_augment_config`` are its keyword
+    arguments).  The speeds, the gains and the noise are drawn on the device from ``generator`` (a CUDA torch.Generator;
+    torch's default one if None), in that order; SpecAugment draws its bands on the host with the reference's RNG calls.
+    All four are off by default."""
 
     def __init__(self, num_mel_bins=80, sample_rate=16000, frame_length_ms=25.0, frame_shift_ms=10.0, preemphasis=0.97,
                  normalization=True, global_mean=None, global_std=None, device=None, volume_perturb=False, gaussian_noise=0.0,
-                 spec_augment=False, spec_augment_config=None, generator=None):
+                 spec_augment=False, spec_augment_config=None, generator=None, speed_perturb=False):
         self.F, self.sr = num_mel_bins, sample_rate
         self.frame_len = int(sample_rate * frame_length_ms * 0.001)
         self.frame_shift = int(sample_rate * frame_shift_ms * 0.001)
@@ -92,14 +97,19 @@ class FbankExtractor:
         self.spec_augment = bool(spec_augment)
         self.spec_augment_config = dict(spec_augment_config or {})
         self.generator = generator
+        self.speed_perturb = bool(speed_perturb)
+        # target rates of the three speeds, from float64 on the host as the reference computes them
+        self.speed_rates = [int(sample_rate * s) for s in SPEEDS]
+        self._speed_rates_d = None
 
     @classmethod
     def from_config(cls, data_params, sample_rate=16000, is_eval=False, device=None):
         """The extractor AudioDataset(data_params, ..., is_eval) stands for (otrans/data/audio.py:31-73): num_mel_bins,
         normalization with the optional global_cmvn prefix (<prefix>.mean.npy / .std.npy), and in training spec_augment
         (+ spec_augment_config), volume_perturb and gaussian_noise.  speed_perturb is accepted and ignored, as the reference
-        has it commented out.  The reference calls spec_augment(feature) with its defaults; the shipped configs set the same
-        values, and here spec_augment_config is passed on."""
+        has it commented out; to speed-perturb, pass ``speed_perturb=True`` to the constructor.  The reference calls
+        spec_augment(feature) with its defaults; the shipped configs set the same values, and here spec_augment_config is
+        passed on."""
         p = data_params
         kind = p.get('feature_extractor', 'torchaudio')
         if kind in ('psf', 'python_speech_feature'):
@@ -120,9 +130,52 @@ class FbankExtractor:
     def n_frames(self, n_samples):
         return 0 if n_samples < self.frame_len else 1 + (n_samples - self.frame_len) // self.frame_shift
 
-    def __call__(self, waves, lengths=None, gains=None, noise=None):
+    def _resample_plan(self, B, N, sample_rate, speeds):
+        """Host half of the rate / speed step -> None when no row changes rate, else (input rates [B], target rates [B] or
+        None when the speeds are drawn on the device, output width).  Raises ValueError on a bad argument."""
+        src = ops.resample_rates(self.sr if sample_rate is None else sample_rate, B, 'sample_rate')
+        if speeds is None:
+            if not self.speed_perturb:
+                if src == [self.sr] * B:
+                    return None
+                dst = [self.sr] * B
+                return self._checked(src, dst, ops.resample_width(N, src, dst))
+            if min(self.speed_rates) < 1:
+                raise ValueError(f'speed perturbation at {self.sr} Hz gives target rates {self.speed_rates}')
+            return self._checked(src, None, ops.resample_width(N, src, [max(self.speed_rates)] * B))
+        if isinstance(speeds, torch.Tensor):
+            speeds = speeds.tolist()
+        speeds = list(speeds)
+        if len(speeds) != B:
+            raise ValueError(f'speeds must be one ratio per utterance, {B}, got {len(speeds)}')
+        dst = []
+        for s in speeds:
+            try:
+                s = float(s)
+            except (TypeError, ValueError):
+                raise ValueError(f'speed ratios must be numbers, got {s!r}') from None
+            if not (s > 0.0 and math.isfinite(s)) or not 1 <= int(self.sr * s) <= ops.INT32_MAX:
+                raise ValueError(f'speed ratio {s} at {self.sr} Hz gives no positive int32 target rate')
+            dst.append(int(self.sr * s))
+        if dst == src:
+            return None
+        return self._checked(src, dst, ops.resample_width(N, src, dst))
+
+    @staticmethod
+    def _checked(src, dst, width):
+        if width > ops.INT32_MAX:
+            raise ValueError(f'resampling gives {width} samples per utterance, past int32')
+        return src, dst, width
+
+    def __call__(self, waves, lengths=None, gains=None, noise=None, sample_rate=None, speeds=None):
         """``gains`` f32 [B] (linear factors) and ``noise`` f32 [B, F] replace what volume_perturb / gaussian_noise would
-        draw, for checking exact values; either applies whether or not its option is on."""
+        draw, for checking exact values; either applies whether or not its option is on.  ``speeds`` (one ratio per
+        utterance) likewise replaces the speed_perturb draw.
+
+        ``sample_rate`` is the rate of the input, one int or one per utterance (default: the extractor's).  A row at another
+        rate is resampled to the extractor's, or, when it is also speed-perturbed, straight to int(sr * ratio) in the same
+        pass.  Order, as the reference's: resample -> volume gain (applied where the fbank loads the samples) -> fbank ->
+        CMVN + noise -> SpecAugment."""
         if isinstance(waves, (list, tuple)):
             lens = [int(w.numel()) for w in waves]
             N = max(lens)
@@ -130,9 +183,20 @@ class FbankExtractor:
             for i, w in enumerate(waves):
                 buf[i, :lens[i]] = w.reshape(-1).float()
             waves, lengths = buf, torch.tensor(lens, dtype=torch.int32)
+        plan = self._resample_plan(waves.shape[0], waves.shape[1], sample_rate, speeds)
         waves = waves.to(self.device, torch.float32).contiguous()
         lengths = lengths.to(self.device, torch.int32).contiguous()
         B, N = waves.shape
+        if plan is not None:
+            src, dst, width = plan
+            if dst is None:                     # drawn on the device, before the gains and the noise
+                if self._speed_rates_d is None:
+                    self._speed_rates_d = torch.tensor(self.speed_rates, dtype=torch.int32, device=self.device)
+                pick = torch.randint(len(SPEEDS), (B,), generator=self.generator, device=self.device)
+                dst = self._speed_rates_d[pick]
+                src = torch.tensor(src, dtype=torch.int32).to(self.device)
+            waves, lengths = ops.resample(waves, lengths, src, dst, width=width)
+            B, N = waves.shape
         if gains is None and self.volume_perturb:
             db = torch.empty(B, dtype=torch.float32, device=self.device).uniform_(-1.6, 1.6, generator=self.generator)
             gains = torch.pow(10.0, db / 20.0)

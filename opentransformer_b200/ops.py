@@ -6,6 +6,7 @@ captured into a CUDA graph (recognize.BeamDecoder captures a decode step, train.
 """
 import ctypes
 import math
+import operator
 
 import torch
 
@@ -775,6 +776,86 @@ def frame_stack(x, n, s, T2, alpha=1.0, table=None, out=None):
 
 
 CTC_LOSS_MAX_LABELS = 1023   # padded target width of otb_ctc_loss
+
+
+INT32_MAX = 2 ** 31 - 1
+
+
+def resample_rates(freq, B, name):
+    """A rate argument of resample(): an int or B of them (a sequence or a tensor, read on the host) -> list of B ints,
+    each a positive integer.  Raises ValueError otherwise."""
+    if isinstance(freq, torch.Tensor):
+        if freq.dim() == 0:
+            freq = freq.item()
+        else:
+            if freq.is_floating_point() or freq.is_complex() or freq.dtype == torch.bool:
+                raise ValueError(f'{name} must hold integer rates, got a {freq.dtype} tensor')
+            freq = freq.tolist()
+    if isinstance(freq, (list, tuple)):
+        if len(freq) != B:
+            raise ValueError(f'{name} must be one rate or {B} of them, got {len(freq)}')
+        rates = list(freq)
+    else:
+        rates = [freq] * B
+    out = []
+    for r in rates:
+        if isinstance(r, float) and r.is_integer():
+            r = int(r)
+        try:
+            if isinstance(r, bool):
+                raise TypeError
+            r = operator.index(r)
+        except TypeError:
+            raise ValueError(f'{name}: sample rates must be integers, got {r!r}') from None
+        if not 0 < r <= INT32_MAX:
+            raise ValueError(f'{name}: sample rates must be positive int32 integers, got {r}')
+        out.append(r)
+    return out
+
+
+def resample_width(N, orig, new):
+    """Columns resample() writes for a [B, N] input: the longest row's ceil(new N / orig), from host rates."""
+    return max(1, max(-(-n * N // o) for o, n in zip(orig, new)))
+
+
+def resample(x, lengths, orig_freq, new_freq, width=None):
+    """Band-limited resampling, one rate pair per row (otb_resample): x f32 [B, N] (row b's first lengths[b] samples; the
+    padding is never read), lengths i32 [B] on the device -> (out f32 [B, width], out_lengths i32 [B] on the device), row b of
+    out equal to torchaudio.functional.resample(x[b, :lengths[b]], orig[b], new[b]) at its defaults (sinc_interp_hann,
+    lowpass_filter_width 6, rolloff 0.99) and zero past out_lengths[b] = ceil(new N_b / orig).  Rows with orig == new are
+    copied bit for bit.
+
+    orig_freq / new_freq: an int, or one per row as a sequence or an integer tensor; they are checked on the host and
+    width = max over rows of ceil(new N / orig) is computed there, so nothing waits for the device.  Rates already held as
+    CUDA int32 [B] tensors are passed on as they are when ``width`` (at least every row's output length) is given, which
+    is how FbankExtractor passes speeds drawn on the device; a row with a rate <= 0 then comes out empty."""
+    on_device = width is not None and all(isinstance(f, torch.Tensor) and f.is_cuda for f in (orig_freq, new_freq))
+    if x.dim() != 2:
+        raise ValueError(f'resample: x must be [B, N], got {tuple(x.shape)}')
+    B, N = x.shape
+    if not on_device:
+        orig = resample_rates(orig_freq, B, 'orig_freq')
+        new = resample_rates(new_freq, B, 'new_freq')
+        need = resample_width(N, orig, new)
+        width = need if width is None else int(width)
+        if width < need:
+            raise ValueError(f'resample: width {width} is shorter than the longest output, {need}')
+    if not 1 <= width <= INT32_MAX:
+        raise ValueError(f'resample: {width} output samples per row is past int32')
+    _need(x, torch.float32, 'x')
+    _need(lengths, torch.int32, 'lengths')
+    if on_device:
+        rates = torch.stack([_need(orig_freq, torch.int32, 'orig_freq'), _need(new_freq, torch.int32, 'new_freq')])
+    else:
+        rates = torch.tensor([orig, new], dtype=torch.int32).to(x.device)
+    if rates.shape != (2, B) or lengths.shape != (B,):
+        raise ValueError(f'resample: rates and lengths must be [B] = [{B}]')
+    out = torch.empty(B, width, dtype=torch.float32, device=x.device)
+    out_len = torch.empty(B, dtype=torch.int32, device=x.device)
+    check(_lib.lib().otb_resample(_p(x), x.stride(0), _p(lengths), _p(rates[0]), _p(rates[1]), _p(out), width, _p(out_len), B,
+                                  width, _stream()), 'otb_resample')
+    _count()
+    return out, out_len
 
 
 def ctc_loss(logits, B, T, V, in_len, targets, tgt_len, blank=0, want_grad=False, grad_scale=1.0, scale_dev=None):
