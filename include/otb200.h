@@ -551,6 +551,43 @@ int otb_conv_col2im_relu(const void* dcol, const void* h1, void* dpre1, int B, i
 int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T, int F, int C1, int kt1, int kf1, int st1,
                     int sf1, int kt2, int kf2, int st2, int sf2, void* stream);
 
+/* ---- Transducer (RNN-T) model (DESIGN.md 4.22).  The lattice of utterance b: nodes (t, u), t < t_len[b] <= T frames and
+ * u <= u_len[b] <= U1 - 1 labels, stored padded as [B, T, U1] with u fastest; node (b, t, u) is row (b T + t) U1 + u.  Every
+ * call skips the nodes past t_len or u_len and writes zeros for them.  Blank is token 0; labels i32 [B, ldy] hold y_1 .. y_U
+ * (u_len[b] of each row count; a label outside [1, V) has no arc).
+ * otb_rnnt_joint: Hj bf16 [B T U1, D] = tanh(Ep[b T + t] + Pp[b U1 + u]) of Ep bf16 [B T, D] and Pp bf16 [B U1, D], D % 8 == 0.
+ *   t_len / u_len may be NULL: every node is valid.
+ * otb_rnnt_joint_bwd: dZ = dHj (1 - Hj^2) -> dEp bf16 [B T, D] (sum over u <= u_len) and dPp bf16 [B U1, D] (sum over
+ *   t < t_len), each in ascending order in fp32: no atomics, repeated calls are bit-identical.  D even.
+ * otb_rnnt_logprob: rows [row0, row0 + rows) of the lattice, logits f32 [rows, ld] (ld % 4 == 0, 16-byte aligned) ->
+ *   lp f32 [B T U1, 3] rows row0.. = (logsumexp, log p(blank), log p(y_{u+1}); -inf at u = u_len).
+ * otb_rnnt_loss: one CTA per utterance over lp, in fp64: alpha f64 [B T U1] scratch, nll f32 [B] the negative log-likelihood summed
+ *   over all alignments (+inf when t_len <= 0), loss f32 [1] = mean_b nll, grad f32 [B T U1, 2] = grad_scale
+ *   (* *grad_scale_dev when not NULL) / B * d nll_b / d (log p(blank), log p(y_{u+1})).  U1 <= 1024.
+ * otb_rnnt_dlogits: dz bf16 [rows, ldd] = [k = 0] a + [k = y] c - softmax(logits)_k (a + c) of the same rows, with lp's
+ *   logsumexp and (a, c) = grad of the node; columns >= V are zero.
+ * otb_rnnt_greedy_step: one step of batched greedy search over B utterances, after otb_logsoftmax_topk (k = 1) of the joint's
+ *   logits: idx i32 [B] the arg-max, logp f32 [B, ldlp] the log-probs.  A row whose frame[b] < t_len[b] takes idx, or blank
+ *   when n_sym[b] >= max_sym or n_out[b] >= max_len, and adds its log-prob to score[b].  A label goes to ids i32 [B, max_len]
+ *   at n_out[b], and the predictor state computed from it (h_new / c_new f32 [layers, B, H], pp_new bf16 [B, D]) replaces the
+ *   row's (h, c, pp); blank moves frame[b] on and copies ep bf16 [B T, D] row b T + frame[b] into ep_cur bf16 [B, D], or,
+ *   past the last frame, decrements *active.  Ended rows are left unchanged. */
+int otb_rnnt_joint(const void* ep, const void* pp, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len, void* out,
+                   void* stream);
+int otb_rnnt_joint_bwd(const void* dh, const void* h, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len,
+                       void* dep, void* dpp, void* stream);
+int otb_rnnt_logprob(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
+                     const int32_t* u_len, const int32_t* labels, int ldy, float* lp, void* stream);
+int otb_rnnt_loss(const float* lp, int B, int T, int U1, const int32_t* t_len, const int32_t* u_len, double* alpha, float* nll,
+                  float* loss, float* grad, float grad_scale, const float* grad_scale_dev, void* stream);
+int otb_rnnt_dlogits(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
+                     const int32_t* u_len, const int32_t* labels, int ldy, const float* lp, const float* grad, void* dz, int ldd,
+                     void* stream);
+int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const float* h_new, const float* c_new, const void* pp_new,
+                         float* h, float* c, void* pp, int layers, int B, int H, int D, const void* ep, int T, void* ep_cur,
+                         const int32_t* t_len, int32_t* frame, int32_t* n_sym, int32_t* n_out, int32_t* ids, int max_len,
+                         int max_sym, float* score, int32_t* active, void* stream);
+
 /* SpecAugment (data/augment.py:9-41) applied on the device: zero n_freq frequency bands and n_time time bands per
  * utterance.  x f32 [B,T,F] in place; bands i32 [B, 2*(n_freq+n_time)] = (f0, width)*n_freq, (t0, width)*n_time drawn
  * on the host with the reference's RNG call order. */

@@ -111,6 +111,13 @@ _SIGS = {
     'otb_ctc_prefix_advance': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     'otb_ctc_nbest_score': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, _P]),
     'otb_token_logprob': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P]),
+    'otb_rnnt_joint': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
+    'otb_rnnt_joint_bwd': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
+    'otb_rnnt_logprob': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
+    'otb_rnnt_loss': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, c_float, _P, _P]),
+    'otb_rnnt_dlogits': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, _P, c_int, _P]),
+    'otb_rnnt_greedy_step': (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P,
+                                     _P, _P, c_int, c_int, _P, _P, _P]),
     'otb_nbest_rescore': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_float, c_int, c_int, c_int64, _P, _P, _P, _P]),
     'otb_edit_distance': (c_int, [_P, c_int, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P, _P]),
     'otb_mwer_coeff': (c_int, [_P, _P, _P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P]),

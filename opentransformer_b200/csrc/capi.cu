@@ -630,6 +630,65 @@ int otb_token_logprob(const float* logits, int ld, int rows, int V, const int32_
     RET("otb_token_logprob", token_logprob_launch(ST(stream), logits, ld, rows, V, target, out));
 }
 
+static const char* rnnt_lattice_check(int B, int T, int U1, const void* t_len, const void* u_len, int64_t row0, int rows) {
+    if (B < 1 || T < 1 || U1 < 1) return "empty lattice";
+    if (!t_len || !u_len) return "null lengths";
+    if (row0 < 0 || rows < 0 || row0 + rows > (int64_t)B * T * U1) return "rows outside the lattice";
+    return nullptr;
+}
+
+int otb_rnnt_joint(const void* ep, const void* pp, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len, void* out,
+                   void* stream) {
+    if (!ep || !pp || !out) return fail("otb_rnnt_joint", "null operand");
+    if ((t_len == nullptr) != (u_len == nullptr)) return fail("otb_rnnt_joint", "t_len and u_len are given together");
+    RET("otb_rnnt_joint", rnnt_joint_launch(ST(stream), reinterpret_cast<const bf16*>(ep), reinterpret_cast<const bf16*>(pp), B, T, U1,
+                                            D, t_len, u_len, reinterpret_cast<bf16*>(out)));
+}
+
+int otb_rnnt_joint_bwd(const void* dh, const void* h, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len,
+                       void* dep, void* dpp, void* stream) {
+    if (!dh || !h || !dep || !dpp) return fail("otb_rnnt_joint_bwd", "null operand");
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_joint_bwd", e);
+    RET("otb_rnnt_joint_bwd", rnnt_joint_bwd_launch(ST(stream), reinterpret_cast<const bf16*>(dh), reinterpret_cast<const bf16*>(h), B,
+                                                    T, U1, D, t_len, u_len, reinterpret_cast<bf16*>(dep), reinterpret_cast<bf16*>(dpp)));
+}
+
+int otb_rnnt_logprob(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
+                     const int32_t* u_len, const int32_t* labels, int ldy, float* lp, void* stream) {
+    if ((rows > 0 && !logits) || !labels || !lp) return fail("otb_rnnt_logprob", "null operand");
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, row0, rows)) return fail("otb_rnnt_logprob", e);
+    RET("otb_rnnt_logprob", rnnt_logprob_launch(ST(stream), logits, ld, rows, (long long)row0, V, T, U1, t_len, u_len, labels, ldy, lp));
+}
+
+int otb_rnnt_loss(const float* lp, int B, int T, int U1, const int32_t* t_len, const int32_t* u_len, double* alpha, float* nll,
+                  float* loss, float* grad, float grad_scale, const float* grad_scale_dev, void* stream) {
+    if (!lp || !alpha || !nll || !loss || !grad) return fail("otb_rnnt_loss", "null operand");
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_loss", e);
+    RET("otb_rnnt_loss", rnnt_loss_launch(ST(stream), lp, B, T, U1, t_len, u_len, alpha, nll, loss, grad, grad_scale, grad_scale_dev));
+}
+
+int otb_rnnt_dlogits(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
+                     const int32_t* u_len, const int32_t* labels, int ldy, const float* lp, const float* grad, void* dz, int ldd,
+                     void* stream) {
+    if ((rows > 0 && !logits) || !labels || !lp || !grad || !dz) return fail("otb_rnnt_dlogits", "null operand");
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, row0, rows)) return fail("otb_rnnt_dlogits", e);
+    RET("otb_rnnt_dlogits", rnnt_dlogits_launch(ST(stream), logits, ld, rows, (long long)row0, V, T, U1, t_len, u_len, labels, ldy, lp,
+                                                grad, reinterpret_cast<bf16*>(dz), ldd));
+}
+
+int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const float* h_new, const float* c_new, const void* pp_new,
+                         float* h, float* c, void* pp, int layers, int B, int H, int D, const void* ep, int T, void* ep_cur,
+                         const int32_t* t_len, int32_t* frame, int32_t* n_sym, int32_t* n_out, int32_t* ids, int max_len,
+                         int max_sym, float* score, int32_t* active, void* stream) {
+    if (!idx || !logp || !h_new || !c_new || !pp_new || !h || !c || !pp || !ep || !ep_cur || !t_len || !frame || !n_sym || !n_out ||
+        !ids || !score || !active)
+        return fail("otb_rnnt_greedy_step", "null operand");
+    RET("otb_rnnt_greedy_step",
+        rnnt_greedy_step_launch(ST(stream), idx, logp, ldlp, h_new, c_new, reinterpret_cast<const bf16*>(pp_new), h, c,
+                                reinterpret_cast<bf16*>(pp), layers, B, H, D, reinterpret_cast<const bf16*>(ep), T,
+                                reinterpret_cast<bf16*>(ep_cur), t_len, frame, n_sym, n_out, ids, max_len, max_sym, score, active));
+}
+
 int otb_nbest_rescore(const int32_t* tgt, int Lp, const int32_t* len, const float* s1, const float* tok_lp, int M, int B, int K,
                       float weight, int nbest, int Lout, int64_t pad_id, int64_t* ids, int32_t* out_len, float* out_score,
                       void* stream) {

@@ -304,6 +304,22 @@ const char* utt_cmvn_launch(cudaStream_t st, float* x, int B, int Tmax, int F, c
 const char* resample_launch(cudaStream_t st, const float* x, int ldx, const int* n_in, const int* orig, const int* new_rate, float* y,
                             int ldy, int* n_out, int B, int width);
 
+const char* rnnt_joint_launch(cudaStream_t st, const bf16* ep, const bf16* pp, int B, int T, int U1, int D, const int* t_len,
+                              const int* u_len, bf16* out);
+const char* rnnt_joint_bwd_launch(cudaStream_t st, const bf16* dh, const bf16* h, int B, int T, int U1, int D, const int* t_len,
+                                  const int* u_len, bf16* dep, bf16* dpp);
+const char* rnnt_logprob_launch(cudaStream_t st, const float* logits, int ld, int rows, long long row0, int V, int T, int U1,
+                                const int* t_len, const int* u_len, const int* labels, int ldy, float* lp);
+const char* rnnt_loss_launch(cudaStream_t st, const float* lp, int B, int T, int U1, const int* t_len, const int* u_len, double* alpha,
+                             float* nll, float* loss, float* grad, float grad_scale, const float* scale_dev);
+const char* rnnt_dlogits_launch(cudaStream_t st, const float* logits, int ld, int rows, long long row0, int V, int T, int U1,
+                                const int* t_len, const int* u_len, const int* labels, int ldy, const float* lp, const float* grad,
+                                bf16* dz, int ldd);
+const char* rnnt_greedy_step_launch(cudaStream_t st, const int* idx, const float* logp, int ldlp, const float* h_new,
+                                    const float* c_new, const bf16* pp_new, float* h, float* c, bf16* pp, int layers, int B, int H,
+                                    int D, const bf16* ep, int T, bf16* ep_cur, const int* t_len, int* frame, int* n_sym, int* n_out,
+                                    int* ids, int max_len, int max_sym, float* score, int* active);
+
 // LSTM recurrence (lstm.cu): units per CTA, grid and dynamic shared memory of the two persistent kernels for hidden size H
 struct LstmPlan {
     int units, grid;

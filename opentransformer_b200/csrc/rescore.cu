@@ -12,15 +12,12 @@
 
 #include "launch.cuh"
 #include "otb_internal.h"
+#include "row_lse.cuh"
 
 namespace otb {
 
 static constexpr int TLP_WARPS = 8;
-static constexpr int TLP_UNROLL = 4;          // float4 loads in flight per lane
 static constexpr int RESCORE_KMAX = 32;       // one lane per first-pass hypothesis
-
-// (m, s) <- the online log-sum-exp state after the values whose maximum is mg >= m (-inf-safe)
-__device__ __forceinline__ float rescale(float s, float m, float mg) { return m == mg ? s : s * expf(m - mg); }
 
 __global__ void __launch_bounds__(TLP_WARPS * 32) token_logprob_kernel(const float* __restrict__ logits, int ld, int rows, int V,
                                                                        const int* __restrict__ target, float* __restrict__ out) {
@@ -33,42 +30,8 @@ __global__ void __launch_bounds__(TLP_WARPS * 32) token_logprob_kernel(const flo
         return;
     }
     const float* x = logits + (size_t)r * ld;
-    const float4* x4 = reinterpret_cast<const float4*>(x);
-    const int nv = V >> 2;
-    float m = -INFINITY, s = 0.f;
-    for (int i0 = lane; i0 < nv; i0 += 32 * TLP_UNROLL) {
-        float4 v[TLP_UNROLL];
-#pragma unroll
-        for (int j = 0; j < TLP_UNROLL; ++j) {
-            const int i = i0 + 32 * j;
-            v[j] = i < nv ? __ldcs(x4 + i) : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-        }
-        float mg = m;
-#pragma unroll
-        for (int j = 0; j < TLP_UNROLL; ++j) mg = fmaxf(mg, fmaxf(fmaxf(v[j].x, v[j].y), fmaxf(v[j].z, v[j].w)));
-        if (mg == -INFINITY) continue;
-        float acc = rescale(s, m, mg);
-#pragma unroll
-        for (int j = 0; j < TLP_UNROLL; ++j)
-            acc += expf(v[j].x - mg) + expf(v[j].y - mg) + expf(v[j].z - mg) + expf(v[j].w - mg);
-        s = acc;
-        m = mg;
-    }
-    for (int i = 4 * nv + lane; i < V; i += 32) {     // the last V % 4 columns
-        const float xv = x[i];
-        const float mg = fmaxf(m, xv);
-        if (mg == -INFINITY) continue;
-        s = rescale(s, m, mg) + expf(xv - mg);
-        m = mg;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float om = __shfl_xor_sync(0xffffffffu, m, o);
-        const float os = __shfl_xor_sync(0xffffffffu, s, o);
-        const float mg = fmaxf(m, om);
-        if (mg != -INFINITY) s = rescale(s, m, mg) + rescale(os, om, mg);
-        m = mg;
-    }
+    float m, s;
+    warp_row_lse(x, V, lane, m, s);
     if (lane == 0) out[r] = tgt < V ? (x[tgt] - m) - logf(s) : NAN;
 }
 

@@ -255,12 +255,7 @@ class RecurrentLanguageModel(nn.Module):
     def _build_pack(self):
         emb = self.embedding.weight.detach().to(BF16).contiguous()
         tied = self.output_project.weight is self.embedding.weight
-        layers = []
-        for k in range(self.num_layers):
-            w_ih = getattr(self.rnn, f'weight_ih_l{k}').detach().to(BF16).contiguous()
-            bias = (getattr(self.rnn, f'bias_ih_l{k}') + getattr(self.rnn, f'bias_hh_l{k}')).detach().float().contiguous()
-            layers.append({'ih': train.Lin(w_ih, w_ih.t().contiguous(), bias, f'rnn.weight_ih_l{k}', f'rnn.bias_ih_l{k}'),
-                           'w_hh': getattr(self.rnn, f'weight_hh_l{k}').detach().to(BF16).contiguous()})
+        layers = train.lstm_layers(self.rnn, lambda p: p.detach().to(BF16).contiguous(), 'rnn.')
         return {'emb': emb, 'wout': emb if tied else _w(self.output_project), 'bout': _b(self.output_project), 'layers': layers}
 
     def _check_device(self, device):
@@ -278,20 +273,7 @@ class RecurrentLanguageModel(nn.Module):
         self._check_device(tok.device)
         L, N = tok.shape
         x = ops.embedding(tok.reshape(-1), pk['emb'])
-        hs, cs, tape = [], [], []
-        for k, p in enumerate(pk['layers']):
-            gx = ops.linear(x, p['ih'].w, p['ih'].b, out_f32=True)
-            h0 = hidden[0][k].float().contiguous() if hidden is not None else None
-            c0 = hidden[1][k].float().contiguous() if hidden is not None else None
-            y, h_n, c_n, gates, c_all = ops.lstm_fwd(gx, p['w_hh'], L, N, h0, c0, train=record, barrier=barrier)
-            hs.append(h_n)
-            cs.append(c_n)
-            if record:
-                tape.append((x, gates, c_all, y))
-            x = y
-            if drop_seed is not None and self.dropout > 0.0 and k + 1 < self.num_layers:
-                x = ops.dropout_add(y, None, self.dropout, drop_seed, RNNLM_SITE + k)
-        return x, torch.stack(hs), torch.stack(cs), tape
+        return train.lstm_stack_fwd(x, pk['layers'], L, N, self.dropout, drop_seed, RNNLM_SITE, hidden, record, barrier)
 
     def _logits(self, x, pk):
         return train.head_fwd(x, pk['wout'], pk['bout'], self.ld_logits)
@@ -343,17 +325,7 @@ class RecurrentLanguageModel(nn.Module):
         g = train.Grads()
         tied = self.output_project.weight is self.embedding.weight
         dy = train.head_bwd(dlogits, x, pk['wout'], g, 'embedding.weight' if tied else 'output_project.weight', 'output_project.bias')
-        for k in reversed(range(self.num_layers)):
-            p = pk['layers'][k]
-            xk, gates, c_all, y = tape[k]
-            dg = ops.lstm_bwd(dy, p['w_hh'], gates, c_all, L, N)
-            # W_hh sees h_{t-1}: the rows of step t >= 1 against the output of step t - 1 (zero initial state)
-            whh = f'rnn.weight_hh_l{k}'
-            g[whh] = ops.linear_wgrad(dg[N:], y[:-N]) if L > 1 else torch.zeros(p['w_hh'].shape, dtype=torch.float32, device=dg.device)
-            dy = train.linear_bwd(dg, xk, p['ih'], g)
-            g[f'rnn.bias_hh_l{k}'] = g[p['ih'].bname].clone()       # both biases enter the gates alike
-            if k > 0 and drop_seed is not None and self.dropout > 0.0:
-                dy = ops.dropout_add(dy, None, self.dropout, drop_seed, RNNLM_SITE + k - 1)
+        dy = train.lstm_stack_bwd(dy, tape, pk['layers'], L, N, g, self.dropout, drop_seed, RNNLM_SITE)
         train.embedding_bwd(tok, dy, pk['emb'], 1.0, g, 'embedding.weight')
         return loss, g
 

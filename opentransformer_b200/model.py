@@ -10,8 +10,9 @@ import torch.nn as nn
 
 from . import ops
 from . import train
+from .lm import RecurrentLanguageModel, _LSTMParams
 from .modules import (ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder,
-                      TransformerEncoder, _lengths)
+                      TransformerEncoder, _Packed, _lengths)
 
 BuildFrontEnd = {'concat': ConcatFeatureFrontEnd, 'concat-with-linear': ConcatWithLinearFrontEnd, 'conv': ConvFrontEnd}
 BuildEncoder = {'transformer': TransformerEncoder, 'conformer': ConformerEncoder}
@@ -261,4 +262,107 @@ class CTCModel(nn.Module):
         pass
 
 
-End2EndModel = {'ctc': CTCModel, 'speech2text': SpeechToText}
+class PredictionNetwork(nn.Module):
+    """The transducer's prediction network: embedding (V x hidden) and an LSTM stack with nn.LSTM's parameters
+    (lm._LSTMParams: keys rnn.weight_ih_l0 ...), no output layer; dropout between layers in training.  Compute: the LSTM
+    kernels of csrc/lstm.cu through train.lstm_stack_fwd / lstm_stack_bwd."""
+
+    def __init__(self, vocab_size, hidden_size, num_layers=1, dropout=0.0):
+        super().__init__()
+        if hidden_size % 8:
+            raise NotImplementedError(f'PredictionNetwork: the LSTM kernels need hidden_size a multiple of 8, got {hidden_size}')
+        if not 0.0 <= float(dropout) < 1.0:
+            raise ValueError(f'PredictionNetwork: dropout must be in [0, 1), got {dropout}')
+        self.vocab_size, self.hidden_size, self.num_layers = vocab_size, hidden_size, num_layers
+        self.dropout = float(dropout)
+        self.embedding = nn.Embedding(vocab_size, hidden_size)
+        self.rnn = _LSTMParams(hidden_size, hidden_size, num_layers)
+        self._checked = None
+
+    _check_device = RecurrentLanguageModel._check_device
+
+
+class JointNetwork(nn.Module):
+    """z = output_layer(tanh(enc_proj(h_t) + dec_proj(g_u))): enc_proj Linear(encoder d_model -> inner), dec_proj
+    Linear(hidden -> inner, no bias), output_layer Linear(inner -> V).  Compute: otb_rnnt_joint between the projection
+    GEMMs and the output layer's."""
+
+    def __init__(self, encoder_size, hidden_size, inner_size, vocab_size):
+        super().__init__()
+        if inner_size % 8:
+            raise NotImplementedError(f'JointNetwork: the joint kernels need inner_size a multiple of 8, got {inner_size}')
+        self.inner_size, self.vocab_size = inner_size, vocab_size
+        self.enc_proj = nn.Linear(encoder_size, inner_size)
+        self.dec_proj = nn.Linear(hidden_size, inner_size, bias=False)
+        self.output_layer = nn.Linear(inner_size, vocab_size)
+
+    @property
+    def ld_logits(self):
+        return (self.vocab_size + 7) // 8 * 8
+
+
+class TransducerModel(nn.Module):
+    """RNN-T (DESIGN.md 4.22): front end + encoder as for SpeechToText, a PredictionNetwork (`decoder`, over [BLK, y_1 ..
+    y_U]) and a JointNetwork (`joint`), trained with the transducer loss -- the negative log-likelihood of the transcript
+    summed over all alignments of the [T', U + 1] lattice, averaged over the batch (torchaudio.functional.rnnt_loss with
+    reduction 'mean') -- on truth[:, 1:-1] with targets_length - 1 labels, blank BLK = 0.  Checkpoint sections
+    'frontend', 'encoder', 'decoder', 'joint' (what eval.py loads).
+
+    forward: train() with gradients -> one autograd node over the hand-written backward (train_pass); train() without
+    gradients -> the training-mode forward; eval() -> the fused inference pass.  Greedy recognition: TransducerRecognizer."""
+
+    def __init__(self, params):
+        super().__init__()
+        self.params = params
+        if params.get('decoder_type', 'rnn') != 'rnn':
+            raise NotImplementedError(f"TransducerModel: decoder_type {params['decoder_type']!r}; the prediction network is an "
+                                      "LSTM stack ('rnn')")
+        self.frontend = BuildFrontEnd[params['frontend_type']](**params['frontend'])
+        self.encoder = BuildEncoder[params['encoder_type']](**params['encoder'])
+        self.decoder = PredictionNetwork(**params['decoder'])
+        self.vocab_size = self.decoder.vocab_size
+        self.joint = JointNetwork(self.encoder.d_model, self.decoder.hidden_size, params['joint']['inner_size'], self.vocab_size)
+        self.blank = 0
+        self._pack = _Packed(self, lambda: train.transducer_operands(self, train.LayerPack(self)))
+
+    encode_bf16 = SpeechToText.encode_bf16
+
+    def forward(self, inputs, targets):
+        """-> (loss, None).  targets['targets_length'] (label count including <S/E>, data/loader.py:94) is required."""
+        truth, tlen = targets['targets'], targets.get('targets_length')
+        if tlen is None:
+            raise ValueError("TransducerModel needs targets['targets_length'] (label count including <S/E>, data/loader.py:94)")
+        if self.training:
+            run = train.loss_with_grad if torch.is_grad_enabled() else train.loss_train_mode
+            return run(self, inputs['inputs'], inputs['mask'], truth, tlen), None
+        with torch.no_grad():
+            mem, lengths, B, T2 = self.encode_bf16(inputs['inputs'], inputs['mask'])
+            loss, _ = train.transducer_head(self, self._pack.get(), mem, B, T2, lengths, truth, tlen)
+        return loss, None
+
+    train_pass = train.transducer_forward_backward
+    mix_batch = train.mixspeech_halves
+    check_fused_trainer = SpeechToText.check_fused_trainer
+
+    def train_batch(self, inputs, mask, truth, truth_length=None):
+        if truth_length is None:
+            raise TypeError('FusedTrainer.step(inputs, mask, truth, truth_length) for a TransducerModel: truth_length is required')
+        return SpeechToText.train_batch(self, inputs, mask, truth, truth_length)
+
+    def save_checkpoint(self, params, name):
+        torch.save({'params': params, 'frontend': self.frontend.state_dict(), 'encoder': self.encoder.state_dict(),
+                    'decoder': self.decoder.state_dict(), 'joint': self.joint.state_dict()}, name)
+
+    def load_model(self, chkpt):
+        """eval.py:36-49 for a transducer checkpoint: sections 'frontend' (when present), 'encoder', 'decoder' and 'joint'."""
+        if 'frontend' in chkpt:
+            self.frontend.load_state_dict(chkpt['frontend'])
+        self.encoder.load_state_dict(chkpt['encoder'])
+        self.decoder.load_state_dict(chkpt['decoder'])
+        self.joint.load_state_dict(chkpt['joint'])
+
+    def set_epoch(self, epoch):
+        pass
+
+
+End2EndModel = {'ctc': CTCModel, 'speech2text': SpeechToText, 'transducer': TransducerModel}

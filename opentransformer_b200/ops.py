@@ -1320,3 +1320,106 @@ def embedding(tok, emb, out=None):
     check(_lib.lib().otb_embedding(_p(tok), _p(emb), _p(out), N, d, emb.shape[0], _stream()), 'otb_embedding')
     _count()
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# transducer (RNN-T) model: joint network, lattice log-probs, loss and greedy step (include/otb200.h "Transducer")
+# ------------------------------------------------------------------------------------------------
+RNNT_MAX_LABELS = 1023
+
+
+def _rnnt_lengths(t_len, u_len):
+    _need(t_len, torch.int32, 't_len'); _need(u_len, torch.int32, 'u_len')
+    return t_len, u_len
+
+
+def rnnt_joint(ep, pp, B, T, U1, t_len=None, u_len=None, out=None):
+    """Hj bf16 [B*T*U1, D] = tanh(ep[b*T + t] + pp[b*U1 + u]) over the padded lattice, u fastest (otb_rnnt_joint); ep bf16
+    [B*T, D], pp bf16 [B*U1, D].  Nodes with t >= t_len[b] or u > u_len[b] (i32 [B]) are zero; without lengths every node
+    is valid."""
+    _need(ep, BF16, 'ep'); _need(pp, BF16, 'pp')
+    D = ep.shape[1]
+    if ep.shape[0] != B * T or tuple(pp.shape) != (B * U1, D):
+        raise ValueError(f'rnnt_joint: ep must be [B*T, D] = [{B * T}, D] and pp [B*U1, D] = [{B * U1}, {D}], got '
+                         f'{tuple(ep.shape)} and {tuple(pp.shape)}')
+    if (t_len is None) != (u_len is None):
+        raise ValueError('rnnt_joint: t_len and u_len are given together')
+    if t_len is not None:
+        _rnnt_lengths(t_len, u_len)
+    if out is None:
+        out = torch.empty(B * T * U1, D, dtype=BF16, device=ep.device)
+    check(_lib.lib().otb_rnnt_joint(_p(ep), _p(pp), B, T, U1, D, _p(t_len), _p(u_len), _p(out), _stream()), 'otb_rnnt_joint')
+    _count()
+    return out
+
+
+def rnnt_joint_bwd(dh, h, B, T, U1, t_len, u_len):
+    """Backward of rnnt_joint from dh = dHj bf16 [B*T*U1, D] and its output h -> (dEp bf16 [B*T, D], dPp bf16 [B*U1, D]):
+    dZ = dh (1 - h^2) summed over u and over t, in a fixed order (otb_rnnt_joint_bwd)."""
+    _need(dh, BF16, 'dh'); _need(h, BF16, 'h'); _rnnt_lengths(t_len, u_len)
+    D = h.shape[1]
+    dep = torch.empty(B * T, D, dtype=BF16, device=h.device)
+    dpp = torch.empty(B * U1, D, dtype=BF16, device=h.device)
+    check(_lib.lib().otb_rnnt_joint_bwd(_p(dh), _p(h), B, T, U1, D, _p(t_len), _p(u_len), _p(dep), _p(dpp), _stream()),
+          'otb_rnnt_joint_bwd')
+    _count()
+    return dep, dpp
+
+
+def rnnt_logprob(logits, row0, V, B, T, U1, t_len, u_len, labels, lp):
+    """Lattice rows [row0, row0 + rows) of logits f32 [rows, ld] -> lp f32 [B*T*U1, 3] rows row0.. = (logsumexp, log p(blank),
+    log p(labels[b, u])) (otb_rnnt_logprob); labels i32 [B, >= U1 - 1]."""
+    _mat(logits, 'logits', torch.float32); _rnnt_lengths(t_len, u_len); _need(labels, torch.int32, 'labels')
+    _need(lp, torch.float32, 'lp')
+    check(_lib.lib().otb_rnnt_logprob(_p(logits), logits.stride(0), logits.shape[0], row0, V, B, T, U1, _p(t_len), _p(u_len),
+                                      _p(labels), labels.stride(0), _p(lp), _stream()), 'otb_rnnt_logprob')
+    _count()
+    return lp
+
+
+def rnnt_loss(lp, B, T, U1, t_len, u_len, grad_scale=1.0, scale_dev=None):
+    """The RNN-T loss over the lattice log-probs lp (rnnt_logprob) -> (loss 0-d = mean_b nll_b, nll f32 [B], grad f32
+    [B*T*U1, 2] = grad_scale (x the f32 device scalar scale_dev) / B * d nll_b / d (log p(blank), log p(label)))
+    (otb_rnnt_loss)."""
+    _need(lp, torch.float32, 'lp'); _rnnt_lengths(t_len, u_len)
+    if U1 - 1 > RNNT_MAX_LABELS:
+        raise ValueError(f'rnnt_loss: transcripts of {U1 - 1} labels; at most {RNNT_MAX_LABELS} are supported')
+    if scale_dev is not None:
+        _need(scale_dev, torch.float32, 'scale_dev')
+    dev = lp.device
+    alpha = torch.empty(B * T * U1, dtype=torch.float64, device=dev)
+    nll = torch.empty(B, dtype=torch.float32, device=dev)
+    loss = torch.empty(1, dtype=torch.float32, device=dev)
+    grad = torch.empty(B * T * U1, 2, dtype=torch.float32, device=dev)
+    check(_lib.lib().otb_rnnt_loss(_p(lp), B, T, U1, _p(t_len), _p(u_len), _p(alpha), _p(nll), _p(loss), _p(grad), float(grad_scale),
+                                   _p(scale_dev), _stream()), 'otb_rnnt_loss')
+    _count(2)
+    return loss[0], nll, grad
+
+
+def rnnt_dlogits(logits, row0, V, B, T, U1, t_len, u_len, labels, lp, grad, out=None):
+    """dz bf16 [rows, ld] = [k = blank] a + [k = label] c - softmax_k (a + c) of the lattice rows [row0, row0 + rows) in
+    logits f32 [rows, ld], with lp's logsumexp and (a, c) = grad of the node (otb_rnnt_dlogits); columns >= V are zero."""
+    _mat(logits, 'logits', torch.float32); _rnnt_lengths(t_len, u_len); _need(labels, torch.int32, 'labels')
+    _need(lp, torch.float32, 'lp'); _need(grad, torch.float32, 'grad')
+    rows, ld = logits.shape[0], logits.shape[1]
+    if out is None:
+        out = torch.empty(rows, ld, dtype=BF16, device=logits.device)
+    check(_lib.lib().otb_rnnt_dlogits(_p(logits), logits.stride(0), rows, row0, V, B, T, U1, _p(t_len), _p(u_len), _p(labels),
+                                      labels.stride(0), _p(lp), _p(grad), _p(out), out.stride(0), _stream()), 'otb_rnnt_dlogits')
+    _count()
+    return out
+
+
+def rnnt_greedy_step(idx, logp, h_new, c_new, pp_new, h, c, pp, ep, T, ep_cur, t_len, frame, n_sym, n_out, ids, max_sym, score,
+                     active):
+    """One step of batched greedy transducer search (otb_rnnt_greedy_step): the decision of every row from the arg-max idx
+    i32 [B] and log-probs logp f32 [B, ld] of the joint, the predictor state (h, c f32 [layers, B, H], pp bf16 [B, D]) moved
+    forward from (h_new, c_new, pp_new) where a row emitted, and the frame state (ep_cur, frame, n_sym, n_out, ids i32
+    [B, max_len], score, active) updated in place."""
+    layers, B, H = h.shape
+    D = pp.shape[1]
+    check(_lib.lib().otb_rnnt_greedy_step(_p(idx), _p(logp), logp.stride(0), _p(h_new), _p(c_new), _p(pp_new), _p(h), _p(c), _p(pp),
+                                          layers, B, H, D, _p(ep), T, _p(ep_cur), _p(t_len), _p(frame), _p(n_sym), _p(n_out),
+                                          _p(ids), ids.shape[1], max_sym, _p(score), _p(active), _stream()), 'otb_rnnt_greedy_step')
+    _count()

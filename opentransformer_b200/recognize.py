@@ -25,6 +25,7 @@ otrans/recognize/base.py it needs.  Same constructor, same ``recognize`` / ``enc
 import torch
 
 from . import ops
+from . import train
 from .ctc_fusion import CTCFusedSearch
 from .lm import LMCache
 from .model import ctc_align_logits
@@ -817,6 +818,126 @@ class CTCRecognizer(Recognizer):
         return best if self.idx2unit is None else self.translate(best)
 
 
+class _TransducerGreedy:
+    """The greedy transducer search of one geometry (B utterances, T' frames) over one set of model operands: its buffers,
+    and the CUDA graph of STEPS steps once captured."""
+
+    STEPS = 16          # search steps per graph replay: the host reads the active-row counter once per replay
+
+    def __init__(self, model, op, B, T2, max_len, max_sym, device, use_graph):
+        self.model, self.op, self.B, self.T2 = model, op, B, T2
+        self.max_sym, self.use_graph = max_sym, use_graph
+        D, H, L = model.joint.inner_size, model.decoder.hidden_size, model.decoder.num_layers
+        i32 = dict(dtype=torch.int32, device=device)
+        self.ep = torch.empty(B * T2, D, dtype=ops.BF16, device=device)
+        self.ep_cur = torch.empty(B, D, dtype=ops.BF16, device=device)
+        self.pp = torch.empty(B, D, dtype=ops.BF16, device=device)
+        self.h = torch.empty(L, B, H, dtype=torch.float32, device=device)
+        self.c = torch.empty(L, B, H, dtype=torch.float32, device=device)
+        self.logp = torch.empty(B, model.joint.ld_logits, dtype=torch.float32, device=device)
+        self.val = torch.empty(B, 1, dtype=torch.float32, device=device)
+        self.idx = torch.empty(B, 1, **i32)
+        self.tok = torch.zeros(B, dtype=torch.long, device=device)
+        self.t_len, self.frame, self.n_sym, self.n_out = (torch.zeros(B, **i32) for _ in range(4))
+        self.ids = torch.zeros(B, max_len, **i32)
+        self.score = torch.zeros(B, dtype=torch.float32, device=device)
+        self.active = torch.zeros(1, **i32)
+        self.bar = torch.zeros(2, **i32)            # the LSTM kernels' grid barrier, owned here: a graph must not allocate one
+        self.graph = None
+
+    def _predict(self, hidden):
+        """The prediction network one token on from hidden (None: the zero state) for self.tok -> (h, c, dec_proj(h))."""
+        op = self.op
+        x = ops.embedding(self.tok, op['emb'])
+        y, h, c, _ = train.lstm_stack_fwd(x, op['layers'], 1, self.B, hidden=hidden, barrier=self.bar)
+        return h, c, ops.linear(y, op['dec_w'])
+
+    def _steps(self):
+        op, m = self.op, self.model
+        for _ in range(self.STEPS):
+            hj = ops.rnnt_joint(self.ep_cur, self.pp, self.B, 1, 1)
+            logits = ops.linear(hj, op['out_w'], op['out_b'], ops.EPI_BIAS, out_f32=True, n_out=m.joint.ld_logits)
+            ops.logsoftmax_topk(logits, m.vocab_size, 1, out_val=self.val, out_idx=self.idx, out_logp=self.logp)
+            self.tok.copy_(self.idx.view(-1))
+            h, c, pp = self._predict((self.h, self.c))          # every row's next state, kept only where a label is emitted
+            ops.rnnt_greedy_step(self.idx, self.logp, h, c, pp, self.h, self.c, self.pp, self.ep, self.T2, self.ep_cur,
+                                 self.t_len, self.frame, self.n_sym, self.n_out, self.ids, self.max_sym, self.score, self.active)
+
+    def run(self, mem, lengths):
+        B, T2 = self.B, self.T2
+        enc = self.op['enc']
+        ops.linear(mem, enc.w, enc.b, ops.EPI_BIAS, out=self.ep)
+        self.t_len.copy_(lengths)
+        for t in (self.frame, self.n_sym, self.n_out, self.ids, self.score):
+            t.zero_()
+        self.active.copy_((lengths > 0).sum().view(1))
+        self.ep_cur.copy_(self.ep.view(B, T2, -1)[:, 0])
+        self.tok.zero_()                                        # the prediction network starts from BLK and the zero state
+        h, c, pp = self._predict(None)
+        self.h.copy_(h)
+        self.c.copy_(c)
+        self.pp.copy_(pp)
+        # every step moves each live row one frame on or emits one of its at most max_len labels
+        blocks = -(-(T2 + self.ids.shape[1]) // self.STEPS)
+        for _ in range(blocks):
+            if self.graph is not None:
+                self.graph.replay()
+            else:
+                self._steps()
+                if self.use_graph:          # after one eager block (the warm-up), capture the same block
+                    self.graph = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(self.graph):
+                        self._steps()
+            if int(self.active.item()) == 0:
+                break
+        return self.ids.clone(), self.n_out.clone(), self.score.clone()
+
+
+class TransducerRecognizer(Recognizer):
+    """Greedy search of a TransducerModel (DESIGN.md 4.22), batched on the device.  At each step every live utterance takes
+    the arg-max of the joint's log-probs at its current frame and predictor state (ties to the lower id): a label is
+    emitted and the prediction network advances, at most max_symbols_per_frame times per frame and max_len tokens in all
+    (after which only blank is taken); blank moves to the next frame.  The score is the sum of the chosen log-probs,
+    blanks included.  All decisions run in one kernel per step (otb_rnnt_greedy_step); a block of steps is captured in a
+    CUDA graph (use_graph=False: launched one by one) and replayed until a device counter shows every utterance past its
+    last frame.  Beam search, LM fusion and n-gram scoring are not implemented."""
+
+    def __init__(self, model, idx2unit=None, max_symbols_per_frame=5, max_len=1023, ngpu=1, use_graph=True, lm=None,
+                 ngram_lm=None, mode='greedy'):
+        if mode != 'greedy':
+            raise NotImplementedError(f"TransducerRecognizer: only mode='greedy' is implemented, got {mode!r}")
+        if lm is not None:
+            raise NotImplementedError('TransducerRecognizer: LM fusion into the transducer search is not implemented; use lm=None')
+        if ngram_lm is not None:
+            raise NotImplementedError('TransducerRecognizer: n-gram LM scoring (KenLM) is not implemented; use ngram_lm=None')
+        if not 1 <= max_len <= ops.RNNT_MAX_LABELS:
+            raise ValueError(f'TransducerRecognizer: max_len must be in [1, {ops.RNNT_MAX_LABELS}], got {max_len}')
+        if max_symbols_per_frame < 1:
+            raise ValueError(f'TransducerRecognizer: max_symbols_per_frame must be >= 1, got {max_symbols_per_frame}')
+        super().__init__(model, idx2unit, None, None, ngpu)
+        self.max_len, self.max_symbols_per_frame, self.use_graph = int(max_len), int(max_symbols_per_frame), bool(use_graph)
+        self._search = None
+
+    def recognize_ids(self, inputs, inputs_mask):
+        """-> (ids i32 [B, max_len], 0 after each utterance's tokens; lengths i32 [B]; scores f32 [B]), on the device."""
+        with torch.no_grad():
+            mem, lengths, B, T2 = self.model.encode_bf16(inputs, inputs_mask)
+            op = self.model._pack.get()
+            s = self._search
+            # a graph bakes in its buffers and the operands: a new geometry or new weights get a new search
+            if s is None or s.op is not op or (s.B, s.T2, s.ep.device) != (B, T2, mem.device):
+                self._search = s = _TransducerGreedy(self.model, op, B, T2, self.max_len, self.max_symbols_per_frame, mem.device,
+                                                     self.use_graph)
+            self.model.decoder._check_device(mem.device)
+            return s.run(mem, lengths)
+
+    def recognize(self, inputs, inputs_mask):
+        """translate() of the 1-best token lists (the id lists when idx2unit is None), as CTCRecognizer.recognize."""
+        ids, n, _ = self.recognize_ids(inputs, inputs_mask)
+        best = [row[:k] for row, k in zip(ids.cpu().tolist(), n.cpu().tolist())]
+        return best if self.idx2unit is None else self.translate(best)
+
+
 def build_recognizer(model_type, model, lm, args, idx2unit):
     """otrans/recognize/__init__.py:5-21."""
     if model_type == 'speech2text':
@@ -838,4 +959,8 @@ def build_recognizer(model_type, model, lm, args, idx2unit):
             idx2unit=idx2unit, ngpu=args.ngpu, mode=args.mode, alpha=args.alpha, beta=args.beta,
             apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False), rescore_weight=getattr(args, 'rescore_weight', 1.0),
             lm_fusion=getattr(args, 'lm_fusion', False))
+    if model_type == 'transducer':
+        return TransducerRecognizer(model=model, idx2unit=idx2unit, max_len=getattr(args, 'max_len', 1023), ngpu=args.ngpu,
+                                    lm=lm, ngram_lm=getattr(args, 'ngram_lm', None), mode=getattr(args, 'mode', 'greedy'),
+                                    max_symbols_per_frame=getattr(args, 'max_symbols_per_frame', 5))
     raise NotImplementedError(model_type)

@@ -19,8 +19,8 @@ How a model plugs into training -- three methods on its class, and nothing here 
     model.mix_batch(*batch, seed=, step=, scale=, lam=) -> (batch of pass 1, batch of pass 2)
                                                       MixSpeech's two half-batches (mixspeech_halves; speech models only)
 
-batch is (inputs, mask, truth, truth_length or None) for a SpeechToText (forward_backward) and a CTCModel
-(ctc_forward_backward), (inputs, targets) for the language models (lm.py).  grad_sink: name -> fp32 tensor the gradients
+batch is (inputs, mask, truth, truth_length or None) for a SpeechToText (forward_backward), a CTCModel
+(ctc_forward_backward) and a TransducerModel (transducer_forward_backward), (inputs, targets) for the language models (lm.py).  grad_sink: name -> fp32 tensor the gradients
 (x grad_scale) are ADDED into (a gradient accumulation buffer); grad_scale: a float, or an f32 0-d device tensor that the
 kernels making the loss gradient read on the device (MixSpeech's lambda / accum_steps); bf16_of: see LayerPack; drop_seed: int32 device tensor [1],
 the dropout seed of THIS pass (read on the device), required when a dropout rate is non-zero.  The only torch autograd node is `_TrainingLoss` (loss_with_grad), which
@@ -152,9 +152,11 @@ class EncoderPack(LayerPack):
     320-channel front end: the heads).  `rates`: stack name -> the residual_dropout rate of every block; `attn_rates`: stack
     name -> attn_dropout_rates of every block."""
 
-    def __init__(self, model, bf16_of=None):
+    def __init__(self, model, bf16_of=None, with_decoder=True):
         super().__init__(model, bf16_of)
-        fe, enc, dec = model.frontend, model.encoder, getattr(model, 'decoder', None)
+        # with_decoder False: the model's `decoder` is no attention stack (a transducer's prediction network)
+        fe, enc = model.frontend, model.encoder
+        dec = getattr(model, 'decoder', None) if with_decoder else None
         self.conformer = isinstance(enc, ConformerEncoder)
         if not (isinstance(fe, (ConvFrontEnd, ConcatFeatureFrontEnd)) and isinstance(enc, (TransformerEncoder, ConformerEncoder))
                 and (dec is None or isinstance(dec, TransformerDecoder))):
@@ -915,6 +917,167 @@ def ctc_forward_backward(model, inputs, mask, truth, truth_length, want_grads=Tr
         return loss, None
     g = Grads(grad_sink)
     _encoder_bwd(model, pk, tr, head_bwd(dctc, mem, wc, g, *_CTC_HEAD), g)
+    return loss, g
+
+
+# dropout site of the output of the transducer's prediction-network LSTM layer k: RNNT_SITE + k, clear of the speech
+# model's (ENC_SITE, DEC_SITE, MWER_SITE and ATTN_SITE + those) and the language models' (lm.py)
+RNNT_SITE = 10000
+# bytes of fp32 logits the transducer's output layer holds at once: the lattice rows run through it in chunks of this size
+RNNT_WORKSPACE_BYTES = 512 << 20
+
+
+def lstm_layers(rnn, w, prefix):
+    """The operands of an _LSTMParams stack (lm.py) named `prefix` + its parameter names: per layer the input projection
+    as a Lin (bf16 W_ih, its transpose, the fp32 sum of both biases), W_hh bf16 (w casts a parameter) and the names of
+    W_hh and b_hh."""
+    layers = []
+    for k in range(rnn.num_layers):
+        w_ih = w(getattr(rnn, f'weight_ih_l{k}'))
+        bias = (getattr(rnn, f'bias_ih_l{k}') + getattr(rnn, f'bias_hh_l{k}')).detach().float().contiguous()
+        layers.append({'ih': Lin(w_ih, w_ih.t().contiguous(), bias, f'{prefix}weight_ih_l{k}', f'{prefix}bias_ih_l{k}'),
+                       'w_hh': w(getattr(rnn, f'weight_hh_l{k}')), 'whh': f'{prefix}weight_hh_l{k}', 'bhh': f'{prefix}bias_hh_l{k}'})
+    return layers
+
+
+def lstm_stack_fwd(x, layers, L, N, dropout=0.0, drop_seed=None, site0=0, hidden=None, record=False, barrier=None):
+    """An LSTM stack over x bf16 [L*N, I] (time-major) -> (output of the top layer bf16 [L*N, H], h_n, c_n f32 [layers, N,
+    H], tape).  hidden: (h0, c0) f32 [layers, N, H] or None; with drop_seed, dropout on the output of every layer but the
+    last (site site0 + k); record: keep what lstm_stack_bwd reads (per layer: input, gates, c_t, output); barrier: see
+    ops.lstm_fwd.  The recurrent LM and the transducer's prediction network."""
+    hs, cs, tape = [], [], []
+    for k, p in enumerate(layers):
+        gx = ops.linear(x, p['ih'].w, p['ih'].b, out_f32=True)
+        h0 = hidden[0][k].float().contiguous() if hidden is not None else None
+        c0 = hidden[1][k].float().contiguous() if hidden is not None else None
+        y, h_n, c_n, gates, c_all = ops.lstm_fwd(gx, p['w_hh'], L, N, h0, c0, train=record, barrier=barrier)
+        hs.append(h_n)
+        cs.append(c_n)
+        if record:
+            tape.append((x, gates, c_all, y))
+        x = y
+        if drop_seed is not None and dropout > 0.0 and k + 1 < len(layers):
+            x = ops.dropout_add(y, None, dropout, drop_seed, site0 + k)
+    return x, torch.stack(hs), torch.stack(cs), tape
+
+
+def lstm_stack_bwd(dy, tape, layers, L, N, g, dropout=0.0, drop_seed=None, site0=0):
+    """Backward through time of lstm_stack_fwd(record=True, zero initial state) from dy bf16 [L*N, H]: the parameter
+    gradients into g (added into its sink when it has one) -> the gradient of the stack's input bf16 [L*N, I]."""
+    acc = g.sink is not None
+    for k in reversed(range(len(layers))):
+        p = layers[k]
+        xk, gates, c_all, y = tape[k]
+        dg = ops.lstm_bwd(dy, p['w_hh'], gates, c_all, L, N)
+        # W_hh sees h_{t-1}: the rows of step t >= 1 against the output of step t - 1 (zero initial state)
+        if L > 1:
+            g[p['whh']] = ops.linear_wgrad(dg[N:], y[:-N], out=g.out(p['whh']), accumulate=acc)
+        else:
+            _acc_out(g, p['whh'], p['w_hh'].shape, dg.device)
+        dy = linear_bwd(dg, xk, p['ih'], g)
+        # both biases enter the gates alike
+        if acc:
+            g[p['bhh']] = ops.colsum(dg, out=g.out(p['bhh']), accumulate=True)
+        else:
+            g[p['bhh']] = g[p['ih'].bname].clone()
+        if k > 0 and drop_seed is not None and dropout > 0.0:
+            dy = ops.dropout_add(dy, None, dropout, drop_seed, site0 + k - 1)
+    return dy
+
+
+def transducer_operands(model, pk):
+    """The prediction network's and the joint network's operands of a TransducerModel, cast by the LayerPack pk."""
+    j, d = model.joint, model.decoder
+    return {'enc': pk._lin(j.enc_proj), 'dec_w': pk.w(j.dec_proj.weight), 'out_w': pk.w(j.output_layer.weight),
+            'out_b': _f(j.output_layer.bias), 'emb': pk.w(d.embedding.weight), 'layers': lstm_layers(d.rnn, pk.w, 'decoder.rnn.')}
+
+
+def transducer_head(model, op, mem, B, T2, lengths, truth, truth_length, drop_seed=None, g=None, grad_scale=1.0,
+                    workspace_bytes=None):
+    """The transducer half above the encoder (DESIGN.md 4.22): enc_proj over the memory bf16 [B*T', d], the prediction
+    network over [BLK, y_1 .. y_U] (y = truth[:, 1:-1], truth_length - 1 labels), dec_proj, the joint over the padded
+    lattice [B, T', U + 1] and the RNN-T loss, with the output layer run over chunks of lattice rows holding at most
+    workspace_bytes (RNNT_WORKSPACE_BYTES) of fp32 logits.  op: transducer_operands.  -> (loss 0-d f32 = mean_b nll_b,
+    dmem bf16 [B*T', d] or None).  With g (a Grads) the backward runs: each chunk's logits are recomputed, turned into
+    bf16 dlogits and sent through the dgrad and the accumulating wgrad GEMMs, then the joint, the projections and the
+    prediction network run backward into g; the loss gradient is scaled by grad_scale (a float or an f32 device scalar)."""
+    dev = mem.device
+    V, D = model.vocab_size, model.joint.inner_size
+    dec = model.decoder
+    labels = truth[:, 1:-1].to(torch.int32).contiguous()
+    u_len = (truth_length.to(dev).to(torch.int32) - 1).contiguous()
+    U1 = labels.shape[1] + 1
+    if U1 - 1 > ops.RNNT_MAX_LABELS:
+        raise ValueError(f'transducer: transcripts of {U1 - 1} labels; at most {ops.RNNT_MAX_LABELS} are supported')
+    dec._check_device(dev)
+    tok = torch.cat((torch.zeros(B, 1, dtype=torch.long, device=dev), truth[:, 1:-1].to(dev)), dim=1).t().contiguous()  # [U1, B]
+    want = g is not None
+    x = ops.embedding(tok.view(-1), op['emb'])
+    y, _, _, tape = lstm_stack_fwd(x, op['layers'], U1, B, dec.dropout, drop_seed, RNNT_SITE, record=want)
+    H = y.shape[1]
+    gb = y.view(U1, B, H).transpose(0, 1).contiguous().view(B * U1, H)                # utterance-major predictor rows
+    enc = op['enc']
+    ep = ops.linear(mem, enc.w, enc.b, EPI_BIAS)
+    pp = ops.linear(gb, op['dec_w'])
+    hj = ops.rnnt_joint(ep, pp, B, T2, U1, lengths, u_len)
+    rows, ld = B * T2 * U1, model.joint.ld_logits
+    chunk = max(8, (workspace_bytes or RNNT_WORKSPACE_BYTES) // (4 * ld) // 8 * 8)
+    ws = torch.empty(min(chunk, rows), ld, dtype=torch.float32, device=dev)
+    lp = torch.empty(rows, 3, dtype=torch.float32, device=dev)
+    spans = [(r0, min(rows, r0 + chunk)) for r0 in range(0, rows, chunk)]
+
+    def logits(r0, r1):
+        return ops.linear(hj[r0:r1], op['out_w'], op['out_b'], EPI_BIAS, out=ws[:r1 - r0])
+
+    for r0, r1 in spans:
+        ops.rnnt_logprob(logits(r0, r1), r0, V, B, T2, U1, lengths, u_len, labels, lp)
+    s, sdev = _loss_scale(grad_scale, 1.0)
+    loss, _, grad = ops.rnnt_loss(lp, B, T2, U1, lengths, u_len, s, sdev)
+    if not want:
+        return loss, None
+
+    dw = _acc_out(g, 'joint.output_layer.weight', op['out_w'].shape, dev)
+    db = torch.zeros(ld, dtype=torch.float32, device=dev)
+    wt = torch.zeros(D, ld, dtype=BF16, device=dev)
+    wt[:, :V] = op['out_w'].t()
+    dl = torch.empty(ws.shape, dtype=BF16, device=dev)
+    dhj = torch.empty(rows, D, dtype=BF16, device=dev)
+    for r0, r1 in spans:
+        dz = ops.rnnt_dlogits(logits(r0, r1), r0, V, B, T2, U1, lengths, u_len, labels, lp, grad, out=dl[:r1 - r0])
+        ops.linear_wgrad(dz[:, :V], hj[r0:r1], out=dw, accumulate=True)
+        ops.colsum(dz, out=db, accumulate=True)
+        ops.linear(dz, wt, out=dhj[r0:r1])
+    g.put('joint.output_layer.bias', db[:V])
+    del ws, dl
+    dep, dpp = ops.rnnt_joint_bwd(dhj, hj, B, T2, U1, lengths, u_len)
+    del dhj, hj
+    dmem = linear_bwd(dep, mem, enc, g)
+    acc = g.sink is not None
+    g['joint.dec_proj.weight'] = ops.linear_wgrad(dpp, gb, out=g.out('joint.dec_proj.weight'), accumulate=acc)
+    dgb = ops.linear(dpp, op['dec_w'].t().contiguous())
+    dy = dgb.view(B, U1, H).transpose(0, 1).contiguous().view(U1 * B, H)
+    dx = lstm_stack_bwd(dy, tape, op['layers'], U1, B, g, dec.dropout, drop_seed, RNNT_SITE)
+    embedding_bwd(tok, dx, op['emb'], 1.0, g, 'decoder.embedding.weight')
+    return loss, dmem
+
+
+def transducer_forward_backward(model, inputs, mask, truth, truth_length, want_grads=True, grad_sink=None, grad_scale=1.0,
+                                bf16_of=None, drop_seed=None):
+    """TransducerModel.train_pass (the contract is at the top of this file): front end + encoder (_encoder_fwd), then
+    transducer_head (enc_proj, the prediction network over [BLK, y], dec_proj, the joint and the chunked RNN-T loss) against
+    truth[:, 1:-1] with truth_length - 1 labels, and the backward in reverse ending in _encoder_bwd.  Arguments as
+    ctc_forward_backward's; truth_length is required."""
+    if truth_length is None:
+        raise ValueError('transducer_forward_backward: a TransducerModel needs truth_length')
+    pk = EncoderPack(model, bf16_of, with_decoder=False)
+    need_drop_seed(drop_seed, pk.rates['encoder'] + _flat(pk.attn_rates['encoder']) + [model.decoder.dropout])
+    op = transducer_operands(model, pk)
+    mem, tr = _encoder_fwd(model, pk, inputs, mask, drop_seed)
+    g = Grads(grad_sink) if want_grads else None
+    loss, dmem = transducer_head(model, op, mem, tr.B, tr.T2, tr.lengths, truth, truth_length, drop_seed, g, grad_scale)
+    if not want_grads:
+        return loss, None
+    _encoder_bwd(model, pk, tr, dmem, g)
     return loss, g
 
 
