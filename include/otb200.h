@@ -588,6 +588,34 @@ int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const 
                          const int32_t* t_len, int32_t* frame, int32_t* n_sym, int32_t* n_out, int32_t* ids, int max_len,
                          int max_sym, float* score, int32_t* active, void* stream);
 
+/* ---- Transducer beam search: alignment-length synchronous decoding (ALSD), DESIGN.md 4.22.  Utterance b owns the K
+ * hypothesis slots (1 <= K <= 15) of rows b K .. b K + K - 1 of every [B K, ...] array.  A slot holds score f32 (-inf:
+ * empty), slot_u its label count u, frame its frame t (t < t_len[b] while live) and node its last label's node in the
+ * utterance's node table (node_par / node_tok i32 [B, n_cap], n_cap >= K (T + max_len) + 1; node 0 is the empty sequence,
+ * n_nodes i32 [B] the nodes in use).
+ * otb_rnnt_beam_step: one search step for every utterance with done[b] == 0, after otb_logsoftmax_topk (k1 = min(K + 1, V))
+ *   of the joint's logits at each slot: logp f32 [B K, ldlp] the log-probs (column 0 blank), val / idx [B K, k1] the top
+ *   k1.  Each live slot forms a blank candidate (a final when t + 1 = t_len[b]) and, while u < max_len, one per each of its
+ *   min(K, V - 1) best labels; a label candidate whose sequence equals a live blank candidate's is log-added into it; the K
+ *   best (score descending, ties to the lower parent slot, blank before labels, labels in top-k order) become the new slots,
+ *   with par i32 [B K] the parent slot (0..K-1) and tok i64 [B K] the label taken (0: blank or empty).  Finals go into the
+ *   n-best f_score / f_node / f_u [B, W] (f_n i32 [B] entries; ties to the earlier step, then the lower slot).  The
+ *   utterance ends when no slot is live, or f_n = W and logsumexp(live scores) <= f_score[W - 1]: done[b] = 1, *active -= 1,
+ *   and ids i32 [B, W, max_len] (0-padded), lengths i32 [B, W] and out_score f32 [B, W] get the n-best, best first (unfilled
+ *   entries: length 0, score -inf).  An ended utterance's slots get par = their own slot and tok = 0.
+ * otb_rnnt_beam_gather: (h, c) f32 [layers, B K, H] and pp bf16 [B K, D] of row b K + par[r] -> (hg, cg, ppg) row r, and ep
+ *   bf16 [B T, D] row b T + frame[r] -> ep_cur bf16 [B K, D] row r.
+ * otb_rnnt_beam_commit: (h, c, pp) row r = (hn, cn, ppn) row r where tok[r] > 0, else (hg, cg, ppg) row r. */
+int otb_rnnt_beam_step(const float* logp, int ldlp, const float* val, const int32_t* idx, int k1, int B, int K, int W, int V, int T,
+                       int max_len, const int32_t* t_len, float* score, int32_t* slot_u, int32_t* frame, int32_t* node, int32_t* par,
+                       int64_t* tok, int32_t* node_par, int32_t* node_tok, int n_cap, int32_t* n_nodes, float* f_score,
+                       int32_t* f_node, int32_t* f_u, int32_t* f_n, int32_t* done, int32_t* active, int32_t* ids, int32_t* lengths,
+                       float* out_score, void* stream);
+int otb_rnnt_beam_gather(const int32_t* par, const int32_t* frame, int B, int K, int layers, int H, int D, int T, const float* h,
+                         const float* c, const void* pp, const void* ep, float* hg, float* cg, void* ppg, void* ep_cur, void* stream);
+int otb_rnnt_beam_commit(const int64_t* tok, int rows, int layers, int H, int D, const float* hg, const float* cg, const void* ppg,
+                         const float* hn, const float* cn, const void* ppn, float* h, float* c, void* pp, void* stream);
+
 /* SpecAugment (data/augment.py:9-41) applied on the device: zero n_freq frequency bands and n_time time bands per
  * utterance.  x f32 [B,T,F] in place; bands i32 [B, 2*(n_freq+n_time)] = (f0, width)*n_freq, (t0, width)*n_time drawn
  * on the host with the reference's RNG call order. */

@@ -118,6 +118,10 @@ _SIGS = {
     'otb_rnnt_dlogits': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, _P, c_int, _P]),
     'otb_rnnt_greedy_step': (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P,
                                      _P, _P, c_int, c_int, _P, _P, _P]),
+    'otb_rnnt_beam_step': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P,
+                                   _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'otb_rnnt_beam_gather': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'otb_rnnt_beam_commit': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'otb_nbest_rescore': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_float, c_int, c_int, c_int64, _P, _P, _P, _P]),
     'otb_edit_distance': (c_int, [_P, c_int, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P, _P]),
     'otb_mwer_coeff': (c_int, [_P, _P, _P, c_int, _P, c_int, c_int, c_float, _P, _P, _P, _P]),

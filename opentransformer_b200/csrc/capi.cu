@@ -689,6 +689,37 @@ int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const 
                                 reinterpret_cast<bf16*>(ep_cur), t_len, frame, n_sym, n_out, ids, max_len, max_sym, score, active));
 }
 
+int otb_rnnt_beam_step(const float* logp, int ldlp, const float* val, const int32_t* idx, int k1, int B, int K, int W, int V, int T,
+                       int max_len, const int32_t* t_len, float* score, int32_t* slot_u, int32_t* frame, int32_t* node, int32_t* par,
+                       int64_t* tok, int32_t* node_par, int32_t* node_tok, int n_cap, int32_t* n_nodes, float* f_score,
+                       int32_t* f_node, int32_t* f_u, int32_t* f_n, int32_t* done, int32_t* active, int32_t* ids, int32_t* lengths,
+                       float* out_score, void* stream) {
+    if (!logp || !val || !idx || !t_len || !score || !slot_u || !frame || !node || !par || !tok || !node_par || !node_tok ||
+        !n_nodes || !f_score || !f_node || !f_u || !f_n || !done || !active || !ids || !lengths || !out_score)
+        return fail("otb_rnnt_beam_step", "null operand");
+    RET("otb_rnnt_beam_step",
+        rnnt_beam_step_launch(ST(stream), logp, ldlp, val, idx, k1, B, K, W, V, T, max_len, t_len, score, slot_u, frame, node, par,
+                              reinterpret_cast<long long*>(tok), node_par, node_tok, n_cap, n_nodes, f_score, f_node, f_u, f_n, done,
+                              active, ids, lengths, out_score));
+}
+
+int otb_rnnt_beam_gather(const int32_t* par, const int32_t* frame, int B, int K, int layers, int H, int D, int T, const float* h,
+                         const float* c, const void* pp, const void* ep, float* hg, float* cg, void* ppg, void* ep_cur, void* stream) {
+    if (!par || !frame || !h || !c || !pp || !ep || !hg || !cg || !ppg || !ep_cur) return fail("otb_rnnt_beam_gather", "null operand");
+    RET("otb_rnnt_beam_gather",
+        rnnt_beam_gather_launch(ST(stream), par, frame, B, K, layers, H, D, T, h, c, reinterpret_cast<const bf16*>(pp),
+                                reinterpret_cast<const bf16*>(ep), hg, cg, reinterpret_cast<bf16*>(ppg), reinterpret_cast<bf16*>(ep_cur)));
+}
+
+int otb_rnnt_beam_commit(const int64_t* tok, int rows, int layers, int H, int D, const float* hg, const float* cg, const void* ppg,
+                         const float* hn, const float* cn, const void* ppn, float* h, float* c, void* pp, void* stream) {
+    if (!tok || !hg || !cg || !ppg || !hn || !cn || !ppn || !h || !c || !pp) return fail("otb_rnnt_beam_commit", "null operand");
+    RET("otb_rnnt_beam_commit",
+        rnnt_beam_commit_launch(ST(stream), reinterpret_cast<const long long*>(tok), rows, layers, H, D, hg, cg,
+                                reinterpret_cast<const bf16*>(ppg), hn, cn, reinterpret_cast<const bf16*>(ppn), h, c,
+                                reinterpret_cast<bf16*>(pp)));
+}
+
 int otb_nbest_rescore(const int32_t* tgt, int Lp, const int32_t* len, const float* s1, const float* tok_lp, int M, int B, int K,
                       float weight, int nbest, int Lout, int64_t pad_id, int64_t* ids, int32_t* out_len, float* out_score,
                       void* stream) {

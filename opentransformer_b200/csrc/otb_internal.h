@@ -319,6 +319,16 @@ const char* rnnt_greedy_step_launch(cudaStream_t st, const int* idx, const float
                                     const float* c_new, const bf16* pp_new, float* h, float* c, bf16* pp, int layers, int B, int H,
                                     int D, const bf16* ep, int T, bf16* ep_cur, const int* t_len, int* frame, int* n_sym, int* n_out,
                                     int* ids, int max_len, int max_sym, float* score, int* active);
+const char* rnnt_beam_step_launch(cudaStream_t st, const float* logp, int ldlp, const float* val, const int* idx, int k1, int B, int K,
+                                  int W, int V, int T, int max_len, const int* t_len, float* score, int* slot_u, int* frame, int* node,
+                                  int* par, long long* tok, int* node_par, int* node_tok, int n_cap, int* n_nodes, float* f_score,
+                                  int* f_node, int* f_u, int* f_n, int* done, int* active, int* ids, int* lengths, float* out_score);
+const char* rnnt_beam_gather_launch(cudaStream_t st, const int* par, const int* frame, int B, int K, int layers, int H, int D, int T,
+                                    const float* h, const float* c, const bf16* pp, const bf16* ep, float* hg, float* cg, bf16* ppg,
+                                    bf16* ep_cur);
+const char* rnnt_beam_commit_launch(cudaStream_t st, const long long* tok, int rows, int layers, int H, int D, const float* hg,
+                                    const float* cg, const bf16* ppg, const float* hn, const float* cn, const bf16* ppn, float* h,
+                                    float* c, bf16* pp);
 
 // LSTM recurrence (lstm.cu): units per CTA, grid and dynamic shared memory of the two persistent kernels for hidden size H
 struct LstmPlan {

@@ -1423,3 +1423,47 @@ def rnnt_greedy_step(idx, logp, h_new, c_new, pp_new, h, c, pp, ep, T, ep_cur, t
                                           layers, B, H, D, _p(ep), T, _p(ep_cur), _p(t_len), _p(frame), _p(n_sym), _p(n_out),
                                           _p(ids), ids.shape[1], max_sym, _p(score), _p(active), _stream()), 'otb_rnnt_greedy_step')
     _count()
+
+
+RNNT_BEAM_MAX = 15          # beam width: K + 1 log-probs per slot from logsoftmax_topk, whose k is at most 16
+
+
+def rnnt_beam_step(logp, val, idx, V, T, t_len, state, out):
+    """One step of the transducer's ALSD beam search (otb_rnnt_beam_step) for every utterance not yet ended, from the
+    joint's log-probs at each slot: logp f32 [B*K, ld] and the top min(K + 1, V) (val f32, idx i32 [B*K, k1]) of
+    logsoftmax_topk.  state: dict of the search's device arrays, updated in place -- the slots (score f32, u, frame, node i32
+    [B*K]), the step's actions (par i32, tok i64 [B*K]), the node table (node_par, node_tok i32 [B, n_cap], n_nodes i32 [B]),
+    the n-best so far (f_score f32, f_node, f_u i32 [B, W], f_n i32 [B]), done i32 [B] and active i32 [1].  out: (ids i32
+    [B, W, max_len], lengths i32 [B, W], scores f32 [B, W]), written for each utterance when it ends."""
+    s = state
+    _need(logp, torch.float32, 'logp'); _need(val, torch.float32, 'val'); _need(idx, torch.int32, 'idx')
+    B, W = s['f_score'].shape
+    K = s['score'].numel() // B
+    ids, lengths, scores = out
+    check(_lib.lib().otb_rnnt_beam_step(_p(logp), logp.stride(0), _p(val), _p(idx), idx.shape[1], B, K, W, V, T, ids.shape[2],
+                                        _p(t_len), _p(s['score']), _p(s['u']), _p(s['frame']), _p(s['node']), _p(s['par']),
+                                        _p(s['tok']), _p(s['node_par']), _p(s['node_tok']), s['node_par'].shape[1],
+                                        _p(s['n_nodes']), _p(s['f_score']), _p(s['f_node']), _p(s['f_u']), _p(s['f_n']),
+                                        _p(s['done']), _p(s['active']), _p(ids), _p(lengths), _p(scores), _stream()),
+          'otb_rnnt_beam_step')
+    _count()
+
+
+def rnnt_beam_gather(par, frame, K, h, c, pp, ep, T, hg, cg, ppg, ep_cur):
+    """Each slot row r of utterance b = r // K takes the predictor state of row b*K + par[r]: (h, c) f32 [layers, B*K, H]
+    and pp bf16 [B*K, D] -> (hg, cg, ppg) row r; and its frame's encoder projection, ep bf16 [B*T, D] row b*T + frame[r]
+    -> ep_cur bf16 [B*K, D] row r (otb_rnnt_beam_gather)."""
+    layers, BK, H = h.shape
+    D = pp.shape[1]
+    check(_lib.lib().otb_rnnt_beam_gather(_p(par), _p(frame), BK // K, K, layers, H, D, T, _p(h), _p(c), _p(pp), _p(ep), _p(hg),
+                                          _p(cg), _p(ppg), _p(ep_cur), _stream()), 'otb_rnnt_beam_gather')
+    _count()
+
+
+def rnnt_beam_commit(tok, hg, cg, ppg, hn, cn, ppn, h, c, pp):
+    """(h, c, pp) row r = the predictor's output (hn, cn, ppn) row r where tok[r] (i64) is a label, else the gathered
+    (hg, cg, ppg) row r (otb_rnnt_beam_commit)."""
+    layers, BK, H = h.shape
+    check(_lib.lib().otb_rnnt_beam_commit(_p(tok), BK, layers, H, pp.shape[1], _p(hg), _p(cg), _p(ppg), _p(hn), _p(cn), _p(ppn),
+                                          _p(h), _p(c), _p(pp), _stream()), 'otb_rnnt_beam_commit')
+    _count()

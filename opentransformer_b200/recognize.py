@@ -893,19 +893,148 @@ class _TransducerGreedy:
         return self.ids.clone(), self.n_out.clone(), self.score.clone()
 
 
+class _TransducerALSD:
+    """The ALSD beam search of one geometry (B utterances, T' frames, K slots each, an n-best of W, max_len labels) over one
+    set of model operands: its buffers, the node table, and the CUDA graph of STEPS steps once captured.  Every array is at
+    B*K slot rows; the step is rnnt_joint -> output layer -> logsoftmax_topk -> otb_rnnt_beam_step -> otb_rnnt_beam_gather ->
+    the prediction network one token on -> otb_rnnt_beam_commit."""
+
+    STEPS = 16
+
+    def __init__(self, model, op, B, T2, K, W, max_len, device, use_graph):
+        self.model, self.op, self.B, self.T2, self.K, self.use_graph = model, op, B, T2, K, use_graph
+        D, H, L = model.joint.inner_size, model.decoder.hidden_size, model.decoder.num_layers
+        BK, V = B * K, model.vocab_size
+        f32, i32 = dict(dtype=torch.float32, device=device), dict(dtype=torch.int32, device=device)
+        self.ep = torch.empty(B * T2, D, dtype=ops.BF16, device=device)
+        self.ep_cur, self.pp, self.ppg = (torch.empty(BK, D, dtype=ops.BF16, device=device) for _ in range(3))
+        self.h, self.c, self.hg, self.cg = (torch.empty(L, BK, H, **f32) for _ in range(4))
+        self.logp = torch.empty(BK, model.joint.ld_logits, **f32)
+        self.k1 = min(K + 1, V)
+        self.val = torch.empty(BK, self.k1, **f32)
+        self.idx = torch.empty(BK, self.k1, **i32)
+        n_cap = K * (T2 + max_len) + 1                  # the root and at most K new nodes per step, T_b + max_len steps
+        self.state = dict(score=torch.empty(BK, **f32), u=torch.empty(BK, **i32), frame=torch.empty(BK, **i32),
+                          node=torch.empty(BK, **i32), par=torch.empty(BK, **i32),
+                          tok=torch.zeros(BK, dtype=torch.long, device=device),
+                          node_par=torch.zeros(B, n_cap, **i32), node_tok=torch.zeros(B, n_cap, **i32),
+                          n_nodes=torch.empty(B, **i32), f_score=torch.empty(B, W, **f32), f_node=torch.empty(B, W, **i32),
+                          f_u=torch.empty(B, W, **i32), f_n=torch.empty(B, **i32), done=torch.empty(B, **i32),
+                          active=torch.empty(1, **i32))
+        self.t_len = torch.zeros(B, **i32)
+        self.out = (torch.zeros(B, W, max_len, **i32), torch.zeros(B, W, **i32), torch.empty(B, W, **f32))
+        self.bar = torch.zeros(2, **i32)
+        self.graph = None
+
+    def _predict(self, hidden):
+        op = self.op
+        x = ops.embedding(self.state['tok'], op['emb'])
+        y, h, c, _ = train.lstm_stack_fwd(x, op['layers'], 1, self.B * self.K, hidden=hidden, barrier=self.bar)
+        return h, c, ops.linear(y, op['dec_w'])
+
+    def step_phases(self):
+        """One search step as its seven phases, in order (tools/transducer_beam.py times each)."""
+        op, m, s = self.op, self.model, self.state
+        box = {}
+
+        def joint():
+            box['hj'] = ops.rnnt_joint(self.ep_cur, self.pp, self.B * self.K, 1, 1)
+
+        def output_layer():
+            box['logits'] = ops.linear(box['hj'], op['out_w'], op['out_b'], ops.EPI_BIAS, out_f32=True, n_out=m.joint.ld_logits)
+
+        def topk():
+            ops.logsoftmax_topk(box['logits'], m.vocab_size, self.k1, out_val=self.val, out_idx=self.idx, out_logp=self.logp)
+
+        def beam_step():
+            ops.rnnt_beam_step(self.logp, self.val, self.idx, m.vocab_size, self.T2, self.t_len, s, self.out)
+
+        def gather():
+            ops.rnnt_beam_gather(s['par'], s['frame'], self.K, self.h, self.c, self.pp, self.ep, self.T2, self.hg, self.cg,
+                                 self.ppg, self.ep_cur)
+
+        def predictor():            # every slot's next state, kept only where it took a label
+            box['new'] = self._predict((self.hg, self.cg))
+
+        def commit():
+            ops.rnnt_beam_commit(s['tok'], self.hg, self.cg, self.ppg, *box['new'], self.h, self.c, self.pp)
+        return [joint, output_layer, topk, beam_step, gather, predictor, commit]
+
+    def _steps(self):
+        for _ in range(self.STEPS):
+            for phase in self.step_phases():
+                phase()
+
+    def start(self, mem, lengths):
+        """The state before the first step: one live slot per utterance with a frame, the empty sequence at frame 0."""
+        B, T2, K, s = self.B, self.T2, self.K, self.state
+        enc = self.op['enc']
+        ops.linear(mem, enc.w, enc.b, ops.EPI_BIAS, out=self.ep)
+        self.t_len.copy_(lengths)
+        s['score'].fill_(float('-inf'))
+        s['score'].view(B, K)[:, 0].masked_fill_(lengths > 0, 0.0)
+        for k in ('u', 'frame', 'node', 'par', 'tok', 'f_n', 'done'):
+            s[k].zero_()
+        s['n_nodes'].fill_(1)
+        s['active'].fill_(B)                    # an utterance without frames ends at the first step
+        for t in self.out[:2]:
+            t.zero_()
+        self.out[2].fill_(float('-inf'))
+        self.ep_cur.view(B, K, -1).copy_(self.ep.view(B, T2, -1)[:, :1])
+        h, c, pp = self._predict(None)          # every slot from BLK and the zero state
+        self.h.copy_(h)
+        self.c.copy_(c)
+        self.pp.copy_(pp)
+
+    def run(self, mem, lengths):
+        self.start(mem, lengths)
+        s = self.state
+        self.steps = 0
+        # every step moves each live hypothesis one frame or one label on: T_b + max_len steps end every utterance
+        blocks = -(-(self.T2 + self.out[0].shape[2]) // self.STEPS)
+        for _ in range(blocks):
+            if self.graph is not None:
+                self.graph.replay()
+            else:
+                self._steps()
+                if self.use_graph:
+                    self.graph = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(self.graph):
+                        self._steps()
+            self.steps += self.STEPS
+            if int(s['active'].item()) == 0:
+                break
+        return tuple(t.clone() for t in self.out)
+
+
 class TransducerRecognizer(Recognizer):
-    """Greedy search of a TransducerModel (DESIGN.md 4.22), batched on the device.  At each step every live utterance takes
-    the arg-max of the joint's log-probs at its current frame and predictor state (ties to the lower id): a label is
-    emitted and the prediction network advances, at most max_symbols_per_frame times per frame and max_len tokens in all
-    (after which only blank is taken); blank moves to the next frame.  The score is the sum of the chosen log-probs,
-    blanks included.  All decisions run in one kernel per step (otb_rnnt_greedy_step); a block of steps is captured in a
-    CUDA graph (use_graph=False: launched one by one) and replayed until a device counter shows every utterance past its
-    last frame.  Beam search, LM fusion and n-gram scoring are not implemented."""
+    """Search of a TransducerModel (DESIGN.md 4.22), batched on the device.
+
+    mode='greedy': at each step every live utterance takes the arg-max of the joint's log-probs at its current frame and
+    predictor state (ties to the lower id): a label is emitted and the prediction network advances, at most
+    max_symbols_per_frame times per frame and max_len tokens in all (after which only blank is taken); blank moves to the
+    next frame.  The score is the sum of the chosen log-probs, blanks included.  All decisions run in one kernel per step
+    (otb_rnnt_greedy_step).  beam_width is ignored and nbest must be 1.
+
+    mode='alsd': alignment-length synchronous beam search (Saon et al. 2020) with beam_width K (1..15) hypotheses per
+    utterance and an n-best of nbest (1..K).  Every hypothesis takes one lattice step per search step: blank (one frame on)
+    or one of its K best labels (while it has fewer than max_len); hypotheses with the same labels at the same step are
+    merged by log-adding their scores, so a score sums every alignment of its labels the beam kept.  A hypothesis that takes
+    blank on its last frame is a final; the n-best holds the nbest best finals, and an utterance ends when no hypothesis is
+    live or the live ones together can no longer beat the n-best's worst.  max_symbols_per_frame does not apply: ALSD
+    bounds labels by max_len alone.  One kernel per step makes every decision (otb_rnnt_beam_step).
+
+    Both modes capture a block of steps in a CUDA graph (use_graph=False: launched one by one) and replay it until a device
+    counter shows every utterance ended.  The default and modified beam searches, LM fusion and n-gram scoring are not
+    implemented."""
 
     def __init__(self, model, idx2unit=None, max_symbols_per_frame=5, max_len=1023, ngpu=1, use_graph=True, lm=None,
-                 ngram_lm=None, mode='greedy'):
-        if mode != 'greedy':
-            raise NotImplementedError(f"TransducerRecognizer: only mode='greedy' is implemented, got {mode!r}")
+                 ngram_lm=None, mode='greedy', beam_width=5, nbest=1):
+        if mode == 'beam':
+            raise NotImplementedError("TransducerRecognizer: the default (Graves) beam search is not implemented; "
+                                      "mode='alsd' is the transducer beam search")
+        if mode not in ('greedy', 'alsd'):
+            raise NotImplementedError(f"TransducerRecognizer: mode must be 'greedy' or 'alsd', got {mode!r}")
         if lm is not None:
             raise NotImplementedError('TransducerRecognizer: LM fusion into the transducer search is not implemented; use lm=None')
         if ngram_lm is not None:
@@ -914,26 +1043,49 @@ class TransducerRecognizer(Recognizer):
             raise ValueError(f'TransducerRecognizer: max_len must be in [1, {ops.RNNT_MAX_LABELS}], got {max_len}')
         if max_symbols_per_frame < 1:
             raise ValueError(f'TransducerRecognizer: max_symbols_per_frame must be >= 1, got {max_symbols_per_frame}')
+        if mode == 'alsd':
+            if not 1 <= beam_width <= ops.RNNT_BEAM_MAX:
+                raise ValueError(f'TransducerRecognizer: beam_width must be in [1, {ops.RNNT_BEAM_MAX}], got {beam_width}')
+            if not 1 <= nbest <= beam_width:
+                raise ValueError(f'TransducerRecognizer: nbest must be in [1, beam_width = {beam_width}], got {nbest}')
+        elif nbest != 1:
+            raise ValueError(f"TransducerRecognizer: greedy search has one hypothesis, got nbest={nbest}; use mode='alsd'")
         super().__init__(model, idx2unit, None, None, ngpu)
         self.max_len, self.max_symbols_per_frame, self.use_graph = int(max_len), int(max_symbols_per_frame), bool(use_graph)
+        self.mode, self.beam_width, self.nbest = mode, int(beam_width), int(nbest)
         self._search = None
 
     def recognize_ids(self, inputs, inputs_mask):
-        """-> (ids i32 [B, max_len], 0 after each utterance's tokens; lengths i32 [B]; scores f32 [B]), on the device."""
+        """greedy: -> (ids i32 [B, max_len], 0 after each utterance's tokens; lengths i32 [B]; scores f32 [B]);
+        alsd: -> (ids i32 [B, nbest, max_len]; lengths i32 [B, nbest]; scores f32 [B, nbest]), best first, entries past the
+        finals found with length 0 and score -inf; on the device."""
         with torch.no_grad():
             mem, lengths, B, T2 = self.model.encode_bf16(inputs, inputs_mask)
             op = self.model._pack.get()
             s = self._search
             # a graph bakes in its buffers and the operands: a new geometry or new weights get a new search
             if s is None or s.op is not op or (s.B, s.T2, s.ep.device) != (B, T2, mem.device):
-                self._search = s = _TransducerGreedy(self.model, op, B, T2, self.max_len, self.max_symbols_per_frame, mem.device,
-                                                     self.use_graph)
+                if self.mode == 'alsd':
+                    s = _TransducerALSD(self.model, op, B, T2, self.beam_width, self.nbest, self.max_len, mem.device,
+                                        self.use_graph)
+                else:
+                    s = _TransducerGreedy(self.model, op, B, T2, self.max_len, self.max_symbols_per_frame, mem.device,
+                                          self.use_graph)
+                self._search = s
             self.model.decoder._check_device(mem.device)
             return s.run(mem, lengths)
 
     def recognize(self, inputs, inputs_mask):
-        """translate() of the 1-best token lists (the id lists when idx2unit is None), as CTCRecognizer.recognize."""
-        ids, n, _ = self.recognize_ids(inputs, inputs_mask)
+        """greedy: translate() of the 1-best token lists (the id lists when idx2unit is None), as CTCRecognizer.recognize.
+        alsd: (nbest_translate(ids), scores), as SpeechToTextRecognizer.recognize: with idx2unit, each utterance's n-best
+        strings (an entry without a final is ''); without, the id tensor [B, nbest, max_len]."""
+        ids, n, sc = self.recognize_ids(inputs, inputs_mask)
+        if self.mode == 'alsd':
+            if self.idx2unit is None:
+                return self.nbest_translate(ids), sc
+            # the EOS that ends nbest_translate's rows: ids past each length are padding (0), which has no unit
+            cut = torch.arange(ids.shape[2], device=ids.device) >= n.unsqueeze(2)
+            return self.nbest_translate(ids.masked_fill(cut, EOS).long()), sc
         best = [row[:k] for row, k in zip(ids.cpu().tolist(), n.cpu().tolist())]
         return best if self.idx2unit is None else self.translate(best)
 
@@ -962,5 +1114,6 @@ def build_recognizer(model_type, model, lm, args, idx2unit):
     if model_type == 'transducer':
         return TransducerRecognizer(model=model, idx2unit=idx2unit, max_len=getattr(args, 'max_len', 1023), ngpu=args.ngpu,
                                     lm=lm, ngram_lm=getattr(args, 'ngram_lm', None), mode=getattr(args, 'mode', 'greedy'),
-                                    max_symbols_per_frame=getattr(args, 'max_symbols_per_frame', 5))
+                                    max_symbols_per_frame=getattr(args, 'max_symbols_per_frame', 5),
+                                    beam_width=getattr(args, 'beam_width', 5), nbest=getattr(args, 'nbest', 1))
     raise NotImplementedError(model_type)
