@@ -118,7 +118,8 @@ int otb_dropout_bwd(const void* dy, int lddy, void* out, int ldo, uint8_t* mask,
  * head h starts at column q_col0/k_col0/v_col0 + d_k*h.  d_k is 64 or 96 (96 is the width of the shipped Conformer
  * configuration, d_model 384 / 4 heads); any other value returns non-zero with otb_last_error().
  * bd (optional, f32 [H,B,Tq,ldbd]) holds relative-position scores, bias(i,j) = bd[h,b,i, j-i+Tq-1] (the gather of
- * attention.py:196-215 done by indexing).  resid (optional, bf16 [B*Tq, ldr]) is added to the output (the rel-pos
+ * attention.py:196-215 done by indexing); it needs Tq == Tk, no causal mask and ldbd >= 2 Tq - 1, as otb_attention_bwd
+ * and otb_attention_probs do, and is refused otherwise.  resid (optional, bf16 [B*Tq, ldr]) is added to the output (the rel-pos
  * attention of the shipped Conformer has no output projection, SURVEY.md 8a quirks).  lse (optional, f32 [B,H,Tq])
  * receives the per-row log-sum-exp (log2 units) otb_attention_bwd needs; the backward is 64-wide, so lse requires
  * d_k = 64. */
@@ -269,7 +270,8 @@ int otb_decode_persistent(const otb_mega_model* model, const void* kvx, const in
  * hand-written backward of each forward op above.  bf16 activations / gradients, fp32 parameter gradients. */
 
 /* Backward of otb_attention (d_k = 64, no resid; lse as that forward stored it): dq, dk, dv written at column offsets
- * d*_col0 + 64*h of their matrices (e.g. the three thirds of one [M,3d] dqkv buffer).  dsum f32 [B,H,Tq] is scratch.
+ * d*_col0 + 64*h of their matrices (e.g. the three thirds of one [M,3d] dqkv buffer).  out and dout are read at rows
+ * [0, B*Tq) only, however many rows q has.  dsum f32 [B,H,Tq] receives D = rowsum(dout * out).
  * wgmma, scores recomputed.  bd and dbd are both NULL, or both set for rel-pos attention: the forward was otb_attention with
  * the band bd f32 [H, B*Tq, ldbd] (Tq == Tk, not causal).  The band is added to the recomputed scores, and its gradient dS
  * (the gradient of the raw score sum, which includes 1/sqrt(d_k)) is written to dbd bf16 [H, B*Tq, lddbd] at column

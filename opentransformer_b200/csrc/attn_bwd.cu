@@ -351,7 +351,8 @@ const char* attn_bwd_launch(cudaStream_t st, const void* q, int ldq, int q_rows,
     if ((err = encode_tmap_2d(&tq, q, (uint64_t)ldq, (uint64_t)q_rows, (uint64_t)ldq, 64, 128))) return err;
     if ((err = encode_tmap_2d(&tk, k, (uint64_t)ldk, (uint64_t)k_rows, (uint64_t)ldk, 64, 128))) return err;
     if ((err = encode_tmap_2d(&tv, v, (uint64_t)ldv, (uint64_t)k_rows, (uint64_t)ldv, 64, 128))) return err;
-    if ((err = encode_tmap_2d(&tdo, p.dout, (uint64_t)p.lddo, (uint64_t)q_rows, (uint64_t)p.lddo, 64, 128))) return err;
+    // dO has B*Tq rows, whatever q holds: the last query tile reads TMA zero fill past them, not the caller's memory
+    if ((err = encode_tmap_2d(&tdo, p.dout, (uint64_t)p.lddo, (uint64_t)p.B * p.Tq, (uint64_t)p.lddo, 64, 128))) return err;
     const dim3 gq((p.Tq + 127) / 128, p.H, p.B), gk((p.Tk + 127) / 128, p.H, p.B);
     if (p.bd) {
         if ((err = launch<attn_bwd_dq_kernel<true>>(gq, 256, ABW_SMEM_DQ, st, tq, tk, tv, tdo, p))) return err;

@@ -214,6 +214,11 @@ int otb_attention(const void* q, int ldq, int q_rows, const void* k, int ldk, in
     if (d_k != 64 && d_k != 96) return fail("otb_attention", "head width d_k must be 64 or 96");
     if (lse && d_k != 64) return fail("otb_attention", "lse is for the 64-wide backward: it needs d_k = 64");
     if (q_col0 % 8 || k_col0 % 8 || v_col0 % 8 || ldo % 8) return fail("otb_attention", "column offsets / ldo must be multiples of 8");
+    if (bd) {   // the kernel reads band row i at columns Tq - 1 - i + j for every visible key j
+        if (causal) return fail("otb_attention", "the rel-pos band is for non-causal attention");
+        if (Tq != Tk) return fail("otb_attention", "the rel-pos band needs Tq == Tk");
+        if (ldbd < 2 * Tq - 1) return fail("otb_attention", "band pitches must hold 2 Tq - 1 columns");
+    }
     AttnParams p;
     p.B = B; p.H = H; p.Tq = Tq; p.Tk = Tk;
     p.kv_len = kv_len; p.causal = causal;

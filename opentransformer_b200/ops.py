@@ -231,17 +231,59 @@ def check_head_dim(d_k):
         raise NotImplementedError(f'the sm_90a attention kernels support head widths d_k in {HEAD_DIMS}, got {d_k}')
 
 
+def _head_cols(op, t, col0, width, name):
+    """Heads read or write columns [col0, col0 + width) of matrix t."""
+    if t.dim() != 2 or col0 < 0 or col0 + width > t.shape[1]:
+        raise ValueError(f'{op}: {name} must be a matrix with columns [{col0}, {col0 + width}) for the heads, got {tuple(t.shape)}')
+
+
+def _rows_cols(op, t, rows, cols, name):
+    """A matrix the kernel reads or writes at rows [0, rows) and columns [0, cols)."""
+    if t.shape[0] < rows or t.shape[1] < cols:
+        raise ValueError(f'{op}: {name} must have at least {rows} rows and {cols} columns, got {tuple(t.shape)}')
+
+
+def _kv_len(op, kv_len, B):
+    if kv_len is not None:
+        _need(kv_len, torch.int32, 'kv_len')
+        if kv_len.numel() < B:
+            raise ValueError(f'{op}: kv_len must hold one length per batch entry ({B}), got {kv_len.numel()}')
+
+
+def _band(op, bd, B, H, Tq, Tk, causal, dtype, name):
+    """The rel-pos band (or its gradient): H*B*Tq rows of at least 2 Tq - 1 columns, for non-causal self-attention."""
+    _need(bd, dtype, name)
+    if Tq != Tk or causal:
+        raise ValueError(f'{op}: the rel-pos band is for non-causal self-attention (Tq == Tk)')
+    if bd.dim() < 2 or bd.shape[-1] < 2 * Tq - 1 or bd.numel() // bd.shape[-1] < H * B * Tq:
+        raise ValueError(f'{op}: {name} must have {H * B * Tq} rows of at least {2 * Tq - 1} columns, got {tuple(bd.shape)}')
+
+
 def _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, out=None, bd=None, resid=None, d_k=64,
-               with_lse=False):
-    """otb_attention -> (out bf16 [B*Tq, H*d_k], lse f32 [B,H,Tq] if with_lse else None)."""
+               with_lse=False, lse=None):
+    """otb_attention -> (out bf16 [B*Tq, H*d_k], lse f32 [B,H,Tq] (written into lse when given) if with_lse else None)."""
     for t, n in ((q, 'q'), (k, 'k'), (v, 'v')):
         _need(t, BF16, n)
     check_head_dim(d_k)
+    for t, c0, n in ((q, q_col0, 'q'), (k, k_col0, 'k'), (v, v_col0, 'v')):
+        _head_cols('attention', t, c0, H * d_k, n)
+    if out is not None:
+        _rows_cols('attention', _mat(out, 'out'), B * Tq, H * d_k, 'out')
+    if resid is not None:
+        _rows_cols('attention', _mat(resid, 'resid'), B * Tq, H * d_k, 'resid')
+    if bd is not None:
+        _band('attention', bd, B, H, Tq, Tk, causal, torch.float32, 'bd')
+    _kv_len('attention', kv_len, B)
+    if with_lse and lse is not None:
+        _need(lse, torch.float32, 'lse')
+        if tuple(lse.shape) != (B, H, Tq):
+            raise ValueError(f'attention: lse must be [{B}, {H}, {Tq}], got {tuple(lse.shape)}')
     if out is None:
         out = torch.empty(B * Tq, H * d_k, dtype=BF16, device=q.device)
-    lse = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device) if with_lse else None
-    if kv_len is not None:
-        _need(kv_len, torch.int32, 'kv_len')
+    if not with_lse:
+        lse = None
+    elif lse is None:
+        lse = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device)
     check(_lib.lib().otb_attention(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out),
                                    out.stride(0), B, H, Tq, Tk, _p(kv_len), 1 if causal else 0, q_col0, k_col0, v_col0, _p(bd),
                                    bd.shape[-1] if bd is not None else 0, _p(resid), resid.stride(0) if resid is not None else 0,
@@ -519,10 +561,12 @@ def decode_persistent(model_c, kvx, mem_len, kc, vc, state, B, T, max_steps, wor
 # ------------------------------------------------------------------------------------------------
 # training step: backward kernels (include/otb200.h "Training step")
 # ------------------------------------------------------------------------------------------------
-def attention_train(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, v_col0=0, bd=None):
+def attention_train(q, k, v, B, H, Tq, Tk, kv_len=None, causal=False, q_col0=0, k_col0=0, v_col0=0, bd=None, out=None,
+                    lse=None):
     """attention (d_k 64, the width of the backward) + the per-row log-sum-exp the backward needs
-    -> (out bf16 [B*Tq, H*64], lse f32 [B,H,Tq]).  bd: the rel-pos band, as for attention()."""
-    return _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, bd=bd, with_lse=True)
+    -> (out bf16 [B*Tq, H*64], lse f32 [B,H,Tq]), written into out / lse when given.  bd: the rel-pos band, as for
+    attention()."""
+    return _attention(q, k, v, B, H, Tq, Tk, kv_len, causal, q_col0, k_col0, v_col0, out=out, bd=bd, with_lse=True, lse=lse)
 
 
 def rel_band_ld(T):
@@ -531,25 +575,44 @@ def rel_band_ld(T):
 
 
 def attention_bwd(q, k, v, out, dout, lse, B, H, Tq, Tk, dq, dk, dv, kv_len=None, causal=False, q_col0=0, k_col0=0,
-                  v_col0=0, dq_col0=0, dk_col0=0, dv_col0=0, bd=None, dbd=None):
+                  v_col0=0, dq_col0=0, dk_col0=0, dv_col0=0, bd=None, dbd=None, dsum=None):
     """Gradients of otb_attention written into dq/dk/dv (bf16 matrices, column offsets d*_col0).  With the rel-pos band bd
     f32 [H, B*Tq, ld] of the forward, its gradient is written into dbd bf16 [H, B*Tq, rel_band_ld(Tq)], which the caller
-    zeroes."""
+    zeroes.  Returns D = rowsum(dout * out) f32 [B,H,Tq], written into dsum when given."""
     for t, n in ((q, 'q'), (k, 'k'), (v, 'v'), (out, 'out'), (dout, 'dout'), (dq, 'dq'), (dk, 'dk'), (dv, 'dv')):
         _mat(t, n)
-    dsum = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device)
+    d = H * 64    # the backward is 64-wide
+    for t, c0, n in ((q, q_col0, 'q'), (k, k_col0, 'k'), (v, v_col0, 'v'), (dq, dq_col0, 'dq'), (dk, dk_col0, 'dk'),
+                     (dv, dv_col0, 'dv')):
+        _head_cols('attention_bwd', t, c0, d, n)
+    for t, n in ((out, 'out'), (dout, 'dout')):
+        _rows_cols('attention_bwd', t, B * Tq, d, n)
+    for t, rows, n in ((dq, B * Tq, 'dq'), (dk, B * Tk, 'dk'), (dv, B * Tk, 'dv')):
+        _rows_cols('attention_bwd', t, rows, 0, n)
+    _need(lse, torch.float32, 'lse')
+    if tuple(lse.shape) != (B, H, Tq):
+        raise ValueError(f'attention_bwd: lse must be [{B}, {H}, {Tq}], got {tuple(lse.shape)}')
+    if dsum is not None:
+        _need(dsum, torch.float32, 'dsum')
+        if tuple(dsum.shape) != (B, H, Tq):
+            raise ValueError(f'attention_bwd: dsum must be [{B}, {H}, {Tq}], got {tuple(dsum.shape)}')
+    _kv_len('attention_bwd', kv_len, B)
     ldbd = lddbd = 0
+    if (bd is None) != (dbd is None):
+        raise ValueError('attention_bwd: bd and dbd must both be given or both be None')
     if bd is not None:
-        if causal:
-            raise ValueError('attention_bwd: the rel-pos band is for non-causal self-attention')
-        _need(bd, torch.float32, 'bd'); _need(dbd, BF16, 'dbd')
+        _band('attention_bwd', bd, B, H, Tq, Tk, causal, torch.float32, 'bd')
+        _band('attention_bwd', dbd, B, H, Tq, Tk, causal, BF16, 'dbd')
         ldbd, lddbd = bd.shape[-1], dbd.shape[-1]
+    if dsum is None:
+        dsum = torch.empty(B, H, Tq, dtype=torch.float32, device=q.device)
     check(_lib.lib().otb_attention_bwd(_p(q), q.stride(0), q.shape[0], _p(k), k.stride(0), k.shape[0], _p(v), v.stride(0), _p(out),
                                        out.stride(0), _p(dout), dout.stride(0), _p(lse), _p(dsum), _p(dq), dq.stride(0), dq_col0,
                                        _p(dk), dk.stride(0), dk_col0, _p(dv), dv.stride(0), dv_col0, B, H, Tq, Tk, _p(kv_len),
                                        1 if causal else 0, q_col0, k_col0, v_col0, _p(bd), ldbd, _p(dbd), lddbd, _stream()),
           'otb_attention_bwd')
     _count(2)
+    return dsum
 
 
 def conformer_conv_train(x, lengths, w, wb, gamma, beta, running_mean, running_var, num_batches, B, T, momentum=0.1, eps=1e-5):

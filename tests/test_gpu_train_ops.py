@@ -1,6 +1,4 @@
 """GPU parity of the backward kernels (training step) against torch fp32 autograd on the same bf16-rounded operands."""
-import math
-
 import pytest
 import torch
 import torch.nn.functional as F
@@ -91,63 +89,6 @@ def test_relu_bwd_and_embed_bwd():
     ops.embed_bwd(tok, dx, dE, 16.0)
     ref = torch.ones(V, d, device=DEV).index_add_(0, tok, dx.float() * 16.0)
     torch.testing.assert_close(dE, ref, rtol=1e-4, atol=1e-2)
-
-
-def _attn_ref(q, k, v, B, H, Tq, Tk, kv_len, causal):
-    """fp32 reference with autograd; q [B*Tq, H*64], k/v [B*Tk, H*64]."""
-    qh = q.view(B, Tq, H, 64).transpose(1, 2)
-    kh = k.view(B, Tk, H, 64).transpose(1, 2)
-    vh = v.view(B, Tk, H, 64).transpose(1, 2)
-    s = qh @ kh.transpose(-1, -2) / 8.0
-    mask = torch.ones(B, 1, Tq, Tk, dtype=torch.bool, device=q.device)
-    if kv_len is not None:
-        mask = mask & (torch.arange(Tk, device=q.device)[None, None, None, :] < kv_len.view(B, 1, 1, 1))
-    if causal:
-        mask = mask & torch.tril(torch.ones(Tq, Tk, dtype=torch.bool, device=q.device))[None, None]
-    s = s.masked_fill(~mask, float('-inf'))
-    o = torch.softmax(s, -1) @ vh
-    return o.transpose(1, 2).reshape(B * Tq, H * 64)
-
-
-@pytest.mark.parametrize('B,H,Tq,Tk,causal,ragged,cross', [
-    (3, 4, 249, 249, False, True, False), (2, 4, 30, 30, True, False, False), (2, 4, 31, 249, False, True, True),
-    (2, 2, 300, 300, True, False, False), (1, 4, 128, 128, False, False, False), (2, 1, 257, 130, False, True, True)])
-def test_attention_backward(B, H, Tq, Tk, causal, ragged, cross):
-    d = H * 64
-    kv_len = None
-    if ragged:
-        kv_len = torch.tensor([Tk - (7 * i) % max(1, Tk // 2) for i in range(B)], dtype=torch.int32, device=DEV)
-    if cross:
-        qm, kvm = _bf(B * Tq, d, seed=20, scale=0.7), _bf(B * Tk, 2 * d, seed=21, scale=0.7)
-        q, k, v, qc, kc, vc = qm, kvm, kvm, 0, 0, d
-    else:
-        qkv = _bf(B * Tq, 3 * d, seed=22, scale=0.7)
-        q = k = v = qkv
-        qc, kc, vc = 0, d, 2 * d
-    dout = _bf(B * Tq, d, seed=23)
-    out, lse = ops.attention_train(q, k, v, B, H, Tq, Tk, kv_len=kv_len, causal=causal, q_col0=qc, k_col0=kc, v_col0=vc)
-    out_plain = ops.attention(q, k, v, B, H, Tq, Tk, kv_len=kv_len, causal=causal, q_col0=qc, k_col0=kc, v_col0=vc)
-    assert torch.equal(out, out_plain)
-    qf = q[:, qc:qc + d].float().clone().requires_grad_(True)
-    kf = k[:, kc:kc + d].float().clone().requires_grad_(True)
-    vf = v[:, vc:vc + d].float().clone().requires_grad_(True)
-    ref = _attn_ref(qf, kf, vf, B, H, Tq, Tk, kv_len.long() if kv_len is not None else None, causal)
-    ref.backward(dout.float())
-    if cross:
-        dq = torch.full((B * Tq, d), float('nan'), dtype=BF, device=DEV)
-        dkv = torch.full((B * Tk, 2 * d), float('nan'), dtype=BF, device=DEV)
-        ops.attention_bwd(q, k, v, out, dout, lse, B, H, Tq, Tk, dq, dkv, dkv, kv_len=kv_len, causal=causal, q_col0=qc,
-                          k_col0=kc, v_col0=vc, dq_col0=0, dk_col0=0, dv_col0=d)
-        gq, gk, gv = dq, dkv[:, :d], dkv[:, d:]
-    else:
-        dqkv = torch.full((B * Tq, 3 * d), float('nan'), dtype=BF, device=DEV)
-        ops.attention_bwd(q, k, v, out, dout, lse, B, H, Tq, Tk, dqkv, dqkv, dqkv, kv_len=kv_len, causal=causal, q_col0=qc,
-                          k_col0=kc, v_col0=vc, dq_col0=0, dk_col0=d, dv_col0=2 * d)
-        gq, gk, gv = dqkv[:, :d], dqkv[:, d:2 * d], dqkv[:, 2 * d:]
-    rq, rk, rv = _rel(gq, qf.grad), _rel(gk, kf.grad), _rel(gv, vf.grad)
-    print(f'attention bwd B={B} H={H} Tq={Tq} Tk={Tk} causal={causal}: out {_rel(out, ref):.2e} dq {rq:.2e} dk {rk:.2e} dv {rv:.2e}')
-    assert torch.isfinite(gq.float()).all() and torch.isfinite(gk.float()).all() and torch.isfinite(gv.float()).all()
-    assert _rel(out, ref) < 1e-2 and rq < 2e-2 and rk < 2e-2 and rv < 2e-2
 
 
 def test_ls_ce_train_grad_and_fixed_lr_scheduled_adam():
