@@ -210,9 +210,11 @@ int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int l
 /* Fused log_softmax (+ lm_weight * lm_logp) + per-row top-k (decoder/transformer.py:206 + speech2text.py:102-112):
  * logits f32 [rows, ldl] -> out_val f32 [rows,k] (log-prob values, descending), out_idx i32 [rows,k];
  * out_logp (optional, f32 [rows, ld_logp]) additionally receives the full log-prob rows.  1 <= k <= min(16, V), V <= 49152;
- * ties go to the lower vocabulary id. */
-int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, int k,
-                        int rows, float* out_val, int32_t* out_idx, float* out_logp, int ld_logp, void* stream);
+ * ties go to the lower vocabulary id.  lm_exempt < 0 (lm_beta must be 0): as above.  lm_exempt in [0, V) (the transducer's
+ * shallow fusion, DESIGN.md 4.22): column lm_exempt keeps its log-prob, every other column i gets
+ * + (lm_weight * lm_logp[i] + lm_beta) (+ lm_beta when lm_logp is NULL), and out_logp receives the plain log-probs. */
+int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, float lm_beta,
+                        int lm_exempt, int k, int rows, float* out_val, int32_t* out_idx, float* out_logp, int ld_logp, void* stream);
 /* One step of ancestral sampling from logits f32 [N, ldl] (DESIGN.md 4.11) on the beam state, rows never reordered: every
  * live row n draws token = argmax_{v < V} (logits[n, v] - log(-log u)), ties to the lower id, with
  * u = rng_u01(rng_key(rng_key(rng_key(seed, step), n), v)) (csrc/counter_rng.cuh), step = st->ctrl[0] and seed the int32
@@ -573,7 +575,10 @@ int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T,
  *   when n_sym[b] >= max_sym or n_out[b] >= max_len, and adds its log-prob to score[b].  A label goes to ids i32 [B, max_len]
  *   at n_out[b], and the predictor state computed from it (h_new / c_new f32 [layers, B, H], pp_new bf16 [B, D]) replaces the
  *   row's (h, c, pp); blank moves frame[b] on and copies ep bf16 [B T, D] row b T + frame[b] into ep_cur bf16 [B, D], or,
- *   past the last frame, decrements *active.  Ended rows are left unchanged. */
+ *   past the last frame, decrements *active.  Ended rows are left unchanged.  LM shallow fusion (all three optional, NULL:
+ *   none): val f32 [B] the fused value of idx (otb_logsoftmax_topk with blank exempt), which a label adds to score in place
+ *   of its log-prob; emit i32 [B] = 1 where the row emitted a label this step, else 0; lm_pos i32 [B] = the label's LM
+ *   position (n_out after it, 1..max_len) where it emitted, else -1. */
 int otb_rnnt_joint(const void* ep, const void* pp, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len, void* out,
                    void* stream);
 int otb_rnnt_joint_bwd(const void* dh, const void* h, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len,
@@ -588,7 +593,8 @@ int otb_rnnt_dlogits(const float* logits, int ld, int rows, int64_t row0, int V,
 int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const float* h_new, const float* c_new, const void* pp_new,
                          float* h, float* c, void* pp, int layers, int B, int H, int D, const void* ep, int T, void* ep_cur,
                          const int32_t* t_len, int32_t* frame, int32_t* n_sym, int32_t* n_out, int32_t* ids, int max_len,
-                         int max_sym, float* score, int32_t* active, void* stream);
+                         int max_sym, float* score, int32_t* active, const float* val, int32_t* emit, int32_t* lm_pos,
+                         void* stream);
 
 /* ---- Transducer beam search: alignment-length synchronous decoding (ALSD), DESIGN.md 4.22.  Utterance b owns the K
  * hypothesis slots (1 <= K <= 15) of rows b K .. b K + K - 1 of every [B K, ...] array.  A slot holds score f32 (-inf:
@@ -605,6 +611,12 @@ int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const 
  *   utterance ends when no slot is live, or f_n = W and logsumexp(live scores) <= f_score[W - 1]: done[b] = 1, *active -= 1,
  *   and ids i32 [B, W, max_len] (0-padded), lengths i32 [B, W] and out_score f32 [B, W] get the n-best, best first (unfilled
  *   entries: length 0, score -inf).  An ended utterance's slots get par = their own slot and tok = 0.
+ *   LM shallow fusion: val holds the fused label values (otb_logsoftmax_topk with blank exempt) and no decision changes;
+ *   beta > 0 makes the end bound logsumexp(live score + beta (max_len - u)).  lm_src / lm_ext (optional, i32 [B K]): each
+ *   new slot's parent row b K + par and 1 where it took a label.  anc (optional, i32 [B K, Lpos], Lpos >= max_len + 1,
+ *   with anc_tmp the same size of scratch and lm_pos i32 [B K]): each slot's LM cache rows b n_cap + node of its labels,
+ *   position 0 the empty sequence's node 0, kept up to date; lm_pos = the new label's position u where the slot took one,
+ *   else -1.  Ended utterances: lm_src = the row itself, lm_ext = 0, lm_pos = -1.
  * otb_rnnt_beam_gather: (h, c) f32 [layers, B K, H] and pp bf16 [B K, D] of row b K + par[r] -> (hg, cg, ppg) row r, and ep
  *   bf16 [B T, D] row b T + frame[r] -> ep_cur bf16 [B K, D] row r.
  * otb_rnnt_beam_commit: (h, c, pp) row r = (hn, cn, ppn) row r where tok[r] > 0, else (hg, cg, ppg) row r. */
@@ -612,7 +624,8 @@ int otb_rnnt_beam_step(const float* logp, int ldlp, const float* val, const int3
                        int max_len, const int32_t* t_len, float* score, int32_t* slot_u, int32_t* frame, int32_t* node, int32_t* par,
                        int64_t* tok, int32_t* node_par, int32_t* node_tok, int n_cap, int32_t* n_nodes, float* f_score,
                        int32_t* f_node, int32_t* f_u, int32_t* f_n, int32_t* done, int32_t* active, int32_t* ids, int32_t* lengths,
-                       float* out_score, void* stream);
+                       float* out_score, float beta, int32_t* lm_src, int32_t* lm_ext, int32_t* anc, int32_t* anc_tmp, int32_t* lm_pos,
+                       int Lpos, void* stream);
 int otb_rnnt_beam_gather(const int32_t* par, const int32_t* frame, int B, int K, int layers, int H, int D, int T, const float* h,
                          const float* c, const void* pp, const void* ep, float* hg, float* cg, void* ppg, void* ep_cur, void* stream);
 int otb_rnnt_beam_commit(const int64_t* tok, int rows, int layers, int H, int D, const float* hg, const float* cg, const void* ppg,

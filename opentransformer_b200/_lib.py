@@ -66,7 +66,7 @@ _SIGS = {
     'otb_ls_ce': (c_int, [_P, c_int, _P, c_int, c_int, c_float, c_int, _P, _P, _P, _P, c_int, c_int, _P]),
     'otb_beam_init': (c_int, [POINTER(BeamStateC), _P]),
     'otb_beam_step': (c_int, [_P, c_int, c_int, _P, c_int, c_float, _P, _P, POINTER(BeamStateC), _P, _P, _P]),
-    'otb_logsoftmax_topk': (c_int, [_P, c_int, c_int, _P, c_int, c_float, c_int, c_int, _P, _P, _P, c_int, _P]),
+    'otb_logsoftmax_topk': (c_int, [_P, c_int, c_int, _P, c_int, c_float, c_float, c_int, c_int, c_int, _P, _P, _P, c_int, _P]),
     'otb_sample_step': (c_int, [_P, c_int, c_int, POINTER(BeamStateC), _P, _P]),
     'otb_beam_reconstruct': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P]),
     'otb_beam_finalize': (c_int, [POINTER(BeamStateC), c_float, c_float, c_int, _P, _P, _P]),
@@ -117,9 +117,9 @@ _SIGS = {
     'otb_rnnt_loss': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, c_float, _P, _P]),
     'otb_rnnt_dlogits': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, _P, c_int, _P]),
     'otb_rnnt_greedy_step': (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P,
-                                     _P, _P, c_int, c_int, _P, _P, _P]),
+                                     _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     'otb_rnnt_beam_step': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P,
-                                   _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+                                   _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_float, _P, _P, _P, _P, _P, c_int, _P]),
     'otb_rnnt_beam_gather': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'otb_rnnt_beam_commit': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'otb_nbest_rescore': (c_int, [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_float, c_int, c_int, c_int64, _P, _P, _P, _P]),

@@ -347,6 +347,9 @@ const char* beam_init_launch(cudaStream_t stream, BeamState st) {
 
 // ------------------------------------------------------------------------------------------------
 // Fused  log_softmax(logits[row]) (+ lm_weight * lm_logp[row])  ->  top-k (values, vocabulary ids)
+// With lm_exempt >= 0 (the transducer's fusion, DESIGN.md 4.22) column lm_exempt (blank) keeps its plain log-prob and every
+// other column gets  + (lm_weight * lm_logp + lm_beta)  (+ lm_beta alone without lm_logp); out_logp then holds the plain
+// log-probs.  lm_exempt < 0 is the attention decoder's fusion, unchanged.
 // decoder/transformer.py:206 + recognize/speech2text.py:102-112 in ONE pass over the logits: the row is
 // staged in smem once (coalesced), so the [N,V] log-prob matrix is never written or re-read.  Values are
 // formed exactly as the stand-alone log-softmax kernel does (x - (max + log sum exp(x - max))) before the
@@ -357,7 +360,8 @@ static constexpr int TOPK_THREADS = 256;
 
 __global__ void __launch_bounds__(TOPK_THREADS) logsoftmax_topk_kernel(const float* __restrict__ logits, int ldl, int V,
                                                                        const float* __restrict__ lm_logp, int ld_lm,
-                                                                       float lm_weight, int k, float* __restrict__ out_val,
+                                                                       float lm_weight, float lm_beta, int lm_exempt, int k,
+                                                                       float* __restrict__ out_val,
                                                                        int* __restrict__ out_idx,
                                                                        float* __restrict__ out_logp, int ld_logp) {
     extern __shared__ float srow[];   // [V]
@@ -398,10 +402,15 @@ __global__ void __launch_bounds__(TOPK_THREADS) logsoftmax_topk_kernel(const flo
     const float lse = bc;
     const float* lm = lm_logp ? lm_logp + (size_t)row * ld_lm : nullptr;
     for (int i = tid; i < V; i += TOPK_THREADS) {
-        float v = srow[i] - lse;
-        if (lm) v = v + lm_weight * lm[i];
+        const float p = srow[i] - lse;
+        float v = p;
+        if (lm_exempt < 0) {
+            if (lm) v = v + lm_weight * lm[i];
+        } else if (i != lm_exempt) {
+            v = lm ? v + (lm_weight * lm[i] + lm_beta) : v + lm_beta;
+        }
         srow[i] = v;
-        if (out_logp) out_logp[(size_t)row * ld_logp + i] = v;
+        if (out_logp) out_logp[(size_t)row * ld_logp + i] = lm_exempt < 0 ? v : p;
     }
     __syncthreads();
     // per-warp top-k over a contiguous slice: k rounds of (lane-local scan of smem, warp arg-max), round r taking the best
@@ -444,15 +453,17 @@ __global__ void __launch_bounds__(TOPK_THREADS) logsoftmax_topk_kernel(const flo
 }
 
 const char* logsoftmax_topk_launch(cudaStream_t stream, const float* logits, int ldl, int V, const float* lm_logp,
-                                   int ld_lm, float lm_weight, int k, int rows, float* out_val, int* out_idx,
-                                   float* out_logp, int ld_logp) {
+                                   int ld_lm, float lm_weight, float lm_beta, int lm_exempt, int k, int rows, float* out_val,
+                                   int* out_idx, float* out_logp, int ld_logp) {
     if (k < 1 || k > KMAX) return "logsoftmax_topk: k must be in [1,16]";
+    if (lm_exempt >= V) return "logsoftmax_topk: the LM-exempt column must be below V";
+    if (lm_exempt < 0 && lm_beta != 0.f) return "logsoftmax_topk: lm_beta needs an LM-exempt column";
     if (V < 1 || V > 48 * 1024) return "logsoftmax_topk: vocabulary too large for one CTA's shared memory";
     // past V the scan has nothing left to pick and would return its sentinel (-inf, id 0x7fffffff) as a token
     if (k > V) return "logsoftmax_topk: k must not exceed the vocabulary size V";
     const size_t smem = (size_t)V * sizeof(float);
     return launch<logsoftmax_topk_kernel>(dim3(rows), dim3(TOPK_THREADS), smem, stream, logits, ldl, V, lm_logp, ld_lm,
-                                          lm_weight, k, out_val, out_idx, out_logp, ld_logp);
+                                          lm_weight, lm_beta, lm_exempt, k, out_val, out_idx, out_logp, ld_logp);
 }
 
 }  // namespace otb

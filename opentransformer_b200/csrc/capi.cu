@@ -327,11 +327,11 @@ int otb_beam_step(const float* logp, int ldl, int V, const float* lm_logp, int l
                                           reinterpret_cast<long long*>(dbg_ktok), dbg_offs, topk_val, topk_idx));
 }
 
-int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, int k,
-                        int rows, float* out_val, int32_t* out_idx, float* out_logp, int ld_logp, void* stream) {
+int otb_logsoftmax_topk(const float* logits, int ldl, int V, const float* lm_logp, int ld_lm, float lm_weight, float lm_beta,
+                        int lm_exempt, int k, int rows, float* out_val, int32_t* out_idx, float* out_logp, int ld_logp, void* stream) {
     if (!logits || !out_val || !out_idx || rows < 1) return fail("otb_logsoftmax_topk", "bad arguments");
-    RET("otb_logsoftmax_topk", logsoftmax_topk_launch(ST(stream), logits, ldl, V, lm_logp, ld_lm, lm_weight, k, rows,
-                                                      out_val, out_idx, out_logp, ld_logp));
+    RET("otb_logsoftmax_topk", logsoftmax_topk_launch(ST(stream), logits, ldl, V, lm_logp, ld_lm, lm_weight, lm_beta, lm_exempt, k,
+                                                      rows, out_val, out_idx, out_logp, ld_logp));
 }
 
 int otb_sample_step(const float* logits, int ldl, int V, const otb_beam_state* st, const int32_t* seed, void* stream) {
@@ -684,28 +684,31 @@ int otb_rnnt_dlogits(const float* logits, int ld, int rows, int64_t row0, int V,
 int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const float* h_new, const float* c_new, const void* pp_new,
                          float* h, float* c, void* pp, int layers, int B, int H, int D, const void* ep, int T, void* ep_cur,
                          const int32_t* t_len, int32_t* frame, int32_t* n_sym, int32_t* n_out, int32_t* ids, int max_len,
-                         int max_sym, float* score, int32_t* active, void* stream) {
+                         int max_sym, float* score, int32_t* active, const float* val, int32_t* emit, int32_t* lm_pos,
+                         void* stream) {
     if (!idx || !logp || !h_new || !c_new || !pp_new || !h || !c || !pp || !ep || !ep_cur || !t_len || !frame || !n_sym || !n_out ||
         !ids || !score || !active)
         return fail("otb_rnnt_greedy_step", "null operand");
     RET("otb_rnnt_greedy_step",
         rnnt_greedy_step_launch(ST(stream), idx, logp, ldlp, h_new, c_new, reinterpret_cast<const bf16*>(pp_new), h, c,
                                 reinterpret_cast<bf16*>(pp), layers, B, H, D, reinterpret_cast<const bf16*>(ep), T,
-                                reinterpret_cast<bf16*>(ep_cur), t_len, frame, n_sym, n_out, ids, max_len, max_sym, score, active));
+                                reinterpret_cast<bf16*>(ep_cur), t_len, frame, n_sym, n_out, ids, max_len, max_sym, score, active, val,
+                                emit, lm_pos));
 }
 
 int otb_rnnt_beam_step(const float* logp, int ldlp, const float* val, const int32_t* idx, int k1, int B, int K, int W, int V, int T,
                        int max_len, const int32_t* t_len, float* score, int32_t* slot_u, int32_t* frame, int32_t* node, int32_t* par,
                        int64_t* tok, int32_t* node_par, int32_t* node_tok, int n_cap, int32_t* n_nodes, float* f_score,
                        int32_t* f_node, int32_t* f_u, int32_t* f_n, int32_t* done, int32_t* active, int32_t* ids, int32_t* lengths,
-                       float* out_score, void* stream) {
+                       float* out_score, float beta, int32_t* lm_src, int32_t* lm_ext, int32_t* anc, int32_t* anc_tmp, int32_t* lm_pos,
+                       int Lpos, void* stream) {
     if (!logp || !val || !idx || !t_len || !score || !slot_u || !frame || !node || !par || !tok || !node_par || !node_tok ||
         !n_nodes || !f_score || !f_node || !f_u || !f_n || !done || !active || !ids || !lengths || !out_score)
         return fail("otb_rnnt_beam_step", "null operand");
     RET("otb_rnnt_beam_step",
         rnnt_beam_step_launch(ST(stream), logp, ldlp, val, idx, k1, B, K, W, V, T, max_len, t_len, score, slot_u, frame, node, par,
                               reinterpret_cast<long long*>(tok), node_par, node_tok, n_cap, n_nodes, f_score, f_node, f_u, f_n, done,
-                              active, ids, lengths, out_score));
+                              active, ids, lengths, out_score, beta, lm_src, lm_ext, anc, anc_tmp, lm_pos, Lpos));
 }
 
 int otb_rnnt_beam_gather(const int32_t* par, const int32_t* frame, int B, int K, int layers, int H, int D, int T, const float* h,

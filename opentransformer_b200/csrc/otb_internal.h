@@ -217,8 +217,8 @@ const char* beam_step_launch(cudaStream_t stream, const float* logp, int ldl, in
                              float lm_weight, BeamState st, long long* dbg_ktok, int* dbg_offs, const float* pre_val,
                              const int* pre_idx);
 const char* logsoftmax_topk_launch(cudaStream_t stream, const float* logits, int ldl, int V, const float* lm_logp,
-                                   int ld_lm, float lm_weight, int k, int rows, float* out_val, int* out_idx,
-                                   float* out_logp, int ld_logp);
+                                   int ld_lm, float lm_weight, float lm_beta, int lm_exempt, int k, int rows, float* out_val,
+                                   int* out_idx, float* out_logp, int ld_logp);
 const char* sample_step_launch(cudaStream_t stream, const float* logits, int ldl, int V, BeamState st, const int* seed);
 const char* beam_reconstruct_launch(cudaStream_t stream, BeamState st, long long* preds, int ld, int steps);
 const char* beam_finalize_launch(cudaStream_t stream, BeamState st, float penalty, float lamda, int nbest,
@@ -318,11 +318,13 @@ const char* rnnt_dlogits_launch(cudaStream_t st, const float* logits, int ld, in
 const char* rnnt_greedy_step_launch(cudaStream_t st, const int* idx, const float* logp, int ldlp, const float* h_new,
                                     const float* c_new, const bf16* pp_new, float* h, float* c, bf16* pp, int layers, int B, int H,
                                     int D, const bf16* ep, int T, bf16* ep_cur, const int* t_len, int* frame, int* n_sym, int* n_out,
-                                    int* ids, int max_len, int max_sym, float* score, int* active);
+                                    int* ids, int max_len, int max_sym, float* score, int* active, const float* val, int* emit,
+                                    int* lm_pos);
 const char* rnnt_beam_step_launch(cudaStream_t st, const float* logp, int ldlp, const float* val, const int* idx, int k1, int B, int K,
                                   int W, int V, int T, int max_len, const int* t_len, float* score, int* slot_u, int* frame, int* node,
                                   int* par, long long* tok, int* node_par, int* node_tok, int n_cap, int* n_nodes, float* f_score,
-                                  int* f_node, int* f_u, int* f_n, int* done, int* active, int* ids, int* lengths, float* out_score);
+                                  int* f_node, int* f_u, int* f_n, int* done, int* active, int* ids, int* lengths, float* out_score,
+                                  float beta, int* lm_src, int* lm_ext, int* anc, int* anc_tmp, int* lm_pos, int Lpos);
 const char* rnnt_beam_gather_launch(cudaStream_t st, const int* par, const int* frame, int B, int K, int layers, int H, int D, int T,
                                     const float* h, const float* c, const bf16* pp, const bf16* ep, float* hg, float* cg, bf16* ppg,
                                     bf16* ep_cur);

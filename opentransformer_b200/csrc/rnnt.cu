@@ -234,6 +234,9 @@ __global__ void __launch_bounds__(RNNT_WARPS * 32) rnnt_dlogits_kernel(const flo
 // out); its log-prob is added to the score.  A label is appended to ids and the predictor state computed from it (h_new,
 // c_new [layers, B, H] f32, pp_new [B, D] bf16) replaces the row's (h, c, pp); a blank moves the row to its next frame and
 // copies that frame's encoder projection into ep_cur, or ends the row (active -= 1).  Ended rows are left as they are.
+// LM fusion (val non-null): val [B] is the fused value of the arg-max (otb_logsoftmax_topk with blank exempt), and a
+// label adds it to the score in place of its log-prob; emit [B] (optional) gets 1 where the row emitted and 0 elsewhere,
+// lm_pos [B] (optional) the label's LM position n_out (1 .. max_len) where it emitted and -1 elsewhere.
 __global__ void __launch_bounds__(128) rnnt_greedy_step_kernel(const int* __restrict__ idx, const float* __restrict__ logp, int ldlp,
                                                                const float* __restrict__ h_new, const float* __restrict__ c_new,
                                                                const bf16* __restrict__ pp_new, float* __restrict__ h,
@@ -242,7 +245,9 @@ __global__ void __launch_bounds__(128) rnnt_greedy_step_kernel(const int* __rest
                                                                bf16* __restrict__ ep_cur, const int* __restrict__ t_len,
                                                                int* __restrict__ frame, int* __restrict__ n_sym,
                                                                int* __restrict__ n_out, int* __restrict__ ids, int max_len,
-                                                               int max_sym, float* __restrict__ score, int* __restrict__ active) {
+                                                               int max_sym, float* __restrict__ score, int* __restrict__ active,
+                                                               const float* __restrict__ val, int* __restrict__ emit,
+                                                               int* __restrict__ lm_pos) {
     __shared__ int s_act;      // 0: ended, 1: emitted, 2: moved to the next frame
     __shared__ int s_t;
     const int b = blockIdx.x;
@@ -252,7 +257,7 @@ __global__ void __launch_bounds__(128) rnnt_greedy_step_kernel(const int* __rest
         if (t < Tb) {
             const int k = n_out[b];
             const int tok = (n_sym[b] < max_sym && k < max_len) ? idx[b] : 0;
-            score[b] += logp[(size_t)b * ldlp + tok];
+            score[b] += (val != nullptr && tok != 0) ? val[b] : logp[(size_t)b * ldlp + tok];
             if (tok != 0) {
                 ids[(size_t)b * max_len + k] = tok;
                 n_out[b] = k + 1;
@@ -270,6 +275,8 @@ __global__ void __launch_bounds__(128) rnnt_greedy_step_kernel(const int* __rest
             }
         }
         s_act = act;
+        if (emit) emit[b] = act == 1;
+        if (lm_pos) lm_pos[b] = act == 1 ? n_out[b] : -1;
     }
     __syncthreads();
     if (s_act == 1) {
@@ -340,11 +347,13 @@ const char* rnnt_dlogits_launch(cudaStream_t st, const float* logits, int ld, in
 const char* rnnt_greedy_step_launch(cudaStream_t st, const int* idx, const float* logp, int ldlp, const float* h_new,
                                     const float* c_new, const bf16* pp_new, float* h, float* c, bf16* pp, int layers, int B, int H,
                                     int D, const bf16* ep, int T, bf16* ep_cur, const int* t_len, int* frame, int* n_sym, int* n_out,
-                                    int* ids, int max_len, int max_sym, float* score, int* active) {
+                                    int* ids, int max_len, int max_sym, float* score, int* active, const float* val, int* emit,
+                                    int* lm_pos) {
     if (B < 1 || T < 1 || layers < 1 || H < 1 || D < 1) return "rnnt_greedy_step: empty problem";
     if (max_len < 1 || max_sym < 1) return "rnnt_greedy_step: need max_len >= 1 and max_sym >= 1";
     return launch<rnnt_greedy_step_kernel>(B, 128, 0, st, idx, logp, ldlp, h_new, c_new, pp_new, h, c, pp, layers, B, H, D, ep, T,
-                                           ep_cur, t_len, frame, n_sym, n_out, ids, max_len, max_sym, score, active);
+                                           ep_cur, t_len, frame, n_sym, n_out, ids, max_len, max_sym, score, active, val, emit,
+                                           lm_pos);
 }
 
 }  // namespace otb

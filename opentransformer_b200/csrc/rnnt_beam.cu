@@ -28,8 +28,20 @@ __device__ __forceinline__ bool same_chain(const int* __restrict__ par, const in
     return true;
 }
 
+// The end rule's bound of kept candidate c: its score, plus beta per label it may still take when beta > 0
+__device__ __forceinline__ float end_bound(const float* c_sc, const int* s_u, int c, int KL, float beta, int max_len) {
+    if (!(beta > 0.f)) return c_sc[c];
+    const int a = c / (KL + 1), u = s_u[a] + (c - a * (KL + 1) > 0);
+    return c_sc[c] + beta * (float)(max_len - u);
+}
+
 // Candidate c = j (K' + 1) + q of slot j: q = 0 blank, q >= 1 the q-th best label.  That index is the formation order the
 // tie rule uses (parent slot ascending, blank before labels, labels in top-k order).
+// LM fusion (DESIGN.md 4.22) changes no decision here: val already holds the fused label values.  beta > 0 (a bonus per
+// label) only loosens the end bound to logsumexp(s + beta (max_len - u)).  lm_src / lm_ext (optional, i32 [B K]) tell the
+// LM carry each new slot's parent row b K + par and whether it took a label; anc (optional, i32 [B K, Lpos], with anc_tmp
+// the same size of scratch and lm_pos i32 [B K]) lists the LM cache rows b n_cap + node of each slot's labels from
+// position 0 (<S/E>, node 0), and lm_pos is the new label's position u where the slot took one, -1 elsewhere.
 __global__ void __launch_bounds__(RNNT_BEAM_THREADS, 1)
     rnnt_beam_step_kernel(const float* __restrict__ logp, int ldlp, const float* __restrict__ val, const int* __restrict__ idx,
                           int k1, int K, int W, int V, int T, int max_len, const int* __restrict__ t_len, float* __restrict__ score,
@@ -37,10 +49,12 @@ __global__ void __launch_bounds__(RNNT_BEAM_THREADS, 1)
                           long long* __restrict__ tok, int* __restrict__ node_par, int* __restrict__ node_tok, int n_cap,
                           int* __restrict__ n_nodes, float* __restrict__ f_score, int* __restrict__ f_node, int* __restrict__ f_u,
                           int* __restrict__ f_n, int* __restrict__ done, int* __restrict__ active, int* __restrict__ ids,
-                          int* __restrict__ lengths, float* __restrict__ out_score) {
+                          int* __restrict__ lengths, float* __restrict__ out_score, float beta, int* __restrict__ lm_src,
+                          int* __restrict__ lm_ext, int* __restrict__ anc, int* __restrict__ anc_tmp, int* __restrict__ lm_pos,
+                          int Lpos) {
     __shared__ float s_sc[RNNT_BEAM_KMAX], s_final[RNNT_BEAM_KMAX], s_merge[RNNT_BEAM_KMAX];
     __shared__ int s_u[RNNT_BEAM_KMAX], s_fr[RNNT_BEAM_KMAX], s_nd[RNNT_BEAM_KMAX], s_partner[RNNT_BEAM_KMAX];
-    __shared__ int s_sel[RNNT_BEAM_KMAX], s_new_node[RNNT_BEAM_KMAX];
+    __shared__ int s_sel[RNNT_BEAM_KMAX], s_new_node[RNNT_BEAM_KMAX], s_from[RNNT_BEAM_KMAX], s_lab[RNNT_BEAM_KMAX];
     __shared__ float c_sc[RNNT_BEAM_THREADS];
     __shared__ int c_tok[RNNT_BEAM_THREADS];
     __shared__ int s_end;
@@ -49,6 +63,11 @@ __global__ void __launch_bounds__(RNNT_BEAM_THREADS, 1)
         if (tid < K) {
             par[row0 + tid] = tid;
             tok[row0 + tid] = 0;
+            if (lm_src) {
+                lm_src[row0 + tid] = row0 + tid;
+                lm_ext[row0 + tid] = 0;
+            }
+            if (anc) lm_pos[row0 + tid] = -1;
         }
         return;
     }
@@ -168,12 +187,13 @@ __global__ void __launch_bounds__(RNNT_BEAM_THREADS, 1)
             }
         }
         n_nodes[b] = nn;
-        // end: no live hypothesis, or F full and the live set's total probability no more than F's worst
+        // end: no live hypothesis, or F full and the live set's total probability no more than F's worst.  With a label
+        // bonus beta > 0 a hypothesis can gain up to beta (max_len - u): the bound adds it (beta <= 0: the plain scores).
         bool end = n_sel == 0;
         if (!end && nf == W) {
-            const float m = c_sc[s_sel[0]];
-            float s = 0.f;
-            for (int r = 0; r < n_sel; ++r) s += expf(c_sc[s_sel[r]] - m);
+            float m = -INFINITY, s = 0.f;
+            for (int r = 0; r < n_sel; ++r) m = fmaxf(m, end_bound(c_sc, s_u, s_sel[r], KL, beta, max_len));
+            for (int r = 0; r < n_sel; ++r) s += expf(end_bound(c_sc, s_u, s_sel[r], KL, beta, max_len) - m);
             end = m + logf(s) <= fs[W - 1];
         }
         s_end = end;
@@ -185,18 +205,53 @@ __global__ void __launch_bounds__(RNNT_BEAM_THREADS, 1)
     __syncthreads();
     if (tid < K) {
         const size_t r = (size_t)row0 + tid;
+        int a = tid, lab = 0;
         if (tid < n_sel) {
-            const int c = s_sel[tid], a = c / (KL + 1), qq = c - a * (KL + 1);
+            const int c = s_sel[tid], qq = c - c / (KL + 1) * (KL + 1);
+            a = c / (KL + 1);
+            lab = qq > 0;
             score[r] = c_sc[c];
-            slot_u[r] = s_u[a] + (qq > 0);
+            slot_u[r] = s_u[a] + lab;
             frame[r] = s_fr[a] + (qq == 0);
             node[r] = s_new_node[tid];
             par[r] = a;
-            tok[r] = qq > 0 ? c_tok[c] : 0;
+            tok[r] = lab ? c_tok[c] : 0;
         } else {            // empty: keeps its own (finite) predictor state and frame
             score[r] = -INFINITY;
             par[r] = tid;
             tok[r] = 0;
+        }
+        if (lm_src) {
+            lm_src[r] = row0 + a;
+            lm_ext[r] = lab;
+        }
+        s_from[tid] = a;
+        s_lab[tid] = lab;
+    }
+    // Transformer LM: a slot's cache rows are its parent's (positions 0 .. u_parent), plus its new node's at u where it took a
+    // label; copied through anc_tmp, since a parent's row can be a child's destination
+    if (anc != nullptr) {
+        __syncthreads();
+        for (int s = 0; s < K; ++s) {
+            const int a = s_from[s];
+            if (a == s) continue;
+            const int* from = anc + (size_t)(row0 + a) * Lpos;
+            int* to = anc_tmp + (size_t)(row0 + s) * Lpos;
+            for (int p = tid; p <= s_u[a]; p += RNNT_BEAM_THREADS) to[p] = from[p];
+        }
+        __syncthreads();
+        for (int s = 0; s < K; ++s) {
+            const int a = s_from[s];
+            if (a == s) continue;
+            const int* from = anc_tmp + (size_t)(row0 + s) * Lpos;
+            int* to = anc + (size_t)(row0 + s) * Lpos;
+            for (int p = tid; p <= s_u[a]; p += RNNT_BEAM_THREADS) to[p] = from[p];
+        }
+        if (tid < K) {
+            const int u = s_u[s_from[tid]] + 1;
+            const bool lab = s_lab[tid];
+            if (lab) anc[(size_t)(row0 + tid) * Lpos + u] = b * n_cap + s_new_node[tid];
+            lm_pos[row0 + tid] = lab ? u : -1;
         }
     }
     if (s_end) {            // the n-best, best first: ids padded with 0, unfilled entries length 0 and score -inf
@@ -269,7 +324,8 @@ __global__ void __launch_bounds__(128) rnnt_beam_commit_kernel(const long long* 
 const char* rnnt_beam_step_launch(cudaStream_t st, const float* logp, int ldlp, const float* val, const int* idx, int k1, int B, int K,
                                   int W, int V, int T, int max_len, const int* t_len, float* score, int* slot_u, int* frame, int* node,
                                   int* par, long long* tok, int* node_par, int* node_tok, int n_cap, int* n_nodes, float* f_score,
-                                  int* f_node, int* f_u, int* f_n, int* done, int* active, int* ids, int* lengths, float* out_score) {
+                                  int* f_node, int* f_u, int* f_n, int* done, int* active, int* ids, int* lengths, float* out_score,
+                                  float beta, int* lm_src, int* lm_ext, int* anc, int* anc_tmp, int* lm_pos, int Lpos) {
     if (B < 1 || T < 1) return "rnnt_beam_step: empty batch";
     if (K < 1 || K > RNNT_BEAM_KMAX) return "rnnt_beam_step: beam width K must be in [1, 15]";
     if (W < 1 || W > K) return "rnnt_beam_step: nbest W must be in [1, K]";
@@ -278,9 +334,13 @@ const char* rnnt_beam_step_launch(cudaStream_t st, const float* logp, int ldlp, 
     if (ldlp < V) return "rnnt_beam_step: log-prob rows narrower than V";
     if (max_len < 1 || max_len > 1023) return "rnnt_beam_step: max_len must be in [1, 1023]";
     if ((long long)n_cap < (long long)K * (T + max_len) + 1) return "rnnt_beam_step: node table narrower than K (T + max_len) + 1";
+    if ((lm_src == nullptr) != (lm_ext == nullptr)) return "rnnt_beam_step: lm_src and lm_ext go together";
+    if (anc != nullptr && (anc_tmp == nullptr || lm_pos == nullptr || Lpos < max_len + 1))
+        return "rnnt_beam_step: anc needs anc_tmp, lm_pos and Lpos >= max_len + 1";
+    if ((long long)B * n_cap > 0x7fffffffLL) return "rnnt_beam_step: B n_cap must fit in 32 bits";
     return launch<rnnt_beam_step_kernel>(B, RNNT_BEAM_THREADS, 0, st, logp, ldlp, val, idx, k1, K, W, V, T, max_len, t_len, score,
                                          slot_u, frame, node, par, tok, node_par, node_tok, n_cap, n_nodes, f_score, f_node, f_u, f_n,
-                                         done, active, ids, lengths, out_score);
+                                         done, active, ids, lengths, out_score, beta, lm_src, lm_ext, anc, anc_tmp, lm_pos, Lpos);
 }
 
 const char* rnnt_beam_gather_launch(cudaStream_t st, const int* par, const int* frame, int B, int K, int layers, int H, int D, int T,

@@ -402,8 +402,11 @@ def log_softmax(x, V, out=None):
     return out
 
 
-def logsoftmax_topk(logits, V, k, lm_logp=None, lm_weight=0.0, out_val=None, out_idx=None, out_logp=None):
-    """Fused log-softmax (+ LM shallow fusion) + per-row top-k.  logits f32 [rows, ld]."""
+def logsoftmax_topk(logits, V, k, lm_logp=None, lm_weight=0.0, out_val=None, out_idx=None, out_logp=None, lm_beta=0.0,
+                    lm_exempt=-1):
+    """Fused log-softmax (+ LM shallow fusion) + per-row top-k.  logits f32 [rows, ld].  lm_exempt >= 0 (the transducer's
+    fusion): that column (blank) gets no LM term, every other one gets + (lm_weight * lm_logp + lm_beta), and out_logp keeps
+    the plain log-probs; the defaults are the attention decoder's fusion."""
     _need(logits, torch.float32, 'logits')
     rows = logits.shape[0]
     if out_val is None:
@@ -411,7 +414,7 @@ def logsoftmax_topk(logits, V, k, lm_logp=None, lm_weight=0.0, out_val=None, out
     if out_idx is None:
         out_idx = torch.empty(rows, k, dtype=torch.int32, device=logits.device)
     check(_lib.lib().otb_logsoftmax_topk(_p(logits), logits.stride(0), V, _p(lm_logp),
-                                         lm_logp.stride(0) if lm_logp is not None else 0, lm_weight, k, rows,
+                                         lm_logp.stride(0) if lm_logp is not None else 0, lm_weight, lm_beta, lm_exempt, k, rows,
                                          _p(out_val), _p(out_idx), _p(out_logp),
                                          out_logp.stride(0) if out_logp is not None else 0, _stream()),
           'otb_logsoftmax_topk')
@@ -1475,30 +1478,42 @@ def rnnt_dlogits(logits, row0, V, B, T, U1, t_len, u_len, labels, lp, grad, out=
 
 
 def rnnt_greedy_step(idx, logp, h_new, c_new, pp_new, h, c, pp, ep, T, ep_cur, t_len, frame, n_sym, n_out, ids, max_sym, score,
-                     active):
+                     active, val=None, emit=None, lm_pos=None):
     """One step of batched greedy transducer search (otb_rnnt_greedy_step): the decision of every row from the arg-max idx
     i32 [B] and log-probs logp f32 [B, ld] of the joint, the predictor state (h, c f32 [layers, B, H], pp bf16 [B, D]) moved
     forward from (h_new, c_new, pp_new) where a row emitted, and the frame state (ep_cur, frame, n_sym, n_out, ids i32
-    [B, max_len], score, active) updated in place."""
+    [B, max_len], score, active) updated in place.  LM fusion: val f32 [B] the arg-max's fused value, which an emitted label
+    adds to the score; emit i32 [B] <- 1 where the row emitted; lm_pos i32 [B] <- the label's LM position n_out, else -1."""
+    for t, name in ((val, 'val'), (emit, 'emit'), (lm_pos, 'lm_pos')):
+        if t is not None:
+            _need(t, torch.float32 if name == 'val' else torch.int32, name)
     layers, B, H = h.shape
     D = pp.shape[1]
     check(_lib.lib().otb_rnnt_greedy_step(_p(idx), _p(logp), logp.stride(0), _p(h_new), _p(c_new), _p(pp_new), _p(h), _p(c), _p(pp),
                                           layers, B, H, D, _p(ep), T, _p(ep_cur), _p(t_len), _p(frame), _p(n_sym), _p(n_out),
-                                          _p(ids), ids.shape[1], max_sym, _p(score), _p(active), _stream()), 'otb_rnnt_greedy_step')
+                                          _p(ids), ids.shape[1], max_sym, _p(score), _p(active), _p(val), _p(emit), _p(lm_pos),
+                                          _stream()), 'otb_rnnt_greedy_step')
     _count()
 
 
 RNNT_BEAM_MAX = 15          # beam width: K + 1 log-probs per slot from logsoftmax_topk, whose k is at most 16
 
 
-def rnnt_beam_step(logp, val, idx, V, T, t_len, state, out):
+def rnnt_beam_step(logp, val, idx, V, T, t_len, state, out, beta=0.0, lm=None):
     """One step of the transducer's ALSD beam search (otb_rnnt_beam_step) for every utterance not yet ended, from the
     joint's log-probs at each slot: logp f32 [B*K, ld] and the top min(K + 1, V) (val f32, idx i32 [B*K, k1]) of
     logsoftmax_topk.  state: dict of the search's device arrays, updated in place -- the slots (score f32, u, frame, node i32
     [B*K]), the step's actions (par i32, tok i64 [B*K]), the node table (node_par, node_tok i32 [B, n_cap], n_nodes i32 [B]),
     the n-best so far (f_score f32, f_node, f_u i32 [B, W], f_n i32 [B]), done i32 [B] and active i32 [1].  out: (ids i32
-    [B, W, max_len], lengths i32 [B, W], scores f32 [B, W]), written for each utterance when it ends."""
+    [B, W, max_len], lengths i32 [B, W], scores f32 [B, W]), written for each utterance when it ends.
+    LM fusion (val holds the fused label values): beta > 0 loosens the end bound by beta per label still to come; lm, a dict
+    of i32 outputs for the LM carry: src and ext [B*K], and for the Transformer LM anc / anc_tmp [B*K, Lpos] and pos [B*K]."""
     s = state
+    lm = lm or {}
+    for k in ('src', 'ext', 'anc', 'anc_tmp', 'pos'):
+        if lm.get(k) is not None:
+            _need(lm[k], torch.int32, k)
+    anc = lm.get('anc')
     _need(logp, torch.float32, 'logp'); _need(val, torch.float32, 'val'); _need(idx, torch.int32, 'idx')
     B, W = s['f_score'].shape
     K = s['score'].numel() // B
@@ -1507,7 +1522,9 @@ def rnnt_beam_step(logp, val, idx, V, T, t_len, state, out):
                                         _p(t_len), _p(s['score']), _p(s['u']), _p(s['frame']), _p(s['node']), _p(s['par']),
                                         _p(s['tok']), _p(s['node_par']), _p(s['node_tok']), s['node_par'].shape[1],
                                         _p(s['n_nodes']), _p(s['f_score']), _p(s['f_node']), _p(s['f_u']), _p(s['f_n']),
-                                        _p(s['done']), _p(s['active']), _p(ids), _p(lengths), _p(scores), _stream()),
+                                        _p(s['done']), _p(s['active']), _p(ids), _p(lengths), _p(scores), float(beta),
+                                        _p(lm.get('src')), _p(lm.get('ext')), _p(anc), _p(lm.get('anc_tmp')), _p(lm.get('pos')),
+                                        anc.shape[1] if anc is not None else 0, _stream()),
           'otb_rnnt_beam_step')
     _count()
 

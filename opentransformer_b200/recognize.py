@@ -26,7 +26,7 @@ import torch
 
 from . import ops
 from . import train
-from .ctc_fusion import CTCFusedSearch
+from .ctc_fusion import CTCFusedSearch, FusedLMRows
 from .lm import LMCache
 from .model import ctc_align_logits
 from .modules import encoder_attn_weights
@@ -818,13 +818,14 @@ class CTCRecognizer(Recognizer):
         return best if self.idx2unit is None else self.translate(best)
 
 
-class _TransducerGreedy:
+class _TransducerGreedy(FusedLMRows):
     """The greedy transducer search of one geometry (B utterances, T' frames) over one set of model operands: its buffers,
-    and the CUDA graph of STEPS steps once captured."""
+    and the CUDA graph of STEPS steps once captured.  With an LM (shallow fusion, DESIGN.md 4.22) each row also carries
+    log p_lm(. | <S/E>, its labels): the LM runs on every row's arg-max after the step, and the rows that emitted keep it."""
 
     STEPS = 16          # search steps per graph replay: the host reads the active-row counter once per replay
 
-    def __init__(self, model, op, B, T2, max_len, max_sym, device, use_graph):
+    def __init__(self, model, op, B, T2, max_len, max_sym, device, use_graph, lm=None, lm_weight=0.0, beta=0.0):
         self.model, self.op, self.B, self.T2 = model, op, B, T2
         self.max_sym, self.use_graph = max_sym, use_graph
         D, H, L = model.joint.inner_size, model.decoder.hidden_size, model.decoder.num_layers
@@ -844,6 +845,15 @@ class _TransducerGreedy:
         self.active = torch.zeros(1, **i32)
         self.bar = torch.zeros(2, **i32)            # the LSTM kernels' grid barrier, owned here: a graph must not allocate one
         self.graph = None
+        self.lm, self.lm_weight, self.beta = lm, float(lm_weight), float(beta)
+        if lm is not None:
+            # one LM row per utterance; the Transformer LM's cache is linear, position p of utterance b at row b L + p
+            L = max_len + 1
+            row = torch.arange(B, device=device)
+            self._init_lm(lm, B, L, B * L, row * L, torch.zeros_like(row), device)
+            if self.anc is not None:
+                self.anc.copy_(row[:, None] * L + torch.arange(L, device=device))
+            self.lm_pk = lm._pack.get()
 
     def _predict(self, hidden):
         """The prediction network one token on from hidden (None: the zero state) for self.tok -> (h, c, dec_proj(h))."""
@@ -857,11 +867,19 @@ class _TransducerGreedy:
         for _ in range(self.STEPS):
             hj = ops.rnnt_joint(self.ep_cur, self.pp, self.B, 1, 1)
             logits = ops.linear(hj, op['out_w'], op['out_b'], ops.EPI_BIAS, out_f32=True, n_out=m.joint.ld_logits)
-            ops.logsoftmax_topk(logits, m.vocab_size, 1, out_val=self.val, out_idx=self.idx, out_logp=self.logp)
+            if self.lm is None:
+                ops.logsoftmax_topk(logits, m.vocab_size, 1, out_val=self.val, out_idx=self.idx, out_logp=self.logp)
+            else:
+                _fused_topk(self, logits, m.vocab_size, 1)
             self.tok.copy_(self.idx.view(-1))
             h, c, pp = self._predict((self.h, self.c))          # every row's next state, kept only where a label is emitted
+            fused = self.lm is not None
             ops.rnnt_greedy_step(self.idx, self.logp, h, c, pp, self.h, self.c, self.pp, self.ep, self.T2, self.ep_cur,
-                                 self.t_len, self.frame, self.n_sym, self.n_out, self.ids, self.max_sym, self.score, self.active)
+                                 self.t_len, self.frame, self.n_sym, self.n_out, self.ids, self.max_sym, self.score, self.active,
+                                 val=self.val if fused else None, emit=self.ext if fused else None,
+                                 lm_pos=self.pos if fused else None)
+            if fused:
+                self.follow(None)                               # the LM on every row's arg-max, kept where it was emitted
 
     def run(self, mem, lengths):
         B, T2 = self.B, self.T2
@@ -877,6 +895,8 @@ class _TransducerGreedy:
         self.h.copy_(h)
         self.c.copy_(c)
         self.pp.copy_(pp)
+        if self.lm is not None:
+            self.start_lm()
         # every step moves each live row one frame on or emits one of its at most max_len labels
         blocks = -(-(T2 + self.ids.shape[1]) // self.STEPS)
         for _ in range(blocks):
@@ -893,15 +913,17 @@ class _TransducerGreedy:
         return self.ids.clone(), self.n_out.clone(), self.score.clone()
 
 
-class _TransducerALSD:
+class _TransducerALSD(FusedLMRows):
     """The ALSD beam search of one geometry (B utterances, T' frames, K slots each, an n-best of W, max_len labels) over one
     set of model operands: its buffers, the node table, and the CUDA graph of STEPS steps once captured.  Every array is at
     B*K slot rows; the step is rnnt_joint -> output layer -> logsoftmax_topk -> otb_rnnt_beam_step -> otb_rnnt_beam_gather ->
-    the prediction network one token on -> otb_rnnt_beam_commit."""
+    the prediction network one token on -> otb_rnnt_beam_commit.  With an LM (shallow fusion, DESIGN.md 4.22) each slot
+    also carries log p_lm(. | <S/E>, its labels), following its parent slot and advanced by the LM where it took a label;
+    the Transformer LM's K/V are stored once per node of the node table, [blocks, B n_cap, d], node 0 the <S/E>."""
 
     STEPS = 16
 
-    def __init__(self, model, op, B, T2, K, W, max_len, device, use_graph):
+    def __init__(self, model, op, B, T2, K, W, max_len, device, use_graph, lm=None, lm_weight=0.0, beta=0.0):
         self.model, self.op, self.B, self.T2, self.K, self.use_graph = model, op, B, T2, K, use_graph
         D, H, L = model.joint.inner_size, model.decoder.hidden_size, model.decoder.num_layers
         BK, V = B * K, model.vocab_size
@@ -925,6 +947,13 @@ class _TransducerALSD:
         self.out = (torch.zeros(B, W, max_len, **i32), torch.zeros(B, W, **i32), torch.empty(B, W, **f32))
         self.bar = torch.zeros(2, **i32)
         self.graph = None
+        self.lm, self.lm_weight, self.beta = lm, float(lm_weight), float(beta)
+        if lm is not None:
+            row = torch.arange(BK, device=device)
+            self._init_lm(lm, BK, max_len + 1, B * n_cap, (row // K) * n_cap, torch.where(row % K == 0, 0, -1), device)
+            self.tok = self.state['tok']                # the LM reads the label each slot took
+            self.lm_out = dict(src=self.src, ext=self.ext, anc=self.anc, anc_tmp=self.anc_tmp, pos=self.pos)
+            self.lm_pk = lm._pack.get()
 
     def _predict(self, hidden):
         op = self.op
@@ -944,10 +973,18 @@ class _TransducerALSD:
             box['logits'] = ops.linear(box['hj'], op['out_w'], op['out_b'], ops.EPI_BIAS, out_f32=True, n_out=m.joint.ld_logits)
 
         def topk():
-            ops.logsoftmax_topk(box['logits'], m.vocab_size, self.k1, out_val=self.val, out_idx=self.idx, out_logp=self.logp)
+            if self.lm is None:
+                ops.logsoftmax_topk(box['logits'], m.vocab_size, self.k1, out_val=self.val, out_idx=self.idx,
+                                    out_logp=self.logp)
+            else:
+                _fused_topk(self, box['logits'], m.vocab_size, self.k1)
 
         def beam_step():
-            ops.rnnt_beam_step(self.logp, self.val, self.idx, m.vocab_size, self.T2, self.t_len, s, self.out)
+            if self.lm is None:
+                ops.rnnt_beam_step(self.logp, self.val, self.idx, m.vocab_size, self.T2, self.t_len, s, self.out)
+            else:
+                ops.rnnt_beam_step(self.logp, self.val, self.idx, m.vocab_size, self.T2, self.t_len, s, self.out, self.beta,
+                                   self.lm_out)
 
         def gather():
             ops.rnnt_beam_gather(s['par'], s['frame'], self.K, self.h, self.c, self.pp, self.ep, self.T2, self.hg, self.cg,
@@ -958,7 +995,10 @@ class _TransducerALSD:
 
         def commit():
             ops.rnnt_beam_commit(s['tok'], self.hg, self.cg, self.ppg, *box['new'], self.h, self.c, self.pp)
-        return [joint, output_layer, topk, beam_step, gather, predictor, commit]
+
+        def lm():                   # every slot's LM rows from its parent, the LM one token on where it took a label
+            self.follow(self.src)
+        return [joint, output_layer, topk, beam_step, gather, predictor, commit] + ([lm] if self.lm is not None else [])
 
     def _steps(self):
         for _ in range(self.STEPS):
@@ -985,6 +1025,8 @@ class _TransducerALSD:
         self.h.copy_(h)
         self.c.copy_(c)
         self.pp.copy_(pp)
+        if self.lm is not None:
+            self.start_lm()
 
     def run(self, mem, lengths):
         self.start(mem, lengths)
@@ -1007,6 +1049,13 @@ class _TransducerALSD:
         return tuple(t.clone() for t in self.out)
 
 
+def _fused_topk(search, logits, V, k):
+    """logsoftmax_topk with the transducer's fusion: labels valued lp + lm_weight * lm + beta, blank (column 0) its plain
+    log-prob, out_logp the plain log-probs.  At lm_weight 0 the LM rows are not read (0 * -inf would be NaN)."""
+    ops.logsoftmax_topk(logits, V, k, search.lm_rows if search.lm_weight != 0 else None, search.lm_weight, out_val=search.val,
+                        out_idx=search.idx, out_logp=search.logp, lm_beta=search.beta, lm_exempt=0)
+
+
 class TransducerRecognizer(Recognizer):
     """Search of a TransducerModel (DESIGN.md 4.22), batched on the device.
 
@@ -1024,19 +1073,38 @@ class TransducerRecognizer(Recognizer):
     live or the live ones together can no longer beat the n-best's worst.  max_symbols_per_frame does not apply: ALSD
     bounds labels by max_len alone.  One kernel per step makes every decision (otb_rnnt_beam_step).
 
+    lm (the Transformer or the recurrent LM of opentransformer_b200.lm), without apply_lm_rescoring: shallow fusion in
+    either mode (DESIGN.md 4.22).  A label k taken by a hypothesis with labels y adds lp(k) + lm_weight *
+    log p_lm(k | <S/E>, y) + beta, blank adds lp(blank) alone; the labels a hypothesis offers (greedy: its arg-max) are
+    chosen by that fused value, and the scores are the fused totals.  No end-of-sentence term is added.
+
+    apply_lm_rescoring (ALSD only): the LM is not fused; the search keeps beam_width finals, which are re-ranked by
+    s + rescore_weight * log P_lm(y <S/E>) (DESIGN.md 4.10), and the nbest best are returned.
+
     Both modes capture a block of steps in a CUDA graph (use_graph=False: launched one by one) and replay it until a device
-    counter shows every utterance ended.  The default and modified beam searches, LM fusion and n-gram scoring are not
-    implemented."""
+    counter shows every utterance ended.  The default and modified beam searches and n-gram scoring are not implemented."""
 
     def __init__(self, model, idx2unit=None, max_symbols_per_frame=5, max_len=1023, ngpu=1, use_graph=True, lm=None,
-                 ngram_lm=None, mode='greedy', beam_width=5, nbest=1):
+                 ngram_lm=None, mode='greedy', beam_width=5, nbest=1, lm_weight=0.1, beta=0.0, apply_lm_rescoring=False,
+                 rescore_weight=1.0):
         if mode == 'beam':
             raise NotImplementedError("TransducerRecognizer: the default (Graves) beam search is not implemented; "
                                       "mode='alsd' is the transducer beam search")
         if mode not in ('greedy', 'alsd'):
             raise NotImplementedError(f"TransducerRecognizer: mode must be 'greedy' or 'alsd', got {mode!r}")
-        if lm is not None:
-            raise NotImplementedError('TransducerRecognizer: LM fusion into the transducer search is not implemented; use lm=None')
+        if apply_lm_rescoring:
+            if mode != 'alsd':
+                raise ValueError("TransducerRecognizer: apply_lm_rescoring re-ranks an n-best; greedy search has one "
+                                 "hypothesis, use mode='alsd'")
+            check_lm_rescoring('TransducerRecognizer', lm, model.vocab_size)
+        elif lm is not None:
+            check_lm_fusion('TransducerRecognizer', lm, model.vocab_size)
+            if not lm_weight >= 0:
+                raise ValueError(f'TransducerRecognizer: lm_weight must be >= 0, got {lm_weight}: the early end of the '
+                                 'ALSD search needs the LM term to be at most 0')
+            if lm.model_type == 'transformer_lm' and max_len + 1 > ops.DECODE_MAX_LEN:
+                raise ValueError(f"TransducerRecognizer: the Transformer LM's cached attention holds {ops.DECODE_MAX_LEN} "
+                                 f'positions, <S/E> and max_len = {max_len} labels need {max_len + 1}')
         if ngram_lm is not None:
             raise NotImplementedError('TransducerRecognizer: n-gram LM scoring (KenLM) is not implemented; use ngram_lm=None')
         if not 1 <= max_len <= ops.RNNT_MAX_LABELS:
@@ -1050,9 +1118,11 @@ class TransducerRecognizer(Recognizer):
                 raise ValueError(f'TransducerRecognizer: nbest must be in [1, beam_width = {beam_width}], got {nbest}')
         elif nbest != 1:
             raise ValueError(f"TransducerRecognizer: greedy search has one hypothesis, got nbest={nbest}; use mode='alsd'")
-        super().__init__(model, idx2unit, None, None, ngpu)
+        super().__init__(model, idx2unit, lm, lm_weight, ngpu)
         self.max_len, self.max_symbols_per_frame, self.use_graph = int(max_len), int(max_symbols_per_frame), bool(use_graph)
         self.mode, self.beam_width, self.nbest = mode, int(beam_width), int(nbest)
+        self.lm_weight, self.beta = float(lm_weight), float(beta)
+        self.apply_lm_rescoring, self.rescore_weight = bool(apply_lm_rescoring), float(rescore_weight)
         self._search = None
 
     def recognize_ids(self, inputs, inputs_mask):
@@ -1062,18 +1132,29 @@ class TransducerRecognizer(Recognizer):
         with torch.no_grad():
             mem, lengths, B, T2 = self.model.encode_bf16(inputs, inputs_mask)
             op = self.model._pack.get()
+            fuse = self.lm if self.lm is not None and not self.apply_lm_rescoring else None
             s = self._search
-            # a graph bakes in its buffers and the operands: a new geometry or new weights get a new search
-            if s is None or s.op is not op or (s.B, s.T2, s.ep.device) != (B, T2, mem.device):
+            # a graph bakes in its buffers and the operands: a new geometry or new weights (the model's or the fused LM's)
+            # get a new search
+            if (s is None or s.op is not op or (s.B, s.T2, s.ep.device) != (B, T2, mem.device)
+                    or (fuse is not None and s.lm_pk is not fuse._pack.get())):
+                fusion = dict(lm=fuse, lm_weight=self.lm_weight, beta=self.beta)
                 if self.mode == 'alsd':
-                    s = _TransducerALSD(self.model, op, B, T2, self.beam_width, self.nbest, self.max_len, mem.device,
-                                        self.use_graph)
+                    W = self.beam_width if self.apply_lm_rescoring else self.nbest
+                    s = _TransducerALSD(self.model, op, B, T2, self.beam_width, W, self.max_len, mem.device,
+                                        self.use_graph, **fusion)
                 else:
                     s = _TransducerGreedy(self.model, op, B, T2, self.max_len, self.max_symbols_per_frame, mem.device,
-                                          self.use_graph)
+                                          self.use_graph, **fusion)
                 self._search = s
             self.model.decoder._check_device(mem.device)
-            return s.run(mem, lengths)
+            out = s.run(mem, lengths)
+            if not self.apply_lm_rescoring:
+                return out
+            ids, n, sc = out
+            ids, n, sc = rescore_nbest(ids, sc, [lambda x, y, K, Lp: lm_token_logprob(self.lm, x, y)], self.rescore_weight,
+                                       self.nbest, width=self.max_len, pad=PAD, lengths=n)
+            return ids.int(), n, sc
 
     def recognize(self, inputs, inputs_mask):
         """greedy: translate() of the 1-best token lists (the id lists when idx2unit is None), as CTCRecognizer.recognize.
@@ -1115,5 +1196,8 @@ def build_recognizer(model_type, model, lm, args, idx2unit):
         return TransducerRecognizer(model=model, idx2unit=idx2unit, max_len=getattr(args, 'max_len', 1023), ngpu=args.ngpu,
                                     lm=lm, ngram_lm=getattr(args, 'ngram_lm', None), mode=getattr(args, 'mode', 'greedy'),
                                     max_symbols_per_frame=getattr(args, 'max_symbols_per_frame', 5),
-                                    beam_width=getattr(args, 'beam_width', 5), nbest=getattr(args, 'nbest', 1))
+                                    beam_width=getattr(args, 'beam_width', 5), nbest=getattr(args, 'nbest', 1),
+                                    lm_weight=getattr(args, 'lm_weight', 0.1), beta=getattr(args, 'beta', 0.0),
+                                    apply_lm_rescoring=getattr(args, 'apply_lm_rescoring', False),
+                                    rescore_weight=getattr(args, 'rescore_weight', 1.0))
     raise NotImplementedError(model_type)
