@@ -1,8 +1,8 @@
 """LM shallow fusion in the CTC prefix beam search (DESIGN.md 4.19): ctcdecode's search with a neural LM as its scorer.
 
 One frame is the search step (otb_ctc_prefix_beam_step: one CTA per utterance, the frame index from a device counter, the
-slots in global memory) followed by one LM step over all B * beam rows; the frame is captured in a CUDA graph and replayed
-T' times from the host without a synchronisation.  The LM state follows the slots: a row that kept its prefix carries its
+slots in global memory) followed by one LM step over all B * beam rows; the frame runs T' times from the host without a
+synchronisation, as a graphs.CapturedStep (the first frame eager, the others replays of its capture).  The LM state follows the slots: a row that kept its prefix carries its
 source slot's LM row (and LSTM state), a row that extended runs the LM on its new token.
 
   * Recurrent LM: (h, c) per slot, gathered by source slot, then the embedding, the input GEMM, one otb_lstm_fwd step per
@@ -14,6 +14,7 @@ source slot's LM row (and LSTM state), a row that extended runs the LM on its ne
 import torch
 
 from . import ops
+from .graphs import CapturedStep
 
 BOS = 1
 
@@ -118,7 +119,6 @@ class CTCFusedSearch(FusedLMRows):
                              f'attention takes at most {ops.DECODE_MAX_LEN} positions')
         self.B, self.W, self.T, self.K = B, beam, T, K
         self.lm_weight, self.beta, self.blank = float(lm_weight), float(beta), blank
-        self.use_graph = use_graph
         N = B * beam
         i32 = dict(dtype=torch.int32, device=device)
         # Transformer LM cache rows: per utterance the BOS node and one node per (frame, slot); positions 0 .. T' - 1
@@ -134,8 +134,16 @@ class CTCFusedSearch(FusedLMRows):
         self.ids = torch.zeros(B, beam, T, **i32)
         self.lengths = torch.zeros(B, beam, **i32)
         self.scores = torch.zeros(B, beam, dtype=torch.float32, device=device)
-        self.graph = None
-        self._graph_pk = None
+        # one frame, captured on the first and replayed; the graph bakes in the LM pack's addresses
+        self.frame = CapturedStep(self._frame, self._packs, use_graph)
+
+    @property
+    def graph(self):
+        """The captured frame (None until the first frame of the graph path)."""
+        return self.frame.graph
+
+    def _packs(self):
+        return (self.lm._pack.get(),)
 
     def _frame(self):
         ops.ctc_prefix_beam_step(self.top_lp, self.top_id, self.B, self.T, self.in_len, self.W, self.blank, self.lm_rows,
@@ -148,38 +156,13 @@ class CTCFusedSearch(FusedLMRows):
         self.ctl.zero_()
         self.start_lm()
 
-    def _capture(self):
-        # warm-up outside capture (the weight pack, kernel attributes), then capture one frame; _start() resets what the
-        # warm-up advanced
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            self._frame()
-        torch.cuda.current_stream().wait_stream(s)
-        self.graph = torch.cuda.CUDAGraph()
-        n0 = ops.COUNTERS['launches']
-        with torch.cuda.graph(self.graph):
-            self._frame()
-        self.launches_per_frame = ops.COUNTERS['launches'] - n0
-        ops.COUNTERS['launches'] = n0
-
     def run(self, top_lp, top_id, in_len):
         """top_lp / top_id [B*T', K] of ctc_frame_topk, in_len i32 [B] -> (ids i64 [B, beam, T'] best first, lengths i32
         [B, beam], scores f32 [B, beam]: the fused totals log(p_b + p_nb))."""
         self.top_lp.copy_(top_lp)
         self.top_id.copy_(top_id)
         self.in_len.copy_(in_len)
-        if self.use_graph:
-            pk = self.lm._pack.get()
-            if self.graph is None or self._graph_pk is not pk:
-                # the LM's pack was rebuilt (load_state_dict, an optimizer step): the graph bakes in its addresses
-                self._graph_pk = pk
-                self._capture()
         self._start()
         for _ in range(self.T):
-            if self.use_graph:
-                self.graph.replay()
-                ops.COUNTERS['launches'] += self.launches_per_frame
-            else:
-                self._frame()
+            self.frame()
         return self.ids.long(), self.lengths.clone(), self.scores.clone()

@@ -27,6 +27,7 @@ import torch
 from . import ops
 from . import train
 from .ctc_fusion import CTCFusedSearch, FusedLMRows
+from .graphs import CapturedStep, lru_get, read_device
 from .lm import LMCache
 from .model import ctc_align_logits
 from .modules import encoder_attn_weights
@@ -220,7 +221,8 @@ class BeamDecoder:
     """KV-cached incremental decoder + device-side beam search for one (batch, beam, T, max_len) shape.
 
     Buffers are allocated once; one decode step (decoder on the newest token -> log-softmax -> beam
-    kernel) is captured into a CUDA graph on first use and replayed for every step.
+    kernel) is self.step, a graphs.CapturedStep: the first step runs eagerly, is captured, and every later step replays it
+    (a new weight pack, the decoder's or the fused LM's, captures again).
 
     ctc = (assistor, weight, P) adds the CTC prefix term of joint CTC/attention decoding (DESIGN.md 4.9): setup() takes
     the head's log-probs, and a step scores each hypothesis' P best tokens with
@@ -268,8 +270,7 @@ class BeamDecoder:
         # eager (test / debug) mode also materialises the full log-probs; keep_logp=True does so on the graph path (parity traces)
         self.keep_logp = (not use_graph) if keep_logp is None else bool(keep_logp)
         self.use_graph = use_graph
-        self.graph = None
-        self._graph_pk = None      # the bf16 weight packs whose device pointers the captured graph bakes in (kept alive with it)
+        self.step = CapturedStep(self._step_kernels, self._packs, use_graph)     # one decode step
         self.lm_logp = None
         self.lm_weight = 0.0
         self.lm = self.lm_cache = self._lstm_bar = None
@@ -398,51 +399,14 @@ class BeamDecoder:
         st.step_topk(self.topk_val, self.topk_idx)
         ctc.advance(st, self.mem_len)
 
-    def step(self):
-        if not self.use_graph:
-            return self._step_kernels()
-        packs = self._packs()
-        if self.graph is not None and any(a is not b for a, b in zip(self._graph_pk, packs)):
-            # parameters changed (load_state_dict / optimizer step): a pack was rebuilt at new addresses, the captured
-            # kernels would read the old (stale or recycled) weights -- drop the graph and capture again
-            self.graph = None
-        if self.graph is None:
-            self._graph_pk = packs
-            # warm-up outside capture (lazy func attributes, caches), then restore the state it advanced (the CTC prefix
-            # state needs no copy: a step reads the half of its ping-pong that the step counter names and writes the other)
-            snap = [t.clone() for t in (self.state.tok_hist, self.state.par_hist, self.state.last_tok,
-                                        self.state.scores, self.state.flag, self.state.anc, self.state.ctrl)]
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                self._step_kernels()
-            torch.cuda.current_stream().wait_stream(s)
-            for t, c in zip((self.state.tok_hist, self.state.par_hist, self.state.last_tok, self.state.scores,
-                             self.state.flag, self.state.anc, self.state.ctrl), snap):
-                t.copy_(c)
-            self.graph = torch.cuda.CUDAGraph()
-            n0 = ops.COUNTERS['launches']
-            with torch.cuda.graph(self.graph):
-                self._step_kernels()
-            self.launches_per_step = ops.COUNTERS['launches'] - n0
-            ops.COUNTERS['launches'] = n0                      # capture records, it does not launch
-            for t, c in zip((self.state.tok_hist, self.state.par_hist, self.state.last_tok, self.state.scores,
-                             self.state.flag, self.state.anc, self.state.ctrl), snap):
-                t.copy_(c)
-        self.graph.replay()
-        ops.COUNTERS['launches'] += self.launches_per_step
+    @property
+    def graph(self):
+        """The captured decode step (None until the first step of the graph path)."""
+        return self.step.graph
 
     def _read_ctrl(self):
-        """{step, done, ...} of the search state on the host.  The copy lands in pinned memory and the thread SLEEPS on a
-        blocking-sync event instead of spinning in cudaStreamSynchronize (`.item()`): a server keeps many of these loops
-        alive on few cores (16 lanes x 8 ranks on one host in bench.py)."""
-        if getattr(self, '_ctrl_pin', None) is None:
-            self._ctrl_pin = torch.zeros(4, dtype=torch.int32).pin_memory()
-            self._ctrl_ev = torch.cuda.Event(blocking=True)
-        self._ctrl_pin.copy_(self.state.ctrl, non_blocking=True)
-        self._ctrl_ev.record()
-        self._ctrl_ev.synchronize()
-        return self._ctrl_pin
+        """{step, done, ...} of the search state on the host (graphs.read_device)."""
+        return read_device(self.state.ctrl)
 
     def run(self, max_steps, poll_every=8):
         """Run up to max_steps decode steps; stops early once the device reports every hypothesis ended
@@ -603,14 +567,9 @@ class SpeechToTextRecognizer(Recognizer):
         lm = (self.lm, float(self.lm_weight)) if self._lm_fused() else None
         rows = samples or self.beam_width
         key = (B, rows, T2, self.max_len, device.index, ctc[1:] if ctc else None, lm, 'sample' if samples else 'beam')
-        bd = self._decoders.pop(key, None)
-        if bd is None:
-            while self.max_decoders is not None and len(self._decoders) >= self.max_decoders:
-                self._decoders.pop(next(iter(self._decoders)))          # the least recently used goes, with its buffers
-            bd = BeamDecoder(self.model.decoder, B, rows, T2, self.max_len, device, self.use_graph,
-                             persistent=self.persistent, ctc=ctc, lm=lm, sample=bool(samples))
-        self._decoders[key] = bd          # (re-)inserted as the most recently used
-        return bd
+        return lru_get(self._decoders, key, self.max_decoders, lambda: BeamDecoder(
+            self.model.decoder, B, rows, T2, self.max_len, device, self.use_graph, persistent=self.persistent, ctc=ctc, lm=lm,
+            sample=bool(samples)))
 
     def _lm_fused(self):
         """The LM enters the search by shallow fusion (it rescores the n-best instead under apply_lm_rescoring)."""
@@ -767,14 +726,8 @@ class CTCRecognizer(Recognizer):
     def _fused_search(self, B, T2, K, device):
         """The fused search of one geometry; the most recent few are kept (each owns its buffers and its graph)."""
         key = (B, T2, K, device.index, self.lm, float(self.lm_weight), float(self.beta))   # launch arguments a graph bakes in
-        search = self._searches.pop(key, None)
-        if search is None:
-            while len(self._searches) >= 2:
-                self._searches.pop(next(iter(self._searches)))
-            search = CTCFusedSearch(self.lm, B, self.beam_width, T2, K, device, self.lm_weight, self.beta,
-                                    self.model.assistor.blank, self.use_graph)
-        self._searches[key] = search
-        return search
+        return lru_get(self._searches, key, 2, lambda: CTCFusedSearch(
+            self.lm, B, self.beam_width, T2, K, device, self.lm_weight, self.beta, self.model.assistor.blank, self.use_graph))
 
     def recognize_ids(self, inputs, inputs_mask):
         """-> (ids i64 [B, nbest, T'] best first, 0 after each hypothesis' end; lengths i32 [B, nbest]; scores f32 [B, nbest]),
@@ -818,34 +771,89 @@ class CTCRecognizer(Recognizer):
         return best if self.idx2unit is None else self.translate(best)
 
 
-class _TransducerGreedy(FusedLMRows):
-    """The greedy transducer search of one geometry (B utterances, T' frames) over one set of model operands: its buffers,
-    and the CUDA graph of STEPS steps once captured.  With an LM (shallow fusion, DESIGN.md 4.22) each row also carries
-    log p_lm(. | <S/E>, its labels): the LM runs on every row's arg-max after the step, and the rows that emitted keep it."""
+class _TransducerSearch(FusedLMRows):
+    """A transducer search of one geometry (B utterances, T' frames, N rows) over the model's current operands: the encoder
+    projection Ep, the prediction network, the LM-fusion set-up, and the loop of blocks of STEPS steps.  A block is a
+    graphs.CapturedStep keyed on the model's and the fused LM's weight packs, so new weights recapture it in place; the
+    host reads the live-row counter once per block.  A subclass allocates its own buffers (self.out: what run returns,
+    self.active: the live-row counter) and writes start_rows (its state before the first step) and _step."""
 
-    STEPS = 16          # search steps per graph replay: the host reads the active-row counter once per replay
+    STEPS = 16          # search steps per graph replay: the host reads the live-row counter once per replay
 
-    def __init__(self, model, op, B, T2, max_len, max_sym, device, use_graph, lm=None, lm_weight=0.0, beta=0.0):
-        self.model, self.op, self.B, self.T2 = model, op, B, T2
-        self.max_sym, self.use_graph = max_sym, use_graph
+    def __init__(self, model, B, T2, N, k, max_len, device, use_graph, lm, lm_weight, beta):
+        self.model, self.B, self.T2, self.max_len = model, B, T2, max_len
         D, H, L = model.joint.inner_size, model.decoder.hidden_size, model.decoder.num_layers
-        i32 = dict(dtype=torch.int32, device=device)
+        f32, i32 = dict(dtype=torch.float32, device=device), dict(dtype=torch.int32, device=device)
         self.ep = torch.empty(B * T2, D, dtype=ops.BF16, device=device)
-        self.ep_cur = torch.empty(B, D, dtype=ops.BF16, device=device)
-        self.pp = torch.empty(B, D, dtype=ops.BF16, device=device)
-        self.h = torch.empty(L, B, H, dtype=torch.float32, device=device)
-        self.c = torch.empty(L, B, H, dtype=torch.float32, device=device)
-        self.logp = torch.empty(B, model.joint.ld_logits, dtype=torch.float32, device=device)
-        self.val = torch.empty(B, 1, dtype=torch.float32, device=device)
-        self.idx = torch.empty(B, 1, **i32)
-        self.tok = torch.zeros(B, dtype=torch.long, device=device)
-        self.t_len, self.frame, self.n_sym, self.n_out = (torch.zeros(B, **i32) for _ in range(4))
+        self.ep_cur, self.pp = (torch.empty(N, D, dtype=ops.BF16, device=device) for _ in range(2))
+        self.h, self.c = (torch.empty(L, N, H, **f32) for _ in range(2))
+        self.logp = torch.empty(N, model.joint.ld_logits, **f32)
+        self.val = torch.empty(N, k, **f32)
+        self.idx = torch.empty(N, k, **i32)
+        self.tok = torch.zeros(N, dtype=torch.long, device=device)
+        self.t_len = torch.zeros(B, **i32)
+        self.bar = torch.zeros(2, **i32)            # the LSTM kernels' grid barrier, owned here: a graph must not allocate one
+        self.lm, self.lm_weight, self.beta = lm, float(lm_weight), float(beta)
+        self.op = None                              # the model's operands, read by start()
+        self.block = CapturedStep(self._steps, self._packs, use_graph)
+
+    def _packs(self):
+        return (self.op,) if self.lm is None else (self.op, self.lm._pack.get())
+
+    def _predict(self, hidden):
+        """The prediction network one token on from hidden (None: the zero state) for every row's self.tok -> (h, c,
+        dec_proj(h))."""
+        op = self.op
+        x = ops.embedding(self.tok, op['emb'])
+        y, h, c, _ = train.lstm_stack_fwd(x, op['layers'], 1, self.tok.numel(), hidden=hidden, barrier=self.bar)
+        return h, c, ops.linear(y, op['dec_w'])
+
+    def start(self, mem, lengths):
+        """The state before the first step: Ep of the memory, the subclass's rows, every row's prediction network from BLK
+        and the zero state, and the LM on <S/E>."""
+        self.op = self.model._pack.get()
+        enc = self.op['enc']
+        ops.linear(mem, enc.w, enc.b, ops.EPI_BIAS, out=self.ep)
+        self.t_len.copy_(lengths)
+        self.start_rows(lengths)
+        self.tok.zero_()
+        h, c, pp = self._predict(None)
+        self.h.copy_(h)
+        self.c.copy_(c)
+        self.pp.copy_(pp)
+        if self.lm is not None:
+            self.start_lm()
+
+    def _steps(self):
+        for _ in range(self.STEPS):
+            self._step()
+
+    def run(self, mem, lengths):
+        self.start(mem, lengths)
+        self.steps = 0
+        # every step moves each live row one frame on or one label on: T_b + max_len steps end every utterance
+        for _ in range(-(-(self.T2 + self.max_len) // self.STEPS)):
+            self.block()
+            self.steps += self.STEPS
+            if int(read_device(self.active)[0]) == 0:
+                break
+        return tuple(t.clone() for t in self.out)
+
+
+class _TransducerGreedy(_TransducerSearch):
+    """The greedy transducer search: one row per utterance.  With an LM (shallow fusion, DESIGN.md 4.22) each row also
+    carries log p_lm(. | <S/E>, its labels): the LM runs on every row's arg-max after the step, and the rows that emitted
+    keep it."""
+
+    def __init__(self, model, B, T2, max_len, max_sym, device, use_graph, lm=None, lm_weight=0.0, beta=0.0):
+        super().__init__(model, B, T2, B, 1, max_len, device, use_graph, lm, lm_weight, beta)
+        self.max_sym = max_sym
+        i32 = dict(dtype=torch.int32, device=device)
+        self.frame, self.n_sym, self.n_out = (torch.zeros(B, **i32) for _ in range(3))
         self.ids = torch.zeros(B, max_len, **i32)
         self.score = torch.zeros(B, dtype=torch.float32, device=device)
+        self.out = (self.ids, self.n_out, self.score)
         self.active = torch.zeros(1, **i32)
-        self.bar = torch.zeros(2, **i32)            # the LSTM kernels' grid barrier, owned here: a graph must not allocate one
-        self.graph = None
-        self.lm, self.lm_weight, self.beta = lm, float(lm_weight), float(beta)
         if lm is not None:
             # one LM row per utterance; the Transformer LM's cache is linear, position p of utterance b at row b L + p
             L = max_len + 1
@@ -853,113 +861,62 @@ class _TransducerGreedy(FusedLMRows):
             self._init_lm(lm, B, L, B * L, row * L, torch.zeros_like(row), device)
             if self.anc is not None:
                 self.anc.copy_(row[:, None] * L + torch.arange(L, device=device))
-            self.lm_pk = lm._pack.get()
 
-    def _predict(self, hidden):
-        """The prediction network one token on from hidden (None: the zero state) for self.tok -> (h, c, dec_proj(h))."""
-        op = self.op
-        x = ops.embedding(self.tok, op['emb'])
-        y, h, c, _ = train.lstm_stack_fwd(x, op['layers'], 1, self.B, hidden=hidden, barrier=self.bar)
-        return h, c, ops.linear(y, op['dec_w'])
-
-    def _steps(self):
-        op, m = self.op, self.model
-        for _ in range(self.STEPS):
-            hj = ops.rnnt_joint(self.ep_cur, self.pp, self.B, 1, 1)
-            logits = ops.linear(hj, op['out_w'], op['out_b'], ops.EPI_BIAS, out_f32=True, n_out=m.joint.ld_logits)
-            if self.lm is None:
-                ops.logsoftmax_topk(logits, m.vocab_size, 1, out_val=self.val, out_idx=self.idx, out_logp=self.logp)
-            else:
-                _fused_topk(self, logits, m.vocab_size, 1)
-            self.tok.copy_(self.idx.view(-1))
-            h, c, pp = self._predict((self.h, self.c))          # every row's next state, kept only where a label is emitted
-            fused = self.lm is not None
-            ops.rnnt_greedy_step(self.idx, self.logp, h, c, pp, self.h, self.c, self.pp, self.ep, self.T2, self.ep_cur,
-                                 self.t_len, self.frame, self.n_sym, self.n_out, self.ids, self.max_sym, self.score, self.active,
-                                 val=self.val if fused else None, emit=self.ext if fused else None,
-                                 lm_pos=self.pos if fused else None)
-            if fused:
-                self.follow(None)                               # the LM on every row's arg-max, kept where it was emitted
-
-    def run(self, mem, lengths):
-        B, T2 = self.B, self.T2
-        enc = self.op['enc']
-        ops.linear(mem, enc.w, enc.b, ops.EPI_BIAS, out=self.ep)
-        self.t_len.copy_(lengths)
+    def start_rows(self, lengths):
         for t in (self.frame, self.n_sym, self.n_out, self.ids, self.score):
             t.zero_()
         self.active.copy_((lengths > 0).sum().view(1))
-        self.ep_cur.copy_(self.ep.view(B, T2, -1)[:, 0])
-        self.tok.zero_()                                        # the prediction network starts from BLK and the zero state
-        h, c, pp = self._predict(None)
-        self.h.copy_(h)
-        self.c.copy_(c)
-        self.pp.copy_(pp)
-        if self.lm is not None:
-            self.start_lm()
-        # every step moves each live row one frame on or emits one of its at most max_len labels
-        blocks = -(-(T2 + self.ids.shape[1]) // self.STEPS)
-        for _ in range(blocks):
-            if self.graph is not None:
-                self.graph.replay()
-            else:
-                self._steps()
-                if self.use_graph:          # after one eager block (the warm-up), capture the same block
-                    self.graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(self.graph):
-                        self._steps()
-            if int(self.active.item()) == 0:
-                break
-        return self.ids.clone(), self.n_out.clone(), self.score.clone()
+        self.ep_cur.copy_(self.ep.view(self.B, self.T2, -1)[:, 0])
+
+    def _step(self):
+        op, m = self.op, self.model
+        hj = ops.rnnt_joint(self.ep_cur, self.pp, self.B, 1, 1)
+        logits = ops.linear(hj, op['out_w'], op['out_b'], ops.EPI_BIAS, out_f32=True, n_out=m.joint.ld_logits)
+        if self.lm is None:
+            ops.logsoftmax_topk(logits, m.vocab_size, 1, out_val=self.val, out_idx=self.idx, out_logp=self.logp)
+        else:
+            _fused_topk(self, logits, m.vocab_size, 1)
+        self.tok.copy_(self.idx.view(-1))
+        h, c, pp = self._predict((self.h, self.c))          # every row's next state, kept only where a label is emitted
+        fused = self.lm is not None
+        ops.rnnt_greedy_step(self.idx, self.logp, h, c, pp, self.h, self.c, self.pp, self.ep, self.T2, self.ep_cur,
+                             self.t_len, self.frame, self.n_sym, self.n_out, self.ids, self.max_sym, self.score, self.active,
+                             val=self.val if fused else None, emit=self.ext if fused else None,
+                             lm_pos=self.pos if fused else None)
+        if fused:
+            self.follow(None)                               # the LM on every row's arg-max, kept where it was emitted
 
 
-class _TransducerALSD(FusedLMRows):
-    """The ALSD beam search of one geometry (B utterances, T' frames, K slots each, an n-best of W, max_len labels) over one
-    set of model operands: its buffers, the node table, and the CUDA graph of STEPS steps once captured.  Every array is at
-    B*K slot rows; the step is rnnt_joint -> output layer -> logsoftmax_topk -> otb_rnnt_beam_step -> otb_rnnt_beam_gather ->
-    the prediction network one token on -> otb_rnnt_beam_commit.  With an LM (shallow fusion, DESIGN.md 4.22) each slot
-    also carries log p_lm(. | <S/E>, its labels), following its parent slot and advanced by the LM where it took a label;
-    the Transformer LM's K/V are stored once per node of the node table, [blocks, B n_cap, d], node 0 the <S/E>."""
+class _TransducerALSD(_TransducerSearch):
+    """The ALSD beam search (K slots per utterance, an n-best of W, max_len labels): its buffers and the node table.  Every
+    array is at B*K slot rows; the step is rnnt_joint -> output layer -> logsoftmax_topk -> otb_rnnt_beam_step ->
+    otb_rnnt_beam_gather -> the prediction network one token on -> otb_rnnt_beam_commit.  With an LM (shallow fusion,
+    DESIGN.md 4.22) each slot also carries log p_lm(. | <S/E>, its labels), following its parent slot and advanced by the
+    LM where it took a label; the Transformer LM's K/V are stored once per node of the node table, [blocks, B n_cap, d],
+    node 0 the <S/E>."""
 
-    STEPS = 16
-
-    def __init__(self, model, op, B, T2, K, W, max_len, device, use_graph, lm=None, lm_weight=0.0, beta=0.0):
-        self.model, self.op, self.B, self.T2, self.K, self.use_graph = model, op, B, T2, K, use_graph
+    def __init__(self, model, B, T2, K, W, max_len, device, use_graph, lm=None, lm_weight=0.0, beta=0.0):
+        BK = B * K
+        self.K, self.k1 = K, min(K + 1, model.vocab_size)
+        super().__init__(model, B, T2, BK, self.k1, max_len, device, use_graph, lm, lm_weight, beta)
         D, H, L = model.joint.inner_size, model.decoder.hidden_size, model.decoder.num_layers
-        BK, V = B * K, model.vocab_size
         f32, i32 = dict(dtype=torch.float32, device=device), dict(dtype=torch.int32, device=device)
-        self.ep = torch.empty(B * T2, D, dtype=ops.BF16, device=device)
-        self.ep_cur, self.pp, self.ppg = (torch.empty(BK, D, dtype=ops.BF16, device=device) for _ in range(3))
-        self.h, self.c, self.hg, self.cg = (torch.empty(L, BK, H, **f32) for _ in range(4))
-        self.logp = torch.empty(BK, model.joint.ld_logits, **f32)
-        self.k1 = min(K + 1, V)
-        self.val = torch.empty(BK, self.k1, **f32)
-        self.idx = torch.empty(BK, self.k1, **i32)
+        self.ppg = torch.empty(BK, D, dtype=ops.BF16, device=device)
+        self.hg, self.cg = (torch.empty(L, BK, H, **f32) for _ in range(2))
         n_cap = K * (T2 + max_len) + 1                  # the root and at most K new nodes per step, T_b + max_len steps
+        if lm is not None:
+            row = torch.arange(BK, device=device)
+            self._init_lm(lm, BK, max_len + 1, B * n_cap, (row // K) * n_cap, torch.where(row % K == 0, 0, -1), device)
+            self.lm_out = dict(src=self.src, ext=self.ext, anc=self.anc, anc_tmp=self.anc_tmp, pos=self.pos)
+        # tok: the label each slot took, read by the prediction network and the LM
         self.state = dict(score=torch.empty(BK, **f32), u=torch.empty(BK, **i32), frame=torch.empty(BK, **i32),
-                          node=torch.empty(BK, **i32), par=torch.empty(BK, **i32),
-                          tok=torch.zeros(BK, dtype=torch.long, device=device),
+                          node=torch.empty(BK, **i32), par=torch.empty(BK, **i32), tok=self.tok,
                           node_par=torch.zeros(B, n_cap, **i32), node_tok=torch.zeros(B, n_cap, **i32),
                           n_nodes=torch.empty(B, **i32), f_score=torch.empty(B, W, **f32), f_node=torch.empty(B, W, **i32),
                           f_u=torch.empty(B, W, **i32), f_n=torch.empty(B, **i32), done=torch.empty(B, **i32),
                           active=torch.empty(1, **i32))
-        self.t_len = torch.zeros(B, **i32)
+        self.active = self.state['active']
         self.out = (torch.zeros(B, W, max_len, **i32), torch.zeros(B, W, **i32), torch.empty(B, W, **f32))
-        self.bar = torch.zeros(2, **i32)
-        self.graph = None
-        self.lm, self.lm_weight, self.beta = lm, float(lm_weight), float(beta)
-        if lm is not None:
-            row = torch.arange(BK, device=device)
-            self._init_lm(lm, BK, max_len + 1, B * n_cap, (row // K) * n_cap, torch.where(row % K == 0, 0, -1), device)
-            self.tok = self.state['tok']                # the LM reads the label each slot took
-            self.lm_out = dict(src=self.src, ext=self.ext, anc=self.anc, anc_tmp=self.anc_tmp, pos=self.pos)
-            self.lm_pk = lm._pack.get()
-
-    def _predict(self, hidden):
-        op = self.op
-        x = ops.embedding(self.state['tok'], op['emb'])
-        y, h, c, _ = train.lstm_stack_fwd(x, op['layers'], 1, self.B * self.K, hidden=hidden, barrier=self.bar)
-        return h, c, ops.linear(y, op['dec_w'])
 
     def step_phases(self):
         """One search step as its seven phases, in order (tools/transducer_beam.py times each)."""
@@ -1000,20 +957,16 @@ class _TransducerALSD(FusedLMRows):
             self.follow(self.src)
         return [joint, output_layer, topk, beam_step, gather, predictor, commit] + ([lm] if self.lm is not None else [])
 
-    def _steps(self):
-        for _ in range(self.STEPS):
-            for phase in self.step_phases():
-                phase()
+    def _step(self):
+        for phase in self.step_phases():
+            phase()
 
-    def start(self, mem, lengths):
-        """The state before the first step: one live slot per utterance with a frame, the empty sequence at frame 0."""
+    def start_rows(self, lengths):
+        """One live slot per utterance with a frame, the empty sequence at frame 0."""
         B, T2, K, s = self.B, self.T2, self.K, self.state
-        enc = self.op['enc']
-        ops.linear(mem, enc.w, enc.b, ops.EPI_BIAS, out=self.ep)
-        self.t_len.copy_(lengths)
         s['score'].fill_(float('-inf'))
         s['score'].view(B, K)[:, 0].masked_fill_(lengths > 0, 0.0)
-        for k in ('u', 'frame', 'node', 'par', 'tok', 'f_n', 'done'):
+        for k in ('u', 'frame', 'node', 'par', 'f_n', 'done'):
             s[k].zero_()
         s['n_nodes'].fill_(1)
         s['active'].fill_(B)                    # an utterance without frames ends at the first step
@@ -1021,32 +974,6 @@ class _TransducerALSD(FusedLMRows):
             t.zero_()
         self.out[2].fill_(float('-inf'))
         self.ep_cur.view(B, K, -1).copy_(self.ep.view(B, T2, -1)[:, :1])
-        h, c, pp = self._predict(None)          # every slot from BLK and the zero state
-        self.h.copy_(h)
-        self.c.copy_(c)
-        self.pp.copy_(pp)
-        if self.lm is not None:
-            self.start_lm()
-
-    def run(self, mem, lengths):
-        self.start(mem, lengths)
-        s = self.state
-        self.steps = 0
-        # every step moves each live hypothesis one frame or one label on: T_b + max_len steps end every utterance
-        blocks = -(-(self.T2 + self.out[0].shape[2]) // self.STEPS)
-        for _ in range(blocks):
-            if self.graph is not None:
-                self.graph.replay()
-            else:
-                self._steps()
-                if self.use_graph:
-                    self.graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(self.graph):
-                        self._steps()
-            self.steps += self.STEPS
-            if int(s['active'].item()) == 0:
-                break
-        return tuple(t.clone() for t in self.out)
 
 
 def _fused_topk(search, logits, V, k):
@@ -1082,7 +1009,7 @@ class TransducerRecognizer(Recognizer):
     s + rescore_weight * log P_lm(y <S/E>) (DESIGN.md 4.10), and the nbest best are returned.
 
     Both modes capture a block of steps in a CUDA graph (use_graph=False: launched one by one) and replay it until a device
-    counter shows every utterance ended.  The default and modified beam searches and n-gram scoring are not implemented."""
+    counter shows every utterance ended; new weights, the model's or the fused LM's, capture it again.  The default and modified beam searches and n-gram scoring are not implemented."""
 
     def __init__(self, model, idx2unit=None, max_symbols_per_frame=5, max_len=1023, ngpu=1, use_graph=True, lm=None,
                  ngram_lm=None, mode='greedy', beam_width=5, nbest=1, lm_weight=0.1, beta=0.0, apply_lm_rescoring=False,
@@ -1131,20 +1058,16 @@ class TransducerRecognizer(Recognizer):
         finals found with length 0 and score -inf; on the device."""
         with torch.no_grad():
             mem, lengths, B, T2 = self.model.encode_bf16(inputs, inputs_mask)
-            op = self.model._pack.get()
-            fuse = self.lm if self.lm is not None and not self.apply_lm_rescoring else None
             s = self._search
-            # a graph bakes in its buffers and the operands: a new geometry or new weights (the model's or the fused LM's)
-            # get a new search
-            if (s is None or s.op is not op or (s.B, s.T2, s.ep.device) != (B, T2, mem.device)
-                    or (fuse is not None and s.lm_pk is not fuse._pack.get())):
-                fusion = dict(lm=fuse, lm_weight=self.lm_weight, beta=self.beta)
+            # a search owns the buffers of one geometry; new weights (the model's or the fused LM's) recapture its graph
+            if s is None or (s.B, s.T2, s.ep.device) != (B, T2, mem.device):
+                fusion = dict(lm=None if self.apply_lm_rescoring else self.lm, lm_weight=self.lm_weight, beta=self.beta)
                 if self.mode == 'alsd':
                     W = self.beam_width if self.apply_lm_rescoring else self.nbest
-                    s = _TransducerALSD(self.model, op, B, T2, self.beam_width, W, self.max_len, mem.device,
-                                        self.use_graph, **fusion)
+                    s = _TransducerALSD(self.model, B, T2, self.beam_width, W, self.max_len, mem.device, self.use_graph,
+                                        **fusion)
                 else:
-                    s = _TransducerGreedy(self.model, op, B, T2, self.max_len, self.max_symbols_per_frame, mem.device,
+                    s = _TransducerGreedy(self.model, B, T2, self.max_len, self.max_symbols_per_frame, mem.device,
                                           self.use_graph, **fusion)
                 self._search = s
             self.model.decoder._check_device(mem.device)

@@ -47,6 +47,7 @@ import torch
 from . import ops
 from . import modules
 from .dp import allreduce_mean_, broadcast_from_first_, rank_in
+from .graphs import CapturedStep, lru_get
 from .modules import (ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder,
                       TransformerEncoder, _lengths)
 from .ops import BF16, EPI_BIAS, EPI_RESID, EPI_TABLE, EPI_RELU
@@ -1250,7 +1251,7 @@ class FusedTrainer:
         self.use_graph = use_graph
         self.graph_after = 2          # capture a CUDA graph for an input geometry once it has been seen this many times
         self.max_graphs = 8           # LRU bound: every graph owns a private pool with the whole activation tape
-        self._graphs = {}             # key -> (graph, inputs, mask, truth, loss, launches), most recently used last
+        self._graphs = {}             # key -> (graphs.CapturedStep of _micro, its static batch), most recently used last
         self._seen = {}
         # training-mode BatchNorm buffers (Conformer): updated by every micro-step, inside the graph when one is replayed
         self.bn_buffers = [t for n, t in model.named_buffers() if n.startswith('encoder.') and
@@ -1374,45 +1375,23 @@ class FusedTrainer:
     def _graph_for(self, batch):
         """The ~870 launches of one micro-batch captured once per input geometry and replayed: launched one by one from
         Python the step is host-bound.
-        Real ASR batches have a new (T, L) almost every step, so a geometry runs EAGERLY until it has recurred
-        `graph_after` times, and at most `max_graphs` graphs are kept (least recently used first out): use_graph pays off
-        with bucketed / padded batches (otrans/data/bucket.py), it must not grow memory without bound otherwise.
-        Returns None when this call should run eagerly."""
+        Real ASR batches have a new (T, L) almost every step, so a geometry runs EAGERLY until its `graph_after`-th
+        sighting, which runs eagerly on the static inputs and captures (graphs.CapturedStep): replays start at the next
+        sighting.  At most `max_graphs` graphs are kept (least recently used first out): use_graph pays off with bucketed /
+        padded batches (otrans/data/bucket.py), it must not grow memory without bound otherwise.
+        Returns None when this call should run eagerly, else (the captured micro-step, its static inputs)."""
         dev = batch[0].device
         key = tuple(None if t is None else tuple(t.shape) for t in batch) + (dev.index,)
-        ent = self._graphs.pop(key, None)
-        if ent is None:
+        if key not in self._graphs:
             n = self._seen.get(key, 0) + 1
             if len(self._seen) > 4096:
                 self._seen.clear()
             self._seen[key] = n
             if n < self.graph_after:
                 return None
-            while len(self._graphs) >= self.max_graphs:
-                self._graphs.pop(next(iter(self._graphs)))        # drops the graph and its memory pool
-            static = tuple(None if t is None else t.to(dev).clone() for t in batch)
-            snap = self.flat_g.clone()
-            bn_snap = [t.clone() for t in self.bn_buffers]          # the warm-up must not count as a step
-            if self.mixspeech:      # nor draw lambda or masks: a resumed run continues the same sequence
-                bn_snap += [self.drop_seed.clone(), self.mix_step.clone()]
-            cur = torch.cuda.current_stream()
-            side = torch.cuda.Stream()
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):          # warm-up outside capture: lazy kernel attributes, cached tables
-                self._micro(static)
-            cur.wait_stream(side)
-            self.flat_g.copy_(snap)
-            for t, v in zip(self.bn_buffers + ([self.drop_seed, self.mix_step] if self.mixspeech else []), bn_snap):
-                t.copy_(v)
-            graph = torch.cuda.CUDAGraph()
-            n0 = ops.COUNTERS['launches']
-            with torch.cuda.graph(graph):
-                loss = self._micro(static)
-            launches = ops.COUNTERS['launches'] - n0
-            ops.COUNTERS['launches'] = n0           # capture records, it does not launch
-            ent = (graph, static, loss, launches)
-        self._graphs[key] = ent       # (re-)insert as most recently used
-        return ent
+
+        return lru_get(self._graphs, key, self.max_graphs,         # evicting a graph drops its memory pool
+                       lambda: (CapturedStep(self._micro), tuple(None if t is None else t.to(dev).clone() for t in batch)))
 
     # ---- optimizer state: the reference's checkpoint (trainer.py:280-290, loaded by run.py:54-61 with -ct -ios) ----
 
@@ -1527,14 +1506,13 @@ class FusedTrainer:
                 batch = self._with_nbest(batch)
             ent = self._graph_for(batch) if self.use_graph else None
             if ent is not None:
-                graph, static, loss, launches = ent
+                micro, static = ent
                 for s, t in zip(static, batch):
                     if s is not None:
                         s.copy_(t)
-                graph.replay()
-                ops.COUNTERS['launches'] += launches
+                loss = micro(static)
                 if self.bn_buffers:
-                    modules.bump_param_generation()     # the replay moved the running statistics
+                    modules.bump_param_generation()     # a replay moved the running statistics
             else:
                 loss = self._micro(batch)
             self.micro += 1

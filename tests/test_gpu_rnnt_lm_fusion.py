@@ -120,16 +120,16 @@ def test_context_lm_carries_each_hypothesis_prefix(kind, mode, K, W):
 
 
 @pytest.mark.parametrize('kind', ['transformer', 'rnn'])
-def test_new_lm_pack_recaptures(kind):
+def test_new_lm_pack_recaptures_in_place(kind):
     model, x, mask = _setup()
     lm = _lm(kind, 9)
     rec = TransducerRecognizer(model, lm=lm, lm_weight=0.5, beta=0.2, mode='alsd', beam_width=4, nbest=2, max_len=30)
     with torch.no_grad():
         a = [t.clone() for t in rec.recognize_ids(x, mask)]
-        s0 = rec._search
+        s0, g0 = rec._search, rec._search.block.graph
         lm.load_state_dict(_lm(kind, 10).state_dict())
         b = [t.clone() for t in rec.recognize_ids(x, mask)]
-        assert rec._search is not s0
+        assert rec._search is s0 and g0 is not None and s0.block.graph is not None and s0.block.graph is not g0
         fresh = TransducerRecognizer(model, lm=lm, lm_weight=0.5, beta=0.2, mode='alsd', beam_width=4, nbest=2,
                                      max_len=30).recognize_ids(x, mask)
     for u, v in zip(b, fresh):

@@ -262,7 +262,7 @@ def test_residual_dropout_gradients_with_replayed_masks():
     # FusedTrainer with the CUDA graph: replays must not freeze the mask
     tr = train.FusedTrainer(model, accum_steps=1, use_graph=True)
     losses = [float(tr.step(x.to(DEV), mask.to(DEV), tgt.to(DEV))) for _ in range(4)]
-    print('FusedTrainer losses with dropout (graph from the 2nd step on):', losses)
+    print('FusedTrainer losses with dropout (captured at the 2nd step, replayed from the 3rd):', losses)
     assert len(set(losses)) == 4
 
 

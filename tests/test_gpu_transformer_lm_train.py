@@ -217,7 +217,7 @@ def test_fused_trainer_graph_replays():
     tr_ = train.FusedTrainer(lm.train(), accum_steps=4, use_graph=True)
     x, y = batches[0][0].to(DEV), batches[0][1].to(DEV)
     dropped = [float(tr_.step(x, y)) for _ in range(4)]
-    print('FusedTrainer losses with dropout, one batch (graph from the 2nd step on):', dropped)
+    print('FusedTrainer losses with dropout, one batch (captured at the 2nd step, replayed from the 3rd):', dropped)
     assert len(tr_._graphs) == 1 and len(set(dropped)) == 4
 
 
@@ -246,7 +246,9 @@ ADAM_LAUNCHES = 3       # otb_sumsq + otb_adam_step_sched
 
 
 @pytest.mark.parametrize('rate', [0.0, 0.1])
-def test_speech_micro_step_launches_unchanged(rate):
+def test_speech_micro_step_launches_eager_and_replayed(rate):
+    """A speech micro-step launches its recorded kernels eagerly, its captured graph holds them, and a replay counts
+    them."""
     from tests.test_gpu_train import _batch as speech_batch, _build, _params as speech_params
     params = speech_params(n_enc=1, n_dec=1)
     params['encoder']['residual_dropout'] = rate
@@ -265,4 +267,7 @@ def test_speech_micro_step_launches_unchanged(rate):
     tr_.step(x, mask, tgt)
     tr_.step(x, mask, tgt)                      # the second sighting captures the graph
     (ent,) = tr_._graphs.values()
-    assert ent[3] == SPEECH_MICRO_LAUNCHES[rate], ent[3]
+    assert ent[0].launches == SPEECH_MICRO_LAUNCHES[rate], ent[0].launches
+    n0 = ops.COUNTERS['launches']
+    tr_.step(x, mask, tgt)                      # a replay, no optimizer step
+    assert ops.COUNTERS['launches'] - n0 == SPEECH_MICRO_LAUNCHES[rate]

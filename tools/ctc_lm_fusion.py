@@ -78,7 +78,7 @@ def main():
             re_ = se.run(lp, tok, lengths)
             rec = CTCRecognizer(model, lm=lm, lm_weight=LMW, beta=BETA, beam_width=W, mode='beam', lm_fusion=True)
             res['notes'][name] = {'eager_equals_graph': all(bool(torch.equal(p, q)) for p, q in zip(rg, re_)),
-                                  'launches_per_frame': sg.launches_per_frame,
+                                  'launches_per_frame': sg.frame.launches,
                                   'mean_1best_len': float(rg[1][:, 0].float().mean())}
             variants = {'unfused_search': unfused,
                         'fused_graph': lambda: sg.run(lp, tok, lengths),
@@ -92,7 +92,7 @@ def main():
                              sg.top_lp, sg.top_id, B, T2, sg.in_len, W, 0, sg.lm_rows, LMW, BETA, sg.slots, sg.ctl, sg.nodes,
                              sg.src, sg.tok, sg.ext, sg.ids, sg.lengths, sg.scores, sg.anc, sg.anc_tmp, sg.pos)),
                          'lm_step': lambda: se._lm_step(),
-                         'frame_graph_replay': lambda: (last(), sg.graph.replay())}
+                         'frame_graph_replay': lambda: (last(), sg.frame.graph.replay())}
             ms = res['ms_per_batch'].setdefault(name, {})
             fr = res['ms_per_frame'].setdefault(name, {})
             for _ in range(a.reps):

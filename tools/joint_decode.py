@@ -69,10 +69,10 @@ def main():
     _, _, steps0 = rec0.recognize_ids(x, mask)
     _, _, steps = rec.recognize_ids(x, mask)
     bd = next(iter(rec._decoders.values()))
-    assert steps0 == steps == max_len and bd.graph is not None and not bd.persistent
+    assert steps0 == steps == max_len and bd.step.graph is not None and not bd.persistent
     ctc, st = bd.ctc, bd.state
     res = {'card': card(), 'batch': B, 'frames': T, 'encoder_frames': ctc.T, 'beam': beam, 'candidates': ctc.P, 'steps': steps,
-           'ctc_weight': a.weight, 'launches_per_step': bd.launches_per_step, 'reps': a.reps,
+           'ctc_weight': a.weight, 'launches_per_step': bd.step.launches, 'reps': a.reps,
            'ctc_buffers_mb': round(sum(t.numel() * t.element_size() for t in (ctc.lp, ctc.gamma, ctc.psi, ctc.gamma_cand,
                                                                                ctc.psi_cand, ctc.cand_val, ctc.cand_id)) / 1e6, 1),
            'ms': {}}

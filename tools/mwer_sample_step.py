@@ -72,8 +72,8 @@ def main():
         out['sample_full_length_decode_ms'] = [timed(lambda: tr._with_nbest(batch), args.iters) for _ in range(args.reps)]
         out['sample_full_length_Lp'] = int(tr._with_nbest(batch)[-1].shape[1])
     bd = next(iter(trainers['sample']._recognizer._decoders.values()))
-    out['sample_decoder'] = {'persistent': bd.persistent, 'captured_step': bd.graph is not None,
-                             'launches_per_step': getattr(bd, 'launches_per_step', None)}
+    out['sample_decoder'] = {'persistent': bd.persistent, 'captured_step': bd.step.graph is not None,
+                             'launches_per_step': bd.step.launches}
     print(json.dumps(out))
 
 

@@ -32,7 +32,7 @@ def phase_times(model, x, mask, K, steps):
     """Mean device ms of each phase of an ALSD step over the first `steps` steps of a search (eager)."""
     with torch.no_grad():
         mem, lengths, B, T2 = model.encode_bf16(x, mask)
-        s = _TransducerALSD(model, model._pack.get(), B, T2, K, 1, MAX_LEN, x.device, use_graph=False)
+        s = _TransducerALSD(model, B, T2, K, 1, MAX_LEN, x.device, use_graph=False)
         s.start(mem, lengths)
         names = ['joint', 'output_layer', 'logsoftmax_topk', 'beam_step', 'gather', 'predictor', 'commit']
         ev = []
