@@ -12,7 +12,7 @@ from . import ops
 from . import train
 from .lm import RecurrentLanguageModel, _LSTMParams
 from .modules import (ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder,
-                      TransformerEncoder, _Packed, _lengths)
+                      TransformerEncoder, _Packed, _lengths, _no_train, encoder_input_bf16)
 
 BuildFrontEnd = {'concat': ConcatFeatureFrontEnd, 'concat-with-linear': ConcatWithLinearFrontEnd, 'conv': ConvFrontEnd}
 BuildEncoder = {'transformer': TransformerEncoder, 'conformer': ConformerEncoder}
@@ -87,17 +87,10 @@ class SpeechToText(nn.Module):
     def encode_bf16(self, inputs, mask, attn_sink=None):
         """frontend + encoder on the fused path -> (memory bf16 [B*T',D], lengths i32 [B], B, T').  attn_sink (a list):
         each encoder block's attention weights f32 [B, H, T', T'] are appended to it."""
-        fe, enc = self.frontend, self.encoder
-        B, T, _ = inputs.shape
-        T2 = fe.output_length(T)
-        lengths = _lengths(fe.output_mask(mask))
-        if enc.fuse_abs_posenc():
-            scale, table = enc.pos_emb.scale_and_table(T2, inputs.device)
-            x, _ = fe.forward_bf16(inputs, scale, table)
-        else:
-            x, _ = fe.forward_bf16(inputs)
-            x = enc.apply_posenc_bf16(x, B, T2)
-        return enc.forward_bf16(x, B, T2, lengths, attn_sink), lengths, B, T2
+        fe, B = self.frontend, inputs.shape[0]
+        _no_train(fe)
+        x, lengths, T2, _ = encoder_input_bf16(fe, self.encoder, inputs, mask, fe._pack.get())
+        return self.encoder.forward_bf16(x, B, T2, lengths, attn_sink), lengths, B, T2
 
     def forward_logits(self, inputs, mask, targets_in):
         """encoder + teacher-forced decoder (the forward half of speech2text.py:39-56) -> logits f32 [B,L,V]."""

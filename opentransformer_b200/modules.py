@@ -195,27 +195,75 @@ class ConvFrontEnd(nn.Module):
             mask = mask[:, start::step][:, :t]
         return mask
 
-    def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
-        """x f32 [B,T,F] -> bf16 [B*T', D].  When posenc_* are given, x*scale+PE is fused into the Linear
-        epilogue (pos.py:56) so the encoder can skip its own positional-encoding pass."""
-        _no_train(self)
-        pk = self._pack.get()
+    def training_pack(self, bf16):
+        """The operands of a training pass: the inference layout, built afresh, and the transposes of w2 and wo that the
+        backward's dgrad GEMMs take.  bf16 is not used: these weights are padded and permuted in fp32."""
+        pk = self._build_pack()
+        pk['w2_t'] = pk['w2'].t().contiguous()           # [kt2*kf2*C1p, C2]
+        pk['wo_t'] = pk['wo'].t().contiguous()           # [F2*C2, D]
+        return pk
+
+    def rows_bf16(self, x, pk, posenc_scale=None, posenc_table=None, keep=False):
+        """The forward of recognition and training: x f32 [B,T,F] -> (bf16 [B*T', D], T', saved).  pk: the inference pack
+        or training_pack().  When posenc_* are given, x*scale+PE is fused into the Linear epilogue (pos.py:56), or applied
+        after front_end_layer_norm, so the encoder can skip its own positional-encoding pass.  saved: what backward reads
+        when keep, else None."""
         B, T, F = x.shape
         if F != self.input_size:
             raise ValueError(f'expected {self.input_size} features, got {F}')
         x = x.contiguous().float()
         T2 = self.output_length(T)
         h1 = ops.conv1_relu(x, pk['w1'], pk['b1'], geom=self.geom)
-        h2 = ops.conv2_relu(h1, pk['w2'], pk['b2'], B, T, F, geom=self.geom)
+        h2 = ops.conv2_relu(h1, pk['w2'], pk['b2'], B, T, F, geom=self.geom)     # [B*T2, F2*C2]
+        y_ln = None     # the Linear's output under front_end_layer_norm, kept for its backward
         if posenc_table is not None and not self.front_end_layer_norm:
             y = ops.linear(h2, pk['wo'], pk['bo'], EPI_TABLE, alpha=posenc_scale, table=posenc_table, period=T2)
         else:
             y = ops.linear(h2, pk['wo'], pk['bo'], EPI_BIAS)
             if self.front_end_layer_norm:
-                y = ops.layernorm(y, *pk['ln'])
+                y_ln, y = y, ops.layernorm(y, *pk['ln'])
             if posenc_table is not None:
                 y = ops.scale_add_table(y, posenc_scale, posenc_table, T2)
-        return y, T2
+        saved = {'x': x, 'h1': h1, 'h2': h2, 'y_ln': y_ln, 'scale': posenc_scale} if keep else None
+        return y, T2, saved
+
+    def backward(self, dx, pk, saved, g):
+        """Backward of rows_bf16 from dx, the gradient of its output (bf16 [B*T', D]): x = (h2 Wo^T + bo) * scale + PE
+        (without posenc: h2 Wo^T + bo) -> conv2 (implicit-GEMM forward, im2col GEMMs backward) -> conv1.  pk: the
+        training_pack().  The parameter gradients go into g (train.Grads) under their names in the model ('frontend.*'), in
+        the reference's layouts: output_layer's columns back in c*F2 + f order, the C1p channel padding cut off."""
+        acc = g.sink is not None
+        x, h1, h2 = saved['x'], saved['h1'], saved['h2']
+        B, T, F = x.shape
+        (T2, F2) = self.sizes(T)[1]
+        C1p, C2, C1 = pk['C1p'], pk['w2'].shape[0], self.conv1.conv_layer.out_channels
+        kt1, kf1, _, _, kt2, kf2, _, _ = self.geom
+        dyl = ops.scale_add_table(dx, saved['scale']) if saved['scale'] is not None else dx   # d(h2 Wo^T + bo) = scale * dx
+        if saved['y_ln'] is not None:                                                         # through front_end_layer_norm
+            wname, bname = 'frontend.layer_norm.weight', 'frontend.layer_norm.bias'
+            dyl, g[wname], g[bname] = ops.layernorm_bwd(dyl, saved['y_ln'], pk['ln'][0], dgamma=g.out(wname),
+                                                        dbeta=g.out(bname), accumulate=acc)
+        D_out = self.output_size
+        dwo = ops.linear_wgrad(dyl, h2)                                               # [D, F2*C2], feature index f*C2 + c
+        g.put('frontend.output_layer.weight', dwo.view(D_out, F2, C2).permute(0, 2, 1).reshape(D_out, C2 * F2))
+        g['frontend.output_layer.bias'] = ops.colsum(dyl, out=g.out('frontend.output_layer.bias'), accumulate=acc)
+        dh2 = ops.linear(dyl, pk['wo_t'])                                             # [B*T2, F2*C2]
+        dpre2 = ops.relu_bwd(dh2, h2).view(B * T2 * F2, C2)
+        col = ops.conv_im2col(h1, B, T, F, C1p, geom=self.geom)
+        dw2 = ops.linear_wgrad(dpre2, col)                                            # [C2, kt2*kf2*C1p], k = (kh*kf2+kw)*C1p + c
+        g.put('frontend.conv2.conv_layer.weight', dw2.view(C2, kt2, kf2, C1p)[..., :C1].permute(0, 3, 1, 2))
+        g['frontend.conv2.conv_layer.bias'] = ops.colsum(dpre2, out=g.out('frontend.conv2.conv_layer.bias'), accumulate=acc)
+        dcol = ops.linear(dpre2, pk['w2_t'])                                          # [B*T2*F2, kt2*kf2*C1p]
+        del col
+        dpre1 = ops.conv_col2im_relu(dcol, h1, B, T, F, C1p, geom=self.geom)
+        g1 = ops.conv1_wgrad(dpre1, x, B, T, F, C1p, geom=self.geom)                  # [C1p, kt1*kf1 taps + bias]
+        g.put('frontend.conv1.conv_layer.weight', g1[:C1, :kt1 * kf1].reshape(C1, 1, kt1, kf1))
+        g.put('frontend.conv1.conv_layer.bias', g1[:C1, kt1 * kf1])
+
+    def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
+        """x f32 [B,T,F] -> (bf16 [B*T', D], T'): rows_bf16 on the inference pack."""
+        _no_train(self)
+        return self.rows_bf16(x, self._pack.get(), posenc_scale, posenc_table)[:2]
 
     def forward(self, x, mask):
         y, T2 = self.forward_bf16(x)
@@ -242,6 +290,7 @@ class ConcatFeatureFrontEnd(nn.Module):
         self.input_size = input_size
         self.nframes = left_frames + right_frames + 1
         self.output_size = self.nframes * input_size
+        self._pack = _Packed(self, self._build_pack)
         if frame_rate < 10:
             raise ValueError(f'concat front end: frame_rate {frame_rate} gives stride int(frame_rate / 10) = 0; it must be >= 10')
         if left_frames < 0 or right_frames < 0:
@@ -274,15 +323,30 @@ class ConcatFeatureFrontEnd(nn.Module):
             mask = torch.cat([mask, torch.zeros(B, pad, dtype=mask.dtype, device=mask.device)], dim=1)
         return mask[:, self.left_frames::self.stride]
 
-    def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
-        """x f32 [B,T,F] -> (bf16 [B*T', W], T'), W = n F rounded up to 8 (zero columns past n F).  When posenc_* are
-        given, x*scale+PE is applied in the same pass (otb_frame_stack's epilogue)."""
+    def _build_pack(self, bf16=None):
+        return {}
+
+    def training_pack(self, bf16):
+        """The operands of a training pass, laid out as the inference pack.  bf16: a parameter -> its bf16 copy."""
+        return self._build_pack(bf16)
+
+    def rows_bf16(self, x, pk, posenc_scale=None, posenc_table=None, keep=False):
+        """The forward of recognition and training: x f32 [B,T,F] -> (bf16 [B*T', W], T', None), W = n F rounded up to 8
+        (zero columns past n F).  When posenc_* are given, x*scale+PE is applied in the same pass (otb_frame_stack's
+        epilogue).  No parameters: pk is empty, and backward needs nothing saved."""
         B, T, F = x.shape
         if F != self.input_size:
             raise ValueError(f'expected {self.input_size} features, got {F}')
         T2 = self.output_length(T)
         alpha = 1.0 if posenc_table is None else posenc_scale
-        return ops.frame_stack(x.contiguous().float(), self.nframes, self.stride, T2, alpha, posenc_table), T2
+        return ops.frame_stack(x.contiguous().float(), self.nframes, self.stride, T2, alpha, posenc_table), T2, None
+
+    def backward(self, dx, pk, saved, g):
+        """The reference stacks without gradient (concat.py:35-37), and there are no parameters: nothing to do."""
+
+    def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
+        """x f32 [B,T,F] -> (bf16 [B*T', W], T'): rows_bf16."""
+        return self.rows_bf16(x, self._pack.get(), posenc_scale, posenc_table)[:2]
 
     def forward(self, x, mask):
         m = self.output_mask(mask)
@@ -310,25 +374,40 @@ class ConcatWithLinearFrontEnd(ConcatFeatureFrontEnd):
                                       'concat.py:55); use dropout 0.0')
         self.linear = nn.Linear(self.output_size, output_size)
         self.dropout = dropout
-        self._pack = _Packed(self, lambda: (self.pack_linear(_w(self.linear)), _b(self.linear)))
 
-    def pack_linear(self, w):
-        """The Linear weight bf16 [D, n F] as the GEMM takes it: K zero-padded to the stacked rows' width."""
+    def _build_pack(self, bf16=None):
+        """{'w': the Linear weight bf16 [D, n F] as the GEMM takes it, K zero-padded to the stacked rows' width, 'b': its
+        fp32 bias}.  bf16: a parameter -> its bf16 copy (a cast by default)."""
+        w = bf16(self.linear.weight) if bf16 is not None else _w(self.linear)
         K = (self.output_size + 7) // 8 * 8
-        if K == w.shape[1]:
-            return w.contiguous()
-        wp = torch.zeros(w.shape[0], K, dtype=BF16, device=w.device)
-        wp[:, :w.shape[1]] = w
-        return wp
+        if K != w.shape[1]:
+            wp = torch.zeros(w.shape[0], K, dtype=BF16, device=w.device)
+            wp[:, :w.shape[1]] = w
+            w = wp
+        return {'w': w.contiguous(), 'b': _b(self.linear)}
+
+    def rows_bf16(self, x, pk, posenc_scale=None, posenc_table=None, keep=False):
+        """The forward of recognition and training: x f32 [B,T,F] -> (bf16 [B*T', D], T', saved).  pk: the inference pack
+        or training_pack().  When posenc_* are given, x*scale+PE is fused into the Linear epilogue.  saved: what backward
+        reads when keep, else None."""
+        stack, T2, _ = super().rows_bf16(x, pk)
+        if posenc_table is not None:
+            y = ops.linear(stack, pk['w'], pk['b'], EPI_TABLE, alpha=posenc_scale, table=posenc_table, period=T2)
+        else:
+            y = ops.linear(stack, pk['w'], pk['b'], EPI_BIAS)
+        return y, T2, {'stack': stack, 'scale': posenc_scale} if keep else None
+
+    def backward(self, dx, pk, saved, g):
+        """Backward of rows_bf16 from dx, the gradient of its output (bf16 [B*T', D]): the Linear's gradients into g
+        (train.Grads) as 'frontend.linear.*', the padding columns cut off.  The stacking has no gradient (concat.py:35-37)."""
+        dy = ops.scale_add_table(dx, saved['scale']) if saved['scale'] is not None else dx
+        g.put('frontend.linear.weight', ops.linear_wgrad(dy, saved['stack'])[:, :self.output_size])
+        g['frontend.linear.bias'] = ops.colsum(dy, out=g.out('frontend.linear.bias'), accumulate=g.sink is not None)
 
     def forward_bf16(self, x, posenc_scale=None, posenc_table=None):
-        """x f32 [B,T,F] -> (bf16 [B*T', D], T').  When posenc_* are given, x*scale+PE is fused into the Linear epilogue."""
+        """x f32 [B,T,F] -> (bf16 [B*T', D], T'): rows_bf16 on the inference pack."""
         _no_train(self)
-        stack, T2 = super().forward_bf16(x)
-        w, b = self._pack.get()
-        if posenc_table is not None:
-            return ops.linear(stack, w, b, EPI_TABLE, alpha=posenc_scale, table=posenc_table, period=T2), T2
-        return ops.linear(stack, w, b, EPI_BIAS), T2
+        return self.rows_bf16(x, self._pack.get(), posenc_scale, posenc_table)[:2]
 
     def forward(self, x, mask):
         m = self.output_mask(mask)
@@ -497,7 +576,53 @@ class TransformerEncoderLayer(nn.Module):
         return _ffn(x, pk['ffn'], x, None if nb else pk['ln2'])
 
 
-class TransformerEncoder(nn.Module):
+class _SpeechEncoder(nn.Module):
+    """The positional input and module-level forward that TransformerEncoder and ConformerEncoder share.  Abs-pos encoders
+    scale their input and add PE (pos.py:56); rel-pos encoders take it as it is and give PE[-(T-1)..T-1] to their
+    attention (encoder/transformer.py:116-119, encoder/conformer.py:140-149)."""
+
+    def fuse_abs_posenc(self):
+        """True when x*scale+PE may be fused into the front end's last kernel."""
+        return self.positional_encoding and not self.relative_positional
+
+    def rel_pos_table(self, T, device):
+        """PE[-(T-1) .. T-1] bf16 [2T-1, d], the GEMM operand of the rel-pos attention's pos_proj (cached per T and device);
+        None for an encoder without rel-pos attention."""
+        if not (self.positional_encoding and self.relative_positional):
+            return None
+        key = (T, device.index)
+        p = self._pos_cache.get(key)
+        if p is None:
+            p = ops.scale_add_table(ops.sinusoid_table(2 * T - 1, self.d_model, -(T - 1), device))
+            self._pos_cache[key] = p
+        return p
+
+    def apply_posenc_bf16(self, x, B, T):
+        if self.fuse_abs_posenc():
+            scale, table = self.pos_emb.scale_and_table(T, x.device)
+            return ops.scale_add_table(x, scale, table, T)
+        return x if x.dtype == BF16 else ops.scale_add_table(x)
+
+    def forward(self, inputs, mask):
+        B, T, D = inputs.shape
+        x = self.apply_posenc_bf16(inputs.contiguous().view(B * T, D), B, T)
+        sink = [] if self.return_attn_weights else None
+        y = self.forward_bf16(x, B, T, _lengths(mask), sink)
+        return y.float().view(B, T, D), mask, encoder_attn_weights(len(self.blocks), sink)
+
+
+def encoder_input_bf16(frontend, encoder, x, mask, pk, keep=False):
+    """The front half of a speech model, for recognition and training: x f32 [B,T,F], mask bool [B,T] -> (the encoder's
+    input bf16 [B*T', d], lengths i32 [B], T', what frontend.backward reads when keep).  An abs-pos encoder's x*scale+PE is
+    fused into the front end; a rel-pos encoder takes the front end's rows as they are.  pk: the front end's operands."""
+    T2 = frontend.output_length(x.shape[1])
+    lengths = _lengths(frontend.output_mask(mask))
+    scale, table = encoder.pos_emb.scale_and_table(T2, x.device) if encoder.fuse_abs_posenc() else (None, None)
+    y, _, saved = frontend.rows_bf16(x, pk, scale, table, keep)
+    return y, lengths, T2, saved
+
+
+class TransformerEncoder(_SpeechEncoder):
     """forward(inputs f32 [B,T,D], mask bool [B,T]) -> (f32 [B,T,D], mask, attn_weights)
 
     ``attn_weights`` maps 'enc_block_i' -> {'slf_attn_weights': P}.  The fused attention kernel never forms P, so by
@@ -512,6 +637,7 @@ class TransformerEncoder(nn.Module):
         super().__init__()
         self.d_model = d_model
         self.normalize_before = normalize_before
+        self.positional_encoding = True     # ConformerEncoder's switch: the reference's Transformer encoder always has one
         self.relative_positional = relative_positional
         self.pos_emb = PositionalEncoding(d_model, pos_dropout)
         self.blocks = nn.ModuleList([
@@ -525,42 +651,17 @@ class TransformerEncoder(nn.Module):
         self._pos_cache = {}
         self.return_attn_weights = False
 
-    def _rel_pos(self, T, device):
-        key = (T, device.index)
-        p = self._pos_cache.get(key)
-        if p is None:   # PE[-(T-1) .. T-1] (encoder/transformer.py:117-119), bf16 GEMM operand of pos_proj
-            p = ops.scale_add_table(ops.sinusoid_table(2 * T - 1, self.d_model, -(T - 1), device))
-            self._pos_cache[key] = p
-        return p
-
     def forward_bf16(self, x, B, T, lengths, attn_sink=None):
         """x bf16 [B*T, d] with the positional encoding already applied (abs-pos) / the raw front-end output (rel-pos).
         attn_sink (a list): each block's attention weights f32 [B, H, T, T] are appended to it."""
         _no_train(self)
         pk = self._pack.get()
-        pos = self._rel_pos(T, x.device) if self.relative_positional else None
+        pos = self.rel_pos_table(T, x.device)
         for blk, bpk in zip(self.blocks, pk['blocks']):
             x = blk.run(x, bpk, B, T, lengths, pos_bf16=pos, attn_sink=attn_sink)
         if self.normalize_before:
             x = ops.layernorm(x, *pk['norm'])
         return x
-
-    def fuse_abs_posenc(self):
-        """True when x*sqrt(d)+PE may be fused into the front end's Linear epilogue."""
-        return not self.relative_positional
-
-    def apply_posenc_bf16(self, x, B, T):
-        if self.relative_positional:       # enc_output = inputs (encoder/transformer.py:116): no x*sqrt(d)+PE
-            return x if x.dtype == BF16 else ops.scale_add_table(x)
-        scale, table = self.pos_emb.scale_and_table(T, x.device)
-        return ops.scale_add_table(x, scale, table, T)
-
-    def forward(self, inputs, mask):
-        B, T, D = inputs.shape
-        x = self.apply_posenc_bf16(inputs.contiguous().view(B * T, D), B, T)
-        sink = [] if self.return_attn_weights else None
-        y = self.forward_bf16(x, B, T, _lengths(mask), sink)
-        return y.float().view(B, T, D), mask, encoder_attn_weights(len(self.blocks), sink)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -712,7 +813,7 @@ class ConformerEncoderBlock(nn.Module):
         return ops.layernorm(x, *pk['post_ln'], *pk['final_ln'])   # post_ffn_norm then final_norm, one kernel
 
 
-class ConformerEncoder(nn.Module):
+class ConformerEncoder(_SpeechEncoder):
     """forward(inputs f32 [B,T,D], mask bool [B,T]) -> (f32 [B,T,D], mask, attn_weights)   (encoder/conformer.py:117-164)
 
     The reference applies F.dropout(p=residual_dropout) with training=True even in eval() (conformer.py:53,58,63,72),
@@ -739,38 +840,14 @@ class ConformerEncoder(nn.Module):
         self._pos_cache = {}
         self.return_attn_weights = False
 
-    def fuse_abs_posenc(self):
-        return self.positional_encoding and not self.relative_positional
-
-    def apply_posenc_bf16(self, x, B, T):
-        if self.positional_encoding and not self.relative_positional:
-            scale, table = self.pos_emb.scale_and_table(T, x.device)
-            return ops.scale_add_table(x, scale, table, T)
-        return x if x.dtype == BF16 else ops.scale_add_table(x)
-
-    def _rel_pos(self, T, device):
-        key = (T, device.index)
-        p = self._pos_cache.get(key)
-        if p is None:   # PE[-(T-1) .. T-1] (encoder/conformer.py:140-143), bf16 GEMM operand
-            p = ops.scale_add_table(ops.sinusoid_table(2 * T - 1, self.d_model, -(T - 1), device))
-            self._pos_cache[key] = p
-        return p
-
     def forward_bf16(self, x, B, T, lengths, attn_sink=None):
         """attn_sink (a list): each block's attention weights f32 [B, H, T, T] are appended to it."""
         _no_train(self)
         pks = self._pack.get()
-        pos = self._rel_pos(T, x.device) if (self.positional_encoding and self.relative_positional) else None
+        pos = self.rel_pos_table(T, x.device)
         for blk, pk in zip(self.blocks, pks):
             x = blk.run(x, pk, B, T, lengths, pos, attn_sink)
         return x
-
-    def forward(self, inputs, mask):
-        B, T, D = inputs.shape
-        x = self.apply_posenc_bf16(inputs.contiguous().view(B * T, D), B, T)
-        sink = [] if self.return_attn_weights else None
-        y = self.forward_bf16(x, B, T, _lengths(mask), sink)
-        return y.float().view(B, T, D), mask, encoder_attn_weights(len(self.blocks), sink)
 
 
 # ------------------------------------------------------------------------------------------------

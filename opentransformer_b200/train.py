@@ -35,6 +35,9 @@ attention's output dropout (`slf_attn_dropout`, the decoder's `src_attn_dropout`
 ffn_dropout and pos_dropout must be 0 (as shipped) and raise otherwise.  The encoder may also be the shipped Conformer
 layout with 64-wide heads (macaron feed-forward, rel-pos attention, then the convolution module with training-mode
 BatchNorm; encoder/conformer.py:75-89).
+The front end is not written here: its forward is the one recognition runs (modules.encoder_input_bf16, which also fuses
+the encoder's positional input), told to keep what the backward reads, and its backward sits beside it on its class
+(ConvFrontEnd.backward, ...).
 The CTC-only model (model/ctc.py) is the front-end + encoder half (_encoder_fwd / _encoder_bwd) with the CTC head and
 otb_ctc_loss in place of the decoder; the Transformer language model is the encoder layer (enc_layer_fwd / enc_layer_bwd)
 under the causal mask.  All four models share the vocabulary head (head_fwd / head_bwd) and embedding_bwd.
@@ -48,9 +51,8 @@ from . import ops
 from . import modules
 from .dp import allreduce_mean_, broadcast_from_first_, rank_in
 from .graphs import CapturedStep, lru_get
-from .modules import (ConcatFeatureFrontEnd, ConcatWithLinearFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder,
-                      TransformerEncoder, _lengths)
-from .ops import BF16, EPI_BIAS, EPI_RESID, EPI_TABLE, EPI_RELU
+from .modules import ConcatFeatureFrontEnd, ConformerEncoder, ConvFrontEnd, TransformerDecoder, TransformerEncoder
+from .ops import BF16, EPI_BIAS, EPI_RESID, EPI_RELU
 
 
 def _bf(t):
@@ -184,25 +186,11 @@ class EncoderPack(LayerPack):
             raise NotImplementedError('training path: learnable positional scale (pos_dropout > 0)')
         self.rates = {name: check_blocks(stack.blocks) for name, stack in stacks}
         self.attn_rates = {name: [attn_dropout_rates(b) for b in stack.blocks] for name, stack in stacks}
-        self.fe = self._frontend(fe)
+        self.fe = fe.training_pack(self.w)
         self.enc = [self._conf_layer(b) if self.conformer else self.enc_layer(b) for b in enc.blocks]
         # pre-norm stacks end with one more LayerNorm (encoder/transformer.py:96-97,131-132; decoder/transformer.py:151-152,178-179)
         self.enc_pre = bool(getattr(enc, 'normalize_before', False))
         self.enc_norm = self._ln(enc.norm) if self.enc_pre else None
-
-    def _frontend(self, fe):
-        """The front end's operands: the conv front end's packed weights and their transposes; concat-with-linear's
-        Linear (K padded as the stacked rows); nothing for concat."""
-        if isinstance(fe, ConcatWithLinearFrontEnd):
-            return {'w': fe.pack_linear(self.w(fe.linear.weight)), 'b': _f(fe.linear.bias)}
-        if isinstance(fe, ConcatFeatureFrontEnd):
-            return {}
-        pk = dict(fe._build_pack())
-        pk['w2_t'] = pk['w2'].t().contiguous()           # [kt2*kf2*C1p, C2]
-        pk['wo_t'] = pk['wo'].t().contiguous()           # [F2*C2, D]
-        if fe.front_end_layer_norm:
-            pk['ln'] = self._ln(fe.layer_norm)
-        return pk
 
     def _conf_layer(self, b):
         """A Conformer block: the rel-pos projection as ONE GEMM producing [q+u | q+v | k | v] (W_ext = [Wq; Wq; Wk; Wv],
@@ -619,71 +607,37 @@ def embedding_bwd(tok, dx, emb, scale, g, name):
     ops.embed_bwd(tok, dx, g[name], scale)
 
 
-# h1, h2: the conv front end's activations (h2 the input of its Linear, y its output when front_end_layer_norm follows);
-# for concat-with-linear h2 holds the stacked rows, the input of its Linear, and h1 is None; for concat all are None
-_EncTrace = namedtuple('_EncTrace', 'x_in h1 h2 y tape pe scale lengths enc_last drops B T F T2 F2')
+# fe: what the front end's backward reads (its rows_bf16's saved); pe: the rel-pos table of a Conformer
+_EncTrace = namedtuple('_EncTrace', 'fe tape pe lengths enc_last drops B T2')
 
 
 def _encoder_fwd(model, pk, inputs, mask, drop_seed):
-    """Front end + encoder in training mode, the half shared by SpeechToText and CTCModel -> (memory bf16 [B*T', d],
-    _EncTrace: what _encoder_bwd reads)."""
-    fe, enc = model.frontend, model.encoder
-    dev = inputs.device
-    conformer = pk.conformer
-    B, T, F = inputs.shape
+    """Front end + encoder in training mode, the half shared by SpeechToText, CTCModel and TransducerModel -> (memory bf16
+    [B*T', d], _EncTrace: what _encoder_bwd reads).  The front half is the one recognition runs (encoder_input_bf16), on
+    the training pack's front-end operands."""
+    enc = model.encoder
+    B = inputs.shape[0]
     H = enc.blocks[0].n_heads
-    x_in = inputs.contiguous().float()
-    T2 = fe.output_length(T)
-    lengths = _lengths(fe.output_mask(mask))
-    fpk = pk.fe
-    scale, table = None, None
-    if enc.fuse_abs_posenc():
-        scale, table = enc.pos_emb.scale_and_table(T2, dev)
-    # rel-pos encoders take the front end's output as is (encoder/conformer.py:141-149)
-    h1, h2, y, F2 = None, None, None, None
-    if isinstance(fe, ConvFrontEnd):
-        F2 = fe.sizes(T)[1][1]
-        h1 = ops.conv1_relu(x_in, fpk['w1'], fpk['b1'], geom=fe.geom)
-        h2 = ops.conv2_relu(h1, fpk['w2'], fpk['b2'], B, T, F, geom=fe.geom)    # [B*T2, F2*C2]
-        lin = (fpk['wo'], fpk['bo'])
-    elif isinstance(fe, ConcatWithLinearFrontEnd):
-        h2 = ops.frame_stack(x_in, fe.nframes, fe.stride, T2)                     # [B*T2, n F rounded up to 8]
-        lin = (fpk['w'], fpk['b'])
-    if h2 is None:      # concat: the stacked frames are the encoder's input
-        x = ops.frame_stack(x_in, fe.nframes, fe.stride, T2, 1.0 if scale is None else scale, table)
-    elif 'ln' in fpk:   # front_end_layer_norm (conv.py:150-151), then the encoder's scale and positions
-        y = ops.linear(h2, *lin, EPI_BIAS)
-        x = _norm(y, fpk['ln'])
-        if scale is not None:
-            x = ops.scale_add_table(x, scale, table, T2)
-    elif scale is not None:
-        x = ops.linear(h2, *lin, EPI_TABLE, alpha=scale, table=table, period=T2)
-    else:
-        x = ops.linear(h2, *lin, EPI_BIAS)
+    x, lengths, T2, fe_saved = modules.encoder_input_bf16(model.frontend, enc, inputs, mask, pk.fe, keep=True)
     e_drop = _drops(pk.rates['encoder'], pk.attn_rates['encoder'], drop_seed, ENC_SITE, _enc_sites(enc))
     enc_tape = []
-    pe = enc._rel_pos(T2, dev) if conformer else None
+    pe = enc.rel_pos_table(T2, inputs.device)
     for p, drop in zip(pk.enc, e_drop):
-        if conformer:
+        if pk.conformer:
             x, t = _conformer_block_fwd(p, x, B, H, T2, lengths, pe, drop)
         else:
             x, t = enc_layer_fwd(p, x, pk.enc_pre, B, H, T2, lengths, drop)
         enc_tape.append(t)
-    if conformer:       # the running statistics moved: the inference pack, which folds BatchNorm, must be rebuilt
+    if pk.conformer:    # the running statistics moved: the inference pack, which folds BatchNorm, must be rebuilt
         modules.bump_param_generation()
     mem = _norm(x, pk.enc_norm) if pk.enc_pre else x
-    return mem, _EncTrace(x_in=x_in, h1=h1, h2=h2, y=y, tape=enc_tape, pe=pe, scale=scale, lengths=lengths, enc_last=x, drops=e_drop,
-                          B=B, T=T, F=F, T2=T2, F2=F2)
+    return mem, _EncTrace(fe=fe_saved, tape=enc_tape, pe=pe, lengths=lengths, enc_last=x, drops=e_drop, B=B, T2=T2)
 
 
 def _encoder_bwd(model, pk, tr, dx, g):
     """Backward of _encoder_fwd from dx = the gradient of the memory (bf16 [B*T', d]): encoder layers in reverse, then the
-    front end.  Parameter gradients go into g."""
-    fe, enc = model.frontend, model.encoder
-    acc = g.sink is not None
-    B, T, F, T2, F2 = tr.B, tr.T, tr.F, tr.T2, tr.F2
-    H = enc.blocks[0].n_heads
-    fpk = pk.fe
+    front end's backward.  Parameter gradients go into g."""
+    B, T2, H = tr.B, tr.T2, model.encoder.blocks[0].n_heads
     if pk.enc_pre:
         dx = _ln_bwd(dx, tr.enc_last, pk.enc_norm, g)
     for i in reversed(range(len(pk.enc))):
@@ -691,39 +645,7 @@ def _encoder_bwd(model, pk, tr, dx, g):
             dx = _conformer_block_bwd(pk.enc[i], tr.tape[i], dx, g, B, H, T2, tr.lengths, tr.pe, tr.drops[i])
         else:
             dx = enc_layer_bwd(pk.enc[i], tr.tape[i], dx, pk.enc_pre, g, B, H, T2, tr.lengths, tr.drops[i])
-
-    # front end: x = (h2 Wo^T + bo) * sqrt(d) + PE (abs-pos; rel-pos: x = h2 Wo^T + bo) -> conv2 (implicit-GEMM forward,
-    # im2col GEMMs backward) -> conv1.  The concat front ends stack without gradient (concat.py:35-37): concat-with-linear
-    # stops at its Linear's parameters, concat at the encoder's input.
-    h1, h2 = tr.h1, tr.h2
-    if isinstance(fe, ConcatFeatureFrontEnd):
-        if isinstance(fe, ConcatWithLinearFrontEnd):
-            dyl = ops.scale_add_table(dx, tr.scale) if tr.scale is not None else dx
-            g.put('frontend.linear.weight', ops.linear_wgrad(dyl, h2)[:, :fe.output_size])   # the padding columns cut off
-            g['frontend.linear.bias'] = ops.colsum(dyl, out=g.out('frontend.linear.bias'), accumulate=acc)
-        return
-    C1p, C2 = fpk['C1p'], fpk['w2'].shape[0]
-    kt1, kf1, _, _, kt2, kf2, _, _ = fe.geom
-    dyl = ops.scale_add_table(dx, tr.scale) if tr.scale is not None else dx      # d(h2 Wo^T + bo) = sqrt(d) * dx
-    if tr.y is not None:                                                          # through front_end_layer_norm
-        dyl = _ln_bwd(dyl, tr.y, fpk['ln'], g)
-    D_out = fe.output_size
-    dwo = ops.linear_wgrad(dyl, h2)                                               # [D, F2*C2], feature index f*C2 + c
-    g.put('frontend.output_layer.weight', dwo.view(D_out, F2, C2).permute(0, 2, 1).reshape(D_out, C2 * F2))
-    g['frontend.output_layer.bias'] = ops.colsum(dyl, out=g.out('frontend.output_layer.bias'), accumulate=acc)
-    dh2 = ops.linear(dyl, fpk['wo_t'])                                            # [B*T2, F2*C2]
-    dpre2 = ops.relu_bwd(dh2, h2).view(B * T2 * F2, C2)
-    col = ops.conv_im2col(h1, B, T, F, C1p, geom=fe.geom)
-    C1 = fe.conv1.conv_layer.out_channels
-    dw2 = ops.linear_wgrad(dpre2, col)                                            # [C2, kt2*kf2*C1p], k = (kh*kf2+kw)*C1p + c
-    g.put('frontend.conv2.conv_layer.weight', dw2.view(C2, kt2, kf2, C1p)[..., :C1].permute(0, 3, 1, 2))
-    g['frontend.conv2.conv_layer.bias'] = ops.colsum(dpre2, out=g.out('frontend.conv2.conv_layer.bias'), accumulate=acc)
-    dcol = ops.linear(dpre2, fpk['w2_t'])                                         # [B*T2*F2, kt2*kf2*C1p]
-    del col
-    dpre1 = ops.conv_col2im_relu(dcol, h1, B, T, F, C1p, geom=fe.geom)
-    g1 = ops.conv1_wgrad(dpre1, tr.x_in, B, T, F, C1p, geom=fe.geom)              # [C1p, kt1*kf1 taps + bias]
-    g.put('frontend.conv1.conv_layer.weight', g1[:C1, :kt1 * kf1].reshape(C1, 1, kt1, kf1))
-    g.put('frontend.conv1.conv_layer.bias', g1[:C1, kt1 * kf1])
+    model.frontend.backward(dx, pk.fe, tr.fe, g)
 
 
 def _ctc_head(model, pk):
