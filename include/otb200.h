@@ -578,18 +578,38 @@ int otb_conv1_wgrad(const void* dpre1, const float* x, float* out, int B, int T,
  *   past the last frame, decrements *active.  Ended rows are left unchanged.  LM shallow fusion (all three optional, NULL:
  *   none): val f32 [B] the fused value of idx (otb_logsoftmax_topk with blank exempt), which a label adds to score in place
  *   of its log-prob; emit i32 [B] = 1 where the row emitted a label this step, else 0; lm_pos i32 [B] = the label's LM
- *   position (n_out after it, 1..max_len) where it emitted, else -1. */
+ *   position (n_out after it, 1..max_len) where it emitted, else -1.
+ * Pruned lattice (pruned RNN-T): joint, joint_bwd, logprob, loss and dlogits take (s_begin, S).  s_begin i32 [B, T] non-NULL
+ *   keeps at frame t the S label positions u = s_begin[b T + t] + k, k < S (2 <= S <= 1024), stored [B, T, S] with k
+ *   fastest: node (b, t, k) is row (b T + t) S + k, and every [B T U1, .] array above is [B T S, .].  A node outside its
+ *   frame's band does not exist: the loss's alignments stay inside the bands, and an utterance without such an alignment
+ *   gets nll +inf and zero gradients.  dPp row (b, u) sums over the frames whose band holds u.  NULL: the full lattice.
+ * otb_rnnt_simple_lse: the simple joint's node log-probs for logits am[b T + t] + lm[b U1 + u] (am f32 [B T, lda], lm f32
+ *   [B U1, ldl]) -> lp f32 [B T U1, 3] as otb_rnnt_logprob writes them, in fp32 through one [T, V] x [V, U1] product per
+ *   utterance, and the row maxima m_am f32 [B T], m_lm f32 [B U1] the backward reads.
+ * otb_rnnt_simple_bwd: from otb_rnnt_loss's grad over that lp, scaled by scale (* *scale_dev when not NULL): d am bf16
+ *   [B T, ldd] and d lm bf16 [B U1, ldd], columns >= V zero; the one-hot terms summed in a fixed order, no atomics.
+ * otb_rnnt_prune_ranges: s_begin i32 [B, T] from the simple loss's grad [B T U1, 2]: the S-wide window of largest occupancy
+ *   at each frame, then the range rule of DESIGN.md 4.22 (s_0 = 0, non-decreasing, consecutive bands overlap, the last
+ *   band holds U_b).  Frames past t_len get 0. */
 int otb_rnnt_joint(const void* ep, const void* pp, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len, void* out,
-                   void* stream);
+                   const int32_t* s_begin, int S, void* stream);
 int otb_rnnt_joint_bwd(const void* dh, const void* h, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len,
-                       void* dep, void* dpp, void* stream);
+                       void* dep, void* dpp, const int32_t* s_begin, int S, void* stream);
 int otb_rnnt_logprob(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
-                     const int32_t* u_len, const int32_t* labels, int ldy, float* lp, void* stream);
+                     const int32_t* u_len, const int32_t* labels, int ldy, float* lp, const int32_t* s_begin, int S, void* stream);
 int otb_rnnt_loss(const float* lp, int B, int T, int U1, const int32_t* t_len, const int32_t* u_len, double* alpha, float* nll,
-                  float* loss, float* grad, float grad_scale, const float* grad_scale_dev, void* stream);
+                  float* loss, float* grad, float grad_scale, const float* grad_scale_dev, const int32_t* s_begin, int S, void* stream);
 int otb_rnnt_dlogits(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
                      const int32_t* u_len, const int32_t* labels, int ldy, const float* lp, const float* grad, void* dz, int ldd,
-                     void* stream);
+                     const int32_t* s_begin, int S, void* stream);
+int otb_rnnt_simple_lse(const float* am, int lda, const float* lm, int ldl, int V, int B, int T, int U1, const int32_t* t_len,
+                        const int32_t* u_len, const int32_t* labels, int ldy, float* lp, float* m_am, float* m_lm, void* stream);
+int otb_rnnt_simple_bwd(const float* am, int lda, const float* lm, int ldl, int V, int B, int T, int U1, const int32_t* t_len,
+                        const int32_t* u_len, const int32_t* labels, int ldy, const float* lp, const float* m_am, const float* m_lm,
+                        const float* grad, float scale, const float* scale_dev, void* d_am, void* d_lm, int ldd, void* stream);
+int otb_rnnt_prune_ranges(const float* grad, int B, int T, int U1, const int32_t* t_len, const int32_t* u_len, int S, int32_t* s_begin,
+                          void* stream);
 int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const float* h_new, const float* c_new, const void* pp_new,
                          float* h, float* c, void* pp, int layers, int B, int H, int D, const void* ep, int T, void* ep_cur,
                          const int32_t* t_len, int32_t* frame, int32_t* n_sym, int32_t* n_out, int32_t* ids, int max_len,

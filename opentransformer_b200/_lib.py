@@ -111,11 +111,16 @@ _SIGS = {
     'otb_ctc_prefix_advance': (c_int, [POINTER(BeamStateC), _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     'otb_ctc_nbest_score': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_int, _P, _P]),
     'otb_token_logprob': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P]),
-    'otb_rnnt_joint': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
-    'otb_rnnt_joint_bwd': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
-    'otb_rnnt_logprob': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
-    'otb_rnnt_loss': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, c_float, _P, _P]),
-    'otb_rnnt_dlogits': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, _P, c_int, _P]),
+    'otb_rnnt_joint': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P]),
+    'otb_rnnt_joint_bwd': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P]),
+    'otb_rnnt_logprob': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, c_int, _P]),
+    'otb_rnnt_loss': (c_int, [_P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, c_float, _P, _P, c_int, _P]),
+    'otb_rnnt_dlogits': (c_int, [_P, c_int, c_int, c_int64, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, _P, c_int, _P, c_int,
+                                 _P]),
+    'otb_rnnt_simple_lse': (c_int, [_P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, _P, _P]),
+    'otb_rnnt_simple_bwd': (c_int, [_P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, _P, _P, c_float, _P,
+                                    _P, _P, c_int, _P]),
+    'otb_rnnt_prune_ranges': (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int, _P, _P]),
     'otb_rnnt_greedy_step': (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P, _P,
                                      _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     'otb_rnnt_beam_step': (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P,

@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libotb200.so')
-SOURCES = ['gemm_tc.cu', 'attn_tc.cu', 'attn_probs.cu', 'attn_bwd.cu', 'backward.cu', 'conformer_train.cu', 'lstm.cu', 'ops_simt.cu', 'beam.cu', 'decode_group.cu', 'loss.cu', 'ctc.cu', 'ctc_decode.cu', 'ctc_align.cu', 'ctc_prefix.cu', 'ctc_score.cu', 'rescore.cu', 'mwer.cu', 'mixspeech.cu', 'frame_stack.cu', 'fbank.cu', 'resample.cu', 'rnnt.cu', 'rnnt_beam.cu', 'capi.cu']
+SOURCES = ['gemm_tc.cu', 'attn_tc.cu', 'attn_probs.cu', 'attn_bwd.cu', 'backward.cu', 'conformer_train.cu', 'lstm.cu', 'ops_simt.cu', 'beam.cu', 'decode_group.cu', 'loss.cu', 'ctc.cu', 'ctc_decode.cu', 'ctc_align.cu', 'ctc_prefix.cu', 'ctc_score.cu', 'rescore.cu', 'mwer.cu', 'mixspeech.cu', 'frame_stack.cu', 'fbank.cu', 'resample.cu', 'rnnt.cu', 'rnnt_pruned.cu', 'rnnt_beam.cu', 'capi.cu']
 HEADERS = ['otb_internal.h', 'ptx.cuh', 'beam_common.cuh', 'launch.cuh', 'counter_rng.cuh', 'dropout.cuh', 'ctc_trellis.cuh', 'row_lse.cuh', os.path.join('..', '..', 'include', 'otb200.h')]
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-lineinfo',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v', '--expt-relaxed-constexpr']

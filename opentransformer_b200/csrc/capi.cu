@@ -642,43 +642,76 @@ static const char* rnnt_lattice_check(int B, int T, int U1, const void* t_len, c
     return nullptr;
 }
 
+// rows of the stored lattice: B T U1, or B T S when banded
+static int64_t rnnt_rows(int B, int T, int U1, const void* s_begin, int S) { return (int64_t)B * T * (s_begin ? S : U1); }
+
 int otb_rnnt_joint(const void* ep, const void* pp, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len, void* out,
-                   void* stream) {
+                   const int32_t* s_begin, int S, void* stream) {
     if (!ep || !pp || !out) return fail("otb_rnnt_joint", "null operand");
     if ((t_len == nullptr) != (u_len == nullptr)) return fail("otb_rnnt_joint", "t_len and u_len are given together");
     RET("otb_rnnt_joint", rnnt_joint_launch(ST(stream), reinterpret_cast<const bf16*>(ep), reinterpret_cast<const bf16*>(pp), B, T, U1,
-                                            D, t_len, u_len, reinterpret_cast<bf16*>(out)));
+                                            D, t_len, u_len, s_begin, S, reinterpret_cast<bf16*>(out)));
 }
 
 int otb_rnnt_joint_bwd(const void* dh, const void* h, int B, int T, int U1, int D, const int32_t* t_len, const int32_t* u_len,
-                       void* dep, void* dpp, void* stream) {
+                       void* dep, void* dpp, const int32_t* s_begin, int S, void* stream) {
     if (!dh || !h || !dep || !dpp) return fail("otb_rnnt_joint_bwd", "null operand");
     if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_joint_bwd", e);
     RET("otb_rnnt_joint_bwd", rnnt_joint_bwd_launch(ST(stream), reinterpret_cast<const bf16*>(dh), reinterpret_cast<const bf16*>(h), B,
-                                                    T, U1, D, t_len, u_len, reinterpret_cast<bf16*>(dep), reinterpret_cast<bf16*>(dpp)));
+                                                    T, U1, D, t_len, u_len, s_begin, S, reinterpret_cast<bf16*>(dep),
+                                                    reinterpret_cast<bf16*>(dpp)));
 }
 
 int otb_rnnt_logprob(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
-                     const int32_t* u_len, const int32_t* labels, int ldy, float* lp, void* stream) {
+                     const int32_t* u_len, const int32_t* labels, int ldy, float* lp, const int32_t* s_begin, int S, void* stream) {
     if ((rows > 0 && !logits) || !labels || !lp) return fail("otb_rnnt_logprob", "null operand");
-    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, row0, rows)) return fail("otb_rnnt_logprob", e);
-    RET("otb_rnnt_logprob", rnnt_logprob_launch(ST(stream), logits, ld, rows, (long long)row0, V, T, U1, t_len, u_len, labels, ldy, lp));
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_logprob", e);
+    if (row0 < 0 || rows < 0 || row0 + rows > rnnt_rows(B, T, U1, s_begin, S)) return fail("otb_rnnt_logprob", "rows outside the lattice");
+    RET("otb_rnnt_logprob", rnnt_logprob_launch(ST(stream), logits, ld, rows, (long long)row0, V, T, U1, t_len, u_len, labels, ldy,
+                                                s_begin, S, lp));
 }
 
 int otb_rnnt_loss(const float* lp, int B, int T, int U1, const int32_t* t_len, const int32_t* u_len, double* alpha, float* nll,
-                  float* loss, float* grad, float grad_scale, const float* grad_scale_dev, void* stream) {
+                  float* loss, float* grad, float grad_scale, const float* grad_scale_dev, const int32_t* s_begin, int S, void* stream) {
     if (!lp || !alpha || !nll || !loss || !grad) return fail("otb_rnnt_loss", "null operand");
     if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_loss", e);
-    RET("otb_rnnt_loss", rnnt_loss_launch(ST(stream), lp, B, T, U1, t_len, u_len, alpha, nll, loss, grad, grad_scale, grad_scale_dev));
+    RET("otb_rnnt_loss", rnnt_loss_launch(ST(stream), lp, B, T, U1, t_len, u_len, s_begin, S, alpha, nll, loss, grad, grad_scale,
+                                          grad_scale_dev));
 }
 
 int otb_rnnt_dlogits(const float* logits, int ld, int rows, int64_t row0, int V, int B, int T, int U1, const int32_t* t_len,
                      const int32_t* u_len, const int32_t* labels, int ldy, const float* lp, const float* grad, void* dz, int ldd,
-                     void* stream) {
+                     const int32_t* s_begin, int S, void* stream) {
     if ((rows > 0 && !logits) || !labels || !lp || !grad || !dz) return fail("otb_rnnt_dlogits", "null operand");
-    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, row0, rows)) return fail("otb_rnnt_dlogits", e);
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_dlogits", e);
+    if (row0 < 0 || rows < 0 || row0 + rows > rnnt_rows(B, T, U1, s_begin, S)) return fail("otb_rnnt_dlogits", "rows outside the lattice");
     RET("otb_rnnt_dlogits", rnnt_dlogits_launch(ST(stream), logits, ld, rows, (long long)row0, V, T, U1, t_len, u_len, labels, ldy, lp,
-                                                grad, reinterpret_cast<bf16*>(dz), ldd));
+                                                grad, s_begin, S, reinterpret_cast<bf16*>(dz), ldd));
+}
+
+int otb_rnnt_simple_lse(const float* am, int lda, const float* lm, int ldl, int V, int B, int T, int U1, const int32_t* t_len,
+                        const int32_t* u_len, const int32_t* labels, int ldy, float* lp, float* m_am, float* m_lm, void* stream) {
+    if (!am || !lm || !labels || !lp || !m_am || !m_lm) return fail("otb_rnnt_simple_lse", "null operand");
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_simple_lse", e);
+    RET("otb_rnnt_simple_lse", rnnt_simple_lse_launch(ST(stream), am, lda, lm, ldl, V, B, T, U1, t_len, u_len, labels, ldy, lp, m_am,
+                                                      m_lm));
+}
+
+int otb_rnnt_simple_bwd(const float* am, int lda, const float* lm, int ldl, int V, int B, int T, int U1, const int32_t* t_len,
+                        const int32_t* u_len, const int32_t* labels, int ldy, const float* lp, const float* m_am, const float* m_lm,
+                        const float* grad, float scale, const float* scale_dev, void* d_am, void* d_lm, int ldd, void* stream) {
+    if (!am || !lm || !labels || !lp || !m_am || !m_lm || !grad || !d_am || !d_lm) return fail("otb_rnnt_simple_bwd", "null operand");
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_simple_bwd", e);
+    RET("otb_rnnt_simple_bwd", rnnt_simple_bwd_launch(ST(stream), am, lda, lm, ldl, V, B, T, U1, t_len, u_len, labels, ldy, lp, m_am,
+                                                      m_lm, grad, scale, scale_dev, reinterpret_cast<bf16*>(d_am),
+                                                      reinterpret_cast<bf16*>(d_lm), ldd));
+}
+
+int otb_rnnt_prune_ranges(const float* grad, int B, int T, int U1, const int32_t* t_len, const int32_t* u_len, int S, int32_t* s_begin,
+                          void* stream) {
+    if (!grad || !s_begin) return fail("otb_rnnt_prune_ranges", "null operand");
+    if (const char* e = rnnt_lattice_check(B, T, U1, t_len, u_len, 0, 0)) return fail("otb_rnnt_prune_ranges", e);
+    RET("otb_rnnt_prune_ranges", rnnt_prune_ranges_launch(ST(stream), grad, B, T, U1, t_len, u_len, S, s_begin));
 }
 
 int otb_rnnt_greedy_step(const int32_t* idx, const float* logp, int ldlp, const float* h_new, const float* c_new, const void* pp_new,

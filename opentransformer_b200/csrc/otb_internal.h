@@ -305,16 +305,26 @@ const char* resample_launch(cudaStream_t st, const float* x, int ldx, const int*
                             int ldy, int* n_out, int B, int width);
 
 const char* rnnt_joint_launch(cudaStream_t st, const bf16* ep, const bf16* pp, int B, int T, int U1, int D, const int* t_len,
-                              const int* u_len, bf16* out);
+                              const int* u_len, const int* s_begin, int S, bf16* out);
 const char* rnnt_joint_bwd_launch(cudaStream_t st, const bf16* dh, const bf16* h, int B, int T, int U1, int D, const int* t_len,
-                                  const int* u_len, bf16* dep, bf16* dpp);
+                                  const int* u_len, const int* s_begin, int S, bf16* dep, bf16* dpp);
 const char* rnnt_logprob_launch(cudaStream_t st, const float* logits, int ld, int rows, long long row0, int V, int T, int U1,
-                                const int* t_len, const int* u_len, const int* labels, int ldy, float* lp);
-const char* rnnt_loss_launch(cudaStream_t st, const float* lp, int B, int T, int U1, const int* t_len, const int* u_len, double* alpha,
-                             float* nll, float* loss, float* grad, float grad_scale, const float* scale_dev);
+                                const int* t_len, const int* u_len, const int* labels, int ldy, const int* s_begin, int S, float* lp);
+const char* rnnt_loss_launch(cudaStream_t st, const float* lp, int B, int T, int U1, const int* t_len, const int* u_len,
+                             const int* s_begin, int S, double* alpha, float* nll, float* loss, float* grad, float grad_scale,
+                             const float* scale_dev);
 const char* rnnt_dlogits_launch(cudaStream_t st, const float* logits, int ld, int rows, long long row0, int V, int T, int U1,
                                 const int* t_len, const int* u_len, const int* labels, int ldy, const float* lp, const float* grad,
-                                bf16* dz, int ldd);
+                                const int* s_begin, int S, bf16* dz, int ldd);
+const char* rnnt_simple_lse_launch(cudaStream_t st, const float* am, int lda, const float* lm, int ldl, int V, int B, int T, int U1,
+                                   const int* t_len, const int* u_len, const int* labels, int ldy, float* lp, float* m_am,
+                                   float* m_lm);
+const char* rnnt_simple_bwd_launch(cudaStream_t st, const float* am, int lda, const float* lm, int ldl, int V, int B, int T, int U1,
+                                   const int* t_len, const int* u_len, const int* labels, int ldy, const float* lp, const float* m_am,
+                                   const float* m_lm, const float* grad, float scale, const float* scale_dev, bf16* d_am,
+                                   bf16* d_lm, int ldd);
+const char* rnnt_prune_ranges_launch(cudaStream_t st, const float* grad, int B, int T, int U1, const int* t_len, const int* u_len,
+                                     int S, int* s_begin);
 const char* rnnt_greedy_step_launch(cudaStream_t st, const int* idx, const float* logp, int ldlp, const float* h_new,
                                     const float* c_new, const bf16* pp_new, float* h, float* c, bf16* pp, int layers, int B, int H,
                                     int D, const bf16* ep, int T, bf16* ep_cur, const int* t_len, int* frame, int* n_sym, int* n_out,

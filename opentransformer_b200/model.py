@@ -278,16 +278,28 @@ class PredictionNetwork(nn.Module):
 class JointNetwork(nn.Module):
     """z = output_layer(tanh(enc_proj(h_t) + dec_proj(g_u))): enc_proj Linear(encoder d_model -> inner), dec_proj
     Linear(hidden -> inner, no bias), output_layer Linear(inner -> V).  Compute: otb_rnnt_joint between the projection
-    GEMMs and the output layer's."""
+    GEMMs and the output layer's.
 
-    def __init__(self, encoder_size, hidden_size, inner_size, vocab_size):
+    prune_range S (an int >= 2, or None): pruned RNN-T training (DESIGN.md 4.22).  The simple joint simple_am_proj(h_t) +
+    simple_lm_proj(g_u) (Linear(encoder d_model -> V), Linear(hidden -> V)) picks S label positions per frame, and the
+    objective is simple_loss_scale * L_simple + L_pruned.  Recognition never reads the simple projections."""
+
+    def __init__(self, encoder_size, hidden_size, inner_size, vocab_size, prune_range=None, simple_loss_scale=0.5):
         super().__init__()
         if inner_size % 8:
             raise NotImplementedError(f'JointNetwork: the joint kernels need inner_size a multiple of 8, got {inner_size}')
+        if prune_range is not None and (isinstance(prune_range, bool) or not isinstance(prune_range, int) or prune_range < 2):
+            raise ValueError(f'JointNetwork: prune_range must be an int >= 2 or None, got {prune_range!r}')
+        if isinstance(simple_loss_scale, bool) or not isinstance(simple_loss_scale, (int, float)) or not simple_loss_scale >= 0:
+            raise ValueError(f'JointNetwork: simple_loss_scale must be a number >= 0, got {simple_loss_scale!r}')
         self.inner_size, self.vocab_size = inner_size, vocab_size
+        self.prune_range, self.simple_loss_scale = prune_range, float(simple_loss_scale)
         self.enc_proj = nn.Linear(encoder_size, inner_size)
         self.dec_proj = nn.Linear(hidden_size, inner_size, bias=False)
         self.output_layer = nn.Linear(inner_size, vocab_size)
+        if prune_range is not None:
+            self.simple_am_proj = nn.Linear(encoder_size, vocab_size)
+            self.simple_lm_proj = nn.Linear(hidden_size, vocab_size)
 
     @property
     def ld_logits(self):
@@ -314,9 +326,14 @@ class TransducerModel(nn.Module):
         self.encoder = BuildEncoder[params['encoder_type']](**params['encoder'])
         self.decoder = PredictionNetwork(**params['decoder'])
         self.vocab_size = self.decoder.vocab_size
-        self.joint = JointNetwork(self.encoder.d_model, self.decoder.hidden_size, params['joint']['inner_size'], self.vocab_size)
+        jp = params['joint']
+        self.joint = JointNetwork(self.encoder.d_model, self.decoder.hidden_size, jp['inner_size'], self.vocab_size,
+                                  jp.get('prune_range'), jp.get('simple_loss_scale', 0.5))
         self.blank = 0
-        self._pack = _Packed(self, lambda: train.transducer_operands(self, train.LayerPack(self)))
+        # the inference pack (recognition and the eval-mode loss); the simple projections, which only the pruned loss
+        # reads, are cast separately
+        self._pack = _Packed(self, lambda: train.transducer_operands(self, train.LayerPack(self), simple=False))
+        self._simple_pack = _Packed(self, lambda: train.simple_operands(self, train.LayerPack(self)))
 
     encode_bf16 = SpeechToText.encode_bf16
 
@@ -330,7 +347,10 @@ class TransducerModel(nn.Module):
             return run(self, inputs['inputs'], inputs['mask'], truth, tlen), None
         with torch.no_grad():
             mem, lengths, B, T2 = self.encode_bf16(inputs['inputs'], inputs['mask'])
-            loss, _ = train.transducer_head(self, self._pack.get(), mem, B, T2, lengths, truth, tlen)
+            op = self._pack.get()
+            if self.joint.prune_range is not None:
+                op = dict(op, simple=self._simple_pack.get())
+            loss, _ = train.transducer_head(self, op, mem, B, T2, lengths, truth, tlen)
         return loss, None
 
     train_pass = train.transducer_forward_backward

@@ -1399,10 +1399,23 @@ def _rnnt_lengths(t_len, u_len):
     return t_len, u_len
 
 
-def rnnt_joint(ep, pp, B, T, U1, t_len=None, u_len=None, out=None):
+def _rnnt_band(s_begin, S, B, T, U1):
+    """-> (row width of the stored lattice, S as the kernels take it): (U1, 0) for the full lattice, (S, S) for the band
+    s_begin i32 [B, T] of width S (pruned RNN-T)."""
+    if s_begin is None:
+        return U1, 0
+    _need(s_begin, torch.int32, 's_begin')
+    if s_begin.numel() != B * T:
+        raise ValueError(f's_begin must be [B, T] = [{B}, {T}], got {tuple(s_begin.shape)}')
+    if not isinstance(S, int) or S < 2:
+        raise ValueError(f'the band width S must be an int >= 2, got {S!r}')
+    return S, S
+
+
+def rnnt_joint(ep, pp, B, T, U1, t_len=None, u_len=None, out=None, s_begin=None, S=None):
     """Hj bf16 [B*T*U1, D] = tanh(ep[b*T + t] + pp[b*U1 + u]) over the padded lattice, u fastest (otb_rnnt_joint); ep bf16
     [B*T, D], pp bf16 [B*U1, D].  Nodes with t >= t_len[b] or u > u_len[b] (i32 [B]) are zero; without lengths every node
-    is valid."""
+    is valid.  With s_begin i32 [B, T] (pruned RNN-T): [B*T*S, D], row (b*T + t)*S + k holding u = s_begin[b, t] + k."""
     _need(ep, BF16, 'ep'); _need(pp, BF16, 'pp')
     D = ep.shape[1]
     if ep.shape[0] != B * T or tuple(pp.shape) != (B * U1, D):
@@ -1412,69 +1425,123 @@ def rnnt_joint(ep, pp, B, T, U1, t_len=None, u_len=None, out=None):
         raise ValueError('rnnt_joint: t_len and u_len are given together')
     if t_len is not None:
         _rnnt_lengths(t_len, u_len)
+    W, Sk = _rnnt_band(s_begin, S, B, T, U1)
     if out is None:
-        out = torch.empty(B * T * U1, D, dtype=BF16, device=ep.device)
-    check(_lib.lib().otb_rnnt_joint(_p(ep), _p(pp), B, T, U1, D, _p(t_len), _p(u_len), _p(out), _stream()), 'otb_rnnt_joint')
+        out = torch.empty(B * T * W, D, dtype=BF16, device=ep.device)
+    check(_lib.lib().otb_rnnt_joint(_p(ep), _p(pp), B, T, U1, D, _p(t_len), _p(u_len), _p(out), _p(s_begin), Sk, _stream()),
+          'otb_rnnt_joint')
     _count()
     return out
 
 
-def rnnt_joint_bwd(dh, h, B, T, U1, t_len, u_len):
+def rnnt_joint_bwd(dh, h, B, T, U1, t_len, u_len, s_begin=None, S=None):
     """Backward of rnnt_joint from dh = dHj bf16 [B*T*U1, D] and its output h -> (dEp bf16 [B*T, D], dPp bf16 [B*U1, D]):
-    dZ = dh (1 - h^2) summed over u and over t, in a fixed order (otb_rnnt_joint_bwd)."""
+    dZ = dh (1 - h^2) summed over u and over t, in a fixed order (otb_rnnt_joint_bwd).  s_begin, S: as rnnt_joint."""
     _need(dh, BF16, 'dh'); _need(h, BF16, 'h'); _rnnt_lengths(t_len, u_len)
+    _, Sk = _rnnt_band(s_begin, S, B, T, U1)
     D = h.shape[1]
     dep = torch.empty(B * T, D, dtype=BF16, device=h.device)
     dpp = torch.empty(B * U1, D, dtype=BF16, device=h.device)
-    check(_lib.lib().otb_rnnt_joint_bwd(_p(dh), _p(h), B, T, U1, D, _p(t_len), _p(u_len), _p(dep), _p(dpp), _stream()),
-          'otb_rnnt_joint_bwd')
+    check(_lib.lib().otb_rnnt_joint_bwd(_p(dh), _p(h), B, T, U1, D, _p(t_len), _p(u_len), _p(dep), _p(dpp), _p(s_begin), Sk,
+                                        _stream()), 'otb_rnnt_joint_bwd')
     _count()
     return dep, dpp
 
 
-def rnnt_logprob(logits, row0, V, B, T, U1, t_len, u_len, labels, lp):
+def rnnt_logprob(logits, row0, V, B, T, U1, t_len, u_len, labels, lp, s_begin=None, S=None):
     """Lattice rows [row0, row0 + rows) of logits f32 [rows, ld] -> lp f32 [B*T*U1, 3] rows row0.. = (logsumexp, log p(blank),
-    log p(labels[b, u])) (otb_rnnt_logprob); labels i32 [B, >= U1 - 1]."""
+    log p(labels[b, u])) (otb_rnnt_logprob); labels i32 [B, >= U1 - 1].  s_begin, S: as rnnt_joint (lp [B*T*S, 3])."""
     _mat(logits, 'logits', torch.float32); _rnnt_lengths(t_len, u_len); _need(labels, torch.int32, 'labels')
     _need(lp, torch.float32, 'lp')
+    _, Sk = _rnnt_band(s_begin, S, B, T, U1)
     check(_lib.lib().otb_rnnt_logprob(_p(logits), logits.stride(0), logits.shape[0], row0, V, B, T, U1, _p(t_len), _p(u_len),
-                                      _p(labels), labels.stride(0), _p(lp), _stream()), 'otb_rnnt_logprob')
+                                      _p(labels), labels.stride(0), _p(lp), _p(s_begin), Sk, _stream()), 'otb_rnnt_logprob')
     _count()
     return lp
 
 
-def rnnt_loss(lp, B, T, U1, t_len, u_len, grad_scale=1.0, scale_dev=None):
+def rnnt_loss(lp, B, T, U1, t_len, u_len, grad_scale=1.0, scale_dev=None, s_begin=None, S=None):
     """The RNN-T loss over the lattice log-probs lp (rnnt_logprob) -> (loss 0-d = mean_b nll_b, nll f32 [B], grad f32
     [B*T*U1, 2] = grad_scale (x the f32 device scalar scale_dev) / B * d nll_b / d (log p(blank), log p(label)))
-    (otb_rnnt_loss)."""
+    (otb_rnnt_loss).  s_begin, S: the alignments restricted to the bands (as rnnt_joint; lp and grad [B*T*S, .]); an
+    utterance with no alignment inside them has nll +inf and zero gradients."""
     _need(lp, torch.float32, 'lp'); _rnnt_lengths(t_len, u_len)
     if U1 - 1 > RNNT_MAX_LABELS:
         raise ValueError(f'rnnt_loss: transcripts of {U1 - 1} labels; at most {RNNT_MAX_LABELS} are supported')
     if scale_dev is not None:
         _need(scale_dev, torch.float32, 'scale_dev')
+    W, Sk = _rnnt_band(s_begin, S, B, T, U1)
     dev = lp.device
-    alpha = torch.empty(B * T * U1, dtype=torch.float64, device=dev)
+    alpha = torch.empty(B * T * W, dtype=torch.float64, device=dev)
     nll = torch.empty(B, dtype=torch.float32, device=dev)
     loss = torch.empty(1, dtype=torch.float32, device=dev)
-    grad = torch.empty(B * T * U1, 2, dtype=torch.float32, device=dev)
+    grad = torch.empty(B * T * W, 2, dtype=torch.float32, device=dev)
     check(_lib.lib().otb_rnnt_loss(_p(lp), B, T, U1, _p(t_len), _p(u_len), _p(alpha), _p(nll), _p(loss), _p(grad), float(grad_scale),
-                                   _p(scale_dev), _stream()), 'otb_rnnt_loss')
+                                   _p(scale_dev), _p(s_begin), Sk, _stream()), 'otb_rnnt_loss')
     _count(2)
     return loss[0], nll, grad
 
 
-def rnnt_dlogits(logits, row0, V, B, T, U1, t_len, u_len, labels, lp, grad, out=None):
+def rnnt_dlogits(logits, row0, V, B, T, U1, t_len, u_len, labels, lp, grad, out=None, s_begin=None, S=None):
     """dz bf16 [rows, ld] = [k = blank] a + [k = label] c - softmax_k (a + c) of the lattice rows [row0, row0 + rows) in
-    logits f32 [rows, ld], with lp's logsumexp and (a, c) = grad of the node (otb_rnnt_dlogits); columns >= V are zero."""
+    logits f32 [rows, ld], with lp's logsumexp and (a, c) = grad of the node (otb_rnnt_dlogits); columns >= V are zero.
+    s_begin, S: as rnnt_joint."""
     _mat(logits, 'logits', torch.float32); _rnnt_lengths(t_len, u_len); _need(labels, torch.int32, 'labels')
     _need(lp, torch.float32, 'lp'); _need(grad, torch.float32, 'grad')
+    _, Sk = _rnnt_band(s_begin, S, B, T, U1)
     rows, ld = logits.shape[0], logits.shape[1]
     if out is None:
         out = torch.empty(rows, ld, dtype=BF16, device=logits.device)
     check(_lib.lib().otb_rnnt_dlogits(_p(logits), logits.stride(0), rows, row0, V, B, T, U1, _p(t_len), _p(u_len), _p(labels),
-                                      labels.stride(0), _p(lp), _p(grad), _p(out), out.stride(0), _stream()), 'otb_rnnt_dlogits')
+                                      labels.stride(0), _p(lp), _p(grad), _p(out), out.stride(0), _p(s_begin), Sk, _stream()),
+          'otb_rnnt_dlogits')
     _count()
     return out
+
+
+def rnnt_simple_lse(am, lm, V, B, T, U1, t_len, u_len, labels):
+    """The simple joint of pruned RNN-T (otb_rnnt_simple_lse): logits am[b*T + t] + lm[b*U1 + u] of am f32 [B*T, >= V] and
+    lm f32 [B*U1, >= V] -> (lp f32 [B*T*U1, 3] as rnnt_logprob's, m_am f32 [B*T], m_lm f32 [B*U1] the row maxima)."""
+    _mat(am, 'am', torch.float32); _mat(lm, 'lm', torch.float32); _rnnt_lengths(t_len, u_len); _need(labels, torch.int32, 'labels')
+    if am.shape[0] != B * T or lm.shape[0] != B * U1:
+        raise ValueError(f'rnnt_simple_lse: am must have B*T = {B * T} rows and lm B*U1 = {B * U1}, got {am.shape[0]} and '
+                         f'{lm.shape[0]}')
+    dev = am.device
+    lp = torch.empty(B * T * U1, 3, dtype=torch.float32, device=dev)
+    m_am = torch.empty(B * T, dtype=torch.float32, device=dev)
+    m_lm = torch.empty(B * U1, dtype=torch.float32, device=dev)
+    check(_lib.lib().otb_rnnt_simple_lse(_p(am), am.stride(0), _p(lm), lm.stride(0), V, B, T, U1, _p(t_len), _p(u_len), _p(labels),
+                                         labels.stride(0), _p(lp), _p(m_am), _p(m_lm), _stream()), 'otb_rnnt_simple_lse')
+    _count()
+    return lp, m_am, m_lm
+
+
+def rnnt_simple_bwd(am, lm, V, B, T, U1, t_len, u_len, labels, lp, m_am, m_lm, grad, scale=1.0, scale_dev=None, ldd=None):
+    """Backward of the simple joint (otb_rnnt_simple_bwd) from grad = rnnt_loss's over rnnt_simple_lse's lp, times scale (x
+    the f32 device scalar scale_dev) -> (d am bf16 [B*T, ldd], d lm bf16 [B*U1, ldd]), columns >= V zero."""
+    _mat(am, 'am', torch.float32); _mat(lm, 'lm', torch.float32); _rnnt_lengths(t_len, u_len); _need(labels, torch.int32, 'labels')
+    _need(grad, torch.float32, 'grad')
+    if scale_dev is not None:
+        _need(scale_dev, torch.float32, 'scale_dev')
+    ldd = ldd or (V + 7) // 8 * 8
+    d_am = torch.empty(B * T, ldd, dtype=BF16, device=am.device)
+    d_lm = torch.empty(B * U1, ldd, dtype=BF16, device=am.device)
+    check(_lib.lib().otb_rnnt_simple_bwd(_p(am), am.stride(0), _p(lm), lm.stride(0), V, B, T, U1, _p(t_len), _p(u_len), _p(labels),
+                                         labels.stride(0), _p(lp), _p(m_am), _p(m_lm), _p(grad), float(scale), _p(scale_dev),
+                                         _p(d_am), _p(d_lm), ldd, _stream()), 'otb_rnnt_simple_bwd')
+    _count()
+    return d_am, d_lm
+
+
+def rnnt_prune_ranges(grad, B, T, U1, t_len, u_len, S):
+    """The band of each frame for pruned RNN-T (otb_rnnt_prune_ranges): s_begin i32 [B, T] from the simple loss's node
+    gradients grad f32 [B*T*U1, 2] (rnnt_loss), by the range rule of DESIGN.md 4.22."""
+    _need(grad, torch.float32, 'grad'); _rnnt_lengths(t_len, u_len)
+    s_begin = torch.empty(B, T, dtype=torch.int32, device=grad.device)
+    check(_lib.lib().otb_rnnt_prune_ranges(_p(grad), B, T, U1, _p(t_len), _p(u_len), int(S), _p(s_begin), _stream()),
+          'otb_rnnt_prune_ranges')
+    _count()
+    return s_begin
 
 
 def rnnt_greedy_step(idx, logp, h_new, c_new, pp_new, h, c, pp, ep, T, ep_cur, t_len, frame, n_sym, n_out, ids, max_sym, score,

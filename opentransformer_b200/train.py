@@ -908,11 +908,55 @@ def lstm_stack_bwd(dy, tape, layers, L, N, g, dropout=0.0, drop_seed=None, site0
     return dy
 
 
-def transducer_operands(model, pk):
-    """The prediction network's and the joint network's operands of a TransducerModel, cast by the LayerPack pk."""
+def transducer_operands(model, pk, simple=True):
+    """The prediction network's and the joint network's operands of a TransducerModel, cast by the LayerPack pk; with
+    simple and a prune_range, also the simple joint's (simple_operands) under 'simple'."""
     j, d = model.joint, model.decoder
-    return {'enc': pk._lin(j.enc_proj), 'dec_w': pk.w(j.dec_proj.weight), 'out_w': pk.w(j.output_layer.weight),
-            'out_b': _f(j.output_layer.bias), 'emb': pk.w(d.embedding.weight), 'layers': lstm_layers(d.rnn, pk.w, 'decoder.rnn.')}
+    op = {'enc': pk._lin(j.enc_proj), 'dec_w': pk.w(j.dec_proj.weight), 'out_w': pk.w(j.output_layer.weight),
+          'out_b': _f(j.output_layer.bias), 'emb': pk.w(d.embedding.weight), 'layers': lstm_layers(d.rnn, pk.w, 'decoder.rnn.')}
+    if simple and j.prune_range is not None:
+        op['simple'] = simple_operands(model, pk)
+    return op
+
+
+def simple_operands(model, pk):
+    """simple_am_proj and simple_lm_proj of a pruned TransducerModel as Lin, W^T zero-padded to [K, ld_logits] so that the
+    dgrad GEMM takes the padded bf16 gradient rows as they are."""
+    j = model.joint
+    ld, V = j.ld_logits, j.vocab_size
+
+    def lin(m):
+        x = pk._lin(m)
+        wt = torch.zeros(x.w.shape[1], ld, dtype=BF16, device=x.w.device)
+        wt[:, :V] = x.wt
+        return x._replace(wt=wt)
+
+    return {'am': lin(j.simple_am_proj), 'lm': lin(j.simple_lm_proj)}
+
+
+def _padded_linear_bwd(dz, x, lin, V, g, resid=None):
+    """linear_bwd for a Linear(K -> V) whose output gradient dz bf16 [M, ld] is zero-padded past V (lin.wt [K, ld])."""
+    acc = g.sink is not None
+    g[lin.wname] = ops.linear_wgrad(dz[:, :V], x, out=g.out(lin.wname), accumulate=acc)
+    db = torch.zeros(dz.shape[1], dtype=torch.float32, device=dz.device)
+    ops.colsum(dz, out=db, accumulate=True)
+    g.put(lin.bname, db[:V])
+    if resid is not None:
+        return ops.linear(dz, lin.wt, None, EPI_RESID, resid=resid)
+    return ops.linear(dz, lin.wt)
+
+
+def _simple_joint(model, op, mem, gb, B, T2, U1, lengths, u_len, labels):
+    """The pruned loss's simple joint: am = simple_am_proj(memory), lm = simple_lm_proj(g) in f32, its node log-probs,
+    loss (unit gradient scale) and node gradients, and the bands s_begin i32 [B, T'] (DESIGN.md 4.22)."""
+    V, ld, S = model.vocab_size, model.joint.ld_logits, model.joint.prune_range
+    sp = op['simple']
+    am = ops.linear(mem, sp['am'].w, sp['am'].b, EPI_BIAS, out=torch.empty(B * T2, ld, dtype=torch.float32, device=mem.device))
+    lm = ops.linear(gb, sp['lm'].w, sp['lm'].b, EPI_BIAS, out=torch.empty(B * U1, ld, dtype=torch.float32, device=mem.device))
+    lp, m_am, m_lm = ops.rnnt_simple_lse(am, lm, V, B, T2, U1, lengths, u_len, labels)
+    loss, _, grad = ops.rnnt_loss(lp, B, T2, U1, lengths, u_len)
+    s_begin = ops.rnnt_prune_ranges(grad, B, T2, U1, lengths, u_len, S)
+    return loss, s_begin, (am, lm, lp, m_am, m_lm, grad)
 
 
 def transducer_head(model, op, mem, B, T2, lengths, truth, truth_length, drop_seed=None, g=None, grad_scale=1.0,
@@ -923,7 +967,10 @@ def transducer_head(model, op, mem, B, T2, lengths, truth, truth_length, drop_se
     workspace_bytes (RNNT_WORKSPACE_BYTES) of fp32 logits.  op: transducer_operands.  -> (loss 0-d f32 = mean_b nll_b,
     dmem bf16 [B*T', d] or None).  With g (a Grads) the backward runs: each chunk's logits are recomputed, turned into
     bf16 dlogits and sent through the dgrad and the accumulating wgrad GEMMs, then the joint, the projections and the
-    prediction network run backward into g; the loss gradient is scaled by grad_scale (a float or an f32 device scalar)."""
+    prediction network run backward into g; the loss gradient is scaled by grad_scale (a float or an f32 device scalar).
+    With the joint's prune_range S (op['simple'] present): the simple joint picks S label positions per frame on the device,
+    the joint and the output layer run over the [B, T', S] band only, and the loss is simple_loss_scale * L_simple +
+    L_pruned."""
     dev = mem.device
     V, D = model.vocab_size, model.joint.inner_size
     dec = model.decoder
@@ -942,8 +989,14 @@ def transducer_head(model, op, mem, B, T2, lengths, truth, truth_length, drop_se
     enc = op['enc']
     ep = ops.linear(mem, enc.w, enc.b, EPI_BIAS)
     pp = ops.linear(gb, op['dec_w'])
-    hj = ops.rnnt_joint(ep, pp, B, T2, U1, lengths, u_len)
-    rows, ld = B * T2 * U1, model.joint.ld_logits
+    pruned = 'simple' in op
+    S = model.joint.prune_range if pruned else None
+    band = {}
+    if pruned:
+        loss_s, s_begin, simple = _simple_joint(model, op, mem, gb, B, T2, U1, lengths, u_len, labels)
+        band = {'s_begin': s_begin, 'S': S}
+    hj = ops.rnnt_joint(ep, pp, B, T2, U1, lengths, u_len, **band)
+    rows, ld = B * T2 * (S if pruned else U1), model.joint.ld_logits
     chunk = max(8, (workspace_bytes or RNNT_WORKSPACE_BYTES) // (4 * ld) // 8 * 8)
     ws = torch.empty(min(chunk, rows), ld, dtype=torch.float32, device=dev)
     lp = torch.empty(rows, 3, dtype=torch.float32, device=dev)
@@ -953,9 +1006,12 @@ def transducer_head(model, op, mem, B, T2, lengths, truth, truth_length, drop_se
         return ops.linear(hj[r0:r1], op['out_w'], op['out_b'], EPI_BIAS, out=ws[:r1 - r0])
 
     for r0, r1 in spans:
-        ops.rnnt_logprob(logits(r0, r1), r0, V, B, T2, U1, lengths, u_len, labels, lp)
+        ops.rnnt_logprob(logits(r0, r1), r0, V, B, T2, U1, lengths, u_len, labels, lp, **band)
     s, sdev = _loss_scale(grad_scale, 1.0)
-    loss, _, grad = ops.rnnt_loss(lp, B, T2, U1, lengths, u_len, s, sdev)
+    loss, _, grad = ops.rnnt_loss(lp, B, T2, U1, lengths, u_len, s, sdev, **band)
+    if pruned:
+        alpha = model.joint.simple_loss_scale
+        loss = alpha * loss_s + loss
     if not want:
         return loss, None
 
@@ -966,18 +1022,27 @@ def transducer_head(model, op, mem, B, T2, lengths, truth, truth_length, drop_se
     dl = torch.empty(ws.shape, dtype=BF16, device=dev)
     dhj = torch.empty(rows, D, dtype=BF16, device=dev)
     for r0, r1 in spans:
-        dz = ops.rnnt_dlogits(logits(r0, r1), r0, V, B, T2, U1, lengths, u_len, labels, lp, grad, out=dl[:r1 - r0])
+        dz = ops.rnnt_dlogits(logits(r0, r1), r0, V, B, T2, U1, lengths, u_len, labels, lp, grad, out=dl[:r1 - r0], **band)
         ops.linear_wgrad(dz[:, :V], hj[r0:r1], out=dw, accumulate=True)
         ops.colsum(dz, out=db, accumulate=True)
         ops.linear(dz, wt, out=dhj[r0:r1])
     g.put('joint.output_layer.bias', db[:V])
     del ws, dl
-    dep, dpp = ops.rnnt_joint_bwd(dhj, hj, B, T2, U1, lengths, u_len)
+    dep, dpp = ops.rnnt_joint_bwd(dhj, hj, B, T2, U1, lengths, u_len, **band)
     del dhj, hj
     dmem = linear_bwd(dep, mem, enc, g)
     acc = g.sink is not None
     g['joint.dec_proj.weight'] = ops.linear_wgrad(dpp, gb, out=g.out('joint.dec_proj.weight'), accumulate=acc)
     dgb = ops.linear(dpp, op['dec_w'].t().contiguous())
+    if pruned:
+        # the simple loss trains the simple projections and flows into the memory and the predictor; no gradient
+        # flows through the bands
+        am, lm, lp_s, m_am, m_lm, grad_s = simple
+        s_s, sdev_s = _loss_scale(grad_scale, model.joint.simple_loss_scale)
+        d_am, d_lm = ops.rnnt_simple_bwd(am, lm, V, B, T2, U1, lengths, u_len, labels, lp_s, m_am, m_lm, grad_s, s_s, sdev_s, ld)
+        del am, lm
+        dmem = _padded_linear_bwd(d_am, mem, op['simple']['am'], V, g, resid=dmem)
+        dgb = _padded_linear_bwd(d_lm, gb, op['simple']['lm'], V, g, resid=dgb)
     dy = dgb.view(B, U1, H).transpose(0, 1).contiguous().view(U1 * B, H)
     dx = lstm_stack_bwd(dy, tape, op['layers'], U1, B, g, dec.dropout, drop_seed, RNNT_SITE)
     embedding_bwd(tok, dx, op['emb'], 1.0, g, 'decoder.embedding.weight')

@@ -6,9 +6,12 @@ GLU, residual_dropout 0.1), a 1 x 320 LSTM prediction network and a 512-wide joi
   - TransducerRecognizer.recognize (greedy) on the same batch;
   - the transducer kernels alone on the step's lattice (CUDA events over repeated launches), and the output layer's GEMMs.
 
+With --prune-range S it also times the FusedTrainer step of the full and of the pruned loss (joint prune_range S,
+DESIGN.md 4.22) in the same run, with their peak memory, at 30-label transcripts and at 200-label ones.
+
 It prints the card, its power limit and its maximum SM clock, read in the same run.  Needs a GPU.
 
-    python tools/transducer.py [--iters 10]
+    python tools/transducer.py [--iters 10] [--prune-range 5]
 """
 import argparse
 import json
@@ -32,11 +35,49 @@ def params():
             'decoder': dict(vocab_size=4234, hidden_size=320, num_layers=1, dropout=0.0), 'joint': {'inner_size': 512}}
 
 
+def _batch(B, T, L, V, dev, seed=1):
+    g = torch.Generator().manual_seed(seed)
+    lens = torch.randint(int(0.8 * T), T + 1, (B,), generator=g)
+    lens[0] = T
+    mask = (torch.arange(T)[None] < lens[:, None]).to(dev)
+    x = (torch.randn(B, T, 80, generator=g).to(dev) * mask.unsqueeze(2))
+    tgt = torch.randint(2, V, (B, L), generator=g)
+    tgt[:, 0] = 1
+    tgt[:, -1] = 1
+    return x, mask, tgt.to(dev), torch.full((B,), L - 1).to(dev)
+
+
+def full_vs_pruned(S, B, T, iters, dev):
+    """FusedTrainer step time (CUDA graph, CUDA events after warm-up) and peak memory of the full and the pruned loss,
+    alternated in one run, at 30- and 200-label transcripts."""
+    out = []
+    for labels in (30, 200):
+        x, mask, tgt, tlen = _batch(B, T, labels + 2, 4234, dev)
+        row = {'labels': labels}
+        for name, prune in (('full', None), ('pruned', S)):
+            p = params()
+            p['joint'] = dict(p['joint'], prune_range=prune)
+            torch.manual_seed(0)
+            model = TransducerModel(p).to(dev).train()
+            tr = train.FusedTrainer(model, accum_steps=1, use_graph=True)
+            tr.step(x, mask, tgt, tlen)
+            torch.cuda.synchronize()
+            torch.cuda.reset_peak_memory_stats()
+            row[f'{name}_step_ms'] = timed(lambda: tr.step(x, mask, tgt, tlen), iters)
+            row[f'{name}_peak_GB'] = torch.cuda.max_memory_allocated() / 1e9
+            row[f'{name}_loss'] = float(tr.step(x, mask, tgt, tlen))
+            del tr, model
+            torch.cuda.empty_cache()
+        out.append(row)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--iters', type=int, default=10)
     ap.add_argument('--batch', type=int, default=32)
     ap.add_argument('--frames', type=int, default=1000)
+    ap.add_argument('--prune-range', type=int, default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('tools/transducer.py measures on the GPU; none is visible')
@@ -103,6 +144,11 @@ def main():
         logits = ops.linear(hj[:chunk], op['out_w'], op['out_b'], ops.EPI_BIAS, out=ws)
         k['dlogits_chunk_ms'] = timed(lambda: ops.rnnt_dlogits(logits, 0, V, B, T2, U1, lengths, u_len, labels, lp, grad), a.iters)
         res['kernels'] = k
+    if a.prune_range is not None:
+        del tr, rec, hj, ws, logits, lp, grad
+        torch.cuda.empty_cache()
+        res['prune_range'] = a.prune_range
+        res['full_vs_pruned'] = full_vs_pruned(a.prune_range, a.batch, a.frames, a.iters, dev)
     print(json.dumps(res, indent=1))
 
 
