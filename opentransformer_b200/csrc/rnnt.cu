@@ -177,7 +177,7 @@ __global__ void __launch_bounds__(RNNT_MAX_U1) rnnt_loss_kernel(const float* __r
     for (int i = threadIdx.x; i < T * W; i += blockDim.x) {      // nodes past T_b or U_b
         if (i / W >= Tb || i % W + (sb ? sb[i / W] : 0) > Ub) g[2 * i] = g[2 * i + 1] = 0.f;
     }
-    if (Tb < 1) {       // no frame: no alignment
+    if (Tb < 1 || Ub < 0) {     // no frame, or a negative label count: no node, no alignment
         if (threadIdx.x == 0) nll[b] = INFINITY;
         return;
     }

@@ -10,7 +10,9 @@
 //                              d am[t,v] = D[t,v] - exp(am[t,v] - m_t) sum_u P[t,u] exp(lm[u,v] - m_u)
 //                              d lm[u,v] = D[u,v] - exp(lm[u,v] - m_u) sum_t P[t,u] exp(am[t,v] - m_t)
 //                            with D the one-hot part (scale a at column 0, scale c at column y_{u+1}), summed by one thread
-//                            per row in ascending order (no atomics); bf16 out, columns >= V zero.
+//                            per row in ascending order (no atomics); bf16 out, columns >= V zero.  A node whose
+//                            factorized sum left the normal fp32 range (SJ_ACC_MIN) has Z from the logits directly,
+//                            and the backward subtracts its term w exp(am[t,v] + lm[u,v] - Z) on its own.
 //   rnnt_prune_ranges_kernel one CTA per utterance: the window of S label positions with the largest occupancy at every
 //                            frame, then the range rule of DESIGN.md 4.22.
 #include <math.h>
@@ -25,6 +27,23 @@ static constexpr int SJ_K = 32;           // reduction chunk (columns of V in th
 static constexpr int SJ_COLS = 64;        // columns of V per CTA of the backward
 static constexpr int SJ_THREADS = 256;
 static constexpr int PRUNE_THREADS = 256;
+// The factorized sum acc = sum_v exp(am[t,v] - m_t) exp(lm[u,v] - m_u) is exact to a few ulps only while its terms are
+// normal numbers.  A term below 2^-126 (subnormal factor or product) carries an absolute error up to 2^-149, so the V
+// terms together up to V 2^-149; against acc >= 2^-100 that is below V 2^-49, under one f32 ulp for any V < 2^25.  A
+// node with acc < 2^-100 (every logit sum at least 69.3 below m_t + m_u; 0 or -inf when it is above 87 or 103) takes
+// Z from the logits directly instead.  The backward recognizes those nodes by m_t + m_u - Z > 100 ln 2 and adds their
+// exact term, so the factorized product never scales a node by exp(m_t + m_u - Z) > 2^100.
+static constexpr float SJ_ACC_MIN = 0x1p-100f;
+static constexpr float SJ_GAP_MAX = 69.3147181f;     // 100 ln 2
+
+// Z = max_v (am[v] + lm[v]) + log sum_v exp(am[v] + lm[v] - max), one thread, ascending v in fp32
+__device__ __forceinline__ float simple_lse_direct(const float* xa, const float* xl, int V) {
+    float m = -INFINITY;
+    for (int v = 0; v < V; ++v) m = fmaxf(m, xa[v] + xl[v]);
+    float s = 0.f;
+    for (int v = 0; v < V; ++v) s += expf((xa[v] + xl[v]) - m);
+    return m + logf(s);
+}
 
 __device__ __forceinline__ int simple_label(const int* labels, int ldy, int b, int u, int Ub, int V) {
     if (u >= Ub) return -1;
@@ -92,7 +111,7 @@ __global__ void __launch_bounds__(SJ_THREADS) rnnt_simple_lse_kernel(const float
         }
         const float* xa = am + ((size_t)b * T + t) * lda;
         const float* xl = lm + ((size_t)b * U1 + u) * ldl;
-        const float z = mx[ti] + mx[SJ_ROWS + uj + 8 * q] + logf(acc[q]);
+        const float z = acc[q] < SJ_ACC_MIN ? simple_lse_direct(xa, xl, V) : mx[ti] + mx[SJ_ROWS + uj + 8 * q] + logf(acc[q]);
         const int y = simple_label(labels, ldy, b, u, Ub, V);
         o[0] = z;
         o[1] = (xa[0] + xl[0]) - z;
@@ -113,6 +132,8 @@ __global__ void __launch_bounds__(SJ_THREADS) rnnt_simple_bwd_kernel(const float
     __shared__ float ps[SJ_ROWS][SJ_K + 1];          // P of the CTA's rows against the chunk's reduction rows
     __shared__ float ey[SJ_K][SJ_COLS + 1];          // exp(other - m) of the chunk's reduction rows
     __shared__ float dsum[SJ_ROWS][SJ_COLS + 1];     // the one-hot part D
+    __shared__ float pw[SJ_ROWS][SJ_K + 1];          // w of the nodes whose Z the forward took directly, else 0
+    __shared__ int s_exact;                          // some such node with w != 0 seen so far
     const int b = blockIdx.z, v0 = blockIdx.x * SJ_COLS;
     const int n_am = (T + SJ_ROWS - 1) / SJ_ROWS;
     const bool side_am = (int)blockIdx.y < n_am;
@@ -134,19 +155,29 @@ __global__ void __launch_bounds__(SJ_THREADS) rnnt_simple_bwd_kernel(const float
     const float* m_oth = side_am ? m_lm : m_am;
 
     const int ri = threadIdx.x / 8, cj = threadIdx.x % 8;       // own row r0 + ri, columns v0 + cj + 8 q
-    float acc[8];
+    const float* x = own + (own0 + r0 + ri) * ld_own;
+    float acc[8], exact[8];
 #pragma unroll
-    for (int q = 0; q < 8; ++q) acc[q] = 0.f;
+    for (int q = 0; q < 8; ++q) acc[q] = exact[q] = 0.f;
+    if (threadIdx.x == 0) s_exact = 0;
+    __syncthreads();
     for (int j0 = 0; j0 < n_red; j0 += SJ_K) {
         for (int e = threadIdx.x; e < SJ_ROWS * SJ_K; e += SJ_THREADS) {
             const int i = e / SJ_K, j = e % SJ_K;
-            float p = 0.f;
+            float p = 0.f, pe = 0.f;
             if (r0 + i < n_own && j0 + j < n_red) {
                 const size_t k = node(r0 + i, j0 + j);
                 const float w = sc * (grad[2 * k] + grad[2 * k + 1]);
-                p = w * expf(m_own[own0 + r0 + i] + m_oth[oth0 + j0 + j] - lp[3 * k]);
+                const float gap = m_own[own0 + r0 + i] + m_oth[oth0 + j0 + j] - lp[3 * k];
+                if (gap > SJ_GAP_MAX) {         // Z came from the logits directly (forward): the node's own term below
+                    pe = w;
+                    if (w != 0.f) s_exact = 1;
+                } else {
+                    p = w * expf(gap);
+                }
             }
             ps[i][j] = p;
+            pw[i][j] = pe;
         }
         for (int e = threadIdx.x; e < SJ_K * SJ_COLS; e += SJ_THREADS) {
             const int j = e / SJ_COLS, v = e % SJ_COLS;
@@ -160,6 +191,19 @@ __global__ void __launch_bounds__(SJ_THREADS) rnnt_simple_bwd_kernel(const float
             const float p = ps[ri][j];
 #pragma unroll
             for (int q = 0; q < 8; ++q) acc[q] = fmaf(p, ey[j][cj + 8 * q], acc[q]);
+        }
+        if (s_exact) {      // w exp(own + other - Z) of the nodes left out of ps, ascending j
+            for (int j = 0; j < SJ_K; ++j) {
+                const float pe = pw[ri][j];
+                if (pe == 0.f) continue;
+                const float z = lp[3 * node(r0 + ri, j0 + j)];
+                const float* y = oth + (oth0 + j0 + j) * ld_oth;
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const int v = v0 + cj + 8 * q;
+                    if (v < V) exact[q] += pe * expf((x[v] + y[v]) - z);
+                }
+            }
         }
         __syncthreads();
     }
@@ -194,14 +238,14 @@ __global__ void __launch_bounds__(SJ_THREADS) rnnt_simple_bwd_kernel(const float
     const int i = r0 + ri;
     if (i >= (side_am ? T : U1)) return;
     bf16* out = (side_am ? d_am : d_lm) + (own0 + i) * ldd;
-    const bool live = i < n_own;
-    const float* x = own + (own0 + i) * ld_own;
+    const bool live = i < n_own, with_exact = s_exact;
 #pragma unroll
     for (int q = 0; q < 8; ++q) {
         const int v = v0 + cj + 8 * q;
         if (v >= ldd) continue;
         float d = 0.f;
         if (live && v < V) d = dsum[ri][cj + 8 * q] - expf(x[v] - m_own[own0 + i]) * acc[q];
+        if (with_exact) d -= exact[q];
         out[v] = __float2bfloat16_rn(d);
     }
 }
